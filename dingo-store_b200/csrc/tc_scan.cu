@@ -7,13 +7,16 @@
 //   tc_fill_pairs_kernel     gather the (TF32-rounded) queries of every list into one contiguous block
 //   tc_items_kernel          emit work items (list chunk x query group) + the list of sampled items
 //   tc_scan_kernel           *** the hot kernel: TMA -> smem ring -> wgmma (TF32, register accumulators) -> epilogue ***
-//   tc_tau_kernel            per-query capture threshold from the sampled rows (radix select)
-//   tc_final_fast_kernel     per-query window select + exact FP32 (AVX-512 order) rerank + certification
-//                            (tc_final_kernel: the streaming variant for candidate buffers that do not fit shared memory)
-//   tc_coarse_select_kernel  coarse-quantiser finish: register-resident radix select + exact rerank of the window
-//                            (tc_coarse_final_fast_kernel / tc_coarse_final_kernel: one-sort / streaming fallbacks)
+//   tc_tau_warp_kernel       per-query capture threshold from the sampled rows (warp radix select)
+//                            (tc_tau_kernel: the block form for queries with more sampled spans than a warp stages)
+//   tc_final_hybrid_kernel   per-query window select + exact FP32 (AVX-512 order) rerank + certification
+//                            (tc_final_kernel: the streaming form for windows or query rows that do not fit)
+//   tc_coarse_select_hybrid_kernel / tc_coarse_select_kernel
+//                            coarse-quantiser finish: register-resident radix select + exact rerank of the window
+//                            (tc_coarse_final_kernel: the streaming form for what they cannot finish)
 //   tc_compact_flags_kernel  list of uncertified queries for the exact re-run
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -279,7 +282,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
   const long long list_base = p.list_off[I.list];
   int rows = I.row_end - I.row_begin;
-  if (p.mode == 0) rows = min(rows, p.sample_rows);
+  if (p.mode == 0) rows = min(rows, TC_SAMPLE);
   const int ntiles = (rows + TC_BM - 1) / TC_BM;
   for (int t = 0; t < ntiles; ++t) {
     // row metadata first: its loads overlap the MMAs
@@ -326,7 +329,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
                 }
               }
             } else if (p.mode == 0) {
-              if (t == 0 && r < p.sample_rows) p.sample[((size_t)I.sample_slot * TC_NQT + n) * p.sample_rows + r] = valid[h] ? score : TC_INF;
+              if (t == 0 && r < TC_SAMPLE) p.sample[((size_t)I.sample_slot * TC_NQT + n) * TC_SAMPLE + r] = valid[h] ? score : TC_INF;
             } else if (inrange[h]) {
               float* dst = p.dense + (size_t)s_q[n] * p.dense_ld + (I.row_begin + r);
               if (p.dense_accum) *dst = *dst + score;
@@ -388,11 +391,11 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const TcItem I = p.items[it];
         const long long base_row = p.list_off[I.list] + I.row_begin;
         int rows = I.row_end - I.row_begin;
-        if (p.mode == 0) rows = min(rows, p.sample_rows);
+        if (p.mode == 0) rows = min(rows, TC_SAMPLE);
         const int ntiles = (rows + TC_BM - 1) / TC_BM;
         const int b_rows = I.nq <= 16 ? 16 : (I.nq <= 32 ? 32 : (I.nq <= 64 ? 64 : 128));
         const CUtensorMap* tb = I.nq <= 16 ? &tmB16 : (I.nq <= 32 ? &tmB32 : (I.nq <= 64 ? &tmB64 : &tmB128));
-        const bool small_a = p.mode == 0 && p.sample_rows == TC_SAMPLE;  // 32-row sample box, else the full 128-row tile
+        const bool small_a = p.mode == 0;  // 32-row sample box, else the full 128-row tile
         const CUtensorMap* ta = small_a ? &tmA32 : &tmA;
         const uint32_t bytes = (small_a ? (uint32_t)(TC_SAMPLE * 128) : TC_A_BYTES) + (uint32_t)b_rows * 128u;
         const CUtensorMap* tbl = I.nq <= 16 ? &tmBlo16 : (I.nq <= 32 ? &tmBlo32 : (I.nq <= 64 ? &tmBlo64 : &tmBlo128));
@@ -468,13 +471,9 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 // ---------------------------------------------------------------------------------------------
-// per-query capture threshold T.  tau = the k-th smallest sampled score bounds the k-th smallest score overall (A_k)
-// from above.  Thin samples (32 rows per span, ~1 % of the probed rows) leave tau far above A_k + 2 eps and T = tau:
-// the finish kernel certifies A_k + 2 eps <= T and sends the rare failure to the exact scan.  Dense samples (the whole
-// first tile, used when a query probes few local lists) put tau close to A_k, so T = tau + 2 eps: then
-// A_k + 2 eps <= T by construction and certification can only fail on a buffer overflow.
+// per-query capture threshold T.  tau = the k-th smallest sampled score (TC_SAMPLE rows per span) bounds the k-th
+// smallest score overall (A_k) from above; tc_tau_with_margin turns it into T.
 // ---------------------------------------------------------------------------------------------
-__device__ uint32_t block_kth_key(const unsigned long long* keys, int n, int k);
 __device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm, int d, bool split);
 
 // Capture threshold from the sampled k-th score tau.  The finish kernel certifies A_k + 2 eps <= T (A_k = k-th captured
@@ -497,21 +496,22 @@ __device__ __forceinline__ float tc_tau_with_margin(float tau, float two_eps, in
 }
 
 constexpr int TAU_PL = 4096;  // (sample slot, column) pairs staged per query
-constexpr int TAU_SORT = 4096;  // sampled scores sorted in one shot when they fit
 
+// Block form of the threshold kernel, for the queries tc_tau_warp_kernel hands back (more sampled spans than a warp
+// stages): one (sample slot, column) pair per sampled span, then the k-th smallest finite sampled score, selected by the
+// whole CTA straight from the sample buffer.
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_tau_kernel(const long long* __restrict__ probes, const int* __restrict__ pos, const int* __restrict__ cnt,
               const int* __restrict__ item_off, const int* __restrict__ list_len, const TcItem* __restrict__ items, int nprobe,
-              const float* __restrict__ sample, int srows, int k, int pool_cap, int l2, const float* __restrict__ qnorm,
-              float max_norm, int d, int margin, int cand_cap, float* tau, const int* redo) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int s_np;
+              const float* __restrict__ sample, int k, int l2, const float* __restrict__ qnorm, float max_norm, int d,
+              int cand_cap, float* tau, const int* __restrict__ redo) {
+  __shared__ int2 s_pairs[TAU_PL];
+  __shared__ BlockSelShared S;
+  __shared__ int s_np, s_cle;
   const int q = blockIdx.x;
-  if (redo && !redo[q]) return;  // only the queries the warp kernel could not finish
-  int2* s_pairs = reinterpret_cast<int2*>(smem);  // [TAU_PL]
+  if (!redo[q]) return;  // finished by the warp kernel
   if (threadIdx.x == 0) s_np = 0;
-  BlockSelect sel;
-  sel.init(smem + (size_t)TAU_PL * 8, pool_cap, k);  // barrier inside
+  __syncthreads();
   for (int j = threadIdx.x; j < nprobe; j += blockDim.x) {
     const long long l = probes[(size_t)q * nprobe + j];
     if (l < 0) continue;
@@ -528,58 +528,28 @@ tc_tau_kernel(const long long* __restrict__ probes, const int* __restrict__ pos,
     }
   }
   __syncthreads();
-  const int np_all = s_np;
-  const int np = min(np_all, TAU_PL);
-  const int tot = np * srows;
-  if (np_all <= TAU_PL && tot <= TAU_SORT) {  // common case: radix-select the k-th smallest sampled score in shared memory
-    unsigned long long* vals = reinterpret_cast<unsigned long long*>(smem + (size_t)TAU_PL * 8);
-    __shared__ int s_fin;
-    if (threadIdx.x == 0) s_fin = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < tot; i += blockDim.x) {
-      const int2 pr = s_pairs[i / srows];
-      const float v = sample[((size_t)pr.x * TC_NQT + pr.y) * srows + (i % srows)];
-      if (v < TC_INF) vals[atomicAdd(&s_fin, 1)] = (unsigned long long)f2ord(v) << 32;
-    }
-    __syncthreads();
-    const int nfin = s_fin;
-    const uint32_t kth = nfin >= k ? block_kth_key(vals, nfin, k) : 0u;
-    if (nfin < k) { if (threadIdx.x == 0) tau[q] = TC_INF; return; }
-    const float two_eps = 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, false);
-    if (margin) { if (threadIdx.x == 0) tau[q] = __fadd_rn(ord2f(kth), two_eps); return; }  // dense samples: always
-    __shared__ int s_cle;
-    auto count_le = [&](float lim) {  // block-wide count of sampled scores <= lim (all threads call)
-      __syncthreads();
-      if (threadIdx.x == 0) s_cle = 0;
-      __syncthreads();
-      int c = 0;
-      for (int i = threadIdx.x; i < nfin; i += blockDim.x) c += ord2f((uint32_t)(vals[i] >> 32)) <= lim ? 1 : 0;
-      c = __reduce_add_sync(0xffffffffu, c);
-      if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_cle, c);
-      __syncthreads();
-      return s_cle;
-    };
-    const float t = tc_tau_with_margin(ord2f(kth), two_eps, cand_cap, count_le);
-    if (threadIdx.x == 0) tau[q] = t;
-    return;
-  }
-  for (int base = 0; base < tot; base += blockDim.x) {
-    sel.maybe_prune(blockDim.x);
-    const int i = base + threadIdx.x;
-    if (i < tot) {
-      const int2 pr = s_pairs[i / srows];
-      const int s = i % srows;
-      const float v = sample[((size_t)pr.x * TC_NQT + pr.y) * srows + s];
-      if (v < TC_INF) {
-        const uint32_t key = f2ord(v);
-        if (sel.passes(key, i)) sel.push(key, i);
-      }
-    }
-  }
-  sel.prune();
+  const int np = s_np;
   // more sampled spans than the staging area holds: capture everything (overflow then falls back to the exact scan)
-  if (threadIdx.x == 0)
-    tau[q] = (np_all <= TAU_PL && *sel.count >= k) ? __fadd_rn(ord2f(sel.kd[k - 1]), margin ? 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, false) : 0.f) : TC_INF;
+  if (np > TAU_PL) { if (threadIdx.x == 0) tau[q] = TC_INF; return; }
+  const int tot = np * TC_SAMPLE;
+  auto sampled = [&](int i) { const int2 pr = s_pairs[i / TC_SAMPLE]; return sample[((size_t)pr.x * TC_NQT + pr.y) * TC_SAMPLE + i % TC_SAMPLE]; };
+  auto count_le = [&](float lim) {  // block-wide count of sampled scores <= lim (all threads call)
+    __syncthreads();
+    if (threadIdx.x == 0) s_cle = 0;
+    __syncthreads();
+    int c = 0;
+    for (int i = threadIdx.x; i < tot; i += blockDim.x) c += sampled(i) <= lim ? 1 : 0;
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_cle, c);
+    __syncthreads();
+    return s_cle;
+  };
+  if (count_le(FLT_MAX) < k) { if (threadIdx.x == 0) tau[q] = TC_INF; return; }  // fewer than k finite sampled scores
+  const float kth = ord2f(block_kth_key_any(k, S, [&](auto f) {
+    for (int i = threadIdx.x; i < tot; i += blockDim.x) { const float v = sampled(i); if (v < TC_INF) f(f2ord(v)); }
+  }));
+  const float t = tc_tau_with_margin(kth, 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, false), cand_cap, count_le);
+  if (threadIdx.x == 0) tau[q] = t;
 }
 
 
@@ -673,18 +643,7 @@ __device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm,
   return operand + accum;
 }
 
-// ---- block-wide bitonic sorts in shared memory (ascending), m = power of two ----
-__device__ __forceinline__ void block_sort_u64(unsigned long long* keys, int m) {
-  for (int size = 2; size <= m; size <<= 1)
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = threadIdx.x; i < (m >> 1); i += blockDim.x) {
-        const int pos = 2 * i - (i & (stride - 1)), j = pos + stride;
-        const unsigned long long a = keys[pos], b = keys[j];
-        if (((pos & size) == 0) ? (b < a) : (a < b)) { keys[pos] = b; keys[j] = a; }
-      }
-      __syncthreads();
-    }
-}
+// ---- block-wide bitonic sort in shared memory (ascending), m = power of two ----
 __device__ __forceinline__ void block_sort_pair(uint32_t* kd, long long* kid, int m) {
   for (int size = 2; size <= m; size <<= 1)
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
@@ -699,161 +658,17 @@ __device__ __forceinline__ void block_sort_pair(uint32_t* kd, long long* kid, in
     }
 }
 
-// Fast window select shared by the list-scan finish and the coarse finish.  keys[0..n) = (ord(approx score) << 32 | row),
-// unsorted, padded storage for the next power of two.  Sorts once, takes the k-th approximate score, re-scores the
-// in-window prefix exactly (reference order) and returns the exact top-k in (ex_kd, ex_id)[0..k).
-// Returns the number of exact entries kept (<= k) and whether the prefix fit in `maxw`.
-// k-th smallest (k >= 1, n >= k) of the 32-bit keys stored in the high halves of keys[0..n): 4-pass radix select with a
-// 256-bin shared histogram (no sorting network, ~10 barriers).  All threads call; returns the key to all threads.
-__device__ uint32_t block_kth_key(const unsigned long long* keys, int n, int k) {
-  __shared__ int s_hist[256];
-  __shared__ uint32_t s_prefix;
-  __shared__ int s_k;
-  if (threadIdx.x == 0) { s_prefix = 0; s_k = k; }
-  for (int pass = 0; pass < 4; ++pass) {
-    const int shift = 24 - 8 * pass;
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
-    __syncthreads();
-    const uint32_t prefix = s_prefix;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-      const uint32_t key = (uint32_t)(keys[i] >> 32);
-      if (pass == 0 || ((key ^ prefix) >> (shift + 8)) == 0) atomicAdd(&s_hist[(key >> shift) & 255], 1);
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {  // warp 0: locate the bin that holds the k-th element
-      const int lane = threadIdx.x;
-      int loc[8], sum = 0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { loc[j] = s_hist[lane * 8 + j]; sum += loc[j]; }
-      int incl = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-      const int kk = s_k;
-      const int before = incl - sum;
-      if (before < kk && kk <= incl) {  // exactly one lane
-        int acc = before;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (acc < kk && kk <= acc + loc[j]) { s_prefix = prefix | ((uint32_t)(lane * 8 + j) << shift); s_k = kk - acc; }
-          acc += loc[j];
-        }
-      }
-    }
-    __syncthreads();
-  }
-  return s_prefix;
-}
-
-// Window select shared by the list-scan finish and the coarse finish.  keys[0..n) = (ord(approx score) << 32 | row),
-// unsorted.  Finds the k-th approximate score (radix select), gathers every row whose score is within two_eps of it,
-// re-scores those rows exactly (reference order) and sorts the exact (key, id) pairs: ex_kd/ex_id[0..returned).
-// Returns the number of exact entries kept (<= k); *fits = the window fit in `maxw` rows.
-template <bool L2, bool ROW_IS_ID>
-__device__ int window_select(const unsigned long long* keys, int n, int k, float two_eps, const float* qs, const float* __restrict__ vecs,
-                             const long long* __restrict__ ids, int d, uint32_t* ex_kd, long long* ex_id, int* rows, int maxw, bool* fits,
-                             float* a_k_out, int* s_m) {
-  const float a_k = n >= k ? ord2f(block_kth_key(keys, n, k)) : TC_INF;
-  const float window = a_k + two_eps;
-  if (threadIdx.x == 0) *s_m = 0;
-  __syncthreads();
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const unsigned long long e = keys[i];
-    if (ord2f((uint32_t)(e >> 32)) <= window) {
-      const int pos = atomicAdd(s_m, 1);
-      if (pos < maxw) rows[pos] = (int)(uint32_t)(e & 0xffffffffull);
-    }
-  }
-  __syncthreads();
-  int m = *s_m;
-  *fits = m <= maxw;
-  m = min(m, maxw);
-  *a_k_out = a_k;
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  const bool vec = (d & 3) == 0;
-  {  // pull every in-window row into L2 at once (random 3 KB gathers: latency-bound otherwise)
-    const int lines = (d * 4 + 127) / 128;
-    for (int i = threadIdx.x; i < m * lines; i += blockDim.x) {
-      const char* ptr = reinterpret_cast<const char*>(vecs + (size_t)(uint32_t)rows[i / lines] * d) + (size_t)(i % lines) * 128;
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
-    }
-  }
-  const int nquads = blockDim.x >> 2;
-  for (int base = 0; base < m; base += nquads) {
-    const int i = base + quad;
-    const bool valid = i < m;
-    const long long row = (long long)(uint32_t)rows[valid ? i : 0];
-    const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
-    if (valid && t == 0) { ex_kd[i] = f2ord(L2 ? v : -v); ex_id[i] = ROW_IS_ID ? row : ids[row]; }
-  }
-  int e2 = 2;
-  while (e2 < m) e2 <<= 1;
-  __syncthreads();
-  for (int i = m + threadIdx.x; i < e2; i += blockDim.x) { ex_kd[i] = KEY_SENTINEL_D; ex_id[i] = KEY_SENTINEL_ID; }
-  __syncthreads();
-  block_sort_pair(ex_kd, ex_id, e2);
-  return min(m, k);
-}
-
-constexpr int FIN_THREADS = 128;   // finish kernels: many small CTAs hide their barrier / gather latency better than few big ones
-constexpr int FIN_MAXW = 1024;     // in-window rows re-scored per query on the fast path (more -> exact re-run)
-constexpr int COARSE_FAST = 8192;  // coarse rows handled by the register-select / one-sort path
-
-template <bool L2>
-static __global__ void __launch_bounds__(SCAN_THREADS)
-tc_final_fast_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
-                     const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
-                     const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k, float* out_dist,
-                     long long* out_ids, int* flags, const int* redo) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int s_m;
-  const int qi = blockIdx.x;
-  if (redo && !redo[qi]) return;  // only the queries the warp kernel could not finish
-  float* qs = reinterpret_cast<float*>(smem);
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
-  long long* ex_id = reinterpret_cast<long long*>(smem + qbytes);                    // [FIN_MAXW]
-  uint32_t* ex_kd = reinterpret_cast<uint32_t*>(smem + qbytes + (size_t)FIN_MAXW * 8);  // [FIN_MAXW]
-  int* rows = reinterpret_cast<int*>(smem + qbytes + (size_t)FIN_MAXW * 12);            // [FIN_MAXW]
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem + qbytes + (size_t)FIN_MAXW * 16);  // [cap]
-  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = q[(size_t)qi * d + i];
-  const int total = cand_cnt[qi];
-  const int n = min(total, cap);
-  for (int i = threadIdx.x; i < n; i += blockDim.x) keys[i] = cand[(size_t)qi * cap + i];
-  __syncthreads();
-  bool fits;
-  float a_k;
-  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, false);
-  const int have = window_select<L2, false>(keys, n, k, two_eps, qs, vecs, ids, d, ex_kd, ex_id, rows, FIN_MAXW, &fits, &a_k, &s_m);
-  const float tq = tau[qi];
-  const bool certified = fits && (total <= cap) && (tq == TC_INF || a_k + two_eps <= tq);
-  for (int i = threadIdx.x; i < k; i += blockDim.x) {
-    float api = 0.f;
-    long long id = -1;
-    if (i < have) {
-      const float v = ord2f(ex_kd[i]);
-      const float raw = L2 ? v : -v;
-      api = L2 ? raw : __fsub_rn(1.0f, raw);
-      id = ex_id[i];
-    }
-    out_dist[(size_t)qi * k + i] = api;
-    out_ids[(size_t)qi * k + i] = id;
-  }
-  if (threadIdx.x == 0) flags[qi] = certified ? 0 : 1;
-}
-
-
 // ---------------------------------------------------------------------------------------------
-// Finish kernel for the common case (at most HF_MAXW rows inside the 2*eps window): one 128-thread CTA per query.  Same
-// rule as tc_final_fast_kernel — k-th approximate score A_k, every captured row with score <= A_k + 2 eps re-scored
-// exactly in the reference order, exact top-k by (distance, id), certification — but the selection is done by ONE warp
-// with shuffles / ballots and a warp-private histogram (no block-wide radix passes), all 32 quads of the CTA then
-// re-score the window rows together (the ~40 random 3 KB row gathers per query are what this kernel waits on, so they are
-// all issued at once) and a rank sort orders the exact pairs: three block barriers in total, 16 CTAs per SM.
-// Queries whose window is larger set redo[q] = 1 and are finished by the block kernel.
+// Finish kernel for the common case (at most HF_MAXW rows inside the 2*eps window): one 128-thread CTA per query.
+// k-th approximate score A_k (block radix select), every captured row with score <= A_k + 2 eps re-scored exactly in the
+// reference order, exact top-k by (distance, id), certification.  All 32 quads of the CTA re-score the window rows
+// together (the ~40 random 3 KB row gathers per query are what this kernel waits on, so they are all issued at once) and a
+// rank sort orders the exact pairs: 16 CTAs per SM.  Queries whose window is larger set redo[q] = 1 and are finished by
+// tc_final_kernel.
 // ---------------------------------------------------------------------------------------------
 constexpr int HF_THREADS = 128;
 constexpr int HF_STAGE = 512;   // captured keys staged in shared memory (the rest is re-read from global / L2 in every pass)
 constexpr int HF_MAXW = 256;
-constexpr int HF_ROW_BYTES = 48 * 1024;  // dynamic shared memory for the staged window rows (+ the query row)
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
@@ -862,16 +677,13 @@ __device__ __forceinline__ void cp_async_wait_all() {
   asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
-// The ~40 window rows of a query are random 3 KB gathers from HBM: what the kernel waits on.  They are staged into
-// shared memory with 16-byte cp.async copies (no registers held, so a CTA keeps a whole group of rows in flight), then
-// quads re-score them from shared memory in the reference order.  rows_g rows of `pitch` bytes per group (d % 4 == 0).
 template <bool L2>
 static __global__ void __launch_bounds__(HF_THREADS)
 tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
                        const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
-                       const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k, int rows_g, int pitch,
+                       const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k,
                        float* out_dist, long long* out_ids, int* flags, int* redo) {
-  extern __shared__ __align__(16) unsigned char s_dyn[];  // [pitch] query row, then rows_g staged rows
+  extern __shared__ __align__(16) unsigned char s_dyn[];  // the query row (d % 4 == 0)
   __shared__ BlockSelShared S;
   __shared__ unsigned long long s_keys[HF_STAGE];
   __shared__ int s_rows[HF_MAXW];
@@ -884,15 +696,14 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   const int n = min(total, cap);
   const unsigned long long* c = cand + (size_t)qi * cap;
   const int nst = min(n, HF_STAGE);
-  const int cpr = d >> 2;  // 16-byte chunks per row
-  for (int i = threadIdx.x; i < cpr; i += HF_THREADS) cp_async16(s_dyn + (size_t)i * 16, q + (size_t)qi * d + i * 4);
+  for (int i = threadIdx.x; i < (d >> 2); i += HF_THREADS) cp_async16(s_dyn + (size_t)i * 16, q + (size_t)qi * d + i * 4);
   for (int i = threadIdx.x; i < nst; i += HF_THREADS) s_keys[i] = c[i];
-  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, false);
   if (threadIdx.x == 0) s_m = 0;
   __syncthreads();
   auto key_at = [&](int i) -> unsigned long long { return i < nst ? s_keys[i] : c[i]; };
   float a_k = TC_INF;
   if (n >= k) a_k = ord2f(block_kth_key_any(k, S, [&](auto f) { for (int i = threadIdx.x; i < n; i += HF_THREADS) f((uint32_t)(key_at(i) >> 32)); }));
+  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, false);
   {
     const float window = a_k + two_eps;
     for (int base = 0; base < n; base += HF_THREADS) {
@@ -913,63 +724,33 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   if (m > HF_MAXW) { if (threadIdx.x == 0) redo[qi] = 1; return; }
   const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
   const float* qs = reinterpret_cast<const float*>(s_dyn);
-  if (rows_g <= 0) {
-    // direct form: every in-window row is prefetched towards L2 at once, then 32 quads score 32 rows per round straight from
-    // global memory (no staging buffer: 16 CTAs per SM keep ~500 rows in flight per SM)
-    const int lines = (d * 4 + 127) / 128;
-    for (int i = threadIdx.x; i < m * lines; i += HF_THREADS) {
-      const char* ptr = reinterpret_cast<const char*>(vecs + (size_t)(uint32_t)s_rows[i / lines] * d) + (size_t)(i % lines) * 128;
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
-    }
-    cp_async_wait_all();  // the query row
-    __syncthreads();
-    for (int base = 0; base < m; base += HF_THREADS / 4) {
-      const int i = base + quad;
-      const bool valid = i < m;
-      const long long row = (long long)(uint32_t)s_rows[valid ? i : 0];
-      const long long id = valid ? ids[row] : -1;
-      const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, true);
-      if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = id; }
-    }
-    __syncthreads();
-  } else {
-  unsigned char* stage = s_dyn + pitch;
-  for (int g0 = 0; g0 < m; g0 += rows_g) {
-    const int ng = min(rows_g, m - g0);
-    for (int i = threadIdx.x; i < ng * cpr; i += HF_THREADS) {
-      const int r = i / cpr, ch = i - r * cpr;
-      cp_async16(stage + (size_t)r * pitch + (size_t)ch * 16, vecs + (size_t)(uint32_t)s_rows[g0 + r] * d + ch * 4);
-    }
-    if (threadIdx.x < ng) s_id[g0 + threadIdx.x] = ids[(uint32_t)s_rows[g0 + threadIdx.x]];
-    cp_async_wait_all();
-    __syncthreads();
-    for (int base = 0; base < ng; base += HF_THREADS / 4) {
-      const int i = base + quad;
-      const bool valid = i < ng;
-      const float v = quad_distance<L2>(reinterpret_cast<const float*>(stage + (size_t)(valid ? i : 0) * pitch), qs, d, t, true);
-      if (valid && t == 0) s_kd[g0 + i] = f2ord(L2 ? v : -v);
-    }
-    __syncthreads();
+  // every in-window row is prefetched towards L2 at once, then 32 quads score 32 rows per round straight from global memory
+  // (no staging buffer: 16 CTAs per SM keep ~500 rows in flight per SM)
+  const int lines = (d * 4 + 127) / 128;
+  for (int i = threadIdx.x; i < m * lines; i += HF_THREADS) {
+    const char* ptr = reinterpret_cast<const char*>(vecs + (size_t)(uint32_t)s_rows[i / lines] * d) + (size_t)(i % lines) * 128;
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
   }
+  cp_async_wait_all();  // the query row
+  __syncthreads();
+  for (int base = 0; base < m; base += HF_THREADS / 4) {
+    const int i = base + quad;
+    const bool valid = i < m;
+    const long long row = (long long)(uint32_t)s_rows[valid ? i : 0];
+    const long long id = valid ? ids[row] : -1;
+    const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, true);
+    if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = id; }
   }
-  const int have = min(m, k);
-  for (int e = threadIdx.x; e < m; e += HF_THREADS) {
-    const uint32_t d0 = s_kd[e];
-    const long long i0 = s_id[e];
-    int rank = 0;
-    for (int j = 0; j < m; ++j) {
-      const uint32_t dj = s_kd[j];
-      const long long ij = s_id[j];
-      rank += (key_less(dj, ij, d0, i0) || (dj == d0 && ij == i0 && j < e)) ? 1 : 0;
-    }
+  __syncthreads();
+  block_rank_sort(s_kd, s_id, m, [&](int rank, int e) {
     if (rank < k) {
-      const float v = ord2f(d0);
+      const float v = ord2f(s_kd[e]);
       const float raw = L2 ? v : -v;
       out_dist[(size_t)qi * k + rank] = L2 ? raw : __fsub_rn(1.0f, raw);
-      out_ids[(size_t)qi * k + rank] = i0;
+      out_ids[(size_t)qi * k + rank] = s_id[e];
     }
-  }
-  for (int i = have + threadIdx.x; i < k; i += HF_THREADS) { out_dist[(size_t)qi * k + i] = 0.f; out_ids[(size_t)qi * k + i] = -1; }
+  });
+  for (int i = min(m, k) + threadIdx.x; i < k; i += HF_THREADS) { out_dist[(size_t)qi * k + i] = 0.f; out_ids[(size_t)qi * k + i] = -1; }
   if (threadIdx.x == 0) {
     const float tq = tau[qi];
     flags[qi] = (total <= cap ? 0 : 2) | ((tq == TC_INF || a_k + two_eps <= tq) ? 0 : 1);  // 1: threshold too tight, 2: capture overflow
@@ -977,114 +758,13 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   }
 }
 
-template <bool L2>
-static __global__ void __launch_bounds__(SCAN_THREADS)
-tc_coarse_final_fast_kernel(const float* __restrict__ dense, long long ld, int nrows, const float* __restrict__ qnorm, float max_norm,
-                            const float* __restrict__ q, const float* __restrict__ vecs, int d, int k, int maxw,
-                            long long id_offset, int api_scores, long long* out_probes, float* out_raw, const int* redo) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int s_m;
-  const int qi = blockIdx.x;
-  if (redo && !redo[qi]) return;  // only the queries the register-select kernel could not finish
-  float* qs = reinterpret_cast<float*>(smem);
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
-  long long* ex_id = reinterpret_cast<long long*>(smem + qbytes);                       // [maxw]   maxw = pow2(nrows)
-  uint32_t* ex_kd = reinterpret_cast<uint32_t*>(smem + qbytes + (size_t)maxw * 8);      // [maxw]
-  int* rows = reinterpret_cast<int*>(smem + qbytes + (size_t)maxw * 12);                // [maxw]
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem + qbytes + (size_t)maxw * 16);  // [maxw]
-  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = q[(size_t)qi * d + i];
-  for (int i = threadIdx.x; i < nrows; i += blockDim.x) keys[i] = ((unsigned long long)f2ord(dense[(size_t)qi * ld + i]) << 32) | (unsigned)i;
-  __syncthreads();
-  bool fits;
-  float a_k;
-  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true);
-  const int have = window_select<L2, true>(keys, nrows, k, two_eps, qs, vecs, nullptr, d, ex_kd, ex_id, rows, maxw, &fits, &a_k, &s_m);
-  for (int i = threadIdx.x; i < k; i += blockDim.x) {
-    out_probes[(size_t)qi * k + i] = i < have ? ex_id[i] + id_offset : -1;
-    if (out_raw) {
-      const float v = i < have ? ord2f(ex_kd[i]) : 0.f;
-      const float raw = L2 ? v : -v;
-      out_raw[(size_t)qi * k + i] = api_scores ? v : raw;  // api_scores: the ranking score itself (L2 distance | -ip), ascending
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
-// Register-resident select (coarse finish): each of SEL_THREADS threads holds KPT keys, so a query's whole score row
+// Register-resident select (coarse finish): each of SEL_THREADS threads holds KPT <= 32 keys, so a query's whole score row
 // lives in registers and the CTA needs only ~13 KB of shared memory (8 CTAs per SM hide each other's barriers).
 // ---------------------------------------------------------------------------------------------
 constexpr int SEL_THREADS = 256;
-constexpr int SEL_BINS = 1024;   // histogram bins per narrowing step (10 bits)
-constexpr int SEL_WCAP = 512;    // window rows re-scored per query (more -> the one-sort fallback kernel)
-
-struct SelShared {
-  int hist[SEL_BINS];
-  uint32_t red[2][SEL_THREADS / 32];
-  uint32_t lo, hi;
-  int k, c_le, m, ns;
-};
-
-// k-th smallest (k >= 1, at least k live keys) of the CTA's keys; 0xFFFFFFFF marks an empty slot.  Range-normalised
-// radix select: bin = (key - lo) >> shift over the live range [lo, hi], narrow to the bin that holds the k-th key and
-// repeat until bins are one key wide (two steps for the ~2^20-wide ranges of real score rows; never more than four).
-// On return S.c_le = number of keys <= the result when known exactly, else k + 1.
-template <int KPT>
-__device__ uint32_t reg_kth_key(const uint32_t (&key)[KPT], int k, SelShared& S) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t mn = 0xFFFFFFFFu, mx = 0u;
-#pragma unroll
-  for (int j = 0; j < KPT; ++j)
-    if (key[j] != 0xFFFFFFFFu) { mn = min(mn, key[j]); mx = max(mx, key[j]); }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o)); mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o)); }
-  if (lane == 0) { S.red[0][warp] = mn; S.red[1][warp] = mx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t a = 0xFFFFFFFFu, b = 0u;
-    for (int w = 0; w < SEL_THREADS / 32; ++w) { a = min(a, S.red[0][w]); b = max(b, S.red[1][w]); }
-    S.lo = a; S.hi = b; S.k = k; S.c_le = k + 1;
-  }
-  __syncthreads();
-  for (;;) {
-    const uint32_t lo = S.lo, hi = S.hi;
-    const int kk = S.k;
-    const uint32_t range = hi - lo;
-    if (range == 0) return lo;  // every remaining key is equal
-    const int bits = 32 - __clz(range);
-    const int shift = max(0, bits - 10);
-    for (int i = threadIdx.x; i < SEL_BINS; i += SEL_THREADS) S.hist[i] = 0;
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < KPT; ++j)
-      if (key[j] >= lo && key[j] <= hi) atomicAdd(&S.hist[(key[j] - lo) >> shift], 1);
-    __syncthreads();
-    if (warp == 0) {  // locate the bin that holds the kk-th key: 32 bins per lane
-      int sum = 0;
-      for (int j = 0; j < SEL_BINS / 32; ++j) sum += S.hist[lane * (SEL_BINS / 32) + j];
-      int incl = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-      const int before = incl - sum;
-      if (before < kk && kk <= incl) {  // exactly one lane
-        int acc = before;
-        for (int j = 0; j < SEL_BINS / 32; ++j) {
-          const int c = S.hist[lane * (SEL_BINS / 32) + j];
-          if (acc < kk && kk <= acc + c) {
-            const uint32_t nlo = lo + ((uint32_t)(lane * (SEL_BINS / 32) + j) << shift);
-            S.lo = nlo;
-            S.hi = min(hi, nlo + ((1u << shift) - 1u));
-            S.k = kk - acc;
-            if (shift == 0) S.c_le = (k - kk) + acc + c;
-            break;
-          }
-          acc += c;
-        }
-      }
-    }
-    __syncthreads();
-    if (shift == 0) return S.lo;
-  }
-}
+constexpr int SEL_MAX_ROWS = 32 * SEL_THREADS;  // score rows the register select holds
+constexpr int SEL_WCAP = 512;    // window rows re-scored per query (more -> tc_coarse_final_kernel)
 
 // Coarse finish: top-nprobe rows of one query's dense score row.
 //   full mode (out_raw != NULL or ties at the k-th score): re-score every row within 2*eps of the k-th approximate score
@@ -1092,17 +772,18 @@ __device__ uint32_t reg_kth_key(const uint32_t (&key)[KPT], int k, SelShared& S)
 //   set mode  (probe tables, whose order nobody reads): rows more than 2*eps below the k-th score are certainly among
 //     the exact top-k (only the k - 1 rows below it can beat them), rows more than 2*eps above are certainly not; only the
 //     few rows in between are re-scored to fill the remaining slots.
-// flags[qi] = 1 when the window overflowed SEL_WCAP: the one-sort kernel then redoes that query.
+// flags[qi] = 1 when the window overflowed SEL_WCAP: tc_coarse_final_kernel then redoes that query.
 template <bool L2, int KPT>
 static __global__ void __launch_bounds__(SEL_THREADS)
 tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows, const float* __restrict__ qnorm, float max_norm,
                         const float* __restrict__ q, const float* __restrict__ vecs, int d, int k, long long id_offset, int api_scores,
                         long long* out_probes, float* out_raw, int* flags, const int* redo_in) {
   extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ SelShared S;
+  __shared__ BlockSelShared S;
   __shared__ int s_rows[SEL_WCAP];
   __shared__ uint32_t s_kd[SEL_WCAP];
   __shared__ long long s_id[SEL_WCAP];
+  __shared__ int s_m, s_ns;
   const int qi = blockIdx.x;
   if (redo_in && !redo_in[qi]) { if (threadIdx.x == 0) flags[qi] = 0; return; }  // finished by the warp kernel
   float* qs = reinterpret_cast<float*>(smem);
@@ -1113,24 +794,27 @@ tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows
     const int r = threadIdx.x + j * SEL_THREADS;
     key[j] = r < nrows ? f2ord(dense[(size_t)qi * ld + r]) : 0xFFFFFFFFu;
   }
-  const uint32_t kth = reg_kth_key<KPT>(key, k, S);  // barriers inside: qs is visible afterwards
+  const uint32_t kth = block_kth_key_any(k, S, [&](auto f) {  // barriers inside: qs is visible afterwards
+#pragma unroll
+    for (int j = 0; j < KPT; ++j) if (key[j] != 0xFFFFFFFFu) f(key[j]);
+  });
   const float a_k = ord2f(kth);
   const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true);
   const uint32_t thr_hi = f2ord(__fadd_ru(a_k, two_eps));
   const bool set_mode = out_raw == nullptr && S.c_le == k;
   const uint32_t thr_lo = f2ord(__fsub_rd(a_k, two_eps));
-  if (threadIdx.x == 0) { S.m = 0; S.ns = 0; }
+  if (threadIdx.x == 0) { s_m = 0; s_ns = 0; }
   __syncthreads();
 #pragma unroll
   for (int j = 0; j < KPT; ++j) {
     if (key[j] > thr_hi) continue;  // empty slots (0xFFFFFFFF) drop out here too
     const int r = threadIdx.x + j * SEL_THREADS;
-    if (set_mode && key[j] <= thr_lo) out_probes[(size_t)qi * k + atomicAdd(&S.ns, 1)] = r + id_offset;
-    else { const int pos = atomicAdd(&S.m, 1); if (pos < SEL_WCAP) s_rows[pos] = r; }
+    if (set_mode && key[j] <= thr_lo) out_probes[(size_t)qi * k + atomicAdd(&s_ns, 1)] = r + id_offset;
+    else { const int pos = atomicAdd(&s_m, 1); if (pos < SEL_WCAP) s_rows[pos] = r; }
   }
   __syncthreads();
-  const int m = S.m, ns = S.ns;
-  if (m > SEL_WCAP) {  // degenerate score row (many near-equal scores): redo on the one-sort path
+  const int m = s_m, ns = s_ns;
+  if (m > SEL_WCAP) {  // degenerate score row (many near-equal scores): redo on the streaming kernel
     if (threadIdx.x == 0) flags[qi] = 1;
     return;
   }
@@ -1165,7 +849,7 @@ tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows
 // Coarse finish for small centroid tables (nrows <= 32 * KPT <= 1024): one 128-thread CTA per query.  Warp 0 holds the
 // score row in registers and does the selection (same full / set modes and +-2 eps rule as tc_coarse_select_kernel) with
 // shuffles / ballots; all 32 quads then re-score the window rows together; a rank sort orders them.  Three block
-// barriers.  Queries whose re-score window exceeds HC_MAXW rows set flags[qi] = 1 and go to the block kernels.
+// barriers.  Queries whose re-score window exceeds HC_MAXW rows set flags[qi] = 1 and go to tc_coarse_select_kernel.
 constexpr int HC_THREADS = 128;
 constexpr int HC_MAXW = 256;
 template <bool L2, int KPT>
@@ -1214,7 +898,7 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
   }
   __syncthreads();
   const int m = s_m, ns = s_ns;
-  if (m > HC_MAXW) { if (threadIdx.x == 0) flags[qi] = 1; return; }  // (the block kernel rewrites the whole output row)
+  if (m > HC_MAXW) { if (threadIdx.x == 0) flags[qi] = 1; return; }  // (tc_coarse_select_kernel rewrites the whole output row)
   const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
   const bool vec = (d & 3) == 0;
   const float* qrow = q + (size_t)qi * d;
@@ -1227,28 +911,85 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
   }
   __syncthreads();
   const int need = k - ns;  // slots still open (set mode), all k otherwise
-  for (int e = threadIdx.x; e < m; e += HC_THREADS) {
-    const uint32_t d0 = s_kd[e];
-    const long long i0 = s_id[e];
-    int rank = 0;
-    for (int j = 0; j < m; ++j) {
-      const uint32_t dj = s_kd[j];
-      const long long ij = s_id[j];
-      rank += (key_less(dj, ij, d0, i0) || (dj == d0 && ij == i0 && j < e)) ? 1 : 0;
-    }
+  block_rank_sort(s_kd, s_id, m, [&](int rank, int e) {
     if (rank < need) {
-      out_probes[(size_t)qi * k + ns + rank] = i0 + id_offset;
+      out_probes[(size_t)qi * k + ns + rank] = s_id[e] + id_offset;
       if (out_raw) {
-        const float v = ord2f(d0);
+        const float v = ord2f(s_kd[e]);
         out_raw[(size_t)qi * k + rank] = api_scores ? v : (L2 ? v : -v);
       }
     }
-  }
+  });
   for (int i = m + threadIdx.x; i < need; i += HC_THREADS) {
     out_probes[(size_t)qi * k + ns + i] = -1;
     if (out_raw) out_raw[(size_t)qi * k + i] = 0.f;
   }
   if (threadIdx.x == 0) flags[qi] = 0;
+}
+
+// Streaming window select, the fallback of both finishes (no limit on the number of keys or of window rows).  key_at(i),
+// i < n, is (ord(approximate score) << 32 | row); id_of(row) is the id a row is reported under.  Pass 1: A_k = k-th
+// smallest approximate score (+inf when n < k).  Pass 2: every row with score <= A_k + two_eps re-scored exactly in the
+// reference order, FIN_SEG rows at a time, into `sel`, which ends holding the exact top-k by (distance, id).
+// smem: tc_stream_smem(d, pool_cap) bytes.  Returns A_k + two_eps.  All SCAN_THREADS threads call.
+static size_t tc_stream_smem(int d, int pool_cap) { return ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_SEG * 4 + BlockSelect::smem_bytes(pool_cap); }
+
+template <bool L2, class KeyAt, class IdOf>
+__device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned char* smem, int pool_cap, const float* __restrict__ qrow,
+                                                  const float* __restrict__ vecs, int d, int n, int k, float two_eps, KeyAt key_at,
+                                                  IdOf id_of) {
+  __shared__ int s_m;
+  float* qs = reinterpret_cast<float*>(smem);
+  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
+  int* s_rows = reinterpret_cast<int*>(smem + qbytes);  // [FIN_SEG]
+  unsigned char* pool = smem + qbytes + (size_t)FIN_SEG * 4;
+  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = qrow[i];
+  sel.init(pool, pool_cap, k);
+  // pass 1: k-th smallest approximate score
+  for (int base = 0; base < n; base += blockDim.x) {
+    sel.maybe_prune(blockDim.x);
+    const int i = base + threadIdx.x;
+    if (i < n) {
+      const unsigned long long e = key_at(i);
+      const uint32_t key = (uint32_t)(e >> 32);
+      const long long row = (long long)(e & 0xffffffffull);
+      if (sel.passes(key, row)) sel.push(key, row);
+    }
+  }
+  sel.prune();
+  const float a_k = *sel.count >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
+  __syncthreads();
+  const float window = a_k + two_eps;  // +inf when fewer than k rows
+  // pass 2: exact distances (reference AVX-512 order) of every row inside the window
+  sel.init(pool, pool_cap, k);
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
+  const bool vec = (d & 3) == 0;
+  for (int seg = 0; seg < n; seg += FIN_SEG) {
+    if (threadIdx.x == 0) s_m = 0;
+    __syncthreads();
+    const int e1 = min(n, seg + FIN_SEG);
+    for (int i = seg + threadIdx.x; i < e1; i += blockDim.x) {
+      const unsigned long long e = key_at(i);
+      if (ord2f((uint32_t)(e >> 32)) <= window) s_rows[atomicAdd(&s_m, 1)] = (int)(uint32_t)(e & 0xffffffffull);
+    }
+    __syncthreads();
+    const int m = s_m;
+    for (int base = 0; base < m; base += SCAN_QUADS) {
+      sel.maybe_prune(SCAN_QUADS);
+      const int i = base + quad;
+      const bool valid = i < m;
+      const uint32_t row = (uint32_t)s_rows[valid ? i : 0];
+      const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
+      if (valid && t == 0) {
+        const uint32_t key = f2ord(L2 ? v : -v);
+        const long long id = id_of(row);
+        if (sel.passes(key, id)) sel.push(key, id);
+      }
+    }
+    __syncthreads();
+  }
+  sel.prune();
+  return window;
 }
 
 template <bool L2>
@@ -1258,66 +999,16 @@ tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restri
                 const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k, int pool_cap,
                 float* out_dist, long long* out_ids, int* flags, const int* redo) {
   extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int s_m;
   const int qi = blockIdx.x;
-  if (redo && !redo[qi]) return;
-  float* qs = reinterpret_cast<float*>(smem);
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
-  int* s_rows = reinterpret_cast<int*>(smem + qbytes);  // [FIN_SEG]
-  unsigned char* pool = smem + qbytes + (size_t)FIN_SEG * 4;
-  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = q[(size_t)qi * d + i];
+  if (redo && !redo[qi]) return;  // finished by the hybrid kernel
   const int total = cand_cnt[qi];
-  const int n = min(total, cap);
   const unsigned long long* c = cand + (size_t)qi * cap;
   BlockSelect sel;
-  sel.init(pool, pool_cap, k);
-  // pass 1: k-th smallest approximate score among the captured rows
-  for (int base = 0; base < n; base += blockDim.x) {
-    sel.maybe_prune(blockDim.x);
-    const int i = base + threadIdx.x;
-    if (i < n) {
-      const unsigned long long e = c[i];
-      const uint32_t key = (uint32_t)(e >> 32);
-      const long long row = (long long)(e & 0xffffffffull);
-      if (sel.passes(key, row)) sel.push(key, row);
-    }
-  }
-  sel.prune();
-  const int have1 = *sel.count;
-  const float a_k = have1 >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
-  __syncthreads();
-  const float window = a_k + 2.f * tc_eps(L2, qnorm[qi], max_norm, d, false);  // +inf when fewer than k rows were captured
+  const float window = tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k,
+                                            2.f * tc_eps(L2, qnorm[qi], max_norm, d, false), [&](int i) { return c[i]; },
+                                            [&](uint32_t row) { return ids[row]; });
   const float tq = tau[qi];
   const bool certified = (total <= cap) && (tq == TC_INF || window <= tq);
-  // pass 2: exact distances (reference AVX-512 order) of every captured row inside the window, FIN_SEG at a time
-  sel.init(pool, pool_cap, k);
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  const bool vec = (d & 3) == 0;
-  for (int seg = 0; seg < n; seg += FIN_SEG) {
-    if (threadIdx.x == 0) s_m = 0;
-    __syncthreads();
-    const int e1 = min(n, seg + FIN_SEG);
-    for (int i = seg + threadIdx.x; i < e1; i += blockDim.x) {
-      const unsigned long long e = c[i];
-      if (ord2f((uint32_t)(e >> 32)) <= window) s_rows[atomicAdd(&s_m, 1)] = (int)(uint32_t)(e & 0xffffffffull);
-    }
-    __syncthreads();
-    const int m = s_m;
-    for (int base = 0; base < m; base += SCAN_QUADS) {
-      sel.maybe_prune(SCAN_QUADS);
-      const int i = base + quad;
-      const bool valid = i < m;
-      const long long row = (long long)(uint32_t)s_rows[valid ? i : 0];
-      const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
-      if (valid && t == 0) {
-        const uint32_t key = f2ord(L2 ? v : -v);
-        const long long id = ids[row];
-        if (sel.passes(key, id)) sel.push(key, id);
-      }
-    }
-    __syncthreads();
-  }
-  sel.prune();
   const int have = *sel.count;
   for (int i = threadIdx.x; i < k; i += blockDim.x) {
     float api = 0.f;
@@ -1339,55 +1030,15 @@ template <bool L2>
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_coarse_final_kernel(const float* __restrict__ dense, long long ld, int nrows, const float* __restrict__ qnorm, float max_norm,
                        const float* __restrict__ q, const float* __restrict__ vecs, int d, int k, int pool_cap,
-                       long long id_offset, int api_scores, long long* out_probes, float* out_raw) {
+                       long long id_offset, int api_scores, long long* out_probes, float* out_raw, const int* redo) {
   extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int s_m;
   const int qi = blockIdx.x;
-  float* qs = reinterpret_cast<float*>(smem);
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
-  int* s_rows = reinterpret_cast<int*>(smem + qbytes);
-  unsigned char* pool = smem + qbytes + (size_t)FIN_SEG * 4;
-  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = q[(size_t)qi * d + i];
+  if (redo && !redo[qi]) return;  // finished by the register select
   const float* row_scores = dense + (size_t)qi * ld;
   BlockSelect sel;
-  sel.init(pool, pool_cap, k);
-  for (int base = 0; base < nrows; base += blockDim.x) {
-    sel.maybe_prune(blockDim.x);
-    const int i = base + threadIdx.x;
-    if (i < nrows) {
-      const float v = row_scores[i];
-      if (v < TC_INF) { const uint32_t key = f2ord(v); if (sel.passes(key, i)) sel.push(key, i); }
-    }
-  }
-  sel.prune();
-  const float a_k = *sel.count >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
-  __syncthreads();
-  const float window = a_k + 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true);
-  sel.init(pool, pool_cap, k);
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  const bool vec = (d & 3) == 0;
-  for (int seg = 0; seg < nrows; seg += FIN_SEG) {
-    if (threadIdx.x == 0) s_m = 0;
-    __syncthreads();
-    const int e1 = min(nrows, seg + FIN_SEG);
-    for (int i = seg + threadIdx.x; i < e1; i += blockDim.x)
-      if (row_scores[i] <= window) s_rows[atomicAdd(&s_m, 1)] = i;
-    __syncthreads();
-    const int m = s_m;
-    for (int base = 0; base < m; base += SCAN_QUADS) {
-      sel.maybe_prune(SCAN_QUADS);
-      const int i = base + quad;
-      const bool valid = i < m;
-      const int row = s_rows[valid ? i : 0];
-      const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
-      if (valid && t == 0) {
-        const uint32_t key = f2ord(L2 ? v : -v);
-        if (sel.passes(key, row)) sel.push(key, row);
-      }
-    }
-    __syncthreads();
-  }
-  sel.prune();
+  tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, nrows, k, 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true),
+                       [&](int i) { return ((unsigned long long)f2ord(row_scores[i]) << 32) | (unsigned)i; },
+                       [](uint32_t row) { return (long long)row; });
   const int have = *sel.count;
   for (int i = threadIdx.x; i < k; i += blockDim.x) {
     out_probes[(size_t)qi * k + i] = i < have ? sel.kid[i] + id_offset : -1;
@@ -1489,7 +1140,6 @@ static int tc_cand_cap(int k) { return std::min(16384, std::max(8192, next_pow2(
 // Per-device one-time setup: cudaFuncSetAttribute applies to the CURRENT device only, and one process may hold indexes
 // on several GPUs (b200vs_params.device), so the opt-in shared-memory limits are raised once per device ordinal.
 constexpr int TC_MAX_DEVICES = 64;
-constexpr int TC_FAST_SMEM = 200 * 1024;  // opt-in limit of the one-sort finish kernels
 static std::mutex g_tc_init_mu;
 static int g_dev_sms[TC_MAX_DEVICES] = {0};
 static int tc_init(int device) {
@@ -1498,15 +1148,10 @@ static int tc_init(int device) {
   if (g_dev_sms[device]) return g_dev_sms[device];
   const int sms = device_sm_count(device);
   B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_tau_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_fast_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_FAST_SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_fast_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_FAST_SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_fast_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_FAST_SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_fast_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_FAST_SMEM));
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   g_dev_sms[device] = sms;  // only after every attribute call succeeded
@@ -1600,14 +1245,7 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   auto& S = ix->scratch;
   ix->phase(IndexBase::PH_PLAN, s);
   TcPlan P = tc_prepare(ix, v, nq, q, probes, nprobe, s);
-  // rows sampled per span for the thresholds: 32 (one TMA box, capture threshold = tau) by default.
-  // B200VS_SAMPLE_ROWS=128 samples the whole first tile of each span and captures under tau + 2 eps: certified by
-  // construction (no fallback except on overflow) at the price of a longer sample / threshold pass — the setting for data
-  // whose thin samples fail certification often.  Measured on the benchmark (list-sharded over 4 GPUs as well) the thin
-  // sample wins: the finish kernel is bound by per-query latency, not by the number of captured rows.
-  const char* env_srows = getenv("B200VS_SAMPLE_ROWS");
-  const int srows = env_srows && atoi(env_srows) == TC_BM && P.sbound * TC_NQT * TC_BM * 4 <= (4LL << 30) ? TC_BM : TC_SAMPLE;
-  float* sample = S.alloc<float>((size_t)P.sbound * TC_NQT * srows);
+  float* sample = S.alloc<float>((size_t)P.sbound * TC_NQT * TC_SAMPLE);
   float* tau = S.alloc<float>(nq);
   unsigned long long* cand = S.alloc<unsigned long long>((size_t)nq * cap);
   int* cand_cnt = S.alloc<int>(nq);
@@ -1617,11 +1255,10 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   B200VS_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)nq * 4, s));
 
   TcParams p = tc_params(v, P, d, l2);
-  p.sample = sample; p.sample_rows = srows; p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
+  p.sample = sample; p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
   p.filt.has_range = sc.has_range; p.filt.negate = sc.negate; p.filt.rmin = sc.rmin; p.filt.rmax = sc.rmax;
   p.filt.sorted_ids = sc.sorted_ids_dev; p.filt.n_ids = sc.n_ids;
   const int pool = select_pool_cap(k, SCAN_THREADS);
-  const size_t sel_smem = BlockSelect::smem_bytes(pool);
 
   // 1) sample pass -> per-query capture thresholds
   p.mode = 0; p.work_counter = P.work;
@@ -1629,13 +1266,9 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   tc_launch(P, p, P.sbound, s);
   ix->phase(IndexBase::PH_TAU, s);
   int* redo = S.alloc<int>(nq);
-  const size_t tau_smem = (size_t)TAU_PL * 8 + std::max(sel_smem, (size_t)TAU_SORT * 8);
-  if (srows == TC_SAMPLE) {  // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
-    tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qnorm, v.max_norm, d, cap, tau, redo);
-    tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, tau_smem, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, srows, k, pool, l2 ? 1 : 0, P.qnorm, v.max_norm, d, 0, cap, tau, redo);
-  } else {
-    tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, tau_smem, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, srows, k, pool, l2 ? 1 : 0, P.qnorm, v.max_norm, d, 1, cap, tau, nullptr);
-  }
+  // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
+  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qnorm, v.max_norm, d, cap, tau, redo);
+  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qnorm, v.max_norm, d, cap, tau, redo);
   // 2) capture pass: stream every probed list chunk once, keep rows under the threshold
   p.mode = 1; p.work_counter = P.work + 1;
   ix->phase(IndexBase::PH_CAPTURE, s);
@@ -1646,26 +1279,17 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   }
   // 3) window select + exact rerank + certification
   ix->phase(IndexBase::PH_FINAL, s);
-  const size_t fast_smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_MAXW * 16 + (size_t)cap * 8;
   const int* fin_redo = nullptr;
-  const int hf_pitch = d * 4 + 16;  // staged row pitch: 16-byte aligned, rows land on different banks
-  static const bool hf_direct = !(getenv("B200VS_FINAL_STAGED") && atoi(getenv("B200VS_FINAL_STAGED")) != 0);
-  const int hf_rows = hf_direct ? 0 : std::min(32, std::max(HF_ROW_BYTES, 2 * hf_pitch) / hf_pitch - 1);
-  const size_t hsm = (size_t)(hf_rows + 1) * hf_pitch;
-  if (2 * k <= HF_MAXW && hsm <= 96 * 1024) {  // warp select + block re-score; the block kernels below only redo queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, hf_rows, hf_pitch, out_dist, out_ids, flags, redo);
-    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, hf_rows, hf_pitch, out_dist, out_ids, flags, redo);
+  const size_t hsm = (size_t)d * 4;  // the query row
+  if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
+    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, redo);
+    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, redo);
     fin_redo = redo;
     ix->launch_count(1);
   }
-  if (fast_smem <= (size_t)TC_FAST_SMEM) {  // one 64-bit sort of the captured rows + a small exact sort
-    if (l2) tc_final_fast_kernel<true><<<(unsigned)nq, SCAN_THREADS, fast_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, fin_redo);
-    else tc_final_fast_kernel<false><<<(unsigned)nq, SCAN_THREADS, fast_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, fin_redo);
-  } else {
-    const size_t fin_smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_SEG * 4 + sel_smem;
-    if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
-    else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
-  }
+  const size_t fin_smem = tc_stream_smem(d, pool);
+  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
+  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
   tc_compact_flags_kernel<<<1, 1024, 0, s>>>(flags, (int)nq, qmap, qcount);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
@@ -1751,11 +1375,13 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   tc_scan_kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(a_hi, a_hi, b16, b32, b64, b128, a_lo, l16, l32, l64, l128, p);
   B200VS_CUDA(cudaGetLastError());
   ix->phase(IndexBase::PH_COARSE_FINAL, s);
-  const int maxw = std::max(2, next_pow2(nrows));
-  const size_t fast_smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)maxw * 24;
-  if (nrows <= COARSE_FAST && nprobe <= nrows && fast_smem <= (size_t)TC_FAST_SMEM) {
+  const int pool = select_pool_cap(nprobe, SCAN_THREADS);
+  const size_t fin_smem = tc_stream_smem(d, pool);
+  if (fin_smem > 160 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "coarse quantiser: dimension / nprobe too large for one SM's shared memory");
+  const int* fin_redo = nullptr;
+  if (nrows <= SEL_MAX_ROWS && nprobe <= nrows) {
     // warp-select / block-re-score kernel for small tables, then the register-resident block select (8 CTAs per SM) for larger tables
-    // and for the queries the warp kernel flagged, then the one-sort kernel for what is still flagged (normally none)
+    // and for the queries the warp kernel flagged, then the streaming kernel for what is still flagged (normally none)
     int* redo0 = S.alloc<int>(nq);
     int* redo = S.alloc<int>(nq);
     const size_t qsm = ((size_t)d * 4 + 15) / 16 * 16;
@@ -1776,16 +1402,11 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
     else if (kpt <= 16) { if (l2) B200VS_SEL(true, 16); else B200VS_SEL(false, 16); }
     else { if (l2) B200VS_SEL(true, 32); else B200VS_SEL(false, 32); }
 #undef B200VS_SEL
-    if (l2) tc_coarse_final_fast_kernel<true><<<(unsigned)nq, FIN_THREADS, fast_smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, maxw, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, redo);
-    else tc_coarse_final_fast_kernel<false><<<(unsigned)nq, FIN_THREADS, fast_smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, maxw, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, redo);
+    fin_redo = redo;
     ix->launch_count(1);
-  } else {
-    const int pool = select_pool_cap(nprobe, SCAN_THREADS);
-    const size_t smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_SEG * 4 + BlockSelect::smem_bytes(pool);
-    if (smem > 160 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "coarse quantiser: dimension / nprobe too large for one SM's shared memory");
-    if (l2) tc_coarse_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, pool, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw);
-    else tc_coarse_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, pool, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw);
   }
+  if (l2) tc_coarse_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, pool, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, fin_redo);
+  else tc_coarse_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, pool, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, fin_redo);
   B200VS_CUDA(cudaGetLastError());
   ix->phase(IndexBase::PH_OTHER, s);
   ix->launch_count(4);

@@ -55,8 +55,7 @@ struct TcParams {
   int* work_counter;        // dynamic scheduler: next work index
   const int* pair_query;    // [npairs] query index of each gathered row
   int mode;                 // 0 = sample pass, 1 = capture pass, 2 = dense pass (every score written)
-  float* sample;            // mode 0: [sample_items, TC_NQT, sample_rows]
-  int sample_rows;          // TC_SAMPLE (32-row box) or TC_BM (the whole first tile of each span)
+  float* sample;            // mode 0: [sample_items, TC_NQT, TC_SAMPLE]
   const float* tau;         // mode 1: [nq] capture threshold on the approximate score
   unsigned long long* cand; // mode 1: [nq, cap]  (ord(score) << 32 | arena row)
   int* cand_cnt;            // mode 1: [nq]

@@ -7,7 +7,7 @@
 //                      the warp's registers or a small staged array (<= ~1024 keys: threshold and coarse kernels).
 //   block_kth_key_any  all threads of the CTA feed one shared histogram.  Right as soon as a CTA owns the query anyway: a lone
 //                      warp executes dependent selection code at ~25 ns per instruction (nothing hides its latencies).
-// Each kernel uses the form that measured faster (DESIGN.md 4.2, profiles/round2/README.md).
+// Each kernel uses the form that measured faster (DESIGN.md 4.2).
 #pragma once
 #include "common.cuh"
 

@@ -4,8 +4,8 @@ The tile scan only SELECTS rows with approximate scores a = e + noise, |noise| <
 returned top-k must equal the exact scan's.  This file checks the selection rules themselves, independent of any kernel:
 
   single rank      tau = k-th smallest SAMPLED approximate score; capture a <= T; window a <= A_k + 2 eps (A_k = k-th
-                   smallest captured); certified iff no overflow and A_k + 2 eps <= T.  T = tau (thin samples) or
-                   T = tau + 2 eps (dense samples: always certified).
+                   smallest captured); certified iff no overflow and A_k + 2 eps <= T.  T = tau, or T = tau + 2 eps
+                   (the margin branch of tc_tau_with_margin: always certified).
   coarse set mode  rows with a <= A_k - 2 eps are certainly in the exact top-k, rows with a > A_k + 2 eps certainly not.
   list-sharded     every rank captures under the MIN over ranks of tau; a query is certified when ANY rank certifies
                    (that rank's A_k bounds the global one from above); each rank returns the exact top-k of its own

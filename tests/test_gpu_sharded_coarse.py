@@ -120,10 +120,14 @@ def test_coarse_split_by_queries_equals_plain_search():
 
 
 @pytest.mark.parametrize("metric", [b200vs.L2, b200vs.IP])
-@pytest.mark.parametrize("nlist", [2048, 4096, 8192, 10000])
-def test_coarse_large_tables_match_oracle(metric, nlist):
+@pytest.mark.parametrize("nlist,dups", [(2048, 0), (4096, 0), (8192, 0), (10000, 0), (2048, 600), (1024, 300)],
+                         ids=["2048", "4096", "8192", "10000", "2048-dup600", "1024-dup300"])
+def test_coarse_large_tables_match_oracle(metric, nlist, dups):
     """Every register-select width (8 / 16 / 32 keys per thread) and the generic path above 8192 centroids, on a
-    trained state loaded from outside (random centroids, duplicates included so exact ties occur)."""
+    trained state loaded from outside (random centroids, duplicates included so exact ties occur).  dups > 0 repeats one
+    centroid that often, with a query on it: more rows tie at the k-th score than the re-score window holds (512 rows in
+    the register select used at 2048 centroids, 256 in the small-table kernel used at 1024), so the next finish kernel
+    takes that query."""
     require_gpu()
     import torch
     d, nq, nprobe = 64, 96, 48
@@ -131,10 +135,14 @@ def test_coarse_large_tables_match_oracle(metric, nlist):
     cent = rng.random((nlist, d), dtype=np.float32)
     cent[5] = cent[4]
     cent[nlist - 1] = cent[7]
+    if dups:
+        cent[8:8 + dups] = 1.0  # the nearest row for L2 and the largest inner product for IP
     ix = b200vs.Index(b200vs.IVF_FLAT, metric, d, nlist=nlist)
     ix.set_trained_state(b200vs.ivf_state_blob(cent, metric))
     xq = rng.random((nq, d), dtype=np.float32)
     xq[0] = cent[4]
+    if dups:
+        xq[1] = cent[8]
     q = torch.from_numpy(xq).cuda()
     sc = torch.empty((nq, nprobe), dtype=torch.float32, device="cuda")
     pl = torch.empty((nq, nprobe), dtype=torch.int64, device="cuda")
