@@ -355,6 +355,17 @@ struct FlatIndex : IndexBase {
     run_scan(this, job(sc), nq, q, k, od, nullptr, oi, nullptr, s);
   }
 
+  void debug_tc_scores(int64_t nq, const float* xq, bool split, float* out_scores, float* out_eps, cudaStream_t s) override {
+    if ((double)nq * (double)rows * 4 > (double)(1LL << 30)) fail(B200VS_EILLEGAL_PARAMETERS, "score matrix larger than 1 GiB");
+    const float* q = prepare_queries(nq, xq, s);
+    float* ds = scratch.alloc<float>((size_t)std::max<int64_t>(nq * rows, 1));
+    float* de = scratch.alloc<float>(nq);
+    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, split, ds, de, s);
+    if (rows > 0) B200VS_CUDA(cudaMemcpyAsync(out_scores, ds, (size_t)nq * rows * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(out_eps, de, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+  }
+
   // VectorIndexFlat::RangeSearch, vector_index_flat.cc:267-323: radius -> 1 - radius for IP / cosine (:282-285);
   // faiss range_search keeps L2 dis < radius, IP ip > radius.
   void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,

@@ -1338,42 +1338,55 @@ bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe) 
   return true;
 }
 
-// Coarse quantiser: ONE dense launch of the tile kernel in split mode — error-compensated TF32, the three products
-// hi*hi + lo*hi + hi*lo accumulate into the same register accumulators (the lo operands ride in the next ring stage).  The
-// operand error drops to 2^-19 relative, so the exact re-score window stays a few dozen rows even when all centroid
-// distances are nearly equal (uniform high-dimensional data); what remains of eps is the FP32 accumulation term.
-void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int nprobe, long long* out_probes,
-               float* out_raw, cudaStream_t s) {
+// One dense launch of the tile kernel (mode 2): dense[q * v.arena_rows + r] = approximate score of query q against row r
+// (L2: ||x||^2 - 2 <q, x>; IP: -<q, x>; tombstoned rows +inf).  qb_lo == nullptr: single-pass TF32, qb holds the RN-rounded
+// queries and the tensor core truncates the rows a_hi.  Otherwise the error-compensated split pass: the three products
+// hi*hi + lo*hi + hi*lo accumulate into the same register accumulators (the lo operands ride in the next ring stage).
+static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* qb, const float* qb_lo, const float* a_hi,
+                          const float* a_lo, float* dense, cudaStream_t s) {
   const int num_sms = tc_init(ix->device);
   const int d = ix->dim;
   const int nrows = (int)v.arena_rows;
+  const bool split = qb_lo != nullptr;
   auto& S = ix->scratch;
-  float* qhi = S.alloc<float>((size_t)nq * d);
-  float* qlo = S.alloc<float>((size_t)nq * d);
-  float* qnorm = S.alloc<float>(nq);
   const int chunk = nrows <= 16384 ? TC_BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
   const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, TC_NQT));
   TcItem* items = S.alloc<TcItem>(nitems);
   int* totals = S.alloc<int>(4);
   int* work = S.alloc<int>(4);
-  float* dense = S.alloc<float>((size_t)nq * nrows);
-  ix->phase(IndexBase::PH_COARSE_PREP, s);
   B200VS_CUDA(cudaMemsetAsync(work, 0, 16, s));
-  tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qhi, qlo, qnorm);
   tc_coarse_items_kernel<<<(unsigned)cdiv(nitems, 128), 128, 0, s>>>(nrows, (int)nq, chunk, items, totals);
   TcPlan P;
   memset(&P, 0, sizeof(P));
   P.items = items; P.totals = totals;
   TcParams p = tc_params(v, P, d, l2);
   p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.pair_query = nullptr;
-  const CUtensorMap a_hi = make_tmap(v.vecs_hi, nrows, d, TC_BM), a_lo = make_tmap(v.vecs_lo, nrows, d, TC_BM);
-  const CUtensorMap b16 = make_tmap(qhi, nq, d, 16), b32 = make_tmap(qhi, nq, d, 32), b64 = make_tmap(qhi, nq, d, 64), b128 = make_tmap(qhi, nq, d, 128);
-  const CUtensorMap l16 = make_tmap(qlo, nq, d, 16), l32 = make_tmap(qlo, nq, d, 32), l64 = make_tmap(qlo, nq, d, 64), l128 = make_tmap(qlo, nq, d, 128);
+  const CUtensorMap ta = make_tmap(a_hi, nrows, d, TC_BM), ta_lo = split ? make_tmap(a_lo, nrows, d, TC_BM) : ta;
+  const CUtensorMap b16 = make_tmap(qb, nq, d, 16), b32 = make_tmap(qb, nq, d, 32), b64 = make_tmap(qb, nq, d, 64), b128 = make_tmap(qb, nq, d, 128);
+  const CUtensorMap l16 = split ? make_tmap(qb_lo, nq, d, 16) : b16, l32 = split ? make_tmap(qb_lo, nq, d, 32) : b32;
+  const CUtensorMap l64 = split ? make_tmap(qb_lo, nq, d, 64) : b64, l128 = split ? make_tmap(qb_lo, nq, d, 128) : b128;
   const int grid = (int)std::min<int64_t>(num_sms, std::max(1, nitems));
-  p.work_counter = work; p.split = 1; p.dense_accum = 0; p.add_norm = 1;
+  p.work_counter = work; p.split = split ? 1 : 0; p.dense_accum = 0; p.add_norm = 1;
   ix->phase(IndexBase::PH_COARSE_SCAN, s);
-  tc_scan_kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(a_hi, a_hi, b16, b32, b64, b128, a_lo, l16, l32, l64, l128, p);
+  tc_scan_kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
   B200VS_CUDA(cudaGetLastError());
+}
+
+// Coarse quantiser: ONE dense launch of the tile kernel in split mode (error-compensated TF32).  The operand error drops
+// to 2^-19 relative, so the exact re-score window stays a few dozen rows even when all centroid distances are nearly
+// equal (uniform high-dimensional data); what remains of eps is the FP32 accumulation term.
+void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int nprobe, long long* out_probes,
+               float* out_raw, cudaStream_t s) {
+  const int d = ix->dim;
+  const int nrows = (int)v.arena_rows;
+  auto& S = ix->scratch;
+  float* qhi = S.alloc<float>((size_t)nq * d);
+  float* qlo = S.alloc<float>((size_t)nq * d);
+  float* qnorm = S.alloc<float>(nq);
+  float* dense = S.alloc<float>((size_t)nq * nrows);
+  ix->phase(IndexBase::PH_COARSE_PREP, s);
+  tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qhi, qlo, qnorm);
+  tc_dense_scan(ix, v, l2, nq, qhi, qlo, v.vecs_hi, v.vecs_lo, dense, s);
   ix->phase(IndexBase::PH_COARSE_FINAL, s);
   const int pool = select_pool_cap(nprobe, SCAN_THREADS);
   const size_t fin_smem = tc_stream_smem(d, pool);
@@ -1410,6 +1423,35 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   B200VS_CUDA(cudaGetLastError());
   ix->phase(IndexBase::PH_OTHER, s);
   ix->launch_count(4);
+}
+
+static __global__ void tc_eps_kernel(const float* __restrict__ qnorm, long long nq, int l2, float max_norm, int d, int split, float* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nq) out[i] = tc_eps(l2 != 0, qnorm[i], max_norm, d, split != 0);
+}
+
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, bool split, float* out_scores,
+                     float* out_eps, cudaStream_t s) {
+  const int d = ix->dim;
+  auto& S = ix->scratch;
+  float* qb = S.alloc<float>((size_t)nq * d);
+  float* qb_lo = split ? S.alloc<float>((size_t)nq * d) : nullptr;
+  float* qnorm = S.alloc<float>(nq);
+  if (split) tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qb, qb_lo, qnorm);
+  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qb, qnorm);
+  B200VS_CUDA(cudaGetLastError());
+  if (v.arena_rows > 0) {
+    const float *a_hi = v.vecs, *a_lo = nullptr;
+    if (split) {  // the same row split the IVF coarse quantiser keeps for its centroids
+      float* hi = S.alloc<float>((size_t)v.arena_rows * d);
+      float* lo = S.alloc<float>((size_t)v.arena_rows * d);
+      launch_split_rows(v.vecs, v.arena_rows, d, hi, lo, s);
+      a_hi = hi; a_lo = lo;
+    }
+    tc_dense_scan(ix, v, l2, nq, qb, qb_lo, a_hi, a_lo, out_scores, s);
+  }
+  tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qnorm, nq, l2 ? 1 : 0, v.max_norm, d, split ? 1 : 0, out_eps);
+  B200VS_CUDA(cudaGetLastError());
 }
 
 }  // namespace b200vs

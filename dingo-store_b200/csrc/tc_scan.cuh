@@ -104,6 +104,12 @@ bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe);
 void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int nprobe, long long* out_probes,
                float* out_raw, cudaStream_t s);
 
+// Diagnostics (b200vs_debug_tc_scores; no search path calls it): the tile kernel's dense approximate scores of q (device,
+// prepared) against every arena row, out_scores [nq, v.arena_rows], and the tc_eps() the finish kernels use, out_eps [nq].
+// split = false: list-scan arithmetic; true: the coarse pass's hi / lo arithmetic.
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, bool split, float* out_scores,
+                     float* out_eps, cudaStream_t s);
+
 float device_max_norm(IndexBase* ix, const float* norms_sq, int64_t n, cudaStream_t s);  // sqrt(max ||x||^2)
 void launch_row_norms(const float* x, int64_t n, int d, float* out, cudaStream_t s);     // out[i] = <x_i, x_i>
 void launch_split_rows(const float* x, int64_t n, int d, float* hi, float* lo, cudaStream_t s);

@@ -28,7 +28,7 @@ ABI_SYMBOLS = [
     "b200vs_add_with_ids_device", "b200vs_assign_device", "b200vs_reserve_lists", "b200vs_export_list", "b200vs_set_coalescing", "b200vs_reconstruct", "b200vs_sub_type",
     "b200vs_shard_unique_id", "b200vs_shard_create", "b200vs_shard_destroy", "b200vs_shard_list_range", "b200vs_shard_train",
     "b200vs_shard_broadcast_state", "b200vs_shard_add", "b200vs_shard_add_device", "b200vs_shard_remove_ids", "b200vs_shard_plan_add_device",
-    "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device",
+    "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
 ]
 
 
@@ -120,6 +120,7 @@ def lib():
     L.b200vs_shard_plan_commit.argtypes = [vp]
     L.b200vs_shard_search.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_shard_search_device.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_debug_tc_scores.argtypes = [vp, i64, vp, i32, vp, vp]
     _lib = L
     return L
 
@@ -290,6 +291,18 @@ class Index:
 
     def set_profiling(self, on):
         _check(self.L.b200vs_set_profiling(self.h, int(bool(on))))
+
+    def tc_scores(self, xq, split=False):
+        """Diagnostics (FLAT): the tile kernel's approximate scores [nq, rows] of every stored row (storage order,
+        tombstoned rows +inf) and the per-query error bound eps [nq] the finish kernels use."""
+        xq = _f32(xq)
+        nq = xq.shape[0]
+        rows = self.get_count() + self.get_deleted_count()
+        S = np.zeros((nq, rows), dtype=np.float32)
+        E = np.zeros(nq, dtype=np.float32)
+        _check(self.L.b200vs_debug_tc_scores(self.h, nq, xq.ctypes.data if xq.size else None, int(bool(split)),
+                                             S.ctypes.data, E.ctypes.data))
+        return S, E
 
     def export_lists(self, nlist, with_vectors=True, code_size=0):
         n = self.get_count()

@@ -248,11 +248,11 @@ int b200vs_scan_finish(b200vs_scan* scan, float* out_dist, int64_t* out_ids);
 void b200vs_scan_abort(b200vs_scan* scan);
 
 /* Counters of the last search on this index: [0] kernels launched, [1] queries served by the tensor-core
- * candidate pass, [2] queries that failed certification and were re-run on the exact path; with profiling on
- * (b200vs_set_profiling) also [3] device time of the dominant list-scan kernel in ns (CUDA events on the launch
- * stream), [4] rows in the distinct probed lists, [5] distinct probed lists, [6] work items of the tile scan,
- * [7] its tensor-core work (128-row tiles x padded query columns).  Profiling synchronises the stream
- * inside the call: never leave it on in a timed run. */
+ * candidate pass; with profiling on (b200vs_set_profiling) also [2] queries of the tensor-core pass that failed
+ * certification and were re-run on the exact path (0 with profiling off), [3] device time of the dominant list-scan
+ * kernel in ns (CUDA events on the launch stream), [4] rows in the distinct probed lists, [5] distinct probed lists,
+ * [6] work items of the tile scan, [7] its tensor-core work (128-row tiles x padded query columns).  Profiling
+ * synchronises the stream inside the call: never leave it on in a timed run. */
 int b200vs_last_search_stats(b200vs_index* idx, int64_t stats[8]);
 /* With profiling on: device milliseconds (CUDA events on the launch stream) the last search spent in each phase of the
  * IVF tile path: [0] coarse prep, [1] coarse scan, [2] coarse select + exact re-score, [3] work planning + query
@@ -261,6 +261,14 @@ int b200vs_last_search_stats(b200vs_index* idx, int64_t stats[8]);
  * the per-shard top-k.  Unused slots are 0. */
 int b200vs_last_phase_times(b200vs_index* idx, float ms[16]);
 int b200vs_set_profiling(b200vs_index* idx, int on);
+
+/* Diagnostics (tests only): the tile kernel's approximate scores of a FLAT index's rows.  split = 0: list-scan
+ * arithmetic (rows truncated by the tensor core, queries rounded to TF32); split = 1: the coarse pass's hi/lo
+ * arithmetic.  xq [nq, dim] RAW (normalised inside for COSINE, as search does); out_scores [nq, rows] with rows =
+ * count + deleted count in storage order (L2: ||x||^2 - 2<q,x>; IP / cosine: -<q,x>; tombstoned rows +inf);
+ * out_eps [nq] = the tc_eps() value the finish kernels use for that query and mode.  Non-FLAT indexes, dim % 4 != 0
+ * and dim < 32: EILLEGAL_PARAMETERS. */
+int b200vs_debug_tc_scores(b200vs_index* idx, int64_t nq, const float* xq, int32_t split, float* out_scores, float* out_eps);
 
 const char* b200vs_last_error(void);
 const char* b200vs_version(void);
