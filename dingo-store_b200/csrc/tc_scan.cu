@@ -285,27 +285,32 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
   if (p.mode == 0) rows = min(rows, TC_SAMPLE);
   const int ntiles = (rows + TC_BM - 1) / TC_BM;
   for (int t = 0; t < ntiles; ++t) {
-    // row metadata first: its loads overlap the MMAs
+    // row metadata first: its loads overlap the MMAs.  The id and norm loads do not depend on each other, and the masks
+    // that read the id are applied after the MMAs, so no warp waits for a global round trip before its first wgmma
     bool inrange[2], valid[2];
-    long long arow[2];
+    long long arow[2], id[2];
     float nrm[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = t * TC_BM + row0 + 8 * h;
       inrange[h] = r < rows;
-      valid[h] = inrange[h];
       arow[h] = list_base + I.row_begin + r;
+      id[h] = -1;
       nrm[h] = 0.f;
-      if (valid[h]) {
-        const long long id = p.ids[arow[h]];
-        valid[h] = id >= 0 && filter_pass(p.filt, id);
-        if (valid[h] && p.l2 && p.add_norm) nrm[h] = p.norms[arow[h]];
+      if (inrange[h]) {
+        id[h] = p.ids[arow[h]];
+        if (p.l2 && p.add_norm) nrm[h] = p.norms[arow[h]];
       }
     }
     float acc[N / 2];
     const bool mma = t * TC_BM + wg * 64 < rows;  // else this warpgroup's half of the last tile holds no item rows
     tc_mma_tile<N>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
     if (!mma) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      valid[h] = inrange[h] && id[h] >= 0 && filter_pass(p.filt, id[h]);
+      if (!valid[h]) nrm[h] = 0.f;
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = t * TC_BM + row0 + 8 * h;  // row within the item

@@ -24,7 +24,7 @@ namespace b200vs {
 constexpr int TC_BM = 128;        // database rows per tile (two warpgroups x wgmma M = 64)
 constexpr int TC_BK = 32;         // floats per K block = 128 B = one swizzle span
 constexpr int TC_NQT = 128;       // queries per work item (wgmma N <= 128): a probed list chunk is re-streamed only beyond 128 queries
-constexpr int TC_STAGES = 5;      // TMA->MMA ring depth (5 x 32 KB; + 24 KB of capture staging: ~40 KB per SM stay free for co-resident small kernels)
+constexpr int TC_STAGES = 6;      // TMA->MMA ring depth (6 x 32 KB; + 24 KB of capture staging: ~220 KB, the bytes in flight bound the HBM rate; DESIGN §4.2)
 constexpr int TC_THREADS = 288;   // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA + scheduler
 constexpr int TC_CHUNK = 512;     // rows per work item (list chunk): fine grain for dynamic load balance
 constexpr int TC_SPAN = 2048;     // one sampled chunk per TC_SPAN rows of a list
