@@ -268,6 +268,9 @@ struct HnswDev {
 
 constexpr int HNSW_THREADS = 128;   // one CTA per query: warp 0 walks the graph, all 32 quads score a hop's neighbours together
 constexpr int HNSW_CAND_SMEM = 1024; // candidate-heap entries kept in shared memory (the levels near the root); deeper ones spill to global
+// Heap form: the visited set admits every node to the candidate heap at most once, so n + 1 entries per query always
+// suffice.  When nq · (n + 1) entries exceed this budget the queries run in chunks of fewer CTAs.
+constexpr size_t HNSW_CAND_POOL_BYTES = 512ull << 20;
 
 struct HeapEnt { float d; unsigned int id; };
 
@@ -321,8 +324,8 @@ __device__ void h_pop(const HeapRef& h, int& n) {
 template <bool L2, bool FAST>
 __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev g, const float* __restrict__ queries, long long nq,
                                                                   int k, int ef, FilterDev filt, unsigned int* visited /*[nq, words]*/,
-                                                                  long long words, HeapEnt* cand_pool, int cand_cap, float* out_dist,
-                                                                  long long* out_ids, int* err_flag) {
+                                                                  long long words, HeapEnt* cand_pool, long long cand_cap, float* out_dist,
+                                                                  long long* out_ids) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ float s_d[32];
   __shared__ unsigned int s_id[32];
@@ -472,7 +475,6 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
   // ---- base layer: searchBaseLayerST ----
   int ntop = 0, ncand = 0;
   float lower = 3.402823466e+38f;
-  bool overflow = false;
   if (warp == 0) {
     const long long lab = g.labels[cur];
     const bool ok = !g.deleted[cur] && filter_pass(filt, lab);
@@ -500,7 +502,7 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
             if (!stop) { node = ce.id; h_pop<false>(cand, ncand); go = 1; }
           }
           go = __shfl_sync(0xffffffffu, go, 0);
-          if (!go || overflow) { m = -1; break; }
+          if (!go) { m = -1; break; }
           node = __shfl_sync(0xffffffffu, node, 0);
           size = (int)g.link0[(size_t)node * (g.maxM0 + 1)];
           c0 = 0;
@@ -536,8 +538,7 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
         for (int i = 0; i < m; ++i) {
           const float dd = s_d[i];
           if (ntop < ef || lower > dd) {
-            if (ncand >= cand_cap) { overflow = true; break; }
-            h_push<false>(cand, ncand, dd, s_id[i]);
+            h_push<false>(cand, ncand, dd, s_id[i]);  // fresh nodes only: ncand <= n < cand_cap
             if ((amask >> i) & 1u) h_push<true>(top, ntop, dd, s_id[i]);
             if (ntop > ef) h_pop<true>(top, ntop);
             if (ntop > 0) lower = top.get(0).d;
@@ -545,11 +546,9 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
         }
       }
       lower = __shfl_sync(0xffffffffu, lower, 0);
-      overflow = __shfl_sync(0xffffffffu, (int)overflow, 0) != 0;
     }
   }
   if (threadIdx.x == 0) {
-    if (overflow) atomicExch(err_flag, 1);
     // keep the k best, emit ascending by (distance, label)
     while (ntop > k) h_pop<true>(top, ntop);
     for (int i = 0; i < ntop; ++i) {  // selection sort of <= k entries
@@ -734,31 +733,35 @@ struct HnswIndex : IndexBase {
     g.n = G.n; g.d = dim; g.maxM = (int)G.maxM; g.maxM0 = (int)G.maxM0; g.maxlevel = G.maxlevel; g.l2 = metric == B200VS_L2;
     g.enterpoint = G.enterpoint; g.has_deletions = G.ndeleted > 0;
     const long long words = (G.n + 31) / 32;
-    unsigned int* visited = scratch.alloc<unsigned int>((size_t)nq * words);
-    const int cand_cap = (int)std::max<int64_t>(HNSW_CAND_SMEM, std::min<int64_t>(G.n + 1, 65536));
-    HeapEnt* cand = scratch.alloc<HeapEnt>((size_t)nq * cand_cap);
-    int* err = scratch.alloc<int>(1);
-    B200VS_CUDA(cudaMemsetAsync(visited, 0, (size_t)nq * words * 4, s));
-    B200VS_CUDA(cudaMemsetAsync(err, 0, 4, s));
     FilterDev f;
     f.has_range = sc.has_range; f.negate = sc.negate; f.rmin = sc.rmin; f.rmax = sc.rmax; f.sorted_ids = sc.sorted_ids_dev; f.n_ids = sc.n_ids;
     const size_t qbytes = ((size_t)dim * 4 + 15) / 16 * 16;
     const size_t smem = qbytes + (size_t)(ef_run + 1) * sizeof(HeapEnt) + (size_t)HNSW_CAND_SMEM * sizeof(HeapEnt);
     if (smem > 200 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "efsearch / dimension too large for the search kernel");
-    const unsigned grid = (unsigned)nq;
-    ScopedKernelTimer timer(this, s, profiling);
     const bool fast = !(f.has_range || f.sorted_ids != nullptr) && !g.has_deletions && ef_run + 1 <= HNSW_CAND_SMEM && G.n < (1LL << 31);
+    // the merged-array form keeps everything in shared memory; the heap form needs n + 1 candidate slots per query
+    const long long cand_cap = fast ? 0 : G.n + 1;
+    const int64_t chunk = fast ? nq : std::max<int64_t>(1, std::min<int64_t>(nq, (int64_t)(HNSW_CAND_POOL_BYTES / ((size_t)cand_cap * sizeof(HeapEnt)))));
+    unsigned int* visited = scratch.alloc<unsigned int>((size_t)chunk * words);
+    HeapEnt* cand = fast ? nullptr : scratch.alloc<HeapEnt>((size_t)chunk * cand_cap);
+    ScopedKernelTimer timer(this, s, profiling);
 #define B200VS_HNSW_LAUNCH(L2_, FAST_)                                                                                              \
   do {                                                                                                                             \
     B200VS_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<L2_, FAST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     \
-    hnsw_search_kernel<L2_, FAST_><<<grid, HNSW_THREADS, smem, s>>>(g, q, nq, k, ef_run, f, visited, words, cand, cand_cap, od, oi, err); \
+    hnsw_search_kernel<L2_, FAST_><<<(unsigned)m, HNSW_THREADS, smem, s>>>(g, q + (size_t)a * dim, m, k, ef_run, f, visited, words,  \
+                                                                          cand, cand_cap, od + (size_t)a * k, oi + (size_t)a * k);  \
   } while (0)
-    if (g.l2) { if (fast) B200VS_HNSW_LAUNCH(true, true); else B200VS_HNSW_LAUNCH(true, false); }
-    else { if (fast) B200VS_HNSW_LAUNCH(false, true); else B200VS_HNSW_LAUNCH(false, false); }
+    for (int64_t a = 0; a < nq; a += chunk) {  // chunks share one visited / candidate pool, in stream order
+      const int64_t m = std::min(chunk, nq - a);
+      B200VS_CUDA(cudaMemsetAsync(visited, 0, (size_t)m * words * 4, s));
+      if (g.l2) { if (fast) B200VS_HNSW_LAUNCH(true, true); else B200VS_HNSW_LAUNCH(true, false); }
+      else { if (fast) B200VS_HNSW_LAUNCH(false, true); else B200VS_HNSW_LAUNCH(false, false); }
+      B200VS_CUDA(cudaGetLastError());
+      launch_count(1);
+    }
 #undef B200VS_HNSW_LAUNCH
+    if (!fast) stats[6] += nq;
     timer.stop();
-    B200VS_CUDA(cudaGetLastError());
-    launch_count(1);
   }
 
   int64_t count() const override { return G.n - G.ndeleted; }

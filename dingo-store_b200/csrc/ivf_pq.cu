@@ -359,6 +359,11 @@ struct IvfPqIndex : IndexBase {
     if (mode == kFlat) { flat->add(n, x, in_ids, upsert); return; }
     std::unique_lock<std::shared_mutex> wl(rw);
     if (mode == kNone) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    // one residual row of shared memory per warp: 4 warps per CTA while they fit, fewer at large d (opt-in above 48 KB)
+    constexpr size_t kEncodeSmemMax = 227 * 1024;
+    const size_t row_bytes = (size_t)dim * 4;
+    if (row_bytes > kEncodeSmemMax) fail(B200VS_EILLEGAL_PARAMETERS, "dimension too large for the PQ encoder's shared-memory residual");
+    const int wpb = (int)std::min<size_t>(4, kEncodeSmemMax / row_bytes);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
@@ -372,8 +377,8 @@ struct IvfPqIndex : IndexBase {
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
     if (metric == B200VS_COSINE) launch_normalize_faiss(st, n, dim, stream);
     assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, st_list);
-    const int wpb = 4;
-    pq_encode_kernel<<<(unsigned)cdiv(n, wpb), wpb * 32, (size_t)wpb * dim * 4, stream>>>(st, st_list, centroids.p, codebooks.p, n, dim, M, st_codes);
+    B200VS_CUDA(cudaFuncSetAttribute(pq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wpb * row_bytes)));
+    pq_encode_kernel<<<(unsigned)cdiv(n, wpb), wpb * 32, (size_t)wpb * row_bytes, stream>>>(st, st_list, centroids.p, codebooks.p, n, dim, M, st_codes);
     B200VS_CUDA(cudaGetLastError());
     std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
@@ -463,6 +468,10 @@ struct IvfPqIndex : IndexBase {
   // raw threshold (L2: dis < thr; IP: dis > thr), at most k of them, closest first; out_counts = hits per query.
   void scan_codes(int64_t nq, const float* xq, int k, const SearchCtx& sc, bool has_thr, float thr_raw, float* od, long long* oi, int* oc,
                   cudaStream_t s) {
+    const int T = M * KSUB;
+    const int pool_cap = select_pool_cap(k, PQ_THREADS);
+    const size_t smem = (size_t)T * 4 + BlockSelect::smem_bytes(pool_cap);  // checked before anything is launched
+    if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
     const float* q = prepare_queries(nq, xq, s);
     const bool l2 = metric == B200VS_L2;
     int nprobe = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchIvfPqParamNprobe, raw_ivf_pq.cc:170
@@ -474,22 +483,19 @@ struct IvfPqIndex : IndexBase {
     float* coarse = scratch.alloc<float>((size_t)nq * nprobe);
     run_scan(this, cj, nq, q, nprobe, nullptr, coarse, probes, nullptr, s);
     if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
-    const int T = M * KSUB;
     float* sim = scratch.alloc<float>((size_t)nq * T);
     pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, sim);
     PqScanArgs a;
     a.codes = codes.p; a.ids = ids.p; a.probes = probes; a.coarse = coarse; a.list_off = L.d_off.p; a.list_len = L.d_len.p;
     a.sim = sim; a.pre = l2 ? pre.p : nullptr; a.M = M; a.nprobe = nprobe; a.k = k;
     a.nsplit = (int)std::max<int64_t>(1, std::min<int64_t>(nprobe, (device_sm_count(device) * 2 + nq - 1) / nq));
-    a.pool_cap = select_pool_cap(k, PQ_THREADS);
+    a.pool_cap = pool_cap;
     a.has_thr = has_thr ? 1 : 0;
     a.thr_key = has_thr ? f2ord(l2 ? thr_raw : -thr_raw) : 0;
     a.ws_kd = scratch.alloc<uint32_t>((size_t)nq * a.nsplit * k);
     a.ws_kid = scratch.alloc<long long>((size_t)nq * a.nsplit * k);
     a.filt.has_range = sc.has_range; a.filt.negate = sc.negate; a.filt.rmin = sc.rmin; a.filt.rmax = sc.rmax;
     a.filt.sorted_ids = sc.sorted_ids_dev; a.filt.n_ids = sc.n_ids;
-    const size_t smem = (size_t)T * 4 + BlockSelect::smem_bytes(a.pool_cap);
-    if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
     const size_t smem2 = BlockSelect::smem_bytes(a.pool_cap);
     dim3 grid(a.nsplit, (unsigned)nq);
     ScopedKernelTimer timer(this, s, profiling);

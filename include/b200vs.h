@@ -251,7 +251,8 @@ void b200vs_scan_abort(b200vs_scan* scan);
  * candidate pass; with profiling on (b200vs_set_profiling) also [2] queries of the tensor-core pass that failed
  * certification and were re-run on the exact path (0 with profiling off), [3] device time of the dominant list-scan
  * kernel in ns (CUDA events on the launch stream), [4] rows in the distinct probed lists, [5] distinct probed lists,
- * [6] work items of the tile scan, [7] its tensor-core work (128-row tiles x padded query columns).  Profiling
+ * [6] work items of the tile scan, [7] its tensor-core work (128-row tiles x padded query columns).  HNSW fills [0] and
+ * [6] = queries walked with the candidate-heap form (id filter, tombstones or ef >= 1024; 0 = merged-array form).  Profiling
  * synchronises the stream inside the call: never leave it on in a timed run. */
 int b200vs_last_search_stats(b200vs_index* idx, int64_t stats[8]);
 /* With profiling on: device milliseconds (CUDA events on the launch stream) the last search spent in each phase of the
