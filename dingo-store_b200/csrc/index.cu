@@ -355,12 +355,12 @@ struct FlatIndex : IndexBase {
     run_scan(this, job(sc), nq, q, k, od, nullptr, oi, nullptr, s);
   }
 
-  void debug_tc_scores(int64_t nq, const float* xq, bool split, float* out_scores, float* out_eps, cudaStream_t s) override {
+  void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) override {
     if ((double)nq * (double)rows * 4 > (double)(1LL << 30)) fail(B200VS_EILLEGAL_PARAMETERS, "score matrix larger than 1 GiB");
     const float* q = prepare_queries(nq, xq, s);
     float* ds = scratch.alloc<float>((size_t)std::max<int64_t>(nq * rows, 1));
     float* de = scratch.alloc<float>(nq);
-    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, split, ds, de, s);
+    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, (TcArith)arith, ds, de, s);
     if (rows > 0) B200VS_CUDA(cudaMemcpyAsync(out_scores, ds, (size_t)nq * rows * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(out_eps, de, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
@@ -430,6 +430,11 @@ struct IvfFlatIndex : IndexBase {
   DevBuf<float> vecs;            // arena [arena_cap, d]
   DevBuf<long long> ids;         // arena
   DevBuf<float> norms;           // arena
+  // FP16 mirror of the arena, kept in lockstep with vecs: the tile list scan streams it instead of the FP32 rows (half
+  // the bytes; DESIGN.md 3, 4.2).  Kept when dim % 8 == 0 (16-byte FP16 row pitch for TMA) and while it could be allocated.
+  DevBuf<__half> vecs_h;         // [arena_cap, d]  RN(x * 2^-e) per row
+  DevBuf<float> hscale;          // [arena_cap]     2^e
+  bool mirror = false;
   IvfLists L;                    // host bookkeeping + device list_off/list_len
   float max_norm = 0.f;
   float cent_max_norm = 0.f;
@@ -448,8 +453,24 @@ struct IvfFlatIndex : IndexBase {
     v.vecs = vecs.p; v.ids = ids.p; v.norms = norms.p; v.arena_rows = L.arena_used; v.list_off = L.d_off.p; v.list_len = L.d_len.p;
     v.nlist = nlist; v.total_chunks = L.total_chunks; v.max_chunks_per_list = L.max_chunks_per_list; v.max_norm = max_norm;
     v.owned_frac = nlist > 0 ? (float)L.nonempty_lists / (float)nlist : 1.f;
+    if (mirror) { v.vecs_h = vecs_h.p; v.hscale = hscale.p; }
     return v;
   }
+
+  // grow the mirror with the arena (rows_cap rows, the first `keep` kept).  Out of device memory drops the mirror, and
+  // the list scan streams the FP32 rows instead.
+  void mirror_reserve(int64_t rows_cap, int64_t keep) {
+    if (!mirror) return;
+    try {
+      vecs_h.reserve((size_t)rows_cap * dim, (size_t)keep * dim, stream);
+      hscale.reserve((size_t)rows_cap, (size_t)keep, stream);
+    } catch (const CudaError&) {
+      if (cudaGetLastError() != cudaErrorMemoryAllocation) throw;
+      vecs_h.free(); hscale.free();
+      mirror = false;
+    }
+  }
+  void mirror_reset() { vecs_h.free(); hscale.free(); mirror = dim % 8 == 0; }
 
   IvfFlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_IVF_FLAT, m, d, p) {
     nlist = p.nlist > 0 ? p.nlist : 2048;  // Constant::kCreateIvfFlatParamNcentroids
@@ -477,6 +498,7 @@ struct IvfFlatIndex : IndexBase {
     B200VS_CUDA(cudaStreamSynchronize(stream));
     L.init(k, stream);
     vecs.free(); ids.free(); norms.free();
+    mirror_reset();
     trained = true;
   }
 
@@ -576,7 +598,7 @@ struct IvfFlatIndex : IndexBase {
   int64_t count() const override { return L.live; }
   int64_t deleted_count() const override { return L.dead; }
   int64_t memory_size() const override {
-    return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + centroids.cap * 4);
+    return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + centroids.cap * 4 + vecs_h.cap * 2 + hscale.cap * 4);
   }
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override;
   int64_t export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) override;
@@ -691,15 +713,21 @@ void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, con
     vecs.reserve((size_t)arena_rows * dim, (size_t)L.arena_used_before * dim, stream);
     ids.reserve((size_t)arena_rows, (size_t)L.arena_used_before, stream);
     norms.reserve((size_t)arena_rows, (size_t)L.arena_used_before, stream);
+    mirror_reserve(arena_rows, L.arena_used_before);
   }, [&](int64_t src, int64_t dst, int64_t len) {
     B200VS_CUDA(cudaMemcpyAsync(vecs.p + (size_t)dst * dim, vecs.p + (size_t)src * dim, (size_t)len * dim * 4, cudaMemcpyDeviceToDevice, stream));
     B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)len * 8, cudaMemcpyDeviceToDevice, stream));
     B200VS_CUDA(cudaMemcpyAsync(norms.p + dst, norms.p + src, (size_t)len * 4, cudaMemcpyDeviceToDevice, stream));
+    if (mirror) {
+      B200VS_CUDA(cudaMemcpyAsync(vecs_h.p + (size_t)dst * dim, vecs_h.p + (size_t)src * dim, (size_t)len * dim * 2, cudaMemcpyDeviceToDevice, stream));
+      B200VS_CUDA(cudaMemcpyAsync(hscale.p + dst, hscale.p + src, (size_t)len * 4, cudaMemcpyDeviceToDevice, stream));
+    }
   });
   for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], h_ids_in[i]);
   B200VS_CUDA(cudaMemcpyAsync(st_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, stream));
   float* st_norms = scratch.alloc<float>(n);
   launch_scatter_rows(st, st_ids, st_slots, n, dim, vecs.p, ids.p, norms.p, st_norms, stream);
+  if (mirror) launch_half_rows(vecs.p, st_slots, n, dim, vecs_h.p, hscale.p, stream);
   max_norm = std::max(max_norm, device_max_norm(this, st_norms, n, stream));
   L.upload(stream);
   B200VS_CUDA(cudaStreamSynchronize(stream));
@@ -730,6 +758,8 @@ void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
   vecs.reserve((size_t)L.arena_cap * dim, 0, stream);
   ids.reserve((size_t)L.arena_cap, 0, stream);
   norms.reserve((size_t)L.arena_cap, 0, stream);
+  mirror_reset();
+  mirror_reserve(L.arena_cap, 0);
   B200VS_CUDA(cudaMemsetAsync(ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
   L.h_ids.assign(L.arena_cap, -1);
   L.upload(stream);
@@ -756,9 +786,10 @@ void IvfFlatIndex::maybe_compact() {
   ni.reserve(std::max<int64_t>(new_rows, 1), 0, stream);
   nn.reserve(std::max<int64_t>(new_rows, 1), 0, stream);
   const int64_t m = (int64_t)src.size();
+  long long* d_dst = nullptr;
   if (m) {
     long long* d_src = scratch.alloc<long long>(m);
-    long long* d_dst = scratch.alloc<long long>(m);
+    d_dst = scratch.alloc<long long>(m);
     B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), m * 8, cudaMemcpyHostToDevice, stream));
     B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), m * 8, cudaMemcpyHostToDevice, stream));
     launch_move_rows(vecs.p, ids.p, norms.p, d_src, d_dst, m, dim, nv.p, ni.p, nn.p, stream);
@@ -767,6 +798,11 @@ void IvfFlatIndex::maybe_compact() {
   std::swap(vecs.p, nv.p); std::swap(vecs.cap, nv.cap);
   std::swap(ids.p, ni.p); std::swap(ids.cap, ni.cap);
   std::swap(norms.p, nn.p); std::swap(norms.cap, nn.cap);
+  if (mirror) {  // re-derived from the moved FP32 rows: the same bits as moving the old mirror rows
+    vecs_h.free(); hscale.free();
+    mirror_reserve(std::max<int64_t>(new_rows, 1), 0);
+    if (mirror && m) launch_half_rows(vecs.p, d_dst, m, dim, vecs_h.p, hscale.p, stream);
+  }
   L.commit_compaction();
   L.upload(stream);
   B200VS_CUDA(cudaStreamSynchronize(stream));

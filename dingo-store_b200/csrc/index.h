@@ -265,8 +265,8 @@ struct IndexBase {
   }
   virtual int resolve_nprobe_api(const SearchCtx& sc) const { (void)sc; return 1; }
   // b200vs_debug_tc_scores: xq device (raw), outputs host [nq, count() + deleted_count()] and [nq]
-  virtual void debug_tc_scores(int64_t nq, const float* xq, bool split, float* out_scores, float* out_eps, cudaStream_t s) {
-    (void)nq; (void)xq; (void)split; (void)out_scores; (void)out_eps; (void)s;
+  virtual void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) {
+    (void)nq; (void)xq; (void)arith; (void)out_scores; (void)out_eps; (void)s;
     fail(B200VS_EILLEGAL_PARAMETERS, "tensor-core score diagnostics only exist for FLAT");
   }
 

@@ -2,11 +2,13 @@
 //
 // Kernels:
 //   tc_prep_queries_kernel   round queries to TF32 (RN), ||q||^2
+//                            (tc_prep_queries_half_kernel: power-of-two scale + FP16 (RN), for the FP16 mirror)
+//   tc_half_rows_kernel      the FP16 mirror of arena rows (power-of-two scale per row + FP16 RN)
 //   tc_count_pairs_kernel    invert the probe table: how many queries probe each list
 //   tc_plan_kernel           exclusive scans -> pair offsets, work-item offsets
-//   tc_fill_pairs_kernel     gather the (TF32-rounded) queries of every list into one contiguous block
+//   tc_fill_pairs_kernel     gather the (rounded) queries of every list into one contiguous block
 //   tc_items_kernel          emit work items (list chunk x query group) + the list of sampled items
-//   tc_scan_kernel           *** the hot kernel: TMA -> smem ring -> wgmma (TF32, register accumulators) -> epilogue ***
+//   tc_scan_kernel           *** the hot kernel: TMA -> smem ring -> wgmma (TF32 or FP16, register accumulators) -> epilogue ***
 //   tc_tau_warp_kernel       per-query capture threshold from the sampled rows (warp radix select)
 //                            (tc_tau_kernel: the block form for queries with more sampled spans than a warp stages)
 //   tc_final_hybrid_kernel   per-query window select + exact FP32 (AVX-512 order) rerank + certification
@@ -79,6 +81,45 @@ static __global__ void tc_prep_queries_split_kernel(const float* __restrict__ q,
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if (lane == 0) qnorm[w] = acc;
 }
+// FP16 operands: x * 2^-e rounded to nearest, with e chosen so that max |x_i| * 2^-e lies in [2^14, 2^15) (no overflow;
+// underflow costs at most 2^-25 * 2^e <= 2^-39 max |x_i| per element).  Scaling by a power of two is exact in FP32, so
+// the only rounding is the one to FP16 (DESIGN.md 4.2).  A zero vector keeps e = 0.
+__device__ __forceinline__ int tc_half_exp(float maxabs) { return maxabs > 0.f ? ilogbf(maxabs) - 14 : 0; }
+
+// one warp per row: dst = the scaled FP16 row, *scale = 2^e; returns <x, x> (FP32, this warp's order) to lane 0.
+__device__ __forceinline__ float tc_half_row(const float* __restrict__ src, int d, __half* __restrict__ dst, float* scale) {
+  const int lane = threadIdx.x & 31;
+  float m = 0.f, acc = 0.f;
+  for (int i = lane; i < d; i += 32) { const float v = src[i]; m = fmaxf(m, fabsf(v)); acc = fmaf(v, v, acc); }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o)); acc += __shfl_xor_sync(0xffffffffu, acc, o); }
+  const int e = tc_half_exp(m);
+  for (int i = lane; i < d; i += 32) dst[i] = __float2half_rn(ldexpf(src[i], -e));
+  if (lane == 0) *scale = ldexpf(1.f, e);
+  return acc;
+}
+
+static __global__ void tc_prep_queries_half_kernel(const float* __restrict__ q, long long nq, int d, __half* __restrict__ qh,
+                                                   float* __restrict__ qscale, float* __restrict__ qnorm) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (w >= nq) return;
+  const float n2 = tc_half_row(q + (size_t)w * d, d, qh + (size_t)w * d, qscale + w);
+  if ((threadIdx.x & 31) == 0) qnorm[w] = n2;
+}
+
+static __global__ void tc_half_rows_kernel(const float* __restrict__ x, const long long* __restrict__ rows, long long n, int d,
+                                           __half* __restrict__ half, float* __restrict__ scale) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (w >= n) return;
+  const long long r = rows ? rows[w] : w;
+  tc_half_row(x + (size_t)r * d, d, half + (size_t)r * d, scale + r);
+}
+void launch_half_rows(const float* x, const long long* rows, int64_t n, int d, __half* half, float* scale, cudaStream_t s) {
+  if (n <= 0) return;
+  tc_half_rows_kernel<<<(unsigned)cdiv(n * 32, 256), 256, 0, s>>>(x, rows, n, d, half, scale);
+  B200VS_CUDA(cudaGetLastError());
+}
+
 static __global__ void tc_split_rows_kernel(const float* __restrict__ x, long long n, float* __restrict__ hi, float* __restrict__ lo) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -155,10 +196,10 @@ static __global__ void tc_plan_kernel(const int* __restrict__ cnt, const int* __
   }
 }
 
-// one warp per (query, probe): place the pair and copy the rounded query row
+// one warp per (query, probe): place the pair and copy the rounded query row (row_bytes = d * 4 or d * 2, a multiple of 16)
 static __global__ void tc_fill_pairs_kernel(const long long* __restrict__ probes, const int* __restrict__ pos,
                                             const int* __restrict__ pair_off, const int* __restrict__ list_len, long long n,
-                                            int nprobe, int d, const float* __restrict__ q32, int* pair_query, float* bws) {
+                                            int nprobe, int row_bytes, const void* __restrict__ qop, int* pair_query, void* bws) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
@@ -167,9 +208,9 @@ static __global__ void tc_fill_pairs_kernel(const long long* __restrict__ probes
   const int p = pair_off[l] + pos[w];
   const int q = (int)(w / nprobe);
   if (lane == 0) pair_query[p] = q;
-  const float4* src = reinterpret_cast<const float4*>(q32 + (size_t)q * d);
-  float4* dst = reinterpret_cast<float4*>(bws + (size_t)p * d);
-  for (int i = lane; i < (d >> 2); i += 32) dst[i] = src[i];
+  const uint4* src = reinterpret_cast<const uint4*>(static_cast<const char*>(qop) + (size_t)q * row_bytes);
+  uint4* dst = reinterpret_cast<uint4*>(static_cast<char*>(bws) + (size_t)p * row_bytes);
+  for (int i = lane; i < (row_bytes >> 4); i += 32) dst[i] = src[i];
 }
 
 // items of list l live at item_off[l] + chunk * ngroups + group  (the groups of one chunk are adjacent: the
@@ -206,13 +247,16 @@ static __global__ void tc_items_kernel(const int* __restrict__ cnt, const int* _
 // ---------------------------------------------------------------------------------------------
 // THE HOT KERNEL.  Persistent (one CTA per SM), warp-specialised, dynamically scheduled:
 //   warp 8 (one lane): scheduler + TMA producer — claims the next work item with one atomicAdd, publishes it through
-//                      a 4-deep smem queue, then per K block loads the A tile = 128 list rows x 32 floats (16 KB,
-//                      EVICT_FIRST: streamed once) and the B tile = 16/32/64/128 gathered queries x 32 floats (EVICT_LAST)
+//                      a 4-deep smem queue, then per K block loads the A tile = 128 list rows x 128 B (16 KB,
+//                      EVICT_FIRST: streamed once) and the B tile = 16/32/64/128 gathered queries x 128 B (EVICT_LAST)
 //   warps 0-7        : two consumer warpgroups; warpgroup g owns rows [64g, 64g + 64) of every 128-row tile.  Per K block
-//                      4 x wgmma (M=64, N=16..128, K=8) TF32 with the accumulators in registers, then the epilogue on those
-//                      registers: add ||x||^2, then sample / capture (staged in shared memory, flushed per item) / dense
-//                      store.  The producer keeps filling the ring while the epilogue runs.
-// Algorithmic HBM bytes per item: rows x (d*4 + 4 + 8)  (vector, norm, id), read exactly once.
+//                      4 x wgmma (M=64, N=16..128, K = 8 TF32 or 16 FP16) with the accumulators in registers, then the
+//                      epilogue on those registers: undo the power-of-two scales (FP16), add ||x||^2, then sample / capture
+//                      (staged in shared memory, flushed per item) / dense store.  The producer keeps filling the ring while
+//                      the epilogue runs.
+// HALF = false: K block = 32 floats of the FP32 rows; HALF = true: 64 halves of the FP16 mirror, so a row costs half the
+// tile loads.  Algorithmic HBM bytes per item: rows x (d*4 + 4 + 8) (vector, norm, id), or rows x (d*2 + 4 + 4 + 8) on the
+// mirror (+ scale), read exactly once.
 // ---------------------------------------------------------------------------------------------
 constexpr int TC_CWARPS = 8;  // consumer warps (two warpgroups); the producer is warp TC_CWARPS
 
@@ -226,7 +270,7 @@ struct TcRing {  // a consumer's position in the TMA ring
 
 // One 128-row tile: this warpgroup's 64 x N scores into acc.  Every consumer warp waits for and releases every stage,
 // also when its warpgroup has no rows in the tile (mma = false).
-template <int N>
+template <bool HALF, int N>
 __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool mma, uint8_t* sA, uint8_t* sB, uint64_t* full_bar,
                                             uint64_t* empty_bar, TcRing& ring, float (&acc)[N / 2]) {
   const int lane = threadIdx.x & 31;
@@ -238,7 +282,8 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
     mbar_wait(&full_bar[s_hi], ring.phase);
     ring.next();
     int s_lo = 0;
-    if (p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
+    const bool split = !HALF && p.split;
+    if (split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
       s_lo = ring.stage;
       mbar_wait(&full_bar[s_lo], ring.phase);
       ring.next();
@@ -249,8 +294,11 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
       wgmma_fence_operands(acc);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < TC_BK / 8; ++k) wgmma_tf32<N>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
-      if (p.split) {  // + lo*hi + hi*lo into the same accumulator
+      for (int k = 0; k < TC_BK / 8; ++k) {  // one 32-byte K step each
+        if constexpr (HALF) wgmma_f16<N>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+        else wgmma_tf32<N>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+      }
+      if (split) {  // + lo*hi + hi*lo into the same accumulator
         const uint64_t adesc_lo = make_desc_k128(smem_u32(sA + (size_t)s_lo * TC_A_BYTES + a_off));
         const uint64_t bdesc_lo = make_desc_k128(smem_u32(sB + (size_t)s_lo * TC_B_BYTES));
 #pragma unroll
@@ -266,17 +314,17 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
     __syncwarp();
     if (lane == 0) {
       mbar_arrive(&empty_bar[s_hi]);
-      if (p.split) mbar_arrive(&empty_bar[s_lo]);
+      if (split) mbar_arrive(&empty_bar[s_lo]);
     }
   }
 }
 
 // One work item on the consumer warps; N = query columns of the B tile (16 / 32 / 64 / 128).
 // Thread layout of the accumulators: rows row0 and row0 + 8 of the tile, columns 8j + col0 + {0, 1}.
-template <int N>
+template <bool HALF, int N>
 __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem& I, int kblocks, uint8_t* sA, uint8_t* sB,
                                                 uint64_t* full_bar, uint64_t* empty_bar, TcRing& ring, const float* s_tau,
-                                                const int* s_q, unsigned long long* hit_key, int* hit_q, int* hit_n) {
+                                                const int* s_q, const float* s_qs, unsigned long long* hit_key, int* hit_q, int* hit_n) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
@@ -289,7 +337,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
     // that read the id are applied after the MMAs, so no warp waits for a global round trip before its first wgmma
     bool inrange[2], valid[2];
     long long arow[2], id[2];
-    float nrm[2];
+    float nrm[2], hs[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = t * TC_BM + row0 + 8 * h;
@@ -297,14 +345,16 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
       arow[h] = list_base + I.row_begin + r;
       id[h] = -1;
       nrm[h] = 0.f;
+      hs[h] = 1.f;
       if (inrange[h]) {
         id[h] = p.ids[arow[h]];
         if (p.l2 && p.add_norm) nrm[h] = p.norms[arow[h]];
+        if constexpr (HALF) hs[h] = p.hscale[arow[h]];
       }
     }
     float acc[N / 2];
     const bool mma = t * TC_BM + wg * 64 < rows;  // else this warpgroup's half of the last tile holds no item rows
-    tc_mma_tile<N>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
+    tc_mma_tile<HALF, N>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
     if (!mma) continue;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -320,7 +370,8 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
         for (int c = 0; c < 2; ++c) {
           const int n = 8 * j + col0 + c;
           if (n < I.nq) {
-            const float dot = acc[4 * j + 2 * h + c];
+            // FP16: both scales are powers of two, so hs * qs and the product with the accumulator are exact
+            const float dot = HALF ? acc[4 * j + 2 * h + c] * (hs[h] * s_qs[n]) : acc[4 * j + 2 * h + c];
             const float score = p.l2 ? fmaf(-2.f, dot, nrm[h]) : -dot;
             if (p.mode == 1) {
               if (valid[h] && score <= s_tau[n]) {
@@ -346,6 +397,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
   }
 }
 
+template <bool HALF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA32,
                const __grid_constant__ CUtensorMap tmB16, const __grid_constant__ CUtensorMap tmB32,
@@ -362,6 +414,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __shared__ int s_sched[TC_SQ];
   __shared__ float s_tau[2][TC_NQT];
   __shared__ int s_q[2][TC_NQT];
+  __shared__ float s_qs[2][TC_NQT];
   // capture staging, one buffer per consumer warp: hits are appended with a shared-memory atomic and written out
   // (one global atomicAdd per hit, a whole warp of them in flight) when the item ends, so the score loop never
   // waits on a global round trip
@@ -379,7 +432,8 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
   const int nwork = p.mode == 0 ? p.totals[2] : p.totals[0];
-  const int kblocks = (p.d + TC_BK - 1) / TC_BK;
+  const int kbk = HALF ? 2 * TC_BK : TC_BK;  // elements per K block (128 B)
+  const int kblocks = (p.d + kbk - 1) / kbk;
 
   if (warp == TC_CWARPS) {
     if (lane == 0) {  // ---------------- scheduler + TMA producer ----------------
@@ -410,22 +464,22 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             // last tile of a list: fetch only the 32-row boxes that hold list rows (the rest of the stage keeps stale
             // data, whose scores the epilogue masks) instead of streaming up to 127 rows of the neighbouring list
             const int trows = rows - t * TC_BM;
-            const int nbox = (p.mode == 1 && !p.split && trows <= TC_BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
+            const int nbox = (p.mode == 1 && (HALF || !p.split) && trows <= TC_BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
             const uint32_t saved = nbox ? TC_A_BYTES - (uint32_t)nbox * (TC_SAMPLE * 128) : 0u;
             mbar_arrive_expect_tx(&full_bar[stage], bytes - saved);
             if (nbox) {
               for (int j = 0; j < nbox; ++j)
-                tma_load_2d(sA + (size_t)stage * TC_A_BYTES + (size_t)j * (TC_SAMPLE * 128), &tmA32, &full_bar[stage], kb * TC_BK,
+                tma_load_2d(sA + (size_t)stage * TC_A_BYTES + (size_t)j * (TC_SAMPLE * 128), &tmA32, &full_bar[stage], kb * kbk,
                             (int)(base_row + (long long)t * TC_BM + j * TC_SAMPLE), kEvictFirst);
             } else
-            tma_load_2d(sA + (size_t)stage * TC_A_BYTES, ta, &full_bar[stage], kb * TC_BK, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
-            tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tb, &full_bar[stage], kb * TC_BK, I.pair_begin, kEvictLast);
+            tma_load_2d(sA + (size_t)stage * TC_A_BYTES, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+            tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tb, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
             if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-            if (p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
+            if (!HALF && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
               mbar_wait(&empty_bar[stage], phase ^ 1);
               mbar_arrive_expect_tx(&full_bar[stage], bytes);
-              tma_load_2d(sA + (size_t)stage * TC_A_BYTES, &tmAlo, &full_bar[stage], kb * TC_BK, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
-              tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tbl, &full_bar[stage], kb * TC_BK, I.pair_begin, kEvictLast);
+              tma_load_2d(sA + (size_t)stage * TC_A_BYTES, &tmAlo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+              tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tbl, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
               if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
             }
           }
@@ -451,10 +505,11 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int q = p.pair_query ? p.pair_query[I.pair_begin + et] : I.pair_begin + et;
       s_q[buf][et] = q;
       s_tau[buf][et] = p.mode == 1 ? p.tau[q] : 0.f;
+      if (HALF) s_qs[buf][et] = p.qscale[q];
     }
     asm volatile("bar.sync 1, %0;" ::"n"(TC_CWARPS * 32) : "memory");
 #define B200VS_CONSUME(N_) \
-  tc_consume_item<N_>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_hit_key[warp], s_hit_q[warp], &s_hit_n[warp])
+  tc_consume_item<HALF, N_>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf], s_hit_key[warp], s_hit_q[warp], &s_hit_n[warp])
     if (I.nq <= 16) B200VS_CONSUME(16);
     else if (I.nq <= 32) B200VS_CONSUME(32);
     else if (I.nq <= 64) B200VS_CONSUME(64);
@@ -479,7 +534,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // per-query capture threshold T.  tau = the k-th smallest sampled score (TC_SAMPLE rows per span) bounds the k-th
 // smallest score overall (A_k) from above; tc_tau_with_margin turns it into T.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm, int d, bool split);
+__device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm, int d, int arith);
 
 // Capture threshold from the sampled k-th score tau.  The finish kernel certifies A_k + 2 eps <= T (A_k = k-th captured
 // score); a query that fails is re-run on the exact scan, and a single re-scanned query of a large shard stalls every rank
@@ -508,7 +563,7 @@ constexpr int TAU_PL = 4096;  // (sample slot, column) pairs staged per query
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_tau_kernel(const long long* __restrict__ probes, const int* __restrict__ pos, const int* __restrict__ cnt,
               const int* __restrict__ item_off, const int* __restrict__ list_len, const TcItem* __restrict__ items, int nprobe,
-              const float* __restrict__ sample, int k, int l2, const float* __restrict__ qnorm, float max_norm, int d,
+              const float* __restrict__ sample, int k, int l2, const float* __restrict__ qnorm, float max_norm, int d, int arith,
               int cand_cap, float* tau, const int* __restrict__ redo) {
   __shared__ int2 s_pairs[TAU_PL];
   __shared__ BlockSelShared S;
@@ -553,7 +608,7 @@ tc_tau_kernel(const long long* __restrict__ probes, const int* __restrict__ pos,
   const float kth = ord2f(block_kth_key_any(k, S, [&](auto f) {
     for (int i = threadIdx.x; i < tot; i += blockDim.x) { const float v = sampled(i); if (v < TC_INF) f(f2ord(v)); }
   }));
-  const float t = tc_tau_with_margin(kth, 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, false), cand_cap, count_le);
+  const float t = tc_tau_with_margin(kth, 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, arith), cand_cap, count_le);
   if (threadIdx.x == 0) tau[q] = t;
 }
 
@@ -567,8 +622,8 @@ constexpr int WT_PAIRS = 64;
 static __global__ void __launch_bounds__(WT_WARPS * 32)
 tc_tau_warp_kernel(const long long* __restrict__ probes, const int* __restrict__ pos, const int* __restrict__ cnt,
                    const int* __restrict__ item_off, const int* __restrict__ list_len, const TcItem* __restrict__ items, int nprobe,
-                   const float* __restrict__ sample, int k, int nq, int l2, const float* __restrict__ qnorm, float max_norm, int d, int cap,
-                   float* tau, int* redo) {
+                   const float* __restrict__ sample, int k, int nq, int l2, const float* __restrict__ qnorm, float max_norm, int d, int arith,
+                   int cap, float* tau, int* redo) {
   __shared__ int s_hist[WT_WARPS][WS_BINS];
   __shared__ int s_pair[WT_WARPS][WT_PAIRS];
   __shared__ uint32_t s_val[WT_WARPS][WT_PAIRS * TC_SAMPLE];
@@ -626,7 +681,7 @@ tc_tau_warp_kernel(const long long* __restrict__ probes, const int* __restrict__
     int c_le;
     const uint32_t* vals = s_val[warp];
     t = ord2f(warp_kth_key(k, s_hist[warp], [&](auto f) { for (int i = lane; i < nfin; i += 32) f(vals[i]); }, c_le));
-    t = tc_tau_with_margin(t, 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, false), cap,
+    t = tc_tau_with_margin(t, 2.f * tc_eps(l2 != 0, qnorm[q], max_norm, d, arith), cap,
                            [&](float lim) { int c = 0; for (int i = lane; i < nfin; i += 32) c += ord2f(vals[i]) <= lim ? 1 : 0; return __reduce_add_sync(0xffffffffu, c); });
   }
   if (lane == 0) tau[q] = t;
@@ -637,13 +692,22 @@ tc_tau_warp_kernel(const long long* __restrict__ probes, const int* __restrict__
 // ---------------------------------------------------------------------------------------------
 constexpr int FIN_SEG = 2048;  // in-window rows staged per round
 
-__device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm, int d, bool split) {
-  // rigorous bound on |approx score - exact score| (DESIGN.md 4.2).  Operand term: single-pass TF32 = rows truncated
-  // (< 2^-10 relative) + query rounded to nearest (<= 2^-11) = 1.5 * 2^-10 (the 2^-21 cross term and the FP32 accumulation
-  // are covered by the second summand); split pass (hi*hi + lo*hi + hi*lo) -> 2^-19.
+__device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm, int d, int arith) {
+  // rigorous bound on |approx score - exact score| (DESIGN.md 4.2).  Operand term (relative to ||q|| max ||x||):
+  //   TF32 single pass: rows truncated (< 2^-10 relative) + query rounded to nearest (<= 2^-11) = 1.5 * 2^-10 (the 2^-21
+  //     cross term and the FP32 accumulation are covered by the second summand);
+  //   split pass (hi*hi + lo*hi + hi*lo): 2^-19;
+  //   FP16: each operand vector is off by at most delta = 2^-11 + sqrt(d) 2^-39 of its norm (RN, plus underflow below the
+  //     power-of-two scale), so the dot product by at most 2 delta + delta^2; the FP16 products are exact in FP32.
   // Accumulation term: FP32 sums of d terms on both sides (tensor core, norms, and the exact kernel itself).
   const float qn = sqrtf(qnorm_sq);
-  const float operand = (l2 ? 2.f : 1.f) * (split ? 1.9073486e-6f /*2^-19*/ : 0.0014648438f /*2^-10 + 2^-11*/) * qn * max_norm;
+  float rel = 0.0014648438f;  // 2^-10 + 2^-11
+  if (arith == TC_ARITH_SPLIT) rel = 1.9073486e-6f;  // 2^-19
+  else if (arith == TC_ARITH_FP16) {
+    const float delta = __fadd_ru(4.8828125e-4f /*2^-11*/, __fmul_ru(sqrtf((float)d), 1.8189894e-12f /*2^-39*/));
+    rel = __fmaf_ru(delta, delta, 2.f * delta);
+  }
+  const float operand = (l2 ? 2.f : 1.f) * rel * qn * max_norm;
   const float accum = 2.f * (float)(d + 64) * 5.9604645e-8f /*2^-24*/ * (l2 ? (max_norm + qn) * (max_norm + qn) : qn * max_norm);
   return operand + accum;
 }
@@ -686,7 +750,7 @@ template <bool L2>
 static __global__ void __launch_bounds__(HF_THREADS)
 tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
                        const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
-                       const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k,
+                       const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int arith, int k,
                        float* out_dist, long long* out_ids, int* flags, int* redo) {
   extern __shared__ __align__(16) unsigned char s_dyn[];  // the query row (d % 4 == 0)
   __shared__ BlockSelShared S;
@@ -708,7 +772,7 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   auto key_at = [&](int i) -> unsigned long long { return i < nst ? s_keys[i] : c[i]; };
   float a_k = TC_INF;
   if (n >= k) a_k = ord2f(block_kth_key_any(k, S, [&](auto f) { for (int i = threadIdx.x; i < n; i += HF_THREADS) f((uint32_t)(key_at(i) >> 32)); }));
-  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, false);
+  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith);
   {
     const float window = a_k + two_eps;
     for (int base = 0; base < n; base += HF_THREADS) {
@@ -804,7 +868,7 @@ tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows
     for (int j = 0; j < KPT; ++j) if (key[j] != 0xFFFFFFFFu) f(key[j]);
   });
   const float a_k = ord2f(kth);
-  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true);
+  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, TC_ARITH_SPLIT);
   const uint32_t thr_hi = f2ord(__fadd_ru(a_k, two_eps));
   const bool set_mode = out_raw == nullptr && S.c_le == k;
   const uint32_t thr_lo = f2ord(__fsub_rd(a_k, two_eps));
@@ -882,7 +946,7 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
       for (int j = 0; j < KPT; ++j) if (key[j] != 0xFFFFFFFFu) f(key[j]);
     }, c_le);
     const float a_k = ord2f(kth);
-    const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true);
+    const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, TC_ARITH_SPLIT);
     const uint32_t thr_hi = f2ord(__fadd_ru(a_k, two_eps));
     const uint32_t thr_lo = f2ord(__fsub_rd(a_k, two_eps));
     const bool set_mode = out_raw == nullptr && c_le == k;
@@ -1001,7 +1065,7 @@ template <bool L2>
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
                 const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
-                const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int k, int pool_cap,
+                const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int arith, int k, int pool_cap,
                 float* out_dist, long long* out_ids, int* flags, const int* redo) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int qi = blockIdx.x;
@@ -1010,7 +1074,7 @@ tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restri
   const unsigned long long* c = cand + (size_t)qi * cap;
   BlockSelect sel;
   const float window = tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k,
-                                            2.f * tc_eps(L2, qnorm[qi], max_norm, d, false), [&](int i) { return c[i]; },
+                                            2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith), [&](int i) { return c[i]; },
                                             [&](uint32_t row) { return ids[row]; });
   const float tq = tau[qi];
   const bool certified = (total <= cap) && (tq == TC_INF || window <= tq);
@@ -1041,7 +1105,7 @@ tc_coarse_final_kernel(const float* __restrict__ dense, long long ld, int nrows,
   if (redo && !redo[qi]) return;  // finished by the register select
   const float* row_scores = dense + (size_t)qi * ld;
   BlockSelect sel;
-  tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, nrows, k, 2.f * tc_eps(L2, qnorm[qi], max_norm, d, true),
+  tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, nrows, k, 2.f * tc_eps(L2, qnorm[qi], max_norm, d, TC_ARITH_SPLIT),
                        [&](int i) { return ((unsigned long long)f2ord(row_scores[i]) << 32) | (unsigned)i; },
                        [](uint32_t row) { return (long long)row; });
   const int have = *sel.count;
@@ -1119,14 +1183,16 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// row-major float matrix [rows, d]; box = 32 floats (128 B) x box_rows, 128-byte swizzle
-static CUtensorMap make_tmap(const float* base, int64_t rows, int d, int box_rows) {
+// row-major matrix [rows, d] of floats (half = false) or halves; box = 128 B of K (32 floats / 64 halves) x box_rows,
+// 128-byte swizzle
+static CUtensorMap make_tmap(const void* base, int64_t rows, int d, int box_rows, bool half = false) {
   CUtensorMap m;
   cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)std::max<int64_t>(rows, 1)};
-  cuuint64_t gstride[1] = {(cuuint64_t)d * 4};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)d * (half ? 2 : 4)};
+  cuuint32_t box[2] = {(cuuint32_t)(half ? 2 * TC_BK : TC_BK), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
+  CUresult r = get_encode()(&m, half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim,
+                            gstride, box, estr,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) fail(B200VS_EINTERNAL, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
@@ -1152,7 +1218,8 @@ static int tc_init(int device) {
   std::lock_guard<std::mutex> g(g_tc_init_mu);
   if (g_dev_sms[device]) return g_dev_sms[device];
   const int sms = device_sm_count(device);
-  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
@@ -1178,9 +1245,10 @@ bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int np
 
 // everything the passes share: rounded queries, pair inversion, gathered B block, work items, tensor maps
 struct TcPlan {
-  float* q32; float* qnorm;
+  bool half;  // the FP16 mirror (v.vecs_h) instead of the FP32 rows
+  void* qop; float* qnorm; float* qscale;
   int *cnt, *pos, *pair_off, *item_off, *totals, *pair_query, *sample_list, *work;
-  float* bws;
+  void* bws;
   TcItem* items;
   int64_t bound, sbound, npairs;
   CUtensorMap tmA, tmA32, tmB16, tmB32, tmB64, tmB128;
@@ -1196,8 +1264,11 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.npairs = nq * nprobe;
   P.bound = tc_item_bound(v, P.npairs);
   P.sbound = tc_sample_bound(v, P.npairs);
-  P.q32 = S.alloc<float>((size_t)nq * d);
+  P.half = v.vecs_h != nullptr;
+  const int esz = P.half ? 2 : 4;  // operand bytes per element
+  P.qop = S.alloc<unsigned char>((size_t)nq * d * esz);
   P.qnorm = S.alloc<float>(nq);
+  P.qscale = P.half ? S.alloc<float>(nq) : nullptr;
   P.cnt = S.alloc<int>(v.nlist);
   P.pos = S.alloc<int>(P.npairs);
   P.pair_off = S.alloc<int>(v.nlist);
@@ -1206,22 +1277,24 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.work = S.alloc<int>(4);
   P.pair_query = S.alloc<int>(P.npairs);
   P.sample_list = S.alloc<int>(P.sbound);
-  P.bws = S.alloc<float>((size_t)(P.npairs + TC_NQT) * d);
+  P.bws = S.alloc<unsigned char>((size_t)(P.npairs + TC_NQT) * d * esz);
   P.items = S.alloc<TcItem>(P.bound);
   B200VS_CUDA(cudaMemsetAsync(P.cnt, 0, (size_t)v.nlist * 4, s));
   B200VS_CUDA(cudaMemsetAsync(P.work, 0, 16, s));
-  tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, P.q32, P.qnorm);
+  if (P.half) tc_prep_queries_half_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<__half*>(P.qop), P.qscale, P.qnorm);
+  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(P.qop), P.qnorm);
   tc_count_pairs_kernel<<<(unsigned)cdiv(P.npairs, 256), 256, 0, s>>>(probes, P.npairs, P.cnt, P.pos);
   tc_plan_kernel<<<1, 1024, 0, s>>>(P.cnt, v.list_len, v.nlist, P.pair_off, P.item_off, P.totals);
-  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, d, P.q32, P.pair_query, P.bws);
+  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, d * esz, P.qop, P.pair_query, P.bws);
   tc_items_kernel<<<(unsigned)cdiv(v.nlist, 128), 128, 0, s>>>(P.cnt, v.list_len, P.pair_off, P.item_off, v.nlist, P.items, P.totals, P.sample_list);
   B200VS_CUDA(cudaGetLastError());
-  P.tmA = make_tmap(v.vecs, v.arena_rows, d, TC_BM);
-  P.tmA32 = make_tmap(v.vecs, v.arena_rows, d, TC_SAMPLE);
-  P.tmB16 = make_tmap(P.bws, P.npairs + TC_NQT, d, 16);
-  P.tmB32 = make_tmap(P.bws, P.npairs + TC_NQT, d, 32);
-  P.tmB64 = make_tmap(P.bws, P.npairs + TC_NQT, d, 64);
-  P.tmB128 = make_tmap(P.bws, P.npairs + TC_NQT, d, 128);
+  const void* rows = P.half ? static_cast<const void*>(v.vecs_h) : static_cast<const void*>(v.vecs);
+  P.tmA = make_tmap(rows, v.arena_rows, d, TC_BM, P.half);
+  P.tmA32 = make_tmap(rows, v.arena_rows, d, TC_SAMPLE, P.half);
+  P.tmB16 = make_tmap(P.bws, P.npairs + TC_NQT, d, 16, P.half);
+  P.tmB32 = make_tmap(P.bws, P.npairs + TC_NQT, d, 32, P.half);
+  P.tmB64 = make_tmap(P.bws, P.npairs + TC_NQT, d, 64, P.half);
+  P.tmB128 = make_tmap(P.bws, P.npairs + TC_NQT, d, 128, P.half);
   ix->launch_count(5);
   return P;
 }
@@ -1231,12 +1304,14 @@ static TcParams tc_params(const TcView& v, const TcPlan& P, int d, bool l2) {
   memset(&p, 0, sizeof(p));
   p.ids = v.ids; p.norms = v.norms; p.list_off = v.list_off; p.d = d; p.items = P.items; p.totals = P.totals;
   p.sample_list = P.sample_list; p.pair_query = P.pair_query; p.l2 = l2 ? 1 : 0; p.add_norm = 1;
+  p.hscale = v.hscale; p.qscale = P.qscale;
   return p;
 }
 
 static void tc_launch(const TcPlan& P, const TcParams& p, int64_t work_bound, cudaStream_t s) {
   const int grid = (int)std::min<int64_t>(P.num_sms, std::max<int64_t>(1, work_bound));
-  tc_scan_kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(P.tmA, P.tmA32, P.tmB16, P.tmB32, P.tmB64, P.tmB128, P.tmA, P.tmB16, P.tmB32, P.tmB64, P.tmB128, p);
+  if (P.half) tc_scan_kernel<true><<<grid, TC_THREADS, TC_SMEM, s>>>(P.tmA, P.tmA32, P.tmB16, P.tmB32, P.tmB64, P.tmB128, P.tmA, P.tmB16, P.tmB32, P.tmB64, P.tmB128, p);
+  else tc_scan_kernel<false><<<grid, TC_THREADS, TC_SMEM, s>>>(P.tmA, P.tmA32, P.tmB16, P.tmB32, P.tmB64, P.tmB128, P.tmA, P.tmB16, P.tmB32, P.tmB64, P.tmB128, p);
   B200VS_CUDA(cudaGetLastError());
 }
 
@@ -1272,8 +1347,9 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   ix->phase(IndexBase::PH_TAU, s);
   int* redo = S.alloc<int>(nq);
   // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
-  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qnorm, v.max_norm, d, cap, tau, redo);
-  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qnorm, v.max_norm, d, cap, tau, redo);
+  const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
+  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qnorm, v.max_norm, d, arith, cap, tau, redo);
+  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qnorm, v.max_norm, d, arith, cap, tau, redo);
   // 2) capture pass: stream every probed list chunk once, keep rows under the threshold
   p.mode = 1; p.work_counter = P.work + 1;
   ix->phase(IndexBase::PH_CAPTURE, s);
@@ -1287,14 +1363,14 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   const int* fin_redo = nullptr;
   const size_t hsm = (size_t)d * 4;  // the query row
   if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, redo);
-    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, out_dist, out_ids, flags, redo);
+    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
+    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
     fin_redo = redo;
     ix->launch_count(1);
   }
   const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
-  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, k, pool, out_dist, out_ids, flags, fin_redo);
+  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
+  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
   tc_compact_flags_kernel<<<1, 1024, 0, s>>>(flags, (int)nq, qmap, qcount);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
@@ -1347,12 +1423,13 @@ bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe) 
 // (L2: ||x||^2 - 2 <q, x>; IP: -<q, x>; tombstoned rows +inf).  qb_lo == nullptr: single-pass TF32, qb holds the RN-rounded
 // queries and the tensor core truncates the rows a_hi.  Otherwise the error-compensated split pass: the three products
 // hi*hi + lo*hi + hi*lo accumulate into the same register accumulators (the lo operands ride in the next ring stage).
-static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* qb, const float* qb_lo, const float* a_hi,
-                          const float* a_lo, float* dense, cudaStream_t s) {
+// hscale != nullptr: qb and a_hi are scaled FP16 (the list scan's FP16 arithmetic), qscale / hscale their scales.
+static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const void* qb, const float* qb_lo, const void* a_hi,
+                          const float* a_lo, const float* qscale, const float* hscale, float* dense, cudaStream_t s) {
   const int num_sms = tc_init(ix->device);
   const int d = ix->dim;
   const int nrows = (int)v.arena_rows;
-  const bool split = qb_lo != nullptr;
+  const bool split = qb_lo != nullptr, half = hscale != nullptr;
   auto& S = ix->scratch;
   const int chunk = nrows <= 16384 ? TC_BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
   const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, TC_NQT));
@@ -1365,15 +1442,17 @@ static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, c
   memset(&P, 0, sizeof(P));
   P.items = items; P.totals = totals;
   TcParams p = tc_params(v, P, d, l2);
-  p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.pair_query = nullptr;
-  const CUtensorMap ta = make_tmap(a_hi, nrows, d, TC_BM), ta_lo = split ? make_tmap(a_lo, nrows, d, TC_BM) : ta;
-  const CUtensorMap b16 = make_tmap(qb, nq, d, 16), b32 = make_tmap(qb, nq, d, 32), b64 = make_tmap(qb, nq, d, 64), b128 = make_tmap(qb, nq, d, 128);
+  p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.pair_query = nullptr; p.hscale = hscale; p.qscale = qscale;
+  const CUtensorMap ta = make_tmap(a_hi, nrows, d, TC_BM, half), ta_lo = split ? make_tmap(a_lo, nrows, d, TC_BM) : ta;
+  const CUtensorMap b16 = make_tmap(qb, nq, d, 16, half), b32 = make_tmap(qb, nq, d, 32, half), b64 = make_tmap(qb, nq, d, 64, half),
+                    b128 = make_tmap(qb, nq, d, 128, half);
   const CUtensorMap l16 = split ? make_tmap(qb_lo, nq, d, 16) : b16, l32 = split ? make_tmap(qb_lo, nq, d, 32) : b32;
   const CUtensorMap l64 = split ? make_tmap(qb_lo, nq, d, 64) : b64, l128 = split ? make_tmap(qb_lo, nq, d, 128) : b128;
   const int grid = (int)std::min<int64_t>(num_sms, std::max(1, nitems));
   p.work_counter = work; p.split = split ? 1 : 0; p.dense_accum = 0; p.add_norm = 1;
   ix->phase(IndexBase::PH_COARSE_SCAN, s);
-  tc_scan_kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
+  if (half) tc_scan_kernel<true><<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
+  else tc_scan_kernel<false><<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
   B200VS_CUDA(cudaGetLastError());
 }
 
@@ -1391,7 +1470,7 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   float* dense = S.alloc<float>((size_t)nq * nrows);
   ix->phase(IndexBase::PH_COARSE_PREP, s);
   tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qhi, qlo, qnorm);
-  tc_dense_scan(ix, v, l2, nq, qhi, qlo, v.vecs_hi, v.vecs_lo, dense, s);
+  tc_dense_scan(ix, v, l2, nq, qhi, qlo, v.vecs_hi, v.vecs_lo, nullptr, nullptr, dense, s);
   ix->phase(IndexBase::PH_COARSE_FINAL, s);
   const int pool = select_pool_cap(nprobe, SCAN_THREADS);
   const size_t fin_smem = tc_stream_smem(d, pool);
@@ -1430,32 +1509,41 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   ix->launch_count(4);
 }
 
-static __global__ void tc_eps_kernel(const float* __restrict__ qnorm, long long nq, int l2, float max_norm, int d, int split, float* out) {
+static __global__ void tc_eps_kernel(const float* __restrict__ qnorm, long long nq, int l2, float max_norm, int d, int arith, float* out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nq) out[i] = tc_eps(l2 != 0, qnorm[i], max_norm, d, split != 0);
+  if (i < nq) out[i] = tc_eps(l2 != 0, qnorm[i], max_norm, d, arith);
 }
 
-void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, bool split, float* out_scores,
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, float* out_scores,
                      float* out_eps, cudaStream_t s) {
   const int d = ix->dim;
   auto& S = ix->scratch;
-  float* qb = S.alloc<float>((size_t)nq * d);
+  const bool split = arith == TC_ARITH_SPLIT, half = arith == TC_ARITH_FP16;
+  void* qb = S.alloc<unsigned char>((size_t)nq * d * (half ? 2 : 4));
   float* qb_lo = split ? S.alloc<float>((size_t)nq * d) : nullptr;
   float* qnorm = S.alloc<float>(nq);
-  if (split) tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qb, qb_lo, qnorm);
-  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qb, qnorm);
+  float* qscale = half ? S.alloc<float>(nq) : nullptr;
+  if (split) tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(qb), qb_lo, qnorm);
+  else if (half) tc_prep_queries_half_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<__half*>(qb), qscale, qnorm);
+  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(qb), qnorm);
   B200VS_CUDA(cudaGetLastError());
   if (v.arena_rows > 0) {
-    const float *a_hi = v.vecs, *a_lo = nullptr;
+    const void* a_hi = v.vecs;
+    const float *a_lo = nullptr, *hscale = nullptr;
     if (split) {  // the same row split the IVF coarse quantiser keeps for its centroids
       float* hi = S.alloc<float>((size_t)v.arena_rows * d);
       float* lo = S.alloc<float>((size_t)v.arena_rows * d);
       launch_split_rows(v.vecs, v.arena_rows, d, hi, lo, s);
       a_hi = hi; a_lo = lo;
+    } else if (half) {  // the same mirror an IVF-Flat index keeps for its lists
+      __half* h = S.alloc<__half>((size_t)v.arena_rows * d);
+      float* sc = S.alloc<float>(v.arena_rows);
+      launch_half_rows(v.vecs, nullptr, v.arena_rows, d, h, sc, s);
+      a_hi = h; hscale = sc;
     }
-    tc_dense_scan(ix, v, l2, nq, qb, qb_lo, a_hi, a_lo, out_scores, s);
+    tc_dense_scan(ix, v, l2, nq, qb, qb_lo, a_hi, a_lo, qscale, hscale, out_scores, s);
   }
-  tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qnorm, nq, l2 ? 1 : 0, v.max_norm, d, split ? 1 : 0, out_eps);
+  tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qnorm, nq, l2 ? 1 : 0, v.max_norm, d, arith, out_eps);
   B200VS_CUDA(cudaGetLastError());
 }
 

@@ -7,14 +7,15 @@
 // from HBM ONCE PER BATCH and multiplied against all queries that probe it — the one place on this path where
 // the work is a dense contraction (SURVEY.md §8d).
 //
-// Exactness: the MMA runs in TF32 (operands truncated to 10 mantissa bits), so its scores only SELECT
-// candidates.  Per query the engine keeps every row whose approximate score is within 2*eps of the k-th best
+// Exactness: the MMA runs in TF32 (operands truncated to 10 mantissa bits) or, on an IVF-Flat index's FP16 mirror, in
+// FP16 (rows and queries scaled by a power of two and rounded to nearest), so its scores only SELECT candidates.  Per query the engine keeps every row whose approximate score is within 2*eps of the k-th best
 // approximate score (eps = rigorous bound on the TF32 score error); all of those are re-scored by the exact
 // FP32 kernel in the reference's AVX-512 order, so the returned ids and distances are identical to the exact
 // path.  Queries whose window cannot be certified (candidate overflow / threshold too tight) are re-run on
 // the exact scan.  See DESIGN.md §Tensor-core candidate pass.
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 
 #include "filter.cuh"
 #include "index.h"
@@ -22,7 +23,7 @@
 namespace b200vs {
 
 constexpr int TC_BM = 128;        // database rows per tile (two warpgroups x wgmma M = 64)
-constexpr int TC_BK = 32;         // floats per K block = 128 B = one swizzle span
+constexpr int TC_BK = 32;         // floats per K block = 128 B = one swizzle span (64 halves on the FP16 path)
 constexpr int TC_NQT = 128;       // queries per work item (wgmma N <= 128): a probed list chunk is re-streamed only beyond 128 queries
 constexpr int TC_STAGES = 6;      // TMA->MMA ring depth (6 x 32 KB; + 24 KB of capture staging: ~220 KB, the bytes in flight bound the HBM rate; DESIGN §4.2)
 constexpr int TC_THREADS = 288;   // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA + scheduler
@@ -65,6 +66,8 @@ struct TcParams {
   int dense_accum;          // mode 2: add to the stored score instead of overwriting (split-precision passes 2 and 3)
   int add_norm;             // include the ||x||^2 term (off for the correction passes)
   int split;                // error-compensated TF32: hi*hi + lo*hi + hi*lo into one accumulator (coarse quantiser)
+  const float* hscale;      // FP16 path: [arena rows] power-of-two scale of each row of the mirror
+  const float* qscale;      // FP16 path: [nq] power-of-two scale of each query
   int l2;
   FilterDev filt;
 };
@@ -87,6 +90,15 @@ struct TcView {
   long long id_offset = 0;   // tc_coarse on a slice of the centroid table: added to the returned row indices
   float owned_frac = 1.f;    // share of the lists that hold rows here (a list-sharded rank owns 1 / world of them)
   bool api_scores = false;   // tc_coarse: return the ascending ranking score (L2 distance | -ip) instead of the raw metric value
+  const __half* vecs_h = nullptr;  // optional FP16 mirror of vecs (x * 2^-e per row, rounded to nearest): the list scan
+  const float* hscale = nullptr;   //   streams it instead of the FP32 rows; hscale[r] = 2^e (DESIGN.md 3, 4.2)
+};
+
+// Arithmetic of the tile kernel's scores, and so of the error bound tc_eps()
+enum TcArith : int {
+  TC_ARITH_TF32 = 0,   // rows truncated to TF32, queries rounded to nearest (list scan without a mirror)
+  TC_ARITH_SPLIT = 1,  // error-compensated hi / lo TF32 (coarse quantiser)
+  TC_ARITH_FP16 = 2,   // rows and queries scaled by powers of two and rounded to FP16 (list scan on the mirror)
 };
 
 // true when this search can use the tensor-core pass (otherwise the caller runs the exact scan)
@@ -106,12 +118,16 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
 
 // Diagnostics (b200vs_debug_tc_scores; no search path calls it): the tile kernel's dense approximate scores of q (device,
 // prepared) against every arena row, out_scores [nq, v.arena_rows], and the tc_eps() the finish kernels use, out_eps [nq].
-// split = false: list-scan arithmetic; true: the coarse pass's hi / lo arithmetic.
-void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, bool split, float* out_scores,
+// arith: TC_ARITH_TF32 = list scan without a mirror, TC_ARITH_SPLIT = the coarse pass's hi / lo arithmetic,
+// TC_ARITH_FP16 = list scan on an FP16 mirror (a temporary one is made from v.vecs inside the call).
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, float* out_scores,
                      float* out_eps, cudaStream_t s);
 
 float device_max_norm(IndexBase* ix, const float* norms_sq, int64_t n, cudaStream_t s);  // sqrt(max ||x||^2)
 void launch_row_norms(const float* x, int64_t n, int d, float* out, cudaStream_t s);     // out[i] = <x_i, x_i>
 void launch_split_rows(const float* x, int64_t n, int d, float* hi, float* lo, cudaStream_t s);
+// FP16 mirror rows: for i < n, row r = rows ? rows[i] : i, half[r] = RN(x[r] * 2^-e), scale[r] = 2^e with
+// max |x[r]| * 2^-e in [2^14, 2^15) (a zero row: scale 1).  d % 8 == 0.
+void launch_half_rows(const float* x, const long long* rows, int64_t n, int d, __half* half, float* scale, cudaStream_t s);
 
 }  // namespace b200vs
