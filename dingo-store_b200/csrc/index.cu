@@ -187,19 +187,114 @@ void check_batch_ids_unique(int64_t n, const int64_t* ids) {  // CheckVectorIdDu
 }
 
 // ============================================================================================
+// Device rows of a Flat index or an IVF-Flat arena: FP32 rows, ids (-1 = tombstone / unused slot), ||x||^2 and, when
+// the owner asks for it and dim % 8 == 0 (16-byte FP16 row pitch for TMA), the FP16 mirror the tile list scan streams
+// instead of the FP32 rows (DESIGN.md 3, 4.2).  Every write of the rows goes through here, so the arrays stay in step.
+// The owner decides capacities and slots; the store moves rows.  All work runs on the owner's stream.
+// ============================================================================================
+struct RowStore {
+  IndexBase* const ix;     // scratch for the device copies of host-side row lists
+  const int d;
+  const cudaStream_t s;
+  const bool want_mirror;
+  DevBuf<float> vecs;      // [cap, d]
+  DevBuf<long long> ids;   // [cap]
+  DevBuf<float> norms;     // [cap]
+  DevBuf<__half> vecs_h;   // [cap, d]  RN(x * 2^-e) per row
+  DevBuf<float> hscale;    // [cap]     2^e
+  bool mirror;             // the mirror is kept: wanted, and no allocation of it failed since the last reset()
+  float max_norm = 0.f;    // max ||x|| over every row written: grows only (tc_eps)
+
+  RowStore(IndexBase* owner, bool half)
+      : ix(owner), d(owner->dim), s(owner->stream), want_mirror(half && d % 8 == 0), mirror(want_mirror) {}
+
+  // grow to cap rows keeping the first `keep`.  Out of device memory drops the mirror, and the list scan streams the
+  // FP32 rows instead.
+  void grow(int64_t cap, int64_t keep) {
+    vecs.reserve((size_t)cap * d, (size_t)keep * d, s);
+    ids.reserve(cap, keep, s);
+    norms.reserve(cap, keep, s);
+    if (mirror && !(vecs_h.try_reserve((size_t)cap * d, (size_t)keep * d, s) && hscale.try_reserve(cap, keep, s))) {
+      vecs_h.free(); hscale.free();
+      mirror = false;
+    }
+  }
+  // drop every row and buffer; the mirror is wanted again
+  void reset() {
+    vecs.free(); ids.free(); norms.free(); vecs_h.free(); hscale.free();
+    mirror = want_mirror;
+  }
+  // copy rows [src, src + n) to [dst, dst + n) (list relocation)
+  void move(int64_t src, int64_t dst, int64_t n) {
+    B200VS_CUDA(cudaMemcpyAsync(vecs.p + (size_t)dst * d, vecs.p + (size_t)src * d, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, s));
+    B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
+    B200VS_CUDA(cudaMemcpyAsync(norms.p + dst, norms.p + src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+    if (mirror) {
+      B200VS_CUDA(cudaMemcpyAsync(vecs_h.p + (size_t)dst * d, vecs_h.p + (size_t)src * d, (size_t)n * d * 2, cudaMemcpyDeviceToDevice, s));
+      B200VS_CUDA(cudaMemcpyAsync(hscale.p + dst, hscale.p + src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+    }
+  }
+  // x / xids: device rows and ids; row i goes to slot slots[i]
+  void write(const float* x, const long long* xids, const std::vector<long long>& slots) {
+    const int64_t n = (int64_t)slots.size();
+    long long* d_slots = ix->scratch.alloc<long long>(n);
+    float* row_norms = ix->scratch.alloc<float>(n);
+    B200VS_CUDA(cudaMemcpyAsync(d_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    launch_scatter_rows(x, xids, d_slots, n, d, vecs.p, ids.p, norms.p, row_norms, s);
+    if (mirror) launch_half_rows(vecs.p, d_slots, n, d, vecs_h.p, hscale.p, s);  // re-derived from the stored rows
+    max_norm = std::max(max_norm, device_max_norm(ix, row_norms, n, s));
+  }
+  // ids[r] = -1 for every listed row
+  void tombstone(const std::vector<int64_t>& rows) {
+    if (rows.empty()) return;
+    long long* d_rows = ix->scratch.alloc<long long>(rows.size());
+    B200VS_CUDA(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, s));
+    launch_set_ids(ids.p, d_rows, (int64_t)rows.size(), -1, s);
+    B200VS_CUDA(cudaStreamSynchronize(s));
+  }
+  // compaction: fresh buffers of cap rows holding row src[i] at dst[i].  The mirror is re-derived from the moved FP32
+  // rows, which gives the same bits as moving the old mirror rows.
+  void gather(const std::vector<long long>& src, const std::vector<long long>& dst, int64_t cap) {
+    const int64_t n = (int64_t)src.size();
+    DevBuf<float> nv; DevBuf<long long> ni; DevBuf<float> nn;
+    nv.reserve((size_t)cap * d, 0, s); ni.reserve(cap, 0, s); nn.reserve(cap, 0, s);
+    long long* d_dst = nullptr;
+    if (n) {
+      long long* d_src = ix->scratch.alloc<long long>(n);
+      d_dst = ix->scratch.alloc<long long>(n);
+      B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), n * 8, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), n * 8, cudaMemcpyHostToDevice, s));
+      launch_move_rows(vecs.p, ids.p, norms.p, d_src, d_dst, n, d, nv.p, ni.p, nn.p, s);
+    }
+    B200VS_CUDA(cudaStreamSynchronize(s));
+    vecs.swap(nv); ids.swap(ni); norms.swap(nn);
+    if (mirror) {
+      vecs_h.free(); hscale.free();
+      grow(cap, 0);  // the FP32 arrays already hold cap rows: allocates the mirror only
+      if (mirror && n) launch_half_rows(vecs.p, d_dst, n, d, vecs_h.p, hscale.p, s);
+    }
+  }
+  int64_t bytes() const { return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + vecs_h.cap * 2 + hscale.cap * 4); }
+  // the row fields of a tile-scan view; the owner adds the list layout
+  TcView view() const {
+    TcView v;
+    v.vecs = vecs.p; v.ids = ids.p; v.norms = norms.p; v.max_norm = max_norm;
+    if (mirror) { v.vecs_h = vecs_h.p; v.hscale = hscale.p; }
+    return v;
+  }
+};
+
+// ============================================================================================
 // Flat
 // ============================================================================================
 struct FlatIndex : IndexBase {
-  DevBuf<float> vecs;
-  DevBuf<long long> ids;
-  DevBuf<float> norms;
+  RowStore store{this, false};  // no mirror: a Flat search keeps its TF32 arithmetic
   int64_t rows = 0;
   std::vector<int64_t> h_ids;
   std::unordered_map<int64_t, int64_t> id2row;
   int64_t ndeleted = 0;
   DevBuf<long long> d_off1;  // the single "list" of a Flat index, for the tile-scan view
   DevBuf<int> d_len1;
-  float max_norm = 0.f;
 
   FlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_FLAT, m, d, p) {
     d_off1.reserve(1, 0, stream); d_len1.reserve(1, 0, stream);
@@ -213,26 +308,14 @@ struct FlatIndex : IndexBase {
     B200VS_CUDA(cudaStreamSynchronize(stream));
   }
   TcView view() const {
-    TcView v;
-    v.vecs = vecs.p; v.ids = ids.p; v.norms = norms.p; v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
-    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks; v.max_norm = max_norm;
+    TcView v = store.view();
+    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
+    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
     return v;
   }
 
-  void reserve_rows(int64_t need) {
-    if ((size_t)need * dim <= vecs.cap) return;
-    int64_t ncap = std::max<int64_t>(need, std::max<int64_t>(1024, (int64_t)(vecs.cap / dim) * 3 / 2));
-    vecs.reserve((size_t)ncap * dim, (size_t)rows * dim, stream);
-    ids.reserve((size_t)ncap, (size_t)rows, stream);
-    norms.reserve((size_t)ncap, (size_t)rows, stream);
-  }
-
   void tombstone(const std::vector<int64_t>& rws) {
-    if (rws.empty()) return;
-    long long* d_rows = scratch.alloc<long long>(rws.size());
-    B200VS_CUDA(cudaMemcpyAsync(d_rows, rws.data(), rws.size() * 8, cudaMemcpyHostToDevice, stream));
-    launch_set_ids(ids.p, d_rows, (int64_t)rws.size(), -1, stream);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
+    store.tombstone(rws);
     for (int64_t r : rws) h_ids[r] = -1;
     ndeleted += (int64_t)rws.size();
   }
@@ -245,20 +328,7 @@ struct FlatIndex : IndexBase {
     const int64_t live = (int64_t)src.size();
     dst.resize(live);
     for (int64_t i = 0; i < live; ++i) dst[i] = i;
-    DevBuf<float> nv; DevBuf<long long> ni; DevBuf<float> nn;
-    const int64_t ncap = std::max<int64_t>(1024, live * 5 / 4);
-    nv.reserve((size_t)ncap * dim, 0, stream); ni.reserve(ncap, 0, stream); nn.reserve(ncap, 0, stream);
-    long long* d_src = scratch.alloc<long long>(live + 1);
-    long long* d_dst = scratch.alloc<long long>(live + 1);
-    if (live) {
-      B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), live * 8, cudaMemcpyHostToDevice, stream));
-      B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), live * 8, cudaMemcpyHostToDevice, stream));
-      launch_move_rows(vecs.p, ids.p, norms.p, d_src, d_dst, live, dim, nv.p, ni.p, nn.p, stream);
-    }
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    std::swap(vecs.p, nv.p); std::swap(vecs.cap, nv.cap);
-    std::swap(ids.p, ni.p); std::swap(ids.cap, ni.cap);
-    std::swap(norms.p, nn.p); std::swap(norms.cap, nn.cap);
+    store.gather(src, dst, std::max<int64_t>(1024, live * 5 / 4));
     std::vector<int64_t> nh(live);
     id2row.clear();
     for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
@@ -282,19 +352,16 @@ struct FlatIndex : IndexBase {
       if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
     }
     tombstone(dead);
-    reserve_rows(rows + n);
+    const int64_t cap = (int64_t)store.ids.cap;
+    if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
     float* st = scratch.alloc<float>((size_t)n * dim);
     long long* st_ids = scratch.alloc<long long>(n);
-    long long* st_slots = scratch.alloc<long long>(n);
     std::vector<long long> slots(n);
     for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
     B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(st_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, stream));
     if (metric == B200VS_COSINE && !loading) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
-    float* st_norms = scratch.alloc<float>(n);
-    launch_scatter_rows(st, st_ids, st_slots, n, dim, vecs.p, ids.p, norms.p, st_norms, stream);
-    max_norm = std::max(max_norm, device_max_norm(this, st_norms, n, stream));
+    store.write(st, st_ids, slots);
     B200VS_CUDA(cudaStreamSynchronize(stream));
     h_ids.resize(rows + n);
     for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = in_ids[i]; id2row[in_ids[i]] = rows + i; }
@@ -309,7 +376,7 @@ struct FlatIndex : IndexBase {
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
-    rows = 0; ndeleted = 0; max_norm = 0.f;
+    rows = 0; ndeleted = 0; store.max_norm = 0.f;
     h_ids.clear(); id2row.clear();
     publish_len();
   }
@@ -335,7 +402,7 @@ struct FlatIndex : IndexBase {
   ScanJob job(const SearchCtx& sc) const {
     ScanJob j;
     j.l2 = metric == B200VS_L2;
-    j.vecs = vecs.p; j.ids = ids.p; j.d = dim; j.mode = 0; j.n = rows; j.sc = &sc;
+    j.vecs = store.vecs.p; j.ids = store.ids.p; j.d = dim; j.mode = 0; j.n = rows; j.sc = &sc;
     return j;
   }
 
@@ -349,7 +416,7 @@ struct FlatIndex : IndexBase {
       return;
     }
     if (flat_small_eligible(device, nq, rows, dim, k, sc)) {  // one query per task is the reference's own shape: single-launch path
-      flat_small_search(this, metric == B200VS_L2, vecs.p, ids.p, rows, nq, q, k, sc, od, oi, s);
+      flat_small_search(this, metric == B200VS_L2, store.vecs.p, store.ids.p, rows, nq, q, k, sc, od, oi, s);
       return;
     }
     run_scan(this, job(sc), nq, q, k, od, nullptr, oi, nullptr, s);
@@ -385,13 +452,13 @@ struct FlatIndex : IndexBase {
       auto it = id2row.find(in_ids[i]);
       if (found) found[i] = it != id2row.end() ? 1 : 0;
       if (it != id2row.end())
-        B200VS_CUDA(cudaMemcpyAsync(out + (size_t)i * dim, vecs.p + (size_t)it->second * dim, (size_t)dim * 4, cudaMemcpyDeviceToHost, stream));
+        B200VS_CUDA(cudaMemcpyAsync(out + (size_t)i * dim, store.vecs.p + (size_t)it->second * dim, (size_t)dim * 4, cudaMemcpyDeviceToHost, stream));
     }
     B200VS_CUDA(cudaStreamSynchronize(stream));
   }
   int64_t count() const override { return rows - ndeleted; }
   int64_t deleted_count() const override { return ndeleted; }
-  int64_t memory_size() const override { return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4); }
+  int64_t memory_size() const override { return store.bytes(); }
 
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override {
     RwSharedGuard rl(this);
@@ -403,7 +470,7 @@ struct FlatIndex : IndexBase {
     if (vectors && ndeleted) tmp.resize((size_t)rows * dim);
     if (vectors) {
       float* dst = ndeleted ? tmp.data() : vectors;
-      B200VS_CUDA(cudaMemcpy(dst, vecs.p, (size_t)rows * dim * 4, cudaMemcpyDeviceToHost));
+      B200VS_CUDA(cudaMemcpy(dst, store.vecs.p, (size_t)rows * dim * 4, cudaMemcpyDeviceToHost));
     }
     int64_t o = 0;
     for (int64_t r = 0; r < rows; ++r) {
@@ -427,16 +494,8 @@ struct IvfFlatIndex : IndexBase {
   DevBuf<float> centroids;       // [nlist, d]
   DevBuf<long long> cent_ids;    // iota
   DevBuf<float> cent_norms;      // ||c||^2 (tensor-core coarse pass)
-  DevBuf<float> vecs;            // arena [arena_cap, d]
-  DevBuf<long long> ids;         // arena
-  DevBuf<float> norms;           // arena
-  // FP16 mirror of the arena, kept in lockstep with vecs: the tile list scan streams it instead of the FP32 rows (half
-  // the bytes; DESIGN.md 3, 4.2).  Kept when dim % 8 == 0 (16-byte FP16 row pitch for TMA) and while it could be allocated.
-  DevBuf<__half> vecs_h;         // [arena_cap, d]  RN(x * 2^-e) per row
-  DevBuf<float> hscale;          // [arena_cap]     2^e
-  bool mirror = false;
+  RowStore store{this, true};    // the arena, [L.arena_cap] rows, with the FP16 mirror the list scan streams
   IvfLists L;                    // host bookkeeping + device list_off/list_len
-  float max_norm = 0.f;
   float cent_max_norm = 0.f;
   DevBuf<float> cent_hi, cent_lo;  // error-compensated split of the centroids (tc_coarse)
   DevBuf<long long> d_coff;  // the centroid table seen as one "list" by the tensor-core coarse pass
@@ -449,28 +508,11 @@ struct IvfFlatIndex : IndexBase {
     return v;
   }
   TcView view() const {
-    TcView v;
-    v.vecs = vecs.p; v.ids = ids.p; v.norms = norms.p; v.arena_rows = L.arena_used; v.list_off = L.d_off.p; v.list_len = L.d_len.p;
-    v.nlist = nlist; v.total_chunks = L.total_chunks; v.max_chunks_per_list = L.max_chunks_per_list; v.max_norm = max_norm;
-    v.owned_frac = nlist > 0 ? (float)L.nonempty_lists / (float)nlist : 1.f;
-    if (mirror) { v.vecs_h = vecs_h.p; v.hscale = hscale.p; }
+    TcView v = store.view();
+    v.arena_rows = L.arena_used; v.list_off = L.d_off.p; v.list_len = L.d_len.p;
+    v.nlist = nlist; v.total_chunks = L.total_chunks; v.max_chunks_per_list = L.max_chunks_per_list;
     return v;
   }
-
-  // grow the mirror with the arena (rows_cap rows, the first `keep` kept).  Out of device memory drops the mirror, and
-  // the list scan streams the FP32 rows instead.
-  void mirror_reserve(int64_t rows_cap, int64_t keep) {
-    if (!mirror) return;
-    try {
-      vecs_h.reserve((size_t)rows_cap * dim, (size_t)keep * dim, stream);
-      hscale.reserve((size_t)rows_cap, (size_t)keep, stream);
-    } catch (const CudaError&) {
-      if (cudaGetLastError() != cudaErrorMemoryAllocation) throw;
-      vecs_h.free(); hscale.free();
-      mirror = false;
-    }
-  }
-  void mirror_reset() { vecs_h.free(); hscale.free(); mirror = dim % 8 == 0; }
 
   IvfFlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_IVF_FLAT, m, d, p) {
     nlist = p.nlist > 0 ? p.nlist : 2048;  // Constant::kCreateIvfFlatParamNcentroids
@@ -497,8 +539,7 @@ struct IvfFlatIndex : IndexBase {
     B200VS_CUDA(cudaMemcpyAsync(d_clen.p, &k, 4, cudaMemcpyHostToDevice, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
     L.init(k, stream);
-    vecs.free(); ids.free(); norms.free();
-    mirror_reset();
+    store.reset();
     trained = true;
   }
 
@@ -589,7 +630,7 @@ struct IvfFlatIndex : IndexBase {
   ScanJob list_job(const SearchCtx& sc, const long long* probes, int nprobe) const {
     ScanJob j;
     j.l2 = metric == B200VS_L2;
-    j.vecs = vecs.p; j.ids = ids.p; j.d = dim; j.mode = 1; j.probes = probes; j.nprobe = nprobe;
+    j.vecs = store.vecs.p; j.ids = store.ids.p; j.d = dim; j.mode = 1; j.probes = probes; j.nprobe = nprobe;
     j.list_off = L.d_off.p; j.list_len = L.d_len.p; j.sc = &sc;
     j.avg_candidates = nlist > 0 ? (double)L.total_len() * nprobe / nlist : 0;
     return j;
@@ -598,10 +639,11 @@ struct IvfFlatIndex : IndexBase {
   int64_t count() const override { return L.live; }
   int64_t deleted_count() const override { return L.dead; }
   int64_t memory_size() const override {
-    return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + centroids.cap * 4 + vecs_h.cap * 2 + hscale.cap * 4);
+    return store.bytes() + (int64_t)centroids.cap * 4;
   }
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override;
   int64_t export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) override;
+  int64_t copy_list(int list, int64_t cap, float* vectors, int64_t* out_ids);
 };
 
 void IvfFlatIndex::train(int64_t n, const float* x) {
@@ -692,7 +734,6 @@ void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, con
     h_ids_in = h_ids_buf.data();
   }
   if (upsert) remove_locked(n, h_ids_in);  // ivf_flat.cc:115-118
-  long long* st_slots = scratch.alloc<long long>(n);
   if (metric == B200VS_COSINE && !prepared) launch_normalize_faiss(st, n, dim, stream);
   const long long* st_list = lists_dev;
   if (!st_list) {
@@ -709,26 +750,10 @@ void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, con
     if (h_list[i] < 0 || h_list[i] >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
     need[h_list[i]]++;
   }
-  L.reserve_for(need, [&](int64_t arena_rows) {
-    vecs.reserve((size_t)arena_rows * dim, (size_t)L.arena_used_before * dim, stream);
-    ids.reserve((size_t)arena_rows, (size_t)L.arena_used_before, stream);
-    norms.reserve((size_t)arena_rows, (size_t)L.arena_used_before, stream);
-    mirror_reserve(arena_rows, L.arena_used_before);
-  }, [&](int64_t src, int64_t dst, int64_t len) {
-    B200VS_CUDA(cudaMemcpyAsync(vecs.p + (size_t)dst * dim, vecs.p + (size_t)src * dim, (size_t)len * dim * 4, cudaMemcpyDeviceToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)len * 8, cudaMemcpyDeviceToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(norms.p + dst, norms.p + src, (size_t)len * 4, cudaMemcpyDeviceToDevice, stream));
-    if (mirror) {
-      B200VS_CUDA(cudaMemcpyAsync(vecs_h.p + (size_t)dst * dim, vecs_h.p + (size_t)src * dim, (size_t)len * dim * 2, cudaMemcpyDeviceToDevice, stream));
-      B200VS_CUDA(cudaMemcpyAsync(hscale.p + dst, hscale.p + src, (size_t)len * 4, cudaMemcpyDeviceToDevice, stream));
-    }
-  });
+  L.reserve_for(need, [&](int64_t arena_rows) { store.grow(arena_rows, L.arena_used_before); },
+                [&](int64_t src, int64_t dst, int64_t len) { store.move(src, dst, len); });
   for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], h_ids_in[i]);
-  B200VS_CUDA(cudaMemcpyAsync(st_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-  float* st_norms = scratch.alloc<float>(n);
-  launch_scatter_rows(st, st_ids, st_slots, n, dim, vecs.p, ids.p, norms.p, st_norms, stream);
-  if (mirror) launch_half_rows(vecs.p, st_slots, n, dim, vecs_h.p, hscale.p, stream);
-  max_norm = std::max(max_norm, device_max_norm(this, st_norms, n, stream));
+  store.write(st, st_ids, slots);
   L.upload(stream);
   B200VS_CUDA(cudaStreamSynchronize(stream));
 }
@@ -754,13 +779,9 @@ void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
   const int64_t tail = std::max<int64_t>(used / 64, 4096);  // room for lists that still outgrow their reservation
   L.arena_used = L.arena_used_before = used;
   L.arena_cap = used + tail;
-  vecs.free(); ids.free(); norms.free();
-  vecs.reserve((size_t)L.arena_cap * dim, 0, stream);
-  ids.reserve((size_t)L.arena_cap, 0, stream);
-  norms.reserve((size_t)L.arena_cap, 0, stream);
-  mirror_reset();
-  mirror_reserve(L.arena_cap, 0);
-  B200VS_CUDA(cudaMemsetAsync(ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
+  store.reset();
+  store.grow(L.arena_cap, 0);
+  B200VS_CUDA(cudaMemsetAsync(store.ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
   L.h_ids.assign(L.arena_cap, -1);
   L.upload(stream);
 }
@@ -768,12 +789,7 @@ void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
 int64_t IvfFlatIndex::remove_locked(int64_t n, const int64_t* del) {
   std::vector<int64_t> rws;
   L.remove_ids(n, del, rws);
-  if (!rws.empty()) {
-    long long* d_rows = scratch.alloc<long long>(rws.size());
-    B200VS_CUDA(cudaMemcpyAsync(d_rows, rws.data(), rws.size() * 8, cudaMemcpyHostToDevice, stream));
-    launch_set_ids(ids.p, d_rows, (int64_t)rws.size(), -1, stream);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
+  store.tombstone(rws);
   return (int64_t)rws.size();
 }
 
@@ -781,28 +797,7 @@ void IvfFlatIndex::maybe_compact() {
   if (!L.needs_compaction()) return;
   std::vector<long long> src, dst;
   const int64_t new_rows = L.plan_compaction(src, dst);
-  DevBuf<float> nv; DevBuf<long long> ni; DevBuf<float> nn;
-  nv.reserve((size_t)std::max<int64_t>(new_rows, 1) * dim, 0, stream);
-  ni.reserve(std::max<int64_t>(new_rows, 1), 0, stream);
-  nn.reserve(std::max<int64_t>(new_rows, 1), 0, stream);
-  const int64_t m = (int64_t)src.size();
-  long long* d_dst = nullptr;
-  if (m) {
-    long long* d_src = scratch.alloc<long long>(m);
-    d_dst = scratch.alloc<long long>(m);
-    B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), m * 8, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), m * 8, cudaMemcpyHostToDevice, stream));
-    launch_move_rows(vecs.p, ids.p, norms.p, d_src, d_dst, m, dim, nv.p, ni.p, nn.p, stream);
-  }
-  B200VS_CUDA(cudaStreamSynchronize(stream));
-  std::swap(vecs.p, nv.p); std::swap(vecs.cap, nv.cap);
-  std::swap(ids.p, ni.p); std::swap(ids.cap, ni.cap);
-  std::swap(norms.p, nn.p); std::swap(norms.cap, nn.cap);
-  if (mirror) {  // re-derived from the moved FP32 rows: the same bits as moving the old mirror rows
-    vecs_h.free(); hscale.free();
-    mirror_reserve(std::max<int64_t>(new_rows, 1), 0);
-    if (mirror && m) launch_half_rows(vecs.p, d_dst, m, dim, vecs_h.p, hscale.p, stream);
-  }
+  store.gather(src, dst, std::max<int64_t>(new_rows, 1));
   L.commit_compaction();
   L.upload(stream);
   B200VS_CUDA(cudaStreamSynchronize(stream));
@@ -902,23 +897,10 @@ void IvfFlatIndex::export_lists(int64_t* list_off, float* vectors, uint8_t*, int
   RwSharedGuard rl(this);
   std::lock_guard<std::mutex> gl(gpu_mu);
   set_device();
-  std::vector<float> rowbuf;
   int64_t o = 0;
   for (int l = 0; l < nlist; ++l) {
     if (list_off) list_off[l] = o;
-    const auto& m = L.lists[l];
-    if (m.len == 0) continue;
-    if (vectors) {
-      rowbuf.resize((size_t)m.len * dim);
-      B200VS_CUDA(cudaMemcpy(rowbuf.data(), vecs.p + (size_t)m.off * dim, (size_t)m.len * dim * 4, cudaMemcpyDeviceToHost));
-    }
-    for (int p = 0; p < m.len; ++p) {
-      const int64_t id = L.h_ids[m.off + p];
-      if (id < 0) continue;
-      if (out_ids) out_ids[o] = id;
-      if (vectors) memcpy(vectors + (size_t)o * dim, rowbuf.data() + (size_t)p * dim, (size_t)dim * 4);
-      ++o;
-    }
+    o += copy_list(l, INT64_MAX, vectors ? vectors + (size_t)o * dim : nullptr, out_ids ? out_ids + o : nullptr);
   }
   if (list_off) list_off[nlist] = o;
 }
@@ -929,11 +911,17 @@ int64_t IvfFlatIndex::export_list(int list, int64_t cap, float* vectors, int64_t
   if (list < 0 || list >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
   set_device();
   quiesce();
+  return copy_list(list, cap, vectors, out_ids);
+}
+
+// the live rows of one list, in list order: the first `cap` go to vectors / out_ids (either may be null); returns how many
+// there are.  The caller holds rw (shared) and gpu_mu.
+int64_t IvfFlatIndex::copy_list(int list, int64_t cap, float* vectors, int64_t* out_ids) {
   const auto& m = L.lists[list];
   std::vector<float> rowbuf;
   if (vectors && m.len) {
     rowbuf.resize((size_t)m.len * dim);
-    B200VS_CUDA(cudaMemcpy(rowbuf.data(), vecs.p + (size_t)m.off * dim, (size_t)m.len * dim * 4, cudaMemcpyDeviceToHost));
+    B200VS_CUDA(cudaMemcpy(rowbuf.data(), store.vecs.p + (size_t)m.off * dim, (size_t)m.len * dim * 4, cudaMemcpyDeviceToHost));
   }
   int64_t o = 0;
   for (int p = 0; p < m.len; ++p) {

@@ -38,14 +38,23 @@ struct DevBuf {
   DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { if (p) cudaFree(p); }
   void free() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  void swap(DevBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
   // grow to >= n elements; keeps the first `keep` elements (copied on `s`)
   void reserve(size_t n, size_t keep, cudaStream_t s) {
-    if (n <= cap) return;
+    if (!try_reserve(n, keep, s)) throw CudaError("cudaMalloc of " + std::to_string(n * sizeof(T)) + " B failed: out of memory");
+  }
+  // reserve() that returns false, changing nothing, when the device is out of memory.  The failed allocation is cleared
+  // from the runtime's last error, so a later cudaGetLastError() check does not report it again.
+  bool try_reserve(size_t n, size_t keep, cudaStream_t s) {
+    if (n <= cap) return true;
     T* np = nullptr;
-    B200VS_CUDA(cudaMalloc(&np, n * sizeof(T)));
+    const cudaError_t e = cudaMalloc(&np, n * sizeof(T));
+    if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); return false; }
+    B200VS_CUDA(e);
     if (keep && p) B200VS_CUDA(cudaMemcpyAsync(np, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s));
     if (p) { B200VS_CUDA(cudaStreamSynchronize(s)); cudaFree(p); }
     p = np; cap = n;
+    return true;
   }
 };
 

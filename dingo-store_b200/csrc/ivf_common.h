@@ -32,7 +32,6 @@ struct IvfLists {
   int64_t live = 0, dead = 0, garbage = 0;
   int64_t total_chunks = 0;      // sum of ceil(len / 512) — tensor-core work-item bound (tc_scan.cuh TC_CHUNK = 512)
   int max_chunks_per_list = 0;
-  int nonempty_lists = 0;        // lists that hold rows here (a list-sharded rank owns only some)
   DevBuf<long long> d_off;
   DevBuf<int> d_len;
   // compaction plan
@@ -56,12 +55,11 @@ struct IvfLists {
     const size_t n = lists.size();
     std::vector<long long> off(n);
     std::vector<int> len(n);
-    total_chunks = 0; max_chunks_per_list = 0; nonempty_lists = 0;
+    total_chunks = 0; max_chunks_per_list = 0;
     for (size_t i = 0; i < n; ++i) {
       off[i] = lists[i].off; len[i] = lists[i].len;
       const int c = (lists[i].len + 511) / 512;
       total_chunks += c; max_chunks_per_list = std::max(max_chunks_per_list, c);
-      if (lists[i].len > 0) ++nonempty_lists;
     }
     B200VS_CUDA(cudaMemcpyAsync(d_off.p, off.data(), n * 8, cudaMemcpyHostToDevice, s));
     B200VS_CUDA(cudaMemcpyAsync(d_len.p, len.data(), n * 4, cudaMemcpyHostToDevice, s));

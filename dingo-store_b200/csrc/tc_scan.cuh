@@ -88,7 +88,6 @@ struct TcView {
   const float* vecs_lo = nullptr;  //   hi = x with the low 13 mantissa bits cleared, lo = x - hi (both exact)
   bool flat = false;         // single list covering rows [0, arena_rows)
   long long id_offset = 0;   // tc_coarse on a slice of the centroid table: added to the returned row indices
-  float owned_frac = 1.f;    // share of the lists that hold rows here (a list-sharded rank owns 1 / world of them)
   bool api_scores = false;   // tc_coarse: return the ascending ranking score (L2 distance | -ip) instead of the raw metric value
   const __half* vecs_h = nullptr;  // optional FP16 mirror of vecs (x * 2^-e per row, rounded to nearest): the list scan
   const float* hscale = nullptr;   //   streams it instead of the FP32 rows; hscale[r] = 2^e (DESIGN.md 3, 4.2)
