@@ -12,6 +12,7 @@
 //
 // Replaces faiss exhaustive_{L2sqr,inner_product}_seq + HeapBlockResultHandler behind VectorIndexFlat::Search
 // (src/vector/vector_index_flat.cc:249-252) for nq < 16.
+#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 
@@ -216,10 +217,25 @@ static __global__ void __launch_bounds__(FS_THREADS) flat_small_kernel(const FsA
   }
 }
 
+constexpr int FS_MAX_D = 2048;
+constexpr size_t FS_MAX_SMEM = (size_t)FS_PAIRS * 12 + (size_t)FS_MAX_D * 4;  // pair buffer + query row: 44 KB at d = 2048
+
+// The pair buffer (36 KB) plus a query row of up to 8 KB is requested as dynamic shared memory; with the kernel's ~6 KB of
+// static shared memory that passes the 48 KB a launch gets without opting in once d > 1592.  Both instantiations are opted
+// in to the largest request once per device.
+static void fs_opt_in(int device) {
+  static std::atomic<bool> done[64];
+  const bool cached = device >= 0 && device < 64;
+  if (cached && done[device].load(std::memory_order_acquire)) return;
+  B200VS_CUDA(cudaFuncSetAttribute(flat_small_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_MAX_SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(flat_small_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FS_MAX_SMEM));
+  if (cached) done[device].store(true, std::memory_order_release);
+}
+
 bool flat_small_eligible(int device, int64_t nq, int64_t n, int d, int k, const SearchCtx& sc) {
   if (sc.exact_only) return false;              // "exact_only" callers ask for the general path explicitly (tests compare the two)
   if (nq < 1 || nq >= 16 || n < 4096) return false;
-  if (2 * k > FS_CT || d > 2048) return false;  // rank-sort buffer; query row + pair buffer within 48 KB of dynamic shared memory
+  if (2 * k > FS_CT || d > FS_MAX_D) return false;  // rank-sort buffer; pair buffer + query row = FS_MAX_SMEM (launcher opts in past 48 KB)
   if (nq > 4 && (double)n * d * 4 > 40e6) return false;  // more than a few queries re-stream the table: only while it stays in L2 (50 MB on an H100)
   const int nslices = std::min(2 * device_sm_count(device), FS_PAIRS / std::max(1, k));
   return cdiv(n, nslices) <= FS_PAIRS;          // a slice's rows must fit the pair buffer (tables beyond ~900 K rows: general path)
@@ -247,6 +263,8 @@ void flat_small_search(IndexBase* ix, bool l2, const float* vecs, const long lon
   a.dbg = debug ? S.alloc<long long>(8) : nullptr;
   B200VS_CUDA(cudaMemsetAsync(a.tickets, 0, (size_t)nq * 8, s));
   const size_t smem = (size_t)FS_PAIRS * 12 + ((size_t)d * 4 + 15) / 16 * 16;
+  if (smem > FS_MAX_SMEM) fail(B200VS_EINTERNAL, "flat_small_search called on an ineligible dimension");
+  fs_opt_in(ix->device);
   dim3 grid(nslices, (unsigned)nq);
   if (l2) flat_small_kernel<true><<<grid, FS_THREADS, smem, s>>>(a);
   else flat_small_kernel<false><<<grid, FS_THREADS, smem, s>>>(a);

@@ -14,7 +14,8 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("metric,om", [(b200vs.L2, oracle_lib.L2), (b200vs.IP, oracle_lib.IP), (b200vs.COSINE, oracle_lib.COSINE)])
-@pytest.mark.parametrize("n,d,k", [(100_000, 128, 10), (5000, 96, 1), (33_333, 100, 32), (20_000, 7, 10)])
+@pytest.mark.parametrize("n,d,k", [(100_000, 128, 10), (5000, 96, 1), (33_333, 100, 32), (20_000, 7, 10),
+                                   (4096, 2048, 64)])
 def test_flat_small_batches_match_oracle(oracle, metric, om, n, d, k):
     require_gpu()
     rng = np.random.default_rng(n + d)
