@@ -499,12 +499,14 @@ struct IvfFlatIndex : IndexBase {
   float cent_max_norm = 0.f;
   DevBuf<float> cent_hi, cent_lo;  // error-compensated split of the centroids (tc_coarse)
   DevBuf<long long> d_coff;  // the centroid table seen as one "list" by the tensor-core coarse pass
-  DevBuf<int> d_clen;
-  TcView cent_view() const {
+  // Centroid rows [c0, c0 + rows) of a centroid table (the installed one, or k-means' current one), with its error-compensated
+  // split and norms, as the one list tc_coarse scans; the rows it returns are numbered from c0.
+  TcView coarse_view(const float* vecs, const float* hi, const float* lo, const float* norms, float max_norm, int c0, int rows) const {
     TcView v;
-    v.vecs = centroids.p; v.ids = cent_ids.p; v.norms = cent_norms.p; v.arena_rows = nlist; v.list_off = d_coff.p; v.list_len = d_clen.p;
-    v.nlist = 1; v.flat = true; v.total_chunks = (nlist + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
-    v.max_norm = cent_max_norm; v.vecs_hi = cent_hi.p; v.vecs_lo = cent_lo.p;
+    v.vecs = vecs + (size_t)c0 * dim; v.vecs_hi = hi + (size_t)c0 * dim; v.vecs_lo = lo + (size_t)c0 * dim;
+    v.ids = cent_ids.p + c0; v.norms = norms + c0; v.max_norm = max_norm; v.id_offset = c0;
+    v.arena_rows = rows; v.list_off = d_coff.p;
+    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
     return v;
   }
   TcView view() const {
@@ -534,9 +536,8 @@ struct IvfFlatIndex : IndexBase {
     cent_hi.reserve((size_t)k * dim, 0, stream); cent_lo.reserve((size_t)k * dim, 0, stream);
     launch_split_rows(centroids.p, k, dim, cent_hi.p, cent_lo.p, stream);
     cent_max_norm = device_max_norm(this, cent_norms.p, k, stream);
-    d_coff.reserve(1, 0, stream); d_clen.reserve(1, 0, stream);
+    d_coff.reserve(1, 0, stream);
     B200VS_CUDA(cudaMemsetAsync(d_coff.p, 0, 8, stream));
-    B200VS_CUDA(cudaMemcpyAsync(d_clen.p, &k, 4, cudaMemcpyHostToDevice, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
     L.init(k, stream);
     store.reset();
@@ -618,7 +619,8 @@ struct IvfFlatIndex : IndexBase {
   long long* coarse(int64_t nq, const float* q, int nprobe, cudaStream_t s, bool allow_tc = true, long long* out = nullptr) {
     long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
     if (allow_tc && tc_coarse_eligible(this, nq, nlist, nprobe)) {  // dense TF32 scores + certified exact re-score
-      tc_coarse(this, cent_view(), metric == B200VS_L2, nq, q, nprobe, probes, nullptr, s);
+      tc_coarse(this, coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, 0, nlist), metric == B200VS_L2, nq, q,
+                nprobe, probes, nullptr, s);
       return probes;
     }
     ScanJob j;
@@ -670,9 +672,7 @@ void IvfFlatIndex::train(int64_t n, const float* x) {
       float* nr = scratch.alloc<float>(kk);
       launch_split_rows(cd, kk, dim, hi, lo, stream);
       launch_row_norms(cd, kk, dim, nr, stream);
-      cv.vecs = cd; cv.ids = cent_ids.p; cv.norms = nr; cv.arena_rows = kk; cv.list_off = d_coff.p; cv.list_len = nullptr;
-      cv.nlist = 1; cv.flat = true; cv.total_chunks = (kk + TC_CHUNK - 1) / TC_CHUNK; cv.max_chunks_per_list = (int)cv.total_chunks;
-      cv.max_norm = device_max_norm(this, nr, kk, stream); cv.vecs_hi = hi; cv.vecs_lo = lo;
+      cv = coarse_view(cd, hi, lo, nr, device_max_norm(this, nr, kk, stream), 0, kk);
     }
     ScanJob j;
     j.l2 = metric == B200VS_L2;
@@ -843,10 +843,8 @@ void IvfFlatIndex::coarse_range_dev(int64_t nq, const float* xq, int nprobe, int
   const float* q = prepare_queries(nq, xq, s);
   const int rows = c1 - c0;
   if (tc_coarse_eligible(this, nq, rows, nprobe)) {
-    TcView v = cent_view();
-    v.vecs += (size_t)c0 * dim; v.vecs_hi += (size_t)c0 * dim; v.vecs_lo += (size_t)c0 * dim; v.ids += c0; v.norms += c0;
-    v.arena_rows = rows; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
-    v.id_offset = c0; v.api_scores = true;
+    TcView v = coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, c0, rows);
+    v.api_scores = true;
     tc_coarse(this, v, metric == B200VS_L2, nq, q, nprobe, out_lists, out_score, s);
     return;
   }

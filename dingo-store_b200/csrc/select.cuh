@@ -15,6 +15,31 @@
 
 namespace b200vs {
 
+// In-place block-wide bitonic sort of kd / kid[0, n), ascending by (key, id).  Only the smallest power of two m >= max(n, 2)
+// is sorted: [n, m) is filled with sentinels first, so both arrays must hold m entries.  All threads call.
+__device__ __forceinline__ void block_bitonic_sort(uint32_t* kd, long long* kid, int n) {
+  int m = 2;
+  while (m < n) m <<= 1;
+  __syncthreads();
+  for (int i = n + threadIdx.x; i < m; i += blockDim.x) { kd[i] = KEY_SENTINEL_D; kid[i] = KEY_SENTINEL_ID; }
+  __syncthreads();
+  for (int size = 2; size <= m; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = threadIdx.x; i < (m >> 1); i += blockDim.x) {
+        const int pos = 2 * i - (i & (stride - 1));
+        const int j = pos + stride;
+        const bool up = ((pos & size) == 0);
+        const uint32_t ad = kd[pos], bd = kd[j];
+        const long long ai = kid[pos], bi = kid[j];
+        const bool lt = key_less(bd, bi, ad, ai);  // b < a
+        const bool gt = key_less(ad, ai, bd, bi);  // a < b
+        if (up ? lt : gt) { kd[pos] = bd; kd[j] = ad; kid[pos] = bi; kid[j] = ai; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 struct BlockSelect {
   uint32_t* kd;    // [cap]
   long long* kid;  // [cap]
@@ -47,37 +72,11 @@ struct BlockSelect {
     kd[p] = d; kid[p] = id;
   }
 
-  // in-place bitonic sort of the whole pool (ascending); all threads call
-  __device__ void sort_pool() {
-    const int n = *count;
-    // only sort the smallest power of two covering n (the rest of the pool is never read)
-    int m = 2;
-    while (m < n) m <<= 1;
-    __syncthreads();
-    for (int i = n + threadIdx.x; i < m; i += blockDim.x) { kd[i] = KEY_SENTINEL_D; kid[i] = KEY_SENTINEL_ID; }
-    __syncthreads();
-    for (int size = 2; size <= m; size <<= 1) {
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        for (int i = threadIdx.x; i < (m >> 1); i += blockDim.x) {
-          const int pos = 2 * i - (i & (stride - 1));
-          const int j = pos + stride;
-          const bool up = ((pos & size) == 0);
-          const uint32_t ad = kd[pos], bd = kd[j];
-          const long long ai = kid[pos], bi = kid[j];
-          const bool lt = key_less(bd, bi, ad, ai);  // b < a
-          const bool gt = key_less(ad, ai, bd, bi);  // a < b
-          if (up ? lt : gt) { kd[pos] = bd; kd[j] = ad; kid[pos] = bi; kid[j] = ai; }
-        }
-        __syncthreads();
-      }
-    }
-  }
-
   // sort, keep best k, tighten threshold; all threads call
   __device__ void prune() {
     __syncthreads();
     const int n = *count;
-    sort_pool();
+    block_bitonic_sort(kd, kid, n);  // the pool's capacity is a power of two >= n
     if (threadIdx.x == 0) {
       *count = n < k ? n : k;
       if (n >= k) { *thr_d = kd[k - 1]; *thr_id = kid[k - 1]; }

@@ -24,6 +24,7 @@
 #include <cstdlib>
 #include <vector>
 #include <mutex>
+#include <type_traits>
 
 #include "scan_kernels.cuh"
 #include "sm90_ptx.cuh"
@@ -154,6 +155,9 @@ static __global__ void tc_count_pairs_kernel(const long long* __restrict__ probe
   pos[i] = l >= 0 ? atomicAdd(cnt + l, 1) : -1;
 }
 
+// A work item's nq queries fill a B tile of 16 << tc_bcols_log(nq) = 16 / 32 / 64 / 128 rows (the wgmma N), read through TcMaps::b[]
+__device__ __forceinline__ int tc_bcols_log(int nq) { return nq <= 16 ? 0 : (nq <= 32 ? 1 : (nq <= 64 ? 2 : 3)); }
+
 __device__ __forceinline__ int tc_items_of(int c, int len) {
   return (c > 0 && len > 0) ? ((c + TC_NQT - 1) / TC_NQT) * ((len + TC_CHUNK - 1) / TC_CHUNK) : 0;
 }
@@ -240,7 +244,7 @@ static __global__ void tc_items_kernel(const int* __restrict__ cnt, const int* _
       it.pad[0] = it.pad[1] = 0;
       items[base + ch * ng + g] = it;
       // profiling aid: tensor-core work = 128-row tiles x padded query columns
-      atomicAdd(totals + 3, ((it.row_end - it.row_begin + TC_BM - 1) / TC_BM) * (it.nq <= 16 ? 16 : (it.nq <= 32 ? 32 : (it.nq <= 64 ? 64 : 128))));
+      atomicAdd(totals + 3, ((it.row_end - it.row_begin + TC_BM - 1) / TC_BM) * (16 << tc_bcols_log(it.nq)));
     }
 }
 
@@ -348,7 +352,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
       hs[h] = 1.f;
       if (inrange[h]) {
         id[h] = p.ids[arow[h]];
-        if (p.l2 && p.add_norm) nrm[h] = p.norms[arow[h]];
+        if (p.l2) nrm[h] = p.norms[arow[h]];
         if constexpr (HALF) hs[h] = p.hscale[arow[h]];
       }
     }
@@ -387,9 +391,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
             } else if (p.mode == 0) {
               if (t == 0 && r < TC_SAMPLE) p.sample[((size_t)I.sample_slot * TC_NQT + n) * TC_SAMPLE + r] = valid[h] ? score : TC_INF;
             } else if (inrange[h]) {
-              float* dst = p.dense + (size_t)s_q[n] * p.dense_ld + (I.row_begin + r);
-              if (p.dense_accum) *dst = *dst + score;
-              else *dst = valid[h] ? score : TC_INF;
+              p.dense[(size_t)s_q[n] * p.dense_ld + (I.row_begin + r)] = valid[h] ? score : TC_INF;
             }
           }
         }
@@ -397,14 +399,15 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
   }
 }
 
+// The tile kernel's TMA descriptors (make_tc_maps): a / a32 = the A rows in 128-row / 32-row boxes, b[i] = the B block in
+// 16 << i row boxes, a_lo / b_lo = the split pass's lo operands (the hi maps again when there are none).  The kernel only
+// takes the maps' addresses: a copy would land in local memory, where TMA cannot read it.
+struct TcMaps {
+  CUtensorMap a, a32, b[4], a_lo, b_lo[4];
+};
+
 template <bool HALF>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA32,
-               const __grid_constant__ CUtensorMap tmB16, const __grid_constant__ CUtensorMap tmB32,
-               const __grid_constant__ CUtensorMap tmB64, const __grid_constant__ CUtensorMap tmB128,
-               const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo16,
-               const __grid_constant__ CUtensorMap tmBlo32, const __grid_constant__ CUtensorMap tmBlo64,
-               const __grid_constant__ CUtensorMap tmBlo128, const TcParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
@@ -425,7 +428,8 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x < TC_CWARPS) s_hit_n[threadIdx.x] = 0;
   if (warp == TC_CWARPS && lane == 0) {
-    prefetch_tmap(&tmA); prefetch_tmap(&tmA32); prefetch_tmap(&tmB16); prefetch_tmap(&tmB32); prefetch_tmap(&tmB64); prefetch_tmap(&tmB128);
+    prefetch_tmap(&maps.a); prefetch_tmap(&maps.a32);
+    for (int i = 0; i < 4; ++i) prefetch_tmap(&maps.b[i]);
     for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], TC_CWARPS); }
     for (int i = 0; i < TC_SQ; ++i) { mbar_init(&sched_full[i], 1); mbar_init(&sched_empty[i], TC_CWARPS); }
     fence_barrier_init();
@@ -452,12 +456,12 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int rows = I.row_end - I.row_begin;
         if (p.mode == 0) rows = min(rows, TC_SAMPLE);
         const int ntiles = (rows + TC_BM - 1) / TC_BM;
-        const int b_rows = I.nq <= 16 ? 16 : (I.nq <= 32 ? 32 : (I.nq <= 64 ? 64 : 128));
-        const CUtensorMap* tb = I.nq <= 16 ? &tmB16 : (I.nq <= 32 ? &tmB32 : (I.nq <= 64 ? &tmB64 : &tmB128));
+        const int bl = tc_bcols_log(I.nq);
+        const CUtensorMap* tb = &maps.b[bl];
         const bool small_a = p.mode == 0;  // 32-row sample box, else the full 128-row tile
-        const CUtensorMap* ta = small_a ? &tmA32 : &tmA;
-        const uint32_t bytes = (small_a ? (uint32_t)(TC_SAMPLE * 128) : TC_A_BYTES) + (uint32_t)b_rows * 128u;
-        const CUtensorMap* tbl = I.nq <= 16 ? &tmBlo16 : (I.nq <= 32 ? &tmBlo32 : (I.nq <= 64 ? &tmBlo64 : &tmBlo128));
+        const CUtensorMap* ta = small_a ? &maps.a32 : &maps.a;
+        const uint32_t bytes = (small_a ? (uint32_t)(TC_SAMPLE * 128) : TC_A_BYTES) + (16u << bl) * 128u;
+        const CUtensorMap* tbl = &maps.b_lo[bl];
         for (int t = 0; t < ntiles; ++t)
           for (int kb = 0; kb < kblocks; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -469,7 +473,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_arrive_expect_tx(&full_bar[stage], bytes - saved);
             if (nbox) {
               for (int j = 0; j < nbox; ++j)
-                tma_load_2d(sA + (size_t)stage * TC_A_BYTES + (size_t)j * (TC_SAMPLE * 128), &tmA32, &full_bar[stage], kb * kbk,
+                tma_load_2d(sA + (size_t)stage * TC_A_BYTES + (size_t)j * (TC_SAMPLE * 128), &maps.a32, &full_bar[stage], kb * kbk,
                             (int)(base_row + (long long)t * TC_BM + j * TC_SAMPLE), kEvictFirst);
             } else
             tma_load_2d(sA + (size_t)stage * TC_A_BYTES, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
@@ -478,7 +482,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (!HALF && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
               mbar_wait(&empty_bar[stage], phase ^ 1);
               mbar_arrive_expect_tx(&full_bar[stage], bytes);
-              tma_load_2d(sA + (size_t)stage * TC_A_BYTES, &tmAlo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+              tma_load_2d(sA + (size_t)stage * TC_A_BYTES, &maps.a_lo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
               tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tbl, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
               if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
             }
@@ -508,13 +512,15 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (HALF) s_qs[buf][et] = p.qscale[q];
     }
     asm volatile("bar.sync 1, %0;" ::"n"(TC_CWARPS * 32) : "memory");
-#define B200VS_CONSUME(N_) \
-  tc_consume_item<HALF, N_>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf], s_hit_key[warp], s_hit_q[warp], &s_hit_n[warp])
-    if (I.nq <= 16) B200VS_CONSUME(16);
-    else if (I.nq <= 32) B200VS_CONSUME(32);
-    else if (I.nq <= 64) B200VS_CONSUME(64);
-    else B200VS_CONSUME(128);
-#undef B200VS_CONSUME
+    auto consume = [&](auto n) {
+      tc_consume_item<HALF, decltype(n)::value>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf],
+                                                s_hit_key[warp], s_hit_q[warp], &s_hit_n[warp]);
+    };
+    const int bl = tc_bcols_log(I.nq);
+    if (bl == 0) consume(std::integral_constant<int, 16>());
+    else if (bl == 1) consume(std::integral_constant<int, 32>());
+    else if (bl == 2) consume(std::integral_constant<int, 64>());
+    else consume(std::integral_constant<int, 128>());
     if (p.mode == 1) {  // flush this warp's staged hits
       __syncwarp();
       const int nh = min(s_hit_n[warp], TC_HITS);
@@ -712,19 +718,20 @@ __device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm,
   return operand + accum;
 }
 
-// ---- block-wide bitonic sort in shared memory (ascending), m = power of two ----
-__device__ __forceinline__ void block_sort_pair(uint32_t* kd, long long* kid, int m) {
-  for (int size = 2; size <= m; size <<= 1)
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = threadIdx.x; i < (m >> 1); i += blockDim.x) {
-        const int pos = 2 * i - (i & (stride - 1)), j = pos + stride;
-        const uint32_t ad = kd[pos], bd = kd[j];
-        const long long ai = kid[pos], bi = kid[j];
-        const bool swap = ((pos & size) == 0) ? key_less(bd, bi, ad, ai) : key_less(ad, ai, bd, bi);
-        if (swap) { kd[pos] = bd; kd[j] = ad; kid[pos] = bi; kid[j] = ai; }
-      }
-      __syncthreads();
-    }
+// The window rows s_rows[0, m) re-scored exactly in the reference order by the block's NQUADS quads, one row per quad per
+// round: s_kd[i] = ord(ranking score), s_id[i] = id_of(row).  The id is loaded before the distance so that the two overlap.
+template <bool L2, int NQUADS, class IdOf>
+__device__ __forceinline__ void tc_rescore_window(const int* s_rows, int m, const float* __restrict__ vecs, const float* qrow, int d,
+                                                  bool vec, IdOf id_of, uint32_t* s_kd, long long* s_id) {
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
+  for (int base = 0; base < m; base += NQUADS) {
+    const int i = base + quad;
+    const bool valid = i < m;
+    const long long row = (long long)s_rows[valid ? i : 0];  // rows < 2^31
+    const long long id = valid ? id_of(row) : -1;
+    const float v = quad_distance<L2>(vecs + (size_t)row * d, qrow, d, t, vec);
+    if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = id; }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -791,7 +798,6 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   __syncthreads();
   const int m = s_m;
   if (m > HF_MAXW) { if (threadIdx.x == 0) redo[qi] = 1; return; }
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
   const float* qs = reinterpret_cast<const float*>(s_dyn);
   // every in-window row is prefetched towards L2 at once, then 32 quads score 32 rows per round straight from global memory
   // (no staging buffer: 16 CTAs per SM keep ~500 rows in flight per SM)
@@ -802,14 +808,7 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   }
   cp_async_wait_all();  // the query row
   __syncthreads();
-  for (int base = 0; base < m; base += HF_THREADS / 4) {
-    const int i = base + quad;
-    const bool valid = i < m;
-    const long long row = (long long)(uint32_t)s_rows[valid ? i : 0];
-    const long long id = valid ? ids[row] : -1;
-    const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, true);
-    if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = id; }
-  }
+  tc_rescore_window<L2, HF_THREADS / 4>(s_rows, m, vecs, qs, d, true, [&](long long row) { return ids[row]; }, s_kd, s_id);
   __syncthreads();
   block_rank_sort(s_kd, s_id, m, [&](int rank, int e) {
     if (rank < k) {
@@ -888,21 +887,8 @@ tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows
     return;
   }
   if (threadIdx.x == 0) flags[qi] = 0;
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  const bool vec = (d & 3) == 0;
-  for (int base = 0; base < m; base += SEL_THREADS / 4) {
-    const int i = base + quad;
-    const bool valid = i < m;
-    const long long row = (long long)s_rows[valid ? i : 0];
-    const float v = quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
-    if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = row; }
-  }
-  int e2 = 2;
-  while (e2 < m) e2 <<= 1;
-  __syncthreads();
-  for (int i = m + threadIdx.x; i < e2; i += SEL_THREADS) { s_kd[i] = KEY_SENTINEL_D; s_id[i] = KEY_SENTINEL_ID; }
-  __syncthreads();
-  block_sort_pair(s_kd, s_id, e2);
+  tc_rescore_window<L2, SEL_THREADS / 4>(s_rows, m, vecs, qs, d, (d & 3) == 0, [](long long row) { return row; }, s_kd, s_id);
+  block_bitonic_sort(s_kd, s_id, m);  // pads to a power of two <= SEL_WCAP (itself one)
   const int need = k - ns;  // slots still open (set mode), all k otherwise
   for (int i = threadIdx.x; i < need; i += SEL_THREADS) {
     const bool have = i < m;
@@ -968,16 +954,7 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
   __syncthreads();
   const int m = s_m, ns = s_ns;
   if (m > HC_MAXW) { if (threadIdx.x == 0) flags[qi] = 1; return; }  // (tc_coarse_select_kernel rewrites the whole output row)
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  const bool vec = (d & 3) == 0;
-  const float* qrow = q + (size_t)qi * d;
-  for (int base = 0; base < m; base += HC_THREADS / 4) {
-    const int i = base + quad;
-    const bool valid = i < m;
-    const long long row = (long long)s_rows[valid ? i : 0];
-    const float v = quad_distance<L2>(vecs + (size_t)row * d, qrow, d, t, vec);
-    if (valid && t == 0) { s_kd[i] = f2ord(L2 ? v : -v); s_id[i] = row; }
-  }
+  tc_rescore_window<L2, HC_THREADS / 4>(s_rows, m, vecs, q + (size_t)qi * d, d, (d & 3) == 0, [](long long row) { return row; }, s_kd, s_id);
   __syncthreads();
   const int need = k - ns;  // slots still open (set mode), all k otherwise
   block_rank_sort(s_kd, s_id, m, [&](int rank, int e) {
@@ -1199,6 +1176,20 @@ static CUtensorMap make_tmap(const void* base, int64_t rows, int d, int box_rows
   return m;
 }
 
+// A = the rows [a_rows, d], B = the query block [b_rows, d]; FP16 when half (the optional lo operands are always FP32)
+static TcMaps make_tc_maps(const void* a, const float* a_lo, int64_t a_rows, const void* b, const float* b_lo, int64_t b_rows, int d,
+                           bool half) {
+  TcMaps m;
+  m.a = make_tmap(a, a_rows, d, TC_BM, half);
+  m.a32 = make_tmap(a, a_rows, d, TC_SAMPLE, half);
+  m.a_lo = a_lo ? make_tmap(a_lo, a_rows, d, TC_BM) : m.a;
+  for (int i = 0; i < 4; ++i) {
+    m.b[i] = make_tmap(b, b_rows, d, 16 << i, half);
+    m.b_lo[i] = b_lo ? make_tmap(b_lo, b_rows, d, 16 << i) : m.b[i];
+  }
+  return m;
+}
+
 static int64_t tc_item_bound(const TcView& v, int64_t npairs) {
   return (npairs / TC_NQT + 1) * (int64_t)std::max(1, v.max_chunks_per_list) + v.total_chunks;
 }
@@ -1243,15 +1234,38 @@ bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int np
   return true;
 }
 
+// Queries rounded for one arithmetic, with ||q||^2 in norm: op = the TF32 (RN) rows, or the scaled FP16 rows with their
+// power-of-two scales in scale; the split arithmetic also keeps the TF32 remainder in lo.
+struct TcQueries {
+  void* op;
+  float *lo, *norm, *scale;
+};
+
+static TcQueries tc_round_queries(IndexBase* ix, TcArith arith, int64_t nq, const float* q, cudaStream_t s) {
+  const int d = ix->dim;
+  auto& S = ix->scratch;
+  TcQueries r{};
+  r.op = S.alloc<unsigned char>((size_t)nq * d * (arith == TC_ARITH_FP16 ? 2 : 4));
+  if (arith == TC_ARITH_SPLIT) r.lo = S.alloc<float>((size_t)nq * d);
+  r.norm = S.alloc<float>(nq);
+  if (arith == TC_ARITH_FP16) r.scale = S.alloc<float>(nq);
+  const unsigned grid = (unsigned)cdiv(nq * 32, 256);
+  if (arith == TC_ARITH_SPLIT) tc_prep_queries_split_kernel<<<grid, 256, 0, s>>>(q, nq, d, static_cast<float*>(r.op), r.lo, r.norm);
+  else if (arith == TC_ARITH_FP16) tc_prep_queries_half_kernel<<<grid, 256, 0, s>>>(q, nq, d, static_cast<__half*>(r.op), r.scale, r.norm);
+  else tc_prep_queries_kernel<<<grid, 256, 0, s>>>(q, nq, d, static_cast<float*>(r.op), r.norm);
+  B200VS_CUDA(cudaGetLastError());
+  return r;
+}
+
 // everything the passes share: rounded queries, pair inversion, gathered B block, work items, tensor maps
 struct TcPlan {
   bool half;  // the FP16 mirror (v.vecs_h) instead of the FP32 rows
-  void* qop; float* qnorm; float* qscale;
+  TcQueries qry;
   int *cnt, *pos, *pair_off, *item_off, *totals, *pair_query, *sample_list, *work;
   void* bws;
   TcItem* items;
   int64_t bound, sbound, npairs;
-  CUtensorMap tmA, tmA32, tmB16, tmB32, tmB64, tmB128;
+  TcMaps maps;
   int num_sms;
 };
 
@@ -1266,9 +1280,7 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.sbound = tc_sample_bound(v, P.npairs);
   P.half = v.vecs_h != nullptr;
   const int esz = P.half ? 2 : 4;  // operand bytes per element
-  P.qop = S.alloc<unsigned char>((size_t)nq * d * esz);
-  P.qnorm = S.alloc<float>(nq);
-  P.qscale = P.half ? S.alloc<float>(nq) : nullptr;
+  P.qry = tc_round_queries(ix, P.half ? TC_ARITH_FP16 : TC_ARITH_TF32, nq, q, s);
   P.cnt = S.alloc<int>(v.nlist);
   P.pos = S.alloc<int>(P.npairs);
   P.pair_off = S.alloc<int>(v.nlist);
@@ -1281,37 +1293,31 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.items = S.alloc<TcItem>(P.bound);
   B200VS_CUDA(cudaMemsetAsync(P.cnt, 0, (size_t)v.nlist * 4, s));
   B200VS_CUDA(cudaMemsetAsync(P.work, 0, 16, s));
-  if (P.half) tc_prep_queries_half_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<__half*>(P.qop), P.qscale, P.qnorm);
-  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(P.qop), P.qnorm);
   tc_count_pairs_kernel<<<(unsigned)cdiv(P.npairs, 256), 256, 0, s>>>(probes, P.npairs, P.cnt, P.pos);
   tc_plan_kernel<<<1, 1024, 0, s>>>(P.cnt, v.list_len, v.nlist, P.pair_off, P.item_off, P.totals);
-  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, d * esz, P.qop, P.pair_query, P.bws);
+  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, d * esz, P.qry.op, P.pair_query, P.bws);
   tc_items_kernel<<<(unsigned)cdiv(v.nlist, 128), 128, 0, s>>>(P.cnt, v.list_len, P.pair_off, P.item_off, v.nlist, P.items, P.totals, P.sample_list);
   B200VS_CUDA(cudaGetLastError());
   const void* rows = P.half ? static_cast<const void*>(v.vecs_h) : static_cast<const void*>(v.vecs);
-  P.tmA = make_tmap(rows, v.arena_rows, d, TC_BM, P.half);
-  P.tmA32 = make_tmap(rows, v.arena_rows, d, TC_SAMPLE, P.half);
-  P.tmB16 = make_tmap(P.bws, P.npairs + TC_NQT, d, 16, P.half);
-  P.tmB32 = make_tmap(P.bws, P.npairs + TC_NQT, d, 32, P.half);
-  P.tmB64 = make_tmap(P.bws, P.npairs + TC_NQT, d, 64, P.half);
-  P.tmB128 = make_tmap(P.bws, P.npairs + TC_NQT, d, 128, P.half);
+  P.maps = make_tc_maps(rows, nullptr, v.arena_rows, P.bws, nullptr, P.npairs + TC_NQT, d, P.half);
   ix->launch_count(5);
   return P;
 }
 
-static TcParams tc_params(const TcView& v, const TcPlan& P, int d, bool l2) {
-  TcParams p;
-  memset(&p, 0, sizeof(p));
-  p.ids = v.ids; p.norms = v.norms; p.list_off = v.list_off; p.d = d; p.items = P.items; p.totals = P.totals;
-  p.sample_list = P.sample_list; p.pair_query = P.pair_query; p.l2 = l2 ? 1 : 0; p.add_norm = 1;
-  p.hscale = v.hscale; p.qscale = P.qscale;
+// The parameters both tile passes share; the caller sets the mode and what that mode reads and writes.
+static TcParams tc_params(const TcView& v, int d, bool l2, const TcItem* items, const int* totals, const float* hscale,
+                          const float* qscale) {
+  TcParams p{};
+  p.ids = v.ids; p.norms = v.norms; p.list_off = v.list_off; p.d = d; p.l2 = l2 ? 1 : 0;
+  p.items = items; p.totals = totals; p.hscale = hscale; p.qscale = qscale;
   return p;
 }
 
-static void tc_launch(const TcPlan& P, const TcParams& p, int64_t work_bound, cudaStream_t s) {
-  const int grid = (int)std::min<int64_t>(P.num_sms, std::max<int64_t>(1, work_bound));
-  if (P.half) tc_scan_kernel<true><<<grid, TC_THREADS, TC_SMEM, s>>>(P.tmA, P.tmA32, P.tmB16, P.tmB32, P.tmB64, P.tmB128, P.tmA, P.tmB16, P.tmB32, P.tmB64, P.tmB128, p);
-  else tc_scan_kernel<false><<<grid, TC_THREADS, TC_SMEM, s>>>(P.tmA, P.tmA32, P.tmB16, P.tmB32, P.tmB64, P.tmB128, P.tmA, P.tmB16, P.tmB32, P.tmB64, P.tmB128, p);
+// One persistent launch of the tile kernel: at most one CTA per SM and per work item.
+static void tc_launch(bool half, int num_sms, int64_t work_bound, const TcMaps& maps, const TcParams& p, cudaStream_t s) {
+  const int grid = (int)std::min<int64_t>(num_sms, std::max<int64_t>(1, work_bound));
+  auto* kernel = half ? tc_scan_kernel<true> : tc_scan_kernel<false>;
+  kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(maps, p);
   B200VS_CUDA(cudaGetLastError());
 }
 
@@ -1334,7 +1340,8 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   int* qcount = S.alloc<int>(1);
   B200VS_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)nq * 4, s));
 
-  TcParams p = tc_params(v, P, d, l2);
+  TcParams p = tc_params(v, d, l2, P.items, P.totals, v.hscale, P.qry.scale);
+  p.sample_list = P.sample_list; p.pair_query = P.pair_query;
   p.sample = sample; p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
   p.filt.has_range = sc.has_range; p.filt.negate = sc.negate; p.filt.rmin = sc.rmin; p.filt.rmax = sc.rmax;
   p.filt.sorted_ids = sc.sorted_ids_dev; p.filt.n_ids = sc.n_ids;
@@ -1343,19 +1350,19 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   // 1) sample pass -> per-query capture thresholds
   p.mode = 0; p.work_counter = P.work;
   ix->phase(IndexBase::PH_SAMPLE, s);
-  tc_launch(P, p, P.sbound, s);
+  tc_launch(P.half, P.num_sms, P.sbound, P.maps, p, s);
   ix->phase(IndexBase::PH_TAU, s);
   int* redo = S.alloc<int>(nq);
   // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
   const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
-  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qnorm, v.max_norm, d, arith, cap, tau, redo);
-  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qnorm, v.max_norm, d, arith, cap, tau, redo);
+  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
+  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
   // 2) capture pass: stream every probed list chunk once, keep rows under the threshold
   p.mode = 1; p.work_counter = P.work + 1;
   ix->phase(IndexBase::PH_CAPTURE, s);
   {
     ScopedKernelTimer timer(ix, s, ix->profiling);
-    tc_launch(P, p, P.bound, s);
+    tc_launch(P.half, P.num_sms, P.bound, P.maps, p, s);
     timer.stop();
   }
   // 3) window select + exact rerank + certification
@@ -1363,14 +1370,14 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   const int* fin_redo = nullptr;
   const size_t hsm = (size_t)d * 4;  // the query row
   if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
-    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
+    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
+    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
     fin_redo = redo;
     ix->launch_count(1);
   }
   const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
-  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qnorm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
+  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
+  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
   tc_compact_flags_kernel<<<1, 1024, 0, s>>>(flags, (int)nq, qmap, qcount);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
@@ -1420,16 +1427,16 @@ bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe) 
 }
 
 // One dense launch of the tile kernel (mode 2): dense[q * v.arena_rows + r] = approximate score of query q against row r
-// (L2: ||x||^2 - 2 <q, x>; IP: -<q, x>; tombstoned rows +inf).  qb_lo == nullptr: single-pass TF32, qb holds the RN-rounded
-// queries and the tensor core truncates the rows a_hi.  Otherwise the error-compensated split pass: the three products
-// hi*hi + lo*hi + hi*lo accumulate into the same register accumulators (the lo operands ride in the next ring stage).
-// hscale != nullptr: qb and a_hi are scaled FP16 (the list scan's FP16 arithmetic), qscale / hscale their scales.
-static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const void* qb, const float* qb_lo, const void* a_hi,
-                          const float* a_lo, const float* qscale, const float* hscale, float* dense, cudaStream_t s) {
+// (L2: ||x||^2 - 2 <q, x>; IP: -<q, x>; tombstoned rows +inf).  qr.lo == nullptr: single-pass TF32, qr.op holds the
+// RN-rounded queries and the tensor core truncates the rows a_hi.  Otherwise the error-compensated split pass: the three
+// products hi*hi + lo*hi + hi*lo accumulate into the same register accumulators (the lo operands ride in the next ring
+// stage).  hscale != nullptr: qr.op and a_hi are scaled FP16 (the list scan's FP16 arithmetic), qr.scale / hscale their scales.
+static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const TcQueries& qr, const void* a_hi, const float* a_lo,
+                          const float* hscale, float* dense, cudaStream_t s) {
   const int num_sms = tc_init(ix->device);
   const int d = ix->dim;
   const int nrows = (int)v.arena_rows;
-  const bool split = qb_lo != nullptr, half = hscale != nullptr;
+  const bool half = hscale != nullptr;
   auto& S = ix->scratch;
   const int chunk = nrows <= 16384 ? TC_BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
   const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, TC_NQT));
@@ -1438,22 +1445,30 @@ static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, c
   int* work = S.alloc<int>(4);
   B200VS_CUDA(cudaMemsetAsync(work, 0, 16, s));
   tc_coarse_items_kernel<<<(unsigned)cdiv(nitems, 128), 128, 0, s>>>(nrows, (int)nq, chunk, items, totals);
-  TcPlan P;
-  memset(&P, 0, sizeof(P));
-  P.items = items; P.totals = totals;
-  TcParams p = tc_params(v, P, d, l2);
-  p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.pair_query = nullptr; p.hscale = hscale; p.qscale = qscale;
-  const CUtensorMap ta = make_tmap(a_hi, nrows, d, TC_BM, half), ta_lo = split ? make_tmap(a_lo, nrows, d, TC_BM) : ta;
-  const CUtensorMap b16 = make_tmap(qb, nq, d, 16, half), b32 = make_tmap(qb, nq, d, 32, half), b64 = make_tmap(qb, nq, d, 64, half),
-                    b128 = make_tmap(qb, nq, d, 128, half);
-  const CUtensorMap l16 = split ? make_tmap(qb_lo, nq, d, 16) : b16, l32 = split ? make_tmap(qb_lo, nq, d, 32) : b32;
-  const CUtensorMap l64 = split ? make_tmap(qb_lo, nq, d, 64) : b64, l128 = split ? make_tmap(qb_lo, nq, d, 128) : b128;
-  const int grid = (int)std::min<int64_t>(num_sms, std::max(1, nitems));
-  p.work_counter = work; p.split = split ? 1 : 0; p.dense_accum = 0; p.add_norm = 1;
+  TcParams p = tc_params(v, d, l2, items, totals, hscale, qr.scale);
+  p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.work_counter = work; p.split = qr.lo != nullptr ? 1 : 0;
+  const TcMaps maps = make_tc_maps(a_hi, a_lo, nrows, qr.op, qr.lo, nq, d, half);
   ix->phase(IndexBase::PH_COARSE_SCAN, s);
-  if (half) tc_scan_kernel<true><<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
-  else tc_scan_kernel<false><<<grid, TC_THREADS, TC_SMEM, s>>>(ta, ta, b16, b32, b64, b128, ta_lo, l16, l32, l64, l128, p);
-  B200VS_CUDA(cudaGetLastError());
+  tc_launch(half, num_sms, nitems, maps, p, s);
+}
+
+// The register-select finish of the coarse pass, in its warp form (HYBRID: 32 threads hold the score row) or its block form
+// (SEL_THREADS threads), at the smallest width KPT, 2 KPT, ..., 32 keys per thread that holds the row.
+template <bool HYBRID, bool L2, int KPT>
+static void tc_coarse_select(const TcView& v, int64_t nq, const float* dense, const float* qnorm, const float* q, int d, int k,
+                             long long* out_probes, float* out_raw, int* flags, const int* redo_in, cudaStream_t s) {
+  const int nrows = (int)v.arena_rows;
+  if constexpr (KPT < 32) {
+    if (nrows > (HYBRID ? 32 : SEL_THREADS) * KPT)
+      return tc_coarse_select<HYBRID, L2, 2 * KPT>(v, nq, dense, qnorm, q, d, k, out_probes, out_raw, flags, redo_in, s);
+  }
+  const int api = v.api_scores ? 1 : 0;
+  if constexpr (HYBRID)
+    tc_coarse_select_hybrid_kernel<L2, KPT><<<(unsigned)nq, HC_THREADS, 0, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, k,
+                                                                               v.id_offset, api, out_probes, out_raw, flags);
+  else
+    tc_coarse_select_kernel<L2, KPT><<<(unsigned)nq, SEL_THREADS, ((size_t)d * 4 + 15) / 16 * 16, s>>>(
+        dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, k, v.id_offset, api, out_probes, out_raw, flags, redo_in);
 }
 
 // Coarse quantiser: ONE dense launch of the tile kernel in split mode (error-compensated TF32).  The operand error drops
@@ -1464,13 +1479,11 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   const int d = ix->dim;
   const int nrows = (int)v.arena_rows;
   auto& S = ix->scratch;
-  float* qhi = S.alloc<float>((size_t)nq * d);
-  float* qlo = S.alloc<float>((size_t)nq * d);
-  float* qnorm = S.alloc<float>(nq);
-  float* dense = S.alloc<float>((size_t)nq * nrows);
   ix->phase(IndexBase::PH_COARSE_PREP, s);
-  tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, qhi, qlo, qnorm);
-  tc_dense_scan(ix, v, l2, nq, qhi, qlo, v.vecs_hi, v.vecs_lo, nullptr, nullptr, dense, s);
+  const TcQueries qr = tc_round_queries(ix, TC_ARITH_SPLIT, nq, q, s);
+  const float* qnorm = qr.norm;
+  float* dense = S.alloc<float>((size_t)nq * nrows);
+  tc_dense_scan(ix, v, l2, nq, qr, v.vecs_hi, v.vecs_lo, nullptr, dense, s);
   ix->phase(IndexBase::PH_COARSE_FINAL, s);
   const int pool = select_pool_cap(nprobe, SCAN_THREADS);
   const size_t fin_smem = tc_stream_smem(d, pool);
@@ -1481,24 +1494,15 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
     // and for the queries the warp kernel flagged, then the streaming kernel for what is still flagged (normally none)
     int* redo0 = S.alloc<int>(nq);
     int* redo = S.alloc<int>(nq);
-    const size_t qsm = ((size_t)d * 4 + 15) / 16 * 16;
-    const int kpt = (nrows + SEL_THREADS - 1) / SEL_THREADS;
     const int* redo_in = nullptr;
     if (nrows <= 1024 && 2 * nprobe <= HC_MAXW) {
-#define B200VS_HSEL(L2_, KPT_) tc_coarse_select_hybrid_kernel<L2_, KPT_><<<(unsigned)nq, HC_THREADS, 0, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, redo0)
-      if (nrows <= 256) { if (l2) B200VS_HSEL(true, 8); else B200VS_HSEL(false, 8); }
-      else if (nrows <= 512) { if (l2) B200VS_HSEL(true, 16); else B200VS_HSEL(false, 16); }
-      else { if (l2) B200VS_HSEL(true, 32); else B200VS_HSEL(false, 32); }
-#undef B200VS_HSEL
+      if (l2) tc_coarse_select<true, true, 8>(v, nq, dense, qnorm, q, d, nprobe, out_probes, out_raw, redo0, nullptr, s);
+      else tc_coarse_select<true, false, 8>(v, nq, dense, qnorm, q, d, nprobe, out_probes, out_raw, redo0, nullptr, s);
       redo_in = redo0;
       ix->launch_count(1);
     }
-#define B200VS_SEL(L2_, KPT_) tc_coarse_select_kernel<L2_, KPT_><<<(unsigned)nq, SEL_THREADS, qsm, s>>>(dense, nrows, nrows, qnorm, v.max_norm, q, v.vecs, d, nprobe, v.id_offset, v.api_scores ? 1 : 0, out_probes, out_raw, redo, redo_in)
-    if (kpt <= 4) { if (l2) B200VS_SEL(true, 4); else B200VS_SEL(false, 4); }
-    else if (kpt <= 8) { if (l2) B200VS_SEL(true, 8); else B200VS_SEL(false, 8); }
-    else if (kpt <= 16) { if (l2) B200VS_SEL(true, 16); else B200VS_SEL(false, 16); }
-    else { if (l2) B200VS_SEL(true, 32); else B200VS_SEL(false, 32); }
-#undef B200VS_SEL
+    if (l2) tc_coarse_select<false, true, 4>(v, nq, dense, qnorm, q, d, nprobe, out_probes, out_raw, redo, redo_in, s);
+    else tc_coarse_select<false, false, 4>(v, nq, dense, qnorm, q, d, nprobe, out_probes, out_raw, redo, redo_in, s);
     fin_redo = redo;
     ix->launch_count(1);
   }
@@ -1519,14 +1523,7 @@ void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const 
   const int d = ix->dim;
   auto& S = ix->scratch;
   const bool split = arith == TC_ARITH_SPLIT, half = arith == TC_ARITH_FP16;
-  void* qb = S.alloc<unsigned char>((size_t)nq * d * (half ? 2 : 4));
-  float* qb_lo = split ? S.alloc<float>((size_t)nq * d) : nullptr;
-  float* qnorm = S.alloc<float>(nq);
-  float* qscale = half ? S.alloc<float>(nq) : nullptr;
-  if (split) tc_prep_queries_split_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(qb), qb_lo, qnorm);
-  else if (half) tc_prep_queries_half_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<__half*>(qb), qscale, qnorm);
-  else tc_prep_queries_kernel<<<(unsigned)cdiv(nq * 32, 256), 256, 0, s>>>(q, nq, d, static_cast<float*>(qb), qnorm);
-  B200VS_CUDA(cudaGetLastError());
+  const TcQueries qr = tc_round_queries(ix, arith, nq, q, s);
   if (v.arena_rows > 0) {
     const void* a_hi = v.vecs;
     const float *a_lo = nullptr, *hscale = nullptr;
@@ -1541,9 +1538,9 @@ void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const 
       launch_half_rows(v.vecs, nullptr, v.arena_rows, d, h, sc, s);
       a_hi = h; hscale = sc;
     }
-    tc_dense_scan(ix, v, l2, nq, qb, qb_lo, a_hi, a_lo, qscale, hscale, out_scores, s);
+    tc_dense_scan(ix, v, l2, nq, qr, a_hi, a_lo, hscale, out_scores, s);
   }
-  tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qnorm, nq, l2 ? 1 : 0, v.max_norm, d, arith, out_eps);
+  tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qr.norm, nq, l2 ? 1 : 0, v.max_norm, d, arith, out_eps);
   B200VS_CUDA(cudaGetLastError());
 }
 

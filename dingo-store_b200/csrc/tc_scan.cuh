@@ -63,8 +63,6 @@ struct TcParams {
   int cap;
   float* dense;             // mode 2: [nq, dense_ld] approximate scores (row = column index)
   long long dense_ld;
-  int dense_accum;          // mode 2: add to the stored score instead of overwriting (split-precision passes 2 and 3)
-  int add_norm;             // include the ||x||^2 term (off for the correction passes)
   int split;                // error-compensated TF32: hi*hi + lo*hi + hi*lo into one accumulator (coarse quantiser)
   const float* hscale;      // FP16 path: [arena rows] power-of-two scale of each row of the mirror
   const float* qscale;      // FP16 path: [nq] power-of-two scale of each query
