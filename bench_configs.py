@@ -3,7 +3,7 @@
 
   cfg1  Flat L2, 100K x 128, top-10, batch = 1            (the reference's own CPU-runnable case)
   cfg2  IVF-Flat L2, 1M x 768, nlist 1024, nprobe 32, batch 256, top-10
-  cfg3  IVF-PQ IP, 10M x 768, M = 96, nbits 8, nlist 2048, nprobe 64, batch 1024, top-100   (--pq-n)
+  cfg3  IVF-PQ IP, 10M x 768, M = 96, nbits 8, nlist 2048, nprobe 64, batch 1024, top-100   (--pq-n, --pq-nbits, --pq-m)
   cfg4  HNSW cosine, 1M x 768, M = 16, efConstruction 200, efSearch 128, batch 512          (--hnsw-n; concurrent host build)
   cfg5  IVF-Flat L2, (rows-per-GPU x world) x 1536, nlist 2048 per GPU, nprobe 64, batch 4096, top-10, list-sharded over
         the GPUs of the box through b200vs_shard_* — run under torchrun (BASELINE: 100 M rows over 8 GPUs = 77 GB per GPU, more
@@ -28,6 +28,7 @@ import torch  # noqa: E402
 
 import b200vs  # noqa: E402
 import oracle_lib  # noqa: E402
+import pq_codes  # noqa: E402
 import b200vs.shard as shard_host  # noqa: E402
 
 
@@ -132,9 +133,10 @@ def cfg2(o, cores):
             "fallback_queries": st[2], "search_stats": st}
 
 
-def cfg3(o, cores, n):
-    d, M, nlist, nprobe, nq, k = 768, 96, 2048, 64, 1024, 100
-    ix = b200vs.Index(b200vs.IVF_PQ, b200vs.IP, d, nlist=nlist, pq_m=M, pq_nbits=8)
+def cfg3(o, cores, n, nbits=8, M=96):
+    d, nlist, nprobe, nq, k = 768, 2048, 64, 1024, 100
+    ksub, code_size = 1 << nbits, pq_codes.code_size(M, nbits)
+    ix = b200vs.Index(b200vs.IVF_PQ, b200vs.IP, d, nlist=nlist, pq_m=M, pq_nbits=nbits)
     g = torch.Generator(device="cuda")
     g.manual_seed(1234)
     t0 = time.time()
@@ -160,21 +162,26 @@ def cfg3(o, cores, n):
     # parity on a sample: oracle LUT scan over the exported codes with the GPU-trained state
     blob = ix.get_trained_state()
     cent = blob[48:48 + nlist * d * 4].view(np.float32).reshape(nlist, d)
-    cb = blob[48 + nlist * d * 4:].view(np.float32).reshape(M, 256, d // M)
-    off, _, codes, lids = ix.export_lists(nlist, with_vectors=False, code_size=M)
+    cb = blob[48 + nlist * d * 4:].view(np.float32).reshape(M, ksub, d // M)
+    off, _, codes, lids = ix.export_lists(nlist, with_vectors=False, code_size=code_size)
     ns = 32
     t = time.perf_counter()
-    Do, Io = o.ivfpq_search(oracle_lib.IP, cent, cb, off, codes, lids, xq[:ns], k, nprobe, nthreads=cores)
+    if nbits == 8:
+        Do, Io = o.ivfpq_search(oracle_lib.IP, cent, cb, off, codes, lids, xq[:ns], k, nprobe, nthreads=cores)
+    else:
+        Do, Io = pq_codes.ivfpq_search(o, oracle_lib.IP, cent, cb, off, codes, lids, xq[:ns], k, nprobe, nthreads=cores)
     cpu_s = time.perf_counter() - t
     lookups = float(st[4]) * M * 0 + 0  # per-batch lookups need the per-query probe sizes: use avg list len
     avg_len = n / nlist
     lookups = nq * nprobe * avg_len * M
-    return {"config": f"cfg3 IVF-PQ IP {n}x768 M=96 nbits=8 nlist=2048 nprobe=64 batch=1024 top-100", "scaled_from": "10M x 768" if n < 10_000_000 else None,
+    return {"config": f"cfg3 IVF-PQ IP {n}x768 M={M} nbits={nbits} nlist=2048 nprobe=64 batch=1024 top-100", "scaled_from": "10M x 768" if n < 10_000_000 else None,
             "qps_device": nq / dev_ms * 1e3, "ms_per_batch_device": dev_ms, "qps_e2e": nq / e2e_ms * 1e3,
             "ids_bit_exact_sample": bool(np.array_equal(I[:ns], Io)), "recall_at_100_vs_oracle": float(np.mean([len(set(a) & set(b)) / k for a, b in zip(I[:ns], Io)])),
             "max_rel_dist_err": float(np.max(np.abs(D[:ns] - Do) / np.maximum(np.abs(Do), 1e-6))),
-            "roofline": {"bound": "shared-memory LUT", "kernel": "pq_scan_select_kernel", "kernel_ms": st[3] / 1e6, "lookups_per_batch": lookups,
-                         "achieved_lookups_per_s": lookups / max(st[3] * 1e-9, 1e-9), "bytes_scan_equiv_gbs": lookups / max(st[3], 1), "hbm_peak_gbs": peak()},
+            "roofline": {"bound": "shared-memory LUT", "kernel": "pq_scan_select_kernel" if nbits == 8 else f"pq_scan_packed_kernel<IP, {nbits}>",
+                         "kernel_ms": st[3] / 1e6, "lookups_per_batch": lookups,
+                         "achieved_lookups_per_s": lookups / max(st[3] * 1e-9, 1e-9), "bytes_scan_equiv_gbs": lookups / max(st[3], 1), "hbm_peak_gbs": peak(),
+                         **({} if nbits == 8 else {"code_size": code_size, "code_bytes_per_batch": nq * nprobe * avg_len * code_size})},
             "cpu_baseline": {"qps": ns / cpu_s, "cores": cores, "kind": "port", "sample": f"first {ns} queries, {cores} threads"},
             "train_seconds": t_train, "add_seconds": t_add, "search_stats": st}
 
@@ -472,6 +479,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="1,2,3,4")
     ap.add_argument("--pq-n", type=int, default=10_000_000)
+    ap.add_argument("--pq-nbits", type=int, default=8, help="cfg3: bits per PQ code, 1-8")
+    ap.add_argument("--pq-m", type=int, default=96, help="cfg3: sub-quantisers (768 must divide by it)")
     ap.add_argument("--hnsw-n", type=int, default=1_000_000)
     ap.add_argument("--hnsw-build-threads", type=int, default=64)
     ap.add_argument("--cfg5-rows", type=int, default=6_250_000, help="cfg5: database rows per GPU (6.25 M x 1536 f32 = 38 GB of an 80 GB H100)")
@@ -481,7 +490,7 @@ def main():
     a = ap.parse_args()
     o = oracle_lib.load()
     cores = os.cpu_count() or 1
-    fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads),
+    fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch)}
     rank = int(os.environ.get("RANK", 0))

@@ -11,7 +11,11 @@
 //   IP     : dis = <q, c[list]> (hooked AVX-512 order) + sum_m sim[m][code_m],      sim[m][j] = <q_m, cw[m][j]>
 //   L2     : dis = ||q - c[list]||^2 + sum_m (T[list][m][code_m] - 2 sim[m][code_m]), T = ||cw||^2 + 2 <c_m, cw>
 //   LUT sums run sequentially over m in FP32.
-// Kernels: pq_sim_kernel (per-query LUT), pq_precompute_kernel (T), pq_encode_kernel, pq_scan_select_kernel.
+// Codes: nbits in [1, 8], ksub = 2^nbits, faiss PQEncoderGeneric layout: a row is code_size = ceil(M*nbits/8) bytes and
+//   code m occupies bits [m*nbits, (m+1)*nbits) of the row's little-endian bit stream (LSB first in each byte), pad bits
+//   zero.  At nbits = 8 that is one byte per code.
+// Kernels: pq_sim_kernel (per-query LUT), pq_precompute_kernel (T), pq_encode_kernel (+ pq_pack_kernel below 8 bits),
+//   pq_scan_select_kernel (8 bits), pq_scan_packed_kernel<L2, NBITS> (1-7 bits).
 #include <algorithm>
 #include <memory>
 
@@ -25,8 +29,12 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p);
 
 namespace {
 
-constexpr int KSUB = 256;
+constexpr int KSUB = 256;       // the 8-bit scan kernel's LUT row
 constexpr int PQ_THREADS = 512;  // code-scan CTA: one 96 KB LUT serves 16 warps (2 CTAs per SM -> 32 warps hide the code-load latency)
+// packed-code scan CTA: the LUT is at most M * 128 floats (12 KB at M = 96, 4 bits), so shared memory no longer limits the
+// CTAs per SM; 256 threads x 4 CTAs keep 32 warps resident within 64 registers (see DESIGN.md §4.3 for the ptxas figures)
+constexpr int PQP_THREADS = 256;
+constexpr int PQP_MIN_CTAS = 4;
 
 __device__ __forceinline__ float ip_seq(const float* a, const float* b, int n) {
   float r = 0.f;
@@ -35,32 +43,32 @@ __device__ __forceinline__ float ip_seq(const float* a, const float* b, int n) {
 }
 
 // sim[q][m][j] = <q_m, cw[m][j]>
-__global__ void pq_sim_kernel(const float* __restrict__ q, const float* __restrict__ cb, long long nq, int d, int M, float* sim) {
+__global__ void pq_sim_kernel(const float* __restrict__ q, const float* __restrict__ cb, long long nq, int d, int M, int ksub, float* sim) {
   const int dsub = d / M;
   const long long qi = blockIdx.x;
   const float* qv = q + (size_t)qi * d;
-  for (int i = threadIdx.x; i < M * KSUB; i += blockDim.x) {
-    const int m = i / KSUB;
-    sim[(size_t)qi * M * KSUB + i] = ip_seq(qv + m * dsub, cb + (size_t)i * dsub, dsub);
+  for (int i = threadIdx.x; i < M * ksub; i += blockDim.x) {
+    const int m = i / ksub;
+    sim[(size_t)qi * M * ksub + i] = ip_seq(qv + m * dsub, cb + (size_t)i * dsub, dsub);
   }
 }
 
 // T[l][m][j] = ||cw||^2 + 2 <c_l,m , cw>
-__global__ void pq_precompute_kernel(const float* __restrict__ cent, const float* __restrict__ cb, int d, int M, float* pre) {
+__global__ void pq_precompute_kernel(const float* __restrict__ cent, const float* __restrict__ cb, int d, int M, int ksub, float* pre) {
   const int dsub = d / M;
   const int l = blockIdx.x;
-  for (int i = threadIdx.x; i < M * KSUB; i += blockDim.x) {
-    const int m = i / KSUB;
+  for (int i = threadIdx.x; i < M * ksub; i += blockDim.x) {
+    const int m = i / ksub;
     const float* cw = cb + (size_t)i * dsub;
     const float r2 = ip_seq(cw, cw, dsub);
     const float cr = ip_seq(cent + (size_t)l * d + m * dsub, cw, dsub);
-    pre[(size_t)l * M * KSUB + i] = __fadd_rn(r2, __fmul_rn(2.f, cr));
+    pre[(size_t)l * M * ksub + i] = __fadd_rn(r2, __fmul_rn(2.f, cr));
   }
 }
 
-// one warp per row: code[m] = argmin_j ||(x - c)_m - cw[m][j]||^2
+// one warp per row: code[m] = argmin_j ||(x - c)_m - cw[m][j]||^2 over j < ksub, one byte per code
 __global__ void pq_encode_kernel(const float* __restrict__ x, const long long* __restrict__ list, const float* __restrict__ cent,
-                                 const float* __restrict__ cb, long long n, int d, int M, unsigned char* codes_out) {
+                                 const float* __restrict__ cb, long long n, int d, int M, int ksub, unsigned char* codes_out) {
   extern __shared__ float s_res[];  // [warps_per_block][d]
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long w = (long long)blockIdx.x * (blockDim.x >> 5) + wib;
@@ -75,8 +83,8 @@ __global__ void pq_encode_kernel(const float* __restrict__ x, const long long* _
     const float* rs = res + m * dsub;
     float best = __int_as_float(0x7f800000);
     int bj = 0x7fffffff;
-    for (int j = lane; j < KSUB; j += 32) {
-      const float* cw = cb + ((size_t)m * KSUB + j) * dsub;
+    for (int j = lane; j < ksub; j += 32) {  // lanes >= ksub keep (inf, INT_MAX) and never win the reduction
+      const float* cw = cb + ((size_t)m * ksub + j) * dsub;
       float v = 0.f;
       for (int i = 0; i < dsub; ++i) { const float t = __fsub_rn(rs[i], cw[i]); v = __fadd_rn(v, __fmul_rn(t, t)); }
       if (v < best) { best = v; bj = j; }
@@ -91,38 +99,54 @@ __global__ void pq_encode_kernel(const float* __restrict__ x, const long long* _
   }
 }
 
-__global__ void scatter_codes_kernel(const unsigned char* __restrict__ src, const long long* __restrict__ src_ids,
-                                     const long long* __restrict__ slots, long long n, int M, unsigned char* codes, long long* ids) {
+// byte-per-code rows [n, M] -> packed rows [n, cs]: one thread per output byte, pad bits zero
+__global__ void pq_pack_kernel(const unsigned char* __restrict__ src, long long n, int M, int nbits, int cs, unsigned char* dst) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * M) return;
-  const long long r = i / M;
-  const int m = (int)(i % M);
+  if (i >= n * cs) return;
+  const long long r = i / cs;
+  const int b0 = (int)(i % cs) * 8;
+  const unsigned char* c = src + (size_t)r * M;
+  unsigned v = 0;
+  for (int t = 0; t < 8; ++t) {
+    const int m = (b0 + t) / nbits;
+    if (m < M) v |= ((c[m] >> ((b0 + t) % nbits)) & 1u) << t;
+  }
+  dst[i] = (unsigned char)v;
+}
+
+// rows of cs code bytes go to their slots
+__global__ void scatter_codes_kernel(const unsigned char* __restrict__ src, const long long* __restrict__ src_ids,
+                                     const long long* __restrict__ slots, long long n, int cs, unsigned char* codes, long long* ids) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * cs) return;
+  const long long r = i / cs;
+  const int m = (int)(i % cs);
   const long long s = slots[r];
-  codes[(size_t)s * M + m] = src[i];
+  codes[(size_t)s * cs + m] = src[i];
   if (m == 0) ids[s] = src_ids[r];
 }
 
 __global__ void move_codes_kernel(const unsigned char* __restrict__ scodes, const long long* __restrict__ sids,
-                                  const long long* __restrict__ src_rows, const long long* __restrict__ dst_rows, long long n, int M,
+                                  const long long* __restrict__ src_rows, const long long* __restrict__ dst_rows, long long n, int cs,
                                   unsigned char* dcodes, long long* dids) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * M) return;
-  const long long r = i / M;
-  const int m = (int)(i % M);
-  dcodes[(size_t)dst_rows[r] * M + m] = scodes[(size_t)src_rows[r] * M + m];
+  if (i >= n * cs) return;
+  const long long r = i / cs;
+  const int m = (int)(i % cs);
+  dcodes[(size_t)dst_rows[r] * cs + m] = scodes[(size_t)src_rows[r] * cs + m];
   if (m == 0) dids[dst_rows[r]] = sids[src_rows[r]];
 }
 
 struct PqScanArgs {
-  const unsigned char* codes;
+  const unsigned char* codes;  // [rows, code_size]
   const long long* ids;
   const long long* probes;  // [nq, nprobe]
   const float* coarse;      // [nq, nprobe] raw metric value (ip or L2)
   const long long* list_off;
   const int* list_len;
-  const float* sim;  // [nq, M*256]
-  const float* pre;  // [nlist, M*256] (L2) or null
-  int M, nprobe, k, nsplit, pool_cap;
+  const float* sim;  // [nq, M*ksub]
+  const float* pre;  // [nlist, M*ksub] (L2) or null
+  int M, code_size, nprobe, k, nsplit, pool_cap;
   int has_thr;       // range search: fixed initial threshold (strict), k = max results kept
   uint32_t thr_key;
   uint32_t* ws_kd;
@@ -207,15 +231,148 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_scan_select_kernel(const PqScan
   }
 }
 
+// Packed codes (NBITS < 8): 128 codes of a row take exactly 4*NBITS 32-bit words, so the row is read in chunks of
+// 128 codes whose bit offsets are compile-time constants.  Chunk c of a row (words [4*NBITS*c, 4*NBITS*(c+1))) in the
+// widest loads the row stride allows; words past the row's code_size bytes read as 0.
+template <int NBITS>
+__device__ __forceinline__ void pq_load_chunk(const unsigned char* code, int cs, int c, uint32_t (&w)[4 * NBITS]) {
+  const int w0 = c * 4 * NBITS;
+  if ((cs & 15) == 0) {  // rows 16-byte aligned
+    const uint4* p = reinterpret_cast<const uint4*>(code);
+    const int nv = cs >> 4;
+#pragma unroll
+    for (int i = 0; i < NBITS; ++i) {
+      const uint4 v = c * NBITS + i < nv ? p[c * NBITS + i] : make_uint4(0u, 0u, 0u, 0u);
+      w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
+    }
+  } else if ((cs & 3) == 0) {
+    const uint32_t* p = reinterpret_cast<const uint32_t*>(code);
+    const int nw = cs >> 2;
+#pragma unroll
+    for (int i = 0; i < 4 * NBITS; ++i) w[i] = w0 + i < nw ? p[w0 + i] : 0u;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4 * NBITS; ++i) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int b = 0; b < 4; ++b) {
+        const int o = (w0 + i) * 4 + b;
+        if (o < cs) v |= (uint32_t)code[o] << (8 * b);
+      }
+      w[i] = v;
+    }
+  }
+}
+
+// dis += tab[j * ksub + code_j] for j = 0 .. n-1 of one chunk (n = 128, or the row's remaining codes when TAIL), in order.
+// Code j sits at bit j*NBITS of the chunk: a shift of one word, or a funnel shift of two when it straddles a word boundary.
+template <int NBITS, bool TAIL>
+__device__ __forceinline__ float pq_sum_chunk(float dis, const float* tab, const uint32_t (&w)[4 * NBITS], int n) {
+  constexpr int KS = 1 << NBITS;
+#pragma unroll
+  for (int j = 0; j < 128; ++j) {
+    const int bit = j * NBITS, a = bit >> 5, s = bit & 31;
+    const uint32_t v = s + NBITS <= 32 ? w[a] >> s : __funnelshift_r(w[a], w[a + 1], s);
+    if (!TAIL || j < n) dis = __fadd_rn(dis, tab[j * KS + (v & (KS - 1))]);
+  }
+  return dis;
+}
+
+// The 8-bit kernel's scheme on packed rows: block (split, query), probes split round-robin, LUT [M, 2^NBITS] in shared
+// memory (L2: rebuilt per probed list), one thread per code row, the same select and range-threshold epilogue.  A LUT
+// row has at most 32 words, so the 32 lanes of a lookup touch 32 distinct banks at most: one wavefront per lookup.
+template <bool L2, int NBITS>
+__global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kernel(const PqScanArgs a) {
+  constexpr int KS = 1 << NBITS;
+  extern __shared__ __align__(16) unsigned char smem[];
+  float* tab = reinterpret_cast<float*>(smem);
+  const int M = a.M, T = M * KS, cs = a.code_size;
+  const int qi = blockIdx.y, split = blockIdx.x;
+  BlockSelect sel;
+  sel.init(smem + (size_t)T * 4, a.pool_cap, a.k);
+  if (a.has_thr && threadIdx.x == 0) { *sel.thr_d = a.thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
+  __syncthreads();
+  const float* simq = a.sim + (size_t)qi * T;
+  if (!L2) {
+    for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = simq[i];
+    __syncthreads();
+  }
+  for (int p = split; p < a.nprobe; p += a.nsplit) {
+    const long long l = a.probes[(size_t)qi * a.nprobe + p];
+    if (l < 0) continue;
+    const int len = a.list_len[l];
+    if (len <= 0) continue;
+    const float dis0 = a.coarse[(size_t)qi * a.nprobe + p];
+    if (L2) {  // fvec_madd(n, precomputed, -2, sim, tab)
+      __syncthreads();
+      const float* pl = a.pre + (size_t)l * T;
+      for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = __fadd_rn(pl[i], __fmul_rn(-2.0f, simq[i]));
+      __syncthreads();
+    }
+    const long long base = a.list_off[l];
+    for (int r0 = 0; r0 < len; r0 += blockDim.x) {
+      sel.maybe_prune(blockDim.x);
+      const int r = r0 + threadIdx.x;
+      if (r < len) {
+        const long long row = base + r;
+        const long long id = a.ids[row];
+        if (id >= 0 && filter_pass(a.filt, id)) {
+          const unsigned char* code = a.codes + (size_t)row * cs;
+          float dis = dis0;
+          uint32_t w[4 * NBITS];
+          int c = 0;
+          for (; (c + 1) * 128 <= M; ++c) {
+            pq_load_chunk<NBITS>(code, cs, c, w);
+            dis = pq_sum_chunk<NBITS, false>(dis, tab + c * 128 * KS, w, 128);
+          }
+          if (c * 128 < M) {
+            pq_load_chunk<NBITS>(code, cs, c, w);
+            dis = pq_sum_chunk<NBITS, true>(dis, tab + c * 128 * KS, w, M - c * 128);
+          }
+          const uint32_t key = f2ord(L2 ? dis : -dis);
+          if (sel.passes(key, id)) sel.push(key, id);
+        }
+      }
+    }
+  }
+  sel.prune();
+  const int have = *sel.count;
+  uint32_t* okd = a.ws_kd + ((size_t)qi * a.nsplit + split) * a.k;
+  long long* oki = a.ws_kid + ((size_t)qi * a.nsplit + split) * a.k;
+  for (int i = threadIdx.x; i < a.k; i += blockDim.x) {
+    okd[i] = i < have ? sel.kd[i] : KEY_SENTINEL_D;
+    oki[i] = i < have ? sel.kid[i] : KEY_SENTINEL_ID;
+  }
+}
+
+template <bool L2>
+void launch_pq_scan_packed(int nbits, dim3 grid, size_t smem, cudaStream_t s, const PqScanArgs& a) {
+  auto go = [&](auto kern) {
+    B200VS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    kern<<<grid, PQP_THREADS, smem, s>>>(a);
+  };
+  switch (nbits) {
+    case 1: go(pq_scan_packed_kernel<L2, 1>); break;
+    case 2: go(pq_scan_packed_kernel<L2, 2>); break;
+    case 3: go(pq_scan_packed_kernel<L2, 3>); break;
+    case 4: go(pq_scan_packed_kernel<L2, 4>); break;
+    case 5: go(pq_scan_packed_kernel<L2, 5>); break;
+    case 6: go(pq_scan_packed_kernel<L2, 6>); break;
+    case 7: go(pq_scan_packed_kernel<L2, 7>); break;
+    default: fail(B200VS_EINTERNAL, "no packed-code scan kernel for this nbits");
+  }
+}
+
 }  // namespace
 
 struct IvfPqIndex : IndexBase {
   enum Mode { kNone, kFlat, kIvfPq } mode = kNone;
   int nlist, M, nbits;
+  int ksub, code_size;              // 2^nbits codewords per sub-space; bytes per packed code row
   std::unique_ptr<IndexBase> flat;  // inner Flat index when there is too little data to train (ivf_pq.cc:339-353)
   DevBuf<float> centroids, codebooks, pre;
   DevBuf<long long> cent_ids;
-  DevBuf<unsigned char> codes;
+  DevBuf<unsigned char> codes;      // [rows, code_size]
   DevBuf<long long> ids;
   IvfLists L;
 
@@ -223,8 +380,14 @@ struct IvfPqIndex : IndexBase {
     nlist = p.nlist > 0 ? p.nlist : 2048;      // Constant::kCreateIvfPqParamNcentroids
     M = p.pq_m > 0 ? p.pq_m : 64;              // kCreateIvfPqParamNsubvector
     nbits = p.pq_nbits > 0 ? p.pq_nbits : 8;   // kCreateIvfPqParamNbitsPerIdx
-    if (nbits != 8) fail(B200VS_EILLEGAL_PARAMETERS, "only nbits_per_idx = 8 is implemented");
+    if (nbits > 16) fail(B200VS_EILLEGAL_PARAMETERS, "nbits_per_idx must be in (0, 16]");
+    if (nbits > 8)
+      fail(B200VS_EILLEGAL_PARAMETERS, "nbits_per_idx 9-16 is not supported: the per-query LUT (M * 2^nbits floats) does not fit in "
+                                       "shared memory, and the L2 precomputed table (nlist * M * 2^nbits floats) outgrows faiss's "
+                                       "precomputed-table limit at realistic nlist");
     if (d % M != 0) fail(B200VS_EILLEGAL_PARAMETERS, "dimension must be divisible by nsubvector");
+    ksub = 1 << nbits;
+    code_size = (M * nbits + 7) / 8;
   }
   bool is_trained() const override { return mode != kNone; }
   int sub_type() const override { return mode == kFlat ? (int)B200VS_FLAT : mode == kIvfPq ? (int)B200VS_IVF_PQ : -1; }  // ivf_pq.cc:474
@@ -233,14 +396,14 @@ struct IvfPqIndex : IndexBase {
     quiesce();
     centroids.free(); codebooks.free(); pre.free(); cent_ids.free();
     centroids.reserve((size_t)nlist * dim, 0, stream);
-    codebooks.reserve((size_t)M * KSUB * (dim / M), 0, stream);
+    codebooks.reserve((size_t)M * ksub * (dim / M), 0, stream);
     cent_ids.reserve(nlist, 0, stream);
     B200VS_CUDA(cudaMemcpyAsync(centroids.p, h_cent, (size_t)nlist * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(codebooks.p, h_cb, (size_t)M * KSUB * (dim / M) * 4, cudaMemcpyHostToDevice, stream));
+    B200VS_CUDA(cudaMemcpyAsync(codebooks.p, h_cb, (size_t)M * ksub * (dim / M) * 4, cudaMemcpyHostToDevice, stream));
     launch_iota(cent_ids.p, nlist, stream);
     if (metric == B200VS_L2) {
-      pre.reserve((size_t)nlist * M * KSUB, 0, stream);
-      pq_precompute_kernel<<<nlist, 256, 0, stream>>>(centroids.p, codebooks.p, dim, M, pre.p);
+      pre.reserve((size_t)nlist * M * ksub, 0, stream);
+      pq_precompute_kernel<<<nlist, 256, 0, stream>>>(centroids.p, codebooks.p, dim, M, ksub, pre.p);
       B200VS_CUDA(cudaGetLastError());
     }
     B200VS_CUDA(cudaStreamSynchronize(stream));
@@ -249,16 +412,17 @@ struct IvfPqIndex : IndexBase {
     mode = kIvfPq;
   }
 
-  // blob: int64 hdr[6] = {magic 'IVPQ', nlist, dim, metric, M, nbits}; centroids[nlist*dim]; codebooks[M*256*dsub]
+  // blob: int64 hdr[6] = {magic 'IVPQ', nlist, dim, metric, M, nbits}; centroids[nlist*dim]; codebooks[M*2^nbits*dsub]
   void set_state(const void* blob, size_t len) override {
     std::unique_lock<std::shared_mutex> wl(rw);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     if (len < 48) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
-    if (hdr[0] != 0x51505649 || hdr[2] != dim || hdr[4] != M || hdr[5] != 8) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF-PQ state blob");
+    if (hdr[0] != 0x51505649 || hdr[2] != dim || hdr[4] != M) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF-PQ state blob");
+    if (hdr[5] != nbits) fail(B200VS_EILLEGAL_PARAMETERS, "IVF-PQ state blob has another nbits_per_idx than this index");
     nlist = (int)hdr[1];
-    const size_t nc = (size_t)nlist * dim, ncb = (size_t)M * KSUB * (dim / M);
+    const size_t nc = (size_t)nlist * dim, ncb = (size_t)M * ksub * (dim / M);
     if (len < 48 + (nc + ncb) * 4) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
     const float* f = (const float*)((const char*)blob + 48);
     install(f, f + nc);
@@ -266,11 +430,11 @@ struct IvfPqIndex : IndexBase {
   int64_t get_state(void* blob, size_t cap) override {
     RwSharedGuard rl(this);
     if (mode != kIvfPq) return 0;
-    const size_t nc = (size_t)nlist * dim, ncb = (size_t)M * KSUB * (dim / M);
+    const size_t nc = (size_t)nlist * dim, ncb = (size_t)M * ksub * (dim / M);
     const size_t need = 48 + (nc + ncb) * 4;
     if (!blob || cap < need) return (int64_t)need;
     set_device();
-    int64_t hdr[6] = {0x51505649, nlist, dim, (int64_t)metric, M, 8};
+    int64_t hdr[6] = {0x51505649, nlist, dim, (int64_t)metric, M, nbits};
     memcpy(blob, hdr, 48);
     B200VS_CUDA(cudaMemcpy((char*)blob + 48, centroids.p, nc * 4, cudaMemcpyDeviceToHost));
     B200VS_CUDA(cudaMemcpy((char*)blob + 48 + nc * 4, codebooks.p, ncb * 4, cudaMemcpyDeviceToHost));
@@ -295,7 +459,7 @@ struct IvfPqIndex : IndexBase {
     {
       std::unique_lock<std::shared_mutex> wl(rw);
       if (mode != kNone) return;
-      const int64_t need = std::max<int64_t>(256LL * nlist, 256LL * KSUB);
+      const int64_t need = std::max<int64_t>(256LL * nlist, 256LL * ksub);
       if (n < need) {  // inner index = Flat
         flat.reset(make_flat(metric, dim, params));
         mode = kFlat;
@@ -316,7 +480,7 @@ struct IvfPqIndex : IndexBase {
                [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) { assign_dev(cd, kk, cid.p, xd, dim, l2, m, out); },
                [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); });
     // PQ training set: <= 256 * ksub vectors (fvecs_maybe_subsample, seed 1234), residuals to their centroid
-    int64_t m = std::min<int64_t>(n, 256LL * KSUB);
+    int64_t m = std::min<int64_t>(n, 256LL * ksub);
     std::vector<int64_t> perm(n);
     for (int64_t i = 0; i < n; ++i) perm[i] = i;
     if (m < n) {
@@ -344,13 +508,13 @@ struct IvfPqIndex : IndexBase {
     }
     // one k-means per sub-space (ksub centroids, 25 iterations, L2)
     const int dsub = dim / M;
-    std::vector<float> cb((size_t)M * KSUB * dsub), slice((size_t)m * dsub), cbm;
+    std::vector<float> cb((size_t)M * ksub * dsub), slice((size_t)m * dsub), cbm;
     for (int mm = 0; mm < M; ++mm) {
       for (int64_t i = 0; i < m; ++i) memcpy(&slice[(size_t)i * dsub], &sub[(size_t)i * dim + mm * dsub], (size_t)dsub * 4);
-      kmeans_gpu(this, B200VS_L2, dsub, m, slice.data(), KSUB, 25, 256, 1234, cbm,
+      kmeans_gpu(this, B200VS_L2, dsub, m, slice.data(), ksub, 25, 256, 1234, cbm,
                  [&](const float* xs, int64_t mr, const float* cs, int kk, long long* out) { assign_dev(cs, kk, cid.p, xs, dsub, true, mr, out); },
                  [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); });
-      memcpy(&cb[(size_t)mm * KSUB * dsub], cbm.data(), (size_t)KSUB * dsub * 4);
+      memcpy(&cb[(size_t)mm * ksub * dsub], cbm.data(), (size_t)ksub * dsub * 4);
     }
     install(cent.data(), cb.data());
   }
@@ -378,30 +542,37 @@ struct IvfPqIndex : IndexBase {
     if (metric == B200VS_COSINE) launch_normalize_faiss(st, n, dim, stream);
     assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, st_list);
     B200VS_CUDA(cudaFuncSetAttribute(pq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wpb * row_bytes)));
-    pq_encode_kernel<<<(unsigned)cdiv(n, wpb), wpb * 32, (size_t)wpb * row_bytes, stream>>>(st, st_list, centroids.p, codebooks.p, n, dim, M, st_codes);
+    pq_encode_kernel<<<(unsigned)cdiv(n, wpb), wpb * 32, (size_t)wpb * row_bytes, stream>>>(st, st_list, centroids.p, codebooks.p, n, dim, M, ksub, st_codes);
     B200VS_CUDA(cudaGetLastError());
+    if (nbits < 8) {
+      unsigned char* packed = scratch.alloc<unsigned char>((size_t)n * code_size);
+      pq_pack_kernel<<<(unsigned)cdiv(n * code_size, 256), 256, 0, stream>>>(st_codes, n, M, nbits, code_size, packed);
+      B200VS_CUDA(cudaGetLastError());
+      st_codes = packed;
+    }
     std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
     append_encoded(n, st_codes, st_ids, in_ids, h_list.data());
   }
 
-  // rows already encoded (device codes [n, M], device ids) go to the tails of their lists; callers hold the write lock
+  // rows already encoded (device codes [n, code_size], device ids) go to the tails of their lists; callers hold the write lock
   void append_encoded(int64_t n, const unsigned char* d_codes, const long long* d_ids, const int64_t* h_ids_in, const long long* h_list) {
+    const size_t cs = (size_t)code_size;
     std::vector<long long> slots(n);
     long long* st_slots = scratch.alloc<long long>(n);
     std::vector<int> need(nlist, 0);
     for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
     L.reserve_for(need, [&](int64_t rows) {
-      codes.reserve((size_t)rows * M, (size_t)L.arena_used_before * M, stream);
+      codes.reserve((size_t)rows * cs, (size_t)L.arena_used_before * cs, stream);
       ids.reserve((size_t)rows, (size_t)L.arena_used_before, stream);
     }, [&](int64_t src, int64_t dst, int64_t len) {
-      B200VS_CUDA(cudaMemcpyAsync(codes.p + (size_t)dst * M, codes.p + (size_t)src * M, (size_t)len * M, cudaMemcpyDeviceToDevice, stream));
+      B200VS_CUDA(cudaMemcpyAsync(codes.p + (size_t)dst * cs, codes.p + (size_t)src * cs, (size_t)len * cs, cudaMemcpyDeviceToDevice, stream));
       B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)len * 8, cudaMemcpyDeviceToDevice, stream));
     });
     for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], h_ids_in[i]);
     B200VS_CUDA(cudaMemcpyAsync(st_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    scatter_codes_kernel<<<(unsigned)cdiv(n * M, 256), 256, 0, stream>>>(d_codes, d_ids, st_slots, n, M, codes.p, ids.p);
+    scatter_codes_kernel<<<(unsigned)cdiv(n * code_size, 256), 256, 0, stream>>>(d_codes, d_ids, st_slots, n, code_size, codes.p, ids.p);
     B200VS_CUDA(cudaGetLastError());
     L.upload(stream);
     B200VS_CUDA(cudaStreamSynchronize(stream));
@@ -423,14 +594,14 @@ struct IvfPqIndex : IndexBase {
     std::vector<long long> src, dst;
     const int64_t new_rows = std::max<int64_t>(1, L.plan_compaction(src, dst));
     DevBuf<unsigned char> nc; DevBuf<long long> ni;
-    nc.reserve((size_t)new_rows * M, 0, stream); ni.reserve(new_rows, 0, stream);
+    nc.reserve((size_t)new_rows * code_size, 0, stream); ni.reserve(new_rows, 0, stream);
     const int64_t m = (int64_t)src.size();
     if (m) {
       long long* d_src = scratch.alloc<long long>(m);
       long long* d_dst = scratch.alloc<long long>(m);
       B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), m * 8, cudaMemcpyHostToDevice, stream));
       B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), m * 8, cudaMemcpyHostToDevice, stream));
-      move_codes_kernel<<<(unsigned)cdiv(m * M, 256), 256, 0, stream>>>(codes.p, ids.p, d_src, d_dst, m, M, nc.p, ni.p);
+      move_codes_kernel<<<(unsigned)cdiv(m * code_size, 256), 256, 0, stream>>>(codes.p, ids.p, d_src, d_dst, m, code_size, nc.p, ni.p);
       B200VS_CUDA(cudaGetLastError());
     }
     B200VS_CUDA(cudaStreamSynchronize(stream));
@@ -468,8 +639,9 @@ struct IvfPqIndex : IndexBase {
   // raw threshold (L2: dis < thr; IP: dis > thr), at most k of them, closest first; out_counts = hits per query.
   void scan_codes(int64_t nq, const float* xq, int k, const SearchCtx& sc, bool has_thr, float thr_raw, float* od, long long* oi, int* oc,
                   cudaStream_t s) {
-    const int T = M * KSUB;
-    const int pool_cap = select_pool_cap(k, PQ_THREADS);
+    const int T = M * ksub;
+    const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
+    const int pool_cap = select_pool_cap(k, threads);
     const size_t smem = (size_t)T * 4 + BlockSelect::smem_bytes(pool_cap);  // checked before anything is launched
     if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
     const float* q = prepare_queries(nq, xq, s);
@@ -484,10 +656,10 @@ struct IvfPqIndex : IndexBase {
     run_scan(this, cj, nq, q, nprobe, nullptr, coarse, probes, nullptr, s);
     if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
     float* sim = scratch.alloc<float>((size_t)nq * T);
-    pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, sim);
+    pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, ksub, sim);
     PqScanArgs a;
     a.codes = codes.p; a.ids = ids.p; a.probes = probes; a.coarse = coarse; a.list_off = L.d_off.p; a.list_len = L.d_len.p;
-    a.sim = sim; a.pre = l2 ? pre.p : nullptr; a.M = M; a.nprobe = nprobe; a.k = k;
+    a.sim = sim; a.pre = l2 ? pre.p : nullptr; a.M = M; a.code_size = code_size; a.nprobe = nprobe; a.k = k;
     a.nsplit = (int)std::max<int64_t>(1, std::min<int64_t>(nprobe, (device_sm_count(device) * 2 + nq - 1) / nq));
     a.pool_cap = pool_cap;
     a.has_thr = has_thr ? 1 : 0;
@@ -499,16 +671,21 @@ struct IvfPqIndex : IndexBase {
     const size_t smem2 = BlockSelect::smem_bytes(a.pool_cap);
     dim3 grid(a.nsplit, (unsigned)nq);
     ScopedKernelTimer timer(this, s, profiling);
-    if (l2) {
+    if (nbits < 8) {
+      if (l2) launch_pq_scan_packed<true>(nbits, grid, smem, s, a);
+      else launch_pq_scan_packed<false>(nbits, grid, smem, s, a);
+    } else if (l2) {
       B200VS_CUDA(cudaFuncSetAttribute(pq_scan_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       pq_scan_select_kernel<true><<<grid, PQ_THREADS, smem, s>>>(a);
-      timer.stop();
-      B200VS_CUDA(cudaFuncSetAttribute(merge_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      merge_select_kernel<true><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, nullptr, oi, oc, nullptr, nullptr);
     } else {
       B200VS_CUDA(cudaFuncSetAttribute(pq_scan_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       pq_scan_select_kernel<false><<<grid, PQ_THREADS, smem, s>>>(a);
-      timer.stop();
+    }
+    timer.stop();
+    if (l2) {
+      B200VS_CUDA(cudaFuncSetAttribute(merge_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      merge_select_kernel<true><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, nullptr, oi, oc, nullptr, nullptr);
+    } else {
       B200VS_CUDA(cudaFuncSetAttribute(merge_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       merge_select_kernel<false><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, nullptr, oi, oc, nullptr, nullptr);
     }
@@ -565,7 +742,7 @@ struct IvfPqIndex : IndexBase {
         get_state(st.data(), st.size());
         const int64_t n = count();
         std::vector<int64_t> off((size_t)nlist + 1, 0), fids((size_t)n);
-        std::vector<uint8_t> cds((size_t)n * M);
+        std::vector<uint8_t> cds((size_t)n * code_size);
         export_lists(off.data(), nullptr, cds.data(), fids.data());
         hdr[6] = n; hdr[7] = st_len;
         wr(hdr, sizeof(hdr)); wr(st.data(), st.size()); wr(off.data(), off.size() * 8); wr(fids.data(), fids.size() * 8); wr(cds.data(), cds.size());
@@ -599,9 +776,11 @@ struct IvfPqIndex : IndexBase {
       } else if (hdr[1] == kIvfPq) {
         std::vector<unsigned char> st((size_t)hdr[7]);
         rd(st.data(), st.size());
+        if (st.size() < 48 || ((const int64_t*)st.data())[5] != nbits)  // nbits travels in the embedded trained-state blob
+          fail(B200VS_EINTERNAL, "index file does not match this index (nbits_per_idx)");
         set_state(st.data(), st.size());  // centroids, codebooks, precomputed table; nlist from the blob
         std::vector<int64_t> off((size_t)nlist + 1), fids((size_t)n);
-        std::vector<uint8_t> cds((size_t)n * M);
+        std::vector<uint8_t> cds((size_t)n * code_size);
         rd(off.data(), off.size() * 8); rd(fids.data(), fids.size() * 8); rd(cds.data(), cds.size());
         if (off[nlist] != n) fail(B200VS_EINTERNAL, "corrupt index file (list offsets)");
         std::unique_lock<std::shared_mutex> wl(rw);
@@ -613,9 +792,9 @@ struct IvfPqIndex : IndexBase {
         for (int64_t a = 0; a < n; a += 262144) {
           const int64_t m = std::min<int64_t>(262144, n - a);
           scratch.reset(stream);
-          unsigned char* d_codes = scratch.alloc<unsigned char>((size_t)m * M);
+          unsigned char* d_codes = scratch.alloc<unsigned char>((size_t)m * code_size);
           long long* d_ids = scratch.alloc<long long>(m);
-          B200VS_CUDA(cudaMemcpyAsync(d_codes, cds.data() + (size_t)a * M, (size_t)m * M, cudaMemcpyHostToDevice, stream));
+          B200VS_CUDA(cudaMemcpyAsync(d_codes, cds.data() + (size_t)a * code_size, (size_t)m * code_size, cudaMemcpyHostToDevice, stream));
           B200VS_CUDA(cudaMemcpyAsync(d_ids, fids.data() + a, (size_t)m * 8, cudaMemcpyHostToDevice, stream));
           append_encoded(m, d_codes, d_ids, fids.data() + a, h_list.data() + a);
         }
@@ -635,15 +814,16 @@ struct IvfPqIndex : IndexBase {
       if (list_off) list_off[l] = o;
       const auto& m = L.lists[l];
       if (m.len == 0) continue;
+      const size_t cs = (size_t)code_size;
       if (out_codes) {
-        buf.resize((size_t)m.len * M);
-        B200VS_CUDA(cudaMemcpy(buf.data(), codes.p + (size_t)m.off * M, (size_t)m.len * M, cudaMemcpyDeviceToHost));
+        buf.resize((size_t)m.len * cs);
+        B200VS_CUDA(cudaMemcpy(buf.data(), codes.p + (size_t)m.off * cs, (size_t)m.len * cs, cudaMemcpyDeviceToHost));
       }
       for (int p = 0; p < m.len; ++p) {
         const int64_t id = L.h_ids[m.off + p];
         if (id < 0) continue;
         if (out_ids) out_ids[o] = id;
-        if (out_codes) memcpy(out_codes + (size_t)o * M, buf.data() + (size_t)p * M, (size_t)M);
+        if (out_codes) memcpy(out_codes + (size_t)o * cs, buf.data() + (size_t)p * cs, cs);
         ++o;
       }
     }

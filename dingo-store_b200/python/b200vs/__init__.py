@@ -481,7 +481,11 @@ class BruteForceScan:
 
 
 def ivfpq_state_blob(centroids, codebooks, metric):
-    """Trained-state blob of an IVF-PQ index: centroids [nlist, d] + codebooks [M, 256, d/M]."""
+    """Trained-state blob of an IVF-PQ index: centroids [nlist, d] + codebooks [M, 2^nbits, d/M] (nbits 1-8, taken from
+    the codebook shape: 256 codewords -> 8 bits)."""
     c, cb = _f32(centroids), _f32(codebooks)
-    hdr = np.array([0x51505649, c.shape[0], c.shape[1], metric, cb.shape[0], 8], dtype=np.int64)
+    ksub = cb.shape[1]
+    if ksub < 2 or ksub > 256 or ksub & (ksub - 1):
+        raise ValueError(f"codebooks must have 2^nbits codewords per sub-space, nbits 1-8 (got {ksub})")
+    hdr = np.array([0x51505649, c.shape[0], c.shape[1], metric, cb.shape[0], ksub.bit_length() - 1], dtype=np.int64)
     return np.concatenate([hdr.view(np.uint8), c.reshape(-1).view(np.uint8), cb.reshape(-1).view(np.uint8)])

@@ -53,7 +53,7 @@ typedef enum {
 typedef struct {
   int32_t nlist;        /* ncentroids; default 2048 */
   int32_t pq_m;         /* nsubvector; default 64   */
-  int32_t pq_nbits;     /* nbits_per_idx; default 8 (only 8 is implemented) */
+  int32_t pq_nbits;     /* nbits_per_idx 1-8 (faiss bit-packed codes); <= 0 -> 8; 9-16 refused (EILLEGAL_PARAMETERS) */
   int32_t hnsw_m;       /* nlinks */
   int32_t hnsw_efc;     /* efconstruction */
   int64_t max_elements; /* hnsw max_elements */
@@ -144,7 +144,7 @@ int b200vs_load(b200vs_index* idx, const char* path);
 /* Export the inverted lists in list-major order (list l owns rows [list_off[l], list_off[l+1])) so a CPU
  * implementation can search the identical index.  Any output pointer may be NULL.  Flat: nlist = 1. */
 int b200vs_export_lists(b200vs_index* idx, int64_t* list_off /*[nlist+1]*/, float* vectors /*[count,dim]*/,
-                        uint8_t* codes /*[count,pq_m]*/, int64_t* ids /*[count]*/);
+                        uint8_t* codes /*[count, ceil(pq_m*pq_nbits/8)]*/, int64_t* ids /*[count]*/);
 
 /* One inverted list (live rows only, stored order): writes up to `cap` rows into vectors [cap, dim] / ids [cap] (either may
  * be NULL) and the list's live row count into *count.  Lets a checker rebuild exactly the lists a query probes without
