@@ -8,6 +8,8 @@
   cfg5  IVF-Flat L2, (rows-per-GPU x world) x 1536, nlist 2048 per GPU, nprobe 64, batch 4096, top-10, list-sharded over
         the GPUs of the box through b200vs_shard_* — run under torchrun (BASELINE: 100 M rows over 8 GPUs = 77 GB per GPU, more
         than an 80 GB H100 holds: default 6.25 M rows per GPU, 50 M over 8)
+  cfg6  Binary Flat Hamming, 1M x 256 bits, batch 1024, top-10
+  cfg7  Binary IVF-Flat Hamming, 10M x 512 bits, nlist 2048, nprobe 80, batch 1024, top-10   (--bin-n, --bin-dim)
 Each line: device-resident QPS (CUDA events), e2e QPS through the host-pointer C ABI, parity with the oracle on a
 bounded sample, the dominant kernel's time from the library's profiling mode and the algorithmic figure of
 SURVEY.md §8(d).  Scaled sizes are stated in the line ("scaled_from").
@@ -29,6 +31,7 @@ import torch  # noqa: E402
 import b200vs  # noqa: E402
 import oracle_lib  # noqa: E402
 import pq_codes  # noqa: E402
+import binary_oracle  # noqa: E402
 import b200vs.shard as shard_host  # noqa: E402
 
 
@@ -475,6 +478,73 @@ def cfg_brute(o, cores):
             "cpu_baseline_seconds_scaled": cpu_s, "cpu_cores": cores}
 
 
+# __popc issues 16 per clock per SM on sm_90 (CUDA programming guide throughput table; not measured): 132 SMs at ~1.7 GHz
+POPC_BOUND_WORDS_PER_S = 16 * 132 * 1.7e9
+
+
+def rnd_bits(n, nb, seed):
+    g = torch.Generator(device="cuda")
+    g.manual_seed(seed)
+    out = np.empty((n, nb), np.uint8)
+    for a in range(0, n, 1 << 20):
+        m = min(1 << 20, n - a)
+        out[a:a + m] = torch.randint(0, 256, (m, nb), generator=g, device="cuda", dtype=torch.uint8).cpu().numpy()
+    return out
+
+
+def binary_line(name, ix, xq, k, word_popcounts, Do, Io, oracle_q, **kw):
+    """Device / e2e QPS, list-scan kernel time, word popcounts per second against the popcount bound, parity on the first
+    oracle_q queries."""
+    nq = xq.shape[0]
+    dev_ms, e2e_ms, st, D, I = time_search(ix, xq, k, **kw)
+    kernel_s = st[3] / 1e9
+    return {"config": name, "qps_device": nq / dev_ms * 1e3, "ms_per_batch_device": dev_ms, "qps_e2e": nq / e2e_ms * 1e3,
+            "ids_bit_exact": bool(np.array_equal(I[:oracle_q], Io)), "dist_bit_exact": bool(np.array_equal(D[:oracle_q].view(np.uint32), Do.view(np.uint32))),
+            "parity_sample": f"first {oracle_q} of {nq} queries against tests/binary_oracle.py",
+            "roofline": {"bound": "popcount issue rate", "kernel": "scan_select_kernel<HammingDist>", "kernel_ms": kernel_s * 1e3,
+                         "word_popcounts": word_popcounts, "achieved": word_popcounts / max(kernel_s, 1e-12), "unit": "word popcounts/s",
+                         "peak": POPC_BOUND_WORDS_PER_S, "frac": word_popcounts / max(kernel_s, 1e-12) / POPC_BOUND_WORDS_PER_S,
+                         "peak_source": "16 __popc / clock / SM (CUDA programming guide) x 132 SMs x 1.7 GHz, not measured"},
+            "path": "exact Hamming scan (query-major)", "search_stats": st}
+
+
+def cfg6(o, cores, oracle_q=64):
+    n, dim, nq, k = 1_000_000, 256, 1024, 10
+    nb, w = dim // 8, (dim // 8 + 3) // 4
+    xb = rnd_bits(n, nb, 1234)
+    ids = np.arange(1, n + 1, dtype=np.int64)
+    ix = b200vs.Index(b200vs.BINARY_FLAT, b200vs.HAMMING, dim)
+    for a in range(0, n, 1 << 18):
+        ix.add(xb[a:a + (1 << 18)], ids[a:a + (1 << 18)])
+    xq = rnd_bits(nq, nb, 4321)
+    Do, Io = binary_oracle.flat_search(xb, ids, xq[:oracle_q], k)
+    return binary_line(f"cfg6 Binary Flat Hamming {n}x{dim} bits batch={nq} top-{k}", ix, xq, k, nq * n * w, Do, Io, oracle_q)
+
+
+def cfg7(o, cores, n, dim, oracle_q=16):
+    nlist, nprobe, nq, k = 2048, 80, 1024, 10
+    nb, w = dim // 8, (dim // 8 + 3) // 4
+    xb = rnd_bits(n, nb, 1234)
+    ids = np.arange(1, n + 1, dtype=np.int64)
+    ix = b200vs.Index(b200vs.BINARY_IVF_FLAT, b200vs.HAMMING, dim, nlist=nlist)
+    t = time.perf_counter()
+    ix.train(xb)
+    train_s = time.perf_counter() - t
+    for a in range(0, n, 1 << 20):
+        ix.add(xb[a:a + (1 << 20)], ids[a:a + (1 << 20)])
+    xq = rnd_bits(nq, nb, 4321)
+    cent = ix.get_trained_state()[32:].reshape(-1, nb)
+    off, _, codes, lids = ix.export_lists(cent.shape[0])
+    P = binary_oracle.probes(cent, xq, min(nprobe, cent.shape[0]))
+    rows = int(np.diff(off)[P].sum())  # candidate rows over the batch: each is one row of w word popcounts
+    Do, Io = binary_oracle.ivf_search(cent, off, codes, lids, xq[:oracle_q], k, nprobe)
+    line = binary_line(f"cfg7 Binary IVF-Flat Hamming {n}x{dim} bits nlist={nlist} nprobe={nprobe} batch={nq} top-{k}", ix, xq, k, rows * w,
+                       Do, Io, oracle_q, nprobe=nprobe)
+    line["scaled_from"] = None if (n, dim) == (10_000_000, 512) else "10M x 512 bits"
+    line["train_seconds"] = train_s
+    return line
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="1,2,3,4")
@@ -486,13 +556,16 @@ def main():
     ap.add_argument("--cfg5-rows", type=int, default=6_250_000, help="cfg5: database rows per GPU (6.25 M x 1536 f32 = 38 GB of an 80 GB H100)")
     ap.add_argument("--cfg5-batch", type=int, default=4096)
     ap.add_argument("--cfg5-steps", type=int, default=10)
+    ap.add_argument("--bin-n", type=int, default=10_000_000, help="cfg7: database rows")
+    ap.add_argument("--bin-dim", type=int, default=512, help="cfg7: bits per row (multiple of 8)")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     o = oracle_lib.load()
     cores = os.cpu_count() or 1
     fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
-           "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch)}
+           "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
+           "6": lambda: cfg6(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}
     rank = int(os.environ.get("RANK", 0))
     for c in a.configs.split(","):
         t0 = time.time()

@@ -58,7 +58,13 @@ SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s
   return sc;
 }
 
-void check_search_args(IndexBase* ix, int64_t nq, const float* xq, const b200vs_search_params* sp) {
+// the float entry points (train / add / search / range search) on a binary index, and the binary ones on a float index
+void check_row_type(IndexBase* ix, bool binary_call) {
+  if (ix->binary() != binary_call)
+    fail(B200VS_EILLEGAL_PARAMETERS, binary_call ? "binary entry point on a float index" : "float entry point on a binary index");
+}
+
+void check_search_args(IndexBase* ix, int64_t nq, const void* xq, const b200vs_search_params* sp) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");  // flat.cc:208-210
   if (ix->type == B200VS_HNSW && sp && (sp->efsearch < 0 || sp->efsearch > 1024))
     fail(B200VS_EILLEGAL_PARAMETERS, "efsearch is illegal, " + std::to_string(sp->efsearch) + ", must between 0 and 1024");  // hnsw.cc:332-336
@@ -73,7 +79,13 @@ int b200vs_create(b200vs_type type, b200vs_metric metric, int32_t dim, const b20
     if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
     *out = nullptr;
     if (dim <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "dimension must be > 0");
-    if (metric != B200VS_L2 && metric != B200VS_IP && metric != B200VS_COSINE) fail(B200VS_EILLEGAL_PARAMETERS, "unsupported metric type");
+    const bool binary = type == B200VS_BINARY_FLAT || type == B200VS_BINARY_IVF_FLAT;
+    if (binary) {  // vector_index_utils.cc:1075-1140: HAMMING only, dimension in bits, dim % 8 == 0, dim <= kVectorMaxDimension
+      if (metric != B200VS_HAMMING) fail(B200VS_EILLEGAL_PARAMETERS, "binary indexes support only METRIC_TYPE_HAMMING");
+      if (dim % 8 != 0 || dim > 32768) fail(B200VS_EILLEGAL_PARAMETERS, "binary dimension must be a multiple of 8 in (0, 32768]");
+    } else if (metric != B200VS_L2 && metric != B200VS_IP && metric != B200VS_COSINE) {
+      fail(B200VS_EILLEGAL_PARAMETERS, "unsupported metric type");
+    }
     b200vs_params p;
     memset(&p, 0, sizeof(p));
     if (params) p = *params;
@@ -86,6 +98,8 @@ int b200vs_create(b200vs_type type, b200vs_metric metric, int32_t dim, const b20
       case B200VS_IVF_FLAT: impl = make_ivf_flat(metric, dim, p); break;
       case B200VS_IVF_PQ: impl = make_ivf_pq(metric, dim, p); break;
       case B200VS_HNSW: impl = make_hnsw(metric, dim, p); break;
+      case B200VS_BINARY_FLAT: impl = make_binary_flat(dim, p); break;
+      case B200VS_BINARY_IVF_FLAT: impl = make_binary_ivf(dim, p); break;
       default: fail(B200VS_EILLEGAL_PARAMETERS, "unknown index type");
     }
     *out = new b200vs_index{impl};
@@ -102,6 +116,7 @@ void b200vs_destroy(b200vs_index* h) {
 int b200vs_train(b200vs_index* h, int64_t n, const float* x) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    check_row_type(ix, false);
     if (n <= 0 || !x) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");  // ivf_flat.cc:646-649
     ix->train(n, x);
     return B200VS_OK;
@@ -126,6 +141,7 @@ int64_t b200vs_get_trained_state(b200vs_index* h, void* blob, size_t cap) {
 int b200vs_add_with_ids(b200vs_index* h, int64_t n, const float* x, const int64_t* ids, int upsert) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    check_row_type(ix, false);
     if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");  // flat.cc:123-125
     ix->add(n, x, ids, upsert != 0);
     return B200VS_OK;
@@ -173,7 +189,8 @@ int b200vs_remove_ids(b200vs_index* h, int64_t n, const int64_t* ids, int64_t* n
     const int64_t r = ix->remove(n, ids);
     if (n_removed) *n_removed = r < 0 ? 0 : r;
     // IVF types: "remove not found vector id" -> EVECTOR_INVALID (ivf_flat.cc:180-184); untrained -> OK (r == -1)
-    if (r == 0 && (ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ)) fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
+    if (r == 0 && (ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ || ix->type == B200VS_BINARY_IVF_FLAT))
+      fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
     return B200VS_OK;
   });
 }
@@ -182,6 +199,7 @@ int b200vs_search_device(b200vs_index* h, int64_t nq, const float* xq_dev, int32
                          float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    check_row_type(ix, false);
     check_search_args(ix, nq, xq_dev, sp);
     if (k <= 0) return B200VS_OK;  // "topk <= 0 -> OK", flat.cc:212
     if (!out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
@@ -236,6 +254,7 @@ int b200vs_search_probes_device(b200vs_index* h, int64_t nq, const float* xq_dev
 int b200vs_debug_tc_scores(b200vs_index* h, int64_t nq, const float* xq, int32_t split, float* out_scores, float* out_eps) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    if (ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, "binary indexes have no tensor-core scores");
     if (ix->type != B200VS_FLAT) fail(B200VS_EILLEGAL_PARAMETERS, "tensor-core score diagnostics only exist for FLAT");
     if (ix->dim % 4 != 0 || ix->dim < 32) fail(B200VS_EILLEGAL_PARAMETERS, "the tile kernel needs dim % 4 == 0 and dim >= 32");
     if (nq <= 0 || !xq || !out_scores || !out_eps) fail(B200VS_EILLEGAL_PARAMETERS, "bad diagnostic arguments");
@@ -362,6 +381,7 @@ int b200vs_search(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const
                   int64_t* out_ids) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    check_row_type(ix, false);
     check_search_args(ix, nq, xq, sp);
     if (k <= 0) return B200VS_OK;
     if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
@@ -388,6 +408,7 @@ int b200vs_range_search(b200vs_index* h, int64_t nq, const float* xq, float radi
                         const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
+    check_row_type(ix, false);
     check_search_args(ix, nq, xq, sp);
     if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // hnsw.cc:487-493
     if (max_results <= 0 || !out_ids || !out_dist || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
@@ -545,6 +566,7 @@ int b200vs_scan_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t
     if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
     *out = nullptr;
     if (dim <= 0) fail(B200VS_EVECTOR_INVALID, "vector index dimension is invalid");  // vector_reader.cc:1889-1894
+    if (metric == B200VS_HAMMING) fail(B200VS_EVECTOR_NOT_SUPPORT, "brute-force scan of binary vectors is not implemented");
     if (metric != B200VS_L2 && metric != B200VS_IP && metric != B200VS_COSINE) fail(B200VS_EILLEGAL_PARAMETERS, "unsupported metric type");
     if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
     if (k <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "topk must be > 0");
@@ -616,6 +638,102 @@ int b200vs_scan_finish(b200vs_scan* st, float* out_dist, int64_t* out_ids) {
 }
 
 void b200vs_scan_abort(b200vs_scan* st) { delete st; }
+
+// ---- binary indexes (binary.cu): packed rows, dim / 8 bytes each ----
+int b200vs_train_binary(b200vs_index* h, int64_t n, const uint8_t* x) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, true);
+    if (n <= 0 || !x) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
+    ix->train_binary(n, x);
+    return B200VS_OK;
+  });
+}
+
+int b200vs_add_with_ids_binary(b200vs_index* h, int64_t n, const uint8_t* x, const int64_t* ids, int upsert) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, true);
+    if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+    ix->add_binary(n, x, ids, upsert != 0);
+    return B200VS_OK;
+  });
+}
+
+int b200vs_search_binary_device(b200vs_index* h, int64_t nq, const uint8_t* xq_dev, int32_t k, const b200vs_search_params* sp,
+                                float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, true);
+    check_search_args(ix, nq, xq_dev, sp);
+    if (k <= 0) return B200VS_OK;
+    if (!out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    ix->set_device();
+    LaneGuard lane(ix, (cudaStream_t)stream);
+    ix->reset_stats();
+    SearchCtx sc = make_ctx(ix, sp, lane.stream);
+    ix->search_binary_dev(nq, xq_dev, k, sc, out_dist_dev, (long long*)out_ids_dev, lane.stream);
+    ix->phases_finish(lane.stream);
+    if (!stream) B200VS_CUDA(cudaStreamSynchronize(lane.stream));
+    return B200VS_OK;
+  });
+}
+
+int b200vs_search_binary(b200vs_index* h, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
+                         int64_t* out_ids) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, true);
+    check_search_args(ix, nq, xq, sp);
+    if (k <= 0) return B200VS_OK;
+    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    ix->set_device();
+    LaneGuard lane(ix, nullptr);
+    cudaStream_t s = lane.stream;
+    ix->reset_stats();
+    uint8_t* dq = ix->scratch.alloc<uint8_t>((size_t)nq * (ix->dim / 8));
+    float* dd = ix->scratch.alloc<float>((size_t)nq * k);
+    long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
+    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * (ix->dim / 8), cudaMemcpyHostToDevice, s));
+    SearchCtx sc = make_ctx(ix, sp, s);
+    ix->search_binary_dev(nq, dq, k, sc, dd, di, s);
+    ix->phases_finish(s);
+    B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+    return B200VS_OK;
+  });
+}
+
+int b200vs_range_search_binary(b200vs_index* h, int64_t nq, const uint8_t* xq, float radius, int32_t max_results,
+                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, true);
+    check_search_args(ix, nq, xq, sp);
+    if (max_results <= 0 || !out_ids || !out_dist || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    ix->set_device();
+    LaneGuard lane(ix, nullptr);
+    cudaStream_t s = lane.stream;
+    ix->reset_stats();
+    uint8_t* dq = ix->scratch.alloc<uint8_t>((size_t)nq * (ix->dim / 8));
+    float* dd = ix->scratch.alloc<float>((size_t)nq * max_results);
+    long long* di = ix->scratch.alloc<long long>((size_t)nq * max_results);
+    int* dc = ix->scratch.alloc<int>((size_t)nq);
+    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * (ix->dim / 8), cudaMemcpyHostToDevice, s));
+    SearchCtx sc = make_ctx(ix, sp, s);
+    ix->range_search_binary_dev(nq, dq, radius, max_results, sc, dd, di, dc, s);
+    ix->phases_finish(s);
+    B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * max_results * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * max_results * 8, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+    return B200VS_OK;
+  });
+}
 
 int b200vs_last_phase_times(b200vs_index* h, float ms[16]) {
   return guarded([&]() -> int {

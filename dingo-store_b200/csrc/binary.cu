@@ -1,0 +1,585 @@
+// binary.cu — Binary Flat and Binary IVF-Flat: Hamming search over packed bits.
+//
+// The GPU replacements of the faiss::IndexBinary instantiations of the Flat and IVF-Flat plugins
+// (VectorIndexFlat<IndexBinary, IndexBinaryIDMap2>, src/vector/vector_index_flat.cc:71, :99-102;
+// VectorIndexIvfFlat<IndexBinary>, vector_index_ivf_flat.cc:62; built by vector_index_factory.cc:73-80, :381-425).
+//
+// Rows are packed bits, dim / 8 bytes each.  On the device a row takes w = ceil(dim / 32) 32-bit words, zero padded, and
+// queries are padded the same way, so the padding adds 0 to every XOR popcount.  Searches run on the exact scan
+// (scan_select_kernel<HammingDist> + merge_select_kernel, scan_kernels.cuh) with key f2ord((float)distance): distances
+// are exact integers <= 32768, so the key orders them like the integers and results are ordered by (distance, id).
+#include <cmath>
+#include <cstdio>
+
+#include "index.h"
+#include "ivf_common.h"
+
+namespace b200vs {
+
+namespace {
+
+// dst[r, j] = bytes 4j .. 4j+3 of packed row r (little-endian word), zero past nbytes
+__global__ void pad_rows_kernel(const uint8_t* __restrict__ src, long long n, int nbytes, int w, uint32_t* __restrict__ dst) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * w) return;
+  const long long r = i / w;
+  const int j = (int)(i % w);
+  const uint8_t* row = src + (size_t)r * nbytes;
+  uint32_t v = 0;
+  for (int b = 0; b < 4; ++b)
+    if (4 * j + b < nbytes) v |= (uint32_t)row[4 * j + b] << (8 * b);
+  dst[i] = v;
+}
+
+// dst row dst_rows[r] = src row (src_rows ? src_rows[r] : r), words and id
+__global__ void copy_rows_kernel(const uint32_t* __restrict__ src, const long long* __restrict__ sids, const long long* __restrict__ src_rows,
+                                 const long long* __restrict__ dst_rows, long long n, int w, uint32_t* dst, long long* dids) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * w) return;
+  const long long r = i / w;
+  const int j = (int)(i % w);
+  const long long sr = src_rows ? src_rows[r] : r, dr = dst_rows[r];
+  dst[(size_t)dr * w + j] = src[(size_t)sr * w + j];
+  if (j == 0) dids[dr] = sids[sr];
+}
+
+int words_of(int dim) { return (dim / 8 + 3) / 4; }
+
+}  // namespace
+
+// Device rows of a binary index: [cap, w] words and ids (-1 = tombstone / unused slot).  The owner decides capacities and
+// slots; the store moves rows.  All work runs on the owner's stream.
+struct BinRows {
+  IndexBase* const ix;
+  const int w;
+  DevBuf<uint32_t> words;
+  DevBuf<long long> ids;
+  explicit BinRows(IndexBase* owner) : ix(owner), w(words_of(owner->dim)) {}
+
+  void grow(int64_t cap, int64_t keep) {
+    words.reserve((size_t)cap * w, (size_t)keep * w, ix->stream);
+    ids.reserve(cap, keep, ix->stream);
+  }
+  void reset() { words.free(); ids.free(); }
+  void move(int64_t src, int64_t dst, int64_t n) {
+    B200VS_CUDA(cudaMemcpyAsync(words.p + (size_t)dst * w, words.p + (size_t)src * w, (size_t)n * w * 4, cudaMemcpyDeviceToDevice, ix->stream));
+    B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)n * 8, cudaMemcpyDeviceToDevice, ix->stream));
+  }
+  void copy(const uint32_t* src, const long long* sids, const long long* src_rows, const long long* dst_rows, int64_t n, uint32_t* dst,
+            long long* dids) {
+    if (n <= 0) return;
+    copy_rows_kernel<<<(unsigned)cdiv(n * w, 256), 256, 0, ix->stream>>>(src, sids, src_rows, dst_rows, n, w, dst, dids);
+    B200VS_CUDA(cudaGetLastError());
+  }
+  // x / xids: device padded rows and ids; row i goes to slot slots[i]
+  void write(const uint32_t* x, const long long* xids, const std::vector<long long>& slots) {
+    const int64_t n = (int64_t)slots.size();
+    long long* d_slots = ix->scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(d_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ix->stream));
+    copy(x, xids, nullptr, d_slots, n, words.p, ids.p);
+  }
+  void tombstone(const std::vector<int64_t>& rows) {
+    if (rows.empty()) return;
+    long long* d_rows = ix->scratch.alloc<long long>(rows.size());
+    B200VS_CUDA(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, ix->stream));
+    launch_set_ids(ids.p, d_rows, (int64_t)rows.size(), -1, ix->stream);
+    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+  }
+  // compaction: fresh buffers of cap rows holding row src[i] at dst[i]
+  void gather(const std::vector<long long>& src, const std::vector<long long>& dst, int64_t cap) {
+    const int64_t n = (int64_t)src.size();
+    DevBuf<uint32_t> nw; DevBuf<long long> ni;
+    nw.reserve((size_t)cap * w, 0, ix->stream); ni.reserve(cap, 0, ix->stream);
+    if (n) {
+      long long* d_src = ix->scratch.alloc<long long>(n);
+      long long* d_dst = ix->scratch.alloc<long long>(n);
+      B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), n * 8, cudaMemcpyHostToDevice, ix->stream));
+      B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), n * 8, cudaMemcpyHostToDevice, ix->stream));
+      copy(words.p, ids.p, d_src, d_dst, n, nw.p, ni.p);
+    }
+    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+    words.swap(nw); ids.swap(ni);
+  }
+  // rows [r0, r0 + n) as packed bytes [n, dim / 8] on the host
+  void download(int64_t r0, int64_t n, uint8_t* out) const {
+    if (n <= 0) return;
+    const int nb = ix->dim / 8;
+    std::vector<uint32_t> tmp((size_t)n * w);
+    B200VS_CUDA(cudaMemcpy(tmp.data(), words.p + (size_t)r0 * w, tmp.size() * 4, cudaMemcpyDeviceToHost));
+    for (int64_t i = 0; i < n; ++i) memcpy(out + (size_t)i * nb, tmp.data() + (size_t)i * w, nb);
+  }
+  int64_t bytes() const { return (int64_t)(words.cap * 4 + ids.cap * 8); }
+};
+
+// Shared by both binary types: the float entry points are refused (api.cu checks first), rows arrive packed.
+struct BinaryIndex : IndexBase {
+  const int nb, w;  // bytes per packed row; 32-bit words per padded row
+  BinaryIndex(b200vs_type t, int d, const b200vs_params& p) : IndexBase(t, B200VS_HAMMING, d, p), nb(d / 8), w(words_of(d)) {}
+
+  void add(int64_t, const float*, const int64_t*, bool) override { fail(B200VS_EILLEGAL_PARAMETERS, "float entry point on a binary index"); }
+  void search_dev(int64_t, const float*, int, const SearchCtx&, float*, long long*, cudaStream_t) override {
+    fail(B200VS_EILLEGAL_PARAMETERS, "float entry point on a binary index");
+  }
+
+  // packed device rows -> padded words in scratch
+  const uint32_t* pad(int64_t n, const uint8_t* x_dev, cudaStream_t s) {
+    uint32_t* out = scratch.alloc<uint32_t>((size_t)std::max<int64_t>(n, 1) * w);
+    if (n > 0) {
+      pad_rows_kernel<<<(unsigned)cdiv(n * w, 256), 256, 0, s>>>(x_dev, n, nb, w, out);
+      B200VS_CUDA(cudaGetLastError());
+      launch_count(1);
+    }
+    return out;
+  }
+  // host packed rows -> padded device words in scratch (writers: on the index stream)
+  const uint32_t* upload(int64_t n, const uint8_t* x) {
+    uint8_t* raw = scratch.alloc<uint8_t>((size_t)n * nb);
+    B200VS_CUDA(cudaMemcpyAsync(raw, x, (size_t)n * nb, cudaMemcpyHostToDevice, stream));
+    return pad(n, raw, stream);
+  }
+  ScanJob hamming_job(const uint32_t* rows, const long long* ids, long long n) const {
+    ScanJob j;
+    j.hamming = true;
+    j.vecs = reinterpret_cast<const float*>(rows); j.ids = ids; j.d = w; j.mode = 0; j.n = n;
+    return j;
+  }
+  // IndexBinary::range_search takes an int radius (flat.cc:304-308): the float is truncated toward zero, and hits have
+  // dis < radius.  Every radius above dim + 1 admits the same rows, so larger values (and +inf) are clamped there first.
+  float radius_threshold(float radius) const {
+    if (std::isnan(radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");
+    return std::trunc(std::min(radius, (float)(dim + 1)));
+  }
+
+  // Own container (not faiss write_index_binary): header, trained-state blob, list offsets, ids, then the live rows packed,
+  // dim / 8 bytes each, in list-major order.
+  struct BinHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
+  void save(const std::string& path) override;
+  void load(const std::string& path) override;
+};
+
+namespace {
+void wr(FILE* f, const void* p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short write"); }
+void rd(FILE* f, void* p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short read / truncated index file"); }
+}  // namespace
+
+void BinaryIndex::save(const std::string& path) {
+  RwSharedGuard hold(this);
+  const int64_t st_len = get_state(nullptr, 0);
+  std::vector<unsigned char> st((size_t)std::max<int64_t>(st_len, 0));
+  if (st_len > 0) get_state(st.data(), st.size());
+  const int nl = export_nlist();
+  const int64_t n = count();
+  std::vector<int64_t> off(nl + 1, 0), ids((size_t)n);
+  std::vector<uint8_t> rows((size_t)n * nb);
+  if (n) export_lists(off.data(), nullptr, rows.data(), ids.data());
+  FILE* f = fopen(path.c_str(), "wb");
+  if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
+  try {
+    BinHdr h;
+    memcpy(h.magic, "B2VSBIN1", 8);
+    h.type = type; h.metric = metric; h.dim = dim; h.nlist = nl; h.state_len = st_len > 0 ? st_len : 0; h.count = n;
+    wr(f, &h, sizeof(h));
+    wr(f, st.data(), st.size());
+    wr(f, off.data(), off.size() * 8);
+    wr(f, ids.data(), ids.size() * 8);
+    wr(f, rows.data(), rows.size());
+  } catch (...) { fclose(f); throw; }
+  fclose(f);
+}
+
+void BinaryIndex::load(const std::string& path) {
+  FILE* f = fopen(path.c_str(), "rb");
+  if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
+  try {
+    BinHdr h;
+    rd(f, &h, sizeof(h));
+    if (memcmp(h.magic, "B2VSBIN1", 8) != 0 || h.type != (int)type || h.metric != (int)metric || h.dim != dim)
+      fail(B200VS_EINTERNAL, "index file does not match this index (type / metric / dimension)");
+    if (count() != 0) fail(B200VS_EINTERNAL, "load into a non-empty index");
+    {
+      const long here = ftell(f);
+      fseek(f, 0, SEEK_END);
+      const long fsize = ftell(f);
+      fseek(f, here, SEEK_SET);
+      const double need = (double)h.state_len + ((double)h.nlist + 1) * 8 + (double)h.count * (8 + (double)nb);
+      if (h.state_len < 0 || h.count < 0 || h.nlist < 0 || h.nlist > (1 << 24) || need > (double)(fsize - here))
+        fail(B200VS_EINTERNAL, "corrupt index file (header sizes exceed the file)");
+    }
+    std::vector<unsigned char> st((size_t)h.state_len);
+    rd(f, st.data(), st.size());
+    if (h.state_len > 0) set_state(st.data(), st.size());
+    std::vector<int64_t> off((size_t)h.nlist + 1), ids((size_t)h.count);
+    std::vector<uint8_t> rows((size_t)h.count * nb);
+    rd(f, off.data(), off.size() * 8);
+    rd(f, ids.data(), ids.size() * 8);
+    rd(f, rows.data(), rows.size());
+    for (int64_t a = 0; a < h.count; a += 32768) {
+      const int64_t m = std::min<int64_t>(32768, h.count - a);
+      add_binary(m, rows.data() + (size_t)a * nb, ids.data() + a, false);
+    }
+  } catch (...) { fclose(f); throw; }
+  fclose(f);
+}
+
+// ============================================================================================
+// Binary Flat: IndexBinaryFlat under IndexBinaryIDMap2 (vector_index_flat.cc:99-102, :121-264), with the float Flat's
+// policies: append, tombstone, compaction at half dead.
+// ============================================================================================
+struct BinaryFlatIndex : BinaryIndex {
+  BinRows store{this};
+  int64_t rows = 0;
+  std::vector<int64_t> h_ids;
+  std::unordered_map<int64_t, int64_t> id2row;
+  int64_t ndeleted = 0;
+
+  BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {}
+  void train_binary(int64_t, const uint8_t*) override {}  // a Flat index needs no training (flat.cc Train returns OK)
+
+  void tombstone(const std::vector<int64_t>& rws) {
+    store.tombstone(rws);
+    for (int64_t r : rws) h_ids[r] = -1;
+    ndeleted += (int64_t)rws.size();
+  }
+  void compact_if_needed() {
+    if (ndeleted == 0 || ndeleted * 2 < rows) return;
+    std::vector<long long> src, dst;
+    for (int64_t r = 0; r < rows; ++r) if (h_ids[r] >= 0) src.push_back(r);
+    const int64_t live = (int64_t)src.size();
+    dst.resize(live);
+    for (int64_t i = 0; i < live; ++i) dst[i] = i;
+    store.gather(src, dst, std::max<int64_t>(1024, live * 5 / 4));
+    std::vector<int64_t> nh(live);
+    id2row.clear();
+    for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
+    h_ids.swap(nh);
+    rows = live; ndeleted = 0;
+  }
+  // AddOrUpsert (flat.cc:121-162): duplicate ids in the batch are refused, existing ids are always removed first
+  void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool) override {
+    check_batch_ids_unique(n, in_ids);
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    std::vector<int64_t> dead;
+    for (int64_t i = 0; i < n; ++i) {
+      auto it = id2row.find(in_ids[i]);
+      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
+    }
+    tombstone(dead);
+    const int64_t cap = (int64_t)store.ids.cap;
+    if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
+    const uint32_t* st = upload(n, x);
+    long long* st_ids = scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
+    std::vector<long long> slots(n);
+    for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
+    store.write(st, st_ids, slots);
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    h_ids.resize(rows + n);
+    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = in_ids[i]; id2row[in_ids[i]] = rows + i; }
+    rows += n;
+    compact_if_needed();
+  }
+  // Delete (flat.cc:171-203): ids that are not present are ignored
+  int64_t remove(int64_t n, const int64_t* del) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    std::vector<int64_t> dead;
+    for (int64_t i = 0; i < n; ++i) {
+      auto it = id2row.find(del[i]);
+      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
+    }
+    tombstone(dead);
+    compact_if_needed();
+    return (int64_t)dead.size();
+  }
+  ScanJob job(const SearchCtx& sc) const {
+    ScanJob j = hamming_job(store.words.p, store.ids.p, rows);
+    j.sc = &sc;
+    return j;
+  }
+  void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+    ScanJob j = job(sc);
+    j.dominant = true;
+    run_scan(this, j, nq, reinterpret_cast<const float*>(pad(nq, xq, s)), k, od, nullptr, oi, nullptr, s);
+  }
+  void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc, float* od,
+                               long long* oi, int* oc, cudaStream_t s) override {
+    ScanJob j = job(sc);
+    j.has_thr = true;
+    j.thr_raw = radius_threshold(radius);
+    run_scan(this, j, nq, reinterpret_cast<const float*>(pad(nq, xq, s)), max_results, od, nullptr, oi, oc, s);
+  }
+  int64_t count() const override { return rows - ndeleted; }
+  int64_t deleted_count() const override { return ndeleted; }
+  int64_t memory_size() const override { return store.bytes(); }
+  void export_lists(int64_t* list_off, float* vectors, uint8_t* codes, int64_t* out_ids) override {
+    if (vectors) fail(B200VS_EILLEGAL_PARAMETERS, "binary indexes export packed rows through codes; vectors must be NULL");
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    if (list_off) { list_off[0] = 0; list_off[1] = rows - ndeleted; }
+    std::vector<uint8_t> all;
+    if (codes && rows) { all.resize((size_t)rows * nb); store.download(0, rows, all.data()); }
+    int64_t o = 0;
+    for (int64_t r = 0; r < rows; ++r) {
+      if (h_ids[r] < 0) continue;
+      if (out_ids) out_ids[o] = h_ids[r];
+      if (codes) memcpy(codes + (size_t)o * nb, all.data() + (size_t)r * nb, nb);
+      ++o;
+    }
+  }
+};
+
+IndexBase* make_binary_flat(int d, const b200vs_params& p) { return new BinaryFlatIndex(d, p); }
+
+// ============================================================================================
+// Binary IVF-Flat: IndexBinaryIVF with an IndexBinaryFlat quantiser (vector_index_ivf_flat.cc:62).  Lists live in the
+// IvfLists arena with the float IVF-Flat's relocation and compaction policy; rows move as words.
+// ============================================================================================
+struct BinaryIvfIndex : BinaryIndex {
+  int nlist;  // degenerates to 1 at train time with fewer rows than nlist (ivf_flat.cc:578-641)
+  bool trained = false;
+  DevBuf<uint32_t> cent;       // [nlist, w] padded binary centroids
+  DevBuf<long long> cent_ids;  // iota: the list ids the coarse pass returns
+  BinRows store{this};
+  IvfLists L;
+
+  BinaryIvfIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_IVF_FLAT, d, p) {
+    nlist = p.nlist > 0 ? p.nlist : 2048;  // Constant::kCreateBinaryIvfFlatParamNcentroids (constant.h:180)
+  }
+  bool is_trained() const override { return trained; }
+  int export_nlist() const override { return nlist; }
+  int nlist_now() const override { return nlist; }
+
+  // packed centroids [k, dim / 8] (host)
+  void install_centroids(const uint8_t* host_c, int k) {
+    quiesce();
+    nlist = k;
+    scratch.reset(stream);
+    const uint32_t* st = upload(k, host_c);
+    cent.free(); cent_ids.free();
+    cent.reserve((size_t)k * w, 0, stream);
+    cent_ids.reserve(k, 0, stream);
+    B200VS_CUDA(cudaMemcpyAsync(cent.p, st, (size_t)k * w * 4, cudaMemcpyDeviceToDevice, stream));
+    launch_iota(cent_ids.p, k, stream);
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    L.init(k, stream);
+    store.reset();
+    trained = true;
+  }
+
+  // trained-state blob: int64 hdr[4] = {magic 'IVFB', nlist, dim, metric}; uint8 centroids[nlist * dim / 8]
+  void set_state(const void* blob, size_t len) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    if (len < 32) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
+    const int64_t* hdr = (const int64_t*)blob;
+    if (hdr[0] != 0x42465649 || hdr[2] != dim || hdr[3] != B200VS_HAMMING) fail(B200VS_EILLEGAL_PARAMETERS, "bad binary IVF state blob");
+    if (hdr[1] <= 0 || hdr[1] > (1 << 24)) fail(B200VS_EILLEGAL_PARAMETERS, "bad list count in state blob");
+    const int k = (int)hdr[1];
+    if (len < 32 + (size_t)k * nb) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
+    install_centroids((const uint8_t*)blob + 32, k);
+  }
+  int64_t get_state(void* blob, size_t cap) override {
+    RwSharedGuard rl(this);
+    if (!trained) return 0;
+    const size_t need = 32 + (size_t)nlist * nb;
+    if (!blob || cap < need) return (int64_t)need;
+    set_device();
+    int64_t hdr[4] = {0x42465649, nlist, dim, (int64_t)metric};
+    memcpy(blob, hdr, 32);
+    std::vector<uint32_t> tmp((size_t)nlist * w);
+    B200VS_CUDA(cudaMemcpy(tmp.data(), cent.p, tmp.size() * 4, cudaMemcpyDeviceToHost));
+    for (int c = 0; c < nlist; ++c) memcpy((uint8_t*)blob + 32 + (size_t)c * nb, tmp.data() + (size_t)c * w, nb);
+    return (int64_t)need;
+  }
+
+  // IndexBinaryIVF::train: binary_to_real (bit i = byte i >> 3, bit i & 7, LSB first -> 2b - 1), faiss::Clustering with L2
+  // on the +-1 rows (kmeans_gpu: same subsample permutation, seed, iterations and split_clusters as IVF-Flat), and
+  // real_to_binary (bit set where the coordinate is > 0).  Only the training subsample is expanded to floats: the rows
+  // kmeans_gpu would draw, in its order, so it sees exactly what it would see on the whole expanded set.
+  void train_binary(int64_t n, const uint8_t* x) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    if (trained) return;  // ivf_flat.cc:670-672
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    const int k = n < nlist ? 1 : nlist;  // "data size too small, nlist degenerate to 1"
+    const int max_pts = 256, niter = 10;
+    const int64_t seed = 1234;
+    std::vector<int64_t> pick;
+    int64_t m = n;
+    if (n > (int64_t)k * max_pts) { kmeans_rand_perm(pick, n, seed); m = (int64_t)k * max_pts; }
+    // kmeans_gpu holds the +-1 sample on the device: refuse a sample that cannot fit there before it is built on the host
+    // (dim 32768 with nlist 2048 is 68 GB); EINTERNAL like any device allocation failure, and the index stays untrained
+    size_t free_b = 0, total_b = 0;
+    B200VS_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const double sample_b = (double)m * dim * 4;
+    if (sample_b > (double)free_b)
+      fail(B200VS_EINTERNAL, "binary training sample of " + std::to_string((long long)(sample_b / 1e6)) + " MB (+-1 floats) does not fit in " +
+                                 std::to_string((long long)(free_b / 1000000)) + " MB of free device memory");
+    std::vector<float> pm1((size_t)m * dim);  // bad_alloc -> EINTERNAL, index stays untrained
+    for (int64_t i = 0; i < m; ++i) {
+      const uint8_t* row = x + (size_t)(pick.empty() ? i : pick[i]) * nb;
+      float* o = pm1.data() + (size_t)i * dim;
+      for (int b = 0; b < dim; ++b) o[b] = ((row[b >> 3] >> (b & 7)) & 1) ? 1.0f : -1.0f;
+    }
+    DevBuf<long long> iota;
+    std::vector<float> c;
+    // if the device fills up in between, kmeans_gpu's DevBuf::reserve fails the same way (CudaError -> EINTERNAL)
+    kmeans_gpu(this, B200VS_L2, dim, m, pm1.data(), k, niter, max_pts, seed, c, [&](const float* xd, int64_t mm, const float* cd, int kk, long long* out) {
+      ScanJob j;
+      j.vecs = cd; j.ids = iota.p; j.d = dim; j.mode = 0; j.n = kk;
+      const int64_t chunk = 32768;
+      for (int64_t a = 0; a < mm; a += chunk) {
+        const auto mark = scratch.mark();
+        run_scan(this, j, std::min(chunk, mm - a), xd + (size_t)a * dim, 1, nullptr, nullptr, out + a, nullptr, stream);
+        scratch.release(mark);
+      }
+    }, [&](int kk) { iota.reserve(kk, 0, stream); launch_iota(iota.p, kk, stream); });
+    std::vector<uint8_t> bin((size_t)k * nb, 0);
+    for (int ci = 0; ci < k; ++ci)
+      for (int b = 0; b < dim; ++b)
+        if (c[(size_t)ci * dim + b] > 0.0f) bin[(size_t)ci * nb + (b >> 3)] |= (uint8_t)(1u << (b & 7));
+    install_centroids(bin.data(), k);
+  }
+
+  int resolve_nprobe(const SearchCtx& sc) const {
+    const int np = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchBinaryIvfFlatParamNprobe (constant.h:181), ivf_flat.cc:207-209
+    return std::min(np, nlist);                    // ivf_flat.cc:234
+  }
+  // IndexBinaryFlat quantiser: the nprobe nearest lists by (Hamming distance, list id)
+  long long* coarse(int64_t nq, const uint32_t* q, int nprobe, cudaStream_t s, long long* out = nullptr) {
+    long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
+    run_scan(this, hamming_job(cent.p, cent_ids.p, nlist), nq, reinterpret_cast<const float*>(q), nprobe, nullptr, nullptr, probes, nullptr, s);
+    return probes;
+  }
+  ScanJob list_job(const SearchCtx& sc, const long long* probes, int nprobe) const {
+    ScanJob j = hamming_job(store.words.p, store.ids.p, 0);
+    j.mode = 1; j.probes = probes; j.nprobe = nprobe; j.list_off = L.d_off.p; j.list_len = L.d_len.p; j.sc = &sc;
+    j.avg_candidates = nlist > 0 ? (double)L.total_len() * nprobe / nlist : 0;
+    return j;
+  }
+
+  void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool upsert) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");  // ivf_flat.cc:111-113
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    if (upsert) remove_locked(n, in_ids);  // ivf_flat.cc:115-118
+    const uint32_t* st = upload(n, x);
+    long long* st_ids = scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
+    // nearest centroid, ties to the smaller list id (the coarse pass with nprobe = 1)
+    long long* lists = scratch.alloc<long long>(n);
+    for (int64_t a = 0; a < n; a += 32768) {
+      const auto mark = scratch.mark();  // each chunk's select workspace is handed back before the next
+      coarse(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, stream, lists + a);
+      scratch.release(mark);
+    }
+    std::vector<long long> h_list(n), slots(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    std::vector<int> need(nlist, 0);
+    for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
+    L.reserve_for(need, [&](int64_t arena_rows) { store.grow(arena_rows, L.arena_used_before); },
+                  [&](int64_t src, int64_t dst, int64_t len) { store.move(src, dst, len); });
+    for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], in_ids[i]);
+    store.write(st, st_ids, slots);
+    L.upload(stream);
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+  }
+  int64_t remove_locked(int64_t n, const int64_t* del) {
+    std::vector<int64_t> rws;
+    L.remove_ids(n, del, rws);
+    store.tombstone(rws);
+    return (int64_t)rws.size();
+  }
+  // Delete (ivf_flat.cc:162-189): untrained -> OK; nothing removed -> EVECTOR_INVALID (api.cu)
+  int64_t remove(int64_t n, const int64_t* del) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    if (!trained) return -1;
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    const int64_t r = remove_locked(n, del);
+    if (L.needs_compaction()) {
+      std::vector<long long> src, dst;
+      const int64_t new_rows = L.plan_compaction(src, dst);
+      store.gather(src, dst, std::max<int64_t>(new_rows, 1));
+      L.commit_compaction();
+      L.upload(stream);
+    }
+    return r;
+  }
+
+  void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+    if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_flat.cc:224-227
+    const uint32_t* q = pad(nq, xq, s);
+    const int nprobe = resolve_nprobe(sc);
+    long long* probes = coarse(nq, q, nprobe, s);
+    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+    ScanJob j = list_job(sc, probes, nprobe);
+    j.dominant = true;
+    run_scan(this, j, nq, reinterpret_cast<const float*>(q), k, od, nullptr, oi, nullptr, s);
+  }
+  void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc, float* od,
+                               long long* oi, int* oc, cudaStream_t s) override {
+    if (!trained) {
+      fill_empty_results(nq, max_results, od, oi, s);
+      B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
+      return;
+    }
+    const float thr = radius_threshold(radius);
+    const uint32_t* q = pad(nq, xq, s);
+    const int nprobe = resolve_nprobe(sc);
+    long long* probes = coarse(nq, q, nprobe, s);
+    ScanJob j = list_job(sc, probes, nprobe);  // ivf_flat.cc:342-345
+    j.has_thr = true;
+    j.thr_raw = thr;
+    run_scan(this, j, nq, reinterpret_cast<const float*>(q), max_results, od, nullptr, oi, oc, s);
+  }
+
+  int64_t count() const override { return L.live; }
+  int64_t deleted_count() const override { return L.dead; }
+  int64_t memory_size() const override { return store.bytes() + (int64_t)cent.cap * 4; }
+  void export_lists(int64_t* list_off, float* vectors, uint8_t* codes, int64_t* out_ids) override {
+    if (vectors) fail(B200VS_EILLEGAL_PARAMETERS, "binary indexes export packed rows through codes; vectors must be NULL");
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    int64_t o = 0;
+    std::vector<uint8_t> buf;
+    for (int l = 0; l < nlist; ++l) {
+      if (list_off) list_off[l] = o;
+      if (!trained) continue;
+      const ListMeta& m = L.lists[l];
+      if (codes && m.len) { buf.resize((size_t)m.len * nb); store.download(m.off, m.len, buf.data()); }
+      for (int p = 0; p < m.len; ++p) {
+        const int64_t id = L.h_ids[m.off + p];
+        if (id < 0) continue;
+        if (out_ids) out_ids[o] = id;
+        if (codes) memcpy(codes + (size_t)o * nb, buf.data() + (size_t)p * nb, nb);
+        ++o;
+      }
+    }
+    if (list_off) list_off[nlist] = o;
+  }
+};
+
+IndexBase* make_binary_ivf(int d, const b200vs_params& p) { return new BinaryIvfIndex(d, p); }
+
+}  // namespace b200vs

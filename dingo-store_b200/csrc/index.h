@@ -279,6 +279,25 @@ struct IndexBase {
     fail(B200VS_EILLEGAL_PARAMETERS, "tensor-core score diagnostics only exist for FLAT");
   }
 
+  // ---- binary indexes (B200VS_BINARY_FLAT / B200VS_BINARY_IVF_FLAT, binary.cu): rows are packed bits, dim / 8 bytes each.
+  // A float index refuses these, and the float entry points refuse a binary index (b200vs_*_binary, api.cu).
+  bool binary() const { return type == B200VS_BINARY_FLAT || type == B200VS_BINARY_IVF_FLAT; }
+  virtual void train_binary(int64_t n, const uint8_t* x) { (void)n; (void)x; fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index"); }
+  virtual void add_binary(int64_t n, const uint8_t* x, const int64_t* ids, bool upsert) {
+    (void)n; (void)x; (void)ids; (void)upsert;
+    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
+  }
+  // xq: device rows [nq, dim / 8]; distances are Hamming distances
+  virtual void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
+    (void)nq; (void)xq; (void)k; (void)sc; (void)out_dist; (void)out_ids; (void)s;
+    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
+  }
+  virtual void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc,
+                                       float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
+    (void)nq; (void)xq; (void)radius; (void)max_results; (void)sc; (void)out_dist; (void)out_ids; (void)out_counts; (void)s;
+    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
+  }
+
   virtual void reconstruct(int64_t n, const int64_t* ids, float* out, uint8_t* found) {
     (void)n; (void)ids; (void)out; (void)found;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "reconstruct is implemented for HNSW and FLAT");
@@ -341,10 +360,13 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_pq(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p);
+IndexBase* make_binary_flat(int d, const b200vs_params& p);
+IndexBase* make_binary_ivf(int d, const b200vs_params& p);
 
 // ---- generic exact scan + select driver (scan_kernels.cuh) ----
 struct ScanJob {
   bool l2 = true;
+  bool hamming = false;  // binary rows: vecs / queries hold 32-bit words, d = words per row; l2 stays true (ascending)
   const float* vecs = nullptr;
   const long long* ids = nullptr;
   int d = 0;

@@ -169,6 +169,14 @@ struct IvfLists {
 void launch_kmeans_accumulate(const float* x, const long long* assign, int64_t n, int d, double scale, long long* sums,
                               int* counts, cudaStream_t s);
 
+// the first rows of this permutation of [0, m) are k-means' training subsample (seed) and initial centroids (seed + 1)
+inline void kmeans_rand_perm(std::vector<int64_t>& perm, int64_t m, int64_t sd) {
+  perm.resize(m);
+  for (int64_t i = 0; i < m; ++i) perm[i] = i;
+  std::mt19937 mt((unsigned)sd);
+  for (int64_t i = 0; i + 1 < m; ++i) { int64_t i2 = i + (int64_t)(mt() % (unsigned long)(m - i)); std::swap(perm[i], perm[i2]); }
+}
+
 // faiss::Clustering-shaped Lloyd k-means with the assignment step on the GPU (public algorithm; the
 // reference reaches it through index_->train at vector_index_ivf_flat.cc:695 / raw_ivf_pq.cc:485).
 // x_host RAW rows; cosine rows are normalised on the device first.  `assign(xd, m, cd, k, out)` labels m device
@@ -177,18 +185,12 @@ template <class AssignFn, class PrepFn>
 void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const float* x_host, int k, int niter,
                 int max_pts, int64_t seed, std::vector<float>& cent, AssignFn assign, PrepFn prepare_ids) {
   cudaStream_t s = ix->stream;
-  auto rand_perm = [](std::vector<int64_t>& perm, int64_t m, int64_t sd) {
-    perm.resize(m);
-    for (int64_t i = 0; i < m; ++i) perm[i] = i;
-    std::mt19937 mt((unsigned)sd);
-    for (int64_t i = 0; i + 1 < m; ++i) { int64_t i2 = i + (int64_t)(mt() % (unsigned long)(m - i)); std::swap(perm[i], perm[i2]); }
-  };
   std::vector<float> sub;
   const float* xs = x_host;
   int64_t m = n;
   if (n > (int64_t)k * max_pts) {
     std::vector<int64_t> perm;
-    rand_perm(perm, n, seed);
+    kmeans_rand_perm(perm, n, seed);
     m = (int64_t)k * max_pts;
     sub.resize((size_t)m * d);
     for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * d], x_host + (size_t)perm[i] * d, (size_t)d * 4);
@@ -213,7 +215,7 @@ void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const flo
   if (m == k) { memcpy(cent.data(), init_src, (size_t)m * d * 4); return; }
   {
     std::vector<int64_t> perm;
-    rand_perm(perm, m, seed + 1);
+    kmeans_rand_perm(perm, m, seed + 1);
     for (int i = 0; i < k; ++i) memcpy(&cent[(size_t)i * d], init_src + (size_t)perm[i] * d, (size_t)d * 4);
   }
   // fixed-point scale: a sum of m rows of magnitude <= amax stays below 2^62

@@ -73,15 +73,21 @@ static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const f
   const unsigned slots = qcount ? (unsigned)std::min<int64_t>(nq, std::max(1, 592 / nsplit)) : (unsigned)nq;
   dim3 grid(nsplit, slots);
   ScopedKernelTimer timer(ix, s, ix->profiling && job.dominant);
-  if (job.l2) {
-    ensure_smem(scan_select_kernel<true>, smem1);
-    scan_select_kernel<true><<<grid, SCAN_THREADS, smem1, s>>>(a);
+  if (job.hamming) {
+    ensure_smem(scan_select_kernel<HammingDist>, smem1);
+    scan_select_kernel<HammingDist><<<grid, SCAN_THREADS, smem1, s>>>(a);
+    timer.stop();
+    ensure_smem(merge_select_kernel<true>, smem2);
+    merge_select_kernel<true><<<slots, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, nsplit, k, cap, out_dist, out_raw, out_ids, out_counts, qmap, qcount);
+  } else if (job.l2) {
+    ensure_smem(scan_select_kernel<Fp32Dist<true>>, smem1);
+    scan_select_kernel<Fp32Dist<true>><<<grid, SCAN_THREADS, smem1, s>>>(a);
     timer.stop();
     ensure_smem(merge_select_kernel<true>, smem2);
     merge_select_kernel<true><<<slots, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, nsplit, k, cap, out_dist, out_raw, out_ids, out_counts, qmap, qcount);
   } else {
-    ensure_smem(scan_select_kernel<false>, smem1);
-    scan_select_kernel<false><<<grid, SCAN_THREADS, smem1, s>>>(a);
+    ensure_smem(scan_select_kernel<Fp32Dist<false>>, smem1);
+    scan_select_kernel<Fp32Dist<false>><<<grid, SCAN_THREADS, smem1, s>>>(a);
     timer.stop();
     ensure_smem(merge_select_kernel<false>, smem2);
     merge_select_kernel<false><<<slots, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, nsplit, k, cap, out_dist, out_raw, out_ids, out_counts, qmap, qcount);

@@ -45,7 +45,38 @@ inline size_t scan_smem_bytes(int d, int nprobe, int pool_cap) {
   return q + pf + BlockSelect::smem_bytes(pool_cap);
 }
 
+// Per-row distance of the exact scan.  Fp32Dist: the reference's FP32 order (quad_distance); d = floats per row.
 template <bool L2>
+struct Fp32Dist {
+  static constexpr bool kL2 = L2;
+  static __device__ __forceinline__ float eval(const float* vecs, long long row, const float* qs, int d, int t, bool vec) {
+    return quad_distance<L2>(vecs + (size_t)row * d, qs, d, t, vec);
+  }
+};
+// HammingDist: binary rows, d = 32-bit words per (zero-padded) row, vecs / qs hold the words.  sum popc(q ^ x) over the
+// row in int, returned as float: exact (<= 32768 bits), so the key f2ord(dist) orders rows like the integer distance.
+// Thread t of the quad takes words 4t..4t+3 of every 16-word chunk (vec: 16-byte loads) or words t, t+4, ...
+struct HammingDist {
+  static constexpr bool kL2 = true;
+  static __device__ __forceinline__ float eval(const float* vecs, long long row, const float* qs, int d, int t, bool vec) {
+    const uint32_t* x = reinterpret_cast<const uint32_t*>(vecs) + (size_t)row * d;
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(qs);
+    int s = 0;
+    if (vec) {
+      for (int i = 4 * t; i < d; i += 16) {
+        const uint4 a = *reinterpret_cast<const uint4*>(x + i), b = *reinterpret_cast<const uint4*>(q + i);
+        s += __popc(a.x ^ b.x) + __popc(a.y ^ b.y) + __popc(a.z ^ b.z) + __popc(a.w ^ b.w);
+      }
+    } else {
+      for (int i = t; i < d; i += 4) s += __popc(x[i] ^ q[i]);
+    }
+    s += __shfl_xor_sync(0xffffffffu, s, 1, 4);
+    s += __shfl_xor_sync(0xffffffffu, s, 2, 4);
+    return (float)s;
+  }
+};
+
+template <class Dist>
 static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsigned char* smem, const int slot, const int split, const int qi) {
   const int d = a.d;
   float* qs = reinterpret_cast<float*>(smem);
@@ -110,9 +141,9 @@ static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsig
       }
       if (__ballot_sync(0xffffffffu, valid) == 0u) continue;  // warp-uniform skip
       if (!valid) row = safe_row;
-      const float v = quad_distance<L2>(a.vecs + (size_t)row * d, qs, d, t, vec);
+      const float v = Dist::eval(a.vecs, row, qs, d, t, vec);
       if (valid && t == 0) {
-        const uint32_t key = f2ord(L2 ? v : -v);
+        const uint32_t key = f2ord(Dist::kL2 ? v : -v);
         if (sel.passes(key, id)) sel.push(key, id);
       }
     }
@@ -129,13 +160,13 @@ static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsig
 
 // Plain launch: grid (nsplit, nq).  Mapped launch (a.qcount != NULL, the re-run of uncertified queries): a small grid in y
 // strides over the *a.qcount live slots, so the usual "nothing to redo" case costs a handful of empty CTAs.
-template <bool L2>
+template <class Dist>
 static __global__ void __launch_bounds__(SCAN_THREADS) scan_select_kernel(const ScanArgs a) {
   extern __shared__ __align__(16) unsigned char smem[];
-  if (!a.qcount) { scan_select_body<L2>(a, smem, blockIdx.y, blockIdx.x, blockIdx.y); return; }
+  if (!a.qcount) { scan_select_body<Dist>(a, smem, blockIdx.y, blockIdx.x, blockIdx.y); return; }
   const int n = *a.qcount;
   for (int slot = blockIdx.y; slot < n; slot += gridDim.y) {
-    scan_select_body<L2>(a, smem, slot, blockIdx.x, a.qmap[slot]);
+    scan_select_body<Dist>(a, smem, slot, blockIdx.x, a.qmap[slot]);
     __syncthreads();
   }
 }

@@ -13,8 +13,9 @@ PKG_ROOT = os.path.abspath(os.path.join(_HERE, "..", ".."))       # dingo-store_
 REPO_ROOT = os.path.abspath(os.path.join(PKG_ROOT, ".."))
 LIB_PATH = os.path.join(PKG_ROOT, "libb200vs.so")
 
-FLAT, IVF_FLAT, IVF_PQ, HNSW = 0, 1, 2, 3
-L2, IP, COSINE = 1, 2, 3
+FLAT, IVF_FLAT, IVF_PQ, HNSW, BINARY_FLAT, BINARY_IVF_FLAT = 0, 1, 2, 3, 4, 5
+L2, IP, COSINE, HAMMING = 1, 2, 3, 4
+BINARY_TYPES = (BINARY_FLAT, BINARY_IVF_FLAT)
 OK, EILLEGAL_PARAMETERS, EVECTOR_INVALID, EVECTOR_NOT_TRAIN, EVECTOR_NOT_SUPPORT, EINTERNAL, EVECTOR_ID_DUPLICATED = range(7)
 
 # every symbol include/b200vs.h declares (checked by tests/test_abi.py without a GPU)
@@ -29,6 +30,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_unique_id", "b200vs_shard_create", "b200vs_shard_destroy", "b200vs_shard_list_range", "b200vs_shard_train",
     "b200vs_shard_broadcast_state", "b200vs_shard_add", "b200vs_shard_add_device", "b200vs_shard_remove_ids", "b200vs_shard_plan_add_device",
     "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
+    "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
 ]
 
 
@@ -121,6 +123,11 @@ def lib():
     L.b200vs_shard_search.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_shard_search_device.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_debug_tc_scores.argtypes = [vp, i64, vp, i32, vp, vp]
+    L.b200vs_train_binary.argtypes = [vp, i64, vp]
+    L.b200vs_add_with_ids_binary.argtypes = [vp, i64, vp, vp, ctypes.c_int]
+    L.b200vs_search_binary.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_search_binary_device.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_range_search_binary.argtypes = [vp, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     _lib = L
     return L
 
@@ -139,6 +146,10 @@ def _i64(a):
     return np.ascontiguousarray(a, dtype=np.int64)
 
 
+def _u8(a):
+    return np.ascontiguousarray(a, dtype=np.uint8)
+
+
 def make_search_params(nprobe=0, efsearch=0, id_range=None, sorted_ids=None, negate=False, exact_only=False):
     sp = SearchParams()
     sp.nprobe, sp.efsearch, sp.exact_only = int(nprobe), int(efsearch), int(bool(exact_only))
@@ -155,7 +166,9 @@ def make_search_params(nprobe=0, efsearch=0, id_range=None, sorted_ids=None, neg
 
 class Index:
     """Thin owner of a b200vs_index handle.  Method names follow the reference plugin virtuals
-    (src/vector/vector_index.h:148-202): train / add / upsert / delete / search / range_search / get_count ..."""
+    (src/vector/vector_index.h:148-202): train / add / upsert / delete / search / range_search / get_count ...
+    Binary types (BINARY_FLAT / BINARY_IVF_FLAT, metric HAMMING): dim counts bits, and train / add / search /
+    range_search / search_device take packed uint8 rows [n, dim / 8] and call the b200vs_*_binary entry points."""
 
     def __init__(self, index_type, metric, dim, nlist=0, pq_m=0, pq_nbits=0, hnsw_m=0, hnsw_efc=0, max_elements=0,
                  device=0, hnsw_build_threads=0):
@@ -178,8 +191,24 @@ class Index:
         except Exception:
             pass
 
+    @property
+    def binary(self):
+        return self.type in BINARY_TYPES
+
+    def _rows(self, x):
+        """(array, rows) of x in the index's row type: float32 [n, dim], or packed uint8 [n, dim / 8] for binary types."""
+        if self.binary:
+            x = _u8(x)
+            return x, (x.shape[0] if x.ndim == 2 else x.size // max(self.dim // 8, 1))
+        x = _f32(x)
+        return x, (x.shape[0] if x.ndim == 2 else x.size // self.dim)
+
     # ---- write path ----
     def train(self, x):
+        if self.binary:
+            x, n = self._rows(x)
+            _check(self.L.b200vs_train_binary(self.h, n, x.ctypes.data if x.size else None))
+            return
         x = _f32(x)
         n = x.shape[0] if x.ndim == 2 else x.size // self.dim
         _check(self.L.b200vs_train(self.h, n, x.ctypes.data))
@@ -199,6 +228,10 @@ class Index:
         return buf[:got]
 
     def add(self, x, ids, upsert=False):
+        if self.binary:
+            x, ids = _u8(x), _i64(ids)
+            _check(self.L.b200vs_add_with_ids_binary(self.h, ids.size, x.ctypes.data if x.size else None, ids.ctypes.data if ids.size else None, int(upsert)))
+            return
         x, ids = _f32(x), _i64(ids)
         _check(self.L.b200vs_add_with_ids(self.h, ids.size, x.ctypes.data if x.size else None, ids.ctypes.data if ids.size else None, int(upsert)))
 
@@ -223,20 +256,22 @@ class Index:
 
     # ---- read path ----
     def search(self, xq, k, **kw):
-        xq = _f32(xq)
-        nq = xq.shape[0] if xq.ndim == 2 else xq.size // self.dim
+        xq, nq = self._rows(xq)
         sp, keep = make_search_params(**kw)
         D = np.zeros((nq, max(k, 0)), dtype=np.float32)
         I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
-        _check(self.L.b200vs_search(self.h, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data, I.ctypes.data))
+        fn = self.L.b200vs_search_binary if self.binary else self.L.b200vs_search
+        _check(fn(self.h, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data, I.ctypes.data))
         return D, I
 
     def search_raw(self, nq, xq_ptr, k, out_dist_ptr, out_ids_ptr, sp=None):
         """Host-pointer call with caller-owned (e.g. pinned) buffers — the e2e benchmark leg."""
-        _check(self.L.b200vs_search(self.h, nq, xq_ptr, k, ctypes.byref(sp) if sp is not None else None, out_dist_ptr, out_ids_ptr))
+        fn = self.L.b200vs_search_binary if self.binary else self.L.b200vs_search
+        _check(fn(self.h, nq, xq_ptr, k, ctypes.byref(sp) if sp is not None else None, out_dist_ptr, out_ids_ptr))
 
     def search_device(self, nq, xq_dev_ptr, k, out_dist_dev_ptr, out_ids_dev_ptr, stream=None, sp=None):
-        _check(self.L.b200vs_search_device(self.h, nq, xq_dev_ptr, k, ctypes.byref(sp) if sp is not None else None,
+        fn = self.L.b200vs_search_binary_device if self.binary else self.L.b200vs_search_device
+        _check(fn(self.h, nq, xq_dev_ptr, k, ctypes.byref(sp) if sp is not None else None,
                                            out_dist_dev_ptr, out_ids_dev_ptr, stream))
 
     def coarse_device(self, nq, xq_dev_ptr, nprobe, list_begin, list_end, out_score_dev_ptr, out_lists_dev_ptr, stream=None):
@@ -247,13 +282,13 @@ class Index:
                                                   out_dist_dev_ptr, out_ids_dev_ptr, stream))
 
     def range_search(self, xq, radius, max_results=1024, **kw):
-        xq = _f32(xq)
-        nq = xq.shape[0] if xq.ndim == 2 else xq.size // self.dim
+        xq, nq = self._rows(xq)
         sp, keep = make_search_params(**kw)
         D = np.zeros((nq, max_results), dtype=np.float32)
         I = np.full((nq, max_results), -1, dtype=np.int64)
         C = np.zeros(nq, dtype=np.int32)
-        _check(self.L.b200vs_range_search(self.h, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
+        fn = self.L.b200vs_range_search_binary if self.binary else self.L.b200vs_range_search
+        _check(fn(self.h, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
                                           ctypes.byref(sp), D.ctypes.data, I.ctypes.data, C.ctypes.data))
         return D, I, C
 
@@ -306,6 +341,9 @@ class Index:
         return S, E
 
     def export_lists(self, nlist, with_vectors=True, code_size=0):
+        """(list_off, vectors, codes, ids).  Binary types: codes = the packed rows [n, dim / 8], vectors = None."""
+        if self.binary:
+            with_vectors, code_size = False, self.dim // 8
         n = self.get_count()
         off = np.zeros(nlist + 1, dtype=np.int64)
         vec = np.zeros((n, self.dim), dtype=np.float32) if with_vectors else None
@@ -430,6 +468,13 @@ def ivf_state_blob(centroids, metric):
     c = _f32(centroids)
     hdr = np.array([0x43465649, c.shape[0], c.shape[1], metric], dtype=np.int64)
     return np.concatenate([hdr.view(np.uint8), c.reshape(-1).view(np.uint8)])
+
+
+def binary_ivf_state_blob(centroids):
+    """Trained-state blob of a binary IVF-Flat index: packed centroids [nlist, dim / 8] (DESIGN.md §Trained-state blobs)."""
+    c = _u8(centroids)
+    hdr = np.array([0x42465649, c.shape[0], c.shape[1] * 8, HAMMING], dtype=np.int64)
+    return np.concatenate([hdr.view(np.uint8), c.reshape(-1)])
 
 
 def merge_topk_device(device, nparts, nq, k, parts_dist_ptr, parts_ids_ptr, out_dist_ptr, out_ids_ptr, stream=None):

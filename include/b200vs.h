@@ -33,9 +33,16 @@ extern "C" {
 typedef struct b200vs_index b200vs_index; /* opaque */
 
 /* replaces VectorIndexFactory::New type switch, src/vector/vector_index_factory.cc:40-95 */
-typedef enum { B200VS_FLAT = 0, B200VS_IVF_FLAT = 1, B200VS_IVF_PQ = 2, B200VS_HNSW = 3 } b200vs_type;
-/* mirrors pb::common::MetricType L2 / INNER_PRODUCT / COSINE */
-typedef enum { B200VS_L2 = 1, B200VS_IP = 2, B200VS_COSINE = 3 } b200vs_metric;
+typedef enum {
+  B200VS_FLAT = 0, B200VS_IVF_FLAT = 1, B200VS_IVF_PQ = 2, B200VS_HNSW = 3,
+  /* VECTOR_INDEX_TYPE_BINARY_FLAT / _BINARY_IVF_FLAT (vector_index_factory.cc:73-80): faiss IndexBinaryFlat under
+   * IndexBinaryIDMap2 and IndexBinaryIVF.  dim counts BITS (dim % 8 == 0, 0 < dim <= 32768); rows are packed, dim / 8 bytes
+   * each, byte j = binary_values[j] (vector_index_utils.cc:597-599); metric must be B200VS_HAMMING.  They are served by the
+   * b200vs_*_binary entry points; the float ones refuse them (EILLEGAL_PARAMETERS), and vice versa. */
+  B200VS_BINARY_FLAT = 4, B200VS_BINARY_IVF_FLAT = 5
+} b200vs_type;
+/* mirrors pb::common::MetricType L2 / INNER_PRODUCT / COSINE / HAMMING */
+typedef enum { B200VS_L2 = 1, B200VS_IP = 2, B200VS_COSINE = 3, B200VS_HAMMING = 4 } b200vs_metric;
 
 typedef enum {
   B200VS_OK = 0,
@@ -119,6 +126,21 @@ int b200vs_search_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int
 int b200vs_range_search(b200vs_index* idx, int64_t nq, const float* xq, float radius, int32_t max_results,
                         const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
 
+/* Binary indexes (B200VS_BINARY_FLAT / B200VS_BINARY_IVF_FLAT): the same calls on packed rows x / xq [n, dim / 8].
+ * Distances are the faiss int32 Hamming distances, returned as float (exact) and emitted as is, with no 1 - x
+ * (FillSearchResult, vector_index_utils.cc:640-650).  Results are ordered by (distance, id).  train: Flat no-op; IVF trains
+ * faiss IndexBinaryIVF-style (binary_to_real, L2 k-means on the +-1 rows, real_to_binary; nlist degenerates to 1 with fewer
+ * rows than nlist).  range_search: radius is truncated toward zero and hits have distance < (int)radius
+ * (IndexBinary::range_search, flat.cc:304-308).  Search of an untrained IVF index returns empty results. */
+int b200vs_train_binary(b200vs_index* idx, int64_t n, const uint8_t* x);
+int b200vs_add_with_ids_binary(b200vs_index* idx, int64_t n, const uint8_t* x, const int64_t* ids, int upsert);
+int b200vs_search_binary(b200vs_index* idx, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
+                         float* out_dist, int64_t* out_ids);
+int b200vs_search_binary_device(b200vs_index* idx, int64_t nq, const uint8_t* xq_dev, int32_t k, const b200vs_search_params* sp,
+                                float* out_dist_dev, int64_t* out_ids_dev, void* stream);
+int b200vs_range_search_binary(b200vs_index* idx, int64_t nq, const uint8_t* xq, float radius, int32_t max_results,
+                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
+
 /* Stored vectors by id — what VectorIndexHnsw::Search returns per hit when reconstruct = true (hnswlib getDataByLabel,
  * vector_index_hnsw.cc:383-395; cosine indexes never reconstruct, :469-472).  out [n, dim]; found[n] = 1 / 0 (unknown or
  * deleted id: row left untouched).  Implemented for HNSW and FLAT. */
@@ -144,7 +166,8 @@ int b200vs_load(b200vs_index* idx, const char* path);
 /* Export the inverted lists in list-major order (list l owns rows [list_off[l], list_off[l+1])) so a CPU
  * implementation can search the identical index.  Any output pointer may be NULL.  Flat: nlist = 1. */
 int b200vs_export_lists(b200vs_index* idx, int64_t* list_off /*[nlist+1]*/, float* vectors /*[count,dim]*/,
-                        uint8_t* codes /*[count, ceil(pq_m*pq_nbits/8)]*/, int64_t* ids /*[count]*/);
+                        uint8_t* codes /*[count, ceil(pq_m*pq_nbits/8)]; binary: [count, dim/8], vectors must be NULL*/,
+                        int64_t* ids /*[count]*/);
 
 /* One inverted list (live rows only, stored order): writes up to `cap` rows into vectors [cap, dim] / ids [cap] (either may
  * be NULL) and the list's live row count into *count.  Lets a checker rebuild exactly the lists a query probes without
