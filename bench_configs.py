@@ -189,18 +189,28 @@ def cfg3(o, cores, n, nbits=8, M=96):
             "train_seconds": t_train, "add_seconds": t_add, "search_stats": st}
 
 
-def cfg4(o, cores, n, build_threads=64):
-    """HNSW cosine.  The graph is built by the engine with `build_threads` concurrent host writers — what the reference does
-    with its thread pool (vector_index_hnsw.cc:229-243; such a graph is not reproducible run to run) — and the oracle adopts
-    that very graph (oracle_hnsw_import), so both sides search the SAME index, as for the IVF types."""
+def cfg4(o, cores, n, build_threads=64, build="host", build_batch=0):
+    """HNSW cosine.  build = "host": the graph is built by the engine with `build_threads` concurrent host writers — what the
+    reference does with its thread pool (vector_index_hnsw.cc:229-243; such a graph is not reproducible run to run).
+    build = "device": b200vs_hnsw_add_batched with `build_batch` rows per batch (0 = the library default).  Either way the
+    oracle adopts that very graph (oracle_hnsw_import), so both sides search the SAME index, as for the IVF types."""
     d, M, efc, ef, nq, k = 768, 16, 200, 128, 512, 10
     xb = rnd(n, d, 1234)
     labels = np.arange(1, n + 1, dtype=np.int64)
     ix = b200vs.Index(b200vs.HNSW, b200vs.COSINE, d, hnsw_m=M, hnsw_efc=efc, max_elements=n * 2, hnsw_build_threads=build_threads)
+    phases = {}
+    if build == "device":
+        ix.set_profiling(True)  # CUDA events between the phases of every batch; no synchronisation until the call ends
     t0 = time.time()
     for a in range(0, n, 65536):
-        ix.add(xb[a:a + 65536], labels[a:a + 65536])
+        if build == "device":
+            ix.add_batched(xb[a:a + 65536], labels[a:a + 65536], batch=build_batch)
+            for p in ("build_search", "build_select", "build_link"):
+                phases[p] = phases.get(p, 0.0) + ix.phase_times()[p] / 1e3
+        else:
+            ix.add(xb[a:a + 65536], labels[a:a + 65536])
     t_build = time.time() - t0
+    ix.set_profiling(False)
     xq = rnd(nq, d, 4321)
     dev_ms, e2e_ms, st, D, I = time_search(ix, xq, k, steps=5, warmup=2, efsearch=ef)
     h = oracle_lib.OracleHnsw(o, oracle_lib.COSINE, d, n, M, efc)
@@ -230,7 +240,9 @@ def cfg4(o, cores, n, build_threads=64):
                          "peak": peak(), "frac": bytes_batch / max(st[3], 1) / peak()},
             "cpu_baseline": {"qps": nq / cpu_s, "cores": cores, "kind": "port", "sample": f"all {nq} queries, {cores} threads",
                              "reference_shape_16_threads_qps": 64 / cpu16_s},
-            "build_seconds_engine": t_build, "oracle_import_seconds": t_import, "search_stats": st}
+            "build": build, "build_seconds_engine": t_build, "oracle_import_seconds": t_import, "search_stats": st,
+            **({"graph": f"built on the device by b200vs_hnsw_add_batched, batch {build_batch or 'default'}; the oracle searches the same graph",
+                "build_phase_seconds": phases} if build == "device" else {})}
 
 def cfg5(o, cores, rows_per_gpu, steps=10, warmup=3, dim=1536, nlist_per_gpu=2048, nprobe=64, nq=4096, k=10, in_flight=2, verify=256, oracle_q=8):
     """BASELINE config 5: one logical IVF-Flat index list-sharded over the world's GPUs behind b200vs_shard_*.
@@ -553,6 +565,8 @@ def main():
     ap.add_argument("--pq-m", type=int, default=96, help="cfg3: sub-quantisers (768 must divide by it)")
     ap.add_argument("--hnsw-n", type=int, default=1_000_000)
     ap.add_argument("--hnsw-build-threads", type=int, default=64)
+    ap.add_argument("--hnsw-build", choices=("host", "device"), default="host", help="cfg4: graph built by host writers or on the device")
+    ap.add_argument("--hnsw-build-batch", type=int, default=0, help="cfg4 --hnsw-build device: rows per batch (0 = library default)")
     ap.add_argument("--cfg5-rows", type=int, default=6_250_000, help="cfg5: database rows per GPU (6.25 M x 1536 f32 = 38 GB of an 80 GB H100)")
     ap.add_argument("--cfg5-batch", type=int, default=4096)
     ap.add_argument("--cfg5-steps", type=int, default=10)
@@ -562,7 +576,7 @@ def main():
     a = ap.parse_args()
     o = oracle_lib.load()
     cores = os.cpu_count() or 1
-    fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads),
+    fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads, a.hnsw_build, a.hnsw_build_batch),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
            "6": lambda: cfg6(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}

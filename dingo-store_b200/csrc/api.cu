@@ -148,6 +148,25 @@ int b200vs_add_with_ids(b200vs_index* h, int64_t n, const float* x, const int64_
   });
 }
 
+int b200vs_hnsw_add_batched(b200vs_index* h, int64_t n, const float* x, const int64_t* ids, int32_t batch) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    if (ix->type != B200VS_HNSW) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction needs an HNSW index");
+    if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+    hnsw_add_batched(ix, n, x, ids, batch);
+    return B200VS_OK;
+  });
+}
+
+int b200vs_debug_hnsw_build_scratch_limit(b200vs_index* h, int64_t bytes) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    if (ix->type != B200VS_HNSW || bytes < 0) fail(B200VS_EILLEGAL_PARAMETERS, "scratch limit needs an HNSW index and bytes >= 0");
+    hnsw_build_scratch_limit(ix, bytes);
+    return B200VS_OK;
+  });
+}
+
 int b200vs_add_with_ids_device(b200vs_index* h, int64_t n, const float* x_dev, const int64_t* ids_dev, const int64_t* lists_dev, int upsert) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);

@@ -23,6 +23,9 @@
 #include <mutex>
 #include <random>
 #include <thread>
+#include <unordered_set>
+
+#include <cub/cub.cuh>
 
 #include "index.h"
 #include "scan_kernels.cuh"
@@ -565,6 +568,452 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
   }
 }
 
+// ---------------- batched construction on the device (DESIGN §4.4) ----------------
+// A batch of rows is inserted against the graph as it was at the batch start: construction search per (row, level), then
+// forward links per (row, level) from the search result plus the batch's earlier rows, then reverse links grouped per
+// (level, target).  Candidate lists are ordered by the 64-bit key ord(distance) << 32 | node id, so every tie is broken by
+// insertion index and nothing depends on thread timing.
+constexpr int HNSW_BUILD_MAX_BATCH = 8192;  // rows per batch (the peer matrix is batch^2 floats)
+constexpr int HNSW_BUILD_DEFAULT_BATCH = 2048;
+constexpr size_t HNSW_BUILD_SMEM = 200 * 1024;
+
+struct HnswBuildDev {  // the device mirror as the link kernels write it
+  const float* data;
+  unsigned int* link0;
+  const long long* up_off;
+  unsigned int* linkup;
+  int d, M, maxM, maxM0, efc;
+  __device__ __forceinline__ unsigned int* links(unsigned int node, int level) const {
+    return level == 0 ? link0 + (size_t)node * (maxM0 + 1) : linkup + up_off[node] + (size_t)(level - 1) * (maxM + 1);
+  }
+};
+
+__device__ __forceinline__ unsigned long long cand_key(float d, unsigned int id) { return ((unsigned long long)f2ord(d) << 32) | id; }
+
+// ascending sort of keys[0, p2) (p2 a power of two), all threads of the CTA
+__device__ void bitonic_sort(unsigned long long* keys, int p2) {
+  __syncthreads();
+  for (int k = 2; k <= p2; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int x = threadIdx.x; x < p2; x += HNSW_THREADS) {
+        const int y = x ^ j;
+        if (y > x) {
+          const unsigned long long a = keys[x], b = keys[y];
+          if ((a > b) == ((x & k) == 0)) { keys[x] = b; keys[y] = a; }
+        }
+      }
+      __syncthreads();
+    }
+}
+
+// HostGraph::heuristic over the ascending candidates C[0, c): keeps a candidate unless a node already kept is closer to it
+// than the base; fewer than lim candidates are all kept.  sel[0, return) ascending.  All 32 quads score one candidate against
+// up to 32 kept nodes per round.
+template <bool L2>
+__device__ int heuristic_select(const unsigned long long* C, int c, int lim, unsigned int* sel, const float* data, int d) {
+  __syncthreads();
+  if (c < lim) {
+    for (int i = threadIdx.x; i < c; i += HNSW_THREADS) sel[i] = (unsigned int)C[i];
+    __syncthreads();
+    return c;
+  }
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
+  const bool vec = (d & 3) == 0;
+  int nsel = 0;
+  for (int k = 0; k < c && nsel < lim; ++k) {
+    const unsigned int cand = (unsigned int)C[k];
+    const float dq = ord2f((unsigned int)(C[k] >> 32));
+    bool bad = false;
+    for (int s0 = 0; s0 < nsel; s0 += 32) {
+      const int s = s0 + quad;
+      float v = quad_distance<L2>(data + (size_t)sel[s < nsel ? s : 0] * d, data + (size_t)cand * d, d, t, vec);
+      if (!L2) v = __fsub_rn(1.0f, v);
+      if (s < nsel && v < dq) bad = true;
+    }
+    if (!__syncthreads_or(bad)) {
+      if (threadIdx.x == 0) sel[nsel] = cand;
+      ++nsel;
+      __syncthreads();
+    }
+  }
+  return nsel;
+}
+
+// Construction search: one CTA per batch row.  Greedy descent from the entry point through the levels above the row's own,
+// then HostGraph::search_layer with ef = efc at every level from min(level, maxlevel) down to 0, each starting from the
+// closest node found one level up.  out[(slot_off[r] + l) * efc ...] = the result at level l, ascending by (distance, node);
+// out_cnt = its length.  FAST = no tombstones and efc + 1 <= HNSW_CAND_SMEM: the merged-array form of hnsw_search_kernel;
+// otherwise the two heaps, the candidate heap spilling to cand_pool.  The visited bitset is cleared per level.
+template <bool L2, bool FAST>
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_search_kernel(const HnswDev g, int efc, const int* __restrict__ levels, long long row0,
+                                                                        long long n0, const long long* __restrict__ slot_off,
+                                                                        unsigned int* visited, long long words, HeapEnt* cand_pool,
+                                                                        long long cand_cap, HeapEnt* out, int* out_cnt) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ float s_d[32];
+  __shared__ unsigned int s_id[32];
+  __shared__ int s_m;
+  __shared__ unsigned int s_cur;
+  __shared__ float s_curdist;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r = row0 + blockIdx.x;
+  const int d = g.d;
+  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
+  float* qs = reinterpret_cast<float*>(smem);
+  HeapEnt* top_sm = reinterpret_cast<HeapEnt*>(smem + qbytes);
+  HeapEnt* cand_sm = reinterpret_cast<HeapEnt*>(smem + qbytes + (size_t)(efc + 1) * sizeof(HeapEnt));
+  for (int i = threadIdx.x; i < d; i += HNSW_THREADS) qs[i] = g.data[(size_t)(n0 + r) * d + i];
+  __syncthreads();
+  const bool vec = (d & 3) == 0;
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
+  unsigned int* vis = visited + (size_t)blockIdx.x * words;
+  const int lev = levels[r];
+  const int top_level = min(lev, g.maxlevel);
+  auto score = [&](int m) {
+    const unsigned int row = s_id[quad < m ? quad : 0];
+    float v = quad_distance<L2>(g.data + (size_t)row * d, qs, d, t, vec);
+    if (!L2) v = __fsub_rn(1.0f, v);
+    if (quad < m && t == 0) s_d[quad] = v;
+  };
+  auto links = [&](unsigned int node, int level) -> const unsigned int* {
+    return level == 0 ? g.link0 + (size_t)node * (g.maxM0 + 1) : g.linkup + g.up_off[node] + (size_t)(level - 1) * (g.maxM + 1);
+  };
+
+  unsigned int cur = g.enterpoint;
+  if (threadIdx.x == 0) s_id[0] = cur;
+  __syncthreads();
+  score(1);
+  __syncthreads();
+  float curdist = s_d[0];
+  for (int level = g.maxlevel; level > lev; --level) {  // greedy descent (add_point: only when the row's level is below maxlevel)
+    bool changed = true;
+    while (changed) {
+      changed = false;
+      const unsigned int* l = links(cur, level);
+      const int size = (int)l[0];
+      for (int c0 = 0; c0 < size; c0 += 32) {
+        const int m = min(32, size - c0);
+        __syncthreads();
+        if (warp == 0 && lane < m) s_id[lane] = l[1 + c0 + lane];
+        __syncthreads();
+        score(m);
+        __syncthreads();
+        for (int i = 0; i < m; ++i) {
+          const float dd = s_d[i];
+          if (dd < curdist) { curdist = dd; cur = s_id[i]; changed = true; }
+        }
+      }
+    }
+  }
+
+  for (int level = top_level; level >= 0; --level) {
+    __syncthreads();
+    for (long long w = threadIdx.x; w < words; w += HNSW_THREADS) vis[w] = 0u;
+    __syncthreads();
+    HeapEnt* res = out + (size_t)(slot_off[r] + level) * efc;
+    if (FAST) {
+      HeapEnt* T = top_sm;
+      HeapEnt* T2 = cand_sm;
+      int ntop = 1;
+      if (threadIdx.x == 0) { T[0].d = curdist; T[0].id = cur; vis[cur >> 5] |= 1u << (cur & 31); }
+      unsigned int node = 0;
+      int size = 0, c0 = 0;
+      bool expanding = false;
+      for (;;) {
+        __syncthreads();
+        if (warp == 0) {
+          int m = -1;
+          for (;;) {
+            if (!expanding) {
+              int idx = -1;
+              for (int b0 = 0; b0 < ntop && idx < 0; b0 += 32) {
+                const int i = b0 + lane;
+                const bool open = i < ntop && (T[i].id >> 31) == 0u;
+                const unsigned msk = __ballot_sync(0xffffffffu, open);
+                if (msk) idx = b0 + __ffs(msk) - 1;
+              }
+              if (idx < 0) { m = -1; break; }
+              node = T[idx].id;
+              __syncwarp();
+              if (lane == 0) T[idx].id = node | 0x80000000u;
+              size = (int)links(node, level)[0];
+              c0 = 0;
+              expanding = true;
+            }
+            if (c0 >= size) { expanding = false; continue; }
+            const unsigned int* l = links(node, level) + 1 + c0;
+            const int cnt = min(32, size - c0);
+            c0 += 32;
+            unsigned int nb = 0;
+            bool fresh = false;
+            if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
+            const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
+            if (fresh) {
+              atomicOr(&vis[nb >> 5], 1u << (nb & 31));
+              s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
+            }
+            m = __popc(mask);
+            if (m > 0) break;
+          }
+          if (lane == 0) s_m = m;
+        }
+        __syncthreads();
+        const int m = s_m;
+        if (m < 0) break;
+        score(m);
+        __syncthreads();
+        for (int tix = threadIdx.x; tix < ntop; tix += HNSW_THREADS) {
+          const HeapEnt e = T[tix];
+          int c = 0;
+          for (int j = 0; j < m; ++j) c += s_d[j] < e.d ? 1 : 0;
+          if (tix + c < efc) T2[tix + c] = e;
+        }
+        if (threadIdx.x < m) {
+          const float dj = s_d[threadIdx.x];
+          int rank = 0;
+          for (int i = 0; i < m; ++i) rank += (s_d[i] < dj || (s_d[i] == dj && i < (int)threadIdx.x)) ? 1 : 0;
+          int lo = 0, hi = ntop;
+          while (lo < hi) { const int mid = (lo + hi) >> 1; if (T[mid].d <= dj) lo = mid + 1; else hi = mid; }
+          if (rank + lo < efc) { HeapEnt e; e.d = dj; e.id = s_id[threadIdx.x]; T2[rank + lo] = e; }
+        }
+        ntop = min(efc, ntop + m);
+        HeapEnt* tmp = T; T = T2; T2 = tmp;
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {  // T is ascending in distance; equal distances go by node id
+        for (int i = 0; i < ntop; ++i) {
+          HeapEnt e = T[i];
+          e.id &= 0x7fffffffu;
+          int j = i;
+          while (j > 0 && res[j - 1].d == e.d && res[j - 1].id > e.id) { res[j] = res[j - 1]; --j; }
+          res[j] = e;
+        }
+        out_cnt[slot_off[r] + level] = ntop;
+        if (ntop > 0) { s_cur = res[0].id; s_curdist = res[0].d; }
+      }
+    } else {
+      const HeapRef top{top_sm, top_sm, efc + 1};
+      const HeapRef cand{cand_sm, cand_pool + (size_t)blockIdx.x * cand_cap, HNSW_CAND_SMEM};
+      int ntop = 0, ncand = 0;
+      float lower = 3.402823466e+38f;
+      if (warp == 0) {
+        const bool ok = !g.deleted[cur];
+        if (lane == 0) {
+          if (ok) { h_push<true>(top, ntop, curdist, cur); h_push<false>(cand, ncand, curdist, cur); }
+          else h_push<false>(cand, ncand, 3.402823466e+38f, cur);
+          vis[cur >> 5] |= 1u << (cur & 31);
+        }
+        lower = ok ? curdist : 3.402823466e+38f;
+      }
+      unsigned int node = 0;
+      int size = 0, c0 = 0;
+      bool expanding = false;
+      for (;;) {
+        __syncthreads();
+        if (warp == 0) {
+          int m = -1;
+          for (;;) {
+            if (!expanding) {
+              int go = 0;
+              if (lane == 0 && ncand > 0) {
+                const HeapEnt ce = cand.get(0);
+                if (!(ce.d > lower && ntop == efc)) { node = ce.id; h_pop<false>(cand, ncand); go = 1; }
+              }
+              go = __shfl_sync(0xffffffffu, go, 0);
+              if (!go) { m = -1; break; }
+              node = __shfl_sync(0xffffffffu, node, 0);
+              size = (int)links(node, level)[0];
+              c0 = 0;
+              expanding = true;
+            }
+            if (c0 >= size) { expanding = false; continue; }
+            const unsigned int* l = links(node, level) + 1 + c0;
+            const int cnt = min(32, size - c0);
+            c0 += 32;
+            unsigned int nb = 0;
+            bool fresh = false;
+            if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
+            const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
+            if (fresh) {
+              atomicOr(&vis[nb >> 5], 1u << (nb & 31));
+              s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
+            }
+            m = __popc(mask);
+            if (m > 0) break;
+          }
+          if (lane == 0) s_m = m;
+        }
+        __syncthreads();
+        const int m = s_m;
+        if (m < 0) break;
+        score(m);
+        __syncthreads();
+        if (warp == 0) {
+          bool allowed = false;
+          if (lane < m) allowed = !g.deleted[s_id[lane]];
+          const unsigned int amask = __ballot_sync(0xffffffffu, allowed);
+          if (lane == 0) {
+            for (int i = 0; i < m; ++i) {
+              const float dd = s_d[i];
+              if (ntop < efc || lower > dd) {
+                h_push<false>(cand, ncand, dd, s_id[i]);
+                if ((amask >> i) & 1u) h_push<true>(top, ntop, dd, s_id[i]);
+                if (ntop > efc) h_pop<true>(top, ntop);
+                if (ntop > 0) lower = top.get(0).d;
+              }
+            }
+          }
+          lower = __shfl_sync(0xffffffffu, lower, 0);
+        }
+      }
+      if (threadIdx.x == 0) {
+        const int cnt = ntop;
+        while (ntop > 0) { const HeapEnt e = top.get(0); h_pop<true>(top, ntop); res[ntop] = e; }  // largest first -> ascending
+        for (int i = 1; i < cnt; ++i) {
+          const HeapEnt e = res[i];
+          int j = i;
+          while (j > 0 && res[j - 1].d == e.d && res[j - 1].id > e.id) { res[j] = res[j - 1]; --j; }
+          res[j] = e;
+        }
+        out_cnt[slot_off[r] + level] = cnt;
+        if (cnt > 0) { s_cur = res[0].id; s_curdist = res[0].d; }
+      }
+    }
+    if (threadIdx.x == 0 && out_cnt[slot_off[r] + level] == 0) { s_cur = cur; s_curdist = curdist; }
+    __syncthreads();
+    cur = s_cur;
+    curdist = s_curdist;
+  }
+}
+
+// Peer distances of a batch: peer[i * nb + j] for j < i only (the link kernel reads no other entry), one quad per pair, in
+// pair_distance_kernel's arithmetic (quad_distance, 1 - ip for IP and cosine).
+template <bool L2>
+__global__ void __launch_bounds__(256) hnsw_peer_distance_kernel(const float* __restrict__ rows, int nb, int d, float* __restrict__ peer) {
+  const long long pair = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+  const int t = threadIdx.x & 3;
+  const long long total = (long long)nb * (nb - 1) / 2;
+  const bool valid = pair < total;
+  const long long p = valid ? pair : 0;
+  long long i = (long long)((1.0 + sqrt(1.0 + 8.0 * (double)p)) / 2.0);  // p = i (i - 1) / 2 + j, 0 <= j < i
+  while (i * (i - 1) / 2 > p) --i;
+  while ((i + 1) * i / 2 <= p) ++i;
+  const long long j = p - i * (i - 1) / 2;
+  float v = quad_distance<L2>(rows + (size_t)i * d, rows + (size_t)j * d, d, t, (d & 3) == 0);
+  if (!L2) v = __fsub_rn(1.0f, v);
+  if (valid && t == 0) peer[(size_t)i * nb + j] = v;
+}
+
+// deleted[ids[k]] = 1: the tombstones of one batch in one launch
+__global__ void hnsw_tombstone_kernel(unsigned char* deleted, const unsigned int* __restrict__ ids, long long n) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) deleted[ids[k]] = 1;
+}
+
+// Forward links: one CTA per (row, level) task.  Candidates = the search result at that level merged with the batch's earlier
+// rows j < i whose level reaches it (peer distances from the pair matrix), best efc by key; heuristic(M) of those is written
+// farthest first, as HostGraph::connect writes it.  Each kept target t emits the reverse-link key (level, t, i) into
+// trip[task * M + s]; unused slots hold ~0.
+template <bool L2>
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_link_kernel(const HnswBuildDev b, long long n0, int nb, const int* __restrict__ levels,
+                                                                      int maxlevel, const float* __restrict__ peer, const long long* __restrict__ slot_off,
+                                                                      const HeapEnt* __restrict__ sres, const int* __restrict__ scnt,
+                                                                      const int2* __restrict__ tasks, unsigned long long* trip) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ int s_cp;
+  const int2 task = tasks[blockIdx.x];
+  const int i = task.x, l = task.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem);
+  const int top_level = min(levels[i], maxlevel);
+  const long long slot = slot_off[i] + l;
+  const int cs = l <= top_level ? scnt[slot] : 0;
+  for (int k = threadIdx.x; k < cs; k += HNSW_THREADS) keys[k] = cand_key(sres[(size_t)slot * b.efc + k].d, sres[(size_t)slot * b.efc + k].id);
+  __syncthreads();
+  // a peer can only enter a full list below its last key (peer ids are larger than every graph node's)
+  const unsigned long long tau = cs == b.efc ? keys[cs - 1] : ~0ull;
+  if (warp == 0) {
+    int cp = 0;
+    for (int j0 = 0; j0 < i; j0 += 32) {
+      const int j = j0 + lane;
+      unsigned long long key = ~0ull;
+      if (j < i && levels[j] >= l) key = cand_key(peer[(size_t)i * nb + j], (unsigned int)(n0 + j));
+      const bool ok = key < tau;
+      const unsigned int mask = __ballot_sync(0xffffffffu, ok);
+      if (ok) keys[cs + cp + __popc(mask & ((1u << lane) - 1u))] = key;
+      cp += __popc(mask);
+    }
+    if (lane == 0) s_cp = cp;
+  }
+  __syncthreads();
+  int c = cs + s_cp;
+  if (s_cp > 0) {
+    int p2 = 1;
+    while (p2 < c) p2 <<= 1;
+    for (int k = c + threadIdx.x; k < p2; k += HNSW_THREADS) keys[k] = ~0ull;
+    bitonic_sort(keys, p2);
+    c = min(c, b.efc);
+  }
+  unsigned int* sel = reinterpret_cast<unsigned int*>(smem + (size_t)(b.efc + nb) * 2 * sizeof(unsigned long long));
+  const int nsel = heuristic_select<L2>(keys, c, b.M, sel, b.data, b.d);
+  unsigned int* list = b.links((unsigned int)(n0 + i), l);
+  for (int s = threadIdx.x; s < nsel; s += HNSW_THREADS) list[1 + s] = sel[nsel - 1 - s];
+  if (threadIdx.x == 0) list[0] = (unsigned int)nsel;
+  for (int s = threadIdx.x; s < b.M; s += HNSW_THREADS)
+    trip[(size_t)blockIdx.x * b.M + s] = s < nsel ? ((unsigned long long)l << 52) | ((unsigned long long)sel[s] << 20) | (unsigned long long)i : ~0ull;
+}
+
+// Reverse links: keys sorted ascending group the sources of every (level, target) in call order.  The CTA of a group's first
+// key appends the sources when they fit into the target's list, and otherwise rewrites the list as heuristic(list ∪ sources,
+// Mmax) farthest first (connect's shrink).  Entries past the new size keep their old values, as in connect.
+template <bool L2>
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_reverse_kernel(const HnswBuildDev b, long long n0, const unsigned long long* __restrict__ keys,
+                                                                         long long total) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ int s_ns;
+  const long long k0 = blockIdx.x;
+  const unsigned long long key = keys[k0];
+  if (key == ~0ull) return;
+  if (k0 > 0 && (keys[k0 - 1] >> 20) == (key >> 20)) return;
+  if (threadIdx.x == 0) {
+    long long e = k0 + 1;
+    while (e < total && (keys[e] >> 20) == (key >> 20)) ++e;
+    s_ns = (int)(e - k0);
+  }
+  __syncthreads();
+  const int ns = s_ns;
+  const int l = (int)(key >> 52);
+  const unsigned int tgt = (unsigned int)((key >> 20) & 0xffffffffu);
+  const int mcur = l ? b.maxM : b.maxM0;
+  unsigned int* list = b.links(tgt, l);
+  const int sz = (int)list[0];
+  auto source = [&](int s) { return (unsigned int)(n0 + (long long)(keys[k0 + s] & 0xfffffu)); };
+  if (sz + ns <= mcur) {
+    for (int s = threadIdx.x; s < ns; s += HNSW_THREADS) list[1 + sz + s] = source(s);
+    __syncthreads();
+    if (threadIdx.x == 0) list[0] = (unsigned int)(sz + ns);
+    return;
+  }
+  unsigned long long* cand = reinterpret_cast<unsigned long long*>(smem);
+  const int c = sz + ns;
+  int p2 = 1;
+  while (p2 < c) p2 <<= 1;
+  unsigned int* sel = reinterpret_cast<unsigned int*>(smem + (size_t)p2 * sizeof(unsigned long long));
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
+  const bool vec = (b.d & 3) == 0;
+  for (int c0 = 0; c0 < p2; c0 += 32) {
+    const int x = c0 + quad;
+    const unsigned int id = x < sz ? list[1 + x] : x < c ? source(x - sz) : tgt;
+    float v = quad_distance<L2>(b.data + (size_t)id * b.d, b.data + (size_t)tgt * b.d, b.d, t, vec);
+    if (!L2) v = __fsub_rn(1.0f, v);
+    if (t == 0 && x < p2) cand[x] = x < c ? cand_key(v, id) : ~0ull;
+  }
+  bitonic_sort(cand, p2);
+  const int nsel = heuristic_select<L2>(cand, c, mcur, sel, b.data, b.d);
+  for (int s = threadIdx.x; s < nsel; s += HNSW_THREADS) list[1 + s] = sel[nsel - 1 - s];
+  if (threadIdx.x == 0) list[0] = (unsigned int)nsel;
+}
+
 }  // namespace
 
 struct HnswIndex : IndexBase {
@@ -670,6 +1119,255 @@ struct HnswIndex : IndexBase {
     }
     dirty = true;
   }
+  // b200vs_hnsw_add_batched: the rule of DESIGN §4.4.  The host plans every batch first on a copy of the bookkeeping it needs
+  // (levels from a copy of G.rng in call order, the batch schedule, tombstones, node ids, entry point); the device mirror then
+  // builds the links batch after batch in stream order.  G (and its generator) changes only once the device work has
+  // finished: a call that fails on the way leaves the index as it was and marks the mirror for a full re-upload.
+  int64_t build_scratch_limit = 0;  // b200vs_debug_hnsw_build_scratch_limit: device scratch bytes one call may take, 0 = no cap
+
+  void add_batched(int64_t n, const float* x, const int64_t* in_ids, int batch) {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
+    if (G.n + n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction holds at most 2^31 - 1 nodes");
+    batch = batch <= 0 ? HNSW_BUILD_DEFAULT_BATCH : std::min(batch, HNSW_BUILD_MAX_BATCH);
+    const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
+    const int bmax = (int)std::min<int64_t>(batch, n);  // largest batch of this call
+    const size_t qbytes = ((size_t)dim * 4 + 15) / 16 * 16;
+    const size_t smem_search = qbytes + (size_t)(efc + 1) * sizeof(HeapEnt) + (size_t)HNSW_CAND_SMEM * sizeof(HeapEnt);
+    const size_t smem_link = (size_t)(efc + bmax) * 2 * sizeof(unsigned long long) + (size_t)M * 4;
+    const size_t smem_rev = (size_t)(maxM0 + bmax) * 2 * sizeof(unsigned long long) + (size_t)maxM0 * 4;
+    if (smem_search > HNSW_BUILD_SMEM || smem_link > HNSW_BUILD_SMEM || smem_rev > HNSW_BUILD_SMEM)
+      fail(B200VS_EILLEGAL_PARAMETERS, "efconstruction / dimension / batch too large for the batched construction kernels");
+    set_device();
+    cudaStream_t s = stream;
+    upload(s);
+    quiesce();
+
+    // ---- plan (host), on copies: G is not touched until the device work is done ----
+    const int64_t n0_call = G.n, ntot = G.n + n;
+    std::vector<float> rows((size_t)n * dim);
+    for (int64_t i = 0; i < n; ++i) {
+      const float* xi = x + (size_t)i * dim;
+      float* o = &rows[(size_t)i * dim];
+      if (metric != B200VS_COSINE) { memcpy(o, xi, (size_t)dim * 4); continue; }
+      float norm = 0.0f;  // NormalizeVectorForHnsw, as add() does it
+      for (int j = 0; j < dim; ++j) norm += xi[j] * xi[j];
+      norm = 1.0f / (sqrtf(norm) + 1e-30f);
+      for (int j = 0; j < dim; ++j) o[j] = xi[j] * norm;
+    }
+    std::default_random_engine rng = G.rng;
+    std::vector<int> lev(n);
+    {
+      std::uniform_real_distribution<double> U(0.0, 1.0);
+      for (int64_t i = 0; i < n; ++i) lev[i] = (int)(-log(U(rng)) * G.mult);
+    }
+    struct Batch { int64_t a, b; int maxlevel; tableint ep; bool deletions; int64_t task0, ntask, dead0, ndead; };
+    std::vector<Batch> plan;
+    std::vector<long long> slot_off(n);
+    std::vector<int2> tasks;
+    std::vector<unsigned int> dead;               // nodes tombstoned at each batch start (Batch::dead0, ndead)
+    std::unordered_map<int64_t, tableint> fresh;  // labels inserted by this call -> their latest node (live)
+    int64_t gn = G.n, ndel = G.ndeleted;
+    int maxlevel = G.maxlevel;
+    tableint ep = G.enterpoint;
+    int64_t max_slots = 0;
+    std::unordered_set<int64_t> in_batch;
+    for (int64_t a = 0; a < n;) {
+      Batch B;
+      B.a = a;
+      const int64_t lim = gn == 0 ? 1 : std::min<int64_t>(batch, gn);
+      in_batch.clear();
+      int64_t e = a;
+      while (e < n && e - a < lim && in_batch.insert(in_ids[e]).second) ++e;
+      B.b = e;
+      B.dead0 = (int64_t)dead.size();
+      for (int64_t i = a; i < e; ++i) {  // add_point's tombstone of a label already present
+        auto f = fresh.find(in_ids[i]);
+        if (f != fresh.end()) { dead.push_back(f->second); continue; }
+        auto it = G.lookup.find(in_ids[i]);
+        if (it != G.lookup.end() && !G.deleted[it->second]) dead.push_back(it->second);
+      }
+      B.ndead = (int64_t)dead.size() - B.dead0;
+      ndel += B.ndead;
+      B.maxlevel = maxlevel; B.ep = ep; B.deletions = ndel > 0;
+      B.task0 = (int64_t)tasks.size();
+      long long slots = 0;
+      for (int64_t i = a; i < e; ++i) {
+        fresh[in_ids[i]] = (tableint)(gn++);
+        slot_off[i] = slots;
+        slots += std::min(lev[i], B.maxlevel) + 1;
+        for (int l = 0; l <= lev[i]; ++l) tasks.push_back(make_int2((int)(i - a), l));
+      }
+      max_slots = std::max<int64_t>(max_slots, slots);
+      B.ntask = (int64_t)tasks.size() - B.task0;
+      for (int64_t i = a; i < e; ++i)  // entry point in call order
+        if (lev[i] > maxlevel) { ep = (tableint)(n0_call + i); maxlevel = lev[i]; }
+      plan.push_back(B);
+      a = e;
+    }
+    long long up_old = 0;
+    for (int64_t i = 0; i < n0_call; ++i) up_old += (long long)G.linkup[i].size();
+    std::vector<long long> off(n + 1);
+    off[0] = up_old;
+    for (int64_t i = 0; i < n; ++i) off[i + 1] = off[i] + (long long)lev[i] * (maxM + 1);
+    const long long up_new = off[n];
+    G.reserve(std::max<int64_t>(G.cap, ntot));  // capacity only: nothing observable changes
+    std::vector<unsigned int> up((size_t)std::max<long long>(up_new, 1)), l0((size_t)ntot * (maxM0 + 1));
+
+    try {
+      // ---- device mirror: append the call's rows, empty link lists and upper-level slots (beyond G.n: unseen by searches) ----
+      d_data.reserve((size_t)ntot * dim, (size_t)n0_call * dim, s);
+      d_labels.reserve(ntot, n0_call, s); d_deleted.reserve(ntot, n0_call, s); d_upoff.reserve(ntot + 1, n0_call, s);
+      d_link0.reserve((size_t)ntot * (maxM0 + 1), (size_t)n0_call * (maxM0 + 1), s);
+      d_linkup.reserve((size_t)std::max<long long>(up_new, 1), (size_t)up_old, s);
+      B200VS_CUDA(cudaMemcpyAsync(d_data.p + (size_t)n0_call * dim, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemcpyAsync(d_labels.p + n0_call, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemsetAsync(d_deleted.p + n0_call, 0, (size_t)n, s));
+      B200VS_CUDA(cudaMemcpyAsync(d_upoff.p + n0_call, off.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemsetAsync(d_link0.p + (size_t)n0_call * (maxM0 + 1), 0, (size_t)n * (maxM0 + 1) * 4, s));
+      if (up_new > up_old) B200VS_CUDA(cudaMemsetAsync(d_linkup.p + up_old, 0, (size_t)(up_new - up_old) * 4, s));
+
+      // ---- scratch, freed at the end of the call ----
+      size_t scratch_bytes = 0;
+      auto take = [&](auto& buf, size_t count) {  // a device reservation counted against build_scratch_limit
+        if (count <= buf.cap) return;
+        const size_t after = scratch_bytes + (count - buf.cap) * sizeof(*buf.p);
+        if (build_scratch_limit > 0 && after > (size_t)build_scratch_limit)
+          throw CudaError("HNSW batched construction: device scratch over the limit (out of memory)");
+        buf.reserve(count, 0, s);  // a grown buffer needs none of its old contents
+        scratch_bytes = after;
+      };
+      const bool any_heap = efc + 1 > HNSW_CAND_SMEM || std::any_of(plan.begin(), plan.end(), [](const Batch& B) { return B.deletions; });
+      const long long words_max = (ntot + 31) / 32;
+      const size_t row_bytes = (size_t)words_max * 4 + (any_heap ? (size_t)(ntot + 1) * sizeof(HeapEnt) : 0);
+      const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(bmax, (int64_t)(HNSW_CAND_POOL_BYTES / row_bytes)));
+      int64_t max_task = 1;
+      for (const Batch& B : plan) max_task = std::max(max_task, B.ntask);
+      const size_t ntrip = (size_t)max_task * M;
+      DevBuf<unsigned int> d_vis, d_dead;
+      DevBuf<HeapEnt> d_pool, d_sres;
+      DevBuf<int> d_scnt, d_lev;
+      DevBuf<long long> d_slot;
+      DevBuf<int2> d_tasks;
+      DevBuf<float> d_peer;  // grows with the batches (1, 1, 2, 4, ... rows)
+      DevBuf<unsigned long long> d_trip, d_trip_sorted;
+      DevBuf<unsigned char> d_sort;
+      take(d_vis, (size_t)chunk * words_max);
+      if (any_heap) take(d_pool, (size_t)chunk * (ntot + 1));
+      take(d_sres, (size_t)std::max<int64_t>(max_slots, 1) * efc);
+      take(d_scnt, (size_t)std::max<int64_t>(max_slots, 1));
+      take(d_lev, (size_t)n);
+      take(d_slot, (size_t)n);
+      take(d_tasks, std::max<size_t>(tasks.size(), 1));
+      take(d_dead, std::max<size_t>(dead.size(), 1));
+      take(d_trip, ntrip); take(d_trip_sorted, ntrip);
+      size_t sort_bytes = 0;
+      B200VS_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, d_trip.p, d_trip_sorted.p, (int)ntrip, 0, 64, s));
+      take(d_sort, std::max<size_t>(sort_bytes, 1));
+      B200VS_CUDA(cudaMemcpyAsync(d_lev.p, lev.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemcpyAsync(d_slot.p, slot_off.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+      if (!tasks.empty()) B200VS_CUDA(cudaMemcpyAsync(d_tasks.p, tasks.data(), tasks.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+      if (!dead.empty()) B200VS_CUDA(cudaMemcpyAsync(d_dead.p, dead.data(), dead.size() * 4, cudaMemcpyHostToDevice, s));
+
+      const bool l2 = metric == B200VS_L2;
+      auto setsmem = [](const void* fn) { B200VS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HNSW_BUILD_SMEM)); };
+      if (l2) {
+        setsmem((const void*)hnsw_build_search_kernel<true, true>); setsmem((const void*)hnsw_build_search_kernel<true, false>);
+        setsmem((const void*)hnsw_build_link_kernel<true>); setsmem((const void*)hnsw_build_reverse_kernel<true>);
+      } else {
+        setsmem((const void*)hnsw_build_search_kernel<false, true>); setsmem((const void*)hnsw_build_search_kernel<false, false>);
+        setsmem((const void*)hnsw_build_link_kernel<false>); setsmem((const void*)hnsw_build_reverse_kernel<false>);
+      }
+      if (profiling) for (int p = PH_BUILD_SEARCH; p <= PH_BUILD_LINK; ++p) phase_ms[p] = 0.f;
+      HnswBuildDev bd;
+      bd.data = d_data.p; bd.link0 = d_link0.p; bd.up_off = d_upoff.p; bd.linkup = d_linkup.p;
+      bd.d = dim; bd.M = M; bd.maxM = maxM; bd.maxM0 = maxM0; bd.efc = efc;
+      for (const Batch& B : plan) {
+        if (B.ndead > 0) {
+          hnsw_tombstone_kernel<<<(unsigned)cdiv(B.ndead, 256), 256, 0, s>>>(d_deleted.p, d_dead.p + B.dead0, B.ndead);
+          B200VS_CUDA(cudaGetLastError());
+        }
+        const long long n0 = n0_call + B.a;
+        const int nb = (int)(B.b - B.a);
+        if (n0 == 0) continue;  // the first row of an empty graph goes in alone, without links
+        if (nb > 1) take(d_peer, (size_t)nb * nb);
+        HnswDev g;
+        g.data = d_data.p; g.labels = d_labels.p; g.link0 = d_link0.p; g.up_off = d_upoff.p; g.linkup = d_linkup.p; g.deleted = d_deleted.p;
+        g.n = n0; g.d = dim; g.maxM = maxM; g.maxM0 = maxM0; g.maxlevel = B.maxlevel; g.l2 = l2; g.enterpoint = B.ep;
+        g.has_deletions = B.deletions;
+        const bool fast = !B.deletions && efc + 1 <= HNSW_CAND_SMEM;
+        const long long words = (n0 + 31) / 32, cand_cap = fast ? 0 : n0 + 1;
+        phase(PH_BUILD_SEARCH, s);
+        for (int64_t r0 = 0; r0 < nb; r0 += chunk) {
+          const unsigned m = (unsigned)std::min<int64_t>(chunk, nb - r0);
+#define B200VS_BUILD_SEARCH(L2_, FAST_)                                                                                                  \
+  hnsw_build_search_kernel<L2_, FAST_><<<m, HNSW_THREADS, smem_search, s>>>(g, efc, d_lev.p + B.a, r0, n0, d_slot.p + B.a, d_vis.p, words, \
+                                                                            d_pool.p, cand_cap, d_sres.p, d_scnt.p)
+          if (l2) { if (fast) B200VS_BUILD_SEARCH(true, true); else B200VS_BUILD_SEARCH(true, false); }
+          else { if (fast) B200VS_BUILD_SEARCH(false, true); else B200VS_BUILD_SEARCH(false, false); }
+#undef B200VS_BUILD_SEARCH
+          B200VS_CUDA(cudaGetLastError());
+        }
+        phase(PH_BUILD_SELECT, s);
+        if (nb > 1) {
+          const unsigned grid = (unsigned)cdiv((int64_t)nb * (nb - 1) / 2 * 4, 256);
+          const float* brows = d_data.p + (size_t)n0 * dim;
+          if (l2) hnsw_peer_distance_kernel<true><<<grid, 256, 0, s>>>(brows, nb, dim, d_peer.p);
+          else hnsw_peer_distance_kernel<false><<<grid, 256, 0, s>>>(brows, nb, dim, d_peer.p);
+          B200VS_CUDA(cudaGetLastError());
+        }
+        const size_t smem_l = (size_t)(efc + nb) * 2 * sizeof(unsigned long long) + (size_t)M * 4;
+        if (l2) hnsw_build_link_kernel<true><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(bd, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
+        else hnsw_build_link_kernel<false><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(bd, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
+        B200VS_CUDA(cudaGetLastError());
+        phase(PH_BUILD_LINK, s);
+        const int nt = (int)(B.ntask * M);
+        size_t tb = sort_bytes;
+        B200VS_CUDA(cub::DeviceRadixSort::SortKeys(d_sort.p, tb, d_trip.p, d_trip_sorted.p, nt, 0, 64, s));
+        const size_t smem_r = (size_t)(maxM0 + nb) * 2 * sizeof(unsigned long long) + (size_t)maxM0 * 4;
+        if (l2) hnsw_build_reverse_kernel<true><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(bd, n0, d_trip_sorted.p, nt);
+        else hnsw_build_reverse_kernel<false><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(bd, n0, d_trip_sorted.p, nt);
+        B200VS_CUDA(cudaGetLastError());
+        phase(-1, s);
+      }
+      phases_finish(s);
+      if (up_new > 0) B200VS_CUDA(cudaMemcpyAsync(up.data(), d_linkup.p, (size_t)up_new * 4, cudaMemcpyDeviceToHost, s));
+      B200VS_CUDA(cudaMemcpyAsync(l0.data(), d_link0.p, l0.size() * 4, cudaMemcpyDeviceToHost, s));
+      B200VS_CUDA(cudaStreamSynchronize(s));
+    } catch (...) {
+      // the mirror's link lists may hold part of the call: rebuild it from G, which is unchanged, at the next search
+      for (auto& m : phase_marks) cudaEventDestroy(m.second);
+      phase_marks.clear();
+      dirty = true;
+      uploaded_rows = 0;
+      throw;
+    }
+
+    // ---- commit: G takes the call's rows in call order (add_point's bookkeeping) and the device's link lists ----
+    for (int64_t i = 0; i < n; ++i) {
+      auto it = G.lookup.find(in_ids[i]);
+      if (it != G.lookup.end()) {
+        if (!G.deleted[it->second]) { G.deleted[it->second] = 1; ++G.ndeleted; }
+        G.lookup.erase(it);
+      }
+      const tableint c = (tableint)G.n++;
+      G.lookup[in_ids[i]] = c;
+      memcpy(&G.data[(size_t)c * dim], &rows[(size_t)i * dim], (size_t)dim * 4);
+      G.labels[c] = in_ids[i]; G.levels[c] = lev[i]; G.deleted[c] = 0;
+      G.linkup[c].assign((size_t)lev[i] * (maxM + 1), 0);
+    }
+    G.enterpoint = ep; G.maxlevel = maxlevel; G.rng = rng;
+    memcpy(G.link0.data(), l0.data(), l0.size() * 4);
+    long long acc = 0;
+    for (int64_t i = 0; i < ntot; ++i) {
+      const size_t sz = G.linkup[i].size();
+      if (sz) memcpy(G.linkup[i].data(), &up[acc], sz * 4);
+      acc += (long long)sz;
+    }
+    uploaded_rows = ntot;
+    dirty = false;
+  }
+
   // hnswlib getDataByLabel (hnsw.cc:383-395): the stored (for cosine: normalised) vector of a live label
   void reconstruct(int64_t n, const int64_t* in_ids, float* out, uint8_t* found) override {
     RwSharedGuard rl(this);
@@ -814,5 +1512,13 @@ struct HnswIndex : IndexBase {
 };
 
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p) { return new HnswIndex(m, d, p); }
+
+void hnsw_add_batched(IndexBase* ix, int64_t n, const float* x, const int64_t* ids, int batch) {
+  static_cast<HnswIndex*>(ix)->add_batched(n, x, ids, batch);
+}
+void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes) {
+  std::unique_lock<std::shared_mutex> wl(ix->rw);
+  static_cast<HnswIndex*>(ix)->build_scratch_limit = bytes;
+}
 
 }  // namespace b200vs

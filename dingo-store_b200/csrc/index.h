@@ -184,7 +184,9 @@ struct IndexBase {
   // overlapping searches interleave — they are diagnostics — but there is no data race)
   std::atomic<int64_t> stats[8] = {};
   // profiling only (one caller at a time): CUDA-event marks between the phases of a search, b200vs_last_phase_times
-  enum Phase { PH_COARSE_PREP = 0, PH_COARSE_SCAN, PH_COARSE_FINAL, PH_PLAN, PH_SAMPLE, PH_TAU, PH_CAPTURE, PH_FINAL, PH_FALLBACK, PH_OTHER, PH_COMM, PH_MERGE, PH_COUNT };
+  enum Phase { PH_COARSE_PREP = 0, PH_COARSE_SCAN, PH_COARSE_FINAL, PH_PLAN, PH_SAMPLE, PH_TAU, PH_CAPTURE, PH_FINAL, PH_FALLBACK, PH_OTHER, PH_COMM, PH_MERGE,
+               PH_BUILD_SEARCH, PH_BUILD_SELECT, PH_BUILD_LINK,  // b200vs_hnsw_add_batched: construction search / forward links / reverse links
+               PH_COUNT };
   float phase_ms[PH_COUNT] = {0};
   std::vector<std::pair<int, cudaEvent_t>> phase_marks;
   void phase(int id, cudaStream_t s) {  // "phase id starts here"
@@ -415,6 +417,9 @@ void launch_iota(long long* p, int64_t n, cudaStream_t s);
 void launch_negate(float* p, int64_t n, cudaStream_t s);
 // out[i*nr + j] = L2 ? ||a_i - b_j||^2 : 1 - <a_i, b_j>, reference summation order (VectorCalcDistance)
 void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s);
+// b200vs_hnsw_add_batched (hnsw.cu); ix must be an HNSW index
+void hnsw_add_batched(IndexBase* ix, int64_t n, const float* x, const int64_t* ids, int batch);
+void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes);  // b200vs_debug_hnsw_build_scratch_limit
 void launch_merge_api(int nparts, int64_t nq, int k, const float* pd, const long long* pi, float* od, long long* oi,
                       cudaStream_t s);
 

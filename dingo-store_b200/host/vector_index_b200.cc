@@ -10,6 +10,7 @@
 namespace dingodb {
 
 int32_t VectorIndexB200::max_range_search_result_count = 1024;
+int64_t VectorIndexB200::hnsw_device_build_min_rows = 0;
 
 namespace {
 
@@ -104,6 +105,9 @@ butil::Status VectorIndexB200::AddOrUpsert(const std::vector<pb::common::VectorW
   for (size_t i = 0; i < vs.size(); ++i) ids[i] = vs[i].id();
   const std::vector<float> x = ExtractVectorValue(vs, dimension_);
   std::shared_lock<std::shared_mutex> gate(write_gate_);
+  if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW && hnsw_device_build_min_rows > 0 &&
+      (int64_t)vs.size() >= hnsw_device_build_min_rows)
+    return ToStatus(b200vs_hnsw_add_batched(index_, (int64_t)vs.size(), x.data(), ids.data(), 0));
   int rc = b200vs_add_with_ids(index_, (int64_t)vs.size(), x.data(), ids.data(), is_upsert ? 1 : 0);
   if (rc == B200VS_EVECTOR_NOT_TRAIN) {  // "train with this batch and try again", ivf_flat.cc:133-150
     status = Train(vs);

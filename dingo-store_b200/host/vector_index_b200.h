@@ -66,6 +66,9 @@ class VectorIndexB200 : public VectorIndex {
 
   // largest result count RangeSearch keeps per query (FLAGS_vector_index_max_range_search_result_count, vector_reader.cc:60)
   static int32_t max_range_search_result_count;
+  // HNSW Add / Upsert calls of at least this many rows build the graph on the GPU in batches (b200vs_hnsw_add_batched,
+  // library default batch); smaller calls keep the host builder.  0 = off: every call takes the host builder.
+  static int64_t hnsw_device_build_min_rows;
 
  private:
   butil::Status AddOrUpsert(const std::vector<pb::common::VectorWithId>& vector_with_ids, bool is_upsert);

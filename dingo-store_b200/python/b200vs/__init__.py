@@ -31,6 +31,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_broadcast_state", "b200vs_shard_add", "b200vs_shard_add_device", "b200vs_shard_remove_ids", "b200vs_shard_plan_add_device",
     "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
+    "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit",
 ]
 
 
@@ -128,6 +129,8 @@ def lib():
     L.b200vs_search_binary.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_search_binary_device.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_range_search_binary.argtypes = [vp, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_hnsw_add_batched.argtypes = [vp, i64, vp, vp, i32]
+    L.b200vs_debug_hnsw_build_scratch_limit.argtypes = [vp, i64]
     _lib = L
     return L
 
@@ -238,6 +241,15 @@ class Index:
     def upsert(self, x, ids):
         self.add(x, ids, upsert=True)
 
+    def add_batched(self, x, ids, batch=0):
+        """HNSW Add / Upsert built on the GPU in batches of `batch` rows (0 = the library default; 1 = the host builder's graph)."""
+        x, ids = _f32(x), _i64(ids)
+        _check(self.L.b200vs_hnsw_add_batched(self.h, ids.size, x.ctypes.data if x.size else None, ids.ctypes.data if ids.size else None, int(batch)))
+
+    def set_build_scratch_limit(self, nbytes):
+        """Diagnostics: cap the device scratch of one add_batched call (0 = no cap); a call over it fails and changes nothing."""
+        _check(self.L.b200vs_debug_hnsw_build_scratch_limit(self.h, int(nbytes)))
+
     def add_device(self, n, x_dev_ptr, ids_dev_ptr, lists_dev_ptr=None, upsert=False):
         _check(self.L.b200vs_add_with_ids_device(self.h, n, x_dev_ptr, ids_dev_ptr, lists_dev_ptr, int(upsert)))
 
@@ -316,7 +328,8 @@ class Index:
         _check(self.L.b200vs_last_search_stats(self.h, ctypes.byref(a)))
         return list(a)
 
-    PHASES = ("coarse_prep", "coarse_scan", "coarse_final", "plan", "sample", "tau", "capture", "final", "fallback", "other", "comm", "merge")
+    PHASES = ("coarse_prep", "coarse_scan", "coarse_final", "plan", "sample", "tau", "capture", "final", "fallback", "other", "comm", "merge",
+              "build_search", "build_select", "build_link")
 
     def phase_times(self):
         """{phase: device ms} of the last search (profiling mode only)."""

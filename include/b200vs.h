@@ -102,6 +102,26 @@ int64_t b200vs_get_trained_state(b200vs_index* idx, void* blob, size_t cap); /* 
 int b200vs_add_with_ids(b200vs_index* idx, int64_t n, const float* x, const int64_t* ids, int upsert);
 int b200vs_remove_ids(b200vs_index* idx, int64_t n, const int64_t* ids, int64_t* n_removed);
 
+/* HNSW Add / Upsert with the graph built on the GPU in deterministic batches (DESIGN.md §4.4).  Host pointers; same semantics
+ * as b200vs_add_with_ids on an HNSW index: cosine rows are normalised, an id already present is replaced (its old node is
+ * tombstoned), an id repeated within the call is not refused and its last row wins.  Rows go in in call order; every row of a
+ * batch searches the graph as it was at the batch start and also links to the batch's earlier rows.  Batches hold
+ * min(batch, rows already in the graph) rows, so they grow 1, 1, 2, 4, ... from an empty index.
+ *   batch <= 0: the default, 2048 rows (measured at cfg4, DESIGN §4.4); larger values are capped at 8192.
+ *   batch == 1: the graph b200vs_add_with_ids builds with one writer, byte for byte (data without exact distance ties).
+ * Levels, entry point and max level always equal the host builder's.  Empty / null input and a non-HNSW index:
+ * EILLEGAL_PARAMETERS; more rows than max_elements: EINTERNAL "exceeds max elements".  efconstruction, dimension and batch
+ * must fit the kernels' 200 KB of shared memory (roughly efconstruction + batch <= 12800; efconstruction >= 1024 runs the
+ * search's candidate-heap form), else EILLEGAL_PARAMETERS.  Every refusal leaves the index unchanged, and so does a call that
+ * fails on the device (EINTERNAL, e.g. out of memory): the graph changes only once the whole call has run.  Takes the writer
+ * lock. */
+int b200vs_hnsw_add_batched(b200vs_index* idx, int64_t n, const float* x, const int64_t* ids, int32_t batch);
+/* Diagnostics (tests only): cap the device scratch one b200vs_hnsw_add_batched call of this index may allocate beyond the graph
+ * (bytes; 0 = no cap, the default).  A call that needs more fails with EINTERNAL, as on a device out of memory, at the
+ * allocation that crosses the cap (the peer matrix grows with the batches, so this can be mid-call, after earlier batches ran),
+ * and leaves the index as it was.  Non-HNSW index or bytes < 0: EILLEGAL_PARAMETERS. */
+int b200vs_debug_hnsw_build_scratch_limit(b200vs_index* idx, int64_t bytes);
+
 /* VectorIndex::Search — flat.cc:205-264, ivf_flat.cc:191-275, raw_ivf_pq.cc:157-210, hnsw.cc:318-485.
  * xq row-major [nq,dim] RAW; out_dist [nq,k], out_ids [nq,k]. */
 int b200vs_search(b200vs_index* idx, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
@@ -282,7 +302,8 @@ int b200vs_last_search_stats(b200vs_index* idx, int64_t stats[8]);
  * IVF tile path: [0] coarse prep, [1] coarse scan, [2] coarse select + exact re-score, [3] work planning + query
  * gather, [4] sample pass, [5] thresholds, [6] list scan (capture), [7] final select + exact re-score, [8] exact
  * fallback for uncertified queries, [9] other, [10] collectives of a sharded search (b200vs_shard_search*), [11] pack + merge of
- * the per-shard top-k.  Unused slots are 0. */
+ * the per-shard top-k.  After b200vs_hnsw_add_batched: [12] construction search, [13] peer distances + forward links,
+ * [14] reverse links, summed over the call's batches.  Unused slots are 0. */
 int b200vs_last_phase_times(b200vs_index* idx, float ms[16]);
 int b200vs_set_profiling(b200vs_index* idx, int on);
 
