@@ -12,10 +12,10 @@
 // (single writer, deterministic) with the hooked AVX-512 distance order, so a graph built here equals the graph
 // the CPU path builds from the same insertion order; the device holds a mirror that is refreshed lazily.
 //
-// Search kernel (hnsw_search_kernel): one warp per query.  Upper layers: greedy descent.  Base layer: the
-// reference's searchBaseLayerST loop — pop the closest candidate, gather its <= 2M neighbour rows, compute the
-// unvisited neighbours' distances as one batch (8 quads per warp, exact AVX-512 order, so the traversal is
-// identical to the CPU traversal), then apply the heap updates in neighbour order.
+// Search (hnsw_search_kernel) and batched construction (hnsw_build_search_kernel) share one device graph walk: one
+// 128-thread CTA per query or row; greedy descent through the upper levels, then the reference's searchBaseLayerST at one
+// level, whose hops score the <= 32 unvisited neighbours of a node together (32 quads, exact AVX-512 order, so the
+// traversal is the CPU traversal).  See "The walk of one CTA" below and DESIGN §4.4.
 #include <algorithm>
 #include <cmath>
 #include <queue>
@@ -255,27 +255,46 @@ struct HostGraph {
   }
 };
 
-// ---------------- device search ----------------
+// ---------------- device graph walk: search and batched construction ----------------
+// The device mirror of HostGraph's first n nodes.  The construction's link and reverse kernels write its link lists.
 struct HnswDev {
   const float* data;
   const long long* labels;
-  const unsigned int* link0;
+  unsigned int* link0;
   const long long* up_off;
-  const unsigned int* linkup;
+  unsigned int* linkup;
   const unsigned char* deleted;
   long long n;
-  int d, maxM, maxM0, maxlevel, l2;
+  int d, maxM, maxM0, maxlevel, efc;
   unsigned int enterpoint;
-  int has_deletions;
+  int has_deletions, M;
+  // HostGraph::ll: [size, link...] of a node at a level
+  __device__ __forceinline__ unsigned int* links(unsigned int node, int level) const {
+    return level == 0 ? link0 + (size_t)node * (maxM0 + 1) : linkup + up_off[node] + (size_t)(level - 1) * (maxM + 1);
+  }
 };
+
+// HostGraph::dist on the device: quad lane t's part of the exact AVX-512 order, then hnswlib's InnerProductDistance
+// (1 - ip) for IP and cosine
+template <bool L2>
+__device__ __forceinline__ float hnsw_distance(const float* x, const float* y, int d, int t, bool vec) {
+  const float v = quad_distance<L2>(x, y, d, t, vec);
+  return L2 ? v : __fsub_rn(1.0f, v);
+}
 
 constexpr int HNSW_THREADS = 128;   // one CTA per query: warp 0 walks the graph, all 32 quads score a hop's neighbours together
 constexpr int HNSW_CAND_SMEM = 1024; // candidate-heap entries kept in shared memory (the levels near the root); deeper ones spill to global
 // Heap form: the visited set admits every node to the candidate heap at most once, so n + 1 entries per query always
 // suffice.  When nq · (n + 1) entries exceed this budget the queries run in chunks of fewer CTAs.
 constexpr size_t HNSW_CAND_POOL_BYTES = 512ull << 20;
+constexpr size_t HNSW_SMEM_LIMIT = 200 * 1024;  // dynamic shared memory of every HNSW kernel
 
 struct HeapEnt { float d; unsigned int id; };
+
+// Dynamic shared memory of a walk kernel: the query (padded to 16 bytes), the result array or heap [ef + 1], then the
+// candidate heap's shared part [HNSW_CAND_SMEM], which the merged-array form uses as its second array.
+__host__ __device__ __forceinline__ size_t walk_qbytes(int d) { return ((size_t)d * 4 + 15) / 16 * 16; }
+size_t walk_smem_bytes(int d, int ef) { return walk_qbytes(d) + (size_t)(ef + 1) * sizeof(HeapEnt) + (size_t)HNSW_CAND_SMEM * sizeof(HeapEnt); }
 
 // Binary heap operated by ONE lane.  MAXH: largest distance on top.  Entries [0, nsm) live in shared memory, the rest in
 // global memory: a sift walks a root-to-leaf path, whose upper levels (the hot ones) are the shared part.
@@ -313,17 +332,232 @@ __device__ void h_pop(const HeapRef& h, int& n) {
   if (n > 0) h.set(i, last);
 }
 
-// One CTA (128 threads) per query.  Warp 0 runs hnswlib's control flow (greedy descent of the upper layers, then
-// searchBaseLayerST): it pops the closest candidate, reads its link list 32 neighbours at a time, keeps the unvisited ones in
-// list order; then ALL 32 quads of the CTA compute those rows' distances in one round (exact AVX-512 order, so the traversal
-// is the CPU traversal); lane 0 applies the heap updates in neighbour order.  Two block barriers per batch of <= 32 neighbours.
-// FAST (no id filter, no tombstones — every accepted neighbour enters both of hnswlib's queues): the two binary heaps collapse
-// into ONE ascending array T of the best <= ef nodes with an "expanded" flag per entry.  The next candidate is the first
-// unexpanded entry of T; a hop's <= 32 scored neighbours are merged into T by all 128 threads at once (each thread places one
-// old entry and at most one new one at its rank), instead of ~30 sift-up / sift-down sequences executed by a single lane at one
-// dependent instruction per ~25 ns — that lone-lane heap work was 80 % of a hop.  The visited set, the order in which nodes
-// are expanded and the returned ids / distances are those of searchBaseLayerST (exact-distance ties between different nodes,
-// which std::priority_queue orders by heap position, are the one place the two can differ).
+// The walk of one CTA (128 threads), shared by the search and the construction search.  Warp 0 runs hnswlib's control flow:
+// greedy descent of the upper levels, then a base walk at one level, which takes the next node to expand, reads its link
+// list 32 neighbours at a time and keeps the unvisited ones in list order; then ALL 32 quads of the CTA compute those rows'
+// distances in one round (exact AVX-512 order, so the traversal is the CPU traversal).  Two block barriers per batch of
+// <= 32 neighbours.  The base walk has two forms, which differ in how they pick the next node and take in a scored batch:
+// - merged array (FAST: no id filter, no tombstones, so every accepted neighbour enters both of hnswlib's queues): the two
+//   binary heaps collapse into ONE ascending array T of the best <= ef nodes with an "expanded" flag per entry.  The next
+//   node is the first unexpanded entry of T; a batch is merged into T by all 128 threads at once (each thread places one
+//   old entry and at most one new one at its rank), instead of ~30 sift-up / sift-down sequences executed by a single lane
+//   at one dependent instruction per ~25 ns — that lone-lane heap work was 80 % of a hop.
+// - two heaps (searchBaseLayerST): lane 0 pops the closest candidate and applies the heap updates in neighbour order; the
+//   candidate heap spills to global memory past HNSW_CAND_SMEM entries.
+// The visited set, the order in which nodes are expanded and the result are those of searchBaseLayerST in both forms
+// (exact-distance ties between different nodes, which std::priority_queue orders by heap position, are the one place the
+// merged array can differ).
+struct Cursor {  // warp 0: the node being expanded and how far into its link list the walk is
+  unsigned int node;
+  int size, c0;
+  bool expanding;
+};
+
+template <bool L2>
+struct Walk {
+  const HnswDev& g;
+  const float* qs;    // the query, in shared memory
+  unsigned int* vis;  // the visited bitset
+  float* s_d;         // [32] in shared memory: the distances of a scoring round
+  unsigned int* s_id; // [32] in shared memory: the nodes of a scoring round
+  int* s_m;           // in shared memory: rows to score this round; -1 = the walk is over
+  // g.d; this thread's quad and lane in it.  The two kernels spell the quad index (and the candidate heap's address) in
+  // different but equal ways: ptxas allocates registers differently for each spelling, and these are the ones that keep every
+  // instantiation of both kernels within its register allocation and free of new spills (DESIGN §4.4).
+  int d, quad, t;
+  bool vec;           // rows are 16-byte aligned
+
+  // distances of s_id[0, m) -> s_d[0, m): one row per quad, every thread of the CTA calls (m <= 32)
+  __device__ __forceinline__ void score(int m) const {
+    const float v = hnsw_distance<L2>(g.data + (size_t)s_id[quad < m ? quad : 0] * d, qs, d, t, vec);
+    if (quad < m && t == 0) s_d[quad] = v;
+  }
+  __device__ __forceinline__ float score_one(unsigned int node) const {
+    if (threadIdx.x == 0) s_id[0] = node;
+    __syncthreads();
+    score(1);
+    __syncthreads();
+    return s_d[0];
+  }
+  // Warp 0: the next <= 32 unvisited neighbours at `level` of the node being expanded, marked visited and packed in list
+  // order into s_id.  When the node's list is used up, next(node) picks the node to expand next, or returns false when the
+  // walk is over.  Returns the batch size, -1 when the walk is over.
+  template <class Next>
+  __device__ __forceinline__ int collect(Cursor& c, int level, Next& next) const {
+    const int lane = threadIdx.x & 31;
+    for (;;) {
+      if (!c.expanding) {
+        if (!next(c.node)) return -1;
+        c.size = (int)g.links(c.node, level)[0];
+        c.c0 = 0;
+        c.expanding = true;
+      }
+      if (c.c0 >= c.size) { c.expanding = false; continue; }
+      const unsigned int* l = g.links(c.node, level) + 1 + c.c0;
+      const int cnt = min(32, c.size - c.c0);
+      c.c0 += 32;
+      unsigned int nb = 0;
+      bool fresh = false;
+      if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
+      const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
+      if (fresh) {
+        atomicOr(&vis[nb >> 5], 1u << (nb & 31));
+        s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
+      }
+      const int m = __popc(mask);
+      if (m > 0) return m;
+    }
+  }
+  // One round of a base walk: warp 0 collects the next batch, the CTA scores it into s_d.  Returns its size (-1: the walk is
+  // over), the same on every thread.
+  template <class Next>
+  __device__ __forceinline__ int round(Cursor& c, int level, Next& next) const {
+    __syncthreads();  // (A) the walk's arrays complete, s_d / s_id of the previous round consumed
+    if ((threadIdx.x >> 5) == 0) {
+      const int m = collect(c, level, next);
+      if ((threadIdx.x & 31) == 0) *s_m = m;
+    }
+    __syncthreads();  // (B) s_id / s_m published
+    const int m = *s_m;
+    if (m >= 0) {
+      score(m);
+      __syncthreads();  // (C) s_d complete
+    }
+    return m;
+  }
+};
+
+// Greedy descent through the levels from_level down to stop_level + 1, moving from (cur, curdist) to any closer neighbour
+// until none is closer.  Every thread tracks the same state.
+template <bool L2>
+__device__ __forceinline__ void descend(const Walk<L2>& w, int from_level, int stop_level, unsigned int& cur, float& curdist) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int level = from_level; level > stop_level; --level) {
+    bool changed = true;
+    while (changed) {
+      changed = false;
+      __builtin_assume(level > 0);  // an upper level: links() needs no level-0 branch
+      const unsigned int* l = w.g.links(cur, level);
+      const int size = (int)l[0];
+      for (int c0 = 0; c0 < size; c0 += 32) {
+        const int m = min(32, size - c0);
+        __syncthreads();  // previous round's s_d / s_id fully consumed
+        if (warp == 0 && lane < m) w.s_id[lane] = l[1 + c0 + lane];
+        __syncthreads();
+        w.score(m);
+        __syncthreads();
+        for (int i = 0; i < m; ++i) {
+          const float dd = w.s_d[i];
+          if (dd < curdist) { curdist = dd; cur = w.s_id[i]; changed = true; }
+        }
+      }
+    }
+  }
+}
+
+// Base walk at `level`, merged-array form, from (cur, curdist) with capacity ef.  T (id bit 31 = expanded) and T2 are the
+// two buffers of the merge, [ef] each; on return T holds the ascending result and the return value is its length.
+template <bool L2>
+__device__ __forceinline__ int walk_merged(const Walk<L2>& w, int level, int ef, unsigned int cur, float curdist, HeapEnt*& T, HeapEnt* T2) {
+  const int lane = threadIdx.x & 31;
+  int ntop = 1;
+  if (threadIdx.x == 0) { T[0].d = curdist; T[0].id = cur; w.vis[cur >> 5] |= 1u << (cur & 31); }
+  auto next = [&](unsigned int& node) {  // first unexpanded entry = closest open candidate
+    int idx = -1;
+    for (int b0 = 0; b0 < ntop && idx < 0; b0 += 32) {
+      const int i = b0 + lane;
+      const bool open = i < ntop && (T[i].id >> 31) == 0u;
+      const unsigned msk = __ballot_sync(0xffffffffu, open);
+      if (msk) idx = b0 + __ffs(msk) - 1;
+    }
+    if (idx < 0) return false;
+    node = T[idx].id;
+    __syncwarp();
+    if (lane == 0) T[idx].id = node | 0x80000000u;
+    return true;
+  };
+  Cursor c{};
+  for (;;) {
+    const int m = w.round(c, level, next);
+    if (m < 0) break;
+    // merge the m scored neighbours into T (ascending, old entries first among equals), keep the best ef
+    for (int tix = threadIdx.x; tix < ntop; tix += HNSW_THREADS) {
+      const HeapEnt e = T[tix];
+      int cnt = 0;
+      for (int j = 0; j < m; ++j) cnt += w.s_d[j] < e.d ? 1 : 0;
+      if (tix + cnt < ef) T2[tix + cnt] = e;
+    }
+    if (threadIdx.x < m) {
+      const float dj = w.s_d[threadIdx.x];
+      int rank = 0;
+      for (int i = 0; i < m; ++i) rank += (w.s_d[i] < dj || (w.s_d[i] == dj && i < (int)threadIdx.x)) ? 1 : 0;
+      int lo = 0, hi = ntop;  // number of old entries with d <= dj
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (T[mid].d <= dj) lo = mid + 1; else hi = mid; }
+      if (rank + lo < ef) { HeapEnt e; e.d = dj; e.id = w.s_id[threadIdx.x]; T2[rank + lo] = e; }
+    }
+    ntop = min(ef, ntop + m);
+    HeapEnt* tmp = T; T = T2; T2 = tmp;
+  }
+  __syncthreads();
+  return ntop;
+}
+
+// Base walk at `level`, two-heap form, from (cur, curdist) with capacity ef: top = the result max-heap [ef + 1], cand = the
+// candidate min-heap.  allowed(node): the node may enter the result (else it is only traversed).  strict_stop: the walk
+// stops at a candidate farther than the result only once the result holds ef nodes.  Returns the size of top on thread 0.
+template <bool L2, class Allowed>
+__device__ __forceinline__ int walk_heaps(const Walk<L2>& w, int level, int ef, bool strict_stop, Allowed allowed, unsigned int cur,
+                                          float curdist, const HeapRef& top, const HeapRef& cand) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int ntop = 0, ncand = 0;
+  float lower = 3.402823466e+38f;
+  if (warp == 0) {
+    const bool ok = allowed(cur);
+    if (lane == 0) {
+      if (ok) { h_push<true>(top, ntop, curdist, cur); h_push<false>(cand, ncand, curdist, cur); }
+      else h_push<false>(cand, ncand, 3.402823466e+38f, cur);
+      w.vis[cur >> 5] |= 1u << (cur & 31);
+    }
+    lower = ok ? curdist : 3.402823466e+38f;
+  }
+  auto next = [&](unsigned int& node) {  // pop the closest candidate unless the walk stops here
+    int go = 0;
+    if (lane == 0 && ncand > 0) {
+      const HeapEnt ce = cand.get(0);
+      const bool stop = ce.d > lower && (ntop == ef || !strict_stop);
+      if (!stop) { node = ce.id; h_pop<false>(cand, ncand); go = 1; }
+    }
+    go = __shfl_sync(0xffffffffu, go, 0);
+    if (!go) return false;
+    node = __shfl_sync(0xffffffffu, node, 0);
+    return true;
+  };
+  Cursor c{};
+  for (;;) {
+    const int m = w.round(c, level, next);
+    if (m < 0) break;
+    if (warp == 0) {
+      const unsigned int amask = __ballot_sync(0xffffffffu, lane < m && allowed(w.s_id[lane]));
+      if (lane == 0) {
+        for (int i = 0; i < m; ++i) {
+          const float dd = w.s_d[i];
+          if (ntop < ef || lower > dd) {
+            h_push<false>(cand, ncand, dd, w.s_id[i]);  // fresh nodes only: ncand <= n < the pool's n + 1 entries
+            if ((amask >> i) & 1u) h_push<true>(top, ntop, dd, w.s_id[i]);
+            if (ntop > ef) h_pop<true>(top, ntop);
+            if (ntop > 0) lower = top.get(0).d;
+          }
+        }
+      }
+      lower = __shfl_sync(0xffffffffu, lower, 0);
+    }
+  }
+  return ntop;
+}
+
+// Search: one CTA per query.  Descent to level 0 from the entry point, then the base walk with ef: the merged-array form
+// when FAST, else the two heaps with the id filter and tombstones as the "allowed" test and hnswlib's strict stop rule
+// whenever anything is filtered out.  Emits the k best ascending by (distance, label).
 template <bool L2, bool FAST>
 __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev g, const float* __restrict__ queries, long long nq,
                                                                   int k, int ef, FilterDev filt, unsigned int* visited /*[nq, words]*/,
@@ -332,135 +566,25 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ float s_d[32];
   __shared__ unsigned int s_id[32];
-  __shared__ int s_m;  // rows to score this round; -1 = the walk is over
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ int s_m;
   const long long qi = blockIdx.x;
   const int d = g.d;
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
   float* qs = reinterpret_cast<float*>(smem);
-  HeapEnt* top_sm = reinterpret_cast<HeapEnt*>(smem + qbytes);                                   // [ef + 1]
-  HeapEnt* cand_sm = reinterpret_cast<HeapEnt*>(smem + qbytes + (size_t)(ef + 1) * sizeof(HeapEnt));  // [HNSW_CAND_SMEM]
+  HeapEnt* top_sm = reinterpret_cast<HeapEnt*>(smem + walk_qbytes(d));                                      // [ef + 1]
+  HeapEnt* cand_sm = reinterpret_cast<HeapEnt*>(smem + walk_qbytes(d) + (size_t)(ef + 1) * sizeof(HeapEnt));  // [HNSW_CAND_SMEM]
   for (int i = threadIdx.x; i < d; i += HNSW_THREADS) qs[i] = queries[(size_t)qi * d + i];
   if (g.n == 0) {
     for (int i = threadIdx.x; i < k; i += HNSW_THREADS) { out_dist[(size_t)qi * k + i] = 0.f; out_ids[(size_t)qi * k + i] = -1; }
     return;
   }
   __syncthreads();
-  const bool vec = (d & 3) == 0;
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  unsigned int* vis = visited + (size_t)qi * words;
-  const HeapRef top{top_sm, top_sm, ef + 1};
-  const HeapRef cand{cand_sm, cand_pool + (size_t)qi * cand_cap, HNSW_CAND_SMEM};
-  const bool filtered = filt.has_range || filt.sorted_ids != nullptr;
-  const bool strict_stop = filtered || g.has_deletions;
-
-  // distances of s_id[0..m) -> s_d[0..m): one row per quad, every thread of the CTA calls (m <= 32)
-  auto score = [&](int m) {
-    const unsigned int row = s_id[quad < m ? quad : 0];
-    float v = quad_distance<L2>(g.data + (size_t)row * d, qs, d, t, vec);
-    if (!L2) v = __fsub_rn(1.0f, v);  // hnswlib InnerProductDistance
-    if (quad < m && t == 0) s_d[quad] = v;
-  };
-
-  // ---- entry point ----
+  const Walk<L2> w{g, qs, visited + (size_t)qi * words, s_d, s_id, &s_m, d, (int)threadIdx.x >> 2, (int)threadIdx.x & 3, (d & 3) == 0};
   unsigned int cur = g.enterpoint;
-  if (threadIdx.x == 0) s_id[0] = cur;
-  __syncthreads();
-  score(1);
-  __syncthreads();
-  float curdist = s_d[0];
-  // ---- upper layers: greedy descent (every thread tracks the same state) ----
-  for (int level = g.maxlevel; level > 0; --level) {
-    bool changed = true;
-    while (changed) {
-      changed = false;
-      const unsigned int* l = g.linkup + g.up_off[cur] + (size_t)(level - 1) * (g.maxM + 1);
-      const int size = (int)l[0];
-      for (int c0 = 0; c0 < size; c0 += 32) {
-        const int m = min(32, size - c0);
-        __syncthreads();  // previous round's s_d / s_id fully consumed
-        if (warp == 0 && lane < m) s_id[lane] = l[1 + c0 + lane];
-        __syncthreads();
-        score(m);
-        __syncthreads();
-        for (int i = 0; i < m; ++i) {
-          const float dd = s_d[i];
-          if (dd < curdist) { curdist = dd; cur = s_id[i]; changed = true; }
-        }
-      }
-    }
-  }
+  float curdist = w.score_one(cur);
+  descend(w, g.maxlevel, 0, cur, curdist);
   if (FAST) {
-    // ---- base layer, merged-array form.  T = cand_sm region reused: [2][ef] entries (id bit 31 = expanded) ----
-    HeapEnt* T = top_sm;            // [ef + 1]
-    HeapEnt* T2 = cand_sm;          // [>= ef + 1] (HNSW_CAND_SMEM >= ef + 1 is checked on the host)
-    int ntop = 1;
-    if (threadIdx.x == 0) { T[0].d = curdist; T[0].id = cur; vis[cur >> 5] |= 1u << (cur & 31); }
-    unsigned int node = 0;
-    int size = 0, c0 = 0;
-    bool expanding = false;
-    for (;;) {
-      __syncthreads();  // (A) T complete, s_d / s_id of the previous round consumed
-      if (warp == 0) {
-        int m = -1;
-        for (;;) {
-          if (!expanding) {
-            int idx = -1;
-            for (int b0 = 0; b0 < ntop && idx < 0; b0 += 32) {  // first unexpanded entry = closest open candidate
-              const int i = b0 + lane;
-              const bool open = i < ntop && (T[i].id >> 31) == 0u;
-              const unsigned msk = __ballot_sync(0xffffffffu, open);
-              if (msk) idx = b0 + __ffs(msk) - 1;
-            }
-            if (idx < 0) { m = -1; break; }
-            node = T[idx].id;
-            __syncwarp();
-            if (lane == 0) T[idx].id = node | 0x80000000u;
-            size = (int)g.link0[(size_t)node * (g.maxM0 + 1)];
-            c0 = 0;
-            expanding = true;
-          }
-          if (c0 >= size) { expanding = false; continue; }
-          const unsigned int* l = g.link0 + (size_t)node * (g.maxM0 + 1) + 1 + c0;
-          const int cnt = min(32, size - c0);
-          c0 += 32;
-          unsigned int nb = 0;
-          bool fresh = false;
-          if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
-          const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
-          if (fresh) {
-            atomicOr(&vis[nb >> 5], 1u << (nb & 31));
-            s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
-          }
-          m = __popc(mask);
-          if (m > 0) break;
-        }
-        if (lane == 0) s_m = m;
-      }
-      __syncthreads();  // (B)
-      const int m = s_m;
-      if (m < 0) break;
-      score(m);
-      __syncthreads();  // (C) s_d complete
-      // merge the m scored neighbours into T (ascending, old entries first among equals), keep the best ef
-      for (int tix = threadIdx.x; tix < ntop; tix += HNSW_THREADS) {
-        const HeapEnt e = T[tix];
-        int c = 0;
-        for (int j = 0; j < m; ++j) c += s_d[j] < e.d ? 1 : 0;
-        if (tix + c < ef) T2[tix + c] = e;
-      }
-      if (threadIdx.x < m) {
-        const float dj = s_d[threadIdx.x];
-        int rank = 0;
-        for (int i = 0; i < m; ++i) rank += (s_d[i] < dj || (s_d[i] == dj && i < (int)threadIdx.x)) ? 1 : 0;
-        int lo = 0, hi = ntop;  // number of old entries with d <= dj
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (T[mid].d <= dj) lo = mid + 1; else hi = mid; }
-        if (rank + lo < ef) { HeapEnt e; e.d = dj; e.id = s_id[threadIdx.x]; T2[rank + lo] = e; }
-      }
-      ntop = min(ef, ntop + m);
-      HeapEnt* tmp = T; T = T2; T2 = tmp;
-    }
-    __syncthreads();
+    HeapEnt* T = top_sm;
+    const int ntop = walk_merged(w, 0, ef, cur, curdist, T, cand_sm);  // HNSW_CAND_SMEM >= ef + 1 is checked on the host
     if (threadIdx.x == 0) {  // emit the k best ascending by (distance, label)
       const int have = min(ntop, k);
       for (int i = 0; i < have; ++i) {
@@ -475,82 +599,11 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
     }
     return;
   }
-  // ---- base layer: searchBaseLayerST ----
-  int ntop = 0, ncand = 0;
-  float lower = 3.402823466e+38f;
-  if (warp == 0) {
-    const long long lab = g.labels[cur];
-    const bool ok = !g.deleted[cur] && filter_pass(filt, lab);
-    if (lane == 0) {
-      if (ok) { h_push<true>(top, ntop, curdist, cur); h_push<false>(cand, ncand, curdist, cur); }
-      else h_push<false>(cand, ncand, 3.402823466e+38f, cur);
-      vis[cur >> 5] |= 1u << (cur & 31);
-    }
-    lower = ok ? curdist : 3.402823466e+38f;
-  }
-  // warp 0 state that survives across rounds: the node being expanded and how far into its link list we are
-  unsigned int node = 0;
-  int size = 0, c0 = 0;
-  bool expanding = false;
-  for (;;) {
-    __syncthreads();  // (A) s_d / s_id of the previous round consumed by everyone
-    if (warp == 0) {
-      int m = -1;
-      for (;;) {  // find the next non-empty batch of unvisited neighbours
-        if (!expanding) {
-          int go = 0;
-          if (lane == 0 && ncand > 0) {
-            const HeapEnt ce = cand.get(0);
-            const bool stop = ce.d > lower && (ntop == ef || !strict_stop);
-            if (!stop) { node = ce.id; h_pop<false>(cand, ncand); go = 1; }
-          }
-          go = __shfl_sync(0xffffffffu, go, 0);
-          if (!go) { m = -1; break; }
-          node = __shfl_sync(0xffffffffu, node, 0);
-          size = (int)g.link0[(size_t)node * (g.maxM0 + 1)];
-          c0 = 0;
-          expanding = true;
-        }
-        if (c0 >= size) { expanding = false; continue; }
-        const unsigned int* l = g.link0 + (size_t)node * (g.maxM0 + 1) + 1 + c0;
-        const int cnt = min(32, size - c0);
-        c0 += 32;
-        unsigned int nb = 0;
-        bool fresh = false;
-        if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
-        const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
-        if (fresh) {
-          atomicOr(&vis[nb >> 5], 1u << (nb & 31));
-          s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
-        }
-        m = __popc(mask);
-        if (m > 0) break;
-      }
-      if (lane == 0) s_m = m;
-    }
-    __syncthreads();  // (B) s_id / s_m published
-    const int m = s_m;
-    if (m < 0) break;
-    score(m);
-    __syncthreads();  // (C) s_d complete
-    if (warp == 0) {
-      bool allowed = false;
-      if (lane < m) { const unsigned int c = s_id[lane]; allowed = !g.deleted[c] && filter_pass(filt, g.labels[c]); }
-      const unsigned int amask = __ballot_sync(0xffffffffu, allowed);
-      if (lane == 0) {
-        for (int i = 0; i < m; ++i) {
-          const float dd = s_d[i];
-          if (ntop < ef || lower > dd) {
-            h_push<false>(cand, ncand, dd, s_id[i]);  // fresh nodes only: ncand <= n < cand_cap
-            if ((amask >> i) & 1u) h_push<true>(top, ntop, dd, s_id[i]);
-            if (ntop > ef) h_pop<true>(top, ntop);
-            if (ntop > 0) lower = top.get(0).d;
-          }
-        }
-      }
-      lower = __shfl_sync(0xffffffffu, lower, 0);
-    }
-  }
+  const HeapRef top{top_sm, top_sm, ef + 1};
+  const HeapRef cand{cand_sm, cand_pool + (size_t)qi * cand_cap, HNSW_CAND_SMEM};
+  const bool strict_stop = filt.has_range || filt.sorted_ids != nullptr || g.has_deletions;
+  int ntop = walk_heaps(w, 0, ef, strict_stop, [&](unsigned int c) { return !g.deleted[c] && filter_pass(filt, g.labels[c]); },
+                        cur, curdist, top, cand);
   if (threadIdx.x == 0) {
     // keep the k best, emit ascending by (distance, label)
     while (ntop > k) h_pop<true>(top, ntop);
@@ -575,18 +628,6 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_search_kernel(const HnswDev
 // insertion index and nothing depends on thread timing.
 constexpr int HNSW_BUILD_MAX_BATCH = 8192;  // rows per batch (the peer matrix is batch^2 floats)
 constexpr int HNSW_BUILD_DEFAULT_BATCH = 2048;
-constexpr size_t HNSW_BUILD_SMEM = 200 * 1024;
-
-struct HnswBuildDev {  // the device mirror as the link kernels write it
-  const float* data;
-  unsigned int* link0;
-  const long long* up_off;
-  unsigned int* linkup;
-  int d, M, maxM, maxM0, efc;
-  __device__ __forceinline__ unsigned int* links(unsigned int node, int level) const {
-    return level == 0 ? link0 + (size_t)node * (maxM0 + 1) : linkup + up_off[node] + (size_t)(level - 1) * (maxM + 1);
-  }
-};
 
 __device__ __forceinline__ unsigned long long cand_key(float d, unsigned int id) { return ((unsigned long long)f2ord(d) << 32) | id; }
 
@@ -626,8 +667,7 @@ __device__ int heuristic_select(const unsigned long long* C, int c, int lim, uns
     bool bad = false;
     for (int s0 = 0; s0 < nsel; s0 += 32) {
       const int s = s0 + quad;
-      float v = quad_distance<L2>(data + (size_t)sel[s < nsel ? s : 0] * d, data + (size_t)cand * d, d, t, vec);
-      if (!L2) v = __fsub_rn(1.0f, v);
+      const float v = hnsw_distance<L2>(data + (size_t)sel[s < nsel ? s : 0] * d, data + (size_t)cand * d, d, t, vec);
       if (s < nsel && v < dq) bad = true;
     }
     if (!__syncthreads_or(bad)) {
@@ -639,147 +679,43 @@ __device__ int heuristic_select(const unsigned long long* C, int c, int lim, uns
   return nsel;
 }
 
-// Construction search: one CTA per batch row.  Greedy descent from the entry point through the levels above the row's own,
-// then HostGraph::search_layer with ef = efc at every level from min(level, maxlevel) down to 0, each starting from the
-// closest node found one level up.  out[(slot_off[r] + l) * efc ...] = the result at level l, ascending by (distance, node);
-// out_cnt = its length.  FAST = no tombstones and efc + 1 <= HNSW_CAND_SMEM: the merged-array form of hnsw_search_kernel;
-// otherwise the two heaps, the candidate heap spilling to cand_pool.  The visited bitset is cleared per level.
+// Construction search: one CTA per batch row r, whose vector is node g.n + r.  Greedy descent from the entry point through
+// the levels above the row's own, then HostGraph::search_layer with ef = efc at every level from min(level, maxlevel) down to
+// 0, each starting from the closest node found one level up.  out[(slot_off[r] + l) * efc ...] = the result at level l,
+// ascending by (distance, node); out_cnt = its length.  FAST = no tombstones and efc + 1 <= HNSW_CAND_SMEM: the merged-array
+// form; otherwise the two heaps with tombstones as the "allowed" test and the strict stop rule.  The visited bitset is
+// cleared per level.
 template <bool L2, bool FAST>
-__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_search_kernel(const HnswDev g, int efc, const int* __restrict__ levels, long long row0,
-                                                                        long long n0, const long long* __restrict__ slot_off,
-                                                                        unsigned int* visited, long long words, HeapEnt* cand_pool,
-                                                                        long long cand_cap, HeapEnt* out, int* out_cnt) {
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_search_kernel(const HnswDev g, const int* __restrict__ levels, long long row0,
+                                                                        const long long* __restrict__ slot_off, unsigned int* visited,
+                                                                        long long words, HeapEnt* cand_pool, long long cand_cap, HeapEnt* out,
+                                                                        int* out_cnt) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ float s_d[32];
   __shared__ unsigned int s_id[32];
   __shared__ int s_m;
   __shared__ unsigned int s_cur;
   __shared__ float s_curdist;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long r = row0 + blockIdx.x;
-  const int d = g.d;
-  const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
+  const int d = g.d, efc = g.efc;
   float* qs = reinterpret_cast<float*>(smem);
-  HeapEnt* top_sm = reinterpret_cast<HeapEnt*>(smem + qbytes);
-  HeapEnt* cand_sm = reinterpret_cast<HeapEnt*>(smem + qbytes + (size_t)(efc + 1) * sizeof(HeapEnt));
-  for (int i = threadIdx.x; i < d; i += HNSW_THREADS) qs[i] = g.data[(size_t)(n0 + r) * d + i];
+  HeapEnt* top_sm = reinterpret_cast<HeapEnt*>(smem + walk_qbytes(d));
+  HeapEnt* cand_sm = top_sm + efc + 1;
+  for (int i = threadIdx.x; i < d; i += HNSW_THREADS) qs[i] = g.data[(size_t)(g.n + r) * d + i];
   __syncthreads();
-  const bool vec = (d & 3) == 0;
-  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
-  unsigned int* vis = visited + (size_t)blockIdx.x * words;
+  const Walk<L2> w{g, qs, visited + (size_t)blockIdx.x * words, s_d, s_id, &s_m, d, (int)(threadIdx.x >> 2), (int)(threadIdx.x & 3), (d & 3) == 0};
   const int lev = levels[r];
-  const int top_level = min(lev, g.maxlevel);
-  auto score = [&](int m) {
-    const unsigned int row = s_id[quad < m ? quad : 0];
-    float v = quad_distance<L2>(g.data + (size_t)row * d, qs, d, t, vec);
-    if (!L2) v = __fsub_rn(1.0f, v);
-    if (quad < m && t == 0) s_d[quad] = v;
-  };
-  auto links = [&](unsigned int node, int level) -> const unsigned int* {
-    return level == 0 ? g.link0 + (size_t)node * (g.maxM0 + 1) : g.linkup + g.up_off[node] + (size_t)(level - 1) * (g.maxM + 1);
-  };
-
   unsigned int cur = g.enterpoint;
-  if (threadIdx.x == 0) s_id[0] = cur;
-  __syncthreads();
-  score(1);
-  __syncthreads();
-  float curdist = s_d[0];
-  for (int level = g.maxlevel; level > lev; --level) {  // greedy descent (add_point: only when the row's level is below maxlevel)
-    bool changed = true;
-    while (changed) {
-      changed = false;
-      const unsigned int* l = links(cur, level);
-      const int size = (int)l[0];
-      for (int c0 = 0; c0 < size; c0 += 32) {
-        const int m = min(32, size - c0);
-        __syncthreads();
-        if (warp == 0 && lane < m) s_id[lane] = l[1 + c0 + lane];
-        __syncthreads();
-        score(m);
-        __syncthreads();
-        for (int i = 0; i < m; ++i) {
-          const float dd = s_d[i];
-          if (dd < curdist) { curdist = dd; cur = s_id[i]; changed = true; }
-        }
-      }
-    }
-  }
-
-  for (int level = top_level; level >= 0; --level) {
+  float curdist = w.score_one(cur);
+  descend(w, g.maxlevel, lev, cur, curdist);  // (add_point: only when the row's level is below maxlevel)
+  for (int level = min(lev, g.maxlevel); level >= 0; --level) {
     __syncthreads();
-    for (long long w = threadIdx.x; w < words; w += HNSW_THREADS) vis[w] = 0u;
+    for (long long x = threadIdx.x; x < words; x += HNSW_THREADS) w.vis[x] = 0u;
     __syncthreads();
     HeapEnt* res = out + (size_t)(slot_off[r] + level) * efc;
     if (FAST) {
       HeapEnt* T = top_sm;
-      HeapEnt* T2 = cand_sm;
-      int ntop = 1;
-      if (threadIdx.x == 0) { T[0].d = curdist; T[0].id = cur; vis[cur >> 5] |= 1u << (cur & 31); }
-      unsigned int node = 0;
-      int size = 0, c0 = 0;
-      bool expanding = false;
-      for (;;) {
-        __syncthreads();
-        if (warp == 0) {
-          int m = -1;
-          for (;;) {
-            if (!expanding) {
-              int idx = -1;
-              for (int b0 = 0; b0 < ntop && idx < 0; b0 += 32) {
-                const int i = b0 + lane;
-                const bool open = i < ntop && (T[i].id >> 31) == 0u;
-                const unsigned msk = __ballot_sync(0xffffffffu, open);
-                if (msk) idx = b0 + __ffs(msk) - 1;
-              }
-              if (idx < 0) { m = -1; break; }
-              node = T[idx].id;
-              __syncwarp();
-              if (lane == 0) T[idx].id = node | 0x80000000u;
-              size = (int)links(node, level)[0];
-              c0 = 0;
-              expanding = true;
-            }
-            if (c0 >= size) { expanding = false; continue; }
-            const unsigned int* l = links(node, level) + 1 + c0;
-            const int cnt = min(32, size - c0);
-            c0 += 32;
-            unsigned int nb = 0;
-            bool fresh = false;
-            if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
-            const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
-            if (fresh) {
-              atomicOr(&vis[nb >> 5], 1u << (nb & 31));
-              s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
-            }
-            m = __popc(mask);
-            if (m > 0) break;
-          }
-          if (lane == 0) s_m = m;
-        }
-        __syncthreads();
-        const int m = s_m;
-        if (m < 0) break;
-        score(m);
-        __syncthreads();
-        for (int tix = threadIdx.x; tix < ntop; tix += HNSW_THREADS) {
-          const HeapEnt e = T[tix];
-          int c = 0;
-          for (int j = 0; j < m; ++j) c += s_d[j] < e.d ? 1 : 0;
-          if (tix + c < efc) T2[tix + c] = e;
-        }
-        if (threadIdx.x < m) {
-          const float dj = s_d[threadIdx.x];
-          int rank = 0;
-          for (int i = 0; i < m; ++i) rank += (s_d[i] < dj || (s_d[i] == dj && i < (int)threadIdx.x)) ? 1 : 0;
-          int lo = 0, hi = ntop;
-          while (lo < hi) { const int mid = (lo + hi) >> 1; if (T[mid].d <= dj) lo = mid + 1; else hi = mid; }
-          if (rank + lo < efc) { HeapEnt e; e.d = dj; e.id = s_id[threadIdx.x]; T2[rank + lo] = e; }
-        }
-        ntop = min(efc, ntop + m);
-        HeapEnt* tmp = T; T = T2; T2 = tmp;
-      }
-      __syncthreads();
+      const int ntop = walk_merged(w, level, efc, cur, curdist, T, cand_sm);
       if (threadIdx.x == 0) {  // T is ascending in distance; equal distances go by node id
         for (int i = 0; i < ntop; ++i) {
           HeapEnt e = T[i];
@@ -794,78 +730,7 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_search_kernel(const H
     } else {
       const HeapRef top{top_sm, top_sm, efc + 1};
       const HeapRef cand{cand_sm, cand_pool + (size_t)blockIdx.x * cand_cap, HNSW_CAND_SMEM};
-      int ntop = 0, ncand = 0;
-      float lower = 3.402823466e+38f;
-      if (warp == 0) {
-        const bool ok = !g.deleted[cur];
-        if (lane == 0) {
-          if (ok) { h_push<true>(top, ntop, curdist, cur); h_push<false>(cand, ncand, curdist, cur); }
-          else h_push<false>(cand, ncand, 3.402823466e+38f, cur);
-          vis[cur >> 5] |= 1u << (cur & 31);
-        }
-        lower = ok ? curdist : 3.402823466e+38f;
-      }
-      unsigned int node = 0;
-      int size = 0, c0 = 0;
-      bool expanding = false;
-      for (;;) {
-        __syncthreads();
-        if (warp == 0) {
-          int m = -1;
-          for (;;) {
-            if (!expanding) {
-              int go = 0;
-              if (lane == 0 && ncand > 0) {
-                const HeapEnt ce = cand.get(0);
-                if (!(ce.d > lower && ntop == efc)) { node = ce.id; h_pop<false>(cand, ncand); go = 1; }
-              }
-              go = __shfl_sync(0xffffffffu, go, 0);
-              if (!go) { m = -1; break; }
-              node = __shfl_sync(0xffffffffu, node, 0);
-              size = (int)links(node, level)[0];
-              c0 = 0;
-              expanding = true;
-            }
-            if (c0 >= size) { expanding = false; continue; }
-            const unsigned int* l = links(node, level) + 1 + c0;
-            const int cnt = min(32, size - c0);
-            c0 += 32;
-            unsigned int nb = 0;
-            bool fresh = false;
-            if (lane < cnt) { nb = l[lane]; fresh = ((vis[nb >> 5] >> (nb & 31)) & 1u) == 0u; }
-            const unsigned int mask = __ballot_sync(0xffffffffu, fresh);
-            if (fresh) {
-              atomicOr(&vis[nb >> 5], 1u << (nb & 31));
-              s_id[__popc(mask & ((1u << lane) - 1u))] = nb;
-            }
-            m = __popc(mask);
-            if (m > 0) break;
-          }
-          if (lane == 0) s_m = m;
-        }
-        __syncthreads();
-        const int m = s_m;
-        if (m < 0) break;
-        score(m);
-        __syncthreads();
-        if (warp == 0) {
-          bool allowed = false;
-          if (lane < m) allowed = !g.deleted[s_id[lane]];
-          const unsigned int amask = __ballot_sync(0xffffffffu, allowed);
-          if (lane == 0) {
-            for (int i = 0; i < m; ++i) {
-              const float dd = s_d[i];
-              if (ntop < efc || lower > dd) {
-                h_push<false>(cand, ncand, dd, s_id[i]);
-                if ((amask >> i) & 1u) h_push<true>(top, ntop, dd, s_id[i]);
-                if (ntop > efc) h_pop<true>(top, ntop);
-                if (ntop > 0) lower = top.get(0).d;
-              }
-            }
-          }
-          lower = __shfl_sync(0xffffffffu, lower, 0);
-        }
-      }
+      int ntop = walk_heaps(w, level, efc, true, [&](unsigned int c) { return !g.deleted[c]; }, cur, curdist, top, cand);
       if (threadIdx.x == 0) {
         const int cnt = ntop;
         while (ntop > 0) { const HeapEnt e = top.get(0); h_pop<true>(top, ntop); res[ntop] = e; }  // largest first -> ascending
@@ -887,7 +752,7 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_search_kernel(const H
 }
 
 // Peer distances of a batch: peer[i * nb + j] for j < i only (the link kernel reads no other entry), one quad per pair, in
-// pair_distance_kernel's arithmetic (quad_distance, 1 - ip for IP and cosine).
+// pair_distance_kernel's arithmetic (hnsw_distance).
 template <bool L2>
 __global__ void __launch_bounds__(256) hnsw_peer_distance_kernel(const float* __restrict__ rows, int nb, int d, float* __restrict__ peer) {
   const long long pair = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
@@ -899,8 +764,7 @@ __global__ void __launch_bounds__(256) hnsw_peer_distance_kernel(const float* __
   while (i * (i - 1) / 2 > p) --i;
   while ((i + 1) * i / 2 <= p) ++i;
   const long long j = p - i * (i - 1) / 2;
-  float v = quad_distance<L2>(rows + (size_t)i * d, rows + (size_t)j * d, d, t, (d & 3) == 0);
-  if (!L2) v = __fsub_rn(1.0f, v);
+  const float v = hnsw_distance<L2>(rows + (size_t)i * d, rows + (size_t)j * d, d, t, (d & 3) == 0);
   if (valid && t == 0) peer[(size_t)i * nb + j] = v;
 }
 
@@ -915,7 +779,7 @@ __global__ void hnsw_tombstone_kernel(unsigned char* deleted, const unsigned int
 // farthest first, as HostGraph::connect writes it.  Each kept target t emits the reverse-link key (level, t, i) into
 // trip[task * M + s]; unused slots hold ~0.
 template <bool L2>
-__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_link_kernel(const HnswBuildDev b, long long n0, int nb, const int* __restrict__ levels,
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_link_kernel(const HnswDev b, long long n0, int nb, const int* __restrict__ levels,
                                                                       int maxlevel, const float* __restrict__ peer, const long long* __restrict__ slot_off,
                                                                       const HeapEnt* __restrict__ sres, const int* __restrict__ scnt,
                                                                       const int2* __restrict__ tasks, unsigned long long* trip) {
@@ -967,7 +831,7 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_link_kernel(const Hns
 // key appends the sources when they fit into the target's list, and otherwise rewrites the list as heuristic(list ∪ sources,
 // Mmax) farthest first (connect's shrink).  Entries past the new size keep their old values, as in connect.
 template <bool L2>
-__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_reverse_kernel(const HnswBuildDev b, long long n0, const unsigned long long* __restrict__ keys,
+__global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_reverse_kernel(const HnswDev b, long long n0, const unsigned long long* __restrict__ keys,
                                                                          long long total) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ int s_ns;
@@ -1004,14 +868,28 @@ __global__ void __launch_bounds__(HNSW_THREADS) hnsw_build_reverse_kernel(const 
   for (int c0 = 0; c0 < p2; c0 += 32) {
     const int x = c0 + quad;
     const unsigned int id = x < sz ? list[1 + x] : x < c ? source(x - sz) : tgt;
-    float v = quad_distance<L2>(b.data + (size_t)id * b.d, b.data + (size_t)tgt * b.d, b.d, t, vec);
-    if (!L2) v = __fsub_rn(1.0f, v);
+    const float v = hnsw_distance<L2>(b.data + (size_t)id * b.d, b.data + (size_t)tgt * b.d, b.d, t, vec);
     if (t == 0 && x < p2) cand[x] = x < c ? cand_key(v, id) : ~0ull;
   }
   bitonic_sort(cand, p2);
   const int nsel = heuristic_select<L2>(cand, c, mcur, sel, b.data, b.d);
   for (int s = threadIdx.x; s < nsel; s += HNSW_THREADS) list[1 + s] = sel[nsel - 1 - s];
   if (threadIdx.x == 0) list[0] = (unsigned int)nsel;
+}
+
+// NormalizeVectorForHnsw (vector_index_utils.cc:493-500): the row cosine stores and searches, o = x / (|x| + 1e-30)
+void normalize_for_hnsw(const float* x, int d, float* o) {
+  float norm = 0.0f;
+  for (int j = 0; j < d; ++j) norm += x[j] * x[j];
+  norm = 1.0f / (sqrtf(norm) + 1e-30f);
+  for (int j = 0; j < d; ++j) o[j] = x[j] * norm;
+}
+
+// f(L2, FAST), both as std::integral_constant: the one place a walk kernel's instantiation is chosen
+template <class F>
+void dispatch_walk(bool l2, bool fast, F&& f) {
+  if (l2) { if (fast) f(std::true_type(), std::true_type()); else f(std::true_type(), std::false_type()); }
+  else { if (fast) f(std::false_type(), std::true_type()); else f(std::false_type(), std::false_type()); }
 }
 
 }  // namespace
@@ -1026,6 +904,15 @@ struct HnswIndex : IndexBase {
   DevBuf<long long> d_labels, d_upoff;
   DevBuf<unsigned int> d_link0, d_linkup;
   DevBuf<unsigned char> d_deleted;
+
+  // the device mirror as the kernels see it: its first n nodes, entered at ep on level maxlevel
+  HnswDev dev_graph(long long n, int maxlevel, tableint ep, bool deletions) const {
+    HnswDev g;
+    g.data = d_data.p; g.labels = d_labels.p; g.link0 = d_link0.p; g.up_off = d_upoff.p; g.linkup = d_linkup.p; g.deleted = d_deleted.p;
+    g.n = n; g.d = dim; g.M = (int)G.M; g.maxM = (int)G.maxM; g.maxM0 = (int)G.maxM0; g.efc = (int)G.efc;
+    g.maxlevel = maxlevel; g.enterpoint = ep; g.has_deletions = deletions;
+    return g;
+  }
 
   HnswIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_HNSW, m, d, p) {
     if (p.hnsw_m <= 0 || p.hnsw_efc <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "hnsw nlinks / efconstruction must be > 0");
@@ -1088,10 +975,7 @@ struct HnswIndex : IndexBase {
     auto prepared = [&](int64_t i, std::vector<float>& tmp) -> const float* {
       const float* xi = x + (size_t)i * dim;
       if (metric != B200VS_COSINE) return xi;
-      float norm = 0.0f;  // NormalizeVectorForHnsw, vector_index_utils.cc:493-500
-      for (int j = 0; j < dim; ++j) norm += xi[j] * xi[j];
-      norm = 1.0f / (sqrtf(norm) + 1e-30f);
-      for (int j = 0; j < dim; ++j) tmp[j] = xi[j] * norm;
+      normalize_for_hnsw(xi, dim, tmp.data());
       return tmp.data();
     };
     const int nthreads = (int)std::min<int64_t>(std::max(1, params.hnsw_build_threads), n);
@@ -1132,11 +1016,10 @@ struct HnswIndex : IndexBase {
     batch = batch <= 0 ? HNSW_BUILD_DEFAULT_BATCH : std::min(batch, HNSW_BUILD_MAX_BATCH);
     const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
     const int bmax = (int)std::min<int64_t>(batch, n);  // largest batch of this call
-    const size_t qbytes = ((size_t)dim * 4 + 15) / 16 * 16;
-    const size_t smem_search = qbytes + (size_t)(efc + 1) * sizeof(HeapEnt) + (size_t)HNSW_CAND_SMEM * sizeof(HeapEnt);
+    const size_t smem_search = walk_smem_bytes(dim, efc);
     const size_t smem_link = (size_t)(efc + bmax) * 2 * sizeof(unsigned long long) + (size_t)M * 4;
     const size_t smem_rev = (size_t)(maxM0 + bmax) * 2 * sizeof(unsigned long long) + (size_t)maxM0 * 4;
-    if (smem_search > HNSW_BUILD_SMEM || smem_link > HNSW_BUILD_SMEM || smem_rev > HNSW_BUILD_SMEM)
+    if (smem_search > HNSW_SMEM_LIMIT || smem_link > HNSW_SMEM_LIMIT || smem_rev > HNSW_SMEM_LIMIT)
       fail(B200VS_EILLEGAL_PARAMETERS, "efconstruction / dimension / batch too large for the batched construction kernels");
     set_device();
     cudaStream_t s = stream;
@@ -1147,13 +1030,8 @@ struct HnswIndex : IndexBase {
     const int64_t n0_call = G.n, ntot = G.n + n;
     std::vector<float> rows((size_t)n * dim);
     for (int64_t i = 0; i < n; ++i) {
-      const float* xi = x + (size_t)i * dim;
-      float* o = &rows[(size_t)i * dim];
-      if (metric != B200VS_COSINE) { memcpy(o, xi, (size_t)dim * 4); continue; }
-      float norm = 0.0f;  // NormalizeVectorForHnsw, as add() does it
-      for (int j = 0; j < dim; ++j) norm += xi[j] * xi[j];
-      norm = 1.0f / (sqrtf(norm) + 1e-30f);
-      for (int j = 0; j < dim; ++j) o[j] = xi[j] * norm;
+      if (metric == B200VS_COSINE) normalize_for_hnsw(x + (size_t)i * dim, dim, &rows[(size_t)i * dim]);
+      else memcpy(&rows[(size_t)i * dim], x + (size_t)i * dim, (size_t)dim * 4);
     }
     std::default_random_engine rng = G.rng;
     std::vector<int> lev(n);
@@ -1270,18 +1148,12 @@ struct HnswIndex : IndexBase {
       if (!dead.empty()) B200VS_CUDA(cudaMemcpyAsync(d_dead.p, dead.data(), dead.size() * 4, cudaMemcpyHostToDevice, s));
 
       const bool l2 = metric == B200VS_L2;
-      auto setsmem = [](const void* fn) { B200VS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HNSW_BUILD_SMEM)); };
-      if (l2) {
-        setsmem((const void*)hnsw_build_search_kernel<true, true>); setsmem((const void*)hnsw_build_search_kernel<true, false>);
-        setsmem((const void*)hnsw_build_link_kernel<true>); setsmem((const void*)hnsw_build_reverse_kernel<true>);
-      } else {
-        setsmem((const void*)hnsw_build_search_kernel<false, true>); setsmem((const void*)hnsw_build_search_kernel<false, false>);
-        setsmem((const void*)hnsw_build_link_kernel<false>); setsmem((const void*)hnsw_build_reverse_kernel<false>);
-      }
+      auto setsmem = [](const void* fn) { B200VS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HNSW_SMEM_LIMIT)); };
+      for (const bool fast : {true, false})
+        dispatch_walk(l2, fast, [&](auto L2_, auto FAST_) { setsmem((const void*)hnsw_build_search_kernel<decltype(L2_)::value, decltype(FAST_)::value>); });
+      if (l2) { setsmem((const void*)hnsw_build_link_kernel<true>); setsmem((const void*)hnsw_build_reverse_kernel<true>); }
+      else { setsmem((const void*)hnsw_build_link_kernel<false>); setsmem((const void*)hnsw_build_reverse_kernel<false>); }
       if (profiling) for (int p = PH_BUILD_SEARCH; p <= PH_BUILD_LINK; ++p) phase_ms[p] = 0.f;
-      HnswBuildDev bd;
-      bd.data = d_data.p; bd.link0 = d_link0.p; bd.up_off = d_upoff.p; bd.linkup = d_linkup.p;
-      bd.d = dim; bd.M = M; bd.maxM = maxM; bd.maxM0 = maxM0; bd.efc = efc;
       for (const Batch& B : plan) {
         if (B.ndead > 0) {
           hnsw_tombstone_kernel<<<(unsigned)cdiv(B.ndead, 256), 256, 0, s>>>(d_deleted.p, d_dead.p + B.dead0, B.ndead);
@@ -1291,23 +1163,19 @@ struct HnswIndex : IndexBase {
         const int nb = (int)(B.b - B.a);
         if (n0 == 0) continue;  // the first row of an empty graph goes in alone, without links
         if (nb > 1) take(d_peer, (size_t)nb * nb);
-        HnswDev g;
-        g.data = d_data.p; g.labels = d_labels.p; g.link0 = d_link0.p; g.up_off = d_upoff.p; g.linkup = d_linkup.p; g.deleted = d_deleted.p;
-        g.n = n0; g.d = dim; g.maxM = maxM; g.maxM0 = maxM0; g.maxlevel = B.maxlevel; g.l2 = l2; g.enterpoint = B.ep;
-        g.has_deletions = B.deletions;
+        const HnswDev g = dev_graph(n0, B.maxlevel, B.ep, B.deletions);
         const bool fast = !B.deletions && efc + 1 <= HNSW_CAND_SMEM;
         const long long words = (n0 + 31) / 32, cand_cap = fast ? 0 : n0 + 1;
         phase(PH_BUILD_SEARCH, s);
-        for (int64_t r0 = 0; r0 < nb; r0 += chunk) {
-          const unsigned m = (unsigned)std::min<int64_t>(chunk, nb - r0);
-#define B200VS_BUILD_SEARCH(L2_, FAST_)                                                                                                  \
-  hnsw_build_search_kernel<L2_, FAST_><<<m, HNSW_THREADS, smem_search, s>>>(g, efc, d_lev.p + B.a, r0, n0, d_slot.p + B.a, d_vis.p, words, \
-                                                                            d_pool.p, cand_cap, d_sres.p, d_scnt.p)
-          if (l2) { if (fast) B200VS_BUILD_SEARCH(true, true); else B200VS_BUILD_SEARCH(true, false); }
-          else { if (fast) B200VS_BUILD_SEARCH(false, true); else B200VS_BUILD_SEARCH(false, false); }
-#undef B200VS_BUILD_SEARCH
-          B200VS_CUDA(cudaGetLastError());
-        }
+        dispatch_walk(l2, fast, [&](auto L2_, auto FAST_) {
+          const auto kernel = hnsw_build_search_kernel<decltype(L2_)::value, decltype(FAST_)::value>;
+          for (int64_t r0 = 0; r0 < nb; r0 += chunk) {
+            const unsigned m = (unsigned)std::min<int64_t>(chunk, nb - r0);
+            kernel<<<m, HNSW_THREADS, smem_search, s>>>(g, d_lev.p + B.a, r0, d_slot.p + B.a, d_vis.p, words, d_pool.p, cand_cap, d_sres.p,
+                                                       d_scnt.p);
+            B200VS_CUDA(cudaGetLastError());
+          }
+        });
         phase(PH_BUILD_SELECT, s);
         if (nb > 1) {
           const unsigned grid = (unsigned)cdiv((int64_t)nb * (nb - 1) / 2 * 4, 256);
@@ -1317,16 +1185,16 @@ struct HnswIndex : IndexBase {
           B200VS_CUDA(cudaGetLastError());
         }
         const size_t smem_l = (size_t)(efc + nb) * 2 * sizeof(unsigned long long) + (size_t)M * 4;
-        if (l2) hnsw_build_link_kernel<true><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(bd, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
-        else hnsw_build_link_kernel<false><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(bd, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
+        if (l2) hnsw_build_link_kernel<true><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(g, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
+        else hnsw_build_link_kernel<false><<<(unsigned)B.ntask, HNSW_THREADS, smem_l, s>>>(g, n0, nb, d_lev.p + B.a, B.maxlevel, d_peer.p, d_slot.p + B.a, d_sres.p, d_scnt.p, d_tasks.p + B.task0, d_trip.p);
         B200VS_CUDA(cudaGetLastError());
         phase(PH_BUILD_LINK, s);
         const int nt = (int)(B.ntask * M);
         size_t tb = sort_bytes;
         B200VS_CUDA(cub::DeviceRadixSort::SortKeys(d_sort.p, tb, d_trip.p, d_trip_sorted.p, nt, 0, 64, s));
         const size_t smem_r = (size_t)(maxM0 + nb) * 2 * sizeof(unsigned long long) + (size_t)maxM0 * 4;
-        if (l2) hnsw_build_reverse_kernel<true><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(bd, n0, d_trip_sorted.p, nt);
-        else hnsw_build_reverse_kernel<false><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(bd, n0, d_trip_sorted.p, nt);
+        if (l2) hnsw_build_reverse_kernel<true><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(g, n0, d_trip_sorted.p, nt);
+        else hnsw_build_reverse_kernel<false><<<(unsigned)nt, HNSW_THREADS, smem_r, s>>>(g, n0, d_trip_sorted.p, nt);
         B200VS_CUDA(cudaGetLastError());
         phase(-1, s);
       }
@@ -1426,16 +1294,12 @@ struct HnswIndex : IndexBase {
     if (G.n == 0) { fill_empty_results(nq, k, od, oi, s); return; }
     const float* q = prepare_queries(nq, xq, s);
     const int ef_run = std::max(ef, k);  // searchKnn: max(ef_, k)
-    HnswDev g;
-    g.data = d_data.p; g.labels = d_labels.p; g.link0 = d_link0.p; g.up_off = d_upoff.p; g.linkup = d_linkup.p; g.deleted = d_deleted.p;
-    g.n = G.n; g.d = dim; g.maxM = (int)G.maxM; g.maxM0 = (int)G.maxM0; g.maxlevel = G.maxlevel; g.l2 = metric == B200VS_L2;
-    g.enterpoint = G.enterpoint; g.has_deletions = G.ndeleted > 0;
+    const HnswDev g = dev_graph(G.n, G.maxlevel, G.enterpoint, G.ndeleted > 0);
     const long long words = (G.n + 31) / 32;
     FilterDev f;
     f.has_range = sc.has_range; f.negate = sc.negate; f.rmin = sc.rmin; f.rmax = sc.rmax; f.sorted_ids = sc.sorted_ids_dev; f.n_ids = sc.n_ids;
-    const size_t qbytes = ((size_t)dim * 4 + 15) / 16 * 16;
-    const size_t smem = qbytes + (size_t)(ef_run + 1) * sizeof(HeapEnt) + (size_t)HNSW_CAND_SMEM * sizeof(HeapEnt);
-    if (smem > 200 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "efsearch / dimension too large for the search kernel");
+    const size_t smem = walk_smem_bytes(dim, ef_run);
+    if (smem > HNSW_SMEM_LIMIT) fail(B200VS_EILLEGAL_PARAMETERS, "efsearch / dimension too large for the search kernel");
     const bool fast = !(f.has_range || f.sorted_ids != nullptr) && !g.has_deletions && ef_run + 1 <= HNSW_CAND_SMEM && G.n < (1LL << 31);
     // the merged-array form keeps everything in shared memory; the heap form needs n + 1 candidate slots per query
     const long long cand_cap = fast ? 0 : G.n + 1;
@@ -1443,21 +1307,18 @@ struct HnswIndex : IndexBase {
     unsigned int* visited = scratch.alloc<unsigned int>((size_t)chunk * words);
     HeapEnt* cand = fast ? nullptr : scratch.alloc<HeapEnt>((size_t)chunk * cand_cap);
     ScopedKernelTimer timer(this, s, profiling);
-#define B200VS_HNSW_LAUNCH(L2_, FAST_)                                                                                              \
-  do {                                                                                                                             \
-    B200VS_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<L2_, FAST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     \
-    hnsw_search_kernel<L2_, FAST_><<<(unsigned)m, HNSW_THREADS, smem, s>>>(g, q + (size_t)a * dim, m, k, ef_run, f, visited, words,  \
-                                                                          cand, cand_cap, od + (size_t)a * k, oi + (size_t)a * k);  \
-  } while (0)
-    for (int64_t a = 0; a < nq; a += chunk) {  // chunks share one visited / candidate pool, in stream order
-      const int64_t m = std::min(chunk, nq - a);
-      B200VS_CUDA(cudaMemsetAsync(visited, 0, (size_t)m * words * 4, s));
-      if (g.l2) { if (fast) B200VS_HNSW_LAUNCH(true, true); else B200VS_HNSW_LAUNCH(true, false); }
-      else { if (fast) B200VS_HNSW_LAUNCH(false, true); else B200VS_HNSW_LAUNCH(false, false); }
-      B200VS_CUDA(cudaGetLastError());
-      launch_count(1);
-    }
-#undef B200VS_HNSW_LAUNCH
+    dispatch_walk(metric == B200VS_L2, fast, [&](auto L2_, auto FAST_) {
+      const auto kernel = hnsw_search_kernel<decltype(L2_)::value, decltype(FAST_)::value>;
+      B200VS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HNSW_SMEM_LIMIT));
+      for (int64_t a = 0; a < nq; a += chunk) {  // chunks share one visited / candidate pool, in stream order
+        const int64_t m = std::min(chunk, nq - a);
+        B200VS_CUDA(cudaMemsetAsync(visited, 0, (size_t)m * words * 4, s));
+        kernel<<<(unsigned)m, HNSW_THREADS, smem, s>>>(g, q + (size_t)a * dim, m, k, ef_run, f, visited, words, cand, cand_cap,
+                                                      od + (size_t)a * k, oi + (size_t)a * k);
+        B200VS_CUDA(cudaGetLastError());
+        launch_count(1);
+      }
+    });
     if (!fast) stats[6] += nq;
     timer.stop();
   }

@@ -5,6 +5,10 @@ for byte (and so the oracle's).  Larger batches give another graph, defined by t
 HNSW graph with the host builder's levels and entry point, as good as the host graph, and searched exactly like the oracle
 searches it once adopted."""
 
+import json
+import os
+import sys
+
 import numpy as np
 import pytest
 
@@ -12,6 +16,11 @@ import b200vs
 import oracle_lib
 from b200vs import COSINE, FLAT, HNSW, IP, L2
 from gpu_util import assert_same_results, recall, require_gpu
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.join(HERE, "golden"))
+
+import make_hnsw_batched_golden as golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -146,6 +155,14 @@ def test_deterministic():
         a = build(L2, 32, xb, labels, 16, 100, batch=batch, calls=2).get_trained_state()
         b = build(L2, 32, xb, labels, 16, 100, batch=batch, calls=2).get_trained_state()
         assert np.array_equal(a, b), f"batch {batch}: two builds differ"
+
+
+def test_batched_graphs_match_frozen_hashes():
+    """Graphs of batch > 1 builds, in both construction-search forms, are those of tests/golden/hnsw_batched_graphs.json."""
+    want = json.load(open(os.path.join(HERE, "golden", "hnsw_batched_graphs.json")))
+    assert sorted(want) == sorted(golden.CASES)
+    for name in sorted(want):
+        assert golden.graph_hash(name) == want[name], f"graph of case {name} changed"
 
 
 @pytest.mark.parametrize("metric", [L2, IP])
