@@ -296,18 +296,21 @@ int b200vs_debug_tc_scores(b200vs_index* h, int64_t nq, const float* xq, int32_t
 namespace {
 
 // one host-pointer search: H2D, search, D2H, wait.  xq / outputs may be pinned staging (coalesced batches) or caller memory.
-void host_search_once(IndexBase* ix, int64_t nq, const float* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
+// xq holds nq rows of ix->query_row_bytes(): floats, or packed bits on a binary index.
+void host_search_once(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   ix->set_device();
   LaneGuard lane(ix, nullptr);  // a free lane on its own stream, so concurrent callers overlap
   cudaStream_t s = lane.stream;
   ix->reset_stats();
-  float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
+  const size_t qbytes = (size_t)nq * ix->query_row_bytes();
+  unsigned char* dq = ix->scratch.alloc<unsigned char>(qbytes);
   float* dd = ix->scratch.alloc<float>((size_t)nq * k);
   long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-  B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * ix->dim * 4, cudaMemcpyHostToDevice, s));
+  B200VS_CUDA(cudaMemcpyAsync(dq, xq, qbytes, cudaMemcpyHostToDevice, s));
   SearchCtx sc = make_ctx(ix, sp, s);
-  ix->search_dev(nq, dq, k, sc, dd, di, s);
+  if (ix->binary()) ix->search_binary_dev(nq, dq, k, sc, dd, di, s);
+  else ix->search_dev(nq, reinterpret_cast<const float*>(dq), k, sc, dd, di, s);
   ix->phases_finish(s);
   B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
@@ -326,9 +329,10 @@ constexpr int64_t kCoalesceMaxBatch = 4096; // queries per shared batch (the ser
 void run_coalesced(IndexBase* ix, std::vector<CoalesceReq*>& batch) {
   int64_t total = 0;
   for (auto* r : batch) total += r->nq;
-  const int k = batch[0]->k, d = ix->dim;
+  const int k = batch[0]->k;
+  const size_t row = ix->query_row_bytes();
   // pinned staging owned by the calling (leader) thread: queries in, results out (one H2D, one D2H of each kind)
-  const size_t qbytes = (size_t)total * d * 4, dbytes = (size_t)total * k * 4, ibytes = (size_t)total * k * 8;
+  const size_t qbytes = (size_t)total * row, dbytes = (size_t)total * k * 4, ibytes = (size_t)total * k * 8;
   const size_t need = qbytes + dbytes + ibytes + 64;
   static thread_local void* pin = nullptr;
   static thread_local size_t pin_cap = 0;
@@ -339,11 +343,11 @@ void run_coalesced(IndexBase* ix, std::vector<CoalesceReq*>& batch) {
     B200VS_CUDA(cudaHostAlloc(&pin, need * 2, cudaHostAllocPortable));  // portable: the calling thread may serve indexes on several devices
     pin_cap = need * 2;
   }
-  float* hq = reinterpret_cast<float*>(pin);
-  float* hd = reinterpret_cast<float*>(reinterpret_cast<char*>(pin) + ((qbytes + 15) & ~(size_t)15));
+  char* hq = reinterpret_cast<char*>(pin);
+  float* hd = reinterpret_cast<float*>(hq + ((qbytes + 15) & ~(size_t)15));
   int64_t* hi = reinterpret_cast<int64_t*>(reinterpret_cast<char*>(hd) + ((dbytes + 15) & ~(size_t)15));
   int64_t off = 0;
-  for (auto* r : batch) { memcpy(hq + (size_t)off * d, r->xq, (size_t)r->nq * d * 4); off += r->nq; }
+  for (auto* r : batch) { memcpy(hq + (size_t)off * row, r->xq, (size_t)r->nq * row); off += r->nq; }
   host_search_once(ix, total, hq, k, &batch[0]->sp, hd, hi);
   off = 0;
   for (auto* r : batch) {
@@ -353,7 +357,7 @@ void run_coalesced(IndexBase* ix, std::vector<CoalesceReq*>& batch) {
   }
 }
 
-int coalesced_search(IndexBase* ix, int64_t nq, const float* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
+int coalesced_search(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
   Coalescer& C = ix->coalescer;
   CoalesceReq me;
   me.nq = nq; me.xq = xq; me.k = k; me.out_dist = out_dist; me.out_ids = out_ids;
@@ -392,6 +396,15 @@ int coalesced_search(IndexBase* ix, int64_t nq, const float* xq, int k, const b2
   return me.rc;
 }
 
+// the host-pointer search of b200vs_search and b200vs_search_binary (arguments already checked)
+int host_search(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
+  // small filter-free requests share batches with concurrent callers (the reference issues one query per pool task)
+  if (nq <= kCoalesceMaxReq && ix->coalescer.enabled.load() && !(sp && sp->sorted_ids) && !ix->profiling)
+    return coalesced_search(ix, nq, xq, k, sp, out_dist, out_ids);
+  host_search_once(ix, nq, xq, k, sp, out_dist, out_ids);
+  return B200VS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -404,16 +417,13 @@ int b200vs_search(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const
     check_search_args(ix, nq, xq, sp);
     if (k <= 0) return B200VS_OK;
     if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    // small filter-free requests share batches with concurrent callers (the reference issues one query per pool task)
-    if (nq <= kCoalesceMaxReq && ix->coalescer.enabled.load() && !(sp && sp->sorted_ids) && !ix->profiling)
-      return coalesced_search(ix, nq, xq, k, sp, out_dist, out_ids);
-    host_search_once(ix, nq, xq, k, sp, out_dist, out_ids);
-    return B200VS_OK;
+    return host_search(ix, nq, xq, k, sp, out_dist, out_ids);
   });
 }
 
-/* Request coalescing of b200vs_search (on by default): concurrent host-pointer calls of <= 64 queries without id-list filters
- * are merged into shared batches.  stats (nullable): [0] batches run, [1] requests served through them. */
+/* Request coalescing of b200vs_search and b200vs_search_binary (on by default): concurrent host-pointer calls of <= 64
+ * queries without id-list filters are merged into shared batches.  stats (nullable): [0] batches run, [1] requests served
+ * through them. */
 int b200vs_set_coalescing(b200vs_index* h, int on, int64_t stats[2]) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
@@ -553,6 +563,42 @@ int b200vs_calc_distance(int32_t device, int32_t algorithm, b200vs_metric metric
       throw;
     }
     dl.free(); dr.free(); dn.free(); dout.free();
+    cudaStreamDestroy(s);
+    return B200VS_OK;
+  });
+}
+
+// CalcHammingDistanceByFaiss (vector_index_utils.cc:333-357): packed rows zero-padded to 32-bit words, then the pair kernel
+// with the Hamming functor
+int b200vs_calc_distance_binary(int32_t device, int32_t nbytes, int64_t nl, const uint8_t* left, int64_t nr, const uint8_t* right,
+                                float* out) {
+  return guarded([&]() -> int {
+    if (nbytes <= 0 || nbytes > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "binary row size must be in (0, 4096] bytes");
+    if (nl < 0 || nr < 0) fail(B200VS_EILLEGAL_PARAMETERS, "bad distance-matrix shape");
+    if (nl == 0 || nr == 0) return B200VS_OK;
+    if (!left || !right || !out) fail(B200VS_EILLEGAL_PARAMETERS, "null operand");
+    const int w = (nbytes + 3) / 4;
+    B200VS_CUDA(cudaSetDevice(device));
+    cudaStream_t s = nullptr;
+    B200VS_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    DevBuf<uint8_t> raw;
+    DevBuf<uint32_t> wl, wr;
+    DevBuf<float> dout;
+    try {
+      raw.reserve((size_t)std::max(nl, nr) * nbytes, 0, s);
+      wl.reserve((size_t)nl * w, 0, s); wr.reserve((size_t)nr * w, 0, s); dout.reserve((size_t)nl * nr, 0, s);
+      B200VS_CUDA(cudaMemcpyAsync(raw.p, left, (size_t)nl * nbytes, cudaMemcpyHostToDevice, s));
+      launch_pad_rows(raw.p, nl, nbytes, wl.p, s);
+      B200VS_CUDA(cudaMemcpyAsync(raw.p, right, (size_t)nr * nbytes, cudaMemcpyHostToDevice, s));
+      launch_pad_rows(raw.p, nr, nbytes, wr.p, s);
+      launch_pair_hamming(wl.p, nl, wr.p, nr, w, dout.p, s);
+      B200VS_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)nl * nr * 4, cudaMemcpyDeviceToHost, s));
+      B200VS_CUDA(cudaStreamSynchronize(s));
+    } catch (...) {
+      cudaStreamSynchronize(s); raw.free(); wl.free(); wr.free(); dout.free(); cudaStreamDestroy(s);
+      throw;
+    }
+    raw.free(); wl.free(); wr.free(); dout.free();
     cudaStreamDestroy(s);
     return B200VS_OK;
   });
@@ -707,22 +753,7 @@ int b200vs_search_binary(b200vs_index* h, int64_t nq, const uint8_t* xq, int32_t
     check_search_args(ix, nq, xq, sp);
     if (k <= 0) return B200VS_OK;
     if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, nullptr);
-    cudaStream_t s = lane.stream;
-    ix->reset_stats();
-    uint8_t* dq = ix->scratch.alloc<uint8_t>((size_t)nq * (ix->dim / 8));
-    float* dd = ix->scratch.alloc<float>((size_t)nq * k);
-    long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * (ix->dim / 8), cudaMemcpyHostToDevice, s));
-    SearchCtx sc = make_ctx(ix, sp, s);
-    ix->search_binary_dev(nq, dq, k, sc, dd, di, s);
-    ix->phases_finish(s);
-    B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    return B200VS_OK;
+    return host_search(ix, nq, xq, k, sp, out_dist, out_ids);
   });
 }
 

@@ -47,6 +47,13 @@ int words_of(int dim) { return (dim / 8 + 3) / 4; }
 
 }  // namespace
 
+void launch_pad_rows(const uint8_t* src, int64_t n, int nbytes, uint32_t* dst, cudaStream_t s) {
+  const int w = (nbytes + 3) / 4;
+  if (n <= 0) return;
+  pad_rows_kernel<<<(unsigned)cdiv(n * w, 256), 256, 0, s>>>(src, n, nbytes, w, dst);
+  B200VS_CUDA(cudaGetLastError());
+}
+
 // Device rows of a binary index: [cap, w] words and ids (-1 = tombstone / unused slot).  The owner decides capacities and
 // slots; the store moves rows.  All work runs on the owner's stream.
 struct BinRows {
@@ -125,8 +132,7 @@ struct BinaryIndex : IndexBase {
   const uint32_t* pad(int64_t n, const uint8_t* x_dev, cudaStream_t s) {
     uint32_t* out = scratch.alloc<uint32_t>((size_t)std::max<int64_t>(n, 1) * w);
     if (n > 0) {
-      pad_rows_kernel<<<(unsigned)cdiv(n * w, 256), 256, 0, s>>>(x_dev, n, nb, w, out);
-      B200VS_CUDA(cudaGetLastError());
+      launch_pad_rows(x_dev, n, nb, out, s);
       launch_count(1);
     }
     return out;

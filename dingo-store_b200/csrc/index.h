@@ -120,10 +120,11 @@ constexpr int kLanes = 8;
 // unchanged reference caller slices every batch into single-query tasks on a 16-thread pool (src/vector/vector_index.cc:54,
 // :244-271), so the plugin sees many concurrent nq = 1 calls.  Callers queue here; the one that finds no leader active
 // becomes the leader, takes every compatible pending request (same k / nprobe / efsearch / exact_only, no id filters) and
-// runs them as ONE batch — large enough batches reach the tensor-core tile path — then hands the results back.
+// runs them as ONE batch — large enough batches reach the tensor-core tile path — then hands the results back.  Float
+// and binary indexes share it: a request's queries are nq rows of the index's query_row_bytes().
 struct CoalesceReq {
   int64_t nq = 0;
-  const float* xq = nullptr;
+  const void* xq = nullptr;
   int k = 0;
   b200vs_search_params sp{};
   float* out_dist = nullptr;
@@ -284,6 +285,7 @@ struct IndexBase {
   // ---- binary indexes (B200VS_BINARY_FLAT / B200VS_BINARY_IVF_FLAT, binary.cu): rows are packed bits, dim / 8 bytes each.
   // A float index refuses these, and the float entry points refuse a binary index (b200vs_*_binary, api.cu).
   bool binary() const { return type == B200VS_BINARY_FLAT || type == B200VS_BINARY_IVF_FLAT; }
+  size_t query_row_bytes() const { return binary() ? (size_t)dim / 8 : (size_t)dim * 4; }  // one host query row
   virtual void train_binary(int64_t n, const uint8_t* x) { (void)n; (void)x; fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index"); }
   virtual void add_binary(int64_t n, const uint8_t* x, const int64_t* ids, bool upsert) {
     (void)n; (void)x; (void)ids; (void)upsert;
@@ -417,6 +419,10 @@ void launch_iota(long long* p, int64_t n, cudaStream_t s);
 void launch_negate(float* p, int64_t n, cudaStream_t s);
 // out[i*nr + j] = L2 ? ||a_i - b_j||^2 : 1 - <a_i, b_j>, reference summation order (VectorCalcDistance)
 void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s);
+// out[i*nr + j] = popcount(a_i XOR b_j) over w-word zero-padded binary rows (b200vs_calc_distance_binary)
+void launch_pair_hamming(const uint32_t* a, int64_t nl, const uint32_t* b, int64_t nr, int w, float* out, cudaStream_t s);
+// packed binary rows [n, nbytes] -> zero-padded 32-bit words [n, ceil(nbytes / 4)] (binary.cu)
+void launch_pad_rows(const uint8_t* src, int64_t n, int nbytes, uint32_t* dst, cudaStream_t s);
 // b200vs_hnsw_add_batched (hnsw.cu); ix must be an HNSW index
 void hnsw_add_batched(IndexBase* ix, int64_t n, const float* x, const int64_t* ids, int batch);
 void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes);  // b200vs_debug_hnsw_build_scratch_limit

@@ -159,7 +159,9 @@ void launch_negate(float* p, int64_t n, cudaStream_t s) {
 
 // VectorCalcDistance (src/vector/vector_index_utils.cc:48-124): one quad per (left, right) pair, reference order.
 // Consecutive quads share the left row and walk the right rows, so a CTA re-reads a handful of rows from L1/L2.
-template <bool L2>
+// Dist is the exact scan's per-row functor (scan_kernels.cuh): Fp32Dist<L2> on float rows (d floats), HammingDist on
+// zero-padded binary rows (d 32-bit words).
+template <class Dist>
 static __global__ void __launch_bounds__(256) pair_distance_kernel(const float* __restrict__ a, long long nl, const float* __restrict__ b,
                                                                    long long nr, int d, float* __restrict__ out) {
   const long long pair = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
@@ -168,16 +170,23 @@ static __global__ void __launch_bounds__(256) pair_distance_kernel(const float* 
   const bool valid = pair < total;
   const long long p = valid ? pair : 0;
   const long long i = p / nr, j = p % nr;
-  const float v = quad_distance<L2>(a + (size_t)i * d, b + (size_t)j * d, d, t, (d & 3) == 0);
-  if (valid && t == 0) out[p] = L2 ? v : __fsub_rn(1.0f, v);
+  const float v = Dist::eval(a, i, b + (size_t)j * d, d, t, (d & 3) == 0);
+  if (valid && t == 0) out[p] = Dist::kL2 ? v : __fsub_rn(1.0f, v);
 }
-void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s) {
+template <class Dist>
+static void launch_pair(const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s) {
   const int64_t total = nl * nr;
   if (total <= 0) return;
   const unsigned grid = (unsigned)((total * 4 + 255) / 256);
-  if (l2) pair_distance_kernel<true><<<grid, 256, 0, s>>>(a, nl, b, nr, d, out);
-  else pair_distance_kernel<false><<<grid, 256, 0, s>>>(a, nl, b, nr, d, out);
+  pair_distance_kernel<Dist><<<grid, 256, 0, s>>>(a, nl, b, nr, d, out);
   B200VS_CUDA(cudaGetLastError());
+}
+void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s) {
+  if (l2) launch_pair<Fp32Dist<true>>(a, nl, b, nr, d, out, s);
+  else launch_pair<Fp32Dist<false>>(a, nl, b, nr, d, out, s);
+}
+void launch_pair_hamming(const uint32_t* a, int64_t nl, const uint32_t* b, int64_t nr, int w, float* out, cudaStream_t s) {
+  launch_pair<HammingDist>(reinterpret_cast<const float*>(a), nl, reinterpret_cast<const float*>(b), nr, w, out, s);
 }
 
 void launch_iota(long long* p, int64_t n, cudaStream_t s) {

@@ -36,9 +36,11 @@ enum Errno { OK = 0, EINTERNAL = 10000, EILLEGAL_PARAMTETERS = 10010, EVECTOR_IN
 }  // namespace error
 namespace common {
 enum ValueType { FLOAT = 0, UINT8 = 1 };
-enum MetricType { METRIC_TYPE_NONE = 0, METRIC_TYPE_L2 = 1, METRIC_TYPE_INNER_PRODUCT = 2, METRIC_TYPE_COSINE = 3 };
+enum MetricType { METRIC_TYPE_NONE = 0, METRIC_TYPE_L2 = 1, METRIC_TYPE_INNER_PRODUCT = 2, METRIC_TYPE_COSINE = 3,
+                  METRIC_TYPE_HAMMING = 4 };
 enum VectorIndexType { VECTOR_INDEX_TYPE_NONE = 0, VECTOR_INDEX_TYPE_FLAT = 1, VECTOR_INDEX_TYPE_IVF_FLAT = 2,
-                       VECTOR_INDEX_TYPE_IVF_PQ = 3, VECTOR_INDEX_TYPE_HNSW = 4 };
+                       VECTOR_INDEX_TYPE_IVF_PQ = 3, VECTOR_INDEX_TYPE_HNSW = 4, VECTOR_INDEX_TYPE_BINARY_FLAT = 7,
+                       VECTOR_INDEX_TYPE_BINARY_IVF_FLAT = 8 };
 
 class Vector {
  public:
@@ -50,10 +52,16 @@ class Vector {
   std::vector<float>* mutable_float_values() { return &float_values_; }
   int float_values_size() const { return (int)float_values_.size(); }
   void add_float_values(float v) { float_values_.push_back(v); }
+  // repeated bytes: one packed byte per element, read as binary_values()[j][0]
+  const std::vector<std::string>& binary_values() const { return binary_values_; }
+  std::vector<std::string>* mutable_binary_values() { return &binary_values_; }
+  int binary_values_size() const { return (int)binary_values_.size(); }
+  void add_binary_values(const std::string& v) { binary_values_.push_back(v); }
  private:
   int32_t dimension_ = 0;
   ValueType value_type_ = FLOAT;
   std::vector<float> float_values_;
+  std::vector<std::string> binary_values_;
 };
 class VectorWithId {
  public:
@@ -76,8 +84,10 @@ class VectorSearchParameter {
   SearchIvfParam* mutable_ivf_pq() { return &ivf_pq_; }
   const SearchHnswParam& hnsw() const { return hnsw_; }
   SearchHnswParam* mutable_hnsw() { return &hnsw_; }
+  const SearchIvfParam& binary_ivf_flat() const { return binary_ivf_flat_; }
+  SearchIvfParam* mutable_binary_ivf_flat() { return &binary_ivf_flat_; }
  private:
-  SearchIvfParam ivf_flat_, ivf_pq_;
+  SearchIvfParam ivf_flat_, ivf_pq_, binary_ivf_flat_;
   SearchHnswParam hnsw_;
 };
 struct CreateFlatParam { int32_t dimension_ = 0; MetricType metric_type_ = METRIC_TYPE_L2;
@@ -87,6 +97,8 @@ struct CreateIvfPqParam : CreateIvfFlatParam { int32_t nsubvector_ = 0, nbits_pe
   int32_t nsubvector() const { return nsubvector_; } int32_t nbits_per_idx() const { return nbits_per_idx_; } };
 struct CreateHnswParam : CreateFlatParam { int32_t efconstruction_ = 0, nlinks_ = 0; int64_t max_elements_ = 0;
   int32_t efconstruction() const { return efconstruction_; } int32_t nlinks() const { return nlinks_; } int64_t max_elements() const { return max_elements_; } };
+struct CreateBinaryFlatParam : CreateFlatParam {};           // dimension in bits
+struct CreateBinaryIvfFlatParam : CreateIvfFlatParam {};
 class VectorIndexParameter {
  public:
   VectorIndexType vector_index_type() const { return type_; }
@@ -99,9 +111,14 @@ class VectorIndexParameter {
   CreateIvfPqParam* mutable_ivf_pq_parameter() { return &ivf_pq_; }
   const CreateHnswParam& hnsw_parameter() const { return hnsw_; }
   CreateHnswParam* mutable_hnsw_parameter() { return &hnsw_; }
+  const CreateBinaryFlatParam& binary_flat_parameter() const { return binary_flat_; }
+  CreateBinaryFlatParam* mutable_binary_flat_parameter() { return &binary_flat_; }
+  const CreateBinaryIvfFlatParam& binary_ivf_flat_parameter() const { return binary_ivf_flat_; }
+  CreateBinaryIvfFlatParam* mutable_binary_ivf_flat_parameter() { return &binary_ivf_flat_; }
  private:
   VectorIndexType type_ = VECTOR_INDEX_TYPE_NONE;
   CreateFlatParam flat_; CreateIvfFlatParam ivf_flat_; CreateIvfPqParam ivf_pq_; CreateHnswParam hnsw_;
+  CreateBinaryFlatParam binary_flat_; CreateBinaryIvfFlatParam binary_ivf_flat_;
 };
 struct RegionEpoch { int64_t conf_version = 0, version = 0; };
 struct Range { std::string start_key, end_key; };
@@ -200,6 +217,7 @@ class VectorIndex {
   virtual void LockWrite() = 0;
   virtual void UnlockWrite() = 0;
   virtual butil::Status Train(std::vector<float>& train_datas) = 0;
+  virtual butil::Status Train(std::vector<uint8_t>&) { return butil::Status::OK(); }  // vector_index.h:195
   virtual butil::Status Train(const std::vector<pb::common::VectorWithId>& vectors) = 0;
   virtual bool NeedToRebuild() = 0;
   virtual bool NeedTrain() { return false; }

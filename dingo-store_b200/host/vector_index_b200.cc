@@ -27,11 +27,41 @@ butil::Status CheckVectorDimension(const std::vector<pb::common::VectorWithId>& 
   return butil::Status::OK();
 }
 
+// The UINT8 branch of CheckVectorDimension (utils.cc:502-530) for binary indexes; dimension counts bits.  A FLOAT vector
+// is refused here too: the reference lets it through to ExtractVectorValue<uint8_t>, which has no rows for it (:594-599).
+butil::Status CheckBinaryVectorDimension(const std::vector<pb::common::VectorWithId>& vs, int dimension) {
+  for (const auto& v : vs) {
+    if (v.vector().value_type() != pb::common::ValueType::UINT8)
+      return butil::Status(pb::error::Errno::EVECTOR_INVALID, "invalid value type");
+    if (v.vector().binary_values_size() != dimension / 8)
+      return butil::Status(pb::error::Errno::EVECTOR_INVALID, "binary vector dimension not match, " + std::to_string(v.vector().binary_values_size()) + " " + std::to_string(dimension) + "/bit");
+    if (v.vector().dimension() != dimension)
+      return butil::Status(pb::error::Errno::EVECTOR_INVALID, "vector dimension not match, " + std::to_string(v.vector().dimension()) + " " + std::to_string(dimension));
+  }
+  return butil::Status::OK();
+}
+
 // ExtractVectorValue<float> (memcpy into one row-major array; normalisation happens on the device), utils.cc:563-609
 std::vector<float> ExtractVectorValue(const std::vector<pb::common::VectorWithId>& vs, int dimension) {
   std::vector<float> out(vs.size() * (size_t)dimension);
   for (size_t i = 0; i < vs.size(); ++i) memcpy(out.data() + i * dimension, vs[i].vector().float_values().data(), (size_t)dimension * sizeof(float));
   return out;
+}
+
+// ExtractVectorValue<uint8_t>, utils.cc:594-599: byte j of a packed row = binary_values[j][0]
+std::vector<uint8_t> ExtractBinaryVectorValue(const std::vector<pb::common::VectorWithId>& vs, int dimension) {
+  const size_t nb = (size_t)dimension / 8;
+  std::vector<uint8_t> out(vs.size() * nb);
+  for (size_t i = 0; i < vs.size(); ++i)
+    for (size_t j = 0; j < nb; ++j) out[i * nb + j] = static_cast<uint8_t>(vs[i].vector().binary_values()[j][0]);
+  return out;
+}
+
+// the nprobe knob of the index's type (ivf_flat.cc:207-209 for the binary one; 0 = the library default)
+int32_t NprobeOf(pb::common::VectorIndexType type, const pb::common::VectorSearchParameter& parameter) {
+  if (type == pb::common::VECTOR_INDEX_TYPE_IVF_PQ) return parameter.ivf_pq().nprobe();
+  if (type == pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT) return parameter.binary_ivf_flat().nprobe();
+  return parameter.ivf_flat().nprobe();
 }
 
 struct LoweredFilters {
@@ -60,10 +90,16 @@ VectorIndexB200::VectorIndexB200(int64_t id, const pb::common::VectorIndexParame
     case pb::common::VECTOR_INDEX_TYPE_HNSW:
       type = B200VS_HNSW; dimension_ = p.hnsw_parameter().dimension(); metric_type_ = p.hnsw_parameter().metric_type();
       bp.hnsw_m = p.hnsw_parameter().nlinks(); bp.hnsw_efc = p.hnsw_parameter().efconstruction(); bp.max_elements = p.hnsw_parameter().max_elements(); break;
+    case pb::common::VECTOR_INDEX_TYPE_BINARY_FLAT:  // dimension in bits
+      type = B200VS_BINARY_FLAT; dimension_ = p.binary_flat_parameter().dimension(); metric_type_ = p.binary_flat_parameter().metric_type(); break;
+    case pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT:
+      type = B200VS_BINARY_IVF_FLAT; dimension_ = p.binary_ivf_flat_parameter().dimension(); metric_type_ = p.binary_ivf_flat_parameter().metric_type();
+      bp.nlist = p.binary_ivf_flat_parameter().ncentroids(); break;
     default: break;
   }
-  // "not support metric type, use L2" — flat.cc:91-96
+  // "not support metric type, use L2" — flat.cc:91-96.  A binary type with any metric but HAMMING is refused by the library.
   b200vs_metric m = metric_type_ == pb::common::METRIC_TYPE_INNER_PRODUCT ? B200VS_IP : metric_type_ == pb::common::METRIC_TYPE_COSINE ? B200VS_COSINE : B200VS_L2;
+  if (Binary() && metric_type_ == pb::common::METRIC_TYPE_HAMMING) m = B200VS_HAMMING;
   b200vs_create(type, m, dimension_, &bp, &index_);  // a failed create leaves index_ null: every call then returns EINTERNAL
 }
 
@@ -98,21 +134,27 @@ bool VectorIndexB200::IsExceedsMaxElements(int64_t vector_size) {  // hnsw.cc:54
 
 butil::Status VectorIndexB200::AddOrUpsert(const std::vector<pb::common::VectorWithId>& vs, bool is_upsert) {
   if (vs.empty()) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "vector_with_ids is empty");  // flat.cc:123-125
-  auto status = CheckVectorDimension(vs, dimension_);
+  const bool binary = Binary();
+  auto status = binary ? CheckBinaryVectorDimension(vs, dimension_) : CheckVectorDimension(vs, dimension_);
   if (!status.ok()) return status;
   if (!index_) return ToStatus(B200VS_EINTERNAL);
   std::vector<int64_t> ids(vs.size());
   for (size_t i = 0; i < vs.size(); ++i) ids[i] = vs[i].id();
-  const std::vector<float> x = ExtractVectorValue(vs, dimension_);
+  const std::vector<float> x = binary ? std::vector<float>() : ExtractVectorValue(vs, dimension_);
+  const std::vector<uint8_t> xb = binary ? ExtractBinaryVectorValue(vs, dimension_) : std::vector<uint8_t>();
+  auto add = [&]() {
+    return binary ? b200vs_add_with_ids_binary(index_, (int64_t)vs.size(), xb.data(), ids.data(), is_upsert ? 1 : 0)
+                  : b200vs_add_with_ids(index_, (int64_t)vs.size(), x.data(), ids.data(), is_upsert ? 1 : 0);
+  };
   std::shared_lock<std::shared_mutex> gate(write_gate_);
   if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW && hnsw_device_build_min_rows > 0 &&
       (int64_t)vs.size() >= hnsw_device_build_min_rows)
     return ToStatus(b200vs_hnsw_add_batched(index_, (int64_t)vs.size(), x.data(), ids.data(), 0));
-  int rc = b200vs_add_with_ids(index_, (int64_t)vs.size(), x.data(), ids.data(), is_upsert ? 1 : 0);
+  int rc = add();
   if (rc == B200VS_EVECTOR_NOT_TRAIN) {  // "train with this batch and try again", ivf_flat.cc:133-150
     status = Train(vs);
     if (!status.ok()) return status;
-    rc = b200vs_add_with_ids(index_, (int64_t)vs.size(), x.data(), ids.data(), is_upsert ? 1 : 0);
+    rc = add();
   }
   return ToStatus(rc);
 }
@@ -182,21 +224,28 @@ butil::Status VectorIndexB200::Search(const std::vector<pb::common::VectorWithId
   if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW &&
       (parameter.hnsw().efsearch() < 0 || parameter.hnsw().efsearch() > 1024))                           // hnsw.cc:332-336
     return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "efsearch is illegal, " + std::to_string(parameter.hnsw().efsearch()) + ", must between 0 and 1024");
-  auto status = CheckVectorDimension(vs, dimension_);
+  const bool binary = Binary();
+  auto status = binary ? CheckBinaryVectorDimension(vs, dimension_) : CheckVectorDimension(vs, dimension_);
   if (!status.ok()) return status;
   if (!index_) return ToStatus(B200VS_EINTERNAL);
   LoweredFilters lf;
   status = LowerFilters(index_, filters, lf);
   if (!status.ok()) return status;
-  lf.sp.nprobe = vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_PQ ? parameter.ivf_pq().nprobe() : parameter.ivf_flat().nprobe();
+  lf.sp.nprobe = NprobeOf(vector_index_type, parameter);
   lf.sp.efsearch = parameter.hnsw().efsearch();
-  const std::vector<float> x = ExtractVectorValue(vs, dimension_);
   std::vector<float> distances((size_t)topk * vs.size(), 0.0f);
   std::vector<int64_t> labels((size_t)topk * vs.size(), -1);  // flat.cc:218-219
-  const int rc = b200vs_search(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+  int rc;
+  if (binary) {
+    const std::vector<uint8_t> x = ExtractBinaryVectorValue(vs, dimension_);
+    rc = b200vs_search_binary(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+  } else {
+    const std::vector<float> x = ExtractVectorValue(vs, dimension_);
+    rc = b200vs_search(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+  }
   if (rc != B200VS_OK) return ToStatus(rc);
   // reconstruct: only the HNSW plugin honours it, and never for cosine (hnsw.cc:383-395, :469-472 "force reconstruct false");
-  // the faiss plugins ignore the flag (flat.cc:205, ivf_flat.cc:191)
+  // the faiss plugins, binary ones included, ignore the flag (flat.cc:205, ivf_flat.cc:191)
   std::vector<float> stored;
   std::vector<uint8_t> found;
   if (reconstruct && vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW && metric_type_ != pb::common::METRIC_TYPE_COSINE) {
@@ -208,6 +257,8 @@ butil::Status VectorIndexB200::Search(const std::vector<pb::common::VectorWithId
     if (rrc != B200VS_OK) return ToStatus(rrc);
   }
   // FillSearchResult, utils.cc:611-655: one result per query appended; label < 0 skipped; distances arrive in API semantics
+  // (HAMMING: the distance as is, value type UINT8, :640-646)
+  const pb::common::ValueType value_type = binary ? pb::common::ValueType::UINT8 : pb::common::ValueType::FLOAT;
   for (size_t row = 0; row < vs.size(); ++row) {
     auto& result = results.emplace_back();
     for (size_t i = 0; i < topk; ++i) {
@@ -217,7 +268,7 @@ butil::Status VectorIndexB200::Search(const std::vector<pb::common::VectorWithId
       auto* vwi = vwd->mutable_vector_with_id();
       vwi->set_id(labels[pos]);
       vwi->mutable_vector()->set_dimension(dimension_);
-      vwi->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
+      vwi->mutable_vector()->set_value_type(value_type);
       if (!found.empty()) {
         if (!found[pos]) return butil::Status(pb::error::EINTERNAL, "getDataByLabel failed, label: " + std::to_string(labels[pos]));  // hnsw.cc:389-394
         for (int32_t j = 0; j < dimension_; ++j) vwi->mutable_vector()->add_float_values(stored[pos * (size_t)dimension_ + j]);
@@ -246,20 +297,28 @@ butil::Status VectorIndexB200::RangeSearch(const std::vector<pb::common::VectorW
   if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW)
     return butil::Status(pb::error::Errno::EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // hnsw.cc:487-493
   if (vs.empty()) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "vector_with_ids is empty");   // flat.cc:271-273
-  auto status = CheckVectorDimension(vs, dimension_);
+  const bool binary = Binary();
+  auto status = binary ? CheckBinaryVectorDimension(vs, dimension_) : CheckVectorDimension(vs, dimension_);
   if (!status.ok()) return status;
   if (!index_) return ToStatus(B200VS_EINTERNAL);
   LoweredFilters lf;
   status = LowerFilters(index_, filters, lf);
   if (!status.ok()) return status;
-  lf.sp.nprobe = vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_PQ ? parameter.ivf_pq().nprobe() : parameter.ivf_flat().nprobe();
+  lf.sp.nprobe = NprobeOf(vector_index_type, parameter);
   const int32_t cap = max_range_search_result_count;
-  const std::vector<float> x = ExtractVectorValue(vs, dimension_);
   std::vector<float> distances((size_t)cap * vs.size());
   std::vector<int64_t> labels((size_t)cap * vs.size());
   std::vector<int32_t> counts(vs.size());
-  const int rc = b200vs_range_search(index_, (int64_t)vs.size(), x.data(), radius, cap, &lf.sp, distances.data(), labels.data(), counts.data());
+  int rc;
+  if (binary) {
+    const std::vector<uint8_t> x = ExtractBinaryVectorValue(vs, dimension_);
+    rc = b200vs_range_search_binary(index_, (int64_t)vs.size(), x.data(), radius, cap, &lf.sp, distances.data(), labels.data(), counts.data());
+  } else {
+    const std::vector<float> x = ExtractVectorValue(vs, dimension_);
+    rc = b200vs_range_search(index_, (int64_t)vs.size(), x.data(), radius, cap, &lf.sp, distances.data(), labels.data(), counts.data());
+  }
   if (rc != B200VS_OK) return ToStatus(rc);
+  const pb::common::ValueType value_type = binary ? pb::common::ValueType::UINT8 : pb::common::ValueType::FLOAT;  // :672-674
   for (size_t row = 0; row < vs.size(); ++row) {  // FillRangeSearchResult, utils.cc:657-700
     auto& result = results.emplace_back();
     for (int32_t i = 0; i < counts[row]; ++i) {
@@ -268,7 +327,7 @@ butil::Status VectorIndexB200::RangeSearch(const std::vector<pb::common::VectorW
       auto* vwi = vwd->mutable_vector_with_id();
       vwi->set_id(labels[pos]);
       vwi->mutable_vector()->set_dimension(dimension_);
-      vwi->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
+      vwi->mutable_vector()->set_value_type(value_type);
       vwd->set_distance(distances[pos]);
       vwd->set_metric_type(metric_type_);
     }
@@ -277,8 +336,12 @@ butil::Status VectorIndexB200::RangeSearch(const std::vector<pb::common::VectorW
 }
 
 butil::Status VectorIndexB200::Train(std::vector<float>& train_datas) {
-  if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_FLAT || vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW)
+  if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_FLAT || vector_index_type == pb::common::VECTOR_INDEX_TYPE_HNSW ||
+      vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_FLAT)
     return butil::Status::OK();  // flat.cc:464-466, hnsw.cc:560
+  // the reference aborts the process here (DINGO_LOG(FATAL), ivf_flat.cc:694-697); a status leaves the server running
+  if (vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT)
+    return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "a binary ivf_flat index trains on uint8 rows, not float");
   const size_t data_size = dimension_ > 0 ? train_datas.size() / dimension_ : 0;
   if (data_size == 0) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "data size invalid");  // ivf_flat.cc:646-649
   if (train_datas.size() % dimension_ != 0)
@@ -287,7 +350,29 @@ butil::Status VectorIndexB200::Train(std::vector<float>& train_datas) {
   return ToStatus(b200vs_train(index_, (int64_t)data_size, train_datas.data()));
 }
 
-butil::Status VectorIndexB200::Train(const std::vector<pb::common::VectorWithId>& vectors) {  // ivf_flat.cc:714-733
+butil::Status VectorIndexB200::Train(std::vector<uint8_t>& train_datas) {  // ivf_flat.cc:578-641
+  if (vector_index_type != pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT) return butil::Status::OK();  // base default, vector_index.h:195
+  const size_t nb = dimension_ > 0 ? (size_t)dimension_ / 8 : 0;
+  const size_t data_size = nb > 0 ? train_datas.size() / nb : 0;
+  if (data_size == 0) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "data size invalid");
+  if (train_datas.size() % nb != 0)
+    return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "dimension not match " + std::to_string(train_datas.size()) + " * CHAR_BIT(8) " + std::to_string(dimension_));
+  if (!index_) return ToStatus(B200VS_EINTERNAL);
+  return ToStatus(b200vs_train_binary(index_, (int64_t)data_size, train_datas.data()));
+}
+
+butil::Status VectorIndexB200::Train(const std::vector<pb::common::VectorWithId>& vectors) {  // ivf_flat.cc:714-745
+  if (Binary()) {
+    const size_t nb = dimension_ > 0 ? (size_t)dimension_ / 8 : 0;
+    std::vector<uint8_t> train_datas;
+    train_datas.reserve(nb * vectors.size());
+    for (const auto& v : vectors) {
+      if ((size_t)v.vector().binary_values_size() != nb)
+        return butil::Status(pb::error::EINTERNAL, "binary_ivf_flat index dimension not match");
+      for (const auto& b : v.vector().binary_values()) train_datas.push_back(static_cast<uint8_t>(b[0]));
+    }
+    return Train(train_datas);
+  }
   std::vector<float> train_datas;
   train_datas.reserve((size_t)dimension_ * vectors.size());
   for (const auto& v : vectors) {
@@ -299,7 +384,8 @@ butil::Status VectorIndexB200::Train(const std::vector<pb::common::VectorWithId>
 }
 
 bool VectorIndexB200::NeedTrain() {
-  return vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_FLAT || vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_PQ;
+  return vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_FLAT || vector_index_type == pb::common::VECTOR_INDEX_TYPE_IVF_PQ ||
+         vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT;
 }
 bool VectorIndexB200::IsTrained() { return index_ && b200vs_is_trained(index_) != 0; }
 bool VectorIndexB200::NeedToSave(int64_t last_save_log_behind) { return SupportSave() && last_save_log_behind > 10000; }  // flat.cc:515-531
@@ -327,6 +413,9 @@ butil::Status VectorIndexB200Utils::CalcDistance(int algorithm_type, pb::common:
                                                  std::vector<pb::common::Vector>& result_op_right_vectors, int device) {
   if (algorithm_type != B200VS_ALGORITHM_FAISS && algorithm_type != B200VS_ALGORITHM_HNSWLIB)
     return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "invalid algorithm type : ALGORITHM_NONE");     // utils.cc:70-76
+  if (metric_type == pb::common::METRIC_TYPE_HAMMING)
+    return CalcHammingDistance(algorithm_type, op_left_vectors, op_right_vectors, is_return_normlize, distances, result_op_left_vectors,
+                               result_op_right_vectors, device);
   if (metric_type != pb::common::METRIC_TYPE_L2 && metric_type != pb::common::METRIC_TYPE_INNER_PRODUCT && metric_type != pb::common::METRIC_TYPE_COSINE)
     return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "invalid metric_type type : METRIC_TYPE_NONE");  // utils.cc:151-157
   distances.clear();
@@ -356,6 +445,48 @@ butil::Status VectorIndexB200Utils::CalcDistance(int algorithm_type, pb::common:
     };
     fill(result_op_left_vectors, lo, nl);
     fill(result_op_right_vectors, ro, nr);
+  }
+  return butil::Status::OK();
+}
+
+// CalcHammingDistanceByFaiss (utils.cc:146-149, :333-357): popcount of the XOR over the packed bytes of binary_values
+butil::Status VectorIndexB200Utils::CalcHammingDistance(int algorithm_type, const std::vector<pb::common::Vector>& op_left_vectors,
+                                                        const std::vector<pb::common::Vector>& op_right_vectors, bool is_return_normlize,
+                                                        std::vector<std::vector<float>>& distances,
+                                                        std::vector<pb::common::Vector>& result_op_left_vectors,
+                                                        std::vector<pb::common::Vector>& result_op_right_vectors, int device) {
+  // CalcDistanceByHnswlib has no HAMMING case: its switch falls through to an OK status and leaves every output as it
+  // was (utils.cc:160-189).  The same here.
+  if (algorithm_type == B200VS_ALGORITHM_HNSWLIB) return butil::Status::OK();
+  distances.clear();
+  distances.resize(op_left_vectors.size());  // CalcDistanceCore, utils.cc:86-88
+  if (op_left_vectors.empty() || op_right_vectors.empty()) return butil::Status::OK();
+  // the reference sizes every pair by the left vector and reads past a shorter right one: a mismatch is refused instead
+  const size_t nb = op_left_vectors[0].binary_values().size();
+  for (const auto& v : op_left_vectors) if (v.binary_values().size() != nb) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "op_left_vectors dimension not match");
+  for (const auto& v : op_right_vectors) if (v.binary_values().size() != nb) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "op_right_vectors dimension not match");
+  const size_t nl = op_left_vectors.size(), nr = op_right_vectors.size();
+  auto pack = [nb](const std::vector<pb::common::Vector>& vs) {
+    std::vector<uint8_t> x(vs.size() * nb);
+    for (size_t i = 0; i < vs.size(); ++i)
+      for (size_t j = 0; j < nb; ++j) x[i * nb + j] = static_cast<uint8_t>(vs[i].binary_values()[j][0]);
+    return x;
+  };
+  const std::vector<uint8_t> left = pack(op_left_vectors), right = pack(op_right_vectors);
+  std::vector<float> out(nl * nr);
+  const int rc = b200vs_calc_distance_binary(device, (int32_t)nb, (int64_t)nl, left.data(), (int64_t)nr, right.data(), out.data());
+  if (rc != B200VS_OK) return AbiStatus(rc);
+  for (size_t i = 0; i < nl; ++i) distances[i].assign(out.begin() + i * nr, out.begin() + (i + 1) * nr);
+  if (is_return_normlize) {  // ResultOpBinaryVectorAssignment, utils.cc:439-444: the inputs, dimension in bits, UINT8
+    auto fill = [nb](std::vector<pb::common::Vector>& dst, const std::vector<pb::common::Vector>& src) {
+      dst = src;
+      for (auto& v : dst) {
+        v.set_dimension((int32_t)(nb * 8));
+        v.set_value_type(pb::common::ValueType::UINT8);
+      }
+    };
+    fill(result_op_left_vectors, op_left_vectors);
+    fill(result_op_right_vectors, op_right_vectors);
   }
   return butil::Status::OK();
 }

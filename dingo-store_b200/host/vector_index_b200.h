@@ -1,9 +1,10 @@
 // vector_index_b200.h — drop-in subclass of dingodb::VectorIndex backed by libb200vs (include/b200vs.h).
 //
-// One class serves the four plugin types; VectorIndexFactory::New{Flat,IvfFlat,IvfPq,Hnsw}
+// One class serves the six plugin types; VectorIndexFactory::New{Flat,IvfFlat,IvfPq,Hnsw,BinaryFlat,BinaryIvfFlat}
 // (src/vector/vector_index_factory.cc:40-95) would return it instead of VectorIndexFlat / VectorIndexIvfFlat /
-// VectorIndexIvfPq / VectorIndexHnsw.  The class does only what the reference plugins do around their faiss /
-// hnswlib calls: argument checks with the same status codes, pb -> flat-array marshalling
+// VectorIndexIvfPq / VectorIndexHnsw and their faiss::IndexBinary instantiations.  Binary types hold packed UINT8
+// vectors (binary_values, dimension in bits) under METRIC_TYPE_HAMMING.  The class does only what the reference plugins
+// do around their faiss / hnswlib calls: argument checks with the same status codes, pb -> flat-array marshalling
 // (CheckVectorDimension / ExtractVectorValue / FillSearchResult, src/vector/vector_index_utils.cc:502-655), filter
 // lowering, and the write lock bookkeeping; all arithmetic is behind the C ABI.
 #pragma once
@@ -54,6 +55,7 @@ class VectorIndexB200 : public VectorIndex {
   void LockWrite() override { write_gate_.lock(); }
   void UnlockWrite() override { write_gate_.unlock(); }
   butil::Status Train(std::vector<float>& train_datas) override;
+  butil::Status Train(std::vector<uint8_t>& train_datas) override;  // packed rows, dimension / 8 bytes each
   butil::Status Train(const std::vector<pb::common::VectorWithId>& vectors) override;
   bool NeedToRebuild() override { return false; }
   bool NeedTrain() override;
@@ -73,6 +75,9 @@ class VectorIndexB200 : public VectorIndex {
  private:
   butil::Status AddOrUpsert(const std::vector<pb::common::VectorWithId>& vector_with_ids, bool is_upsert);
   butil::Status ToStatus(int rc) const;
+  bool Binary() const {
+    return vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_FLAT || vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT;
+  }
 
   b200vs_index* index_ = nullptr;
   int32_t dimension_ = 0;
@@ -88,6 +93,12 @@ class VectorIndexB200Utils {
                                     const std::vector<pb::common::Vector>& op_right_vectors, bool is_return_normlize,
                                     std::vector<std::vector<float>>& distances, std::vector<pb::common::Vector>& result_op_left_vectors,
                                     std::vector<pb::common::Vector>& result_op_right_vectors, int device = 0);
+
+ private:
+  static butil::Status CalcHammingDistance(int algorithm_type, const std::vector<pb::common::Vector>& op_left_vectors,
+                                           const std::vector<pb::common::Vector>& op_right_vectors, bool is_return_normlize,
+                                           std::vector<std::vector<float>>& distances, std::vector<pb::common::Vector>& result_op_left_vectors,
+                                           std::vector<pb::common::Vector>& result_op_right_vectors, int device);
 };
 
 // The inner loop of VectorReader::BruteForceSearch (src/vector/vector_reader.cc:1873-2048): the caller keeps the RocksDB

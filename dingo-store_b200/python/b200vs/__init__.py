@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_broadcast_state", "b200vs_shard_add", "b200vs_shard_add_device", "b200vs_shard_remove_ids", "b200vs_shard_plan_add_device",
     "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
-    "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit",
+    "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
 ]
 
 
@@ -94,6 +94,7 @@ def lib():
     L.b200vs_last_search_stats.argtypes = [vp, ctypes.POINTER(i64 * 8)]
     L.b200vs_last_phase_times.argtypes = [vp, ctypes.POINTER(ctypes.c_float * 16)]
     L.b200vs_calc_distance.argtypes = [i32, i32, ctypes.c_int, i32, i64, vp, i64, vp, vp, vp, vp]
+    L.b200vs_calc_distance_binary.argtypes = [i32, i32, i64, vp, i64, vp, vp]
     L.b200vs_scan_begin.argtypes = [i32, ctypes.c_int, i32, i64, vp, i32, ctypes.POINTER(SearchParams), ctypes.POINTER(vp)]
     L.b200vs_scan_push.argtypes = [vp, i64, vp, vp]
     L.b200vs_scan_finish.argtypes = [vp, vp, vp]
@@ -509,6 +510,19 @@ def calc_distance(algorithm, metric, left, right, return_normalized=False, devic
                                       right.ctypes.data if right.size else None, out.ctypes.data if out.size else None,
                                       lo.ctypes.data if lo is not None and lo.size else None, ro.ctypes.data if ro is not None and ro.size else None))
     return (out, lo, ro) if return_normalized else out
+
+
+def calc_distance_binary(left, right, device=0):
+    """Hamming distance matrix [nl, nr] of packed uint8 rows [nl, nbytes] / [nr, nbytes] (exact integers, as float32)."""
+    left, right = _u8(left), _u8(right)
+    nl, nr = left.shape[0], right.shape[0]
+    nbytes = left.shape[1] if left.ndim == 2 else 0
+    if right.ndim != 2 or right.shape[1] != nbytes:
+        raise ValueError(f"right rows must have the left rows' {nbytes} bytes")
+    out = np.zeros((nl, nr), dtype=np.float32)
+    _check(lib().b200vs_calc_distance_binary(device, nbytes, nl, left.ctypes.data if left.size else None, nr,
+                                             right.ctypes.data if right.size else None, out.ctypes.data if out.size else None))
+    return out
 
 
 class BruteForceScan:

@@ -126,10 +126,11 @@ int b200vs_debug_hnsw_build_scratch_limit(b200vs_index* idx, int64_t bytes);
  * xq row-major [nq,dim] RAW; out_dist [nq,k], out_ids [nq,k]. */
 int b200vs_search(b200vs_index* idx, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
                   float* out_dist, int64_t* out_ids);
-/* b200vs_search coalesces concurrent callers (SURVEY 8b): the unchanged reference slices every batch into one-query tasks
- * on its 16-thread pool (src/vector/vector_index.cc:54, :244-271), so the plugin sees many concurrent nq = 1 calls.  Calls
- * of <= 64 queries without id-list filters queue inside the library; the caller that finds no leader active runs every
- * compatible pending request (same k / nprobe / efsearch / exact_only / id range) as ONE batch and hands the results back.
+/* b200vs_search and b200vs_search_binary coalesce concurrent callers (SURVEY 8b): the unchanged reference slices every batch
+ * into one-query tasks on its 16-thread pool (src/vector/vector_index.cc:54, :244-271), so the plugin sees many concurrent
+ * nq = 1 calls.  Calls of <= 64 queries without id-list filters (and with profiling off) queue inside the library; the caller
+ * that finds no leader active runs every compatible pending request (same k / nprobe / efsearch / exact_only / id range) as
+ * ONE batch and hands the results back.
  * on: 1 / 0 switch it, < 0 only reads; stats (nullable): [0] batches run, [1] requests served through them. */
 int b200vs_set_coalescing(b200vs_index* idx, int on, int64_t stats[2]);
 
@@ -274,6 +275,12 @@ int b200vs_reserve_lists(b200vs_index* idx, const int64_t* rows_per_list, int32_
 enum { B200VS_ALGORITHM_FAISS = 1, B200VS_ALGORITHM_HNSWLIB = 2 };  /* pb::index::AlgorithmType */
 int b200vs_calc_distance(int32_t device, int32_t algorithm, b200vs_metric metric, int32_t dim, int64_t nl, const float* left,
                          int64_t nr, const float* right, float* out, float* left_out, float* right_out);
+/* The same matrix for METRIC_TYPE_HAMMING (CalcHammingDistanceByFaiss, vector_index_utils.cc:333-357).  Host pointers,
+ * packed rows left [nl, nbytes], right [nr, nbytes]; out [nl, nr] = popcount(left_i XOR right_j) over the nbytes bytes,
+ * as float (an exact integer).  nbytes <= 0 or > 4096 (32768 bits, the binary index limit): EILLEGAL_PARAMETERS; then
+ * nl == 0 or nr == 0 returns OK and computes nothing. */
+int b200vs_calc_distance_binary(int32_t device, int32_t nbytes, int64_t nl, const uint8_t* left, int64_t nr, const uint8_t* right,
+                                float* out);
 
 /* Streaming brute-force search over vectors that are NOT in an index: VectorReader::BruteForceSearch
  * (src/vector/vector_reader.cc:1873-2048), which scans the region's vector column family, builds a temporary Flat
