@@ -277,10 +277,9 @@ def test_training():
         blobs.append(ix.get_trained_state())
     assert np.array_equal(blobs[0], blobs[1])  # deterministic
     cent = blobs[0][32:].reshape(nlist, dim // 8)
+    # +-1 rows have integer sums, so the engine's fixed-point k-means equals the oracle's float one exactly
     ocent = bo.kmeans(oracle_lib_load(), xb, dim, nlist)
-    obj = bo.hamming(xb[:4000], cent).min(1).mean()
-    oobj = bo.hamming(xb[:4000], ocent).min(1).mean()
-    assert obj <= 1.15 * oobj, (obj, oobj)
+    assert np.array_equal(cent, ocent)
     ix.add(xb, ids)
     off, _, codes, lids = ix.export_lists(nlist)
     assert_rows_in_oracle_lists(off, lids, ids, bo.assign(xb, cent))
