@@ -277,8 +277,8 @@ int b200vs_debug_tc_scores(b200vs_index* h, int64_t nq, const float* xq, int32_t
     if (ix->type != B200VS_FLAT) fail(B200VS_EILLEGAL_PARAMETERS, "tensor-core score diagnostics only exist for FLAT");
     if (ix->dim % 4 != 0 || ix->dim < 32) fail(B200VS_EILLEGAL_PARAMETERS, "the tile kernel needs dim % 4 == 0 and dim >= 32");
     if (nq <= 0 || !xq || !out_scores || !out_eps) fail(B200VS_EILLEGAL_PARAMETERS, "bad diagnostic arguments");
-    if (split < 0 || split > 2) fail(B200VS_EILLEGAL_PARAMETERS, "split must be 0, 1 or 2");
-    if (split == 2 && ix->dim % 8 != 0) fail(B200VS_EILLEGAL_PARAMETERS, "the FP16 arithmetic needs dim % 8 == 0");
+    if (split < 0 || split > 4) fail(B200VS_EILLEGAL_PARAMETERS, "split must be 0, 1, 2, 3 or 4");
+    if ((split == 2 || split == 4) && ix->dim % 8 != 0) fail(B200VS_EILLEGAL_PARAMETERS, "the FP16 arithmetic needs dim % 8 == 0");
     std::shared_lock<std::shared_mutex> rl(ix->rw);
     ix->set_device();
     LaneGuard lane(ix, nullptr);

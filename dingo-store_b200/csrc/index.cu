@@ -427,7 +427,9 @@ struct FlatIndex : IndexBase {
     const float* q = prepare_queries(nq, xq, s);
     float* ds = scratch.alloc<float>((size_t)std::max<int64_t>(nq * rows, 1));
     float* de = scratch.alloc<float>(nq);
-    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, (TcArith)arith, ds, de, s);
+    const bool sample = arith >= 3;  // 3 / 4: the sample pass in the TF32 / FP16 list-scan arithmetic
+    const TcArith a = sample ? (arith == 4 ? TC_ARITH_FP16 : TC_ARITH_TF32) : (TcArith)arith;
+    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, a, sample, ds, de, s);
     if (rows > 0) B200VS_CUDA(cudaMemcpyAsync(out_scores, ds, (size_t)nq * rows * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(out_eps, de, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));

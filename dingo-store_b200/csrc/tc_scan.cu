@@ -135,16 +135,16 @@ void launch_split_rows(const float* x, int64_t n, int d, float* hi, float* lo, c
   tc_split_rows_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, s>>>(x, tot, hi, lo);
   B200VS_CUDA(cudaGetLastError());
 }
-// coarse pass: items = (row chunk) x (query group); B rows are the query rows themselves
-static __global__ void tc_coarse_items_kernel(int nrows, int nq, int chunk, TcItem* items, int* totals) {
-  const int nc = (nrows + chunk - 1) / chunk, ng = (nq + TC_NQT - 1) / TC_NQT;
+// coarse pass: items = (row chunk) x (group of nqt <= TC_NQT queries); B rows are the query rows themselves
+static __global__ void tc_coarse_items_kernel(int nrows, int nq, int chunk, int nqt, TcItem* items, int* totals) {
+  const int nc = (nrows + chunk - 1) / chunk, ng = (nq + nqt - 1) / nqt;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) { totals[0] = nc * ng; totals[1] = nq; totals[2] = 0; }
   if (i >= nc * ng) return;
   const int ch = i / ng, g = i % ng;
   TcItem it;
   it.list = 0; it.row_begin = ch * chunk; it.row_end = min(nrows, (ch + 1) * chunk);
-  it.pair_begin = g * TC_NQT; it.nq = min(TC_NQT, nq - g * TC_NQT); it.sample_slot = -1; it.pad[0] = it.pad[1] = 0;
+  it.pair_begin = g * nqt; it.nq = min(nqt, nq - g * nqt); it.sample_slot = -1; it.pad[0] = it.pad[1] = 0;
   items[i] = it;
 }
 
@@ -249,7 +249,7 @@ static __global__ void tc_items_kernel(const int* __restrict__ cnt, const int* _
 }
 
 // ---------------------------------------------------------------------------------------------
-// THE HOT KERNEL.  Persistent (one CTA per SM), warp-specialised, dynamically scheduled:
+// THE HOT KERNEL.  Persistent (one CTA per SM in its capture form), warp-specialised, dynamically scheduled:
 //   warp 8 (one lane): scheduler + TMA producer — claims the next work item with one atomicAdd, publishes it through
 //                      a 4-deep smem queue, then per K block loads the A tile = 128 list rows x 128 B (16 KB,
 //                      EVICT_FIRST: streamed once) and the B tile = 16/32/64/128 gathered queries x 128 B (EVICT_LAST)
@@ -261,24 +261,46 @@ static __global__ void tc_items_kernel(const int* __restrict__ cnt, const int* _
 // HALF = false: K block = 32 floats of the FP32 rows; HALF = true: 64 halves of the FP16 mirror, so a row costs half the
 // tile loads.  Algorithmic HBM bytes per item: rows x (d*4 + 4 + 8) (vector, norm, id), or rows x (d*2 + 4 + 4 + 8) on the
 // mirror (+ scale), read exactly once.
+//
+// Two instantiations per operand type (TcCfg).  The capture / dense form is the one above.  The sample pass only ever
+// scores the first TC_SAMPLE rows of an item, so its form has one consumer warpgroup and a 3-stage ring of 32-row A boxes,
+// without capture staging: three of its CTAs share an SM, so three times as many items' start-up round trips overlap.
+// Both forms run the same per-row wgmma sequence and epilogue (tc_mma_tile / tc_consume_item) on stages that start on a
+// 1024-byte boundary, so a sampled score is bit for bit the score the capture pass computes for that (row, query).
 // ---------------------------------------------------------------------------------------------
-constexpr int TC_CWARPS = 8;  // consumer warps (two warpgroups); the producer is warp TC_CWARPS
+template <bool SAMPLE>
+struct TcCfg {
+  static constexpr bool IS_SAMPLE = SAMPLE;      // mode 0 only; the other form runs modes 1 and 2
+  static constexpr int CWARPS = SAMPLE ? 4 : 8;  // consumer warps (one or two warpgroups); the producer is warp CWARPS
+  static constexpr int THREADS = CWARPS * 32 + 32;
+  static constexpr int MIN_CTAS = SAMPLE ? 3 : 1;  // CTAs per SM the launch bounds reserve registers for
+  // TMA -> MMA ring.  Capture: 6 x 32 KB (+ 24 KB of capture staging: ~220 KB; the bytes in flight bound the HBM rate,
+  // DESIGN §4.2).  Sample: 3 x (4 KB A box + 16 KB B tile) = 61 KB with the alignment slack.  Both strides are multiples
+  // of 1024, the period of the 128-byte swizzle.
+  static constexpr int STAGES = SAMPLE ? 3 : 6;
+  static constexpr uint32_t A_STAGE = SAMPLE ? TC_SAMPLE * 128 : TC_A_BYTES;
+  static constexpr uint32_t B_STAGE = TC_B_BYTES;
+  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + 1024;
+};
 
+template <int STAGES>
 struct TcRing {  // a consumer's position in the TMA ring
   int stage = 0;
   uint32_t phase = 0;
   __device__ __forceinline__ void next() {
-    if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
   }
 };
 
 // One 128-row tile: this warpgroup's 64 x N scores into acc.  Every consumer warp waits for and releases every stage,
-// also when its warpgroup has no rows in the tile (mma = false).
-template <bool HALF, int N>
+// also when its warpgroup has no rows in the tile (mma = false).  In the sample form a stage holds 32 A rows, so the
+// M = 64 wgmma also reads the 32 rows after them (the next stage, or the first B tile): their scores land in accumulator
+// rows 32-63, which the epilogue never stores (as with the stale rows of a partly loaded capture stage).
+template <bool HALF, int N, class C>
 __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool mma, uint8_t* sA, uint8_t* sB, uint64_t* full_bar,
-                                            uint64_t* empty_bar, TcRing& ring, float (&acc)[N / 2]) {
+                                            uint64_t* empty_bar, TcRing<C::STAGES>& ring, float (&acc)[N / 2]) {
   const int lane = threadIdx.x & 31;
-  const uint32_t a_off = (uint32_t)(threadIdx.x >> 7) * 64u * 128u;
+  const uint32_t a_off = (uint32_t)(threadIdx.x >> 7) * 64u * 128u;  // warpgroup g: rows [64g, 64g + 64)
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
   for (int kb = 0; kb < kblocks; ++kb) {
@@ -286,15 +308,15 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
     mbar_wait(&full_bar[s_hi], ring.phase);
     ring.next();
     int s_lo = 0;
-    const bool split = !HALF && p.split;
+    const bool split = !HALF && !C::IS_SAMPLE && p.split;
     if (split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
       s_lo = ring.stage;
       mbar_wait(&full_bar[s_lo], ring.phase);
       ring.next();
     }
     if (mma) {
-      const uint64_t adesc = make_desc_k128(smem_u32(sA + (size_t)s_hi * TC_A_BYTES + a_off));
-      const uint64_t bdesc = make_desc_k128(smem_u32(sB + (size_t)s_hi * TC_B_BYTES));
+      const uint64_t adesc = make_desc_k128(smem_u32(sA + (size_t)s_hi * C::A_STAGE + a_off));
+      const uint64_t bdesc = make_desc_k128(smem_u32(sB + (size_t)s_hi * C::B_STAGE));
       wgmma_fence_operands(acc);
       wgmma_fence();
 #pragma unroll
@@ -303,8 +325,8 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
         else wgmma_tf32<N>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
       }
       if (split) {  // + lo*hi + hi*lo into the same accumulator
-        const uint64_t adesc_lo = make_desc_k128(smem_u32(sA + (size_t)s_lo * TC_A_BYTES + a_off));
-        const uint64_t bdesc_lo = make_desc_k128(smem_u32(sB + (size_t)s_lo * TC_B_BYTES));
+        const uint64_t adesc_lo = make_desc_k128(smem_u32(sA + (size_t)s_lo * C::A_STAGE + a_off));
+        const uint64_t bdesc_lo = make_desc_k128(smem_u32(sB + (size_t)s_lo * C::B_STAGE));
 #pragma unroll
         for (int k = 0; k < TC_BK / 8; ++k) {
           wgmma_tf32<N>(acc, adesc_lo + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), 1u);
@@ -325,16 +347,16 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
 
 // One work item on the consumer warps; N = query columns of the B tile (16 / 32 / 64 / 128).
 // Thread layout of the accumulators: rows row0 and row0 + 8 of the tile, columns 8j + col0 + {0, 1}.
-template <bool HALF, int N>
+template <bool HALF, int N, class C>
 __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem& I, int kblocks, uint8_t* sA, uint8_t* sB,
-                                                uint64_t* full_bar, uint64_t* empty_bar, TcRing& ring, const float* s_tau,
+                                                uint64_t* full_bar, uint64_t* empty_bar, TcRing<C::STAGES>& ring, const float* s_tau,
                                                 const int* s_q, const float* s_qs, unsigned long long* hit_key, int* hit_q, int* hit_n) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
   const long long list_base = p.list_off[I.list];
   int rows = I.row_end - I.row_begin;
-  if (p.mode == 0) rows = min(rows, TC_SAMPLE);
+  if constexpr (C::IS_SAMPLE) rows = min(rows, TC_SAMPLE);
   const int ntiles = (rows + TC_BM - 1) / TC_BM;
   for (int t = 0; t < ntiles; ++t) {
     // row metadata first: its loads overlap the MMAs.  The id and norm loads do not depend on each other, and the masks
@@ -358,7 +380,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
     }
     float acc[N / 2];
     const bool mma = t * TC_BM + wg * 64 < rows;  // else this warpgroup's half of the last tile holds no item rows
-    tc_mma_tile<HALF, N>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
+    tc_mma_tile<HALF, N, C>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
     if (!mma) continue;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -377,7 +399,9 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
             // FP16: both scales are powers of two, so hs * qs and the product with the accumulator are exact
             const float dot = HALF ? acc[4 * j + 2 * h + c] * (hs[h] * s_qs[n]) : acc[4 * j + 2 * h + c];
             const float score = p.l2 ? fmaf(-2.f, dot, nrm[h]) : -dot;
-            if (p.mode == 1) {
+            if constexpr (C::IS_SAMPLE) {
+              if (t == 0 && r < TC_SAMPLE) p.sample[((size_t)I.sample_slot * TC_NQT + n) * TC_SAMPLE + r] = valid[h] ? score : TC_INF;
+            } else if (p.mode == 1) {
               if (valid[h] && score <= s_tau[n]) {
                 const int q = s_q[n];
                 const unsigned long long key = ((unsigned long long)f2ord(score) << 32) | (unsigned long long)(uint32_t)arow[h];
@@ -388,8 +412,6 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
                   if (sl < p.cap) p.cand[(size_t)q * p.cap + sl] = key;
                 }
               }
-            } else if (p.mode == 0) {
-              if (t == 0 && r < TC_SAMPLE) p.sample[((size_t)I.sample_slot * TC_NQT + n) * TC_SAMPLE + r] = valid[h] ? score : TC_INF;
             } else if (inrange[h]) {
               p.dense[(size_t)s_q[n] * p.dense_ld + (I.row_begin + r)] = valid[h] ? score : TC_INF;
             }
@@ -406,13 +428,16 @@ struct TcMaps {
   CUtensorMap a, a32, b[4], a_lo, b_lo[4];
 };
 
-template <bool HALF>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
+// SAMPLE = true: the sample pass (mode 0) only; false: the capture (mode 1) and dense (mode 2) passes.
+template <bool HALF, bool SAMPLE>
+__global__ void __launch_bounds__(TcCfg<SAMPLE>::THREADS, TcCfg<SAMPLE>::MIN_CTAS)
+tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
+  using C = TcCfg<SAMPLE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
-  uint8_t* sB = smem + (size_t)TC_STAGES * TC_A_BYTES;
-  __shared__ __align__(8) uint64_t full_bar[TC_STAGES], empty_bar[TC_STAGES];
+  uint8_t* sB = smem + (size_t)C::STAGES * C::A_STAGE;
+  __shared__ __align__(8) uint64_t full_bar[C::STAGES], empty_bar[C::STAGES];
   __shared__ __align__(8) uint64_t sched_full[TC_SQ], sched_empty[TC_SQ];
   __shared__ int s_sched[TC_SQ];
   __shared__ float s_tau[2][TC_NQT];
@@ -420,33 +445,35 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_con
   __shared__ float s_qs[2][TC_NQT];
   // capture staging, one buffer per consumer warp: hits are appended with a shared-memory atomic and written out
   // (one global atomicAdd per hit, a whole warp of them in flight) when the item ends, so the score loop never
-  // waits on a global round trip
-  __shared__ unsigned long long s_hit_key[TC_CWARPS][TC_HITS];
-  __shared__ int s_hit_q[TC_CWARPS][TC_HITS];
-  __shared__ int s_hit_n[TC_CWARPS];
+  // waits on a global round trip.  The sample form captures nothing and keeps a one-entry placeholder.
+  constexpr int HW = SAMPLE ? 1 : C::CWARPS, HN = SAMPLE ? 1 : TC_HITS;
+  __shared__ unsigned long long s_hit_key[HW][HN];
+  __shared__ int s_hit_q[HW][HN];
+  __shared__ int s_hit_n[HW];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x < TC_CWARPS) s_hit_n[threadIdx.x] = 0;
-  if (warp == TC_CWARPS && lane == 0) {
+  const int mode = SAMPLE ? 0 : p.mode;
+  if (threadIdx.x < HW) s_hit_n[threadIdx.x] = 0;
+  if (warp == C::CWARPS && lane == 0) {
     prefetch_tmap(&maps.a); prefetch_tmap(&maps.a32);
     for (int i = 0; i < 4; ++i) prefetch_tmap(&maps.b[i]);
-    for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], TC_CWARPS); }
-    for (int i = 0; i < TC_SQ; ++i) { mbar_init(&sched_full[i], 1); mbar_init(&sched_empty[i], TC_CWARPS); }
+    for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], C::CWARPS); }
+    for (int i = 0; i < TC_SQ; ++i) { mbar_init(&sched_full[i], 1); mbar_init(&sched_empty[i], C::CWARPS); }
     fence_barrier_init();
   }
   __syncthreads();
-  const int nwork = p.mode == 0 ? p.totals[2] : p.totals[0];
+  const int nwork = mode == 0 ? p.totals[2] : p.totals[0];
   const int kbk = HALF ? 2 * TC_BK : TC_BK;  // elements per K block (128 B)
   const int kblocks = (p.d + kbk - 1) / kbk;
 
-  if (warp == TC_CWARPS) {
+  if (warp == C::CWARPS) {
     if (lane == 0) {  // ---------------- scheduler + TMA producer ----------------
       int stage = 0, slot = 0;
       uint32_t phase = 0, sphase = 0;
       for (;;) {
         mbar_wait(&sched_empty[slot], sphase ^ 1);
         const int w = atomicAdd(p.work_counter, 1);
-        const int it = w < nwork ? (p.mode == 0 ? p.sample_list[w] : w) : -1;
+        const int it = w < nwork ? (mode == 0 ? p.sample_list[w] : w) : -1;
         s_sched[slot] = it;
         mbar_arrive(&sched_full[slot]);
         if (++slot == TC_SQ) { slot = 0; sphase ^= 1; }
@@ -454,11 +481,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_con
         const TcItem I = p.items[it];
         const long long base_row = p.list_off[I.list] + I.row_begin;
         int rows = I.row_end - I.row_begin;
-        if (p.mode == 0) rows = min(rows, TC_SAMPLE);
+        if (mode == 0) rows = min(rows, TC_SAMPLE);
         const int ntiles = (rows + TC_BM - 1) / TC_BM;
         const int bl = tc_bcols_log(I.nq);
         const CUtensorMap* tb = &maps.b[bl];
-        const bool small_a = p.mode == 0;  // 32-row sample box, else the full 128-row tile
+        const bool small_a = mode == 0;  // 32-row sample box, else the full 128-row tile
         const CUtensorMap* ta = small_a ? &maps.a32 : &maps.a;
         const uint32_t bytes = (small_a ? (uint32_t)(TC_SAMPLE * 128) : TC_A_BYTES) + (16u << bl) * 128u;
         const CUtensorMap* tbl = &maps.b_lo[bl];
@@ -468,31 +495,31 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_con
             // last tile of a list: fetch only the 32-row boxes that hold list rows (the rest of the stage keeps stale
             // data, whose scores the epilogue masks) instead of streaming up to 127 rows of the neighbouring list
             const int trows = rows - t * TC_BM;
-            const int nbox = (p.mode == 1 && (HALF || !p.split) && trows <= TC_BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
+            const int nbox = (mode == 1 && (HALF || !p.split) && trows <= TC_BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
             const uint32_t saved = nbox ? TC_A_BYTES - (uint32_t)nbox * (TC_SAMPLE * 128) : 0u;
             mbar_arrive_expect_tx(&full_bar[stage], bytes - saved);
             if (nbox) {
               for (int j = 0; j < nbox; ++j)
-                tma_load_2d(sA + (size_t)stage * TC_A_BYTES + (size_t)j * (TC_SAMPLE * 128), &maps.a32, &full_bar[stage], kb * kbk,
+                tma_load_2d(sA + (size_t)stage * C::A_STAGE + (size_t)j * (TC_SAMPLE * 128), &maps.a32, &full_bar[stage], kb * kbk,
                             (int)(base_row + (long long)t * TC_BM + j * TC_SAMPLE), kEvictFirst);
             } else
-            tma_load_2d(sA + (size_t)stage * TC_A_BYTES, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
-            tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tb, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
-            if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-            if (!HALF && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
+            tma_load_2d(sA + (size_t)stage * C::A_STAGE, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+            tma_load_2d(sB + (size_t)stage * C::B_STAGE, tb, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
+            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+            if (!HALF && !SAMPLE && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
               mbar_wait(&empty_bar[stage], phase ^ 1);
               mbar_arrive_expect_tx(&full_bar[stage], bytes);
-              tma_load_2d(sA + (size_t)stage * TC_A_BYTES, &maps.a_lo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
-              tma_load_2d(sB + (size_t)stage * TC_B_BYTES, tbl, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
-              if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+              tma_load_2d(sA + (size_t)stage * C::A_STAGE, &maps.a_lo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+              tma_load_2d(sB + (size_t)stage * C::B_STAGE, tbl, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
+              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
           }
       }
     }
     return;
   }
-  // ---------------- consumers: warps 0-7 ----------------
-  TcRing ring;
+  // ---------------- consumers: warps 0 .. CWARPS - 1 ----------------
+  TcRing<C::STAGES> ring;
   uint32_t sphase = 0;
   int slot = 0;
   for (int icount = 0;; ++icount) {
@@ -508,29 +535,30 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_scan_kernel(const __grid_con
     if (et < I.nq) {
       const int q = p.pair_query ? p.pair_query[I.pair_begin + et] : I.pair_begin + et;
       s_q[buf][et] = q;
-      s_tau[buf][et] = p.mode == 1 ? p.tau[q] : 0.f;
+      s_tau[buf][et] = mode == 1 ? p.tau[q] : 0.f;
       if (HALF) s_qs[buf][et] = p.qscale[q];
     }
-    asm volatile("bar.sync 1, %0;" ::"n"(TC_CWARPS * 32) : "memory");
+    asm volatile("bar.sync 1, %0;" ::"n"(C::CWARPS * 32) : "memory");
+    const int hw = SAMPLE ? 0 : warp;
     auto consume = [&](auto n) {
-      tc_consume_item<HALF, decltype(n)::value>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf],
-                                                s_hit_key[warp], s_hit_q[warp], &s_hit_n[warp]);
+      tc_consume_item<HALF, decltype(n)::value, C>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf],
+                                                   s_hit_key[hw], s_hit_q[hw], &s_hit_n[hw]);
     };
     const int bl = tc_bcols_log(I.nq);
     if (bl == 0) consume(std::integral_constant<int, 16>());
     else if (bl == 1) consume(std::integral_constant<int, 32>());
     else if (bl == 2) consume(std::integral_constant<int, 64>());
     else consume(std::integral_constant<int, 128>());
-    if (p.mode == 1) {  // flush this warp's staged hits
+    if (mode == 1) {  // flush this warp's staged hits
       __syncwarp();
-      const int nh = min(s_hit_n[warp], TC_HITS);
+      const int nh = min(s_hit_n[hw], TC_HITS);
       for (int i = lane; i < nh; i += 32) {
-        const int q = s_hit_q[warp][i];
+        const int q = s_hit_q[hw][i];
         const int sl = atomicAdd(p.cand_cnt + q, 1);
-        if (sl < p.cap) p.cand[(size_t)q * p.cap + sl] = s_hit_key[warp][i];
+        if (sl < p.cap) p.cand[(size_t)q * p.cap + sl] = s_hit_key[hw][i];
       }
       __syncwarp();
-      if (lane == 0) s_hit_n[warp] = 0;
+      if (lane == 0) s_hit_n[hw] = 0;
       __syncwarp();
     }
   }
@@ -1202,23 +1230,43 @@ static int tc_cand_cap(int k) { return std::min(16384, std::max(8192, next_pow2(
 // Per-device one-time setup: cudaFuncSetAttribute applies to the CURRENT device only, and one process may hold indexes
 // on several GPUs (b200vs_params.device), so the opt-in shared-memory limits are raised once per device ordinal.
 constexpr int TC_MAX_DEVICES = 64;
+struct TcDevice {
+  int sms = 0;
+  int sample_ctas[2] = {0, 0};  // resident CTAs per SM of the sample form, [HALF]
+};
 static std::mutex g_tc_init_mu;
-static int g_dev_sms[TC_MAX_DEVICES] = {0};
-static int tc_init(int device) {
+static TcDevice g_tc_dev[TC_MAX_DEVICES];
+
+template <bool HALF>
+static int tc_sample_ctas_per_sm() {
+  using C = TcCfg<true>;
+  auto* kernel = tc_scan_kernel<HALF, true>;
+  B200VS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  int n = 0;
+  B200VS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, C::THREADS, C::SMEM));
+  if (getenv("B200VS_DEBUG_FLAGS")) fprintf(stderr, "[b200vs] tc sample kernel (%s): %d CTAs per SM\n", HALF ? "fp16" : "tf32", n);
+  return std::max(1, n);
+}
+
+static TcDevice tc_init(int device) {
   if (device < 0 || device >= TC_MAX_DEVICES) fail(B200VS_EILLEGAL_PARAMETERS, "bad CUDA device ordinal");
   std::lock_guard<std::mutex> g(g_tc_init_mu);
-  if (g_dev_sms[device]) return g_dev_sms[device];
-  const int sms = device_sm_count(device);
-  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
+  if (g_tc_dev[device].sms) return g_tc_dev[device];
+  TcDevice dev;
+  dev.sms = device_sm_count(device);
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<false>::SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<false>::SMEM));
+  dev.sample_ctas[0] = tc_sample_ctas_per_sm<false>();
+  dev.sample_ctas[1] = tc_sample_ctas_per_sm<true>();
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  g_dev_sms[device] = sms;  // only after every attribute call succeeded
-  return sms;
+  g_tc_dev[device] = dev;  // only after every attribute call succeeded
+  return dev;
 }
 
 bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc) {
@@ -1266,15 +1314,14 @@ struct TcPlan {
   TcItem* items;
   int64_t bound, sbound, npairs;
   TcMaps maps;
-  int num_sms;
+  TcDevice dev;
 };
 
 static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {
-  const int num_sms = tc_init(ix->device);
   const int d = ix->dim;
   auto& S = ix->scratch;
   TcPlan P;
-  P.num_sms = num_sms;
+  P.dev = tc_init(ix->device);
   P.npairs = nq * nprobe;
   P.bound = tc_item_bound(v, P.npairs);
   P.sbound = tc_sample_bound(v, P.npairs);
@@ -1313,11 +1360,20 @@ static TcParams tc_params(const TcView& v, int d, bool l2, const TcItem* items, 
   return p;
 }
 
-// One persistent launch of the tile kernel: at most one CTA per SM and per work item.
-static void tc_launch(bool half, int num_sms, int64_t work_bound, const TcMaps& maps, const TcParams& p, cudaStream_t s) {
-  const int grid = (int)std::min<int64_t>(num_sms, std::max<int64_t>(1, work_bound));
-  auto* kernel = half ? tc_scan_kernel<true> : tc_scan_kernel<false>;
-  kernel<<<grid, TC_THREADS, TC_SMEM, s>>>(maps, p);
+// One persistent launch of the tile kernel, at most one CTA per work item: the sample pass (mode 0) runs the sample form
+// with as many CTAs per SM as fit, the other passes one capture-form CTA per SM.  All CTAs draw items from the same
+// work counter, so a loose work_bound (a host-side bound on the item count) costs no more than one empty claim per CTA.
+static void tc_launch(const TcDevice& dev, bool half, int64_t work_bound, const TcMaps& maps, const TcParams& p, cudaStream_t s) {
+  const bool sample = p.mode == 0;
+  const int64_t slots = (int64_t)dev.sms * (sample ? dev.sample_ctas[half ? 1 : 0] : 1);
+  const int grid = (int)std::min<int64_t>(slots, std::max<int64_t>(1, work_bound));
+  if (sample) {
+    auto* kernel = half ? tc_scan_kernel<true, true> : tc_scan_kernel<false, true>;
+    kernel<<<grid, TcCfg<true>::THREADS, TcCfg<true>::SMEM, s>>>(maps, p);
+  } else {
+    auto* kernel = half ? tc_scan_kernel<true, false> : tc_scan_kernel<false, false>;
+    kernel<<<grid, TcCfg<false>::THREADS, TcCfg<false>::SMEM, s>>>(maps, p);
+  }
   B200VS_CUDA(cudaGetLastError());
 }
 
@@ -1350,7 +1406,7 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   // 1) sample pass -> per-query capture thresholds
   p.mode = 0; p.work_counter = P.work;
   ix->phase(IndexBase::PH_SAMPLE, s);
-  tc_launch(P.half, P.num_sms, P.sbound, P.maps, p, s);
+  tc_launch(P.dev, P.half, P.sbound, P.maps, p, s);
   ix->phase(IndexBase::PH_TAU, s);
   int* redo = S.alloc<int>(nq);
   // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
@@ -1362,7 +1418,7 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   ix->phase(IndexBase::PH_CAPTURE, s);
   {
     ScopedKernelTimer timer(ix, s, ix->profiling);
-    tc_launch(P.half, P.num_sms, P.bound, P.maps, p, s);
+    tc_launch(P.dev, P.half, P.bound, P.maps, p, s);
     timer.stop();
   }
   // 3) window select + exact rerank + certification
@@ -1433,23 +1489,33 @@ bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe) 
 // stage).  hscale != nullptr: qr.op and a_hi are scaled FP16 (the list scan's FP16 arithmetic), qr.scale / hscale their scales.
 static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const TcQueries& qr, const void* a_hi, const float* a_lo,
                           const float* hscale, float* dense, cudaStream_t s) {
-  const int num_sms = tc_init(ix->device);
+  const TcDevice dev = tc_init(ix->device);
   const int d = ix->dim;
   const int nrows = (int)v.arena_rows;
   const bool half = hscale != nullptr;
   auto& S = ix->scratch;
   const int chunk = nrows <= 16384 ? TC_BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
-  const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, TC_NQT));
+  // Query-group width (the wgmma N): with every item MMA-bound, the launch takes about (waves of items over the SMs) x
+  // (width).  Take the widest group that minimises that product: at 1024 centroids x 1024 queries on 132 SMs, 128 items of
+  // 64 queries instead of 64 items of 128 (half the chip idle).  Narrower ties (256 items of 32) re-read the row tiles from
+  // L2 twice as often for no less MMA time.  A score does not depend on the width: each element's K order is the same.
+  int nqt = TC_NQT;
+  int64_t best = INT64_MAX;
+  for (int w = TC_NQT; w >= 16; w >>= 1) {
+    const int64_t cost = cdiv(cdiv(nrows, chunk) * cdiv(nq, w), dev.sms) * w;
+    if (cost < best) { best = cost; nqt = w; }
+  }
+  const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, nqt));
   TcItem* items = S.alloc<TcItem>(nitems);
   int* totals = S.alloc<int>(4);
   int* work = S.alloc<int>(4);
   B200VS_CUDA(cudaMemsetAsync(work, 0, 16, s));
-  tc_coarse_items_kernel<<<(unsigned)cdiv(nitems, 128), 128, 0, s>>>(nrows, (int)nq, chunk, items, totals);
+  tc_coarse_items_kernel<<<(unsigned)cdiv(nitems, 128), 128, 0, s>>>(nrows, (int)nq, chunk, nqt, items, totals);
   TcParams p = tc_params(v, d, l2, items, totals, hscale, qr.scale);
   p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.work_counter = work; p.split = qr.lo != nullptr ? 1 : 0;
   const TcMaps maps = make_tc_maps(a_hi, a_lo, nrows, qr.op, qr.lo, nq, d, half);
   ix->phase(IndexBase::PH_COARSE_SCAN, s);
-  tc_launch(half, num_sms, nitems, maps, p, s);
+  tc_launch(dev, half, nitems, maps, p, s);
 }
 
 // The register-select finish of the coarse pass, in its warp form (HYBRID: 32 threads hold the score row) or its block form
@@ -1518,11 +1584,30 @@ static __global__ void tc_eps_kernel(const float* __restrict__ qnorm, long long 
   if (i < nq) out[i] = tc_eps(l2 != 0, qnorm[i], max_norm, d, arith);
 }
 
-void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, float* out_scores,
-                     float* out_eps, cudaStream_t s) {
+// Diagnostics: the sample pass's scores on a one-list (Flat) view, scattered to out [nq, nrows].  Query q sits in column
+// pos[q] % TC_NQT of query group pos[q] / TC_NQT; span sp of the list is sampled by that group's item of chunk
+// sp * TC_SPAN / TC_CHUNK (the lookup tc_tau_warp_kernel makes).  One thread per (query, span, sampled row).
+static __global__ void tc_debug_sample_scores_kernel(const int* __restrict__ pos, const int* __restrict__ cnt,
+                                                     const int* __restrict__ item_off, const TcItem* __restrict__ items,
+                                                     const float* __restrict__ sample, long long nq, int nrows, float* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int nspan = (nrows + TC_SPAN - 1) / TC_SPAN;
+  if (i >= nq * nspan * TC_SAMPLE) return;
+  const int r = (int)(i % TC_SAMPLE), sp = (int)(i / TC_SAMPLE % nspan);
+  const long long q = i / ((long long)TC_SAMPLE * nspan);
+  const int row = sp * TC_SPAN + r;
+  if (row >= nrows) return;
+  const int ng = (cnt[0] + TC_NQT - 1) / TC_NQT, g = pos[q] / TC_NQT, n = pos[q] % TC_NQT;
+  const int slot = items[item_off[0] + sp * (TC_SPAN / TC_CHUNK) * ng + g].sample_slot;
+  out[(size_t)q * nrows + row] = sample[((size_t)slot * TC_NQT + n) * TC_SAMPLE + r];
+}
+
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, bool sample,
+                     float* out_scores, float* out_eps, cudaStream_t s) {
   const int d = ix->dim;
   auto& S = ix->scratch;
   const bool split = arith == TC_ARITH_SPLIT, half = arith == TC_ARITH_FP16;
+  if (sample && (split || !v.flat)) fail(B200VS_EILLEGAL_PARAMETERS, "sample-pass scores exist for one-list views in the list-scan arithmetic");
   const TcQueries qr = tc_round_queries(ix, arith, nq, q, s);
   if (v.arena_rows > 0) {
     const void* a_hi = v.vecs;
@@ -1538,7 +1623,24 @@ void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const 
       launch_half_rows(v.vecs, nullptr, v.arena_rows, d, h, sc, s);
       a_hi = h; hscale = sc;
     }
-    tc_dense_scan(ix, v, l2, nq, qr, a_hi, a_lo, hscale, out_scores, s);
+    if (!sample) {
+      tc_dense_scan(ix, v, l2, nq, qr, a_hi, a_lo, hscale, out_scores, s);
+    } else {  // the search's own planning and sample launch, every query probing the one list
+      TcView sv = v;
+      sv.vecs_h = half ? static_cast<const __half*>(a_hi) : nullptr;
+      sv.hscale = hscale;
+      long long* probes = S.alloc<long long>(nq);
+      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
+      const TcPlan P = tc_prepare(ix, sv, nq, q, probes, 1, s);
+      float* smp = S.alloc<float>((size_t)P.sbound * TC_NQT * TC_SAMPLE);
+      TcParams p = tc_params(sv, d, l2, P.items, P.totals, sv.hscale, P.qry.scale);
+      p.sample_list = P.sample_list; p.pair_query = P.pair_query; p.sample = smp;
+      p.mode = 0; p.work_counter = P.work;
+      tc_launch(P.dev, P.half, P.sbound, P.maps, p, s);
+      B200VS_CUDA(cudaMemsetAsync(out_scores, 0xFF, (size_t)nq * v.arena_rows * 4, s));  // NaN: not sampled
+      const int64_t n = nq * cdiv(v.arena_rows, TC_SPAN) * TC_SAMPLE;
+      tc_debug_sample_scores_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(P.pos, P.cnt, P.item_off, P.items, smp, nq, (int)v.arena_rows, out_scores);
+    }
   }
   tc_eps_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(qr.norm, nq, l2 ? 1 : 0, v.max_norm, d, arith, out_eps);
   B200VS_CUDA(cudaGetLastError());

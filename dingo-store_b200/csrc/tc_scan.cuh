@@ -25,8 +25,6 @@ namespace b200vs {
 constexpr int TC_BM = 128;        // database rows per tile (two warpgroups x wgmma M = 64)
 constexpr int TC_BK = 32;         // floats per K block = 128 B = one swizzle span (64 halves on the FP16 path)
 constexpr int TC_NQT = 128;       // queries per work item (wgmma N <= 128): a probed list chunk is re-streamed only beyond 128 queries
-constexpr int TC_STAGES = 6;      // TMA->MMA ring depth (6 x 32 KB; + 24 KB of capture staging: ~220 KB, the bytes in flight bound the HBM rate; DESIGN §4.2)
-constexpr int TC_THREADS = 288;   // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA + scheduler
 constexpr int TC_CHUNK = 512;     // rows per work item (list chunk): fine grain for dynamic load balance
 constexpr int TC_SPAN = 2048;     // one sampled chunk per TC_SPAN rows of a list
 constexpr int TC_HITS = 256;      // captured rows staged per consumer warp between flushes
@@ -34,7 +32,6 @@ constexpr int TC_SAMPLE = 32;     // sampled rows per span for the threshold est
 constexpr int TC_SQ = 4;          // scheduler queue depth (items the producer may run ahead)
 constexpr uint32_t TC_A_BYTES = TC_BM * 128;
 constexpr uint32_t TC_B_BYTES = TC_NQT * 128;
-constexpr size_t TC_SMEM = (size_t)TC_STAGES * (TC_A_BYTES + TC_B_BYTES) + 1024;
 
 struct TcItem {
   int list;
@@ -117,8 +114,10 @@ void tc_coarse(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
 // prepared) against every arena row, out_scores [nq, v.arena_rows], and the tc_eps() the finish kernels use, out_eps [nq].
 // arith: TC_ARITH_TF32 = list scan without a mirror, TC_ARITH_SPLIT = the coarse pass's hi / lo arithmetic,
 // TC_ARITH_FP16 = list scan on an FP16 mirror (a temporary one is made from v.vecs inside the call).
-void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, float* out_scores,
-                     float* out_eps, cudaStream_t s);
+// sample (v.flat, TC_ARITH_TF32 or TC_ARITH_FP16): the sample pass's scores instead, from the kernel's sample
+// configuration, for the rows it samples (the first TC_SAMPLE rows of every TC_SPAN); every other row is NaN.
+void tc_debug_scores(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, TcArith arith, bool sample,
+                     float* out_scores, float* out_eps, cudaStream_t s);
 
 float device_max_norm(IndexBase* ix, const float* norms_sq, int64_t n, cudaStream_t s);  // sqrt(max ||x||^2)
 void launch_row_norms(const float* x, int64_t n, int d, float* out, cudaStream_t s);     // out[i] = <x_i, x_i>

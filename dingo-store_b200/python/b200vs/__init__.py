@@ -341,16 +341,20 @@ class Index:
     def set_profiling(self, on):
         _check(self.L.b200vs_set_profiling(self.h, int(bool(on))))
 
-    def tc_scores(self, xq, split=False, half=False):
+    def tc_scores(self, xq, split=False, half=False, sample=False):
         """Diagnostics (FLAT): the tile kernel's approximate scores [nq, rows] of every stored row (storage order,
         tombstoned rows +inf) and the per-query error bound eps [nq] the finish kernels use.  split: the coarse pass's
-        hi / lo arithmetic; half: the FP16 arithmetic of an IVF-Flat list scan on its FP16 mirror; neither: TF32."""
+        hi / lo arithmetic; half: the FP16 arithmetic of an IVF-Flat list scan on its FP16 mirror; neither: TF32.
+        sample: the threshold sample pass's scores (TF32, or FP16 with half) for the rows it samples, NaN elsewhere."""
         xq = _f32(xq)
         nq = xq.shape[0]
         rows = self.get_count() + self.get_deleted_count()
         S = np.zeros((nq, rows), dtype=np.float32)
         E = np.zeros(nq, dtype=np.float32)
-        _check(self.L.b200vs_debug_tc_scores(self.h, nq, xq.ctypes.data if xq.size else None, 2 if half else int(bool(split)),
+        if sample and split:
+            raise ValueError("the sample pass has no split arithmetic")
+        mode = (4 if half else 3) if sample else (2 if half else int(bool(split)))
+        _check(self.L.b200vs_debug_tc_scores(self.h, nq, xq.ctypes.data if xq.size else None, mode,
                                              S.ctypes.data, E.ctypes.data))
         return S, E
 

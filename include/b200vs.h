@@ -317,10 +317,12 @@ int b200vs_set_profiling(b200vs_index* idx, int on);
 /* Diagnostics (tests only): the tile kernel's approximate scores of a FLAT index's rows.  split = 0: list-scan
  * arithmetic without an FP16 mirror (rows truncated by the tensor core, queries rounded to TF32); split = 1: the coarse
  * pass's hi/lo arithmetic; split = 2: the list scan on an IVF-Flat FP16 mirror (rows and queries scaled by powers of two
- * and rounded to FP16; needs dim % 8 == 0).  xq [nq, dim] RAW (normalised inside for COSINE, as search does); out_scores [nq, rows] with rows =
+ * and rounded to FP16; needs dim % 8 == 0).  split = 3 / 4: the threshold sample pass's scores in the arithmetic of
+ * split = 0 / 2, from the tile kernel's sample configuration, for the rows it samples (the first 32 rows of every
+ * 2048-row span, with the index as one list); every other row is NaN.  xq [nq, dim] RAW (normalised inside for COSINE, as search does); out_scores [nq, rows] with rows =
  * count + deleted count in storage order (L2: ||x||^2 - 2<q,x>; IP / cosine: -<q,x>; tombstoned rows +inf);
  * out_eps [nq] = the tc_eps() value the finish kernels use for that query and mode.  Non-FLAT indexes, dim % 4 != 0,
- * dim < 32, split = 2 with dim % 8 != 0 and any other split value: EILLEGAL_PARAMETERS. */
+ * dim < 32, split = 2 or 4 with dim % 8 != 0 and any other split value: EILLEGAL_PARAMETERS. */
 int b200vs_debug_tc_scores(b200vs_index* idx, int64_t nq, const float* xq, int32_t split, float* out_scores, float* out_eps);
 
 const char* b200vs_last_error(void);
