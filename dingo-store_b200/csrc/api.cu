@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "index.h"
+#include "ivf_common.h"
 
 using namespace b200vs;
 
@@ -703,6 +704,105 @@ int b200vs_scan_finish(b200vs_scan* st, float* out_dist, int64_t* out_ids) {
 }
 
 void b200vs_scan_abort(b200vs_scan* st) { delete st; }
+
+// ---- streaming brute-force range scan: VectorReader::BruteForceRangeSearch (src/vector/vector_reader.cc:2050-2202) ----
+// No temporary index: each pushed tile goes straight to range_append_kernel, which appends its hits in row order.
+struct b200vs_scan_range {
+  int device = 0;
+  int dim = 0;
+  int64_t nq = 0;
+  int max_results = 0;
+  bool l2 = true, cosine = false;
+  float thr_raw = 0;  // L2: dist < radius; IP / cosine: ip > 1 - radius (vector_index_flat.cc:282-285)
+  SearchCtx sc;       // sc.sorted_ids_dev points into allow
+  cudaStream_t s = nullptr;
+  DevBuf<float> q, x, out_d;  // queries [nq, dim], tile [rows, dim], results [nq, max_results]
+  DevBuf<long long> ids, allow, out_i;
+  DevBuf<int> counts;         // [nq] hits kept so far
+  ~b200vs_scan_range() {
+    cudaSetDevice(device);
+    if (s) cudaStreamSynchronize(s);
+    q.free(); x.free(); out_d.free(); ids.free(); allow.free(); out_i.free(); counts.free();
+    if (s) cudaStreamDestroy(s);
+  }
+};
+
+int b200vs_scan_range_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t nq, const float* xq, float radius,
+                            int32_t max_results, const b200vs_search_params* sp, b200vs_scan_range** out) {
+  return guarded([&]() -> int {
+    if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
+    *out = nullptr;
+    if (dim <= 0) fail(B200VS_EVECTOR_INVALID, "vector index dimension is invalid");  // as b200vs_scan_begin
+    if (metric == B200VS_HAMMING) fail(B200VS_EVECTOR_NOT_SUPPORT, "brute-force scan of binary vectors is not implemented");
+    if (metric != B200VS_L2 && metric != B200VS_IP && metric != B200VS_COSINE) fail(B200VS_EILLEGAL_PARAMETERS, "unsupported metric type");
+    if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+    if (max_results <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be > 0");
+    std::unique_ptr<b200vs_scan_range> st(new b200vs_scan_range());
+    st->device = device; st->dim = dim; st->nq = nq; st->max_results = max_results;
+    st->l2 = metric == B200VS_L2;
+    st->cosine = metric == B200VS_COSINE;
+    st->thr_raw = st->l2 ? radius : 1.0F - radius;
+    B200VS_CUDA(cudaSetDevice(device));
+    B200VS_CUDA(cudaStreamCreateWithFlags(&st->s, cudaStreamNonBlocking));
+    const size_t nr = (size_t)nq * max_results;
+    st->q.reserve((size_t)nq * dim, 0, st->s);
+    st->out_d.reserve(nr, 0, st->s); st->out_i.reserve(nr, 0, st->s); st->counts.reserve((size_t)nq, 0, st->s);
+    if (sp) {  // the filters as make_ctx resolves them for an index search, copied: the caller's list need not outlive begin
+      st->sc.has_range = sp->has_range; st->sc.negate = sp->negate; st->sc.rmin = sp->range_min; st->sc.rmax = sp->range_max;
+      if (sp->sorted_ids) {
+        st->allow.reserve((size_t)std::max<int64_t>(sp->n_ids, 1), 0, st->s);
+        if (sp->n_ids > 0) B200VS_CUDA(cudaMemcpyAsync(st->allow.p, sp->sorted_ids, (size_t)sp->n_ids * 8, cudaMemcpyHostToDevice, st->s));
+        st->sc.sorted_ids_dev = st->allow.p;
+        st->sc.n_ids = sp->n_ids;
+      }
+    }
+    B200VS_CUDA(cudaMemcpyAsync(st->q.p, xq, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, st->s));
+    if (st->cosine) launch_normalize_faiss(st->q.p, nq, dim, st->s);  // NormalizeVectorForFaiss, as a Flat index searches
+    B200VS_CUDA(cudaMemsetAsync(st->out_d.p, 0, nr * 4, st->s));
+    B200VS_CUDA(cudaMemsetAsync(st->out_i.p, 0xFF, nr * 8, st->s));  // id -1 = empty slot
+    B200VS_CUDA(cudaMemsetAsync(st->counts.p, 0, (size_t)nq * 4, st->s));
+    B200VS_CUDA(cudaStreamSynchronize(st->s));
+    *out = st.release();
+    return B200VS_OK;
+  });
+}
+
+int b200vs_scan_range_push(b200vs_scan_range* st, int64_t n, const float* x, const int64_t* ids) {
+  return guarded([&]() -> int {
+    if (!st) fail(B200VS_EILLEGAL_PARAMETERS, "null scan handle");
+    if (n <= 0) return B200VS_OK;
+    if (!x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "null tile");
+    check_batch_ids_unique(n, ids);  // the Flat add of the reference's per-tile index refuses a repeated id
+    B200VS_CUDA(cudaSetDevice(st->device));
+    st->x.reserve((size_t)n * st->dim, 0, st->s);
+    st->ids.reserve((size_t)n, 0, st->s);
+    B200VS_CUDA(cudaMemcpyAsync(st->x.p, x, (size_t)n * st->dim * 4, cudaMemcpyHostToDevice, st->s));
+    B200VS_CUDA(cudaMemcpyAsync(st->ids.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, st->s));
+    if (st->cosine) launch_normalize_faiss(st->x.p, n, st->dim, st->s);  // vector_index_flat.cc:155
+    launch_range_append(st->l2, st->x.p, st->ids.p, n, st->dim, st->nq, st->q.p, st->sc, st->thr_raw, st->max_results,
+                        st->out_d.p, st->out_i.p, st->counts.p, st->s);
+    B200VS_CUDA(cudaStreamSynchronize(st->s));  // the caller may reuse its buffers, and the next push rewrites the tile
+    return B200VS_OK;
+  });
+}
+
+int b200vs_scan_range_finish(b200vs_scan_range* st, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  const int rc = guarded([&]() -> int {
+    if (!st) fail(B200VS_EILLEGAL_PARAMETERS, "null scan handle");
+    if (!out_dist || !out_ids || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    B200VS_CUDA(cudaSetDevice(st->device));
+    const size_t nr = (size_t)st->nq * st->max_results;
+    B200VS_CUDA(cudaMemcpyAsync(out_dist, st->out_d.p, nr * 4, cudaMemcpyDeviceToHost, st->s));
+    B200VS_CUDA(cudaMemcpyAsync(out_ids, st->out_i.p, nr * 8, cudaMemcpyDeviceToHost, st->s));
+    B200VS_CUDA(cudaMemcpyAsync(out_counts, st->counts.p, (size_t)st->nq * 4, cudaMemcpyDeviceToHost, st->s));
+    B200VS_CUDA(cudaStreamSynchronize(st->s));
+    return B200VS_OK;
+  });
+  delete st;
+  return rc;
+}
+
+void b200vs_scan_range_abort(b200vs_scan_range* st) { delete st; }
 
 // ---- binary indexes (binary.cu): packed rows, dim / 8 bytes each ----
 int b200vs_train_binary(b200vs_index* h, int64_t n, const uint8_t* x) {

@@ -407,6 +407,11 @@ struct ScopedKernelTimer {  // CUDA events on the launching stream; synchronises
 void run_scan(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* out_dist,
               float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s);
 
+// b200vs_scan_range_push: append the hits of one tile [n, d] to each query's running list in row order (range_append_kernel).
+// thr_raw is the raw threshold (L2: dist < thr; IP: ip > thr); counts[nq] persists across calls.
+void launch_range_append(bool l2, const float* vecs, const long long* ids, int64_t n, int d, int64_t nq, const float* queries,
+                         const SearchCtx& sc, float thr_raw, int max_results, float* out_dist, long long* out_ids, int* counts,
+                         cudaStream_t s);
 void launch_normalize_faiss(float* x, int64_t n, int d, cudaStream_t s);
 void launch_normalize_hnsw(const float* x, float* out, int64_t n, int d, cudaStream_t s);
 void launch_scatter_rows(const float* src, const long long* src_ids, const long long* slots, int64_t n, int d,

@@ -96,6 +96,27 @@ static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const f
   ix->launch_count(2);
 }
 
+void launch_range_append(bool l2, const float* vecs, const long long* ids, int64_t n, int d, int64_t nq, const float* queries,
+                         const SearchCtx& sc, float thr_raw, int max_results, float* out_dist, long long* out_ids, int* counts,
+                         cudaStream_t s) {
+  if (n <= 0 || nq <= 0) return;
+  RangeAppendArgs a;
+  a.vecs = vecs; a.ids = ids; a.n = n; a.d = d; a.queries = queries;
+  a.filt.has_range = sc.has_range; a.filt.negate = sc.negate; a.filt.rmin = sc.rmin; a.filt.rmax = sc.rmax;
+  a.filt.sorted_ids = sc.sorted_ids_dev; a.filt.n_ids = sc.n_ids;
+  a.thr_key = f2ord(l2 ? thr_raw : -thr_raw);
+  a.max_results = max_results; a.out_dist = out_dist; a.out_ids = out_ids; a.counts = counts;
+  const size_t smem = range_append_smem_bytes(d);
+  if (l2) {
+    ensure_smem(range_append_kernel<Fp32Dist<true>>, smem);
+    range_append_kernel<Fp32Dist<true>><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(a);
+  } else {
+    ensure_smem(range_append_kernel<Fp32Dist<false>>, smem);
+    range_append_kernel<Fp32Dist<false>><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(a);
+  }
+  B200VS_CUDA(cudaGetLastError());
+}
+
 __global__ void mark_probed_kernel(const long long* probes, long long n, int* flags) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && probes[i] >= 0) flags[probes[i]] = 1;

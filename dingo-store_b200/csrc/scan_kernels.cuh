@@ -171,6 +171,84 @@ static __global__ void __launch_bounds__(SCAN_THREADS) scan_select_kernel(const 
   }
 }
 
+// Ordered range append (b200vs_scan_range_push, VectorReader::BruteForceRangeSearch): the hits of one tile are appended
+// to each query's running list in row order, until the list holds max_results.  One CTA per query (blockIdx.x, so more
+// than 65535 queries fit); the CTA walks the rows SCAN_QUADS at a time, one quad per row, and compacts the step's hits
+// with warp ballots and a prefix over the warps.  No atomics: the result does not depend on scheduling.
+struct RangeAppendArgs {
+  const float* vecs;      // [n, d] tile (normalised for cosine)
+  const long long* ids;   // [n], < 0 = never a hit
+  long long n;
+  int d;
+  const float* queries;   // [nq, d] (normalised for cosine)
+  FilterDev filt;
+  uint32_t thr_key;       // hit: f2ord(L2 ? dist : -ip) < thr_key (L2: dist < radius; IP: ip > 1 - radius)
+  int max_results;
+  float* out_dist;        // [nq, max_results] API distances
+  long long* out_ids;     // [nq, max_results]
+  int* counts;            // [nq] hits kept so far; read and written back by every launch
+};
+
+constexpr int RANGE_WARPS = SCAN_THREADS / 32;
+// dynamic shared memory: the query (16-byte padded), then the per-warp hit counts of two steps
+inline size_t range_append_smem_bytes(int d) { return ((size_t)d * 4 + 15) / 16 * 16 + 2 * RANGE_WARPS * sizeof(int); }
+
+template <class Dist>
+static __global__ void __launch_bounds__(SCAN_THREADS) range_append_kernel(const RangeAppendArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  constexpr int kWarps = RANGE_WARPS;
+  const long long qi = blockIdx.x;
+  int count = a.counts[qi];
+  if (count >= a.max_results) return;
+  const int d = a.d;
+  float* qs = reinterpret_cast<float*>(smem);
+  // per-step hit count of each warp, double-buffered: one barrier per step
+  int (*warp_hits)[kWarps] = reinterpret_cast<int (*)[kWarps]>(smem + ((size_t)d * 4 + 15) / 16 * 16);
+  for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = a.queries[(size_t)qi * d + i];
+  __syncthreads();
+  const int quad = threadIdx.x >> 2, t = threadIdx.x & 3, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool vec = (d & 3) == 0;
+  float* od = a.out_dist + (size_t)qi * a.max_results;
+  long long* oi = a.out_ids + (size_t)qi * a.max_results;
+  int buf = 0;
+  for (long long base = 0; base < a.n; base += SCAN_QUADS) {
+    const long long row = base + quad;
+    bool valid = row < a.n;
+    long long id = -1;
+    if (valid) {
+      id = a.ids[row];
+      valid = id >= 0 && filter_pass(a.filt, id);
+    }
+    bool hit = false;
+    float v = 0.f;
+    if (__ballot_sync(0xffffffffu, valid) != 0u) {  // warp-uniform skip
+      v = Dist::eval(a.vecs, row < a.n ? row : base, qs, d, t, vec);
+      hit = valid && f2ord(Dist::kL2 ? v : -v) < a.thr_key;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, hit && t == 0);  // bit 4j = row base + 8 warp + j
+    if (lane == 0) warp_hits[buf][warp] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) {
+      const int c = warp_hits[buf][w];
+      before += w < warp ? c : 0;
+      total += c;
+    }
+    if (hit && t == 0) {
+      const int pos = count + before + __popc(m & ((1u << lane) - 1u));
+      if (pos < a.max_results) {
+        od[pos] = Dist::kL2 ? v : __fsub_rn(1.0f, v);  // FillRangeSearchResult: squared L2, or 1 - ip
+        oi[pos] = id;
+      }
+    }
+    count += total;
+    buf ^= 1;
+    if (count >= a.max_results) break;  // block-uniform: every thread summed the same counts
+  }
+  if (threadIdx.x == 0) a.counts[qi] = min(count, a.max_results);
+}
+
 // Merge the per-split partial lists of each query and emit results.
 //   out_dist: API semantics (L2: squared distance; IP: 1 - ip)        [nq, k] or NULL
 //   out_raw : raw metric value (L2 distance or ip)                     [nq, k] or NULL

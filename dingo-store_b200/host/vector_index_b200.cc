@@ -172,14 +172,14 @@ butil::Status VectorIndexB200::Delete(const std::vector<int64_t>& delete_ids) {
 butil::Status VectorIndexB200::Save(const std::string& path) { return ToStatus(index_ ? b200vs_save(index_, path.c_str()) : B200VS_EINTERNAL); }
 butil::Status VectorIndexB200::Load(const std::string& path) { return ToStatus(index_ ? b200vs_load(index_, path.c_str()) : B200VS_EINTERNAL); }
 
-// Lower the reference's host-side functors (vector_index.h:67-146) to the device form.  RangeFilterFunctor and
-// SortFilterFunctor — the only two ever constructed in src/ (vector_index.cc:1342, vector_reader.cc:1777) — map
-// directly; any other functor is evaluated over the index's ids on the host into a sorted allow-list.
-static butil::Status LowerFilters(b200vs_index* index, const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters,
-                                  LoweredFilters& out) {
+// The index-free part of the lowering: RangeFilterFunctor and SortFilterFunctor — the only two ever constructed in src/
+// (vector_index.cc:1342, vector_reader.cc:1777) — map directly to the device form (several ranges intersect; the first
+// sort functor becomes the id list).  Every other functor, a second sort functor included, is returned in `generic`.
+// Returns whether an id list was taken.
+static bool LowerIdFilters(const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters, LoweredFilters& out,
+                           std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& generic) {
   memset(&out.sp, 0, sizeof(out.sp));
   bool have_list = false;
-  std::vector<VectorIndex::FilterFunctor*> generic;
   for (const auto& f : filters) {
     if (!f) continue;
     if (auto* r = dynamic_cast<VectorIndex::RangeFilterFunctor*>(f.get())) {
@@ -191,9 +191,19 @@ static butil::Status LowerFilters(b200vs_index* index, const std::vector<std::sh
       out.sp.negate = s->IsNegation() ? 1 : 0;
       have_list = true;
     } else {
-      generic.push_back(f.get());
+      generic.push_back(f);
     }
   }
+  if (have_list) { out.sp.sorted_ids = out.ids.data(); out.sp.n_ids = (int64_t)out.ids.size(); }
+  return have_list;
+}
+
+// Lower the reference's host-side functors (vector_index.h:67-146) to the device form: LowerIdFilters, then any other
+// functor is evaluated over the index's ids on the host into a sorted allow-list.
+static butil::Status LowerFilters(b200vs_index* index, const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters,
+                                  LoweredFilters& out) {
+  std::vector<std::shared_ptr<VectorIndex::FilterFunctor>> generic;
+  bool have_list = LowerIdFilters(filters, out, generic);
   if (!generic.empty()) {  // generic fallback: Check() over every id held by the index
     int64_t n = 0;
     if (b200vs_count(index, &n) != B200VS_OK) return butil::Status(pb::error::EINTERNAL, b200vs_last_error());
@@ -202,7 +212,7 @@ static butil::Status LowerFilters(b200vs_index* index, const std::vector<std::sh
     std::vector<int64_t> allow;
     for (int64_t id : all) {
       bool ok = true;
-      for (auto* g : generic) ok = ok && g->Check(id);
+      for (const auto& g : generic) ok = ok && g->Check(id);
       if (ok && have_list) { const bool in = std::binary_search(out.ids.begin(), out.ids.end(), id); ok = out.sp.negate ? !in : in; }
       if (ok) allow.push_back(id);
     }
@@ -528,6 +538,69 @@ butil::Status BruteForceScannerB200::Finish(std::vector<pb::index::VectorWithDis
     for (uint32_t i = 0; i < topk_; ++i) {
       const size_t pos = row * topk_ + i;
       if (labels[pos] < 0) continue;
+      auto* vwd = results[row].add_vector_with_distances();
+      vwd->mutable_vector_with_id()->set_id(labels[pos]);
+      vwd->mutable_vector_with_id()->mutable_vector()->set_dimension(dimension_);
+      vwd->mutable_vector_with_id()->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
+      vwd->set_distance(distances[pos]);
+      vwd->set_metric_type(metric_type_);
+    }
+  return butil::Status::OK();
+}
+
+BruteForceRangeScannerB200::BruteForceRangeScannerB200(pb::common::MetricType metric_type, int32_t dimension,
+                                                       const std::vector<pb::common::VectorWithId>& vector_with_ids, float radius,
+                                                       const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters, int device)
+    : metric_type_(metric_type), dimension_(dimension), nq_(vector_with_ids.size()), cap_(VectorIndexB200::max_range_search_result_count) {
+  if (dimension <= 0) { init_status_ = butil::Status(pb::error::EVECTOR_INVALID, "vector index dimension is invalid"); return; }  // as the top-k scanner
+  if (vector_with_ids.empty()) { init_status_ = butil::Status(pb::error::EILLEGAL_PARAMTETERS, "vector_with_ids is empty"); return; }
+  init_status_ = CheckVectorDimension(vector_with_ids, dimension);
+  if (!init_status_.ok()) return;
+  LoweredFilters lf;
+  LowerIdFilters(filters, lf, host_filters_);
+  const std::vector<float> x = ExtractVectorValue(vector_with_ids, dimension);
+  init_status_ = AbiStatus(b200vs_scan_range_begin(device, AbiMetric(metric_type), dimension, (int64_t)nq_, x.data(), radius, cap_, &lf.sp, &scan_));
+}
+BruteForceRangeScannerB200::~BruteForceRangeScannerB200() { if (scan_) b200vs_scan_range_abort(scan_); }
+
+butil::Status BruteForceRangeScannerB200::Push(const std::vector<pb::common::VectorWithId>& batch) {
+  if (!init_status_.ok()) return init_status_;
+  if (batch.empty()) return butil::Status::OK();
+  auto status = CheckVectorDimension(batch, dimension_);
+  if (!status.ok()) return status;
+  if (!host_filters_.empty()) {  // the reader's temporary Flat index refuses a repeated id before any filter runs
+    std::unordered_set<int64_t> seen;
+    for (const auto& v : batch)
+      if (!seen.insert(v.id()).second) return butil::Status(pb::error::EVECTOR_ID_DUPLICATED, "vector id duplicated: " + std::to_string(v.id()));
+  }
+  std::vector<int64_t> ids;
+  std::vector<float> x;
+  ids.reserve(batch.size());
+  x.reserve(batch.size() * (size_t)dimension_);
+  for (const auto& v : batch) {  // the AND of the host functors, as FlatIDSelector applies them (vector_index_flat.cc:293-296)
+    bool ok = true;
+    for (const auto& f : host_filters_) ok = ok && f->Check(v.id());
+    if (!ok) continue;
+    ids.push_back(v.id());
+    x.insert(x.end(), v.vector().float_values().begin(), v.vector().float_values().end());
+  }
+  if (ids.empty()) return butil::Status::OK();
+  return AbiStatus(b200vs_scan_range_push(scan_, (int64_t)ids.size(), x.data(), ids.data()));
+}
+
+butil::Status BruteForceRangeScannerB200::Finish(std::vector<pb::index::VectorWithDistanceResult>& results) {
+  if (!init_status_.ok()) return init_status_;
+  results.resize(nq_);
+  std::vector<float> distances(nq_ * (size_t)cap_);
+  std::vector<int64_t> labels(nq_ * (size_t)cap_);
+  std::vector<int32_t> counts(nq_);
+  b200vs_scan_range* s = scan_;
+  scan_ = nullptr;  // finish frees the handle
+  const int rc = b200vs_scan_range_finish(s, distances.data(), labels.data(), counts.data());
+  if (rc != B200VS_OK) return AbiStatus(rc);
+  for (size_t row = 0; row < nq_; ++row)  // FillRangeSearchResult, utils.cc:657-694; left unsorted (reader.cc:2187-2189)
+    for (int32_t i = 0; i < counts[row]; ++i) {
+      const size_t pos = row * (size_t)cap_ + i;
       auto* vwd = results[row].add_vector_with_distances();
       vwd->mutable_vector_with_id()->set_id(labels[pos]);
       vwd->mutable_vector_with_id()->mutable_vector()->set_dimension(dimension_);

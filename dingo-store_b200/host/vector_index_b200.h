@@ -122,4 +122,29 @@ class BruteForceScannerB200 {
   uint32_t topk_;
 };
 
+// The inner loop of VectorReader::BruteForceRangeSearch (src/vector/vector_reader.cc:2050-2202), the path that also serves
+// every range search of an HNSW index (RangeSearch returns EVECTOR_NOT_SUPPORT there).  Each pushed batch is range-searched
+// on the GPU without a temporary index; per query the first VectorIndexB200::max_range_search_result_count hits in scan
+// order are kept (batches in push order, rows in batch order), unsorted, as the reader keeps them.  Range and sort functors
+// run on the GPU; any other functor is applied on the host in Push, so a row is kept only when every filter passes it.
+class BruteForceRangeScannerB200 {
+ public:
+  BruteForceRangeScannerB200(pb::common::MetricType metric_type, int32_t dimension, const std::vector<pb::common::VectorWithId>& vector_with_ids,
+                             float radius, const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters, int device = 0);
+  ~BruteForceRangeScannerB200();
+  BruteForceRangeScannerB200(const BruteForceRangeScannerB200&) = delete;
+  BruteForceRangeScannerB200& operator=(const BruteForceRangeScannerB200&) = delete;
+  butil::Status Push(const std::vector<pb::common::VectorWithId>& vector_with_id_batch);
+  butil::Status Finish(std::vector<pb::index::VectorWithDistanceResult>& results);  // scan order, one entry per query
+
+ private:
+  b200vs_scan_range* scan_ = nullptr;
+  butil::Status init_status_;
+  pb::common::MetricType metric_type_;
+  int32_t dimension_;
+  size_t nq_;
+  int32_t cap_;
+  std::vector<std::shared_ptr<VectorIndex::FilterFunctor>> host_filters_;  // the functors the GPU form cannot express
+};
+
 }  // namespace dingodb

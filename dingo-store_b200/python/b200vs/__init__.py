@@ -32,6 +32,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
+    "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
 ]
 
 
@@ -100,6 +101,11 @@ def lib():
     L.b200vs_scan_finish.argtypes = [vp, vp, vp]
     L.b200vs_scan_abort.argtypes = [vp]
     L.b200vs_scan_abort.restype = None
+    L.b200vs_scan_range_begin.argtypes = [i32, ctypes.c_int, i32, i64, vp, f32, i32, ctypes.POINTER(SearchParams), ctypes.POINTER(vp)]
+    L.b200vs_scan_range_push.argtypes = [vp, i64, vp, vp]
+    L.b200vs_scan_range_finish.argtypes = [vp, vp, vp, vp]
+    L.b200vs_scan_range_abort.argtypes = [vp]
+    L.b200vs_scan_range_abort.restype = None
     L.b200vs_set_profiling.argtypes = [vp, ctypes.c_int]
     L.b200vs_last_error.restype = ctypes.c_char_p
     L.b200vs_version.restype = ctypes.c_char_p
@@ -553,6 +559,36 @@ class BruteForceScan:
     def __del__(self):
         if getattr(self, "h", None):
             lib().b200vs_scan_abort(self.h)
+            self.h = None
+
+
+class BruteForceRangeScan:
+    """Streaming brute-force range search over tiles of vectors that are not in an index
+    (VectorReader::BruteForceRangeSearch): per query, the first max_results hits in scan order, unsorted."""
+
+    def __init__(self, metric, dim, xq, radius, max_results=1024, device=0, **kw):
+        xq = _f32(xq)
+        self.nq, self.max_results = xq.shape[0], max_results
+        sp, self._keep = make_search_params(**kw)
+        self.h = ctypes.c_void_p()
+        _check(lib().b200vs_scan_range_begin(device, metric, dim, self.nq, xq.ctypes.data if xq.size else None, float(radius),
+                                             max_results, ctypes.byref(sp), ctypes.byref(self.h)))
+
+    def push(self, x, ids):
+        x, ids = _f32(x), _i64(ids)
+        _check(lib().b200vs_scan_range_push(self.h, ids.size, x.ctypes.data if x.size else None, ids.ctypes.data if ids.size else None))
+
+    def finish(self):
+        D = np.zeros((self.nq, self.max_results), dtype=np.float32)
+        I = np.full((self.nq, self.max_results), -1, dtype=np.int64)
+        C = np.zeros(self.nq, dtype=np.int32)
+        h, self.h = self.h, None
+        _check(lib().b200vs_scan_range_finish(h, D.ctypes.data, I.ctypes.data, C.ctypes.data))
+        return D, I, C
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            lib().b200vs_scan_range_abort(self.h)
             self.h = None
 
 

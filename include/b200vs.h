@@ -297,6 +297,33 @@ int b200vs_scan_push(b200vs_scan* scan, int64_t n, const float* x, const int64_t
 int b200vs_scan_finish(b200vs_scan* scan, float* out_dist, int64_t* out_ids);
 void b200vs_scan_abort(b200vs_scan* scan);
 
+/* Streaming brute-force RANGE search over vectors that are not in an index: VectorReader::BruteForceRangeSearch
+ * (src/vector/vector_reader.cc:2050-2202), which scans the same tiles, range-searches a temporary Flat index per tile with
+ * one query per task (vector_index_flat.cc:267-323) and appends each tile's hits per query until
+ * FLAGS_vector_index_max_range_search_result_count (later hits are dropped; the reader does not sort).  The rule:
+ *   - a row is a hit when its id is >= 0, it passes the filters, and its exact FP32 value (the value b200vs_range_search
+ *     computes on a Flat index, bit for bit) is strictly inside the radius: L2 dist < radius; IP / COSINE ip > 1 - radius
+ *     (COSINE rows and queries are normalised as a Flat index normalises them);
+ *   - per query the result is the FIRST max_results hits in scan order: tiles in push order, rows in their order within a
+ *     tile.  Unlike b200vs_range_search, which keeps the closest max_results, nothing is sorted.  The in-tile order is the
+ *     storage order a one-query faiss Flat range search visits; that is upstream faiss behaviour, recalled, not pinned
+ *     against the reference build;
+ *   - distances in API semantics: squared L2, or 1 - ip (FillRangeSearchResult, vector_index_utils.cc:657-694).
+ * All pointers are host pointers.
+ *   scan_range_begin : argument checks and statuses of b200vs_scan_begin, then max_results <= 0 -> EILLEGAL_PARAMETERS; the
+ *                      queries and filters (id range, sorted id list, negate) are copied; a failed allocation returns
+ *                      EINTERNAL and no handle;
+ *   scan_range_push  : one tile (n <= 0: no-op); a repeated id inside the tile -> EVECTOR_ID_DUPLICATED, the tile adds
+ *                      nothing and the handle stays usable; returns when the tile has been scanned;
+ *   scan_range_finish: out_counts[nq] = hits kept; out_dist / out_ids [nq, max_results] hold them in scan order in slots
+ *                      [0, count), then id -1, distance 0.  Frees the handle, also when it fails. */
+typedef struct b200vs_scan_range b200vs_scan_range;
+int b200vs_scan_range_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t nq, const float* xq, float radius,
+                            int32_t max_results, const b200vs_search_params* sp, b200vs_scan_range** out);
+int b200vs_scan_range_push(b200vs_scan_range* scan, int64_t n, const float* x, const int64_t* ids);
+int b200vs_scan_range_finish(b200vs_scan_range* scan, float* out_dist, int64_t* out_ids, int32_t* out_counts);
+void b200vs_scan_range_abort(b200vs_scan_range* scan);
+
 /* Counters of the last search on this index: [0] kernels launched, [1] queries served by the tensor-core
  * candidate pass; with profiling on (b200vs_set_profiling) also [2] queries of the tensor-core pass that failed
  * certification and were re-run on the exact path (0 with profiling off), [3] device time of the dominant list-scan
