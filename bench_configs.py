@@ -9,6 +9,7 @@
         the GPUs of the box through b200vs_shard_* — run under torchrun (BASELINE: 100 M rows over 8 GPUs = 77 GB per GPU, more
         than an 80 GB H100 holds: default 6.25 M rows per GPU, 50 M over 8)
   cfg6  Binary Flat Hamming, 1M x 256 bits, batch 1024, top-10
+  cfg6s Binary Flat Hamming, 16384 x 256 bits, batch 128, top-10 (below the tile scan's work threshold: exact scan)
   cfg7  Binary IVF-Flat Hamming, 10M x 512 bits, nlist 2048, nprobe 80, batch 1024, top-10   (--bin-n, --bin-dim)
 Each line: device-resident QPS (CUDA events), e2e QPS through the host-pointer C ABI, parity with the oracle on a
 bounded sample, the dominant kernel's time from the library's profiling mode and the algorithmic figure of
@@ -504,20 +505,25 @@ def rnd_bits(n, nb, seed):
     return out
 
 
+EXACT_ONLY = False
+
+
 def binary_line(name, ix, xq, k, word_popcounts, Do, Io, oracle_q, **kw):
     """Device / e2e QPS, list-scan kernel time, word popcounts per second against the popcount bound, parity on the first
     oracle_q queries."""
     nq = xq.shape[0]
-    dev_ms, e2e_ms, st, D, I = time_search(ix, xq, k, **kw)
+    dev_ms, e2e_ms, st, D, I = time_search(ix, xq, k, exact_only=EXACT_ONLY, **kw)
     kernel_s = st[3] / 1e9
+    tile = st[1] > 0
     return {"config": name, "qps_device": nq / dev_ms * 1e3, "ms_per_batch_device": dev_ms, "qps_e2e": nq / e2e_ms * 1e3,
             "ids_bit_exact": bool(np.array_equal(I[:oracle_q], Io)), "dist_bit_exact": bool(np.array_equal(D[:oracle_q].view(np.uint32), Do.view(np.uint32))),
             "parity_sample": f"first {oracle_q} of {nq} queries against tests/binary_oracle.py",
-            "roofline": {"bound": "popcount issue rate", "kernel": "scan_select_kernel<HammingDist>", "kernel_ms": kernel_s * 1e3,
+            "roofline": {"bound": "popcount issue rate", "kernel": "bt_scan_kernel<1> (capture)" if tile else "scan_select_kernel<HammingDist>", "kernel_ms": kernel_s * 1e3,
                          "word_popcounts": word_popcounts, "achieved": word_popcounts / max(kernel_s, 1e-12), "unit": "word popcounts/s",
                          "peak": POPC_BOUND_WORDS_PER_S, "frac": word_popcounts / max(kernel_s, 1e-12) / POPC_BOUND_WORDS_PER_S,
                          "peak_source": "16 __popc / clock / SM (CUDA programming guide) x 132 SMs x 1.7 GHz, not measured"},
-            "path": "exact Hamming scan (query-major)", "search_stats": st}
+            "bit_pairs_per_s": word_popcounts * 32 / max(kernel_s, 1e-12),
+            "path": "BMMA tile scan (list-major)" if tile else "exact Hamming scan (query-major)", "search_stats": st}
 
 
 def cfg6(o, cores, oracle_q=64):
@@ -531,6 +537,19 @@ def cfg6(o, cores, oracle_q=64):
     xq = rnd_bits(nq, nb, 4321)
     Do, Io = binary_oracle.flat_search(xb, ids, xq[:oracle_q], k)
     return binary_line(f"cfg6 Binary Flat Hamming {n}x{dim} bits batch={nq} top-{k}", ix, xq, k, nq * n * w, Do, Io, oracle_q)
+
+
+def cfg6s(o, cores, oracle_q=64):
+    """Below the tile scan's work threshold (nq x rows < 2^23): the exact scan is the faster path and serves it."""
+    n, dim, nq, k = 16384, 256, 128, 10
+    nb, w = dim // 8, (dim // 8 + 3) // 4
+    xb = rnd_bits(n, nb, 1234)
+    ids = np.arange(1, n + 1, dtype=np.int64)
+    ix = b200vs.Index(b200vs.BINARY_FLAT, b200vs.HAMMING, dim)
+    ix.add(xb, ids)
+    xq = rnd_bits(nq, nb, 4321)
+    Do, Io = binary_oracle.flat_search(xb, ids, xq[:oracle_q], k)
+    return binary_line(f"cfg6s Binary Flat Hamming {n}x{dim} bits batch={nq} top-{k}", ix, xq, k, nq * n * w, Do, Io, oracle_q)
 
 
 def cfg7(o, cores, n, dim, oracle_q=16):
@@ -572,14 +591,17 @@ def main():
     ap.add_argument("--cfg5-steps", type=int, default=10)
     ap.add_argument("--bin-n", type=int, default=10_000_000, help="cfg7: database rows")
     ap.add_argument("--bin-dim", type=int, default=512, help="cfg7: bits per row (multiple of 8)")
+    ap.add_argument("--exact-only", action="store_true", help="cfg6 / cfg7: search with exact_only (the query-major exact scan)")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
+    global EXACT_ONLY
+    EXACT_ONLY = a.exact_only
     o = oracle_lib.load()
     cores = os.cpu_count() or 1
     fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads, a.hnsw_build, a.hnsw_build_batch),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
-           "6": lambda: cfg6(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}
+           "6": lambda: cfg6(o, cores), "6s": lambda: cfg6s(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}
     rank = int(os.environ.get("RANK", 0))
     for c in a.configs.split(","):
         t0 = time.time()

@@ -5,12 +5,15 @@
 // VectorIndexIvfFlat<IndexBinary>, vector_index_ivf_flat.cc:62; built by vector_index_factory.cc:73-80, :381-425).
 //
 // Rows are packed bits, dim / 8 bytes each.  On the device a row takes w = ceil(dim / 32) 32-bit words, zero padded, and
-// queries are padded the same way, so the padding adds 0 to every XOR popcount.  Searches run on the exact scan
-// (scan_select_kernel<HammingDist> + merge_select_kernel, scan_kernels.cuh) with key f2ord((float)distance): distances
-// are exact integers <= 32768, so the key orders them like the integers and results are ordered by (distance, id).
+// queries are padded the same way, so the padding adds 0 to every XOR popcount.  Batches with enough work (bt_eligible)
+// run on the BMMA tile scan (binary_tile.cu); the rest, range searches and the coarse quantiser run on the exact scan
+// (scan_select_kernel<HammingDist> + merge_select_kernel, scan_kernels.cuh).  Both use the key f2ord((float)distance):
+// distances are exact integers <= 32768, so the key orders them like the integers and results are ordered by
+// (distance, id), identical on both paths.
 #include <cmath>
 #include <cstdio>
 
+#include "binary_tile.cuh"
 #include "index.h"
 #include "ivf_common.h"
 
@@ -237,8 +240,27 @@ struct BinaryFlatIndex : BinaryIndex {
   std::vector<int64_t> h_ids;
   std::unordered_map<int64_t, int64_t> id2row;
   int64_t ndeleted = 0;
+  DevBuf<long long> d_off1;  // the single "list" of a Flat index, for the tile scan
+  DevBuf<int> d_len1;
 
-  BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {}
+  BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {
+    d_off1.reserve(1, 0, stream); d_len1.reserve(1, 0, stream);
+    B200VS_CUDA(cudaMemsetAsync(d_off1.p, 0, 8, stream));
+    B200VS_CUDA(cudaMemsetAsync(d_len1.p, 0, 4, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+  }
+  void publish_len() {
+    const int len = (int)std::min<int64_t>(rows, 0x7fffffff);
+    B200VS_CUDA(cudaMemcpyAsync(d_len1.p, &len, 4, cudaMemcpyHostToDevice, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+  }
+  TcView view() const {
+    TcView v;
+    v.vecs = reinterpret_cast<const float*>(store.words.p); v.ids = store.ids.p;
+    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
+    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
+    return v;
+  }
   void train_binary(int64_t, const uint8_t*) override {}  // a Flat index needs no training (flat.cc Train returns OK)
 
   void tombstone(const std::vector<int64_t>& rws) {
@@ -259,6 +281,7 @@ struct BinaryFlatIndex : BinaryIndex {
     for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
     h_ids.swap(nh);
     rows = live; ndeleted = 0;
+    publish_len();
   }
   // AddOrUpsert (flat.cc:121-162): duplicate ids in the batch are refused, existing ids are always removed first
   void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool) override {
@@ -286,6 +309,7 @@ struct BinaryFlatIndex : BinaryIndex {
     h_ids.resize(rows + n);
     for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = in_ids[i]; id2row[in_ids[i]] = rows + i; }
     rows += n;
+    publish_len();
     compact_if_needed();
   }
   // Delete (flat.cc:171-203): ids that are not present are ignored
@@ -310,9 +334,17 @@ struct BinaryFlatIndex : BinaryIndex {
     return j;
   }
   void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+    const uint32_t* q = pad(nq, xq, s);
+    const TcView v = view();
+    if (bt_eligible(v, nq, k, 1, (double)rows, sc)) {
+      long long* probes = scratch.alloc<long long>(nq);
+      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
+      bt_search(this, v, w, nq, q, k, probes, 1, job(sc), od, oi, s);
+      return;
+    }
     ScanJob j = job(sc);
     j.dominant = true;
-    run_scan(this, j, nq, reinterpret_cast<const float*>(pad(nq, xq, s)), k, od, nullptr, oi, nullptr, s);
+    run_scan(this, j, nq, reinterpret_cast<const float*>(q), k, od, nullptr, oi, nullptr, s);
   }
   void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc, float* od,
                                long long* oi, int* oc, cudaStream_t s) override {
@@ -469,6 +501,13 @@ struct BinaryIvfIndex : BinaryIndex {
     run_scan(this, hamming_job(cent.p, cent_ids.p, nlist), nq, reinterpret_cast<const float*>(q), nprobe, nullptr, nullptr, probes, nullptr, s);
     return probes;
   }
+  TcView view() const {
+    TcView v;
+    v.vecs = reinterpret_cast<const float*>(store.words.p); v.ids = store.ids.p;
+    v.arena_rows = L.arena_used; v.list_off = L.d_off.p; v.list_len = L.d_len.p;
+    v.nlist = nlist; v.total_chunks = L.total_chunks; v.max_chunks_per_list = L.max_chunks_per_list;
+    return v;
+  }
   ScanJob list_job(const SearchCtx& sc, const long long* probes, int nprobe) const {
     ScanJob j = hamming_job(store.words.p, store.ids.p, 0);
     j.mode = 1; j.probes = probes; j.nprobe = nprobe; j.list_off = L.d_off.p; j.list_len = L.d_len.p; j.sc = &sc;
@@ -537,6 +576,12 @@ struct BinaryIvfIndex : BinaryIndex {
     const int nprobe = resolve_nprobe(sc);
     long long* probes = coarse(nq, q, nprobe, s);
     if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+    const TcView v = view();
+    const ScanJob lj = list_job(sc, probes, nprobe);
+    if (L.live > 0 && bt_eligible(v, nq, k, nprobe, lj.avg_candidates, sc)) {
+      bt_search(this, v, w, nq, q, k, probes, nprobe, lj, od, oi, s);
+      return;
+    }
     ScanJob j = list_job(sc, probes, nprobe);
     j.dominant = true;
     run_scan(this, j, nq, reinterpret_cast<const float*>(q), k, od, nullptr, oi, nullptr, s);

@@ -1136,6 +1136,9 @@ static __global__ void tc_compact_flags_kernel(const int* __restrict__ flags, in
   __syncthreads();
   if (threadIdx.x == 0) *count = s_cnt;
 }
+void tc_compact_flags(const int* flags, int nq, int* qmap, int* count, cudaStream_t s) {
+  tc_compact_flags_kernel<<<1, 1024, 0, s>>>(flags, nq, qmap, count);
+}
 
 static __global__ void max_norm_kernel(const float* __restrict__ n2, long long n, float* out) {
   float m = 0.f;
@@ -1225,7 +1228,7 @@ static int64_t tc_sample_bound(const TcView& v, int64_t npairs) {  // spans are 
   const int64_t max_spans = (v.max_chunks_per_list + 3) / 4 + 1;
   return (npairs / TC_NQT + 1) * max_spans + (v.total_chunks + 3) / 4 + v.nlist;
 }
-static int tc_cand_cap(int k) { return std::min(16384, std::max(8192, next_pow2(256 * k))); }
+int tc_cand_cap(int k) { return std::min(16384, std::max(8192, next_pow2(256 * k))); }
 
 // Per-device one-time setup: cudaFuncSetAttribute applies to the CURRENT device only, and one process may hold indexes
 // on several GPUs (b200vs_params.device), so the opt-in shared-memory limits are raised once per device ordinal.
@@ -1273,8 +1276,12 @@ bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int np
   if (sc.exact_only) return false;
   if (ix->dim % 4 != 0 || ix->dim < 32) return false;      // TMA: 16-byte row pitch; tiny d is not worth a tile
   if (k > 128 || nq < 16) return false;                    // wide k / tiny batches: exact scan
-  if (v.arena_rows <= 0 || v.arena_rows >= (1LL << 31)) return false;
   if (!v.norms || !v.vecs) return false;
+  return tc_plan_fits(v, nq, nprobe);
+}
+
+bool tc_plan_fits(const TcView& v, int64_t nq, int nprobe) {
+  if (v.arena_rows <= 0 || v.arena_rows >= (1LL << 31)) return false;
   const int64_t npairs = nq * nprobe;
   if (npairs >= (1LL << 30)) return false;
   if (tc_item_bound(v, npairs) >= (1LL << 28)) return false;
@@ -1305,29 +1312,13 @@ static TcQueries tc_round_queries(IndexBase* ix, TcArith arith, int64_t nq, cons
   return r;
 }
 
-// everything the passes share: rounded queries, pair inversion, gathered B block, work items, tensor maps
-struct TcPlan {
-  bool half;  // the FP16 mirror (v.vecs_h) instead of the FP32 rows
-  TcQueries qry;
-  int *cnt, *pos, *pair_off, *item_off, *totals, *pair_query, *sample_list, *work;
-  void* bws;
-  TcItem* items;
-  int64_t bound, sbound, npairs;
-  TcMaps maps;
-  TcDevice dev;
-};
-
-static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {
-  const int d = ix->dim;
+TcPairs tc_plan_pairs(IndexBase* ix, const TcView& v, int64_t nq, const long long* probes, int nprobe, const void* qrows,
+                      int row_bytes, cudaStream_t s) {
   auto& S = ix->scratch;
-  TcPlan P;
-  P.dev = tc_init(ix->device);
+  TcPairs P;
   P.npairs = nq * nprobe;
   P.bound = tc_item_bound(v, P.npairs);
   P.sbound = tc_sample_bound(v, P.npairs);
-  P.half = v.vecs_h != nullptr;
-  const int esz = P.half ? 2 : 4;  // operand bytes per element
-  P.qry = tc_round_queries(ix, P.half ? TC_ARITH_FP16 : TC_ARITH_TF32, nq, q, s);
   P.cnt = S.alloc<int>(v.nlist);
   P.pos = S.alloc<int>(P.npairs);
   P.pair_off = S.alloc<int>(v.nlist);
@@ -1336,18 +1327,38 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.work = S.alloc<int>(4);
   P.pair_query = S.alloc<int>(P.npairs);
   P.sample_list = S.alloc<int>(P.sbound);
-  P.bws = S.alloc<unsigned char>((size_t)(P.npairs + TC_NQT) * d * esz);
+  P.bws = S.alloc<unsigned char>((size_t)(P.npairs + TC_NQT) * row_bytes);
   P.items = S.alloc<TcItem>(P.bound);
   B200VS_CUDA(cudaMemsetAsync(P.cnt, 0, (size_t)v.nlist * 4, s));
   B200VS_CUDA(cudaMemsetAsync(P.work, 0, 16, s));
   tc_count_pairs_kernel<<<(unsigned)cdiv(P.npairs, 256), 256, 0, s>>>(probes, P.npairs, P.cnt, P.pos);
   tc_plan_kernel<<<1, 1024, 0, s>>>(P.cnt, v.list_len, v.nlist, P.pair_off, P.item_off, P.totals);
-  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, d * esz, P.qry.op, P.pair_query, P.bws);
+  tc_fill_pairs_kernel<<<(unsigned)cdiv(P.npairs * 32, 256), 256, 0, s>>>(probes, P.pos, P.pair_off, v.list_len, P.npairs, nprobe, row_bytes, qrows, P.pair_query, P.bws);
   tc_items_kernel<<<(unsigned)cdiv(v.nlist, 128), 128, 0, s>>>(P.cnt, v.list_len, P.pair_off, P.item_off, v.nlist, P.items, P.totals, P.sample_list);
   B200VS_CUDA(cudaGetLastError());
+  ix->launch_count(4);
+  return P;
+}
+
+// everything the float passes share: the pair plan, rounded queries, tensor maps
+struct TcPlan : TcPairs {
+  bool half;  // the FP16 mirror (v.vecs_h) instead of the FP32 rows
+  TcQueries qry;
+  TcMaps maps;
+  TcDevice dev;
+};
+
+static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {
+  const int d = ix->dim;
+  TcPlan P;
+  P.dev = tc_init(ix->device);
+  P.half = v.vecs_h != nullptr;
+  const int esz = P.half ? 2 : 4;  // operand bytes per element
+  P.qry = tc_round_queries(ix, P.half ? TC_ARITH_FP16 : TC_ARITH_TF32, nq, q, s);
+  static_cast<TcPairs&>(P) = tc_plan_pairs(ix, v, nq, probes, nprobe, P.qry.op, d * esz, s);
   const void* rows = P.half ? static_cast<const void*>(v.vecs_h) : static_cast<const void*>(v.vecs);
   P.maps = make_tc_maps(rows, nullptr, v.arena_rows, P.bws, nullptr, P.npairs + TC_NQT, d, P.half);
-  ix->launch_count(5);
+  ix->launch_count(1);
   return P;
 }
 
@@ -1376,9 +1387,6 @@ static void tc_launch(const TcDevice& dev, bool half, int64_t work_bound, const 
   }
   B200VS_CUDA(cudaGetLastError());
 }
-
-void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const int* qmap, const int* qcount, const float* queries,
-                     int k, float* out_dist, long long* out_ids, cudaStream_t s);
 
 void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
                int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
@@ -1434,7 +1442,7 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   const size_t fin_smem = tc_stream_smem(d, pool);
   if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
   else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
-  tc_compact_flags_kernel<<<1, 1024, 0, s>>>(flags, (int)nq, qmap, qcount);
+  tc_compact_flags(flags, (int)nq, qmap, qcount, s);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
   ix->stats[1] = nq;

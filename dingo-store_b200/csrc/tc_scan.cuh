@@ -97,6 +97,25 @@ enum TcArith : int {
 
 // true when this search can use the tensor-core pass (otherwise the caller runs the exact scan)
 bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc);
+// the plan-size half of tc_eligible: the view's rows, the (query, probe) pairs, work items and sample buffer fit the plan
+bool tc_plan_fits(const TcView& v, int64_t nq, int nprobe);
+
+// Probes -> (list, query) pairs -> work items, shared by the float and the binary tile scans.  Uses v.nlist, v.list_len
+// and the chunk counts.  qrows: device query rows of row_bytes each (a multiple of 16), copied pair by pair into bws.
+struct TcPairs {
+  int *cnt, *pos, *pair_off, *item_off, *totals, *pair_query, *sample_list, *work;
+  void* bws;  // [npairs + TC_NQT] gathered query rows: a work item's B block is nq <= TC_NQT consecutive rows
+  TcItem* items;
+  int64_t bound, sbound, npairs;  // host bounds on the work items and on the sampled items
+};
+TcPairs tc_plan_pairs(IndexBase* ix, const TcView& v, int64_t nq, const long long* probes, int nprobe, const void* qrows,
+                      int row_bytes, cudaStream_t s);
+int tc_cand_cap(int k);  // captured rows kept per query
+// qmap[0, *count) = the queries whose flags[q] != 0, in no particular order
+void tc_compact_flags(const int* flags, int nq, int* qmap, int* count, cudaStream_t s);
+// exact re-run of the queries in qmap[0, *qcount) (kernels.cu)
+void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const int* qmap, const int* qcount, const float* queries,
+                     int k, float* out_dist, long long* out_ids, cudaStream_t s);
 
 // probes: device [nq, nprobe] list indices (for Flat: all zeros, nprobe = 1).  q: device queries, already
 // normalised for cosine.  Writes API-semantics results; uncertified queries are re-run on the exact scan.

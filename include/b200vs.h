@@ -81,7 +81,7 @@ typedef struct {
   int64_t range_min, range_max;
   const int64_t* sorted_ids; /* ascending id list (HOST pointer), or NULL */
   int64_t n_ids;
-  int32_t exact_only; /* 1 = force the exact FP32 scan (skip the tensor-core candidate pass) */
+  int32_t exact_only; /* 1 = force the exact scan: FP32 on float indexes, Hamming on binary indexes (skip the tile scan) */
   int32_t reserved;
 } b200vs_search_params;
 
@@ -328,12 +328,14 @@ void b200vs_scan_range_abort(b200vs_scan_range* scan);
  * candidate pass; with profiling on (b200vs_set_profiling) also [2] queries of the tensor-core pass that failed
  * certification and were re-run on the exact path (0 with profiling off), [3] device time of the dominant list-scan
  * kernel in ns (CUDA events on the launch stream), [4] rows in the distinct probed lists, [5] distinct probed lists,
- * [6] work items of the tile scan, [7] its tensor-core work (128-row tiles x padded query columns).  HNSW fills [0] and
+ * [6] work items of the tile scan, [7] its tensor-core work (128-row tiles x padded query columns).  Binary indexes
+ * keep these meanings for their BMMA tile scan: [1] queries it served, [2] queries re-run on the exact Hamming scan
+ * (capture overflow, or fewer than k eligible sampled rows), [3] its capture kernel.  HNSW fills [0] and
  * [6] = queries walked with the candidate-heap form (id filter, tombstones or ef >= 1024; 0 = merged-array form).  Profiling
  * synchronises the stream inside the call: never leave it on in a timed run. */
 int b200vs_last_search_stats(b200vs_index* idx, int64_t stats[8]);
 /* With profiling on: device milliseconds (CUDA events on the launch stream) the last search spent in each phase of the
- * IVF tile path: [0] coarse prep, [1] coarse scan, [2] coarse select + exact re-score, [3] work planning + query
+ * IVF tile path (binary tile scans fill [3]-[9] the same way; [7] is their final select): [0] coarse prep, [1] coarse scan, [2] coarse select + exact re-score, [3] work planning + query
  * gather, [4] sample pass, [5] thresholds, [6] list scan (capture), [7] final select + exact re-score, [8] exact
  * fallback for uncertified queries, [9] other, [10] collectives of a sharded search (b200vs_shard_search*), [11] pack + merge of
  * the per-shard top-k.  After b200vs_hnsw_add_batched: [12] construction search, [13] peer distances + forward links,
