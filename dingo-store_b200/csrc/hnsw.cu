@@ -455,6 +455,9 @@ __device__ __forceinline__ void descend(const Walk<L2>& w, int from_level, int s
   }
 }
 
+// a before b in the merged walk's order: the float order, with every NaN after every number (and NaNs equal)
+__device__ __forceinline__ bool d_before(float a, float b) { return a < b || (b != b && a == a); }
+
 // Base walk at `level`, merged-array form, from (cur, curdist) with capacity ef.  T (id bit 31 = expanded) and T2 are the
 // two buffers of the merge, [ef] each; on return T holds the ascending result and the return value is its length.
 template <bool L2>
@@ -480,19 +483,22 @@ __device__ __forceinline__ int walk_merged(const Walk<L2>& w, int level, int ef,
   for (;;) {
     const int m = w.round(c, level, next);
     if (m < 0) break;
-    // merge the m scored neighbours into T (ascending, old entries first among equals), keep the best ef
+    // merge the m scored neighbours into T (ascending, old entries first among equals), keep the best ef.  The ranks are
+    // counted in an order that puts NaN (an inner product that overflowed to +inf and -inf) after every number, so the
+    // destinations always form a permutation.  With plain float compares a NaN broke that: two entries took one slot,
+    // another slot of T2 kept stale shared memory, and its id was walked.
     for (int tix = threadIdx.x; tix < ntop; tix += HNSW_THREADS) {
       const HeapEnt e = T[tix];
       int cnt = 0;
-      for (int j = 0; j < m; ++j) cnt += w.s_d[j] < e.d ? 1 : 0;
+      for (int j = 0; j < m; ++j) cnt += d_before(w.s_d[j], e.d) ? 1 : 0;
       if (tix + cnt < ef) T2[tix + cnt] = e;
     }
     if (threadIdx.x < m) {
       const float dj = w.s_d[threadIdx.x];
       int rank = 0;
-      for (int i = 0; i < m; ++i) rank += (w.s_d[i] < dj || (w.s_d[i] == dj && i < (int)threadIdx.x)) ? 1 : 0;
-      int lo = 0, hi = ntop;  // number of old entries with d <= dj
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (T[mid].d <= dj) lo = mid + 1; else hi = mid; }
+      for (int i = 0; i < m; ++i) rank += (d_before(w.s_d[i], dj) || (!d_before(dj, w.s_d[i]) && i < (int)threadIdx.x)) ? 1 : 0;
+      int lo = 0, hi = ntop;  // number of old entries not after dj
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (!d_before(dj, T[mid].d)) lo = mid + 1; else hi = mid; }
       if (rank + lo < ef) { HeapEnt e; e.d = dj; e.id = w.s_id[threadIdx.x]; T2[rank + lo] = e; }
     }
     ntop = min(ef, ntop + m);

@@ -620,7 +620,8 @@ struct IvfFlatIndex : IndexBase {
 
   long long* coarse(int64_t nq, const float* q, int nprobe, cudaStream_t s, bool allow_tc = true, long long* out = nullptr) {
     long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
-    if (allow_tc && tc_coarse_eligible(this, nq, nlist, nprobe)) {  // dense TF32 scores + certified exact re-score
+    if (allow_tc && tc_coarse_eligible(this, nq, nlist, nprobe) && tc_norms_in_range(metric == B200VS_L2, cent_max_norm)) {
+      // dense TF32 scores + certified exact re-score
       tc_coarse(this, coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, 0, nlist), metric == B200VS_L2, nq, q,
                 nprobe, probes, nullptr, s);
       return probes;
@@ -844,7 +845,7 @@ void IvfFlatIndex::coarse_range_dev(int64_t nq, const float* xq, int nprobe, int
   if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
   const float* q = prepare_queries(nq, xq, s);
   const int rows = c1 - c0;
-  if (tc_coarse_eligible(this, nq, rows, nprobe)) {
+  if (tc_coarse_eligible(this, nq, rows, nprobe) && tc_norms_in_range(metric == B200VS_L2, cent_max_norm)) {
     TcView v = coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, c0, rows);
     v.api_scores = true;
     tc_coarse(this, v, metric == B200VS_L2, nq, q, nprobe, out_lists, out_score, s);

@@ -396,7 +396,8 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
         for (int c = 0; c < 2; ++c) {
           const int n = 8 * j + col0 + c;
           if (n < I.nq) {
-            // FP16: both scales are powers of two, so hs * qs and the product with the accumulator are exact
+            // FP16: both scales are powers of two, so hs * qs and the product with the accumulator are exact while they
+            // stay normal; below that they underflow (to 0 under 2^-149), which tc_eps's absolute term covers
             const float dot = HALF ? acc[4 * j + 2 * h + c] * (hs[h] * s_qs[n]) : acc[4 * j + 2 * h + c];
             const float score = p.l2 ? fmaf(-2.f, dot, nrm[h]) : -dot;
             if constexpr (C::IS_SAMPLE) {
@@ -734,7 +735,22 @@ __device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm,
   //   FP16: each operand vector is off by at most delta = 2^-11 + sqrt(d) 2^-39 of its norm (RN, plus underflow below the
   //     power-of-two scale), so the dot product by at most 2 delta + delta^2; the FP16 products are exact in FP32.
   // Accumulation term: FP32 sums of d terms on both sides (tensor core, norms, and the exact kernel itself).
-  const float qn = sqrtf(qnorm_sq);
+  // Both terms are relative; below the normal range rounding errs by an absolute amount, which the underflow term covers:
+  //   * the norms: a FP32 sum of d squares loses at most d * 2^-149 to underflow, so ||v|| <= sqrt(n2) + sqrt(d) 2^-74.5;
+  //   * the tensor core may flush subnormal operands, products and partial sums: < 2^-126 per product and per add
+  //     (at most 6d of them with the split pass, doubled by L2's 2 <q, x>), and < 2^-126 |partner| per flushed operand,
+  //     so at most 2^-124 sqrt(d) (||q|| + ||x||) over the row (x 2 for hi and lo);
+  //   * FP16: hscale * qscale underflows to 0 only below 2^-149, and then |<q, x>| < d 2^30 hscale qscale <= d 2^-119;
+  //     a subnormal acc * (hscale * qscale) errs by <= 2^-150;
+  //   * the exact FP32 sums on the CUDA cores round gradually: <= 2^-150 per operation.
+  //   Together <= (d + 64) 2^-118 + sqrt(d) (||q|| + max ||x||) 2^-122.
+  // Range: the bound is only returned while A (below) <= 2^125, so every norm, score, partial sum and exact distance stays
+  // finite with room for the rounding; beyond it, or for a NaN norm, eps = +inf and the finish kernels hand the query to
+  // the exact scan.
+  const float qn = sqrtf(qnorm_sq) + sqrtf((float)d) * 0x1p-74f;
+  max_norm += sqrtf((float)d) * 0x1p-74f;
+  const float A = l2 ? (max_norm + qn) * (max_norm + qn) : qn * max_norm;
+  if (!(A <= 0x1p125f)) return TC_INF;
   float rel = 0.0014648438f;  // 2^-10 + 2^-11
   if (arith == TC_ARITH_SPLIT) rel = 1.9073486e-6f;  // 2^-19
   else if (arith == TC_ARITH_FP16) {
@@ -742,8 +758,9 @@ __device__ __forceinline__ float tc_eps(bool l2, float qnorm_sq, float max_norm,
     rel = __fmaf_ru(delta, delta, 2.f * delta);
   }
   const float operand = (l2 ? 2.f : 1.f) * rel * qn * max_norm;
-  const float accum = 2.f * (float)(d + 64) * 5.9604645e-8f /*2^-24*/ * (l2 ? (max_norm + qn) * (max_norm + qn) : qn * max_norm);
-  return operand + accum;
+  const float accum = 2.f * (float)(d + 64) * 5.9604645e-8f /*2^-24*/ * A;
+  const float under = (float)(d + 64) * 0x1p-118f + sqrtf((float)d) * (qn + max_norm) * 0x1p-122f;
+  return operand + accum + under;
 }
 
 // The window rows s_rows[0, m) re-scored exactly in the reference order by the block's NQUADS quads, one row per quad per
@@ -808,6 +825,11 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   float a_k = TC_INF;
   if (n >= k) a_k = ord2f(block_kth_key_any(k, S, [&](auto f) { for (int i = threadIdx.x; i < n; i += HF_THREADS) f((uint32_t)(key_at(i) >> 32)); }));
   const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith);
+  if (!(two_eps < TC_INF)) {  // outside the range eps covers (the scores may be inf or NaN): the exact scan re-runs it
+    cp_async_wait_all();      // the query row
+    if (threadIdx.x == 0) { flags[qi] = 1; redo[qi] = 0; }
+    return;
+  }
   {
     const float window = a_k + two_eps;
     for (int base = 0; base < n; base += HF_THREADS) {
@@ -910,7 +932,9 @@ tc_coarse_select_kernel(const float* __restrict__ dense, long long ld, int nrows
   }
   __syncthreads();
   const int m = s_m, ns = s_ns;
-  if (m > SEL_WCAP) {  // degenerate score row (many near-equal scores): redo on the streaming kernel
+  // degenerate score row (many near-equal scores), or eps = +inf (NaN scores drop out of the window): redo on the
+  // streaming kernel, which then re-scores every row
+  if (m > SEL_WCAP || !(two_eps < TC_INF)) {
     if (threadIdx.x == 0) flags[qi] = 1;
     return;
   }
@@ -977,7 +1001,7 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
       ns += __popc(ms);
       m += __popc(mw);
     }
-    if (lane == 0) { s_m = m; s_ns = ns; }
+    if (lane == 0) { s_m = two_eps < TC_INF ? m : HC_MAXW + 1; s_ns = ns; }  // eps = +inf: as tc_coarse_select_kernel
   }
   __syncthreads();
   const int m = s_m, ns = s_ns;
@@ -1005,7 +1029,8 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
 // i < n, is (ord(approximate score) << 32 | row); id_of(row) is the id a row is reported under.  Pass 1: A_k = k-th
 // smallest approximate score (+inf when n < k).  Pass 2: every row with score <= A_k + two_eps re-scored exactly in the
 // reference order, FIN_SEG rows at a time, into `sel`, which ends holding the exact top-k by (distance, id).
-// smem: tc_stream_smem(d, pool_cap) bytes.  Returns A_k + two_eps.  All SCAN_THREADS threads call.
+// smem: tc_stream_smem(d, pool_cap) bytes.  Returns A_k + two_eps (NaN when two_eps = +inf: then pass 2 takes every row).
+// All SCAN_THREADS threads call.
 static size_t tc_stream_smem(int d, int pool_cap) { return ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_SEG * 4 + BlockSelect::smem_bytes(pool_cap); }
 
 template <bool L2, class KeyAt, class IdOf>
@@ -1033,7 +1058,9 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
   sel.prune();
   const float a_k = *sel.count >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
   __syncthreads();
-  const float window = a_k + two_eps;  // +inf when fewer than k rows
+  // window = A_k + two_eps (+inf when fewer than k rows) as a key; eps = +inf (outside the range it bounds): every row,
+  // NaN scores included (a NaN fails every float comparison, but its key 0xFFFFFFFF is the largest)
+  const uint32_t wkey = two_eps < TC_INF ? f2ord(a_k + two_eps) : 0xFFFFFFFFu;
   // pass 2: exact distances (reference AVX-512 order) of every row inside the window
   sel.init(pool, pool_cap, k);
   const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
@@ -1044,7 +1071,7 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
     const int e1 = min(n, seg + FIN_SEG);
     for (int i = seg + threadIdx.x; i < e1; i += blockDim.x) {
       const unsigned long long e = key_at(i);
-      if (ord2f((uint32_t)(e >> 32)) <= window) s_rows[atomicAdd(&s_m, 1)] = (int)(uint32_t)(e & 0xffffffffull);
+      if ((uint32_t)(e >> 32) <= wkey) s_rows[atomicAdd(&s_m, 1)] = (int)(uint32_t)(e & 0xffffffffull);
     }
     __syncthreads();
     const int m = s_m;
@@ -1063,7 +1090,7 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
     __syncthreads();
   }
   sel.prune();
-  return window;
+  return ord2f(wkey);
 }
 
 template <bool L2>
@@ -1075,12 +1102,13 @@ tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restri
   extern __shared__ __align__(16) unsigned char smem[];
   const int qi = blockIdx.x;
   if (redo && !redo[qi]) return;  // finished by the hybrid kernel
+  const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith);
+  if (!(two_eps < TC_INF)) { if (threadIdx.x == 0) flags[qi] = 1; return; }  // the exact scan re-runs it
   const int total = cand_cnt[qi];
   const unsigned long long* c = cand + (size_t)qi * cap;
   BlockSelect sel;
-  const float window = tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k,
-                                            2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith), [&](int i) { return c[i]; },
-                                            [&](uint32_t row) { return ids[row]; });
+  const float window = tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k, two_eps,
+                                            [&](int i) { return c[i]; }, [&](uint32_t row) { return ids[row]; });
   const float tq = tau[qi];
   const bool certified = (total <= cap) && (tq == TC_INF || window <= tq);
   const int have = *sel.count;
@@ -1277,7 +1305,15 @@ bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int np
   if (ix->dim % 4 != 0 || ix->dim < 32) return false;      // TMA: 16-byte row pitch; tiny d is not worth a tile
   if (k > 128 || nq < 16) return false;                    // wide k / tiny batches: exact scan
   if (!v.norms || !v.vecs) return false;
+  if (!tc_norms_in_range(ix->metric == B200VS_L2, v.max_norm)) return false;
   return tc_plan_fits(v, nq, nprobe);
+}
+
+// tc_eps returns +inf once A > 2^125.  For L2, A = (||q|| + max ||x||)^2 >= max ||x||^2 for every query (rounding is
+// monotone); for IP, A = ||q|| max ||x|| with ||q|| > 0 (tc_eps's underflow allowance), so an infinite max ||x|| makes
+// every A infinite.  A NaN max ||x|| fails both tests.
+bool tc_norms_in_range(bool l2, float max_norm) {
+  return l2 ? max_norm * max_norm <= 0x1p125f : max_norm <= FLT_MAX;
 }
 
 bool tc_plan_fits(const TcView& v, int64_t nq, int nprobe) {

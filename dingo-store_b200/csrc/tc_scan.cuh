@@ -99,6 +99,9 @@ enum TcArith : int {
 bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc);
 // the plan-size half of tc_eligible: the view's rows, the (query, probe) pairs, work items and sample buffer fit the plan
 bool tc_plan_fits(const TcView& v, int64_t nq, int nprobe);
+// false when no query can have a finite error bound against rows of this max ||x|| (tc_eps), so the tile passes would
+// only be thrown away: L2 with max ||x||^2 > 2^125, IP / cosine with max ||x|| not finite
+bool tc_norms_in_range(bool l2, float max_norm);
 
 // Probes -> (list, query) pairs -> work items, shared by the float and the binary tile scans.  Uses v.nlist, v.list_len
 // and the chunk counts.  qrows: device query rows of row_bytes each (a multiple of 16), copied pair by pair into bws.
