@@ -4,6 +4,8 @@
   cfg1  Flat L2, 100K x 128, top-10, batch = 1            (the reference's own CPU-runnable case)
   cfg2  IVF-Flat L2, 1M x 768, nlist 1024, nprobe 32, batch 256, top-10
   cfg3  IVF-PQ IP, 10M x 768, M = 96, nbits 8, nlist 2048, nprobe 64, batch 1024, top-100   (--pq-n, --pq-nbits, --pq-m)
+  cfg3s cfg3 through the list-sharded deployment b200vs_shard_* (world 1 on one GPU, beside the plain search at the same
+        shape; under torchrun over the box's GPUs, n / world rows per GPU)                    (--pq-n, --pq-nbits, --pq-m)
   cfg4  HNSW cosine, 1M x 768, M = 16, efConstruction 200, efSearch 128, batch 512          (--hnsw-n; concurrent host build)
   cfg5  IVF-Flat L2, (rows-per-GPU x world) x 1536, nlist 2048 per GPU, nprobe 64, batch 4096, top-10, list-sharded over
         the GPUs of the box through b200vs_shard_* — run under torchrun (BASELINE: 100 M rows over 8 GPUs = 77 GB per GPU, more
@@ -188,6 +190,93 @@ def cfg3(o, cores, n, nbits=8, M=96):
                          **({} if nbits == 8 else {"code_size": code_size, "code_bytes_per_batch": nq * nprobe * avg_len * code_size})},
             "cpu_baseline": {"qps": ns / cpu_s, "cores": cores, "kind": "port", "sample": f"first {ns} queries, {cores} threads"},
             "train_seconds": t_train, "add_seconds": t_add, "search_stats": st}
+
+
+def cfg3s(o, cores, n, nbits=8, M=96, steps=5, warmup=2, oracle_q=32):
+    """cfg3 through the list-sharded deployment (b200vs_shard_*): shard_train, shard_add_device (rows generated on the
+    device, n / world per rank), the sharded search.  At world 1 the plain b200vs_search runs on the same index next to it;
+    under torchrun rank 0 gathers the exported codes for the oracle.  Rank 0 returns the JSON line."""
+    import torch.distributed as dist
+    rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
+    torch.cuda.set_device(local)
+    dev = torch.device("cuda", local)
+    if world > 1 and not dist.is_initialized():
+        dist.init_process_group("nccl", device_id=dev)
+    d, nlist, nprobe, nq, k = 768, 2048, 64, 1024, 100
+    ksub, code_size = 1 << nbits, pq_codes.code_size(M, nbits)
+    ix = b200vs.Index(b200vs.IVF_PQ, b200vs.IP, d, nlist=nlist, pq_m=M, pq_nbits=nbits, device=local)
+    idb = None
+    if world > 1:
+        t = torch.from_numpy(b200vs.Shard.unique_id() if rank == 0 else np.zeros(128, np.uint8)).to(dev)
+        dist.broadcast(t, 0)
+        idb = t.cpu().numpy()
+    sh = b200vs.Shard(ix, rank, world, idb, lanes=2)
+    g = torch.Generator(device=dev)
+    g.manual_seed(1234 + rank)
+    t0 = time.time()
+    ntrain = max(256 * nlist // world, 65536)  # rank 0 needs 256 * 2^nbits rows for the codebooks
+    sh.train(torch.randn((ntrain, d), generator=g, device=dev).cpu().numpy())
+    t_train = time.time() - t0
+    t0 = time.time()
+    n_per = n // world
+    for a in range(0, n_per, 131072):
+        m = min(131072, n_per - a)
+        x = torch.randn((m, d), generator=g, device=dev)
+        ids = torch.arange(rank * n_per + a + 1, rank * n_per + a + 1 + m, dtype=torch.int64, device=dev)
+        torch.cuda.synchronize()
+        sh.add_device(m, x.data_ptr(), ids.data_ptr())
+    t_add = time.time() - t0
+    xq = rnd(nq, d, 4321, "normal")
+    sp, _keep = b200vs.make_search_params(nprobe=nprobe)
+    q = torch.from_numpy(xq).to(dev)
+    od = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    oi = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    st = torch.cuda.Stream(device=dev)
+    for _ in range(warmup):
+        sh.search_device(nq, q.data_ptr(), k, od.data_ptr(), oi.data_ptr(), stream=st.cuda_stream, sp=sp)
+    st.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(st)
+    for _ in range(steps):
+        sh.search_device(nq, q.data_ptr(), k, od.data_ptr(), oi.data_ptr(), stream=st.cuda_stream, sp=sp)
+    e1.record(st)
+    st.synchronize()
+    dev_ms = e0.elapsed_time(e1) / steps
+    t = time.perf_counter()
+    for _ in range(steps):
+        D, I = sh.search(xq, k, nprobe=nprobe)
+    e2e_ms = (time.perf_counter() - t) / steps * 1e3
+    plain = None
+    if world == 1:  # the unsharded search on the same index, same shape
+        p_dev, p_e2e, p_st, Dp, Ip = time_search(ix, xq, k, steps=steps, warmup=warmup, nprobe=nprobe)
+        plain = {"qps_device": nq / p_dev * 1e3, "ms_per_batch_device": p_dev, "qps_e2e": nq / p_e2e * 1e3,
+                 "ids_equal_sharded": bool(np.array_equal(I, Ip)), "dist_bits_equal_sharded": bool(np.array_equal(D.view(np.uint32), Dp.view(np.uint32)))}
+    blob = ix.get_trained_state()
+    cent = blob[48:48 + nlist * d * 4].view(np.float32).reshape(nlist, d)
+    cb = blob[48 + nlist * d * 4:].view(np.float32).reshape(M, ksub, d // M)
+    off, _, codes, lids = ix.export_lists(nlist, with_vectors=False, code_size=code_size)
+    if world > 1:
+        parts = [None] * world
+        dist.all_gather_object(parts, (off, codes, lids))
+        if rank != 0:
+            sh.close()
+            return None
+        off = np.zeros(nlist + 1, np.int64)
+        gc, gi = [], []
+        for l in range(nlist):
+            for (po, pc, pi) in parts:
+                gc.append(pc[po[l]:po[l + 1]])
+                gi.append(pi[po[l]:po[l + 1]])
+            off[l + 1] = off[l] + sum(int(po[l + 1] - po[l]) for (po, _, _) in parts)
+        codes, lids = np.concatenate(gc, 0), np.concatenate(gi, 0)
+    sh.close()
+    Do, Io = pq_codes.ivfpq_search(o, oracle_lib.IP, cent, cb, off, codes, lids, xq[:oracle_q], k, nprobe, nthreads=cores)
+    return {"config": f"cfg3s IVF-PQ IP {n}x768 M={M} nbits={nbits} nlist=2048 nprobe=64 batch=1024 top-100, list-sharded over {world} GPU(s)",
+            "scaled_from": "10M x 768" if n < 10_000_000 else None, "world": world,
+            "qps_device": nq / dev_ms * 1e3, "ms_per_batch_device": dev_ms, "qps_e2e": nq / e2e_ms * 1e3,
+            "ids_bit_exact_sample": bool(np.array_equal(I[:oracle_q], Io)),
+            "dist_bit_exact_sample": bool(np.array_equal(D[:oracle_q].view(np.uint32), Do.view(np.uint32))),
+            "plain_b200vs_search_same_shape": plain, "train_seconds": t_train, "add_seconds": t_add}
 
 
 def cfg4(o, cores, n, build_threads=64, build="host", build_batch=0):
@@ -600,6 +689,7 @@ def main():
     cores = os.cpu_count() or 1
     fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads, a.hnsw_build, a.hnsw_build_batch),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
+           "3s": lambda: cfg3s(o, cores, a.pq_n, a.pq_nbits, a.pq_m),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
            "6": lambda: cfg6(o, cores), "6s": lambda: cfg6s(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}
     rank = int(os.environ.get("RANK", 0))

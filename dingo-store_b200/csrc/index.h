@@ -238,44 +238,47 @@ struct IndexBase {
   // scan for caller-supplied (merged) probes
   virtual void coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) {
     (void)nq; (void)xq; (void)nprobe; (void)c0; (void)c1; (void)out_score; (void)out_lists; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
   }
   virtual void search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
                                  long long* oi, cudaStream_t s) {
     (void)nq; (void)xq; (void)k; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
   }
-  // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT only ----
+  // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT and IVF_PQ ----
   // rows / ids already on this device.  lists_dev (nullable) = the inverted list of every row, decided by the caller;
   // prepared = store the rows exactly as given (cosine rows are already normalised).
   virtual void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
     (void)n; (void)x_dev; (void)ids_dev; (void)lists_dev; (void)upsert; (void)prepared;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
   }
   // nearest-centroid assignment of prepared rows (faiss quantizer->assign): out_lists_dev[n], on stream s (a lane must be held)
   virtual void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) {
     (void)n; (void)x_dev; (void)out_lists_dev; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "list assignment only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "list assignment only exists for IVF_FLAT and IVF_PQ");
   }
   // pre-size every inverted list (rows_per_list[nlist]) in ONE arena allocation: bulk builds of large shards never
   // relocate a list or re-allocate the arena (a 77 GB shard cannot afford a 2x peak)
   virtual void reserve_lists(const int64_t* rows_per_list, int nlist) {
     (void)rows_per_list; (void)nlist;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "list reservation only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "list reservation only exists for IVF_FLAT and IVF_PQ");
   }
   virtual int nlist_now() const { return 1; }
   // probe table (set semantics, order unspecified) of prepared queries into a caller buffer
   virtual void coarse_probes_dev(int64_t nq, const float* q_prepared, int nprobe, long long* out_lists, cudaStream_t s) {
     (void)nq; (void)q_prepared; (void)nprobe; (void)out_lists; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
   }
   // search_probes_dev on queries that are already prepared (normalised for cosine)
   virtual void search_probes_prepared_dev(int64_t nq, const float* q_prepared, int k, const long long* probes, int nprobe, const SearchCtx& sc,
                                           float* od, long long* oi, cudaStream_t s) {
     (void)nq; (void)q_prepared; (void)k; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT");
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
   }
   virtual int resolve_nprobe_api(const SearchCtx& sc) const { (void)sc; return 1; }
+  // refusals of search_probes_prepared_dev that depend only on nq, k and the trained state (IVF-PQ: the LUT + select pool
+  // must fit one SM's shared memory); a sharded search checks them on every rank before its first collective
+  virtual void check_probe_search(int64_t nq, int k) const { (void)nq; (void)k; }
   // b200vs_debug_tc_scores: xq device (raw), outputs host [nq, count() + deleted_count()] and [nq]
   virtual void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) {
     (void)nq; (void)xq; (void)arith; (void)out_scores; (void)out_eps; (void)s;
@@ -364,6 +367,12 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_pq(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p);
+// IVF-PQ training in the two stages of its train (ivf_pq.cu), for the list-sharded trainer (shard.cu); ix must be an IVF_PQ
+// index, whose lists and trained state stay untouched.  Coarse: k centroids of n raw rows.  State: the codebooks of the PQ
+// rule on the n rows' residuals to the centroids cent [nlist, dim], returned with cent as a trained-state blob.
+int ivf_pq_ksub(IndexBase* ix);
+void ivf_pq_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent);
+void ivf_pq_train_state(IndexBase* ix, int64_t n, const float* x, const std::vector<float>& cent, std::vector<unsigned char>& blob);
 IndexBase* make_binary_flat(int d, const b200vs_params& p);
 IndexBase* make_binary_ivf(int d, const b200vs_params& p);
 

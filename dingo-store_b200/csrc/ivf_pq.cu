@@ -345,6 +345,24 @@ __global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kern
   }
 }
 
+// dis0[i] (i = query * nprobe + p) = the coarse pass's raw value (L2 distance or ip) of the query and list probes[i], for
+// probes that come from the caller (a list-sharded search merges them from several ranks, and the ABI carries list ids
+// only).  It is bit-equal to what the coarse pass of scan_codes hands the LUT scan: the exact scan's quad_distance on
+// (centroid row, query), then its merge's (key, raw) round trip (which turns an ip of +0 into -0).  One quad per
+// (query, probe); -1 probes and empty lists are skipped, as the LUT scans never read them.
+template <bool L2>
+__global__ void pq_dis0_kernel(const float* __restrict__ q, const float* __restrict__ cent, const long long* __restrict__ probes,
+                               const int* __restrict__ list_len, long long n, int nprobe, int d, bool vec, float* dis0) {
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+  const int t = threadIdx.x & 3;
+  const long long l = i < n ? probes[i] : -1;
+  const bool valid = l >= 0 && list_len[l] > 0;
+  // every quad of the warp takes part in quad_distance's shuffles: an idle quad evaluates query 0 against centroid 0
+  const long long qi = valid ? i / nprobe : 0;
+  const float v = quad_distance<L2>(cent + (size_t)(valid ? l : 0) * d, q + (size_t)qi * d, d, t, vec);
+  if (valid && t == 0) dis0[i] = L2 ? ord2f(f2ord(v)) : -ord2f(f2ord(-v));
+}
+
 template <bool L2>
 void launch_pq_scan_packed(int nbits, dim3 grid, size_t smem, cudaStream_t s, const PqScanArgs& a) {
   auto go = [&](auto kern) {
@@ -441,14 +459,15 @@ struct IvfPqIndex : IndexBase {
     return (int64_t)need;
   }
 
-  void assign_dev(const float* cd, int kk, const long long* cid, const float* x_dev, int dd, bool l2, int64_t n, long long* out) {
+  void assign_dev(const float* cd, int kk, const long long* cid, const float* x_dev, int dd, bool l2, int64_t n, long long* out,
+                  cudaStream_t s) {
     ScanJob j;
     j.l2 = l2; j.vecs = cd; j.ids = cid; j.d = dd; j.mode = 0; j.n = kk;
     const int64_t chunk = 32768;
     for (int64_t a = 0; a < n; a += chunk) {
       const int64_t m = std::min(chunk, n - a);
       const auto mark = scratch.mark();
-      run_scan(this, j, m, x_dev + (size_t)a * dd, 1, nullptr, nullptr, out + a, nullptr, stream);
+      run_scan(this, j, m, x_dev + (size_t)a * dd, 1, nullptr, nullptr, out + a, nullptr, s);
       scratch.release(mark);
     }
   }
@@ -472,13 +491,27 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
+    std::vector<float> cent, cb;
+    train_coarse_locked(n, x, nlist, cent);
+    train_codebooks_locked(n, x, cent, cb);
+    install(cent.data(), cb.data());
+  }
+
+  // The two stages of train, also run separately by the list-sharded trainer (shard.cu).  Callers hold rw and gpu_mu, with
+  // the scratch reset.  Coarse stage: k centroids of the n rows (level-1 quantiser, niter 10).
+  void train_coarse_locked(int64_t n, const float* x, int k, std::vector<float>& cent) {
     const bool l2 = metric == B200VS_L2;
     DevBuf<long long> cid;
-    // level-1 quantiser (niter 10)
-    std::vector<float> cent;
-    kmeans_gpu(this, metric, dim, n, x, nlist, 10, 256, 1234, cent,
-               [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) { assign_dev(cd, kk, cid.p, xd, dim, l2, m, out); },
+    kmeans_gpu(this, metric, dim, n, x, k, 10, 256, 1234, cent,
+               [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) { assign_dev(cd, kk, cid.p, xd, dim, l2, m, out, stream); },
                [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); });
+  }
+
+  // PQ stage: the codebooks [M, ksub, dsub] of the n rows' residuals to the centroids cent [nc, dim]
+  void train_codebooks_locked(int64_t n, const float* x, const std::vector<float>& cent, std::vector<float>& cb) {
+    const bool l2 = metric == B200VS_L2;
+    const int nc = (int)(cent.size() / dim);
+    DevBuf<long long> cid;
     // PQ training set: <= 256 * ksub vectors (fvecs_maybe_subsample, seed 1234), residuals to their centroid
     int64_t m = std::min<int64_t>(n, 256LL * ksub);
     std::vector<int64_t> perm(n);
@@ -491,12 +524,12 @@ struct IvfPqIndex : IndexBase {
     for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * dim], x + (size_t)perm[i] * dim, (size_t)dim * 4);
     DevBuf<float> xd, cd;
     DevBuf<long long> asg;
-    xd.reserve((size_t)m * dim, 0, stream); cd.reserve((size_t)nlist * dim, 0, stream); asg.reserve(m, 0, stream);
+    xd.reserve((size_t)m * dim, 0, stream); cd.reserve((size_t)nc * dim, 0, stream); asg.reserve(m, 0, stream);
     B200VS_CUDA(cudaMemcpyAsync(xd.p, sub.data(), (size_t)m * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(cd.p, cent.data(), (size_t)nlist * dim * 4, cudaMemcpyHostToDevice, stream));
+    B200VS_CUDA(cudaMemcpyAsync(cd.p, cent.data(), (size_t)nc * dim * 4, cudaMemcpyHostToDevice, stream));
     if (metric == B200VS_COSINE) launch_normalize_faiss(xd.p, m, dim, stream);
-    cid.free(); cid.reserve(nlist, 0, stream); launch_iota(cid.p, nlist, stream);
-    assign_dev(cd.p, nlist, cid.p, xd.p, dim, l2, m, asg.p);
+    cid.free(); cid.reserve(nc, 0, stream); launch_iota(cid.p, nc, stream);
+    assign_dev(cd.p, nc, cid.p, xd.p, dim, l2, m, asg.p, stream);
     std::vector<long long> h_asg(m);
     B200VS_CUDA(cudaMemcpyAsync(h_asg.data(), asg.p, (size_t)m * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaMemcpyAsync(sub.data(), xd.p, (size_t)m * dim * 4, cudaMemcpyDeviceToHost, stream));
@@ -508,39 +541,45 @@ struct IvfPqIndex : IndexBase {
     }
     // one k-means per sub-space (ksub centroids, 25 iterations, L2)
     const int dsub = dim / M;
-    std::vector<float> cb((size_t)M * ksub * dsub), slice((size_t)m * dsub), cbm;
+    std::vector<float> slice((size_t)m * dsub), cbm;
+    cb.assign((size_t)M * ksub * dsub, 0.f);
     for (int mm = 0; mm < M; ++mm) {
       for (int64_t i = 0; i < m; ++i) memcpy(&slice[(size_t)i * dsub], &sub[(size_t)i * dim + mm * dsub], (size_t)dsub * 4);
       kmeans_gpu(this, B200VS_L2, dsub, m, slice.data(), ksub, 25, 256, 1234, cbm,
-                 [&](const float* xs, int64_t mr, const float* cs, int kk, long long* out) { assign_dev(cs, kk, cid.p, xs, dsub, true, mr, out); },
+                 [&](const float* xs, int64_t mr, const float* cs, int kk, long long* out) { assign_dev(cs, kk, cid.p, xs, dsub, true, mr, out, stream); },
                  [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); });
       memcpy(&cb[(size_t)mm * ksub * dsub], cbm.data(), (size_t)ksub * dsub * 4);
     }
-    install(cent.data(), cb.data());
   }
-
-  void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override {
-    if (mode == kFlat) { flat->add(n, x, in_ids, upsert); return; }
+  // runs f with rw and gpu_mu held and the scratch reset, as train does
+  template <class F>
+  void locked_stage(F&& f) {
     std::unique_lock<std::shared_mutex> wl(rw);
-    if (mode == kNone) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-    // one residual row of shared memory per warp: 4 warps per CTA while they fit, fewer at large d (opt-in above 48 KB)
-    constexpr size_t kEncodeSmemMax = 227 * 1024;
-    const size_t row_bytes = (size_t)dim * 4;
-    if (row_bytes > kEncodeSmemMax) fail(B200VS_EILLEGAL_PARAMETERS, "dimension too large for the PQ encoder's shared-memory residual");
-    const int wpb = (int)std::min<size_t>(4, kEncodeSmemMax / row_bytes);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
     scratch.reset(stream);
-    if (upsert) remove_locked(n, in_ids);
-    float* st = scratch.alloc<float>((size_t)n * dim);
-    long long* st_ids = scratch.alloc<long long>(n);
-    long long* st_list = scratch.alloc<long long>(n);
+    f();
+  }
+
+  // the list-building calls (device write path, coarse slices, caller-supplied probes) need the IVF-PQ mode's lists
+  void require_lists() const {
+    if (mode == kFlat) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode (too few training rows) has no inverted lists");
+    if (mode == kNone) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+  }
+
+  // warps per CTA of pq_encode_kernel: one residual row of shared memory per warp, 4 warps while they fit, fewer at large d
+  // (opt-in above 48 KB).  Checked before anything changes.
+  int encode_warps() const {
+    constexpr size_t kEncodeSmemMax = 227 * 1024;
+    const size_t row_bytes = (size_t)dim * 4;
+    if (row_bytes > kEncodeSmemMax) fail(B200VS_EILLEGAL_PARAMETERS, "dimension too large for the PQ encoder's shared-memory residual");
+    return (int)std::min<size_t>(4, kEncodeSmemMax / row_bytes);
+  }
+  // prepared rows st [n, dim] and their lists -> code rows [n, code_size] in the scratch (packed below 8 bits), on `stream`
+  const unsigned char* encode_locked(int64_t n, const float* st, const long long* st_list, int wpb) {
+    const size_t row_bytes = (size_t)dim * 4;
     unsigned char* st_codes = scratch.alloc<unsigned char>((size_t)n * M);
-    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    if (metric == B200VS_COSINE) launch_normalize_faiss(st, n, dim, stream);
-    assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, st_list);
     B200VS_CUDA(cudaFuncSetAttribute(pq_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wpb * row_bytes)));
     pq_encode_kernel<<<(unsigned)cdiv(n, wpb), wpb * 32, (size_t)wpb * row_bytes, stream>>>(st, st_list, centroids.p, codebooks.p, n, dim, M, ksub, st_codes);
     B200VS_CUDA(cudaGetLastError());
@@ -550,10 +589,103 @@ struct IvfPqIndex : IndexBase {
       B200VS_CUDA(cudaGetLastError());
       st_codes = packed;
     }
+    return st_codes;
+  }
+
+  void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override {
+    if (mode == kFlat) { flat->add(n, x, in_ids, upsert); return; }
+    std::unique_lock<std::shared_mutex> wl(rw);
+    if (mode == kNone) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    const int wpb = encode_warps();
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    if (upsert) remove_locked(n, in_ids);
+    float* st = scratch.alloc<float>((size_t)n * dim);
+    long long* st_ids = scratch.alloc<long long>(n);
+    long long* st_list = scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
+    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
+    if (metric == B200VS_COSINE) launch_normalize_faiss(st, n, dim, stream);
+    assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, st_list, stream);
+    const unsigned char* st_codes = encode_locked(n, st, st_list, wpb);
     std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
     append_encoded(n, st_codes, st_ids, in_ids, h_list.data());
+  }
+
+  // b200vs_add_with_ids_device: the host add's steps on device rows (upsert removes first; cosine rows are normalised on
+  // a copy unless `prepared`; lists_dev NULL = nearest centroid), so codes, ids and list layout equal a host add's
+  void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    require_lists();
+    const int wpb = encode_warps();
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    std::vector<int64_t> h_ids(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    if (upsert) remove_locked(n, h_ids.data());
+    const float* st = x_dev;
+    if (metric == B200VS_COSINE && !prepared) {  // the normaliser works in place: keep the caller's rows intact
+      float* cp = scratch.alloc<float>((size_t)n * dim);
+      B200VS_CUDA(cudaMemcpyAsync(cp, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
+      launch_normalize_faiss(cp, n, dim, stream);
+      st = cp;
+    }
+    const long long* st_list = lists_dev;
+    if (!st_list) {
+      long long* tmp = scratch.alloc<long long>(n);
+      assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, tmp, stream);
+      st_list = tmp;
+    }
+    std::vector<long long> h_list(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    for (int64_t i = 0; i < n; ++i)
+      if (h_list[i] < 0 || h_list[i] >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
+    const unsigned char* st_codes = encode_locked(n, st, st_list, wpb);
+    append_encoded(n, st_codes, ids_dev, h_ids.data(), h_list.data());
+  }
+
+  // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
+  void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) override {
+    require_lists();
+    assign_dev(centroids.p, nlist, cent_ids.p, x_dev, dim, metric == B200VS_L2, n, out_lists_dev, s);
+  }
+
+  // one code + id arena holding every list at its final size (+ 1/16 slack), as IvfFlatIndex::reserve_lists
+  void reserve_lists(const int64_t* rows_per_list, int n_lists) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    require_lists();
+    if (n_lists != nlist) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: list count does not match the trained index");
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    if (L.live + L.dead > 0) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists needs an empty index");
+    for (int l = 0; l < nlist; ++l)
+      if (rows_per_list[l] < 0 || rows_per_list[l] >= (1LL << 31) - 64) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: bad list size");
+    int64_t used = 0;
+    for (int l = 0; l < nlist; ++l) {
+      const int64_t want = rows_per_list[l];
+      ListMeta& m = L.lists[l];
+      m.off = used; m.len = 0; m.dead = 0;
+      m.cap = want ? IvfLists::round32(want + want / 16 + 32) : 0;
+      used += m.cap;
+    }
+    const int64_t tail = std::max<int64_t>(used / 64, 4096);  // room for lists that still outgrow their reservation
+    L.arena_used = L.arena_used_before = used;
+    L.arena_cap = used + tail;
+    codes.free(); ids.free();
+    codes.reserve((size_t)L.arena_cap * code_size, 0, stream);
+    ids.reserve((size_t)L.arena_cap, 0, stream);
+    B200VS_CUDA(cudaMemsetAsync(ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
+    L.h_ids.assign(L.arena_cap, -1);
+    L.upload(stream);
   }
 
   // rows already encoded (device codes [n, code_size], device ids) go to the tails of their lists; callers hold the write lock
@@ -637,24 +769,46 @@ struct IvfPqIndex : IndexBase {
 
   // coarse quantiser -> per-query LUT -> code scan + select -> merge.  Range mode (has_thr): keep hits strictly inside the
   // raw threshold (L2: dis < thr; IP: dis > thr), at most k of them, closest first; out_counts = hits per query.
+  // shared memory of the LUT scan's CTA (LUT + select pool), refused above one SM's 227 KB
+  size_t scan_smem(int k) const {
+    const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
+    const size_t smem = (size_t)M * ksub * 4 + BlockSelect::smem_bytes(select_pool_cap(k, threads));
+    if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
+    return smem;
+  }
+  int resolve_nprobe(const SearchCtx& sc) const {
+    const int nprobe = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchIvfPqParamNprobe, raw_ivf_pq.cc:170
+    return std::min(nprobe, nlist);                      // raw_ivf_pq.cc:190
+  }
+  // the coarse quantiser of scan_codes over centroid rows [c0, c1): top-nprobe GLOBAL list ids, and the raw coarse values
+  // (L2 distance or ip) when out_raw is set
+  void coarse_rows(int64_t nq, const float* q, int nprobe, int c0, int c1, float* out_raw, long long* out_lists, cudaStream_t s) {
+    ScanJob cj;
+    cj.l2 = metric == B200VS_L2; cj.vecs = centroids.p + (size_t)c0 * dim; cj.ids = cent_ids.p + c0; cj.d = dim; cj.mode = 0; cj.n = c1 - c0;
+    run_scan(this, cj, nq, q, nprobe, nullptr, out_raw, out_lists, nullptr, s);
+  }
+
   void scan_codes(int64_t nq, const float* xq, int k, const SearchCtx& sc, bool has_thr, float thr_raw, float* od, long long* oi, int* oc,
                   cudaStream_t s) {
+    scan_smem(k);  // checked before anything is launched
+    const float* q = prepare_queries(nq, xq, s);
+    const int nprobe = resolve_nprobe(sc);
+    // coarse quantiser: top-nprobe lists + raw coarse values
+    long long* probes = scratch.alloc<long long>((size_t)nq * nprobe);
+    float* coarse = scratch.alloc<float>((size_t)nq * nprobe);
+    coarse_rows(nq, q, nprobe, 0, nlist, coarse, probes, s);
+    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+    scan_lists(nq, q, k, sc, probes, coarse, nprobe, has_thr, thr_raw, od, oi, oc, s);
+  }
+
+  // per-query LUT -> code scan + select of the probed lists -> merge.  q prepared; coarse = dis0 per (query, probe).
+  void scan_lists(int64_t nq, const float* q, int k, const SearchCtx& sc, const long long* probes, const float* coarse, int nprobe,
+                  bool has_thr, float thr_raw, float* od, long long* oi, int* oc, cudaStream_t s) {
     const int T = M * ksub;
     const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
     const int pool_cap = select_pool_cap(k, threads);
-    const size_t smem = (size_t)T * 4 + BlockSelect::smem_bytes(pool_cap);  // checked before anything is launched
-    if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
-    const float* q = prepare_queries(nq, xq, s);
+    const size_t smem = scan_smem(k);
     const bool l2 = metric == B200VS_L2;
-    int nprobe = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchIvfPqParamNprobe, raw_ivf_pq.cc:170
-    nprobe = std::min(nprobe, nlist);              // raw_ivf_pq.cc:190
-    // coarse quantiser: top-nprobe lists + raw coarse values
-    ScanJob cj;
-    cj.l2 = l2; cj.vecs = centroids.p; cj.ids = cent_ids.p; cj.d = dim; cj.mode = 0; cj.n = nlist;
-    long long* probes = scratch.alloc<long long>((size_t)nq * nprobe);
-    float* coarse = scratch.alloc<float>((size_t)nq * nprobe);
-    run_scan(this, cj, nq, q, nprobe, nullptr, coarse, probes, nullptr, s);
-    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
     float* sim = scratch.alloc<float>((size_t)nq * T);
     pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, ksub, sim);
     PqScanArgs a;
@@ -691,6 +845,50 @@ struct IvfPqIndex : IndexBase {
     }
     B200VS_CUDA(cudaGetLastError());
     launch_count(3);
+  }
+
+  // ---- list-sharded building blocks (include/b200vs.h), in the IVF-PQ mode only ----
+  int nlist_now() const override { return nlist; }
+  int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
+  // b200vs_coarse_device: the coarse pass of scan_codes on rows [c0, c1); score = L2 distance or -ip, in (score, list id) order
+  void coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) override {
+    require_lists();
+    if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
+    coarse_rows(nq, prepare_queries(nq, xq, s), nprobe, c0, c1, out_score, out_lists, s);
+    if (metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);  // -> ascending ranking score
+  }
+  void coarse_probes_dev(int64_t nq, const float* q_prepared, int nprobe, long long* out_lists, cudaStream_t s) override {
+    require_lists();
+    coarse_rows(nq, q_prepared, nprobe, 0, nlist, nullptr, out_lists, s);
+  }
+  // refusals of a probe-driven search that depend on its arguments and the trained state only: a sharded search checks them
+  // before its first collective
+  void check_probe_search(int64_t nq, int k) const override {
+    require_lists();
+    if (nq > 65535) fail(B200VS_EILLEGAL_PARAMETERS, "batch too large (max 65535 queries per call)");
+    scan_smem(k);
+  }
+  void search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
+                         long long* oi, cudaStream_t s) override {
+    if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }
+    require_lists();
+    search_probes_prepared_dev(nq, prepare_queries(nq, xq, s), k, probes, nprobe, sc, od, oi, s);
+  }
+  // the LUT scan of scan_codes on caller-supplied probes; dis0 is recomputed per (query, probe) by pq_dis0_kernel
+  void search_probes_prepared_dev(int64_t nq, const float* q, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
+                                  long long* oi, cudaStream_t s) override {
+    if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }
+    check_probe_search(nq, k);
+    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+    const long long n = (long long)nq * nprobe;
+    float* dis0 = scratch.alloc<float>((size_t)n);
+    const bool vec = (dim & 3) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0;  // the load width only, not the arithmetic
+    const unsigned grid = (unsigned)cdiv(n * 4, 256);
+    if (n <= 0) {
+    } else if (metric == B200VS_L2) pq_dis0_kernel<true><<<grid, 256, 0, s>>>(q, centroids.p, probes, L.d_len.p, n, nprobe, dim, vec, dis0);
+    else pq_dis0_kernel<false><<<grid, 256, 0, s>>>(q, centroids.p, probes, L.d_len.p, n, nprobe, dim, vec, dis0);
+    B200VS_CUDA(cudaGetLastError());
+    scan_lists(nq, q, k, sc, probes, dis0, nprobe, false, 0.f, od, oi, nullptr, s);
   }
 
   // VectorIndexRawIvfPq::RangeSearch, vector_index_raw_ivf_pq.cc:212-278: faiss IndexIVFPQ::range_search on the codes —
@@ -832,5 +1030,29 @@ struct IvfPqIndex : IndexBase {
 };
 
 IndexBase* make_ivf_pq(b200vs_metric m, int d, const b200vs_params& p) { return new IvfPqIndex(m, d, p); }
+
+static IvfPqIndex* as_ivf_pq(IndexBase* ix) {
+  auto* p = dynamic_cast<IvfPqIndex*>(ix);
+  if (!p) fail(B200VS_EINTERNAL, "not an IVF_PQ index");
+  return p;
+}
+
+int ivf_pq_ksub(IndexBase* ix) { return as_ivf_pq(ix)->ksub; }
+
+void ivf_pq_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent) {
+  IvfPqIndex* p = as_ivf_pq(ix);
+  p->locked_stage([&] { p->train_coarse_locked(n, x, k, cent); });
+}
+
+void ivf_pq_train_state(IndexBase* ix, int64_t n, const float* x, const std::vector<float>& cent, std::vector<unsigned char>& blob) {
+  IvfPqIndex* p = as_ivf_pq(ix);
+  std::vector<float> cb;
+  p->locked_stage([&] { p->train_codebooks_locked(n, x, cent, cb); });
+  const int64_t hdr[6] = {0x51505649, (int64_t)(cent.size() / p->dim), p->dim, (int64_t)p->metric, p->M, p->nbits};
+  blob.resize(48 + (cent.size() + cb.size()) * 4);
+  memcpy(blob.data(), hdr, 48);
+  memcpy(blob.data() + 48, cent.data(), cent.size() * 4);
+  memcpy(blob.data() + 48 + cent.size() * 4, cb.data(), cb.size() * 4);
+}
 
 }  // namespace b200vs

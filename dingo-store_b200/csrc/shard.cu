@@ -1,11 +1,12 @@
 // shard.cu — list-sharded multi-GPU deployment behind the C ABI (b200vs_shard_*, include/b200vs.h).
 //
-// One process per GPU.  Every rank holds the replicated centroid table of ONE logical IVF-Flat index and the rows of the
-// inverted lists it owns (contiguous blocks of lists per rank — equivalently Raft regions mapped to GPUs,
-// src/vector/vector_index.h:54-55).  A batched search is:
+// One process per GPU.  Every rank holds the replicated trained state (centroids; IVF-PQ: and codebooks) of ONE logical
+// IVF-Flat or IVF-PQ index and the rows of the inverted lists it owns (contiguous blocks of lists per rank — equivalently
+// Raft regions mapped to GPUs, src/vector/vector_index.h:54-55).  A batched search is:
 //   1. coarse quantiser on this rank's SLICE of the batch (all ranks hold all queries), one all-gather of the probe table
 //      (the faiss quantizer->search step of IndexIVF::search, src/vector/vector_index_ivf_flat.cc:247-251);
-//   2. tile scan of the probed lists this rank owns (csrc/tc_scan.cu) -> exact local top-k;
+//   2. scan of the probed lists this rank owns (IVF-Flat: the tile scan, csrc/tc_scan.cu; IVF-PQ: the LUT scan, with the
+//      coarse value of every probe recomputed on the rank, csrc/ivf_pq.cu) -> exact local top-k;
 //   3. ONE ncclAllGather of the packed per-shard top-k ((distance, id) 16-byte records) over NVLink, then the k-way merge
 //      kernel — the engine's analogue of VectorIndexWrapper::MergeSearchResults (src/vector/vector_index.cc:1056-1108).
 // Rows are routed to their list owner at add time (b200vs_shard_add*: assignment on the sender, grouped ncclSend/ncclRecv).
@@ -335,6 +336,76 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
   L.last = s;
 }
 
+// Replicate rank `root`'s trained state on every rank (b200vs_shard_broadcast_state; the caller holds add_mu).
+void broadcast_state_locked(b200vs_shard* sh, int root) {
+  IndexBase* ix = sh->ix;
+  ix->set_device();
+  DevBuf<long long> len;
+  len.reserve(1, 0, sh->ws);
+  long long need = sh->rank == root ? (long long)ix->get_state(nullptr, 0) : 0;
+  if (sh->rank == root && need <= 0) fail(B200VS_EVECTOR_NOT_TRAIN, "root has no trained state");
+  B200VS_CUDA(cudaMemcpyAsync(len.p, &need, 8, cudaMemcpyHostToDevice, sh->ws));
+  if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(len.p, len.p, 1, ncclInt64, root, sh->lanes[0]->comm, sh->ws));
+  B200VS_CUDA(cudaMemcpyAsync(&need, len.p, 8, cudaMemcpyDeviceToHost, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  std::vector<unsigned char> blob((size_t)need);
+  if (sh->rank == root) ix->get_state(blob.data(), blob.size());
+  DevBuf<unsigned char> db;
+  db.reserve((size_t)need, 0, sh->ws);
+  if (sh->rank == root) B200VS_CUDA(cudaMemcpyAsync(db.p, blob.data(), (size_t)need, cudaMemcpyHostToDevice, sh->ws));
+  if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(db.p, db.p, (size_t)need, ncclUint8, root, sh->lanes[0]->comm, sh->ws));
+  if (sh->rank != root) {
+    B200VS_CUDA(cudaMemcpyAsync(blob.data(), db.p, (size_t)need, cudaMemcpyDeviceToHost, sh->ws));
+    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+    ix->set_state(blob.data(), blob.size());
+  } else {
+    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  }
+}
+
+// b200vs_shard_train on IVF_PQ.  The per-rank row counts are exchanged first, so that a refusal for too few rows happens on
+// every rank at once.  Coarse stage: each rank clusters its rows into nlist / world centroids with the k-means of IVF-PQ's
+// own train (exact assignment), one all-gather.  PQ stage: rank 0 trains the codebooks with train's PQ rule on the
+// residuals of its rows to the global centroids, and the state broadcast replicates the result.  At world = 1 this is
+// b200vs_train step for step, so the trained state is byte-equal.
+void shard_train_pq(b200vs_shard* sh, int64_t n, const float* x) {
+  IndexBase* ix = sh->ix;
+  std::lock_guard<std::mutex> g(sh->add_mu);
+  const int W = sh->world, d = ix->dim, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
+  if (nlist % W != 0) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: nlist must be a multiple of the world size");
+  if (ix->sub_type() == B200VS_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode has no inverted lists to shard");
+  const int nl = nlist / W;
+  const long long pq_rows = 256LL * ivf_pq_ksub(ix);
+  ix->set_device();
+  std::vector<long long> counts((size_t)W, (n > 0 && !x) ? -1 : (long long)n);  // rows of every rank (a null x counts as none)
+  if (W > 1) {
+    DevBuf<long long> dc;
+    dc.reserve((size_t)W, 0, sh->ws);
+    B200VS_CUDA(cudaMemcpyAsync(dc.p + sh->rank, &counts[sh->rank], 8, cudaMemcpyHostToDevice, sh->ws));
+    B200VS_NCCL(nccl().AllGather(dc.p + sh->rank, dc.p, 1, ncclInt64, sh->lanes[0]->comm, sh->ws));
+    B200VS_CUDA(cudaMemcpyAsync(counts.data(), dc.p, (size_t)W * 8, cudaMemcpyDeviceToHost, sh->ws));
+    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  }
+  for (int r = 0; r < W; ++r)
+    if (counts[r] < nl)
+      fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank " + std::to_string(r) + " has fewer training rows than nlist / world centroids");
+  if (counts[0] < pq_rows) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank 0 needs 256 * 2^nbits training rows for the PQ codebooks");
+  std::vector<float> local, cent((size_t)nlist * d);
+  ivf_pq_train_coarse(ix, n, x, nl, local);
+  DevBuf<float> all;
+  all.reserve((size_t)nlist * d, 0, sh->ws);
+  B200VS_CUDA(cudaMemcpyAsync(all.p + (size_t)sh->rank * nl * d, local.data(), (size_t)nl * d * 4, cudaMemcpyHostToDevice, sh->ws));
+  if (W > 1) B200VS_NCCL(nccl().AllGather(all.p + (size_t)sh->rank * nl * d, all.p, (size_t)nl * d, ncclFloat, sh->lanes[0]->comm, sh->ws));
+  B200VS_CUDA(cudaMemcpyAsync(cent.data(), all.p, (size_t)nlist * d * 4, cudaMemcpyDeviceToHost, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  if (sh->rank == 0) {
+    std::vector<unsigned char> blob;
+    ivf_pq_train_state(ix, n, x, cent, blob);
+    ix->set_state(blob.data(), blob.size());
+  }
+  broadcast_state_locked(sh, 0);
+}
+
 }  // namespace
 
 extern "C" {
@@ -356,7 +427,10 @@ int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const ui
     if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
     *out = nullptr;
     IndexBase* ix = index_impl(idx);
-    if (ix->type != B200VS_IVF_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "list sharding is implemented for IVF_FLAT (HNSW: replicas only)");
+    if (ix->type != B200VS_IVF_FLAT && ix->type != B200VS_IVF_PQ)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "list sharding is implemented for IVF_FLAT and IVF_PQ (HNSW: replicas only)");
+    if (ix->type == B200VS_IVF_PQ && ix->sub_type() == B200VS_FLAT)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode (too few training rows) has no inverted lists to shard");
     if (world < 1 || rank < 0 || rank >= world) fail(B200VS_EILLEGAL_PARAMETERS, "bad rank / world");
     if (world > 1 && !id) fail(B200VS_EILLEGAL_PARAMETERS, "null communicator id");
     lanes = std::max(1, std::min(lanes <= 0 ? 2 : lanes, kLanes));
@@ -400,6 +474,10 @@ int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
     IndexBase* ix = sh->ix;
+    if (ix->type == B200VS_IVF_PQ) {
+      shard_train_pq(sh, n, x);
+      return B200VS_OK;
+    }
     if (n <= 0 || !x) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
     std::lock_guard<std::mutex> g(sh->add_mu);
     const int W = sh->world, d = ix->dim, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
@@ -428,35 +506,13 @@ int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
   });
 }
 
-// Replicate rank `root`'s trained state (centroids) on every rank.
+// Replicate rank `root`'s trained state (centroids; IVF-PQ: and codebooks) on every rank.
 int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
     if (root < 0 || root >= sh->world) fail(B200VS_EILLEGAL_PARAMETERS, "bad root");
     std::lock_guard<std::mutex> g(sh->add_mu);
-    ix->set_device();
-    DevBuf<long long> len;
-    len.reserve(1, 0, sh->ws);
-    long long need = sh->rank == root ? (long long)ix->get_state(nullptr, 0) : 0;
-    if (sh->rank == root && need <= 0) fail(B200VS_EVECTOR_NOT_TRAIN, "root has no trained state");
-    B200VS_CUDA(cudaMemcpyAsync(len.p, &need, 8, cudaMemcpyHostToDevice, sh->ws));
-    if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(len.p, len.p, 1, ncclInt64, root, sh->lanes[0]->comm, sh->ws));
-    B200VS_CUDA(cudaMemcpyAsync(&need, len.p, 8, cudaMemcpyDeviceToHost, sh->ws));
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-    std::vector<unsigned char> blob((size_t)need);
-    if (sh->rank == root) ix->get_state(blob.data(), blob.size());
-    DevBuf<unsigned char> db;
-    db.reserve((size_t)need, 0, sh->ws);
-    if (sh->rank == root) B200VS_CUDA(cudaMemcpyAsync(db.p, blob.data(), (size_t)need, cudaMemcpyHostToDevice, sh->ws));
-    if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(db.p, db.p, (size_t)need, ncclUint8, root, sh->lanes[0]->comm, sh->ws));
-    if (sh->rank != root) {
-      B200VS_CUDA(cudaMemcpyAsync(blob.data(), db.p, (size_t)need, cudaMemcpyDeviceToHost, sh->ws));
-      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-      ix->set_state(blob.data(), blob.size());
-    } else {
-      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-    }
+    broadcast_state_locked(sh, root);
     return B200VS_OK;
   });
 }
@@ -676,6 +732,7 @@ int b200vs_shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const f
     ix->set_device();
     cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
     LaneGuard lane(ix, s);
+    ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
     ix->reset_stats();
     shard_search_stream(sh, *sl.lane, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
     ix->phases_finish(s);
@@ -705,6 +762,7 @@ int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* x
       b200vs_shard::SLane& L = *sl.lane;
       s = L.own;
       LaneGuard lane(ix, s);
+      ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
       ix->reset_stats();
       const int64_t per = (nq + W - 1) / W;
       L.q_all.reserve((size_t)per * W * d, 0, s);

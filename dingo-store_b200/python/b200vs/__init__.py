@@ -412,7 +412,7 @@ class Index:
 
 
 class Shard:
-    """One rank of a list-sharded IVF_FLAT index (b200vs_shard_*).  `id_bytes`: the 128-byte rendezvous blob made by
+    """One rank of a list-sharded IVF_FLAT or IVF_PQ index (b200vs_shard_*).  `id_bytes`: the 128-byte rendezvous blob made by
     Shard.unique_id() on rank 0 and distributed by the host (tests: torch.distributed broadcast)."""
 
     @staticmethod

@@ -201,28 +201,34 @@ int b200vs_export_list(b200vs_index* idx, int32_t list, int64_t cap, float* vect
 int b200vs_merge_topk_device(int32_t device, int32_t nparts, int64_t nq, int32_t k, const float* parts_dist,
                              const int64_t* parts_ids, float* out_dist, int64_t* out_ids, void* stream);
 
-/* List-sharded multi-GPU building blocks (IVF_FLAT): every rank holds all centroids but owns only some lists.
+/* List-sharded multi-GPU building blocks (IVF_FLAT, and IVF_PQ in its IVF-PQ mode; an IVF_PQ index in inner-Flat mode has
+ * no lists and returns EVECTOR_NOT_SUPPORT): every rank holds all centroids but owns only some lists.
  * b200vs_coarse_device ranks the centroid rows [list_begin, list_end) only (this rank's share of the coarse work):
  * out_lists = GLOBAL list ids, out_score = the ranking score (L2 distance, or -ip: exact and ascending, so no
  * rounding can reorder ties), both [nq, nprobe] in (score, list id) order, so the per-rank
  * results can be all-gathered and merged with b200vs_merge_topk_device into the global top-nprobe
  * (= faiss quantizer->search(nq, x, nprobe), vector_index_ivf_flat.cc:247-251).  b200vs_search_probes_device then scans
- * the probed lists this rank owns for those (caller-supplied) probes. */
+ * the probed lists this rank owns for those (caller-supplied) probes (IVF_PQ: the coarse value each LUT scan starts from is
+ * recomputed per (query, probe) with the coarse pass's arithmetic, so the results are b200vs_search's bit for bit). */
 int b200vs_coarse_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int32_t nprobe, int32_t list_begin, int32_t list_end,
                          float* out_score_dev, int64_t* out_lists_dev, void* stream);
 int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int32_t k, const int64_t* probes_dev, int32_t nprobe,
                                 const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
 
 /* ---- List-sharded multi-GPU deployment (SURVEY.md 8e; one process per GPU) ----------------------------------------------
- * One LOGICAL IVF_FLAT index over `world` GPUs of one box: the centroid table is replicated, rank r owns the inverted lists
+ * One LOGICAL IVF_FLAT or IVF_PQ index over `world` GPUs of one box: the trained state (centroids; IVF_PQ: and codebooks)
+ * is replicated, rank r owns the inverted lists
  * [r * ceil(nlist / world), (r + 1) * ceil(nlist / world)) (b200vs_shard_list_range) — equivalently Raft regions mapped to
  * GPUs (src/vector/vector_index.h:54-55).  Every entry point below is COLLECTIVE: all ranks call it with the same
  * arguments (except the rows each rank contributes to add).  Communication is NCCL over NVLink, resolved at run time
  * (dlopen libnccl.so.2; override with B200VS_NCCL_LIB), one communicator per batch in flight.
  *   shard_unique_id : rank 0 creates the rendezvous blob; the host passes it to the other ranks out of band (dingo-store: RPC)
- *   shard_create    : wraps an (untrained or trained, still empty) IVF_FLAT index created with the GLOBAL nlist; `lanes` =
- *                     batches that may be in flight (<= 0: 2)
- *   shard_train     : distributed training — each rank clusters its rows into nlist / world centroids, one all-gather
+ *   shard_create    : wraps an (untrained or trained, still empty) IVF_FLAT or IVF_PQ index created with the GLOBAL nlist
+ *                     (IVF_PQ in inner-Flat mode: EVECTOR_NOT_SUPPORT); `lanes` = batches that may be in flight (<= 0: 2)
+ *   shard_train     : distributed training — each rank clusters its rows into nlist / world centroids, one all-gather.
+ *                     IVF_PQ: the row counts are exchanged first (fewer than nlist / world rows on any rank, or fewer than
+ *                     256 * 2^nbits on rank 0: EILLEGAL_PARAMETERS on every rank); rank 0 then trains the codebooks on its
+ *                     rows' residuals and its state is broadcast.  At world = 1 the state equals b200vs_train's.
  *   shard_broadcast_state : or: replicate rank `root`'s trained state (b200vs_train / b200vs_set_trained_state there)
  *   shard_add[_device]    : each rank passes the rows it holds; rows travel to the owner of their nearest centroid's list
  *   shard_plan_add_device / shard_plan_commit : optional first pass of a bulk build (assignment only) that pre-sizes every
@@ -258,13 +264,15 @@ int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const floa
 int b200vs_shard_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, int32_t k,
                                const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
 
-/* Device-pointer write path of a single index (IVF_FLAT): rows and ids already on the index's device.  lists_dev (nullable)
- * = the inverted list of every row when the caller has already assigned them (b200vs_assign_device); returns when done. */
+/* Device-pointer write path of a single index (IVF_FLAT, IVF_PQ in its IVF-PQ mode): rows and ids already on the index's
+ * device.  lists_dev (nullable) = the inverted list of every row when the caller has already assigned them
+ * (b200vs_assign_device); returns when done.  IVF_PQ: codes, ids and list layout equal a host b200vs_add_with_ids's. */
 int b200vs_add_with_ids_device(b200vs_index* idx, int64_t n, const float* x_dev, const int64_t* ids_dev, const int64_t* lists_dev,
                                int upsert);
 /* faiss quantizer->assign: nearest centroid of every (raw) row, out_lists_dev[n]; synchronous. */
 int b200vs_assign_device(b200vs_index* idx, int64_t n, const float* x_dev, int64_t* out_lists_dev);
-/* Pre-size every inverted list of an EMPTY trained IVF_FLAT index (rows_per_list[nlist], host) in one arena allocation. */
+/* Pre-size every inverted list of an EMPTY trained IVF_FLAT or IVF_PQ index (rows_per_list[nlist], host) in one arena
+ * allocation. */
 int b200vs_reserve_lists(b200vs_index* idx, const int64_t* rows_per_list, int32_t nlist);
 
 /* Pairwise distance matrix, the UtilService path UtilServiceImpl::VectorCalcDistance (src/server/util_service.cc:45-92)
