@@ -13,6 +13,9 @@
   cfg6  Binary Flat Hamming, 1M x 256 bits, batch 1024, top-10
   cfg6s Binary Flat Hamming, 16384 x 256 bits, batch 128, top-10 (below the tile scan's work threshold: exact scan)
   cfg7  Binary IVF-Flat Hamming, 10M x 512 bits, nlist 2048, nprobe 80, batch 1024, top-10   (--bin-n, --bin-dim)
+  range IVF-Flat L2 range search at the headline shape (1M x 768, nlist 1024, nprobe 32, batch 1024, max_results 1024,
+        radius keeping ~100 hits a query): the tile range scan against exact_only, alternating in one call; nq = 8 (the exact
+        side of the dispatch); a radius every query's capture overflows; the same search through b200vs_shard_* at world 1
 Each line: device-resident QPS (CUDA events), e2e QPS through the host-pointer C ABI, parity with the oracle on a
 bounded sample, the dominant kernel's time from the library's profiling mode and the algorithmic figure of
 SURVEY.md §8(d).  Scaled sizes are stated in the line ("scaled_from").
@@ -665,6 +668,91 @@ def cfg7(o, cores, n, dim, oracle_q=16):
     return line
 
 
+def card():
+    """The card the numbers were measured on: name and power limit (nvidia-smi), stated beside every number."""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return out.stdout.strip().splitlines()[0]
+    except Exception as e:
+        return f"unknown ({e!r})"
+
+
+def cfg_range(o, cores, steps=5):
+    """Range search at the headline IVF-Flat shape.  The plain call has no device-pointer entry point, so its times are host
+    calls (query upload, [nq, max_results] results back); the sharded call is timed device-resident with CUDA events."""
+    n, d, nlist, nprobe, nq, mr = 1_000_000, 768, 1024, 32, 1024, 1024
+    xb = rnd(n, d, 1234)
+    ix = b200vs.Index(b200vs.IVF_FLAT, b200vs.L2, d, nlist=nlist)
+    ix.train(xb[:nlist * 256])
+    for a in range(0, n, 32768):
+        ix.add(xb[a:a + 32768], np.arange(a + 1, a + 1 + min(32768, n - a), dtype=np.int64))
+    del xb
+    xq = rnd(nq, d, 4321)
+    Dk, _ = ix.search(xq[:64], 100, nprobe=nprobe)
+    radius = float(np.median(Dk[:, 99]))  # ~100 hits a query
+
+    def same(a, b):
+        return bool(np.array_equal(a[2], b[2]) and np.array_equal(a[1], b[1]) and np.array_equal(a[0].view(np.uint32), b[0].view(np.uint32)))
+
+    def timed(q, r, exact):
+        ix.range_search(q, r, mr, nprobe=nprobe, exact_only=exact)
+        t = time.perf_counter()
+        for _ in range(steps):
+            res = ix.range_search(q, r, mr, nprobe=nprobe, exact_only=exact)
+        return (time.perf_counter() - t) / steps * 1e3, res
+
+    def profiled(q, r):
+        ix.set_profiling(True)
+        ix.range_search(q, r, mr, nprobe=nprobe)
+        st, ph = ix.stats(), ix.phase_times()
+        ix.set_profiling(False)
+        return st, ph
+
+    def pair(q, r, reps=3):
+        tile, exact, eq = [], [], True
+        for _ in range(reps):  # alternating, so both see the same machine state
+            tm, a = timed(q, r, False)
+            em, b = timed(q, r, True)
+            tile.append(tm); exact.append(em); eq = eq and same(a, b)
+        st, ph = profiled(q, r)
+        return {"nq": len(q), "ms_per_batch_e2e_tile": tile, "ms_per_batch_e2e_exact_only": exact,
+                "qps_e2e_tile": len(q) / min(tile) * 1e3, "qps_e2e_exact_only": len(q) / min(exact) * 1e3,
+                "ids_dist_counts_equal_all_queries": eq, "mean_hits_kept": float(np.mean(a[2])),
+                "tile_queries": st[1], "rerun_queries": st[2], "capture_kernel_ms": st[3] / 1e6, "phase_ms": ph}
+
+    lines = {"headline": pair(xq, radius), "nq8": pair(xq[:8], radius), "overflow": pair(xq, radius * 4)}
+    sh = b200vs.Shard(ix, 0, 1, None, lanes=2)
+    sp, _keep = b200vs.make_search_params(nprobe=nprobe)
+    dev = torch.device("cuda", 0)
+    q = torch.from_numpy(xq).to(dev)
+    od = torch.empty((nq, mr), dtype=torch.float32, device=dev)
+    oi = torch.empty((nq, mr), dtype=torch.int64, device=dev)
+    oc = torch.empty((nq,), dtype=torch.int32, device=dev)
+    st = torch.cuda.Stream(device=dev)
+    for _ in range(2):
+        sh.range_search_device(nq, q.data_ptr(), radius, mr, od.data_ptr(), oi.data_ptr(), oc.data_ptr(), stream=st.cuda_stream, sp=sp)
+    st.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(st)
+    for _ in range(steps):
+        sh.range_search_device(nq, q.data_ptr(), radius, mr, od.data_ptr(), oi.data_ptr(), oc.data_ptr(), stream=st.cuda_stream, sp=sp)
+    e1.record(st)
+    st.synchronize()
+    dev_ms = e0.elapsed_time(e1) / steps
+    t = time.perf_counter()
+    for _ in range(steps):
+        hs = sh.range_search(xq, radius, mr, nprobe=nprobe)
+    e2e_ms = (time.perf_counter() - t) / steps * 1e3
+    plain = ix.range_search(xq, radius, mr, nprobe=nprobe)
+    dev_res = (od.cpu().numpy(), oi.cpu().numpy(), oc.cpu().numpy())
+    lines["shard_world1"] = {"ms_per_batch_device": dev_ms, "qps_device": nq / dev_ms * 1e3, "ms_per_batch_e2e": e2e_ms,
+                             "qps_e2e": nq / e2e_ms * 1e3, "equal_plain_host": same(hs, plain), "equal_plain_device": same(dev_res, plain)}
+    sh.close()
+    return {"config": "range IVF-Flat L2 1Mx768 nlist=1024 nprobe=32 batch=1024 max_results=1024", "card": card(),
+            "radius": radius, **lines}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="1,2,3,4")
@@ -691,7 +779,8 @@ def main():
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
            "3s": lambda: cfg3s(o, cores, a.pq_n, a.pq_nbits, a.pq_m),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
-           "6": lambda: cfg6(o, cores), "6s": lambda: cfg6s(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim)}
+           "6": lambda: cfg6(o, cores), "6s": lambda: cfg6s(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim),
+           "range": lambda: cfg_range(o, cores)}
     rank = int(os.environ.get("RANK", 0))
     for c in a.configs.split(","):
         t0 = time.time()

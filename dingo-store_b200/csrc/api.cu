@@ -446,6 +446,7 @@ int b200vs_range_search(b200vs_index* h, int64_t nq, const float* xq, float radi
     ix->set_device();
     LaneGuard lane(ix, nullptr);
     cudaStream_t s = lane.stream;
+    ix->reset_stats();
     float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
     float* dd = ix->scratch.alloc<float>((size_t)nq * max_results);
     long long* di = ix->scratch.alloc<long long>((size_t)nq * max_results);

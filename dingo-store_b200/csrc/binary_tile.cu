@@ -434,7 +434,7 @@ void bt_search(IndexBase* ix, const TcView& v, int w, int64_t nq, const uint32_t
   ix->stats[1] = nq;
   // 4) overflowed / unthresholded queries on the exact scan (device-side count: blocks beyond it exit at once)
   ix->phase(IndexBase::PH_FALLBACK, s);
-  run_scan_mapped(ix, exact, nq, qmap, qcount, reinterpret_cast<const float*>(q), k, out_dist, out_ids, s);
+  run_scan_mapped(ix, exact, nq, qmap, qcount, reinterpret_cast<const float*>(q), k, out_dist, nullptr, out_ids, nullptr, s);
   ix->phase(IndexBase::PH_OTHER, s);
   if (ix->profiling) {
     int h = 0, t[4] = {0, 0, 0, 0};

@@ -440,9 +440,17 @@ struct FlatIndex : IndexBase {
   void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
                         long long* oi, int* oc, cudaStream_t s) override {
     const float* q = prepare_queries(nq, xq, s);
+    const float thr = ip_like() ? 1.0F - radius : radius;
+    const TcView v = view();
+    if (rows > 0 && tc_range_eligible(this, v, nq, max_results, 1, sc)) {
+      long long* probes = scratch.alloc<long long>(nq);
+      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
+      tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, 1, sc, od, oi, oc, false, s);
+      return;
+    }
     ScanJob j = job(sc);
     j.has_thr = true;
-    j.thr_raw = ip_like() ? 1.0F - radius : radius;
+    j.thr_raw = thr;
     run_scan(this, j, nq, q, max_results, od, nullptr, oi, oc, s);
   }
 
@@ -489,6 +497,15 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p) { return ne
 // ============================================================================================
 // IVF arena shared by IVF-Flat (and reused by IVF-PQ for ids): see ivf_common.h
 // ============================================================================================
+
+void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s) {
+  if (od) B200VS_CUDA(cudaMemsetAsync(od, 0, (size_t)nq * k * 4, s));
+  B200VS_CUDA(cudaMemsetAsync(oi, 0xFF, (size_t)nq * k * 8, s));  // -1
+}
+void fill_empty_range(int64_t nq, int max_results, float* od, long long* oi, int* oc, cudaStream_t s) {
+  fill_empty_results(nq, max_results, od, oi, s);
+  if (oc) B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
+}
 
 struct IvfFlatIndex : IndexBase {
   int nlist;            // may degenerate to 1 at train time (vector_index_ivf_flat.cc:676-680)
@@ -601,6 +618,13 @@ struct IvfFlatIndex : IndexBase {
   }
   void search_probes_prepared_dev(int64_t nq, const float* q, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
                                   long long* oi, cudaStream_t s) override;
+  void range_search_probes_prepared_dev(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
+                                        const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) override {
+    if (!trained) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
+    range_probes(nq, q, radius, max_results, probes, nprobe, sc, od, oi, oc, true, s);
+  }
+  void range_probes(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe, const SearchCtx& sc,
+                    float* od, long long* oi, int* oc, bool raw_out, cudaStream_t s);
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
   int64_t remove(int64_t n, const int64_t* del) override;
   int64_t remove_locked(int64_t n, const int64_t* del);
@@ -819,10 +843,6 @@ int64_t IvfFlatIndex::remove(int64_t n, const int64_t* del) {
   return r;
 }
 
-void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s) {
-  if (od) B200VS_CUDA(cudaMemsetAsync(od, 0, (size_t)nq * k * 4, s));
-  B200VS_CUDA(cudaMemsetAsync(oi, 0xFF, (size_t)nq * k * 8, s));  // -1
-}
 
 void IvfFlatIndex::search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) {
   if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_flat.cc:224-227
@@ -880,18 +900,28 @@ void IvfFlatIndex::search_probes_prepared_dev(int64_t nq, const float* q, int k,
 
 void IvfFlatIndex::range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc,
                                     float* od, long long* oi, int* oc, cudaStream_t s) {
-  if (!trained) {
-    fill_empty_results(nq, max_results, od, oi, s);
-    if (oc) B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
-    return;
-  }
+  if (!trained) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
   const float* q = prepare_queries(nq, xq, s);
   const int nprobe = resolve_nprobe(sc);
   long long* probes = coarse(nq, q, nprobe, s);
+  range_probes(nq, q, radius, max_results, probes, nprobe, sc, od, oi, oc, false, s);
+}
+
+// range search of prepared queries over the probe table: the tile range scan when it applies, else the exact scan with the
+// range threshold.  raw_out: od = raw metric value instead of the API distance.
+void IvfFlatIndex::range_probes(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
+                                const SearchCtx& sc, float* od, long long* oi, int* oc, bool raw_out, cudaStream_t s) {
+  const float thr = ip_like() ? 1.0F - radius : radius;  // ivf_flat.cc:296-299
+  if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+  const TcView v = view();
+  if (L.live > 0 && tc_range_eligible(this, v, nq, max_results, nprobe, sc)) {
+    tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, nprobe, sc, od, oi, oc, raw_out, s);
+    return;
+  }
   ScanJob j = list_job(sc, probes, nprobe);
   j.has_thr = true;
-  j.thr_raw = ip_like() ? 1.0F - radius : radius;  // ivf_flat.cc:296-299
-  run_scan(this, j, nq, q, max_results, od, nullptr, oi, oc, s);
+  j.thr_raw = thr;
+  run_scan(this, j, nq, q, max_results, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, oc, s);
 }
 
 void IvfFlatIndex::export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) {

@@ -275,6 +275,13 @@ struct IndexBase {
     (void)nq; (void)q_prepared; (void)k; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
   }
+  // range search of prepared queries over caller-supplied probes (the local step of a sharded range search): the hits of
+  // range_search_dev, but od holds the raw metric value (L2 distance | ip), which orders hits as the single-index select does
+  virtual void range_search_probes_prepared_dev(int64_t nq, const float* q_prepared, float radius, int max_results, const long long* probes,
+                                                int nprobe, const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) {
+    (void)nq; (void)q_prepared; (void)radius; (void)max_results; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)oc; (void)s;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven range search only exists for IVF_FLAT and IVF_PQ");
+  }
   virtual int resolve_nprobe_api(const SearchCtx& sc) const { (void)sc; return 1; }
   // refusals of search_probes_prepared_dev that depend only on nq, k and the trained state (IVF-PQ: the LUT + select pool
   // must fit one SM's shared memory); a sharded search checks them on every rank before its first collective

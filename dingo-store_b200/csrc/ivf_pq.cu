@@ -803,7 +803,7 @@ struct IvfPqIndex : IndexBase {
 
   // per-query LUT -> code scan + select of the probed lists -> merge.  q prepared; coarse = dis0 per (query, probe).
   void scan_lists(int64_t nq, const float* q, int k, const SearchCtx& sc, const long long* probes, const float* coarse, int nprobe,
-                  bool has_thr, float thr_raw, float* od, long long* oi, int* oc, cudaStream_t s) {
+                  bool has_thr, float thr_raw, float* od, long long* oi, int* oc, cudaStream_t s, float* oraw = nullptr) {
     const int T = M * ksub;
     const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
     const int pool_cap = select_pool_cap(k, threads);
@@ -838,10 +838,10 @@ struct IvfPqIndex : IndexBase {
     timer.stop();
     if (l2) {
       B200VS_CUDA(cudaFuncSetAttribute(merge_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      merge_select_kernel<true><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, nullptr, oi, oc, nullptr, nullptr);
+      merge_select_kernel<true><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, oraw, oi, oc, nullptr, nullptr);
     } else {
       B200VS_CUDA(cudaFuncSetAttribute(merge_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      merge_select_kernel<false><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, nullptr, oi, oc, nullptr, nullptr);
+      merge_select_kernel<false><<<(unsigned)nq, SCAN_THREADS, smem2, s>>>(a.ws_kd, a.ws_kid, a.nsplit, k, a.pool_cap, od, oraw, oi, oc, nullptr, nullptr);
     }
     B200VS_CUDA(cudaGetLastError());
     launch_count(3);
@@ -879,6 +879,18 @@ struct IvfPqIndex : IndexBase {
                                   long long* oi, cudaStream_t s) override {
     if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }
     check_probe_search(nq, k);
+    scan_lists(nq, q, k, sc, probes, probe_dis0(nq, q, probes, nprobe, s), nprobe, false, 0.f, od, oi, nullptr, s);
+  }
+  // the thresholded LUT scan of range_search_dev on caller-supplied probes, the raw value (L2 distance | ip) in od
+  void range_search_probes_prepared_dev(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
+                                        const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) override {
+    if (mode == kNone) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
+    check_probe_search(nq, max_results);
+    scan_lists(nq, q, max_results, sc, probes, probe_dis0(nq, q, probes, nprobe, s), nprobe, true, ip_like() ? 1.0F - radius : radius,
+               nullptr, oi, oc, s, od);
+  }
+  // dis0 of every (query, probe) of a caller-supplied probe table
+  const float* probe_dis0(int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {
     if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
     const long long n = (long long)nq * nprobe;
     float* dis0 = scratch.alloc<float>((size_t)n);
@@ -888,7 +900,7 @@ struct IvfPqIndex : IndexBase {
     } else if (metric == B200VS_L2) pq_dis0_kernel<true><<<grid, 256, 0, s>>>(q, centroids.p, probes, L.d_len.p, n, nprobe, dim, vec, dis0);
     else pq_dis0_kernel<false><<<grid, 256, 0, s>>>(q, centroids.p, probes, L.d_len.p, n, nprobe, dim, vec, dis0);
     B200VS_CUDA(cudaGetLastError());
-    scan_lists(nq, q, k, sc, probes, dis0, nprobe, false, 0.f, od, oi, nullptr, s);
+    return dis0;
   }
 
   // VectorIndexRawIvfPq::RangeSearch, vector_index_raw_ivf_pq.cc:212-278: faiss IndexIVFPQ::range_search on the codes —
@@ -896,11 +908,7 @@ struct IvfPqIndex : IndexBase {
   // threshold epilogue instead of the k-th-best threshold.  Untrained -> empty results (:219-222).
   void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od, long long* oi,
                         int* oc, cudaStream_t s) override {
-    if (mode == kNone) {
-      fill_empty_results(nq, max_results, od, oi, s);
-      if (oc) B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
-      return;
-    }
+    if (mode == kNone) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
     if (mode == kFlat) {
       std::shared_lock<std::shared_mutex> rl(flat->rw);
       LaneGuard lg(flat.get(), s);

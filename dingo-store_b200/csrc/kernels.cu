@@ -27,13 +27,13 @@ void run_scan(IndexBase* ix, const ScanJob& job, int64_t nq, const float* querie
 
 // exact re-run of the queries listed in qmap[0 .. *qcount) (device-side count; grid sized for nq_max)
 void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const int* qmap, const int* qcount, const float* queries,
-                     int k, float* out_dist, long long* out_ids, cudaStream_t s) {
+                     int k, float* out_dist, float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s) {
   // few queries are ever re-run, but each one re-streams all its candidates: split a query over enough CTAs that a single
   // flagged query of a large index (cfg5: 2.4 GB of probed rows) is not an 8-CTA, 50 ms affair
   const double cand = job.mode == 0 ? (double)job.n : job.avg_candidates;
   int nsplit = (int)std::max(8.0, std::min(128.0, cand / 512.0));
   nsplit = (int)std::max<int64_t>(8, std::min<int64_t>(nsplit, (64LL << 20) / std::max<int64_t>(1, nq_max * k)));  // partial-result workspace
-  run_scan_impl(ix, job, nq_max, queries, k, out_dist, nullptr, out_ids, nullptr, qmap, qcount, nsplit, s);
+  run_scan_impl(ix, job, nq_max, queries, k, out_dist, out_raw, out_ids, out_counts, qmap, qcount, nsplit, s);
 }
 
 static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* out_dist,

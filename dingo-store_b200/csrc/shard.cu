@@ -152,6 +152,17 @@ static __global__ void unpack_parts_kernel(const TopkRec* __restrict__ parts, lo
   d[i] = r.dist; id[i] = r.id;
 }
 
+// merged range results: key (L2 distance | -ip) -> API distance (L2 distance | 1 - ip, as the single-index finish computes it);
+// counts[q] = merged rows of query q (the rows are ascending with -1 padding at the end)
+static __global__ void range_finish_kernel(float* dist, const long long* __restrict__ ids, long long nq, int k, int l2, int* counts) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nq * k) return;
+  const int j = (int)(i % k);
+  const bool hit = ids[i] >= 0;
+  if (hit && !l2) dist[i] = __fsub_rn(1.0f, -dist[i]);
+  if (hit ? (j == k - 1 || ids[i + 1] < 0) : j == 0) counts[i / k] = hit ? j + 1 : 0;
+}
+
 static __global__ void fill_ll_kernel(long long* p, long long n, long long v) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -288,9 +299,12 @@ SearchCtx make_ctx_shard(IndexBase* ix, const b200vs_search_params* sp, cudaStre
   return sc;
 }
 
-// the search proper: queries (all nq of them, raw) are on the device in `xq`; results land in out_* (device) on stream s
-void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
-                         float* out_dist, long long* out_ids, cudaStream_t s) {
+// The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
+// on stream s.  local(q, sc, nprobe) is step 2: it writes this rank's ascending, -1-padded [nq, k] (key, id) lists of the
+// prepared queries q over the gathered probe table L.probes into L.od / L.oi, the key being what the merge orders by.
+template <class LocalScan>
+void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
+                  float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local) {
   IndexBase* ix = sh->ix;
   const int W = sh->world, r = sh->rank, d = ix->dim;
   if (L.last && L.last != s && L.done) B200VS_CUDA(cudaStreamWaitEvent(s, L.done, 0));
@@ -308,10 +322,10 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
   ix->phase(IndexBase::PH_COMM, s);
   if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.probes.p, (size_t)per * nprobe, ncclInt64, L.comm, s));
   ix->phase(IndexBase::PH_OTHER, s);
-  // 2) tile scan of the probed lists this rank owns -> exact local top-k
+  // 2) scan of the probed lists this rank owns -> exact local results
   L.od.reserve((size_t)nq * k, 0, s);
   L.oi.reserve((size_t)nq * k, 0, s);
-  ix->search_probes_prepared_dev(nq, q, k, L.probes.p, nprobe, sc, L.od.p, L.oi.p, s);
+  local(q, sc, nprobe);
   // 3) ONE all-gather of the packed per-shard top-k + merge
   const long long nk = (long long)nq * k;
   L.parts.reserve((size_t)W * nk, 0, s);
@@ -334,6 +348,40 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
   if (!L.done) B200VS_CUDA(cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming));
   B200VS_CUDA(cudaEventRecord(L.done, s));
   L.last = s;
+}
+
+// top-k: the tile scan's exact local top-k, keyed on the API distance
+void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
+                         float* out_dist, long long* out_ids, cudaStream_t s) {
+  IndexBase* ix = sh->ix;
+  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
+    ix->search_probes_prepared_dev(nq, q, k, L.probes.p, nprobe, sc, L.od.p, L.oi.p, s);
+  });
+}
+
+// range: the local range scan keyed on the single-index select's key (L2 distance | -ip) — two distinct inner products can
+// round to the same 1 - ip, and an API-distance merge would then order them by id — then the API distance and the count of
+// every merged row.  The per-rank payload of the all-gather is nq * max_results * 16 bytes.
+void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, float radius, int max_results,
+                        const b200vs_search_params* sp, float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
+  IndexBase* ix = sh->ix;
+  const bool l2 = ix->metric == B200VS_L2;
+  shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
+    int* oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
+    ix->range_search_probes_prepared_dev(nq, q, radius, max_results, L.probes.p, nprobe, sc, L.od.p, L.oi.p, oc, s);
+    if (!l2) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
+  });
+  const long long n = (long long)nq * max_results;
+  range_finish_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(out_dist, out_ids, nq, max_results, l2 ? 1 : 0, out_counts);
+  B200VS_CUDA(cudaGetLastError());
+  ix->launch_count(1);
+}
+
+// refusals of a sharded range search, decided from its arguments alone so that every rank refuses before the first collective
+void check_shard_range(int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
+  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+  if (max_results <= 0 || max_results > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
+  if (!od || !oi || !oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
 }
 
 // Replicate rank `root`'s trained state on every rank (b200vs_shard_broadcast_state; the caller holds add_mu).
@@ -778,6 +826,67 @@ int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* x
       B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
       B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     }  // the lane is released before the host waits: the next batch of this lane may be enqueued behind this one
+    B200VS_CUDA(cudaStreamSynchronize(s));
+    return B200VS_OK;
+  });
+}
+
+int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, float radius, int32_t max_results,
+                                     const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, int32_t* out_counts_dev,
+                                     void* stream) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    IndexBase* ix = sh->ix;
+    SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
+    check_shard_range(nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    ix->set_device();
+    cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
+    LaneGuard lane(ix, s);
+    ix->check_probe_search(nq, max_results);  // before the first collective, alike on every rank
+    ix->reset_stats();
+    shard_range_stream(sh, *sl.lane, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
+    ix->phases_finish(s);
+    if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));
+    return B200VS_OK;
+  });
+}
+
+// Host-pointer variant: as b200vs_shard_search, each rank uploads only its slice of the batch.
+int b200vs_shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, float radius, int32_t max_results,
+                              const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    IndexBase* ix = sh->ix;
+    const int W = sh->world, r = sh->rank, d = ix->dim;
+    cudaStream_t s;
+    {
+      SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
+      check_shard_range(nq, xq, max_results, out_dist, out_ids, out_counts);
+      std::shared_lock<std::shared_mutex> rl(ix->rw);
+      ix->set_device();
+      b200vs_shard::SLane& L = *sl.lane;
+      s = L.own;
+      LaneGuard lane(ix, s);
+      ix->check_probe_search(nq, max_results);  // before the first collective, alike on every rank
+      ix->reset_stats();
+      const int64_t per = (nq + W - 1) / W;
+      L.q_all.reserve((size_t)per * W * d, 0, s);
+      const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
+      float* mine = L.q_all.p + (size_t)per * r * d;
+      if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, xq + (size_t)q0 * d, (size_t)(q1 - q0) * d * 4, cudaMemcpyHostToDevice, s));
+      if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * d, 0, (size_t)(per - (q1 - q0)) * d * 4, s));
+      if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * d, ncclFloat, L.comm, s));
+      const size_t nr = (size_t)nq * max_results;
+      float* dd = ix->scratch.alloc<float>(nr);
+      long long* di = ix->scratch.alloc<long long>(nr);
+      int* dc = ix->scratch.alloc<int>((size_t)nq);
+      shard_range_stream(sh, L, nq, L.q_all.p, radius, max_results, sp, dd, di, dc, s);
+      ix->phases_finish(s);
+      B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
+      B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
+      B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    }  // the lane is released before the host waits
     B200VS_CUDA(cudaStreamSynchronize(s));
     return B200VS_OK;
   });

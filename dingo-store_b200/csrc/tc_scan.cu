@@ -9,10 +9,12 @@
 //   tc_fill_pairs_kernel     gather the (rounded) queries of every list into one contiguous block
 //   tc_items_kernel          emit work items (list chunk x query group) + the list of sampled items
 //   tc_scan_kernel           *** the hot kernel: TMA -> smem ring -> wgmma (TF32 or FP16, register accumulators) -> epilogue ***
+//   tc_range_tau_kernel      range mode: per-query capture threshold from the radius, widened by tc_eps
 //   tc_tau_warp_kernel       per-query capture threshold from the sampled rows (warp radix select)
 //                            (tc_tau_kernel: the block form for queries with more sampled spans than a warp stages)
 //   tc_final_hybrid_kernel   per-query window select + exact FP32 (AVX-512 order) rerank + certification
-//                            (tc_final_kernel: the streaming form for windows or query rows that do not fit)
+//                            (tc_final_kernel: the streaming form for windows or query rows that do not fit; both
+//                            have a range form that re-scores every captured row and keeps the hits)
 //   tc_coarse_select_hybrid_kernel / tc_coarse_select_kernel
 //                            coarse-quantiser finish: register-resident radix select + exact rerank of the window
 //                            (tc_coarse_final_kernel: the streaming form for what they cannot finish)
@@ -798,34 +800,41 @@ __device__ __forceinline__ void cp_async_wait_all() {
   asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
-template <bool L2>
+// RANGE: as tc_final_kernel's; the window is every captured row, and a query whose capture overflowed is handed straight to
+// the exact scan (flags 2) without being re-scored.
+template <bool L2, bool RANGE>
 static __global__ void __launch_bounds__(HF_THREADS)
 tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
                        const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
                        const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int arith, int k,
-                       float* out_dist, long long* out_ids, int* flags, int* redo) {
+                       float* out_dist, long long* out_ids, int* flags, int* redo, uint32_t thr_key, int raw_out, int* out_counts) {
   extern __shared__ __align__(16) unsigned char s_dyn[];  // the query row (d % 4 == 0)
   __shared__ BlockSelShared S;
   __shared__ unsigned long long s_keys[HF_STAGE];
   __shared__ int s_rows[HF_MAXW];
   __shared__ uint32_t s_kd[HF_MAXW];
   __shared__ long long s_id[HF_MAXW];
-  __shared__ int s_m;
+  __shared__ int s_m, s_hits;
   const int lane = threadIdx.x & 31;
   const int qi = blockIdx.x;
   const int total = cand_cnt[qi];
+  if (RANGE && total > cap) {
+    if (threadIdx.x == 0) { flags[qi] = 2; redo[qi] = 0; }
+    return;
+  }
   const int n = min(total, cap);
   const unsigned long long* c = cand + (size_t)qi * cap;
   const int nst = min(n, HF_STAGE);
   for (int i = threadIdx.x; i < (d >> 2); i += HF_THREADS) cp_async16(s_dyn + (size_t)i * 16, q + (size_t)qi * d + i * 4);
   for (int i = threadIdx.x; i < nst; i += HF_THREADS) s_keys[i] = c[i];
-  if (threadIdx.x == 0) s_m = 0;
+  if (threadIdx.x == 0) { s_m = 0; if (RANGE) s_hits = 0; }
   __syncthreads();
   auto key_at = [&](int i) -> unsigned long long { return i < nst ? s_keys[i] : c[i]; };
   float a_k = TC_INF;
-  if (n >= k) a_k = ord2f(block_kth_key_any(k, S, [&](auto f) { for (int i = threadIdx.x; i < n; i += HF_THREADS) f((uint32_t)(key_at(i) >> 32)); }));
+  if (!RANGE && n >= k) a_k = ord2f(block_kth_key_any(k, S, [&](auto f) { for (int i = threadIdx.x; i < n; i += HF_THREADS) f((uint32_t)(key_at(i) >> 32)); }));
   const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith);
-  if (!(two_eps < TC_INF)) {  // outside the range eps covers (the scores may be inf or NaN): the exact scan re-runs it
+  // outside the range eps covers (the scores may be inf or NaN; range: a threshold that is not finite): the exact scan re-runs it
+  if (RANGE ? !(fabsf(tau[qi]) < TC_INF) : !(two_eps < TC_INF)) {
     cp_async_wait_all();      // the query row
     if (threadIdx.x == 0) { flags[qi] = 1; redo[qi] = 0; }
     return;
@@ -836,7 +845,7 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
       const int i = base + threadIdx.x;
       unsigned long long e = 0;
       bool in = false;
-      if (i < n) { e = key_at(i); in = ord2f((uint32_t)(e >> 32)) <= window; }
+      if (i < n) { e = key_at(i); in = RANGE || ord2f((uint32_t)(e >> 32)) <= window; }
       const unsigned msk = __ballot_sync(0xffffffffu, in);
       int wbase = 0;
       if (lane == 0 && msk) wbase = atomicAdd(&s_m, __popc(msk));
@@ -860,19 +869,32 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
   __syncthreads();
   tc_rescore_window<L2, HF_THREADS / 4>(s_rows, m, vecs, qs, d, true, [&](long long row) { return ids[row]; }, s_kd, s_id);
   __syncthreads();
+  int kept = k;
+  if constexpr (RANGE) {  // rows outside the range become sentinels, which rank after every hit
+    int h = 0;
+    for (int i = threadIdx.x; i < m; i += HF_THREADS) {
+      if (s_kd[i] < thr_key) ++h;
+      else { s_kd[i] = KEY_SENTINEL_D; s_id[i] = KEY_SENTINEL_ID; }
+    }
+    h = __reduce_add_sync(0xffffffffu, h);
+    if (lane == 0 && h) atomicAdd(&s_hits, h);
+    __syncthreads();
+    kept = min(s_hits, k);
+  }
   block_rank_sort(s_kd, s_id, m, [&](int rank, int e) {
-    if (rank < k) {
+    if (rank < kept) {
       const float v = ord2f(s_kd[e]);
       const float raw = L2 ? v : -v;
-      out_dist[(size_t)qi * k + rank] = L2 ? raw : __fsub_rn(1.0f, raw);
+      out_dist[(size_t)qi * k + rank] = (L2 || (RANGE && raw_out)) ? raw : __fsub_rn(1.0f, raw);
       out_ids[(size_t)qi * k + rank] = s_id[e];
     }
   });
-  for (int i = min(m, k) + threadIdx.x; i < k; i += HF_THREADS) { out_dist[(size_t)qi * k + i] = 0.f; out_ids[(size_t)qi * k + i] = -1; }
+  for (int i = min(m, kept) + threadIdx.x; i < k; i += HF_THREADS) { out_dist[(size_t)qi * k + i] = 0.f; out_ids[(size_t)qi * k + i] = -1; }
   if (threadIdx.x == 0) {
     const float tq = tau[qi];
-    flags[qi] = (total <= cap ? 0 : 2) | ((tq == TC_INF || a_k + two_eps <= tq) ? 0 : 1);  // 1: threshold too tight, 2: capture overflow
+    flags[qi] = (total <= cap ? 0 : 2) | ((RANGE || tq == TC_INF || a_k + two_eps <= tq) ? 0 : 1);  // 1: threshold too tight, 2: capture overflow
     redo[qi] = 0;
+    if (RANGE) out_counts[qi] = kept;
   }
 }
 
@@ -1030,39 +1052,47 @@ tc_coarse_select_hybrid_kernel(const float* __restrict__ dense, long long ld, in
 // smallest approximate score (+inf when n < k).  Pass 2: every row with score <= A_k + two_eps re-scored exactly in the
 // reference order, FIN_SEG rows at a time, into `sel`, which ends holding the exact top-k by (distance, id).
 // smem: tc_stream_smem(d, pool_cap) bytes.  Returns A_k + two_eps (NaN when two_eps = +inf: then pass 2 takes every row).
-// All SCAN_THREADS threads call.
+// RANGE: no pass 1; every row is re-scored and `sel` keeps the closest k whose exact key is below thr_key (the exact scan's
+// range rule: its select starts from the threshold (thr_key, INT64_MIN)).  All SCAN_THREADS threads call.
 static size_t tc_stream_smem(int d, int pool_cap) { return ((size_t)d * 4 + 15) / 16 * 16 + (size_t)FIN_SEG * 4 + BlockSelect::smem_bytes(pool_cap); }
 
-template <bool L2, class KeyAt, class IdOf>
+template <bool L2, bool RANGE = false, class KeyAt, class IdOf>
 __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned char* smem, int pool_cap, const float* __restrict__ qrow,
                                                   const float* __restrict__ vecs, int d, int n, int k, float two_eps, KeyAt key_at,
-                                                  IdOf id_of) {
+                                                  IdOf id_of, uint32_t thr_key = 0) {
   __shared__ int s_m;
   float* qs = reinterpret_cast<float*>(smem);
   const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
   int* s_rows = reinterpret_cast<int*>(smem + qbytes);  // [FIN_SEG]
   unsigned char* pool = smem + qbytes + (size_t)FIN_SEG * 4;
   for (int i = threadIdx.x; i < d; i += blockDim.x) qs[i] = qrow[i];
-  sel.init(pool, pool_cap, k);
-  // pass 1: k-th smallest approximate score
-  for (int base = 0; base < n; base += blockDim.x) {
-    sel.maybe_prune(blockDim.x);
-    const int i = base + threadIdx.x;
-    if (i < n) {
-      const unsigned long long e = key_at(i);
-      const uint32_t key = (uint32_t)(e >> 32);
-      const long long row = (long long)(e & 0xffffffffull);
-      if (sel.passes(key, row)) sel.push(key, row);
+  uint32_t wkey = 0xFFFFFFFFu;
+  if constexpr (!RANGE) {
+    sel.init(pool, pool_cap, k);
+    // pass 1: k-th smallest approximate score
+    for (int base = 0; base < n; base += blockDim.x) {
+      sel.maybe_prune(blockDim.x);
+      const int i = base + threadIdx.x;
+      if (i < n) {
+        const unsigned long long e = key_at(i);
+        const uint32_t key = (uint32_t)(e >> 32);
+        const long long row = (long long)(e & 0xffffffffull);
+        if (sel.passes(key, row)) sel.push(key, row);
+      }
     }
+    sel.prune();
+    const float a_k = *sel.count >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
+    __syncthreads();
+    // window = A_k + two_eps (+inf when fewer than k rows) as a key; eps = +inf (outside the range it bounds): every row,
+    // NaN scores included (a NaN fails every float comparison, but its key 0xFFFFFFFF is the largest)
+    wkey = two_eps < TC_INF ? f2ord(a_k + two_eps) : 0xFFFFFFFFu;
   }
-  sel.prune();
-  const float a_k = *sel.count >= k ? ord2f(sel.kd[k - 1]) : TC_INF;
-  __syncthreads();
-  // window = A_k + two_eps (+inf when fewer than k rows) as a key; eps = +inf (outside the range it bounds): every row,
-  // NaN scores included (a NaN fails every float comparison, but its key 0xFFFFFFFF is the largest)
-  const uint32_t wkey = two_eps < TC_INF ? f2ord(a_k + two_eps) : 0xFFFFFFFFu;
   // pass 2: exact distances (reference AVX-512 order) of every row inside the window
   sel.init(pool, pool_cap, k);
+  if constexpr (RANGE) {
+    if (threadIdx.x == 0) { *sel.thr_d = thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
+    __syncthreads();
+  }
   const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
   const bool vec = (d & 3) == 0;
   for (int seg = 0; seg < n; seg += FIN_SEG) {
@@ -1093,24 +1123,28 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
   return ord2f(wkey);
 }
 
-template <bool L2>
+// RANGE (tc_range_search): tau holds the range capture threshold, not a sampled one; every captured row is re-scored and
+// the closest k rows whose exact key is below thr_key are kept, as the exact scan keeps them.  out_dist then holds the raw
+// metric value (L2 distance | ip) when raw_out, else the API distance, and out_counts the rows kept.
+template <bool L2, bool RANGE>
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
                 const float* __restrict__ tau, const float* __restrict__ qnorm, float max_norm, const float* __restrict__ q,
                 const float* __restrict__ vecs, const long long* __restrict__ ids, int d, int arith, int k, int pool_cap,
-                float* out_dist, long long* out_ids, int* flags, const int* redo) {
+                float* out_dist, long long* out_ids, int* flags, const int* redo, uint32_t thr_key, int raw_out, int* out_counts) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int qi = blockIdx.x;
   if (redo && !redo[qi]) return;  // finished by the hybrid kernel
   const float two_eps = 2.f * tc_eps(L2, qnorm[qi], max_norm, d, arith);
-  if (!(two_eps < TC_INF)) { if (threadIdx.x == 0) flags[qi] = 1; return; }  // the exact scan re-runs it
+  // outside the range eps covers (range: a threshold that is not finite): the exact scan re-runs it
+  if (RANGE ? !(fabsf(tau[qi]) < TC_INF) : !(two_eps < TC_INF)) { if (threadIdx.x == 0) flags[qi] = 1; return; }
   const int total = cand_cnt[qi];
   const unsigned long long* c = cand + (size_t)qi * cap;
   BlockSelect sel;
-  const float window = tc_stream_window<L2>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k, two_eps,
-                                            [&](int i) { return c[i]; }, [&](uint32_t row) { return ids[row]; });
+  const float window = tc_stream_window<L2, RANGE>(sel, smem, pool_cap, q + (size_t)qi * d, vecs, d, min(total, cap), k, two_eps,
+                                                   [&](int i) { return c[i]; }, [&](uint32_t row) { return ids[row]; }, thr_key);
   const float tq = tau[qi];
-  const bool certified = (total <= cap) && (tq == TC_INF || window <= tq);
+  const bool certified = (total <= cap) && (RANGE || tq == TC_INF || window <= tq);
   const int have = *sel.count;
   for (int i = threadIdx.x; i < k; i += blockDim.x) {
     float api = 0.f;
@@ -1118,13 +1152,16 @@ tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restri
     if (i < have) {
       const float v = ord2f(sel.kd[i]);
       const float raw = L2 ? v : -v;
-      api = L2 ? raw : __fsub_rn(1.0f, raw);
+      api = (L2 || (RANGE && raw_out)) ? raw : __fsub_rn(1.0f, raw);
       id = sel.kid[i];
     }
     out_dist[(size_t)qi * k + i] = api;
     out_ids[(size_t)qi * k + i] = id;
   }
-  if (threadIdx.x == 0) flags[qi] = certified ? 0 : 1;
+  if (threadIdx.x == 0) {
+    flags[qi] = certified ? 0 : 1;
+    if (RANGE) out_counts[qi] = have;
+  }
 }
 
 // coarse quantiser: every approximate score is available (dense row), so the window select is always certified
@@ -1290,12 +1327,16 @@ static TcDevice tc_init(int device) {
   B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<false>::SMEM));
   dev.sample_ctas[0] = tc_sample_ctas_per_sm<false>();
   dev.sample_ctas[1] = tc_sample_ctas_per_sm<true>();
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_coarse_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_final_hybrid_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   g_tc_dev[device] = dev;  // only after every attribute call succeeded
   return dev;
 }
@@ -1424,6 +1465,33 @@ static void tc_launch(const TcDevice& dev, bool half, int64_t work_bound, const 
   B200VS_CUDA(cudaGetLastError());
 }
 
+// The exact scan over what a tile search covers (the probed lists, or the single list of a Flat view): the re-run of the
+// queries the tile passes could not finish.
+static ScanJob tc_exact_job(const TcView& v, bool l2, int d, const long long* probes, int nprobe, const SearchCtx& sc) {
+  ScanJob job;
+  job.l2 = l2; job.vecs = v.vecs; job.ids = v.ids; job.d = d; job.sc = &sc;
+  if (!v.flat) {
+    job.mode = 1; job.probes = probes; job.nprobe = nprobe; job.list_off = v.list_off; job.list_len = v.list_len;
+    job.avg_candidates = v.nlist > 0 ? (double)v.arena_rows * nprobe / v.nlist : 0;
+  }
+  else { job.mode = 0; job.n = v.arena_rows; }
+  return job;
+}
+
+// profiling counters of a tile search: [2] queries re-run on the exact scan, [6] work items of the capture pass,
+// [7] the sum over items of (128-row tiles x padded query columns)
+static void tc_profile_counts(IndexBase* ix, const int* qcount, const int* totals, cudaStream_t s) {
+  int h = 0;
+  B200VS_CUDA(cudaMemcpyAsync(&h, qcount, 4, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  ix->stats[2] = h;
+  int t[4] = {0, 0, 0, 0};
+  B200VS_CUDA(cudaMemcpyAsync(t, totals, 16, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  ix->stats[6] = t[0];
+  ix->stats[7] = t[3];
+}
+
 void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
                int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
   const int d = ix->dim;
@@ -1470,28 +1538,21 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   const int* fin_redo = nullptr;
   const size_t hsm = (size_t)d * 4;  // the query row
   if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
-    else tc_final_hybrid_kernel<false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo);
+    if (l2) tc_final_hybrid_kernel<true, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, 0, nullptr);
+    else tc_final_hybrid_kernel<false, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, 0, nullptr);
     fin_redo = redo;
     ix->launch_count(1);
   }
   const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
-  else tc_final_kernel<false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo);
+  if (l2) tc_final_kernel<true, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, 0, nullptr);
+  else tc_final_kernel<false, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, 0, nullptr);
   tc_compact_flags(flags, (int)nq, qmap, qcount, s);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
   ix->stats[1] = nq;
   // 4) uncertified queries re-run on the exact scan (device-side count: blocks beyond it exit immediately)
-  ScanJob job;
-  job.l2 = l2; job.vecs = v.vecs; job.ids = v.ids; job.d = d; job.sc = &sc;
-  if (!v.flat) {
-    job.mode = 1; job.probes = probes; job.nprobe = nprobe; job.list_off = v.list_off; job.list_len = v.list_len;
-    job.avg_candidates = v.nlist > 0 ? (double)v.arena_rows * nprobe / v.nlist : 0;
-  }
-  else { job.mode = 0; job.n = v.arena_rows; }
   ix->phase(IndexBase::PH_FALLBACK, s);
-  run_scan_mapped(ix, job, nq, qmap, qcount, q, k, out_dist, out_ids, s);
+  run_scan_mapped(ix, tc_exact_job(v, l2, d, probes, nprobe, sc), nq, qmap, qcount, q, k, out_dist, nullptr, out_ids, nullptr, s);
   ix->phase(IndexBase::PH_OTHER, s);
   if (ix->profiling && getenv("B200VS_DEBUG_FLAGS")) {
     std::vector<int> hf(nq), hc(nq);
@@ -1505,17 +1566,105 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
     fprintf(stderr, "[b200vs] tc_search nq=%lld cap=%d captured avg=%.1f max=%d flagged: threshold=%d overflow=%d tau_inf=%d\n", (long long)nq, cap, (double)tot / nq, mx, r1, r2, ninf);
     for (int64_t i = 0, shown = 0; i < nq && shown < 4; ++i) if (hf[i]) { fprintf(stderr, "[b200vs]   q=%lld flag=%d captured=%d tau=%g\n", (long long)i, hf[i], hc[i], ht[i]); ++shown; }
   }
-  if (ix->profiling) {
-    int h = 0;
-    B200VS_CUDA(cudaMemcpyAsync(&h, qcount, 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    ix->stats[2] = h;
-    int t[4] = {0, 0, 0, 0};
-    B200VS_CUDA(cudaMemcpyAsync(t, P.totals, 16, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    ix->stats[6] = t[0];  // work items of the capture pass
-    ix->stats[7] = t[3];  // sum over items of (128-row tiles x padded query columns)
+  if (ix->profiling) tc_profile_counts(ix, qcount, P.totals, s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// range mode of the list scan: the capture threshold comes from the radius (DESIGN.md 4.6)
+// ---------------------------------------------------------------------------------------------
+// tau[q] = a bound on the tile score s~ of every row whose exact FP32 value passes the range test, rounded outwards:
+//   L2: hit => D_fp32 <= thr, and |s~ - (D_fp32 - ||q||^2)| <= eps (tc_eps, which covers the exact kernel's own rounding)
+//       with ||q||^2 the real norm, of which only the FP32 sum qnorm is known: ||q||^2 >= qnorm - (d + 64) 2^-24 qnorm -
+//       d 2^-149, so s~ <= thr - (that) + eps;
+//   IP / cosine: hit => -ip_fp32 <= -thr and |s~ + ip_fp32| <= eps, so s~ <= -thr + eps.
+// NaN when eps or the threshold is not finite: the finish kernels hand such a query to the exact scan.
+static __global__ void tc_range_tau_kernel(const float* __restrict__ qnorm, long long nq, int l2, float thr, float max_norm, int d,
+                                           int arith, float* __restrict__ tau) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nq) return;
+  const float eps = tc_eps(l2 != 0, qnorm[i], max_norm, d, arith);
+  float t;
+  if (l2) {
+    const float qerr = __fmaf_ru((float)(d + 64) * 5.9604645e-8f /*2^-24*/, qnorm[i], (float)d * 0x1p-149f);
+    t = __fadd_ru(__fsub_ru(thr, __fsub_rd(qnorm[i], qerr)), eps);
+  } else {
+    t = __fadd_ru(-thr, eps);
   }
+  tau[i] = (eps < TC_INF && fabsf(t) < TC_INF) ? t : __int_as_float(0x7fffffff);
+}
+
+bool tc_range_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int max_results, int nprobe, const SearchCtx& sc) {
+  if (sc.exact_only) return false;
+  if (ix->dim % 4 != 0 || ix->dim < 32) return false;
+  if (nq < 16 || max_results > 4096) return false;  // tiny batches: exact scan; 4096 = the select's limit
+  if (tc_stream_smem(ix->dim, select_pool_cap(max_results, SCAN_THREADS)) > 160 * 1024) return false;  // streaming finish
+  if (!v.norms || !v.vecs) return false;
+  if (!tc_norms_in_range(ix->metric == B200VS_L2, v.max_norm)) return false;
+  return tc_plan_fits(v, nq, nprobe);
+}
+
+void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, float radius_raw, int max_results,
+                     const long long* probes, int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, int* out_counts,
+                     bool raw_out, cudaStream_t s) {
+  const int d = ix->dim;
+  const int k = max_results;
+  const int cap = tc_cand_cap(k);
+  auto& S = ix->scratch;
+  ix->phase(IndexBase::PH_PLAN, s);
+  TcPlan P = tc_prepare(ix, v, nq, q, probes, nprobe, s);
+  float* tau = S.alloc<float>(nq);
+  unsigned long long* cand = S.alloc<unsigned long long>((size_t)nq * cap);
+  int* cand_cnt = S.alloc<int>(nq);
+  int* flags = S.alloc<int>(nq);
+  int* redo = S.alloc<int>(nq);
+  int* qmap = S.alloc<int>(nq);
+  int* qcount = S.alloc<int>(1);
+  B200VS_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)nq * 4, s));
+  const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
+  // 1) capture thresholds from the radius (no sample pass)
+  ix->phase(IndexBase::PH_TAU, s);
+  tc_range_tau_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(P.qry.norm, nq, l2 ? 1 : 0, radius_raw, v.max_norm, d, arith, tau);
+  // 2) capture pass: every probed list chunk once, rows under the threshold
+  TcParams p = tc_params(v, d, l2, P.items, P.totals, v.hscale, P.qry.scale);
+  p.pair_query = P.pair_query;
+  p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
+  p.filt.has_range = sc.has_range; p.filt.negate = sc.negate; p.filt.rmin = sc.rmin; p.filt.rmax = sc.rmax;
+  p.filt.sorted_ids = sc.sorted_ids_dev; p.filt.n_ids = sc.n_ids;
+  p.mode = 1; p.work_counter = P.work + 1;
+  ix->phase(IndexBase::PH_CAPTURE, s);
+  {
+    ScopedKernelTimer timer(ix, s, ix->profiling);
+    tc_launch(P.dev, P.half, P.bound, P.maps, p, s);
+    timer.stop();
+  }
+  // 3) exact re-score of every captured row, range test, closest max_results
+  ix->phase(IndexBase::PH_FINAL, s);
+  const uint32_t thr_key = f2ord(l2 ? radius_raw : -radius_raw);
+  const int raw = raw_out ? 1 : 0;
+  const int* fin_redo = nullptr;
+  const size_t hsm = (size_t)d * 4;
+  if (hsm <= 96 * 1024) {
+    if (l2) tc_final_hybrid_kernel<true, true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, thr_key, raw, out_counts);
+    else tc_final_hybrid_kernel<false, true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, thr_key, raw, out_counts);
+    fin_redo = redo;
+    ix->launch_count(1);
+  }
+  const int pool = select_pool_cap(k, SCAN_THREADS);
+  const size_t fin_smem = tc_stream_smem(d, pool);
+  if (l2) tc_final_kernel<true, true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, thr_key, raw, out_counts);
+  else tc_final_kernel<false, true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, thr_key, raw, out_counts);
+  tc_compact_flags(flags, (int)nq, qmap, qcount, s);
+  B200VS_CUDA(cudaGetLastError());
+  ix->launch_count(4);
+  ix->stats[1] = nq;
+  // 4) overflowed (and out-of-range) queries re-run on the exact scan's range job
+  ScanJob job = tc_exact_job(v, l2, d, probes, nprobe, sc);
+  job.has_thr = true;
+  job.thr_raw = radius_raw;
+  ix->phase(IndexBase::PH_FALLBACK, s);
+  run_scan_mapped(ix, job, nq, qmap, qcount, q, k, raw_out ? nullptr : out_dist, raw_out ? out_dist : nullptr, out_ids, out_counts, s);
+  ix->phase(IndexBase::PH_OTHER, s);
+  if (ix->profiling) tc_profile_counts(ix, qcount, P.totals, s);
 }
 
 bool tc_coarse_eligible(const IndexBase* ix, int64_t nq, int nrows, int nprobe) {

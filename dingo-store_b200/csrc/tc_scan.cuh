@@ -118,12 +118,22 @@ int tc_cand_cap(int k);  // captured rows kept per query
 void tc_compact_flags(const int* flags, int nq, int* qmap, int* count, cudaStream_t s);
 // exact re-run of the queries in qmap[0, *qcount) (kernels.cu)
 void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const int* qmap, const int* qcount, const float* queries,
-                     int k, float* out_dist, long long* out_ids, cudaStream_t s);
+                     int k, float* out_dist, float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s);
 
 // probes: device [nq, nprobe] list indices (for Flat: all zeros, nprobe = 1).  q: device queries, already
 // normalised for cosine.  Writes API-semantics results; uncertified queries are re-run on the exact scan.
 void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
                int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s);
+
+// Range mode of the list scan (radius_raw: L2 keeps dist < radius_raw, IP / cosine keep ip > radius_raw).  The capture
+// threshold of each query comes from the radius widened by tc_eps; every captured row is re-scored exactly and the closest
+// max_results hits are kept by (distance, id), as the exact scan with the same threshold keeps them.  Queries whose capture
+// overflows re-run on the exact scan.  out_dist: API distances, or the raw metric value (L2 distance | ip) when raw_out;
+// out_counts: rows kept per query.  tc_range_eligible: tc_eligible's conditions without k <= 128, max_results <= 4096.
+bool tc_range_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int max_results, int nprobe, const SearchCtx& sc);
+void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, float radius_raw, int max_results,
+                     const long long* probes, int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, int* out_counts,
+                     bool raw_out, cudaStream_t s);
 
 // Exact top-nprobe of every query against a small row set (the IVF coarse quantiser): dense TF32 score matrix on the
 // tensor cores, then window select + exact FP32 re-score.  Always certified (every score is available).

@@ -29,7 +29,8 @@ ABI_SYMBOLS = [
     "b200vs_add_with_ids_device", "b200vs_assign_device", "b200vs_reserve_lists", "b200vs_export_list", "b200vs_set_coalescing", "b200vs_reconstruct", "b200vs_sub_type",
     "b200vs_shard_unique_id", "b200vs_shard_create", "b200vs_shard_destroy", "b200vs_shard_list_range", "b200vs_shard_train",
     "b200vs_shard_broadcast_state", "b200vs_shard_add", "b200vs_shard_add_device", "b200vs_shard_remove_ids", "b200vs_shard_plan_add_device",
-    "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_debug_tc_scores",
+    "b200vs_shard_plan_commit", "b200vs_shard_search", "b200vs_shard_search_device", "b200vs_shard_range_search",
+    "b200vs_shard_range_search_device", "b200vs_debug_tc_scores",
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
@@ -130,6 +131,8 @@ def lib():
     L.b200vs_shard_plan_commit.argtypes = [vp]
     L.b200vs_shard_search.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_shard_search_device.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_shard_range_search.argtypes = [vp, i64, i64, vp, ctypes.c_float, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_shard_range_search_device.argtypes = [vp, i64, i64, vp, ctypes.c_float, i32, ctypes.POINTER(SearchParams), vp, vp, vp, vp]
     L.b200vs_debug_tc_scores.argtypes = [vp, i64, vp, i32, vp, vp]
     L.b200vs_train_binary.argtypes = [vp, i64, vp]
     L.b200vs_add_with_ids_binary.argtypes = [vp, i64, vp, vp, ctypes.c_int]
@@ -485,6 +488,24 @@ class Shard:
     def search_device(self, nq, xq_dev_ptr, k, out_dist_dev_ptr, out_ids_dev_ptr, stream=None, sp=None, seq=-1):
         _check(lib().b200vs_shard_search_device(self.h, seq, nq, xq_dev_ptr, k, ctypes.byref(sp) if sp is not None else None,
                                                 out_dist_dev_ptr, out_ids_dev_ptr, stream))
+
+    def range_search(self, xq, radius, max_results=1024, seq=-1, **kw):
+        """b200vs_shard_range_search: every rank passes the same batch; returns (distances, ids, counts) of the whole index."""
+        xq = _f32(xq)
+        nq = xq.shape[0]
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(max_results, 0)), dtype=np.float32)
+        I = np.full((nq, max(max_results, 0)), -1, dtype=np.int64)
+        C = np.zeros(nq, dtype=np.int32)
+        _check(lib().b200vs_shard_range_search(self.h, seq, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
+                                               ctypes.byref(sp), D.ctypes.data, I.ctypes.data, C.ctypes.data))
+        return D, I, C
+
+    def range_search_device(self, nq, xq_dev_ptr, radius, max_results, out_dist_dev_ptr, out_ids_dev_ptr, out_counts_dev_ptr,
+                            stream=None, sp=None, seq=-1):
+        _check(lib().b200vs_shard_range_search_device(self.h, seq, nq, xq_dev_ptr, float(radius), max_results,
+                                                      ctypes.byref(sp) if sp is not None else None, out_dist_dev_ptr,
+                                                      out_ids_dev_ptr, out_counts_dev_ptr, stream))
 
 
 def ivf_state_blob(centroids, metric):

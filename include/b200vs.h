@@ -143,7 +143,8 @@ int b200vs_search_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int
 
 /* VectorIndex::RangeSearch — flat.cc:267-323, ivf_flat.cc:278-368 (HNSW: EVECTOR_NOT_SUPPORT, hnsw.cc:487-493).
  * radius in API semantics (mapped 1-r for IP/COSINE, flat.cc:282-285).  At most max_results hits per
- * query are kept (closest first); out_counts[nq] receives the per-query hit count. */
+ * query are kept (closest first); out_counts[nq] receives the per-query hit count.  Flat / IVF-Flat batches of >= 16
+ * queries run on the tile scan's range mode; the results (ids, distances, counts) are those of exact_only. */
 int b200vs_range_search(b200vs_index* idx, int64_t nq, const float* xq, float radius, int32_t max_results,
                         const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
 
@@ -263,6 +264,18 @@ int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const floa
                         float* out_dist, int64_t* out_ids);
 int b200vs_shard_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, int32_t k,
                                const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
+/* shard_range_search[_device]: b200vs_range_search over the sharded index, in shard_search's flow (same sequence numbers,
+ * lanes and communicators: range and top-k batches may be interleaved).  Step 2 is the range scan of the owned probed lists
+ * (IVF_FLAT: the tile range scan; IVF_PQ: the thresholded LUT scan); the all-gathered payload is nq * max_results * 16 bytes
+ * per rank; the merge orders hits as the single-index select does (L2 distance | -ip, then id).  Results (distances, ids and
+ * counts) equal b200vs_range_search on the unsharded index.  Refused on every rank before the first collective: max_results
+ * outside [1, 4096], null outputs, and (IVF_PQ) a LUT + select pool larger than one SM's shared memory; a refused call still
+ * uses up its sequence number. */
+int b200vs_shard_range_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, float radius, int32_t max_results,
+                              const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
+int b200vs_shard_range_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, float radius,
+                                     int32_t max_results, const b200vs_search_params* sp, float* out_dist_dev,
+                                     int64_t* out_ids_dev, int32_t* out_counts_dev, void* stream);
 
 /* Device-pointer write path of a single index (IVF_FLAT, IVF_PQ in its IVF-PQ mode): rows and ids already on the index's
  * device.  lists_dev (nullable) = the inverted list of every row when the caller has already assigned them
