@@ -2,6 +2,8 @@
 // No exception leaves this file: every entry point maps failures to a b200vs_status
 // (reference convention: butil::Status codes, never exceptions across the plugin virtual;
 // src/vector/vector_index_flat.cc:313-315, src/handler/raft_apply_handler.cc:1311-1325).
+#include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <memory>
 #include <new>
@@ -447,6 +449,12 @@ int b200vs_range_search(b200vs_index* h, int64_t nq, const float* xq, float radi
     LaneGuard lane(ix, nullptr);
     cudaStream_t s = lane.stream;
     ix->reset_stats();
+    if (std::isnan(radius)) {  // dis < NaN and ip > 1 - NaN hold for no row: empty results, nothing launched (DESIGN.md 4.6)
+      std::fill_n(out_dist, (size_t)nq * max_results, 0.0F);
+      std::fill_n(out_ids, (size_t)nq * max_results, (int64_t)-1);
+      std::fill_n(out_counts, (size_t)nq, 0);
+      return B200VS_OK;
+    }
     float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
     float* dd = ix->scratch.alloc<float>((size_t)nq * max_results);
     long long* di = ix->scratch.alloc<long long>((size_t)nq * max_results);
@@ -714,6 +722,7 @@ struct b200vs_scan_range {
   int64_t nq = 0;
   int max_results = 0;
   bool l2 = true, cosine = false;
+  bool no_hits = false;  // a NaN radius: no row is a hit, so pushes launch nothing
   float thr_raw = 0;  // L2: dist < radius; IP / cosine: ip > 1 - radius (vector_index_flat.cc:282-285)
   SearchCtx sc;       // sc.sorted_ids_dev points into allow
   cudaStream_t s = nullptr;
@@ -743,6 +752,7 @@ int b200vs_scan_range_begin(int32_t device, b200vs_metric metric, int32_t dim, i
     st->l2 = metric == B200VS_L2;
     st->cosine = metric == B200VS_COSINE;
     st->thr_raw = st->l2 ? radius : 1.0F - radius;
+    st->no_hits = std::isnan(radius);
     B200VS_CUDA(cudaSetDevice(device));
     B200VS_CUDA(cudaStreamCreateWithFlags(&st->s, cudaStreamNonBlocking));
     const size_t nr = (size_t)nq * max_results;
@@ -774,6 +784,7 @@ int b200vs_scan_range_push(b200vs_scan_range* st, int64_t n, const float* x, con
     if (n <= 0) return B200VS_OK;
     if (!x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "null tile");
     check_batch_ids_unique(n, ids);  // the Flat add of the reference's per-tile index refuses a repeated id
+    if (st->no_hits) return B200VS_OK;
     B200VS_CUDA(cudaSetDevice(st->device));
     st->x.reserve((size_t)n * st->dim, 0, st->s);
     st->ids.reserve((size_t)n, 0, st->s);

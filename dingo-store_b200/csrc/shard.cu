@@ -18,11 +18,13 @@
 #include <dlfcn.h>
 #include <nccl.h>
 
+#include <cmath>
 #include <condition_variable>
 #include <memory>
 #include <vector>
 
 #include "index.h"
+#include "ivf_common.h"
 
 namespace b200vs {
 
@@ -368,7 +370,9 @@ void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, co
   const bool l2 = ix->metric == B200VS_L2;
   shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
     int* oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
-    ix->range_search_probes_prepared_dev(nq, q, radius, max_results, L.probes.p, nprobe, sc, L.od.p, L.oi.p, oc, s);
+    // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
+    if (std::isnan(radius)) fill_empty_range(nq, max_results, L.od.p, L.oi.p, oc, s);
+    else ix->range_search_probes_prepared_dev(nq, q, radius, max_results, L.probes.p, nprobe, sc, L.od.p, L.oi.p, oc, s);
     if (!l2) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
   });
   const long long n = (long long)nq * max_results;

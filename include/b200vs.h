@@ -144,7 +144,8 @@ int b200vs_search_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int
 /* VectorIndex::RangeSearch — flat.cc:267-323, ivf_flat.cc:278-368 (HNSW: EVECTOR_NOT_SUPPORT, hnsw.cc:487-493).
  * radius in API semantics (mapped 1-r for IP/COSINE, flat.cc:282-285).  At most max_results hits per
  * query are kept (closest first); out_counts[nq] receives the per-query hit count.  Flat / IVF-Flat batches of >= 16
- * queries run on the tile scan's range mode; the results (ids, distances, counts) are those of exact_only. */
+ * queries run on the tile scan's range mode; the results (ids, distances, counts) are those of exact_only.  A NaN radius
+ * (either sign) admits no row: every count 0, ids -1, distances 0, and nothing is launched. */
 int b200vs_range_search(b200vs_index* idx, int64_t nq, const float* xq, float radius, int32_t max_results,
                         const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
 
@@ -270,7 +271,8 @@ int b200vs_shard_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, con
  * per rank; the merge orders hits as the single-index select does (L2 distance | -ip, then id).  Results (distances, ids and
  * counts) equal b200vs_range_search on the unsharded index.  Refused on every rank before the first collective: max_results
  * outside [1, 4096], null outputs, and (IVF_PQ) a LUT + select pool larger than one SM's shared memory; a refused call still
- * uses up its sequence number. */
+ * uses up its sequence number.  A NaN radius is not refused: every rank contributes no hits and the call returns empty
+ * results, as b200vs_range_search does. */
 int b200vs_shard_range_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, float radius, int32_t max_results,
                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
 int b200vs_shard_range_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, float radius,
@@ -333,7 +335,7 @@ void b200vs_scan_abort(b200vs_scan* scan);
  * All pointers are host pointers.
  *   scan_range_begin : argument checks and statuses of b200vs_scan_begin, then max_results <= 0 -> EILLEGAL_PARAMETERS; the
  *                      queries and filters (id range, sorted id list, negate) are copied; a failed allocation returns
- *                      EINTERNAL and no handle;
+ *                      EINTERNAL and no handle; a NaN radius (either sign) admits no row, so its pushes add nothing;
  *   scan_range_push  : one tile (n <= 0: no-op); a repeated id inside the tile -> EVECTOR_ID_DUPLICATED, the tile adds
  *                      nothing and the handle stays usable; returns when the tile has been scanned;
  *   scan_range_finish: out_counts[nq] = hits kept; out_dist / out_ids [nq, max_results] hold them in scan order in slots
