@@ -7,6 +7,10 @@
   cfg3s cfg3 through the list-sharded deployment b200vs_shard_* (world 1 on one GPU, beside the plain search at the same
         shape; under torchrun over the box's GPUs, n / world rows per GPU)                    (--pq-n, --pq-nbits, --pq-m)
   cfg4  HNSW cosine, 1M x 768, M = 16, efConstruction 200, efSearch 128, batch 512          (--hnsw-n; concurrent host build)
+  1s    Flat L2, 2M x 768, batch 1024, top-10, through the row-sharded deployment b200vs_shard_* at world 1, beside the plain
+        search on the same index (ids and distance bits compared)
+  4s    cfg4's HNSW cosine (1M x 768, M = 16, efSearch 128, batch 512) through the row-sharded deployment at world 1, graph built
+        by b200vs_shard_hnsw_add_batched, beside the plain search on the same index                           (--hnsw-n)
   cfg5  IVF-Flat L2, (rows-per-GPU x world) x 1536, nlist 2048 per GPU, nprobe 64, batch 4096, top-10, list-sharded over
         the GPUs of the box through b200vs_shard_* — run under torchrun (BASELINE: 100 M rows over 8 GPUs = 77 GB per GPU, more
         than an 80 GB H100 holds: default 6.25 M rows per GPU, 50 M over 8)
@@ -678,6 +682,81 @@ def card():
         return f"unknown ({e!r})"
 
 
+def _shard_vs_plain(ix, sh, xq, k, steps, **kw):
+    """Device-resident ms per batch (CUDA events) of the sharded and the plain search on the same index, alternating
+    (three rounds each, the best kept), and whether the two return the same ids and distance bits."""
+    dev = torch.device("cuda", 0)
+    nq = xq.shape[0]
+    q = torch.from_numpy(xq).to(dev)
+    sp, _keep = b200vs.make_search_params(**kw)
+    bufs = {w: (torch.empty((nq, k), dtype=torch.float32, device=dev), torch.empty((nq, k), dtype=torch.int64, device=dev)) for w in ("shard", "plain")}
+    st = torch.cuda.Stream(device=dev)
+    run = {"shard": lambda od, oi: sh.search_device(nq, q.data_ptr(), k, od.data_ptr(), oi.data_ptr(), stream=st.cuda_stream, sp=sp),
+           "plain": lambda od, oi: ix.search_device(nq, q.data_ptr(), k, od.data_ptr(), oi.data_ptr(), stream=st.cuda_stream, sp=sp)}
+    ms = {"shard": [], "plain": []}
+    for w in run:
+        for _ in range(2):
+            run[w](*bufs[w])
+    st.synchronize()
+    for _ in range(3):
+        for w in run:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            for _ in range(steps):
+                run[w](*bufs[w])
+            e1.record(st)
+            st.synchronize()
+            ms[w].append(e0.elapsed_time(e1) / steps)
+    Ds, Is = (t.cpu().numpy() for t in bufs["shard"])
+    Dp, Ip = (t.cpu().numpy() for t in bufs["plain"])
+    return {"ms_per_batch_device_sharded": ms["shard"], "ms_per_batch_device_plain": ms["plain"],
+            "qps_device_sharded": nq / min(ms["shard"]) * 1e3, "qps_device_plain": nq / min(ms["plain"]) * 1e3,
+            "ids_equal": bool(np.array_equal(Is, Ip)), "dist_bits_equal": bool(np.array_equal(Ds.view(np.uint32), Dp.view(np.uint32)))}
+
+
+def cfg1s(o, cores, n=2_000_000, steps=10):
+    """Flat L2 through the row-sharded deployment at world 1: rows generated on the device and added with
+    b200vs_shard_add_device, then the sharded and the plain search of the same index."""
+    d, nq, k = 768, 1024, 10
+    dev = torch.device("cuda", 0)
+    ix = b200vs.Index(b200vs.FLAT, b200vs.L2, d)
+    sh = b200vs.Shard(ix, 0, 1, None, lanes=2)
+    g = torch.Generator(device=dev)
+    g.manual_seed(1234)
+    t0 = time.time()
+    for a in range(0, n, 262144):
+        m = min(262144, n - a)
+        x = torch.rand((m, d), generator=g, device=dev)
+        ids = torch.arange(a + 1, a + 1 + m, dtype=torch.int64, device=dev)
+        torch.cuda.synchronize()
+        sh.add_device(m, x.data_ptr(), ids.data_ptr())
+    t_add = time.time() - t0
+    xq = rnd(nq, d, 4321)
+    line = _shard_vs_plain(ix, sh, xq, k, steps)
+    sh.close()
+    return {"config": f"1s Flat L2 {n}x{d} batch={nq} top-{k}, row-sharded at world 1 (one GPU)", "card": card(), **line,
+            "add_seconds": t_add, "multi_gpu": "not measured (one GPU)"}
+
+
+def cfg4s(o, cores, n, steps=10):
+    """cfg4's HNSW cosine shape through the row-sharded deployment at world 1: the graph is built with
+    b200vs_shard_hnsw_add_batched, then the sharded and the plain search of the same index."""
+    d, nq, k, ef = 768, 512, 10, 128
+    ix = b200vs.Index(b200vs.HNSW, b200vs.COSINE, d, hnsw_m=16, hnsw_efc=200, max_elements=n)
+    sh = b200vs.Shard(ix, 0, 1, None, lanes=2)
+    t0 = time.time()
+    for a in range(0, n, 262144):
+        m = min(262144, n - a)
+        sh.hnsw_add_batched(rnd(m, d, 1234 + a), np.arange(a + 1, a + 1 + m, dtype=np.int64))
+    t_build = time.time() - t0
+    xq = rnd(nq, d, 4321)
+    line = _shard_vs_plain(ix, sh, xq, k, steps, efsearch=ef)
+    sh.close()
+    return {"config": f"4s HNSW cosine {n}x{d} M=16 efSearch={ef} batch={nq} top-{k}, row-sharded at world 1 (one GPU)",
+            "scaled_from": "1M x 768" if n < 1_000_000 else None, "card": card(), **line, "build_seconds": t_build,
+            "multi_gpu": "not measured (one GPU)"}
+
+
 def cfg_range(o, cores, steps=5):
     """Range search at the headline IVF-Flat shape.  The plain call has no device-pointer entry point, so its times are host
     calls (query upload, [nq, max_results] results back); the sharded call is timed device-resident with CUDA events."""
@@ -778,6 +857,7 @@ def main():
     fns = {"1": lambda: cfg1(o, cores), "2": lambda: cfg2(o, cores), "3": lambda: cfg3(o, cores, a.pq_n, a.pq_nbits, a.pq_m), "4": lambda: cfg4(o, cores, a.hnsw_n, a.hnsw_build_threads, a.hnsw_build, a.hnsw_build_batch),
            "calc": lambda: cfg_calc(o, cores), "brute": lambda: cfg_brute(o, cores),
            "3s": lambda: cfg3s(o, cores, a.pq_n, a.pq_nbits, a.pq_m),
+           "1s": lambda: cfg1s(o, cores), "4s": lambda: cfg4s(o, cores, a.hnsw_n),
            "5": lambda: cfg5(o, cores, a.cfg5_rows, steps=a.cfg5_steps, nq=a.cfg5_batch),
            "6": lambda: cfg6(o, cores), "6s": lambda: cfg6s(o, cores), "7": lambda: cfg7(o, cores, a.bin_n, a.bin_dim),
            "range": lambda: cfg_range(o, cores)}

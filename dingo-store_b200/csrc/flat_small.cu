@@ -39,9 +39,10 @@ struct FsArgs {
   long long* part_id;    // [nq, nslices, k]
   int* tickets;          // [nq] zeroed before the launch
   uint32_t* gthr_inv;    // [nq] zeroed: ~(smallest k-th key any slice has published) — an upper bound of the global k-th key
-  float* out_dist;       // [nq, k] API semantics
+  float* out_dist;       // [nq, k] API semantics, or the raw metric value (L2 distance | ip) when raw_out
   long long* out_ids;    // [nq, k]
   long long* dbg;        // optional [8] clock64 stamps of slice 0 and of the merging CTA (B200VS_FS_DEBUG)
+  int raw_out;
 };
 
 __device__ __forceinline__ long long warp_min_ll(long long v) {
@@ -209,7 +210,7 @@ static __global__ void __launch_bounds__(FS_THREADS) flat_small_kernel(const FsA
     const int have = fs_topk_block(s_kd, s_id, n, k, F, [&](int rank, uint32_t kd, long long id) {
       const float v = ord2f(kd);
       const float raw = L2 ? v : -v;
-      a.out_dist[(size_t)qi * k + rank] = L2 ? raw : __fsub_rn(1.0f, raw);
+      a.out_dist[(size_t)qi * k + rank] = (L2 || a.raw_out) ? raw : __fsub_rn(1.0f, raw);
       a.out_ids[(size_t)qi * k + rank] = id;
     });
     for (int i = have + (int)threadIdx.x; i < k; i += FS_THREADS) { a.out_dist[(size_t)qi * k + i] = 0.f; a.out_ids[(size_t)qi * k + i] = -1; }
@@ -242,7 +243,7 @@ bool flat_small_eligible(int device, int64_t nq, int64_t n, int d, int k, const 
 }
 
 void flat_small_search(IndexBase* ix, bool l2, const float* vecs, const long long* ids, int64_t n, int64_t nq, const float* q, int k,
-                       const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
+                       const SearchCtx& sc, float* out_dist, long long* out_ids, bool raw_out, cudaStream_t s) {
   const int d = ix->dim;
   // ~2 CTAs per SM per query, bounded so that the final merge (nslices * k pairs) fits the pair buffer
   int nslices = (int)std::min<int64_t>(std::min(2 * device_sm_count(ix->device), FS_PAIRS / std::max(1, k)), std::max<int64_t>(1, n / 64));
@@ -258,7 +259,7 @@ void flat_small_search(IndexBase* ix, bool l2, const float* vecs, const long lon
   a.part_id = S.alloc<long long>((size_t)nq * nslices * k);
   a.tickets = S.alloc<int>(2 * nq);
   a.gthr_inv = reinterpret_cast<uint32_t*>(a.tickets + nq);
-  a.out_dist = out_dist; a.out_ids = out_ids;
+  a.out_dist = out_dist; a.out_ids = out_ids; a.raw_out = raw_out ? 1 : 0;
   static const bool debug = getenv("B200VS_FS_DEBUG") != nullptr;
   a.dbg = debug ? S.alloc<long long>(8) : nullptr;
   B200VS_CUDA(cudaMemsetAsync(a.tickets, 0, (size_t)nq * 8, s));

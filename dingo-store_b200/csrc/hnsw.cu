@@ -1009,24 +1009,41 @@ struct HnswIndex : IndexBase {
     }
     dirty = true;
   }
+  // add's refusals (batched: add_batched's, for that batch size), which come before either changes anything
+  void check_add(int64_t n, const int64_t*, bool batched, int batch) override {
+    RwSharedGuard rl(this);
+    if (batched) batched_plan(n, batch);
+    else if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
+  }
   // b200vs_hnsw_add_batched: the rule of DESIGN §4.4.  The host plans every batch first on a copy of the bookkeeping it needs
   // (levels from a copy of G.rng in call order, the batch schedule, tombstones, node ids, entry point); the device mirror then
   // builds the links batch after batch in stream order.  G (and its generator) changes only once the device work has
   // finished: a call that fails on the way leaves the index as it was and marks the mirror for a full re-upload.
   int64_t build_scratch_limit = 0;  // b200vs_debug_hnsw_build_scratch_limit: device scratch bytes one call may take, 0 = no cap
 
-  void add_batched(int64_t n, const float* x, const int64_t* in_ids, int batch) {
-    std::unique_lock<std::shared_mutex> wl(rw);
+  // the batch size and the construction kernels' shared memory of add_batched(n rows, batch), after its refusals
+  struct BuildPlan { int batch, bmax; size_t smem_search, smem_link, smem_rev; };
+  BuildPlan batched_plan(int64_t n, int batch) const {
     if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
     if (G.n + n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction holds at most 2^31 - 1 nodes");
-    batch = batch <= 0 ? HNSW_BUILD_DEFAULT_BATCH : std::min(batch, HNSW_BUILD_MAX_BATCH);
-    const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
-    const int bmax = (int)std::min<int64_t>(batch, n);  // largest batch of this call
-    const size_t smem_search = walk_smem_bytes(dim, efc);
-    const size_t smem_link = (size_t)(efc + bmax) * 2 * sizeof(unsigned long long) + (size_t)M * 4;
-    const size_t smem_rev = (size_t)(maxM0 + bmax) * 2 * sizeof(unsigned long long) + (size_t)maxM0 * 4;
-    if (smem_search > HNSW_SMEM_LIMIT || smem_link > HNSW_SMEM_LIMIT || smem_rev > HNSW_SMEM_LIMIT)
+    BuildPlan P;
+    P.batch = batch <= 0 ? HNSW_BUILD_DEFAULT_BATCH : std::min(batch, HNSW_BUILD_MAX_BATCH);
+    P.bmax = (int)std::min<int64_t>(P.batch, n);  // largest batch of this call
+    P.smem_search = walk_smem_bytes(dim, (int)G.efc);
+    P.smem_link = (size_t)((int)G.efc + P.bmax) * 2 * sizeof(unsigned long long) + (size_t)G.M * 4;
+    P.smem_rev = (size_t)((int)G.maxM0 + P.bmax) * 2 * sizeof(unsigned long long) + (size_t)G.maxM0 * 4;
+    if (P.smem_search > HNSW_SMEM_LIMIT || P.smem_link > HNSW_SMEM_LIMIT || P.smem_rev > HNSW_SMEM_LIMIT)
       fail(B200VS_EILLEGAL_PARAMETERS, "efconstruction / dimension / batch too large for the batched construction kernels");
+    return P;
+  }
+
+  void add_batched(int64_t n, const float* x, const int64_t* in_ids, int batch) {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    const BuildPlan P = batched_plan(n, batch);
+    batch = P.batch;
+    const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
+    const int bmax = P.bmax;
+    const size_t smem_search = P.smem_search;
     set_device();
     cudaStream_t s = stream;
     upload(s);
@@ -1292,6 +1309,17 @@ struct HnswIndex : IndexBase {
     B200VS_CUDA(cudaStreamSynchronize(s));
     uploaded_rows = n;
     dirty = false;
+  }
+
+  // b200vs_search's efsearch refusal (hnsw.cc:332-336) and search_dev's shared-memory refusal, from the arguments alone: a rank
+  // whose graph is still empty returns from search_dev before the latter, and a refused search must not leave its efsearch
+  // in the sticky ef
+  void check_row_search(int k, const b200vs_search_params* sp) const override {
+    const int efs = sp ? sp->efsearch : 0;
+    if (efs < 0 || efs > 1024)
+      fail(B200VS_EILLEGAL_PARAMETERS, "efsearch is illegal, " + std::to_string(efs) + ", must between 0 and 1024");
+    if (walk_smem_bytes(dim, std::max(efs > 0 ? efs : ef, k)) > HNSW_SMEM_LIMIT)
+      fail(B200VS_EILLEGAL_PARAMETERS, "efsearch / dimension too large for the search kernel");
   }
 
   void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {

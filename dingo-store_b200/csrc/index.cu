@@ -346,29 +346,53 @@ struct FlatIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
+    float* st = scratch.alloc<float>((size_t)n * dim);
+    long long* st_ids = scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
+    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
+    add_locked(n, st, st_ids, in_ids, loading);
+  }
+
+  // the device-pointer form of add: the rows stay on the device, the caller's host copy of the ids feeds the id map
+  void add_rows_dev(int64_t n, const float* x_dev, const long long* ids_dev, const int64_t* ids_host) override {
+    check_batch_ids_unique(n, ids_host);
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    float* st = const_cast<float*>(x_dev);
+    if (metric == B200VS_COSINE) {  // the normaliser works in place: keep the caller's rows intact
+      st = scratch.alloc<float>((size_t)n * dim);
+      B200VS_CUDA(cudaMemcpyAsync(st, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
+    }
+    add_locked(n, st, ids_dev, ids_host, false);
+  }
+
+  // rw + gpu_mu held, scratch reset, ids unique.  st / st_ids: device rows and ids (st is normalised in place for cosine
+  // unless prepared); h_in: the ids on the host.
+  void add_locked(int64_t n, float* st, const long long* st_ids, const int64_t* h_in, bool prepared) {
     std::vector<int64_t> dead;
     for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(in_ids[i]);
+      auto it = id2row.find(h_in[i]);
       if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
     }
     tombstone(dead);
     const int64_t cap = (int64_t)store.ids.cap;
     if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
-    float* st = scratch.alloc<float>((size_t)n * dim);
-    long long* st_ids = scratch.alloc<long long>(n);
     std::vector<long long> slots(n);
     for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
-    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    if (metric == B200VS_COSINE && !loading) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
+    if (metric == B200VS_COSINE && !prepared) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
     store.write(st, st_ids, slots);
     B200VS_CUDA(cudaStreamSynchronize(stream));
     h_ids.resize(rows + n);
-    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = in_ids[i]; id2row[in_ids[i]] = rows + i; }
+    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = h_in[i]; id2row[h_in[i]] = rows + i; }
     rows += n;
     publish_len();
     compact_if_needed();
   }
+
+  void check_add(int64_t n, const int64_t* in_ids, bool, int) override { check_batch_ids_unique(n, in_ids); }
 
   // streaming brute-force scan (b200vs_scan_*): the tile index is emptied between tiles, buffers are kept
   void clear() override {
@@ -407,19 +431,26 @@ struct FlatIndex : IndexBase {
   }
 
   void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+    search_rows(nq, xq, k, sc, od, oi, false, s);
+  }
+  void search_raw_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+    search_rows(nq, xq, k, sc, od, oi, true, s);
+  }
+  // raw_out: od = raw metric value (L2 distance | ip) instead of the API distance; every path selects the same rows
+  void search_rows(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, bool raw_out, cudaStream_t s) {
     const float* q = prepare_queries(nq, xq, s);
     const TcView v = view();
     if (rows > 0 && tc_eligible(this, v, nq, k, 1, sc)) {
       long long* probes = scratch.alloc<long long>(nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
-      tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, 1, sc, od, oi, s);
+      tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, 1, sc, od, oi, raw_out, s);
       return;
     }
     if (flat_small_eligible(device, nq, rows, dim, k, sc)) {  // one query per task is the reference's own shape: single-launch path
-      flat_small_search(this, metric == B200VS_L2, store.vecs.p, store.ids.p, rows, nq, q, k, sc, od, oi, s);
+      flat_small_search(this, metric == B200VS_L2, store.vecs.p, store.ids.p, rows, nq, q, k, sc, od, oi, raw_out, s);
       return;
     }
-    run_scan(this, job(sc), nq, q, k, od, nullptr, oi, nullptr, s);
+    run_scan(this, job(sc), nq, q, k, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, nullptr, s);
   }
 
   void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) override {
@@ -439,19 +470,27 @@ struct FlatIndex : IndexBase {
   // faiss range_search keeps L2 dis < radius, IP ip > radius.
   void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
                         long long* oi, int* oc, cudaStream_t s) override {
+    range_rows(nq, xq, radius, max_results, sc, od, oi, oc, false, s);
+  }
+  void range_search_raw_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
+                            long long* oi, int* oc, cudaStream_t s) override {
+    range_rows(nq, xq, radius, max_results, sc, od, oi, oc, true, s);
+  }
+  void range_rows(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od, long long* oi, int* oc,
+                  bool raw_out, cudaStream_t s) {
     const float* q = prepare_queries(nq, xq, s);
     const float thr = ip_like() ? 1.0F - radius : radius;
     const TcView v = view();
     if (rows > 0 && tc_range_eligible(this, v, nq, max_results, 1, sc)) {
       long long* probes = scratch.alloc<long long>(nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
-      tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, 1, sc, od, oi, oc, false, s);
+      tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, 1, sc, od, oi, oc, raw_out, s);
       return;
     }
     ScanJob j = job(sc);
     j.has_thr = true;
     j.thr_raw = thr;
-    run_scan(this, j, nq, q, max_results, od, nullptr, oi, oc, s);
+    run_scan(this, j, nq, q, max_results, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, oc, s);
   }
 
   void reconstruct(int64_t n, const int64_t* in_ids, float* out, uint8_t* found) override {
@@ -852,7 +891,7 @@ void IvfFlatIndex::search_dev(int64_t nq, const float* xq, int k, const SearchCt
   if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
   const TcView v = view();
   if (L.live > 0 && tc_eligible(this, v, nq, k, nprobe, sc)) {
-    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, s);
+    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, false, s);
     return;
   }
   ScanJob j = list_job(sc, probes, nprobe);
@@ -890,7 +929,7 @@ void IvfFlatIndex::search_probes_prepared_dev(int64_t nq, const float* q, int k,
   if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
   const TcView v = view();
   if (L.live > 0 && tc_eligible(this, v, nq, k, nprobe, sc)) {
-    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, s);
+    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, false, s);
     return;
   }
   ScanJob j = list_job(sc, probes, nprobe);

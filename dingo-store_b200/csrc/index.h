@@ -252,6 +252,31 @@ struct IndexBase {
     (void)n; (void)x_dev; (void)ids_dev; (void)lists_dev; (void)upsert; (void)prepared;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
   }
+  // ---- building blocks of a row-sharded deployment (shard.cu); FLAT and HNSW ----
+  // the refusals add (batched: b200vs_hnsw_add_batched with `batch`) would give n rows with these host ids, decided before
+  // anything changes, so that every rank of a collective add can agree on one status first
+  virtual void check_add(int64_t n, const int64_t* ids, bool batched, int batch) { (void)n; (void)ids; (void)batched; (void)batch; }
+  // FLAT: add's semantics on rows and ids already on this device; ids_host = the same ids on the host (the id map needs them,
+  // and the caller already holds them).  Only the row-sharded owner calls it: b200vs_add_with_ids_device still refuses FLAT.
+  virtual void add_rows_dev(int64_t n, const float* x_dev, const long long* ids_dev, const int64_t* ids_host) {
+    (void)n; (void)x_dev; (void)ids_dev; (void)ids_host;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "device-row add only exists for FLAT");
+  }
+  // the refusals a search with k and sp's efsearch would meet after the first collective of a row-sharded search, decided
+  // from the arguments and the index's parameters alone, so that every rank refuses alike before it (HNSW: efsearch outside
+  // [0, 1024], as b200vs_search; the walk's shared memory)
+  virtual void check_row_search(int k, const b200vs_search_params* sp) const { (void)k; (void)sp; }
+  // search_dev / range_search_dev, but od holds the raw metric value (L2 distance | ip): the key the single-index select
+  // ranks by, which a merge of several indexes' results has to order by
+  virtual void search_raw_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) {
+    (void)nq; (void)xq; (void)k; (void)sc; (void)od; (void)oi; (void)s;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key search only exists for FLAT");
+  }
+  virtual void range_search_raw_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
+                                    long long* oi, int* oc, cudaStream_t s) {
+    (void)nq; (void)xq; (void)radius; (void)max_results; (void)sc; (void)od; (void)oi; (void)oc; (void)s;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key range search only exists for FLAT");
+  }
   // nearest-centroid assignment of prepared rows (faiss quantizer->assign): out_lists_dev[n], on stream s (a lane must be held)
   virtual void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) {
     (void)n; (void)x_dev; (void)out_lists_dev; (void)s;

@@ -10,6 +10,8 @@
 //   3. ONE ncclAllGather of the packed per-shard top-k ((distance, id) 16-byte records) over NVLink, then the k-way merge
 //      kernel — the engine's analogue of VectorIndexWrapper::MergeSearchResults (src/vector/vector_index.cc:1056-1108).
 // Rows are routed to their list owner at add time (b200vs_shard_add*: assignment on the sender, grouped ncclSend/ncclRecv).
+// FLAT and HNSW shard by row instead (DESIGN.md 4.5): row id lives on rank row_owner_of(id), each rank holds a standalone
+// index of its rows, and a search skips step 1 and runs the whole batch on the rank's index before the same all-gather + merge.
 //
 // NCCL is resolved at run time (dlopen of libnccl.so.2): a single-GPU dingo-store node needs no NCCL at all, and a process
 // that already carries an NCCL (e.g. the one bundled with PyTorch in the test harness) shares it.  Each in-flight lane owns
@@ -189,6 +191,130 @@ static __global__ void count_lists_kernel(const long long* __restrict__ lists, l
   if (i < n) { const long long l = lists[i]; if (l >= 0 && l < nlist) atomicAdd(counts + l, 1ULL); }
 }
 
+// merged Flat IP / cosine results: key -ip -> API distance 1 - ip, rounded as the single-index finish rounds it
+static __global__ void ip_key_to_api_kernel(float* dist, const long long* __restrict__ ids, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && ids[i] >= 0) dist[i] = __fsub_rn(1.0f, -dist[i]);
+}
+
+constexpr int ROUTE_MAX_WORLD = 1024;  // ranks of a row-sharded index
+
+// The owner of a row of a row-sharded (FLAT / HNSW) index: splitmix64's finalizer of the id read as a uint64, mod world.
+// The one definition for the host (b200vs_row_owner) and the device (row routing).  z mod world is taken 16 bits at a
+// time in 32-bit arithmetic, exact for world <= ROUTE_MAX_WORLD (each partial value stays below 2^26), which keeps the
+// 64-bit division routine out of the routing kernels.
+__host__ __device__ __forceinline__ int row_owner_of(long long id, int world) {
+  unsigned long long z = (unsigned long long)id;
+  z ^= z >> 30;
+  z *= 0xbf58476d1ce4e5b9ULL;
+  z ^= z >> 27;
+  z *= 0x94d049bb133111ebULL;
+  z ^= z >> 31;
+  const unsigned w = (unsigned)world, lo = (unsigned)z;
+  unsigned r = (unsigned)(z >> 32) % w;
+  r = ((r << 16) | (lo >> 16)) % w;
+  r = ((r << 16) | (lo & 0xffffu)) % w;
+  return (int)r;
+}
+
+// Stable partition of rows by owner, in tiles of ROUTE_THREADS rows: route_count_kernel counts each tile's rows per owner
+// into an owner-major table cnt[owner * ntiles + tile], route_offsets_kernel scans that table (its exclusive prefix sum is
+// the first output slot of every (owner, tile)), and route_scatter_kernel moves each row to its slot, so each owner's rows
+// keep the caller's order.
+constexpr int ROUTE_THREADS = 256, ROUTE_WARPS = ROUTE_THREADS / 32;  // s_cnt below: ROUTE_WARPS * world ints of shared memory
+constexpr int ROUTE_SCAN_THREADS = 1024;
+
+// This thread's row of the tile: returns (its owner, -1 past n; the rows of that owner before it in its warp), and
+// s_cnt[warp * W + owner] = the warp's rows of that owner.
+static __device__ __forceinline__ int2 route_tile(const long long* __restrict__ ids, long long n, int W, int* s_cnt) {
+  for (int i = threadIdx.x; i < ROUTE_WARPS * W; i += ROUTE_THREADS) s_cnt[i] = 0;
+  __syncthreads();
+  const long long i = (long long)blockIdx.x * ROUTE_THREADS + threadIdx.x;
+  const int o = i < n ? row_owner_of(ids[i], W) : -1;
+  const unsigned peers = __match_any_sync(0xffffffffu, o);
+  const int lane = threadIdx.x & 31;
+  if (o >= 0 && __ffs(peers) - 1 == lane) s_cnt[(threadIdx.x >> 5) * W + o] = __popc(peers);
+  __syncthreads();
+  return make_int2(o, __popc(peers & ((1u << lane) - 1u)));
+}
+
+static __global__ void __launch_bounds__(ROUTE_THREADS) route_count_kernel(const long long* __restrict__ ids, long long n, int W, int* cnt) {
+  extern __shared__ int s_cnt[];
+  route_tile(ids, n, W, s_cnt);
+  for (int o = threadIdx.x; o < W; o += ROUTE_THREADS) {
+    int c = 0;
+    for (int w = 0; w < ROUTE_WARPS; ++w) c += s_cnt[w * W + o];
+    cnt[(size_t)o * gridDim.x + blockIdx.x] = c;
+  }
+}
+
+// One CTA: off[i] = sum of cnt[0, i) over the m = W * ntiles entries, in chunks of ROUTE_SCAN_THREADS (a warp-shuffle scan,
+// one scan of the warp totals, a running carry); owner_cnt[o] = rows of owner o.
+static __global__ void __launch_bounds__(ROUTE_SCAN_THREADS)
+route_offsets_kernel(const int* __restrict__ cnt, long long ntiles, int W, long long* off, long long* owner_cnt) {
+  __shared__ long long s_warp[ROUTE_SCAN_THREADS / 32];
+  __shared__ long long s_carry;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long m = ntiles * W;
+  if (threadIdx.x == 0) s_carry = 0;
+  for (long long base = 0; base < m; base += ROUTE_SCAN_THREADS) {
+    const long long i = base + threadIdx.x;
+    const long long v = i < m ? cnt[i] : 0;
+    long long x = v;
+    for (int sh = 1; sh < 32; sh <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, x, sh);
+      if (lane >= sh) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      long long w = s_warp[lane];
+      for (int sh = 1; sh < 32; sh <<= 1) {
+        const long long y = __shfl_up_sync(0xffffffffu, w, sh);
+        if (lane >= sh) w += y;
+      }
+      s_warp[lane] = w;
+    }
+    __syncthreads();
+    const long long incl = s_carry + (warp ? s_warp[warp - 1] : 0) + x;
+    if (i < m) off[i] = incl - v;
+    __syncthreads();
+    if (threadIdx.x == ROUTE_SCAN_THREADS - 1) s_carry = incl;
+  }
+  __syncthreads();
+  for (int o = threadIdx.x; o < W; o += ROUTE_SCAN_THREADS)
+    owner_cnt[o] = (o + 1 < W ? off[(o + 1) * ntiles] : s_carry) - off[o * ntiles];
+}
+
+static __global__ void __launch_bounds__(ROUTE_THREADS)
+route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ ids, long long n, int d, int W,
+                     const long long* __restrict__ off, float* ox, long long* oids) {
+  extern __shared__ int s_cnt[];
+  __shared__ long long s_dst[ROUTE_THREADS];
+  const int2 t = route_tile(ids, n, W, s_cnt);
+  const int o = t.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (o >= 0) {
+    long long p = off[(size_t)o * gridDim.x + blockIdx.x] + t.y;
+    for (int w = 0; w < warp; ++w) p += s_cnt[w * W + o];
+    s_dst[threadIdx.x] = p;
+  }
+  __syncthreads();
+  const long long r0 = (long long)blockIdx.x * ROUTE_THREADS;
+  const bool vec = (d & 3) == 0 && ((reinterpret_cast<size_t>(x) | reinterpret_cast<size_t>(ox)) & 15) == 0;
+  for (int j = warp; j < ROUTE_THREADS && r0 + j < n; j += ROUTE_WARPS) {  // one warp per row
+    const long long src = r0 + j, dst = s_dst[j];
+    const float* xs = x + (size_t)src * d;
+    float* xd = ox + (size_t)dst * d;
+    if (vec) {
+#pragma unroll 1
+      for (int i = lane; i < (d >> 2); i += 32) reinterpret_cast<float4*>(xd)[i] = reinterpret_cast<const float4*>(xs)[i];
+    } else {
+      for (int i = lane; i < d; i += 32) xd[i] = xs[i];
+    }
+    if (lane == 0) oids[dst] = ids[src];
+  }
+}
+
 }  // namespace b200vs
 
 using namespace b200vs;
@@ -199,6 +325,7 @@ using namespace b200vs;
 struct b200vs_shard {
   IndexBase* ix = nullptr;
   int rank = 0, world = 1, nlanes = 1;
+  bool rows = false;  // sharded by rows (FLAT, HNSW: owner(id) = row_owner_of), else by inverted list (IVF_FLAT, IVF_PQ)
   struct SLane {
     ncclComm_t comm = nullptr;
     std::mutex mu;
@@ -302,8 +429,9 @@ SearchCtx make_ctx_shard(IndexBase* ix, const b200vs_search_params* sp, cudaStre
 }
 
 // The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
-// on stream s.  local(q, sc, nprobe) is step 2: it writes this rank's ascending, -1-padded [nq, k] (key, id) lists of the
-// prepared queries q over the gathered probe table L.probes into L.od / L.oi, the key being what the merge orders by.
+// on stream s.  local(q, sc, nprobe) is step 2: it writes this rank's ascending, -1-padded [nq, k] (key, id) lists into
+// L.od / L.oi, the key being what the merge orders by.  List-sharded: q are the prepared queries and L.probes the gathered
+// probe table.  Row-sharded: there is no coarse step; q are the raw queries (the rank's index prepares them) and nprobe is 0.
 template <class LocalScan>
 void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
                   float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local) {
@@ -311,20 +439,24 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
   const int W = sh->world, r = sh->rank, d = ix->dim;
   if (L.last && L.last != s && L.done) B200VS_CUDA(cudaStreamWaitEvent(s, L.done, 0));
   SearchCtx sc = make_ctx_shard(ix, sp, s);
-  const int nprobe = ix->resolve_nprobe_api(sc);
-  const int64_t per = (nq + W - 1) / W;
-  // cosine: normalise once (NormalizeVectorForFaiss), the coarse pass and the list scan both take prepared queries
-  const float* q = ix->prepare_queries(nq, xq, s);
-  // 1) coarse quantiser on this rank's slice, all-gather of the probe table (in place)
-  L.probes.reserve((size_t)per * W * nprobe, 0, s);
-  const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
-  long long* mine = L.probes.p + (size_t)per * r * nprobe;
-  if (q1 - q0 < per) fill_ll_kernel<<<(unsigned)cdiv(per * nprobe, 256), 256, 0, s>>>(mine, per * nprobe, -1);
-  if (q1 > q0) ix->coarse_probes_dev(q1 - q0, q + (size_t)q0 * d, nprobe, mine, s);
-  ix->phase(IndexBase::PH_COMM, s);
-  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.probes.p, (size_t)per * nprobe, ncclInt64, L.comm, s));
-  ix->phase(IndexBase::PH_OTHER, s);
-  // 2) scan of the probed lists this rank owns -> exact local results
+  const float* q = xq;
+  int nprobe = 0;
+  if (!sh->rows) {
+    nprobe = ix->resolve_nprobe_api(sc);
+    const int64_t per = (nq + W - 1) / W;
+    // cosine: normalise once (NormalizeVectorForFaiss), the coarse pass and the list scan both take prepared queries
+    q = ix->prepare_queries(nq, xq, s);
+    // 1) coarse quantiser on this rank's slice, all-gather of the probe table (in place)
+    L.probes.reserve((size_t)per * W * nprobe, 0, s);
+    const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
+    long long* mine = L.probes.p + (size_t)per * r * nprobe;
+    if (q1 - q0 < per) fill_ll_kernel<<<(unsigned)cdiv(per * nprobe, 256), 256, 0, s>>>(mine, per * nprobe, -1);
+    if (q1 > q0) ix->coarse_probes_dev(q1 - q0, q + (size_t)q0 * d, nprobe, mine, s);
+    ix->phase(IndexBase::PH_COMM, s);
+    if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.probes.p, (size_t)per * nprobe, ncclInt64, L.comm, s));
+    ix->phase(IndexBase::PH_OTHER, s);
+  }
+  // 2) scan of the probed lists this rank owns, or search of the rank's rows -> exact local results
   L.od.reserve((size_t)nq * k, 0, s);
   L.oi.reserve((size_t)nq * k, 0, s);
   local(q, sc, nprobe);
@@ -352,13 +484,29 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
   L.last = s;
 }
 
-// top-k: the tile scan's exact local top-k, keyed on the API distance
+// top-k.  List-sharded: the tile scan's exact local top-k, keyed on the API distance.  Row-sharded FLAT: the rank's search
+// keyed on the single-index select's key (L2 distance | -ip; two distinct inner products can round to the same 1 - ip, and
+// an API-distance merge would then choose and order them by id), the API distance formed after the merge.  Row-sharded
+// HNSW: the rank's graph walk, keyed on the distance the walk itself ranks by (hnsw_distance: L2 distance | 1 - ip).
 void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
                          float* out_dist, long long* out_ids, cudaStream_t s) {
   IndexBase* ix = sh->ix;
+  const bool flat_ip = sh->rows && ix->type == B200VS_FLAT && ix->ip_like();
   shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
-    ix->search_probes_prepared_dev(nq, q, k, L.probes.p, nprobe, sc, L.od.p, L.oi.p, s);
+    if (!sh->rows) {
+      ix->search_probes_prepared_dev(nq, q, k, L.probes.p, nprobe, sc, L.od.p, L.oi.p, s);
+    } else if (ix->type == B200VS_FLAT) {
+      ix->search_raw_dev(nq, q, k, sc, L.od.p, L.oi.p, s);
+      if (flat_ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
+    } else {
+      ix->search_dev(nq, q, k, sc, L.od.p, L.oi.p, s);
+    }
   });
+  if (flat_ip) {
+    ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
+    B200VS_CUDA(cudaGetLastError());
+    ix->launch_count(1);
+  }
 }
 
 // range: the local range scan keyed on the single-index select's key (L2 distance | -ip) — two distinct inner products can
@@ -372,6 +520,7 @@ void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, co
     int* oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
     // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
     if (std::isnan(radius)) fill_empty_range(nq, max_results, L.od.p, L.oi.p, oc, s);
+    else if (sh->rows) ix->range_search_raw_dev(nq, q, radius, max_results, sc, L.od.p, L.oi.p, oc, s);
     else ix->range_search_probes_prepared_dev(nq, q, radius, max_results, L.probes.p, nprobe, sc, L.od.p, L.oi.p, oc, s);
     if (!l2) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
   });
@@ -382,8 +531,9 @@ void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, co
 }
 
 // refusals of a sharded range search, decided from its arguments alone so that every rank refuses before the first collective
-void check_shard_range(int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
+void check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+  if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // as b200vs_range_search
   if (max_results <= 0 || max_results > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
   if (!od || !oi || !oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
 }
@@ -479,15 +629,19 @@ int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const ui
     if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
     *out = nullptr;
     IndexBase* ix = index_impl(idx);
-    if (ix->type != B200VS_IVF_FLAT && ix->type != B200VS_IVF_PQ)
-      fail(B200VS_EVECTOR_NOT_SUPPORT, "list sharding is implemented for IVF_FLAT and IVF_PQ (HNSW: replicas only)");
+    const bool rows = ix->type == B200VS_FLAT || ix->type == B200VS_HNSW;
+    if (!rows && ix->type != B200VS_IVF_FLAT && ix->type != B200VS_IVF_PQ)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "sharding is implemented for FLAT and HNSW (by rows), IVF_FLAT and IVF_PQ (by list)");
     if (ix->type == B200VS_IVF_PQ && ix->sub_type() == B200VS_FLAT)
       fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode (too few training rows) has no inverted lists to shard");
+    if (rows && ix->count() + ix->deleted_count() > 0)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index must be empty when its shard is created");
     if (world < 1 || rank < 0 || rank >= world) fail(B200VS_EILLEGAL_PARAMETERS, "bad rank / world");
+    if (rows && world > ROUTE_MAX_WORLD) fail(B200VS_EILLEGAL_PARAMETERS, "row sharding supports at most 1024 ranks");
     if (world > 1 && !id) fail(B200VS_EILLEGAL_PARAMETERS, "null communicator id");
     lanes = std::max(1, std::min(lanes <= 0 ? 2 : lanes, kLanes));
     std::unique_ptr<b200vs_shard> sh(new b200vs_shard());
-    sh->ix = ix; sh->rank = rank; sh->world = world; sh->nlanes = lanes;
+    sh->ix = ix; sh->rank = rank; sh->world = world; sh->nlanes = lanes; sh->rows = rows;
     ix->set_device();
     B200VS_CUDA(cudaStreamCreateWithFlags(&sh->ws, cudaStreamNonBlocking));
     for (int c = 0; c < lanes; ++c) {
@@ -512,6 +666,7 @@ void b200vs_shard_destroy(b200vs_shard* sh) {
 int b200vs_shard_list_range(b200vs_shard* h, int32_t rank, int32_t* begin, int32_t* end) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists");
     if (rank < 0 || rank >= sh->world) fail(B200VS_EILLEGAL_PARAMETERS, "bad rank");
     const int nl = sh->ix->nlist_now(), per = sh->lists_per_rank();
     if (begin) *begin = std::min(nl, per * rank);
@@ -526,6 +681,7 @@ int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
     IndexBase* ix = sh->ix;
+    if (sh->rows) return B200VS_OK;  // FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
     if (ix->type == B200VS_IVF_PQ) {
       shard_train_pq(sh, n, x);
       return B200VS_OK;
@@ -562,6 +718,8 @@ int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
 int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    // an HNSW state blob is a whole graph: replicating it would put every row on every rank
+    if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no replicated trained state");
     if (root < 0 || root >= sh->world) fail(B200VS_EILLEGAL_PARAMETERS, "bad root");
     std::lock_guard<std::mutex> g(sh->add_mu);
     broadcast_state_locked(sh, root);
@@ -657,6 +815,105 @@ void shard_add_device_impl(b200vs_shard* sh, int64_t n, const float* x_dev, cons
   if (nrecv) ix->add_dev(nrecv, rx.p, rids.p, rlists.p, false, true);
 }
 
+// Row-sharded add (FLAT, HNSW): every row travels RAW to owner(id) (Flat and HNSW normalise cosine rows differently, so the
+// owner's add normalises), and the owner runs the single-index add on the rows it received, in arrival order: rank 0's rows
+// first, then rank 1's, ..., each in its caller's order (an HNSW graph depends on insertion order).  Before any rank changes
+// anything, every owner checks its rows (check_add: a repeated id for FLAT, max_elements for HNSW) and the statuses are
+// all-gathered: every rank returns the first refusal in rank order, or adds.  batched: b200vs_hnsw_add_batched with `batch`.
+void shard_add_rows_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long long* ids_dev, bool batched, int batch) {
+  IndexBase* ix = sh->ix;
+  const int W = sh->world, r = sh->rank, d = ix->dim;
+  cudaStream_t s = sh->ws;
+  ix->set_device();
+  DevBuf<float> sx, rx;
+  DevBuf<long long> sids, rids, cnt_all, tile_off;
+  DevBuf<int> tile_cnt, st;
+  cnt_all.reserve((size_t)W * W, 0, s);
+  long long* mine = cnt_all.p + (size_t)r * W;
+  // stable partition by owner on the device; this rank's row of the counts matrix
+  if (n) {
+    const long long ntiles = cdiv(n, ROUTE_THREADS);
+    const size_t smem = (size_t)ROUTE_WARPS * W * 4;
+    tile_cnt.reserve((size_t)ntiles * W, 0, s); tile_off.reserve((size_t)ntiles * W, 0, s);
+    sx.reserve((size_t)n * d, 0, s); sids.reserve((size_t)n, 0, s);
+    route_count_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(ids_dev, n, W, tile_cnt.p);
+    route_offsets_kernel<<<1, ROUTE_SCAN_THREADS, 0, s>>>(tile_cnt.p, ntiles, W, tile_off.p, mine);
+    route_scatter_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(x_dev, ids_dev, n, d, W, tile_off.p, sx.p, sids.p);
+    B200VS_CUDA(cudaGetLastError());
+  } else {
+    B200VS_CUDA(cudaMemsetAsync(mine, 0, (size_t)W * 8, s));
+  }
+  // counts matrix: every rank learns how many rows each peer sends it
+  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, cnt_all.p, (size_t)W, ncclInt64, sh->lanes[0]->comm, s));
+  std::vector<long long> h_cnt((size_t)W * W);
+  B200VS_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt_all.p, (size_t)W * W * 8, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  std::vector<long long> send_off(W + 1, 0), recv_off(W + 1, 0);
+  for (int w = 0; w < W; ++w) {
+    send_off[w + 1] = send_off[w] + h_cnt[(size_t)r * W + w];
+    recv_off[w + 1] = recv_off[w] + h_cnt[(size_t)w * W + r];
+  }
+  const long long nrecv = recv_off[W];
+  if (W > 1) {
+    rx.reserve((size_t)std::max<long long>(nrecv, 1) * d, 0, s); rids.reserve((size_t)std::max<long long>(nrecv, 1), 0, s);
+    B200VS_NCCL(nccl().GroupStart());
+    for (int w = 0; w < W; ++w) {
+      const long long sc = send_off[w + 1] - send_off[w], rc = recv_off[w + 1] - recv_off[w];
+      if (sc) {
+        B200VS_NCCL(nccl().Send(sx.p + (size_t)send_off[w] * d, (size_t)sc * d, ncclFloat, w, sh->lanes[0]->comm, s));
+        B200VS_NCCL(nccl().Send(sids.p + send_off[w], (size_t)sc, ncclInt64, w, sh->lanes[0]->comm, s));
+      }
+      if (rc) {
+        B200VS_NCCL(nccl().Recv(rx.p + (size_t)recv_off[w] * d, (size_t)rc * d, ncclFloat, w, sh->lanes[0]->comm, s));
+        B200VS_NCCL(nccl().Recv(rids.p + recv_off[w], (size_t)rc, ncclInt64, w, sh->lanes[0]->comm, s));
+      }
+    }
+    B200VS_NCCL(nccl().GroupEnd());
+  } else {  // a world of one receives exactly what it sends
+    rx.swap(sx); rids.swap(sids);
+  }
+  std::vector<int64_t> hid((size_t)nrecv);
+  if (nrecv) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rids.p, (size_t)nrecv * 8, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  // status agreement
+  int code = B200VS_OK;
+  std::string msg;
+  try {
+    ix->check_add(nrecv, hid.data(), batched, batch);
+  } catch (const StatusError& e) {
+    code = e.code; msg = e.msg;
+  }
+  std::vector<int> codes((size_t)W, code);
+  if (W > 1) {
+    st.reserve((size_t)W, 0, s);
+    B200VS_CUDA(cudaMemcpyAsync(st.p + r, &code, 4, cudaMemcpyHostToDevice, s));
+    B200VS_NCCL(nccl().AllGather(st.p + r, st.p, 1, ncclInt32, sh->lanes[0]->comm, s));
+    B200VS_CUDA(cudaMemcpyAsync(codes.data(), st.p, (size_t)W * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+  }
+  for (int w = 0; w < W; ++w)
+    if (codes[w] != B200VS_OK) fail(codes[w], w == r ? msg : "shard add refused by rank " + std::to_string(w));
+  if (!nrecv) return;
+  if (ix->type == B200VS_FLAT) {
+    ix->add_rows_dev(nrecv, rx.p, rids.p, hid.data());
+    return;
+  }
+  std::vector<float> hx((size_t)nrecv * d);  // the HNSW builders take host rows
+  B200VS_CUDA(cudaMemcpyAsync(hx.data(), rx.p, (size_t)nrecv * d * 4, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  if (batched) hnsw_add_batched(ix, nrecv, hx.data(), hid.data(), batch);
+  else ix->add(nrecv, hx.data(), hid.data(), false);
+}
+
+// upload of host rows to the write stream, for the host-pointer variants of the collective adds
+void upload_rows(b200vs_shard* sh, int64_t n, const float* x, const int64_t* ids, DevBuf<float>& dx, DevBuf<long long>& di) {
+  if (!n) return;
+  dx.reserve((size_t)n * sh->ix->dim, 0, sh->ws); di.reserve((size_t)n, 0, sh->ws);
+  B200VS_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n * sh->ix->dim * 4, cudaMemcpyHostToDevice, sh->ws));
+  B200VS_CUDA(cudaMemcpyAsync(di.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+}
+
 }  // namespace
 
 extern "C" {
@@ -668,7 +925,8 @@ int b200vs_shard_add_device(b200vs_shard* h, int64_t n, const float* x_dev, cons
     b200vs_shard* sh = get(h);
     if (n < 0 || (n > 0 && (!x_dev || !ids_dev))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
     std::lock_guard<std::mutex> g(sh->add_mu);
-    shard_add_device_impl(sh, n, x_dev, (const long long*)ids_dev);
+    if (sh->rows) shard_add_rows_impl(sh, n, x_dev, (const long long*)ids_dev, false, 0);
+    else shard_add_device_impl(sh, n, x_dev, (const long long*)ids_dev);
     return B200VS_OK;
   });
 }
@@ -681,13 +939,36 @@ int b200vs_shard_add(b200vs_shard* h, int64_t n, const float* x, const int64_t* 
     sh->ix->set_device();
     DevBuf<float> dx;
     DevBuf<long long> di;
-    if (n) {
-      dx.reserve((size_t)n * sh->ix->dim, 0, sh->ws); di.reserve((size_t)n, 0, sh->ws);
-      B200VS_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n * sh->ix->dim * 4, cudaMemcpyHostToDevice, sh->ws));
-      B200VS_CUDA(cudaMemcpyAsync(di.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, sh->ws));
-      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-    }
-    shard_add_device_impl(sh, n, dx.p, di.p);
+    upload_rows(sh, n, x, ids, dx, di);
+    if (sh->rows) shard_add_rows_impl(sh, n, dx.p, di.p, false, 0);
+    else shard_add_device_impl(sh, n, dx.p, di.p);
+    return B200VS_OK;
+  });
+}
+
+// Collective batched HNSW build of a row-sharded HNSW index: shard_add's routing, then b200vs_hnsw_add_batched with `batch`
+// on the rows each rank received, in arrival order.
+int b200vs_shard_hnsw_add_batched(b200vs_shard* h, int64_t n, const float* x, const int64_t* ids, int32_t batch) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    if (sh->ix->type != B200VS_HNSW) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction needs an HNSW index");
+    if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    sh->ix->set_device();
+    DevBuf<float> dx;
+    DevBuf<long long> di;
+    upload_rows(sh, n, x, ids, dx, di);
+    shard_add_rows_impl(sh, n, dx.p, di.p, true, batch);
+    return B200VS_OK;
+  });
+}
+
+// Owner of every id of a row-sharded index (pure host function): callers place rows where they belong so they travel nowhere.
+int b200vs_row_owner(int32_t world, int64_t n, const int64_t* ids, int32_t* out_rank) {
+  return guarded([&]() -> int {
+    if (world < 1 || world > ROUTE_MAX_WORLD || n < 0 || (n > 0 && (!ids || !out_rank)))
+      fail(B200VS_EILLEGAL_PARAMETERS, "bad row_owner arguments (world must be in [1, 1024])");
+    for (int64_t i = 0; i < n; ++i) out_rank[i] = row_owner_of((long long)ids[i], world);
     return B200VS_OK;
   });
 }
@@ -695,7 +976,8 @@ int b200vs_shard_add(b200vs_shard* h, int64_t n, const float* x, const int64_t* 
 // Collective delete (VectorIndexIvfFlat::Delete, vector_index_ivf_flat.cc:162-189, over all shards): every rank passes the same
 // id list and drops the rows it holds; the removed counts are summed over the ranks.  "remove not found vector id" ->
 // EVECTOR_INVALID only when NO rank held any of the ids (:180-184).  Upsert of a sharded index = this call (a not-found
-// status ignored), then b200vs_shard_add*: the new row may live on another rank than the old one.
+// status ignored), then b200vs_shard_add*: the new row may live on another rank than the old one.  Row-sharded FLAT and
+// HNSW follow their single-index rule instead: unknown ids are ignored and the status is OK.
 int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int64_t* n_removed) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
@@ -716,7 +998,7 @@ int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int6
       B200VS_CUDA(cudaStreamSynchronize(sh->ws));
     }
     if (n_removed) *n_removed = tot[0];
-    if (tot[0] == 0 && tot[1] == 0) fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
+    if (!sh->rows && tot[0] == 0 && tot[1] == 0) fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
     return B200VS_OK;
   });
 }
@@ -727,6 +1009,7 @@ int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int6
 int b200vs_shard_plan_add_device(b200vs_shard* h, int64_t n, const float* x_dev) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
     if (n <= 0 || !x_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad plan arguments");
     std::lock_guard<std::mutex> g(sh->add_mu);
     IndexBase* ix = sh->ix;
@@ -750,6 +1033,7 @@ int b200vs_shard_plan_add_device(b200vs_shard* h, int64_t n, const float* x_dev)
 int b200vs_shard_plan_commit(b200vs_shard* h) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
     std::lock_guard<std::mutex> g(sh->add_mu);
     IndexBase* ix = sh->ix;
     ix->set_device();
@@ -785,6 +1069,7 @@ int b200vs_shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const f
     cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
     LaneGuard lane(ix, s);
     ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
+    if (sh->rows) ix->check_row_search(k, sp);
     ix->reset_stats();
     shard_search_stream(sh, *sl.lane, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
     ix->phases_finish(s);
@@ -815,6 +1100,7 @@ int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* x
       s = L.own;
       LaneGuard lane(ix, s);
       ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
+      if (sh->rows) ix->check_row_search(k, sp);
       ix->reset_stats();
       const int64_t per = (nq + W - 1) / W;
       L.q_all.reserve((size_t)per * W * d, 0, s);
@@ -842,7 +1128,7 @@ int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, c
     b200vs_shard* sh = get(h);
     IndexBase* ix = sh->ix;
     SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
-    check_shard_range(nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
+    check_shard_range(ix, nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
     std::shared_lock<std::shared_mutex> rl(ix->rw);
     ix->set_device();
     cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
@@ -866,7 +1152,7 @@ int b200vs_shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const fl
     cudaStream_t s;
     {
       SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
-      check_shard_range(nq, xq, max_results, out_dist, out_ids, out_counts);
+      check_shard_range(ix, nq, xq, max_results, out_dist, out_ids, out_counts);
       std::shared_lock<std::shared_mutex> rl(ix->rw);
       ix->set_device();
       b200vs_shard::SLane& L = *sl.lane;

@@ -885,7 +885,7 @@ tc_final_hybrid_kernel(const unsigned long long* __restrict__ cand, const int* _
     if (rank < kept) {
       const float v = ord2f(s_kd[e]);
       const float raw = L2 ? v : -v;
-      out_dist[(size_t)qi * k + rank] = (L2 || (RANGE && raw_out)) ? raw : __fsub_rn(1.0f, raw);
+      out_dist[(size_t)qi * k + rank] = (L2 || raw_out) ? raw : __fsub_rn(1.0f, raw);
       out_ids[(size_t)qi * k + rank] = s_id[e];
     }
   });
@@ -1124,8 +1124,8 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
 }
 
 // RANGE (tc_range_search): tau holds the range capture threshold, not a sampled one; every captured row is re-scored and
-// the closest k rows whose exact key is below thr_key are kept, as the exact scan keeps them.  out_dist then holds the raw
-// metric value (L2 distance | ip) when raw_out, else the API distance, and out_counts the rows kept.
+// the closest k rows whose exact key is below thr_key are kept, as the exact scan keeps them, and out_counts holds the rows
+// kept.  In either mode out_dist holds the raw metric value (L2 distance | ip) when raw_out, else the API distance.
 template <bool L2, bool RANGE>
 static __global__ void __launch_bounds__(SCAN_THREADS)
 tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cand_cnt, int cap,
@@ -1152,7 +1152,7 @@ tc_final_kernel(const unsigned long long* __restrict__ cand, const int* __restri
     if (i < have) {
       const float v = ord2f(sel.kd[i]);
       const float raw = L2 ? v : -v;
-      api = (L2 || (RANGE && raw_out)) ? raw : __fsub_rn(1.0f, raw);
+      api = (L2 || raw_out) ? raw : __fsub_rn(1.0f, raw);
       id = sel.kid[i];
     }
     out_dist[(size_t)qi * k + i] = api;
@@ -1493,7 +1493,7 @@ static void tc_profile_counts(IndexBase* ix, const int* qcount, const int* total
 }
 
 void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
-               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
+               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, bool raw_out, cudaStream_t s) {
   const int d = ix->dim;
   const int cap = tc_cand_cap(k);
   auto& S = ix->scratch;
@@ -1537,22 +1537,24 @@ void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float*
   ix->phase(IndexBase::PH_FINAL, s);
   const int* fin_redo = nullptr;
   const size_t hsm = (size_t)d * 4;  // the query row
+  const int raw = raw_out ? 1 : 0;
   if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, 0, nullptr);
-    else tc_final_hybrid_kernel<false, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, 0, nullptr);
+    if (l2) tc_final_hybrid_kernel<true, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, raw, nullptr);
+    else tc_final_hybrid_kernel<false, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, raw, nullptr);
     fin_redo = redo;
     ix->launch_count(1);
   }
   const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, 0, nullptr);
-  else tc_final_kernel<false, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, 0, nullptr);
+  if (l2) tc_final_kernel<true, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, raw, nullptr);
+  else tc_final_kernel<false, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, raw, nullptr);
   tc_compact_flags(flags, (int)nq, qmap, qcount, s);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(5);
   ix->stats[1] = nq;
   // 4) uncertified queries re-run on the exact scan (device-side count: blocks beyond it exit immediately)
   ix->phase(IndexBase::PH_FALLBACK, s);
-  run_scan_mapped(ix, tc_exact_job(v, l2, d, probes, nprobe, sc), nq, qmap, qcount, q, k, out_dist, nullptr, out_ids, nullptr, s);
+  run_scan_mapped(ix, tc_exact_job(v, l2, d, probes, nprobe, sc), nq, qmap, qcount, q, k, raw_out ? nullptr : out_dist,
+                  raw_out ? out_dist : nullptr, out_ids, nullptr, s);
   ix->phase(IndexBase::PH_OTHER, s);
   if (ix->profiling && getenv("B200VS_DEBUG_FLAGS")) {
     std::vector<int> hf(nq), hc(nq);

@@ -121,9 +121,10 @@ void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const in
                      int k, float* out_dist, float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s);
 
 // probes: device [nq, nprobe] list indices (for Flat: all zeros, nprobe = 1).  q: device queries, already
-// normalised for cosine.  Writes API-semantics results; uncertified queries are re-run on the exact scan.
+// normalised for cosine.  Writes API-semantics results, or the raw metric value (L2 distance | ip) when raw_out; uncertified
+// queries are re-run on the exact scan.
 void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
-               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s);
+               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, bool raw_out, cudaStream_t s);
 
 // Range mode of the list scan (radius_raw: L2 keeps dist < radius_raw, IP / cosine keep ip > radius_raw).  The capture
 // threshold of each query comes from the radius widened by tc_eps; every captured row is re-scored exactly and the closest

@@ -34,6 +34,7 @@ ABI_SYMBOLS = [
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
+    "b200vs_shard_hnsw_add_batched", "b200vs_row_owner",
 ]
 
 
@@ -141,6 +142,8 @@ def lib():
     L.b200vs_range_search_binary.argtypes = [vp, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_hnsw_add_batched.argtypes = [vp, i64, vp, vp, i32]
     L.b200vs_debug_hnsw_build_scratch_limit.argtypes = [vp, i64]
+    L.b200vs_shard_hnsw_add_batched.argtypes = [vp, i64, vp, vp, i32]
+    L.b200vs_row_owner.argtypes = [i32, i64, vp, vp]
     _lib = L
     return L
 
@@ -415,8 +418,9 @@ class Index:
 
 
 class Shard:
-    """One rank of a list-sharded IVF_FLAT or IVF_PQ index (b200vs_shard_*).  `id_bytes`: the 128-byte rendezvous blob made by
-    Shard.unique_id() on rank 0 and distributed by the host (tests: torch.distributed broadcast)."""
+    """One rank of a sharded index (b200vs_shard_*): IVF_FLAT and IVF_PQ by inverted list, FLAT and HNSW by row (row_owner).
+    `id_bytes`: the 128-byte rendezvous blob made by Shard.unique_id() on rank 0 and distributed by the host (tests:
+    torch.distributed broadcast)."""
 
     @staticmethod
     def unique_id():
@@ -459,6 +463,12 @@ class Shard:
 
     def add_device(self, n, x_dev_ptr, ids_dev_ptr):
         _check(lib().b200vs_shard_add_device(self.h, n, x_dev_ptr, ids_dev_ptr))
+
+    def hnsw_add_batched(self, x, ids, batch=0):
+        """Row-sharded HNSW: add's routing, then the batched GPU build on the rows each rank received."""
+        x, ids = _f32(x), _i64(ids)
+        _check(lib().b200vs_shard_hnsw_add_batched(self.h, ids.size, x.ctypes.data if x.size else None,
+                                                   ids.ctypes.data if ids.size else None, int(batch)))
 
     def delete(self, ids):
         """Collective delete: every rank passes the same ids; returns the rows removed over all ranks."""
@@ -520,6 +530,15 @@ def binary_ivf_state_blob(centroids):
     c = _u8(centroids)
     hdr = np.array([0x42465649, c.shape[0], c.shape[1] * 8, HAMMING], dtype=np.int64)
     return np.concatenate([hdr.view(np.uint8), c.reshape(-1)])
+
+
+def row_owner(ids, world):
+    """Owner rank of each id of a row-sharded FLAT / HNSW index of `world` ranks (b200vs_row_owner; numpy mirror:
+    b200vs.shard.row_owner)."""
+    ids = _i64(ids)
+    out = np.zeros(ids.size, dtype=np.int32)
+    _check(lib().b200vs_row_owner(int(world), ids.size, ids.ctypes.data if ids.size else None, out.ctypes.data if out.size else None))
+    return out.reshape(ids.shape)
 
 
 def merge_topk_device(device, nparts, nq, k, parts_dist_ptr, parts_ids_ptr, out_dist_ptr, out_ids_ptr, stream=None):

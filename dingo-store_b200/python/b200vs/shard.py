@@ -19,6 +19,19 @@ def split_rows_by_owner(list_ids, nlist_per_rank, world):
     return order, counts
 
 
+def row_owner(ids, world):
+    """Owner rank of each id of a row-sharded FLAT / HNSW index: splitmix64's finalizer of the id read as a uint64, mod world
+    (the rule b200vs_row_owner and the device routing apply)."""
+    z = np.asarray(ids, dtype=np.int64).view(np.uint64).copy()
+    with np.errstate(over="ignore"):
+        z ^= z >> np.uint64(30)
+        z *= np.uint64(0xbf58476d1ce4e5b9)
+        z ^= z >> np.uint64(27)
+        z *= np.uint64(0x94d049bb133111eb)
+        z ^= z >> np.uint64(31)
+    return (z % np.uint64(world)).astype(np.int32)
+
+
 def merge_topk(parts_dist, parts_ids, k):
     """parts_*: [nparts, nq, k] API-semantics distances ascending, id -1 padded -> merged [nq, k]."""
     parts_dist = np.asarray(parts_dist, dtype=np.float32)

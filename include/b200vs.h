@@ -243,7 +243,32 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  *                     seq = batch sequence number: 0, 1, 2, ... the same on every rank, each used exactly once.  Batches are
  *                     enqueued in seq order on every rank (concurrent caller threads simply take turns; the GPU work of
  *                     up to `lanes` batches still overlaps), batch seq uses communicator seq % lanes.  seq < 0 = "next in
- *                     call order" for single-threaded callers.  Results equal b200vs_search on the unsharded index. */
+ *                     call order" for single-threaded callers.  Results equal b200vs_search on the unsharded index.
+ *
+ * Row-sharded FLAT and HNSW (DESIGN.md 4.5): the same entry points serve one logical FLAT or HNSW index.  A row belongs to
+ * rank b200vs_row_owner(id) = splitmix64(id) mod world, so an upsert or a delete always meets the existing row on its owner,
+ * and each rank's index keeps its type's single-index semantics.  On such a shard:
+ *   shard_create    : accepts an EMPTY FLAT or HNSW index (a non-empty one: EVECTOR_NOT_SUPPORT); world <= 1024
+ *   shard_train     : OK, nothing to do (as b200vs_train on FLAT and HNSW)
+ *   shard_broadcast_state, shard_list_range, shard_plan_add_device, shard_plan_commit : EVECTOR_NOT_SUPPORT (no lists, and an
+ *                     HNSW state is a whole graph)
+ *   shard_add[_device] : every row travels raw to its owner, partitioned on the device; an owner receives rank 0's rows first,
+ *                     then rank 1's, ..., each in its caller's order, and runs b200vs_add_with_ids on them in that order.
+ *                     Before any index changes, every owner checks what it received (FLAT: an id repeated anywhere in the
+ *                     collective call -> EVECTOR_ID_DUPLICATED; HNSW: more rows than max_elements -> EINTERNAL, and for
+ *                     shard_hnsw_add_batched the batched builder's refusals for the rows received); every rank
+ *                     then returns the same status and a refused call changes no rank's index
+ *   shard_hnsw_add_batched : HNSW only; shard_add's routing, then b200vs_hnsw_add_batched(batch) on the received rows
+ *   shard_remove_ids : unknown ids are ignored and the status is OK, as b200vs_remove_ids on FLAT and HNSW
+ *   shard_search[_device] : no coarse step: the rank searches its own index with the whole batch (FLAT: b200vs_search's paths,
+ *                     keyed on L2 distance | -ip, the API distance formed after the merge; HNSW: the graph walk with sp's
+ *                     efsearch and filters, keyed on its own distance).  FLAT results equal b200vs_search on one index of all
+ *                     rows bit for bit; HNSW results equal the merge of b200vs_search on every rank's graph.  Refused on
+ *                     every rank before the first collective, from the arguments alone: HNSW efsearch outside [0, 1024]
+ *                     (as b200vs_search) and a walk (max(efsearch or the index's current ef, k)) beyond the search
+ *                     kernel's shared memory, also when this rank's graph is still empty; the refused efsearch is not kept.
+ *   shard_range_search[_device] : FLAT: b200vs_range_search's rule, equal bit for bit.  HNSW: EVECTOR_NOT_SUPPORT on every
+ *                     rank before the first collective (the sequence number is still used up). */
 #define B200VS_SHARD_ID_BYTES 128
 typedef struct b200vs_shard b200vs_shard;
 int b200vs_shard_unique_id(uint8_t id[B200VS_SHARD_ID_BYTES]);
@@ -256,9 +281,15 @@ int b200vs_shard_broadcast_state(b200vs_shard* shard, int32_t root);
 int b200vs_shard_add(b200vs_shard* shard, int64_t n, const float* x, const int64_t* ids);
 int b200vs_shard_add_device(b200vs_shard* shard, int64_t n, const float* x_dev, const int64_t* ids_dev);
 /* collective Delete: every rank passes the same ids; *n_removed = rows removed over all ranks; EVECTOR_INVALID when no rank held
- * any of them (vector_index_ivf_flat.cc:180-184).  shard_add* appends (IndexIVFFlat::add_with_ids); an Upsert is this call (a
- * not-found status ignored) followed by shard_add*. */
+ * any of them (vector_index_ivf_flat.cc:180-184; row-sharded FLAT / HNSW: OK).  shard_add* appends
+ * (IndexIVFFlat::add_with_ids); an Upsert is this call (a not-found status ignored) followed by shard_add*. */
 int b200vs_shard_remove_ids(b200vs_shard* shard, int64_t n, const int64_t* ids, int64_t* n_removed);
+/* collective batched HNSW build of a row-sharded HNSW index (see above); batch as b200vs_hnsw_add_batched */
+int b200vs_shard_hnsw_add_batched(b200vs_shard* shard, int64_t n, const float* x, const int64_t* ids, int32_t batch);
+/* owner rank of each id in a row-sharded index of `world` ranks: splitmix64's finalizer of the id read as a uint64, mod world
+ * (z ^= z >> 30; z *= 0xbf58476d1ce4e5b9; z ^= z >> 27; z *= 0x94d049bb133111eb; z ^= z >> 31); world in [1, 1024].  A pure
+ * host function: no handle, no GPU.  Callers place rows on their owner so that shard_add moves nothing. */
+int b200vs_row_owner(int32_t world, int64_t n, const int64_t* ids, int32_t* out_rank);
 int b200vs_shard_plan_add_device(b200vs_shard* shard, int64_t n, const float* x_dev);
 int b200vs_shard_plan_commit(b200vs_shard* shard);
 int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
