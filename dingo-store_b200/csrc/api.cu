@@ -17,49 +17,7 @@ using namespace b200vs;
 
 namespace {
 
-template <class F>
-int guarded(F&& f) {
-  try {
-    return f();
-  } catch (const StatusError& e) {
-    g_last_error = e.msg;
-    return e.code;
-  } catch (const CudaError& e) {
-    g_last_error = e.what();
-    return B200VS_EINTERNAL;
-  } catch (const std::bad_alloc&) {
-    g_last_error = "out of host memory";
-    return B200VS_EINTERNAL;
-  } catch (const std::exception& e) {
-    g_last_error = e.what();
-    return B200VS_EINTERNAL;
-  } catch (...) {
-    g_last_error = "unknown error";
-    return B200VS_EINTERNAL;
-  }
-}
-
 IndexBase* get(b200vs_index* h) { return index_impl(h); }
-
-// resolve search params; uploads the sorted id list into scratch (stream-ordered)
-SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s) {
-  SearchCtx sc;
-  if (!sp) return sc;
-  sc.nprobe = sp->nprobe;
-  sc.efsearch = sp->efsearch;
-  sc.exact_only = sp->exact_only;
-  sc.has_range = sp->has_range;
-  sc.negate = sp->negate;
-  sc.rmin = sp->range_min;
-  sc.rmax = sp->range_max;
-  if (sp->sorted_ids) {
-    long long* d = ix->scratch.alloc<long long>((size_t)std::max<int64_t>(sp->n_ids, 1));
-    if (sp->n_ids > 0) B200VS_CUDA(cudaMemcpyAsync(d, sp->sorted_ids, (size_t)sp->n_ids * 8, cudaMemcpyHostToDevice, s));
-    sc.sorted_ids_dev = d;
-    sc.n_ids = sp->n_ids;
-  }
-  return sc;
-}
 
 // the float entry points (train / add / search / range search) on a binary index, and the binary ones on a float index
 void check_row_type(IndexBase* ix, bool binary_call) {

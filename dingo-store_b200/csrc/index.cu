@@ -94,6 +94,25 @@ IndexBase::~IndexBase() {
   }
 }
 
+SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s) {
+  SearchCtx sc;
+  if (!sp) return sc;
+  sc.nprobe = sp->nprobe;
+  sc.efsearch = sp->efsearch;
+  sc.exact_only = sp->exact_only;
+  sc.has_range = sp->has_range;
+  sc.negate = sp->negate;
+  sc.rmin = sp->range_min;
+  sc.rmax = sp->range_max;
+  if (sp->sorted_ids) {
+    long long* d = ix->scratch.alloc<long long>((size_t)std::max<int64_t>(sp->n_ids, 1));
+    if (sp->n_ids > 0) B200VS_CUDA(cudaMemcpyAsync(d, sp->sorted_ids, (size_t)sp->n_ids * 8, cudaMemcpyHostToDevice, s));
+    sc.sorted_ids_dev = d;
+    sc.n_ids = sp->n_ids;
+  }
+  return sc;
+}
+
 const float* IndexBase::prepare_queries(int64_t nq, const float* xq_dev, cudaStream_t s) {
   if (metric != B200VS_COSINE) return xq_dev;
   float* q = scratch.alloc<float>((size_t)nq * dim);
@@ -603,13 +622,18 @@ struct IvfFlatIndex : IndexBase {
   }
 
   // trained-state blob: int64 hdr[4] = {magic 'IVFC', nlist, dim, metric}; float centroids[nlist*dim]
+  static constexpr int64_t kStateMagic = 0x43465649;
+  void state_header(void* blob, int k) const {
+    const int64_t hdr[4] = {kStateMagic, k, dim, (int64_t)metric};
+    memcpy(blob, hdr, 32);
+  }
   void set_state(const void* blob, size_t len) override {
     std::unique_lock<std::shared_mutex> wl(rw);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     if (len < 32) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
-    if (hdr[0] != 0x43465649 || hdr[2] != dim) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF state blob");
+    if (hdr[0] != kStateMagic || hdr[2] != dim) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF state blob");
     const int k = (int)hdr[1];
     if (len < 32 + (size_t)k * dim * 4) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
     install_centroids((const float*)((const char*)blob + 32), k);
@@ -620,8 +644,7 @@ struct IvfFlatIndex : IndexBase {
     const size_t need = 32 + (size_t)nlist * dim * 4;
     if (!blob || cap < need) return (int64_t)need;
     set_device();
-    int64_t hdr[4] = {0x43465649, nlist, dim, (int64_t)metric};
-    memcpy(blob, hdr, 32);
+    state_header(blob, nlist);
     B200VS_CUDA(cudaMemcpy((char*)blob + 32, centroids.p, (size_t)nlist * dim * 4, cudaMemcpyDeviceToHost));
     return (int64_t)need;
   }
@@ -1007,5 +1030,27 @@ int64_t IvfFlatIndex::copy_list(int list, int64_t cap, float* vectors, int64_t* 
 }
 
 IndexBase* make_ivf_flat(b200vs_metric m, int d, const b200vs_params& p) { return new IvfFlatIndex(m, d, p); }
+
+static IvfFlatIndex* as_ivf_flat(IndexBase* ix) {
+  auto* p = dynamic_cast<IvfFlatIndex*>(ix);
+  if (!p) fail(B200VS_EINTERNAL, "not an IVF_FLAT index");
+  return p;
+}
+
+void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent) {
+  b200vs_params p = as_ivf_flat(ix)->params;
+  p.nlist = k;
+  IvfFlatIndex loc(ix->metric, ix->dim, p);  // train on an index of its own: ix keeps its state and lists
+  loc.train(n, x);
+  cent.resize((size_t)loc.nlist * loc.dim);
+  B200VS_CUDA(cudaMemcpy(cent.data(), loc.centroids.p, cent.size() * 4, cudaMemcpyDeviceToHost));
+}
+
+void ivf_flat_train_state(IndexBase* ix, const std::vector<float>& cent, std::vector<unsigned char>& blob) {
+  const IvfFlatIndex* f = as_ivf_flat(ix);
+  blob.resize(32 + cent.size() * 4);
+  f->state_header(blob.data(), (int)(cent.size() / f->dim));
+  memcpy(blob.data() + 32, cent.data(), cent.size() * 4);
+}
 
 }  // namespace b200vs

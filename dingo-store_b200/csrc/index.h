@@ -12,6 +12,7 @@
 #include <cstdint>
 #include <cstring>
 #include <mutex>
+#include <new>
 #include <shared_mutex>
 #include <string>
 #include <unordered_map>
@@ -28,6 +29,30 @@ struct StatusError {
   std::string msg;
 };
 [[noreturn]] inline void fail(int code, const std::string& m) { throw StatusError{code, m}; }
+
+// The body of every extern "C" entry point: no exception leaves the library, each failure becomes a b200vs_status and
+// b200vs_last_error's text.
+template <class F>
+int guarded(F&& f) {
+  try {
+    return f();
+  } catch (const StatusError& e) {
+    g_last_error = e.msg;
+    return e.code;
+  } catch (const CudaError& e) {
+    g_last_error = e.what();
+    return B200VS_EINTERNAL;
+  } catch (const std::bad_alloc&) {
+    g_last_error = "out of host memory";
+    return B200VS_EINTERNAL;
+  } catch (const std::exception& e) {
+    g_last_error = e.what();
+    return B200VS_EINTERNAL;
+  } catch (...) {
+    g_last_error = "unknown error";
+    return B200VS_EINTERNAL;
+  }
+}
 
 template <class T>
 struct DevBuf {
@@ -152,6 +177,9 @@ struct SearchCtx {  // resolved per-search parameters, device filter included
   long long n_ids = 0;
   bool has_filter() const { return has_range || sorted_ids_dev; }
 };
+struct IndexBase;
+// resolve search params; uploads the sorted id list into the calling lane's scratch (stream-ordered on s)
+SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s);
 
 struct IndexBase {
   b200vs_type type;
@@ -405,6 +433,10 @@ IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p);
 int ivf_pq_ksub(IndexBase* ix);
 void ivf_pq_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent);
 void ivf_pq_train_state(IndexBase* ix, int64_t n, const float* x, const std::vector<float>& cent, std::vector<unsigned char>& blob);
+// The same two stages for IVF_FLAT (index.cu); ix must be an IVF_FLAT index, which stays untouched.  Coarse: train's k
+// centroids of n >= k raw rows.  State: the trained-state blob of the centroids cent [nlist, dim].
+void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent);
+void ivf_flat_train_state(IndexBase* ix, const std::vector<float>& cent, std::vector<unsigned char>& blob);
 IndexBase* make_binary_flat(int d, const b200vs_params& p);
 IndexBase* make_binary_ivf(int d, const b200vs_params& p);
 

@@ -9,9 +9,11 @@
 //      coarse value of every probe recomputed on the rank, csrc/ivf_pq.cu) -> exact local top-k;
 //   3. ONE ncclAllGather of the packed per-shard top-k ((distance, id) 16-byte records) over NVLink, then the k-way merge
 //      kernel — the engine's analogue of VectorIndexWrapper::MergeSearchResults (src/vector/vector_index.cc:1056-1108).
-// Rows are routed to their list owner at add time (b200vs_shard_add*: assignment on the sender, grouped ncclSend/ncclRecv).
 // FLAT and HNSW shard by row instead (DESIGN.md 4.5): row id lives on rank row_owner_of(id), each rank holds a standalone
 // index of its rows, and a search skips step 1 and runs the whole batch on the rank's index before the same all-gather + merge.
+// Both kinds share one write path: b200vs_shard_add* partitions the rows by owner on the device (list-sharded: the owner of
+// the list the sender assigns the row to), moves them with one grouped ncclSend/ncclRecv, and every rank returns the first
+// refusal in rank order or adds.  A world of one runs the same code with only the NCCL calls left out.
 //
 // NCCL is resolved at run time (dlopen of libnccl.so.2): a single-GPU dingo-store node needs no NCCL at all, and a process
 // that already carries an NCCL (e.g. the one bundled with PyTorch in the test harness) shares it.  Each in-flight lane owns
@@ -172,20 +174,6 @@ static __global__ void fill_ll_kernel(long long* p, long long n, long long v) {
   if (i < n) p[i] = v;
 }
 
-// gather rows by a permutation: dst[i] = src[perm[i]]  (rows, ids, lists)
-static __global__ void gather_rows_kernel(const float* __restrict__ x, const long long* __restrict__ ids, const long long* __restrict__ lists,
-                                          const long long* __restrict__ perm, long long n, int d, float* ox, long long* oids, long long* olists) {
-  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (w >= n) return;
-  const long long src = perm[w];
-  const float4* s4 = reinterpret_cast<const float4*>(x + (size_t)src * d);
-  float4* d4 = reinterpret_cast<float4*>(ox + (size_t)w * d);
-  if ((d & 3) == 0) for (int i = lane; i < (d >> 2); i += 32) d4[i] = s4[i];
-  else for (int i = lane; i < d; i += 32) ox[(size_t)w * d + i] = x[(size_t)src * d + i];
-  if (lane == 0) { oids[w] = ids[src]; olists[w] = lists[src]; }
-}
-
 static __global__ void count_lists_kernel(const long long* __restrict__ lists, long long n, int nlist, unsigned long long* counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { const long long l = lists[i]; if (l >= 0 && l < nlist) atomicAdd(counts + l, 1ULL); }
@@ -197,7 +185,7 @@ static __global__ void ip_key_to_api_kernel(float* dist, const long long* __rest
   if (i < n && ids[i] >= 0) dist[i] = __fsub_rn(1.0f, -dist[i]);
 }
 
-constexpr int ROUTE_MAX_WORLD = 1024;  // ranks of a row-sharded index
+constexpr int ROUTE_MAX_WORLD = 1024;  // ranks of a sharded index (the routing kernels' shared-memory table)
 
 // The owner of a row of a row-sharded (FLAT / HNSW) index: splitmix64's finalizer of the id read as a uint64, mod world.
 // The one definition for the host (b200vs_row_owner) and the device (row routing).  z mod world is taken 16 bits at a
@@ -224,13 +212,26 @@ __host__ __device__ __forceinline__ int row_owner_of(long long id, int world) {
 constexpr int ROUTE_THREADS = 256, ROUTE_WARPS = ROUTE_THREADS / 32;  // s_cnt below: ROUTE_WARPS * world ints of shared memory
 constexpr int ROUTE_SCAN_THREADS = 1024;
 
+// The owner rules of the routing kernels, applied to a row's key.  Row-sharded: the key is the id.  List-sharded: the key is
+// the row's inverted list, which travels with the row; rank r owns the lists [r * per, (r + 1) * per), per = ceil(nlist / W).
+struct RowOwner {
+  static constexpr bool kLists = false;
+  __device__ __forceinline__ int operator()(long long id, int W) const { return row_owner_of(id, W); }
+};
+struct ListOwner {
+  static constexpr bool kLists = true;
+  int per;
+  __device__ __forceinline__ int operator()(long long list, int) const { return (int)list / per; }
+};
+
 // This thread's row of the tile: returns (its owner, -1 past n; the rows of that owner before it in its warp), and
 // s_cnt[warp * W + owner] = the warp's rows of that owner.
-static __device__ __forceinline__ int2 route_tile(const long long* __restrict__ ids, long long n, int W, int* s_cnt) {
+template <class Owner>
+static __device__ __forceinline__ int2 route_tile(const long long* __restrict__ keys, long long n, int W, Owner owner, int* s_cnt) {
   for (int i = threadIdx.x; i < ROUTE_WARPS * W; i += ROUTE_THREADS) s_cnt[i] = 0;
   __syncthreads();
   const long long i = (long long)blockIdx.x * ROUTE_THREADS + threadIdx.x;
-  const int o = i < n ? row_owner_of(ids[i], W) : -1;
+  const int o = i < n ? owner(keys[i], W) : -1;
   const unsigned peers = __match_any_sync(0xffffffffu, o);
   const int lane = threadIdx.x & 31;
   if (o >= 0 && __ffs(peers) - 1 == lane) s_cnt[(threadIdx.x >> 5) * W + o] = __popc(peers);
@@ -238,9 +239,10 @@ static __device__ __forceinline__ int2 route_tile(const long long* __restrict__ 
   return make_int2(o, __popc(peers & ((1u << lane) - 1u)));
 }
 
-static __global__ void __launch_bounds__(ROUTE_THREADS) route_count_kernel(const long long* __restrict__ ids, long long n, int W, int* cnt) {
+template <class Owner>
+static __global__ void __launch_bounds__(ROUTE_THREADS) route_count_kernel(const long long* __restrict__ keys, long long n, int W, Owner owner, int* cnt) {
   extern __shared__ int s_cnt[];
-  route_tile(ids, n, W, s_cnt);
+  route_tile(keys, n, W, owner, s_cnt);
   for (int o = threadIdx.x; o < W; o += ROUTE_THREADS) {
     int c = 0;
     for (int w = 0; w < ROUTE_WARPS; ++w) c += s_cnt[w * W + o];
@@ -286,12 +288,14 @@ route_offsets_kernel(const int* __restrict__ cnt, long long ntiles, int W, long 
     owner_cnt[o] = (o + 1 < W ? off[(o + 1) * ntiles] : s_carry) - off[o * ntiles];
 }
 
+// moves rows, ids and (Owner::kLists) lists to their slots
+template <class Owner>
 static __global__ void __launch_bounds__(ROUTE_THREADS)
-route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ ids, long long n, int d, int W,
-                     const long long* __restrict__ off, float* ox, long long* oids) {
+route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ ids, const long long* __restrict__ lists, long long n, int d,
+                     int W, Owner owner, const long long* __restrict__ off, float* ox, long long* oids, long long* olists) {
   extern __shared__ int s_cnt[];
   __shared__ long long s_dst[ROUTE_THREADS];
-  const int2 t = route_tile(ids, n, W, s_cnt);
+  const int2 t = route_tile(Owner::kLists ? lists : ids, n, W, owner, s_cnt);
   const int o = t.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (o >= 0) {
     long long p = off[(size_t)o * gridDim.x + blockIdx.x] + t.y;
@@ -311,7 +315,10 @@ route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ 
     } else {
       for (int i = lane; i < d; i += 32) xd[i] = xs[i];
     }
-    if (lane == 0) oids[dst] = ids[src];
+    if (lane == 0) {
+      oids[dst] = ids[src];
+      if (Owner::kLists) olists[dst] = lists[src];
+    }
   }
 }
 
@@ -363,25 +370,6 @@ struct b200vs_shard {
 
 namespace {
 
-template <class F>
-int guarded(F&& f) {
-  try {
-    return f();
-  } catch (const StatusError& e) {
-    g_last_error = e.msg;
-    return e.code;
-  } catch (const CudaError& e) {
-    g_last_error = e.what();
-    return B200VS_EINTERNAL;
-  } catch (const std::exception& e) {
-    g_last_error = e.what();
-    return B200VS_EINTERNAL;
-  } catch (...) {
-    g_last_error = "unknown error";
-    return B200VS_EINTERNAL;
-  }
-}
-
 b200vs_shard* get(b200vs_shard* s) {
   if (!s || !s->ix) fail(B200VS_EILLEGAL_PARAMETERS, "null shard handle");
   return s;
@@ -415,17 +403,19 @@ struct SeqLane {
   }
 };
 
-SearchCtx make_ctx_shard(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s) {
-  SearchCtx sc;
-  if (!sp) return sc;
-  sc.nprobe = sp->nprobe; sc.efsearch = sp->efsearch; sc.exact_only = sp->exact_only;
-  sc.has_range = sp->has_range; sc.negate = sp->negate; sc.rmin = sp->range_min; sc.rmax = sp->range_max;
-  if (sp->sorted_ids) {
-    long long* d = ix->scratch.alloc<long long>((size_t)std::max<int64_t>(sp->n_ids, 1));
-    if (sp->n_ids > 0) B200VS_CUDA(cudaMemcpyAsync(d, sp->sorted_ids, (size_t)sp->n_ids * 8, cudaMemcpyHostToDevice, s));
-    sc.sorted_ids_dev = d; sc.n_ids = sp->n_ids;
-  }
-  return sc;
+// All-gathers `count` host values of every rank through the write stream: returns [world, count], rank r's at r * count.
+template <class T>
+std::vector<T> all_gather_host(b200vs_shard* sh, const T* mine, size_t count = 1) {
+  const int W = sh->world;
+  std::vector<T> all((size_t)W * count);
+  DevBuf<T> buf;
+  buf.reserve((size_t)W * count, 0, sh->ws);
+  T* slot = buf.p + (size_t)sh->rank * count;
+  B200VS_CUDA(cudaMemcpyAsync(slot, mine, count * sizeof(T), cudaMemcpyHostToDevice, sh->ws));
+  if (W > 1) B200VS_NCCL(nccl().AllGather(slot, buf.p, count * sizeof(T), ncclUint8, sh->lanes[0]->comm, sh->ws));
+  B200VS_CUDA(cudaMemcpyAsync(all.data(), buf.p, all.size() * sizeof(T), cudaMemcpyDeviceToHost, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  return all;
 }
 
 // The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
@@ -438,7 +428,7 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
   IndexBase* ix = sh->ix;
   const int W = sh->world, r = sh->rank, d = ix->dim;
   if (L.last && L.last != s && L.done) B200VS_CUDA(cudaStreamWaitEvent(s, L.done, 0));
-  SearchCtx sc = make_ctx_shard(ix, sp, s);
+  SearchCtx sc = make_ctx(ix, sp, s);
   const float* q = xq;
   int nprobe = 0;
   if (!sh->rows) {
@@ -507,6 +497,7 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
     B200VS_CUDA(cudaGetLastError());
     ix->launch_count(1);
   }
+  ix->phases_finish(s);
 }
 
 // range: the local range scan keyed on the single-index select's key (L2 distance | -ip) — two distinct inner products can
@@ -528,28 +519,71 @@ void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, co
   range_finish_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(out_dist, out_ids, nq, max_results, l2 ? 1 : 0, out_counts);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(1);
+  ix->phases_finish(s);
 }
 
-// refusals of a sharded range search, decided from its arguments alone so that every rank refuses before the first collective
-void check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
+// Refusals of a sharded read decided from its arguments alone, so that every rank refuses alike.  Top-k: false = k <= 0,
+// nothing to do.
+bool check_shard_topk(int64_t nq, const void* xq, int k, const void* od, const void* oi) {
+  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+  if (k <= 0) return false;
+  if (!od || !oi) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+  return true;
+}
+bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
   if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // as b200vs_range_search
   if (max_results <= 0 || max_results > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
   if (!od || !oi || !oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
+  return true;
 }
 
-// Replicate rank `root`'s trained state on every rank (b200vs_shard_broadcast_state; the caller holds add_mu).
+// One sharded read (k = results per query).  The turn of batch `seq` comes first, so that every call uses its sequence
+// number exactly once, a refused one included; then `refuse` (false: OK, nothing to do), the rw lock, the device and a lane
+// on `stream` (null: the lane's own stream), the refusals every rank meets alike before the first collective, and
+// body(lane, s).  The lane is released before the host waits for a null-stream call, so the lane's next batch may be
+// enqueued behind this one.
+template <class Refuse, class Body>
+void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, const b200vs_search_params* sp, Refuse refuse, Body body) {
+  IndexBase* ix = sh->ix;
+  cudaStream_t s;
+  {
+    SeqLane sl(sh, seq);
+    if (!refuse()) return;
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    ix->set_device();
+    s = stream ? (cudaStream_t)stream : sl.lane->own;
+    LaneGuard lane(ix, s);
+    ix->check_probe_search(nq, k);
+    if (sh->rows) ix->check_row_search(k, sp);
+    ix->reset_stats();
+    body(*sl.lane, s);
+  }
+  if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));
+}
+
+// The host-pointer reads: every rank passes the SAME batch; each rank uploads only its slice and the slices are all-gathered
+// over NVLink, so the PCIe traffic per rank does not grow with the world size.  Returns the batch on the device.
+const float* upload_batch(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, cudaStream_t s) {
+  const int W = sh->world, r = sh->rank, d = sh->ix->dim;
+  const int64_t per = (nq + W - 1) / W;
+  L.q_all.reserve((size_t)per * W * d, 0, s);
+  const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
+  float* mine = L.q_all.p + (size_t)per * r * d;
+  if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, xq + (size_t)q0 * d, (size_t)(q1 - q0) * d * 4, cudaMemcpyHostToDevice, s));
+  if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * d, 0, (size_t)(per - (q1 - q0)) * d * 4, s));
+  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * d, ncclFloat, L.comm, s));
+  return L.q_all.p;
+}
+
+// Replicate rank `root`'s trained state on every rank (b200vs_shard_broadcast_state; the caller holds add_mu).  The length
+// goes first, 0 when the root has no state, so that every rank refuses together.
 void broadcast_state_locked(b200vs_shard* sh, int root) {
   IndexBase* ix = sh->ix;
   ix->set_device();
-  DevBuf<long long> len;
-  len.reserve(1, 0, sh->ws);
-  long long need = sh->rank == root ? (long long)ix->get_state(nullptr, 0) : 0;
-  if (sh->rank == root && need <= 0) fail(B200VS_EVECTOR_NOT_TRAIN, "root has no trained state");
-  B200VS_CUDA(cudaMemcpyAsync(len.p, &need, 8, cudaMemcpyHostToDevice, sh->ws));
-  if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(len.p, len.p, 1, ncclInt64, root, sh->lanes[0]->comm, sh->ws));
-  B200VS_CUDA(cudaMemcpyAsync(&need, len.p, 8, cudaMemcpyDeviceToHost, sh->ws));
-  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  const long long mine = sh->rank == root ? (long long)ix->get_state(nullptr, 0) : 0;
+  const long long need = all_gather_host(sh, &mine)[root];
+  if (need <= 0) fail(B200VS_EVECTOR_NOT_TRAIN, "root has no trained state");
   std::vector<unsigned char> blob((size_t)need);
   if (sh->rank == root) ix->get_state(blob.data(), blob.size());
   DevBuf<unsigned char> db;
@@ -565,43 +599,37 @@ void broadcast_state_locked(b200vs_shard* sh, int root) {
   }
 }
 
-// b200vs_shard_train on IVF_PQ.  The per-rank row counts are exchanged first, so that a refusal for too few rows happens on
-// every rank at once.  Coarse stage: each rank clusters its rows into nlist / world centroids with the k-means of IVF-PQ's
-// own train (exact assignment), one all-gather.  PQ stage: rank 0 trains the codebooks with train's PQ rule on the
-// residuals of its rows to the global centroids, and the state broadcast replicates the result.  At world = 1 this is
-// b200vs_train step for step, so the trained state is byte-equal.
-void shard_train_pq(b200vs_shard* sh, int64_t n, const float* x) {
+// b200vs_shard_train on IVF_FLAT and IVF_PQ.  The per-rank row counts are exchanged first, so that a refusal for too few
+// rows happens on every rank at once.  Coarse stage: each rank clusters its rows into nlist / world centroids with the k-means
+// of its type's own train, one all-gather.  IVF_FLAT: every rank installs the gathered centroids.  IVF_PQ: rank 0 trains the
+// codebooks with train's PQ rule on the residuals of its rows to the global centroids, and the state broadcast replicates
+// the result.  At world = 1 this is b200vs_train step for step, so the trained state is byte-equal.
+void shard_train_locked(b200vs_shard* sh, int64_t n, const float* x) {
   IndexBase* ix = sh->ix;
-  std::lock_guard<std::mutex> g(sh->add_mu);
-  const int W = sh->world, d = ix->dim, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
+  const bool pq = ix->type == B200VS_IVF_PQ;
+  const int W = sh->world, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
   if (nlist % W != 0) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: nlist must be a multiple of the world size");
-  if (ix->sub_type() == B200VS_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode has no inverted lists to shard");
+  if (pq && ix->sub_type() == B200VS_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode has no inverted lists to shard");
   const int nl = nlist / W;
-  const long long pq_rows = 256LL * ivf_pq_ksub(ix);
   ix->set_device();
-  std::vector<long long> counts((size_t)W, (n > 0 && !x) ? -1 : (long long)n);  // rows of every rank (a null x counts as none)
-  if (W > 1) {
-    DevBuf<long long> dc;
-    dc.reserve((size_t)W, 0, sh->ws);
-    B200VS_CUDA(cudaMemcpyAsync(dc.p + sh->rank, &counts[sh->rank], 8, cudaMemcpyHostToDevice, sh->ws));
-    B200VS_NCCL(nccl().AllGather(dc.p + sh->rank, dc.p, 1, ncclInt64, sh->lanes[0]->comm, sh->ws));
-    B200VS_CUDA(cudaMemcpyAsync(counts.data(), dc.p, (size_t)W * 8, cudaMemcpyDeviceToHost, sh->ws));
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-  }
+  const long long rows = x ? (long long)n : 0;  // a null x counts as none
+  const std::vector<long long> counts = all_gather_host(sh, &rows);
   for (int r = 0; r < W; ++r)
     if (counts[r] < nl)
       fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank " + std::to_string(r) + " has fewer training rows than nlist / world centroids");
-  if (counts[0] < pq_rows) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank 0 needs 256 * 2^nbits training rows for the PQ codebooks");
-  std::vector<float> local, cent((size_t)nlist * d);
-  ivf_pq_train_coarse(ix, n, x, nl, local);
-  DevBuf<float> all;
-  all.reserve((size_t)nlist * d, 0, sh->ws);
-  B200VS_CUDA(cudaMemcpyAsync(all.p + (size_t)sh->rank * nl * d, local.data(), (size_t)nl * d * 4, cudaMemcpyHostToDevice, sh->ws));
-  if (W > 1) B200VS_NCCL(nccl().AllGather(all.p + (size_t)sh->rank * nl * d, all.p, (size_t)nl * d, ncclFloat, sh->lanes[0]->comm, sh->ws));
-  B200VS_CUDA(cudaMemcpyAsync(cent.data(), all.p, (size_t)nlist * d * 4, cudaMemcpyDeviceToHost, sh->ws));
-  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  if (pq && counts[0] < 256LL * ivf_pq_ksub(ix))
+    fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank 0 needs 256 * 2^nbits training rows for the PQ codebooks");
+  std::vector<float> local;
+  if (pq) ivf_pq_train_coarse(ix, n, x, nl, local);
+  else ivf_flat_train_coarse(ix, n, x, nl, local);
+  const std::vector<float> cent = all_gather_host(sh, local.data(), local.size());
+  std::vector<unsigned char> blob;
+  if (!pq) {
+    ivf_flat_train_state(ix, cent, blob);
+    ix->set_state(blob.data(), blob.size());
+    return;
+  }
   if (sh->rank == 0) {
-    std::vector<unsigned char> blob;
     ivf_pq_train_state(ix, n, x, cent, blob);
     ix->set_state(blob.data(), blob.size());
   }
@@ -637,7 +665,7 @@ int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const ui
     if (rows && ix->count() + ix->deleted_count() > 0)
       fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index must be empty when its shard is created");
     if (world < 1 || rank < 0 || rank >= world) fail(B200VS_EILLEGAL_PARAMETERS, "bad rank / world");
-    if (rows && world > ROUTE_MAX_WORLD) fail(B200VS_EILLEGAL_PARAMETERS, "row sharding supports at most 1024 ranks");
+    if (world > ROUTE_MAX_WORLD) fail(B200VS_EILLEGAL_PARAMETERS, "sharding supports at most 1024 ranks");
     if (world > 1 && !id) fail(B200VS_EILLEGAL_PARAMETERS, "null communicator id");
     lanes = std::max(1, std::min(lanes <= 0 ? 2 : lanes, kLanes));
     std::unique_ptr<b200vs_shard> sh(new b200vs_shard());
@@ -680,36 +708,9 @@ int b200vs_shard_list_range(b200vs_shard* h, int32_t rank, int32_t* begin, int32
 int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
     if (sh->rows) return B200VS_OK;  // FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
-    if (ix->type == B200VS_IVF_PQ) {
-      shard_train_pq(sh, n, x);
-      return B200VS_OK;
-    }
-    if (n <= 0 || !x) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
     std::lock_guard<std::mutex> g(sh->add_mu);
-    const int W = sh->world, d = ix->dim, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
-    if (nlist % W != 0) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: nlist must be a multiple of the world size");
-    const int nl = nlist / W;
-    b200vs_params p = ix->params;
-    p.nlist = nl;
-    std::unique_ptr<IndexBase> loc(make_ivf_flat(ix->metric, d, p));
-    loc->train(n, x);
-    std::vector<unsigned char> blob((size_t)loc->get_state(nullptr, 0));
-    loc->get_state(blob.data(), blob.size());
-    const int64_t* hdr = reinterpret_cast<const int64_t*>(blob.data());
-    if ((int)hdr[1] != nl) fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: too few training rows on this rank for nlist / world centroids");
-    ix->set_device();
-    DevBuf<float> all;
-    all.reserve((size_t)nlist * d, 0, sh->ws);
-    B200VS_CUDA(cudaMemcpyAsync(all.p + (size_t)sh->rank * nl * d, blob.data() + 32, (size_t)nl * d * 4, cudaMemcpyHostToDevice, sh->ws));
-    if (W > 1) B200VS_NCCL(nccl().AllGather(all.p + (size_t)sh->rank * nl * d, all.p, (size_t)nl * d, ncclFloat, sh->lanes[0]->comm, sh->ws));
-    std::vector<unsigned char> st(32 + (size_t)nlist * d * 4);
-    int64_t h4[4] = {0x43465649, nlist, d, (int64_t)ix->metric};
-    memcpy(st.data(), h4, 32);
-    B200VS_CUDA(cudaMemcpyAsync(st.data() + 32, all.p, (size_t)nlist * d * 4, cudaMemcpyDeviceToHost, sh->ws));
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-    ix->set_state(st.data(), st.size());
+    shard_train_locked(sh, n, x);
     return B200VS_OK;
   });
 }
@@ -752,82 +753,22 @@ const float* assign_rows(b200vs_shard* sh, int64_t n, const float* x_dev, DevBuf
   return xp;
 }
 
-void shard_add_device_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long long* ids_dev) {
-  IndexBase* ix = sh->ix;
-  const int W = sh->world, d = ix->dim;
+// Moves n device rows (rows, ids and, list-sharded, lists) to their owners: a stable partition by owner on the device
+// (route_*_kernel), the counts-matrix all-gather, and one grouped ncclSend / ncclRecv.  A rank receives rank 0's rows
+// first, then rank 1's, ..., each in its caller's order; at world 1 the partitioned rows are the received ones.
+struct Routed {
+  DevBuf<float> x;
+  DevBuf<long long> ids, lists;
+  long long n = 0;
+};
+template <class Owner>
+void route_rows(b200vs_shard* sh, int64_t n, const float* x, const long long* ids, const long long* lists, Owner owner, Routed& out) {
+  const int W = sh->world, r = sh->rank, d = sh->ix->dim;
   cudaStream_t s = sh->ws;
-  ix->set_device();
-  DevBuf<float> prep, sx, rx;
-  DevBuf<long long> lists, perm, sids, slists, rids, rlists, cnt_all;
-  const float* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
-  // owner of every row, stable order by owner (host counting sort over 8 bytes per row)
-  std::vector<long long> h_lists((size_t)n), h_perm((size_t)n);
-  if (n) B200VS_CUDA(cudaMemcpyAsync(h_lists.data(), lists.p, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaStreamSynchronize(s));
-  const int per = sh->lists_per_rank();
-  std::vector<long long> send_cnt(W, 0), send_off(W + 1, 0);
-  for (int64_t i = 0; i < n; ++i) send_cnt[std::min<long long>(W - 1, h_lists[i] / per)]++;
-  for (int w = 0; w < W; ++w) send_off[w + 1] = send_off[w] + send_cnt[w];
-  {
-    std::vector<long long> cur(send_off.begin(), send_off.end() - 1);
-    for (int64_t i = 0; i < n; ++i) h_perm[cur[std::min<long long>(W - 1, h_lists[i] / per)]++] = i;
-  }
-  // counts matrix: every rank learns how many rows each peer sends it
-  cnt_all.reserve((size_t)W * W, 0, s);
-  B200VS_CUDA(cudaMemcpyAsync(cnt_all.p + (size_t)sh->rank * W, send_cnt.data(), (size_t)W * 8, cudaMemcpyHostToDevice, s));
-  if (W > 1) B200VS_NCCL(nccl().AllGather(cnt_all.p + (size_t)sh->rank * W, cnt_all.p, (size_t)W, ncclInt64, sh->lanes[0]->comm, s));
-  std::vector<long long> h_cnt((size_t)W * W);
-  B200VS_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt_all.p, (size_t)W * W * 8, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaStreamSynchronize(s));
-  std::vector<long long> recv_cnt(W), recv_off(W + 1, 0);
-  for (int w = 0; w < W; ++w) { recv_cnt[w] = h_cnt[(size_t)w * W + sh->rank]; recv_off[w + 1] = recv_off[w] + recv_cnt[w]; }
-  const long long nrecv = recv_off[W];
-  // rows sorted by owner
-  if (n) {
-    perm.reserve((size_t)n, 0, s); sx.reserve((size_t)n * d, 0, s); sids.reserve((size_t)n, 0, s); slists.reserve((size_t)n, 0, s);
-    B200VS_CUDA(cudaMemcpyAsync(perm.p, h_perm.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    gather_rows_kernel<<<(unsigned)cdiv(n * 32, 256), 256, 0, s>>>(xp, ids_dev, lists.p, perm.p, n, d, sx.p, sids.p, slists.p);
-    B200VS_CUDA(cudaGetLastError());
-  }
-  rx.reserve((size_t)std::max<long long>(nrecv, 1) * d, 0, s); rids.reserve((size_t)std::max<long long>(nrecv, 1), 0, s);
-  rlists.reserve((size_t)std::max<long long>(nrecv, 1), 0, s);
-  if (W > 1) {
-    B200VS_NCCL(nccl().GroupStart());
-    for (int w = 0; w < W; ++w) {
-      if (send_cnt[w]) {
-        B200VS_NCCL(nccl().Send(sx.p + (size_t)send_off[w] * d, (size_t)send_cnt[w] * d, ncclFloat, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Send(sids.p + send_off[w], (size_t)send_cnt[w], ncclInt64, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Send(slists.p + send_off[w], (size_t)send_cnt[w], ncclInt64, w, sh->lanes[0]->comm, s));
-      }
-      if (recv_cnt[w]) {
-        B200VS_NCCL(nccl().Recv(rx.p + (size_t)recv_off[w] * d, (size_t)recv_cnt[w] * d, ncclFloat, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Recv(rids.p + recv_off[w], (size_t)recv_cnt[w], ncclInt64, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Recv(rlists.p + recv_off[w], (size_t)recv_cnt[w], ncclInt64, w, sh->lanes[0]->comm, s));
-      }
-    }
-    B200VS_NCCL(nccl().GroupEnd());
-  } else if (n) {
-    B200VS_CUDA(cudaMemcpyAsync(rx.p, sx.p, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(rids.p, sids.p, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(rlists.p, slists.p, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
-  }
-  B200VS_CUDA(cudaStreamSynchronize(s));
-  if (nrecv) ix->add_dev(nrecv, rx.p, rids.p, rlists.p, false, true);
-}
-
-// Row-sharded add (FLAT, HNSW): every row travels RAW to owner(id) (Flat and HNSW normalise cosine rows differently, so the
-// owner's add normalises), and the owner runs the single-index add on the rows it received, in arrival order: rank 0's rows
-// first, then rank 1's, ..., each in its caller's order (an HNSW graph depends on insertion order).  Before any rank changes
-// anything, every owner checks its rows (check_add: a repeated id for FLAT, max_elements for HNSW) and the statuses are
-// all-gathered: every rank returns the first refusal in rank order, or adds.  batched: b200vs_hnsw_add_batched with `batch`.
-void shard_add_rows_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long long* ids_dev, bool batched, int batch) {
-  IndexBase* ix = sh->ix;
-  const int W = sh->world, r = sh->rank, d = ix->dim;
-  cudaStream_t s = sh->ws;
-  ix->set_device();
-  DevBuf<float> sx, rx;
-  DevBuf<long long> sids, rids, cnt_all, tile_off;
-  DevBuf<int> tile_cnt, st;
+  ncclComm_t comm = sh->lanes[0]->comm;
+  Routed snd;
+  DevBuf<long long> cnt_all, tile_off;
+  DevBuf<int> tile_cnt;
   cnt_all.reserve((size_t)W * W, 0, s);
   long long* mine = cnt_all.p + (size_t)r * W;
   // stable partition by owner on the device; this rank's row of the counts matrix
@@ -835,16 +776,18 @@ void shard_add_rows_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const 
     const long long ntiles = cdiv(n, ROUTE_THREADS);
     const size_t smem = (size_t)ROUTE_WARPS * W * 4;
     tile_cnt.reserve((size_t)ntiles * W, 0, s); tile_off.reserve((size_t)ntiles * W, 0, s);
-    sx.reserve((size_t)n * d, 0, s); sids.reserve((size_t)n, 0, s);
-    route_count_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(ids_dev, n, W, tile_cnt.p);
+    snd.x.reserve((size_t)n * d, 0, s); snd.ids.reserve((size_t)n, 0, s);
+    if (Owner::kLists) snd.lists.reserve((size_t)n, 0, s);
+    route_count_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(Owner::kLists ? lists : ids, n, W, owner, tile_cnt.p);
     route_offsets_kernel<<<1, ROUTE_SCAN_THREADS, 0, s>>>(tile_cnt.p, ntiles, W, tile_off.p, mine);
-    route_scatter_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(x_dev, ids_dev, n, d, W, tile_off.p, sx.p, sids.p);
+    route_scatter_kernel<<<(unsigned)ntiles, ROUTE_THREADS, smem, s>>>(x, ids, lists, n, d, W, owner, tile_off.p, snd.x.p, snd.ids.p,
+                                                                       snd.lists.p);
     B200VS_CUDA(cudaGetLastError());
   } else {
     B200VS_CUDA(cudaMemsetAsync(mine, 0, (size_t)W * 8, s));
   }
   // counts matrix: every rank learns how many rows each peer sends it
-  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, cnt_all.p, (size_t)W, ncclInt64, sh->lanes[0]->comm, s));
+  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, cnt_all.p, (size_t)W, ncclInt64, comm, s));
   std::vector<long long> h_cnt((size_t)W * W);
   B200VS_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt_all.p, (size_t)W * W * 8, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaStreamSynchronize(s));
@@ -853,56 +796,78 @@ void shard_add_rows_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const 
     send_off[w + 1] = send_off[w] + h_cnt[(size_t)r * W + w];
     recv_off[w + 1] = recv_off[w] + h_cnt[(size_t)w * W + r];
   }
-  const long long nrecv = recv_off[W];
-  if (W > 1) {
-    rx.reserve((size_t)std::max<long long>(nrecv, 1) * d, 0, s); rids.reserve((size_t)std::max<long long>(nrecv, 1), 0, s);
-    B200VS_NCCL(nccl().GroupStart());
-    for (int w = 0; w < W; ++w) {
-      const long long sc = send_off[w + 1] - send_off[w], rc = recv_off[w + 1] - recv_off[w];
-      if (sc) {
-        B200VS_NCCL(nccl().Send(sx.p + (size_t)send_off[w] * d, (size_t)sc * d, ncclFloat, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Send(sids.p + send_off[w], (size_t)sc, ncclInt64, w, sh->lanes[0]->comm, s));
-      }
-      if (rc) {
-        B200VS_NCCL(nccl().Recv(rx.p + (size_t)recv_off[w] * d, (size_t)rc * d, ncclFloat, w, sh->lanes[0]->comm, s));
-        B200VS_NCCL(nccl().Recv(rids.p + recv_off[w], (size_t)rc, ncclInt64, w, sh->lanes[0]->comm, s));
-      }
-    }
-    B200VS_NCCL(nccl().GroupEnd());
-  } else {  // a world of one receives exactly what it sends
-    rx.swap(sx); rids.swap(sids);
+  out.n = recv_off[W];
+  if (W == 1) {  // a world of one receives exactly what it sends
+    out.x.swap(snd.x); out.ids.swap(snd.ids); out.lists.swap(snd.lists);
+    return;
   }
-  std::vector<int64_t> hid((size_t)nrecv);
-  if (nrecv) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rids.p, (size_t)nrecv * 8, cudaMemcpyDeviceToHost, s));
+  const size_t cap = (size_t)std::max<long long>(out.n, 1);
+  out.x.reserve(cap * d, 0, s); out.ids.reserve(cap, 0, s);
+  if (Owner::kLists) out.lists.reserve(cap, 0, s);
+  B200VS_NCCL(nccl().GroupStart());
+  for (int w = 0; w < W; ++w) {
+    const long long so = send_off[w], sc = send_off[w + 1] - so, ro = recv_off[w], rc = recv_off[w + 1] - ro;
+    if (sc) {
+      B200VS_NCCL(nccl().Send(snd.x.p + (size_t)so * d, (size_t)sc * d, ncclFloat, w, comm, s));
+      B200VS_NCCL(nccl().Send(snd.ids.p + so, (size_t)sc, ncclInt64, w, comm, s));
+      if (Owner::kLists) B200VS_NCCL(nccl().Send(snd.lists.p + so, (size_t)sc, ncclInt64, w, comm, s));
+    }
+    if (rc) {
+      B200VS_NCCL(nccl().Recv(out.x.p + (size_t)ro * d, (size_t)rc * d, ncclFloat, w, comm, s));
+      B200VS_NCCL(nccl().Recv(out.ids.p + ro, (size_t)rc, ncclInt64, w, comm, s));
+      if (Owner::kLists) B200VS_NCCL(nccl().Recv(out.lists.p + ro, (size_t)rc, ncclInt64, w, comm, s));
+    }
+  }
+  B200VS_NCCL(nccl().GroupEnd());
+}
+
+// The collective add of both shard kinds.  List-sharded (IVF_FLAT, IVF_PQ): the sender assigns each row to its list, and the
+// row travels PREPARED (normalised for cosine) with its list to the list's owner, which appends it there.  Row-sharded
+// (FLAT, HNSW): every row travels RAW to owner(id) (Flat and HNSW normalise cosine rows differently, so the owner's add
+// normalises), and the owner runs the single-index add on the rows it received, in arrival order (an HNSW graph depends on
+// it).  Before any rank changes anything, every owner checks its rows (check_add: a repeated id for FLAT, max_elements for
+// HNSW, nothing for the list types) and the statuses are all-gathered: every rank returns the first refusal in rank order,
+// or adds.  batched: b200vs_hnsw_add_batched with `batch`.
+void shard_add_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long long* ids_dev, bool batched, int batch) {
+  IndexBase* ix = sh->ix;
+  const int d = ix->dim;
+  cudaStream_t s = sh->ws;
+  ix->set_device();
+  Routed rv;
+  if (sh->rows) {
+    route_rows(sh, n, x_dev, ids_dev, nullptr, RowOwner{}, rv);
+  } else {
+    DevBuf<float> prep;
+    DevBuf<long long> lists;
+    const float* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
+    route_rows(sh, n, xp, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
+  }
+  std::vector<int64_t> hid(sh->rows ? (size_t)rv.n : 0);  // the host ids check_add and the FLAT / HNSW adds take
+  if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaStreamSynchronize(s));
   // status agreement
   int code = B200VS_OK;
   std::string msg;
   try {
-    ix->check_add(nrecv, hid.data(), batched, batch);
+    ix->check_add(rv.n, hid.data(), batched, batch);
   } catch (const StatusError& e) {
     code = e.code; msg = e.msg;
   }
-  std::vector<int> codes((size_t)W, code);
-  if (W > 1) {
-    st.reserve((size_t)W, 0, s);
-    B200VS_CUDA(cudaMemcpyAsync(st.p + r, &code, 4, cudaMemcpyHostToDevice, s));
-    B200VS_NCCL(nccl().AllGather(st.p + r, st.p, 1, ncclInt32, sh->lanes[0]->comm, s));
-    B200VS_CUDA(cudaMemcpyAsync(codes.data(), st.p, (size_t)W * 4, cudaMemcpyDeviceToHost, s));
+  const std::vector<int> codes = all_gather_host(sh, &code);
+  for (int w = 0; w < sh->world; ++w)
+    if (codes[w] != B200VS_OK) fail(codes[w], w == sh->rank ? msg : "shard add refused by rank " + std::to_string(w));
+  if (!rv.n) return;
+  if (!sh->rows) {
+    ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
+  } else if (ix->type == B200VS_FLAT) {
+    ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data());
+  } else {
+    std::vector<float> hx((size_t)rv.n * d);  // the HNSW builders take host rows
+    B200VS_CUDA(cudaMemcpyAsync(hx.data(), rv.x.p, (size_t)rv.n * d * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
+    if (batched) hnsw_add_batched(ix, rv.n, hx.data(), hid.data(), batch);
+    else ix->add(rv.n, hx.data(), hid.data(), false);
   }
-  for (int w = 0; w < W; ++w)
-    if (codes[w] != B200VS_OK) fail(codes[w], w == r ? msg : "shard add refused by rank " + std::to_string(w));
-  if (!nrecv) return;
-  if (ix->type == B200VS_FLAT) {
-    ix->add_rows_dev(nrecv, rx.p, rids.p, hid.data());
-    return;
-  }
-  std::vector<float> hx((size_t)nrecv * d);  // the HNSW builders take host rows
-  B200VS_CUDA(cudaMemcpyAsync(hx.data(), rx.p, (size_t)nrecv * d * 4, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaStreamSynchronize(s));
-  if (batched) hnsw_add_batched(ix, nrecv, hx.data(), hid.data(), batch);
-  else ix->add(nrecv, hx.data(), hid.data(), false);
 }
 
 // upload of host rows to the write stream, for the host-pointer variants of the collective adds
@@ -925,8 +890,7 @@ int b200vs_shard_add_device(b200vs_shard* h, int64_t n, const float* x_dev, cons
     b200vs_shard* sh = get(h);
     if (n < 0 || (n > 0 && (!x_dev || !ids_dev))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
     std::lock_guard<std::mutex> g(sh->add_mu);
-    if (sh->rows) shard_add_rows_impl(sh, n, x_dev, (const long long*)ids_dev, false, 0);
-    else shard_add_device_impl(sh, n, x_dev, (const long long*)ids_dev);
+    shard_add_impl(sh, n, x_dev, (const long long*)ids_dev, false, 0);
     return B200VS_OK;
   });
 }
@@ -940,8 +904,7 @@ int b200vs_shard_add(b200vs_shard* h, int64_t n, const float* x, const int64_t* 
     DevBuf<float> dx;
     DevBuf<long long> di;
     upload_rows(sh, n, x, ids, dx, di);
-    if (sh->rows) shard_add_rows_impl(sh, n, dx.p, di.p, false, 0);
-    else shard_add_device_impl(sh, n, dx.p, di.p);
+    shard_add_impl(sh, n, dx.p, di.p, false, 0);
     return B200VS_OK;
   });
 }
@@ -958,7 +921,7 @@ int b200vs_shard_hnsw_add_batched(b200vs_shard* h, int64_t n, const float* x, co
     DevBuf<float> dx;
     DevBuf<long long> di;
     upload_rows(sh, n, x, ids, dx, di);
-    shard_add_rows_impl(sh, n, dx.p, di.p, true, batch);
+    shard_add_impl(sh, n, dx.p, di.p, true, batch);
     return B200VS_OK;
   });
 }
@@ -987,18 +950,15 @@ int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int6
     std::lock_guard<std::mutex> g(sh->add_mu);
     IndexBase* ix = sh->ix;
     const int64_t local = ix->remove(n, ids);  // -1: untrained (OK, nothing to do)
-    long long tot[2] = {local > 0 ? (long long)local : 0, local < 0 ? 1 : 0};
-    if (sh->world > 1) {
-      ix->set_device();
-      DevBuf<long long> d;
-      d.reserve(2, 0, sh->ws);
-      B200VS_CUDA(cudaMemcpyAsync(d.p, tot, 16, cudaMemcpyHostToDevice, sh->ws));
-      B200VS_NCCL(nccl().AllReduce(d.p, d.p, 2, ncclInt64, ncclSum, sh->lanes[0]->comm, sh->ws));
-      B200VS_CUDA(cudaMemcpyAsync(tot, d.p, 16, cudaMemcpyDeviceToHost, sh->ws));
-      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+    ix->set_device();
+    long long removed = 0;
+    bool untrained = false;
+    for (const int64_t v : all_gather_host(sh, &local)) {
+      if (v > 0) removed += v;
+      untrained |= v < 0;
     }
-    if (n_removed) *n_removed = tot[0];
-    if (!sh->rows && tot[0] == 0 && tot[1] == 0) fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
+    if (n_removed) *n_removed = removed;
+    if (!sh->rows && removed == 0 && !untrained) fail(B200VS_EVECTOR_INVALID, "remove not found vector id");
     return B200VS_OK;
   });
 }
@@ -1059,64 +1019,29 @@ int b200vs_shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const f
                                float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
-    if (nq <= 0 || !xq_dev) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-    if (k <= 0) return B200VS_OK;
-    if (!out_dist_dev || !out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    SeqLane sl(sh, seq);
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
-    LaneGuard lane(ix, s);
-    ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
-    if (sh->rows) ix->check_row_search(k, sp);
-    ix->reset_stats();
-    shard_search_stream(sh, *sl.lane, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
-    ix->phases_finish(s);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));
+    shard_read(sh, seq, stream, nq, k, sp, [&] { return check_shard_topk(nq, xq_dev, k, out_dist_dev, out_ids_dev); },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 shard_search_stream(sh, L, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
+               });
     return B200VS_OK;
   });
 }
 
-// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch; each rank uploads only its
-// slice and the slices are all-gathered over NVLink, so the PCIe traffic per rank does not grow with the world size.
+// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).
 int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                         int64_t* out_ids) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
-    if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-    if (k <= 0) return B200VS_OK;
-    if (!out_dist || !out_ids) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    const int W = sh->world, r = sh->rank, d = ix->dim;
-    cudaStream_t s;
-    float* dd;
-    long long* di;
-    {
-      SeqLane sl(sh, seq);
-      std::shared_lock<std::shared_mutex> rl(ix->rw);
-      ix->set_device();
-      b200vs_shard::SLane& L = *sl.lane;
-      s = L.own;
-      LaneGuard lane(ix, s);
-      ix->check_probe_search(nq, k);  // before the first collective, alike on every rank
-      if (sh->rows) ix->check_row_search(k, sp);
-      ix->reset_stats();
-      const int64_t per = (nq + W - 1) / W;
-      L.q_all.reserve((size_t)per * W * d, 0, s);
-      const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
-      float* mine = L.q_all.p + (size_t)per * r * d;
-      if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, xq + (size_t)q0 * d, (size_t)(q1 - q0) * d * 4, cudaMemcpyHostToDevice, s));
-      if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * d, 0, (size_t)(per - (q1 - q0)) * d * 4, s));
-      if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * d, ncclFloat, L.comm, s));
-      dd = ix->scratch.alloc<float>((size_t)nq * k);
-      di = ix->scratch.alloc<long long>((size_t)nq * k);
-      shard_search_stream(sh, L, nq, L.q_all.p, k, sp, dd, di, s);
-      ix->phases_finish(s);
-      B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
-      B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-    }  // the lane is released before the host waits: the next batch of this lane may be enqueued behind this one
-    B200VS_CUDA(cudaStreamSynchronize(s));
+    shard_read(sh, seq, nullptr, nq, k, sp, [&] { return check_shard_topk(nq, xq, k, out_dist, out_ids); },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 IndexBase* ix = sh->ix;
+                 const float* q = upload_batch(sh, L, nq, xq, s);
+                 float* dd = ix->scratch.alloc<float>((size_t)nq * k);
+                 long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
+                 shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
+                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
+               });
     return B200VS_OK;
   });
 }
@@ -1126,18 +1051,11 @@ int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, c
                                      void* stream) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
-    SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
-    check_shard_range(ix, nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    cudaStream_t s = stream ? (cudaStream_t)stream : sl.lane->own;
-    LaneGuard lane(ix, s);
-    ix->check_probe_search(nq, max_results);  // before the first collective, alike on every rank
-    ix->reset_stats();
-    shard_range_stream(sh, *sl.lane, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
-    ix->phases_finish(s);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));
+    shard_read(sh, seq, stream, nq, max_results, sp,
+               [&] { return check_shard_range(sh->ix, nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev); },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 shard_range_stream(sh, L, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
+               });
     return B200VS_OK;
   });
 }
@@ -1147,37 +1065,20 @@ int b200vs_shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const fl
                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    IndexBase* ix = sh->ix;
-    const int W = sh->world, r = sh->rank, d = ix->dim;
-    cudaStream_t s;
-    {
-      SeqLane sl(sh, seq);  // a refused call still takes its turn, so later sequence numbers do not wait for it
-      check_shard_range(ix, nq, xq, max_results, out_dist, out_ids, out_counts);
-      std::shared_lock<std::shared_mutex> rl(ix->rw);
-      ix->set_device();
-      b200vs_shard::SLane& L = *sl.lane;
-      s = L.own;
-      LaneGuard lane(ix, s);
-      ix->check_probe_search(nq, max_results);  // before the first collective, alike on every rank
-      ix->reset_stats();
-      const int64_t per = (nq + W - 1) / W;
-      L.q_all.reserve((size_t)per * W * d, 0, s);
-      const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
-      float* mine = L.q_all.p + (size_t)per * r * d;
-      if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, xq + (size_t)q0 * d, (size_t)(q1 - q0) * d * 4, cudaMemcpyHostToDevice, s));
-      if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * d, 0, (size_t)(per - (q1 - q0)) * d * 4, s));
-      if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * d, ncclFloat, L.comm, s));
-      const size_t nr = (size_t)nq * max_results;
-      float* dd = ix->scratch.alloc<float>(nr);
-      long long* di = ix->scratch.alloc<long long>(nr);
-      int* dc = ix->scratch.alloc<int>((size_t)nq);
-      shard_range_stream(sh, L, nq, L.q_all.p, radius, max_results, sp, dd, di, dc, s);
-      ix->phases_finish(s);
-      B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
-      B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
-      B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    }  // the lane is released before the host waits
-    B200VS_CUDA(cudaStreamSynchronize(s));
+    shard_read(sh, seq, nullptr, nq, max_results, sp,
+               [&] { return check_shard_range(sh->ix, nq, xq, max_results, out_dist, out_ids, out_counts); },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 IndexBase* ix = sh->ix;
+                 const float* q = upload_batch(sh, L, nq, xq, s);
+                 const size_t nr = (size_t)nq * max_results;
+                 float* dd = ix->scratch.alloc<float>(nr);
+                 long long* di = ix->scratch.alloc<long long>(nr);
+                 int* dc = ix->scratch.alloc<int>((size_t)nq);
+                 shard_range_stream(sh, L, nq, q, radius, max_results, sp, dd, di, dc, s);
+                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+               });
     return B200VS_OK;
   });
 }

@@ -226,13 +226,17 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  * (dlopen libnccl.so.2; override with B200VS_NCCL_LIB), one communicator per batch in flight.
  *   shard_unique_id : rank 0 creates the rendezvous blob; the host passes it to the other ranks out of band (dingo-store: RPC)
  *   shard_create    : wraps an (untrained or trained, still empty) IVF_FLAT or IVF_PQ index created with the GLOBAL nlist
- *                     (IVF_PQ in inner-Flat mode: EVECTOR_NOT_SUPPORT); `lanes` = batches that may be in flight (<= 0: 2)
- *   shard_train     : distributed training — each rank clusters its rows into nlist / world centroids, one all-gather.
- *                     IVF_PQ: the row counts are exchanged first (fewer than nlist / world rows on any rank, or fewer than
- *                     256 * 2^nbits on rank 0: EILLEGAL_PARAMETERS on every rank); rank 0 then trains the codebooks on its
- *                     rows' residuals and its state is broadcast.  At world = 1 the state equals b200vs_train's.
- *   shard_broadcast_state : or: replicate rank `root`'s trained state (b200vs_train / b200vs_set_trained_state there)
- *   shard_add[_device]    : each rank passes the rows it holds; rows travel to the owner of their nearest centroid's list
+ *                     (IVF_PQ in inner-Flat mode: EVECTOR_NOT_SUPPORT); `lanes` = batches that may be in flight (<= 0: 2);
+ *                     world <= 1024 for every shard type (larger: EILLEGAL_PARAMETERS)
+ *   shard_train     : distributed training — the row counts are exchanged first (fewer than nlist / world rows on any rank,
+ *                     a null x counting as none, or for IVF_PQ fewer than 256 * 2^nbits on rank 0: EILLEGAL_PARAMETERS on
+ *                     every rank, the index untouched); each rank clusters its rows into nlist / world centroids, one
+ *                     all-gather.  IVF_PQ: rank 0 then trains the codebooks on its rows' residuals and its state is broadcast.
+ *                     At world = 1 the state equals b200vs_train's.
+ *   shard_broadcast_state : or: replicate rank `root`'s trained state (b200vs_train / b200vs_set_trained_state there); a root
+ *                     without one: EVECTOR_NOT_TRAIN on every rank
+ *   shard_add[_device]    : each rank passes the rows it holds; rows travel to the owner of their nearest centroid's list,
+ *                     which receives rank 0's rows first, then rank 1's, ..., each in its caller's order
  *   shard_plan_add_device / shard_plan_commit : optional first pass of a bulk build (assignment only) that pre-sizes every
  *                     owned list in one allocation — a 77 GB shard cannot afford list relocation or arena re-allocation
  *   shard_search[_device] : all ranks pass the SAME batch.  Coarse quantiser on the rank's slice of the batch + all-gather of
@@ -240,7 +244,8 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  *                     (16-byte (distance, id) records) + k-way merge (VectorIndexWrapper::MergeSearchResults,
  *                     src/vector/vector_index.cc:1056-1108): every rank returns the full merged [nq, k].  The host-pointer
  *                     variant uploads only the rank's slice of the batch and all-gathers the queries over NVLink.
- *                     seq = batch sequence number: 0, 1, 2, ... the same on every rank, each used exactly once.  Batches are
+ *                     seq = batch sequence number: 0, 1, 2, ... the same on every rank, each used exactly once: a refused
+ *                     call, or one with k <= 0 (OK, nothing to do), still uses up its seq.  Batches are
  *                     enqueued in seq order on every rank (concurrent caller threads simply take turns; the GPU work of
  *                     up to `lanes` batches still overlaps), batch seq uses communicator seq % lanes.  seq < 0 = "next in
  *                     call order" for single-threaded callers.  Results equal b200vs_search on the unsharded index.
@@ -248,7 +253,7 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  * Row-sharded FLAT and HNSW (DESIGN.md 4.5): the same entry points serve one logical FLAT or HNSW index.  A row belongs to
  * rank b200vs_row_owner(id) = splitmix64(id) mod world, so an upsert or a delete always meets the existing row on its owner,
  * and each rank's index keeps its type's single-index semantics.  On such a shard:
- *   shard_create    : accepts an EMPTY FLAT or HNSW index (a non-empty one: EVECTOR_NOT_SUPPORT); world <= 1024
+ *   shard_create    : accepts an EMPTY FLAT or HNSW index (a non-empty one: EVECTOR_NOT_SUPPORT)
  *   shard_train     : OK, nothing to do (as b200vs_train on FLAT and HNSW)
  *   shard_broadcast_state, shard_list_range, shard_plan_add_device, shard_plan_commit : EVECTOR_NOT_SUPPORT (no lists, and an
  *                     HNSW state is a whole graph)

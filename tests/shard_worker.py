@@ -4,7 +4,9 @@ hand: `python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.
 Every rank builds its part of ONE logical IVF-Flat index through b200vs_shard_* (distributed training or a broadcast
 trained state, rows routed to their list owner over NCCL), answers the same batches through the sharded search (device
 pointers, host pointers, several batches in flight, explicit sequence numbers from concurrent threads) and rank 0 checks
-every answer against the CPU oracle run on the gathered index: ids and distance bits must be identical."""
+every answer against the CPU oracle run on the gathered index: ids and distance bits must be identical.  Before building,
+every rank checks that a train with too few rows on one rank and a broadcast from an untrained root are refused on every
+rank with the same status."""
 import os
 import sys
 import threading
@@ -47,6 +49,19 @@ def main():
         idb = torch.from_numpy(b200vs.Shard.unique_id() if rank == 0 else np.zeros(128, np.uint8)).to(dev)
         dist.broadcast(idb, 0)
         sh = b200vs.Shard(ix, rank, world, idb.cpu().numpy(), lanes=2)
+        # refusals every rank returns together, before any rank waits in a collective: the last rank trains on fewer than
+        # nlist / world rows, and a broadcast from an untrained root
+        for what, fn, want in (("short train", lambda: sh.train(xb[:nlist // world - 1] if rank == world - 1 else xb),
+                                b200vs.EILLEGAL_PARAMETERS),
+                               ("untrained root", lambda: sh.broadcast_state(0), b200vs.EVECTOR_NOT_TRAIN)):
+            try:
+                fn()
+                got = b200vs.OK
+            except b200vs.B200VSError as e:
+                got = e.code
+            if got != want or ix.is_trained():
+                failures.append(f"metric {metric} {what}: rank {rank} returned {got}, want {want}")
+        note(rank, "collective refusals done")
         if mode == "train":
             sh.train(xb)
         else:  # rank 0 holds an oracle-trained state, everybody receives it
@@ -140,10 +155,12 @@ def main():
         dist.barrier()
         faulthandler.cancel_dump_traceback_later()
         faulthandler.dump_traceback_later(150, exit=True)
+    if rank != 0 and failures:
+        print(f"[shard_worker] rank {rank} FAILED:", "; ".join(failures), file=sys.stderr, flush=True)
     ok = torch.tensor([0 if failures else 1], device=dev)
-    dist.broadcast(ok, 0)
+    dist.all_reduce(ok, op=dist.ReduceOp.MIN)  # a failure seen on any rank fails the worker
     if rank == 0:
-        print("SHARD_WORKER", "OK" if not failures else "FAILED: " + "; ".join(failures), flush=True)
+        print("SHARD_WORKER", "OK" if int(ok.item()) == 1 else "FAILED: " + "; ".join(failures or ["on another rank"]), flush=True)
     dist.destroy_process_group()
     sys.exit(0 if int(ok.item()) == 1 else 1)
 
