@@ -11,7 +11,6 @@
 // distances are exact integers <= 32768, so the key orders them like the integers and results are ordered by
 // (distance, id), identical on both paths.
 #include <cmath>
-#include <cstdio>
 
 #include "binary_tile.cuh"
 #include "index.h"
@@ -88,13 +87,6 @@ struct BinRows {
     B200VS_CUDA(cudaMemcpyAsync(d_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ix->stream));
     copy(x, xids, nullptr, d_slots, n, words.p, ids.p);
   }
-  void tombstone(const std::vector<int64_t>& rows) {
-    if (rows.empty()) return;
-    long long* d_rows = ix->scratch.alloc<long long>(rows.size());
-    B200VS_CUDA(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, ix->stream));
-    launch_set_ids(ids.p, d_rows, (int64_t)rows.size(), -1, ix->stream);
-    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
-  }
   // compaction: fresh buffers of cap rows holding row src[i] at dst[i]
   void gather(const std::vector<long long>& src, const std::vector<long long>& dst, int64_t cap) {
     const int64_t n = (int64_t)src.size();
@@ -111,6 +103,7 @@ struct BinRows {
     words.swap(nw); ids.swap(ni);
   }
   // rows [r0, r0 + n) as packed bytes [n, dim / 8] on the host
+  size_t row_bytes() const { return (size_t)ix->dim / 8; }
   void download(int64_t r0, int64_t n, uint8_t* out) const {
     if (n <= 0) return;
     const int nb = ix->dim / 8;
@@ -119,6 +112,12 @@ struct BinRows {
     for (int64_t i = 0; i < n; ++i) memcpy(out + (size_t)i * nb, tmp.data() + (size_t)i * w, nb);
   }
   int64_t bytes() const { return (int64_t)(words.cap * 4 + ids.cap * 8); }
+  // the row fields of a tile-scan view; the owner adds the list layout
+  TcView view() const {
+    TcView v;
+    v.vecs = reinterpret_cast<const float*>(words.p); v.ids = ids.p;
+    return v;
+  }
 };
 
 // Shared by both binary types: the float entry points are refused (api.cu checks first), rows arrive packed.
@@ -159,130 +158,18 @@ struct BinaryIndex : IndexBase {
     return std::trunc(std::min(radius, (float)(dim + 1)));
   }
 
-  // Own container (not faiss write_index_binary): header, trained-state blob, list offsets, ids, then the live rows packed,
-  // dim / 8 bytes each, in list-major order.
-  struct BinHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
-  void save(const std::string& path) override;
-  void load(const std::string& path) override;
 };
-
-namespace {
-void wr(FILE* f, const void* p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short write"); }
-void rd(FILE* f, void* p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short read / truncated index file"); }
-}  // namespace
-
-void BinaryIndex::save(const std::string& path) {
-  RwSharedGuard hold(this);
-  const int64_t st_len = get_state(nullptr, 0);
-  std::vector<unsigned char> st((size_t)std::max<int64_t>(st_len, 0));
-  if (st_len > 0) get_state(st.data(), st.size());
-  const int nl = export_nlist();
-  const int64_t n = count();
-  std::vector<int64_t> off(nl + 1, 0), ids((size_t)n);
-  std::vector<uint8_t> rows((size_t)n * nb);
-  if (n) export_lists(off.data(), nullptr, rows.data(), ids.data());
-  FILE* f = fopen(path.c_str(), "wb");
-  if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
-  try {
-    BinHdr h;
-    memcpy(h.magic, "B2VSBIN1", 8);
-    h.type = type; h.metric = metric; h.dim = dim; h.nlist = nl; h.state_len = st_len > 0 ? st_len : 0; h.count = n;
-    wr(f, &h, sizeof(h));
-    wr(f, st.data(), st.size());
-    wr(f, off.data(), off.size() * 8);
-    wr(f, ids.data(), ids.size() * 8);
-    wr(f, rows.data(), rows.size());
-  } catch (...) { fclose(f); throw; }
-  fclose(f);
-}
-
-void BinaryIndex::load(const std::string& path) {
-  FILE* f = fopen(path.c_str(), "rb");
-  if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
-  try {
-    BinHdr h;
-    rd(f, &h, sizeof(h));
-    if (memcmp(h.magic, "B2VSBIN1", 8) != 0 || h.type != (int)type || h.metric != (int)metric || h.dim != dim)
-      fail(B200VS_EINTERNAL, "index file does not match this index (type / metric / dimension)");
-    if (count() != 0) fail(B200VS_EINTERNAL, "load into a non-empty index");
-    {
-      const long here = ftell(f);
-      fseek(f, 0, SEEK_END);
-      const long fsize = ftell(f);
-      fseek(f, here, SEEK_SET);
-      const double need = (double)h.state_len + ((double)h.nlist + 1) * 8 + (double)h.count * (8 + (double)nb);
-      if (h.state_len < 0 || h.count < 0 || h.nlist < 0 || h.nlist > (1 << 24) || need > (double)(fsize - here))
-        fail(B200VS_EINTERNAL, "corrupt index file (header sizes exceed the file)");
-    }
-    std::vector<unsigned char> st((size_t)h.state_len);
-    rd(f, st.data(), st.size());
-    if (h.state_len > 0) set_state(st.data(), st.size());
-    std::vector<int64_t> off((size_t)h.nlist + 1), ids((size_t)h.count);
-    std::vector<uint8_t> rows((size_t)h.count * nb);
-    rd(f, off.data(), off.size() * 8);
-    rd(f, ids.data(), ids.size() * 8);
-    rd(f, rows.data(), rows.size());
-    for (int64_t a = 0; a < h.count; a += 32768) {
-      const int64_t m = std::min<int64_t>(32768, h.count - a);
-      add_binary(m, rows.data() + (size_t)a * nb, ids.data() + a, false);
-    }
-  } catch (...) { fclose(f); throw; }
-  fclose(f);
-}
 
 // ============================================================================================
 // Binary Flat: IndexBinaryFlat under IndexBinaryIDMap2 (vector_index_flat.cc:99-102, :121-264), with the float Flat's
 // policies: append, tombstone, compaction at half dead.
 // ============================================================================================
 struct BinaryFlatIndex : BinaryIndex {
-  BinRows store{this};
-  int64_t rows = 0;
-  std::vector<int64_t> h_ids;
-  std::unordered_map<int64_t, int64_t> id2row;
-  int64_t ndeleted = 0;
-  DevBuf<long long> d_off1;  // the single "list" of a Flat index, for the tile scan
-  DevBuf<int> d_len1;
+  FlatRowMap<BinRows> rowmap{this};
 
-  BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {
-    d_off1.reserve(1, 0, stream); d_len1.reserve(1, 0, stream);
-    B200VS_CUDA(cudaMemsetAsync(d_off1.p, 0, 8, stream));
-    B200VS_CUDA(cudaMemsetAsync(d_len1.p, 0, 4, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-  void publish_len() {
-    const int len = (int)std::min<int64_t>(rows, 0x7fffffff);
-    B200VS_CUDA(cudaMemcpyAsync(d_len1.p, &len, 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-  TcView view() const {
-    TcView v;
-    v.vecs = reinterpret_cast<const float*>(store.words.p); v.ids = store.ids.p;
-    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
-    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
-    return v;
-  }
+  BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {}
   void train_binary(int64_t, const uint8_t*) override {}  // a Flat index needs no training (flat.cc Train returns OK)
 
-  void tombstone(const std::vector<int64_t>& rws) {
-    store.tombstone(rws);
-    for (int64_t r : rws) h_ids[r] = -1;
-    ndeleted += (int64_t)rws.size();
-  }
-  void compact_if_needed() {
-    if (ndeleted == 0 || ndeleted * 2 < rows) return;
-    std::vector<long long> src, dst;
-    for (int64_t r = 0; r < rows; ++r) if (h_ids[r] >= 0) src.push_back(r);
-    const int64_t live = (int64_t)src.size();
-    dst.resize(live);
-    for (int64_t i = 0; i < live; ++i) dst[i] = i;
-    store.gather(src, dst, std::max<int64_t>(1024, live * 5 / 4));
-    std::vector<int64_t> nh(live);
-    id2row.clear();
-    for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
-    h_ids.swap(nh);
-    rows = live; ndeleted = 0;
-    publish_len();
-  }
   // AddOrUpsert (flat.cc:121-162): duplicate ids in the batch are refused, existing ids are always removed first
   void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool) override {
     check_batch_ids_unique(n, in_ids);
@@ -291,26 +178,10 @@ struct BinaryFlatIndex : BinaryIndex {
     set_device();
     quiesce();
     scratch.reset(stream);
-    std::vector<int64_t> dead;
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(in_ids[i]);
-      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
-    }
-    tombstone(dead);
-    const int64_t cap = (int64_t)store.ids.cap;
-    if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
     const uint32_t* st = upload(n, x);
     long long* st_ids = scratch.alloc<long long>(n);
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    std::vector<long long> slots(n);
-    for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
-    store.write(st, st_ids, slots);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    h_ids.resize(rows + n);
-    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = in_ids[i]; id2row[in_ids[i]] = rows + i; }
-    rows += n;
-    publish_len();
-    compact_if_needed();
+    rowmap.add(n, st, st_ids, in_ids);
   }
   // Delete (flat.cc:171-203): ids that are not present are ignored
   int64_t remove(int64_t n, const int64_t* del) override {
@@ -319,24 +190,17 @@ struct BinaryFlatIndex : BinaryIndex {
     set_device();
     quiesce();
     scratch.reset(stream);
-    std::vector<int64_t> dead;
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(del[i]);
-      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
-    }
-    tombstone(dead);
-    compact_if_needed();
-    return (int64_t)dead.size();
+    return rowmap.remove(n, del);
   }
   ScanJob job(const SearchCtx& sc) const {
-    ScanJob j = hamming_job(store.words.p, store.ids.p, rows);
+    ScanJob j = hamming_job(rowmap.store.words.p, rowmap.store.ids.p, rowmap.rows);
     j.sc = &sc;
     return j;
   }
   void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
     const uint32_t* q = pad(nq, xq, s);
-    const TcView v = view();
-    if (bt_eligible(v, nq, k, 1, (double)rows, sc)) {
+    const TcView v = rowmap.view();
+    if (bt_eligible(v, nq, k, 1, (double)rowmap.rows, sc)) {
       long long* probes = scratch.alloc<long long>(nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
       bt_search(this, v, w, nq, q, k, probes, 1, job(sc), od, oi, s);
@@ -353,25 +217,16 @@ struct BinaryFlatIndex : BinaryIndex {
     j.thr_raw = radius_threshold(radius);
     run_scan(this, j, nq, reinterpret_cast<const float*>(pad(nq, xq, s)), max_results, od, nullptr, oi, oc, s);
   }
-  int64_t count() const override { return rows - ndeleted; }
-  int64_t deleted_count() const override { return ndeleted; }
-  int64_t memory_size() const override { return store.bytes(); }
+  int64_t count() const override { return rowmap.count(); }
+  int64_t deleted_count() const override { return rowmap.ndeleted; }
+  int64_t memory_size() const override { return rowmap.store.bytes(); }
   void export_lists(int64_t* list_off, float* vectors, uint8_t* codes, int64_t* out_ids) override {
     if (vectors) fail(B200VS_EILLEGAL_PARAMETERS, "binary indexes export packed rows through codes; vectors must be NULL");
     RwSharedGuard rl(this);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
-    if (list_off) { list_off[0] = 0; list_off[1] = rows - ndeleted; }
-    std::vector<uint8_t> all;
-    if (codes && rows) { all.resize((size_t)rows * nb); store.download(0, rows, all.data()); }
-    int64_t o = 0;
-    for (int64_t r = 0; r < rows; ++r) {
-      if (h_ids[r] < 0) continue;
-      if (out_ids) out_ids[o] = h_ids[r];
-      if (codes) memcpy(codes + (size_t)o * nb, all.data() + (size_t)r * nb, nb);
-      ++o;
-    }
+    rowmap.export_rows(list_off, codes, out_ids);
   }
 };
 
@@ -502,8 +357,7 @@ struct BinaryIvfIndex : BinaryIndex {
     return probes;
   }
   TcView view() const {
-    TcView v;
-    v.vecs = reinterpret_cast<const float*>(store.words.p); v.ids = store.ids.p;
+    TcView v = store.view();
     v.arena_rows = L.arena_used; v.list_off = L.d_off.p; v.list_len = L.d_len.p;
     v.nlist = nlist; v.total_chunks = L.total_chunks; v.max_chunks_per_list = L.max_chunks_per_list;
     return v;
@@ -522,7 +376,7 @@ struct BinaryIvfIndex : BinaryIndex {
     set_device();
     quiesce();
     scratch.reset(stream);
-    if (upsert) remove_locked(n, in_ids);  // ivf_flat.cc:115-118
+    if (upsert) L.remove(n, in_ids, store);  // ivf_flat.cc:115-118
     const uint32_t* st = upload(n, x);
     long long* st_ids = scratch.alloc<long long>(n);
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
@@ -533,23 +387,10 @@ struct BinaryIvfIndex : BinaryIndex {
       coarse(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, stream, lists + a);
       scratch.release(mark);
     }
-    std::vector<long long> h_list(n), slots(n);
+    std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
-    std::vector<int> need(nlist, 0);
-    for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
-    L.reserve_for(need, [&](int64_t arena_rows) { store.grow(arena_rows, L.arena_used_before); },
-                  [&](int64_t src, int64_t dst, int64_t len) { store.move(src, dst, len); });
-    for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], in_ids[i]);
-    store.write(st, st_ids, slots);
-    L.upload(stream);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-  int64_t remove_locked(int64_t n, const int64_t* del) {
-    std::vector<int64_t> rws;
-    L.remove_ids(n, del, rws);
-    store.tombstone(rws);
-    return (int64_t)rws.size();
+    L.place(n, h_list.data(), in_ids, st, st_ids, store);
   }
   // Delete (ivf_flat.cc:162-189): untrained -> OK; nothing removed -> EVECTOR_INVALID (api.cu)
   int64_t remove(int64_t n, const int64_t* del) override {
@@ -559,14 +400,8 @@ struct BinaryIvfIndex : BinaryIndex {
     set_device();
     quiesce();
     scratch.reset(stream);
-    const int64_t r = remove_locked(n, del);
-    if (L.needs_compaction()) {
-      std::vector<long long> src, dst;
-      const int64_t new_rows = L.plan_compaction(src, dst);
-      store.gather(src, dst, std::max<int64_t>(new_rows, 1));
-      L.commit_compaction();
-      L.upload(stream);
-    }
+    const int64_t r = L.remove(n, del, store);
+    L.compact_if_needed(store);
     return r;
   }
 
@@ -612,22 +447,7 @@ struct BinaryIvfIndex : BinaryIndex {
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
-    int64_t o = 0;
-    std::vector<uint8_t> buf;
-    for (int l = 0; l < nlist; ++l) {
-      if (list_off) list_off[l] = o;
-      if (!trained) continue;
-      const ListMeta& m = L.lists[l];
-      if (codes && m.len) { buf.resize((size_t)m.len * nb); store.download(m.off, m.len, buf.data()); }
-      for (int p = 0; p < m.len; ++p) {
-        const int64_t id = L.h_ids[m.off + p];
-        if (id < 0) continue;
-        if (out_ids) out_ids[o] = id;
-        if (codes) memcpy(codes + (size_t)o * nb, buf.data() + (size_t)p * nb, nb);
-        ++o;
-      }
-    }
-    if (list_off) list_off[nlist] = o;
+    L.export_lists(nlist, list_off, store, codes, out_ids);
   }
 };
 

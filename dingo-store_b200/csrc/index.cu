@@ -127,8 +127,9 @@ const float* IndexBase::prepare_queries(int64_t nq, const float* xq_dev, cudaStr
 }
 
 // Save / Load (VectorIndex::Save/Load, src/vector/vector_index.h:168-170; reference: faiss::write_index / read_index at
-// vector_index_flat.cc:354,:379 and hnswlib saveIndex at vector_index_hnsw.cc:290).  Own container, not faiss-compatible
-// (SURVEY 8f-4): header, trained-state blob, then the live rows in list-major order exactly as stored.
+// vector_index_flat.cc:354,:379, write_index_binary, and hnswlib saveIndex at vector_index_hnsw.cc:290).  Own container, not
+// faiss-compatible (SURVEY 8f-4): header, trained-state blob, list offsets, ids, then the live rows in list-major order
+// exactly as stored.  Float indexes ("B2VSIDX1") store FP32 rows, binary ones ("B2VSBIN1") packed rows of dim / 8 bytes.
 namespace {
 struct FileHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
 void wr(FILE* f, const void* p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short write"); }
@@ -142,20 +143,22 @@ void IndexBase::save(const std::string& path) {
   if (st_len > 0) get_state(st.data(), st.size());
   const int nl = export_nlist();
   const int64_t n = type == B200VS_HNSW ? 0 : count();  // the HNSW blob already carries rows + labels
+  const size_t rb = query_row_bytes();
   std::vector<int64_t> off(nl + 1, 0), ids((size_t)n);
-  std::vector<float> vec((size_t)n * dim);
-  if (n) export_lists(off.data(), vec.data(), nullptr, ids.data());
+  std::vector<uint8_t> rows((size_t)n * rb);
+  if (n && binary()) export_lists(off.data(), nullptr, rows.data(), ids.data());
+  else if (n) export_lists(off.data(), reinterpret_cast<float*>(rows.data()), nullptr, ids.data());
   FILE* f = fopen(path.c_str(), "wb");
   if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
   try {
     FileHdr h;
-    memcpy(h.magic, "B2VSIDX1", 8);
+    memcpy(h.magic, binary() ? "B2VSBIN1" : "B2VSIDX1", 8);
     h.type = type; h.metric = metric; h.dim = dim; h.nlist = nl; h.state_len = st_len > 0 ? st_len : 0; h.count = n;
     wr(f, &h, sizeof(h));
     wr(f, st.data(), st.size());
     wr(f, off.data(), off.size() * 8);
     wr(f, ids.data(), ids.size() * 8);
-    wr(f, vec.data(), vec.size() * 4);
+    wr(f, rows.data(), rows.size());
   } catch (...) { fclose(f); throw; }
   fclose(f);
 }
@@ -166,15 +169,16 @@ void IndexBase::load(const std::string& path) {
   try {
     FileHdr h;
     rd(f, &h, sizeof(h));
-    if (memcmp(h.magic, "B2VSIDX1", 8) != 0 || h.type != (int)type || h.metric != (int)metric || h.dim != dim)
+    if (memcmp(h.magic, binary() ? "B2VSBIN1" : "B2VSIDX1", 8) != 0 || h.type != (int)type || h.metric != (int)metric || h.dim != dim)
       fail(B200VS_EINTERNAL, "index file does not match this index (type / metric / dimension)");
     if (count() != 0) fail(B200VS_EINTERNAL, "load into a non-empty index");
+    const size_t rb = query_row_bytes();
     {  // the header's sizes must fit the file before anything is allocated from them
       const long here = ftell(f);
       fseek(f, 0, SEEK_END);
       const long fsize = ftell(f);
       fseek(f, here, SEEK_SET);
-      const double need = (double)h.state_len + ((double)h.nlist + 1) * 8 + (double)h.count * (8 + (double)dim * 4);
+      const double need = (double)h.state_len + ((double)h.nlist + 1) * 8 + (double)h.count * (8 + (double)rb);
       if (h.state_len < 0 || h.count < 0 || h.nlist < 0 || h.nlist > (1 << 24) || need > (double)(fsize - here))
         fail(B200VS_EINTERNAL, "corrupt index file (header sizes exceed the file)");
     }
@@ -182,15 +186,16 @@ void IndexBase::load(const std::string& path) {
     rd(f, st.data(), st.size());
     if (h.state_len > 0) set_state(st.data(), st.size());
     std::vector<int64_t> off((size_t)h.nlist + 1), ids((size_t)h.count);
-    std::vector<float> vec((size_t)h.count * dim);
+    std::vector<uint8_t> rows((size_t)h.count * rb);
     rd(f, off.data(), off.size() * 8);
     rd(f, ids.data(), ids.size() * 8);
-    rd(f, vec.data(), vec.size() * 4);
+    rd(f, rows.data(), rows.size());
     loading = true;
     try {
       for (int64_t a = 0; a < h.count; a += 32768) {
         const int64_t m = std::min<int64_t>(32768, h.count - a);
-        add(m, vec.data() + (size_t)a * dim, ids.data() + a, false);
+        if (binary()) add_binary(m, rows.data() + (size_t)a * rb, ids.data() + a, false);
+        else add(m, reinterpret_cast<const float*>(rows.data() + (size_t)a * rb), ids.data() + a, false);
       }
     } catch (...) { loading = false; throw; }
     loading = false;
@@ -263,14 +268,6 @@ struct RowStore {
     if (mirror) launch_half_rows(vecs.p, d_slots, n, d, vecs_h.p, hscale.p, s);  // re-derived from the stored rows
     max_norm = std::max(max_norm, device_max_norm(ix, row_norms, n, s));
   }
-  // ids[r] = -1 for every listed row
-  void tombstone(const std::vector<int64_t>& rows) {
-    if (rows.empty()) return;
-    long long* d_rows = ix->scratch.alloc<long long>(rows.size());
-    B200VS_CUDA(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, s));
-    launch_set_ids(ids.p, d_rows, (int64_t)rows.size(), -1, s);
-    B200VS_CUDA(cudaStreamSynchronize(s));
-  }
   // compaction: fresh buffers of cap rows holding row src[i] at dst[i].  The mirror is re-derived from the moved FP32
   // rows, which gives the same bits as moving the old mirror rows.
   void gather(const std::vector<long long>& src, const std::vector<long long>& dst, int64_t cap) {
@@ -293,6 +290,11 @@ struct RowStore {
       if (mirror && n) launch_half_rows(vecs.p, d_dst, n, d, vecs_h.p, hscale.p, s);
     }
   }
+  // rows [r0, r0 + n) as FP32 rows [n, d] on the host
+  size_t row_bytes() const { return (size_t)d * 4; }
+  void download(int64_t r0, int64_t n, uint8_t* out) const {
+    if (n > 0) B200VS_CUDA(cudaMemcpy(out, vecs.p + (size_t)r0 * d, (size_t)n * d * 4, cudaMemcpyDeviceToHost));
+  }
   int64_t bytes() const { return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + vecs_h.cap * 2 + hscale.cap * 4); }
   // the row fields of a tile-scan view; the owner adds the list layout
   TcView view() const {
@@ -307,54 +309,9 @@ struct RowStore {
 // Flat
 // ============================================================================================
 struct FlatIndex : IndexBase {
-  RowStore store{this, false};  // no mirror: a Flat search keeps its TF32 arithmetic
-  int64_t rows = 0;
-  std::vector<int64_t> h_ids;
-  std::unordered_map<int64_t, int64_t> id2row;
-  int64_t ndeleted = 0;
-  DevBuf<long long> d_off1;  // the single "list" of a Flat index, for the tile-scan view
-  DevBuf<int> d_len1;
+  FlatRowMap<RowStore> rowmap{this, false};  // no mirror: a Flat search keeps its TF32 arithmetic
 
-  FlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_FLAT, m, d, p) {
-    d_off1.reserve(1, 0, stream); d_len1.reserve(1, 0, stream);
-    B200VS_CUDA(cudaMemsetAsync(d_off1.p, 0, 8, stream));
-    B200VS_CUDA(cudaMemsetAsync(d_len1.p, 0, 4, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-  void publish_len() {
-    const int len = (int)std::min<int64_t>(rows, 0x7fffffff);
-    B200VS_CUDA(cudaMemcpyAsync(d_len1.p, &len, 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-  TcView view() const {
-    TcView v = store.view();
-    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
-    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
-    return v;
-  }
-
-  void tombstone(const std::vector<int64_t>& rws) {
-    store.tombstone(rws);
-    for (int64_t r : rws) h_ids[r] = -1;
-    ndeleted += (int64_t)rws.size();
-  }
-
-  void compact_if_needed() {
-    if (ndeleted == 0 || ndeleted * 2 < rows) return;
-    std::vector<long long> src, dst;
-    src.reserve(rows - ndeleted);
-    for (int64_t r = 0; r < rows; ++r) if (h_ids[r] >= 0) src.push_back(r);
-    const int64_t live = (int64_t)src.size();
-    dst.resize(live);
-    for (int64_t i = 0; i < live; ++i) dst[i] = i;
-    store.gather(src, dst, std::max<int64_t>(1024, live * 5 / 4));
-    std::vector<int64_t> nh(live);
-    id2row.clear();
-    for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
-    h_ids.swap(nh);
-    rows = live; ndeleted = 0;
-    publish_len();
-  }
+  FlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_FLAT, m, d, p) {}
 
   // VectorIndexFlat::AddOrUpsert, vector_index_flat.cc:121-162: duplicate ids inside the batch are rejected,
   // pre-existing ids are ALWAYS removed first (add and upsert behave the same), then add_with_ids.
@@ -369,7 +326,8 @@ struct FlatIndex : IndexBase {
     long long* st_ids = scratch.alloc<long long>(n);
     B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    add_locked(n, st, st_ids, in_ids, loading);
+    if (metric == B200VS_COSINE && !loading) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
+    rowmap.add(n, st, st_ids, in_ids);
   }
 
   // the device-pointer form of add: the rows stay on the device, the caller's host copy of the ids feeds the id map
@@ -380,35 +338,14 @@ struct FlatIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
-    float* st = const_cast<float*>(x_dev);
+    const float* st = x_dev;
     if (metric == B200VS_COSINE) {  // the normaliser works in place: keep the caller's rows intact
-      st = scratch.alloc<float>((size_t)n * dim);
-      B200VS_CUDA(cudaMemcpyAsync(st, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
+      float* cp = scratch.alloc<float>((size_t)n * dim);
+      B200VS_CUDA(cudaMemcpyAsync(cp, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
+      launch_normalize_faiss(cp, n, dim, stream);
+      st = cp;
     }
-    add_locked(n, st, ids_dev, ids_host, false);
-  }
-
-  // rw + gpu_mu held, scratch reset, ids unique.  st / st_ids: device rows and ids (st is normalised in place for cosine
-  // unless prepared); h_in: the ids on the host.
-  void add_locked(int64_t n, float* st, const long long* st_ids, const int64_t* h_in, bool prepared) {
-    std::vector<int64_t> dead;
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(h_in[i]);
-      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
-    }
-    tombstone(dead);
-    const int64_t cap = (int64_t)store.ids.cap;
-    if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
-    std::vector<long long> slots(n);
-    for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
-    if (metric == B200VS_COSINE && !prepared) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
-    store.write(st, st_ids, slots);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    h_ids.resize(rows + n);
-    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = h_in[i]; id2row[h_in[i]] = rows + i; }
-    rows += n;
-    publish_len();
-    compact_if_needed();
+    rowmap.add(n, st, ids_dev, ids_host);
   }
 
   void check_add(int64_t n, const int64_t* in_ids, bool, int) override { check_batch_ids_unique(n, in_ids); }
@@ -419,9 +356,8 @@ struct FlatIndex : IndexBase {
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
-    rows = 0; ndeleted = 0; store.max_norm = 0.f;
-    h_ids.clear(); id2row.clear();
-    publish_len();
+    rowmap.store.max_norm = 0.f;
+    rowmap.clear();
   }
 
   // VectorIndexFlat::Delete, vector_index_flat.cc:171-203: unknown ids are ignored (only ids present in
@@ -432,20 +368,13 @@ struct FlatIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
-    std::vector<int64_t> dead;
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(del[i]);
-      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
-    }
-    tombstone(dead);
-    compact_if_needed();
-    return (int64_t)dead.size();
+    return rowmap.remove(n, del);
   }
 
   ScanJob job(const SearchCtx& sc) const {
     ScanJob j;
     j.l2 = metric == B200VS_L2;
-    j.vecs = store.vecs.p; j.ids = store.ids.p; j.d = dim; j.mode = 0; j.n = rows; j.sc = &sc;
+    j.vecs = rowmap.store.vecs.p; j.ids = rowmap.store.ids.p; j.d = dim; j.mode = 0; j.n = rowmap.rows; j.sc = &sc;
     return j;
   }
 
@@ -458,28 +387,29 @@ struct FlatIndex : IndexBase {
   // raw_out: od = raw metric value (L2 distance | ip) instead of the API distance; every path selects the same rows
   void search_rows(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, bool raw_out, cudaStream_t s) {
     const float* q = prepare_queries(nq, xq, s);
-    const TcView v = view();
-    if (rows > 0 && tc_eligible(this, v, nq, k, 1, sc)) {
+    const TcView v = rowmap.view();
+    if (rowmap.rows > 0 && tc_eligible(this, v, nq, k, 1, sc)) {
       long long* probes = scratch.alloc<long long>(nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
       tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, 1, sc, od, oi, raw_out, s);
       return;
     }
-    if (flat_small_eligible(device, nq, rows, dim, k, sc)) {  // one query per task is the reference's own shape: single-launch path
-      flat_small_search(this, metric == B200VS_L2, store.vecs.p, store.ids.p, rows, nq, q, k, sc, od, oi, raw_out, s);
+    if (flat_small_eligible(device, nq, rowmap.rows, dim, k, sc)) {  // one query per task is the reference's own shape: single-launch path
+      flat_small_search(this, metric == B200VS_L2, rowmap.store.vecs.p, rowmap.store.ids.p, rowmap.rows, nq, q, k, sc, od, oi, raw_out, s);
       return;
     }
     run_scan(this, job(sc), nq, q, k, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, nullptr, s);
   }
 
   void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) override {
+    const int64_t rows = rowmap.rows;
     if ((double)nq * (double)rows * 4 > (double)(1LL << 30)) fail(B200VS_EILLEGAL_PARAMETERS, "score matrix larger than 1 GiB");
     const float* q = prepare_queries(nq, xq, s);
     float* ds = scratch.alloc<float>((size_t)std::max<int64_t>(nq * rows, 1));
     float* de = scratch.alloc<float>(nq);
     const bool sample = arith >= 3;  // 3 / 4: the sample pass in the TF32 / FP16 list-scan arithmetic
     const TcArith a = sample ? (arith == 4 ? TC_ARITH_FP16 : TC_ARITH_TF32) : (TcArith)arith;
-    tc_debug_scores(this, view(), metric == B200VS_L2, nq, q, a, sample, ds, de, s);
+    tc_debug_scores(this, rowmap.view(), metric == B200VS_L2, nq, q, a, sample, ds, de, s);
     if (rows > 0) B200VS_CUDA(cudaMemcpyAsync(out_scores, ds, (size_t)nq * rows * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(out_eps, de, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
@@ -499,8 +429,8 @@ struct FlatIndex : IndexBase {
                   bool raw_out, cudaStream_t s) {
     const float* q = prepare_queries(nq, xq, s);
     const float thr = ip_like() ? 1.0F - radius : radius;
-    const TcView v = view();
-    if (rows > 0 && tc_range_eligible(this, v, nq, max_results, 1, sc)) {
+    const TcView v = rowmap.view();
+    if (rowmap.rows > 0 && tc_range_eligible(this, v, nq, max_results, 1, sc)) {
       long long* probes = scratch.alloc<long long>(nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
       tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, 1, sc, od, oi, oc, raw_out, s);
@@ -517,43 +447,30 @@ struct FlatIndex : IndexBase {
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     for (int64_t i = 0; i < n; ++i) {
-      auto it = id2row.find(in_ids[i]);
-      if (found) found[i] = it != id2row.end() ? 1 : 0;
-      if (it != id2row.end())
-        B200VS_CUDA(cudaMemcpyAsync(out + (size_t)i * dim, store.vecs.p + (size_t)it->second * dim, (size_t)dim * 4, cudaMemcpyDeviceToHost, stream));
+      auto it = rowmap.id2row.find(in_ids[i]);
+      if (found) found[i] = it != rowmap.id2row.end() ? 1 : 0;
+      if (it != rowmap.id2row.end())
+        B200VS_CUDA(cudaMemcpyAsync(out + (size_t)i * dim, rowmap.store.vecs.p + (size_t)it->second * dim, (size_t)dim * 4, cudaMemcpyDeviceToHost, stream));
     }
     B200VS_CUDA(cudaStreamSynchronize(stream));
   }
-  int64_t count() const override { return rows - ndeleted; }
-  int64_t deleted_count() const override { return ndeleted; }
-  int64_t memory_size() const override { return store.bytes(); }
+  int64_t count() const override { return rowmap.count(); }
+  int64_t deleted_count() const override { return rowmap.ndeleted; }
+  int64_t memory_size() const override { return rowmap.store.bytes(); }
 
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override {
     RwSharedGuard rl(this);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
-    const int64_t live = rows - ndeleted;
-    if (list_off) { list_off[0] = 0; list_off[1] = live; }
-    std::vector<float> tmp;
-    if (vectors && ndeleted) tmp.resize((size_t)rows * dim);
-    if (vectors) {
-      float* dst = ndeleted ? tmp.data() : vectors;
-      B200VS_CUDA(cudaMemcpy(dst, store.vecs.p, (size_t)rows * dim * 4, cudaMemcpyDeviceToHost));
-    }
-    int64_t o = 0;
-    for (int64_t r = 0; r < rows; ++r) {
-      if (h_ids[r] < 0) continue;
-      if (out_ids) out_ids[o] = h_ids[r];
-      if (vectors && ndeleted) memcpy(vectors + (size_t)o * dim, tmp.data() + (size_t)r * dim, (size_t)dim * 4);
-      ++o;
-    }
+    quiesce();
+    rowmap.export_rows(list_off, reinterpret_cast<uint8_t*>(vectors), out_ids);
   }
 };
 
 IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p) { return new FlatIndex(m, d, p); }
 
 // ============================================================================================
-// IVF arena shared by IVF-Flat (and reused by IVF-PQ for ids): see ivf_common.h
+// IVF-Flat
 // ============================================================================================
 
 void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s) {
@@ -689,8 +606,6 @@ struct IvfFlatIndex : IndexBase {
                     float* od, long long* oi, int* oc, bool raw_out, cudaStream_t s);
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
   int64_t remove(int64_t n, const int64_t* del) override;
-  int64_t remove_locked(int64_t n, const int64_t* del);
-  void maybe_compact();
 
   int resolve_nprobe(const SearchCtx& sc) const {
     int np = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchIvfFlatParamNprobe, ivf_flat.cc:211
@@ -734,7 +649,6 @@ struct IvfFlatIndex : IndexBase {
   }
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override;
   int64_t export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) override;
-  int64_t copy_list(int list, int64_t cap, float* vectors, int64_t* out_ids);
 };
 
 void IvfFlatIndex::train(int64_t n, const float* x) {
@@ -822,7 +736,7 @@ void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, con
     B200VS_CUDA(cudaStreamSynchronize(stream));
     h_ids_in = h_ids_buf.data();
   }
-  if (upsert) remove_locked(n, h_ids_in);  // ivf_flat.cc:115-118
+  if (upsert) L.remove(n, h_ids_in, store);  // ivf_flat.cc:115-118
   if (metric == B200VS_COSINE && !prepared) launch_normalize_faiss(st, n, dim, stream);
   const long long* st_list = lists_dev;
   if (!st_list) {
@@ -830,66 +744,19 @@ void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, con
     assign_dev(st, n, tmp, stream);
     st_list = tmp;
   }
-  std::vector<long long> h_list(n), slots(n);
+  std::vector<long long> h_list(n);
   B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
   B200VS_CUDA(cudaStreamSynchronize(stream));
-  // host: reserve slots (may relocate lists / grow the arena)
-  std::vector<int> need(nlist, 0);
-  for (int64_t i = 0; i < n; ++i) {
-    if (h_list[i] < 0 || h_list[i] >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
-    need[h_list[i]]++;
-  }
-  L.reserve_for(need, [&](int64_t arena_rows) { store.grow(arena_rows, L.arena_used_before); },
-                [&](int64_t src, int64_t dst, int64_t len) { store.move(src, dst, len); });
-  for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], h_ids_in[i]);
-  store.write(st, st_ids, slots);
-  L.upload(stream);
-  B200VS_CUDA(cudaStreamSynchronize(stream));
+  L.place(n, h_list.data(), h_ids_in, st, st_ids, store);
 }
 
-// one arena allocation holding every list at its final size (+ 1/16 slack): bulk builds of large shards
 void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
   std::unique_lock<std::shared_mutex> wl(rw);
   if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-  if (n_lists != nlist) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: list count does not match the trained index");
   std::lock_guard<std::mutex> gl(gpu_mu);
   set_device();
   quiesce();
-  if (L.live + L.dead > 0) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists needs an empty index");
-  int64_t used = 0;
-  for (int l = 0; l < nlist; ++l) {
-    const int64_t want = rows_per_list[l];
-    if (want < 0 || want >= (1LL << 31) - 64) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: bad list size");
-    ListMeta& m = L.lists[l];
-    m.off = used; m.len = 0; m.dead = 0;
-    m.cap = want ? IvfLists::round32(want + want / 16 + 32) : 0;
-    used += m.cap;
-  }
-  const int64_t tail = std::max<int64_t>(used / 64, 4096);  // room for lists that still outgrow their reservation
-  L.arena_used = L.arena_used_before = used;
-  L.arena_cap = used + tail;
-  store.reset();
-  store.grow(L.arena_cap, 0);
-  B200VS_CUDA(cudaMemsetAsync(store.ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
-  L.h_ids.assign(L.arena_cap, -1);
-  L.upload(stream);
-}
-
-int64_t IvfFlatIndex::remove_locked(int64_t n, const int64_t* del) {
-  std::vector<int64_t> rws;
-  L.remove_ids(n, del, rws);
-  store.tombstone(rws);
-  return (int64_t)rws.size();
-}
-
-void IvfFlatIndex::maybe_compact() {
-  if (!L.needs_compaction()) return;
-  std::vector<long long> src, dst;
-  const int64_t new_rows = L.plan_compaction(src, dst);
-  store.gather(src, dst, std::max<int64_t>(new_rows, 1));
-  L.commit_compaction();
-  L.upload(stream);
-  B200VS_CUDA(cudaStreamSynchronize(stream));
+  L.reserve(rows_per_list, n_lists, store);
 }
 
 // VectorIndexIvfFlat::Delete, vector_index_ivf_flat.cc:162-189: untrained -> OK; nothing removed -> EVECTOR_INVALID.
@@ -900,11 +767,10 @@ int64_t IvfFlatIndex::remove(int64_t n, const int64_t* del) {
   set_device();
   quiesce();
   scratch.reset(stream);
-  const int64_t r = remove_locked(n, del);
-  maybe_compact();
+  const int64_t r = L.remove(n, del, store);
+  L.compact_if_needed(store);
   return r;
 }
-
 
 void IvfFlatIndex::search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) {
   if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_flat.cc:224-227
@@ -990,12 +856,8 @@ void IvfFlatIndex::export_lists(int64_t* list_off, float* vectors, uint8_t*, int
   RwSharedGuard rl(this);
   std::lock_guard<std::mutex> gl(gpu_mu);
   set_device();
-  int64_t o = 0;
-  for (int l = 0; l < nlist; ++l) {
-    if (list_off) list_off[l] = o;
-    o += copy_list(l, INT64_MAX, vectors ? vectors + (size_t)o * dim : nullptr, out_ids ? out_ids + o : nullptr);
-  }
-  if (list_off) list_off[nlist] = o;
+  quiesce();
+  L.export_lists(nlist, list_off, store, reinterpret_cast<uint8_t*>(vectors), out_ids);
 }
 
 int64_t IvfFlatIndex::export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) {
@@ -1004,29 +866,7 @@ int64_t IvfFlatIndex::export_list(int list, int64_t cap, float* vectors, int64_t
   if (list < 0 || list >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
   set_device();
   quiesce();
-  return copy_list(list, cap, vectors, out_ids);
-}
-
-// the live rows of one list, in list order: the first `cap` go to vectors / out_ids (either may be null); returns how many
-// there are.  The caller holds rw (shared) and gpu_mu.
-int64_t IvfFlatIndex::copy_list(int list, int64_t cap, float* vectors, int64_t* out_ids) {
-  const auto& m = L.lists[list];
-  std::vector<float> rowbuf;
-  if (vectors && m.len) {
-    rowbuf.resize((size_t)m.len * dim);
-    B200VS_CUDA(cudaMemcpy(rowbuf.data(), store.vecs.p + (size_t)m.off * dim, (size_t)m.len * dim * 4, cudaMemcpyDeviceToHost));
-  }
-  int64_t o = 0;
-  for (int p = 0; p < m.len; ++p) {
-    const int64_t id = L.h_ids[m.off + p];
-    if (id < 0) continue;
-    if (o < cap) {
-      if (out_ids) out_ids[o] = id;
-      if (vectors) memcpy(vectors + (size_t)o * dim, rowbuf.data() + (size_t)p * dim, (size_t)dim * 4);
-    }
-    ++o;
-  }
-  return o;
+  return L.export_list(list, cap, store, reinterpret_cast<uint8_t*>(vectors), out_ids);
 }
 
 IndexBase* make_ivf_flat(b200vs_metric m, int d, const b200vs_params& p) { return new IvfFlatIndex(m, d, p); }

@@ -1,4 +1,12 @@
-// ivf_common.h — inverted-list bookkeeping and GPU k-means shared by IVF-Flat and IVF-PQ.
+// ivf_common.h — row bookkeeping of every index with a row store (Flat, IVF-Flat, IVF-PQ and their binary forms) and the
+// GPU k-means shared by the IVF types.
+//
+// A row store holds an index's device rows: FP32 rows (RowStore, index.cu), padded binary words (BinRows, binary.cu) or PQ
+// code rows (CodeRows, ivf_pq.cu), each with a device id per row (-1 = tombstone / unused slot).  The stores share one
+// shape, used here as a template argument: grow(cap, keep), reset(), move(src, dst, n), write(rows, ids, slots),
+// gather(src, dst, cap), download(r0, n, out) in the export's host format of row_bytes() each, bytes(), and the members
+// ix (the owning index, whose stream and scratch they use) and ids.  The store moves rows; the bookkeeping below decides
+// capacities, slots, tombstones, compaction and export order.
 //
 // Inverted lists live in ONE device arena (rows of the payload array), list l owning rows
 // [off, off+len) with capacity cap >= len.  Appends go in place; a full list is relocated to the arena
@@ -14,8 +22,124 @@
 #include <vector>
 
 #include "index.h"
+#include "tc_scan.cuh"
 
 namespace b200vs {
+
+// ids[r] = -1 for every listed row, on the owner's stream
+inline void tombstone_ids(IndexBase* ix, long long* ids, const std::vector<int64_t>& rows) {
+  if (rows.empty()) return;
+  long long* d_rows = ix->scratch.alloc<long long>(rows.size());
+  B200VS_CUDA(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, ix->stream));
+  launch_set_ids(ids, d_rows, (int64_t)rows.size(), -1, ix->stream);
+  B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+}
+
+// The rows of a Flat index (float or binary): appended in order, tombstoned on delete, compacted at half dead.  The one
+// "list" of rows [0, rows) is what the tile scan sees.
+template <class Store>
+struct FlatRowMap {
+  Store store;
+  int64_t rows = 0;
+  std::vector<int64_t> h_ids;
+  std::unordered_map<int64_t, int64_t> id2row;
+  int64_t ndeleted = 0;
+  DevBuf<long long> d_off1;  // the single "list" of a Flat index, for the tile-scan view
+  DevBuf<int> d_len1;
+
+  template <class... A>
+  explicit FlatRowMap(IndexBase* ix, A... store_args) : store(ix, store_args...) {
+    d_off1.reserve(1, 0, ix->stream); d_len1.reserve(1, 0, ix->stream);
+    B200VS_CUDA(cudaMemsetAsync(d_off1.p, 0, 8, ix->stream));
+    B200VS_CUDA(cudaMemsetAsync(d_len1.p, 0, 4, ix->stream));
+    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+  }
+  int64_t count() const { return rows - ndeleted; }
+  void publish_len() {
+    const int len = (int)std::min<int64_t>(rows, 0x7fffffff);
+    B200VS_CUDA(cudaMemcpyAsync(d_len1.p, &len, 4, cudaMemcpyHostToDevice, store.ix->stream));
+    B200VS_CUDA(cudaStreamSynchronize(store.ix->stream));
+  }
+  TcView view() const {
+    TcView v = store.view();
+    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
+    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
+    return v;
+  }
+
+  // the rows holding these ids become tombstones (unknown ids are ignored); returns how many
+  int64_t tombstone(int64_t n, const int64_t* del) {
+    std::vector<int64_t> dead;
+    for (int64_t i = 0; i < n; ++i) {
+      auto it = id2row.find(del[i]);
+      if (it != id2row.end()) { dead.push_back(it->second); id2row.erase(it); }
+    }
+    tombstone_ids(store.ix, store.ids.p, dead);
+    for (int64_t r : dead) h_ids[r] = -1;
+    ndeleted += (int64_t)dead.size();
+    return (int64_t)dead.size();
+  }
+  int64_t remove(int64_t n, const int64_t* del) {
+    const int64_t r = tombstone(n, del);
+    compact_if_needed();
+    return r;
+  }
+  void compact_if_needed() {
+    if (ndeleted == 0 || ndeleted * 2 < rows) return;
+    std::vector<long long> src, dst;
+    src.reserve(rows - ndeleted);
+    for (int64_t r = 0; r < rows; ++r) if (h_ids[r] >= 0) src.push_back(r);
+    const int64_t live = (int64_t)src.size();
+    dst.resize(live);
+    for (int64_t i = 0; i < live; ++i) dst[i] = i;
+    store.gather(src, dst, std::max<int64_t>(1024, live * 5 / 4));
+    std::vector<int64_t> nh(live);
+    id2row.clear();
+    for (int64_t i = 0; i < live; ++i) { nh[i] = h_ids[src[i]]; id2row[nh[i]] = i; }
+    h_ids.swap(nh);
+    rows = live; ndeleted = 0;
+    publish_len();
+  }
+  // VectorIndexFlat::AddOrUpsert, vector_index_flat.cc:121-162: rows holding one of the ids are removed first, then the n
+  // device rows x / ids_dev (ids_host: the same ids on the host, unique) are appended in order
+  template <class Row>
+  void add(int64_t n, const Row* x, const long long* ids_dev, const int64_t* ids_host) {
+    tombstone(n, ids_host);
+    const int64_t cap = (int64_t)store.ids.cap;
+    if (rows + n > cap) store.grow(std::max<int64_t>(rows + n, std::max<int64_t>(1024, cap * 3 / 2)), rows);
+    std::vector<long long> slots(n);
+    for (int64_t i = 0; i < n; ++i) slots[i] = rows + i;
+    store.write(x, ids_dev, slots);
+    B200VS_CUDA(cudaStreamSynchronize(store.ix->stream));
+    h_ids.resize(rows + n);
+    for (int64_t i = 0; i < n; ++i) { h_ids[rows + i] = ids_host[i]; id2row[ids_host[i]] = rows + i; }
+    rows += n;
+    publish_len();
+    compact_if_needed();
+  }
+  // drop every row, keep the buffers
+  void clear() {
+    rows = 0; ndeleted = 0;
+    h_ids.clear(); id2row.clear();
+    publish_len();
+  }
+  // the live rows in row order: out (rows in the store's host format, nullable) and out_ids (nullable).  Without
+  // tombstones the rows are downloaded straight into out, so a large export holds no second host copy.
+  void export_rows(int64_t* list_off, uint8_t* out, int64_t* out_ids) const {
+    if (list_off) { list_off[0] = 0; list_off[1] = count(); }
+    const size_t rb = store.row_bytes();
+    std::vector<uint8_t> all;
+    if (out && ndeleted) all.resize((size_t)rows * rb);
+    if (out) store.download(0, rows, ndeleted ? all.data() : out);
+    int64_t o = 0;
+    for (int64_t r = 0; r < rows; ++r) {
+      if (h_ids[r] < 0) continue;
+      if (out_ids) out_ids[o] = h_ids[r];
+      if (out && ndeleted) memcpy(out + (size_t)o * rb, all.data() + (size_t)r * rb, rb);
+      ++o;
+    }
+  }
+};
 
 struct ListMeta {
   int64_t off = 0;
@@ -28,21 +152,17 @@ struct IvfLists {
   std::vector<ListMeta> lists;
   std::vector<int64_t> h_ids;  // arena mirror of ids (-1 = tombstone / unused)
   std::unordered_multimap<int64_t, uint64_t> where;  // id -> (list << 32 | pos)
-  int64_t arena_used = 0, arena_used_before = 0, arena_cap = 0;
+  int64_t arena_used = 0, arena_cap = 0;
   int64_t live = 0, dead = 0, garbage = 0;
   int64_t total_chunks = 0;      // sum of ceil(len / 512) — tensor-core work-item bound (tc_scan.cuh TC_CHUNK = 512)
   int max_chunks_per_list = 0;
   DevBuf<long long> d_off;
   DevBuf<int> d_len;
-  // compaction plan
-  std::vector<ListMeta> plan_lists;
-  std::vector<int64_t> plan_ids;
-  int64_t plan_rows = 0;
 
   void init(int nlist, cudaStream_t s) {
     lists.assign(nlist, ListMeta());
     h_ids.clear(); where.clear();
-    arena_used = arena_used_before = arena_cap = 0;
+    arena_used = arena_cap = 0;
     live = dead = garbage = 0;
     d_off.free(); d_len.free();
     d_off.reserve(nlist, 0, s);
@@ -68,48 +188,60 @@ struct IvfLists {
 
   static int32_t round32(int64_t v) { return (int32_t)((v + 31) / 32 * 32); }
 
-  // make room for need[l] more rows in every list. grow(rows): enlarge payload arrays to `rows` keeping
-  // arena_used_before rows; move(src,dst,len): device copy of a relocated list.
-  template <class Grow, class Move>
-  void reserve_for(const std::vector<int>& need, Grow grow, Move move) {
-    struct Rel { int l; int64_t src, dst; int32_t len; };
+  void check_lists(int64_t n, const long long* h_list) const {
+    for (int64_t i = 0; i < n; ++i)
+      if (h_list[i] < 0 || h_list[i] >= (long long)lists.size()) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
+  }
+
+  // n rows go to the tails of their lists h_list: device rows x and ids ids_dev, the same ids on the host in h_ids_in.  A
+  // list without room is relocated to the arena tail with 1.5x capacity, and the arena grows by 1.5x when that runs out.
+  template <class Store, class Row>
+  void place(int64_t n, const long long* h_list, const int64_t* h_ids_in, const Row* x, const long long* ids_dev, Store& store) {
+    check_lists(n, h_list);
+    std::vector<int> need(lists.size(), 0);
+    for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
+    struct Rel { int64_t src, dst; int32_t len; };
     std::vector<Rel> rels;
-    arena_used_before = arena_used;
+    const int64_t used_before = arena_used;
     for (size_t l = 0; l < lists.size(); ++l) {
       if (need[l] == 0) continue;
       ListMeta& m = lists[l];
       if (m.len + need[l] <= m.cap) continue;
       const int32_t ncap = round32(std::max<int64_t>(64, ((int64_t)m.len + need[l]) * 3 / 2));
-      rels.push_back({(int)l, m.off, arena_used, m.len});
+      rels.push_back({m.off, arena_used, m.len});
       garbage += m.cap;
       m.off = arena_used; m.cap = ncap;
       arena_used += ncap;
     }
     if (arena_used > arena_cap) {
       const int64_t ncap = std::max<int64_t>(arena_used, arena_cap * 3 / 2);
-      grow(ncap);
+      store.grow(ncap, used_before);
       arena_cap = ncap;
     }
     h_ids.resize(arena_cap, -1);
     for (const Rel& r : rels) {
       if (r.len == 0) continue;
-      move(r.src, r.dst, (int64_t)r.len);
+      store.move(r.src, r.dst, (int64_t)r.len);
       std::copy(h_ids.begin() + r.src, h_ids.begin() + r.src + r.len, h_ids.begin() + r.dst);
     }
+    std::vector<long long> slots(n);
+    for (int64_t i = 0; i < n; ++i) {
+      const int l = (int)h_list[i];
+      ListMeta& m = lists[l];
+      slots[i] = m.off + m.len;
+      where.emplace(h_ids_in[i], ((uint64_t)l << 32) | (uint32_t)m.len);
+      h_ids[slots[i]] = h_ids_in[i];
+      m.len++;
+    }
+    live += n;
+    store.write(x, ids_dev, slots);
+    upload(store.ix->stream);
   }
 
-  int64_t append(int l, int64_t id) {
-    ListMeta& m = lists[l];
-    const int64_t row = m.off + m.len;
-    where.emplace(id, ((uint64_t)l << 32) | (uint32_t)m.len);
-    h_ids[row] = id;
-    m.len++;
-    live++;
-    return row;
-  }
-
-  // faiss remove_ids(IDSelectorBatch): every entry whose id matches is removed
-  void remove_ids(int64_t n, const int64_t* del, std::vector<int64_t>& rows) {
+  // faiss remove_ids(IDSelectorBatch): every row whose id matches becomes a tombstone; returns how many
+  template <class Store>
+  int64_t remove(int64_t n, const int64_t* del, Store& store) {
+    std::vector<int64_t> rows;
     for (int64_t i = 0; i < n; ++i) {
       auto range = where.equal_range(del[i]);
       for (auto it = range.first; it != range.second; ++it) {
@@ -124,19 +256,23 @@ struct IvfLists {
       }
       where.erase(range.first, range.second);
     }
+    tombstone_ids(store.ix, store.ids.p, rows);
+    return (int64_t)rows.size();
   }
 
-  bool needs_compaction() const { return garbage + dead > std::max<int64_t>(live, 4096); }
-
-  int64_t plan_compaction(std::vector<long long>& src, std::vector<long long>& dst) {
-    plan_lists.assign(lists.size(), ListMeta());
+  // when garbage and tombstones outweigh the live rows: a fresh arena, list by list in list order, each list holding its
+  // live rows in order with room for 1/4 more + 32
+  template <class Store>
+  void compact_if_needed(Store& store) {
+    if (garbage + dead <= std::max<int64_t>(live, 4096)) return;
+    std::vector<ListMeta> nl(lists.size());
+    std::vector<long long> src, dst;
     int64_t used = 0;
-    src.clear(); dst.clear();
     for (size_t l = 0; l < lists.size(); ++l) {
       const ListMeta& m = lists[l];
       const int32_t nlive = m.len - m.dead;
-      ListMeta& pm = plan_lists[l];
-      pm.off = used; pm.len = 0; pm.dead = 0;
+      ListMeta& pm = nl[l];
+      pm.off = used;
       pm.cap = nlive ? round32((int64_t)nlive * 5 / 4 + 32) : 0;
       for (int p = 0; p < m.len; ++p) {
         if (h_ids[m.off + p] < 0) continue;
@@ -146,21 +282,76 @@ struct IvfLists {
       }
       used += pm.cap;
     }
-    plan_rows = used;
-    plan_ids.assign(std::max<int64_t>(used, 1), -1);
-    for (size_t i = 0; i < src.size(); ++i) plan_ids[dst[i]] = h_ids[src[i]];
-    return used;
-  }
-  void commit_compaction() {
-    lists.swap(plan_lists);
-    h_ids.swap(plan_ids);
-    arena_used = arena_used_before = plan_rows;
-    arena_cap = std::max<int64_t>(plan_rows, 1);
+    std::vector<int64_t> nids(std::max<int64_t>(used, 1), -1);
+    for (size_t i = 0; i < src.size(); ++i) nids[dst[i]] = h_ids[src[i]];
+    store.gather(src, dst, std::max<int64_t>(used, 1));
+    lists.swap(nl);
+    h_ids.swap(nids);
+    arena_used = used;
+    arena_cap = std::max<int64_t>(used, 1);
     garbage = 0; dead = 0;
     where.clear();
     for (size_t l = 0; l < lists.size(); ++l)
       for (int p = 0; p < lists[l].len; ++p) where.emplace(h_ids[lists[l].off + p], ((uint64_t)l << 32) | (uint32_t)p);
-    plan_lists.clear(); plan_ids.clear();
+    upload(store.ix->stream);
+  }
+
+  // b200vs_reserve_lists on an empty index: one arena allocation holding every list at its final size (+ 1/16 slack), and a
+  // tail for lists that still outgrow their reservation, so bulk builds never relocate a list or re-allocate the arena.
+  // Every size is checked before anything changes.
+  template <class Store>
+  void reserve(const int64_t* rows_per_list, int n_lists, Store& store) {
+    if (n_lists != (int)lists.size()) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: list count does not match the trained index");
+    if (live + dead > 0) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists needs an empty index");
+    for (int l = 0; l < n_lists; ++l)
+      if (rows_per_list[l] < 0 || rows_per_list[l] >= (1LL << 31) - 64) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: bad list size");
+    int64_t used = 0;
+    for (int l = 0; l < n_lists; ++l) {
+      const int64_t want = rows_per_list[l];
+      ListMeta& m = lists[l];
+      m.off = used; m.len = 0; m.dead = 0;
+      m.cap = want ? round32(want + want / 16 + 32) : 0;
+      used += m.cap;
+    }
+    arena_used = used;
+    arena_cap = used + std::max<int64_t>(used / 64, 4096);
+    store.reset();
+    store.grow(arena_cap, 0);
+    B200VS_CUDA(cudaMemsetAsync(store.ids.p, 0xFF, (size_t)arena_cap * 8, store.ix->stream));  // id -1 = unused slot
+    h_ids.assign(arena_cap, -1);
+    upload(store.ix->stream);
+  }
+
+  // the live rows of list l in list order: the first `cap` of them go to out (the store's host format, nullable) and
+  // out_ids (nullable); returns how many there are.  An untrained index has no lists yet, so none.
+  template <class Store>
+  int64_t export_list(int l, int64_t cap, const Store& store, uint8_t* out, int64_t* out_ids) const {
+    if (l >= (int)lists.size()) return 0;
+    const ListMeta& m = lists[l];
+    const size_t rb = store.row_bytes();
+    std::vector<uint8_t> buf;
+    if (out && m.len) { buf.resize((size_t)m.len * rb); store.download(m.off, m.len, buf.data()); }
+    int64_t o = 0;
+    for (int p = 0; p < m.len; ++p) {
+      const int64_t id = h_ids[m.off + p];
+      if (id < 0) continue;
+      if (o < cap) {
+        if (out_ids) out_ids[o] = id;
+        if (out) memcpy(out + (size_t)o * rb, buf.data() + (size_t)p * rb, rb);
+      }
+      ++o;
+    }
+    return o;
+  }
+  // every list's live rows, list after list; list_off[nlist + 1] (nullable) gets where each list starts
+  template <class Store>
+  void export_lists(int nlist, int64_t* list_off, const Store& store, uint8_t* out, int64_t* out_ids) const {
+    int64_t o = 0;
+    for (int l = 0; l < nlist; ++l) {
+      if (list_off) list_off[l] = o;
+      o += export_list(l, INT64_MAX, store, out ? out + (size_t)o * store.row_bytes() : nullptr, out_ids ? out_ids + o : nullptr);
+    }
+    if (list_off) list_off[nlist] = o;
   }
 };
 

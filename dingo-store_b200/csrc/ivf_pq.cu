@@ -383,6 +383,56 @@ void launch_pq_scan_packed(int nbits, dim3 grid, size_t smem, cudaStream_t s, co
 
 }  // namespace
 
+// Device rows of an IVF-PQ arena: [cap, cs] code bytes and ids (-1 = tombstone / unused slot).  The owner decides
+// capacities and slots; the store moves rows.  All work runs on the owner's stream.
+struct CodeRows {
+  IndexBase* const ix;
+  int cs = 0;  // bytes per packed code row (set by the owner)
+  DevBuf<unsigned char> codes;
+  DevBuf<long long> ids;
+  explicit CodeRows(IndexBase* owner) : ix(owner) {}
+
+  void grow(int64_t cap, int64_t keep) {
+    codes.reserve((size_t)cap * cs, (size_t)keep * cs, ix->stream);
+    ids.reserve(cap, keep, ix->stream);
+  }
+  void reset() { codes.free(); ids.free(); }
+  void move(int64_t src, int64_t dst, int64_t n) {
+    B200VS_CUDA(cudaMemcpyAsync(codes.p + (size_t)dst * cs, codes.p + (size_t)src * cs, (size_t)n * cs, cudaMemcpyDeviceToDevice, ix->stream));
+    B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)n * 8, cudaMemcpyDeviceToDevice, ix->stream));
+  }
+  // x / xids: device code rows and ids; row i goes to slot slots[i]
+  void write(const unsigned char* x, const long long* xids, const std::vector<long long>& slots) {
+    const int64_t n = (int64_t)slots.size();
+    long long* d_slots = ix->scratch.alloc<long long>(n);
+    B200VS_CUDA(cudaMemcpyAsync(d_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ix->stream));
+    scatter_codes_kernel<<<(unsigned)cdiv(n * cs, 256), 256, 0, ix->stream>>>(x, xids, d_slots, n, cs, codes.p, ids.p);
+    B200VS_CUDA(cudaGetLastError());
+  }
+  // compaction: fresh buffers of cap rows holding row src[i] at dst[i]
+  void gather(const std::vector<long long>& src, const std::vector<long long>& dst, int64_t cap) {
+    const int64_t n = (int64_t)src.size();
+    DevBuf<unsigned char> nc; DevBuf<long long> ni;
+    nc.reserve((size_t)cap * cs, 0, ix->stream); ni.reserve(cap, 0, ix->stream);
+    if (n) {
+      long long* d_src = ix->scratch.alloc<long long>(n);
+      long long* d_dst = ix->scratch.alloc<long long>(n);
+      B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), n * 8, cudaMemcpyHostToDevice, ix->stream));
+      B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), n * 8, cudaMemcpyHostToDevice, ix->stream));
+      move_codes_kernel<<<(unsigned)cdiv(n * cs, 256), 256, 0, ix->stream>>>(codes.p, ids.p, d_src, d_dst, n, cs, nc.p, ni.p);
+      B200VS_CUDA(cudaGetLastError());
+    }
+    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+    codes.swap(nc); ids.swap(ni);
+  }
+  // rows [r0, r0 + n) as code rows [n, cs] on the host
+  size_t row_bytes() const { return (size_t)cs; }
+  void download(int64_t r0, int64_t n, uint8_t* out) const {
+    if (n > 0) B200VS_CUDA(cudaMemcpy(out, codes.p + (size_t)r0 * cs, (size_t)n * cs, cudaMemcpyDeviceToHost));
+  }
+  int64_t bytes() const { return (int64_t)(codes.cap + ids.cap * 8); }
+};
+
 struct IvfPqIndex : IndexBase {
   enum Mode { kNone, kFlat, kIvfPq } mode = kNone;
   int nlist, M, nbits;
@@ -390,8 +440,7 @@ struct IvfPqIndex : IndexBase {
   std::unique_ptr<IndexBase> flat;  // inner Flat index when there is too little data to train (ivf_pq.cc:339-353)
   DevBuf<float> centroids, codebooks, pre;
   DevBuf<long long> cent_ids;
-  DevBuf<unsigned char> codes;      // [rows, code_size]
-  DevBuf<long long> ids;
+  CodeRows store{this};             // the arena, [L.arena_cap] code rows
   IvfLists L;
 
   IvfPqIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_IVF_PQ, m, d, p) {
@@ -406,6 +455,7 @@ struct IvfPqIndex : IndexBase {
     if (d % M != 0) fail(B200VS_EILLEGAL_PARAMETERS, "dimension must be divisible by nsubvector");
     ksub = 1 << nbits;
     code_size = (M * nbits + 7) / 8;
+    store.cs = code_size;
   }
   bool is_trained() const override { return mode != kNone; }
   int sub_type() const override { return mode == kFlat ? (int)B200VS_FLAT : mode == kIvfPq ? (int)B200VS_IVF_PQ : -1; }  // ivf_pq.cc:474
@@ -426,7 +476,7 @@ struct IvfPqIndex : IndexBase {
     }
     B200VS_CUDA(cudaStreamSynchronize(stream));
     L.init(nlist, stream);
-    codes.free(); ids.free();
+    store.reset();
     mode = kIvfPq;
   }
 
@@ -601,7 +651,7 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
-    if (upsert) remove_locked(n, in_ids);
+    if (upsert) L.remove(n, in_ids, store);
     float* st = scratch.alloc<float>((size_t)n * dim);
     long long* st_ids = scratch.alloc<long long>(n);
     long long* st_list = scratch.alloc<long long>(n);
@@ -613,7 +663,7 @@ struct IvfPqIndex : IndexBase {
     std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
-    append_encoded(n, st_codes, st_ids, in_ids, h_list.data());
+    L.place(n, h_list.data(), in_ids, st_codes, st_ids, store);
   }
 
   // b200vs_add_with_ids_device: the host add's steps on device rows (upsert removes first; cosine rows are normalised on
@@ -629,7 +679,7 @@ struct IvfPqIndex : IndexBase {
     std::vector<int64_t> h_ids(n);
     B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
-    if (upsert) remove_locked(n, h_ids.data());
+    if (upsert) L.remove(n, h_ids.data(), store);
     const float* st = x_dev;
     if (metric == B200VS_COSINE && !prepared) {  // the normaliser works in place: keep the caller's rows intact
       float* cp = scratch.alloc<float>((size_t)n * dim);
@@ -646,10 +696,9 @@ struct IvfPqIndex : IndexBase {
     std::vector<long long> h_list(n);
     B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
-    for (int64_t i = 0; i < n; ++i)
-      if (h_list[i] < 0 || h_list[i] >= nlist) fail(B200VS_EILLEGAL_PARAMETERS, "list id out of range");
+    L.check_lists(n, h_list.data());  // before the encoder reads the lists' centroids
     const unsigned char* st_codes = encode_locked(n, st, st_list, wpb);
-    append_encoded(n, st_codes, ids_dev, h_ids.data(), h_list.data());
+    L.place(n, h_list.data(), h_ids.data(), st_codes, ids_dev, store);
   }
 
   // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
@@ -658,90 +707,15 @@ struct IvfPqIndex : IndexBase {
     assign_dev(centroids.p, nlist, cent_ids.p, x_dev, dim, metric == B200VS_L2, n, out_lists_dev, s);
   }
 
-  // one code + id arena holding every list at its final size (+ 1/16 slack), as IvfFlatIndex::reserve_lists
   void reserve_lists(const int64_t* rows_per_list, int n_lists) override {
     std::unique_lock<std::shared_mutex> wl(rw);
     require_lists();
-    if (n_lists != nlist) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: list count does not match the trained index");
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     quiesce();
-    if (L.live + L.dead > 0) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists needs an empty index");
-    for (int l = 0; l < nlist; ++l)
-      if (rows_per_list[l] < 0 || rows_per_list[l] >= (1LL << 31) - 64) fail(B200VS_EILLEGAL_PARAMETERS, "reserve_lists: bad list size");
-    int64_t used = 0;
-    for (int l = 0; l < nlist; ++l) {
-      const int64_t want = rows_per_list[l];
-      ListMeta& m = L.lists[l];
-      m.off = used; m.len = 0; m.dead = 0;
-      m.cap = want ? IvfLists::round32(want + want / 16 + 32) : 0;
-      used += m.cap;
-    }
-    const int64_t tail = std::max<int64_t>(used / 64, 4096);  // room for lists that still outgrow their reservation
-    L.arena_used = L.arena_used_before = used;
-    L.arena_cap = used + tail;
-    codes.free(); ids.free();
-    codes.reserve((size_t)L.arena_cap * code_size, 0, stream);
-    ids.reserve((size_t)L.arena_cap, 0, stream);
-    B200VS_CUDA(cudaMemsetAsync(ids.p, 0xFF, (size_t)L.arena_cap * 8, stream));  // id -1 = unused slot
-    L.h_ids.assign(L.arena_cap, -1);
-    L.upload(stream);
+    L.reserve(rows_per_list, n_lists, store);
   }
 
-  // rows already encoded (device codes [n, code_size], device ids) go to the tails of their lists; callers hold the write lock
-  void append_encoded(int64_t n, const unsigned char* d_codes, const long long* d_ids, const int64_t* h_ids_in, const long long* h_list) {
-    const size_t cs = (size_t)code_size;
-    std::vector<long long> slots(n);
-    long long* st_slots = scratch.alloc<long long>(n);
-    std::vector<int> need(nlist, 0);
-    for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
-    L.reserve_for(need, [&](int64_t rows) {
-      codes.reserve((size_t)rows * cs, (size_t)L.arena_used_before * cs, stream);
-      ids.reserve((size_t)rows, (size_t)L.arena_used_before, stream);
-    }, [&](int64_t src, int64_t dst, int64_t len) {
-      B200VS_CUDA(cudaMemcpyAsync(codes.p + (size_t)dst * cs, codes.p + (size_t)src * cs, (size_t)len * cs, cudaMemcpyDeviceToDevice, stream));
-      B200VS_CUDA(cudaMemcpyAsync(ids.p + dst, ids.p + src, (size_t)len * 8, cudaMemcpyDeviceToDevice, stream));
-    });
-    for (int64_t i = 0; i < n; ++i) slots[i] = L.append((int)h_list[i], h_ids_in[i]);
-    B200VS_CUDA(cudaMemcpyAsync(st_slots, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    scatter_codes_kernel<<<(unsigned)cdiv(n * code_size, 256), 256, 0, stream>>>(d_codes, d_ids, st_slots, n, code_size, codes.p, ids.p);
-    B200VS_CUDA(cudaGetLastError());
-    L.upload(stream);
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-  }
-
-  int64_t remove_locked(int64_t n, const int64_t* del) {
-    std::vector<int64_t> rws;
-    L.remove_ids(n, del, rws);
-    if (!rws.empty()) {
-      long long* d_rows = scratch.alloc<long long>(rws.size());
-      B200VS_CUDA(cudaMemcpyAsync(d_rows, rws.data(), rws.size() * 8, cudaMemcpyHostToDevice, stream));
-      launch_set_ids(ids.p, d_rows, (int64_t)rws.size(), -1, stream);
-      B200VS_CUDA(cudaStreamSynchronize(stream));
-    }
-    return (int64_t)rws.size();
-  }
-  void maybe_compact() {
-    if (!L.needs_compaction()) return;
-    std::vector<long long> src, dst;
-    const int64_t new_rows = std::max<int64_t>(1, L.plan_compaction(src, dst));
-    DevBuf<unsigned char> nc; DevBuf<long long> ni;
-    nc.reserve((size_t)new_rows * code_size, 0, stream); ni.reserve(new_rows, 0, stream);
-    const int64_t m = (int64_t)src.size();
-    if (m) {
-      long long* d_src = scratch.alloc<long long>(m);
-      long long* d_dst = scratch.alloc<long long>(m);
-      B200VS_CUDA(cudaMemcpyAsync(d_src, src.data(), m * 8, cudaMemcpyHostToDevice, stream));
-      B200VS_CUDA(cudaMemcpyAsync(d_dst, dst.data(), m * 8, cudaMemcpyHostToDevice, stream));
-      move_codes_kernel<<<(unsigned)cdiv(m * code_size, 256), 256, 0, stream>>>(codes.p, ids.p, d_src, d_dst, m, code_size, nc.p, ni.p);
-      B200VS_CUDA(cudaGetLastError());
-    }
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    std::swap(codes.p, nc.p); std::swap(codes.cap, nc.cap);
-    std::swap(ids.p, ni.p); std::swap(ids.cap, ni.cap);
-    L.commit_compaction();
-    L.upload(stream);
-  }
   int64_t remove(int64_t n, const int64_t* del) override {
     if (mode == kFlat) { const int64_t r = flat->remove(n, del); return r == 0 ? -1 : r; }  // Flat semantics: unknown ids are OK
     std::unique_lock<std::shared_mutex> wl(rw);
@@ -750,8 +724,8 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
-    const int64_t r = remove_locked(n, del);
-    maybe_compact();
+    const int64_t r = L.remove(n, del, store);
+    L.compact_if_needed(store);
     return r;
   }
 
@@ -812,7 +786,7 @@ struct IvfPqIndex : IndexBase {
     float* sim = scratch.alloc<float>((size_t)nq * T);
     pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, ksub, sim);
     PqScanArgs a;
-    a.codes = codes.p; a.ids = ids.p; a.probes = probes; a.coarse = coarse; a.list_off = L.d_off.p; a.list_len = L.d_len.p;
+    a.codes = store.codes.p; a.ids = store.ids.p; a.probes = probes; a.coarse = coarse; a.list_off = L.d_off.p; a.list_len = L.d_len.p;
     a.sim = sim; a.pre = l2 ? pre.p : nullptr; a.M = M; a.code_size = code_size; a.nprobe = nprobe; a.k = k;
     a.nsplit = (int)std::max<int64_t>(1, std::min<int64_t>(nprobe, (device_sm_count(device) * 2 + nq - 1) / nq));
     a.pool_cap = pool_cap;
@@ -922,7 +896,7 @@ struct IvfPqIndex : IndexBase {
   int64_t deleted_count() const override { return mode == kFlat ? flat->deleted_count() : L.dead; }
   int64_t memory_size() const override {
     if (mode == kFlat) return flat->memory_size();
-    return (int64_t)(codes.cap + ids.cap * 8 + centroids.cap * 4 + codebooks.cap * 4 + pre.cap * 4);  // raw_ivf_pq.cc:440-450
+    return store.bytes() + (int64_t)(centroids.cap * 4 + codebooks.cap * 4 + pre.cap * 4);  // raw_ivf_pq.cc:440-450
   }
   // Save / Load (reference: faiss::write_index / read_index of the IndexIVFPQ, vector_index_raw_ivf_pq.cc:298 and :314): own
   // container "B2VSPQ01" = mode, then either the inner Flat index's rows or {trained-state blob, list offsets, ids,
@@ -1002,7 +976,7 @@ struct IvfPqIndex : IndexBase {
           long long* d_ids = scratch.alloc<long long>(m);
           B200VS_CUDA(cudaMemcpyAsync(d_codes, cds.data() + (size_t)a * code_size, (size_t)m * code_size, cudaMemcpyHostToDevice, stream));
           B200VS_CUDA(cudaMemcpyAsync(d_ids, fids.data() + a, (size_t)m * 8, cudaMemcpyHostToDevice, stream));
-          append_encoded(m, d_codes, d_ids, fids.data() + a, h_list.data() + a);
+          L.place(m, h_list.data() + a, fids.data() + a, d_codes, d_ids, store);
         }
       }
     } catch (...) { fclose(f); throw; }
@@ -1014,26 +988,8 @@ struct IvfPqIndex : IndexBase {
     RwSharedGuard rl(this);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
-    std::vector<unsigned char> buf;
-    int64_t o = 0;
-    for (int l = 0; l < nlist; ++l) {
-      if (list_off) list_off[l] = o;
-      const auto& m = L.lists[l];
-      if (m.len == 0) continue;
-      const size_t cs = (size_t)code_size;
-      if (out_codes) {
-        buf.resize((size_t)m.len * cs);
-        B200VS_CUDA(cudaMemcpy(buf.data(), codes.p + (size_t)m.off * cs, (size_t)m.len * cs, cudaMemcpyDeviceToHost));
-      }
-      for (int p = 0; p < m.len; ++p) {
-        const int64_t id = L.h_ids[m.off + p];
-        if (id < 0) continue;
-        if (out_ids) out_ids[o] = id;
-        if (out_codes) memcpy(out_codes + (size_t)o * cs, buf.data() + (size_t)p * cs, cs);
-        ++o;
-      }
-    }
-    if (list_off) list_off[nlist] = o;
+    quiesce();
+    L.export_lists(nlist, list_off, store, out_codes, out_ids);
   }
 };
 

@@ -89,6 +89,37 @@ def test_device_add_assign_and_reserved_lists(oracle):
     assert_same_results(D, I, Dr, Ir)
 
 
+@pytest.mark.parametrize("kind,extra", [(b200vs.IVF_FLAT, {}), (b200vs.IVF_PQ, {"pq_m": 8, "pq_nbits": 4})])
+def test_refused_reservation_leaves_the_index_unchanged(kind, extra):
+    """b200vs_reserve_lists checks every list size before it changes anything: refused for one negative size behind a valid
+    prefix, it leaves the index empty at its old memory size, and later adds and searches answer exactly like an index
+    that was never reserved."""
+    require_gpu()
+    n, d, nlist, nq, k, nprobe = 20000, 32, 16, 64, 10, 4
+    rng = np.random.default_rng(11)
+    xb = rng.random((n, d)).astype(np.float32)
+    ids = np.arange(1, n + 1, dtype=np.int64)
+    ref = b200vs.Index(kind, b200vs.L2, d, nlist=nlist, **extra)
+    ref.train(xb)
+    assert ref.sub_type() == kind
+    ix = b200vs.Index(kind, b200vs.L2, d, nlist=nlist, **extra)
+    ix.set_trained_state(ref.get_trained_state())
+    count0, mem0 = ix.get_count(), ix.get_memory_size()
+    sizes = np.full(nlist, 1000, np.int64)
+    sizes[1] = -1
+    with pytest.raises(b200vs.B200VSError) as e:
+        ix.reserve_lists(sizes)
+    assert e.value.code == b200vs.EILLEGAL_PARAMETERS
+    assert ix.get_count() == count0 == 0
+    assert ix.get_memory_size() == mem0
+    ref.add(xb, ids)
+    ix.add(xb, ids)
+    xq = rng.random((nq, d)).astype(np.float32)
+    D, I = ix.search(xq, k, nprobe=nprobe)
+    Dr, Ir = ref.search(xq, k, nprobe=nprobe)
+    assert_same_results(D, I, Dr, Ir)
+
+
 def test_two_ranks_match_oracle():
     """torchrun --nproc-per-node 2: NCCL rendezvous through the ABI, row routing, sharded search == oracle on the gathered index."""
     require_gpu()
