@@ -31,6 +31,85 @@ void check_search_args(IndexBase* ix, int64_t nq, const void* xq, const b200vs_s
     fail(B200VS_EILLEGAL_PARAMETERS, "efsearch is illegal, " + std::to_string(sp->efsearch) + ", must between 0 and 1024");  // hnsw.cc:332-336
 }
 
+// The prologue and epilogue of every read of one index: the shared lock, the device, a lane on `stream` (null: the lane's
+// own stream), fresh stats and the resolved search parameters, then body(sc, s) on the lane's stream, the profiling phases,
+// and for a null stream the wait for the results.
+template <class Body>
+void index_read(IndexBase* ix, void* stream, const b200vs_search_params* sp, Body body) {
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  ix->set_device();
+  LaneGuard lane(ix, (cudaStream_t)stream);
+  const cudaStream_t s = lane.stream;
+  ix->reset_stats();
+  const SearchCtx sc = make_ctx(ix, sp, s);
+  body(sc, s);
+  ix->phases_finish(s);
+  if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));  // NULL stream: library-owned stream, results ready on return
+}
+
+// One host-pointer read: nq query rows of query_row_bytes() (floats, or packed bits on a binary index) go up, the index
+// answers into scratch, and the results come down into out_dist / out_ids [nq, k] (and, for a range search, out_counts
+// [nq]).  A NaN radius admits no row of a float index: empty results, nothing launched (DESIGN.md 4.6); a binary index
+// refuses it.  xq / outputs may be pinned staging (coalesced batches) or caller memory.
+void host_read(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids,
+               bool range = false, float radius = 0.f, int32_t* out_counts = nullptr) {
+  index_read(ix, nullptr, sp, [&](const SearchCtx& sc, cudaStream_t s) {
+    const size_t nk = (size_t)nq * k;
+    if (range && std::isnan(radius) && !ix->binary()) {
+      std::fill_n(out_dist, nk, 0.0F);
+      std::fill_n(out_ids, nk, (int64_t)-1);
+      std::fill_n(out_counts, (size_t)nq, 0);
+      return;
+    }
+    const size_t qbytes = (size_t)nq * ix->query_row_bytes();
+    SearchReq r;
+    r.nq = nq; r.k = k; r.range = range; r.radius = radius; r.sc = &sc;
+    void* dq = ix->scratch.alloc<unsigned char>(qbytes);
+    r.xq = dq;
+    r.od = ix->scratch.alloc<float>(nk);
+    r.oi = ix->scratch.alloc<long long>(nk);
+    if (range) r.oc = ix->scratch.alloc<int>((size_t)nq);
+    B200VS_CUDA(cudaMemcpyAsync(dq, xq, qbytes, cudaMemcpyHostToDevice, s));
+    ix->search(r, s);
+    ix->phases_finish(s);  // the phases end before the copies back
+    B200VS_CUDA(cudaMemcpyAsync(out_dist, r.od, nk * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(out_ids, r.oi, nk * 8, cudaMemcpyDeviceToHost, s));
+    if (range) B200VS_CUDA(cudaMemcpyAsync(out_counts, r.oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+  });
+}
+
+// b200vs_search_device / b200vs_search_binary_device
+int search_device(b200vs_index* h, int64_t nq, const void* xq_dev, int k, const b200vs_search_params* sp, float* out_dist_dev,
+                  int64_t* out_ids_dev, void* stream, bool binary) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, binary);
+    check_search_args(ix, nq, xq_dev, sp);
+    if (k <= 0) return B200VS_OK;  // "topk <= 0 -> OK", flat.cc:212
+    if (!out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    index_read(ix, stream, sp, [&](const SearchCtx& sc, cudaStream_t s) {
+      SearchReq r;
+      r.nq = nq; r.xq = xq_dev; r.k = k; r.sc = &sc; r.od = out_dist_dev; r.oi = (long long*)out_ids_dev;
+      ix->search(r, s);
+    });
+    return B200VS_OK;
+  });
+}
+
+// b200vs_range_search / b200vs_range_search_binary
+int range_search(b200vs_index* h, int64_t nq, const void* xq, float radius, int max_results, const b200vs_search_params* sp,
+                 float* out_dist, int64_t* out_ids, int32_t* out_counts, bool binary) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, binary);
+    check_search_args(ix, nq, xq, sp);
+    if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // hnsw.cc:487-493
+    if (max_results <= 0 || !out_ids || !out_dist || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
+    host_read(ix, nq, xq, max_results, sp, out_dist, out_ids, true, radius, out_counts);
+    return B200VS_OK;
+  });
+}
+
 }  // namespace
 
 extern "C" {
@@ -177,23 +256,7 @@ int b200vs_remove_ids(b200vs_index* h, int64_t n, const int64_t* ids, int64_t* n
 
 int b200vs_search_device(b200vs_index* h, int64_t nq, const float* xq_dev, int32_t k, const b200vs_search_params* sp,
                          float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, false);
-    check_search_args(ix, nq, xq_dev, sp);
-    if (k <= 0) return B200VS_OK;  // "topk <= 0 -> OK", flat.cc:212
-    if (!out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, (cudaStream_t)stream);
-    cudaStream_t s = lane.stream;
-    ix->reset_stats();
-    SearchCtx sc = make_ctx(ix, sp, s);
-    ix->search_dev(nq, xq_dev, k, sc, out_dist_dev, (long long*)out_ids_dev, s);
-    ix->phases_finish(s);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));  // NULL stream: library-owned stream, results ready on return
-    return B200VS_OK;
-  });
+  return search_device(h, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, false);
 }
 
 int b200vs_coarse_device(b200vs_index* h, int64_t nq, const float* xq_dev, int32_t nprobe, int32_t list_begin, int32_t list_end,
@@ -201,13 +264,9 @@ int b200vs_coarse_device(b200vs_index* h, int64_t nq, const float* xq_dev, int32
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (nq <= 0 || !xq_dev || !out_score_dev || !out_lists_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad coarse arguments");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, (cudaStream_t)stream);
-    ix->reset_stats();
-    ix->coarse_range_dev(nq, xq_dev, nprobe, list_begin, list_end, out_score_dev, (long long*)out_lists_dev, lane.stream);
-    ix->phases_finish(lane.stream);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(lane.stream));
+    index_read(ix, stream, nullptr, [&](const SearchCtx&, cudaStream_t s) {
+      ix->coarse(nq, xq_dev, false, nprobe, list_begin, list_end, out_score_dev, (long long*)out_lists_dev, s);
+    });
     return B200VS_OK;
   });
 }
@@ -219,14 +278,12 @@ int b200vs_search_probes_device(b200vs_index* h, int64_t nq, const float* xq_dev
     check_search_args(ix, nq, xq_dev, sp);
     if (k <= 0) return B200VS_OK;
     if (!probes_dev || nprobe <= 0 || !out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad probe arguments");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, (cudaStream_t)stream);
-    ix->reset_stats();
-    SearchCtx sc = make_ctx(ix, sp, lane.stream);
-    ix->search_probes_dev(nq, xq_dev, k, (const long long*)probes_dev, nprobe, sc, out_dist_dev, (long long*)out_ids_dev, lane.stream);
-    ix->phases_finish(lane.stream);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(lane.stream));
+    index_read(ix, stream, sp, [&](const SearchCtx& sc, cudaStream_t s) {
+      SearchReq r;
+      r.nq = nq; r.xq = xq_dev; r.probes = (const long long*)probes_dev; r.nprobe = nprobe; r.k = k; r.sc = &sc;
+      r.od = out_dist_dev; r.oi = (long long*)out_ids_dev;
+      ix->search(r, s);
+    });
     return B200VS_OK;
   });
 }
@@ -240,14 +297,11 @@ int b200vs_debug_tc_scores(b200vs_index* h, int64_t nq, const float* xq, int32_t
     if (nq <= 0 || !xq || !out_scores || !out_eps) fail(B200VS_EILLEGAL_PARAMETERS, "bad diagnostic arguments");
     if (split < 0 || split > 4) fail(B200VS_EILLEGAL_PARAMETERS, "split must be 0, 1, 2, 3 or 4");
     if ((split == 2 || split == 4) && ix->dim % 8 != 0) fail(B200VS_EILLEGAL_PARAMETERS, "the FP16 arithmetic needs dim % 8 == 0");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, nullptr);
-    cudaStream_t s = lane.stream;
-    ix->reset_stats();
-    float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
-    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * ix->dim * 4, cudaMemcpyHostToDevice, s));
-    ix->debug_tc_scores(nq, dq, split, out_scores, out_eps, s);
+    index_read(ix, nullptr, nullptr, [&](const SearchCtx&, cudaStream_t s) {
+      float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
+      B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * ix->dim * 4, cudaMemcpyHostToDevice, s));
+      ix->debug_tc_scores(nq, dq, split, out_scores, out_eps, s);
+    });
     return B200VS_OK;
   });
 }
@@ -255,28 +309,6 @@ int b200vs_debug_tc_scores(b200vs_index* h, int64_t nq, const float* xq, int32_t
 }  // extern "C"
 
 namespace {
-
-// one host-pointer search: H2D, search, D2H, wait.  xq / outputs may be pinned staging (coalesced batches) or caller memory.
-// xq holds nq rows of ix->query_row_bytes(): floats, or packed bits on a binary index.
-void host_search_once(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  ix->set_device();
-  LaneGuard lane(ix, nullptr);  // a free lane on its own stream, so concurrent callers overlap
-  cudaStream_t s = lane.stream;
-  ix->reset_stats();
-  const size_t qbytes = (size_t)nq * ix->query_row_bytes();
-  unsigned char* dq = ix->scratch.alloc<unsigned char>(qbytes);
-  float* dd = ix->scratch.alloc<float>((size_t)nq * k);
-  long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-  B200VS_CUDA(cudaMemcpyAsync(dq, xq, qbytes, cudaMemcpyHostToDevice, s));
-  SearchCtx sc = make_ctx(ix, sp, s);
-  if (ix->binary()) ix->search_binary_dev(nq, dq, k, sc, dd, di, s);
-  else ix->search_dev(nq, reinterpret_cast<const float*>(dq), k, sc, dd, di, s);
-  ix->phases_finish(s);
-  B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaStreamSynchronize(s));
-}
 
 bool coalesce_compatible(const CoalesceReq& a, const CoalesceReq& b) {
   return a.k == b.k && a.sp.nprobe == b.sp.nprobe && a.sp.efsearch == b.sp.efsearch && a.sp.exact_only == b.sp.exact_only &&
@@ -309,7 +341,7 @@ void run_coalesced(IndexBase* ix, std::vector<CoalesceReq*>& batch) {
   int64_t* hi = reinterpret_cast<int64_t*>(reinterpret_cast<char*>(hd) + ((dbytes + 15) & ~(size_t)15));
   int64_t off = 0;
   for (auto* r : batch) { memcpy(hq + (size_t)off * row, r->xq, (size_t)r->nq * row); off += r->nq; }
-  host_search_once(ix, total, hq, k, &batch[0]->sp, hd, hi);
+  host_read(ix, total, hq, k, &batch[0]->sp, hd, hi);
   off = 0;
   for (auto* r : batch) {
     memcpy(r->out_dist, hd + (size_t)off * k, (size_t)r->nq * k * 4);
@@ -340,7 +372,7 @@ int coalesced_search(IndexBase* ix, int64_t nq, const void* xq, int k, const b20
     int rc = B200VS_OK;
     std::string err;
     try {
-      if (batch.size() == 1) host_search_once(ix, batch[0]->nq, batch[0]->xq, batch[0]->k, &batch[0]->sp, batch[0]->out_dist, batch[0]->out_ids);
+      if (batch.size() == 1) host_read(ix, batch[0]->nq, batch[0]->xq, batch[0]->k, &batch[0]->sp, batch[0]->out_dist, batch[0]->out_ids);
       else run_coalesced(ix, batch);
     } catch (const StatusError& e) { rc = e.code; err = e.msg; }
     catch (const std::exception& e) { rc = B200VS_EINTERNAL; err = e.what(); }
@@ -357,13 +389,21 @@ int coalesced_search(IndexBase* ix, int64_t nq, const void* xq, int k, const b20
   return me.rc;
 }
 
-// the host-pointer search of b200vs_search and b200vs_search_binary (arguments already checked)
-int host_search(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids) {
-  // small filter-free requests share batches with concurrent callers (the reference issues one query per pool task)
-  if (nq <= kCoalesceMaxReq && ix->coalescer.enabled.load() && !(sp && sp->sorted_ids) && !ix->profiling)
-    return coalesced_search(ix, nq, xq, k, sp, out_dist, out_ids);
-  host_search_once(ix, nq, xq, k, sp, out_dist, out_ids);
-  return B200VS_OK;
+// b200vs_search / b200vs_search_binary: small filter-free requests share batches with concurrent callers (the reference
+// issues one query per pool task)
+int host_search(b200vs_index* h, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids,
+                bool binary) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, binary);
+    check_search_args(ix, nq, xq, sp);
+    if (k <= 0) return B200VS_OK;
+    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    if (nq <= kCoalesceMaxReq && ix->coalescer.enabled.load() && !(sp && sp->sorted_ids) && !ix->profiling)
+      return coalesced_search(ix, nq, xq, k, sp, out_dist, out_ids);
+    host_read(ix, nq, xq, k, sp, out_dist, out_ids);
+    return B200VS_OK;
+  });
 }
 
 }  // namespace
@@ -372,14 +412,7 @@ extern "C" {
 
 int b200vs_search(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                   int64_t* out_ids) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, false);
-    check_search_args(ix, nq, xq, sp);
-    if (k <= 0) return B200VS_OK;
-    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    return host_search(ix, nq, xq, k, sp, out_dist, out_ids);
-  });
+  return host_search(h, nq, xq, k, sp, out_dist, out_ids, false);
 }
 
 /* Request coalescing of b200vs_search and b200vs_search_binary (on by default): concurrent host-pointer calls of <= 64
@@ -396,37 +429,7 @@ int b200vs_set_coalescing(b200vs_index* h, int on, int64_t stats[2]) {
 
 int b200vs_range_search(b200vs_index* h, int64_t nq, const float* xq, float radius, int32_t max_results,
                         const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, false);
-    check_search_args(ix, nq, xq, sp);
-    if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // hnsw.cc:487-493
-    if (max_results <= 0 || !out_ids || !out_dist || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, nullptr);
-    cudaStream_t s = lane.stream;
-    ix->reset_stats();
-    if (std::isnan(radius)) {  // dis < NaN and ip > 1 - NaN hold for no row: empty results, nothing launched (DESIGN.md 4.6)
-      std::fill_n(out_dist, (size_t)nq * max_results, 0.0F);
-      std::fill_n(out_ids, (size_t)nq * max_results, (int64_t)-1);
-      std::fill_n(out_counts, (size_t)nq, 0);
-      return B200VS_OK;
-    }
-    float* dq = ix->scratch.alloc<float>((size_t)nq * ix->dim);
-    float* dd = ix->scratch.alloc<float>((size_t)nq * max_results);
-    long long* di = ix->scratch.alloc<long long>((size_t)nq * max_results);
-    int* dc = ix->scratch.alloc<int>((size_t)nq);
-    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * ix->dim * 4, cudaMemcpyHostToDevice, s));
-    SearchCtx sc = make_ctx(ix, sp, s);
-    ix->range_search_dev(nq, dq, radius, max_results, sc, dd, di, dc, s);
-    ix->phases_finish(s);
-    B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * max_results * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * max_results * 8, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    return B200VS_OK;
-  });
+  return range_search(h, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, false);
 }
 
 int b200vs_reconstruct(b200vs_index* h, int64_t n, const int64_t* ids, float* out, uint8_t* found) {
@@ -637,14 +640,11 @@ int b200vs_scan_push(b200vs_scan* st, int64_t n, const float* x, const int64_t* 
     const size_t nk = (size_t)st->nq * st->k;
     if (st->pushed > 0) ix->clear();
     ix->add(n, x, ids, false);  // one temporary Flat index per tile, as the reference builds (vector_reader.cc:1937-1946)
-    {
-      std::shared_lock<std::shared_mutex> rl(ix->rw);
-      ix->set_device();
-      LaneGuard lane(ix, st->s);
-      ix->reset_stats();
-      SearchCtx sc = make_ctx(ix, st->has_sp ? &st->sp : nullptr, st->s);
-      ix->search_dev(st->nq, st->q.p, st->k, sc, st->parts_d.p + nk, st->parts_i.p + nk, st->s);
-    }
+    index_read(ix, st->s, st->has_sp ? &st->sp : nullptr, [&](const SearchCtx& sc, cudaStream_t s) {
+      SearchReq r;
+      r.nq = st->nq; r.xq = st->q.p; r.k = st->k; r.sc = &sc; r.od = st->parts_d.p + nk; r.oi = st->parts_i.p + nk;
+      ix->search(r, s);
+    });
     // running top-k <- merge(running, tile): the reference's per-query priority queues (:1956-1971)
     launch_merge_api(2, st->nq, st->k, st->parts_d.p, st->parts_i.p, st->out_d.p, st->out_i.p, st->s);
     B200VS_CUDA(cudaMemcpyAsync(st->parts_d.p, st->out_d.p, nk * 4, cudaMemcpyDeviceToDevice, st->s));
@@ -797,62 +797,17 @@ int b200vs_add_with_ids_binary(b200vs_index* h, int64_t n, const uint8_t* x, con
 
 int b200vs_search_binary_device(b200vs_index* h, int64_t nq, const uint8_t* xq_dev, int32_t k, const b200vs_search_params* sp,
                                 float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, true);
-    check_search_args(ix, nq, xq_dev, sp);
-    if (k <= 0) return B200VS_OK;
-    if (!out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, (cudaStream_t)stream);
-    ix->reset_stats();
-    SearchCtx sc = make_ctx(ix, sp, lane.stream);
-    ix->search_binary_dev(nq, xq_dev, k, sc, out_dist_dev, (long long*)out_ids_dev, lane.stream);
-    ix->phases_finish(lane.stream);
-    if (!stream) B200VS_CUDA(cudaStreamSynchronize(lane.stream));
-    return B200VS_OK;
-  });
+  return search_device(h, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, true);
 }
 
 int b200vs_search_binary(b200vs_index* h, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                          int64_t* out_ids) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, true);
-    check_search_args(ix, nq, xq, sp);
-    if (k <= 0) return B200VS_OK;
-    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-    return host_search(ix, nq, xq, k, sp, out_dist, out_ids);
-  });
+  return host_search(h, nq, xq, k, sp, out_dist, out_ids, true);
 }
 
 int b200vs_range_search_binary(b200vs_index* h, int64_t nq, const uint8_t* xq, float radius, int32_t max_results,
                                const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
-  return guarded([&]() -> int {
-    IndexBase* ix = get(h);
-    check_row_type(ix, true);
-    check_search_args(ix, nq, xq, sp);
-    if (max_results <= 0 || !out_ids || !out_dist || !out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    LaneGuard lane(ix, nullptr);
-    cudaStream_t s = lane.stream;
-    ix->reset_stats();
-    uint8_t* dq = ix->scratch.alloc<uint8_t>((size_t)nq * (ix->dim / 8));
-    float* dd = ix->scratch.alloc<float>((size_t)nq * max_results);
-    long long* di = ix->scratch.alloc<long long>((size_t)nq * max_results);
-    int* dc = ix->scratch.alloc<int>((size_t)nq);
-    B200VS_CUDA(cudaMemcpyAsync(dq, xq, (size_t)nq * (ix->dim / 8), cudaMemcpyHostToDevice, s));
-    SearchCtx sc = make_ctx(ix, sp, s);
-    ix->range_search_binary_dev(nq, dq, radius, max_results, sc, dd, di, dc, s);
-    ix->phases_finish(s);
-    B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * max_results * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * max_results * 8, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    return B200VS_OK;
-  });
+  return range_search(h, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, true);
 }
 
 int b200vs_last_phase_times(b200vs_index* h, float ms[16]) {

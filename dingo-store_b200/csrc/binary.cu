@@ -126,9 +126,6 @@ struct BinaryIndex : IndexBase {
   BinaryIndex(b200vs_type t, int d, const b200vs_params& p) : IndexBase(t, B200VS_HAMMING, d, p), nb(d / 8), w(words_of(d)) {}
 
   void add(int64_t, const float*, const int64_t*, bool) override { fail(B200VS_EILLEGAL_PARAMETERS, "float entry point on a binary index"); }
-  void search_dev(int64_t, const float*, int, const SearchCtx&, float*, long long*, cudaStream_t) override {
-    fail(B200VS_EILLEGAL_PARAMETERS, "float entry point on a binary index");
-  }
 
   // packed device rows -> padded words in scratch
   const uint32_t* pad(int64_t n, const uint8_t* x_dev, cudaStream_t s) {
@@ -153,9 +150,16 @@ struct BinaryIndex : IndexBase {
   }
   // IndexBinary::range_search takes an int radius (flat.cc:304-308): the float is truncated toward zero, and hits have
   // dis < radius.  Every radius above dim + 1 admits the same rows, so larger values (and +inf) are clamped there first.
-  float radius_threshold(float radius) const {
-    if (std::isnan(radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");
-    return std::trunc(std::min(radius, (float)(dim + 1)));
+  // The threshold of a range search (0 for top-k); a NaN radius is refused before anything is launched.
+  float radius_threshold(const SearchReq& r) const {
+    if (!r.range) return 0.f;
+    if (std::isnan(r.radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");
+    return std::trunc(std::min(r.radius, (float)(dim + 1)));
+  }
+  // the exact scan j of a top-k search (the timed dominant scan), or of a range search with threshold thr
+  static void finish_job(const SearchReq& r, float thr, ScanJob& j) {
+    if (r.range) { j.has_thr = true; j.thr_raw = thr; }
+    else j.dominant = true;
   }
 
 };
@@ -197,25 +201,21 @@ struct BinaryFlatIndex : BinaryIndex {
     j.sc = &sc;
     return j;
   }
-  void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
-    const uint32_t* q = pad(nq, xq, s);
+  // Search / RangeSearch (flat.cc:206-323): Hamming distances are exact, so od is the raw key too
+  void search(const SearchReq& r, cudaStream_t s) override {
+    refuse_probes(r);
+    const float thr = radius_threshold(r);
+    const uint32_t* q = pad(r.nq, static_cast<const uint8_t*>(r.xq), s);
     const TcView v = rowmap.view();
-    if (bt_eligible(v, nq, k, 1, (double)rowmap.rows, sc)) {
-      long long* probes = scratch.alloc<long long>(nq);
-      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
-      bt_search(this, v, w, nq, q, k, probes, 1, job(sc), od, oi, s);
+    ScanJob j = job(*r.sc);
+    if (!r.range && bt_eligible(v, r.nq, r.k, 1, (double)rowmap.rows, *r.sc)) {
+      long long* probes = scratch.alloc<long long>(r.nq);
+      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)r.nq * 8, s));
+      bt_search(this, v, w, r.nq, q, r.k, probes, 1, j, r.od, r.oi, s);
       return;
     }
-    ScanJob j = job(sc);
-    j.dominant = true;
-    run_scan(this, j, nq, reinterpret_cast<const float*>(q), k, od, nullptr, oi, nullptr, s);
-  }
-  void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                               long long* oi, int* oc, cudaStream_t s) override {
-    ScanJob j = job(sc);
-    j.has_thr = true;
-    j.thr_raw = radius_threshold(radius);
-    run_scan(this, j, nq, reinterpret_cast<const float*>(pad(nq, xq, s)), max_results, od, nullptr, oi, oc, s);
+    finish_job(r, thr, j);
+    run_scan(this, j, r.nq, reinterpret_cast<const float*>(q), r.k, r.od, nullptr, r.oi, r.oc, s);
   }
   int64_t count() const override { return rowmap.count(); }
   int64_t deleted_count() const override { return rowmap.ndeleted; }
@@ -351,7 +351,7 @@ struct BinaryIvfIndex : BinaryIndex {
     return std::min(np, nlist);                    // ivf_flat.cc:234
   }
   // IndexBinaryFlat quantiser: the nprobe nearest lists by (Hamming distance, list id)
-  long long* coarse(int64_t nq, const uint32_t* q, int nprobe, cudaStream_t s, long long* out = nullptr) {
+  long long* coarse_lists(int64_t nq, const uint32_t* q, int nprobe, cudaStream_t s, long long* out = nullptr) {
     long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
     run_scan(this, hamming_job(cent.p, cent_ids.p, nlist), nq, reinterpret_cast<const float*>(q), nprobe, nullptr, nullptr, probes, nullptr, s);
     return probes;
@@ -384,7 +384,7 @@ struct BinaryIvfIndex : BinaryIndex {
     long long* lists = scratch.alloc<long long>(n);
     for (int64_t a = 0; a < n; a += 32768) {
       const auto mark = scratch.mark();  // each chunk's select workspace is handed back before the next
-      coarse(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, stream, lists + a);
+      coarse_lists(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, stream, lists + a);
       scratch.release(mark);
     }
     std::vector<long long> h_list(n);
@@ -405,37 +405,25 @@ struct BinaryIvfIndex : BinaryIndex {
     return r;
   }
 
-  void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
-    if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_flat.cc:224-227
-    const uint32_t* q = pad(nq, xq, s);
+  // Search / RangeSearch (ivf_flat.cc:203-350): untrained -> empty results (:224-227); the range scan is the exact one
+  // (:342-345)
+  void search(const SearchReq& r, cudaStream_t s) override {
+    refuse_probes(r);
+    if (!trained) { fill_empty(r, s); return; }
+    const SearchCtx& sc = *r.sc;
+    const float thr = radius_threshold(r);
+    const uint32_t* q = pad(r.nq, static_cast<const uint8_t*>(r.xq), s);
     const int nprobe = resolve_nprobe(sc);
-    long long* probes = coarse(nq, q, nprobe, s);
-    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+    long long* probes = coarse_lists(r.nq, q, nprobe, s);
+    if (profiling && !r.range) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
     const TcView v = view();
-    const ScanJob lj = list_job(sc, probes, nprobe);
-    if (L.live > 0 && bt_eligible(v, nq, k, nprobe, lj.avg_candidates, sc)) {
-      bt_search(this, v, w, nq, q, k, probes, nprobe, lj, od, oi, s);
-      return;
-    }
     ScanJob j = list_job(sc, probes, nprobe);
-    j.dominant = true;
-    run_scan(this, j, nq, reinterpret_cast<const float*>(q), k, od, nullptr, oi, nullptr, s);
-  }
-  void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                               long long* oi, int* oc, cudaStream_t s) override {
-    if (!trained) {
-      fill_empty_results(nq, max_results, od, oi, s);
-      B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
+    if (!r.range && L.live > 0 && bt_eligible(v, r.nq, r.k, nprobe, j.avg_candidates, sc)) {
+      bt_search(this, v, w, r.nq, q, r.k, probes, nprobe, j, r.od, r.oi, s);
       return;
     }
-    const float thr = radius_threshold(radius);
-    const uint32_t* q = pad(nq, xq, s);
-    const int nprobe = resolve_nprobe(sc);
-    long long* probes = coarse(nq, q, nprobe, s);
-    ScanJob j = list_job(sc, probes, nprobe);  // ivf_flat.cc:342-345
-    j.has_thr = true;
-    j.thr_raw = thr;
-    run_scan(this, j, nq, reinterpret_cast<const float*>(q), max_results, od, nullptr, oi, oc, s);
+    finish_job(r, thr, j);
+    run_scan(this, j, r.nq, reinterpret_cast<const float*>(q), r.k, r.od, nullptr, r.oi, r.oc, s);
   }
 
   int64_t count() const override { return L.live; }

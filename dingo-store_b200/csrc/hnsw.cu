@@ -32,8 +32,6 @@
 
 namespace b200vs {
 
-void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s);
-
 namespace {
 
 // ---------------- host distance: same evaluation order as src/simd/distances_avx512.cc:48-143 ----------------
@@ -1311,8 +1309,8 @@ struct HnswIndex : IndexBase {
     dirty = false;
   }
 
-  // b200vs_search's efsearch refusal (hnsw.cc:332-336) and search_dev's shared-memory refusal, from the arguments alone: a rank
-  // whose graph is still empty returns from search_dev before the latter, and a refused search must not leave its efsearch
+  // b200vs_search's efsearch refusal (hnsw.cc:332-336) and search's shared-memory refusal, from the arguments alone: a rank
+  // whose graph is still empty returns from search before the latter, and a refused search must not leave its efsearch
   // in the sticky ef
   void check_row_search(int k, const b200vs_search_params* sp) const override {
     const int efs = sp ? sp->efsearch : 0;
@@ -1322,11 +1320,19 @@ struct HnswIndex : IndexBase {
       fail(B200VS_EILLEGAL_PARAMETERS, "efsearch / dimension too large for the search kernel");
   }
 
-  void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
+  void search(const SearchReq& r, cudaStream_t s) override {
+    refuse_probes(r);
+    if (r.range) fail(B200VS_EVECTOR_NOT_SUPPORT, "range search not supported");
+    if (r.raw) fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key search not supported");
+    const SearchCtx& sc = *r.sc;
+    const int64_t nq = r.nq;
+    const int k = r.k;
+    float* od = r.od;
+    long long* oi = r.oi;
     if (sc.efsearch > 0) ef = sc.efsearch;  // sticky, mutated under the read lock like the reference (hnsw.cc:426-428)
     upload(s);
-    if (G.n == 0) { fill_empty_results(nq, k, od, oi, s); return; }
-    const float* q = prepare_queries(nq, xq, s);
+    if (G.n == 0) { fill_empty(r, s); return; }
+    const float* q = queries(r, s);
     const int ef_run = std::max(ef, k);  // searchKnn: max(ef_, k)
     const HnswDev g = dev_graph(G.n, G.maxlevel, G.enterpoint, G.ndeleted > 0);
     const long long words = (G.n + 31) / 32;

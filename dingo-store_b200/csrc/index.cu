@@ -378,27 +378,26 @@ struct FlatIndex : IndexBase {
     return j;
   }
 
-  void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
-    search_rows(nq, xq, k, sc, od, oi, false, s);
-  }
-  void search_raw_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
-    search_rows(nq, xq, k, sc, od, oi, true, s);
-  }
-  // raw_out: od = raw metric value (L2 distance | ip) instead of the API distance; every path selects the same rows
-  void search_rows(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, bool raw_out, cudaStream_t s) {
-    const float* q = prepare_queries(nq, xq, s);
+  // VectorIndexFlat::Search / RangeSearch, vector_index_flat.cc:206-323: range radius -> 1 - radius for IP / cosine
+  // (:282-285); faiss range_search keeps L2 dis < radius, IP ip > radius.  Every path selects the same rows.
+  void search(const SearchReq& r, cudaStream_t s) override {
+    refuse_probes(r);
+    const float* q = queries(r, s);
+    const float thr = ip_like() ? 1.0F - r.radius : r.radius;
     const TcView v = rowmap.view();
-    if (rowmap.rows > 0 && tc_eligible(this, v, nq, k, 1, sc)) {
-      long long* probes = scratch.alloc<long long>(nq);
-      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
-      tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, 1, sc, od, oi, raw_out, s);
+    if (rowmap.rows > 0 && tc_eligible(this, v, r.nq, r.k, 1, *r.sc, r.range)) {
+      long long* probes = scratch.alloc<long long>(r.nq);
+      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)r.nq * 8, s));
+      tc_search(this, v, r, q, probes, 1, thr, s);
       return;
     }
-    if (flat_small_eligible(device, nq, rowmap.rows, dim, k, sc)) {  // one query per task is the reference's own shape: single-launch path
-      flat_small_search(this, metric == B200VS_L2, rowmap.store.vecs.p, rowmap.store.ids.p, rowmap.rows, nq, q, k, sc, od, oi, raw_out, s);
+    if (!r.range && flat_small_eligible(device, r.nq, rowmap.rows, dim, r.k, *r.sc)) {  // one query per task is the reference's own shape: single-launch path
+      flat_small_search(this, metric == B200VS_L2, rowmap.store.vecs.p, rowmap.store.ids.p, rowmap.rows, r.nq, q, r.k, *r.sc, r.od, r.oi, r.raw, s);
       return;
     }
-    run_scan(this, job(sc), nq, q, k, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, nullptr, s);
+    ScanJob j = job(*r.sc);
+    if (r.range) { j.has_thr = true; j.thr_raw = thr; }
+    run_scan(this, j, r.nq, q, r.k, r.raw ? nullptr : r.od, r.raw ? r.od : nullptr, r.oi, r.oc, s);
   }
 
   void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) override {
@@ -413,33 +412,6 @@ struct FlatIndex : IndexBase {
     if (rows > 0) B200VS_CUDA(cudaMemcpyAsync(out_scores, ds, (size_t)nq * rows * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(out_eps, de, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
-  }
-
-  // VectorIndexFlat::RangeSearch, vector_index_flat.cc:267-323: radius -> 1 - radius for IP / cosine (:282-285);
-  // faiss range_search keeps L2 dis < radius, IP ip > radius.
-  void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                        long long* oi, int* oc, cudaStream_t s) override {
-    range_rows(nq, xq, radius, max_results, sc, od, oi, oc, false, s);
-  }
-  void range_search_raw_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                            long long* oi, int* oc, cudaStream_t s) override {
-    range_rows(nq, xq, radius, max_results, sc, od, oi, oc, true, s);
-  }
-  void range_rows(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od, long long* oi, int* oc,
-                  bool raw_out, cudaStream_t s) {
-    const float* q = prepare_queries(nq, xq, s);
-    const float thr = ip_like() ? 1.0F - radius : radius;
-    const TcView v = rowmap.view();
-    if (rowmap.rows > 0 && tc_range_eligible(this, v, nq, max_results, 1, sc)) {
-      long long* probes = scratch.alloc<long long>(nq);
-      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)nq * 8, s));
-      tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, 1, sc, od, oi, oc, raw_out, s);
-      return;
-    }
-    ScanJob j = job(sc);
-    j.has_thr = true;
-    j.thr_raw = thr;
-    run_scan(this, j, nq, q, max_results, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, oc, s);
   }
 
   void reconstruct(int64_t n, const int64_t* in_ids, float* out, uint8_t* found) override {
@@ -473,13 +445,10 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p) { return ne
 // IVF-Flat
 // ============================================================================================
 
-void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s) {
-  if (od) B200VS_CUDA(cudaMemsetAsync(od, 0, (size_t)nq * k * 4, s));
-  B200VS_CUDA(cudaMemsetAsync(oi, 0xFF, (size_t)nq * k * 8, s));  // -1
-}
-void fill_empty_range(int64_t nq, int max_results, float* od, long long* oi, int* oc, cudaStream_t s) {
-  fill_empty_results(nq, max_results, od, oi, s);
-  if (oc) B200VS_CUDA(cudaMemsetAsync(oc, 0, (size_t)nq * 4, s));
+void fill_empty(const SearchReq& r, cudaStream_t s) {
+  if (r.od) B200VS_CUDA(cudaMemsetAsync(r.od, 0, (size_t)r.nq * r.k * 4, s));
+  B200VS_CUDA(cudaMemsetAsync(r.oi, 0xFF, (size_t)r.nq * r.k * 8, s));  // -1
+  if (r.range && r.oc) B200VS_CUDA(cudaMemsetAsync(r.oc, 0, (size_t)r.nq * 4, s));
 }
 
 struct IvfFlatIndex : IndexBase {
@@ -573,7 +542,7 @@ struct IvfFlatIndex : IndexBase {
     for (int64_t a = 0; a < n; a += chunk) {
       const int64_t m = std::min(chunk, n - a);
       const auto mark = scratch.mark();
-      coarse(m, x_dev + (size_t)a * dim, 1, s, true, out_list_dev + a);
+      coarse_rows(m, x_dev + (size_t)a * dim, 1, 0, nlist, true, nullptr, out_list_dev + a, s);
       scratch.release(mark);  // stream-ordered reuse
     }
   }
@@ -591,19 +560,6 @@ struct IvfFlatIndex : IndexBase {
     if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
     assign_dev(x_dev, n, out_lists_dev, s);
   }
-  void coarse_probes_dev(int64_t nq, const float* q_prepared, int nprobe, long long* out_lists, cudaStream_t s) override {
-    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-    coarse(nq, q_prepared, nprobe, s, true, out_lists);
-  }
-  void search_probes_prepared_dev(int64_t nq, const float* q, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                                  long long* oi, cudaStream_t s) override;
-  void range_search_probes_prepared_dev(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
-                                        const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) override {
-    if (!trained) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
-    range_probes(nq, q, radius, max_results, probes, nprobe, sc, od, oi, oc, true, s);
-  }
-  void range_probes(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe, const SearchCtx& sc,
-                    float* od, long long* oi, int* oc, bool raw_out, cudaStream_t s);
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
   int64_t remove(int64_t n, const int64_t* del) override;
 
@@ -612,26 +568,30 @@ struct IvfFlatIndex : IndexBase {
     return std::min(np, nlist);               // ivf_flat.cc:234
   }
 
-  void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override;
-  void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                        long long* oi, int* oc, cudaStream_t s) override;
-  void coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) override;
-  void search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                         long long* oi, cudaStream_t s) override;
+  void search(const SearchReq& r, cudaStream_t s) override;
+  void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+              cudaStream_t s) override {
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
+    coarse_rows(nq, prepared ? xq : prepare_queries(nq, xq, s), nprobe, c0, c1, true, out_score, out_lists, s);
+  }
 
-  long long* coarse(int64_t nq, const float* q, int nprobe, cudaStream_t s, bool allow_tc = true, long long* out = nullptr) {
-    long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
-    if (allow_tc && tc_coarse_eligible(this, nq, nlist, nprobe) && tc_norms_in_range(metric == B200VS_L2, cent_max_norm)) {
-      // dense TF32 scores + certified exact re-score
-      tc_coarse(this, coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, 0, nlist), metric == B200VS_L2, nq, q,
-                nprobe, probes, nullptr, s);
-      return probes;
+  // the nprobe nearest of centroid rows [c0, c1) of prepared queries: the tensor-core pass (dense TF32 scores + certified
+  // exact re-score) when allowed and the shapes fit, else the exact scan.  out_score: coarse's ascending ranking score.
+  void coarse_rows(int64_t nq, const float* q, int nprobe, int c0, int c1, bool allow_tc, float* out_score, long long* out_lists,
+                   cudaStream_t s) {
+    const int rows = c1 - c0;
+    if (allow_tc && tc_coarse_eligible(this, nq, rows, nprobe) && tc_norms_in_range(metric == B200VS_L2, cent_max_norm)) {
+      TcView v = coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, c0, rows);
+      v.api_scores = out_score != nullptr;
+      tc_coarse(this, v, metric == B200VS_L2, nq, q, nprobe, out_lists, out_score, s);
+      return;
     }
     ScanJob j;
     j.l2 = metric == B200VS_L2;
-    j.vecs = centroids.p; j.ids = cent_ids.p; j.d = dim; j.mode = 0; j.n = nlist;
-    run_scan(this, j, nq, q, nprobe, nullptr, nullptr, probes, nullptr, s);
-    return probes;
+    j.vecs = centroids.p + (size_t)c0 * dim; j.ids = cent_ids.p + c0; j.d = dim; j.mode = 0; j.n = rows;
+    run_scan(this, j, nq, q, nprobe, nullptr, out_score, out_lists, nullptr, s);          // raw metric value
+    if (out_score && metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);   // -> ascending ranking score
   }
   ScanJob list_job(const SearchCtx& sc, const long long* probes, int nprobe) const {
     ScanJob j;
@@ -772,84 +732,30 @@ int64_t IvfFlatIndex::remove(int64_t n, const int64_t* del) {
   return r;
 }
 
-void IvfFlatIndex::search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) {
-  if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_flat.cc:224-227
-  const float* q = prepare_queries(nq, xq, s);
-  const int nprobe = resolve_nprobe(sc);
-  long long* probes = coarse(nq, q, nprobe, s, !sc.exact_only);
-  if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
+// VectorIndexIvfFlat::Search / RangeSearch, vector_index_ivf_flat.cc:203-350: untrained -> empty results (:224-227); range
+// radius -> 1 - radius for IP / cosine (:296-299).  The index's own coarse pass keeps to exact_only for top-k only.
+void IvfFlatIndex::search(const SearchReq& r, cudaStream_t s) {
+  if (!trained) { fill_empty(r, s); return; }
+  const SearchCtx& sc = *r.sc;
+  const float* q = queries(r, s);
+  const int nprobe = r.probes ? r.nprobe : resolve_nprobe(sc);
+  const long long* probes = r.probes;
+  if (!probes) {
+    long long* own = scratch.alloc<long long>((size_t)r.nq * nprobe);
+    coarse_rows(r.nq, q, nprobe, 0, nlist, r.range || !sc.exact_only, nullptr, own, s);
+    probes = own;
+  }
+  if (profiling) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
+  const float thr = ip_like() ? 1.0F - r.radius : r.radius;
   const TcView v = view();
-  if (L.live > 0 && tc_eligible(this, v, nq, k, nprobe, sc)) {
-    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, false, s);
+  if (L.live > 0 && tc_eligible(this, v, r.nq, r.k, nprobe, sc, r.range)) {
+    tc_search(this, v, r, q, probes, nprobe, thr, s);
     return;
   }
   ScanJob j = list_job(sc, probes, nprobe);
-  j.dominant = true;
-  run_scan(this, j, nq, q, k, od, nullptr, oi, nullptr, s);
-}
-
-void IvfFlatIndex::coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) {
-  if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-  if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
-  const float* q = prepare_queries(nq, xq, s);
-  const int rows = c1 - c0;
-  if (tc_coarse_eligible(this, nq, rows, nprobe) && tc_norms_in_range(metric == B200VS_L2, cent_max_norm)) {
-    TcView v = coarse_view(centroids.p, cent_hi.p, cent_lo.p, cent_norms.p, cent_max_norm, c0, rows);
-    v.api_scores = true;
-    tc_coarse(this, v, metric == B200VS_L2, nq, q, nprobe, out_lists, out_score, s);
-    return;
-  }
-  ScanJob j;
-  j.l2 = metric == B200VS_L2;
-  j.vecs = centroids.p + (size_t)c0 * dim; j.ids = cent_ids.p + c0; j.d = dim; j.mode = 0; j.n = rows;
-  run_scan(this, j, nq, q, nprobe, nullptr, out_score, out_lists, nullptr, s);  // raw metric value
-  if (metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);             // -> ascending ranking score
-}
-
-void IvfFlatIndex::search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                                     long long* oi, cudaStream_t s) {
-  if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }
-  search_probes_prepared_dev(nq, prepare_queries(nq, xq, s), k, probes, nprobe, sc, od, oi, s);
-}
-
-void IvfFlatIndex::search_probes_prepared_dev(int64_t nq, const float* q, int k, const long long* probes, int nprobe, const SearchCtx& sc,
-                                              float* od, long long* oi, cudaStream_t s) {
-  if (!trained) { fill_empty_results(nq, k, od, oi, s); return; }
-  if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
-  const TcView v = view();
-  if (L.live > 0 && tc_eligible(this, v, nq, k, nprobe, sc)) {
-    tc_search(this, v, metric == B200VS_L2, nq, q, k, probes, nprobe, sc, od, oi, false, s);
-    return;
-  }
-  ScanJob j = list_job(sc, probes, nprobe);
-  j.dominant = true;
-  run_scan(this, j, nq, q, k, od, nullptr, oi, nullptr, s);
-}
-
-void IvfFlatIndex::range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc,
-                                    float* od, long long* oi, int* oc, cudaStream_t s) {
-  if (!trained) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
-  const float* q = prepare_queries(nq, xq, s);
-  const int nprobe = resolve_nprobe(sc);
-  long long* probes = coarse(nq, q, nprobe, s);
-  range_probes(nq, q, radius, max_results, probes, nprobe, sc, od, oi, oc, false, s);
-}
-
-// range search of prepared queries over the probe table: the tile range scan when it applies, else the exact scan with the
-// range threshold.  raw_out: od = raw metric value instead of the API distance.
-void IvfFlatIndex::range_probes(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
-                                const SearchCtx& sc, float* od, long long* oi, int* oc, bool raw_out, cudaStream_t s) {
-  const float thr = ip_like() ? 1.0F - radius : radius;  // ivf_flat.cc:296-299
-  if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
-  const TcView v = view();
-  if (L.live > 0 && tc_range_eligible(this, v, nq, max_results, nprobe, sc)) {
-    tc_range_search(this, v, metric == B200VS_L2, nq, q, thr, max_results, probes, nprobe, sc, od, oi, oc, raw_out, s);
-    return;
-  }
-  ScanJob j = list_job(sc, probes, nprobe);
-  j.has_thr = true;
-  j.thr_raw = thr;
-  run_scan(this, j, nq, q, max_results, raw_out ? nullptr : od, raw_out ? od : nullptr, oi, oc, s);
+  if (r.range) { j.has_thr = true; j.thr_raw = thr; }
+  else j.dominant = true;
+  run_scan(this, j, r.nq, q, r.k, r.raw ? nullptr : r.od, r.raw ? r.od : nullptr, r.oi, r.oc, s);
 }
 
 void IvfFlatIndex::export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) {

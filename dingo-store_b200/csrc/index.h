@@ -181,6 +181,27 @@ struct IndexBase;
 // resolve search params; uploads the sorted id list into the calling lane's scratch (stream-ordered on s)
 SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s);
 
+// One read of an index (IndexBase::search).  Every pointer is on the index's device.
+struct SearchReq {
+  int64_t nq = 0;
+  const void* xq = nullptr;           // query rows: FP32, or packed bits (dim / 8 bytes) on a binary index
+  bool prepared = false;              // FP32 rows already normalised for cosine
+  const long long* probes = nullptr;  // the caller's probe table [nq, nprobe] (IVF types); null = the index's own coarse pass
+  int nprobe = 0;
+  int k = 0;                          // top-k, or max_results when range
+  bool range = false;                 // range search: the hits inside radius, closest first, at most k of them
+  float radius = 0.f;
+  bool raw = false;                   // od = the raw metric value (L2 distance | ip), the key the single-index select ranks
+                                      // by and a merge of several indexes' results has to order by, instead of the API distance
+  const SearchCtx* sc = nullptr;
+  float* od = nullptr;                // [nq, k]
+  long long* oi = nullptr;            // [nq, k], -1 past the last result
+  int* oc = nullptr;                  // [nq] hits per query (range)
+  const float* fq() const { return static_cast<const float*>(xq); }
+};
+// the results of a search that finds nothing (an untrained or empty index): ids -1, distances 0, range counts 0
+void fill_empty(const SearchReq& r, cudaStream_t s);
+
 struct IndexBase {
   b200vs_type type;
   b200vs_metric metric;
@@ -254,24 +275,15 @@ struct IndexBase {
   virtual void add(int64_t n, const float* x, const int64_t* ids, bool upsert) = 0;
   virtual int64_t remove(int64_t n, const int64_t* ids) = 0;
   virtual void clear() { fail(B200VS_EVECTOR_NOT_SUPPORT, "clear is only implemented for FLAT"); }  // drop every row, keep the buffers
-  // device-pointer search on stream s; scratch already reset; q is RAW (normalise inside for cosine)
-  virtual void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* out_dist, long long* out_ids,
-                          cudaStream_t s) = 0;
-  virtual void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc,
-                                float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
-    (void)nq; (void)xq; (void)radius; (void)max_results; (void)sc; (void)out_dist; (void)out_ids; (void)out_counts; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "range search not supported");
-  }
-  // list-sharded multi-GPU building blocks (IVF types): coarse quantiser over centroid rows [c0, c1) only, and the list
-  // scan for caller-supplied (merged) probes
-  virtual void coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) {
-    (void)nq; (void)xq; (void)nprobe; (void)c0; (void)c1; (void)out_score; (void)out_lists; (void)s;
+  // THE read of an index, on stream s with the lane's scratch already reset: r's top-k or range search.  Each type refuses
+  // the requests it cannot serve (a probe table without inverted lists, range on HNSW).
+  virtual void search(const SearchReq& r, cudaStream_t s) = 0;
+  // the coarse quantiser of the IVF types over centroid rows [c0, c1): out_lists [nq, nprobe] global list ids (set
+  // semantics), and when out_score is set the ascending ranking score of each (L2 distance | -ip) in (score, list id) order
+  virtual void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+                      cudaStream_t s) {
+    (void)nq; (void)xq; (void)prepared; (void)nprobe; (void)c0; (void)c1; (void)out_score; (void)out_lists; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
-  }
-  virtual void search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                                 long long* oi, cudaStream_t s) {
-    (void)nq; (void)xq; (void)k; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
   }
   // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT and IVF_PQ ----
   // rows / ids already on this device.  lists_dev (nullable) = the inverted list of every row, decided by the caller;
@@ -294,17 +306,6 @@ struct IndexBase {
   // from the arguments and the index's parameters alone, so that every rank refuses alike before it (HNSW: efsearch outside
   // [0, 1024], as b200vs_search; the walk's shared memory)
   virtual void check_row_search(int k, const b200vs_search_params* sp) const { (void)k; (void)sp; }
-  // search_dev / range_search_dev, but od holds the raw metric value (L2 distance | ip): the key the single-index select
-  // ranks by, which a merge of several indexes' results has to order by
-  virtual void search_raw_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) {
-    (void)nq; (void)xq; (void)k; (void)sc; (void)od; (void)oi; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key search only exists for FLAT");
-  }
-  virtual void range_search_raw_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od,
-                                    long long* oi, int* oc, cudaStream_t s) {
-    (void)nq; (void)xq; (void)radius; (void)max_results; (void)sc; (void)od; (void)oi; (void)oc; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key range search only exists for FLAT");
-  }
   // nearest-centroid assignment of prepared rows (faiss quantizer->assign): out_lists_dev[n], on stream s (a lane must be held)
   virtual void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) {
     (void)n; (void)x_dev; (void)out_lists_dev; (void)s;
@@ -317,26 +318,8 @@ struct IndexBase {
     fail(B200VS_EVECTOR_NOT_SUPPORT, "list reservation only exists for IVF_FLAT and IVF_PQ");
   }
   virtual int nlist_now() const { return 1; }
-  // probe table (set semantics, order unspecified) of prepared queries into a caller buffer
-  virtual void coarse_probes_dev(int64_t nq, const float* q_prepared, int nprobe, long long* out_lists, cudaStream_t s) {
-    (void)nq; (void)q_prepared; (void)nprobe; (void)out_lists; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
-  }
-  // search_probes_dev on queries that are already prepared (normalised for cosine)
-  virtual void search_probes_prepared_dev(int64_t nq, const float* q_prepared, int k, const long long* probes, int nprobe, const SearchCtx& sc,
-                                          float* od, long long* oi, cudaStream_t s) {
-    (void)nq; (void)q_prepared; (void)k; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
-  }
-  // range search of prepared queries over caller-supplied probes (the local step of a sharded range search): the hits of
-  // range_search_dev, but od holds the raw metric value (L2 distance | ip), which orders hits as the single-index select does
-  virtual void range_search_probes_prepared_dev(int64_t nq, const float* q_prepared, float radius, int max_results, const long long* probes,
-                                                int nprobe, const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) {
-    (void)nq; (void)q_prepared; (void)radius; (void)max_results; (void)probes; (void)nprobe; (void)sc; (void)od; (void)oi; (void)oc; (void)s;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven range search only exists for IVF_FLAT and IVF_PQ");
-  }
   virtual int resolve_nprobe_api(const SearchCtx& sc) const { (void)sc; return 1; }
-  // refusals of search_probes_prepared_dev that depend only on nq, k and the trained state (IVF-PQ: the LUT + select pool
+  // refusals of a search over a caller's probe table that depend only on nq, k and the trained state (IVF-PQ: the LUT + select pool
   // must fit one SM's shared memory); a sharded search checks them on every rank before its first collective
   virtual void check_probe_search(int64_t nq, int k) const { (void)nq; (void)k; }
   // b200vs_debug_tc_scores: xq device (raw), outputs host [nq, count() + deleted_count()] and [nq]
@@ -352,16 +335,6 @@ struct IndexBase {
   virtual void train_binary(int64_t n, const uint8_t* x) { (void)n; (void)x; fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index"); }
   virtual void add_binary(int64_t n, const uint8_t* x, const int64_t* ids, bool upsert) {
     (void)n; (void)x; (void)ids; (void)upsert;
-    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
-  }
-  // xq: device rows [nq, dim / 8]; distances are Hamming distances
-  virtual void search_binary_dev(int64_t nq, const uint8_t* xq, int k, const SearchCtx& sc, float* out_dist, long long* out_ids, cudaStream_t s) {
-    (void)nq; (void)xq; (void)k; (void)sc; (void)out_dist; (void)out_ids; (void)s;
-    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
-  }
-  virtual void range_search_binary_dev(int64_t nq, const uint8_t* xq, float radius, int max_results, const SearchCtx& sc,
-                                       float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
-    (void)nq; (void)xq; (void)radius; (void)max_results; (void)sc; (void)out_dist; (void)out_ids; (void)out_counts; (void)s;
     fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
   }
 
@@ -383,6 +356,11 @@ struct IndexBase {
 
   // helpers shared by the index types
   const float* prepare_queries(int64_t nq, const float* xq_dev, cudaStream_t s);  // cosine -> normalised copy
+  const float* queries(const SearchReq& r, cudaStream_t s) { return r.prepared ? r.fq() : prepare_queries(r.nq, r.fq(), s); }
+  // the refusal of a caller's probe table by a type without inverted lists to probe
+  static void refuse_probes(const SearchReq& r) {
+    if (r.probes) fail(B200VS_EVECTOR_NOT_SUPPORT, "probe-driven search only exists for IVF_FLAT and IVF_PQ");
+  }
   void launch_count(int n = 1) { stats[0] += n; }
 };
 

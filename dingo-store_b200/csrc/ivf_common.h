@@ -460,8 +460,5 @@ void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const flo
 }
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids);
-void fill_empty_results(int64_t nq, int k, float* od, long long* oi, cudaStream_t s);
-// fill_empty_results of a range search, with every count (oc, nullable) zero
-void fill_empty_range(int64_t nq, int max_results, float* od, long long* oi, int* oc, cudaStream_t s);
 
 }  // namespace b200vs

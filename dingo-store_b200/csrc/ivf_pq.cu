@@ -347,7 +347,7 @@ __global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kern
 
 // dis0[i] (i = query * nprobe + p) = the coarse pass's raw value (L2 distance or ip) of the query and list probes[i], for
 // probes that come from the caller (a list-sharded search merges them from several ranks, and the ABI carries list ids
-// only).  It is bit-equal to what the coarse pass of scan_codes hands the LUT scan: the exact scan's quad_distance on
+// only).  It is bit-equal to what the coarse pass of search hands the LUT scan: the exact scan's quad_distance on
 // (centroid row, query), then its merge's (key, raw) round trip (which turns an ip of +0 into -0).  One quad per
 // (query, probe); -1 probes and empty lists are skipped, as the LUT scans never read them.
 template <bool L2>
@@ -729,20 +729,36 @@ struct IvfPqIndex : IndexBase {
     return r;
   }
 
-  void search_dev(int64_t nq, const float* xq, int k, const SearchCtx& sc, float* od, long long* oi, cudaStream_t s) override {
-    if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }  // ivf_pq.cc:159-163
-    if (mode == kFlat) {  // delegate to the inner Flat index, sharing this call's stream and scratch discipline
+  // VectorIndexIvfPq::Search (ivf_pq.cc:159-163: untrained -> empty results) and VectorIndexRawIvfPq::Search / RangeSearch
+  // (raw_ivf_pq.cc:160-278): faiss IndexIVFPQ::search / range_search on the codes; range radius -> 1 - radius for IP / cosine
+  // (:229-232), L2 keeps dis < radius, IP keeps dis > radius: the same LUT scan with a threshold epilogue instead of the
+  // k-th-best threshold.  A caller's probe table takes the place of the coarse pass, dis0 recomputed per (query, probe).
+  void search(const SearchReq& r, cudaStream_t s) override {
+    if (mode == kNone) { fill_empty(r, s); return; }
+    if (mode == kFlat && !r.probes) {  // delegate to the inner Flat index, sharing this call's stream and scratch discipline
       std::shared_lock<std::shared_mutex> rl(flat->rw);
       LaneGuard lg(flat.get(), s);
-      flat->search_dev(nq, xq, k, sc, od, oi, s);  // (an id-list filter lives in the outer lane's scratch: same stream, still locked)
-      for (int i = 0; i < 8; ++i) stats[i] = flat->stats[i].load();
+      flat->search(r, s);  // (an id-list filter lives in the outer lane's scratch: same stream, still locked)
+      if (!r.range) for (int i = 0; i < 8; ++i) stats[i] = flat->stats[i].load();
       return;
     }
-    scan_codes(nq, xq, k, sc, false, 0.f, od, oi, nullptr, s);
+    if (r.probes) check_probe_search(r.nq, r.k);
+    else scan_smem(r.k);  // checked before anything is launched
+    const float* q = queries(r, s);
+    const int nprobe = r.probes ? r.nprobe : resolve_nprobe(*r.sc);
+    const long long* probes = r.probes;
+    float* dis0 = nullptr;
+    if (!probes) {  // coarse quantiser: top-nprobe lists + raw coarse values
+      long long* own = scratch.alloc<long long>((size_t)r.nq * nprobe);
+      dis0 = scratch.alloc<float>((size_t)r.nq * nprobe);
+      coarse_rows(r.nq, q, nprobe, 0, nlist, dis0, own, s);
+      probes = own;
+    }
+    if (profiling) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
+    scan_lists(r.nq, q, r.k, *r.sc, probes, dis0 ? dis0 : probe_dis0(r.nq, q, probes, nprobe, s), nprobe, r.range,
+               ip_like() ? 1.0F - r.radius : r.radius, r.raw ? nullptr : r.od, r.oi, r.oc, s, r.raw ? r.od : nullptr);
   }
 
-  // coarse quantiser -> per-query LUT -> code scan + select -> merge.  Range mode (has_thr): keep hits strictly inside the
-  // raw threshold (L2: dis < thr; IP: dis > thr), at most k of them, closest first; out_counts = hits per query.
   // shared memory of the LUT scan's CTA (LUT + select pool), refused above one SM's 227 KB
   size_t scan_smem(int k) const {
     const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
@@ -754,7 +770,7 @@ struct IvfPqIndex : IndexBase {
     const int nprobe = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchIvfPqParamNprobe, raw_ivf_pq.cc:170
     return std::min(nprobe, nlist);                      // raw_ivf_pq.cc:190
   }
-  // the coarse quantiser of scan_codes over centroid rows [c0, c1): top-nprobe GLOBAL list ids, and the raw coarse values
+  // the coarse quantiser of search over centroid rows [c0, c1): top-nprobe GLOBAL list ids, and the raw coarse values
   // (L2 distance or ip) when out_raw is set
   void coarse_rows(int64_t nq, const float* q, int nprobe, int c0, int c1, float* out_raw, long long* out_lists, cudaStream_t s) {
     ScanJob cj;
@@ -762,20 +778,9 @@ struct IvfPqIndex : IndexBase {
     run_scan(this, cj, nq, q, nprobe, nullptr, out_raw, out_lists, nullptr, s);
   }
 
-  void scan_codes(int64_t nq, const float* xq, int k, const SearchCtx& sc, bool has_thr, float thr_raw, float* od, long long* oi, int* oc,
-                  cudaStream_t s) {
-    scan_smem(k);  // checked before anything is launched
-    const float* q = prepare_queries(nq, xq, s);
-    const int nprobe = resolve_nprobe(sc);
-    // coarse quantiser: top-nprobe lists + raw coarse values
-    long long* probes = scratch.alloc<long long>((size_t)nq * nprobe);
-    float* coarse = scratch.alloc<float>((size_t)nq * nprobe);
-    coarse_rows(nq, q, nprobe, 0, nlist, coarse, probes, s);
-    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
-    scan_lists(nq, q, k, sc, probes, coarse, nprobe, has_thr, thr_raw, od, oi, oc, s);
-  }
-
-  // per-query LUT -> code scan + select of the probed lists -> merge.  q prepared; coarse = dis0 per (query, probe).
+  // per-query LUT -> code scan + select of the probed lists -> merge.  q prepared; coarse = dis0 per (query, probe).  Range
+  // mode (has_thr): keep hits strictly inside the raw threshold (L2: dis < thr; IP: dis > thr), at most k of them, closest
+  // first; out_counts = hits per query.
   void scan_lists(int64_t nq, const float* q, int k, const SearchCtx& sc, const long long* probes, const float* coarse, int nprobe,
                   bool has_thr, float thr_raw, float* od, long long* oi, int* oc, cudaStream_t s, float* oraw = nullptr) {
     const int T = M * ksub;
@@ -824,16 +829,12 @@ struct IvfPqIndex : IndexBase {
   // ---- list-sharded building blocks (include/b200vs.h), in the IVF-PQ mode only ----
   int nlist_now() const override { return nlist; }
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
-  // b200vs_coarse_device: the coarse pass of scan_codes on rows [c0, c1); score = L2 distance or -ip, in (score, list id) order
-  void coarse_range_dev(int64_t nq, const float* xq, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) override {
+  void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+              cudaStream_t s) override {
     require_lists();
     if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
-    coarse_rows(nq, prepare_queries(nq, xq, s), nprobe, c0, c1, out_score, out_lists, s);
-    if (metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);  // -> ascending ranking score
-  }
-  void coarse_probes_dev(int64_t nq, const float* q_prepared, int nprobe, long long* out_lists, cudaStream_t s) override {
-    require_lists();
-    coarse_rows(nq, q_prepared, nprobe, 0, nlist, nullptr, out_lists, s);
+    coarse_rows(nq, prepared ? xq : prepare_queries(nq, xq, s), nprobe, c0, c1, out_score, out_lists, s);
+    if (out_score && metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);  // -> ascending ranking score
   }
   // refusals of a probe-driven search that depend on its arguments and the trained state only: a sharded search checks them
   // before its first collective
@@ -842,30 +843,8 @@ struct IvfPqIndex : IndexBase {
     if (nq > 65535) fail(B200VS_EILLEGAL_PARAMETERS, "batch too large (max 65535 queries per call)");
     scan_smem(k);
   }
-  void search_probes_dev(int64_t nq, const float* xq, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                         long long* oi, cudaStream_t s) override {
-    if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }
-    require_lists();
-    search_probes_prepared_dev(nq, prepare_queries(nq, xq, s), k, probes, nprobe, sc, od, oi, s);
-  }
-  // the LUT scan of scan_codes on caller-supplied probes; dis0 is recomputed per (query, probe) by pq_dis0_kernel
-  void search_probes_prepared_dev(int64_t nq, const float* q, int k, const long long* probes, int nprobe, const SearchCtx& sc, float* od,
-                                  long long* oi, cudaStream_t s) override {
-    if (mode == kNone) { fill_empty_results(nq, k, od, oi, s); return; }
-    check_probe_search(nq, k);
-    scan_lists(nq, q, k, sc, probes, probe_dis0(nq, q, probes, nprobe, s), nprobe, false, 0.f, od, oi, nullptr, s);
-  }
-  // the thresholded LUT scan of range_search_dev on caller-supplied probes, the raw value (L2 distance | ip) in od
-  void range_search_probes_prepared_dev(int64_t nq, const float* q, float radius, int max_results, const long long* probes, int nprobe,
-                                        const SearchCtx& sc, float* od, long long* oi, int* oc, cudaStream_t s) override {
-    if (mode == kNone) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
-    check_probe_search(nq, max_results);
-    scan_lists(nq, q, max_results, sc, probes, probe_dis0(nq, q, probes, nprobe, s), nprobe, true, ip_like() ? 1.0F - radius : radius,
-               nullptr, oi, oc, s, od);
-  }
   // dis0 of every (query, probe) of a caller-supplied probe table
   const float* probe_dis0(int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {
-    if (profiling) profile_probed(this, probes, nq * nprobe, nlist, L.d_len.p, s);
     const long long n = (long long)nq * nprobe;
     float* dis0 = scratch.alloc<float>((size_t)n);
     const bool vec = (dim & 3) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0;  // the load width only, not the arithmetic
@@ -875,21 +854,6 @@ struct IvfPqIndex : IndexBase {
     else pq_dis0_kernel<false><<<grid, 256, 0, s>>>(q, centroids.p, probes, L.d_len.p, n, nprobe, dim, vec, dis0);
     B200VS_CUDA(cudaGetLastError());
     return dis0;
-  }
-
-  // VectorIndexRawIvfPq::RangeSearch, vector_index_raw_ivf_pq.cc:212-278: faiss IndexIVFPQ::range_search on the codes —
-  // radius -> 1 - radius for IP / cosine (:229-232), L2 keeps dis < radius, IP keeps dis > radius; the same LUT scan with a
-  // threshold epilogue instead of the k-th-best threshold.  Untrained -> empty results (:219-222).
-  void range_search_dev(int64_t nq, const float* xq, float radius, int max_results, const SearchCtx& sc, float* od, long long* oi,
-                        int* oc, cudaStream_t s) override {
-    if (mode == kNone) { fill_empty_range(nq, max_results, od, oi, oc, s); return; }
-    if (mode == kFlat) {
-      std::shared_lock<std::shared_mutex> rl(flat->rw);
-      LaneGuard lg(flat.get(), s);
-      flat->range_search_dev(nq, xq, radius, max_results, sc, od, oi, oc, s);
-      return;
-    }
-    scan_codes(nq, xq, max_results, sc, true, ip_like() ? 1.0F - radius : radius, od, oi, oc, s);
   }
 
   int64_t count() const override { return mode == kFlat ? flat->count() : L.live; }

@@ -419,9 +419,10 @@ std::vector<T> all_gather_host(b200vs_shard* sh, const T* mine, size_t count = 1
 }
 
 // The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
-// on stream s.  local(q, sc, nprobe) is step 2: it writes this rank's ascending, -1-padded [nq, k] (key, id) lists into
-// L.od / L.oi, the key being what the merge orders by.  List-sharded: q are the prepared queries and L.probes the gathered
-// probe table.  Row-sharded: there is no coarse step; q are the raw queries (the rank's index prepares them) and nprobe is 0.
+// on stream s.  local(r) is step 2: r is this rank's search of k results per query into L.od / L.oi, which local completes
+// and runs, so that they hold ascending, -1-padded [nq, k] (key, id) lists, the key being what the merge orders by.
+// List-sharded: r searches the prepared queries over the gathered probe table L.probes.  Row-sharded: there is no coarse
+// step, and r searches the raw queries (the rank's index prepares them).
 template <class LocalScan>
 void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
                   float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local) {
@@ -441,7 +442,7 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
     const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
     long long* mine = L.probes.p + (size_t)per * r * nprobe;
     if (q1 - q0 < per) fill_ll_kernel<<<(unsigned)cdiv(per * nprobe, 256), 256, 0, s>>>(mine, per * nprobe, -1);
-    if (q1 > q0) ix->coarse_probes_dev(q1 - q0, q + (size_t)q0 * d, nprobe, mine, s);
+    if (q1 > q0) ix->coarse(q1 - q0, q + (size_t)q0 * d, true, nprobe, 0, ix->nlist_now(), nullptr, mine, s);
     ix->phase(IndexBase::PH_COMM, s);
     if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.probes.p, (size_t)per * nprobe, ncclInt64, L.comm, s));
     ix->phase(IndexBase::PH_OTHER, s);
@@ -449,7 +450,10 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
   // 2) scan of the probed lists this rank owns, or search of the rank's rows -> exact local results
   L.od.reserve((size_t)nq * k, 0, s);
   L.oi.reserve((size_t)nq * k, 0, s);
-  local(q, sc, nprobe);
+  SearchReq req;
+  req.nq = nq; req.xq = q; req.k = k; req.sc = &sc; req.od = L.od.p; req.oi = L.oi.p;
+  if (!sh->rows) { req.prepared = true; req.probes = L.probes.p; req.nprobe = nprobe; }
+  local(req);
   // 3) ONE all-gather of the packed per-shard top-k + merge
   const long long nk = (long long)nq * k;
   L.parts.reserve((size_t)W * nk, 0, s);
@@ -482,15 +486,10 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
                          float* out_dist, long long* out_ids, cudaStream_t s) {
   IndexBase* ix = sh->ix;
   const bool flat_ip = sh->rows && ix->type == B200VS_FLAT && ix->ip_like();
-  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
-    if (!sh->rows) {
-      ix->search_probes_prepared_dev(nq, q, k, L.probes.p, nprobe, sc, L.od.p, L.oi.p, s);
-    } else if (ix->type == B200VS_FLAT) {
-      ix->search_raw_dev(nq, q, k, sc, L.od.p, L.oi.p, s);
-      if (flat_ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
-    } else {
-      ix->search_dev(nq, q, k, sc, L.od.p, L.oi.p, s);
-    }
+  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](SearchReq& r) {
+    r.raw = sh->rows && ix->type == B200VS_FLAT;
+    ix->search(r, s);
+    if (flat_ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
   });
   if (flat_ip) {
     ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
@@ -507,12 +506,12 @@ void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, co
                         const b200vs_search_params* sp, float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
   IndexBase* ix = sh->ix;
   const bool l2 = ix->metric == B200VS_L2;
-  shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](const float* q, const SearchCtx& sc, int nprobe) {
-    int* oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
+  shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](SearchReq& r) {
+    r.range = true; r.radius = radius; r.raw = true;
+    r.oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
     // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
-    if (std::isnan(radius)) fill_empty_range(nq, max_results, L.od.p, L.oi.p, oc, s);
-    else if (sh->rows) ix->range_search_raw_dev(nq, q, radius, max_results, sc, L.od.p, L.oi.p, oc, s);
-    else ix->range_search_probes_prepared_dev(nq, q, radius, max_results, L.probes.p, nprobe, sc, L.od.p, L.oi.p, oc, s);
+    if (std::isnan(radius)) fill_empty(r, s);
+    else ix->search(r, s);
     if (!l2) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
   });
   const long long n = (long long)nq * max_results;

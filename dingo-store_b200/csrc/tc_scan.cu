@@ -1123,7 +1123,7 @@ __device__ __forceinline__ float tc_stream_window(BlockSelect& sel, unsigned cha
   return ord2f(wkey);
 }
 
-// RANGE (tc_range_search): tau holds the range capture threshold, not a sampled one; every captured row is re-scored and
+// RANGE (a range tc_search): tau holds the range capture threshold, not a sampled one; every captured row is re-scored and
 // the closest k rows whose exact key is below thr_key are kept, as the exact scan keeps them, and out_counts holds the rows
 // kept.  In either mode out_dist holds the raw metric value (L2 distance | ip) when raw_out, else the API distance.
 template <bool L2, bool RANGE>
@@ -1341,10 +1341,11 @@ static TcDevice tc_init(int device) {
   return dev;
 }
 
-bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc) {
+bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc, bool range) {
   if (sc.exact_only) return false;
   if (ix->dim % 4 != 0 || ix->dim < 32) return false;      // TMA: 16-byte row pitch; tiny d is not worth a tile
-  if (k > 128 || nq < 16) return false;                    // wide k / tiny batches: exact scan
+  if (nq < 16 || k > (range ? 4096 : 128)) return false;   // tiny batches, wide k: exact scan; 4096 = the select's limit
+  if (range && tc_stream_smem(ix->dim, select_pool_cap(k, SCAN_THREADS)) > 160 * 1024) return false;  // streaming finish
   if (!v.norms || !v.vecs) return false;
   if (!tc_norms_in_range(ix->metric == B200VS_L2, v.max_norm)) return false;
   return tc_plan_fits(v, nq, nprobe);
@@ -1492,85 +1493,6 @@ static void tc_profile_counts(IndexBase* ix, const int* qcount, const int* total
   ix->stats[7] = t[3];
 }
 
-void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
-               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, bool raw_out, cudaStream_t s) {
-  const int d = ix->dim;
-  const int cap = tc_cand_cap(k);
-  auto& S = ix->scratch;
-  ix->phase(IndexBase::PH_PLAN, s);
-  TcPlan P = tc_prepare(ix, v, nq, q, probes, nprobe, s);
-  float* sample = S.alloc<float>((size_t)P.sbound * TC_NQT * TC_SAMPLE);
-  float* tau = S.alloc<float>(nq);
-  unsigned long long* cand = S.alloc<unsigned long long>((size_t)nq * cap);
-  int* cand_cnt = S.alloc<int>(nq);
-  int* flags = S.alloc<int>(nq);
-  int* qmap = S.alloc<int>(nq);
-  int* qcount = S.alloc<int>(1);
-  B200VS_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)nq * 4, s));
-
-  TcParams p = tc_params(v, d, l2, P.items, P.totals, v.hscale, P.qry.scale);
-  p.sample_list = P.sample_list; p.pair_query = P.pair_query;
-  p.sample = sample; p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
-  p.filt.has_range = sc.has_range; p.filt.negate = sc.negate; p.filt.rmin = sc.rmin; p.filt.rmax = sc.rmax;
-  p.filt.sorted_ids = sc.sorted_ids_dev; p.filt.n_ids = sc.n_ids;
-  const int pool = select_pool_cap(k, SCAN_THREADS);
-
-  // 1) sample pass -> per-query capture thresholds
-  p.mode = 0; p.work_counter = P.work;
-  ix->phase(IndexBase::PH_SAMPLE, s);
-  tc_launch(P.dev, P.half, P.sbound, P.maps, p, s);
-  ix->phase(IndexBase::PH_TAU, s);
-  int* redo = S.alloc<int>(nq);
-  // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
-  const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
-  tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
-  tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
-  // 2) capture pass: stream every probed list chunk once, keep rows under the threshold
-  p.mode = 1; p.work_counter = P.work + 1;
-  ix->phase(IndexBase::PH_CAPTURE, s);
-  {
-    ScopedKernelTimer timer(ix, s, ix->profiling);
-    tc_launch(P.dev, P.half, P.bound, P.maps, p, s);
-    timer.stop();
-  }
-  // 3) window select + exact rerank + certification
-  ix->phase(IndexBase::PH_FINAL, s);
-  const int* fin_redo = nullptr;
-  const size_t hsm = (size_t)d * 4;  // the query row
-  const int raw = raw_out ? 1 : 0;
-  if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
-    if (l2) tc_final_hybrid_kernel<true, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, raw, nullptr);
-    else tc_final_hybrid_kernel<false, false><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, 0u, raw, nullptr);
-    fin_redo = redo;
-    ix->launch_count(1);
-  }
-  const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, raw, nullptr);
-  else tc_final_kernel<false, false><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, 0u, raw, nullptr);
-  tc_compact_flags(flags, (int)nq, qmap, qcount, s);
-  B200VS_CUDA(cudaGetLastError());
-  ix->launch_count(5);
-  ix->stats[1] = nq;
-  // 4) uncertified queries re-run on the exact scan (device-side count: blocks beyond it exit immediately)
-  ix->phase(IndexBase::PH_FALLBACK, s);
-  run_scan_mapped(ix, tc_exact_job(v, l2, d, probes, nprobe, sc), nq, qmap, qcount, q, k, raw_out ? nullptr : out_dist,
-                  raw_out ? out_dist : nullptr, out_ids, nullptr, s);
-  ix->phase(IndexBase::PH_OTHER, s);
-  if (ix->profiling && getenv("B200VS_DEBUG_FLAGS")) {
-    std::vector<int> hf(nq), hc(nq);
-    std::vector<float> ht(nq);
-    B200VS_CUDA(cudaMemcpyAsync(hf.data(), flags, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(hc.data(), cand_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaMemcpyAsync(ht.data(), tau, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    long long tot = 0; int mx = 0, r1 = 0, r2 = 0, ninf = 0;
-    for (int64_t i = 0; i < nq; ++i) { tot += hc[i]; mx = std::max(mx, hc[i]); r1 += (hf[i] & 1); r2 += (hf[i] & 2) ? 1 : 0; ninf += std::isinf(ht[i]) ? 1 : 0; }
-    fprintf(stderr, "[b200vs] tc_search nq=%lld cap=%d captured avg=%.1f max=%d flagged: threshold=%d overflow=%d tau_inf=%d\n", (long long)nq, cap, (double)tot / nq, mx, r1, r2, ninf);
-    for (int64_t i = 0, shown = 0; i < nq && shown < 4; ++i) if (hf[i]) { fprintf(stderr, "[b200vs]   q=%lld flag=%d captured=%d tau=%g\n", (long long)i, hf[i], hc[i], ht[i]); ++shown; }
-  }
-  if (ix->profiling) tc_profile_counts(ix, qcount, P.totals, s);
-}
-
 // ---------------------------------------------------------------------------------------------
 // range mode of the list scan: the capture threshold comes from the radius (DESIGN.md 4.6)
 // ---------------------------------------------------------------------------------------------
@@ -1595,22 +1517,14 @@ static __global__ void tc_range_tau_kernel(const float* __restrict__ qnorm, long
   tau[i] = (eps < TC_INF && fabsf(t) < TC_INF) ? t : __int_as_float(0x7fffffff);
 }
 
-bool tc_range_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int max_results, int nprobe, const SearchCtx& sc) {
-  if (sc.exact_only) return false;
-  if (ix->dim % 4 != 0 || ix->dim < 32) return false;
-  if (nq < 16 || max_results > 4096) return false;  // tiny batches: exact scan; 4096 = the select's limit
-  if (tc_stream_smem(ix->dim, select_pool_cap(max_results, SCAN_THREADS)) > 160 * 1024) return false;  // streaming finish
-  if (!v.norms || !v.vecs) return false;
-  if (!tc_norms_in_range(ix->metric == B200VS_L2, v.max_norm)) return false;
-  return tc_plan_fits(v, nq, nprobe);
-}
-
-void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, float radius_raw, int max_results,
-                     const long long* probes, int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, int* out_counts,
-                     bool raw_out, cudaStream_t s) {
+void tc_search(IndexBase* ix, const TcView& v, const SearchReq& r, const float* q, const long long* probes, int nprobe, float thr_raw,
+               cudaStream_t s) {
   const int d = ix->dim;
-  const int k = max_results;
+  const bool l2 = ix->metric == B200VS_L2;
+  const int64_t nq = r.nq;
+  const int k = r.k;
   const int cap = tc_cand_cap(k);
+  const SearchCtx& sc = *r.sc;
   auto& S = ix->scratch;
   ix->phase(IndexBase::PH_PLAN, s);
   TcPlan P = tc_prepare(ix, v, nq, q, probes, nprobe, s);
@@ -1622,16 +1536,32 @@ void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const 
   int* qmap = S.alloc<int>(nq);
   int* qcount = S.alloc<int>(1);
   B200VS_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)nq * 4, s));
-  const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
-  // 1) capture thresholds from the radius (no sample pass)
-  ix->phase(IndexBase::PH_TAU, s);
-  tc_range_tau_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(P.qry.norm, nq, l2 ? 1 : 0, radius_raw, v.max_norm, d, arith, tau);
-  // 2) capture pass: every probed list chunk once, rows under the threshold
+
   TcParams p = tc_params(v, d, l2, P.items, P.totals, v.hscale, P.qry.scale);
   p.pair_query = P.pair_query;
   p.tau = tau; p.cand = cand; p.cand_cnt = cand_cnt; p.cap = cap;
   p.filt.has_range = sc.has_range; p.filt.negate = sc.negate; p.filt.rmin = sc.rmin; p.filt.rmax = sc.rmax;
   p.filt.sorted_ids = sc.sorted_ids_dev; p.filt.n_ids = sc.n_ids;
+  const int pool = select_pool_cap(k, SCAN_THREADS);
+  const int arith = P.half ? TC_ARITH_FP16 : TC_ARITH_TF32;
+
+  // 1) per-query capture thresholds: from the radius, or from the sample pass
+  if (r.range) {
+    ix->phase(IndexBase::PH_TAU, s);
+    tc_range_tau_kernel<<<(unsigned)cdiv(nq, 256), 256, 0, s>>>(P.qry.norm, nq, l2 ? 1 : 0, thr_raw, v.max_norm, d, arith, tau);
+  } else {
+    float* sample = S.alloc<float>((size_t)P.sbound * TC_NQT * TC_SAMPLE);
+    p.sample_list = P.sample_list; p.sample = sample;
+    p.mode = 0; p.work_counter = P.work;
+    ix->phase(IndexBase::PH_SAMPLE, s);
+    tc_launch(P.dev, P.half, P.sbound, P.maps, p, s);
+    ix->phase(IndexBase::PH_TAU, s);
+    // warp per query; the block kernel only redoes queries with more sampled spans than a warp stages
+    tc_tau_warp_kernel<<<(unsigned)cdiv(nq, WT_WARPS), WT_WARPS * 32, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, (int)nq, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
+    tc_tau_kernel<<<(unsigned)nq, SCAN_THREADS, 0, s>>>(probes, P.pos, P.cnt, P.item_off, v.list_len, P.items, nprobe, sample, k, l2 ? 1 : 0, P.qry.norm, v.max_norm, d, arith, cap, tau, redo);
+    ix->launch_count(1);
+  }
+  // 2) capture pass: stream every probed list chunk once, keep rows under the threshold
   p.mode = 1; p.work_counter = P.work + 1;
   ix->phase(IndexBase::PH_CAPTURE, s);
   {
@@ -1639,33 +1569,49 @@ void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const 
     tc_launch(P.dev, P.half, P.bound, P.maps, p, s);
     timer.stop();
   }
-  // 3) exact re-score of every captured row, range test, closest max_results
+  // 3) window select (top-k) or range test + exact rerank + certification
   ix->phase(IndexBase::PH_FINAL, s);
-  const uint32_t thr_key = f2ord(l2 ? radius_raw : -radius_raw);
-  const int raw = raw_out ? 1 : 0;
+  const uint32_t thr_key = r.range ? f2ord(l2 ? thr_raw : -thr_raw) : 0u;
+  const int raw = r.raw ? 1 : 0;
+  float* od = r.od;
+  long long* oi = r.oi;
+  int* oc = r.range ? r.oc : nullptr;
   const int* fin_redo = nullptr;
-  const size_t hsm = (size_t)d * 4;
-  if (hsm <= 96 * 1024) {
-    if (l2) tc_final_hybrid_kernel<true, true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, thr_key, raw, out_counts);
-    else tc_final_hybrid_kernel<false, true><<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, out_dist, out_ids, flags, redo, thr_key, raw, out_counts);
+  const size_t hsm = (size_t)d * 4;  // the query row
+  if (hsm <= 96 * 1024) {  // block select + re-score; the streaming kernel below only redoes queries whose window exceeds HF_MAXW rows
+    const auto hybrid = r.range ? (l2 ? tc_final_hybrid_kernel<true, true> : tc_final_hybrid_kernel<false, true>)
+                                : (l2 ? tc_final_hybrid_kernel<true, false> : tc_final_hybrid_kernel<false, false>);
+    hybrid<<<(unsigned)nq, HF_THREADS, hsm, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, od, oi, flags, redo, thr_key, raw, oc);
     fin_redo = redo;
     ix->launch_count(1);
   }
-  const int pool = select_pool_cap(k, SCAN_THREADS);
   const size_t fin_smem = tc_stream_smem(d, pool);
-  if (l2) tc_final_kernel<true, true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, thr_key, raw, out_counts);
-  else tc_final_kernel<false, true><<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, out_dist, out_ids, flags, fin_redo, thr_key, raw, out_counts);
+  const auto stream_fin = r.range ? (l2 ? tc_final_kernel<true, true> : tc_final_kernel<false, true>)
+                                  : (l2 ? tc_final_kernel<true, false> : tc_final_kernel<false, false>);
+  stream_fin<<<(unsigned)nq, SCAN_THREADS, fin_smem, s>>>(cand, cand_cnt, cap, tau, P.qry.norm, v.max_norm, q, v.vecs, v.ids, d, arith, k, pool, od, oi, flags, fin_redo, thr_key, raw, oc);
   tc_compact_flags(flags, (int)nq, qmap, qcount, s);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(4);
   ix->stats[1] = nq;
-  // 4) overflowed (and out-of-range) queries re-run on the exact scan's range job
+  // 4) uncertified (top-k) or overflowed (range) queries re-run on the exact scan (device-side count: blocks beyond it
+  //    exit immediately)
   ScanJob job = tc_exact_job(v, l2, d, probes, nprobe, sc);
-  job.has_thr = true;
-  job.thr_raw = radius_raw;
+  if (r.range) { job.has_thr = true; job.thr_raw = thr_raw; }
   ix->phase(IndexBase::PH_FALLBACK, s);
-  run_scan_mapped(ix, job, nq, qmap, qcount, q, k, raw_out ? nullptr : out_dist, raw_out ? out_dist : nullptr, out_ids, out_counts, s);
+  run_scan_mapped(ix, job, nq, qmap, qcount, q, k, r.raw ? nullptr : od, r.raw ? od : nullptr, oi, oc, s);
   ix->phase(IndexBase::PH_OTHER, s);
+  if (ix->profiling && getenv("B200VS_DEBUG_FLAGS")) {
+    std::vector<int> hf(nq), hc(nq);
+    std::vector<float> ht(nq);
+    B200VS_CUDA(cudaMemcpyAsync(hf.data(), flags, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(hc.data(), cand_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaMemcpyAsync(ht.data(), tau, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+    long long tot = 0; int mx = 0, r1 = 0, r2 = 0, ninf = 0;
+    for (int64_t i = 0; i < nq; ++i) { tot += hc[i]; mx = std::max(mx, hc[i]); r1 += (hf[i] & 1); r2 += (hf[i] & 2) ? 1 : 0; ninf += std::isinf(ht[i]) ? 1 : 0; }
+    fprintf(stderr, "[b200vs] tc_search nq=%lld cap=%d captured avg=%.1f max=%d flagged: threshold=%d overflow=%d tau_inf=%d\n", (long long)nq, cap, (double)tot / nq, mx, r1, r2, ninf);
+    for (int64_t i = 0, shown = 0; i < nq && shown < 4; ++i) if (hf[i]) { fprintf(stderr, "[b200vs]   q=%lld flag=%d captured=%d tau=%g\n", (long long)i, hf[i], hc[i], ht[i]); ++shown; }
+  }
   if (ix->profiling) tc_profile_counts(ix, qcount, P.totals, s);
 }
 

@@ -95,8 +95,9 @@ enum TcArith : int {
   TC_ARITH_FP16 = 2,   // rows and queries scaled by powers of two and rounded to FP16 (list scan on the mirror)
 };
 
-// true when this search can use the tensor-core pass (otherwise the caller runs the exact scan)
-bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc);
+// true when this search can use the tensor-core pass (otherwise the caller runs the exact scan).  Top-k: k <= 128.  Range
+// (k = max_results): k <= 4096, the select's limit, and the streaming finish's shared memory fits.
+bool tc_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int k, int nprobe, const SearchCtx& sc, bool range);
 // the plan-size half of tc_eligible: the view's rows, the (query, probe) pairs, work items and sample buffer fit the plan
 bool tc_plan_fits(const TcView& v, int64_t nq, int nprobe);
 // false when no query can have a finite error bound against rows of this max ||x|| (tc_eps), so the tile passes would
@@ -120,21 +121,14 @@ void tc_compact_flags(const int* flags, int nq, int* qmap, int* count, cudaStrea
 void run_scan_mapped(IndexBase* ix, const ScanJob& job, int64_t nq_max, const int* qmap, const int* qcount, const float* queries,
                      int k, float* out_dist, float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s);
 
-// probes: device [nq, nprobe] list indices (for Flat: all zeros, nprobe = 1).  q: device queries, already
-// normalised for cosine.  Writes API-semantics results, or the raw metric value (L2 distance | ip) when raw_out; uncertified
-// queries are re-run on the exact scan.
-void tc_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, int k, const long long* probes,
-               int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, bool raw_out, cudaStream_t s);
-
-// Range mode of the list scan (radius_raw: L2 keeps dist < radius_raw, IP / cosine keep ip > radius_raw).  The capture
-// threshold of each query comes from the radius widened by tc_eps; every captured row is re-scored exactly and the closest
-// max_results hits are kept by (distance, id), as the exact scan with the same threshold keeps them.  Queries whose capture
-// overflows re-run on the exact scan.  out_dist: API distances, or the raw metric value (L2 distance | ip) when raw_out;
-// out_counts: rows kept per query.  tc_range_eligible: tc_eligible's conditions without k <= 128, max_results <= 4096.
-bool tc_range_eligible(const IndexBase* ix, const TcView& v, int64_t nq, int max_results, int nprobe, const SearchCtx& sc);
-void tc_range_search(IndexBase* ix, const TcView& v, bool l2, int64_t nq, const float* q, float radius_raw, int max_results,
-                     const long long* probes, int nprobe, const SearchCtx& sc, float* out_dist, long long* out_ids, int* out_counts,
-                     bool raw_out, cudaStream_t s);
+// The tile scan of r over probes: device [nq, nprobe] list indices (for Flat: all zeros, nprobe = 1).  q: device queries,
+// already normalised for cosine.  Top-k: the capture threshold of each query comes from a sample pass.  Range (r.range,
+// thr_raw: L2 keeps dist < thr_raw, IP / cosine keep ip > thr_raw): it comes from the radius widened by tc_eps, and the
+// closest r.k hits are kept by (distance, id), as the exact scan with the same threshold keeps them, with the count of
+// each query in r.oc.  Every captured row is re-scored exactly; r.od holds API distances, or the raw metric value
+// (L2 distance | ip) when r.raw.  Queries the tile passes cannot certify (or whose capture overflows) re-run on the exact scan.
+void tc_search(IndexBase* ix, const TcView& v, const SearchReq& r, const float* q, const long long* probes, int nprobe, float thr_raw,
+               cudaStream_t s);
 
 // Exact top-nprobe of every query against a small row set (the IVF coarse quantiser): dense TF32 score matrix on the
 // tensor cores, then window select + exact FP32 re-score.  Always certified (every score is available).
