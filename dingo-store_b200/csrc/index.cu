@@ -131,7 +131,7 @@ const float* IndexBase::prepare_queries(int64_t nq, const float* xq_dev, cudaStr
 // faiss-compatible (SURVEY 8f-4): header, trained-state blob, list offsets, ids, then the live rows in list-major order
 // exactly as stored.  Float indexes ("B2VSIDX1") store FP32 rows, binary ones ("B2VSBIN1") packed rows of dim / 8 bytes.
 namespace {
-struct FileHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
+using FileHdr = IndexFileHdr;
 void wr(FILE* f, const void* p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short write"); }
 void rd(FILE* f, void* p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short read / truncated index file"); }
 }  // namespace
@@ -339,7 +339,7 @@ struct FlatIndex : IndexBase {
     quiesce();
     scratch.reset(stream);
     const float* st = x_dev;
-    if (metric == B200VS_COSINE) {  // the normaliser works in place: keep the caller's rows intact
+    if (metric == B200VS_COSINE && !loading) {  // the normaliser works in place: keep the caller's rows intact
       float* cp = scratch.alloc<float>((size_t)n * dim);
       B200VS_CUDA(cudaMemcpyAsync(cp, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
       launch_normalize_faiss(cp, n, dim, stream);

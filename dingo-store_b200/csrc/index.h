@@ -202,6 +202,10 @@ struct SearchReq {
 // the results of a search that finds nothing (an untrained or empty index): ids -1, distances 0, range counts 0
 void fill_empty(const SearchReq& r, cudaStream_t s);
 
+// The header of IndexBase::save's container ("B2VSIDX1" / "B2VSBIN1"), followed by the trained-state blob (state_len
+// bytes), the list offsets (nlist + 1 int64), the ids (count int64) and the rows (count rows, list-major).
+struct IndexFileHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
+
 struct IndexBase {
   b200vs_type type;
   b200vs_metric metric;
@@ -291,6 +295,12 @@ struct IndexBase {
   virtual void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
     (void)n; (void)x_dev; (void)ids_dev; (void)lists_dev; (void)upsert; (void)prepared;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
+  }
+  // IVF_PQ: append n code rows that are already encoded (code_size bytes each, as export_lists writes them) with their ids
+  // to the given lists, all on this device — the restore of a snapshot, whose vectors are gone
+  virtual void add_codes_dev(int64_t n, const uint8_t* codes_dev, const long long* ids_dev, const long long* lists_dev) {
+    (void)n; (void)codes_dev; (void)ids_dev; (void)lists_dev;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "appending encoded rows only exists for IVF_PQ");
   }
   // ---- building blocks of a row-sharded deployment (shard.cu); FLAT and HNSW ----
   // the refusals add (batched: b200vs_hnsw_add_batched with `batch`) would give n rows with these host ids, decided before

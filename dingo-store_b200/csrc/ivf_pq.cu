@@ -701,6 +701,21 @@ struct IvfPqIndex : IndexBase {
     L.place(n, h_list.data(), h_ids.data(), st_codes, ids_dev, store);
   }
 
+  void add_codes_dev(int64_t n, const uint8_t* codes_dev, const long long* ids_dev, const long long* lists_dev) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    require_lists();
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    std::vector<int64_t> h_ids(n);
+    std::vector<long long> h_list(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    L.place(n, h_list.data(), h_ids.data(), codes_dev, ids_dev, store);
+  }
+
   // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
   void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) override {
     require_lists();

@@ -21,9 +21,11 @@
 // number, which maps every batch to the same communicator on every rank.
 #include <dlfcn.h>
 #include <nccl.h>
+#include <unistd.h>
 
 #include <cmath>
 #include <condition_variable>
+#include <cstdio>
 #include <memory>
 #include <vector>
 
@@ -288,11 +290,12 @@ route_offsets_kernel(const int* __restrict__ cnt, long long ntiles, int W, long 
     owner_cnt[o] = (o + 1 < W ? off[(o + 1) * ntiles] : s_carry) - off[o * ntiles];
 }
 
-// moves rows, ids and (Owner::kLists) lists to their slots
+// moves rows, ids and (Owner::kLists) lists to their slots.  A row is rb opaque bytes (FP32 rows: 4 * d; IVF-PQ: the
+// stored code row), moved 16, 4 or 1 bytes at a time as the row size and the two base addresses allow.
 template <class Owner>
 static __global__ void __launch_bounds__(ROUTE_THREADS)
-route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ ids, const long long* __restrict__ lists, long long n, int d,
-                     int W, Owner owner, const long long* __restrict__ off, float* ox, long long* oids, long long* olists) {
+route_scatter_kernel(const unsigned char* __restrict__ x, const long long* __restrict__ ids, const long long* __restrict__ lists, long long n,
+                     int rb, int W, Owner owner, const long long* __restrict__ off, unsigned char* ox, long long* oids, long long* olists) {
   extern __shared__ int s_cnt[];
   __shared__ long long s_dst[ROUTE_THREADS];
   const int2 t = route_tile(Owner::kLists ? lists : ids, n, W, owner, s_cnt);
@@ -304,22 +307,51 @@ route_scatter_kernel(const float* __restrict__ x, const long long* __restrict__ 
   }
   __syncthreads();
   const long long r0 = (long long)blockIdx.x * ROUTE_THREADS;
-  const bool vec = (d & 3) == 0 && ((reinterpret_cast<size_t>(x) | reinterpret_cast<size_t>(ox)) & 15) == 0;
+  const size_t base = reinterpret_cast<size_t>(x) | reinterpret_cast<size_t>(ox);
+  const int width = (rb & 15) == 0 && (base & 15) == 0 ? 16 : (rb & 3) == 0 && (base & 3) == 0 ? 4 : 1;
   for (int j = warp; j < ROUTE_THREADS && r0 + j < n; j += ROUTE_WARPS) {  // one warp per row
     const long long src = r0 + j, dst = s_dst[j];
-    const float* xs = x + (size_t)src * d;
-    float* xd = ox + (size_t)dst * d;
-    if (vec) {
+    const unsigned char* xs = x + (size_t)src * rb;
+    unsigned char* xd = ox + (size_t)dst * rb;
+    if (width == 16) {
 #pragma unroll 1
-      for (int i = lane; i < (d >> 2); i += 32) reinterpret_cast<float4*>(xd)[i] = reinterpret_cast<const float4*>(xs)[i];
+      for (int i = lane; i < (rb >> 4); i += 32) reinterpret_cast<uint4*>(xd)[i] = reinterpret_cast<const uint4*>(xs)[i];
+    } else if (width == 4) {
+      for (int i = lane; i < (rb >> 2); i += 32) reinterpret_cast<uint32_t*>(xd)[i] = reinterpret_cast<const uint32_t*>(xs)[i];
     } else {
-      for (int i = lane; i < d; i += 32) xd[i] = xs[i];
+      for (int i = lane; i < rb; i += 32) xd[i] = xs[i];
     }
     if (lane == 0) {
       oids[dst] = ids[src];
       if (Owner::kLists) olists[dst] = lists[src];
     }
   }
+}
+
+// Restore of a list-major rank file: out[i] = the list holding row r0 + i, off[nlist + 1] being the file's list offsets
+// (ascending; the last list wins an empty-list tie, as the rows of a list start at its offset).
+static __global__ void expand_lists_kernel(const long long* __restrict__ off, int nlist, long long r0, long long n, long long* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long row = r0 + i;
+  int lo = 0, hi = nlist - 1;  // the largest l with off[l] <= row
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= row) lo = mid;
+    else hi = mid - 1;
+  }
+  out[i] = lo;
+}
+
+// Rows of a restored rank file that the owner rule does not give to `rank`, counted into *bad (the tile shape of
+// route_count_kernel, with the same Owner functors).
+template <class Owner>
+static __global__ void __launch_bounds__(ROUTE_THREADS)
+owner_check_kernel(const long long* __restrict__ keys, long long n, int W, Owner owner, int rank, unsigned long long* bad) {
+  const long long i = (long long)blockIdx.x * ROUTE_THREADS + threadIdx.x;
+  const bool off_rank = i < n && owner(keys[i], W) != rank;
+  const unsigned msk = __ballot_sync(0xffffffffu, off_rank);
+  if ((threadIdx.x & 31) == 0 && msk) atomicAdd(bad, (unsigned long long)__popc(msk));
 }
 
 }  // namespace b200vs
@@ -416,6 +448,29 @@ std::vector<T> all_gather_host(b200vs_shard* sh, const T* mine, size_t count = 1
   B200VS_CUDA(cudaMemcpyAsync(all.data(), buf.p, all.size() * sizeof(T), cudaMemcpyDeviceToHost, sh->ws));
   B200VS_CUDA(cudaStreamSynchronize(sh->ws));
   return all;
+}
+
+// Status agreement of a collective step: attempt(f) runs this rank's part and keeps its status, agree() all-gathers the
+// statuses and returns the first failure in rank order (OK when every rank succeeded), the same on every rank.
+struct Status {
+  int code = B200VS_OK;
+  std::string msg;
+};
+template <class F>
+Status attempt(F&& f) {
+  Status st;
+  st.code = guarded([&]() -> int { f(); return B200VS_OK; });
+  if (st.code != B200VS_OK) st.msg = g_last_error;
+  return st;
+}
+Status agree(b200vs_shard* sh, const Status& mine, const char* what) {
+  const std::vector<int> codes = all_gather_host(sh, &mine.code);
+  for (int w = 0; w < sh->world; ++w)
+    if (codes[w] != B200VS_OK) return Status{codes[w], w == sh->rank ? mine.msg : std::string(what) + " refused by rank " + std::to_string(w)};
+  return Status{};
+}
+void check(const Status& st) {
+  if (st.code != B200VS_OK) fail(st.code, st.msg);
 }
 
 // The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
@@ -752,17 +807,19 @@ const float* assign_rows(b200vs_shard* sh, int64_t n, const float* x_dev, DevBuf
   return xp;
 }
 
-// Moves n device rows (rows, ids and, list-sharded, lists) to their owners: a stable partition by owner on the device
-// (route_*_kernel), the counts-matrix all-gather, and one grouped ncclSend / ncclRecv.  A rank receives rank 0's rows
-// first, then rank 1's, ..., each in its caller's order; at world 1 the partitioned rows are the received ones.
+// Moves n device rows (rows of rb bytes, ids and, list-sharded, lists) to their owners: a stable partition by owner on the
+// device (route_*_kernel), the counts-matrix all-gather, and one grouped ncclSend / ncclRecv.  A rank receives rank 0's
+// rows first, then rank 1's, ..., each in its caller's order; at world 1 the partitioned rows are the received ones.
 struct Routed {
-  DevBuf<float> x;
+  DevBuf<unsigned char> x;
   DevBuf<long long> ids, lists;
   long long n = 0;
+  const float* rows() const { return reinterpret_cast<const float*>(x.p); }
 };
 template <class Owner>
-void route_rows(b200vs_shard* sh, int64_t n, const float* x, const long long* ids, const long long* lists, Owner owner, Routed& out) {
-  const int W = sh->world, r = sh->rank, d = sh->ix->dim;
+void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long long* ids, const long long* lists, Owner owner, Routed& out) {
+  const int W = sh->world, r = sh->rank, d = rb;  // d: bytes per row below
+  const unsigned char* x = static_cast<const unsigned char*>(xv);
   cudaStream_t s = sh->ws;
   ncclComm_t comm = sh->lanes[0]->comm;
   Routed snd;
@@ -807,12 +864,12 @@ void route_rows(b200vs_shard* sh, int64_t n, const float* x, const long long* id
   for (int w = 0; w < W; ++w) {
     const long long so = send_off[w], sc = send_off[w + 1] - so, ro = recv_off[w], rc = recv_off[w + 1] - ro;
     if (sc) {
-      B200VS_NCCL(nccl().Send(snd.x.p + (size_t)so * d, (size_t)sc * d, ncclFloat, w, comm, s));
+      B200VS_NCCL(nccl().Send(snd.x.p + (size_t)so * d, (size_t)sc * d, ncclUint8, w, comm, s));
       B200VS_NCCL(nccl().Send(snd.ids.p + so, (size_t)sc, ncclInt64, w, comm, s));
       if (Owner::kLists) B200VS_NCCL(nccl().Send(snd.lists.p + so, (size_t)sc, ncclInt64, w, comm, s));
     }
     if (rc) {
-      B200VS_NCCL(nccl().Recv(out.x.p + (size_t)ro * d, (size_t)rc * d, ncclFloat, w, comm, s));
+      B200VS_NCCL(nccl().Recv(out.x.p + (size_t)ro * d, (size_t)rc * d, ncclUint8, w, comm, s));
       B200VS_NCCL(nccl().Recv(out.ids.p + ro, (size_t)rc, ncclInt64, w, comm, s));
       if (Owner::kLists) B200VS_NCCL(nccl().Recv(out.lists.p + ro, (size_t)rc, ncclInt64, w, comm, s));
     }
@@ -834,32 +891,23 @@ void shard_add_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long 
   ix->set_device();
   Routed rv;
   if (sh->rows) {
-    route_rows(sh, n, x_dev, ids_dev, nullptr, RowOwner{}, rv);
+    route_rows(sh, n, x_dev, d * 4, ids_dev, nullptr, RowOwner{}, rv);
   } else {
     DevBuf<float> prep;
     DevBuf<long long> lists;
     const float* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
-    route_rows(sh, n, xp, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
+    route_rows(sh, n, xp, d * 4, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
   }
   std::vector<int64_t> hid(sh->rows ? (size_t)rv.n : 0);  // the host ids check_add and the FLAT / HNSW adds take
   if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaStreamSynchronize(s));
   // status agreement
-  int code = B200VS_OK;
-  std::string msg;
-  try {
-    ix->check_add(rv.n, hid.data(), batched, batch);
-  } catch (const StatusError& e) {
-    code = e.code; msg = e.msg;
-  }
-  const std::vector<int> codes = all_gather_host(sh, &code);
-  for (int w = 0; w < sh->world; ++w)
-    if (codes[w] != B200VS_OK) fail(codes[w], w == sh->rank ? msg : "shard add refused by rank " + std::to_string(w));
+  check(agree(sh, attempt([&] { ix->check_add(rv.n, hid.data(), batched, batch); }), "shard add"));
   if (!rv.n) return;
   if (!sh->rows) {
-    ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
+    ix->add_dev(rv.n, rv.rows(), rv.ids.p, rv.lists.p, false, true);
   } else if (ix->type == B200VS_FLAT) {
-    ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data());
+    ix->add_rows_dev(rv.n, rv.rows(), rv.ids.p, hid.data());
   } else {
     std::vector<float> hx((size_t)rv.n * d);  // the HNSW builders take host rows
     B200VS_CUDA(cudaMemcpyAsync(hx.data(), rv.x.p, (size_t)rv.n * d * 4, cudaMemcpyDeviceToHost, s));
@@ -876,6 +924,458 @@ void upload_rows(b200vs_shard* sh, int64_t n, const float* x, const int64_t* ids
   B200VS_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n * sh->ix->dim * 4, cudaMemcpyHostToDevice, sh->ws));
   B200VS_CUDA(cudaMemcpyAsync(di.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, sh->ws));
   B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+}
+
+// Rows per list of the whole sharded index: every rank's counts counts_dev[nlist] summed over the ranks (collective).
+std::vector<int64_t> sum_list_counts(b200vs_shard* sh, unsigned long long* counts_dev, int nlist) {
+  if (sh->world > 1) B200VS_NCCL(nccl().AllReduce(counts_dev, counts_dev, (size_t)nlist, ncclUint64, ncclSum, sh->lanes[0]->comm, sh->ws));
+  std::vector<int64_t> cnt((size_t)nlist);
+  B200VS_CUDA(cudaMemcpyAsync(cnt.data(), counts_dev, (size_t)nlist * 8, cudaMemcpyDeviceToHost, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  return cnt;
+}
+
+// Pre-sizes the lists this rank owns from the index-wide counts in one arena allocation; the others stay empty here.
+void reserve_owned_lists(b200vs_shard* sh, std::vector<int64_t>& cnt) {
+  const int nlist = (int)cnt.size(), per = sh->lists_per_rank();
+  for (int l = 0; l < nlist; ++l)
+    if (std::min(sh->world - 1, l / per) != sh->rank) cnt[l] = 0;  // lists owned elsewhere stay empty here
+  sh->ix->reserve_lists(cnt.data(), nlist);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Snapshots (b200vs_shard_save / b200vs_shard_load)
+// ---------------------------------------------------------------------------------------------
+// A snapshot of W ranks is <prefix>.<r>-of-<W> per rank, each in its index's own Save container, and <prefix>.manifest:
+// ManifestHdr, then one RankEntry per rank.
+struct ManifestHdr {
+  char magic[8];
+  int32_t version, type, metric, dim;
+  int32_t nlist, pq_m, pq_nbits, hnsw_m, hnsw_efc, world;  // the creation parameters that decide results (0: not used by the type)
+  int64_t max_elements;
+  int64_t state_len;      // list-sharded: bytes of the replicated trained state, 0 when untrained
+  uint64_t state_digest;  // and its digest
+};
+static_assert(sizeof(ManifestHdr) == 72, "manifest header layout");
+struct RankEntry {
+  int64_t rows, bytes;  // live rows of the rank, size of its file
+  uint64_t digest;      // of the whole file
+};
+constexpr char kManifestMagic[8] = {'B', '2', 'V', 'S', 'S', 'H', 'M', '1'};
+constexpr int32_t kManifestVersion = 1;
+constexpr size_t kRestoreChunkBytes = 64u << 20;  // rows read, uploaded and routed per restore round
+
+// 64-bit content digest of a byte stream, fed in pieces of any size: 32-byte blocks, word j of a block through a
+// multiply-rotate mix into lane j (four independent chains, so the host digests at memory speed), the zero-padded tail
+// and the length last, the lanes folded with splitmix64's finalizer.  A check against corrupt, truncated or swapped
+// files, not a cryptographic hash.
+struct Digest {
+  uint64_t h[4] = {0x243f6a8885a308d3ULL, 0x13198a2e03707344ULL, 0xa4093822299f31d0ULL, 0x082efa98ec4e6c89ULL};
+  uint64_t len = 0;
+  unsigned char tail[32];
+  size_t nt = 0;
+  static uint64_t mix(uint64_t h, uint64_t w) {
+    h ^= w * 0x9e3779b97f4a7c15ULL;
+    return ((h << 31) | (h >> 33)) * 0xbf58476d1ce4e5b9ULL;
+  }
+  void block(const unsigned char* b) {
+    uint64_t w[4];
+    memcpy(w, b, 32);
+    for (int j = 0; j < 4; ++j) h[j] = mix(h[j], w[j]);
+  }
+  void update(const void* p, size_t n) {
+    const unsigned char* b = static_cast<const unsigned char*>(p);
+    len += n;
+    if (nt) {
+      const size_t m = std::min(n, 32 - nt);
+      memcpy(tail + nt, b, m);
+      nt += m; b += m; n -= m;
+      if (nt < 32) return;
+      block(tail);
+      nt = 0;
+    }
+    for (; n >= 32; n -= 32, b += 32) block(b);
+    memcpy(tail, b, n);
+    nt = n;
+  }
+  uint64_t value() const {
+    Digest c = *this;
+    if (c.nt) {
+      memset(c.tail + c.nt, 0, 32 - c.nt);
+      c.block(c.tail);
+    }
+    uint64_t z = c.len;
+    for (int j = 0; j < 4; ++j) {
+      z = mix(z, c.h[j]);
+      z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
+      z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
+      z ^= z >> 31;
+    }
+    return z;
+  }
+};
+
+struct File {
+  FILE* f = nullptr;
+  File(const std::string& path, const char* mode) : f(fopen(path.c_str(), mode)) {
+    if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
+  }
+  ~File() { if (f) fclose(f); }
+  File(const File&) = delete;
+  File& operator=(const File&) = delete;
+  int64_t size() {
+    fseeko(f, 0, SEEK_END);
+    const int64_t n = ftello(f);
+    fseeko(f, 0, SEEK_SET);
+    return n;
+  }
+  void read(void* p, size_t n) {
+    if (n && fread(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short read / truncated snapshot file");
+  }
+  void write(const void* p, size_t n) {
+    if (n && fwrite(p, 1, n, f) != n) fail(B200VS_EINTERNAL, "short write");
+  }
+  void close() {
+    FILE* g = f;
+    f = nullptr;
+    if (fclose(g) != 0) fail(B200VS_EINTERNAL, "short write");
+  }
+};
+
+std::string rank_path(const std::string& prefix, int r, int W) {
+  return prefix + "." + std::to_string(r) + "-of-" + std::to_string(W);
+}
+
+// The manifest header a snapshot of this index over W ranks carries (state fields left 0)
+ManifestHdr manifest_of(const IndexBase* ix, int W) {
+  ManifestHdr m;
+  memset(&m, 0, sizeof(m));
+  memcpy(m.magic, kManifestMagic, 8);
+  m.version = kManifestVersion;
+  m.type = ix->type; m.metric = ix->metric; m.dim = ix->dim; m.world = W;
+  const b200vs_params& p = ix->params;
+  if (ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ) m.nlist = p.nlist > 0 ? p.nlist : 2048;
+  if (ix->type == B200VS_IVF_PQ) { m.pq_m = p.pq_m > 0 ? p.pq_m : 64; m.pq_nbits = p.pq_nbits > 0 ? p.pq_nbits : 8; }
+  if (ix->type == B200VS_HNSW) { m.hnsw_m = p.hnsw_m; m.hnsw_efc = p.hnsw_efc; m.max_elements = p.max_elements; }
+  return m;
+}
+
+// The trained state of a list-sharded index (empty when untrained)
+std::vector<unsigned char> state_of(IndexBase* ix) {
+  std::vector<unsigned char> blob((size_t)std::max<int64_t>(ix->get_state(nullptr, 0), 0));
+  if (!blob.empty()) ix->get_state(blob.data(), blob.size());
+  return blob;
+}
+uint64_t digest_of(const std::vector<unsigned char>& v) {
+  Digest d;
+  d.update(v.data(), v.size());
+  return d.value();
+}
+
+// The index's writer lock held across a local snapshot step: adds wait, searches in flight finish first, and the step's own
+// reader holds (RwSharedGuard) see this hold and do not lock again.
+struct WriterHold {
+  std::unique_lock<std::shared_mutex> lk;
+  const IndexBase* prev;
+  explicit WriterHold(IndexBase* ix) : lk(ix->rw), prev(RwSharedGuard::tl_held) { RwSharedGuard::tl_held = ix; }
+  ~WriterHold() { RwSharedGuard::tl_held = prev; }
+};
+
+void shard_save_locked(b200vs_shard* sh, const std::string& prefix) {
+  IndexBase* ix = sh->ix;
+  const int r = sh->rank, W = sh->world;
+  ix->set_device();
+  const std::string mine = rank_path(prefix, r, W), tmp = mine + ".tmp", man = prefix + ".manifest", man_tmp = man + ".tmp";
+  ManifestHdr mh = manifest_of(ix, W);
+  RankEntry e{0, 0, 0};
+  auto cleanup = [&] {  // temporary files only: an earlier snapshot under the same prefix stays as it was
+    unlink(tmp.c_str());
+    if (r == 0) unlink(man_tmp.c_str());
+  };
+  // 1) every rank writes its file under a temporary name
+  Status st = agree(sh, attempt([&] {
+    WriterHold hold(ix);
+    ix->save(tmp);
+    e.rows = ix->count();
+    if (!sh->rows) {
+      const std::vector<unsigned char> blob = state_of(ix);
+      mh.state_len = (int64_t)blob.size();
+      mh.state_digest = digest_of(blob);
+    }
+    File f(tmp, "rb");
+    e.bytes = f.size();
+    std::vector<unsigned char> buf(std::min<size_t>(kRestoreChunkBytes, (size_t)std::max<int64_t>(e.bytes, 1)));
+    Digest d;
+    for (int64_t at = 0; at < e.bytes; at += (int64_t)buf.size()) {
+      const size_t m = (size_t)std::min<int64_t>((int64_t)buf.size(), e.bytes - at);
+      f.read(buf.data(), m);
+      d.update(buf.data(), m);
+    }
+    e.digest = d.value();
+  }), "shard save");
+  if (st.code != B200VS_OK) { cleanup(); check(st); }
+  // 2) rank 0 writes the manifest under a temporary name
+  const std::vector<RankEntry> ents = all_gather_host(sh, &e);
+  st = agree(sh, attempt([&] {
+    if (r != 0) return;
+    File f(man_tmp, "wb");
+    f.write(&mh, sizeof(mh));
+    f.write(ents.data(), ents.size() * sizeof(RankEntry));
+    f.close();
+  }), "shard save");
+  if (st.code != B200VS_OK) { cleanup(); check(st); }
+  // 3) every file is renamed into place, the manifest last
+  st = agree(sh, attempt([&] {
+    if (rename(tmp.c_str(), mine.c_str()) != 0) fail(B200VS_EINTERNAL, "cannot rename " + tmp + " to " + mine);
+  }), "shard save");
+  if (st.code != B200VS_OK) { cleanup(); check(st); }
+  check(agree(sh, attempt([&] {
+    if (r == 0 && rename(man_tmp.c_str(), man.c_str()) != 0) fail(B200VS_EINTERNAL, "cannot rename " + man_tmp + " to " + man);
+  }), "shard save"));
+}
+
+// One rank file of a snapshot, checked against its manifest entry: the sections before the rows are kept, the rows are
+// read again by the restore rounds.
+struct RankFile {
+  std::string path;
+  int64_t rows = 0, rows_at = 0;  // rows stored, and the file offset of the row section
+  int rb = 0;                     // bytes per stored row: FP32 row or IVF-PQ code row
+  std::vector<unsigned char> state;
+  std::vector<int64_t> off, ids;  // list offsets [nlist + 1], ids [rows]
+  int nlist() const { return (int)off.size() - 1; }
+};
+
+// bytes of one stored row of a rank file: an FP32 row, or an IVF-PQ code row of ceil(M * nbits / 8) bytes
+int restore_row_bytes(const IndexBase* ix, const ManifestHdr& mh) {
+  return ix->type == B200VS_IVF_PQ ? (mh.pq_m * mh.pq_nbits + 7) / 8 : ix->dim * 4;
+}
+
+// Reads and checks one rank file.  full = false: the header and the trained state only, for a rank that reads no file of
+// its own but needs the state.  The header's sizes are checked against the file before anything is allocated from them.
+RankFile read_rank_file(IndexBase* ix, const std::string& path, const RankEntry& ent, const ManifestHdr& mh, bool full) {
+  RankFile rf;
+  rf.path = path;
+  File f(path, "rb");
+  const int64_t fsize = f.size();
+  if (full && fsize != ent.bytes) fail(B200VS_EINTERNAL, path + ": size differs from the manifest (truncated or replaced file)");
+  Digest dg;
+  auto rd = [&](void* p, size_t n) { f.read(p, n); dg.update(p, n); };
+  int64_t state_len = 0, nlist = 0, count = 0, here = 0;
+  bool lists = true;  // the file has a list-offset section
+  const char* bad = "does not match the index (type / metric / dimension / nsubvector)";
+  if (ix->type == B200VS_IVF_PQ) {  // "B2VSPQ01": int64 {magic, mode (0 untrained, 2 IVF-PQ), metric, dim, nlist, M, rows, state_len}
+    int64_t h[8];
+    rd(h, sizeof(h));
+    here = sizeof(h);
+    if (memcmp(h, "B2VSPQ01", 8) != 0 || h[2] != ix->metric || h[3] != ix->dim || h[5] != mh.pq_m) fail(B200VS_EINTERNAL, path + ": " + bad);
+    if (h[1] == 2) { nlist = h[4]; count = h[6]; state_len = h[7]; }
+    else if (h[1] == 0) lists = false;  // untrained: the header alone
+    else fail(B200VS_EINTERNAL, path + ": an IVF_PQ index in inner-Flat mode is not a list-sharded snapshot");
+  } else {
+    IndexFileHdr h;
+    rd(&h, sizeof(h));
+    here = sizeof(h);
+    if (memcmp(h.magic, "B2VSIDX1", 8) != 0 || h.type != ix->type || h.metric != ix->metric || h.dim != ix->dim)
+      fail(B200VS_EINTERNAL, path + ": " + bad);
+    nlist = h.nlist; count = h.count; state_len = h.state_len;
+  }
+  rf.rb = restore_row_bytes(ix, mh);
+  const double need = (double)state_len + (lists ? ((double)nlist + 1) * 8 : 0) + (double)count * (8 + (double)rf.rb);
+  if (state_len < 0 || count < 0 || nlist < 0 || nlist > (1 << 24) || (lists && nlist < 1) || need > (double)(fsize - here) ||
+      (full && need != (double)(fsize - here)))
+    fail(B200VS_EINTERNAL, path + ": corrupt snapshot file (header sizes do not match the file)");
+  rf.state.resize((size_t)state_len);
+  rd(rf.state.data(), rf.state.size());
+  const bool list_sharded = ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ;
+  if (list_sharded && ((int64_t)rf.state.size() != mh.state_len || digest_of(rf.state) != mh.state_digest))
+    fail(B200VS_EINTERNAL, path + ": trained state differs from the manifest's");
+  if (!full) return rf;
+  if (lists) {
+    rf.off.resize((size_t)nlist + 1);
+    rd(rf.off.data(), rf.off.size() * 8);
+  } else {
+    rf.off.assign(2, 0);
+  }
+  rf.ids.resize((size_t)count);
+  rd(rf.ids.data(), rf.ids.size() * 8);
+  rf.rows = count;
+  rf.rows_at = ftello(f.f);
+  std::vector<unsigned char> buf(std::min<size_t>(kRestoreChunkBytes, (size_t)std::max<int64_t>(count * rf.rb, 1)));
+  for (int64_t at = 0, total = count * rf.rb; at < total; at += (int64_t)buf.size()) {
+    const size_t m = (size_t)std::min<int64_t>((int64_t)buf.size(), total - at);
+    rd(buf.data(), m);
+  }
+  if (dg.value() != ent.digest) fail(B200VS_EINTERNAL, path + ": content differs from the manifest (swapped or replaced file)");
+  if (ix->type != B200VS_HNSW && count != ent.rows) fail(B200VS_EINTERNAL, path + ": row count differs from the manifest");
+  if (rf.off[0] != 0 || rf.off.back() != count) fail(B200VS_EINTERNAL, path + ": corrupt list offsets");
+  for (size_t l = 0; l + 1 < rf.off.size(); ++l)
+    if (rf.off[l] > rf.off[l + 1]) fail(B200VS_EINTERNAL, path + ": corrupt list offsets");
+  return rf;
+}
+
+// Rows of `keys` (n device values) that the owner rule does not give to this rank
+template <class Owner>
+unsigned long long count_off_rank(b200vs_shard* sh, const long long* keys, int64_t n, Owner owner) {
+  DevBuf<unsigned long long> bad;
+  bad.reserve(1, 0, sh->ws);
+  B200VS_CUDA(cudaMemsetAsync(bad.p, 0, 8, sh->ws));
+  if (n) owner_check_kernel<<<(unsigned)cdiv(n, ROUTE_THREADS), ROUTE_THREADS, 0, sh->ws>>>(keys, n, sh->world, owner, sh->rank, bad.p);
+  B200VS_CUDA(cudaGetLastError());
+  unsigned long long h = 0;
+  B200VS_CUDA(cudaMemcpyAsync(&h, bad.p, 8, cudaMemcpyDeviceToHost, sh->ws));
+  B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+  return h;
+}
+
+// The list of every row [r0, r0 + n) of a rank file, on the device
+void expand_lists(b200vs_shard* sh, const RankFile& rf, int64_t r0, int64_t n, DevBuf<long long>& d_off, long long* out) {
+  d_off.reserve(rf.off.size(), 0, sh->ws);
+  B200VS_CUDA(cudaMemcpyAsync(d_off.p, rf.off.data(), rf.off.size() * 8, cudaMemcpyHostToDevice, sh->ws));
+  if (n) expand_lists_kernel<<<(unsigned)cdiv(n, 256), 256, 0, sh->ws>>>(d_off.p, rf.nlist(), r0, n, out);
+  B200VS_CUDA(cudaGetLastError());
+}
+
+// Same world: every row of rank file rf must be owned by this rank (checked on the device).  graph_ids: HNSW, the labels of
+// the saved graph.
+void check_ownership(b200vs_shard* sh, const RankFile& rf, const std::vector<int64_t>& graph_ids) {
+  const std::vector<int64_t>& ids = sh->ix->type == B200VS_HNSW ? graph_ids : rf.ids;
+  const int64_t n = sh->rows ? (int64_t)ids.size() : rf.rows;
+  DevBuf<long long> keys, d_off;
+  keys.reserve((size_t)std::max<int64_t>(n, 1), 0, sh->ws);
+  unsigned long long bad;
+  if (sh->rows) {
+    if (n) B200VS_CUDA(cudaMemcpyAsync(keys.p, ids.data(), (size_t)n * 8, cudaMemcpyHostToDevice, sh->ws));
+    bad = count_off_rank(sh, keys.p, n, RowOwner{});
+  } else {
+    expand_lists(sh, rf, 0, n, d_off, keys.p);
+    bad = count_off_rank(sh, keys.p, n, ListOwner{(rf.nlist() + sh->world - 1) / sh->world});
+  }
+  if (bad) fail(B200VS_EINTERNAL, rf.path + ": " + std::to_string(bad) + " rows belong to another rank (a rank file loaded on the wrong rank)");
+}
+
+struct PinnedBuf {
+  unsigned char* p = nullptr;
+  explicit PinnedBuf(size_t n) { B200VS_CUDA(cudaHostAlloc((void**)&p, std::max<size_t>(n, 1), cudaHostAllocDefault)); }
+  ~PinnedBuf() { if (p) cudaFreeHost(p); }
+};
+
+void shard_load_locked(b200vs_shard* sh, const std::string& prefix) {
+  IndexBase* ix = sh->ix;
+  const int r = sh->rank, W2 = sh->world;
+  cudaStream_t s = sh->ws;
+  ix->set_device();
+  check(agree(sh, attempt([&] {
+    if (ix->count() + ix->deleted_count() > 0) fail(B200VS_EILLEGAL_PARAMETERS, "shard load needs an empty index on every rank");
+  }), "shard load"));
+  // 1) everything is checked before any index changes: the manifest against the index, every file this rank reads against
+  //    the manifest, and (same world) the owner of every row
+  ManifestHdr mh;
+  std::vector<RankEntry> ents;
+  std::vector<RankFile> files;
+  std::vector<unsigned char> state;  // list-sharded: the snapshot's trained state; HNSW: the rank's graph
+  check(agree(sh, attempt([&] {
+    File f(prefix + ".manifest", "rb");
+    f.read(&mh, sizeof(mh));
+    if (memcmp(mh.magic, kManifestMagic, 8) != 0 || mh.version != kManifestVersion || mh.world < 1 || mh.world > ROUTE_MAX_WORLD)
+      fail(B200VS_EINTERNAL, prefix + ".manifest: not a shard snapshot manifest");
+    ents.resize((size_t)mh.world);
+    f.read(ents.data(), ents.size() * sizeof(RankEntry));
+    if (fgetc(f.f) != EOF) fail(B200VS_EINTERNAL, prefix + ".manifest: trailing bytes");
+    ManifestHdr want = manifest_of(ix, mh.world);
+    want.state_len = mh.state_len; want.state_digest = mh.state_digest;
+    if (memcmp(&want, &mh, sizeof(mh)) != 0)
+      fail(B200VS_EINTERNAL, "snapshot does not match this index (type / metric / dimension / creation parameters)");
+    if (mh.world != W2 && ix->type == B200VS_HNSW)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "an HNSW snapshot restores onto the same number of ranks only (a graph belongs to its rank)");
+    if (!sh->rows && ix->is_trained()) {
+      const std::vector<unsigned char> mine = state_of(ix);
+      if ((int64_t)mine.size() != mh.state_len || digest_of(mine) != mh.state_digest)
+        fail(B200VS_EINTERNAL, "the index's trained state differs from the snapshot's");
+    }
+    for (int fi = r; fi < mh.world; fi += W2) files.push_back(read_rank_file(ix, rank_path(prefix, fi, mh.world), ents[fi], mh, true));
+    if (!sh->rows && mh.state_len > 0)
+      state = files.empty() ? read_rank_file(ix, rank_path(prefix, 0, mh.world), ents[0], mh, false).state : files[0].state;
+    std::vector<int64_t> graph_ids;
+    if (ix->type == B200VS_HNSW) {
+      state = files[0].state;
+      if (!state.empty()) {  // the labels of the saved graph, read through a standalone index
+        std::unique_ptr<IndexBase> g(make_hnsw(ix->metric, ix->dim, ix->params));
+        g->set_state(state.data(), state.size());
+        graph_ids.resize((size_t)g->count());
+        g->export_lists(nullptr, nullptr, nullptr, graph_ids.data());
+      }
+    }
+    if (mh.world == W2) check_ownership(sh, files[0], graph_ids);
+  }), "shard load"));
+  // 2) the trained state: list-sharded, installed unless the index already holds it; HNSW, the graph
+  check(agree(sh, attempt([&] {
+    if (ix->type == B200VS_HNSW && !state.empty()) ix->set_state(state.data(), state.size());
+    if (!sh->rows && !state.empty() && !ix->is_trained()) ix->set_state(state.data(), state.size());
+  }), "shard load"));
+  if (ix->type == B200VS_HNSW || (!sh->rows && mh.state_len == 0)) return;  // no rows to place
+  // 3) list-sharded: every owned list pre-sized from the index-wide list lengths in one arena allocation
+  if (!sh->rows) {
+    const int nlist = ix->nlist_now();
+    std::vector<unsigned long long> mine((size_t)nlist, 0);
+    for (const RankFile& rf : files)
+      for (int l = 0; l < std::min(nlist, rf.nlist()); ++l) mine[l] += (unsigned long long)(rf.off[l + 1] - rf.off[l]);
+    DevBuf<unsigned long long> d_cnt;
+    d_cnt.reserve((size_t)nlist, 0, s);
+    B200VS_CUDA(cudaMemcpyAsync(d_cnt.p, mine.data(), (size_t)nlist * 8, cudaMemcpyHostToDevice, s));
+    std::vector<int64_t> cnt = sum_list_counts(sh, d_cnt.p, nlist);
+    check(agree(sh, attempt([&] { reserve_owned_lists(sh, cnt); }), "shard load"));
+  }
+  // 4) rounds: each rank reads up to kRestoreChunkBytes of rows of its files into a pinned buffer and uploads them; the rows
+  //    travel with their saved list (list-sharded) or by id (FLAT) through shard_add's routing, and the owner appends them
+  //    exactly as stored: no coarse assignment, no normalisation, no encoding
+  struct Chunk { size_t file; int64_t r0, n; };
+  std::vector<Chunk> chunks;
+  const int rb = restore_row_bytes(ix, mh);
+  const int64_t per_chunk = std::max<int64_t>(1, (int64_t)kRestoreChunkBytes / rb);
+  for (size_t fi = 0; fi < files.size(); ++fi)
+    for (int64_t a = 0; a < files[fi].rows; a += per_chunk) chunks.push_back({fi, a, std::min(per_chunk, files[fi].rows - a)});
+  const long long my_rounds = (long long)chunks.size();
+  long long rounds = 0;
+  for (const long long v : all_gather_host(sh, &my_rounds)) rounds = std::max(rounds, v);
+  int64_t most = 0;
+  for (const Chunk& c : chunks) most = std::max(most, c.n);
+  PinnedBuf host((size_t)most * rb);
+  DevBuf<unsigned char> d_rows;
+  DevBuf<long long> d_ids, d_lists, d_off;
+  for (long long k = 0; k < rounds; ++k) {
+    Routed rv;
+    int64_t n = 0;
+    if (k < my_rounds) {
+      const Chunk& c = chunks[(size_t)k];
+      const RankFile& rf = files[c.file];
+      n = c.n;
+      File f(rf.path, "rb");
+      if (fseeko(f.f, rf.rows_at + c.r0 * rb, SEEK_SET) != 0) fail(B200VS_EINTERNAL, "cannot seek in " + rf.path);
+      f.read(host.p, (size_t)n * rb);
+      d_rows.reserve((size_t)n * rb, 0, s); d_ids.reserve((size_t)n, 0, s); d_lists.reserve((size_t)n, 0, s);
+      B200VS_CUDA(cudaMemcpyAsync(d_rows.p, host.p, (size_t)n * rb, cudaMemcpyHostToDevice, s));
+      B200VS_CUDA(cudaMemcpyAsync(d_ids.p, rf.ids.data() + c.r0, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+      if (!sh->rows) expand_lists(sh, rf, c.r0, n, d_off, d_lists.p);
+    }
+    if (sh->rows) route_rows(sh, n, d_rows.p, rb, d_ids.p, nullptr, RowOwner{}, rv);
+    else route_rows(sh, n, d_rows.p, rb, d_ids.p, d_lists.p, ListOwner{sh->lists_per_rank()}, rv);
+    B200VS_CUDA(cudaStreamSynchronize(s));  // the pinned buffer and the sent rows are reused next round
+    check(agree(sh, attempt([&] {
+      if (!rv.n) return;
+      if (ix->type == B200VS_IVF_FLAT) {
+        ix->add_dev(rv.n, rv.rows(), rv.ids.p, rv.lists.p, false, true);
+      } else if (ix->type == B200VS_IVF_PQ) {
+        ix->add_codes_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p);
+      } else {
+        std::vector<int64_t> hid((size_t)rv.n);
+        B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
+        B200VS_CUDA(cudaStreamSynchronize(s));
+        ix->loading = true;  // rows come back exactly as stored (already normalised for cosine)
+        try { ix->add_rows_dev(rv.n, rv.rows(), rv.ids.p, hid.data()); } catch (...) { ix->loading = false; throw; }
+        ix->loading = false;
+      }
+    }), "shard load"));
+  }
 }
 
 }  // namespace
@@ -921,6 +1421,28 @@ int b200vs_shard_hnsw_add_batched(b200vs_shard* h, int64_t n, const float* x, co
     DevBuf<long long> di;
     upload_rows(sh, n, x, ids, dx, di);
     shard_add_impl(sh, n, dx.p, di.p, true, batch);
+    return B200VS_OK;
+  });
+}
+
+// Collective snapshot of the sharded index under `prefix` (every rank passes the same prefix, a path every rank can reach).
+int b200vs_shard_save(b200vs_shard* h, const char* prefix) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    if (!prefix || !*prefix) fail(B200VS_EILLEGAL_PARAMETERS, "null snapshot prefix");
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    shard_save_locked(sh, prefix);
+    return B200VS_OK;
+  });
+}
+
+// Collective restore of a snapshot into the empty indexes of this shard, onto the same or (not HNSW) another world size.
+int b200vs_shard_load(b200vs_shard* h, const char* prefix) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    if (!prefix || !*prefix) fail(B200VS_EILLEGAL_PARAMETERS, "null snapshot prefix");
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    shard_load_locked(sh, prefix);
     return B200VS_OK;
   });
 }
@@ -1001,15 +1523,9 @@ int b200vs_shard_plan_commit(b200vs_shard* h) {
       sh->plan_counts.reserve((size_t)nlist, 0, sh->ws);
       B200VS_CUDA(cudaMemsetAsync(sh->plan_counts.p, 0, (size_t)nlist * 8, sh->ws));
     }
-    if (sh->world > 1) B200VS_NCCL(nccl().AllReduce(sh->plan_counts.p, sh->plan_counts.p, (size_t)nlist, ncclUint64, ncclSum, sh->lanes[0]->comm, sh->ws));
-    std::vector<int64_t> cnt((size_t)nlist);
-    B200VS_CUDA(cudaMemcpyAsync(cnt.data(), sh->plan_counts.p, (size_t)nlist * 8, cudaMemcpyDeviceToHost, sh->ws));
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+    std::vector<int64_t> cnt = sum_list_counts(sh, sh->plan_counts.p, nlist);
     sh->planning = false;
-    const int per = sh->lists_per_rank();
-    for (int l = 0; l < nlist; ++l)
-      if (std::min(sh->world - 1, l / per) != sh->rank) cnt[l] = 0;  // lists owned elsewhere stay empty here
-    ix->reserve_lists(cnt.data(), nlist);
+    reserve_owned_lists(sh, cnt);
     return B200VS_OK;
   });
 }

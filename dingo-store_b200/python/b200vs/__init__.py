@@ -34,7 +34,7 @@ ABI_SYMBOLS = [
     "b200vs_train_binary", "b200vs_add_with_ids_binary", "b200vs_search_binary", "b200vs_search_binary_device", "b200vs_range_search_binary",
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
-    "b200vs_shard_hnsw_add_batched", "b200vs_row_owner",
+    "b200vs_shard_hnsw_add_batched", "b200vs_row_owner", "b200vs_shard_save", "b200vs_shard_load",
 ]
 
 
@@ -144,6 +144,8 @@ def lib():
     L.b200vs_debug_hnsw_build_scratch_limit.argtypes = [vp, i64]
     L.b200vs_shard_hnsw_add_batched.argtypes = [vp, i64, vp, vp, i32]
     L.b200vs_row_owner.argtypes = [i32, i64, vp, vp]
+    L.b200vs_shard_save.argtypes = [vp, ctypes.c_char_p]
+    L.b200vs_shard_load.argtypes = [vp, ctypes.c_char_p]
     _lib = L
     return L
 
@@ -482,6 +484,14 @@ class Shard:
 
     def plan_commit(self):
         _check(lib().b200vs_shard_plan_commit(self.h))
+
+    def save(self, prefix):
+        """b200vs_shard_save (collective): <prefix>.<rank>-of-<world> per rank and <prefix>.manifest."""
+        _check(lib().b200vs_shard_save(self.h, prefix.encode()))
+
+    def load(self, prefix):
+        """b200vs_shard_load (collective): restores a snapshot into this shard's empty indexes, at the same or another world."""
+        _check(lib().b200vs_shard_load(self.h, prefix.encode()))
 
     def search(self, xq, k, seq=-1, **kw):
         xq = _f32(xq)

@@ -273,7 +273,24 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  *                     (as b200vs_search) and a walk (max(efsearch or the index's current ef, k)) beyond the search
  *                     kernel's shared memory, also when this rank's graph is still empty; the refused efsearch is not kept.
  *   shard_range_search[_device] : FLAT: b200vs_range_search's rule, equal bit for bit.  HNSW: EVECTOR_NOT_SUPPORT on every
- *                     rank before the first collective (the sequence number is still used up). */
+ *                     rank before the first collective (the sequence number is still used up).
+ *
+ * Snapshots of every shard kind (DESIGN.md 4.5).  Both calls are collectives of the write path: every rank passes the same
+ * prefix (a path every rank can reach), they use up no search sequence number, and every rank returns the same status.
+ *   shard_save : writes <prefix>.<r>-of-<W> per rank in b200vs_save's container (each one loads with plain b200vs_load) and
+ *                <prefix>.manifest (rank 0): type, metric, dim, the creation parameters that decide results, W, each rank
+ *                file's row count, size and 64-bit digest, and (IVF_FLAT, IVF_PQ) the digest of the trained state.  Files are
+ *                written under temporary names and renamed into place only when every rank has written its own; a failed
+ *                save (EINTERNAL) leaves an earlier snapshot under the same prefix as it was.
+ *   shard_load : restores a snapshot into this shard's indexes, which must be empty (else EILLEGAL_PARAMETERS); a list-sharded
+ *                index may already be trained, with the snapshot's state.  The manifest, every rank file's size and digest
+ *                and (same world) the owner of every row are checked before any index changes: a missing, truncated,
+ *                swapped or mismatched file, or an index that does not match the manifest -> EINTERNAL, every index left
+ *                empty and loadable.  Same world W: rank r restores file r, and its lists, rows and trained state equal the
+ *                saved rank's byte for byte.  Another world W' (FLAT, IVF_FLAT, IVF_PQ): every rank installs the trained
+ *                state, file f is read by rank f mod W', and every row travels to its owner under W' through shard_add's
+ *                routing (rank 0's rows first) with its saved list, stored exactly as saved: no re-assignment, no second
+ *                cosine normalisation, IVF_PQ codes never re-encoded.  HNSW onto W' != W: EVECTOR_NOT_SUPPORT. */
 #define B200VS_SHARD_ID_BYTES 128
 typedef struct b200vs_shard b200vs_shard;
 int b200vs_shard_unique_id(uint8_t id[B200VS_SHARD_ID_BYTES]);
@@ -295,6 +312,9 @@ int b200vs_shard_hnsw_add_batched(b200vs_shard* shard, int64_t n, const float* x
  * (z ^= z >> 30; z *= 0xbf58476d1ce4e5b9; z ^= z >> 27; z *= 0x94d049bb133111eb; z ^= z >> 31); world in [1, 1024].  A pure
  * host function: no handle, no GPU.  Callers place rows on their owner so that shard_add moves nothing. */
 int b200vs_row_owner(int32_t world, int64_t n, const int64_t* ids, int32_t* out_rank);
+/* collective snapshot save / restore of a sharded index (see above) */
+int b200vs_shard_save(b200vs_shard* shard, const char* prefix);
+int b200vs_shard_load(b200vs_shard* shard, const char* prefix);
 int b200vs_shard_plan_add_device(b200vs_shard* shard, int64_t n, const float* x_dev);
 int b200vs_shard_plan_commit(b200vs_shard* shard);
 int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
