@@ -167,7 +167,11 @@ int b200vs_set_trained_state(b200vs_index* h, const void* blob, size_t len) {
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (!blob) fail(B200VS_EILLEGAL_PARAMETERS, "null blob");
+    int64_t live = 0;
+    { std::shared_lock<std::shared_mutex> rl(ix->rw); live = ix->count(); }
     ix->set_state(blob, len);
+    std::unique_lock<std::shared_mutex> wl(ix->rw);
+    ix->train_rows = live;  // the rule's training size: the live count at this call, as a Load sets it
     return B200VS_OK;
   });
 }
@@ -467,7 +471,46 @@ int b200vs_save(b200vs_index* h, const char* path) {
   return guarded([&]() -> int { if (!path) fail(B200VS_EILLEGAL_PARAMETERS, "null path"); get(h)->save(path); return B200VS_OK; });
 }
 int b200vs_load(b200vs_index* h, const char* path) {
-  return guarded([&]() -> int { if (!path) fail(B200VS_EILLEGAL_PARAMETERS, "null path"); get(h)->load(path); return B200VS_OK; });
+  return guarded([&]() -> int {
+    if (!path) fail(B200VS_EILLEGAL_PARAMETERS, "null path");
+    IndexBase* ix = get(h);
+    ix->load(path);
+    std::unique_lock<std::shared_mutex> wl(ix->rw);
+    ix->train_rows = ix->count();  // train_data_size_ = ntotal, vector_index_ivf_flat.cc:503-504
+    return B200VS_OK;
+  });
+}
+
+int b200vs_need_rebuild(b200vs_index* h) {
+  int r = 0;
+  const int rc = guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    r = ix->need_rebuild() ? 1 : 0;
+    return B200VS_OK;
+  });
+  return rc == B200VS_OK ? r : -rc;
+}
+
+int b200vs_rebuild_from(b200vs_index* dst_h, b200vs_index* src_h, int64_t* n_rows) {
+  return guarded([&]() -> int {
+    if (n_rows) *n_rows = 0;
+    IndexBase* dst = get(dst_h);
+    IndexBase* src = get(src_h);
+    if (dst == src) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src are the same index");
+    std::shared_lock<std::shared_mutex> rl(src->rw);  // searches on src go on; its writers wait
+    std::unique_lock<std::shared_mutex> wl(dst->rw);
+    std::lock_guard<std::mutex> gl(dst->gpu_mu);
+    check_rebuild_pair(*dst, *src);
+    if (dst->type == B200VS_FLAT || dst->type == B200VS_BINARY_FLAT)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");  // vector_index_flat.h:111
+    dst->set_device();
+    dst->quiesce();
+    dst->scratch.reset(dst->stream);
+    const int64_t n = dst->rebuild_from(*src);
+    if (n_rows) *n_rows = n;
+    return B200VS_OK;
+  });
 }
 
 int b200vs_export_lists(b200vs_index* h, int64_t* list_off, float* vectors, uint8_t* codes, int64_t* ids) {

@@ -306,6 +306,11 @@ struct BinaryIvfIndex : BinaryIndex {
     set_device();
     quiesce();
     scratch.reset(stream);
+    train_locked(n, x, nullptr);
+  }
+  // train_binary's rule with rw and gpu_mu held, on host packed rows x, or (x_words) on padded rows already on the device,
+  // whose sample is expanded to +-1 floats there
+  void train_locked(int64_t n, const uint8_t* x, const uint32_t* x_words) {
     const int k = n < nlist ? 1 : nlist;  // "data size too small, nlist degenerate to 1"
     const int max_pts = 256, niter = 10;
     const int64_t seed = 1234;
@@ -320,16 +325,9 @@ struct BinaryIvfIndex : BinaryIndex {
     if (sample_b > (double)free_b)
       fail(B200VS_EINTERNAL, "binary training sample of " + std::to_string((long long)(sample_b / 1e6)) + " MB (+-1 floats) does not fit in " +
                                  std::to_string((long long)(free_b / 1000000)) + " MB of free device memory");
-    std::vector<float> pm1((size_t)m * dim);  // bad_alloc -> EINTERNAL, index stays untrained
-    for (int64_t i = 0; i < m; ++i) {
-      const uint8_t* row = x + (size_t)(pick.empty() ? i : pick[i]) * nb;
-      float* o = pm1.data() + (size_t)i * dim;
-      for (int b = 0; b < dim; ++b) o[b] = ((row[b >> 3] >> (b & 7)) & 1) ? 1.0f : -1.0f;
-    }
     DevBuf<long long> iota;
     std::vector<float> c;
-    // if the device fills up in between, kmeans_gpu's DevBuf::reserve fails the same way (CudaError -> EINTERNAL)
-    kmeans_gpu(this, B200VS_L2, dim, m, pm1.data(), k, niter, max_pts, seed, c, [&](const float* xd, int64_t mm, const float* cd, int kk, long long* out) {
+    auto assign = [&](const float* xd, int64_t mm, const float* cd, int kk, long long* out) {
       ScanJob j;
       j.vecs = cd; j.ids = iota.p; j.d = dim; j.mode = 0; j.n = kk;
       const int64_t chunk = 32768;
@@ -338,12 +336,65 @@ struct BinaryIvfIndex : BinaryIndex {
         run_scan(this, j, std::min(chunk, mm - a), xd + (size_t)a * dim, 1, nullptr, nullptr, out + a, nullptr, stream);
         scratch.release(mark);
       }
-    }, [&](int kk) { iota.reserve(kk, 0, stream); launch_iota(iota.p, kk, stream); });
+    };
+    auto prepare_ids = [&](int kk) { iota.reserve(kk, 0, stream); launch_iota(iota.p, kk, stream); };
+    // if the device fills up in between, kmeans_gpu's DevBuf::reserve fails the same way (CudaError -> EINTERNAL)
+    if (x_words) {
+      DevBuf<long long> d_pick;
+      DevBuf<float> pm1;
+      if (!pick.empty()) {
+        d_pick.reserve(m, 0, stream);
+        B200VS_CUDA(cudaMemcpyAsync(d_pick.p, pick.data(), (size_t)m * 8, cudaMemcpyHostToDevice, stream));
+      }
+      pm1.reserve((size_t)m * dim, 0, stream);
+      launch_expand_pm1(x_words, d_pick.p, m, w, dim, pm1.p, stream);
+      kmeans_gpu_dev(this, dim, m, pm1.p, k, niter, max_pts, seed, c, assign, prepare_ids);
+    } else {
+      std::vector<float> pm1((size_t)m * dim);  // bad_alloc -> EINTERNAL, index stays untrained
+      for (int64_t i = 0; i < m; ++i) {
+        const uint8_t* row = x + (size_t)(pick.empty() ? i : pick[i]) * nb;
+        float* o = pm1.data() + (size_t)i * dim;
+        for (int b = 0; b < dim; ++b) o[b] = ((row[b >> 3] >> (b & 7)) & 1) ? 1.0f : -1.0f;
+      }
+      kmeans_gpu(this, B200VS_L2, dim, m, pm1.data(), k, niter, max_pts, seed, c, assign, prepare_ids);
+    }
     std::vector<uint8_t> bin((size_t)k * nb, 0);
     for (int ci = 0; ci < k; ++ci)
       for (int b = 0; b < dim; ++b)
         if (c[(size_t)ci * dim + b] > 0.0f) bin[(size_t)ci * nb + (b >> 3)] |= (uint8_t)(1u << (b & 7));
     install_centroids(bin.data(), k);
+    train_rows = n;
+  }
+
+  // VectorIndexIvfFlat::NeedToRebuild, vector_index_ivf_flat.cc:751-776 (max_points_per_centroid = 256)
+  bool need_rebuild() const override {
+    if (!trained) return false;
+    const int64_t nlist_org = params.nlist > 0 ? params.nlist : 2048;
+    if (nlist == nlist_org && nlist == 1) return false;
+    if (nlist != nlist_org && nlist == 1 && L.live >= 256 * nlist_org) return true;
+    if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
+    return false;
+  }
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+    std::vector<int64_t> ids;
+    std::vector<long long> slots;
+    L.live_slots(ids, slots);
+    sorted_live_rows(this, ids, slots, store.words.p, w, rows, out_ids);
+    return (int64_t)ids.size();
+  }
+  // train on src's padded rows in ascending id order, then add them in that order
+  int64_t rebuild_from(IndexBase& src) override {
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    const int64_t n = src.sorted_rows(rows, ids);
+    if (n == 0) return 0;
+    train_locked(n, nullptr, rows.p);
+    scratch.reset(stream);
+    std::vector<int64_t> h_ids(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids.p, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    place_locked(n, rows.p, ids.p, h_ids.data());
+    return n;
   }
 
   int resolve_nprobe(const SearchCtx& sc) const {
@@ -380,6 +431,10 @@ struct BinaryIvfIndex : BinaryIndex {
     const uint32_t* st = upload(n, x);
     long long* st_ids = scratch.alloc<long long>(n);
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
+    place_locked(n, st, st_ids, in_ids);
+  }
+  // padded device rows st and ids st_ids (in_ids: the same on the host) to the tails of their nearest lists; rw and gpu_mu held
+  void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids) {
     // nearest centroid, ties to the smaller list id (the coarse pass with nprobe = 1)
     long long* lists = scratch.alloc<long long>(n);
     for (int64_t a = 0; a < n; a += 32768) {

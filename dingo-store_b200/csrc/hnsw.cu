@@ -1037,6 +1037,10 @@ struct HnswIndex : IndexBase {
 
   void add_batched(int64_t n, const float* x, const int64_t* in_ids, int batch) {
     std::unique_lock<std::shared_mutex> wl(rw);
+    add_batched_locked(n, x, in_ids, batch, false);
+  }
+  // add_batched with rw held; prepared = rows stored as given (cosine rows are already normalised)
+  void add_batched_locked(int64_t n, const float* x, const int64_t* in_ids, int batch, bool prepared) {
     const BuildPlan P = batched_plan(n, batch);
     batch = P.batch;
     const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
@@ -1051,7 +1055,7 @@ struct HnswIndex : IndexBase {
     const int64_t n0_call = G.n, ntot = G.n + n;
     std::vector<float> rows((size_t)n * dim);
     for (int64_t i = 0; i < n; ++i) {
-      if (metric == B200VS_COSINE) normalize_for_hnsw(x + (size_t)i * dim, dim, &rows[(size_t)i * dim]);
+      if (metric == B200VS_COSINE && !prepared) normalize_for_hnsw(x + (size_t)i * dim, dim, &rows[(size_t)i * dim]);
       else memcpy(&rows[(size_t)i * dim], x + (size_t)i * dim, (size_t)dim * 4);
     }
     std::default_random_engine rng = G.rng;
@@ -1365,6 +1369,28 @@ struct HnswIndex : IndexBase {
 
   int64_t count() const override { return G.n - G.ndeleted; }
   int64_t deleted_count() const override { return G.ndeleted; }
+  // VectorIndexHnsw::NeedToRebuild, hnsw.cc:577-590: tombstones are more than half of every node, live or deleted
+  bool need_rebuild() const override { return G.n > 0 && G.ndeleted > 0 && G.ndeleted > G.n / 2; }
+  // the live nodes' stored rows (cosine: already normalised) in ascending label order, through the batched builder with
+  // the default batch; this fresh index's level generator draws the levels, so the graph has no tombstones
+  int64_t rebuild_from(IndexBase& other) override {
+    const HostGraph& S = static_cast<HnswIndex&>(other).G;
+    std::vector<std::pair<int64_t, int64_t>> live;  // (label, node): labels of live nodes are unique
+    live.reserve((size_t)(S.n - S.ndeleted));
+    for (int64_t i = 0; i < S.n; ++i) if (!S.deleted[i]) live.emplace_back(S.labels[i], i);
+    const int64_t n = (int64_t)live.size();
+    if (n > max_element_limit) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below src's live rows");
+    if (n == 0) return 0;
+    std::sort(live.begin(), live.end());
+    std::vector<float> rows((size_t)n * dim);
+    std::vector<int64_t> ids(n);
+    for (int64_t i = 0; i < n; ++i) {
+      ids[i] = live[i].first;
+      memcpy(&rows[(size_t)i * dim], S.data.data() + (size_t)live[i].second * dim, (size_t)dim * 4);
+    }
+    add_batched_locked(n, rows.data(), ids.data(), 0, true);
+    return n;
+  }
   int64_t memory_size() const override {
     return (int64_t)(G.n * ((G.maxM0 + 1) * 4 + (int64_t)dim * 4 + 8));  // hnsw.cc:612-623: per-element level-0 block
   }

@@ -429,6 +429,15 @@ struct FlatIndex : IndexBase {
   int64_t count() const override { return rowmap.count(); }
   int64_t deleted_count() const override { return rowmap.ndeleted; }
   int64_t memory_size() const override { return rowmap.store.bytes(); }
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+    // the inner Flat of an IVF-PQ region takes its writes under its own lock, not under the outer index's
+    RwSharedGuard rl(this);
+    std::vector<int64_t> ids;
+    std::vector<long long> slots;
+    rowmap.live_slots(ids, slots);
+    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(rowmap.store.vecs.p), dim, rows, out_ids);
+    return (int64_t)ids.size();
+  }
 
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override {
     RwSharedGuard rl(this);
@@ -550,6 +559,37 @@ struct IvfFlatIndex : IndexBase {
   // VectorIndexIvfFlat::Train, vector_index_ivf_flat.cc:644-712 -> faiss IndexIVFFlat::train ->
   // Clustering (niter 10, seed 1234, <= 256 points per centroid); GPU Lloyd iterations here.
   void train(int64_t n, const float* x) override;
+  // train's rule with rw and gpu_mu held: x on the host (raw), or on the device (x_dev: already prepared)
+  void train_locked(int64_t n, const float* x, bool x_dev);
+
+  // VectorIndexIvfFlat::NeedToRebuild, vector_index_ivf_flat.cc:751-776 (max_points_per_centroid = 256)
+  bool need_rebuild() const override {
+    if (!trained) return false;
+    const int64_t nlist_org = params.nlist > 0 ? params.nlist : 2048;
+    if (nlist == nlist_org && nlist == 1) return false;
+    if (nlist != nlist_org && nlist == 1 && L.live >= 256 * nlist_org) return true;
+    if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
+    return false;
+  }
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+    std::vector<int64_t> ids;
+    std::vector<long long> slots;
+    L.live_slots(ids, slots);
+    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(store.vecs.p), dim, rows, out_ids);
+    return (int64_t)ids.size();
+  }
+  // train on src's stored rows in ascending id order, then add them in that order; stored cosine rows are already normalised
+  int64_t rebuild_from(IndexBase& src) override {
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    const int64_t n = src.sorted_rows(rows, ids);
+    if (n == 0) return 0;
+    float* x = reinterpret_cast<float*>(rows.p);
+    train_locked(n, x, true);
+    scratch.reset(stream);
+    add_locked(n, x, ids.p, nullptr, nullptr, false, true);
+    return n;
+  }
 
   void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override;
   void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override;
@@ -619,10 +659,14 @@ void IvfFlatIndex::train(int64_t n, const float* x) {
   set_device();
   quiesce();
   scratch.reset(stream);
+  train_locked(n, x, false);
+}
+
+void IvfFlatIndex::train_locked(int64_t n, const float* x, bool x_dev) {
   int k = nlist;
   if (n < k) k = 1;  // "data size too small, nlist degenerate to 1", ivf_flat.cc:676-680
   std::vector<float> cent;
-  kmeans_gpu(this, metric, dim, n, x, k, 10, 256, 1234, cent, [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) {
+  auto assign = [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) {
     // assignment against the CURRENT centroids cd (device): tensor-core coarse pass when the shapes allow (certified
     // exact labels), else the exact scan
     const int64_t chunk = std::max<int64_t>(1024, std::min<int64_t>(32768, (1LL << 28) / std::max(1, kk)));
@@ -648,12 +692,16 @@ void IvfFlatIndex::train(int64_t n, const float* x) {
       scratch.release(mark);
     }
     scratch.release(mark0);
-  }, [&](int kk) {
+  };
+  auto prepare_ids = [&](int kk) {
     cent_ids.free(); cent_ids.reserve(kk, 0, stream); launch_iota(cent_ids.p, kk, stream);
     d_coff.reserve(1, 0, stream);
     B200VS_CUDA(cudaMemsetAsync(d_coff.p, 0, 8, stream));
-  });
+  };
+  if (x_dev) kmeans_gpu_dev(this, dim, n, x, k, 10, 256, 1234, cent, assign, prepare_ids);
+  else kmeans_gpu(this, metric, dim, n, x, k, 10, 256, 1234, cent, assign, prepare_ids);
   install_centroids(cent.data(), k);
+  train_rows = n;
 }
 
 void IvfFlatIndex::add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) {

@@ -274,6 +274,19 @@ struct IndexBase {
 
   virtual void train(int64_t n, const float* x) { (void)n; (void)x; }
   virtual bool is_trained() const { return true; }
+  // the n of the train call that trained the index (IVF types); after a Load or a set_trained_state, the live count then
+  int64_t train_rows = 0;
+  // VectorIndex::NeedToRebuild (b200vs_need_rebuild): the reference plugin's rule for this type; callers hold rw shared
+  virtual bool need_rebuild() const { return false; }
+  // b200vs_rebuild_from: fill this empty, untrained index (rw and gpu_mu held, scratch reset, check_rebuild_pair passed)
+  // from src's live rows in ascending id order, as a fresh train + add of them would; src is held shared.  Returns the rows.
+  virtual int64_t rebuild_from(IndexBase& src) { (void)src; fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild is not supported for this index type"); }
+  // the live rows in ascending id order on this index's device (rebuild_from's source): rows [n, row words] and ids [n];
+  // returns n.  Callers hold rw.
+  virtual int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& ids) {
+    (void)rows; (void)ids;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "this index type has no row store to rebuild from");
+  }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }
   virtual int64_t get_state(void* blob, size_t cap) { (void)blob; (void)cap; return 0; }
   virtual void add(int64_t n, const float* x, const int64_t* ids, bool upsert) = 0;

@@ -117,6 +117,11 @@ struct FlatRowMap {
     publish_len();
     compact_if_needed();
   }
+  // the live (id, row) pairs in row order
+  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows) const {
+    for (int64_t r = 0; r < rows; ++r)
+      if (h_ids[r] >= 0) { out_ids.push_back(h_ids[r]); out_rows.push_back(r); }
+  }
   // drop every row, keep the buffers
   void clear() {
     rows = 0; ndeleted = 0;
@@ -343,6 +348,12 @@ struct IvfLists {
     }
     return o;
   }
+  // the live (id, arena row) pairs, list after list in list order, as export_lists gives them
+  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows) const {
+    for (const ListMeta& m : lists)
+      for (int p = 0; p < m.len; ++p)
+        if (h_ids[m.off + p] >= 0) { out_ids.push_back(h_ids[m.off + p]); out_rows.push_back(m.off + p); }
+  }
   // every list's live rows, list after list; list_off[nlist + 1] (nullable) gets where each list starts
   template <class Store>
   void export_lists(int nlist, int64_t* list_off, const Store& store, uint8_t* out, int64_t* out_ids) const {
@@ -368,41 +379,17 @@ inline void kmeans_rand_perm(std::vector<int64_t>& perm, int64_t m, int64_t sd) 
   for (int64_t i = 0; i + 1 < m; ++i) { int64_t i2 = i + (int64_t)(mt() % (unsigned long)(m - i)); std::swap(perm[i], perm[i2]); }
 }
 
-// faiss::Clustering-shaped Lloyd k-means with the assignment step on the GPU (public algorithm; the
-// reference reaches it through index_->train at vector_index_ivf_flat.cc:695 / raw_ivf_pq.cc:485).
-// x_host RAW rows; cosine rows are normalised on the device first.  `assign(xd, m, cd, k, out)` labels m device
-// rows against the k device centroids cd; `prepare_ids(k)` lets the caller size its centroid-id array.
+// The Lloyd iterations of kmeans_gpu / kmeans_gpu_dev on the m prepared sample rows xd (device); init_src is the same rows
+// on the host (initial centroids, fixed-point scale).
 template <class AssignFn, class PrepFn>
-void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const float* x_host, int k, int niter,
-                int max_pts, int64_t seed, std::vector<float>& cent, AssignFn assign, PrepFn prepare_ids) {
+void kmeans_lloyd(IndexBase* ix, int d, int64_t m, const float* xd, const float* init_src, int k, int niter, int64_t seed,
+                  std::vector<float>& cent, AssignFn assign, PrepFn prepare_ids) {
   cudaStream_t s = ix->stream;
-  std::vector<float> sub;
-  const float* xs = x_host;
-  int64_t m = n;
-  if (n > (int64_t)k * max_pts) {
-    std::vector<int64_t> perm;
-    kmeans_rand_perm(perm, n, seed);
-    m = (int64_t)k * max_pts;
-    sub.resize((size_t)m * d);
-    for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * d], x_host + (size_t)perm[i] * d, (size_t)d * 4);
-    xs = sub.data();
-  }
-  DevBuf<float> xd, cd;
+  DevBuf<float> cd;
   DevBuf<long long> sums;
   DevBuf<int> counts;
   DevBuf<long long> asg;
-  xd.reserve((size_t)m * d, 0, s);
-  B200VS_CUDA(cudaMemcpyAsync(xd.p, xs, (size_t)m * d * 4, cudaMemcpyHostToDevice, s));
-  if (metric == B200VS_COSINE) launch_normalize_faiss(xd.p, m, d, s);
-  B200VS_CUDA(cudaStreamSynchronize(s));
   cent.assign((size_t)k * d, 0.f);
-  std::vector<float> hx;  // normalised copy for initialisation when cosine
-  const float* init_src = xs;
-  if (metric == B200VS_COSINE) {
-    hx.resize((size_t)m * d);
-    B200VS_CUDA(cudaMemcpy(hx.data(), xd.p, (size_t)m * d * 4, cudaMemcpyDeviceToHost));
-    init_src = hx.data();
-  }
   if (m == k) { memcpy(cent.data(), init_src, (size_t)m * d * 4); return; }
   {
     std::vector<int64_t> perm;
@@ -422,10 +409,10 @@ void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const flo
   std::vector<int> hc(k);
   for (int it = 0; it < niter; ++it) {
     B200VS_CUDA(cudaMemcpyAsync(cd.p, cent.data(), (size_t)k * d * 4, cudaMemcpyHostToDevice, s));
-    assign(xd.p, m, cd.p, k, asg.p);
+    assign(xd, m, cd.p, k, asg.p);
     B200VS_CUDA(cudaMemsetAsync(sums.p, 0, (size_t)k * d * 8, s));
     B200VS_CUDA(cudaMemsetAsync(counts.p, 0, (size_t)k * 4, s));
-    launch_kmeans_accumulate(xd.p, asg.p, m, d, scale, sums.p, counts.p, s);
+    launch_kmeans_accumulate(xd, asg.p, m, d, scale, sums.p, counts.p, s);
     B200VS_CUDA(cudaMemcpyAsync(hs.data(), sums.p, (size_t)k * d * 8, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(hc.data(), counts.p, (size_t)k * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
@@ -458,6 +445,80 @@ void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const flo
   }
   ix->launch_count(2 * niter);
 }
+
+// faiss::Clustering-shaped Lloyd k-means with the assignment step on the GPU (public algorithm; the
+// reference reaches it through index_->train at vector_index_ivf_flat.cc:695 / raw_ivf_pq.cc:485).
+// x_host RAW rows; cosine rows are normalised on the device first.  `assign(xd, m, cd, k, out)` labels m device
+// rows against the k device centroids cd; `prepare_ids(k)` lets the caller size its centroid-id array.
+template <class AssignFn, class PrepFn>
+void kmeans_gpu(IndexBase* ix, b200vs_metric metric, int d, int64_t n, const float* x_host, int k, int niter,
+                int max_pts, int64_t seed, std::vector<float>& cent, AssignFn assign, PrepFn prepare_ids) {
+  cudaStream_t s = ix->stream;
+  std::vector<float> sub;
+  const float* xs = x_host;
+  int64_t m = n;
+  if (n > (int64_t)k * max_pts) {
+    std::vector<int64_t> perm;
+    kmeans_rand_perm(perm, n, seed);
+    m = (int64_t)k * max_pts;
+    sub.resize((size_t)m * d);
+    for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * d], x_host + (size_t)perm[i] * d, (size_t)d * 4);
+    xs = sub.data();
+  }
+  DevBuf<float> xd;
+  xd.reserve((size_t)m * d, 0, s);
+  B200VS_CUDA(cudaMemcpyAsync(xd.p, xs, (size_t)m * d * 4, cudaMemcpyHostToDevice, s));
+  if (metric == B200VS_COSINE) launch_normalize_faiss(xd.p, m, d, s);
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  std::vector<float> hx;  // normalised copy for initialisation when cosine
+  const float* init_src = xs;
+  if (metric == B200VS_COSINE) {
+    hx.resize((size_t)m * d);
+    B200VS_CUDA(cudaMemcpy(hx.data(), xd.p, (size_t)m * d * 4, cudaMemcpyDeviceToHost));
+    init_src = hx.data();
+  }
+  kmeans_lloyd(ix, d, m, xd.p, init_src, k, niter, seed, cent, assign, prepare_ids);
+}
+
+// gather_rows: dst row i = src row (rows ? rows[i] : i), `words` 32-bit words per row, on s
+void launch_gather_words(const uint32_t* src, const long long* rows, int64_t n, int words, uint32_t* dst, cudaStream_t s);
+
+// The subsample kmeans_gpu draws (the first k * max_pts rows of kmeans_rand_perm(n, seed), or every row), as indices of the
+// n rows, uploaded to `out` on s; returns its size m and leaves out empty when every row is used.
+int64_t kmeans_sample_rows(IndexBase* ix, int64_t n, int k, int max_pts, int64_t seed, DevBuf<long long>& out);
+
+// kmeans_gpu on n rows that are already on the device and already prepared (cosine rows normalised: they are not
+// normalised again): the same subsample, drawn by kmeans_rand_perm and gathered on the device, the same initial
+// centroids, iterations and split_clusters, so the centroids equal kmeans_gpu's on the same rows.
+template <class AssignFn, class PrepFn>
+void kmeans_gpu_dev(IndexBase* ix, int d, int64_t n, const float* x_dev, int k, int niter, int max_pts, int64_t seed,
+                    std::vector<float>& cent, AssignFn assign, PrepFn prepare_ids) {
+  cudaStream_t s = ix->stream;
+  DevBuf<long long> pick;
+  const int64_t m = kmeans_sample_rows(ix, n, k, max_pts, seed, pick);
+  DevBuf<float> xd;
+  const float* xs = x_dev;
+  if (pick.p) {
+    xd.reserve((size_t)m * d, 0, s);
+    launch_gather_words(reinterpret_cast<const uint32_t*>(x_dev), pick.p, m, d, reinterpret_cast<uint32_t*>(xd.p), s);
+    xs = xd.p;
+  }
+  std::vector<float> hx((size_t)m * d);
+  B200VS_CUDA(cudaMemcpyAsync(hx.data(), xs, (size_t)m * d * 4, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));
+  kmeans_lloyd(ix, d, m, xs, hx.data(), k, niter, seed, cent, assign, prepare_ids);
+}
+
+// The live rows of an index in ascending id order, on its device (b200vs_rebuild_from): (ids[i], slots[i]) are the live
+// rows in the index's own storage order; they are sorted by id with a stable device radix sort (rows that share an id keep
+// that order), and row slots[i] of src (`words` 32-bit words per row) is gathered into out_rows.  Runs on ix's stream.
+void sorted_live_rows(IndexBase* ix, const std::vector<int64_t>& ids, const std::vector<long long>& slots, const uint32_t* src,
+                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids);
+// out [m, dim] = the +-1 floats (binary_to_real: bit set -> 1, else -1) of padded binary rows words [.., w] (rows ? rows[i] : i)
+void launch_expand_pm1(const uint32_t* words, const long long* rows, int64_t m, int w, int dim, float* out, cudaStream_t s);
+// the refusals b200vs_rebuild_from shares for every type: dst must be empty, untrained, another index of the same type,
+// metric, dimension, result-deciding creation parameters and device
+void check_rebuild_pair(const IndexBase& dst, const IndexBase& src);
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids);
 

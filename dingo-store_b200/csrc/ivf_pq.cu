@@ -545,20 +545,68 @@ struct IvfPqIndex : IndexBase {
     train_coarse_locked(n, x, nlist, cent);
     train_codebooks_locked(n, x, cent, cb);
     install(cent.data(), cb.data());
+    train_rows = n;
+  }
+  int64_t train_need() const { return std::max<int64_t>(256LL * nlist, 256LL * ksub); }
+
+  // VectorIndexIvfPq::NeedToRebuild (ivf_pq.cc:411-436): inner-Flat mode once train's `need` rows are held; IVF-PQ mode
+  // VectorIndexRawIvfPq::NeedToRebuild (raw_ivf_pq.cc:518-526)
+  bool need_rebuild() const override {
+    if (mode == kFlat) {  // the inner index's writers hold its own lock only
+      RwSharedGuard rl(flat.get());
+      return flat->count() >= train_need();
+    }
+    if (mode == kIvfPq) return L.live / 2 >= train_rows;
+    return false;
+  }
+  // from an index in inner-Flat mode: train's rule on its stored rows in ascending id order (IVF-PQ from `need` rows on,
+  // else inner Flat again), then one add of them in that order.  An IVF-PQ mode index keeps only codes: refused.
+  int64_t rebuild_from(IndexBase& other) override {
+    IvfPqIndex& src = static_cast<IvfPqIndex&>(other);
+    if (src.mode == kIvfPq) fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild_from an IVF_PQ index in IVF-PQ mode: only its codes are stored");
+    if (src.mode == kNone) return 0;
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    const int64_t n = src.flat->sorted_rows(rows, ids);
+    if (n == 0) return 0;
+    const float* x = reinterpret_cast<const float*>(rows.p);
+    if (n < train_need()) {
+      std::vector<int64_t> h_ids(n);
+      B200VS_CUDA(cudaMemcpy(h_ids.data(), ids.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
+      std::unique_ptr<IndexBase> f(make_flat(metric, dim, params));
+      f->loading = true;  // stored rows: not normalised again
+      f->add_rows_dev(n, x, ids.p, h_ids.data());
+      f->loading = false;
+      flat = std::move(f);
+      mode = kFlat;
+      train_rows = n;
+      return n;
+    }
+    const int wpb = encode_warps();
+    std::vector<float> cent, cb;
+    train_coarse_locked(n, x, nlist, cent, true);
+    train_codebooks_locked(n, x, cent, cb, true);
+    install(cent.data(), cb.data());
+    train_rows = n;
+    scratch.reset(stream);
+    add_dev_locked(n, x, ids.p, nullptr, false, true, wpb);
+    return n;
   }
 
   // The two stages of train, also run separately by the list-sharded trainer (shard.cu).  Callers hold rw and gpu_mu, with
-  // the scratch reset.  Coarse stage: k centroids of the n rows (level-1 quantiser, niter 10).
-  void train_coarse_locked(int64_t n, const float* x, int k, std::vector<float>& cent) {
+  // the scratch reset.  x: raw host rows, or (x_dev) prepared rows on the device.  Coarse stage: k centroids of the n rows
+  // (level-1 quantiser, niter 10).
+  void train_coarse_locked(int64_t n, const float* x, int k, std::vector<float>& cent, bool x_dev = false) {
     const bool l2 = metric == B200VS_L2;
     DevBuf<long long> cid;
-    kmeans_gpu(this, metric, dim, n, x, k, 10, 256, 1234, cent,
-               [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) { assign_dev(cd, kk, cid.p, xd, dim, l2, m, out, stream); },
-               [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); });
+    auto assign = [&](const float* xd, int64_t m, const float* cd, int kk, long long* out) { assign_dev(cd, kk, cid.p, xd, dim, l2, m, out, stream); };
+    auto prepare_ids = [&](int kk) { cid.free(); cid.reserve(kk, 0, stream); launch_iota(cid.p, kk, stream); };
+    if (x_dev) kmeans_gpu_dev(this, dim, n, x, k, 10, 256, 1234, cent, assign, prepare_ids);
+    else kmeans_gpu(this, metric, dim, n, x, k, 10, 256, 1234, cent, assign, prepare_ids);
   }
 
   // PQ stage: the codebooks [M, ksub, dsub] of the n rows' residuals to the centroids cent [nc, dim]
-  void train_codebooks_locked(int64_t n, const float* x, const std::vector<float>& cent, std::vector<float>& cb) {
+  void train_codebooks_locked(int64_t n, const float* x, const std::vector<float>& cent, std::vector<float>& cb, bool x_dev = false) {
     const bool l2 = metric == B200VS_L2;
     const int nc = (int)(cent.size() / dim);
     DevBuf<long long> cid;
@@ -571,13 +619,19 @@ struct IvfPqIndex : IndexBase {
       for (int64_t i = 0; i + 1 < n; ++i) { int64_t i2 = i + (int64_t)(mt() % (unsigned long)(n - i)); std::swap(perm[i], perm[i2]); }
     }
     std::vector<float> sub((size_t)m * dim);
-    for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * dim], x + (size_t)perm[i] * dim, (size_t)dim * 4);
     DevBuf<float> xd, cd;
-    DevBuf<long long> asg;
+    DevBuf<long long> asg, d_perm;
     xd.reserve((size_t)m * dim, 0, stream); cd.reserve((size_t)nc * dim, 0, stream); asg.reserve(m, 0, stream);
-    B200VS_CUDA(cudaMemcpyAsync(xd.p, sub.data(), (size_t)m * dim * 4, cudaMemcpyHostToDevice, stream));
+    if (x_dev) {  // the same sample, gathered on the device; the rows are already prepared
+      d_perm.reserve(m, 0, stream);
+      B200VS_CUDA(cudaMemcpyAsync(d_perm.p, perm.data(), (size_t)m * 8, cudaMemcpyHostToDevice, stream));
+      launch_gather_words(reinterpret_cast<const uint32_t*>(x), d_perm.p, m, dim, reinterpret_cast<uint32_t*>(xd.p), stream);
+    } else {
+      for (int64_t i = 0; i < m; ++i) memcpy(&sub[(size_t)i * dim], x + (size_t)perm[i] * dim, (size_t)dim * 4);
+      B200VS_CUDA(cudaMemcpyAsync(xd.p, sub.data(), (size_t)m * dim * 4, cudaMemcpyHostToDevice, stream));
+      if (metric == B200VS_COSINE) launch_normalize_faiss(xd.p, m, dim, stream);
+    }
     B200VS_CUDA(cudaMemcpyAsync(cd.p, cent.data(), (size_t)nc * dim * 4, cudaMemcpyHostToDevice, stream));
-    if (metric == B200VS_COSINE) launch_normalize_faiss(xd.p, m, dim, stream);
     cid.free(); cid.reserve(nc, 0, stream); launch_iota(cid.p, nc, stream);
     assign_dev(cd.p, nc, cid.p, xd.p, dim, l2, m, asg.p, stream);
     std::vector<long long> h_asg(m);
@@ -676,6 +730,10 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
+    add_dev_locked(n, x_dev, ids_dev, lists_dev, upsert, prepared, wpb);
+  }
+  // add_dev's steps with rw and gpu_mu held and the scratch reset; wpb = encode_warps()
+  void add_dev_locked(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared, int wpb) {
     std::vector<int64_t> h_ids(n);
     B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));

@@ -398,6 +398,11 @@ bool VectorIndexB200::NeedTrain() {
          vector_index_type == pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT;
 }
 bool VectorIndexB200::IsTrained() { return index_ && b200vs_is_trained(index_) != 0; }
+bool VectorIndexB200::NeedToRebuild() { return index_ && b200vs_need_rebuild(index_) == 1; }
+butil::Status VectorIndexB200::RebuildFrom(VectorIndexB200& old) {
+  if (!index_ || !old.index_) return butil::Status(pb::error::EINTERNAL, "index not created");
+  return ToStatus(b200vs_rebuild_from(index_, old.index_, nullptr));
+}
 bool VectorIndexB200::NeedToSave(int64_t last_save_log_behind) { return SupportSave() && last_save_log_behind > 10000; }  // flat.cc:515-531
 
 namespace {

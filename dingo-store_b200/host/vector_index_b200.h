@@ -57,7 +57,10 @@ class VectorIndexB200 : public VectorIndex {
   butil::Status Train(std::vector<float>& train_datas) override;
   butil::Status Train(std::vector<uint8_t>& train_datas) override;  // packed rows, dimension / 8 bytes each
   butil::Status Train(const std::vector<pb::common::VectorWithId>& vectors) override;
-  bool NeedToRebuild() override { return false; }
+  bool NeedToRebuild() override;  // b200vs_need_rebuild: the reference plugin's rule for this type
+  // Fills this fresh index from old's live rows on the GPU (b200vs_rebuild_from), in place of RebuildVectorIndex's RocksDB
+  // scan, Train and Add: the result equals a train + add of old's rows in ascending id order.  old keeps serving reads.
+  butil::Status RebuildFrom(VectorIndexB200& old);
   bool NeedTrain() override;
   bool IsTrained() override;
   bool NeedToSave(int64_t last_save_log_behind) override;

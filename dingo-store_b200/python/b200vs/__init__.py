@@ -35,6 +35,7 @@ ABI_SYMBOLS = [
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
     "b200vs_shard_hnsw_add_batched", "b200vs_row_owner", "b200vs_shard_save", "b200vs_shard_load",
+    "b200vs_need_rebuild", "b200vs_rebuild_from",
 ]
 
 
@@ -146,6 +147,8 @@ def lib():
     L.b200vs_row_owner.argtypes = [i32, i64, vp, vp]
     L.b200vs_shard_save.argtypes = [vp, ctypes.c_char_p]
     L.b200vs_shard_load.argtypes = [vp, ctypes.c_char_p]
+    L.b200vs_need_rebuild.argtypes = [vp]
+    L.b200vs_rebuild_from.argtypes = [vp, vp, ctypes.POINTER(i64)]
     _lib = L
     return L
 
@@ -411,6 +414,19 @@ class Index:
         if n.value:
             _check(self.L.b200vs_export_list(self.h, list_id, n.value, vec.ctypes.data, ids.ctypes.data, ctypes.byref(n)))
         return vec, ids
+
+    def need_rebuild(self):
+        """VectorIndex::NeedToRebuild: the reference plugin's rebuild rule for this index type."""
+        r = int(self.L.b200vs_need_rebuild(self.h))
+        if r < 0:
+            _check(-r)
+        return bool(r)
+
+    def rebuild_from(self, src):
+        """Fill this fresh index from src's live rows in ascending id order, on the device; returns the rows copied."""
+        n = ctypes.c_int64(0)
+        _check(self.L.b200vs_rebuild_from(self.h, src.h, ctypes.byref(n)))
+        return n.value
 
     def save(self, path):
         _check(self.L.b200vs_save(self.h, path.encode()))

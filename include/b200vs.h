@@ -186,6 +186,39 @@ int32_t b200vs_dimension(b200vs_index* idx);
 int b200vs_save(b200vs_index* idx, const char* path);
 int b200vs_load(b200vs_index* idx, const char* path);
 
+/* VectorIndex::NeedToRebuild (vector_index.h:198): 1 = rebuild, 0 = not, < 0 = a status negated.  The reference plugins' rules
+ * (max_points_per_centroid = 256; count = live rows; train_rows = n of the b200vs_train[_binary] call that trained the index,
+ * or the live count after b200vs_load or at b200vs_set_trained_state; it is not saved):
+ *   IVF_FLAT, BINARY_IVF_FLAT (vector_index_ivf_flat.cc:751-776), nlist_org = the created nlist (default 2048):
+ *                    untrained, or nlist == nlist_org == 1: 0; nlist degenerated to 1: count >= 256 * nlist_org;
+ *                    nlist == nlist_org: count >= 256 * nlist_org and train_rows <= count / 2
+ *   IVF_PQ           inner-Flat mode: count >= max(256 * nlist, 256 * 2^nbits) (b200vs_train's threshold for IVF-PQ);
+ *                    IVF-PQ mode: count / 2 >= train_rows; untrained: 0 (ivf_pq.cc:411-436, raw_ivf_pq.cc:518-526)
+ *   HNSW             deleted > 0 and deleted > (count + deleted) / 2 (vector_index_hnsw.cc:577-590)
+ *   FLAT, BINARY_FLAT: 0 (vector_index_flat.h:111) */
+int b200vs_need_rebuild(b200vs_index* idx);
+
+/* Fill dst, a fresh index, from src's live rows on the device, in place of the host scan + b200vs_train + b200vs_add_with_ids
+ * loop of VectorIndexManager::RebuildVectorIndex (vector_index_manager.cc:864-1013).  dst ends up equal, byte for byte, to a
+ * fresh index trained and then filled with src's live rows in ascending id order (rows sharing an id in an IVF index keep
+ * their list-major export order), the rows taken as stored: cosine rows are already normalised and are not normalised again.
+ *   IVF_FLAT, BINARY_IVF_FLAT : b200vs_train[_binary]'s rule on those rows (nlist degenerates to 1 below nlist rows), then one
+ *                               add of them
+ *   IVF_PQ in inner-Flat mode : b200vs_train's rule (IVF-PQ from max(256 * nlist, 256 * 2^nbits) rows, else inner Flat), then
+ *                               one add; IVF_PQ in IVF-PQ mode keeps only codes: EVECTOR_NOT_SUPPORT
+ *   HNSW                      : b200vs_hnsw_add_batched with the default batch; levels from dst's fresh generator, no tombstones
+ *   FLAT, BINARY_FLAT         : EVECTOR_NOT_SUPPORT
+ * EILLEGAL_PARAMETERS: dst == src, dst not empty or (IVF types) already trained, a different type, metric, dimension, nlist,
+ * nsubvector, nbits, nlinks, efconstruction or device, or an HNSW dst whose max_elements is below src's live rows.  Every
+ * refusal leaves both indexes unchanged.  An empty src: OK, dst stays untrained.  A device failure: EINTERNAL; dst may then be
+ * discarded, src is unchanged.  src is held under its reader lock (its searches go on, its writers wait), dst under its
+ * writer lock (the inner Flat index of an IVF_PQ src under its own reader lock too).  *n_rows (nullable) = rows copied.
+ * Peak device memory: src's rows, a dense copy of its live rows (n x row bytes) with 32 B per row of sort buffers, and dst's
+ * rows, all at once: about three times the live row bytes for IVF_FLAT (plus each IVF-Flat store's FP16 mirror).  A region
+ * that does not fit that on its device (e.g. 6.25 M x 1536 FP32 = 38 GB of rows on an 80 GB GPU) keeps the host rebuild;
+ * the call then fails with EINTERNAL and leaves src unchanged. */
+int b200vs_rebuild_from(b200vs_index* dst, b200vs_index* src, int64_t* n_rows);
+
 /* Export the inverted lists in list-major order (list l owns rows [list_off[l], list_off[l+1])) so a CPU
  * implementation can search the identical index.  Any output pointer may be NULL.  Flat: nlist = 1. */
 int b200vs_export_lists(b200vs_index* idx, int64_t* list_off /*[nlist+1]*/, float* vectors /*[count,dim]*/,
