@@ -25,6 +25,12 @@ void check_row_type(IndexBase* ix, bool binary_call) {
     fail(B200VS_EILLEGAL_PARAMETERS, binary_call ? "binary entry point on a float index" : "float entry point on a binary index");
 }
 
+// The device-pointer add and the list building blocks take FP32 rows: a binary index refuses them as the index layer did
+// before it served binary shards (b200vs_shard_*_binary reach those hooks with packed rows)
+void refuse_binary_rows(IndexBase* ix, const char* what) {
+  if (ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, std::string(what) + " only exists for IVF_FLAT and IVF_PQ");
+}
+
 void check_search_args(IndexBase* ix, int64_t nq, const void* xq, const b200vs_search_params* sp) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");  // flat.cc:208-210
   if (ix->type == B200VS_HNSW && sp && (sp->efsearch < 0 || sp->efsearch > 1024))
@@ -215,6 +221,7 @@ int b200vs_add_with_ids_device(b200vs_index* h, int64_t n, const float* x_dev, c
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (n <= 0 || !x_dev || !ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+    refuse_binary_rows(ix, "device-pointer add");
     ix->add_dev(n, x_dev, (const long long*)ids_dev, (const long long*)lists_dev, upsert != 0, false);
     return B200VS_OK;
   });
@@ -224,6 +231,7 @@ int b200vs_assign_device(b200vs_index* h, int64_t n, const float* x_dev, int64_t
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (n <= 0 || !x_dev || !out_lists_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad assign arguments");
+    refuse_binary_rows(ix, "list assignment");
     std::shared_lock<std::shared_mutex> rl(ix->rw);
     ix->set_device();
     LaneGuard lane(ix, nullptr);
@@ -268,6 +276,7 @@ int b200vs_coarse_device(b200vs_index* h, int64_t nq, const float* xq_dev, int32
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (nq <= 0 || !xq_dev || !out_score_dev || !out_lists_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad coarse arguments");
+    refuse_binary_rows(ix, "coarse quantiser");
     index_read(ix, stream, nullptr, [&](const SearchCtx&, cudaStream_t s) {
       ix->coarse(nq, xq_dev, false, nprobe, list_begin, list_end, out_score_dev, (long long*)out_lists_dev, s);
     });
@@ -282,6 +291,7 @@ int b200vs_search_probes_device(b200vs_index* h, int64_t nq, const float* xq_dev
     check_search_args(ix, nq, xq_dev, sp);
     if (k <= 0) return B200VS_OK;
     if (!probes_dev || nprobe <= 0 || !out_ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad probe arguments");
+    refuse_binary_rows(ix, "probe-driven search");
     index_read(ix, stream, sp, [&](const SearchCtx& sc, cudaStream_t s) {
       SearchReq r;
       r.nq = nq; r.xq = xq_dev; r.probes = (const long long*)probes_dev; r.nprobe = nprobe; r.k = k; r.sc = &sc;

@@ -187,6 +187,17 @@ struct BinaryFlatIndex : BinaryIndex {
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
     rowmap.add(n, st, st_ids, in_ids);
   }
+  // add_binary on packed rows and ids already on this device (the owner of a row-sharded add); ids_host = the same ids
+  void add_rows_dev(int64_t n, const void* x_dev, const long long* ids_dev, const int64_t* ids_host) override {
+    check_batch_ids_unique(n, ids_host);
+    std::unique_lock<std::shared_mutex> wl(rw);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    rowmap.add(n, pad(n, static_cast<const uint8_t*>(x_dev), stream), ids_dev, ids_host);
+  }
+  void check_add(int64_t n, const int64_t* in_ids, bool, int) override { check_batch_ids_unique(n, in_ids); }
   // Delete (flat.cc:171-203): ids that are not present are ignored
   int64_t remove(int64_t n, const int64_t* del) override {
     std::unique_lock<std::shared_mutex> wl(rw);
@@ -269,13 +280,18 @@ struct BinaryIvfIndex : BinaryIndex {
   }
 
   // trained-state blob: int64 hdr[4] = {magic 'IVFB', nlist, dim, metric}; uint8 centroids[nlist * dim / 8]
+  static constexpr int64_t kStateMagic = 0x42465649;
+  void state_header(void* blob, int k) const {
+    const int64_t hdr[4] = {kStateMagic, k, dim, (int64_t)metric};
+    memcpy(blob, hdr, 32);
+  }
   void set_state(const void* blob, size_t len) override {
     std::unique_lock<std::shared_mutex> wl(rw);
     std::lock_guard<std::mutex> gl(gpu_mu);
     set_device();
     if (len < 32) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
-    if (hdr[0] != 0x42465649 || hdr[2] != dim || hdr[3] != B200VS_HAMMING) fail(B200VS_EILLEGAL_PARAMETERS, "bad binary IVF state blob");
+    if (hdr[0] != kStateMagic || hdr[2] != dim || hdr[3] != B200VS_HAMMING) fail(B200VS_EILLEGAL_PARAMETERS, "bad binary IVF state blob");
     if (hdr[1] <= 0 || hdr[1] > (1 << 24)) fail(B200VS_EILLEGAL_PARAMETERS, "bad list count in state blob");
     const int k = (int)hdr[1];
     if (len < 32 + (size_t)k * nb) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
@@ -287,8 +303,7 @@ struct BinaryIvfIndex : BinaryIndex {
     const size_t need = 32 + (size_t)nlist * nb;
     if (!blob || cap < need) return (int64_t)need;
     set_device();
-    int64_t hdr[4] = {0x42465649, nlist, dim, (int64_t)metric};
-    memcpy(blob, hdr, 32);
+    state_header(blob, nlist);
     std::vector<uint32_t> tmp((size_t)nlist * w);
     B200VS_CUDA(cudaMemcpy(tmp.data(), cent.p, tmp.size() * 4, cudaMemcpyDeviceToHost));
     for (int c = 0; c < nlist; ++c) memcpy((uint8_t*)blob + 32 + (size_t)c * nb, tmp.data() + (size_t)c * w, nb);
@@ -312,6 +327,13 @@ struct BinaryIvfIndex : BinaryIndex {
   // whose sample is expanded to +-1 floats there
   void train_locked(int64_t n, const uint8_t* x, const uint32_t* x_words) {
     const int k = n < nlist ? 1 : nlist;  // "data size too small, nlist degenerate to 1"
+    std::vector<uint8_t> bin;
+    kmeans_locked(n, x, x_words, k, bin);
+    install_centroids(bin.data(), k);
+    train_rows = n;
+  }
+  // train_locked's clustering into k <= n packed centroids bin [k, dim / 8], leaving the index as it is (rw and gpu_mu held)
+  void kmeans_locked(int64_t n, const uint8_t* x, const uint32_t* x_words, int k, std::vector<uint8_t>& bin) {
     const int max_pts = 256, niter = 10;
     const int64_t seed = 1234;
     std::vector<int64_t> pick;
@@ -358,12 +380,10 @@ struct BinaryIvfIndex : BinaryIndex {
       }
       kmeans_gpu(this, B200VS_L2, dim, m, pm1.data(), k, niter, max_pts, seed, c, assign, prepare_ids);
     }
-    std::vector<uint8_t> bin((size_t)k * nb, 0);
+    bin.assign((size_t)k * nb, 0);
     for (int ci = 0; ci < k; ++ci)
       for (int b = 0; b < dim; ++b)
         if (c[(size_t)ci * dim + b] > 0.0f) bin[(size_t)ci * nb + (b >> 3)] |= (uint8_t)(1u << (b & 7));
-    install_centroids(bin.data(), k);
-    train_rows = n;
   }
 
   // VectorIndexIvfFlat::NeedToRebuild, vector_index_ivf_flat.cc:751-776 (max_points_per_centroid = 256)
@@ -401,11 +421,36 @@ struct BinaryIvfIndex : BinaryIndex {
     const int np = sc.nprobe > 0 ? sc.nprobe : 80;  // Constant::kSearchBinaryIvfFlatParamNprobe (constant.h:181), ivf_flat.cc:207-209
     return std::min(np, nlist);                    // ivf_flat.cc:234
   }
-  // IndexBinaryFlat quantiser: the nprobe nearest lists by (Hamming distance, list id)
-  long long* coarse_lists(int64_t nq, const uint32_t* q, int nprobe, cudaStream_t s, long long* out = nullptr) {
+  int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
+  // IndexBinaryFlat quantiser over centroid rows [c0, c1) (c1 < 0: every row): the nprobe nearest lists by (Hamming
+  // distance, list id), as global list ids, with their distances in out_dist when it is set
+  long long* coarse_lists(int64_t nq, const uint32_t* q, int nprobe, cudaStream_t s, long long* out = nullptr, int c0 = 0, int c1 = -1,
+                          float* out_dist = nullptr) {
+    if (c1 < 0) c1 = nlist;
     long long* probes = out ? out : scratch.alloc<long long>((size_t)nq * nprobe);
-    run_scan(this, hamming_job(cent.p, cent_ids.p, nlist), nq, reinterpret_cast<const float*>(q), nprobe, nullptr, nullptr, probes, nullptr, s);
+    run_scan(this, hamming_job(cent.p + (size_t)c0 * w, cent_ids.p + c0, c1 - c0), nq, reinterpret_cast<const float*>(q), nprobe, nullptr,
+             out_dist, probes, nullptr, s);
     return probes;
+  }
+  // packed query rows; the list-sharded search's coarse step on its slice of the batch (prepared has no meaning for bits)
+  void coarse(int64_t nq, const void* xq, bool, int nprobe, int c0, int c1, float* out_score, long long* out_lists, cudaStream_t s) override {
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
+    coarse_lists(nq, pad(nq, static_cast<const uint8_t*>(xq), s), nprobe, s, out_lists, c0, c1, out_score);
+  }
+  // nearest list of n padded rows, ties to the smaller list id (the coarse pass with nprobe = 1), in chunks whose select
+  // workspace is handed back before the next
+  void assign_words(int64_t n, const uint32_t* st, long long* lists, cudaStream_t s) {
+    for (int64_t a = 0; a < n; a += 32768) {
+      const auto mark = scratch.mark();
+      coarse_lists(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, s, lists + a);
+      scratch.release(mark);
+    }
+  }
+  // packed rows: the assignment the sender of a list-sharded add routes by (a lane must be held)
+  void assign_lists_dev(int64_t n, const void* x_dev, long long* out_lists_dev, cudaStream_t s) override {
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    assign_words(n, pad(n, static_cast<const uint8_t*>(x_dev), s), out_lists_dev, s);
   }
   TcView view() const {
     TcView v = store.view();
@@ -433,19 +478,33 @@ struct BinaryIvfIndex : BinaryIndex {
     B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
     place_locked(n, st, st_ids, in_ids);
   }
-  // padded device rows st and ids st_ids (in_ids: the same on the host) to the tails of their nearest lists; rw and gpu_mu held
-  void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids) {
-    // nearest centroid, ties to the smaller list id (the coarse pass with nprobe = 1)
-    long long* lists = scratch.alloc<long long>(n);
-    for (int64_t a = 0; a < n; a += 32768) {
-      const auto mark = scratch.mark();  // each chunk's select workspace is handed back before the next
-      coarse_lists(std::min<int64_t>(32768, n - a), st + (size_t)a * w, 1, stream, lists + a);
-      scratch.release(mark);
+  // padded device rows st and ids st_ids (in_ids: the same on the host) to the tails of their lists: lists_dev, or (null) the
+  // nearest ones; rw and gpu_mu held
+  void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids, const long long* lists_dev = nullptr) {
+    if (!lists_dev) {
+      long long* lists = scratch.alloc<long long>(n);
+      assign_words(n, st, lists, stream);
+      lists_dev = lists;
     }
     std::vector<long long> h_list(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
     B200VS_CUDA(cudaStreamSynchronize(stream));
     L.place(n, h_list.data(), in_ids, st, st_ids, store);
+  }
+  // add_binary on packed rows and ids already on this device, to the caller's lists (the owner of a list-sharded add) or
+  // (lists_dev null) the nearest ones; prepared has no meaning for bits
+  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool) override {
+    std::unique_lock<std::shared_mutex> wl(rw);
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    scratch.reset(stream);
+    std::vector<int64_t> h_ids(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    if (upsert) L.remove(n, h_ids.data(), store);
+    place_locked(n, pad(n, static_cast<const uint8_t*>(x_dev), stream), ids_dev, h_ids.data(), lists_dev);
   }
   // Delete (ivf_flat.cc:162-189): untrained -> OK; nothing removed -> EVECTOR_INVALID (api.cu)
   int64_t remove(int64_t n, const int64_t* del) override {
@@ -461,15 +520,14 @@ struct BinaryIvfIndex : BinaryIndex {
   }
 
   // Search / RangeSearch (ivf_flat.cc:203-350): untrained -> empty results (:224-227); the range scan is the exact one
-  // (:342-345)
+  // (:342-345).  A caller's probe table (a list-sharded search) takes the place of the coarse pass.
   void search(const SearchReq& r, cudaStream_t s) override {
-    refuse_probes(r);
     if (!trained) { fill_empty(r, s); return; }
     const SearchCtx& sc = *r.sc;
     const float thr = radius_threshold(r);
     const uint32_t* q = pad(r.nq, static_cast<const uint8_t*>(r.xq), s);
-    const int nprobe = resolve_nprobe(sc);
-    long long* probes = coarse_lists(r.nq, q, nprobe, s);
+    const int nprobe = r.probes ? r.nprobe : resolve_nprobe(sc);
+    const long long* probes = r.probes ? r.probes : coarse_lists(r.nq, q, nprobe, s);
     if (profiling && !r.range) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
     const TcView v = view();
     ScanJob j = list_job(sc, probes, nprobe);
@@ -495,5 +553,28 @@ struct BinaryIvfIndex : BinaryIndex {
 };
 
 IndexBase* make_binary_ivf(int d, const b200vs_params& p) { return new BinaryIvfIndex(d, p); }
+
+static BinaryIvfIndex* as_binary_ivf(IndexBase* ix) {
+  auto* p = dynamic_cast<BinaryIvfIndex*>(ix);
+  if (!p) fail(B200VS_EINTERNAL, "not a BINARY_IVF_FLAT index");
+  return p;
+}
+
+void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, int k, std::vector<uint8_t>& cent) {
+  BinaryIvfIndex* b = as_binary_ivf(ix);
+  std::unique_lock<std::shared_mutex> wl(b->rw);
+  std::lock_guard<std::mutex> gl(b->gpu_mu);
+  b->set_device();
+  b->quiesce();
+  b->scratch.reset(b->stream);
+  b->kmeans_locked(n, x, nullptr, k, cent);
+}
+
+void binary_ivf_train_state(IndexBase* ix, const std::vector<uint8_t>& cent, std::vector<unsigned char>& blob) {
+  const BinaryIvfIndex* b = as_binary_ivf(ix);
+  blob.resize(32 + cent.size());
+  b->state_header(blob.data(), (int)(cent.size() / b->nb));
+  memcpy(blob.data() + 32, cent.data(), cent.size());
+}
 
 }  // namespace b200vs

@@ -331,7 +331,8 @@ struct FlatIndex : IndexBase {
   }
 
   // the device-pointer form of add: the rows stay on the device, the caller's host copy of the ids feeds the id map
-  void add_rows_dev(int64_t n, const float* x_dev, const long long* ids_dev, const int64_t* ids_host) override {
+  void add_rows_dev(int64_t n, const void* xv, const long long* ids_dev, const int64_t* ids_host) override {
+    const float* x_dev = static_cast<const float*>(xv);
     check_batch_ids_unique(n, ids_host);
     std::unique_lock<std::shared_mutex> wl(rw);
     std::lock_guard<std::mutex> gl(gpu_mu);
@@ -592,13 +593,13 @@ struct IvfFlatIndex : IndexBase {
   }
 
   void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override;
-  void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override;
+  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override;
   void add_locked(int64_t n, float* st, const long long* st_ids, const int64_t* h_ids_in, const long long* lists_dev, bool upsert, bool prepared);
   void reserve_lists(const int64_t* rows_per_list, int n_lists) override;
   int nlist_now() const override { return nlist; }
-  void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) override {
+  void assign_lists_dev(int64_t n, const void* x_dev, long long* out_lists_dev, cudaStream_t s) override {
     if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-    assign_dev(x_dev, n, out_lists_dev, s);
+    assign_dev(static_cast<const float*>(x_dev), n, out_lists_dev, s);
   }
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
   int64_t remove(int64_t n, const int64_t* del) override;
@@ -609,10 +610,11 @@ struct IvfFlatIndex : IndexBase {
   }
 
   void search(const SearchReq& r, cudaStream_t s) override;
-  void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+  void coarse(int64_t nq, const void* xv, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
               cudaStream_t s) override {
     if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
     if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
+    const float* xq = static_cast<const float*>(xv);
     coarse_rows(nq, prepared ? xq : prepare_queries(nq, xq, s), nprobe, c0, c1, true, out_score, out_lists, s);
   }
 
@@ -718,7 +720,8 @@ void IvfFlatIndex::add(int64_t n, const float* x, const int64_t* in_ids, bool up
   add_locked(n, st, st_ids, in_ids, nullptr, upsert, loading);
 }
 
-void IvfFlatIndex::add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
+void IvfFlatIndex::add_dev(int64_t n, const void* xv, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
+  const float* x_dev = static_cast<const float*>(xv);
   std::unique_lock<std::shared_mutex> wl(rw);
   if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
   std::lock_guard<std::mutex> gl(gpu_mu);

@@ -295,17 +295,19 @@ struct IndexBase {
   // THE read of an index, on stream s with the lane's scratch already reset: r's top-k or range search.  Each type refuses
   // the requests it cannot serve (a probe table without inverted lists, range on HNSW).
   virtual void search(const SearchReq& r, cudaStream_t s) = 0;
-  // the coarse quantiser of the IVF types over centroid rows [c0, c1): out_lists [nq, nprobe] global list ids (set
-  // semantics), and when out_score is set the ascending ranking score of each (L2 distance | -ip) in (score, list id) order
-  virtual void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+  // the coarse quantiser of the IVF types over centroid rows [c0, c1) (xq: query rows in the index's row format, FP32 or
+  // packed bits): out_lists [nq, nprobe] global list ids (set semantics), and when out_score is set the ascending ranking
+  // score of each (L2 distance | -ip | Hamming distance) in (score, list id) order
+  virtual void coarse(int64_t nq, const void* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
                       cudaStream_t s) {
     (void)nq; (void)xq; (void)prepared; (void)nprobe; (void)c0; (void)c1; (void)out_score; (void)out_lists; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
   }
-  // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT and IVF_PQ ----
+  // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT, IVF_PQ and
+  // BINARY_IVF_FLAT.  Row pointers are in the index's row format: FP32 rows, or packed bits (dim / 8 bytes) on a binary index.
   // rows / ids already on this device.  lists_dev (nullable) = the inverted list of every row, decided by the caller;
   // prepared = store the rows exactly as given (cosine rows are already normalised).
-  virtual void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
+  virtual void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
     (void)n; (void)x_dev; (void)ids_dev; (void)lists_dev; (void)upsert; (void)prepared;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
   }
@@ -315,13 +317,14 @@ struct IndexBase {
     (void)n; (void)codes_dev; (void)ids_dev; (void)lists_dev;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "appending encoded rows only exists for IVF_PQ");
   }
-  // ---- building blocks of a row-sharded deployment (shard.cu); FLAT and HNSW ----
+  // ---- building blocks of a row-sharded deployment (shard.cu); FLAT, BINARY_FLAT and HNSW ----
   // the refusals add (batched: b200vs_hnsw_add_batched with `batch`) would give n rows with these host ids, decided before
   // anything changes, so that every rank of a collective add can agree on one status first
   virtual void check_add(int64_t n, const int64_t* ids, bool batched, int batch) { (void)n; (void)ids; (void)batched; (void)batch; }
-  // FLAT: add's semantics on rows and ids already on this device; ids_host = the same ids on the host (the id map needs them,
-  // and the caller already holds them).  Only the row-sharded owner calls it: b200vs_add_with_ids_device still refuses FLAT.
-  virtual void add_rows_dev(int64_t n, const float* x_dev, const long long* ids_dev, const int64_t* ids_host) {
+  // FLAT, BINARY_FLAT: add's semantics on rows (the index's row format) and ids already on this device; ids_host = the same
+  // ids on the host (the id map needs them, and the caller already holds them).  Only the row-sharded owner calls it:
+  // b200vs_add_with_ids_device still refuses FLAT.
+  virtual void add_rows_dev(int64_t n, const void* x_dev, const long long* ids_dev, const int64_t* ids_host) {
     (void)n; (void)x_dev; (void)ids_dev; (void)ids_host;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "device-row add only exists for FLAT");
   }
@@ -329,8 +332,9 @@ struct IndexBase {
   // from the arguments and the index's parameters alone, so that every rank refuses alike before it (HNSW: efsearch outside
   // [0, 1024], as b200vs_search; the walk's shared memory)
   virtual void check_row_search(int k, const b200vs_search_params* sp) const { (void)k; (void)sp; }
-  // nearest-centroid assignment of prepared rows (faiss quantizer->assign): out_lists_dev[n], on stream s (a lane must be held)
-  virtual void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) {
+  // nearest-centroid assignment of prepared rows (faiss quantizer->assign; the index's row format): out_lists_dev[n], on
+  // stream s (a lane must be held)
+  virtual void assign_lists_dev(int64_t n, const void* x_dev, long long* out_lists_dev, cudaStream_t s) {
     (void)n; (void)x_dev; (void)out_lists_dev; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "list assignment only exists for IVF_FLAT and IVF_PQ");
   }
@@ -440,6 +444,11 @@ void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std:
 void ivf_flat_train_state(IndexBase* ix, const std::vector<float>& cent, std::vector<unsigned char>& blob);
 IndexBase* make_binary_flat(int d, const b200vs_params& p);
 IndexBase* make_binary_ivf(int d, const b200vs_params& p);
+// The same two stages for BINARY_IVF_FLAT (binary.cu); ix must be a BINARY_IVF_FLAT index, whose lists and trained state stay
+// untouched.  Coarse: b200vs_train_binary's k packed centroids [k, dim / 8] of n >= k host packed rows.  State: the
+// trained-state blob of the packed centroids cent [nlist, dim / 8].
+void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, int k, std::vector<uint8_t>& cent);
+void binary_ivf_train_state(IndexBase* ix, const std::vector<uint8_t>& cent, std::vector<unsigned char>& blob);
 
 // ---- generic exact scan + select driver (scan_kernels.cuh) ----
 struct ScanJob {

@@ -722,7 +722,7 @@ struct IvfPqIndex : IndexBase {
 
   // b200vs_add_with_ids_device: the host add's steps on device rows (upsert removes first; cosine rows are normalised on
   // a copy unless `prepared`; lists_dev NULL = nearest centroid), so codes, ids and list layout equal a host add's
-  void add_dev(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override {
+  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override {
     std::unique_lock<std::shared_mutex> wl(rw);
     require_lists();
     const int wpb = encode_warps();
@@ -730,7 +730,7 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     scratch.reset(stream);
-    add_dev_locked(n, x_dev, ids_dev, lists_dev, upsert, prepared, wpb);
+    add_dev_locked(n, static_cast<const float*>(x_dev), ids_dev, lists_dev, upsert, prepared, wpb);
   }
   // add_dev's steps with rw and gpu_mu held and the scratch reset; wpb = encode_warps()
   void add_dev_locked(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared, int wpb) {
@@ -775,9 +775,9 @@ struct IvfPqIndex : IndexBase {
   }
 
   // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
-  void assign_lists_dev(int64_t n, const float* x_dev, long long* out_lists_dev, cudaStream_t s) override {
+  void assign_lists_dev(int64_t n, const void* x_dev, long long* out_lists_dev, cudaStream_t s) override {
     require_lists();
-    assign_dev(centroids.p, nlist, cent_ids.p, x_dev, dim, metric == B200VS_L2, n, out_lists_dev, s);
+    assign_dev(centroids.p, nlist, cent_ids.p, static_cast<const float*>(x_dev), dim, metric == B200VS_L2, n, out_lists_dev, s);
   }
 
   void reserve_lists(const int64_t* rows_per_list, int n_lists) override {
@@ -902,10 +902,11 @@ struct IvfPqIndex : IndexBase {
   // ---- list-sharded building blocks (include/b200vs.h), in the IVF-PQ mode only ----
   int nlist_now() const override { return nlist; }
   int resolve_nprobe_api(const SearchCtx& sc) const override { return resolve_nprobe(sc); }
-  void coarse(int64_t nq, const float* xq, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
+  void coarse(int64_t nq, const void* xv, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
               cudaStream_t s) override {
     require_lists();
     if (c0 < 0 || c1 > nlist || c0 >= c1 || nprobe <= 0 || nprobe > c1 - c0) fail(B200VS_EILLEGAL_PARAMETERS, "bad centroid range / nprobe");
+    const float* xq = static_cast<const float*>(xv);
     coarse_rows(nq, prepared ? xq : prepare_queries(nq, xq, s), nprobe, c0, c1, out_score, out_lists, s);
     if (out_score && metric != B200VS_L2) launch_negate(out_score, nq * nprobe, s);  // -> ascending ranking score
   }

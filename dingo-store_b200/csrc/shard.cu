@@ -11,6 +11,9 @@
 //      kernel — the engine's analogue of VectorIndexWrapper::MergeSearchResults (src/vector/vector_index.cc:1056-1108).
 // FLAT and HNSW shard by row instead (DESIGN.md 4.5): row id lives on rank row_owner_of(id), each rank holds a standalone
 // index of its rows, and a search skips step 1 and runs the whole batch on the rank's index before the same all-gather + merge.
+// The binary types take the same two routes through the b200vs_shard_*_binary entry points: BINARY_IVF_FLAT by list (Hamming
+// coarse pass, binary list scan), BINARY_FLAT by row.  Rows and queries then travel as packed bits, dim / 8 bytes each, and
+// the merge key is the Hamming distance itself.
 // Both kinds share one write path: b200vs_shard_add* partitions the rows by owner on the device (list-sharded: the owner of
 // the list the sender assigns the row to), moves them with one grouped ncclSend/ncclRecv, and every rank returns the first
 // refusal in rank order or adds.  A world of one runs the same code with only the NCCL calls left out.
@@ -160,14 +163,15 @@ static __global__ void unpack_parts_kernel(const TopkRec* __restrict__ parts, lo
   d[i] = r.dist; id[i] = r.id;
 }
 
-// merged range results: key (L2 distance | -ip) -> API distance (L2 distance | 1 - ip, as the single-index finish computes it);
-// counts[q] = merged rows of query q (the rows are ascending with -1 padding at the end)
-static __global__ void range_finish_kernel(float* dist, const long long* __restrict__ ids, long long nq, int k, int l2, int* counts) {
+// merged range results: key (L2 distance | -ip | Hamming distance) -> API distance (L2 distance | 1 - ip | Hamming distance,
+// as the single-index finish computes it; ip = 1: the IP / cosine key); counts[q] = merged rows of query q (the rows are
+// ascending with -1 padding at the end)
+static __global__ void range_finish_kernel(float* dist, const long long* __restrict__ ids, long long nq, int k, int ip, int* counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nq * k) return;
   const int j = (int)(i % k);
   const bool hit = ids[i] >= 0;
-  if (hit && !l2) dist[i] = __fsub_rn(1.0f, -dist[i]);
+  if (hit && ip) dist[i] = __fsub_rn(1.0f, -dist[i]);
   if (hit ? (j == k - 1 || ids[i + 1] < 0) : j == 0) counts[i / k] = hit ? j + 1 : 0;
 }
 
@@ -364,13 +368,13 @@ using namespace b200vs;
 struct b200vs_shard {
   IndexBase* ix = nullptr;
   int rank = 0, world = 1, nlanes = 1;
-  bool rows = false;  // sharded by rows (FLAT, HNSW: owner(id) = row_owner_of), else by inverted list (IVF_FLAT, IVF_PQ)
+  bool rows = false;  // sharded by rows (shard_by_rows: owner(id) = row_owner_of), else by inverted list (shard_by_lists)
   struct SLane {
     ncclComm_t comm = nullptr;
     std::mutex mu;
     DevBuf<long long> probes;   // [per * world, nprobe]
     DevBuf<TopkRec> parts;      // [world, nq, k]
-    DevBuf<float> q_all;        // host-pointer variant: [per * world, d]
+    DevBuf<unsigned char> q_all;  // host-pointer variant: [per * world] query rows of query_row_bytes()
     DevBuf<float> od;           // local / merged results
     DevBuf<long long> oi;
     cudaStream_t own = nullptr;
@@ -402,9 +406,19 @@ struct b200vs_shard {
 
 namespace {
 
+// The two ways an index type is sharded, each decided here only: by row (owner(id) = row_owner_of) or by inverted list
+bool shard_by_rows(b200vs_type t) { return t == B200VS_FLAT || t == B200VS_HNSW || t == B200VS_BINARY_FLAT; }
+bool shard_by_lists(b200vs_type t) { return t == B200VS_IVF_FLAT || t == B200VS_IVF_PQ || t == B200VS_BINARY_IVF_FLAT; }
+
 b200vs_shard* get(b200vs_shard* s) {
   if (!s || !s->ix) fail(B200VS_EILLEGAL_PARAMETERS, "null shard handle");
   return s;
+}
+
+// the float data calls on a binary shard, and the b200vs_shard_*_binary ones on a float shard
+void check_row_type(const b200vs_shard* sh, bool binary_call) {
+  if (sh->ix->binary() != binary_call)
+    fail(B200VS_EILLEGAL_PARAMETERS, binary_call ? "binary entry point on a float shard" : "float entry point on a binary shard");
 }
 
 // Take the turn of batch `seq` (seq < 0: the next one in call order).  Batches are ENQUEUED strictly in sequence order on
@@ -477,27 +491,29 @@ void check(const Status& st) {
 // on stream s.  local(r) is step 2: r is this rank's search of k results per query into L.od / L.oi, which local completes
 // and runs, so that they hold ascending, -1-padded [nq, k] (key, id) lists, the key being what the merge orders by.
 // List-sharded: r searches the prepared queries over the gathered probe table L.probes.  Row-sharded: there is no coarse
-// step, and r searches the raw queries (the rank's index prepares them).
+// step, and r searches the raw queries (the rank's index prepares them).  Queries are rows of query_row_bytes(): FP32, or
+// packed bits on a binary index.
 template <class LocalScan>
-void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
+void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
                   float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local) {
   IndexBase* ix = sh->ix;
-  const int W = sh->world, r = sh->rank, d = ix->dim;
+  const int W = sh->world, r = sh->rank;
+  const size_t qb = ix->query_row_bytes();
   if (L.last && L.last != s && L.done) B200VS_CUDA(cudaStreamWaitEvent(s, L.done, 0));
   SearchCtx sc = make_ctx(ix, sp, s);
-  const float* q = xq;
+  const void* q = xq;
   int nprobe = 0;
   if (!sh->rows) {
     nprobe = ix->resolve_nprobe_api(sc);
     const int64_t per = (nq + W - 1) / W;
     // cosine: normalise once (NormalizeVectorForFaiss), the coarse pass and the list scan both take prepared queries
-    q = ix->prepare_queries(nq, xq, s);
+    if (!ix->binary()) q = ix->prepare_queries(nq, static_cast<const float*>(xq), s);
     // 1) coarse quantiser on this rank's slice, all-gather of the probe table (in place)
     L.probes.reserve((size_t)per * W * nprobe, 0, s);
     const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
     long long* mine = L.probes.p + (size_t)per * r * nprobe;
     if (q1 - q0 < per) fill_ll_kernel<<<(unsigned)cdiv(per * nprobe, 256), 256, 0, s>>>(mine, per * nprobe, -1);
-    if (q1 > q0) ix->coarse(q1 - q0, q + (size_t)q0 * d, true, nprobe, 0, ix->nlist_now(), nullptr, mine, s);
+    if (q1 > q0) ix->coarse(q1 - q0, static_cast<const unsigned char*>(q) + (size_t)q0 * qb, true, nprobe, 0, ix->nlist_now(), nullptr, mine, s);
     ix->phase(IndexBase::PH_COMM, s);
     if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.probes.p, (size_t)per * nprobe, ncclInt64, L.comm, s));
     ix->phase(IndexBase::PH_OTHER, s);
@@ -536,8 +552,9 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const fl
 // top-k.  List-sharded: the tile scan's exact local top-k, keyed on the API distance.  Row-sharded FLAT: the rank's search
 // keyed on the single-index select's key (L2 distance | -ip; two distinct inner products can round to the same 1 - ip, and
 // an API-distance merge would then choose and order them by id), the API distance formed after the merge.  Row-sharded
-// HNSW: the rank's graph walk, keyed on the distance the walk itself ranks by (hnsw_distance: L2 distance | 1 - ip).
-void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, int k, const b200vs_search_params* sp,
+// HNSW: the rank's graph walk, keyed on the distance the walk itself ranks by (hnsw_distance: L2 distance | 1 - ip).  Binary
+// types: the rank's search keyed on the Hamming distance, which is also the API distance.
+void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
                          float* out_dist, long long* out_ids, cudaStream_t s) {
   IndexBase* ix = sh->ix;
   const bool flat_ip = sh->rows && ix->type == B200VS_FLAT && ix->ip_like();
@@ -556,21 +573,22 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
 
 // range: the local range scan keyed on the single-index select's key (L2 distance | -ip) — two distinct inner products can
 // round to the same 1 - ip, and an API-distance merge would then order them by id — then the API distance and the count of
-// every merged row.  The per-rank payload of the all-gather is nq * max_results * 16 bytes.
-void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, float radius, int max_results,
+// every merged row.  Binary types: the rank's b200vs_range_search_binary rule keyed on the Hamming distance (a NaN radius
+// is refused before the read starts).  The per-rank payload of the all-gather is nq * max_results * 16 bytes.
+void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, float radius, int max_results,
                         const b200vs_search_params* sp, float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
   IndexBase* ix = sh->ix;
-  const bool l2 = ix->metric == B200VS_L2;
+  const bool ip = ix->ip_like();
   shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](SearchReq& r) {
     r.range = true; r.radius = radius; r.raw = true;
     r.oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
     // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
     if (std::isnan(radius)) fill_empty(r, s);
     else ix->search(r, s);
-    if (!l2) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
+    if (ip) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
   });
   const long long n = (long long)nq * max_results;
-  range_finish_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(out_dist, out_ids, nq, max_results, l2 ? 1 : 0, out_counts);
+  range_finish_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(out_dist, out_ids, nq, max_results, ip ? 1 : 0, out_counts);
   B200VS_CUDA(cudaGetLastError());
   ix->launch_count(1);
   ix->phases_finish(s);
@@ -584,11 +602,13 @@ bool check_shard_topk(int64_t nq, const void* xq, int k, const void* od, const v
   if (!od || !oi) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
   return true;
 }
-bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, int max_results, const void* od, const void* oi, const void* oc) {
+bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, float radius, int max_results, const void* od, const void* oi,
+                       const void* oc) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
   if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // as b200vs_range_search
   if (max_results <= 0 || max_results > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
   if (!od || !oi || !oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
+  if (ix->binary() && std::isnan(radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");  // as b200vs_range_search_binary
   return true;
 }
 
@@ -617,16 +637,19 @@ void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, 
 }
 
 // The host-pointer reads: every rank passes the SAME batch; each rank uploads only its slice and the slices are all-gathered
-// over NVLink, so the PCIe traffic per rank does not grow with the world size.  Returns the batch on the device.
-const float* upload_batch(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const float* xq, cudaStream_t s) {
-  const int W = sh->world, r = sh->rank, d = sh->ix->dim;
+// over NVLink, so the PCIe traffic per rank does not grow with the world size.  Returns the batch on the device.  Query rows
+// are query_row_bytes() each (FP32, or packed bits on a binary index) and travel as bytes.
+const void* upload_batch(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, cudaStream_t s) {
+  const int W = sh->world, r = sh->rank;
+  const size_t qb = sh->ix->query_row_bytes();
   const int64_t per = (nq + W - 1) / W;
-  L.q_all.reserve((size_t)per * W * d, 0, s);
+  L.q_all.reserve((size_t)per * W * qb, 0, s);
   const int64_t q0 = std::min<int64_t>(nq, per * r), q1 = std::min<int64_t>(nq, per * (r + 1));
-  float* mine = L.q_all.p + (size_t)per * r * d;
-  if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, xq + (size_t)q0 * d, (size_t)(q1 - q0) * d * 4, cudaMemcpyHostToDevice, s));
-  if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * d, 0, (size_t)(per - (q1 - q0)) * d * 4, s));
-  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * d, ncclFloat, L.comm, s));
+  unsigned char* mine = L.q_all.p + (size_t)per * r * qb;
+  const unsigned char* src = static_cast<const unsigned char*>(xq);
+  if (q1 > q0) B200VS_CUDA(cudaMemcpyAsync(mine, src + (size_t)q0 * qb, (size_t)(q1 - q0) * qb, cudaMemcpyHostToDevice, s));
+  if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * qb, 0, (size_t)(per - (q1 - q0)) * qb, s));
+  if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * qb, ncclUint8, L.comm, s));
   return L.q_all.p;
 }
 
@@ -653,12 +676,13 @@ void broadcast_state_locked(b200vs_shard* sh, int root) {
   }
 }
 
-// b200vs_shard_train on IVF_FLAT and IVF_PQ.  The per-rank row counts are exchanged first, so that a refusal for too few
-// rows happens on every rank at once.  Coarse stage: each rank clusters its rows into nlist / world centroids with the k-means
-// of its type's own train, one all-gather.  IVF_FLAT: every rank installs the gathered centroids.  IVF_PQ: rank 0 trains the
-// codebooks with train's PQ rule on the residuals of its rows to the global centroids, and the state broadcast replicates
-// the result.  At world = 1 this is b200vs_train step for step, so the trained state is byte-equal.
-void shard_train_locked(b200vs_shard* sh, int64_t n, const float* x) {
+// b200vs_shard_train on IVF_FLAT and IVF_PQ, b200vs_shard_train_binary on BINARY_IVF_FLAT (x: packed rows).  The per-rank row
+// counts are exchanged first, so that a refusal for too few rows happens on every rank at once.  Coarse stage: each rank
+// clusters its rows into nlist / world centroids with the k-means of its type's own train, one all-gather.  IVF_FLAT and
+// BINARY_IVF_FLAT: every rank installs the gathered centroids.  IVF_PQ: rank 0 trains the codebooks with train's PQ rule on
+// the residuals of its rows to the global centroids, and the state broadcast replicates the result.  At world = 1 this is
+// b200vs_train[_binary] step for step, so the trained state is byte-equal.
+void shard_train_locked(b200vs_shard* sh, int64_t n, const void* xv) {
   IndexBase* ix = sh->ix;
   const bool pq = ix->type == B200VS_IVF_PQ;
   const int W = sh->world, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
@@ -666,18 +690,26 @@ void shard_train_locked(b200vs_shard* sh, int64_t n, const float* x) {
   if (pq && ix->sub_type() == B200VS_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode has no inverted lists to shard");
   const int nl = nlist / W;
   ix->set_device();
-  const long long rows = x ? (long long)n : 0;  // a null x counts as none
+  const long long rows = xv ? (long long)n : 0;  // a null x counts as none
   const std::vector<long long> counts = all_gather_host(sh, &rows);
   for (int r = 0; r < W; ++r)
     if (counts[r] < nl)
       fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank " + std::to_string(r) + " has fewer training rows than nlist / world centroids");
   if (pq && counts[0] < 256LL * ivf_pq_ksub(ix))
     fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank 0 needs 256 * 2^nbits training rows for the PQ codebooks");
+  std::vector<unsigned char> blob;
+  if (ix->binary()) {
+    std::vector<uint8_t> local;
+    binary_ivf_train_coarse(ix, n, static_cast<const uint8_t*>(xv), nl, local);
+    binary_ivf_train_state(ix, all_gather_host(sh, local.data(), local.size()), blob);
+    ix->set_state(blob.data(), blob.size());
+    return;
+  }
+  const float* x = static_cast<const float*>(xv);
   std::vector<float> local;
   if (pq) ivf_pq_train_coarse(ix, n, x, nl, local);
   else ivf_flat_train_coarse(ix, n, x, nl, local);
   const std::vector<float> cent = all_gather_host(sh, local.data(), local.size());
-  std::vector<unsigned char> blob;
   if (!pq) {
     ivf_flat_train_state(ix, cent, blob);
     ix->set_state(blob.data(), blob.size());
@@ -690,30 +722,17 @@ void shard_train_locked(b200vs_shard* sh, int64_t n, const float* x) {
   broadcast_state_locked(sh, 0);
 }
 
-}  // namespace
-
-extern "C" {
-
-int b200vs_shard_unique_id(uint8_t id[B200VS_SHARD_ID_BYTES]) {
-  return guarded([&]() -> int {
-    if (!id) fail(B200VS_EILLEGAL_PARAMETERS, "null id");
-    static_assert(sizeof(ncclUniqueId) <= B200VS_SHARD_ID_BYTES, "ncclUniqueId must fit the ABI's id blob");
-    ncclUniqueId u;
-    B200VS_NCCL(nccl().GetUniqueId(&u));
-    memset(id, 0, B200VS_SHARD_ID_BYTES);
-    memcpy(id, &u, sizeof(u));
-    return B200VS_OK;
-  });
-}
-
-int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const uint8_t id[B200VS_SHARD_ID_BYTES], int32_t lanes, b200vs_shard** out) {
+// b200vs_shard_create (float indexes) and b200vs_shard_create_binary (binary ones)
+int shard_create(b200vs_index* idx, int32_t rank, int32_t world, const uint8_t* id, int32_t lanes, b200vs_shard** out, bool binary_call) {
   return guarded([&]() -> int {
     if (!out) fail(B200VS_EILLEGAL_PARAMETERS, "out is null");
     *out = nullptr;
     IndexBase* ix = index_impl(idx);
-    const bool rows = ix->type == B200VS_FLAT || ix->type == B200VS_HNSW;
-    if (!rows && ix->type != B200VS_IVF_FLAT && ix->type != B200VS_IVF_PQ)
-      fail(B200VS_EVECTOR_NOT_SUPPORT, "sharding is implemented for FLAT and HNSW (by rows), IVF_FLAT and IVF_PQ (by list)");
+    if (binary_call && !ix->binary()) fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
+    if (!binary_call && ix->binary())
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "sharding is implemented for FLAT and HNSW (by rows), IVF_FLAT and IVF_PQ (by list); binary indexes "
+                                       "shard through b200vs_shard_create_binary");
+    const bool rows = shard_by_rows(ix->type);  // else shard_by_lists
     if (ix->type == B200VS_IVF_PQ && ix->sub_type() == B200VS_FLAT)
       fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode (too few training rows) has no inverted lists to shard");
     if (rows && ix->count() + ix->deleted_count() > 0)
@@ -741,6 +760,44 @@ int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const ui
   });
 }
 
+// Distributed training: every rank clusters ITS training rows into nlist / world centroids (faiss::Clustering shape, as
+// b200vs_train), the blocks are all-gathered into the replicated global table.  Build time stays flat as ranks are added.
+int shard_train(b200vs_shard* h, int64_t n, const void* x, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    check_row_type(sh, binary_call);
+    if (sh->rows) return B200VS_OK;  // FLAT, BINARY_FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    shard_train_locked(sh, n, x);
+    return B200VS_OK;
+  });
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200vs_shard_unique_id(uint8_t id[B200VS_SHARD_ID_BYTES]) {
+  return guarded([&]() -> int {
+    if (!id) fail(B200VS_EILLEGAL_PARAMETERS, "null id");
+    static_assert(sizeof(ncclUniqueId) <= B200VS_SHARD_ID_BYTES, "ncclUniqueId must fit the ABI's id blob");
+    ncclUniqueId u;
+    B200VS_NCCL(nccl().GetUniqueId(&u));
+    memset(id, 0, B200VS_SHARD_ID_BYTES);
+    memcpy(id, &u, sizeof(u));
+    return B200VS_OK;
+  });
+}
+
+int b200vs_shard_create(b200vs_index* idx, int32_t rank, int32_t world, const uint8_t id[B200VS_SHARD_ID_BYTES], int32_t lanes, b200vs_shard** out) {
+  return shard_create(idx, rank, world, id, lanes, out, false);
+}
+
+int b200vs_shard_create_binary(b200vs_index* idx, int32_t rank, int32_t world, const uint8_t id[B200VS_SHARD_ID_BYTES], int32_t lanes,
+                               b200vs_shard** out) {
+  return shard_create(idx, rank, world, id, lanes, out, true);
+}
+
 void b200vs_shard_destroy(b200vs_shard* sh) {
   try { delete sh; } catch (...) {}
 }
@@ -757,17 +814,8 @@ int b200vs_shard_list_range(b200vs_shard* h, int32_t rank, int32_t* begin, int32
   });
 }
 
-// Distributed training: every rank clusters ITS training rows into nlist / world centroids (faiss::Clustering shape, as
-// b200vs_train), the blocks are all-gathered into the replicated global table.  Build time stays flat as ranks are added.
-int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    if (sh->rows) return B200VS_OK;  // FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
-    std::lock_guard<std::mutex> g(sh->add_mu);
-    shard_train_locked(sh, n, x);
-    return B200VS_OK;
-  });
-}
+int b200vs_shard_train(b200vs_shard* h, int64_t n, const float* x) { return shard_train(h, n, x, false); }
+int b200vs_shard_train_binary(b200vs_shard* h, int64_t n, const uint8_t* x) { return shard_train(h, n, x, true); }
 
 // Replicate rank `root`'s trained state (centroids; IVF-PQ: and codebooks) on every rank.
 int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
@@ -786,12 +834,12 @@ int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
 
 namespace {
 
-// assignment of n device rows (raw) -> prepared rows (cosine: normalised copy) + lists, on the write stream.
-// Returns the prepared rows (either x itself or `prep`).
-const float* assign_rows(b200vs_shard* sh, int64_t n, const float* x_dev, DevBuf<float>& prep, DevBuf<long long>& lists) {
+// assignment of n device rows (raw, in the index's row format) -> prepared rows (cosine: normalised copy) + lists, on the
+// write stream.  Returns the prepared rows (either x itself or `prep`).
+const void* assign_rows(b200vs_shard* sh, int64_t n, const void* x_dev, DevBuf<float>& prep, DevBuf<long long>& lists) {
   IndexBase* ix = sh->ix;
   cudaStream_t s = sh->ws;
-  const float* xp = x_dev;
+  const void* xp = x_dev;
   if (ix->metric == B200VS_COSINE) {
     prep.reserve((size_t)n * ix->dim, 0, s);
     B200VS_CUDA(cudaMemcpyAsync(prep.p, x_dev, (size_t)n * ix->dim * 4, cudaMemcpyDeviceToDevice, s));
@@ -814,7 +862,6 @@ struct Routed {
   DevBuf<unsigned char> x;
   DevBuf<long long> ids, lists;
   long long n = 0;
-  const float* rows() const { return reinterpret_cast<const float*>(x.p); }
 };
 template <class Owner>
 void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long long* ids, const long long* lists, Owner owner, Routed& out) {
@@ -883,20 +930,21 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
 // normalises), and the owner runs the single-index add on the rows it received, in arrival order (an HNSW graph depends on
 // it).  Before any rank changes anything, every owner checks its rows (check_add: a repeated id for FLAT, max_elements for
 // HNSW, nothing for the list types) and the statuses are all-gathered: every rank returns the first refusal in rank order,
-// or adds.  batched: b200vs_hnsw_add_batched with `batch`.
-void shard_add_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long long* ids_dev, bool batched, int batch) {
+// or adds.  batched: b200vs_hnsw_add_batched with `batch`.  Rows are in the index's row format (FP32, or packed bits on the
+// binary types, which travel as they are: a binary row has no normalisation).
+void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long long* ids_dev, bool batched, int batch) {
   IndexBase* ix = sh->ix;
-  const int d = ix->dim;
+  const int d = ix->dim, rb = (int)ix->query_row_bytes();
   cudaStream_t s = sh->ws;
   ix->set_device();
   Routed rv;
   if (sh->rows) {
-    route_rows(sh, n, x_dev, d * 4, ids_dev, nullptr, RowOwner{}, rv);
+    route_rows(sh, n, x_dev, rb, ids_dev, nullptr, RowOwner{}, rv);
   } else {
     DevBuf<float> prep;
     DevBuf<long long> lists;
-    const float* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
-    route_rows(sh, n, xp, d * 4, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
+    const void* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
+    route_rows(sh, n, xp, rb, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
   }
   std::vector<int64_t> hid(sh->rows ? (size_t)rv.n : 0);  // the host ids check_add and the FLAT / HNSW adds take
   if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
@@ -905,9 +953,9 @@ void shard_add_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long 
   check(agree(sh, attempt([&] { ix->check_add(rv.n, hid.data(), batched, batch); }), "shard add"));
   if (!rv.n) return;
   if (!sh->rows) {
-    ix->add_dev(rv.n, rv.rows(), rv.ids.p, rv.lists.p, false, true);
-  } else if (ix->type == B200VS_FLAT) {
-    ix->add_rows_dev(rv.n, rv.rows(), rv.ids.p, hid.data());
+    ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
+  } else if (ix->type != B200VS_HNSW) {  // FLAT, BINARY_FLAT
+    ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data());
   } else {
     std::vector<float> hx((size_t)rv.n * d);  // the HNSW builders take host rows
     B200VS_CUDA(cudaMemcpyAsync(hx.data(), rv.x.p, (size_t)rv.n * d * 4, cudaMemcpyDeviceToHost, s));
@@ -917,11 +965,12 @@ void shard_add_impl(b200vs_shard* sh, int64_t n, const float* x_dev, const long 
   }
 }
 
-// upload of host rows to the write stream, for the host-pointer variants of the collective adds
-void upload_rows(b200vs_shard* sh, int64_t n, const float* x, const int64_t* ids, DevBuf<float>& dx, DevBuf<long long>& di) {
+// upload of host rows (query_row_bytes() each) to the write stream, for the host-pointer variants of the collective adds
+void upload_rows(b200vs_shard* sh, int64_t n, const void* x, const int64_t* ids, DevBuf<unsigned char>& dx, DevBuf<long long>& di) {
   if (!n) return;
-  dx.reserve((size_t)n * sh->ix->dim, 0, sh->ws); di.reserve((size_t)n, 0, sh->ws);
-  B200VS_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n * sh->ix->dim * 4, cudaMemcpyHostToDevice, sh->ws));
+  const size_t rb = sh->ix->query_row_bytes();
+  dx.reserve((size_t)n * rb, 0, sh->ws); di.reserve((size_t)n, 0, sh->ws);
+  B200VS_CUDA(cudaMemcpyAsync(dx.p, x, (size_t)n * rb, cudaMemcpyHostToDevice, sh->ws));
   B200VS_CUDA(cudaMemcpyAsync(di.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, sh->ws));
   B200VS_CUDA(cudaStreamSynchronize(sh->ws));
 }
@@ -1054,7 +1103,7 @@ ManifestHdr manifest_of(const IndexBase* ix, int W) {
   m.version = kManifestVersion;
   m.type = ix->type; m.metric = ix->metric; m.dim = ix->dim; m.world = W;
   const b200vs_params& p = ix->params;
-  if (ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ) m.nlist = p.nlist > 0 ? p.nlist : 2048;
+  if (shard_by_lists(ix->type)) m.nlist = p.nlist > 0 ? p.nlist : 2048;
   if (ix->type == B200VS_IVF_PQ) { m.pq_m = p.pq_m > 0 ? p.pq_m : 64; m.pq_nbits = p.pq_nbits > 0 ? p.pq_nbits : 8; }
   if (ix->type == B200VS_HNSW) { m.hnsw_m = p.hnsw_m; m.hnsw_efc = p.hnsw_efc; m.max_elements = p.max_elements; }
   return m;
@@ -1139,15 +1188,16 @@ void shard_save_locked(b200vs_shard* sh, const std::string& prefix) {
 struct RankFile {
   std::string path;
   int64_t rows = 0, rows_at = 0;  // rows stored, and the file offset of the row section
-  int rb = 0;                     // bytes per stored row: FP32 row or IVF-PQ code row
+  int rb = 0;                     // bytes per stored row: FP32 row, packed binary row or IVF-PQ code row
   std::vector<unsigned char> state;
   std::vector<int64_t> off, ids;  // list offsets [nlist + 1], ids [rows]
   int nlist() const { return (int)off.size() - 1; }
 };
 
-// bytes of one stored row of a rank file: an FP32 row, or an IVF-PQ code row of ceil(M * nbits / 8) bytes
+// bytes of one stored row of a rank file: an FP32 row, a packed binary row of dim / 8 bytes, or an IVF-PQ code row of
+// ceil(M * nbits / 8) bytes
 int restore_row_bytes(const IndexBase* ix, const ManifestHdr& mh) {
-  return ix->type == B200VS_IVF_PQ ? (mh.pq_m * mh.pq_nbits + 7) / 8 : ix->dim * 4;
+  return ix->type == B200VS_IVF_PQ ? (mh.pq_m * mh.pq_nbits + 7) / 8 : (int)ix->query_row_bytes();
 }
 
 // Reads and checks one rank file.  full = false: the header and the trained state only, for a rank that reads no file of
@@ -1175,7 +1225,7 @@ RankFile read_rank_file(IndexBase* ix, const std::string& path, const RankEntry&
     IndexFileHdr h;
     rd(&h, sizeof(h));
     here = sizeof(h);
-    if (memcmp(h.magic, "B2VSIDX1", 8) != 0 || h.type != ix->type || h.metric != ix->metric || h.dim != ix->dim)
+    if (memcmp(h.magic, ix->binary() ? "B2VSBIN1" : "B2VSIDX1", 8) != 0 || h.type != ix->type || h.metric != ix->metric || h.dim != ix->dim)
       fail(B200VS_EINTERNAL, path + ": " + bad);
     nlist = h.nlist; count = h.count; state_len = h.state_len;
   }
@@ -1186,8 +1236,7 @@ RankFile read_rank_file(IndexBase* ix, const std::string& path, const RankEntry&
     fail(B200VS_EINTERNAL, path + ": corrupt snapshot file (header sizes do not match the file)");
   rf.state.resize((size_t)state_len);
   rd(rf.state.data(), rf.state.size());
-  const bool list_sharded = ix->type == B200VS_IVF_FLAT || ix->type == B200VS_IVF_PQ;
-  if (list_sharded && ((int64_t)rf.state.size() != mh.state_len || digest_of(rf.state) != mh.state_digest))
+  if (shard_by_lists(ix->type) && ((int64_t)rf.state.size() != mh.state_len || digest_of(rf.state) != mh.state_digest))
     fail(B200VS_EINTERNAL, path + ": trained state differs from the manifest's");
   if (!full) return rf;
   if (lists) {
@@ -1313,8 +1362,9 @@ void shard_load_locked(b200vs_shard* sh, const std::string& prefix) {
     if (!sh->rows && !state.empty() && !ix->is_trained()) ix->set_state(state.data(), state.size());
   }), "shard load"));
   if (ix->type == B200VS_HNSW || (!sh->rows && mh.state_len == 0)) return;  // no rows to place
-  // 3) list-sharded: every owned list pre-sized from the index-wide list lengths in one arena allocation
-  if (!sh->rows) {
+  // 3) list-sharded: every owned list pre-sized from the index-wide list lengths in one arena allocation (the binary lists
+  //    grow as they are appended: a binary index has no list reservation)
+  if (!sh->rows && !ix->binary()) {
     const int nlist = ix->nlist_now();
     std::vector<unsigned long long> mine((size_t)nlist, 0);
     for (const RankFile& rf : files)
@@ -1362,20 +1412,124 @@ void shard_load_locked(b200vs_shard* sh, const std::string& prefix) {
     B200VS_CUDA(cudaStreamSynchronize(s));  // the pinned buffer and the sent rows are reused next round
     check(agree(sh, attempt([&] {
       if (!rv.n) return;
-      if (ix->type == B200VS_IVF_FLAT) {
-        ix->add_dev(rv.n, rv.rows(), rv.ids.p, rv.lists.p, false, true);
-      } else if (ix->type == B200VS_IVF_PQ) {
+      if (ix->type == B200VS_IVF_PQ) {
         ix->add_codes_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p);
-      } else {
+      } else if (!sh->rows) {  // IVF_FLAT, BINARY_IVF_FLAT
+        ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
+      } else {  // FLAT, BINARY_FLAT
         std::vector<int64_t> hid((size_t)rv.n);
         B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
         B200VS_CUDA(cudaStreamSynchronize(s));
         ix->loading = true;  // rows come back exactly as stored (already normalised for cosine)
-        try { ix->add_rows_dev(rv.n, rv.rows(), rv.ids.p, hid.data()); } catch (...) { ix->loading = false; throw; }
+        try { ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data()); } catch (...) { ix->loading = false; throw; }
         ix->loading = false;
       }
     }), "shard load"));
   }
+}
+
+// b200vs_shard_add[_device] (float rows) and b200vs_shard_add_binary[_device] (packed rows)
+int shard_add(b200vs_shard* h, int64_t n, const void* x, const int64_t* ids, bool on_device, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    check_row_type(sh, binary_call);
+    if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    if (on_device) {
+      shard_add_impl(sh, n, x, (const long long*)ids, false, 0);
+      return B200VS_OK;
+    }
+    sh->ix->set_device();
+    DevBuf<unsigned char> dx;
+    DevBuf<long long> di;
+    upload_rows(sh, n, x, ids, dx, di);
+    shard_add_impl(sh, n, dx.p, di.p, false, 0);
+    return B200VS_OK;
+  });
+}
+
+// b200vs_shard_search_device / b200vs_shard_search_binary_device
+int shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq_dev, int32_t k, const b200vs_search_params* sp,
+                        float* out_dist_dev, int64_t* out_ids_dev, void* stream, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    shard_read(sh, seq, stream, nq, k, sp,
+               [&] {
+                 check_row_type(sh, binary_call);
+                 return check_shard_topk(nq, xq_dev, k, out_dist_dev, out_ids_dev);
+               },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 shard_search_stream(sh, L, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
+               });
+    return B200VS_OK;
+  });
+}
+
+// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).
+int shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
+                 int64_t* out_ids, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    shard_read(sh, seq, nullptr, nq, k, sp,
+               [&] {
+                 check_row_type(sh, binary_call);
+                 return check_shard_topk(nq, xq, k, out_dist, out_ids);
+               },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 IndexBase* ix = sh->ix;
+                 const void* q = upload_batch(sh, L, nq, xq, s);
+                 float* dd = ix->scratch.alloc<float>((size_t)nq * k);
+                 long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
+                 shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
+                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
+               });
+    return B200VS_OK;
+  });
+}
+
+// b200vs_shard_range_search_device / b200vs_shard_range_search_binary_device
+int shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq_dev, float radius, int32_t max_results,
+                              const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, int32_t* out_counts_dev,
+                              void* stream, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    shard_read(sh, seq, stream, nq, max_results, sp,
+               [&] {
+                 check_row_type(sh, binary_call);
+                 return check_shard_range(sh->ix, nq, xq_dev, radius, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
+               },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 shard_range_stream(sh, L, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
+               });
+    return B200VS_OK;
+  });
+}
+
+// Host-pointer variant: as shard_search, each rank uploads only its slice of the batch.
+int shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq, float radius, int32_t max_results,
+                       const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts, bool binary_call) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    shard_read(sh, seq, nullptr, nq, max_results, sp,
+               [&] {
+                 check_row_type(sh, binary_call);
+                 return check_shard_range(sh->ix, nq, xq, radius, max_results, out_dist, out_ids, out_counts);
+               },
+               [&](b200vs_shard::SLane& L, cudaStream_t s) {
+                 IndexBase* ix = sh->ix;
+                 const void* q = upload_batch(sh, L, nq, xq, s);
+                 const size_t nr = (size_t)nq * max_results;
+                 float* dd = ix->scratch.alloc<float>(nr);
+                 long long* di = ix->scratch.alloc<long long>(nr);
+                 int* dc = ix->scratch.alloc<int>((size_t)nq);
+                 shard_range_stream(sh, L, nq, q, radius, max_results, sp, dd, di, dc, s);
+                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
+                 B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
+               });
+    return B200VS_OK;
+  });
 }
 
 }  // namespace
@@ -1385,28 +1539,13 @@ extern "C" {
 // Collective: every rank passes the rows IT holds (any rows; n may differ per rank, 0 allowed); each row is assigned to its
 // nearest centroid and travels to the rank that owns that list (grouped ncclSend / ncclRecv over NVLink).
 int b200vs_shard_add_device(b200vs_shard* h, int64_t n, const float* x_dev, const int64_t* ids_dev) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    if (n < 0 || (n > 0 && (!x_dev || !ids_dev))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
-    std::lock_guard<std::mutex> g(sh->add_mu);
-    shard_add_impl(sh, n, x_dev, (const long long*)ids_dev, false, 0);
-    return B200VS_OK;
-  });
+  return shard_add(h, n, x_dev, ids_dev, true, false);
 }
-
-int b200vs_shard_add(b200vs_shard* h, int64_t n, const float* x, const int64_t* ids) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
-    std::lock_guard<std::mutex> g(sh->add_mu);
-    sh->ix->set_device();
-    DevBuf<float> dx;
-    DevBuf<long long> di;
-    upload_rows(sh, n, x, ids, dx, di);
-    shard_add_impl(sh, n, dx.p, di.p, false, 0);
-    return B200VS_OK;
-  });
+int b200vs_shard_add_binary_device(b200vs_shard* h, int64_t n, const uint8_t* x_dev, const int64_t* ids_dev) {
+  return shard_add(h, n, x_dev, ids_dev, true, true);
 }
+int b200vs_shard_add(b200vs_shard* h, int64_t n, const float* x, const int64_t* ids) { return shard_add(h, n, x, ids, false, false); }
+int b200vs_shard_add_binary(b200vs_shard* h, int64_t n, const uint8_t* x, const int64_t* ids) { return shard_add(h, n, x, ids, false, true); }
 
 // Collective batched HNSW build of a row-sharded HNSW index: shard_add's routing, then b200vs_hnsw_add_batched with `batch`
 // on the rows each rank received, in arrival order.
@@ -1417,7 +1556,7 @@ int b200vs_shard_hnsw_add_batched(b200vs_shard* h, int64_t n, const float* x, co
     if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
     std::lock_guard<std::mutex> g(sh->add_mu);
     sh->ix->set_device();
-    DevBuf<float> dx;
+    DevBuf<unsigned char> dx;
     DevBuf<long long> di;
     upload_rows(sh, n, x, ids, dx, di);
     shard_add_impl(sh, n, dx.p, di.p, true, batch);
@@ -1490,6 +1629,7 @@ int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int6
 int b200vs_shard_plan_add_device(b200vs_shard* h, int64_t n, const float* x_dev) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    if (sh->ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, "a binary index has no list pre-sizing");
     if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
     if (n <= 0 || !x_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad plan arguments");
     std::lock_guard<std::mutex> g(sh->add_mu);
@@ -1514,6 +1654,7 @@ int b200vs_shard_plan_add_device(b200vs_shard* h, int64_t n, const float* x_dev)
 int b200vs_shard_plan_commit(b200vs_shard* h) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
+    if (sh->ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, "a binary index has no list pre-sizing");
     if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
     std::lock_guard<std::mutex> g(sh->add_mu);
     IndexBase* ix = sh->ix;
@@ -1532,70 +1673,40 @@ int b200vs_shard_plan_commit(b200vs_shard* h) {
 
 int b200vs_shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, int32_t k, const b200vs_search_params* sp,
                                float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, stream, nq, k, sp, [&] { return check_shard_topk(nq, xq_dev, k, out_dist_dev, out_ids_dev); },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 shard_search_stream(sh, L, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
-               });
-    return B200VS_OK;
-  });
+  return shard_search_device(h, seq, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, false);
+}
+int b200vs_shard_search_binary_device(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq_dev, int32_t k,
+                                      const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
+  return shard_search_device(h, seq, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, true);
 }
 
-// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).
 int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                         int64_t* out_ids) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, nullptr, nq, k, sp, [&] { return check_shard_topk(nq, xq, k, out_dist, out_ids); },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 IndexBase* ix = sh->ix;
-                 const float* q = upload_batch(sh, L, nq, xq, s);
-                 float* dd = ix->scratch.alloc<float>((size_t)nq * k);
-                 long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-                 shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
-                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-               });
-    return B200VS_OK;
-  });
+  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, false);
+}
+int b200vs_shard_search_binary(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
+                               float* out_dist, int64_t* out_ids) {
+  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, true);
 }
 
 int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, float radius, int32_t max_results,
                                      const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, int32_t* out_counts_dev,
                                      void* stream) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, stream, nq, max_results, sp,
-               [&] { return check_shard_range(sh->ix, nq, xq_dev, max_results, out_dist_dev, out_ids_dev, out_counts_dev); },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 shard_range_stream(sh, L, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
-               });
-    return B200VS_OK;
-  });
+  return shard_range_search_device(h, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev, stream, false);
+}
+int b200vs_shard_range_search_binary_device(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq_dev, float radius,
+                                            int32_t max_results, const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev,
+                                            int32_t* out_counts_dev, void* stream) {
+  return shard_range_search_device(h, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev, stream, true);
 }
 
-// Host-pointer variant: as b200vs_shard_search, each rank uploads only its slice of the batch.
 int b200vs_shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, float radius, int32_t max_results,
                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, nullptr, nq, max_results, sp,
-               [&] { return check_shard_range(sh->ix, nq, xq, max_results, out_dist, out_ids, out_counts); },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 IndexBase* ix = sh->ix;
-                 const float* q = upload_batch(sh, L, nq, xq, s);
-                 const size_t nr = (size_t)nq * max_results;
-                 float* dd = ix->scratch.alloc<float>(nr);
-                 long long* di = ix->scratch.alloc<long long>(nr);
-                 int* dc = ix->scratch.alloc<int>((size_t)nq);
-                 shard_range_stream(sh, L, nq, q, radius, max_results, sp, dd, di, dc, s);
-                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-               });
-    return B200VS_OK;
-  });
+  return shard_range_search(h, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, false);
+}
+int b200vs_shard_range_search_binary(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, float radius, int32_t max_results,
+                                     const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  return shard_range_search(h, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, true);
 }
 
 }  // extern "C"

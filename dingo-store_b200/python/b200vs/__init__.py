@@ -36,6 +36,9 @@ ABI_SYMBOLS = [
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
     "b200vs_shard_hnsw_add_batched", "b200vs_row_owner", "b200vs_shard_save", "b200vs_shard_load",
     "b200vs_need_rebuild", "b200vs_rebuild_from",
+    "b200vs_shard_create_binary", "b200vs_shard_train_binary", "b200vs_shard_add_binary", "b200vs_shard_add_binary_device",
+    "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
+    "b200vs_shard_range_search_binary_device",
 ]
 
 
@@ -149,6 +152,14 @@ def lib():
     L.b200vs_shard_load.argtypes = [vp, ctypes.c_char_p]
     L.b200vs_need_rebuild.argtypes = [vp]
     L.b200vs_rebuild_from.argtypes = [vp, vp, ctypes.POINTER(i64)]
+    L.b200vs_shard_create_binary.argtypes = [vp, i32, i32, vp, i32, ctypes.POINTER(vp)]
+    L.b200vs_shard_train_binary.argtypes = [vp, i64, vp]
+    L.b200vs_shard_add_binary.argtypes = [vp, i64, vp, vp]
+    L.b200vs_shard_add_binary_device.argtypes = [vp, i64, vp, vp]
+    L.b200vs_shard_search_binary.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_shard_search_binary_device.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_shard_range_search_binary.argtypes = [vp, i64, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
+    L.b200vs_shard_range_search_binary_device.argtypes = [vp, i64, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -542,6 +553,68 @@ class Shard:
         _check(lib().b200vs_shard_range_search_device(self.h, seq, nq, xq_dev_ptr, float(radius), max_results,
                                                       ctypes.byref(sp) if sp is not None else None, out_dist_dev_ptr,
                                                       out_ids_dev_ptr, out_counts_dev_ptr, stream))
+
+
+class BinaryShard(Shard):
+    """One rank of a sharded binary index (b200vs_shard_*_binary): BINARY_IVF_FLAT by inverted list, BINARY_FLAT by row.
+    Rows and queries are packed uint8 [n, dim / 8]; the calls every shard kind shares (list_range, broadcast_state, delete,
+    save, load) are Shard's."""
+
+    def __init__(self, index, rank, world, id_bytes=None, lanes=2):
+        self.ix, self.rank, self.world = index, int(rank), int(world)
+        self.h = ctypes.c_void_p()
+        idb = np.ascontiguousarray(id_bytes, dtype=np.uint8) if id_bytes is not None else None
+        _check(lib().b200vs_shard_create_binary(index.h, rank, world, idb.ctypes.data if idb is not None else None, lanes,
+                                                ctypes.byref(self.h)))
+
+    def _rows(self, x):
+        x = _u8(x)
+        return x, (x.shape[0] if x.ndim == 2 else x.size // max(self.ix.dim // 8, 1))
+
+    def train(self, x):
+        x, n = self._rows(x)
+        _check(lib().b200vs_shard_train_binary(self.h, n, x.ctypes.data if x.size else None))
+
+    def add(self, x, ids):
+        x, ids = _u8(x), _i64(ids)
+        _check(lib().b200vs_shard_add_binary(self.h, ids.size, x.ctypes.data if x.size else None, ids.ctypes.data if ids.size else None))
+
+    def add_device(self, n, x_dev_ptr, ids_dev_ptr):
+        _check(lib().b200vs_shard_add_binary_device(self.h, n, x_dev_ptr, ids_dev_ptr))
+
+    def search(self, xq, k, seq=-1, **kw):
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, k), dtype=np.float32)
+        I = np.full((nq, k), -1, dtype=np.int64)
+        _check(lib().b200vs_shard_search_binary(self.h, seq, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp),
+                                                D.ctypes.data, I.ctypes.data))
+        return D, I
+
+    def search_raw(self, nq, xq_ptr, k, out_dist_ptr, out_ids_ptr, sp=None, seq=-1):
+        _check(lib().b200vs_shard_search_binary(self.h, seq, nq, xq_ptr, k, ctypes.byref(sp) if sp is not None else None, out_dist_ptr,
+                                                out_ids_ptr))
+
+    def search_device(self, nq, xq_dev_ptr, k, out_dist_dev_ptr, out_ids_dev_ptr, stream=None, sp=None, seq=-1):
+        _check(lib().b200vs_shard_search_binary_device(self.h, seq, nq, xq_dev_ptr, k, ctypes.byref(sp) if sp is not None else None,
+                                                       out_dist_dev_ptr, out_ids_dev_ptr, stream))
+
+    def range_search(self, xq, radius, max_results=1024, seq=-1, **kw):
+        """b200vs_shard_range_search_binary: every rank passes the same batch; returns (distances, ids, counts)."""
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(max_results, 0)), dtype=np.float32)
+        I = np.full((nq, max(max_results, 0)), -1, dtype=np.int64)
+        C = np.zeros(nq, dtype=np.int32)
+        _check(lib().b200vs_shard_range_search_binary(self.h, seq, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
+                                                      ctypes.byref(sp), D.ctypes.data, I.ctypes.data, C.ctypes.data))
+        return D, I, C
+
+    def range_search_device(self, nq, xq_dev_ptr, radius, max_results, out_dist_dev_ptr, out_ids_dev_ptr, out_counts_dev_ptr,
+                            stream=None, sp=None, seq=-1):
+        _check(lib().b200vs_shard_range_search_binary_device(self.h, seq, nq, xq_dev_ptr, float(radius), max_results,
+                                                             ctypes.byref(sp) if sp is not None else None, out_dist_dev_ptr,
+                                                             out_ids_dev_ptr, out_counts_dev_ptr, stream))
 
 
 def ivf_state_blob(centroids, metric):

@@ -323,7 +323,30 @@ int b200vs_search_probes_device(b200vs_index* idx, int64_t nq, const float* xq_d
  *                saved rank's byte for byte.  Another world W' (FLAT, IVF_FLAT, IVF_PQ): every rank installs the trained
  *                state, file f is read by rank f mod W', and every row travels to its owner under W' through shard_add's
  *                routing (rank 0's rows first) with its saved list, stored exactly as saved: no re-assignment, no second
- *                cosine normalisation, IVF_PQ codes never re-encoded.  HNSW onto W' != W: EVECTOR_NOT_SUPPORT. */
+ *                cosine normalisation, IVF_PQ codes never re-encoded.  HNSW onto W' != W: EVECTOR_NOT_SUPPORT.
+ *
+ * Binary shards (DESIGN.md 4.5): BINARY_IVF_FLAT is sharded by list like IVF_FLAT, BINARY_FLAT by row like FLAT.  They are
+ * created and fed through the _binary family below, on packed rows and queries of dim / 8 bytes (as b200vs_add_with_ids_binary);
+ * shard_destroy, shard_list_range, shard_broadcast_state (the 'IVFB' state), shard_remove_ids, shard_save, shard_load and
+ * b200vs_row_owner serve both kinds.  On a binary shard:
+ *   shard_create_binary : BINARY_IVF_FLAT (untrained or trained, as IVF_FLAT) or an EMPTY BINARY_FLAT; a float index:
+ *                     EILLEGAL_PARAMETERS.  shard_create keeps refusing binary indexes (EVECTOR_NOT_SUPPORT)
+ *   the float data calls (train, add[_device], search[_device], range_search[_device]): EILLEGAL_PARAMETERS, and the _binary
+ *                     ones on a float shard too (a refused read still uses up its sequence number); shard_plan_add_device
+ *                     and shard_plan_commit: EVECTOR_NOT_SUPPORT; shard_hnsw_add_batched: EILLEGAL_PARAMETERS
+ *   shard_train_binary : BINARY_IVF_FLAT: shard_train's flow with b200vs_train_binary's k-means on each rank's rows (nlist / world
+ *                     packed centroids each, one all-gather); at world = 1 the state equals b200vs_train_binary's.  BINARY_FLAT: OK
+ *   shard_add_binary[_device] : BINARY_IVF_FLAT: the sender assigns each row with the Hamming coarse pass (nearest list, ties to
+ *                     the smaller list id) and the packed row travels to the list's owner; BINARY_FLAT: rows travel to
+ *                     b200vs_row_owner(id), an id repeated in the collective call -> EVECTOR_ID_DUPLICATED on every rank
+ *   shard_search_binary[_device] : BINARY_IVF_FLAT: Hamming coarse pass on the rank's slice + all-gather of the probe table, then
+ *                     the binary list scan (BMMA tile scan or exact Hamming scan, as b200vs_search_binary chooses) of the owned
+ *                     probed lists; BINARY_FLAT: the rank's own rows.  The merge key is the Hamming distance, which is also the
+ *                     API distance.  Results equal b200vs_search_binary on the unsharded index bit for bit.
+ *   shard_range_search_binary[_device] : b200vs_range_search_binary's rule (radius clamped to dim + 1 and truncated, hits have
+ *                     distance < radius), equal bit for bit; a NaN radius: EILLEGAL_PARAMETERS on every rank before the first
+ *                     collective (its sequence number is used up).
+ * Snapshots of binary shards are rank files in b200vs_save's "B2VSBIN1" container; both kinds restore onto another world. */
 #define B200VS_SHARD_ID_BYTES 128
 typedef struct b200vs_shard b200vs_shard;
 int b200vs_shard_unique_id(uint8_t id[B200VS_SHARD_ID_BYTES]);
@@ -367,6 +390,22 @@ int b200vs_shard_range_search(b200vs_shard* shard, int64_t seq, int64_t nq, cons
 int b200vs_shard_range_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, float radius,
                                      int32_t max_results, const b200vs_search_params* sp, float* out_dist_dev,
                                      int64_t* out_ids_dev, int32_t* out_counts_dev, void* stream);
+/* binary shards (see above): packed rows and queries, dim / 8 bytes each */
+int b200vs_shard_create_binary(b200vs_index* idx, int32_t rank, int32_t world, const uint8_t id[B200VS_SHARD_ID_BYTES],
+                               int32_t lanes, b200vs_shard** out);
+int b200vs_shard_train_binary(b200vs_shard* shard, int64_t n, const uint8_t* x);
+int b200vs_shard_add_binary(b200vs_shard* shard, int64_t n, const uint8_t* x, const int64_t* ids);
+int b200vs_shard_add_binary_device(b200vs_shard* shard, int64_t n, const uint8_t* x_dev, const int64_t* ids_dev);
+int b200vs_shard_search_binary(b200vs_shard* shard, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k,
+                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids);
+int b200vs_shard_search_binary_device(b200vs_shard* shard, int64_t seq, int64_t nq, const uint8_t* xq_dev, int32_t k,
+                                      const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
+int b200vs_shard_range_search_binary(b200vs_shard* shard, int64_t seq, int64_t nq, const uint8_t* xq, float radius,
+                                     int32_t max_results, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids,
+                                     int32_t* out_counts);
+int b200vs_shard_range_search_binary_device(b200vs_shard* shard, int64_t seq, int64_t nq, const uint8_t* xq_dev, float radius,
+                                            int32_t max_results, const b200vs_search_params* sp, float* out_dist_dev,
+                                            int64_t* out_ids_dev, int32_t* out_counts_dev, void* stream);
 
 /* Device-pointer write path of a single index (IVF_FLAT, IVF_PQ in its IVF-PQ mode): rows and ids already on the index's
  * device.  lists_dev (nullable) = the inverted list of every row when the caller has already assigned them
