@@ -25,8 +25,8 @@ void check_row_type(IndexBase* ix, bool binary_call) {
     fail(B200VS_EILLEGAL_PARAMETERS, binary_call ? "binary entry point on a float index" : "float entry point on a binary index");
 }
 
-// The device-pointer add and the list building blocks take FP32 rows: a binary index refuses them as the index layer did
-// before it served binary shards (b200vs_shard_*_binary reach those hooks with packed rows)
+// The list building blocks take FP32 rows: a binary index refuses them as the index layer did before it served binary
+// shards (b200vs_shard_*_binary reach those hooks with packed rows)
 void refuse_binary_rows(IndexBase* ix, const char* what) {
   if (ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, std::string(what) + " only exists for IVF_FLAT and IVF_PQ");
 }
@@ -193,7 +193,7 @@ int b200vs_add_with_ids(b200vs_index* h, int64_t n, const float* x, const int64_
     IndexBase* ix = get(h);
     check_row_type(ix, false);
     if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");  // flat.cc:123-125
-    ix->add(n, x, ids, upsert != 0);
+    ix->add(AddReq::host(n, x, ids, upsert != 0));
     return B200VS_OK;
   });
 }
@@ -203,7 +203,10 @@ int b200vs_hnsw_add_batched(b200vs_index* h, int64_t n, const float* x, const in
     IndexBase* ix = get(h);
     if (ix->type != B200VS_HNSW) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction needs an HNSW index");
     if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-    hnsw_add_batched(ix, n, x, ids, batch);
+    AddReq r = AddReq::host(n, x, ids);
+    r.batched = true;
+    r.batch = batch;
+    ix->add(r);
     return B200VS_OK;
   });
 }
@@ -221,8 +224,9 @@ int b200vs_add_with_ids_device(b200vs_index* h, int64_t n, const float* x_dev, c
   return guarded([&]() -> int {
     IndexBase* ix = get(h);
     if (n <= 0 || !x_dev || !ids_dev) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-    refuse_binary_rows(ix, "device-pointer add");
-    ix->add_dev(n, x_dev, (const long long*)ids_dev, (const long long*)lists_dev, upsert != 0, false);
+    if (ix->type != B200VS_IVF_FLAT && ix->type != B200VS_IVF_PQ)
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
+    ix->add(AddReq::device(n, x_dev, (const long long*)ids_dev, (const long long*)lists_dev, upsert != 0));
     return B200VS_OK;
   });
 }
@@ -509,14 +513,10 @@ int b200vs_rebuild_from(b200vs_index* dst_h, b200vs_index* src_h, int64_t* n_row
     IndexBase* src = get(src_h);
     if (dst == src) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src are the same index");
     std::shared_lock<std::shared_mutex> rl(src->rw);  // searches on src go on; its writers wait
-    std::unique_lock<std::shared_mutex> wl(dst->rw);
-    std::lock_guard<std::mutex> gl(dst->gpu_mu);
+    WriteHold hold(dst);
     check_rebuild_pair(*dst, *src);
     if (dst->type == B200VS_FLAT || dst->type == B200VS_BINARY_FLAT)
       fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");  // vector_index_flat.h:111
-    dst->set_device();
-    dst->quiesce();
-    dst->scratch.reset(dst->stream);
     const int64_t n = dst->rebuild_from(*src);
     if (n_rows) *n_rows = n;
     return B200VS_OK;
@@ -692,7 +692,7 @@ int b200vs_scan_push(b200vs_scan* st, int64_t n, const float* x, const int64_t* 
     IndexBase* ix = st->flat;
     const size_t nk = (size_t)st->nq * st->k;
     if (st->pushed > 0) ix->clear();
-    ix->add(n, x, ids, false);  // one temporary Flat index per tile, as the reference builds (vector_reader.cc:1937-1946)
+    ix->add(AddReq::host(n, x, ids));  // one temporary Flat index per tile, as the reference builds (vector_reader.cc:1937-1946)
     index_read(ix, st->s, st->has_sp ? &st->sp : nullptr, [&](const SearchCtx& sc, cudaStream_t s) {
       SearchReq r;
       r.nq = st->nq; r.xq = st->q.p; r.k = st->k; r.sc = &sc; r.od = st->parts_d.p + nk; r.oi = st->parts_i.p + nk;
@@ -833,7 +833,7 @@ int b200vs_train_binary(b200vs_index* h, int64_t n, const uint8_t* x) {
     IndexBase* ix = get(h);
     check_row_type(ix, true);
     if (n <= 0 || !x) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
-    ix->train_binary(n, x);
+    ix->train(n, x);
     return B200VS_OK;
   });
 }
@@ -843,7 +843,7 @@ int b200vs_add_with_ids_binary(b200vs_index* h, int64_t n, const uint8_t* x, con
     IndexBase* ix = get(h);
     check_row_type(ix, true);
     if (n <= 0 || !x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-    ix->add_binary(n, x, ids, upsert != 0);
+    ix->add(AddReq::host(n, x, ids, upsert != 0));
     return B200VS_OK;
   });
 }

@@ -120,12 +120,10 @@ struct BinRows {
   }
 };
 
-// Shared by both binary types: the float entry points are refused (api.cu checks first), rows arrive packed.
+// Shared by both binary types: the float entry points are refused (api.cu), rows arrive packed.
 struct BinaryIndex : IndexBase {
   const int nb, w;  // bytes per packed row; 32-bit words per padded row
   BinaryIndex(b200vs_type t, int d, const b200vs_params& p) : IndexBase(t, B200VS_HAMMING, d, p), nb(d / 8), w(words_of(d)) {}
-
-  void add(int64_t, const float*, const int64_t*, bool) override { fail(B200VS_EILLEGAL_PARAMETERS, "float entry point on a binary index"); }
 
   // packed device rows -> padded words in scratch
   const uint32_t* pad(int64_t n, const uint8_t* x_dev, cudaStream_t s) {
@@ -135,12 +133,6 @@ struct BinaryIndex : IndexBase {
       launch_count(1);
     }
     return out;
-  }
-  // host packed rows -> padded device words in scratch (writers: on the index stream)
-  const uint32_t* upload(int64_t n, const uint8_t* x) {
-    uint8_t* raw = scratch.alloc<uint8_t>((size_t)n * nb);
-    B200VS_CUDA(cudaMemcpyAsync(raw, x, (size_t)n * nb, cudaMemcpyHostToDevice, stream));
-    return pad(n, raw, stream);
   }
   ScanJob hamming_job(const uint32_t* rows, const long long* ids, long long n) const {
     ScanJob j;
@@ -172,39 +164,20 @@ struct BinaryFlatIndex : BinaryIndex {
   FlatRowMap<BinRows> rowmap{this};
 
   BinaryFlatIndex(int d, const b200vs_params& p) : BinaryIndex(B200VS_BINARY_FLAT, d, p) {}
-  void train_binary(int64_t, const uint8_t*) override {}  // a Flat index needs no training (flat.cc Train returns OK)
 
   // AddOrUpsert (flat.cc:121-162): duplicate ids in the batch are refused, existing ids are always removed first
-  void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool) override {
-    check_batch_ids_unique(n, in_ids);
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    const uint32_t* st = upload(n, x);
-    long long* st_ids = scratch.alloc<long long>(n);
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    rowmap.add(n, st, st_ids, in_ids);
+  void add(const AddReq& r) override {
+    if (r.ids) check_batch_ids_unique(r.n, r.ids);
+    WriteHold hold(this);
+    Staged st;
+    stage(r, nb, false, st);
+    if (!r.ids) check_batch_ids_unique(r.n, st.ids);
+    rowmap.add(r.n, pad(r.n, static_cast<const uint8_t*>(st.x), stream), st.ids_dev, st.ids);
   }
-  // add_binary on packed rows and ids already on this device (the owner of a row-sharded add); ids_host = the same ids
-  void add_rows_dev(int64_t n, const void* x_dev, const long long* ids_dev, const int64_t* ids_host) override {
-    check_batch_ids_unique(n, ids_host);
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    rowmap.add(n, pad(n, static_cast<const uint8_t*>(x_dev), stream), ids_dev, ids_host);
-  }
-  void check_add(int64_t n, const int64_t* in_ids, bool, int) override { check_batch_ids_unique(n, in_ids); }
+  void check_add(const AddReq& r) override { check_batch_ids_unique(r.n, r.ids); }
   // Delete (flat.cc:171-203): ids that are not present are ignored
   int64_t remove(int64_t n, const int64_t* del) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
+    WriteHold hold(this);
     return rowmap.remove(n, del);
   }
   ScanJob job(const SearchCtx& sc) const {
@@ -262,12 +235,13 @@ struct BinaryIvfIndex : BinaryIndex {
   int export_nlist() const override { return nlist; }
   int nlist_now() const override { return nlist; }
 
-  // packed centroids [k, dim / 8] (host)
+  // packed centroids [k, dim / 8] (host); the writer hold is taken
   void install_centroids(const uint8_t* host_c, int k) {
-    quiesce();
     nlist = k;
     scratch.reset(stream);
-    const uint32_t* st = upload(k, host_c);
+    uint8_t* raw = scratch.alloc<uint8_t>((size_t)k * nb);
+    B200VS_CUDA(cudaMemcpyAsync(raw, host_c, (size_t)k * nb, cudaMemcpyHostToDevice, stream));
+    const uint32_t* st = pad(k, raw, stream);
     cent.free(); cent_ids.free();
     cent.reserve((size_t)k * w, 0, stream);
     cent_ids.reserve(k, 0, stream);
@@ -286,9 +260,7 @@ struct BinaryIvfIndex : BinaryIndex {
     memcpy(blob, hdr, 32);
   }
   void set_state(const void* blob, size_t len) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
+    WriteHold hold(this);
     if (len < 32) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
     if (hdr[0] != kStateMagic || hdr[2] != dim || hdr[3] != B200VS_HAMMING) fail(B200VS_EILLEGAL_PARAMETERS, "bad binary IVF state blob");
@@ -314,16 +286,12 @@ struct BinaryIvfIndex : BinaryIndex {
   // on the +-1 rows (kmeans_gpu: same subsample permutation, seed, iterations and split_clusters as IVF-Flat), and
   // real_to_binary (bit set where the coordinate is > 0).  Only the training subsample is expanded to floats: the rows
   // kmeans_gpu would draw, in its order, so it sees exactly what it would see on the whole expanded set.
-  void train_binary(int64_t n, const uint8_t* x) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
+  void train(int64_t n, const void* x) override {
+    WriteHold hold(this);
     if (trained) return;  // ivf_flat.cc:670-672
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    train_locked(n, x, nullptr);
+    train_locked(n, static_cast<const uint8_t*>(x), nullptr);
   }
-  // train_binary's rule with rw and gpu_mu held, on host packed rows x, or (x_words) on padded rows already on the device,
+  // train's rule with rw and gpu_mu held, on host packed rows x, or (x_words) on padded rows already on the device,
   // whose sample is expanded to +-1 floats there
   void train_locked(int64_t n, const uint8_t* x, const uint32_t* x_words) {
     const int k = n < nlist ? 1 : nlist;  // "data size too small, nlist degenerate to 1"
@@ -465,55 +433,27 @@ struct BinaryIvfIndex : BinaryIndex {
     return j;
   }
 
-  void add_binary(int64_t n, const uint8_t* x, const int64_t* in_ids, bool upsert) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");  // ivf_flat.cc:111-113
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    if (upsert) L.remove(n, in_ids, store);  // ivf_flat.cc:115-118
-    const uint32_t* st = upload(n, x);
-    long long* st_ids = scratch.alloc<long long>(n);
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    place_locked(n, st, st_ids, in_ids);
+  // untrained -> refused (ivf_flat.cc:111-113); upsert removes the ids first (:115-118); rows go to
+  // the caller's lists (the owner of a list-sharded add) or the nearest ones.  The form has no meaning for bits.
+  void add(const AddReq& r) override {
+    WriteHold hold(this);
+    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
+    Staged st;
+    stage(r, nb, false, st);
+    if (r.upsert) L.remove(r.n, st.ids, store);
+    place_locked(r.n, pad(r.n, static_cast<const uint8_t*>(st.x), stream), st.ids_dev, st.ids, r.lists);
   }
   // padded device rows st and ids st_ids (in_ids: the same on the host) to the tails of their lists: lists_dev, or (null) the
-  // nearest ones; rw and gpu_mu held
+  // nearest ones; the writer hold is taken
   void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids, const long long* lists_dev = nullptr) {
-    if (!lists_dev) {
-      long long* lists = scratch.alloc<long long>(n);
-      assign_words(n, st, lists, stream);
-      lists_dev = lists;
-    }
-    std::vector<long long> h_list(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
+    std::vector<long long> h_list;
+    IvfLists::row_lists(this, n, lists_dev, h_list, [&](long long* out) { assign_words(n, st, out, stream); });
     L.place(n, h_list.data(), in_ids, st, st_ids, store);
-  }
-  // add_binary on packed rows and ids already on this device, to the caller's lists (the owner of a list-sharded add) or
-  // (lists_dev null) the nearest ones; prepared has no meaning for bits
-  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    std::vector<int64_t> h_ids(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    if (upsert) L.remove(n, h_ids.data(), store);
-    place_locked(n, pad(n, static_cast<const uint8_t*>(x_dev), stream), ids_dev, h_ids.data(), lists_dev);
   }
   // Delete (ivf_flat.cc:162-189): untrained -> OK; nothing removed -> EVECTOR_INVALID (api.cu)
   int64_t remove(int64_t n, const int64_t* del) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
+    WriteHold hold(this);
     if (!trained) return -1;
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
     const int64_t r = L.remove(n, del, store);
     L.compact_if_needed(store);
     return r;
@@ -562,11 +502,7 @@ static BinaryIvfIndex* as_binary_ivf(IndexBase* ix) {
 
 void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, int k, std::vector<uint8_t>& cent) {
   BinaryIvfIndex* b = as_binary_ivf(ix);
-  std::unique_lock<std::shared_mutex> wl(b->rw);
-  std::lock_guard<std::mutex> gl(b->gpu_mu);
-  b->set_device();
-  b->quiesce();
-  b->scratch.reset(b->stream);
+  WriteHold hold(b);
   b->kmeans_locked(n, x, nullptr, k, cent);
 }
 

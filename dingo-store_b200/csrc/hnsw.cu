@@ -972,13 +972,34 @@ struct HnswIndex : IndexBase {
     dirty = true; uploaded_rows = 0;
   }
 
-  // VectorIndexHnsw::Upsert, hnsw.cc:203-254 (Add == Upsert; vectors are normalised per row for cosine)
-  void add(int64_t n, const float* x, const int64_t* in_ids, bool) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
+  // VectorIndexHnsw::Upsert, hnsw.cc:203-254 (Add == Upsert; vectors are normalised per row for cosine).  The builders take
+  // host rows: device rows are downloaded first.  batched: b200vs_hnsw_add_batched.
+  void add(const AddReq& r) override {
+    WriteHold hold(this);
+    std::vector<float> hx;
+    std::vector<int64_t> hid;
+    const float* x = static_cast<const float*>(r.x);
+    const int64_t* ids = r.ids;
+    if (r.on_device) {
+      hx.resize((size_t)r.n * dim);
+      B200VS_CUDA(cudaMemcpyAsync(hx.data(), x, hx.size() * 4, cudaMemcpyDeviceToHost, stream));
+      if (!ids) {
+        hid.resize(r.n);
+        B200VS_CUDA(cudaMemcpyAsync(hid.data(), r.ids_dev, (size_t)r.n * 8, cudaMemcpyDeviceToHost, stream));
+        ids = hid.data();
+      }
+      B200VS_CUDA(cudaStreamSynchronize(stream));
+      x = hx.data();
+    }
+    if (r.batched) add_batched_locked(r.n, x, ids, r.batch, r.form != AddReq::RAW);
+    else add_host_locked(r.n, x, ids, r.form != AddReq::RAW);
+  }
+  // the host builder with the writer hold taken; prepared = rows stored as given (cosine rows are already normalised)
+  void add_host_locked(int64_t n, const float* x, const int64_t* in_ids, bool is_prepared) {
     if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
     auto prepared = [&](int64_t i, std::vector<float>& tmp) -> const float* {
       const float* xi = x + (size_t)i * dim;
-      if (metric != B200VS_COSINE) return xi;
+      if (metric != B200VS_COSINE || is_prepared) return xi;
       normalize_for_hnsw(xi, dim, tmp.data());
       return tmp.data();
     };
@@ -1007,11 +1028,11 @@ struct HnswIndex : IndexBase {
     }
     dirty = true;
   }
-  // add's refusals (batched: add_batched's, for that batch size), which come before either changes anything
-  void check_add(int64_t n, const int64_t*, bool batched, int batch) override {
+  // add's refusals (batched: the batched build's, for that batch size), which come before either changes anything
+  void check_add(const AddReq& r) override {
     RwSharedGuard rl(this);
-    if (batched) batched_plan(n, batch);
-    else if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
+    if (r.batched) batched_plan(r.n, r.batch);
+    else if (G.n + r.n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
   }
   // b200vs_hnsw_add_batched: the rule of DESIGN §4.4.  The host plans every batch first on a copy of the bookkeeping it needs
   // (levels from a copy of G.rng in call order, the batch schedule, tombstones, node ids, entry point); the device mirror then
@@ -1019,7 +1040,7 @@ struct HnswIndex : IndexBase {
   // finished: a call that fails on the way leaves the index as it was and marks the mirror for a full re-upload.
   int64_t build_scratch_limit = 0;  // b200vs_debug_hnsw_build_scratch_limit: device scratch bytes one call may take, 0 = no cap
 
-  // the batch size and the construction kernels' shared memory of add_batched(n rows, batch), after its refusals
+  // the batch size and the construction kernels' shared memory of the batched build of n rows, after its refusals
   struct BuildPlan { int batch, bmax; size_t smem_search, smem_link, smem_rev; };
   BuildPlan batched_plan(int64_t n, int batch) const {
     if (G.n + n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");
@@ -1035,21 +1056,15 @@ struct HnswIndex : IndexBase {
     return P;
   }
 
-  void add_batched(int64_t n, const float* x, const int64_t* in_ids, int batch) {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    add_batched_locked(n, x, in_ids, batch, false);
-  }
-  // add_batched with rw held; prepared = rows stored as given (cosine rows are already normalised)
+  // the batched build with the writer hold taken; prepared = rows stored as given (cosine rows are already normalised)
   void add_batched_locked(int64_t n, const float* x, const int64_t* in_ids, int batch, bool prepared) {
     const BuildPlan P = batched_plan(n, batch);
     batch = P.batch;
     const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
     const int bmax = P.bmax;
     const size_t smem_search = P.smem_search;
-    set_device();
     cudaStream_t s = stream;
     upload(s);
-    quiesce();
 
     // ---- plan (host), on copies: G is not touched until the device work is done ----
     const int64_t n0_call = G.n, ntot = G.n + n;
@@ -1440,9 +1455,6 @@ struct HnswIndex : IndexBase {
 
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p) { return new HnswIndex(m, d, p); }
 
-void hnsw_add_batched(IndexBase* ix, int64_t n, const float* x, const int64_t* ids, int batch) {
-  static_cast<HnswIndex*>(ix)->add_batched(n, x, ids, batch);
-}
 void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes) {
   std::unique_lock<std::shared_mutex> wl(ix->rw);
   static_cast<HnswIndex*>(ix)->build_scratch_limit = bytes;

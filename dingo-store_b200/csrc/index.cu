@@ -190,17 +190,30 @@ void IndexBase::load(const std::string& path) {
     rd(f, off.data(), off.size() * 8);
     rd(f, ids.data(), ids.size() * 8);
     rd(f, rows.data(), rows.size());
-    loading = true;
-    try {
-      for (int64_t a = 0; a < h.count; a += 32768) {
-        const int64_t m = std::min<int64_t>(32768, h.count - a);
-        if (binary()) add_binary(m, rows.data() + (size_t)a * rb, ids.data() + a, false);
-        else add(m, reinterpret_cast<const float*>(rows.data() + (size_t)a * rb), ids.data() + a, false);
-      }
-    } catch (...) { loading = false; throw; }
-    loading = false;
+    for (int64_t a = 0; a < h.count; a += 32768)  // the rows come back exactly as stored
+      add(AddReq::host(std::min<int64_t>(32768, h.count - a), rows.data() + (size_t)a * rb, ids.data() + a, false, AddReq::PREPARED));
   } catch (...) { fclose(f); throw; }
   fclose(f);
+}
+
+void IndexBase::stage(const AddReq& r, size_t row_bytes, bool own, Staged& st) {
+  st.x = const_cast<void*>(r.x);
+  st.ids_dev = r.ids_dev;
+  st.ids = r.ids;
+  if (!r.on_device || own) {
+    st.x = scratch.alloc<unsigned char>((size_t)r.n * row_bytes);
+    B200VS_CUDA(cudaMemcpyAsync(st.x, r.x, (size_t)r.n * row_bytes, r.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
+  }
+  if (!r.on_device) {
+    long long* d = scratch.alloc<long long>(r.n);
+    B200VS_CUDA(cudaMemcpyAsync(d, r.ids, (size_t)r.n * 8, cudaMemcpyHostToDevice, stream));
+    st.ids_dev = d;
+  } else if (!r.ids) {
+    st.ids_buf.resize(r.n);
+    B200VS_CUDA(cudaMemcpyAsync(st.ids_buf.data(), r.ids_dev, (size_t)r.n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    st.ids = st.ids_buf.data();
+  }
 }
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids) {  // CheckVectorIdDuplicated, vector_index_utils.cc:551-561
@@ -314,49 +327,24 @@ struct FlatIndex : IndexBase {
   FlatIndex(b200vs_metric m, int d, const b200vs_params& p) : IndexBase(B200VS_FLAT, m, d, p) {}
 
   // VectorIndexFlat::AddOrUpsert, vector_index_flat.cc:121-162: duplicate ids inside the batch are rejected,
-  // pre-existing ids are ALWAYS removed first (add and upsert behave the same), then add_with_ids.
-  void add(int64_t n, const float* x, const int64_t* in_ids, bool) override {
-    check_batch_ids_unique(n, in_ids);
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    float* st = scratch.alloc<float>((size_t)n * dim);
-    long long* st_ids = scratch.alloc<long long>(n);
-    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    if (metric == B200VS_COSINE && !loading) launch_normalize_faiss(st, n, dim, stream);  // flat.cc:155 (normalize_)
-    rowmap.add(n, st, st_ids, in_ids);
+  // pre-existing ids are ALWAYS removed first (add and upsert behave the same), then add_with_ids.  Device rows come from
+  // the owner of a row-sharded add, a snapshot restore and a rebuild.
+  void add(const AddReq& r) override {
+    if (r.ids) check_batch_ids_unique(r.n, r.ids);
+    WriteHold hold(this);
+    const bool normalise = metric == B200VS_COSINE && r.form == AddReq::RAW;  // the normaliser works in place
+    Staged st;
+    stage(r, (size_t)dim * 4, normalise, st);
+    if (!r.ids) check_batch_ids_unique(r.n, st.ids);
+    if (normalise) launch_normalize_faiss(static_cast<float*>(st.x), r.n, dim, stream);  // flat.cc:155 (normalize_)
+    rowmap.add(r.n, static_cast<const float*>(st.x), st.ids_dev, st.ids);
   }
 
-  // the device-pointer form of add: the rows stay on the device, the caller's host copy of the ids feeds the id map
-  void add_rows_dev(int64_t n, const void* xv, const long long* ids_dev, const int64_t* ids_host) override {
-    const float* x_dev = static_cast<const float*>(xv);
-    check_batch_ids_unique(n, ids_host);
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    const float* st = x_dev;
-    if (metric == B200VS_COSINE && !loading) {  // the normaliser works in place: keep the caller's rows intact
-      float* cp = scratch.alloc<float>((size_t)n * dim);
-      B200VS_CUDA(cudaMemcpyAsync(cp, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
-      launch_normalize_faiss(cp, n, dim, stream);
-      st = cp;
-    }
-    rowmap.add(n, st, ids_dev, ids_host);
-  }
-
-  void check_add(int64_t n, const int64_t* in_ids, bool, int) override { check_batch_ids_unique(n, in_ids); }
+  void check_add(const AddReq& r) override { check_batch_ids_unique(r.n, r.ids); }
 
   // streaming brute-force scan (b200vs_scan_*): the tile index is emptied between tiles, buffers are kept
   void clear() override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
+    WriteHold hold(this);
     rowmap.store.max_norm = 0.f;
     rowmap.clear();
   }
@@ -364,11 +352,7 @@ struct FlatIndex : IndexBase {
   // VectorIndexFlat::Delete, vector_index_flat.cc:171-203: unknown ids are ignored (only ids present in
   // rev_map are handed to remove_ids).
   int64_t remove(int64_t n, const int64_t* del) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
+    WriteHold hold(this);
     return rowmap.remove(n, del);
   }
 
@@ -524,9 +508,7 @@ struct IvfFlatIndex : IndexBase {
     memcpy(blob, hdr, 32);
   }
   void set_state(const void* blob, size_t len) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
+    WriteHold hold(this);
     if (len < 32) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
     if (hdr[0] != kStateMagic || hdr[2] != dim) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF state blob");
@@ -559,7 +541,7 @@ struct IvfFlatIndex : IndexBase {
 
   // VectorIndexIvfFlat::Train, vector_index_ivf_flat.cc:644-712 -> faiss IndexIVFFlat::train ->
   // Clustering (niter 10, seed 1234, <= 256 points per centroid); GPU Lloyd iterations here.
-  void train(int64_t n, const float* x) override;
+  void train(int64_t n, const void* x) override;
   // train's rule with rw and gpu_mu held: x on the host (raw), or on the device (x_dev: already prepared)
   void train_locked(int64_t n, const float* x, bool x_dev);
 
@@ -585,16 +567,14 @@ struct IvfFlatIndex : IndexBase {
     DevBuf<long long> ids;
     const int64_t n = src.sorted_rows(rows, ids);
     if (n == 0) return 0;
-    float* x = reinterpret_cast<float*>(rows.p);
-    train_locked(n, x, true);
+    train_locked(n, reinterpret_cast<const float*>(rows.p), true);
     scratch.reset(stream);
-    add_locked(n, x, ids.p, nullptr, nullptr, false, true);
+    add_locked(AddReq::device(n, rows.p, ids.p, nullptr, false, AddReq::PREPARED));
     return n;
   }
 
-  void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override;
-  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override;
-  void add_locked(int64_t n, float* st, const long long* st_ids, const int64_t* h_ids_in, const long long* lists_dev, bool upsert, bool prepared);
+  void add(const AddReq& r) override;
+  void add_locked(const AddReq& r);
   void reserve_lists(const int64_t* rows_per_list, int n_lists) override;
   int nlist_now() const override { return nlist; }
   void assign_lists_dev(int64_t n, const void* x_dev, long long* out_lists_dev, cudaStream_t s) override {
@@ -653,15 +633,11 @@ struct IvfFlatIndex : IndexBase {
   int64_t export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) override;
 };
 
-void IvfFlatIndex::train(int64_t n, const float* x) {
+void IvfFlatIndex::train(int64_t n, const void* x) {
   if (n <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
-  std::unique_lock<std::shared_mutex> wl(rw);
-  std::lock_guard<std::mutex> gl(gpu_mu);
+  WriteHold hold(this);
   if (trained) return;  // ivf_flat.cc:670-672
-  set_device();
-  quiesce();
-  scratch.reset(stream);
-  train_locked(n, x, false);
+  train_locked(n, static_cast<const float*>(x), false);
 }
 
 void IvfFlatIndex::train_locked(int64_t n, const float* x, bool x_dev) {
@@ -706,78 +682,36 @@ void IvfFlatIndex::train_locked(int64_t n, const float* x, bool x_dev) {
   train_rows = n;
 }
 
-void IvfFlatIndex::add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) {
-  std::unique_lock<std::shared_mutex> wl(rw);
-  if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");  // ivf_flat.cc:111-113 (caller trains and retries, :136-150)
-  std::lock_guard<std::mutex> gl(gpu_mu);
-  set_device();
-  quiesce();
-  scratch.reset(stream);
-  float* st = scratch.alloc<float>((size_t)n * dim);
-  long long* st_ids = scratch.alloc<long long>(n);
-  B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
-  B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-  add_locked(n, st, st_ids, in_ids, nullptr, upsert, loading);
-}
-
-void IvfFlatIndex::add_dev(int64_t n, const void* xv, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
-  const float* x_dev = static_cast<const float*>(xv);
-  std::unique_lock<std::shared_mutex> wl(rw);
+// untrained -> refused (ivf_flat.cc:111-113; the caller trains and retries, :136-150); upsert removes the ids first (:115-118)
+void IvfFlatIndex::add(const AddReq& r) {
+  WriteHold hold(this);
   if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-  std::lock_guard<std::mutex> gl(gpu_mu);
-  set_device();
-  quiesce();
-  scratch.reset(stream);
-  float* st = const_cast<float*>(x_dev);
-  if (metric == B200VS_COSINE && !prepared) {  // the normaliser works in place: keep the caller's rows intact
-    st = scratch.alloc<float>((size_t)n * dim);
-    B200VS_CUDA(cudaMemcpyAsync(st, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
-  }
-  add_locked(n, st, ids_dev, nullptr, lists_dev, upsert, prepared);
+  add_locked(r);
 }
 
-// rw + gpu_mu held, scratch reset.  st / st_ids: device rows and ids (st may be normalised in place); h_ids_in: host copy
-// of the ids when the caller has one; lists_dev: precomputed lists or NULL.
-void IvfFlatIndex::add_locked(int64_t n, float* st, const long long* st_ids, const int64_t* h_ids_in, const long long* lists_dev, bool upsert,
-                              bool prepared) {
-  std::vector<int64_t> h_ids_buf;
-  if (!h_ids_in) {
-    h_ids_buf.resize(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_ids_buf.data(), st_ids, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    h_ids_in = h_ids_buf.data();
-  }
-  if (upsert) L.remove(n, h_ids_in, store);  // ivf_flat.cc:115-118
-  if (metric == B200VS_COSINE && !prepared) launch_normalize_faiss(st, n, dim, stream);
-  const long long* st_list = lists_dev;
-  if (!st_list) {
-    long long* tmp = scratch.alloc<long long>(n);
-    assign_dev(st, n, tmp, stream);
-    st_list = tmp;
-  }
-  std::vector<long long> h_list(n);
-  B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-  B200VS_CUDA(cudaStreamSynchronize(stream));
-  L.place(n, h_list.data(), h_ids_in, st, st_ids, store);
+// add with the writer hold taken
+void IvfFlatIndex::add_locked(const AddReq& r) {
+  const bool normalise = metric == B200VS_COSINE && r.form == AddReq::RAW;  // the normaliser works in place
+  Staged st;
+  stage(r, (size_t)dim * 4, normalise, st);
+  if (r.upsert) L.remove(r.n, st.ids, store);
+  float* x = static_cast<float*>(st.x);
+  if (normalise) launch_normalize_faiss(x, r.n, dim, stream);
+  std::vector<long long> h_list;
+  IvfLists::row_lists(this, r.n, r.lists, h_list, [&](long long* out) { assign_dev(x, r.n, out, stream); });
+  L.place(r.n, h_list.data(), st.ids, x, st.ids_dev, store);
 }
 
 void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
-  std::unique_lock<std::shared_mutex> wl(rw);
+  WriteHold hold(this);
   if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-  std::lock_guard<std::mutex> gl(gpu_mu);
-  set_device();
-  quiesce();
   L.reserve(rows_per_list, n_lists, store);
 }
 
 // VectorIndexIvfFlat::Delete, vector_index_ivf_flat.cc:162-189: untrained -> OK; nothing removed -> EVECTOR_INVALID.
 int64_t IvfFlatIndex::remove(int64_t n, const int64_t* del) {
-  std::unique_lock<std::shared_mutex> wl(rw);
+  WriteHold hold(this);
   if (!trained) return -1;  // signalled as OK by the ABI
-  std::lock_guard<std::mutex> gl(gpu_mu);
-  set_device();
-  quiesce();
-  scratch.reset(stream);
   const int64_t r = L.remove(n, del, store);
   L.compact_if_needed(store);
   return r;

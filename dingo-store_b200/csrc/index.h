@@ -202,6 +202,37 @@ struct SearchReq {
 // the results of a search that finds nothing (an untrained or empty index): ids -1, distances 0, range counts 0
 void fill_empty(const SearchReq& r, cudaStream_t s);
 
+// One write of rows into an index (IndexBase::add).  Host rows come with host ids; device rows (on the index's device) come
+// with device ids, and with the same ids on the host when the caller already holds them.
+struct AddReq {
+  enum Form {
+    RAW,       // the caller's rows: the index applies its own cosine rule
+    PREPARED,  // stored exactly as given (already normalised for cosine): a snapshot restore, a routed shard row, a rebuild
+    ENCODED,   // the rows as export_lists writes them: IVF-PQ code rows (code_size bytes each); PREPARED on every other type
+  };
+  int64_t n = 0;
+  const void* x = nullptr;              // rows in the index's row format: FP32, packed bits (dim / 8 bytes), or code rows
+  bool on_device = false;               // x, ids_dev and lists are on the index's device
+  const int64_t* ids = nullptr;         // host ids: always for host rows; optional beside device rows
+  const long long* ids_dev = nullptr;   // device ids of device rows
+  const long long* lists = nullptr;     // device rows: the caller's inverted list of every row (IVF types); null = the nearest
+  bool upsert = false;
+  Form form = RAW;
+  bool batched = false;                 // HNSW: the batched GPU build (b200vs_hnsw_add_batched) with `batch` rows per batch
+  int batch = 0;                        // 0 = the library default
+  static AddReq host(int64_t n, const void* x, const int64_t* ids, bool upsert = false, Form form = RAW) {
+    AddReq r;
+    r.n = n; r.x = x; r.ids = ids; r.upsert = upsert; r.form = form;
+    return r;
+  }
+  static AddReq device(int64_t n, const void* x, const long long* ids_dev, const long long* lists = nullptr, bool upsert = false,
+                       Form form = RAW) {
+    AddReq r;
+    r.n = n; r.x = x; r.on_device = true; r.ids_dev = ids_dev; r.lists = lists; r.upsert = upsert; r.form = form;
+    return r;
+  }
+};
+
 // The header of IndexBase::save's container ("B2VSIDX1" / "B2VSBIN1"), followed by the trained-state blob (state_len
 // bytes), the list offsets (nlist + 1 int64), the ids (count int64) and the rows (count rows, list-major).
 struct IndexFileHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
@@ -264,7 +295,6 @@ struct IndexBase {
   }
   void reset_stats() { for (auto& v : stats) v.store(0, std::memory_order_relaxed); if (profiling) for (auto& v : phase_ms) v = 0.f; }
   bool profiling = false;  // b200vs_set_profiling: time the dominant scan kernel with CUDA events
-  bool loading = false;    // Load(): rows come back exactly as stored (already normalised for cosine)
   virtual int export_nlist() const { return 1; }
 
   IndexBase(b200vs_type t, b200vs_metric m, int d, const b200vs_params& p);
@@ -272,7 +302,8 @@ struct IndexBase {
   void set_device() const { B200VS_CUDA(cudaSetDevice(device)); }
   bool ip_like() const { return metric == B200VS_IP || metric == B200VS_COSINE; }
 
-  virtual void train(int64_t n, const float* x) { (void)n; (void)x; }
+  // rows in the index's row format (FP32, or packed bits on a binary index); a Flat or HNSW index needs no training
+  virtual void train(int64_t n, const void* x) { (void)n; (void)x; }
   virtual bool is_trained() const { return true; }
   // the n of the train call that trained the index (IVF types); after a Load or a set_trained_state, the live count then
   int64_t train_rows = 0;
@@ -289,7 +320,11 @@ struct IndexBase {
   }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }
   virtual int64_t get_state(void* blob, size_t cap) { (void)blob; (void)cap; return 0; }
-  virtual void add(int64_t n, const float* x, const int64_t* ids, bool upsert) = 0;
+  // THE write of rows into an index, under the writer hold.  Each type refuses the requests it cannot serve.
+  virtual void add(const AddReq& r) = 0;
+  // the refusals add(r) would give, decided from r's host ids and sizes before anything changes, so that every rank of a
+  // collective add can agree on one status first (FLAT, BINARY_FLAT: a repeated id; HNSW: max_elements, the batched plan)
+  virtual void check_add(const AddReq& r) { (void)r; }
   virtual int64_t remove(int64_t n, const int64_t* ids) = 0;
   virtual void clear() { fail(B200VS_EVECTOR_NOT_SUPPORT, "clear is only implemented for FLAT"); }  // drop every row, keep the buffers
   // THE read of an index, on stream s with the lane's scratch already reset: r's top-k or range search.  Each type refuses
@@ -303,31 +338,8 @@ struct IndexBase {
     (void)nq; (void)xq; (void)prepared; (void)nprobe; (void)c0; (void)c1; (void)out_score; (void)out_lists; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "coarse quantiser only exists for IVF_FLAT and IVF_PQ");
   }
-  // ---- device-pointer write path and the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT, IVF_PQ and
-  // BINARY_IVF_FLAT.  Row pointers are in the index's row format: FP32 rows, or packed bits (dim / 8 bytes) on a binary index.
-  // rows / ids already on this device.  lists_dev (nullable) = the inverted list of every row, decided by the caller;
-  // prepared = store the rows exactly as given (cosine rows are already normalised).
-  virtual void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) {
-    (void)n; (void)x_dev; (void)ids_dev; (void)lists_dev; (void)upsert; (void)prepared;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "device-pointer add only exists for IVF_FLAT and IVF_PQ");
-  }
-  // IVF_PQ: append n code rows that are already encoded (code_size bytes each, as export_lists writes them) with their ids
-  // to the given lists, all on this device — the restore of a snapshot, whose vectors are gone
-  virtual void add_codes_dev(int64_t n, const uint8_t* codes_dev, const long long* ids_dev, const long long* lists_dev) {
-    (void)n; (void)codes_dev; (void)ids_dev; (void)lists_dev;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "appending encoded rows only exists for IVF_PQ");
-  }
-  // ---- building blocks of a row-sharded deployment (shard.cu); FLAT, BINARY_FLAT and HNSW ----
-  // the refusals add (batched: b200vs_hnsw_add_batched with `batch`) would give n rows with these host ids, decided before
-  // anything changes, so that every rank of a collective add can agree on one status first
-  virtual void check_add(int64_t n, const int64_t* ids, bool batched, int batch) { (void)n; (void)ids; (void)batched; (void)batch; }
-  // FLAT, BINARY_FLAT: add's semantics on rows (the index's row format) and ids already on this device; ids_host = the same
-  // ids on the host (the id map needs them, and the caller already holds them).  Only the row-sharded owner calls it:
-  // b200vs_add_with_ids_device still refuses FLAT.
-  virtual void add_rows_dev(int64_t n, const void* x_dev, const long long* ids_dev, const int64_t* ids_host) {
-    (void)n; (void)x_dev; (void)ids_dev; (void)ids_host;
-    fail(B200VS_EVECTOR_NOT_SUPPORT, "device-row add only exists for FLAT");
-  }
+  // ---- the building blocks of a list-sharded deployment (shard.cu); IVF_FLAT, IVF_PQ and BINARY_IVF_FLAT.  Row pointers
+  // are in the index's row format: FP32 rows, or packed bits (dim / 8 bytes) on a binary index.
   // the refusals a search with k and sp's efsearch would meet after the first collective of a row-sharded search, decided
   // from the arguments and the index's parameters alone, so that every rank refuses alike before it (HNSW: efsearch outside
   // [0, 1024], as b200vs_search; the walk's shared memory)
@@ -356,14 +368,9 @@ struct IndexBase {
   }
 
   // ---- binary indexes (B200VS_BINARY_FLAT / B200VS_BINARY_IVF_FLAT, binary.cu): rows are packed bits, dim / 8 bytes each.
-  // A float index refuses these, and the float entry points refuse a binary index (b200vs_*_binary, api.cu).
+  // The float entry points refuse a binary index, and the b200vs_*_binary ones a float index (api.cu).
   bool binary() const { return type == B200VS_BINARY_FLAT || type == B200VS_BINARY_IVF_FLAT; }
   size_t query_row_bytes() const { return binary() ? (size_t)dim / 8 : (size_t)dim * 4; }  // one host query row
-  virtual void train_binary(int64_t n, const uint8_t* x) { (void)n; (void)x; fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index"); }
-  virtual void add_binary(int64_t n, const uint8_t* x, const int64_t* ids, bool upsert) {
-    (void)n; (void)x; (void)ids; (void)upsert;
-    fail(B200VS_EILLEGAL_PARAMETERS, "binary entry point on a float index");
-  }
 
   virtual void reconstruct(int64_t n, const int64_t* ids, float* out, uint8_t* found) {
     (void)n; (void)ids; (void)out; (void)found;
@@ -382,6 +389,16 @@ struct IndexBase {
   virtual void load(const std::string& path);
 
   // helpers shared by the index types
+  // An AddReq's rows and ids on this device and its ids on the host, with the writer hold taken.  Host rows (row_bytes each)
+  // and ids are uploaded to the scratch on the index stream, ids the caller did not give on the host are downloaded, and
+  // device rows are copied to the scratch only when `own` asks for rows the add may change in place.
+  struct Staged {
+    void* x = nullptr;  // the scratch copy, or the caller's device rows, which are only read
+    const long long* ids_dev = nullptr;
+    const int64_t* ids = nullptr;
+    std::vector<int64_t> ids_buf;
+  };
+  void stage(const AddReq& r, size_t row_bytes, bool own, Staged& st);
   const float* prepare_queries(int64_t nq, const float* xq_dev, cudaStream_t s);  // cosine -> normalised copy
   const float* queries(const SearchReq& r, cudaStream_t s) { return r.prepared ? r.fq() : prepare_queries(r.nq, r.fq(), s); }
   // the refusal of a caller's probe table by a type without inverted lists to probe
@@ -405,6 +422,18 @@ struct RwSharedGuard {
   ~RwSharedGuard() { tl_held = prev; }
   RwSharedGuard(const RwSharedGuard&) = delete;
   RwSharedGuard& operator=(const RwSharedGuard&) = delete;
+};
+
+// The writer prologue: rw exclusively, then gpu_mu, the index's device, every earlier search finished and the scratch reset
+// on the index stream.  Every write of an index (add, remove, train, clear, reserve, trained state) runs under one.
+struct WriteHold {
+  std::unique_lock<std::shared_mutex> wl;
+  std::lock_guard<std::mutex> gl;
+  explicit WriteHold(IndexBase* ix) : wl(ix->rw), gl(ix->gpu_mu) {
+    ix->set_device();
+    ix->quiesce();
+    ix->scratch.reset(ix->stream);
+  }
 };
 
 // RAII: pick a lane for a search on stream `s` (nullptr = a lane-owned stream), lock it, make it the thread's scratch
@@ -511,8 +540,6 @@ void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, i
 void launch_pair_hamming(const uint32_t* a, int64_t nl, const uint32_t* b, int64_t nr, int w, float* out, cudaStream_t s);
 // packed binary rows [n, nbytes] -> zero-padded 32-bit words [n, ceil(nbytes / 4)] (binary.cu)
 void launch_pad_rows(const uint8_t* src, int64_t n, int nbytes, uint32_t* dst, cudaStream_t s);
-// b200vs_hnsw_add_batched (hnsw.cu); ix must be an HNSW index
-void hnsw_add_batched(IndexBase* ix, int64_t n, const float* x, const int64_t* ids, int batch);
 void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes);  // b200vs_debug_hnsw_build_scratch_limit
 void launch_merge_api(int nparts, int64_t nq, int k, const float* pd, const long long* pi, float* od, long long* oi,
                       cudaStream_t s);

@@ -243,6 +243,21 @@ struct IvfLists {
     upload(store.ix->stream);
   }
 
+  // the inverted list of each of n rows an add places, on the device (returned) and in h_list: the caller's device lists,
+  // or (lists null) those assign(out) writes, the nearest; on the owner's stream
+  template <class Assign>
+  static const long long* row_lists(IndexBase* ix, int64_t n, const long long* lists, std::vector<long long>& h_list, Assign assign) {
+    if (!lists) {
+      long long* out = ix->scratch.alloc<long long>(n);
+      assign(out);
+      lists = out;
+    }
+    h_list.resize(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists, (size_t)n * 8, cudaMemcpyDeviceToHost, ix->stream));
+    B200VS_CUDA(cudaStreamSynchronize(ix->stream));
+    return lists;
+  }
+
   // faiss remove_ids(IDSelectorBatch): every row whose id matches becomes a tombstone; returns how many
   template <class Store>
   int64_t remove(int64_t n, const int64_t* del, Store& store) {

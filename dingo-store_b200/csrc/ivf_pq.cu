@@ -482,9 +482,7 @@ struct IvfPqIndex : IndexBase {
 
   // blob: int64 hdr[6] = {magic 'IVPQ', nlist, dim, metric, M, nbits}; centroids[nlist*dim]; codebooks[M*2^nbits*dsub]
   void set_state(const void* blob, size_t len) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
+    WriteHold hold(this);
     if (len < 48) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
     const int64_t* hdr = (const int64_t*)blob;
     if (hdr[0] != 0x51505649 || hdr[2] != dim || hdr[4] != M) fail(B200VS_EILLEGAL_PARAMETERS, "bad IVF-PQ state blob");
@@ -523,24 +521,16 @@ struct IvfPqIndex : IndexBase {
   }
 
   // VectorIndexIvfPq::Train (ivf_pq.cc:327-395) + VectorIndexRawIvfPq::Train (raw_ivf_pq.cc:457-500)
-  void train(int64_t n, const float* x) override {
+  void train(int64_t n, const void* xv) override {
     if (n <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "data size invalid");
-    {
-      std::unique_lock<std::shared_mutex> wl(rw);
-      if (mode != kNone) return;
-      const int64_t need = std::max<int64_t>(256LL * nlist, 256LL * ksub);
-      if (n < need) {  // inner index = Flat
-        flat.reset(make_flat(metric, dim, params));
-        mode = kFlat;
-        return;
-      }
+    WriteHold hold(this);
+    if (mode != kNone) return;
+    if (n < train_need()) {  // inner index = Flat
+      flat.reset(make_flat(metric, dim, params));
+      mode = kFlat;
+      return;
     }
-    std::unique_lock<std::shared_mutex> wl(rw);
-    if (mode != kNone) return;  // another caller trained while the lock was released
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
+    const float* x = static_cast<const float*>(xv);
     std::vector<float> cent, cb;
     train_coarse_locked(n, x, nlist, cent);
     train_codebooks_locked(n, x, cent, cb);
@@ -571,12 +561,8 @@ struct IvfPqIndex : IndexBase {
     if (n == 0) return 0;
     const float* x = reinterpret_cast<const float*>(rows.p);
     if (n < train_need()) {
-      std::vector<int64_t> h_ids(n);
-      B200VS_CUDA(cudaMemcpy(h_ids.data(), ids.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
       std::unique_ptr<IndexBase> f(make_flat(metric, dim, params));
-      f->loading = true;  // stored rows: not normalised again
-      f->add_rows_dev(n, x, ids.p, h_ids.data());
-      f->loading = false;
+      f->add(AddReq::device(n, x, ids.p, nullptr, false, AddReq::PREPARED));
       flat = std::move(f);
       mode = kFlat;
       train_rows = n;
@@ -589,12 +575,11 @@ struct IvfPqIndex : IndexBase {
     install(cent.data(), cb.data());
     train_rows = n;
     scratch.reset(stream);
-    add_dev_locked(n, x, ids.p, nullptr, false, true, wpb);
+    add_locked(AddReq::device(n, x, ids.p, nullptr, false, AddReq::PREPARED), wpb);
     return n;
   }
 
-  // The two stages of train, also run separately by the list-sharded trainer (shard.cu).  Callers hold rw and gpu_mu, with
-  // the scratch reset.  x: raw host rows, or (x_dev) prepared rows on the device.  Coarse stage: k centroids of the n rows
+  // The two stages of train, also run separately by the list-sharded trainer (shard.cu).  Callers take the writer hold.  x: raw host rows, or (x_dev) prepared rows on the device.  Coarse stage: k centroids of the n rows
   // (level-1 quantiser, niter 10).
   void train_coarse_locked(int64_t n, const float* x, int k, std::vector<float>& cent, bool x_dev = false) {
     const bool l2 = metric == B200VS_L2;
@@ -655,17 +640,6 @@ struct IvfPqIndex : IndexBase {
       memcpy(&cb[(size_t)mm * ksub * dsub], cbm.data(), (size_t)ksub * dsub * 4);
     }
   }
-  // runs f with rw and gpu_mu held and the scratch reset, as train does
-  template <class F>
-  void locked_stage(F&& f) {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    f();
-  }
-
   // the list-building calls (device write path, coarse slices, caller-supplied probes) need the IVF-PQ mode's lists
   void require_lists() const {
     if (mode == kFlat) fail(B200VS_EVECTOR_NOT_SUPPORT, "an IVF_PQ index in inner-Flat mode (too few training rows) has no inverted lists");
@@ -696,82 +670,30 @@ struct IvfPqIndex : IndexBase {
     return st_codes;
   }
 
-  void add(int64_t n, const float* x, const int64_t* in_ids, bool upsert) override {
-    if (mode == kFlat) { flat->add(n, x, in_ids, upsert); return; }
-    std::unique_lock<std::shared_mutex> wl(rw);
-    if (mode == kNone) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
-    const int wpb = encode_warps();
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    if (upsert) L.remove(n, in_ids, store);
-    float* st = scratch.alloc<float>((size_t)n * dim);
-    long long* st_ids = scratch.alloc<long long>(n);
-    long long* st_list = scratch.alloc<long long>(n);
-    B200VS_CUDA(cudaMemcpyAsync(st, x, (size_t)n * dim * 4, cudaMemcpyHostToDevice, stream));
-    B200VS_CUDA(cudaMemcpyAsync(st_ids, in_ids, (size_t)n * 8, cudaMemcpyHostToDevice, stream));
-    if (metric == B200VS_COSINE) launch_normalize_faiss(st, n, dim, stream);
-    assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, st_list, stream);
-    const unsigned char* st_codes = encode_locked(n, st, st_list, wpb);
-    std::vector<long long> h_list(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    L.place(n, h_list.data(), in_ids, st_codes, st_ids, store);
-  }
-
-  // b200vs_add_with_ids_device: the host add's steps on device rows (upsert removes first; cosine rows are normalised on
-  // a copy unless `prepared`; lists_dev NULL = nearest centroid), so codes, ids and list layout equal a host add's
-  void add_dev(int64_t n, const void* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
+  // Inner-Flat mode takes host rows only (the inner index has no inverted lists); otherwise upsert removes first, then the rows are normalised for cosine (RAW), assigned to
+  // the caller's lists or the nearest ones, encoded and placed, or placed as given (ENCODED), so that codes, ids and list
+  // layout do not depend on the route
+  void add(const AddReq& r) override {
+    if (mode == kFlat && !r.on_device) { flat->add(r); return; }
+    WriteHold hold(this);
     require_lists();
-    const int wpb = encode_warps();
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    add_dev_locked(n, static_cast<const float*>(x_dev), ids_dev, lists_dev, upsert, prepared, wpb);
+    add_locked(r, r.form == AddReq::ENCODED ? 0 : encode_warps());
   }
-  // add_dev's steps with rw and gpu_mu held and the scratch reset; wpb = encode_warps()
-  void add_dev_locked(int64_t n, const float* x_dev, const long long* ids_dev, const long long* lists_dev, bool upsert, bool prepared, int wpb) {
-    std::vector<int64_t> h_ids(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    if (upsert) L.remove(n, h_ids.data(), store);
-    const float* st = x_dev;
-    if (metric == B200VS_COSINE && !prepared) {  // the normaliser works in place: keep the caller's rows intact
-      float* cp = scratch.alloc<float>((size_t)n * dim);
-      B200VS_CUDA(cudaMemcpyAsync(cp, x_dev, (size_t)n * dim * 4, cudaMemcpyDeviceToDevice, stream));
-      launch_normalize_faiss(cp, n, dim, stream);
-      st = cp;
-    }
-    const long long* st_list = lists_dev;
-    if (!st_list) {
-      long long* tmp = scratch.alloc<long long>(n);
-      assign_dev(centroids.p, nlist, cent_ids.p, st, dim, metric == B200VS_L2, n, tmp, stream);
-      st_list = tmp;
-    }
-    std::vector<long long> h_list(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), st_list, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    L.check_lists(n, h_list.data());  // before the encoder reads the lists' centroids
-    const unsigned char* st_codes = encode_locked(n, st, st_list, wpb);
-    L.place(n, h_list.data(), h_ids.data(), st_codes, ids_dev, store);
-  }
-
-  void add_codes_dev(int64_t n, const uint8_t* codes_dev, const long long* ids_dev, const long long* lists_dev) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
-    require_lists();
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
-    std::vector<int64_t> h_ids(n);
-    std::vector<long long> h_list(n);
-    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaMemcpyAsync(h_list.data(), lists_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
-    B200VS_CUDA(cudaStreamSynchronize(stream));
-    L.place(n, h_list.data(), h_ids.data(), codes_dev, ids_dev, store);
+  // add with the writer hold taken; wpb = encode_warps()
+  void add_locked(const AddReq& r, int wpb) {
+    const bool encoded = r.form == AddReq::ENCODED, normalise = metric == B200VS_COSINE && r.form == AddReq::RAW;
+    Staged st;
+    stage(r, encoded ? (size_t)code_size : (size_t)dim * 4, normalise, st);
+    if (r.upsert) L.remove(r.n, st.ids, store);
+    const float* x = static_cast<const float*>(st.x);
+    if (normalise) launch_normalize_faiss(static_cast<float*>(st.x), r.n, dim, stream);
+    std::vector<long long> h_list;
+    const long long* lists = IvfLists::row_lists(this, r.n, r.lists, h_list, [&](long long* out) {
+      assign_dev(centroids.p, nlist, cent_ids.p, x, dim, metric == B200VS_L2, r.n, out, stream);
+    });
+    L.check_lists(r.n, h_list.data());  // before the encoder reads the lists' centroids
+    const unsigned char* codes = encoded ? static_cast<const unsigned char*>(st.x) : encode_locked(r.n, x, lists, wpb);
+    L.place(r.n, h_list.data(), st.ids, codes, st.ids_dev, store);
   }
 
   // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
@@ -781,22 +703,15 @@ struct IvfPqIndex : IndexBase {
   }
 
   void reserve_lists(const int64_t* rows_per_list, int n_lists) override {
-    std::unique_lock<std::shared_mutex> wl(rw);
+    WriteHold hold(this);
     require_lists();
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
     L.reserve(rows_per_list, n_lists, store);
   }
 
   int64_t remove(int64_t n, const int64_t* del) override {
     if (mode == kFlat) { const int64_t r = flat->remove(n, del); return r == 0 ? -1 : r; }  // Flat semantics: unknown ids are OK
-    std::unique_lock<std::shared_mutex> wl(rw);
+    WriteHold hold(this);
     if (mode == kNone) return -1;
-    std::lock_guard<std::mutex> gl(gpu_mu);
-    set_device();
-    quiesce();
-    scratch.reset(stream);
     const int64_t r = L.remove(n, del, store);
     L.compact_if_needed(store);
     return r;
@@ -986,11 +901,8 @@ struct IvfPqIndex : IndexBase {
         std::vector<float> vec((size_t)n * dim);
         rd(fids.data(), fids.size() * 8); rd(vec.data(), vec.size() * 4);
         { std::unique_lock<std::shared_mutex> wl(rw); flat.reset(make_flat(metric, dim, params)); mode = kFlat; }
-        flat->loading = true;  // rows come back exactly as stored (already normalised for cosine)
-        try {
-          for (int64_t a = 0; a < n; a += 32768) flat->add(std::min<int64_t>(32768, n - a), vec.data() + (size_t)a * dim, fids.data() + a, false);
-        } catch (...) { flat->loading = false; throw; }
-        flat->loading = false;
+        for (int64_t a = 0; a < n; a += 32768)  // the rows come back exactly as stored
+          flat->add(AddReq::host(std::min<int64_t>(32768, n - a), vec.data() + (size_t)a * dim, fids.data() + a, false, AddReq::PREPARED));
       } else if (hdr[1] == kIvfPq) {
         std::vector<unsigned char> st((size_t)hdr[7]);
         rd(st.data(), st.size());
@@ -1001,10 +913,7 @@ struct IvfPqIndex : IndexBase {
         std::vector<uint8_t> cds((size_t)n * code_size);
         rd(off.data(), off.size() * 8); rd(fids.data(), fids.size() * 8); rd(cds.data(), cds.size());
         if (off[nlist] != n) fail(B200VS_EINTERNAL, "corrupt index file (list offsets)");
-        std::unique_lock<std::shared_mutex> wl(rw);
-        std::lock_guard<std::mutex> gl(gpu_mu);
-        set_device();
-        quiesce();
+        WriteHold hold(this);
         std::vector<long long> h_list((size_t)n);
         for (int l = 0; l < nlist; ++l) for (int64_t i = off[l]; i < off[l + 1]; ++i) h_list[(size_t)i] = l;
         for (int64_t a = 0; a < n; a += 262144) {
@@ -1043,13 +952,17 @@ int ivf_pq_ksub(IndexBase* ix) { return as_ivf_pq(ix)->ksub; }
 
 void ivf_pq_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent) {
   IvfPqIndex* p = as_ivf_pq(ix);
-  p->locked_stage([&] { p->train_coarse_locked(n, x, k, cent); });
+  WriteHold hold(p);
+  p->train_coarse_locked(n, x, k, cent);
 }
 
 void ivf_pq_train_state(IndexBase* ix, int64_t n, const float* x, const std::vector<float>& cent, std::vector<unsigned char>& blob) {
   IvfPqIndex* p = as_ivf_pq(ix);
   std::vector<float> cb;
-  p->locked_stage([&] { p->train_codebooks_locked(n, x, cent, cb); });
+  {
+    WriteHold hold(p);
+    p->train_codebooks_locked(n, x, cent, cb);
+  }
   const int64_t hdr[6] = {0x51505649, (int64_t)(cent.size() / p->dim), p->dim, (int64_t)p->metric, p->M, p->nbits};
   blob.resize(48 + (cent.size() + cb.size()) * 4);
   memcpy(blob.data(), hdr, 48);

@@ -928,13 +928,14 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
 // row travels PREPARED (normalised for cosine) with its list to the list's owner, which appends it there.  Row-sharded
 // (FLAT, HNSW): every row travels RAW to owner(id) (Flat and HNSW normalise cosine rows differently, so the owner's add
 // normalises), and the owner runs the single-index add on the rows it received, in arrival order (an HNSW graph depends on
-// it).  Before any rank changes anything, every owner checks its rows (check_add: a repeated id for FLAT, max_elements for
-// HNSW, nothing for the list types) and the statuses are all-gathered: every rank returns the first refusal in rank order,
-// or adds.  batched: b200vs_hnsw_add_batched with `batch`.  Rows are in the index's row format (FP32, or packed bits on the
-// binary types, which travel as they are: a binary row has no normalisation).
+// it).  Either way the owner makes one add of the device rows it received.  Before any rank changes anything, every owner
+// checks that add (check_add: a repeated id for FLAT, max_elements for HNSW, nothing for the list types) and the statuses
+// are all-gathered: every rank returns the first refusal in rank order, or adds.  batched: b200vs_hnsw_add_batched with
+// `batch`.  Rows are in the index's row format (FP32, or packed bits on the binary types, which travel as they are: a
+// binary row has no normalisation).
 void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long long* ids_dev, bool batched, int batch) {
   IndexBase* ix = sh->ix;
-  const int d = ix->dim, rb = (int)ix->query_row_bytes();
+  const int rb = (int)ix->query_row_bytes();
   cudaStream_t s = sh->ws;
   ix->set_device();
   Routed rv;
@@ -949,20 +950,13 @@ void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long l
   std::vector<int64_t> hid(sh->rows ? (size_t)rv.n : 0);  // the host ids check_add and the FLAT / HNSW adds take
   if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaStreamSynchronize(s));
+  AddReq req = AddReq::device(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, sh->rows ? AddReq::RAW : AddReq::PREPARED);
+  req.ids = sh->rows ? hid.data() : nullptr;
+  req.batched = batched;
+  req.batch = batch;
   // status agreement
-  check(agree(sh, attempt([&] { ix->check_add(rv.n, hid.data(), batched, batch); }), "shard add"));
-  if (!rv.n) return;
-  if (!sh->rows) {
-    ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
-  } else if (ix->type != B200VS_HNSW) {  // FLAT, BINARY_FLAT
-    ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data());
-  } else {
-    std::vector<float> hx((size_t)rv.n * d);  // the HNSW builders take host rows
-    B200VS_CUDA(cudaMemcpyAsync(hx.data(), rv.x.p, (size_t)rv.n * d * 4, cudaMemcpyDeviceToHost, s));
-    B200VS_CUDA(cudaStreamSynchronize(s));
-    if (batched) hnsw_add_batched(ix, rv.n, hx.data(), hid.data(), batch);
-    else ix->add(rv.n, hx.data(), hid.data(), false);
-  }
+  check(agree(sh, attempt([&] { ix->check_add(req); }), "shard add"));
+  if (rv.n) ix->add(req);
 }
 
 // upload of host rows (query_row_bytes() each) to the write stream, for the host-pointer variants of the collective adds
@@ -1411,19 +1405,7 @@ void shard_load_locked(b200vs_shard* sh, const std::string& prefix) {
     else route_rows(sh, n, d_rows.p, rb, d_ids.p, d_lists.p, ListOwner{sh->lists_per_rank()}, rv);
     B200VS_CUDA(cudaStreamSynchronize(s));  // the pinned buffer and the sent rows are reused next round
     check(agree(sh, attempt([&] {
-      if (!rv.n) return;
-      if (ix->type == B200VS_IVF_PQ) {
-        ix->add_codes_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p);
-      } else if (!sh->rows) {  // IVF_FLAT, BINARY_IVF_FLAT
-        ix->add_dev(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, true);
-      } else {  // FLAT, BINARY_FLAT
-        std::vector<int64_t> hid((size_t)rv.n);
-        B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
-        B200VS_CUDA(cudaStreamSynchronize(s));
-        ix->loading = true;  // rows come back exactly as stored (already normalised for cosine)
-        try { ix->add_rows_dev(rv.n, rv.x.p, rv.ids.p, hid.data()); } catch (...) { ix->loading = false; throw; }
-        ix->loading = false;
-      }
+      if (rv.n) ix->add(AddReq::device(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, AddReq::ENCODED));
     }), "shard load"));
   }
 }
