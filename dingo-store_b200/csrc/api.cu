@@ -691,6 +691,7 @@ int b200vs_scan_push(b200vs_scan* st, int64_t n, const float* x, const int64_t* 
     if (!x || !ids) fail(B200VS_EILLEGAL_PARAMETERS, "null tile");
     IndexBase* ix = st->flat;
     const size_t nk = (size_t)st->nq * st->k;
+    check_ids_nonnegative(n, ids);  // before the previous tile is cleared
     if (st->pushed > 0) ix->clear();
     ix->add(AddReq::host(n, x, ids));  // one temporary Flat index per tile, as the reference builds (vector_reader.cc:1937-1946)
     index_read(ix, st->s, st->has_sp ? &st->sp : nullptr, [&](const SearchCtx& sc, cudaStream_t s) {

@@ -174,7 +174,7 @@ struct BinaryFlatIndex : BinaryIndex {
     if (!r.ids) check_batch_ids_unique(r.n, st.ids);
     rowmap.add(r.n, pad(r.n, static_cast<const uint8_t*>(st.x), stream), st.ids_dev, st.ids);
   }
-  void check_add(const AddReq& r) override { check_batch_ids_unique(r.n, r.ids); }
+  void check_add(const AddReq& r) override { IndexBase::check_add(r); check_batch_ids_unique(r.n, r.ids); }
   // Delete (flat.cc:171-203): ids that are not present are ignored
   int64_t remove(int64_t n, const int64_t* del) override {
     WriteHold hold(this);
@@ -440,23 +440,21 @@ struct BinaryIvfIndex : BinaryIndex {
     if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");
     Staged st;
     stage(r, nb, false, st);
-    if (r.upsert) L.remove(r.n, st.ids, store);
-    place_locked(r.n, pad(r.n, static_cast<const uint8_t*>(st.x), stream), st.ids_dev, st.ids, r.lists);
+    place_locked(r.n, pad(r.n, static_cast<const uint8_t*>(st.x), stream), st.ids_dev, st.ids, r.lists, r.upsert);
   }
   // padded device rows st and ids st_ids (in_ids: the same on the host) to the tails of their lists: lists_dev, or (null) the
-  // nearest ones; the writer hold is taken
-  void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids, const long long* lists_dev = nullptr) {
+  // nearest ones, as an upsert (IvfLists::place) when upsert; the writer hold is taken
+  void place_locked(int64_t n, const uint32_t* st, const long long* st_ids, const int64_t* in_ids, const long long* lists_dev = nullptr,
+                    bool upsert = false) {
     std::vector<long long> h_list;
     IvfLists::row_lists(this, n, lists_dev, h_list, [&](long long* out) { assign_words(n, st, out, stream); });
-    L.place(n, h_list.data(), in_ids, st, st_ids, store);
+    L.place(n, h_list.data(), in_ids, st, st_ids, store, upsert);
   }
   // Delete (ivf_flat.cc:162-189): untrained -> OK; nothing removed -> EVECTOR_INVALID (api.cu)
   int64_t remove(int64_t n, const int64_t* del) override {
     WriteHold hold(this);
     if (!trained) return -1;
-    const int64_t r = L.remove(n, del, store);
-    L.compact_if_needed(store);
-    return r;
+    return L.remove(n, del, store);
   }
 
   // Search / RangeSearch (ivf_flat.cc:203-350): untrained -> empty results (:224-227); the range scan is the exact one

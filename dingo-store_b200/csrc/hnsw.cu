@@ -991,6 +991,7 @@ struct HnswIndex : IndexBase {
       B200VS_CUDA(cudaStreamSynchronize(stream));
       x = hx.data();
     }
+    check_ids_nonnegative(r.n, ids);
     if (r.batched) add_batched_locked(r.n, x, ids, r.batch, r.form != AddReq::RAW);
     else add_host_locked(r.n, x, ids, r.form != AddReq::RAW);
   }
@@ -1030,6 +1031,7 @@ struct HnswIndex : IndexBase {
   }
   // add's refusals (batched: the batched build's, for that batch size), which come before either changes anything
   void check_add(const AddReq& r) override {
+    IndexBase::check_add(r);
     RwSharedGuard rl(this);
     if (r.batched) batched_plan(r.n, r.batch);
     else if (G.n + r.n > max_element_limit) fail(B200VS_EINTERNAL, "upsert failed, exceeds max elements");

@@ -190,8 +190,31 @@ void IndexBase::load(const std::string& path) {
     rd(f, off.data(), off.size() * 8);
     rd(f, ids.data(), ids.size() * 8);
     rd(f, rows.data(), rows.size());
-    for (int64_t a = 0; a < h.count; a += 32768)  // the rows come back exactly as stored
-      add(AddReq::host(std::min<int64_t>(32768, h.count - a), rows.data() + (size_t)a * rb, ids.data() + a, false, AddReq::PREPARED));
+    // the rows come back exactly as stored, each into the list it was saved in (a row added to a caller's list need not
+    // be in its nearest list, so the lists are not assigned again)
+    std::vector<long long> h_list;
+    if (h.nlist > 1) {
+      if (off[0] != 0 || off[h.nlist] != h.count || !std::is_sorted(off.begin(), off.end())) fail(B200VS_EINTERNAL, "corrupt index file (list offsets)");
+      h_list.resize((size_t)h.count);
+      for (int l = 0; l < h.nlist; ++l) std::fill(h_list.begin() + off[l], h_list.begin() + off[l + 1], (long long)l);
+    }
+    DevBuf<unsigned char> dx;
+    DevBuf<long long> dids, dlist;
+    for (int64_t a = 0; a < h.count; a += 32768) {
+      const int64_t m = std::min<int64_t>(32768, h.count - a);
+      if (h_list.empty()) {
+        add(AddReq::host(m, rows.data() + (size_t)a * rb, ids.data() + a, false, AddReq::PREPARED));
+        continue;
+      }
+      set_device();
+      dx.reserve((size_t)m * rb, 0, stream); dids.reserve(m, 0, stream); dlist.reserve(m, 0, stream);
+      B200VS_CUDA(cudaMemcpy(dx.p, rows.data() + (size_t)a * rb, (size_t)m * rb, cudaMemcpyHostToDevice));
+      B200VS_CUDA(cudaMemcpy(dids.p, ids.data() + a, (size_t)m * 8, cudaMemcpyHostToDevice));
+      B200VS_CUDA(cudaMemcpy(dlist.p, h_list.data() + a, (size_t)m * 8, cudaMemcpyHostToDevice));
+      AddReq r = AddReq::device(m, dx.p, dids.p, dlist.p, false, AddReq::PREPARED);
+      r.ids = ids.data() + a;
+      add(r);
+    }
   } catch (...) { fclose(f); throw; }
   fclose(f);
 }
@@ -214,6 +237,7 @@ void IndexBase::stage(const AddReq& r, size_t row_bytes, bool own, Staged& st) {
     B200VS_CUDA(cudaStreamSynchronize(stream));
     st.ids = st.ids_buf.data();
   }
+  check_ids_nonnegative(r.n, st.ids);
 }
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids) {  // CheckVectorIdDuplicated, vector_index_utils.cc:551-561
@@ -340,7 +364,7 @@ struct FlatIndex : IndexBase {
     rowmap.add(r.n, static_cast<const float*>(st.x), st.ids_dev, st.ids);
   }
 
-  void check_add(const AddReq& r) override { check_batch_ids_unique(r.n, r.ids); }
+  void check_add(const AddReq& r) override { IndexBase::check_add(r); check_batch_ids_unique(r.n, r.ids); }
 
   // streaming brute-force scan (b200vs_scan_*): the tile index is emptied between tiles, buffers are kept
   void clear() override {
@@ -694,12 +718,11 @@ void IvfFlatIndex::add_locked(const AddReq& r) {
   const bool normalise = metric == B200VS_COSINE && r.form == AddReq::RAW;  // the normaliser works in place
   Staged st;
   stage(r, (size_t)dim * 4, normalise, st);
-  if (r.upsert) L.remove(r.n, st.ids, store);
   float* x = static_cast<float*>(st.x);
   if (normalise) launch_normalize_faiss(x, r.n, dim, stream);
   std::vector<long long> h_list;
   IvfLists::row_lists(this, r.n, r.lists, h_list, [&](long long* out) { assign_dev(x, r.n, out, stream); });
-  L.place(r.n, h_list.data(), st.ids, x, st.ids_dev, store);
+  L.place(r.n, h_list.data(), st.ids, x, st.ids_dev, store, r.upsert);
 }
 
 void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
@@ -712,9 +735,7 @@ void IvfFlatIndex::reserve_lists(const int64_t* rows_per_list, int n_lists) {
 int64_t IvfFlatIndex::remove(int64_t n, const int64_t* del) {
   WriteHold hold(this);
   if (!trained) return -1;  // signalled as OK by the ABI
-  const int64_t r = L.remove(n, del, store);
-  L.compact_if_needed(store);
-  return r;
+  return L.remove(n, del, store);
 }
 
 // VectorIndexIvfFlat::Search / RangeSearch, vector_index_ivf_flat.cc:203-350: untrained -> empty results (:224-227); range

@@ -30,6 +30,13 @@ struct StatusError {
 };
 [[noreturn]] inline void fail(int code, const std::string& m) { throw StatusError{code, m}; }
 
+// Vector ids are non-negative: every scan, the oracle and the shard merge read a negative id as a tombstone or an empty
+// result slot.  Every add refuses a batch holding one before it changes anything.
+inline void check_ids_nonnegative(int64_t n, const int64_t* ids) {
+  for (int64_t i = 0; i < n; ++i)
+    if (ids[i] < 0) fail(B200VS_EILLEGAL_PARAMETERS, "vector id is negative: " + std::to_string(ids[i]));
+}
+
 // The body of every extern "C" entry point: no exception leaves the library, each failure becomes a b200vs_status and
 // b200vs_last_error's text.
 template <class F>
@@ -323,8 +330,9 @@ struct IndexBase {
   // THE write of rows into an index, under the writer hold.  Each type refuses the requests it cannot serve.
   virtual void add(const AddReq& r) = 0;
   // the refusals add(r) would give, decided from r's host ids and sizes before anything changes, so that every rank of a
-  // collective add can agree on one status first (FLAT, BINARY_FLAT: a repeated id; HNSW: max_elements, the batched plan)
-  virtual void check_add(const AddReq& r) { (void)r; }
+  // collective add can agree on one status first (every type: a negative id; FLAT, BINARY_FLAT: a repeated id; HNSW:
+  // max_elements, the batched plan).  Overrides begin with this one.
+  virtual void check_add(const AddReq& r) { if (r.ids) check_ids_nonnegative(r.n, r.ids); }
   virtual int64_t remove(int64_t n, const int64_t* ids) = 0;
   virtual void clear() { fail(B200VS_EVECTOR_NOT_SUPPORT, "clear is only implemented for FLAT"); }  // drop every row, keep the buffers
   // THE read of an index, on stream s with the lane's scratch already reset: r's top-k or range search.  Each type refuses
@@ -391,7 +399,8 @@ struct IndexBase {
   // helpers shared by the index types
   // An AddReq's rows and ids on this device and its ids on the host, with the writer hold taken.  Host rows (row_bytes each)
   // and ids are uploaded to the scratch on the index stream, ids the caller did not give on the host are downloaded, and
-  // device rows are copied to the scratch only when `own` asks for rows the add may change in place.
+  // device rows are copied to the scratch only when `own` asks for rows the add may change in place.  A negative id is
+  // refused here, before the add changes anything.
   struct Staged {
     void* x = nullptr;  // the scratch copy, or the caller's device rows, which are only read
     const long long* ids_dev = nullptr;

@@ -10,8 +10,9 @@
 //
 // Inverted lists live in ONE device arena (rows of the payload array), list l owning rows
 // [off, off+len) with capacity cap >= len.  Appends go in place; a full list is relocated to the arena
-// tail with 1.5x capacity; removals tombstone the row (id = -1) and a compaction pass rebuilds the arena when
-// garbage + tombstones outweigh live rows.  Lists stay contiguous so the scan kernels stream them with
+// tail with 1.5x capacity; deletes and upserts tombstone the rows they replace (id = -1), and a write that tombstoned
+// rows ends with a compaction pass that rebuilds the arena when garbage + tombstones outweigh live rows.  Plain appends
+// never compact.  Lists stay contiguous so the scan kernels stream them with
 // 128-B coalesced loads / TMA tiles.  Replaces faiss::ArrayInvertedLists behind IndexIVFFlat/IndexIVFPQ
 // (constructed at src/vector/vector_index_ivf_flat.cc:809-816, vector_index_raw_ivf_pq.cc:554-564).
 #pragma once
@@ -200,9 +201,12 @@ struct IvfLists {
 
   // n rows go to the tails of their lists h_list: device rows x and ids ids_dev, the same ids on the host in h_ids_in.  A
   // list without room is relocated to the arena tail with 1.5x capacity, and the arena grows by 1.5x when that runs out.
+  // upsert: every row already holding one of the ids is tombstoned first, and the write ends as a delete does.
   template <class Store, class Row>
-  void place(int64_t n, const long long* h_list, const int64_t* h_ids_in, const Row* x, const long long* ids_dev, Store& store) {
+  void place(int64_t n, const long long* h_list, const int64_t* h_ids_in, const Row* x, const long long* ids_dev, Store& store,
+             bool upsert = false) {
     check_lists(n, h_list);
+    const int64_t replaced = upsert ? tombstone(n, h_ids_in, store) : 0;
     std::vector<int> need(lists.size(), 0);
     for (int64_t i = 0; i < n; ++i) need[h_list[i]]++;
     struct Rel { int64_t src, dst; int32_t len; };
@@ -241,6 +245,7 @@ struct IvfLists {
     live += n;
     store.write(x, ids_dev, slots);
     upload(store.ix->stream);
+    if (replaced) compact_if_needed(store);
   }
 
   // the inverted list of each of n rows an add places, on the device (returned) and in h_list: the caller's device lists,
@@ -260,7 +265,7 @@ struct IvfLists {
 
   // faiss remove_ids(IDSelectorBatch): every row whose id matches becomes a tombstone; returns how many
   template <class Store>
-  int64_t remove(int64_t n, const int64_t* del, Store& store) {
+  int64_t tombstone(int64_t n, const int64_t* del, Store& store) {
     std::vector<int64_t> rows;
     for (int64_t i = 0; i < n; ++i) {
       auto range = where.equal_range(del[i]);
@@ -279,9 +284,18 @@ struct IvfLists {
     tombstone_ids(store.ix, store.ids.p, rows);
     return (int64_t)rows.size();
   }
+  // a delete: the rows holding these ids become tombstones, then the arena is compacted if needed; returns how many
+  template <class Store>
+  int64_t remove(int64_t n, const int64_t* del, Store& store) {
+    const int64_t r = tombstone(n, del, store);
+    compact_if_needed(store);
+    return r;
+  }
 
-  // when garbage and tombstones outweigh the live rows: a fresh arena, list by list in list order, each list holding its
-  // live rows in order with room for 1/4 more + 32
+  // The end of every write that tombstones rows (remove, an upsert's place): when garbage and tombstones outweigh the live
+  // rows, a fresh arena, list by list in list order, each list holding its live rows in order with room for 1/4 more + 32.
+  // Plain appends do not come here: under them relocation garbage alone outgrows the live rows, and a compaction would
+  // only re-allocate the arena the appends are about to grow again.
   template <class Store>
   void compact_if_needed(Store& store) {
     if (garbage + dead <= std::max<int64_t>(live, 4096)) return;

@@ -670,9 +670,9 @@ struct IvfPqIndex : IndexBase {
     return st_codes;
   }
 
-  // Inner-Flat mode takes host rows only (the inner index has no inverted lists); otherwise upsert removes first, then the rows are normalised for cosine (RAW), assigned to
+  // Inner-Flat mode takes host rows only (the inner index has no inverted lists); otherwise the rows are normalised for cosine (RAW), assigned to
   // the caller's lists or the nearest ones, encoded and placed, or placed as given (ENCODED), so that codes, ids and list
-  // layout do not depend on the route
+  // layout do not depend on the route.  An upsert's placement first removes the rows holding its ids.
   void add(const AddReq& r) override {
     if (mode == kFlat && !r.on_device) { flat->add(r); return; }
     WriteHold hold(this);
@@ -684,7 +684,6 @@ struct IvfPqIndex : IndexBase {
     const bool encoded = r.form == AddReq::ENCODED, normalise = metric == B200VS_COSINE && r.form == AddReq::RAW;
     Staged st;
     stage(r, encoded ? (size_t)code_size : (size_t)dim * 4, normalise, st);
-    if (r.upsert) L.remove(r.n, st.ids, store);
     const float* x = static_cast<const float*>(st.x);
     if (normalise) launch_normalize_faiss(static_cast<float*>(st.x), r.n, dim, stream);
     std::vector<long long> h_list;
@@ -693,7 +692,7 @@ struct IvfPqIndex : IndexBase {
     });
     L.check_lists(r.n, h_list.data());  // before the encoder reads the lists' centroids
     const unsigned char* codes = encoded ? static_cast<const unsigned char*>(st.x) : encode_locked(r.n, x, lists, wpb);
-    L.place(r.n, h_list.data(), st.ids, codes, st.ids_dev, store);
+    L.place(r.n, h_list.data(), st.ids, codes, st.ids_dev, store, r.upsert);
   }
 
   // b200vs_assign_device: nearest centroid of prepared rows, ties to the smaller list id (the host add's assignment)
@@ -712,9 +711,7 @@ struct IvfPqIndex : IndexBase {
     if (mode == kFlat) { const int64_t r = flat->remove(n, del); return r == 0 ? -1 : r; }  // Flat semantics: unknown ids are OK
     WriteHold hold(this);
     if (mode == kNone) return -1;
-    const int64_t r = L.remove(n, del, store);
-    L.compact_if_needed(store);
-    return r;
+    return L.remove(n, del, store);
   }
 
   // VectorIndexIvfPq::Search (ivf_pq.cc:159-163: untrained -> empty results) and VectorIndexRawIvfPq::Search / RangeSearch

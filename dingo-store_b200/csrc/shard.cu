@@ -929,7 +929,7 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
 // (FLAT, HNSW): every row travels RAW to owner(id) (Flat and HNSW normalise cosine rows differently, so the owner's add
 // normalises), and the owner runs the single-index add on the rows it received, in arrival order (an HNSW graph depends on
 // it).  Either way the owner makes one add of the device rows it received.  Before any rank changes anything, every owner
-// checks that add (check_add: a repeated id for FLAT, max_elements for HNSW, nothing for the list types) and the statuses
+// checks that add (check_add: a negative id for every type, a repeated id for FLAT, max_elements for HNSW) and the statuses
 // are all-gathered: every rank returns the first refusal in rank order, or adds.  batched: b200vs_hnsw_add_batched with
 // `batch`.  Rows are in the index's row format (FP32, or packed bits on the binary types, which travel as they are: a
 // binary row has no normalisation).
@@ -947,11 +947,11 @@ void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long l
     const void* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
     route_rows(sh, n, xp, rb, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
   }
-  std::vector<int64_t> hid(sh->rows ? (size_t)rv.n : 0);  // the host ids check_add and the FLAT / HNSW adds take
+  std::vector<int64_t> hid((size_t)rv.n);  // the host ids check_add and the add take
   if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
   B200VS_CUDA(cudaStreamSynchronize(s));
   AddReq req = AddReq::device(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, sh->rows ? AddReq::RAW : AddReq::PREPARED);
-  req.ids = sh->rows ? hid.data() : nullptr;
+  req.ids = hid.data();
   req.batched = batched;
   req.batch = batch;
   // status agreement

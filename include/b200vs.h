@@ -98,7 +98,10 @@ int b200vs_set_trained_state(b200vs_index* idx, const void* blob, size_t len);
 int64_t b200vs_get_trained_state(b200vs_index* idx, void* blob, size_t cap); /* returns bytes needed/written, <0 on error */
 
 /* VectorIndex::Add / Upsert / Delete — flat.cc:121-203, ivf_flat.cc:92-190, hnsw.cc:203-281.
- * ids must be unique within one call (EVECTOR_ID_DUPLICATED); upsert=1 removes pre-existing ids first. */
+ * ids must be unique within one call (EVECTOR_ID_DUPLICATED); upsert=1 removes pre-existing ids first.
+ * Ids must be >= 0 on every index type and every add entry point (the device and sharded variants and b200vs_scan_push
+ * too): a batch holding a negative id is refused with EILLEGAL_PARAMETERS ("vector id is negative: <id>") before anything
+ * changes, since the scans read a negative id as a deleted row or an empty result slot. */
 int b200vs_add_with_ids(b200vs_index* idx, int64_t n, const float* x, const int64_t* ids, int upsert);
 int b200vs_remove_ids(b200vs_index* idx, int64_t n, const int64_t* ids, int64_t* n_removed);
 
