@@ -264,24 +264,31 @@ static __global__ void tc_items_kernel(const int* __restrict__ cnt, const int* _
 // tile loads.  Algorithmic HBM bytes per item: rows x (d*4 + 4 + 8) (vector, norm, id), or rows x (d*2 + 4 + 4 + 8) on the
 // mirror (+ scale), read exactly once.
 //
-// Two instantiations per operand type (TcCfg).  The capture / dense form is the one above.  The sample pass only ever
-// scores the first TC_SAMPLE rows of an item, so its form has one consumer warpgroup and a 3-stage ring of 32-row A boxes,
-// without capture staging: three of its CTAs share an SM, so three times as many items' start-up round trips overlap.
-// Both forms run the same per-row wgmma sequence and epilogue (tc_mma_tile / tc_consume_item) on stages that start on a
-// 1024-byte boundary, so a sampled score is bit for bit the score the capture pass computes for that (row, query).
+// One form per mode and operand type (TcCfg<MODE>).  The capture form (mode 1) is the one above.  The sample pass (mode 0)
+// only ever scores the first TC_SAMPLE rows of an item, so its form has one consumer warpgroup and a 3-stage ring of 32-row
+// A boxes, without capture staging: three of its CTAs share an SM, so three times as many items' start-up round trips
+// overlap.  The dense pass (mode 2: coarse quantiser, labelling, diagnostics) reads a small table from L2 item after item;
+// its form has one consumer warpgroup on 64-row tiles, query groups of at most TC_DENSE_NQT and a 4-stage ring (two split
+// K blocks), so three CTAs share an SM and the pass has three items per SM in flight instead of one.
+// All forms run the same per-row wgmma sequence and epilogue (tc_mma_tile / tc_consume_item) on stages that start on a
+// 1024-byte boundary, so a score does not depend on the form: a sampled score is bit for bit the score the capture pass
+// computes for that (row, query).
 // ---------------------------------------------------------------------------------------------
-template <bool SAMPLE>
+constexpr int TC_DENSE_NQT = 64;  // widest query group of the dense form (its B stage)
+
+template <int Mode>
 struct TcCfg {
-  static constexpr bool IS_SAMPLE = SAMPLE;      // mode 0 only; the other form runs modes 1 and 2
-  static constexpr int CWARPS = SAMPLE ? 4 : 8;  // consumer warps (one or two warpgroups); the producer is warp CWARPS
+  static constexpr int MODE = Mode;                 // 0 = sample, 1 = capture, 2 = dense (TcParams::mode)
+  static constexpr int CWARPS = MODE == 1 ? 8 : 4;  // consumer warps (one or two warpgroups); the producer is warp CWARPS
+  static constexpr int BM = CWARPS / 4 * 64;        // rows per tile: 64 per consumer warpgroup
   static constexpr int THREADS = CWARPS * 32 + 32;
-  static constexpr int MIN_CTAS = SAMPLE ? 3 : 1;  // CTAs per SM the launch bounds reserve registers for
+  static constexpr int MIN_CTAS = MODE == 1 ? 1 : 3;  // CTAs per SM the launch bounds reserve registers for
   // TMA -> MMA ring.  Capture: 6 x 32 KB (+ 24 KB of capture staging: ~220 KB; the bytes in flight bound the HBM rate,
-  // DESIGN §4.2).  Sample: 3 x (4 KB A box + 16 KB B tile) = 61 KB with the alignment slack.  Both strides are multiples
-  // of 1024, the period of the 128-byte swizzle.
-  static constexpr int STAGES = SAMPLE ? 3 : 6;
-  static constexpr uint32_t A_STAGE = SAMPLE ? TC_SAMPLE * 128 : TC_A_BYTES;
-  static constexpr uint32_t B_STAGE = TC_B_BYTES;
+  // DESIGN §4.2).  Sample: 3 x (4 KB A box + 16 KB B tile) = 61 KB with the alignment slack.  Dense: 4 x (8 KB A tile +
+  // 8 KB B tile) = 65 KB.  Every stride is a multiple of 1024, the period of the 128-byte swizzle.
+  static constexpr int STAGES = MODE == 1 ? 6 : (MODE == 0 ? 3 : 4);
+  static constexpr uint32_t A_STAGE = MODE == 0 ? TC_SAMPLE * 128 : BM * 128;
+  static constexpr uint32_t B_STAGE = MODE == 2 ? TC_DENSE_NQT * 128 : TC_B_BYTES;
   static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + 1024;
 };
 
@@ -310,7 +317,7 @@ __device__ __forceinline__ void tc_mma_tile(const TcParams& p, int kblocks, bool
     mbar_wait(&full_bar[s_hi], ring.phase);
     ring.next();
     int s_lo = 0;
-    const bool split = !HALF && !C::IS_SAMPLE && p.split;
+    const bool split = !HALF && C::MODE == 2 && p.split;
     if (split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
       s_lo = ring.stage;
       mbar_wait(&full_bar[s_lo], ring.phase);
@@ -358,8 +365,8 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
   const long long list_base = p.list_off[I.list];
   int rows = I.row_end - I.row_begin;
-  if constexpr (C::IS_SAMPLE) rows = min(rows, TC_SAMPLE);
-  const int ntiles = (rows + TC_BM - 1) / TC_BM;
+  if constexpr (C::MODE == 0) rows = min(rows, TC_SAMPLE);
+  const int ntiles = (rows + C::BM - 1) / C::BM;
   for (int t = 0; t < ntiles; ++t) {
     // row metadata first: its loads overlap the MMAs.  The id and norm loads do not depend on each other, and the masks
     // that read the id are applied after the MMAs, so no warp waits for a global round trip before its first wgmma
@@ -368,7 +375,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
     float nrm[2], hs[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int r = t * TC_BM + row0 + 8 * h;
+      const int r = t * C::BM + row0 + 8 * h;
       inrange[h] = r < rows;
       arow[h] = list_base + I.row_begin + r;
       id[h] = -1;
@@ -381,7 +388,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
       }
     }
     float acc[N / 2];
-    const bool mma = t * TC_BM + wg * 64 < rows;  // else this warpgroup's half of the last tile holds no item rows
+    const bool mma = t * C::BM + wg * 64 < rows;  // else this warpgroup's half of the last tile holds no item rows
     tc_mma_tile<HALF, N, C>(p, kblocks, mma, sA, sB, full_bar, empty_bar, ring, acc);
     if (!mma) continue;
 #pragma unroll
@@ -391,7 +398,7 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int r = t * TC_BM + row0 + 8 * h;  // row within the item
+      const int r = t * C::BM + row0 + 8 * h;  // row within the item
 #pragma unroll
       for (int j = 0; j < N / 8; ++j)
 #pragma unroll
@@ -402,9 +409,9 @@ __device__ __forceinline__ void tc_consume_item(const TcParams& p, const TcItem&
             // stay normal; below that they underflow (to 0 under 2^-149), which tc_eps's absolute term covers
             const float dot = HALF ? acc[4 * j + 2 * h + c] * (hs[h] * s_qs[n]) : acc[4 * j + 2 * h + c];
             const float score = p.l2 ? fmaf(-2.f, dot, nrm[h]) : -dot;
-            if constexpr (C::IS_SAMPLE) {
+            if constexpr (C::MODE == 0) {
               if (t == 0 && r < TC_SAMPLE) p.sample[((size_t)I.sample_slot * TC_NQT + n) * TC_SAMPLE + r] = valid[h] ? score : TC_INF;
-            } else if (p.mode == 1) {
+            } else if constexpr (C::MODE == 1) {
               if (valid[h] && score <= s_tau[n]) {
                 const int q = s_q[n];
                 const unsigned long long key = ((unsigned long long)f2ord(score) << 32) | (unsigned long long)(uint32_t)arow[h];
@@ -431,11 +438,11 @@ struct TcMaps {
   CUtensorMap a, a32, b[4], a_lo, b_lo[4];
 };
 
-// SAMPLE = true: the sample pass (mode 0) only; false: the capture (mode 1) and dense (mode 2) passes.
-template <bool HALF, bool SAMPLE>
-__global__ void __launch_bounds__(TcCfg<SAMPLE>::THREADS, TcCfg<SAMPLE>::MIN_CTAS)
+// MODE = the pass this form runs (TcParams::mode: 0 sample, 1 capture, 2 dense).
+template <bool HALF, int MODE>
+__global__ void __launch_bounds__(TcCfg<MODE>::THREADS, TcCfg<MODE>::MIN_CTAS)
 tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
-  using C = TcCfg<SAMPLE>;
+  using C = TcCfg<MODE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
@@ -448,14 +455,13 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   __shared__ float s_qs[2][TC_NQT];
   // capture staging, one buffer per consumer warp: hits are appended with a shared-memory atomic and written out
   // (one global atomicAdd per hit, a whole warp of them in flight) when the item ends, so the score loop never
-  // waits on a global round trip.  The sample form captures nothing and keeps a one-entry placeholder.
-  constexpr int HW = SAMPLE ? 1 : C::CWARPS, HN = SAMPLE ? 1 : TC_HITS;
+  // waits on a global round trip.  The other forms capture nothing and keep a one-entry placeholder.
+  constexpr int HW = MODE == 1 ? C::CWARPS : 1, HN = MODE == 1 ? TC_HITS : 1;
   __shared__ unsigned long long s_hit_key[HW][HN];
   __shared__ int s_hit_q[HW][HN];
   __shared__ int s_hit_n[HW];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mode = SAMPLE ? 0 : p.mode;
   if (threadIdx.x < HW) s_hit_n[threadIdx.x] = 0;
   if (warp == C::CWARPS && lane == 0) {
     prefetch_tmap(&maps.a); prefetch_tmap(&maps.a32);
@@ -465,7 +471,7 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
     fence_barrier_init();
   }
   __syncthreads();
-  const int nwork = mode == 0 ? p.totals[2] : p.totals[0];
+  const int nwork = MODE == 0 ? p.totals[2] : p.totals[0];
   const int kbk = HALF ? 2 * TC_BK : TC_BK;  // elements per K block (128 B)
   const int kblocks = (p.d + kbk - 1) / kbk;
 
@@ -476,7 +482,7 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
       for (;;) {
         mbar_wait(&sched_empty[slot], sphase ^ 1);
         const int w = atomicAdd(p.work_counter, 1);
-        const int it = w < nwork ? (mode == 0 ? p.sample_list[w] : w) : -1;
+        const int it = w < nwork ? (MODE == 0 ? p.sample_list[w] : w) : -1;
         s_sched[slot] = it;
         mbar_arrive(&sched_full[slot]);
         if (++slot == TC_SQ) { slot = 0; sphase ^= 1; }
@@ -484,21 +490,20 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
         const TcItem I = p.items[it];
         const long long base_row = p.list_off[I.list] + I.row_begin;
         int rows = I.row_end - I.row_begin;
-        if (mode == 0) rows = min(rows, TC_SAMPLE);
-        const int ntiles = (rows + TC_BM - 1) / TC_BM;
+        if (MODE == 0) rows = min(rows, TC_SAMPLE);
+        const int ntiles = (rows + C::BM - 1) / C::BM;
         const int bl = tc_bcols_log(I.nq);
         const CUtensorMap* tb = &maps.b[bl];
-        const bool small_a = mode == 0;  // 32-row sample box, else the full 128-row tile
-        const CUtensorMap* ta = small_a ? &maps.a32 : &maps.a;
-        const uint32_t bytes = (small_a ? (uint32_t)(TC_SAMPLE * 128) : TC_A_BYTES) + (16u << bl) * 128u;
+        const CUtensorMap* ta = MODE == 0 ? &maps.a32 : &maps.a;  // 32-row sample box, else the whole C::BM-row tile
+        const uint32_t bytes = C::A_STAGE + (16u << bl) * 128u;
         const CUtensorMap* tbl = &maps.b_lo[bl];
         for (int t = 0; t < ntiles; ++t)
           for (int kb = 0; kb < kblocks; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             // last tile of a list: fetch only the 32-row boxes that hold list rows (the rest of the stage keeps stale
             // data, whose scores the epilogue masks) instead of streaming up to 127 rows of the neighbouring list
-            const int trows = rows - t * TC_BM;
-            const int nbox = (mode == 1 && (HALF || !p.split) && trows <= TC_BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
+            const int trows = rows - t * C::BM;
+            const int nbox = (MODE == 1 && trows <= C::BM - TC_SAMPLE) ? (trows + TC_SAMPLE - 1) / TC_SAMPLE : 0;
             const uint32_t saved = nbox ? TC_A_BYTES - (uint32_t)nbox * (TC_SAMPLE * 128) : 0u;
             mbar_arrive_expect_tx(&full_bar[stage], bytes - saved);
             if (nbox) {
@@ -506,13 +511,13 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
                 tma_load_2d(sA + (size_t)stage * C::A_STAGE + (size_t)j * (TC_SAMPLE * 128), &maps.a32, &full_bar[stage], kb * kbk,
                             (int)(base_row + (long long)t * TC_BM + j * TC_SAMPLE), kEvictFirst);
             } else
-            tma_load_2d(sA + (size_t)stage * C::A_STAGE, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+            tma_load_2d(sA + (size_t)stage * C::A_STAGE, ta, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * C::BM), kEvictFirst);
             tma_load_2d(sB + (size_t)stage * C::B_STAGE, tb, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
             if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            if (!HALF && !SAMPLE && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
+            if (!HALF && MODE == 2 && p.split) {  // error-compensated pass: the "lo" operands ride in the next ring stage
               mbar_wait(&empty_bar[stage], phase ^ 1);
               mbar_arrive_expect_tx(&full_bar[stage], bytes);
-              tma_load_2d(sA + (size_t)stage * C::A_STAGE, &maps.a_lo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * TC_BM), kEvictFirst);
+              tma_load_2d(sA + (size_t)stage * C::A_STAGE, &maps.a_lo, &full_bar[stage], kb * kbk, (int)(base_row + (long long)t * C::BM), kEvictFirst);
               tma_load_2d(sB + (size_t)stage * C::B_STAGE, tbl, &full_bar[stage], kb * kbk, I.pair_begin, kEvictLast);
               if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
@@ -538,11 +543,11 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
     if (et < I.nq) {
       const int q = p.pair_query ? p.pair_query[I.pair_begin + et] : I.pair_begin + et;
       s_q[buf][et] = q;
-      s_tau[buf][et] = mode == 1 ? p.tau[q] : 0.f;
+      s_tau[buf][et] = MODE == 1 ? p.tau[q] : 0.f;
       if (HALF) s_qs[buf][et] = p.qscale[q];
     }
     asm volatile("bar.sync 1, %0;" ::"n"(C::CWARPS * 32) : "memory");
-    const int hw = SAMPLE ? 0 : warp;
+    const int hw = MODE == 1 ? warp : 0;
     auto consume = [&](auto n) {
       tc_consume_item<HALF, decltype(n)::value, C>(p, I, kblocks, sA, sB, full_bar, empty_bar, ring, s_tau[buf], s_q[buf], s_qs[buf],
                                                    s_hit_key[hw], s_hit_q[hw], &s_hit_n[hw]);
@@ -550,9 +555,9 @@ tc_scan_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
     const int bl = tc_bcols_log(I.nq);
     if (bl == 0) consume(std::integral_constant<int, 16>());
     else if (bl == 1) consume(std::integral_constant<int, 32>());
-    else if (bl == 2) consume(std::integral_constant<int, 64>());
-    else consume(std::integral_constant<int, 128>());
-    if (mode == 1) {  // flush this warp's staged hits
+    else if (MODE == 2 || bl == 2) consume(std::integral_constant<int, 64>());  // the dense form's groups stop at 64
+    else if constexpr (MODE != 2) consume(std::integral_constant<int, 128>());
+    if constexpr (MODE == 1) {  // flush this warp's staged hits
       __syncwarp();
       const int nh = min(s_hit_n[hw], TC_HITS);
       for (int i = lane; i < nh; i += 32) {
@@ -1272,13 +1277,14 @@ static CUtensorMap make_tmap(const void* base, int64_t rows, int d, int box_rows
   return m;
 }
 
-// A = the rows [a_rows, d], B = the query block [b_rows, d]; FP16 when half (the optional lo operands are always FP32)
-static TcMaps make_tc_maps(const void* a, const float* a_lo, int64_t a_rows, const void* b, const float* b_lo, int64_t b_rows, int d,
-                           bool half) {
+// A = the rows [a_rows, d] in a_box-row tiles (the form's TcCfg::BM), B = the query block [b_rows, d]; FP16 when half (the
+// optional lo operands are always FP32)
+static TcMaps make_tc_maps(const void* a, const float* a_lo, int64_t a_rows, int a_box, const void* b, const float* b_lo,
+                           int64_t b_rows, int d, bool half) {
   TcMaps m;
-  m.a = make_tmap(a, a_rows, d, TC_BM, half);
+  m.a = make_tmap(a, a_rows, d, a_box, half);
   m.a32 = make_tmap(a, a_rows, d, TC_SAMPLE, half);
-  m.a_lo = a_lo ? make_tmap(a_lo, a_rows, d, TC_BM) : m.a;
+  m.a_lo = a_lo ? make_tmap(a_lo, a_rows, d, a_box) : m.a;
   for (int i = 0; i < 4; ++i) {
     m.b[i] = make_tmap(b, b_rows, d, 16 << i, half);
     m.b_lo[i] = b_lo ? make_tmap(b_lo, b_rows, d, 16 << i) : m.b[i];
@@ -1301,19 +1307,22 @@ constexpr int TC_MAX_DEVICES = 64;
 struct TcDevice {
   int sms = 0;
   int sample_ctas[2] = {0, 0};  // resident CTAs per SM of the sample form, [HALF]
+  int dense_ctas[2] = {0, 0};   // ... and of the dense form
 };
 static std::mutex g_tc_init_mu;
 static TcDevice g_tc_dev[TC_MAX_DEVICES];
 
-template <bool HALF>
-static int tc_sample_ctas_per_sm() {
-  using C = TcCfg<true>;
-  auto* kernel = tc_scan_kernel<HALF, true>;
+// the sample and dense forms: several CTAs per SM
+template <bool HALF, int MODE>
+static int tc_ctas_per_sm() {
+  using C = TcCfg<MODE>;
+  auto* kernel = tc_scan_kernel<HALF, MODE>;
   B200VS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
   B200VS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
   int n = 0;
   B200VS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, C::THREADS, C::SMEM));
-  if (getenv("B200VS_DEBUG_FLAGS")) fprintf(stderr, "[b200vs] tc sample kernel (%s): %d CTAs per SM\n", HALF ? "fp16" : "tf32", n);
+  if (getenv("B200VS_DEBUG_FLAGS"))
+    fprintf(stderr, "[b200vs] tc %s kernel (%s): %d CTAs per SM\n", MODE == 0 ? "sample" : "dense", HALF ? "fp16" : "tf32", n);
   return std::max(1, n);
 }
 
@@ -1323,10 +1332,12 @@ static TcDevice tc_init(int device) {
   if (g_tc_dev[device].sms) return g_tc_dev[device];
   TcDevice dev;
   dev.sms = device_sm_count(device);
-  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<false>::SMEM));
-  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<false>::SMEM));
-  dev.sample_ctas[0] = tc_sample_ctas_per_sm<false>();
-  dev.sample_ctas[1] = tc_sample_ctas_per_sm<true>();
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<1>::SMEM));
+  B200VS_CUDA(cudaFuncSetAttribute(tc_scan_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcCfg<1>::SMEM));
+  dev.sample_ctas[0] = tc_ctas_per_sm<false, 0>();
+  dev.sample_ctas[1] = tc_ctas_per_sm<true, 0>();
+  dev.dense_ctas[0] = tc_ctas_per_sm<false, 2>();
+  dev.dense_ctas[1] = tc_ctas_per_sm<true, 2>();
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
   B200VS_CUDA(cudaFuncSetAttribute(tc_final_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));  // + static smem
@@ -1435,7 +1446,7 @@ static TcPlan tc_prepare(IndexBase* ix, const TcView& v, int64_t nq, const float
   P.qry = tc_round_queries(ix, P.half ? TC_ARITH_FP16 : TC_ARITH_TF32, nq, q, s);
   static_cast<TcPairs&>(P) = tc_plan_pairs(ix, v, nq, probes, nprobe, P.qry.op, d * esz, s);
   const void* rows = P.half ? static_cast<const void*>(v.vecs_h) : static_cast<const void*>(v.vecs);
-  P.maps = make_tc_maps(rows, nullptr, v.arena_rows, P.bws, nullptr, P.npairs + TC_NQT, d, P.half);
+  P.maps = make_tc_maps(rows, nullptr, v.arena_rows, TcCfg<1>::BM, P.bws, nullptr, P.npairs + TC_NQT, d, P.half);
   ix->launch_count(1);
   return P;
 }
@@ -1449,20 +1460,22 @@ static TcParams tc_params(const TcView& v, int d, bool l2, const TcItem* items, 
   return p;
 }
 
-// One persistent launch of the tile kernel, at most one CTA per work item: the sample pass (mode 0) runs the sample form
-// with as many CTAs per SM as fit, the other passes one capture-form CTA per SM.  All CTAs draw items from the same
-// work counter, so a loose work_bound (a host-side bound on the item count) costs no more than one empty claim per CTA.
+// One persistent launch of the tile kernel in the form of p.mode, at most one CTA per work item: the sample (mode 0) and
+// dense (mode 2) forms with as many CTAs per SM as fit, the capture form (mode 1) one CTA per SM.  All CTAs draw items
+// from the same work counter, so a loose work_bound (a host-side bound on the item count) costs no more than one empty
+// claim per CTA.
+template <int MODE>
+static void tc_launch_form(int ctas_per_sm, const TcDevice& dev, bool half, int64_t work_bound, const TcMaps& maps, const TcParams& p,
+                           cudaStream_t s) {
+  const int grid = (int)std::min<int64_t>((int64_t)dev.sms * ctas_per_sm, std::max<int64_t>(1, work_bound));
+  auto* kernel = half ? tc_scan_kernel<true, MODE> : tc_scan_kernel<false, MODE>;
+  kernel<<<grid, TcCfg<MODE>::THREADS, TcCfg<MODE>::SMEM, s>>>(maps, p);
+}
 static void tc_launch(const TcDevice& dev, bool half, int64_t work_bound, const TcMaps& maps, const TcParams& p, cudaStream_t s) {
-  const bool sample = p.mode == 0;
-  const int64_t slots = (int64_t)dev.sms * (sample ? dev.sample_ctas[half ? 1 : 0] : 1);
-  const int grid = (int)std::min<int64_t>(slots, std::max<int64_t>(1, work_bound));
-  if (sample) {
-    auto* kernel = half ? tc_scan_kernel<true, true> : tc_scan_kernel<false, true>;
-    kernel<<<grid, TcCfg<true>::THREADS, TcCfg<true>::SMEM, s>>>(maps, p);
-  } else {
-    auto* kernel = half ? tc_scan_kernel<true, false> : tc_scan_kernel<false, false>;
-    kernel<<<grid, TcCfg<false>::THREADS, TcCfg<false>::SMEM, s>>>(maps, p);
-  }
+  const int h = half ? 1 : 0;
+  if (p.mode == 0) tc_launch_form<0>(dev.sample_ctas[h], dev, half, work_bound, maps, p, s);
+  else if (p.mode == 1) tc_launch_form<1>(1, dev, half, work_bound, maps, p, s);
+  else tc_launch_form<2>(dev.dense_ctas[h], dev, half, work_bound, maps, p, s);
   B200VS_CUDA(cudaGetLastError());
 }
 
@@ -1635,15 +1648,18 @@ static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, c
   const int nrows = (int)v.arena_rows;
   const bool half = hscale != nullptr;
   auto& S = ix->scratch;
-  const int chunk = nrows <= 16384 ? TC_BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
-  // Query-group width (the wgmma N): with every item MMA-bound, the launch takes about (waves of items over the SMs) x
-  // (width).  Take the widest group that minimises that product: at 1024 centroids x 1024 queries on 132 SMs, 128 items of
-  // 64 queries instead of 64 items of 128 (half the chip idle).  Narrower ties (256 items of 32) re-read the row tiles from
-  // L2 twice as often for no less MMA time.  A score does not depend on the width: each element's K order is the same.
-  int nqt = TC_NQT;
+  using C = TcCfg<2>;
+  const int chunk = nrows <= 16384 ? C::BM : TC_CHUNK;  // small tables: one tile per item so the whole chip has work
+  // Query-group width (the wgmma N): an item is bound by the tiles it moves from L2, not by its MMAs (DESIGN §4.2), and
+  // every stage of it holds C::BM rows + w queries, so the launch takes about (waves of items over the CTA slots) x
+  // (C::BM + w).  Take the widest group that minimises that product: at 1024 centroids x 1024 queries, 256 items of 64
+  // queries fill 3 x 132 slots in one wave.  A score does not depend on the width or the tile: each element's K order is
+  // the same.
+  const int64_t slots = (int64_t)dev.sms * dev.dense_ctas[half ? 1 : 0];
+  int nqt = TC_DENSE_NQT;
   int64_t best = INT64_MAX;
-  for (int w = TC_NQT; w >= 16; w >>= 1) {
-    const int64_t cost = cdiv(cdiv(nrows, chunk) * cdiv(nq, w), dev.sms) * w;
+  for (int w = TC_DENSE_NQT; w >= 16; w >>= 1) {
+    const int64_t cost = cdiv(cdiv(nrows, chunk) * cdiv(nq, w), slots) * (C::BM + w);
     if (cost < best) { best = cost; nqt = w; }
   }
   const int nitems = (int)(cdiv(nrows, chunk) * cdiv(nq, nqt));
@@ -1654,7 +1670,7 @@ static void tc_dense_scan(IndexBase* ix, const TcView& v, bool l2, int64_t nq, c
   tc_coarse_items_kernel<<<(unsigned)cdiv(nitems, 128), 128, 0, s>>>(nrows, (int)nq, chunk, nqt, items, totals);
   TcParams p = tc_params(v, d, l2, items, totals, hscale, qr.scale);
   p.mode = 2; p.dense = dense; p.dense_ld = nrows; p.work_counter = work; p.split = qr.lo != nullptr ? 1 : 0;
-  const TcMaps maps = make_tc_maps(a_hi, a_lo, nrows, qr.op, qr.lo, nq, d, half);
+  const TcMaps maps = make_tc_maps(a_hi, a_lo, nrows, C::BM, qr.op, qr.lo, nq, d, half);
   ix->phase(IndexBase::PH_COARSE_SCAN, s);
   tc_launch(dev, half, nitems, maps, p, s);
 }
