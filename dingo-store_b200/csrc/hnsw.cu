@@ -12,6 +12,9 @@
 // (single writer, deterministic) with the hooked AVX-512 distance order, so a graph built here equals the graph
 // the CPU path builds from the same insertion order; the device holds a mirror that is refreshed lazily.
 //
+// The host graph, the device mirror and the state blob share one layout (DESIGN §5): level-0 lists in link0, the upper-level
+// lists of node i in one linkup pool from up_off[i].  hnsw_links addresses a list on both sides; parse_state reads a blob.
+//
 // Search (hnsw_search_kernel) and batched construction (hnsw_build_search_kernel) share one device graph walk: one
 // 128-thread CTA per query or row; greedy descent through the upper levels, then the reference's searchBaseLayerST at one
 // level, whose hops score the <= 32 unvisited neighbours of a node together (32 quads, exact AVX-512 order, so the
@@ -70,26 +73,33 @@ typedef std::pair<float, tableint> HPair;
 struct ByFirst { bool operator()(HPair const& a, HPair const& b) const noexcept { return a.first < b.first; } };
 typedef std::priority_queue<HPair, std::vector<HPair>, ByFirst> HHeap;
 
+// [count, links...] of a node at a level, in the layout of the host graph, the device mirror and the state blob
+__host__ __device__ __forceinline__ unsigned int* hnsw_links(unsigned int* link0, const int64_t* up_off, unsigned int* linkup, int maxM,
+                                                             int maxM0, unsigned int node, int level) {
+  return level == 0 ? link0 + (size_t)node * (maxM0 + 1) : linkup + up_off[node] + (size_t)(level - 1) * (maxM + 1);
+}
+
 struct HostGraph {
   int metric, d;
   size_t M, maxM, maxM0, efc;
   double mult;
   std::default_random_engine rng;
-  int64_t n = 0, cap = 0;
+  int64_t n = 0;  // nodes inserted; during an add, the per-node arrays also hold the call's laid-out slots beyond n
   int maxlevel = -1;
   tableint enterpoint = (tableint)-1;
   std::vector<float> data;
   std::vector<int64_t> labels;
   std::vector<int> levels;
   std::vector<tableint> link0;
-  std::vector<std::vector<tableint>> linkup;
+  std::vector<int64_t> up_off{0};  // node i's upper-level lists: linkup[up_off[i], up_off[i + 1]), levels[i] · (maxM + 1) entries
+  std::vector<tableint> linkup;
   std::vector<uint8_t> deleted;
   std::unordered_map<int64_t, tableint> lookup;
   std::vector<uint32_t> visited;
   uint32_t tag = 0;
   int64_t ndeleted = 0;
   // concurrent insertion (hnswlib's locking scheme): one lock per node for its link lists, one for the entry point /
-  // max level, one for slot allocation + label map + level generator; every worker owns a visited-tag array
+  // max level, one for slot allocation + label map; every worker owns a visited-tag array
   struct VisitCtx { std::vector<uint32_t> visited; uint32_t tag = 0; };
   std::unique_ptr<std::mutex[]> node_mu;
   int64_t node_mu_cap = 0;
@@ -106,18 +116,36 @@ struct HostGraph {
     node_mu.reset(new std::mutex[(size_t)ncap]);
     node_mu_cap = ncap;
   }
-  void reserve(int64_t ncap) {  // resizeIndex
-    if (ncap <= cap) return;
-    data.resize((size_t)ncap * d); labels.resize(ncap); levels.resize(ncap); link0.resize((size_t)ncap * (maxM0 + 1), 0);
-    linkup.resize(ncap); deleted.resize(ncap, 0); visited.resize(ncap, 0);
-    cap = ncap;
+  std::vector<int> draw_levels(int64_t k, std::default_random_engine& r) const {  // the next k nodes' levels, in node order
+    std::uniform_real_distribution<double> U(0.0, 1.0);
+    std::vector<int> lev((size_t)k);
+    for (int& l : lev) l = (int)(-log(U(r)) * mult);
+    return lev;
+  }
+  void extend_up_off(std::vector<int64_t>& off, const std::vector<int>& lev) const {  // pool offsets of nodes with levels lev
+    for (int l : lev) off.push_back(off.back() + (int64_t)l * (int64_t)(maxM + 1));
+  }
+  // Lays out the slots of a call's nodes, with levels lev, after the slots laid out so far: levels, pool offsets, zeroed
+  // level-0 blocks and pool slots, and room for their rows.  Nothing grows while add_point (or the batched commit) fills them.
+  void append_nodes(const std::vector<int>& lev) {
+    const size_t n1 = levels.size() + lev.size();
+    levels.insert(levels.end(), lev.begin(), lev.end());
+    extend_up_off(up_off, lev);
+    link0.resize(n1 * (maxM0 + 1), 0);
+    linkup.resize((size_t)up_off.back(), 0);
+    data.resize(n1 * d); labels.resize(n1); deleted.resize(n1, 0); visited.resize(n1, 0);
+  }
+  void take_label(int64_t label, tableint c) {  // node c takes the label; the label's old node, if live, becomes a tombstone
+    auto it = lookup.find(label);
+    if (it != lookup.end() && !deleted[it->second]) { deleted[it->second] = 1; ++ndeleted; }
+    lookup[label] = c;
   }
   const float* vec(tableint i) const { return &data[(size_t)i * d]; }
   float dist(const float* a, const float* b) const {
     if (metric == B200VS_L2) return host_avx512_order<true>(a, b, d);
     return 1.0f - host_avx512_order<false>(a, b, d);
   }
-  tableint* ll(tableint i, int level) { return level == 0 ? &link0[(size_t)i * (maxM0 + 1)] : &linkup[i][(size_t)(level - 1) * (maxM + 1)]; }
+  tableint* ll(tableint i, int level) { return hnsw_links(link0.data(), up_off.data(), linkup.data(), (int)maxM, (int)maxM0, i, level); }
 
   template <bool MT>
   HHeap search_layer(tableint ep, const float* q, int layer, VisitCtx* vc = nullptr) {
@@ -197,23 +225,18 @@ struct HostGraph {
     return next_ep;
   }
   // addPoint for a NEW label (replacing an existing label = mark the old node deleted, then insert).  MT = several threads
-  // insert at once (the reference's ParallelFor over addPoint, vector_index_hnsw.cc:229-243); capacity and locks are
-  // reserved by the caller, so no container is re-allocated while workers run.
+  // insert at once (the reference's ParallelFor over addPoint, vector_index_hnsw.cc:229-243).  The caller has laid out the
+  // node's slot (append_nodes, which drew its level) and reserved the locks, so no container grows while workers run.
   template <bool MT>
   void add_point(const float* x, int64_t label, VisitCtx* vc = nullptr) {
     tableint cur_c;
-    int curlevel;
     {
       std::unique_lock<std::mutex> al;
       if (MT) al = std::unique_lock<std::mutex>(lk->alloc_mu);
-      auto it = lookup.find(label);
-      if (it != lookup.end()) { if (!deleted[it->second]) { deleted[it->second] = 1; ++ndeleted; } lookup.erase(it); }
-      if (!MT && n >= cap) reserve(std::max<int64_t>(1024, cap * 2));
       cur_c = (tableint)n++;
-      lookup[label] = cur_c;
-      std::uniform_real_distribution<double> U(0.0, 1.0);
-      curlevel = (int)(-log(U(rng)) * mult);
+      take_label(label, cur_c);
     }
+    const int curlevel = levels[cur_c];
     std::unique_lock<std::mutex> own;
     if (MT) own = std::unique_lock<std::mutex>(node_mu[cur_c]);
     std::unique_lock<std::mutex> gl;
@@ -222,9 +245,7 @@ struct HostGraph {
     if (MT && curlevel <= maxlevelcopy) gl.unlock();
     tableint cur = enterpoint;
     memcpy(&data[(size_t)cur_c * d], x, sizeof(float) * d);
-    labels[cur_c] = label; levels[cur_c] = curlevel; deleted[cur_c] = 0;
-    memset(&link0[(size_t)cur_c * (maxM0 + 1)], 0, (maxM0 + 1) * sizeof(tableint));
-    linkup[cur_c].assign((size_t)curlevel * (maxM + 1), 0);
+    labels[cur_c] = label;
     const float* q = vec(cur_c);
     if ((int)cur != -1) {
       if (curlevel < maxlevelcopy) {
@@ -253,23 +274,67 @@ struct HostGraph {
   }
 };
 
+// The one reader of a state blob (layout and refusals: DESIGN §5): a fresh graph with the parameters of `like`.  A blob whose
+// graph the host builder or the device walk could not traverse within its arrays is refused.
+HostGraph parse_state(const HostGraph& like, const void* blob, size_t len) {
+  HostGraph H;
+  H.init(like.metric, like.d, (int)like.M, (int)like.efc, 100);
+  auto refuse = [](const char* why) { fail(B200VS_EILLEGAL_PARAMETERS, std::string("bad HNSW state blob (") + why + ")"); };
+  auto pad8 = [](uint64_t v) { return (v + 7) / 8 * 8; };
+  const char* base = (const char*)blob;
+  int64_t hdr[8], pool;
+  if (len < 64) refuse("truncated");
+  memcpy(hdr, base, 64);
+  if (hdr[0] != 0x57534E48 || hdr[2] != H.d || hdr[3] != (int64_t)H.M || hdr[4] != (int64_t)H.maxM0) refuse("header");
+  const int64_t n = hdr[1];
+  if (n < 0 || n > (1LL << 31)) refuse("row count");
+  const uint64_t o_off = pad8(64 + (uint64_t)n * 4), o_link0 = o_off + (uint64_t)(n + 1) * 8;
+  if (len < o_link0) refuse("truncated");
+  memcpy(&pool, base + o_off + (uint64_t)n * 8, 8);
+  if (pool < 0 || pool > (int64_t)(len / 4)) refuse("link pool");
+  const uint64_t n0 = (uint64_t)n * (H.maxM0 + 1), o_pool = o_link0 + n0 * 4, o_data = pad8(o_pool + (uint64_t)pool * 4);
+  const uint64_t o_labels = pad8(o_data + (uint64_t)n * H.d * 4), o_end = o_labels + (uint64_t)n * 8;
+  if (len < o_end) refuse("truncated");
+  auto take = [&](auto& v, uint64_t off, uint64_t count) { v.resize(count); if (count) memcpy(v.data(), base + off, count * sizeof(v[0])); };
+  take(H.levels, 64, n); take(H.up_off, o_off, n + 1); take(H.link0, o_link0, n0); take(H.linkup, o_pool, pool);
+  take(H.data, o_data, (uint64_t)n * H.d); take(H.labels, o_labels, n);
+  H.deleted.assign(n, 0);
+  if (len >= o_end + n) take(H.deleted, o_end, n);  // the optional trailing tombstones
+  H.visited.assign(n, 0);
+  if (n == 0 && (hdr[5] != -1 || hdr[6] != (int64_t)(tableint)-1)) refuse("empty graph with an entry point");
+  if (n > 0 && (hdr[6] < 0 || hdr[6] >= n || H.levels[hdr[6]] != hdr[5])) refuse("entry point");
+  H.n = n; H.maxlevel = (int)hdr[5]; H.enterpoint = (tableint)hdr[6];
+  if (H.up_off[0] != 0) refuse("pool offsets");
+  for (int64_t i = 0; i < n; ++i) {  // node i's level and pool slots (up_off[i] <= pool: the sum cannot overflow), then its lists
+    if (H.levels[i] < 0 || H.levels[i] > H.maxlevel) refuse("level");
+    if (H.up_off[i + 1] != H.up_off[i] + (int64_t)H.levels[i] * (int64_t)(H.maxM + 1) || H.up_off[i + 1] > pool) refuse("pool offsets");
+    for (int l = 0; l <= H.levels[i]; ++l) {
+      const tableint* ls = H.ll((tableint)i, l);
+      if (ls[0] > (l ? H.maxM : H.maxM0)) refuse("list count");
+      for (tableint j = 1; j <= ls[0]; ++j)
+        if (ls[j] >= (uint64_t)n || H.levels[ls[j]] < l) refuse("link target");
+    }
+    if (H.deleted[i] > 1) refuse("tombstone");
+    H.ndeleted += H.deleted[i];
+    if (!H.deleted[i]) H.lookup[H.labels[i]] = (tableint)i;
+  }
+  return H;
+}
+
 // ---------------- device graph walk: search and batched construction ----------------
 // The device mirror of HostGraph's first n nodes.  The construction's link and reverse kernels write its link lists.
 struct HnswDev {
   const float* data;
   const long long* labels;
   unsigned int* link0;
-  const long long* up_off;
+  const int64_t* up_off;
   unsigned int* linkup;
   const unsigned char* deleted;
   long long n;
   int d, maxM, maxM0, maxlevel, efc;
   unsigned int enterpoint;
   int has_deletions, M;
-  // HostGraph::ll: [size, link...] of a node at a level
-  __device__ __forceinline__ unsigned int* links(unsigned int node, int level) const {
-    return level == 0 ? link0 + (size_t)node * (maxM0 + 1) : linkup + up_off[node] + (size_t)(level - 1) * (maxM + 1);
-  }
+  __device__ __forceinline__ unsigned int* links(unsigned int node, int level) const { return hnsw_links(link0, up_off, linkup, maxM, maxM0, node, level); }
 };
 
 // HostGraph::dist on the device: quad lane t's part of the exact AVX-512 order, then hnswlib's InnerProductDistance
@@ -905,7 +970,8 @@ struct HnswIndex : IndexBase {
   bool dirty = true;
   int64_t uploaded_rows = 0;
   DevBuf<float> d_data;
-  DevBuf<long long> d_labels, d_upoff;
+  DevBuf<long long> d_labels;
+  DevBuf<int64_t> d_upoff;
   DevBuf<unsigned int> d_link0, d_linkup;
   DevBuf<unsigned char> d_deleted;
 
@@ -924,51 +990,9 @@ struct HnswIndex : IndexBase {
     G.init(metric, d, p.hnsw_m, p.hnsw_efc, 100);  // random_seed = 100, hnsw.cc:181-182
   }
 
-  // blob (the oracle's / this index's export): int64 hdr[8] = {'HNSW', n, d, M, maxM0, maxlevel, enterpoint, metric};
-  // int32 levels[n]; (pad 8) int64 up_off[n+1]; uint32 link0[n*(maxM0+1)]; uint32 linkup[up_off[n]]; (pad 8)
-  // float data[n*d]; (pad 8) int64 labels[n]
   void set_state(const void* blob, size_t len) override {
     std::unique_lock<std::shared_mutex> wl(rw);
-    if (len < 64) fail(B200VS_EILLEGAL_PARAMETERS, "state blob too short");
-    const char* base = (const char*)blob;
-    const int64_t* hdr = (const int64_t*)base;
-    if (hdr[0] != 0x57534E48 || hdr[2] != dim || hdr[3] != (int64_t)G.M) fail(B200VS_EILLEGAL_PARAMETERS, "bad HNSW state blob");
-    const int64_t n = hdr[1];
-    {  // the blob must hold every section BEFORE anything is copied out of it
-      if (n < 0 || n > (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "bad HNSW state blob (row count)");
-      auto pad8 = [](uint64_t v) { return (v + 7) / 8 * 8; };
-      uint64_t need = pad8(64 + (uint64_t)n * 4) + (uint64_t)(n + 1) * 8;
-      if (len < need) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
-      const int64_t* off_chk = (const int64_t*)((const char*)blob + pad8(64 + (uint64_t)n * 4));
-      const int64_t up = off_chk[n];
-      if (up < 0 || up > (int64_t)(len / 4)) fail(B200VS_EILLEGAL_PARAMETERS, "bad HNSW state blob (link pool)");
-      need = pad8(need + (uint64_t)n * (2 * G.M + 1) * 4 + (uint64_t)up * 4);
-      need = pad8(need + (uint64_t)n * dim * 4) + (uint64_t)n * 8;
-      if (len < need) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
-    }
-    HostGraph H;
-    H.init(metric, dim, (int)G.M, (int)G.efc, 100);
-    H.reserve(std::max<int64_t>(n, 1));
-    const char* p = base + 64;
-    memcpy(H.levels.data(), p, n * 4); p += n * 4;
-    p = base + ((p - base) + 7) / 8 * 8;
-    const int64_t* off = (const int64_t*)p; p += (n + 1) * 8;
-    memcpy(H.link0.data(), p, (size_t)n * (H.maxM0 + 1) * 4); p += (size_t)n * (H.maxM0 + 1) * 4;
-    for (int64_t i = 0; i < n; ++i) { H.linkup[i].assign((const tableint*)p + off[i], (const tableint*)p + off[i + 1]); }
-    p += off[n] * 4;
-    p = base + ((p - base) + 7) / 8 * 8;
-    memcpy(H.data.data(), p, (size_t)n * dim * 4); p += (size_t)n * dim * 4;
-    p = base + ((p - base) + 7) / 8 * 8;
-    memcpy(H.labels.data(), p, n * 8);
-    if ((size_t)(p - base) + (size_t)n * 8 > len) fail(B200VS_EILLEGAL_PARAMETERS, "state blob truncated");
-    H.n = n; H.maxlevel = (int)hdr[5]; H.enterpoint = (tableint)hdr[6];
-    const size_t after_labels = (size_t)(p - base) + (size_t)n * 8;
-    if (len >= after_labels + (size_t)n) {  // optional trailing tombstone bytes (written only when something was deleted)
-      memcpy(H.deleted.data(), base + after_labels, (size_t)n);
-      for (int64_t i = 0; i < n; ++i) H.ndeleted += H.deleted[i] ? 1 : 0;
-    }
-    for (int64_t i = 0; i < n; ++i) if (!H.deleted[i]) H.lookup[H.labels[i]] = (tableint)i;
-    G = std::move(H);
+    G = parse_state(G, blob, len);
     dirty = true; uploaded_rows = 0;
   }
 
@@ -1004,20 +1028,22 @@ struct HnswIndex : IndexBase {
       normalize_for_hnsw(xi, dim, tmp.data());
       return tmp.data();
     };
+    // every slot of the call up front: node c takes the generator's c-th draw, as when each insertion drew its own level
+    const int64_t ntot = G.n + n;
+    G.append_nodes(G.draw_levels(n, G.rng));
     const int nthreads = (int)std::min<int64_t>(std::max(1, params.hnsw_build_threads), n);
     if (nthreads <= 1) {  // single writer: deterministic graph (equal to the oracle's for the same insertion order)
       std::vector<float> tmp(dim);
       for (int64_t i = 0; i < n; ++i) G.add_point<false>(prepared(i, tmp), in_ids[i]);
     } else {  // concurrent insertion, as the reference's thread pool does (hnsw.cc:229-243)
-      G.reserve(std::max<int64_t>(G.cap, G.n + n));
-      G.reserve_locks(G.cap);
+      G.reserve_locks(ntot);
       std::atomic<int64_t> next{0};
       if (G.n == 0) { std::vector<float> tmp(dim); G.add_point<false>(prepared(0, tmp), in_ids[0]); next = 1; }  // hnswlib: first element alone
       std::vector<std::thread> ts;
       for (int t = 0; t < nthreads; ++t)
         ts.emplace_back([&]() {
           HostGraph::VisitCtx vc;
-          vc.visited.assign((size_t)G.cap, 0u);
+          vc.visited.assign((size_t)ntot, 0u);
           std::vector<float> tmp(dim);
           for (;;) {
             const int64_t i = next.fetch_add(1);
@@ -1062,7 +1088,7 @@ struct HnswIndex : IndexBase {
   void add_batched_locked(int64_t n, const float* x, const int64_t* in_ids, int batch, bool prepared) {
     const BuildPlan P = batched_plan(n, batch);
     batch = P.batch;
-    const int efc = (int)G.efc, M = (int)G.M, maxM = (int)G.maxM, maxM0 = (int)G.maxM0;
+    const int efc = (int)G.efc, M = (int)G.M, maxM0 = (int)G.maxM0;
     const int bmax = P.bmax;
     const size_t smem_search = P.smem_search;
     cudaStream_t s = stream;
@@ -1076,11 +1102,7 @@ struct HnswIndex : IndexBase {
       else memcpy(&rows[(size_t)i * dim], x + (size_t)i * dim, (size_t)dim * 4);
     }
     std::default_random_engine rng = G.rng;
-    std::vector<int> lev(n);
-    {
-      std::uniform_real_distribution<double> U(0.0, 1.0);
-      for (int64_t i = 0; i < n; ++i) lev[i] = (int)(-log(U(rng)) * G.mult);
-    }
+    const std::vector<int> lev = G.draw_levels(n, rng);
     struct Batch { int64_t a, b; int maxlevel; tableint ep; bool deletions; int64_t task0, ntask, dead0, ndead; };
     std::vector<Batch> plan;
     std::vector<long long> slot_off(n);
@@ -1125,14 +1147,10 @@ struct HnswIndex : IndexBase {
       plan.push_back(B);
       a = e;
     }
-    long long up_old = 0;
-    for (int64_t i = 0; i < n0_call; ++i) up_old += (long long)G.linkup[i].size();
-    std::vector<long long> off(n + 1);
-    off[0] = up_old;
-    for (int64_t i = 0; i < n; ++i) off[i + 1] = off[i] + (long long)lev[i] * (maxM + 1);
-    const long long up_new = off[n];
-    G.reserve(std::max<int64_t>(G.cap, ntot));  // capacity only: nothing observable changes
-    std::vector<unsigned int> up((size_t)std::max<long long>(up_new, 1)), l0((size_t)ntot * (maxM0 + 1));
+    std::vector<int64_t> off{G.up_off[n0_call]};  // the call's nodes' pool offsets
+    G.extend_up_off(off, lev);
+    const int64_t up_old = off[0], up_new = off[n];
+    std::vector<tableint> up((size_t)up_new), l0((size_t)ntot * (maxM0 + 1));  // the link lists coming back from the device
 
     try {
       // ---- device mirror: append the call's rows, empty link lists and upper-level slots (beyond G.n: unseen by searches) ----
@@ -1253,27 +1271,14 @@ struct HnswIndex : IndexBase {
       throw;
     }
 
-    // ---- commit: G takes the call's rows in call order (add_point's bookkeeping) and the device's link lists ----
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = G.lookup.find(in_ids[i]);
-      if (it != G.lookup.end()) {
-        if (!G.deleted[it->second]) { G.deleted[it->second] = 1; ++G.ndeleted; }
-        G.lookup.erase(it);
-      }
-      const tableint c = (tableint)G.n++;
-      G.lookup[in_ids[i]] = c;
-      memcpy(&G.data[(size_t)c * dim], &rows[(size_t)i * dim], (size_t)dim * 4);
-      G.labels[c] = in_ids[i]; G.levels[c] = lev[i]; G.deleted[c] = 0;
-      G.linkup[c].assign((size_t)lev[i] * (maxM + 1), 0);
-    }
-    G.enterpoint = ep; G.maxlevel = maxlevel; G.rng = rng;
-    memcpy(G.link0.data(), l0.data(), l0.size() * 4);
-    long long acc = 0;
-    for (int64_t i = 0; i < ntot; ++i) {
-      const size_t sz = G.linkup[i].size();
-      if (sz) memcpy(G.linkup[i].data(), &up[acc], sz * 4);
-      acc += (long long)sz;
-    }
+    // ---- commit: G lays out the call's nodes and takes their rows in call order (add_point's bookkeeping), the device's link
+    //      lists and the generator state ----
+    G.append_nodes(lev);
+    for (int64_t i = 0; i < n; ++i) G.take_label(in_ids[i], (tableint)(n0_call + i));
+    memcpy(&G.data[(size_t)n0_call * dim], rows.data(), rows.size() * 4);
+    memcpy(&G.labels[n0_call], in_ids, (size_t)n * 8);
+    G.link0 = std::move(l0); G.linkup = std::move(up);
+    G.n = ntot; G.enterpoint = ep; G.maxlevel = maxlevel; G.rng = rng;
     uploaded_rows = ntot;
     dirty = false;
   }
@@ -1312,18 +1317,13 @@ struct HnswIndex : IndexBase {
     if (n > uploaded_rows)
       B200VS_CUDA(cudaMemcpyAsync(d_data.p + (size_t)uploaded_rows * dim, G.data.data() + (size_t)uploaded_rows * dim,
                                   (size_t)(n - uploaded_rows) * dim * 4, cudaMemcpyHostToDevice, s));
-    d_labels.reserve(n, 0, s); d_link0.reserve((size_t)n * (G.maxM0 + 1), 0, s); d_upoff.reserve(n + 1, 0, s); d_deleted.reserve(n, 0, s);
-    std::vector<long long> off(n + 1);
-    long long acc = 0;
-    for (int64_t i = 0; i < n; ++i) { off[i] = acc; acc += (long long)G.linkup[i].size(); }
-    off[n] = acc;
-    std::vector<unsigned int> up((size_t)std::max<long long>(acc, 1));
-    for (int64_t i = 0; i < n; ++i) if (!G.linkup[i].empty()) memcpy(&up[off[i]], G.linkup[i].data(), G.linkup[i].size() * 4);
-    d_linkup.reserve(up.size(), 0, s);
+    const size_t n0 = (size_t)n * (G.maxM0 + 1), pool = (size_t)G.up_off[n];
+    d_labels.reserve(n, 0, s); d_link0.reserve(n0, 0, s); d_upoff.reserve(n + 1, 0, s); d_linkup.reserve(std::max<size_t>(pool, 1), 0, s);
+    d_deleted.reserve(n, 0, s);
     B200VS_CUDA(cudaMemcpyAsync(d_labels.p, G.labels.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(d_link0.p, G.link0.data(), (size_t)n * (G.maxM0 + 1) * 4, cudaMemcpyHostToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(d_upoff.p, off.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(d_linkup.p, up.data(), up.size() * 4, cudaMemcpyHostToDevice, s));
+    B200VS_CUDA(cudaMemcpyAsync(d_link0.p, G.link0.data(), n0 * 4, cudaMemcpyHostToDevice, s));
+    B200VS_CUDA(cudaMemcpyAsync(d_upoff.p, G.up_off.data(), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (pool) B200VS_CUDA(cudaMemcpyAsync(d_linkup.p, G.linkup.data(), pool * 4, cudaMemcpyHostToDevice, s));
     B200VS_CUDA(cudaMemcpyAsync(d_deleted.p, G.deleted.data(), (size_t)n, cudaMemcpyHostToDevice, s));
     B200VS_CUDA(cudaStreamSynchronize(s));
     uploaded_rows = n;
@@ -1425,37 +1425,35 @@ struct HnswIndex : IndexBase {
   int64_t get_state(void* blob, size_t cap) override {
     RwSharedGuard rl(this);
     const int64_t n = G.n;
-    int64_t up = 0;
-    for (int64_t i = 0; i < n; ++i) up += (int64_t)G.linkup[i].size();
-    auto pad8 = [](int64_t v) { return (v + 7) / 8 * 8; };
-    int64_t sz = pad8(64 + n * 4);
-    sz = pad8(sz + (n + 1) * 8 + n * (int64_t)(G.maxM0 + 1) * 4 + up * 4);
-    sz = pad8(sz + n * (int64_t)dim * 4);
-    sz += n * 8;
-    if (G.ndeleted > 0) sz += n;  // trailing tombstone bytes
-    if (!blob || (int64_t)cap < sz) return sz;
-    char* base = (char*)blob;
-    char* p = base;
-    int64_t hdr[8] = {0x57534E48, n, dim, (int64_t)G.M, (int64_t)G.maxM0, G.maxlevel, (int64_t)G.enterpoint, (int64_t)metric};
-    memcpy(p, hdr, 64); p += 64;
-    memcpy(p, G.levels.data(), n * 4); p += n * 4;
-    p = base + pad8(p - base);
-    int64_t* off = (int64_t*)p; p += (n + 1) * 8;
-    int64_t acc = 0;
-    for (int64_t i = 0; i < n; ++i) { off[i] = acc; acc += (int64_t)G.linkup[i].size(); }
-    off[n] = acc;
-    memcpy(p, G.link0.data(), (size_t)n * (G.maxM0 + 1) * 4); p += (size_t)n * (G.maxM0 + 1) * 4;
-    for (int64_t i = 0; i < n; ++i) { memcpy(p, G.linkup[i].data(), G.linkup[i].size() * 4); p += G.linkup[i].size() * 4; }
-    p = base + pad8(p - base);
-    memcpy(p, G.data.data(), (size_t)n * dim * 4); p += (size_t)n * dim * 4;
-    p = base + pad8(p - base);
-    memcpy(p, G.labels.data(), n * 8); p += n * 8;
-    if (G.ndeleted > 0) memcpy(p, G.deleted.data(), (size_t)n);
-    return sz;
+    const int64_t hdr[8] = {0x57534E48, n, dim, (int64_t)G.M, (int64_t)G.maxM0, G.maxlevel, (int64_t)G.enterpoint, (int64_t)metric};
+    struct Section { const void* src; size_t bytes; bool pad8; };  // the blob's sections in order (DESIGN §5); pad8: zeros follow
+    const Section secs[] = {{hdr, 64, false}, {G.levels.data(), (size_t)n * 4, true}, {G.up_off.data(), (size_t)(n + 1) * 8, false},
+                            {G.link0.data(), (size_t)n * (G.maxM0 + 1) * 4, false}, {G.linkup.data(), (size_t)G.up_off[n] * 4, true},
+                            {G.data.data(), (size_t)n * dim * 4, true}, {G.labels.data(), (size_t)n * 8, false},
+                            {G.deleted.data(), G.ndeleted > 0 ? (size_t)n : 0, false}};  // tombstones only when anything is deleted
+    auto end = [](size_t at, const Section& s) { return s.pad8 ? (at + s.bytes + 7) / 8 * 8 : at + s.bytes; };
+    size_t sz = 0;
+    for (const Section& s : secs) sz = end(sz, s);
+    if (!blob || cap < sz) return (int64_t)sz;
+    char* const base = (char*)blob;
+    size_t at = 0;
+    for (const Section& s : secs) {
+      if (s.bytes) memcpy(base + at, s.src, s.bytes);
+      memset(base + at + s.bytes, 0, end(at, s) - at - s.bytes);
+      at = end(at, s);
+    }
+    return (int64_t)sz;
   }
 };
 
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p) { return new HnswIndex(m, d, p); }
+
+std::vector<int64_t> hnsw_state_labels(const IndexBase* ix, const void* blob, size_t len) {
+  const HostGraph H = parse_state(static_cast<const HnswIndex*>(ix)->G, blob, len);
+  std::vector<int64_t> live;
+  for (int64_t i = 0; i < H.n; ++i) if (!H.deleted[i]) live.push_back(H.labels[i]);
+  return live;
+}
 
 void hnsw_build_scratch_limit(IndexBase* ix, int64_t bytes) {
   std::unique_lock<std::shared_mutex> wl(ix->rw);

@@ -470,6 +470,9 @@ IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_flat(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_ivf_pq(b200vs_metric m, int d, const b200vs_params& p);
 IndexBase* make_hnsw(b200vs_metric m, int d, const b200vs_params& p);
+// The live labels, in node order, of the graph in an HNSW state blob for the HNSW index ix, which stays untouched; refuses
+// every blob that set_state refuses (hnsw.cu)
+std::vector<int64_t> hnsw_state_labels(const IndexBase* ix, const void* blob, size_t len);
 // IVF-PQ training in the two stages of its train (ivf_pq.cu), for the list-sharded trainer (shard.cu); ix must be an IVF_PQ
 // index, whose lists and trained state stay untouched.  Coarse: k centroids of n raw rows.  State: the codebooks of the PQ
 // rule on the n rows' residuals to the centroids cent [nlist, dim], returned with cent as a trained-state blob.

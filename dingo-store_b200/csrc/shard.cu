@@ -1341,12 +1341,7 @@ void shard_load_locked(b200vs_shard* sh, const std::string& prefix) {
     std::vector<int64_t> graph_ids;
     if (ix->type == B200VS_HNSW) {
       state = files[0].state;
-      if (!state.empty()) {  // the labels of the saved graph, read through a standalone index
-        std::unique_ptr<IndexBase> g(make_hnsw(ix->metric, ix->dim, ix->params));
-        g->set_state(state.data(), state.size());
-        graph_ids.resize((size_t)g->count());
-        g->export_lists(nullptr, nullptr, nullptr, graph_ids.data());
-      }
+      if (!state.empty()) graph_ids = hnsw_state_labels(ix, state.data(), state.size());  // the labels of the saved graph
     }
     if (mh.world == W2) check_ownership(sh, files[0], graph_ids);
   }), "shard load"));
