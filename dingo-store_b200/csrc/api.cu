@@ -58,7 +58,7 @@ void index_read(IndexBase* ix, void* stream, const b200vs_search_params* sp, Bod
 // [nq]).  A NaN radius admits no row of a float index: empty results, nothing launched (DESIGN.md 4.6); a binary index
 // refuses it.  xq / outputs may be pinned staging (coalesced batches) or caller memory.
 void host_read(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids,
-               bool range = false, float radius = 0.f, int32_t* out_counts = nullptr) {
+               bool range = false, float radius = 0.f, int32_t* out_counts = nullptr, bool deep = false) {
   index_read(ix, nullptr, sp, [&](const SearchCtx& sc, cudaStream_t s) {
     const size_t nk = (size_t)nq * k;
     if (range && std::isnan(radius) && !ix->binary()) {
@@ -69,7 +69,7 @@ void host_read(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_se
     }
     const size_t qbytes = (size_t)nq * ix->query_row_bytes();
     SearchReq r;
-    r.nq = nq; r.k = k; r.range = range; r.radius = radius; r.sc = &sc;
+    r.nq = nq; r.k = k; r.range = range; r.radius = radius; r.sc = &sc; r.deep = deep;
     void* dq = ix->scratch.alloc<unsigned char>(qbytes);
     r.xq = dq;
     r.od = ix->scratch.alloc<float>(nk);
@@ -424,9 +424,35 @@ int host_search(b200vs_index* h, int64_t nq, const void* xq, int k, const b200vs
   });
 }
 
+// b200vs_search_deep / b200vs_search_binary_deep: the deep path for any k up to kDeepMaxK; never coalesced
+int host_search_deep(b200vs_index* h, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist,
+                     int64_t* out_ids, bool binary) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    check_row_type(ix, binary);
+    check_search_args(ix, nq, xq, sp);
+    if (k <= 0) return B200VS_OK;
+    if (k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
+    if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "deep top-k is not implemented for HNSW");
+    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    host_read(ix, nq, xq, k, sp, out_dist, out_ids, false, 0.f, nullptr, true);
+    return B200VS_OK;
+  });
+}
+
 }  // namespace
 
 extern "C" {
+
+int b200vs_search_deep(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
+                       int64_t* out_ids) {
+  return host_search_deep(h, nq, xq, k, sp, out_dist, out_ids, false);
+}
+
+int b200vs_search_binary_deep(b200vs_index* h, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
+                              float* out_dist, int64_t* out_ids) {
+  return host_search_deep(h, nq, xq, k, sp, out_dist, out_ids, true);
+}
 
 int b200vs_search(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                   int64_t* out_ids) {
@@ -639,11 +665,14 @@ struct b200vs_scan {
   cudaStream_t s = nullptr;
   DevBuf<float> q, parts_d, out_d;      // parts = [2, nq, k]: running result, tile result
   DevBuf<long long> parts_i, out_i;
+  bool deep = false;                    // k past the exact scan's shared-memory select: tiles and merge on the deep path
+  DevBuf<float> cat_d;                  // deep merge input [nq, 2k]: each query's running result, then its tile result
+  DevBuf<long long> cat_i;
   int64_t pushed = 0;
   ~b200vs_scan() {
     if (flat) { cudaSetDevice(flat->device); }
     if (s) cudaStreamSynchronize(s);
-    q.free(); parts_d.free(); out_d.free(); parts_i.free(); out_i.free();
+    q.free(); parts_d.free(); out_d.free(); parts_i.free(); out_i.free(); cat_d.free(); cat_i.free();
     delete flat;
     if (s) cudaStreamDestroy(s);
   }
@@ -664,6 +693,8 @@ int b200vs_scan_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t
     std::unique_ptr<b200vs_scan> st(new b200vs_scan());
     st->flat = make_flat(metric, dim, p);
     st->nq = nq; st->k = k;
+    st->deep = !exact_select_fits(dim, 1, k);
+    if (st->deep && k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
     if (sp) {
       st->has_sp = true; st->sp = *sp;
       if (sp->sorted_ids && sp->n_ids > 0) st->allow.assign(sp->sorted_ids, sp->sorted_ids + sp->n_ids);
@@ -675,6 +706,7 @@ int b200vs_scan_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t
     st->q.reserve((size_t)nq * dim, 0, st->s);
     st->parts_d.reserve(2 * nk, 0, st->s); st->parts_i.reserve(2 * nk, 0, st->s);
     st->out_d.reserve(nk, 0, st->s); st->out_i.reserve(nk, 0, st->s);
+    if (st->deep) { st->cat_d.reserve(2 * nk, 0, st->s); st->cat_i.reserve(2 * nk, 0, st->s); }
     B200VS_CUDA(cudaMemcpyAsync(st->q.p, xq, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, st->s));
     B200VS_CUDA(cudaMemsetAsync(st->parts_d.p, 0, 2 * nk * 4, st->s));
     B200VS_CUDA(cudaMemsetAsync(st->parts_i.p, 0xFF, 2 * nk * 8, st->s));  // id -1 = empty slot
@@ -696,11 +728,21 @@ int b200vs_scan_push(b200vs_scan* st, int64_t n, const float* x, const int64_t* 
     ix->add(AddReq::host(n, x, ids));  // one temporary Flat index per tile, as the reference builds (vector_reader.cc:1937-1946)
     index_read(ix, st->s, st->has_sp ? &st->sp : nullptr, [&](const SearchCtx& sc, cudaStream_t s) {
       SearchReq r;
-      r.nq = st->nq; r.xq = st->q.p; r.k = st->k; r.sc = &sc; r.od = st->parts_d.p + nk; r.oi = st->parts_i.p + nk;
+      r.nq = st->nq; r.xq = st->q.p; r.k = st->k; r.sc = &sc; r.od = st->parts_d.p + nk; r.oi = st->parts_i.p + nk; r.deep = st->deep;
       ix->search(r, s);
+      if (!st->deep) return;
+      // running top-k <- the deep select over each query's 2k slots [running, tile]
+      const size_t k = (size_t)st->k;
+      for (int part = 0; part < 2; ++part) {
+        B200VS_CUDA(cudaMemcpy2DAsync(st->cat_d.p + part * k, 2 * k * 4, st->parts_d.p + part * nk, k * 4, k * 4, (size_t)st->nq,
+                                      cudaMemcpyDeviceToDevice, s));
+        B200VS_CUDA(cudaMemcpy2DAsync(st->cat_i.p + part * k, 2 * k * 8, st->parts_i.p + part * nk, k * 8, k * 8, (size_t)st->nq,
+                                      cudaMemcpyDeviceToDevice, s));
+      }
+      run_deep_merge_api(ix, st->nq, st->k, 2 * st->k, st->cat_d.p, st->cat_i.p, st->out_d.p, st->out_i.p, s);
     });
     // running top-k <- merge(running, tile): the reference's per-query priority queues (:1956-1971)
-    launch_merge_api(2, st->nq, st->k, st->parts_d.p, st->parts_i.p, st->out_d.p, st->out_i.p, st->s);
+    if (!st->deep) launch_merge_api(2, st->nq, st->k, st->parts_d.p, st->parts_i.p, st->out_d.p, st->out_i.p, st->s);
     B200VS_CUDA(cudaMemcpyAsync(st->parts_d.p, st->out_d.p, nk * 4, cudaMemcpyDeviceToDevice, st->s));
     B200VS_CUDA(cudaMemcpyAsync(st->parts_i.p, st->out_i.p, nk * 8, cudaMemcpyDeviceToDevice, st->s));
     B200VS_CUDA(cudaStreamSynchronize(st->s));  // the next push rewrites the tile index

@@ -192,6 +192,7 @@ struct BinaryFlatIndex : BinaryIndex {
     const uint32_t* q = pad(r.nq, static_cast<const uint8_t*>(r.xq), s);
     const TcView v = rowmap.view();
     ScanJob j = job(*r.sc);
+    if (r.deep) { run_scan_deep(this, j, r.nq, reinterpret_cast<const float*>(q), r.k, r.od, false, r.oi, s); return; }
     if (!r.range && bt_eligible(v, r.nq, r.k, 1, (double)rowmap.rows, *r.sc)) {
       long long* probes = scratch.alloc<long long>(r.nq);
       B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)r.nq * 8, s));
@@ -469,6 +470,7 @@ struct BinaryIvfIndex : BinaryIndex {
     if (profiling && !r.range) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
     const TcView v = view();
     ScanJob j = list_job(sc, probes, nprobe);
+    if (r.deep) { run_scan_deep(this, j, r.nq, reinterpret_cast<const float*>(q), r.k, r.od, false, r.oi, s); return; }
     if (!r.range && L.live > 0 && bt_eligible(v, r.nq, r.k, nprobe, j.avg_candidates, sc)) {
       bt_search(this, v, w, r.nq, q, r.k, probes, nprobe, j, r.od, r.oi, s);
       return;

@@ -1345,6 +1345,7 @@ struct HnswIndex : IndexBase {
     refuse_probes(r);
     if (r.range) fail(B200VS_EVECTOR_NOT_SUPPORT, "range search not supported");
     if (r.raw) fail(B200VS_EVECTOR_NOT_SUPPORT, "raw-key search not supported");
+    if (r.deep) fail(B200VS_EVECTOR_NOT_SUPPORT, "deep top-k is not implemented for HNSW");
     const SearchCtx& sc = *r.sc;
     const int64_t nq = r.nq;
     const int k = r.k;

@@ -393,6 +393,7 @@ struct FlatIndex : IndexBase {
     refuse_probes(r);
     const float* q = queries(r, s);
     const float thr = ip_like() ? 1.0F - r.radius : r.radius;
+    if (r.deep) { run_scan_deep(this, job(*r.sc), r.nq, q, r.k, r.od, r.raw, r.oi, s); return; }
     const TcView v = rowmap.view();
     if (rowmap.rows > 0 && tc_eligible(this, v, r.nq, r.k, 1, *r.sc, r.range)) {
       long long* probes = scratch.alloc<long long>(r.nq);
@@ -752,6 +753,7 @@ void IvfFlatIndex::search(const SearchReq& r, cudaStream_t s) {
     probes = own;
   }
   if (profiling) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
+  if (r.deep) { run_scan_deep(this, list_job(sc, probes, nprobe), r.nq, q, r.k, r.od, r.raw, r.oi, s); return; }
   const float thr = ip_like() ? 1.0F - r.radius : r.radius;
   const TcView v = view();
   if (L.live > 0 && tc_eligible(this, v, r.nq, r.k, nprobe, sc, r.range)) {

@@ -11,6 +11,7 @@
 #include <condition_variable>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <new>
 #include <shared_mutex>
@@ -20,6 +21,7 @@
 
 #include "../../include/b200vs.h"
 #include "common.cuh"
+#include "deep_select.cuh"
 
 namespace b200vs {
 
@@ -198,6 +200,7 @@ struct SearchReq {
   int k = 0;                          // top-k, or max_results when range
   bool range = false;                 // range search: the hits inside radius, closest first, at most k of them
   float radius = 0.f;
+  bool deep = false;                  // top-k through the deep path (run_deep): any k up to kDeepMaxK, always exact
   bool raw = false;                   // od = the raw metric value (L2 distance | ip), the key the single-index select ranks
                                       // by and a merge of several indexes' results has to order by, instead of the API distance
   const SearchCtx* sc = nullptr;
@@ -530,6 +533,37 @@ struct ScopedKernelTimer {  // CUDA events on the launching stream; synchronises
 // results: out_dist (API), out_raw (raw metric), out_ids, out_counts — any but out_ids may be null
 void run_scan(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* out_dist,
               float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s);
+
+// ---- deep top-k (deep_select.cu): exact top-k for k up to kDeepMaxK, past what the shared-memory select holds ----
+constexpr int kDeepMaxK = B200VS_DEEP_MAX_K;
+// A deep search's candidate space.  mode 0: candidate i of query q is row q * row_stride + i of [0, n) (row_stride 0: one
+// index for every query); mode 1: the probe-prefix positions of the lists probes[q] (the exact scan's map_row rule).
+struct DeepJob {
+  bool l2 = true;         // the key order of the scan: L2 / Hamming distance, or -ip
+  bool api_keys = false;  // the keys are f2ord(API distance) (a merge of result lists): emit the key's own float
+  int mode = 0;
+  long long n = 0, row_stride = 0;
+  const long long* ids = nullptr;
+  const long long* probes = nullptr;
+  int nprobe = 0;
+  const long long* list_off = nullptr;
+  const int* list_len = nullptr;
+};
+// the key pass of queries [q0, q0 + nqc): fills o's keys, eligibility and counts on stream s
+using DeepKeyPass = std::function<void(int64_t q0, int nqc, const DeepKeys& o, cudaStream_t s)>;
+// top-k of nq queries: od [nq, k] (the API distance, or the raw metric value when raw; may be null), oi [nq, k], -1 padded
+void run_deep(IndexBase* ix, const DeepJob& job, int64_t nq, int k, float* od, bool raw, long long* oi, const DeepKeyPass& pass,
+              cudaStream_t s);
+// merge_api_kernel's merge through run_deep: the top k of each query's n API-distance slots cat_d / cat_i [nq, n] (id < 0:
+// empty), ordered by (distance, id), into od / oi [nq, k]
+void run_deep_merge_api(IndexBase* ix, int64_t nq, int k, int n, const float* cat_d, const long long* cat_i, float* od, long long* oi,
+                        cudaStream_t s);
+// whether the exact scan's shared-memory select serves top-k k over d-float rows and nseg probed lists (run_scan, and the
+// merge kernels over the same pool)
+bool exact_select_fits(int d, int nseg, int k);
+// run_deep over the exact scan of job (scan_key_kernel)
+void run_scan_deep(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* od, bool raw, long long* oi,
+                   cudaStream_t s);
 
 // b200vs_scan_range_push: append the hits of one tile [n, d] to each query's running list in row order (range_append_kernel).
 // thr_raw is the raw threshold (L2: dist < thr; IP: ip > thr); counts[nq] persists across calls.

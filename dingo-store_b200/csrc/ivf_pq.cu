@@ -154,17 +154,13 @@ struct PqScanArgs {
   FilterDev filt;
 };
 
-// block (split, query): probes split round-robin; LUT in shared memory; one thread per code row
-template <bool L2>
-__global__ void __launch_bounds__(PQ_THREADS) pq_scan_select_kernel(const PqScanArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
+// block (split, query): probes split round-robin; LUT in shared memory; one thread per code row.  Every eligible row goes to
+// the sink (SelectSink, or DeepKeySink at its probe-prefix position).
+template <bool L2, class Sink>
+__device__ __forceinline__ void pq_scan_rows(const PqScanArgs& a, unsigned char* smem, const int qi, const int split, Sink& sink) {
   float* tab = reinterpret_cast<float*>(smem);
   const int M = a.M, T = M * KSUB;
-  const int qi = blockIdx.y, split = blockIdx.x;
-  BlockSelect sel;
-  sel.init(smem + (size_t)T * 4, a.pool_cap, a.k);
-  if (a.has_thr && threadIdx.x == 0) { *sel.thr_d = a.thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
-  __syncthreads();
+  sink.init(smem + (size_t)T * 4);
   const float* simq = a.sim + (size_t)qi * T;
   if (!L2) {
     for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = simq[i];
@@ -182,9 +178,9 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_scan_select_kernel(const PqScan
       for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = __fadd_rn(pl[i], __fmul_rn(-2.0f, simq[i]));
       __syncthreads();
     }
-    const long long base = a.list_off[l];
+    const long long base = a.list_off[l], pos0 = sink.list_pos(p);
     for (int r0 = 0; r0 < len; r0 += blockDim.x) {
-      sel.maybe_prune(blockDim.x);
+      sink.step(blockDim.x);
       const int r = r0 + threadIdx.x;
       if (r < len) {
         const long long row = base + r;
@@ -215,21 +211,28 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_scan_select_kernel(const PqScan
           } else {
             for (int m = 0; m < M; ++m) dis = __fadd_rn(dis, tab[m * KSUB + code[m]]);
           }
-          const uint32_t key = f2ord(L2 ? dis : -dis);
-          if (sel.passes(key, id)) sel.push(key, id);
+          sink.take(f2ord(L2 ? dis : -dis), id, pos0 + r);
         }
       }
     }
   }
-  sel.prune();
-  const int have = *sel.count;
-  uint32_t* okd = a.ws_kd + ((size_t)qi * a.nsplit + split) * a.k;
-  long long* oki = a.ws_kid + ((size_t)qi * a.nsplit + split) * a.k;
-  for (int i = threadIdx.x; i < a.k; i += blockDim.x) {
-    okd[i] = i < have ? sel.kd[i] : KEY_SENTINEL_D;
-    oki[i] = i < have ? sel.kid[i] : KEY_SENTINEL_ID;
-  }
+  sink.finish();
 }
+template <bool L2>
+__global__ void __launch_bounds__(PQ_THREADS) pq_scan_select_kernel(const PqScanArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const size_t off = ((size_t)blockIdx.y * a.nsplit + blockIdx.x) * a.k;
+  SelectSink sink(a.pool_cap, a.k, a.has_thr, a.thr_key, a.ws_kd + off, a.ws_kid + off);
+  pq_scan_rows<L2>(a, smem, blockIdx.y, blockIdx.x, sink);
+}
+// deep top-k key pass: grid (nsplit, nqc), dynamic shared memory = the LUT
+template <bool L2>
+__global__ void __launch_bounds__(PQ_THREADS) pq_key_kernel(const PqScanArgs a, const DeepKeys o) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  DeepKeySink sink(o, blockIdx.y);
+  pq_scan_rows<L2>(a, smem, blockIdx.y, blockIdx.x, sink);
+}
+
 
 // Packed codes (NBITS < 8): 128 codes of a row take exactly 4*NBITS 32-bit words, so the row is read in chunks of
 // 128 codes whose bit offsets are compile-time constants.  Chunk c of a row (words [4*NBITS*c, 4*NBITS*(c+1))) in the
@@ -281,17 +284,12 @@ __device__ __forceinline__ float pq_sum_chunk(float dis, const float* tab, const
 // The 8-bit kernel's scheme on packed rows: block (split, query), probes split round-robin, LUT [M, 2^NBITS] in shared
 // memory (L2: rebuilt per probed list), one thread per code row, the same select and range-threshold epilogue.  A LUT
 // row has at most 32 words, so the 32 lanes of a lookup touch 32 distinct banks at most: one wavefront per lookup.
-template <bool L2, int NBITS>
-__global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kernel(const PqScanArgs a) {
+template <bool L2, int NBITS, class Sink>
+__device__ __forceinline__ void pq_scan_packed_rows(const PqScanArgs& a, unsigned char* smem, const int qi, const int split, Sink& sink) {
   constexpr int KS = 1 << NBITS;
-  extern __shared__ __align__(16) unsigned char smem[];
   float* tab = reinterpret_cast<float*>(smem);
   const int M = a.M, T = M * KS, cs = a.code_size;
-  const int qi = blockIdx.y, split = blockIdx.x;
-  BlockSelect sel;
-  sel.init(smem + (size_t)T * 4, a.pool_cap, a.k);
-  if (a.has_thr && threadIdx.x == 0) { *sel.thr_d = a.thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
-  __syncthreads();
+  sink.init(smem + (size_t)T * 4);
   const float* simq = a.sim + (size_t)qi * T;
   if (!L2) {
     for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = simq[i];
@@ -309,9 +307,9 @@ __global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kern
       for (int i = threadIdx.x; i < T; i += blockDim.x) tab[i] = __fadd_rn(pl[i], __fmul_rn(-2.0f, simq[i]));
       __syncthreads();
     }
-    const long long base = a.list_off[l];
+    const long long base = a.list_off[l], pos0 = sink.list_pos(p);
     for (int r0 = 0; r0 < len; r0 += blockDim.x) {
-      sel.maybe_prune(blockDim.x);
+      sink.step(blockDim.x);
       const int r = r0 + threadIdx.x;
       if (r < len) {
         const long long row = base + r;
@@ -329,21 +327,27 @@ __global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kern
             pq_load_chunk<NBITS>(code, cs, c, w);
             dis = pq_sum_chunk<NBITS, true>(dis, tab + c * 128 * KS, w, M - c * 128);
           }
-          const uint32_t key = f2ord(L2 ? dis : -dis);
-          if (sel.passes(key, id)) sel.push(key, id);
+          sink.take(f2ord(L2 ? dis : -dis), id, pos0 + r);
         }
       }
     }
   }
-  sel.prune();
-  const int have = *sel.count;
-  uint32_t* okd = a.ws_kd + ((size_t)qi * a.nsplit + split) * a.k;
-  long long* oki = a.ws_kid + ((size_t)qi * a.nsplit + split) * a.k;
-  for (int i = threadIdx.x; i < a.k; i += blockDim.x) {
-    okd[i] = i < have ? sel.kd[i] : KEY_SENTINEL_D;
-    oki[i] = i < have ? sel.kid[i] : KEY_SENTINEL_ID;
-  }
+  sink.finish();
 }
+template <bool L2, int NBITS>
+__global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_scan_packed_kernel(const PqScanArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const size_t off = ((size_t)blockIdx.y * a.nsplit + blockIdx.x) * a.k;
+  SelectSink sink(a.pool_cap, a.k, a.has_thr, a.thr_key, a.ws_kd + off, a.ws_kid + off);
+  pq_scan_packed_rows<L2, NBITS>(a, smem, blockIdx.y, blockIdx.x, sink);
+}
+template <bool L2, int NBITS>
+__global__ void __launch_bounds__(PQP_THREADS, PQP_MIN_CTAS) pq_key_packed_kernel(const PqScanArgs a, const DeepKeys o) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  DeepKeySink sink(o, blockIdx.y);
+  pq_scan_packed_rows<L2, NBITS>(a, smem, blockIdx.y, blockIdx.x, sink);
+}
+
 
 // dis0[i] (i = query * nprobe + p) = the coarse pass's raw value (L2 distance or ip) of the query and list probes[i], for
 // probes that come from the caller (a list-sharded search merges them from several ranks, and the ABI carries list ids
@@ -363,20 +367,26 @@ __global__ void pq_dis0_kernel(const float* __restrict__ q, const float* __restr
   if (valid && t == 0) dis0[i] = L2 ? ord2f(f2ord(v)) : -ord2f(f2ord(-v));
 }
 
+// the packed-code scan of NBITS = nbits: the top-k select, or the deep key pass into *keys when keys is set
 template <bool L2>
-void launch_pq_scan_packed(int nbits, dim3 grid, size_t smem, cudaStream_t s, const PqScanArgs& a) {
-  auto go = [&](auto kern) {
+void launch_pq_scan_packed(int nbits, dim3 grid, size_t smem, cudaStream_t s, const PqScanArgs& a, const DeepKeys* keys = nullptr) {
+  auto go = [&](auto kern, auto key_kern) {
+    if (keys) {
+      B200VS_CUDA(cudaFuncSetAttribute(key_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      key_kern<<<grid, PQP_THREADS, smem, s>>>(a, *keys);
+      return;
+    }
     B200VS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     kern<<<grid, PQP_THREADS, smem, s>>>(a);
   };
   switch (nbits) {
-    case 1: go(pq_scan_packed_kernel<L2, 1>); break;
-    case 2: go(pq_scan_packed_kernel<L2, 2>); break;
-    case 3: go(pq_scan_packed_kernel<L2, 3>); break;
-    case 4: go(pq_scan_packed_kernel<L2, 4>); break;
-    case 5: go(pq_scan_packed_kernel<L2, 5>); break;
-    case 6: go(pq_scan_packed_kernel<L2, 6>); break;
-    case 7: go(pq_scan_packed_kernel<L2, 7>); break;
+    case 1: go(pq_scan_packed_kernel<L2, 1>, pq_key_packed_kernel<L2, 1>); break;
+    case 2: go(pq_scan_packed_kernel<L2, 2>, pq_key_packed_kernel<L2, 2>); break;
+    case 3: go(pq_scan_packed_kernel<L2, 3>, pq_key_packed_kernel<L2, 3>); break;
+    case 4: go(pq_scan_packed_kernel<L2, 4>, pq_key_packed_kernel<L2, 4>); break;
+    case 5: go(pq_scan_packed_kernel<L2, 5>, pq_key_packed_kernel<L2, 5>); break;
+    case 6: go(pq_scan_packed_kernel<L2, 6>, pq_key_packed_kernel<L2, 6>); break;
+    case 7: go(pq_scan_packed_kernel<L2, 7>, pq_key_packed_kernel<L2, 7>); break;
     default: fail(B200VS_EINTERNAL, "no packed-code scan kernel for this nbits");
   }
 }
@@ -727,7 +737,8 @@ struct IvfPqIndex : IndexBase {
       if (!r.range) for (int i = 0; i < 8; ++i) stats[i] = flat->stats[i].load();
       return;
     }
-    if (r.probes) check_probe_search(r.nq, r.k);
+    if (r.deep) lut_smem();
+    else if (r.probes) check_probe_search(r.nq, r.k);
     else scan_smem(r.k);  // checked before anything is launched
     const float* q = queries(r, s);
     const int nprobe = r.probes ? r.nprobe : resolve_nprobe(*r.sc);
@@ -740,6 +751,10 @@ struct IvfPqIndex : IndexBase {
       probes = own;
     }
     if (profiling) profile_probed(this, probes, r.nq * nprobe, nlist, L.d_len.p, s);
+    if (r.deep) {
+      scan_lists_deep(r.nq, q, r.k, *r.sc, probes, dis0 ? dis0 : probe_dis0(r.nq, q, probes, nprobe, s), nprobe, r.od, r.raw, r.oi, s);
+      return;
+    }
     scan_lists(r.nq, q, r.k, *r.sc, probes, dis0 ? dis0 : probe_dis0(r.nq, q, probes, nprobe, s), nprobe, r.range,
                ip_like() ? 1.0F - r.radius : r.radius, r.raw ? nullptr : r.od, r.oi, r.oc, s, r.raw ? r.od : nullptr);
   }
@@ -749,6 +764,12 @@ struct IvfPqIndex : IndexBase {
     const int threads = nbits == 8 ? PQ_THREADS : PQP_THREADS;
     const size_t smem = (size_t)M * ksub * 4 + BlockSelect::smem_bytes(select_pool_cap(k, threads));
     if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector / topk too large for the shared-memory LUT");
+    return smem;
+  }
+  // shared memory of the LUT alone (the deep key pass holds no select pool), refused above one SM's 227 KB
+  size_t lut_smem() const {
+    const size_t smem = (size_t)M * ksub * 4;
+    if (smem > 227 * 1024) fail(B200VS_EILLEGAL_PARAMETERS, "nsubvector too large for the shared-memory LUT");
     return smem;
   }
   int resolve_nprobe(const SearchCtx& sc) const {
@@ -809,6 +830,44 @@ struct IvfPqIndex : IndexBase {
     }
     B200VS_CUDA(cudaGetLastError());
     launch_count(3);
+  }
+
+  // deep top-k (run_deep) over the LUT scan: its key pass runs the scan kernels with DeepKeySink on every query chunk
+  void scan_lists_deep(int64_t nq, const float* q, int k, const SearchCtx& sc, const long long* probes, const float* coarse, int nprobe,
+                       float* od, bool raw, long long* oi, cudaStream_t s) {
+    const int T = M * ksub;
+    const size_t smem = lut_smem();
+    const bool l2 = metric == B200VS_L2;
+    float* sim = scratch.alloc<float>((size_t)nq * T);
+    pq_sim_kernel<<<(unsigned)nq, 256, 0, s>>>(q, codebooks.p, nq, dim, M, ksub, sim);
+    B200VS_CUDA(cudaGetLastError());
+    launch_count(1);
+    PqScanArgs base{};
+    base.codes = store.codes.p; base.ids = store.ids.p; base.list_off = L.d_off.p; base.list_len = L.d_len.p;
+    base.pre = l2 ? pre.p : nullptr; base.M = M; base.code_size = code_size; base.nprobe = nprobe;
+    base.filt.has_range = sc.has_range; base.filt.negate = sc.negate; base.filt.rmin = sc.rmin; base.filt.rmax = sc.rmax;
+    base.filt.sorted_ids = sc.sorted_ids_dev; base.filt.n_ids = sc.n_ids;
+    DeepJob dj;
+    dj.l2 = l2; dj.mode = 1; dj.ids = store.ids.p; dj.probes = probes; dj.nprobe = nprobe; dj.list_off = L.d_off.p; dj.list_len = L.d_len.p;
+    const int sms = device_sm_count(device);
+    run_deep(this, dj, nq, k, od, raw, oi, [&](int64_t q0, int nqc, const DeepKeys& o, cudaStream_t st) {
+      PqScanArgs a = base;
+      a.sim = sim + (size_t)q0 * T; a.probes = probes + (size_t)q0 * nprobe; a.coarse = coarse + (size_t)q0 * nprobe;
+      a.nsplit = std::max(1, std::min(nprobe, sms * 4 / nqc));
+      const dim3 grid(a.nsplit, nqc);
+      if (nbits < 8) {
+        if (l2) launch_pq_scan_packed<true>(nbits, grid, smem, st, a, &o);
+        else launch_pq_scan_packed<false>(nbits, grid, smem, st, a, &o);
+      } else if (l2) {
+        B200VS_CUDA(cudaFuncSetAttribute(pq_key_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        pq_key_kernel<true><<<grid, PQ_THREADS, smem, st>>>(a, o);
+      } else {
+        B200VS_CUDA(cudaFuncSetAttribute(pq_key_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        pq_key_kernel<false><<<grid, PQ_THREADS, smem, st>>>(a, o);
+      }
+      B200VS_CUDA(cudaGetLastError());
+      launch_count(1);
+    }, s);
   }
 
   // ---- list-sharded building blocks (include/b200vs.h), in the IVF-PQ mode only ----

@@ -20,6 +20,54 @@ static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const f
                           float* out_raw, long long* out_ids, int* out_counts, const int* qmap, const int* qcount,
                           int forced_nsplit, cudaStream_t s);
 
+// the rows, candidate space and filters of job's scan
+static ScanArgs scan_args(const ScanJob& job, const float* queries) {
+  ScanArgs a{};
+  a.vecs = job.vecs; a.ids = job.ids; a.queries = queries; a.d = job.d; a.mode = job.mode; a.n = job.n;
+  a.probes = job.probes; a.nprobe = job.nprobe; a.list_off = job.list_off; a.list_len = job.list_len;
+  a.filt.has_range = job.sc ? job.sc->has_range : 0;
+  a.filt.negate = job.sc ? job.sc->negate : 0;
+  a.filt.rmin = job.sc ? job.sc->rmin : 0;
+  a.filt.rmax = job.sc ? job.sc->rmax : 0;
+  a.filt.sorted_ids = job.sc ? job.sc->sorted_ids_dev : nullptr;
+  a.filt.n_ids = job.sc ? job.sc->n_ids : 0;
+  return a;
+}
+
+template <class Dist>
+static void launch_scan_keys(const ScanArgs& a, dim3 grid, size_t smem, const DeepKeys& o, cudaStream_t s) {
+  ensure_smem(scan_key_kernel<Dist>, smem);
+  scan_key_kernel<Dist><<<grid, SCAN_THREADS, smem, s>>>(a, o);
+  B200VS_CUDA(cudaGetLastError());
+}
+
+bool exact_select_fits(int d, int nseg, int k) {
+  return scan_smem_bytes(d, nseg, select_pool_cap(k, SCAN_THREADS)) <= (size_t)kMaxDynSmem;
+}
+
+// Deep top-k over the exact scan: its key pass runs scan_rows with DeepKeySink, each query's candidates split over enough CTAs
+// to fill the SMs (a CTA holds no select pool, so the split costs nothing but the query load)
+void run_scan_deep(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* od, bool raw, long long* oi,
+                   cudaStream_t s) {
+  DeepJob dj;
+  dj.l2 = job.l2; dj.mode = job.mode; dj.n = job.n; dj.ids = job.ids;
+  dj.probes = job.probes; dj.nprobe = job.nprobe; dj.list_off = job.list_off; dj.list_len = job.list_len;
+  const ScanArgs base = scan_args(job, queries);
+  const size_t smem = scan_key_smem_bytes(job.d, job.mode == 0 ? 1 : job.nprobe);
+  const int sms = device_sm_count(ix->device);
+  run_deep(ix, dj, nq, k, od, raw, oi, [&](int64_t q0, int nqc, const DeepKeys& o, cudaStream_t st) {
+    ScanArgs a = base;
+    a.queries = queries + (size_t)q0 * job.d;
+    if (job.mode == 1) a.probes = job.probes + (size_t)q0 * job.nprobe;
+    a.nsplit = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv(o.stride, 4096), std::max(1, sms * 8 / nqc)));
+    const dim3 grid(a.nsplit, nqc);
+    if (job.hamming) launch_scan_keys<HammingDist>(a, grid, smem, o, st);
+    else if (job.l2) launch_scan_keys<Fp32Dist<true>>(a, grid, smem, o, st);
+    else launch_scan_keys<Fp32Dist<false>>(a, grid, smem, o, st);
+    ix->launch_count(1);
+  }, s);
+}
+
 void run_scan(IndexBase* ix, const ScanJob& job, int64_t nq, const float* queries, int k, float* out_dist,
               float* out_raw, long long* out_ids, int* out_counts, cudaStream_t s) {
   run_scan_impl(ix, job, nq, queries, k, out_dist, out_raw, out_ids, out_counts, nullptr, nullptr, 0, s);
@@ -50,18 +98,10 @@ static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const f
   if (forced_nsplit > 0) nsplit = forced_nsplit;
 
   const int cap = select_pool_cap(k, SCAN_THREADS);  // SCAN_THREADS >= SCAN_QUADS: one size for both kernels
-  ScanArgs a;
-  a.vecs = job.vecs; a.ids = job.ids; a.queries = queries; a.d = job.d; a.mode = job.mode; a.n = job.n;
-  a.probes = job.probes; a.nprobe = job.nprobe; a.list_off = job.list_off; a.list_len = job.list_len;
+  ScanArgs a = scan_args(job, queries);
   a.k = k; a.nsplit = nsplit;
   a.ws_kd = ix->scratch.alloc<uint32_t>((size_t)nq * nsplit * k);
   a.ws_kid = ix->scratch.alloc<long long>((size_t)nq * nsplit * k);
-  a.filt.has_range = job.sc ? job.sc->has_range : 0;
-  a.filt.negate = job.sc ? job.sc->negate : 0;
-  a.filt.rmin = job.sc ? job.sc->rmin : 0;
-  a.filt.rmax = job.sc ? job.sc->rmax : 0;
-  a.filt.sorted_ids = job.sc ? job.sc->sorted_ids_dev : nullptr;
-  a.filt.n_ids = job.sc ? job.sc->n_ids : 0;
   a.has_thr = job.has_thr ? 1 : 0;
   a.thr_key = job.has_thr ? f2ord(job.l2 ? job.thr_raw : -job.thr_raw) : 0;
   a.pool_cap = cap;

@@ -8,6 +8,7 @@
 // They are also the rerank stage of the tensor-core candidate pass (tc_ivf.cuh) and its fallback.
 #pragma once
 #include "common.cuh"
+#include "deep_select.cuh"
 #include "filter.cuh"
 #include "select.cuh"
 
@@ -76,8 +77,10 @@ struct HammingDist {
   }
 };
 
-template <class Dist>
-static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsigned char* smem, const int slot, const int split, const int qi) {
+// The exact scan of one query's candidates [r0, r1) of split `split`: every eligible row (a live id that passes the filters)
+// goes to the sink with its key and candidate-space position.  Sink: SelectSink (top-k) or DeepKeySink (deep top-k).
+template <class Dist, class Sink>
+static __device__ __forceinline__ void scan_rows(const ScanArgs& a, unsigned char* smem, const int split, const int qi, Sink& sink) {
   const int d = a.d;
   float* qs = reinterpret_cast<float*>(smem);
   const size_t qbytes = ((size_t)d * 4 + 15) / 16 * 16;
@@ -108,10 +111,7 @@ static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsig
     __syncthreads();
     total = prefix[nseg];
   }
-  BlockSelect sel;
-  sel.init(smem + qbytes + pfbytes, a.pool_cap, a.k);  // contains a barrier (also publishes qs)
-  if (a.has_thr && threadIdx.x == 0) { *sel.thr_d = a.thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
-  __syncthreads();
+  sink.init(smem + qbytes + pfbytes);  // contains a barrier (also publishes qs)
 
   const long long r0 = total * split / a.nsplit, r1 = total * (split + 1) / a.nsplit;
   const int quad = threadIdx.x >> 2, t = threadIdx.x & 3;
@@ -130,7 +130,7 @@ static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsig
   if (r1 > r0) {
     const long long safe_row = map_row(r0);
     for (long long base = r0; base < r1; base += SCAN_QUADS) {
-      sel.maybe_prune(SCAN_QUADS);
+      sink.step(SCAN_QUADS);
       const long long i = base + quad;
       bool valid = i < r1;
       long long row = valid ? map_row(i) : safe_row;
@@ -142,20 +142,17 @@ static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsig
       if (__ballot_sync(0xffffffffu, valid) == 0u) continue;  // warp-uniform skip
       if (!valid) row = safe_row;
       const float v = Dist::eval(a.vecs, row, qs, d, t, vec);
-      if (valid && t == 0) {
-        const uint32_t key = f2ord(Dist::kL2 ? v : -v);
-        if (sel.passes(key, id)) sel.push(key, id);
-      }
+      if (valid && t == 0) sink.take(f2ord(Dist::kL2 ? v : -v), id, i);
     }
   }
-  sel.prune();
-  const int have = *sel.count;
-  uint32_t* okd = a.ws_kd + ((size_t)slot * a.nsplit + split) * a.k;
-  long long* oki = a.ws_kid + ((size_t)slot * a.nsplit + split) * a.k;
-  for (int i = threadIdx.x; i < a.k; i += blockDim.x) {
-    okd[i] = i < have ? sel.kd[i] : KEY_SENTINEL_D;
-    oki[i] = i < have ? sel.kid[i] : KEY_SENTINEL_ID;
-  }
+  sink.finish();
+}
+
+template <class Dist>
+static __device__ __forceinline__ void scan_select_body(const ScanArgs& a, unsigned char* smem, const int slot, const int split, const int qi) {
+  const size_t off = ((size_t)slot * a.nsplit + split) * a.k;
+  SelectSink sink(a.pool_cap, a.k, a.has_thr, a.thr_key, a.ws_kd + off, a.ws_kid + off);
+  scan_rows<Dist>(a, smem, split, qi, sink);
 }
 
 // Plain launch: grid (nsplit, nq).  Mapped launch (a.qcount != NULL, the re-run of uncertified queries): a small grid in y
@@ -169,6 +166,18 @@ static __global__ void __launch_bounds__(SCAN_THREADS) scan_select_kernel(const 
     scan_select_body<Dist>(a, smem, slot, blockIdx.x, a.qmap[slot]);
     __syncthreads();
   }
+}
+
+// Deep top-k key pass: grid (nsplit, nqc), the keys of query blockIdx.y's candidates [r0, r1) of split blockIdx.x.
+// Dynamic shared memory: scan_key_smem_bytes.
+inline size_t scan_key_smem_bytes(int d, int nprobe) {
+  return ((size_t)d * 4 + 15) / 16 * 16 + ((size_t)(nprobe + 1) * 4 + 15) / 16 * 16;
+}
+template <class Dist>
+static __global__ void __launch_bounds__(SCAN_THREADS) scan_key_kernel(const ScanArgs a, const DeepKeys o) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  DeepKeySink sink(o, blockIdx.y);
+  scan_rows<Dist>(a, smem, blockIdx.x, blockIdx.y, sink);
 }
 
 // Ordered range append (b200vs_scan_range_push, VectorReader::BruteForceRangeSearch): the hits of one tile are appended

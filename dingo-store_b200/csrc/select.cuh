@@ -93,6 +93,36 @@ struct BlockSelect {
   }
 };
 
+// The top-k sink of the exact scans (scan_rows, the IVF-PQ LUT scans): a BlockSelect pool, optionally with a fixed range
+// threshold, flushed to one split's partial list okd / oki [k] (sentinel-padded).  DeepKeySink (deep_select.cuh) is the
+// other sink of the same scans.
+struct SelectSink {
+  BlockSelect sel;
+  int cap, k, has_thr;
+  uint32_t thr_key;
+  uint32_t* okd;
+  long long* oki;
+  __device__ SelectSink(int cap_, int k_, int has_thr_, uint32_t thr_key_, uint32_t* okd_, long long* oki_)
+      : cap(cap_), k(k_), has_thr(has_thr_), thr_key(thr_key_), okd(okd_), oki(oki_) {}
+  // all threads call; contains a barrier
+  __device__ void init(unsigned char* pool) {
+    sel.init(pool, cap, k);
+    if (has_thr && threadIdx.x == 0) { *sel.thr_d = thr_key; *sel.thr_id = (long long)0x8000000000000000LL; }
+    __syncthreads();
+  }
+  __device__ __forceinline__ long long list_pos(int) const { return 0; }
+  __device__ __forceinline__ void step(int incoming) { sel.maybe_prune(incoming); }
+  __device__ __forceinline__ void take(uint32_t key, long long id, long long) { if (sel.passes(key, id)) sel.push(key, id); }
+  __device__ void finish() {
+    sel.prune();
+    const int have = *sel.count;
+    for (int i = threadIdx.x; i < k; i += blockDim.x) {
+      okd[i] = i < have ? sel.kd[i] : KEY_SENTINEL_D;
+      oki[i] = i < have ? sel.kid[i] : KEY_SENTINEL_ID;
+    }
+  }
+};
+
 inline int select_pool_cap(int k, int pushes_per_iter) {
   int need = k + pushes_per_iter;
   int c = next_pow2(need);

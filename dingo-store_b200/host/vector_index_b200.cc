@@ -14,6 +14,9 @@ int64_t VectorIndexB200::hnsw_device_build_min_rows = 0;
 
 namespace {
 
+// the service's top_n limit (index_service.cc:197-211): a larger topk is the reader's scalar post-filter over-fetch
+constexpr uint32_t kDeepTopkFrom = 4096;
+
 // CheckVectorDimension, src/vector/vector_index_utils.cc:502-530
 butil::Status CheckVectorDimension(const std::vector<pb::common::VectorWithId>& vs, int dimension) {
   for (const auto& v : vs) {
@@ -245,13 +248,18 @@ butil::Status VectorIndexB200::Search(const std::vector<pb::common::VectorWithId
   lf.sp.efsearch = parameter.hnsw().efsearch();
   std::vector<float> distances((size_t)topk * vs.size(), 0.0f);
   std::vector<int64_t> labels((size_t)topk * vs.size(), -1);  // flat.cc:218-219
+  // above the service's top_n limit (index_service.cc:197-211) the request is the reader's post-filter over-fetch
+  // (vector_reader.cc:119-215): the deep path, which every type but HNSW serves; HNSW keeps b200vs_search and its refusal
+  const bool deep = topk > kDeepTopkFrom && vector_index_type != pb::common::VECTOR_INDEX_TYPE_HNSW;
   int rc;
   if (binary) {
     const std::vector<uint8_t> x = ExtractBinaryVectorValue(vs, dimension_);
-    rc = b200vs_search_binary(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+    rc = (deep ? b200vs_search_binary_deep : b200vs_search_binary)(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp,
+                                                                  distances.data(), labels.data());
   } else {
     const std::vector<float> x = ExtractVectorValue(vs, dimension_);
-    rc = b200vs_search(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+    rc = (deep ? b200vs_search_deep : b200vs_search)(index_, (int64_t)vs.size(), x.data(), (int32_t)topk, &lf.sp, distances.data(),
+                                                     labels.data());
   }
   if (rc != B200VS_OK) return ToStatus(rc);
   // reconstruct: only the HNSW plugin honours it, and never for cosine (hnsw.cc:383-395, :469-472 "force reconstruct false");

@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(PKG_ROOT, "libb200vs.so")
 FLAT, IVF_FLAT, IVF_PQ, HNSW, BINARY_FLAT, BINARY_IVF_FLAT = 0, 1, 2, 3, 4, 5
 L2, IP, COSINE, HAMMING = 1, 2, 3, 4
 BINARY_TYPES = (BINARY_FLAT, BINARY_IVF_FLAT)
+DEEP_MAX_K = 40960  # B200VS_DEEP_MAX_K: the largest k of search_deep
 OK, EILLEGAL_PARAMETERS, EVECTOR_INVALID, EVECTOR_NOT_TRAIN, EVECTOR_NOT_SUPPORT, EINTERNAL, EVECTOR_ID_DUPLICATED = range(7)
 
 # every symbol include/b200vs.h declares (checked by tests/test_abi.py without a GPU)
@@ -38,7 +39,7 @@ ABI_SYMBOLS = [
     "b200vs_need_rebuild", "b200vs_rebuild_from",
     "b200vs_shard_create_binary", "b200vs_shard_train_binary", "b200vs_shard_add_binary", "b200vs_shard_add_binary_device",
     "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
-    "b200vs_shard_range_search_binary_device",
+    "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
 ]
 
 
@@ -142,6 +143,8 @@ def lib():
     L.b200vs_train_binary.argtypes = [vp, i64, vp]
     L.b200vs_add_with_ids_binary.argtypes = [vp, i64, vp, vp, ctypes.c_int]
     L.b200vs_search_binary.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_search_deep.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_search_binary_deep.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_search_binary_device.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_range_search_binary.argtypes = [vp, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_hnsw_add_batched.argtypes = [vp, i64, vp, vp, i32]
@@ -302,6 +305,17 @@ class Index:
         D = np.zeros((nq, max(k, 0)), dtype=np.float32)
         I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
         fn = self.L.b200vs_search_binary if self.binary else self.L.b200vs_search
+        _check(fn(self.h, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data, I.ctypes.data))
+        return D, I
+
+    def search_deep(self, xq, k, **kw):
+        """search() for any k up to DEEP_MAX_K (b200vs_search_deep / b200vs_search_binary_deep): the same results wherever
+        search() answers, past the shared-memory select that bounds it."""
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(k, 0)), dtype=np.float32)
+        I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
+        fn = self.L.b200vs_search_binary_deep if self.binary else self.L.b200vs_search_deep
         _check(fn(self.h, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data, I.ctypes.data))
         return D, I
 

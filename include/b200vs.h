@@ -144,6 +144,23 @@ int b200vs_set_coalescing(b200vs_index* idx, int on, int64_t stats[2]);
 int b200vs_search_device(b200vs_index* idx, int64_t nq, const float* xq_dev, int32_t k,
                          const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
 
+/* Deep top-k: exact search for any k in [1, B200VS_DEEP_MAX_K], past the shared-memory select that bounds b200vs_search
+ * (VectorReader::SearchVector over-fetches top_n x 10 rows for its scalar post-filter, vector_reader.cc:119-215, and the
+ * service allows top_n * batch <= 40960, index_service.cc:197-211).  Host pointers, the arguments of b200vs_search /
+ * b200vs_search_binary, and their results bit for bit wherever those answer: API distances (squared L2, 1 - ip, Hamming),
+ * (distance, id) order with ties to the smaller id, -1 / 0 padding past the eligible rows, the same cosine normalisation and
+ * the same probes from the index's coarse step.  Every search parameter applies (nprobe, id range, sorted id list, negate);
+ * exact_only is accepted, the deep path is always exact.  Types: FLAT, IVF_FLAT, IVF_PQ (inner Flat and IVF-PQ modes),
+ * BINARY_FLAT, BINARY_IVF_FLAT.  k <= 0: OK, nothing done; k > B200VS_DEEP_MAX_K or the wrong row type: EILLEGAL_PARAMETERS;
+ * HNSW: EVECTOR_NOT_SUPPORT.  Never coalesced; runs as an ordinary reader.  Cost: one exact-scan pass per query chunk that
+ * writes a 4-byte key per candidate, then radix-select passes over those keys (DESIGN.md 4.10).
+ * b200vs_last_search_stats[0] counts the launches of the call, [1] is 0. */
+#define B200VS_DEEP_MAX_K 40960
+int b200vs_search_deep(b200vs_index* idx, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
+                       float* out_dist, int64_t* out_ids);
+int b200vs_search_binary_deep(b200vs_index* idx, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
+                              float* out_dist, int64_t* out_ids);
+
 /* VectorIndex::RangeSearch — flat.cc:267-323, ivf_flat.cc:278-368 (HNSW: EVECTOR_NOT_SUPPORT, hnsw.cc:487-493).
  * radius in API semantics (mapped 1-r for IP/COSINE, flat.cc:282-285).  At most max_results hits per
  * query are kept (closest first); out_counts[nq] receives the per-query hit count.  Flat / IVF-Flat batches of >= 16
@@ -443,7 +460,9 @@ int b200vs_calc_distance_binary(int32_t device, int32_t nbytes, int64_t nl, cons
  *   scan_push  : one tile of scanned vectors + ids (host; any size, ids unique inside a tile) -> tile top-k on the GPU,
  *                merged into the running top-k with the (distance, id) rule;
  *   scan_finish: running top-k -> out_dist / out_ids [nq, k] (API distances ascending, -1 padded); frees the handle.
- * The result equals one Flat search over the concatenation of all tiles. */
+ * The result equals one Flat search over the concatenation of all tiles.  A k past the exact scan's shared-memory select
+ * (k > 8192 at small dim, less at large dim) takes each tile's top-k and the merge through the deep path of
+ * b200vs_search_deep, up to B200VS_DEEP_MAX_K; a larger one is refused at scan_begin with EILLEGAL_PARAMETERS. */
 typedef struct b200vs_scan b200vs_scan;
 int b200vs_scan_begin(int32_t device, b200vs_metric metric, int32_t dim, int64_t nq, const float* xq, int32_t k,
                       const b200vs_search_params* sp, b200vs_scan** out);
