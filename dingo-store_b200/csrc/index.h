@@ -370,8 +370,9 @@ struct IndexBase {
   virtual int nlist_now() const { return 1; }
   virtual int resolve_nprobe_api(const SearchCtx& sc) const { (void)sc; return 1; }
   // refusals of a search over a caller's probe table that depend only on nq, k and the trained state (IVF-PQ: the LUT + select pool
-  // must fit one SM's shared memory); a sharded search checks them on every rank before its first collective
-  virtual void check_probe_search(int64_t nq, int k) const { (void)nq; (void)k; }
+  // must fit one SM's shared memory; deep: the LUT alone, the deep key pass holds no select pool); a sharded search checks them on
+  // every rank before its first collective
+  virtual void check_probe_search(int64_t nq, int k, bool deep = false) const { (void)nq; (void)k; (void)deep; }
   // b200vs_debug_tc_scores: xq device (raw), outputs host [nq, count() + deleted_count()] and [nq]
   virtual void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) {
     (void)nq; (void)xq; (void)arith; (void)out_scores; (void)out_eps; (void)s;

@@ -883,10 +883,11 @@ struct IvfPqIndex : IndexBase {
   }
   // refusals of a probe-driven search that depend on its arguments and the trained state only: a sharded search checks them
   // before its first collective
-  void check_probe_search(int64_t nq, int k) const override {
+  void check_probe_search(int64_t nq, int k, bool deep = false) const override {
     require_lists();
     if (nq > 65535) fail(B200VS_EILLEGAL_PARAMETERS, "batch too large (max 65535 queries per call)");
-    scan_smem(k);
+    if (deep) lut_smem();
+    else scan_smem(k);
   }
   // dis0 of every (query, probe) of a caller-supplied probe table
   const float* probe_dis0(int64_t nq, const float* q, const long long* probes, int nprobe, cudaStream_t s) {

@@ -156,6 +156,52 @@ merge_packed_warp_kernel(const TopkRec* __restrict__ parts, int world, long long
   for (int i = min(m, k) + lane; i < k; i += 32) { out_dist[(size_t)q * k + i] = 0.f; out_ids[(size_t)q * k + i] = -1; }
 }
 
+// One round of the deep merge's pairwise tree: runs in [nruns, nqc, k], each ascending by (f2ord(key), id) with id < 0
+// padding at its tail; run i of the output [cdiv(nruns, 2), nqc, k] is the first k records of runs (2i, 2i + 1) in
+// (f2ord(key), id, run) order (a last run without a partner is copied).  Record j of a run lands at j + its rank in the
+// partner run: a lower bound from the left run, an upper bound from the right one, so equal records keep run order, every
+// output slot is written once and the padding lands at the tail.  A record that cannot land below k stops its search at
+// k - j.  FINAL: the output is the last round's single run, written as (distance, id) into od / oi [nqc, k] with -1 / 0 padding.
+// Grid (cdiv(k, MERGE_RUN_THREADS), cdiv(nruns, 2), nqc).
+constexpr int MERGE_RUN_THREADS = 256;
+__device__ __forceinline__ bool rec_less(const TopkRec& a, const TopkRec& b) {  // padding after every record
+  if (a.id < 0) return false;
+  if (b.id < 0) return true;
+  return key_less(f2ord(a.dist), a.id, f2ord(b.dist), b.id);
+}
+template <bool FINAL>
+static __global__ void __launch_bounds__(MERGE_RUN_THREADS)
+merge_runs_kernel(const TopkRec* __restrict__ in, int nruns, int nqc, int k, TopkRec* out, float* od, long long* oi) {
+  const int j = blockIdx.x * MERGE_RUN_THREADS + threadIdx.x;
+  if (j >= k) return;
+  const int pair = blockIdx.y, q = blockIdx.z;
+  const TopkRec* a = in + ((size_t)(2 * pair) * nqc + q) * k;
+  const TopkRec* b = a + (size_t)nqc * k;
+  const bool has_b = 2 * pair + 1 < nruns;
+  const size_t o = ((size_t)pair * nqc + q) * k;
+  auto emit = [&](int pos, TopkRec r) {
+    if (pos >= k) return;
+    if (r.id < 0) { r.dist = 0.f; r.id = -1; }
+    if (FINAL) { od[o + pos] = r.dist; oi[o + pos] = r.id; }
+    else out[o + pos] = r;
+  };
+  const TopkRec ra = a[j];
+  if (!has_b) { emit(j, ra); return; }
+  int lo = 0, hi = k - j;  // a[j]: the records of b strictly before it
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (rec_less(b[mid], ra)) lo = mid + 1; else hi = mid;
+  }
+  emit(j + lo, ra);
+  const TopkRec rb = b[j];
+  lo = 0; hi = k - j;  // b[j]: the records of a not after it
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (!rec_less(rb, a[mid])) lo = mid + 1; else hi = mid;
+  }
+  emit(j + lo, rb);
+}
+
 static __global__ void unpack_parts_kernel(const TopkRec* __restrict__ parts, long long n, float* d, long long* id) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -487,15 +533,82 @@ void check(const Status& st) {
   if (st.code != B200VS_OK) fail(st.code, st.msg);
 }
 
+// Step 3 of a top-k or range read: ONE all-gather of the packed per-shard results L.od / L.oi [nq, k], then the k-way merge
+// into out_* [nq, k].
+void gather_merge(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int k, float* out_dist, long long* out_ids, cudaStream_t s) {
+  IndexBase* ix = sh->ix;
+  const int W = sh->world, r = sh->rank;
+  const long long nk = (long long)nq * k;
+  L.parts.reserve((size_t)W * nk, 0, s);
+  ix->phase(IndexBase::PH_MERGE, s);
+  pack_topk_kernel<<<(unsigned)cdiv(nk, 256), 256, 0, s>>>(L.od.p, L.oi.p, nk, L.parts.p + (size_t)r * nk);
+  ix->phase(IndexBase::PH_COMM, s);
+  if (W > 1) B200VS_NCCL(nccl().AllGather(L.parts.p + (size_t)r * nk, L.parts.p, (size_t)nk * sizeof(TopkRec), ncclUint8, L.comm, s));
+  ix->phase(IndexBase::PH_MERGE, s);
+  if (W * k <= MERGE_MAX) {
+    merge_packed_warp_kernel<<<(unsigned)cdiv(nq, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(L.parts.p, W, nq, k, out_dist, out_ids);
+  } else {  // wide merges: unpack and use the block merge kernel
+    float* pd = ix->scratch.alloc<float>((size_t)W * nk);
+    long long* pi = ix->scratch.alloc<long long>((size_t)W * nk);
+    unpack_parts_kernel<<<(unsigned)cdiv(W * nk, 256), 256, 0, s>>>(L.parts.p, W * nk, pd, pi);
+    launch_merge_api(W, nq, k, pd, pi, out_dist, out_ids, s);
+  }
+  B200VS_CUDA(cudaGetLastError());
+  ix->phase(IndexBase::PH_OTHER, s);
+  ix->launch_count(3);
+}
+
+// Step 3 of a deep read, whose k is bounded by kDeepMaxK and not by shared memory: the per-shard results are gathered and
+// merged one query chunk at a time, nqc queries from (W, k, nq) alone so that every rank agrees, with the gathered records
+// W * nqc * k * 16 B within the deep path's 1 GiB budget (W = 8, k = 40960: 204 queries).  Each chunk: pack, one
+// all-gather, then ceil(log2 W) rounds of merge_runs_kernel (one copy round when W = 1), ping-ponging between L.parts and
+// a scratch buffer of ceil(W / 2) runs when W > 2.
+void gather_merge_runs(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int k, float* out_dist, long long* out_ids, cudaStream_t s) {
+  IndexBase* ix = sh->ix;
+  const int W = sh->world, r = sh->rank;
+  const long long run_bytes = (long long)W * k * (long long)sizeof(TopkRec);
+  const int64_t nqc_max = std::max<int64_t>(1, std::min<int64_t>({nq, (1LL << 30) / run_bytes, 65535}));
+  L.parts.reserve((size_t)W * nqc_max * k, 0, s);
+  TopkRec* tmp = W > 2 ? ix->scratch.alloc<TopkRec>((size_t)((W + 1) / 2) * nqc_max * k) : nullptr;  // W <= 2: one final round
+  for (int64_t q0 = 0; q0 < nq; q0 += nqc_max) {
+    const int nqc = (int)std::min<int64_t>(nqc_max, nq - q0);
+    const long long nk = (long long)nqc * k;
+    ix->phase(IndexBase::PH_MERGE, s);
+    pack_topk_kernel<<<(unsigned)cdiv(nk, 256), 256, 0, s>>>(L.od.p + (size_t)q0 * k, L.oi.p + (size_t)q0 * k, nk, L.parts.p + (size_t)r * nk);
+    ix->phase(IndexBase::PH_COMM, s);
+    if (W > 1) B200VS_NCCL(nccl().AllGather(L.parts.p + (size_t)r * nk, L.parts.p, (size_t)nk * sizeof(TopkRec), ncclUint8, L.comm, s));
+    ix->phase(IndexBase::PH_MERGE, s);
+    const TopkRec* in = L.parts.p;
+    int runs = W, launches = 1;
+    for (;;) {
+      const int pairs = (runs + 1) / 2;
+      const dim3 grid((unsigned)cdiv(k, MERGE_RUN_THREADS), (unsigned)pairs, (unsigned)nqc);
+      if (pairs == 1) {
+        merge_runs_kernel<true><<<grid, MERGE_RUN_THREADS, 0, s>>>(in, runs, nqc, k, nullptr, out_dist + (size_t)q0 * k, out_ids + (size_t)q0 * k);
+        ++launches;
+        break;
+      }
+      TopkRec* out = in == L.parts.p ? tmp : L.parts.p;
+      merge_runs_kernel<false><<<grid, MERGE_RUN_THREADS, 0, s>>>(in, runs, nqc, k, out, nullptr, nullptr);
+      ++launches;
+      in = out;
+      runs = pairs;
+    }
+    B200VS_CUDA(cudaGetLastError());
+    ix->launch_count(launches);
+  }
+  ix->phase(IndexBase::PH_OTHER, s);
+}
+
 // The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
 // on stream s.  local(r) is step 2: r is this rank's search of k results per query into L.od / L.oi, which local completes
 // and runs, so that they hold ascending, -1-padded [nq, k] (key, id) lists, the key being what the merge orders by.
 // List-sharded: r searches the prepared queries over the gathered probe table L.probes.  Row-sharded: there is no coarse
 // step, and r searches the raw queries (the rank's index prepares them).  Queries are rows of query_row_bytes(): FP32, or
-// packed bits on a binary index.
+// packed bits on a binary index.  deep: step 3 is gather_merge_runs instead of gather_merge.
 template <class LocalScan>
 void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
-                  float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local) {
+                  float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local, bool deep = false) {
   IndexBase* ix = sh->ix;
   const int W = sh->world, r = sh->rank;
   const size_t qb = ix->query_row_bytes();
@@ -525,25 +638,9 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const vo
   req.nq = nq; req.xq = q; req.k = k; req.sc = &sc; req.od = L.od.p; req.oi = L.oi.p;
   if (!sh->rows) { req.prepared = true; req.probes = L.probes.p; req.nprobe = nprobe; }
   local(req);
-  // 3) ONE all-gather of the packed per-shard top-k + merge
-  const long long nk = (long long)nq * k;
-  L.parts.reserve((size_t)W * nk, 0, s);
-  ix->phase(IndexBase::PH_MERGE, s);
-  pack_topk_kernel<<<(unsigned)cdiv(nk, 256), 256, 0, s>>>(L.od.p, L.oi.p, nk, L.parts.p + (size_t)r * nk);
-  ix->phase(IndexBase::PH_COMM, s);
-  if (W > 1) B200VS_NCCL(nccl().AllGather(L.parts.p + (size_t)r * nk, L.parts.p, (size_t)nk * sizeof(TopkRec), ncclUint8, L.comm, s));
-  ix->phase(IndexBase::PH_MERGE, s);
-  if (W * k <= MERGE_MAX) {
-    merge_packed_warp_kernel<<<(unsigned)cdiv(nq, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(L.parts.p, W, nq, k, out_dist, out_ids);
-  } else {  // wide merges: unpack and use the block merge kernel
-    float* pd = ix->scratch.alloc<float>((size_t)W * nk);
-    long long* pi = ix->scratch.alloc<long long>((size_t)W * nk);
-    unpack_parts_kernel<<<(unsigned)cdiv(W * nk, 256), 256, 0, s>>>(L.parts.p, W * nk, pd, pi);
-    launch_merge_api(W, nq, k, pd, pi, out_dist, out_ids, s);
-  }
-  B200VS_CUDA(cudaGetLastError());
-  ix->phase(IndexBase::PH_OTHER, s);
-  ix->launch_count(3);
+  // 3) the all-gather of the packed per-shard results + merge
+  if (deep) gather_merge_runs(sh, L, nq, k, out_dist, out_ids, s);
+  else gather_merge(sh, L, nq, k, out_dist, out_ids, s);
   if (!L.done) B200VS_CUDA(cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming));
   B200VS_CUDA(cudaEventRecord(L.done, s));
   L.last = s;
@@ -564,6 +661,27 @@ void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
     if (flat_ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
   });
   if (flat_ip) {
+    ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
+    B200VS_CUDA(cudaGetLastError());
+    ix->launch_count(1);
+  }
+  ix->phases_finish(s);
+}
+
+// deep top-k: the rank's deep search (run_deep) keyed the way the single-index deep path orders its output (float types: the
+// raw metric value, then -ip for IP / cosine; binary types: the Hamming distance), the sorted runs merged chunk by chunk
+// (gather_merge_runs), then the API distance as deep_emit_kernel forms it.  Never keyed on the API distance: two distinct
+// inner products can round to the same 1 - ip, which run_deep orders by -ip and an API-distance merge would order by id.
+void shard_deep_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
+                       float* out_dist, long long* out_ids, cudaStream_t s) {
+  IndexBase* ix = sh->ix;
+  const bool ip = ix->ip_like();
+  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](SearchReq& r) {
+    r.deep = true; r.raw = !ix->binary();
+    ix->search(r, s);
+    if (ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
+  }, true);
+  if (ip) {
     ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
     B200VS_CUDA(cudaGetLastError());
     ix->launch_count(1);
@@ -602,6 +720,14 @@ bool check_shard_topk(int64_t nq, const void* xq, int k, const void* od, const v
   if (!od || !oi) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
   return true;
 }
+// deep top-k: b200vs_search_deep's refusals, in its order
+bool check_shard_deep(const IndexBase* ix, int64_t nq, const void* xq, int k, const void* od, const void* oi) {
+  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+  if (k <= 0) return false;
+  if (k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
+  if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "deep top-k is not implemented for HNSW");
+  return check_shard_topk(nq, xq, k, od, oi);
+}
 bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, float radius, int max_results, const void* od, const void* oi,
                        const void* oc) {
   if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
@@ -618,7 +744,8 @@ bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, float ra
 // body(lane, s).  The lane is released before the host waits for a null-stream call, so the lane's next batch may be
 // enqueued behind this one.
 template <class Refuse, class Body>
-void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, const b200vs_search_params* sp, Refuse refuse, Body body) {
+void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, const b200vs_search_params* sp, Refuse refuse, Body body,
+                bool deep = false) {
   IndexBase* ix = sh->ix;
   cudaStream_t s;
   {
@@ -628,7 +755,7 @@ void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, 
     ix->set_device();
     s = stream ? (cudaStream_t)stream : sl.lane->own;
     LaneGuard lane(ix, s);
-    ix->check_probe_search(nq, k);
+    ix->check_probe_search(nq, k, deep);
     if (sh->rows) ix->check_row_search(k, sp);
     ix->reset_stats();
     body(*sl.lane, s);
@@ -1442,25 +1569,28 @@ int shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq
   });
 }
 
-// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).
+// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).  deep:
+// b200vs_shard_search_deep / b200vs_shard_search_binary_deep.
 int shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
-                 int64_t* out_ids, bool binary_call) {
+                 int64_t* out_ids, bool binary_call, bool deep = false) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
     shard_read(sh, seq, nullptr, nq, k, sp,
                [&] {
                  check_row_type(sh, binary_call);
-                 return check_shard_topk(nq, xq, k, out_dist, out_ids);
+                 return deep ? check_shard_deep(sh->ix, nq, xq, k, out_dist, out_ids) : check_shard_topk(nq, xq, k, out_dist, out_ids);
                },
                [&](b200vs_shard::SLane& L, cudaStream_t s) {
                  IndexBase* ix = sh->ix;
                  const void* q = upload_batch(sh, L, nq, xq, s);
                  float* dd = ix->scratch.alloc<float>((size_t)nq * k);
                  long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-                 shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
+                 if (deep) shard_deep_stream(sh, L, nq, q, k, sp, dd, di, s);
+                 else shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
                  B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
                  B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-               });
+               },
+               deep);
     return B200VS_OK;
   });
 }
@@ -1664,6 +1794,15 @@ int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* x
 int b200vs_shard_search_binary(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
                                float* out_dist, int64_t* out_ids) {
   return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, true);
+}
+
+int b200vs_shard_search_deep(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
+                             float* out_dist, int64_t* out_ids) {
+  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, false, true);
+}
+int b200vs_shard_search_binary_deep(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
+                                    float* out_dist, int64_t* out_ids) {
+  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, true, true);
 }
 
 int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, float radius, int32_t max_results,

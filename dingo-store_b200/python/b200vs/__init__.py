@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_create_binary", "b200vs_shard_train_binary", "b200vs_shard_add_binary", "b200vs_shard_add_binary_device",
     "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
     "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
+    "b200vs_shard_search_deep", "b200vs_shard_search_binary_deep",
 ]
 
 
@@ -163,6 +164,8 @@ def lib():
     L.b200vs_shard_search_binary_device.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_shard_range_search_binary.argtypes = [vp, i64, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_shard_range_search_binary_device.argtypes = [vp, i64, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp, vp]
+    L.b200vs_shard_search_deep.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_shard_search_binary_deep.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     _lib = L
     return L
 
@@ -543,6 +546,17 @@ class Shard:
         _check(lib().b200vs_shard_search(self.h, seq, nq, xq.ctypes.data, k, ctypes.byref(sp), D.ctypes.data, I.ctypes.data))
         return D, I
 
+    def search_deep(self, xq, k, seq=-1, **kw):
+        """b200vs_shard_search_deep: search() for any k up to DEEP_MAX_K, equal to Index.search_deep on the unsharded index."""
+        xq = _f32(xq)
+        nq = xq.shape[0]
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(k, 0)), dtype=np.float32)
+        I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
+        _check(lib().b200vs_shard_search_deep(self.h, seq, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data,
+                                              I.ctypes.data))
+        return D, I
+
     def search_raw(self, nq, xq_ptr, k, out_dist_ptr, out_ids_ptr, sp=None, seq=-1):
         _check(lib().b200vs_shard_search(self.h, seq, nq, xq_ptr, k, ctypes.byref(sp) if sp is not None else None, out_dist_ptr, out_ids_ptr))
 
@@ -603,6 +617,16 @@ class BinaryShard(Shard):
         I = np.full((nq, k), -1, dtype=np.int64)
         _check(lib().b200vs_shard_search_binary(self.h, seq, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp),
                                                 D.ctypes.data, I.ctypes.data))
+        return D, I
+
+    def search_deep(self, xq, k, seq=-1, **kw):
+        """b200vs_shard_search_binary_deep: search() for any k up to DEEP_MAX_K, equal to Index.search_deep on the unsharded index."""
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(k, 0)), dtype=np.float32)
+        I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
+        _check(lib().b200vs_shard_search_binary_deep(self.h, seq, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp),
+                                                     D.ctypes.data, I.ctypes.data))
         return D, I
 
     def search_raw(self, nq, xq_ptr, k, out_dist_ptr, out_ids_ptr, sp=None, seq=-1):

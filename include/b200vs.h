@@ -397,6 +397,23 @@ int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const floa
                         float* out_dist, int64_t* out_ids);
 int b200vs_shard_search_device(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq_dev, int32_t k,
                                const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream);
+/* shard_search_deep / shard_search_binary_deep: b200vs_search_deep / b200vs_search_binary_deep over the sharded index, for
+ * any k in [1, B200VS_DEEP_MAX_K].  Host pointers; collective reads in shard_search's flow (same sequence numbers, lanes and
+ * communicators: deep, top-k and range batches may be interleaved).  Types: list-sharded IVF_FLAT, IVF_PQ and
+ * BINARY_IVF_FLAT, row-sharded FLAT and BINARY_FLAT.  Each rank runs the deep path on its lists or rows, keyed the way the
+ * single-index deep path orders its output (L2 distance | -ip | Hamming distance, then id); the per-rank sorted runs are
+ * all-gathered one query chunk at a time (at most 1 GiB of 16-byte records per chunk on each rank) and merged by a pairwise
+ * merge tree with no shared-memory bound on k (DESIGN.md 4.5, 4.10).  Results (distances, ids, -1 / 0 padding) equal
+ * b200vs_search_deep / b200vs_search_binary_deep bit for bit on one unsharded index holding every rank's rows with the same
+ * trained state, and b200vs_shard_search wherever that answers.  Refused on every rank before the first collective, a refused
+ * call still using up its sequence number: k > B200VS_DEEP_MAX_K, null outputs, a float call on a binary shard or the
+ * reverse, and (IVF_PQ) a LUT alone larger than one SM's shared memory: EILLEGAL_PARAMETERS; row-sharded HNSW:
+ * EVECTOR_NOT_SUPPORT.  k <= 0: OK, nothing done.  b200vs_last_search_stats[0] counts the call's launches; with profiling
+ * on, phase slots [10] (collectives) and [11] (pack + merge) are filled as for shard_search. */
+int b200vs_shard_search_deep(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
+                             float* out_dist, int64_t* out_ids);
+int b200vs_shard_search_binary_deep(b200vs_shard* shard, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k,
+                                    const b200vs_search_params* sp, float* out_dist, int64_t* out_ids);
 /* shard_range_search[_device]: b200vs_range_search over the sharded index, in shard_search's flow (same sequence numbers,
  * lanes and communicators: range and top-k batches may be interleaved).  Step 2 is the range scan of the owned probed lists
  * (IVF_FLAT: the tile range scan; IVF_PQ: the thresholded LUT scan); the all-gathered payload is nq * max_results * 16 bytes
