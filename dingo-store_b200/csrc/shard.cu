@@ -209,16 +209,16 @@ static __global__ void unpack_parts_kernel(const TopkRec* __restrict__ parts, lo
   d[i] = r.dist; id[i] = r.id;
 }
 
-// merged range results: key (L2 distance | -ip | Hamming distance) -> API distance (L2 distance | 1 - ip | Hamming distance,
-// as the single-index finish computes it; ip = 1: the IP / cosine key); counts[q] = merged rows of query q (the rows are
-// ascending with -1 padding at the end)
-static __global__ void range_finish_kernel(float* dist, const long long* __restrict__ ids, long long nq, int k, int ip, int* counts) {
+// The finish of a merged read [nq, k] (merge_key in the read section): ip = 1, the merged key -ip -> the API distance 1 - ip,
+// rounded as the single-index finish rounds it; counts (range, else null): counts[q] = merged rows of query q (the rows are
+// ascending with -1 padding at the end).
+static __global__ void merge_finish_kernel(float* dist, const long long* __restrict__ ids, long long nq, int k, int ip, int* counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nq * k) return;
   const int j = (int)(i % k);
   const bool hit = ids[i] >= 0;
   if (hit && ip) dist[i] = __fsub_rn(1.0f, -dist[i]);
-  if (hit ? (j == k - 1 || ids[i + 1] < 0) : j == 0) counts[i / k] = hit ? j + 1 : 0;
+  if (counts && (hit ? (j == k - 1 || ids[i + 1] < 0) : j == 0)) counts[i / k] = hit ? j + 1 : 0;
 }
 
 static __global__ void fill_ll_kernel(long long* p, long long n, long long v) {
@@ -229,12 +229,6 @@ static __global__ void fill_ll_kernel(long long* p, long long n, long long v) {
 static __global__ void count_lists_kernel(const long long* __restrict__ lists, long long n, int nlist, unsigned long long* counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { const long long l = lists[i]; if (l >= 0 && l < nlist) atomicAdd(counts + l, 1ULL); }
-}
-
-// merged Flat IP / cosine results: key -ip -> API distance 1 - ip, rounded as the single-index finish rounds it
-static __global__ void ip_key_to_api_kernel(float* dist, const long long* __restrict__ ids, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && ids[i] >= 0) dist[i] = __fsub_rn(1.0f, -dist[i]);
 }
 
 constexpr int ROUTE_MAX_WORLD = 1024;  // ranks of a sharded index (the routing kernels' shared-memory table)
@@ -533,66 +527,84 @@ void check(const Status& st) {
   if (st.code != B200VS_OK) fail(st.code, st.msg);
 }
 
-// Step 3 of a top-k or range read: ONE all-gather of the packed per-shard results L.od / L.oi [nq, k], then the k-way merge
-// into out_* [nq, k].
-void gather_merge(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int k, float* out_dist, long long* out_ids, cudaStream_t s) {
-  IndexBase* ix = sh->ix;
-  const int W = sh->world, r = sh->rank;
-  const long long nk = (long long)nq * k;
-  L.parts.reserve((size_t)W * nk, 0, s);
-  ix->phase(IndexBase::PH_MERGE, s);
-  pack_topk_kernel<<<(unsigned)cdiv(nk, 256), 256, 0, s>>>(L.od.p, L.oi.p, nk, L.parts.p + (size_t)r * nk);
-  ix->phase(IndexBase::PH_COMM, s);
-  if (W > 1) B200VS_NCCL(nccl().AllGather(L.parts.p + (size_t)r * nk, L.parts.p, (size_t)nk * sizeof(TopkRec), ncclUint8, L.comm, s));
-  ix->phase(IndexBase::PH_MERGE, s);
-  if (W * k <= MERGE_MAX) {
-    merge_packed_warp_kernel<<<(unsigned)cdiv(nq, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(L.parts.p, W, nq, k, out_dist, out_ids);
-  } else {  // wide merges: unpack and use the block merge kernel
-    float* pd = ix->scratch.alloc<float>((size_t)W * nk);
-    long long* pi = ix->scratch.alloc<long long>((size_t)W * nk);
-    unpack_parts_kernel<<<(unsigned)cdiv(W * nk, 256), 256, 0, s>>>(L.parts.p, W * nk, pd, pi);
-    launch_merge_api(W, nq, k, pd, pi, out_dist, out_ids, s);
-  }
-  B200VS_CUDA(cudaGetLastError());
-  ix->phase(IndexBase::PH_OTHER, s);
-  ix->launch_count(3);
+// One sharded read, as its extern "C" entry point passes it.  k: results per query (range: max_results).  on_device: xq and
+// the outputs are device pointers and the read runs on `stream` (null: the lane's own stream); else they are host pointers,
+// every rank passes the SAME batch (upload_batch), and the call returns with the results on the host.
+enum ReadKind { READ_TOPK, READ_DEEP, READ_RANGE };
+struct ShardRead {
+  ReadKind kind;
+  bool binary_call;  // a b200vs_shard_*_binary* entry point: packed queries
+  bool on_device;
+  void* stream;
+  int64_t seq, nq;
+  const void* xq;
+  float radius;  // range
+  int k;
+  const b200vs_search_params* sp;
+  float* od;
+  int64_t* oi;
+  int32_t* oc;   // range: merged rows per query
+};
+
+// The merge key rule of every sharded read (the table of DESIGN.md 4.5): what each rank's results are keyed on for the pack
+// and the merge, and what merge_finish_kernel does to the merged key.  The single-index select ranks IP / cosine hits by
+// -ip, and two distinct inner products can round to the same 1 - ip (near ip = 2^-10 the spacing of ip is 2^-34 and that of
+// 1 - ip 2^-24), which a merge on the API distance would choose and order by id.  So the reads that equal their single-index
+// call bit for bit (row-sharded FLAT top-k, deep on the float types, range) ask for the raw value (raw), negate ip to -ip
+// before the pack and form 1 - ip after the merge with the single index's own __fsub_rn (neg).  The list-sharded float
+// top-k keeps the API distance: it merges by MergeSearchResults' rule (the regions' results on the distance they return),
+// and another key would change which of two such rows it returns.  HNSW keys on hnsw_distance (L2 distance | 1 - ip), the
+// distance its walk ranks by; its search refuses raw.  The Hamming distance is exact and is the API distance.
+struct MergeKey { bool raw, neg; };
+MergeKey merge_key(const b200vs_shard* sh, ReadKind kind) {
+  const IndexBase* ix = sh->ix;
+  const bool raw = kind == READ_RANGE || (kind == READ_DEEP && !ix->binary()) || (sh->rows && ix->type == B200VS_FLAT);
+  return {raw, raw && ix->ip_like()};  // a binary index's metric is Hamming
 }
 
-// Step 3 of a deep read, whose k is bounded by kDeepMaxK and not by shared memory: the per-shard results are gathered and
-// merged one query chunk at a time, nqc queries from (W, k, nq) alone so that every rank agrees, with the gathered records
-// W * nqc * k * 16 B within the deep path's 1 GiB budget (W = 8, k = 40960: 204 queries).  Each chunk: pack, one
-// all-gather, then ceil(log2 W) rounds of merge_runs_kernel (one copy round when W = 1), ping-ponging between L.parts and
-// a scratch buffer of ceil(W / 2) runs when W > 2.
-void gather_merge_runs(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int k, float* out_dist, long long* out_ids, cudaStream_t s) {
+// Step 3 of a sharded read: the per-shard results L.od / L.oi [nq, k] are packed into 16-byte records, all-gathered and
+// merged into out_* [nq, k], one query chunk at a time.  Top-k and range: the whole batch is one chunk, so ONE all-gather.
+// Deep, whose k is bounded by kDeepMaxK and not by shared memory: nqc queries per chunk from (W, k, nq) alone so that every
+// rank agrees, with the gathered records W * nqc * k * 16 B within the deep path's 1 GiB budget (W = 8, k = 40960: 204
+// queries).  The merge of a chunk: deep, ceil(log2 W) rounds of merge_runs_kernel (one copy round when W = 1), ping-ponging
+// between L.parts and a scratch buffer of ceil(W / 2) runs when W > 2; else the warp merge when W * k <= MERGE_MAX, or
+// unpack and the block merge.
+void gather_merge(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int k, bool deep, float* out_dist, long long* out_ids,
+                  cudaStream_t s) {
   IndexBase* ix = sh->ix;
   const int W = sh->world, r = sh->rank;
   const long long run_bytes = (long long)W * k * (long long)sizeof(TopkRec);
-  const int64_t nqc_max = std::max<int64_t>(1, std::min<int64_t>({nq, (1LL << 30) / run_bytes, 65535}));
+  const int64_t nqc_max = deep ? std::max<int64_t>(1, std::min<int64_t>({nq, (1LL << 30) / run_bytes, 65535})) : nq;
   L.parts.reserve((size_t)W * nqc_max * k, 0, s);
-  TopkRec* tmp = W > 2 ? ix->scratch.alloc<TopkRec>((size_t)((W + 1) / 2) * nqc_max * k) : nullptr;  // W <= 2: one final round
+  TopkRec* tmp = deep && W > 2 ? ix->scratch.alloc<TopkRec>((size_t)((W + 1) / 2) * nqc_max * k) : nullptr;  // W <= 2: one final round
   for (int64_t q0 = 0; q0 < nq; q0 += nqc_max) {
-    const int nqc = (int)std::min<int64_t>(nqc_max, nq - q0);
+    const int64_t nqc = std::min<int64_t>(nqc_max, nq - q0);
     const long long nk = (long long)nqc * k;
+    float* od = out_dist + (size_t)q0 * k;
+    long long* oi = out_ids + (size_t)q0 * k;
     ix->phase(IndexBase::PH_MERGE, s);
     pack_topk_kernel<<<(unsigned)cdiv(nk, 256), 256, 0, s>>>(L.od.p + (size_t)q0 * k, L.oi.p + (size_t)q0 * k, nk, L.parts.p + (size_t)r * nk);
     ix->phase(IndexBase::PH_COMM, s);
     if (W > 1) B200VS_NCCL(nccl().AllGather(L.parts.p + (size_t)r * nk, L.parts.p, (size_t)nk * sizeof(TopkRec), ncclUint8, L.comm, s));
     ix->phase(IndexBase::PH_MERGE, s);
-    const TopkRec* in = L.parts.p;
-    int runs = W, launches = 1;
-    for (;;) {
-      const int pairs = (runs + 1) / 2;
-      const dim3 grid((unsigned)cdiv(k, MERGE_RUN_THREADS), (unsigned)pairs, (unsigned)nqc);
-      if (pairs == 1) {
-        merge_runs_kernel<true><<<grid, MERGE_RUN_THREADS, 0, s>>>(in, runs, nqc, k, nullptr, out_dist + (size_t)q0 * k, out_ids + (size_t)q0 * k);
-        ++launches;
-        break;
+    int launches = 3;  // b200vs_last_search_stats[0]: 3 for a top-k or range merge, whichever kernels it takes
+    if (deep) {  // the pack, the rounds of more than one pair, the final round into out_*
+      const unsigned kb = (unsigned)cdiv(k, MERGE_RUN_THREADS);
+      const TopkRec* in = L.parts.p;
+      int runs = W;
+      for (launches = 2; runs > 2; runs = (runs + 1) / 2, ++launches) {
+        TopkRec* out = in == L.parts.p ? tmp : L.parts.p;
+        merge_runs_kernel<false><<<dim3(kb, (runs + 1) / 2, (unsigned)nqc), MERGE_RUN_THREADS, 0, s>>>(in, runs, (int)nqc, k, out, nullptr, nullptr);
+        in = out;
       }
-      TopkRec* out = in == L.parts.p ? tmp : L.parts.p;
-      merge_runs_kernel<false><<<grid, MERGE_RUN_THREADS, 0, s>>>(in, runs, nqc, k, out, nullptr, nullptr);
-      ++launches;
-      in = out;
-      runs = pairs;
+      merge_runs_kernel<true><<<dim3(kb, 1, (unsigned)nqc), MERGE_RUN_THREADS, 0, s>>>(in, runs, (int)nqc, k, nullptr, od, oi);
+    } else if (W * k <= MERGE_MAX) {
+      merge_packed_warp_kernel<<<(unsigned)cdiv(nqc, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(L.parts.p, W, nqc, k, od, oi);
+    } else {  // wide merges: unpack and use the block merge kernel
+      float* pd = ix->scratch.alloc<float>((size_t)W * nk);
+      long long* pi = ix->scratch.alloc<long long>((size_t)W * nk);
+      unpack_parts_kernel<<<(unsigned)cdiv(W * nk, 256), 256, 0, s>>>(L.parts.p, W * nk, pd, pi);
+      launch_merge_api(W, nqc, k, pd, pi, od, oi, s);
     }
     B200VS_CUDA(cudaGetLastError());
     ix->launch_count(launches);
@@ -600,20 +612,20 @@ void gather_merge_runs(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, int
   ix->phase(IndexBase::PH_OTHER, s);
 }
 
-// The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device)
-// on stream s.  local(r) is step 2: r is this rank's search of k results per query into L.od / L.oi, which local completes
-// and runs, so that they hold ascending, -1-padded [nq, k] (key, id) lists, the key being what the merge orders by.
-// List-sharded: r searches the prepared queries over the gathered probe table L.probes.  Row-sharded: there is no coarse
-// step, and r searches the raw queries (the rank's index prepares them).  Queries are rows of query_row_bytes(): FP32, or
-// packed bits on a binary index.  deep: step 3 is gather_merge_runs instead of gather_merge.
-template <class LocalScan>
-void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
-                  float* out_dist, long long* out_ids, cudaStream_t s, LocalScan local, bool deep = false) {
+// The flow of a sharded read: queries (all nq of them, raw) are on the device in `xq`; merged results land in out_* (device;
+// out_counts: range only) on stream s.  Step 2 is this rank's one search request, keyed by merge_key, into L.od / L.oi:
+// ascending, -1-padded [nq, k] (key, id) lists.  List-sharded: it searches the prepared queries over the gathered probe
+// table L.probes.  Row-sharded: there is no coarse step, and it searches the raw queries (the rank's index prepares them).
+// Queries are rows of query_row_bytes(): FP32, or packed bits on a binary index.
+void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, const ShardRead& rd, const void* xq, float* out_dist, long long* out_ids,
+                  int* out_counts, cudaStream_t s) {
   IndexBase* ix = sh->ix;
   const int W = sh->world, r = sh->rank;
+  const int64_t nq = rd.nq;
+  const int k = rd.k;
   const size_t qb = ix->query_row_bytes();
   if (L.last && L.last != s && L.done) B200VS_CUDA(cudaStreamWaitEvent(s, L.done, 0));
-  SearchCtx sc = make_ctx(ix, sp, s);
+  SearchCtx sc = make_ctx(ix, rd.sp, s);
   const void* q = xq;
   int nprobe = 0;
   if (!sh->rows) {
@@ -634,133 +646,54 @@ void shard_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const vo
   // 2) scan of the probed lists this rank owns, or search of the rank's rows -> exact local results
   L.od.reserve((size_t)nq * k, 0, s);
   L.oi.reserve((size_t)nq * k, 0, s);
+  const MergeKey key = merge_key(sh, rd.kind);
   SearchReq req;
   req.nq = nq; req.xq = q; req.k = k; req.sc = &sc; req.od = L.od.p; req.oi = L.oi.p;
   if (!sh->rows) { req.prepared = true; req.probes = L.probes.p; req.nprobe = nprobe; }
-  local(req);
+  req.raw = key.raw;
+  req.deep = rd.kind == READ_DEEP;
+  if (rd.kind == READ_RANGE) {
+    req.range = true; req.radius = rd.radius;
+    req.oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again by the finish
+  }
+  // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
+  if (req.range && std::isnan(req.radius)) fill_empty(req, s);
+  else ix->search(req, s);
+  if (key.neg) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
   // 3) the all-gather of the packed per-shard results + merge
-  if (deep) gather_merge_runs(sh, L, nq, k, out_dist, out_ids, s);
-  else gather_merge(sh, L, nq, k, out_dist, out_ids, s);
+  gather_merge(sh, L, nq, k, req.deep, out_dist, out_ids, s);
   if (!L.done) B200VS_CUDA(cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming));
   B200VS_CUDA(cudaEventRecord(L.done, s));
   L.last = s;
-}
-
-// top-k.  List-sharded: the tile scan's exact local top-k, keyed on the API distance.  Row-sharded FLAT: the rank's search
-// keyed on the single-index select's key (L2 distance | -ip; two distinct inner products can round to the same 1 - ip, and
-// an API-distance merge would then choose and order them by id), the API distance formed after the merge.  Row-sharded
-// HNSW: the rank's graph walk, keyed on the distance the walk itself ranks by (hnsw_distance: L2 distance | 1 - ip).  Binary
-// types: the rank's search keyed on the Hamming distance, which is also the API distance.
-void shard_search_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
-                         float* out_dist, long long* out_ids, cudaStream_t s) {
-  IndexBase* ix = sh->ix;
-  const bool flat_ip = sh->rows && ix->type == B200VS_FLAT && ix->ip_like();
-  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](SearchReq& r) {
-    r.raw = sh->rows && ix->type == B200VS_FLAT;
-    ix->search(r, s);
-    if (flat_ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
-  });
-  if (flat_ip) {
-    ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
+  // 4) the finish: the merged key -> the API distance, the range counts
+  if (key.neg || req.range) {
+    merge_finish_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq, k, key.neg ? 1 : 0, out_counts);
     B200VS_CUDA(cudaGetLastError());
     ix->launch_count(1);
   }
   ix->phases_finish(s);
 }
 
-// deep top-k: the rank's deep search (run_deep) keyed the way the single-index deep path orders its output (float types: the
-// raw metric value, then -ip for IP / cosine; binary types: the Hamming distance), the sorted runs merged chunk by chunk
-// (gather_merge_runs), then the API distance as deep_emit_kernel forms it.  Never keyed on the API distance: two distinct
-// inner products can round to the same 1 - ip, which run_deep orders by -ip and an API-distance merge would order by id.
-void shard_deep_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, int k, const b200vs_search_params* sp,
-                       float* out_dist, long long* out_ids, cudaStream_t s) {
-  IndexBase* ix = sh->ix;
-  const bool ip = ix->ip_like();
-  shard_stream(sh, L, nq, xq, k, sp, out_dist, out_ids, s, [&](SearchReq& r) {
-    r.deep = true; r.raw = !ix->binary();
-    ix->search(r, s);
-    if (ip) launch_negate(L.od.p, nq * k, s);  // ip -> -ip
-  }, true);
-  if (ip) {
-    ip_key_to_api_kernel<<<(unsigned)cdiv(nq * k, 256), 256, 0, s>>>(out_dist, out_ids, nq * k);
-    B200VS_CUDA(cudaGetLastError());
-    ix->launch_count(1);
+// Refusals of a sharded read decided from its arguments alone, so that every rank refuses alike; each kind keeps the order
+// of its single-index call's refusals.  false: a top-k or deep read with k <= 0, OK with nothing to do.
+bool check_read(const b200vs_shard* sh, const ShardRead& rd) {
+  const IndexBase* ix = sh->ix;
+  check_row_type(sh, rd.binary_call);
+  if (rd.nq <= 0 || !rd.xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+  if (rd.kind == READ_RANGE) {
+    if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // as b200vs_range_search
+    if (rd.k <= 0 || rd.k > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
+    if (!rd.od || !rd.oi || !rd.oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
+    if (ix->binary() && std::isnan(rd.radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");  // as b200vs_range_search_binary
+    return true;
   }
-  ix->phases_finish(s);
-}
-
-// range: the local range scan keyed on the single-index select's key (L2 distance | -ip) — two distinct inner products can
-// round to the same 1 - ip, and an API-distance merge would then order them by id — then the API distance and the count of
-// every merged row.  Binary types: the rank's b200vs_range_search_binary rule keyed on the Hamming distance (a NaN radius
-// is refused before the read starts).  The per-rank payload of the all-gather is nq * max_results * 16 bytes.
-void shard_range_stream(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, const void* xq, float radius, int max_results,
-                        const b200vs_search_params* sp, float* out_dist, long long* out_ids, int* out_counts, cudaStream_t s) {
-  IndexBase* ix = sh->ix;
-  const bool ip = ix->ip_like();
-  shard_stream(sh, L, nq, xq, max_results, sp, out_dist, out_ids, s, [&](SearchReq& r) {
-    r.range = true; r.radius = radius; r.raw = true;
-    r.oc = ix->scratch.alloc<int>((size_t)nq);  // local counts: the merged rows are counted again below
-    // a NaN radius admits no row (DESIGN.md 4.6): this rank contributes empty lists, and still joins the all-gather
-    if (std::isnan(radius)) fill_empty(r, s);
-    else ix->search(r, s);
-    if (ip) launch_negate(L.od.p, nq * max_results, s);  // ip -> -ip
-  });
-  const long long n = (long long)nq * max_results;
-  range_finish_kernel<<<(unsigned)cdiv(n, 256), 256, 0, s>>>(out_dist, out_ids, nq, max_results, ip ? 1 : 0, out_counts);
-  B200VS_CUDA(cudaGetLastError());
-  ix->launch_count(1);
-  ix->phases_finish(s);
-}
-
-// Refusals of a sharded read decided from its arguments alone, so that every rank refuses alike.  Top-k: false = k <= 0,
-// nothing to do.
-bool check_shard_topk(int64_t nq, const void* xq, int k, const void* od, const void* oi) {
-  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-  if (k <= 0) return false;
-  if (!od || !oi) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
-  return true;
-}
-// deep top-k: b200vs_search_deep's refusals, in its order
-bool check_shard_deep(const IndexBase* ix, int64_t nq, const void* xq, int k, const void* od, const void* oi) {
-  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-  if (k <= 0) return false;
-  if (k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
-  if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "deep top-k is not implemented for HNSW");
-  return check_shard_topk(nq, xq, k, od, oi);
-}
-bool check_shard_range(const IndexBase* ix, int64_t nq, const void* xq, float radius, int max_results, const void* od, const void* oi,
-                       const void* oc) {
-  if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
-  if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "RangeSearch not support in Hnsw!!!");  // as b200vs_range_search
-  if (max_results <= 0 || max_results > 4096) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be in [1, 4096]");
-  if (!od || !oi || !oc) fail(B200VS_EILLEGAL_PARAMETERS, "bad range-search outputs");
-  if (ix->binary() && std::isnan(radius)) fail(B200VS_EILLEGAL_PARAMETERS, "radius is NaN");  // as b200vs_range_search_binary
-  return true;
-}
-
-// One sharded read (k = results per query).  The turn of batch `seq` comes first, so that every call uses its sequence
-// number exactly once, a refused one included; then `refuse` (false: OK, nothing to do), the rw lock, the device and a lane
-// on `stream` (null: the lane's own stream), the refusals every rank meets alike before the first collective, and
-// body(lane, s).  The lane is released before the host waits for a null-stream call, so the lane's next batch may be
-// enqueued behind this one.
-template <class Refuse, class Body>
-void shard_read(b200vs_shard* sh, int64_t seq, void* stream, int64_t nq, int k, const b200vs_search_params* sp, Refuse refuse, Body body,
-                bool deep = false) {
-  IndexBase* ix = sh->ix;
-  cudaStream_t s;
-  {
-    SeqLane sl(sh, seq);
-    if (!refuse()) return;
-    std::shared_lock<std::shared_mutex> rl(ix->rw);
-    ix->set_device();
-    s = stream ? (cudaStream_t)stream : sl.lane->own;
-    LaneGuard lane(ix, s);
-    ix->check_probe_search(nq, k, deep);
-    if (sh->rows) ix->check_row_search(k, sp);
-    ix->reset_stats();
-    body(*sl.lane, s);
+  if (rd.k <= 0) return false;
+  if (rd.kind == READ_DEEP) {  // b200vs_search_deep's refusals, in its order
+    if (rd.k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
+    if (ix->type == B200VS_HNSW) fail(B200VS_EVECTOR_NOT_SUPPORT, "deep top-k is not implemented for HNSW");
   }
-  if (!stream) B200VS_CUDA(cudaStreamSynchronize(s));
+  if (!rd.od || !rd.oi) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+  return true;
 }
 
 // The host-pointer reads: every rank passes the SAME batch; each rank uploads only its slice and the slices are all-gathered
@@ -778,6 +711,46 @@ const void* upload_batch(b200vs_shard* sh, b200vs_shard::SLane& L, int64_t nq, c
   if (q1 - q0 < per) B200VS_CUDA(cudaMemsetAsync(mine + (size_t)(q1 - q0) * qb, 0, (size_t)(per - (q1 - q0)) * qb, s));
   if (W > 1) B200VS_NCCL(nccl().AllGather(mine, L.q_all.p, (size_t)per * qb, ncclUint8, L.comm, s));
   return L.q_all.p;
+}
+
+// The body of every sharded read entry point.  The turn of batch `seq` comes first, so that every call uses its sequence
+// number exactly once, a refused one included; then check_read, the rw lock, the device and a lane on the read's stream,
+// the refusals every rank meets alike before the first collective, and shard_stream (host pointers: the batch uploaded
+// before it, the results copied back after it).  The lane is released before the host waits for a null-stream call, so the
+// lane's next batch may be enqueued behind this one.
+int shard_read(b200vs_shard* h, const ShardRead& rd) {
+  return guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    IndexBase* ix = sh->ix;
+    cudaStream_t s;
+    {
+      SeqLane sl(sh, rd.seq);
+      if (!check_read(sh, rd)) return B200VS_OK;
+      std::shared_lock<std::shared_mutex> rl(ix->rw);
+      ix->set_device();
+      s = rd.stream ? (cudaStream_t)rd.stream : sl.lane->own;
+      LaneGuard lane(ix, s);
+      ix->check_probe_search(rd.nq, rd.k, rd.kind == READ_DEEP);
+      if (sh->rows) ix->check_row_search(rd.k, rd.sp);
+      ix->reset_stats();
+      b200vs_shard::SLane& L = *sl.lane;
+      if (rd.on_device) {
+        shard_stream(sh, L, rd, rd.xq, rd.od, (long long*)rd.oi, rd.oc, s);
+      } else {
+        const size_t nk = (size_t)rd.nq * rd.k;
+        const void* q = upload_batch(sh, L, rd.nq, rd.xq, s);
+        float* dd = ix->scratch.alloc<float>(nk);
+        long long* di = ix->scratch.alloc<long long>(nk);
+        int* dc = rd.kind == READ_RANGE ? ix->scratch.alloc<int>((size_t)rd.nq) : nullptr;
+        shard_stream(sh, L, rd, q, dd, di, dc, s);
+        B200VS_CUDA(cudaMemcpyAsync(rd.od, dd, nk * 4, cudaMemcpyDeviceToHost, s));
+        B200VS_CUDA(cudaMemcpyAsync(rd.oi, di, nk * 8, cudaMemcpyDeviceToHost, s));
+        if (dc) B200VS_CUDA(cudaMemcpyAsync(rd.oc, dc, (size_t)rd.nq * 4, cudaMemcpyDeviceToHost, s));
+      }
+    }
+    if (!rd.stream) B200VS_CUDA(cudaStreamSynchronize(s));
+    return B200VS_OK;
+  });
 }
 
 // Replicate rank `root`'s trained state on every rank (b200vs_shard_broadcast_state; the caller holds add_mu).  The length
@@ -1552,93 +1525,6 @@ int shard_add(b200vs_shard* h, int64_t n, const void* x, const int64_t* ids, boo
   });
 }
 
-// b200vs_shard_search_device / b200vs_shard_search_binary_device
-int shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq_dev, int32_t k, const b200vs_search_params* sp,
-                        float* out_dist_dev, int64_t* out_ids_dev, void* stream, bool binary_call) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, stream, nq, k, sp,
-               [&] {
-                 check_row_type(sh, binary_call);
-                 return check_shard_topk(nq, xq_dev, k, out_dist_dev, out_ids_dev);
-               },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 shard_search_stream(sh, L, nq, xq_dev, k, sp, out_dist_dev, (long long*)out_ids_dev, s);
-               });
-    return B200VS_OK;
-  });
-}
-
-// Host-pointer variant (the call a dingo-store node makes): every rank passes the SAME batch (upload_batch).  deep:
-// b200vs_shard_search_deep / b200vs_shard_search_binary_deep.
-int shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
-                 int64_t* out_ids, bool binary_call, bool deep = false) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, nullptr, nq, k, sp,
-               [&] {
-                 check_row_type(sh, binary_call);
-                 return deep ? check_shard_deep(sh->ix, nq, xq, k, out_dist, out_ids) : check_shard_topk(nq, xq, k, out_dist, out_ids);
-               },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 IndexBase* ix = sh->ix;
-                 const void* q = upload_batch(sh, L, nq, xq, s);
-                 float* dd = ix->scratch.alloc<float>((size_t)nq * k);
-                 long long* di = ix->scratch.alloc<long long>((size_t)nq * k);
-                 if (deep) shard_deep_stream(sh, L, nq, q, k, sp, dd, di, s);
-                 else shard_search_stream(sh, L, nq, q, k, sp, dd, di, s);
-                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
-               },
-               deep);
-    return B200VS_OK;
-  });
-}
-
-// b200vs_shard_range_search_device / b200vs_shard_range_search_binary_device
-int shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq_dev, float radius, int32_t max_results,
-                              const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, int32_t* out_counts_dev,
-                              void* stream, bool binary_call) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, stream, nq, max_results, sp,
-               [&] {
-                 check_row_type(sh, binary_call);
-                 return check_shard_range(sh->ix, nq, xq_dev, radius, max_results, out_dist_dev, out_ids_dev, out_counts_dev);
-               },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 shard_range_stream(sh, L, nq, xq_dev, radius, max_results, sp, out_dist_dev, (long long*)out_ids_dev, out_counts_dev, s);
-               });
-    return B200VS_OK;
-  });
-}
-
-// Host-pointer variant: as shard_search, each rank uploads only its slice of the batch.
-int shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const void* xq, float radius, int32_t max_results,
-                       const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts, bool binary_call) {
-  return guarded([&]() -> int {
-    b200vs_shard* sh = get(h);
-    shard_read(sh, seq, nullptr, nq, max_results, sp,
-               [&] {
-                 check_row_type(sh, binary_call);
-                 return check_shard_range(sh->ix, nq, xq, radius, max_results, out_dist, out_ids, out_counts);
-               },
-               [&](b200vs_shard::SLane& L, cudaStream_t s) {
-                 IndexBase* ix = sh->ix;
-                 const void* q = upload_batch(sh, L, nq, xq, s);
-                 const size_t nr = (size_t)nq * max_results;
-                 float* dd = ix->scratch.alloc<float>(nr);
-                 long long* di = ix->scratch.alloc<long long>(nr);
-                 int* dc = ix->scratch.alloc<int>((size_t)nq);
-                 shard_range_stream(sh, L, nq, q, radius, max_results, sp, dd, di, dc, s);
-                 B200VS_CUDA(cudaMemcpyAsync(out_dist, dd, nr * 4, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_ids, di, nr * 8, cudaMemcpyDeviceToHost, s));
-                 B200VS_CUDA(cudaMemcpyAsync(out_counts, dc, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
-               });
-    return B200VS_OK;
-  });
-}
-
 }  // namespace
 
 extern "C" {
@@ -1780,49 +1666,49 @@ int b200vs_shard_plan_commit(b200vs_shard* h) {
 
 int b200vs_shard_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, int32_t k, const b200vs_search_params* sp,
                                float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
-  return shard_search_device(h, seq, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, false);
+  return shard_read(h, {READ_TOPK, false, true, stream, seq, nq, xq_dev, 0.f, k, sp, out_dist_dev, out_ids_dev, nullptr});
 }
 int b200vs_shard_search_binary_device(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq_dev, int32_t k,
                                       const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, void* stream) {
-  return shard_search_device(h, seq, nq, xq_dev, k, sp, out_dist_dev, out_ids_dev, stream, true);
+  return shard_read(h, {READ_TOPK, true, true, stream, seq, nq, xq_dev, 0.f, k, sp, out_dist_dev, out_ids_dev, nullptr});
 }
 
 int b200vs_shard_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
                         int64_t* out_ids) {
-  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, false);
+  return shard_read(h, {READ_TOPK, false, false, nullptr, seq, nq, xq, 0.f, k, sp, out_dist, out_ids, nullptr});
 }
 int b200vs_shard_search_binary(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
                                float* out_dist, int64_t* out_ids) {
-  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, true);
+  return shard_read(h, {READ_TOPK, true, false, nullptr, seq, nq, xq, 0.f, k, sp, out_dist, out_ids, nullptr});
 }
 
 int b200vs_shard_search_deep(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
                              float* out_dist, int64_t* out_ids) {
-  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, false, true);
+  return shard_read(h, {READ_DEEP, false, false, nullptr, seq, nq, xq, 0.f, k, sp, out_dist, out_ids, nullptr});
 }
 int b200vs_shard_search_binary_deep(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, int32_t k, const b200vs_search_params* sp,
                                     float* out_dist, int64_t* out_ids) {
-  return shard_search(h, seq, nq, xq, k, sp, out_dist, out_ids, true, true);
+  return shard_read(h, {READ_DEEP, true, false, nullptr, seq, nq, xq, 0.f, k, sp, out_dist, out_ids, nullptr});
 }
 
 int b200vs_shard_range_search_device(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq_dev, float radius, int32_t max_results,
                                      const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev, int32_t* out_counts_dev,
                                      void* stream) {
-  return shard_range_search_device(h, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev, stream, false);
+  return shard_read(h, {READ_RANGE, false, true, stream, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev});
 }
 int b200vs_shard_range_search_binary_device(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq_dev, float radius,
                                             int32_t max_results, const b200vs_search_params* sp, float* out_dist_dev, int64_t* out_ids_dev,
                                             int32_t* out_counts_dev, void* stream) {
-  return shard_range_search_device(h, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev, stream, true);
+  return shard_read(h, {READ_RANGE, true, true, stream, seq, nq, xq_dev, radius, max_results, sp, out_dist_dev, out_ids_dev, out_counts_dev});
 }
 
 int b200vs_shard_range_search(b200vs_shard* h, int64_t seq, int64_t nq, const float* xq, float radius, int32_t max_results,
                               const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
-  return shard_range_search(h, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, false);
+  return shard_read(h, {READ_RANGE, false, false, nullptr, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts});
 }
 int b200vs_shard_range_search_binary(b200vs_shard* h, int64_t seq, int64_t nq, const uint8_t* xq, float radius, int32_t max_results,
                                      const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
-  return shard_range_search(h, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts, true);
+  return shard_read(h, {READ_RANGE, true, false, nullptr, seq, nq, xq, radius, max_results, sp, out_dist, out_ids, out_counts});
 }
 
 }  // extern "C"
