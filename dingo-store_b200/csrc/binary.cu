@@ -364,18 +364,18 @@ struct BinaryIvfIndex : BinaryIndex {
     if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
     return false;
   }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
     std::vector<int64_t> ids;
     std::vector<long long> slots;
     L.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, store.words.p, w, rows, out_ids);
+    sorted_live_rows(this, ids, slots, store.words.p, w, rows, out_ids, s);
     return (int64_t)ids.size();
   }
   // train on src's padded rows in ascending id order, then add them in that order
   int64_t rebuild_from(IndexBase& src) override {
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.sorted_rows(rows, ids);
+    const int64_t n = src.sorted_rows(rows, ids, src.stream);
     if (n == 0) return 0;
     train_locked(n, nullptr, rows.p);
     scratch.reset(stream);
@@ -500,10 +500,10 @@ static BinaryIvfIndex* as_binary_ivf(IndexBase* ix) {
   return p;
 }
 
-void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, int k, std::vector<uint8_t>& cent) {
+void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, const uint32_t* x_words, int k, std::vector<uint8_t>& cent) {
   BinaryIvfIndex* b = as_binary_ivf(ix);
   WriteHold hold(b);
-  b->kmeans_locked(n, x, nullptr, k, cent);
+  b->kmeans_locked(n, x, x_words, k, cent);
 }
 
 void binary_ivf_train_state(IndexBase* ix, const std::vector<uint8_t>& cent, std::vector<unsigned char>& blob) {

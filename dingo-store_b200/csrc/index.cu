@@ -439,13 +439,13 @@ struct FlatIndex : IndexBase {
   int64_t count() const override { return rowmap.count(); }
   int64_t deleted_count() const override { return rowmap.ndeleted; }
   int64_t memory_size() const override { return rowmap.store.bytes(); }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
     // the inner Flat of an IVF-PQ region takes its writes under its own lock, not under the outer index's
     RwSharedGuard rl(this);
     std::vector<int64_t> ids;
     std::vector<long long> slots;
     rowmap.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(rowmap.store.vecs.p), dim, rows, out_ids);
+    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(rowmap.store.vecs.p), dim, rows, out_ids, s);
     return (int64_t)ids.size();
   }
 
@@ -579,18 +579,18 @@ struct IvfFlatIndex : IndexBase {
     if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
     return false;
   }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids) override {
+  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
     std::vector<int64_t> ids;
     std::vector<long long> slots;
     L.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(store.vecs.p), dim, rows, out_ids);
+    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(store.vecs.p), dim, rows, out_ids, s);
     return (int64_t)ids.size();
   }
   // train on src's stored rows in ascending id order, then add them in that order; stored cosine rows are already normalised
   int64_t rebuild_from(IndexBase& src) override {
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.sorted_rows(rows, ids);
+    const int64_t n = src.sorted_rows(rows, ids, src.stream);
     if (n == 0) return 0;
     train_locked(n, reinterpret_cast<const float*>(rows.p), true);
     scratch.reset(stream);
@@ -791,11 +791,16 @@ static IvfFlatIndex* as_ivf_flat(IndexBase* ix) {
   return p;
 }
 
-void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent) {
+void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, bool x_dev, int k, std::vector<float>& cent) {
   b200vs_params p = as_ivf_flat(ix)->params;
   p.nlist = k;
   IvfFlatIndex loc(ix->metric, ix->dim, p);  // train on an index of its own: ix keeps its state and lists
-  loc.train(n, x);
+  if (x_dev) {
+    WriteHold hold(&loc);
+    loc.train_locked(n, x, true);
+  } else {
+    loc.train(n, x);
+  }
   cent.resize((size_t)loc.nlist * loc.dim);
   B200VS_CUDA(cudaMemcpy(cent.data(), loc.centroids.p, cent.size() * 4, cudaMemcpyDeviceToHost));
 }

@@ -322,10 +322,10 @@ struct IndexBase {
   // b200vs_rebuild_from: fill this empty, untrained index (rw and gpu_mu held, scratch reset, check_rebuild_pair passed)
   // from src's live rows in ascending id order, as a fresh train + add of them would; src is held shared.  Returns the rows.
   virtual int64_t rebuild_from(IndexBase& src) { (void)src; fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild is not supported for this index type"); }
-  // the live rows in ascending id order on this index's device (rebuild_from's source): rows [n, row words] and ids [n];
-  // returns n.  Callers hold rw.
-  virtual int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& ids) {
-    (void)rows; (void)ids;
+  // the live rows in ascending id order on this index's device (rebuild_from's source), built on stream s: rows [n, row
+  // words] and ids [n]; returns n.  Callers hold rw.
+  virtual int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& ids, cudaStream_t s) {
+    (void)rows; (void)ids; (void)s;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "this index type has no row store to rebuild from");
   }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }
@@ -484,15 +484,17 @@ int ivf_pq_ksub(IndexBase* ix);
 void ivf_pq_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent);
 void ivf_pq_train_state(IndexBase* ix, int64_t n, const float* x, const std::vector<float>& cent, std::vector<unsigned char>& blob);
 // The same two stages for IVF_FLAT (index.cu); ix must be an IVF_FLAT index, which stays untouched.  Coarse: train's k
-// centroids of n >= k raw rows.  State: the trained-state blob of the centroids cent [nlist, dim].
-void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, int k, std::vector<float>& cent);
+// centroids of n >= k rows: raw host rows, or (x_dev) prepared rows on ix's device, which are not normalised again
+// (b200vs_rebuild_from's rule).  State: the trained-state blob of the centroids cent [nlist, dim].
+void ivf_flat_train_coarse(IndexBase* ix, int64_t n, const float* x, bool x_dev, int k, std::vector<float>& cent);
 void ivf_flat_train_state(IndexBase* ix, const std::vector<float>& cent, std::vector<unsigned char>& blob);
 IndexBase* make_binary_flat(int d, const b200vs_params& p);
 IndexBase* make_binary_ivf(int d, const b200vs_params& p);
 // The same two stages for BINARY_IVF_FLAT (binary.cu); ix must be a BINARY_IVF_FLAT index, whose lists and trained state stay
-// untouched.  Coarse: b200vs_train_binary's k packed centroids [k, dim / 8] of n >= k host packed rows.  State: the
+// untouched.  Coarse: b200vs_train_binary's k packed centroids [k, dim / 8] of n >= k host packed rows x, or of n padded
+// rows x_words [n, ceil(dim / 32)] on ix's device (x then null), whose sample is expanded to +-1 floats there.  State: the
 // trained-state blob of the packed centroids cent [nlist, dim / 8].
-void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, int k, std::vector<uint8_t>& cent);
+void binary_ivf_train_coarse(IndexBase* ix, int64_t n, const uint8_t* x, const uint32_t* x_words, int k, std::vector<uint8_t>& cent);
 void binary_ivf_train_state(IndexBase* ix, const std::vector<uint8_t>& cent, std::vector<unsigned char>& blob);
 
 // ---- generic exact scan + select driver (scan_kernels.cuh) ----

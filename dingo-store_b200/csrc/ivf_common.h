@@ -538,11 +538,18 @@ void kmeans_gpu_dev(IndexBase* ix, int d, int64_t n, const float* x_dev, int k, 
   kmeans_lloyd(ix, d, m, xs, hx.data(), k, niter, seed, cent, assign, prepare_ids);
 }
 
-// The live rows of an index in ascending id order, on its device (b200vs_rebuild_from): (ids[i], slots[i]) are the live
-// rows in the index's own storage order; they are sorted by id with a stable device radix sort (rows that share an id keep
-// that order), and row slots[i] of src (`words` 32-bit words per row) is gathered into out_rows.  Runs on ix's stream.
-void sorted_live_rows(IndexBase* ix, const std::vector<int64_t>& ids, const std::vector<long long>& slots, const uint32_t* src,
-                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids);
+// The live rows of an index in ascending id order, on its device (b200vs_rebuild_from, b200vs_shard_rebuild_from): (ids[i],
+// slots[i]), i < n, are the live rows in the index's own storage order, on the host or (on_device) on the device, where a
+// null slots stands for 0, 1, ..., n - 1; they are sorted by id with a stable device radix sort (rows that share an id keep
+// that order), and row slots[i] of src (`words` 32-bit words per row) is gathered into out_rows.  Runs on stream s and
+// returns with it synchronised.
+void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids, const long long* slots, bool on_device, const uint32_t* src,
+                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s);
+inline void sorted_live_rows(IndexBase* ix, const std::vector<int64_t>& ids, const std::vector<long long>& slots, const uint32_t* src,
+                             int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
+  sorted_live_rows(ix, (int64_t)ids.size(), reinterpret_cast<const long long*>(ids.data()), slots.data(), false, src, words, out_rows,
+                   out_ids, s);
+}
 // out [m, dim] = the +-1 floats (binary_to_real: bit set -> 1, else -1) of padded binary rows words [.., w] (rows ? rows[i] : i)
 void launch_expand_pm1(const uint32_t* words, const long long* rows, int64_t m, int w, int dim, float* out, cudaStream_t s);
 // the refusals b200vs_rebuild_from shares for every type: dst must be empty, untrained, another index of the same type,

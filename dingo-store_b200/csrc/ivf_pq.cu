@@ -567,7 +567,7 @@ struct IvfPqIndex : IndexBase {
     if (src.mode == kNone) return 0;
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.flat->sorted_rows(rows, ids);
+    const int64_t n = src.flat->sorted_rows(rows, ids, src.flat->stream);
     if (n == 0) return 0;
     const float* x = reinterpret_cast<const float*>(rows.p);
     if (n < train_need()) {

@@ -55,21 +55,29 @@ int64_t kmeans_sample_rows(IndexBase* ix, int64_t n, int k, int max_pts, int64_t
   return m;
 }
 
-void sorted_live_rows(IndexBase* ix, const std::vector<int64_t>& ids, const std::vector<long long>& slots, const uint32_t* src,
-                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids) {
-  const cudaStream_t s = ix->stream;
-  const int64_t n = (int64_t)ids.size();
+void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids, const long long* slots, bool on_device, const uint32_t* src,
+                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
   if (n == 0) return;
   if (n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild holds at most 2^31 - 1 rows");
   DevBuf<long long> keys, vals, sorted_slots;
-  keys.reserve(n, 0, s); vals.reserve(n, 0, s); sorted_slots.reserve(n, 0, s); out_ids.reserve(n, 0, s);
-  B200VS_CUDA(cudaMemcpyAsync(keys.p, ids.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
-  B200VS_CUDA(cudaMemcpyAsync(vals.p, slots.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  const long long* k_in = ids;
+  const long long* v_in = slots;
+  if (!on_device) {
+    keys.reserve(n, 0, s); vals.reserve(n, 0, s);
+    B200VS_CUDA(cudaMemcpyAsync(keys.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    B200VS_CUDA(cudaMemcpyAsync(vals.p, slots, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    k_in = keys.p; v_in = vals.p;
+  } else if (!slots) {  // the rows' own positions
+    vals.reserve(n, 0, s);
+    launch_iota(vals.p, n, s);
+    v_in = vals.p;
+  }
+  sorted_slots.reserve(n, 0, s); out_ids.reserve(n, 0, s);
   size_t tmp_bytes = 0;
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.p, out_ids.p, vals.p, sorted_slots.p, (int)n, 0, 64, s));
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in, out_ids.p, v_in, sorted_slots.p, (int)n, 0, 64, s));
   DevBuf<unsigned char> tmp;
   tmp.reserve(std::max<size_t>(tmp_bytes, 1), 0, s);
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys.p, out_ids.p, vals.p, sorted_slots.p, (int)n, 0, 64, s));
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, k_in, out_ids.p, v_in, sorted_slots.p, (int)n, 0, 64, s));
   out_rows.reserve((size_t)n * words, 0, s);
   launch_gather_words(src, sorted_slots.p, n, words, out_rows.p, s);
   B200VS_CUDA(cudaStreamSynchronize(s));  // the host id and slot lists and the sort's buffers die here

@@ -431,6 +431,9 @@ struct b200vs_shard {
   cudaStream_t ws = nullptr;
   DevBuf<unsigned long long> plan_counts;  // [nlist] rows per list seen by b200vs_shard_plan_add*
   bool planning = false;
+  // the training size of b200vs_shard_need_rebuild's rule for the whole set (list-sharded): the rows shard_train clustered
+  // over every rank, or every rank's live rows summed at shard_broadcast_state / shard_load; not saved, as on one index
+  int64_t train_rows_set = 0;
 
   ~b200vs_shard() {
     if (ix) cudaSetDevice(ix->device);
@@ -525,6 +528,14 @@ Status agree(b200vs_shard* sh, const Status& mine, const char* what) {
 }
 void check(const Status& st) {
   if (st.code != B200VS_OK) fail(st.code, st.msg);
+}
+// A local step of a collective call (allocations, kernels, an index write) that the next collective depends on.  agreed:
+// every rank's status is agreed after it, so a device failure on one rank (an allocation that does not fit) is returned by
+// every rank instead of leaving its peers waiting in that collective.  Else f runs as it is.
+template <class F>
+void local_step(b200vs_shard* sh, bool agreed, const char* what, F&& f) {
+  if (agreed) check(agree(sh, attempt(f), what));
+  else f();
 }
 
 // One sharded read, as its extern "C" entry point passes it.  k: results per query (range: max_results).  on_device: xq and
@@ -761,28 +772,36 @@ void broadcast_state_locked(b200vs_shard* sh, int root) {
   const long long mine = sh->rank == root ? (long long)ix->get_state(nullptr, 0) : 0;
   const long long need = all_gather_host(sh, &mine)[root];
   if (need <= 0) fail(B200VS_EVECTOR_NOT_TRAIN, "root has no trained state");
-  std::vector<unsigned char> blob((size_t)need);
-  if (sh->rank == root) ix->get_state(blob.data(), blob.size());
+  std::vector<unsigned char> blob;
   DevBuf<unsigned char> db;
-  db.reserve((size_t)need, 0, sh->ws);
-  if (sh->rank == root) B200VS_CUDA(cudaMemcpyAsync(db.p, blob.data(), (size_t)need, cudaMemcpyHostToDevice, sh->ws));
+  local_step(sh, true, "shard broadcast_state", [&] {
+    blob.resize((size_t)need);
+    if (sh->rank == root) ix->get_state(blob.data(), blob.size());
+    db.reserve((size_t)need, 0, sh->ws);
+    if (sh->rank == root) B200VS_CUDA(cudaMemcpyAsync(db.p, blob.data(), (size_t)need, cudaMemcpyHostToDevice, sh->ws));
+  });
   if (sh->world > 1) B200VS_NCCL(nccl().Broadcast(db.p, db.p, (size_t)need, ncclUint8, root, sh->lanes[0]->comm, sh->ws));
-  if (sh->rank != root) {
-    B200VS_CUDA(cudaMemcpyAsync(blob.data(), db.p, (size_t)need, cudaMemcpyDeviceToHost, sh->ws));
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-    ix->set_state(blob.data(), blob.size());
-  } else {
-    B200VS_CUDA(cudaStreamSynchronize(sh->ws));
-  }
+  // the install is agreed too: every rank returns the same status, and the caller's next collective finds every rank
+  local_step(sh, true, "shard broadcast_state", [&] {
+    if (sh->rank != root) {
+      B200VS_CUDA(cudaMemcpyAsync(blob.data(), db.p, (size_t)need, cudaMemcpyDeviceToHost, sh->ws));
+      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+      ix->set_state(blob.data(), blob.size());
+    } else {
+      B200VS_CUDA(cudaStreamSynchronize(sh->ws));
+    }
+  });
 }
 
 // b200vs_shard_train on IVF_FLAT and IVF_PQ, b200vs_shard_train_binary on BINARY_IVF_FLAT (x: packed rows).  The per-rank row
 // counts are exchanged first, so that a refusal for too few rows happens on every rank at once.  Coarse stage: each rank
-// clusters its rows into nlist / world centroids with the k-means of its type's own train, one all-gather.  IVF_FLAT and
-// BINARY_IVF_FLAT: every rank installs the gathered centroids.  IVF_PQ: rank 0 trains the codebooks with train's PQ rule on
-// the residuals of its rows to the global centroids, and the state broadcast replicates the result.  At world = 1 this is
-// b200vs_train[_binary] step for step, so the trained state is byte-equal.
-void shard_train_locked(b200vs_shard* sh, int64_t n, const void* xv) {
+// clusters its rows into nlist / world centroids with the k-means of its type's own train, and every rank's status is
+// agreed before the one all-gather.  IVF_FLAT and BINARY_IVF_FLAT: every rank installs the gathered centroids.  IVF_PQ:
+// rank 0 trains the codebooks with train's PQ rule on the residuals of its rows to the global centroids, and the state
+// broadcast replicates the result.  At world = 1 this is b200vs_train[_binary] step for step, so the trained state is
+// byte-equal.  on_device (b200vs_shard_rebuild_from; IVF_FLAT and BINARY_IVF_FLAT): x is on the index's device, prepared
+// FP32 rows or padded binary rows [n, ceil(dim / 32)] words, and is clustered as b200vs_rebuild_from clusters its rows.
+void shard_train_locked(b200vs_shard* sh, int64_t n, const void* xv, bool on_device) {
   IndexBase* ix = sh->ix;
   const bool pq = ix->type == B200VS_IVF_PQ;
   const int W = sh->world, nlist = ix->params.nlist > 0 ? ix->params.nlist : 2048;
@@ -797,29 +816,52 @@ void shard_train_locked(b200vs_shard* sh, int64_t n, const void* xv) {
       fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank " + std::to_string(r) + " has fewer training rows than nlist / world centroids");
   if (pq && counts[0] < 256LL * ivf_pq_ksub(ix))
     fail(B200VS_EILLEGAL_PARAMETERS, "shard_train: rank 0 needs 256 * 2^nbits training rows for the PQ codebooks");
+  int64_t total = 0;
+  for (const long long c : counts) total += c;
   std::vector<unsigned char> blob;
   if (ix->binary()) {
     std::vector<uint8_t> local;
-    binary_ivf_train_coarse(ix, n, static_cast<const uint8_t*>(xv), nl, local);
+    const uint8_t* x = on_device ? nullptr : static_cast<const uint8_t*>(xv);
+    const uint32_t* words = on_device ? static_cast<const uint32_t*>(xv) : nullptr;
+    check(agree(sh, attempt([&] { binary_ivf_train_coarse(ix, n, x, words, nl, local); }), "shard train"));
     binary_ivf_train_state(ix, all_gather_host(sh, local.data(), local.size()), blob);
-    ix->set_state(blob.data(), blob.size());
+    local_step(sh, true, "shard train", [&] { ix->set_state(blob.data(), blob.size()); });
+    sh->train_rows_set = total;
     return;
   }
   const float* x = static_cast<const float*>(xv);
   std::vector<float> local;
-  if (pq) ivf_pq_train_coarse(ix, n, x, nl, local);
-  else ivf_flat_train_coarse(ix, n, x, nl, local);
+  check(agree(sh, attempt([&] {
+    if (pq) ivf_pq_train_coarse(ix, n, x, nl, local);
+    else ivf_flat_train_coarse(ix, n, x, on_device, nl, local);
+  }), "shard train"));
   const std::vector<float> cent = all_gather_host(sh, local.data(), local.size());
   if (!pq) {
     ivf_flat_train_state(ix, cent, blob);
-    ix->set_state(blob.data(), blob.size());
+    local_step(sh, true, "shard train", [&] { ix->set_state(blob.data(), blob.size()); });
+    sh->train_rows_set = total;
     return;
   }
-  if (sh->rank == 0) {
+  local_step(sh, true, "shard train", [&] {
+    if (sh->rank != 0) return;
     ivf_pq_train_state(ix, n, x, cent, blob);
     ix->set_state(blob.data(), blob.size());
-  }
+  });
   broadcast_state_locked(sh, 0);
+  sh->train_rows_set = total;
+}
+
+// Every rank's live rows, summed (collective): the training size the set's rule takes after a state broadcast or a load, as
+// b200vs_set_trained_state and b200vs_load take the live count of one index
+int64_t live_rows_set(b200vs_shard* sh) {
+  long long mine = 0;
+  {
+    std::shared_lock<std::shared_mutex> rl(sh->ix->rw);
+    mine = (long long)sh->ix->count();
+  }
+  int64_t sum = 0;
+  for (const long long v : all_gather_host(sh, &mine)) sum += v;
+  return sum;
 }
 
 // b200vs_shard_create (float indexes) and b200vs_shard_create_binary (binary ones)
@@ -868,7 +910,7 @@ int shard_train(b200vs_shard* h, int64_t n, const void* x, bool binary_call) {
     check_row_type(sh, binary_call);
     if (sh->rows) return B200VS_OK;  // FLAT, BINARY_FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
     std::lock_guard<std::mutex> g(sh->add_mu);
-    shard_train_locked(sh, n, x);
+    shard_train_locked(sh, n, x, false);
     return B200VS_OK;
   });
 }
@@ -926,6 +968,7 @@ int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
     if (root < 0 || root >= sh->world) fail(B200VS_EILLEGAL_PARAMETERS, "bad root");
     std::lock_guard<std::mutex> g(sh->add_mu);
     broadcast_state_locked(sh, root);
+    sh->train_rows_set = live_rows_set(sh);
     return B200VS_OK;
   });
 }
@@ -963,8 +1006,11 @@ struct Routed {
   DevBuf<long long> ids, lists;
   long long n = 0;
 };
+// agreed (b200vs_shard_rebuild_from): the partition (the send copy) and the reservation of the received copy are local_steps
+// with a status agreement each, so a rank that cannot hold them fails on every rank before the exchange.
 template <class Owner>
-void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long long* ids, const long long* lists, Owner owner, Routed& out) {
+void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long long* ids, const long long* lists, Owner owner, Routed& out,
+                bool agreed = false) {
   const int W = sh->world, r = sh->rank, d = rb;  // d: bytes per row below
   const unsigned char* x = static_cast<const unsigned char*>(xv);
   cudaStream_t s = sh->ws;
@@ -972,9 +1018,11 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
   Routed snd;
   DevBuf<long long> cnt_all, tile_off;
   DevBuf<int> tile_cnt;
-  cnt_all.reserve((size_t)W * W, 0, s);
-  long long* mine = cnt_all.p + (size_t)r * W;
+  long long* mine = nullptr;
   // stable partition by owner on the device; this rank's row of the counts matrix
+  local_step(sh, agreed, "shard routing", [&] {
+  cnt_all.reserve((size_t)W * W, 0, s);
+  mine = cnt_all.p + (size_t)r * W;
   if (n) {
     const long long ntiles = cdiv(n, ROUTE_THREADS);
     const size_t smem = (size_t)ROUTE_WARPS * W * 4;
@@ -989,6 +1037,7 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
   } else {
     B200VS_CUDA(cudaMemsetAsync(mine, 0, (size_t)W * 8, s));
   }
+  });
   // counts matrix: every rank learns how many rows each peer sends it
   if (W > 1) B200VS_NCCL(nccl().AllGather(mine, cnt_all.p, (size_t)W, ncclInt64, comm, s));
   std::vector<long long> h_cnt((size_t)W * W);
@@ -1005,8 +1054,10 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
     return;
   }
   const size_t cap = (size_t)std::max<long long>(out.n, 1);
-  out.x.reserve(cap * d, 0, s); out.ids.reserve(cap, 0, s);
-  if (Owner::kLists) out.lists.reserve(cap, 0, s);
+  local_step(sh, agreed, "shard routing", [&] {
+    out.x.reserve(cap * d, 0, s); out.ids.reserve(cap, 0, s);
+    if (Owner::kLists) out.lists.reserve(cap, 0, s);
+  });
   B200VS_NCCL(nccl().GroupStart());
   for (int w = 0; w < W; ++w) {
     const long long so = send_off[w], sc = send_off[w + 1] - so, ro = recv_off[w], rc = recv_off[w + 1] - ro;
@@ -1032,31 +1083,36 @@ void route_rows(b200vs_shard* sh, int64_t n, const void* xv, int rb, const long 
 // checks that add (check_add: a negative id for every type, a repeated id for FLAT, max_elements for HNSW) and the statuses
 // are all-gathered: every rank returns the first refusal in rank order, or adds.  batched: b200vs_hnsw_add_batched with
 // `batch`.  Rows are in the index's row format (FP32, or packed bits on the binary types, which travel as they are: a
-// binary row has no normalisation).
-void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long long* ids_dev, bool batched, int batch) {
+// binary row has no normalisation).  agreed (b200vs_shard_rebuild_from): every local step before a collective (the
+// assignment and its cosine copy, the routing's copies) and the final add are agreed, so a device failure on one rank is
+// returned by every rank.
+void shard_add_impl(b200vs_shard* sh, int64_t n, const void* x_dev, const long long* ids_dev, bool batched, int batch, bool agreed = false) {
   IndexBase* ix = sh->ix;
   const int rb = (int)ix->query_row_bytes();
   cudaStream_t s = sh->ws;
   ix->set_device();
   Routed rv;
   if (sh->rows) {
-    route_rows(sh, n, x_dev, rb, ids_dev, nullptr, RowOwner{}, rv);
+    route_rows(sh, n, x_dev, rb, ids_dev, nullptr, RowOwner{}, rv, agreed);
   } else {
     DevBuf<float> prep;
     DevBuf<long long> lists;
-    const void* xp = n > 0 ? assign_rows(sh, n, x_dev, prep, lists) : x_dev;
-    route_rows(sh, n, xp, rb, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv);
+    const void* xp = x_dev;
+    local_step(sh, agreed, "shard add", [&] { if (n > 0) xp = assign_rows(sh, n, x_dev, prep, lists); });
+    route_rows(sh, n, xp, rb, ids_dev, lists.p, ListOwner{sh->lists_per_rank()}, rv, agreed);
   }
   std::vector<int64_t> hid((size_t)rv.n);  // the host ids check_add and the add take
-  if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
-  B200VS_CUDA(cudaStreamSynchronize(s));
+  local_step(sh, agreed, "shard add", [&] {
+    if (!hid.empty()) B200VS_CUDA(cudaMemcpyAsync(hid.data(), rv.ids.p, hid.size() * 8, cudaMemcpyDeviceToHost, s));
+    B200VS_CUDA(cudaStreamSynchronize(s));
+  });
   AddReq req = AddReq::device(rv.n, rv.x.p, rv.ids.p, rv.lists.p, false, sh->rows ? AddReq::RAW : AddReq::PREPARED);
   req.ids = hid.data();
   req.batched = batched;
   req.batch = batch;
   // status agreement
   check(agree(sh, attempt([&] { ix->check_add(req); }), "shard add"));
-  if (rv.n) ix->add(req);
+  local_step(sh, agreed, "shard add", [&] { if (rv.n) ix->add(req); });
 }
 
 // upload of host rows (query_row_bytes() each) to the write stream, for the host-pointer variants of the collective adds
@@ -1525,6 +1581,104 @@ int shard_add(b200vs_shard* h, int64_t n, const void* x, const int64_t* ids, boo
   });
 }
 
+// ---------------------------------------------------------------------------------------------
+// Rebuilds (b200vs_shard_need_rebuild / b200vs_shard_rebuild_from)
+// ---------------------------------------------------------------------------------------------
+// b200vs_need_rebuild's rule on the figures of the whole set: one all-gather of every rank's (live, tombstoned, trained);
+// the caller holds add_mu.  IVF types: the set is trained when every rank is.
+bool shard_need_rebuild_locked(b200vs_shard* sh) {
+  IndexBase* ix = sh->ix;
+  ix->set_device();
+  long long mine[3];
+  {
+    std::shared_lock<std::shared_mutex> rl(ix->rw);
+    mine[0] = (long long)ix->count(); mine[1] = (long long)ix->deleted_count(); mine[2] = ix->is_trained() ? 1 : 0;
+  }
+  const std::vector<long long> all = all_gather_host(sh, mine, 3);
+  int64_t live = 0, dead = 0;
+  bool trained = true;
+  for (int w = 0; w < sh->world; ++w) {
+    live += all[(size_t)w * 3]; dead += all[(size_t)w * 3 + 1]; trained = trained && all[(size_t)w * 3 + 2] != 0;
+  }
+  switch (ix->type) {
+    case B200VS_IVF_FLAT:
+    case B200VS_BINARY_IVF_FLAT: {  // shard_train refuses rather than degenerate nlist, so only nlist_org == 1 stays out
+      const int64_t nlist_org = ix->params.nlist > 0 ? ix->params.nlist : 2048;
+      return trained && nlist_org != 1 && live >= 256 * nlist_org && sh->train_rows_set <= live / 2;
+    }
+    case B200VS_IVF_PQ: return trained && live / 2 >= sh->train_rows_set;  // a set is in IVF-PQ mode (shard_create)
+    case B200VS_HNSW: return dead > 0 && dead > (live + dead) / 2;       // nodes = live + tombstoned, halved on the sums
+    default: return false;                                                // FLAT, BINARY_FLAT
+  }
+}
+
+// The refusals of b200vs_shard_rebuild_from on this rank, decided before any index changes (src is held shared by the caller)
+void check_shard_rebuild(b200vs_shard* dst, b200vs_shard* src) {
+  if (dst->world != src->world || dst->rank != src->rank) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src differ in world or rank");
+  IndexBase *d = dst->ix, *s = src->ix;
+  std::shared_lock<std::shared_mutex> rl(d->rw);
+  check_rebuild_pair(*d, *s);
+  if (d->type == B200VS_FLAT || d->type == B200VS_BINARY_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");
+  if (d->type == B200VS_IVF_PQ)
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild_from an IVF_PQ set: it stores only codes (rebuild it from host rows with shard_train + shard_add)");
+  if (d->type == B200VS_HNSW && d->params.max_elements > 0 && s->count() > d->params.max_elements)
+    fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below src's live rows");
+}
+
+// List-sharded rebuild (IVF_FLAT, BINARY_IVF_FLAT), every step on dst's write stream and communicator: src's live rows in
+// ascending id order (sorted_live_rows), routed to row_owner(id) (route_rows with RowOwner), sorted again by id after the
+// arrival (rank 0's rows first, each rank's in its own order, so ties keep (src rank, list-major position)), then
+// shard_train's flow and shard_add's flow on those device rows.  Every local step before a collective (the sorts, the
+// routing's and the add's copies, the k-means, the state install, the add) is agreed, so a device failure on one rank, an
+// allocation that does not fit included, is returned by every rank.  Returns the live rows this rank's dst holds.
+int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
+  IndexBase *d = dst->ix, *s = src->ix;
+  const int words = d->binary() ? (d->dim / 8 + 3) / 4 : d->dim;
+  const cudaStream_t ws = dst->ws;
+  d->set_device();
+  // 1) src's live rows sorted by id, behind every write src's own stream holds
+  DevBuf<uint32_t> rows;
+  DevBuf<long long> ids;
+  int64_t n = 0;
+  check(agree(dst, attempt([&] {
+    B200VS_CUDA(cudaStreamSynchronize(s->stream));
+    n = s->sorted_rows(rows, ids, ws);
+  }), "shard rebuild_from"));
+  // 2) to the training owner (the routing's send and receive copies are reserved in agreed steps)
+  Routed rv;
+  route_rows(dst, n, rows.p, words * 4, ids.p, nullptr, RowOwner{}, rv, true);
+  // 3) stable sort of what arrived by id: rows_r
+  DevBuf<uint32_t> tx;
+  DevBuf<long long> tids;
+  const int64_t m = rv.n;
+  check(agree(dst, attempt([&] {
+    B200VS_CUDA(cudaStreamSynchronize(ws));
+    rows.free(); ids.free();
+    sorted_live_rows(d, m, rv.ids.p, nullptr, true, reinterpret_cast<const uint32_t*>(rv.x.p), words, tx, tids, ws);
+  }), "shard rebuild_from"));
+  rv.x.free(); rv.ids.free();
+  int64_t total = 0;
+  for (const long long c : all_gather_host(dst, &m)) total += c;
+  if (total == 0) return 0;  // nothing live anywhere: dst stays untrained
+  // 4, 5) the rank-local coarse k-means, the centroid all-gather, the state install (refuses a rank below nlist / world rows)
+  shard_train_locked(dst, m, m ? tx.p : nullptr, true);
+  // 6) the collective add of rows_r: binary rows go back to their packed dim / 8 bytes
+  const void* xa = tx.p;
+  DevBuf<unsigned char> packed;
+  const size_t nb = d->query_row_bytes();
+  local_step(dst, true, "shard rebuild_from", [&] {
+    if (!d->binary() || nb == (size_t)words * 4 || !m) return;
+    packed.reserve((size_t)m * nb, 0, ws);
+    B200VS_CUDA(cudaMemcpy2DAsync(packed.p, nb, tx.p, (size_t)words * 4, nb, (size_t)m, cudaMemcpyDeviceToDevice, ws));
+    B200VS_CUDA(cudaStreamSynchronize(ws));
+    tx.free();
+    xa = packed.p;
+  });
+  shard_add_impl(dst, m, xa, tids.p, false, 0, true);
+  std::shared_lock<std::shared_mutex> rl(d->rw);
+  return d->count();
+}
+
 }  // namespace
 
 extern "C" {
@@ -1575,6 +1729,46 @@ int b200vs_shard_load(b200vs_shard* h, const char* prefix) {
     if (!prefix || !*prefix) fail(B200VS_EILLEGAL_PARAMETERS, "null snapshot prefix");
     std::lock_guard<std::mutex> g(sh->add_mu);
     shard_load_locked(sh, prefix);
+    if (!sh->rows) sh->train_rows_set = live_rows_set(sh);
+    return B200VS_OK;
+  });
+}
+
+// Collective NeedToRebuild of the whole set: 1, 0, or a status negated; the same answer on every rank.
+int b200vs_shard_need_rebuild(b200vs_shard* h) {
+  int r = 0;
+  const int rc = guarded([&]() -> int {
+    b200vs_shard* sh = get(h);
+    std::lock_guard<std::mutex> g(sh->add_mu);
+    r = shard_need_rebuild_locked(sh) ? 1 : 0;
+    return B200VS_OK;
+  });
+  return rc == B200VS_OK ? r : -rc;
+}
+
+// Collective rebuild of the fresh set dst from the set src (every rank passes its own dst and src).  src's writers wait on
+// its add_mu and its rank index stays under its reader lock, so src's reads go on; none of src's communicators is used.
+// The refusals are agreed before any index changes.  HNSW: each rank's single-index rebuild_from, then one more agreement.
+int b200vs_shard_rebuild_from(b200vs_shard* dst_h, b200vs_shard* src_h, int64_t* n_rows) {
+  return guarded([&]() -> int {
+    if (n_rows) *n_rows = 0;
+    b200vs_shard* dst = get(dst_h);
+    b200vs_shard* src = get(src_h);
+    if (dst == src) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src are the same shard");
+    std::scoped_lock g(src->add_mu, dst->add_mu);
+    RwSharedGuard rl(src->ix);
+    dst->ix->set_device();
+    check(agree(dst, attempt([&] { check_shard_rebuild(dst, src); }), "shard rebuild_from"));
+    int64_t n = 0;
+    if (dst->rows) {  // HNSW: every row already sits on its owner
+      check(agree(dst, attempt([&] {
+        WriteHold hold(dst->ix);
+        n = dst->ix->rebuild_from(*src->ix);
+      }), "shard rebuild_from"));
+    } else {
+      n = shard_rebuild_lists(dst, src);
+    }
+    if (n_rows) *n_rows = n;
     return B200VS_OK;
   });
 }

@@ -41,6 +41,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
     "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
     "b200vs_shard_search_deep", "b200vs_shard_search_binary_deep",
+    "b200vs_shard_need_rebuild", "b200vs_shard_rebuild_from",
 ]
 
 
@@ -166,6 +167,8 @@ def lib():
     L.b200vs_shard_range_search_binary_device.argtypes = [vp, i64, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp, vp]
     L.b200vs_shard_search_deep.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_shard_search_binary_deep.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_shard_need_rebuild.argtypes = [vp]
+    L.b200vs_shard_rebuild_from.argtypes = [vp, vp, ctypes.POINTER(i64)]
     _lib = L
     return L
 
@@ -536,6 +539,20 @@ class Shard:
     def load(self, prefix):
         """b200vs_shard_load (collective): restores a snapshot into this shard's empty indexes, at the same or another world."""
         _check(lib().b200vs_shard_load(self.h, prefix.encode()))
+
+    def need_rebuild(self):
+        """b200vs_shard_need_rebuild (collective): the NeedToRebuild rule on the figures of the whole set."""
+        r = int(lib().b200vs_shard_need_rebuild(self.h))
+        if r < 0:
+            _check(-r)
+        return bool(r)
+
+    def rebuild_from(self, src):
+        """b200vs_shard_rebuild_from (collective): fill this fresh shard from the shard src on the device; returns the live
+        rows this rank's index holds afterwards."""
+        n = ctypes.c_int64(0)
+        _check(lib().b200vs_shard_rebuild_from(self.h, src.h, ctypes.byref(n)))
+        return n.value
 
     def search(self, xq, k, seq=-1, **kw):
         xq = _f32(xq)

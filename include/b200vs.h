@@ -391,6 +391,49 @@ int b200vs_row_owner(int32_t world, int64_t n, const int64_t* ids, int32_t* out_
 /* collective snapshot save / restore of a sharded index (see above) */
 int b200vs_shard_save(b200vs_shard* shard, const char* prefix);
 int b200vs_shard_load(b200vs_shard* shard, const char* prefix);
+
+/* Rebuilds of a sharded set (DESIGN.md 4.9).  Both calls are collectives of the write path, like shard_save / shard_load: every
+ * rank calls them in the same order relative to the other writes of that shard, they use up no search sequence number, and
+ * every rank returns the same status.
+ *
+ * shard_need_rebuild: b200vs_need_rebuild's rule applied to the figures of the whole set (one all-gather of every rank's live
+ * and tombstoned rows), 1 = rebuild, 0 = not, < 0 = a status negated.  train_rows_set is kept in the shard handle, not in the
+ * rank indexes (each rank index's own b200vs_need_rebuild answers as before): the rows shard_train[_binary] clustered over
+ * every rank, or every rank's live rows summed at shard_broadcast_state and shard_load, or the rows shard_rebuild_from
+ * trained dst on; it is not saved.
+ *   IVF_FLAT, BINARY_IVF_FLAT : untrained, or created with nlist 1: 0; else sum(live) >= 256 * nlist and
+ *                               train_rows_set <= sum(live) / 2 (shard_train never degenerates nlist: it refuses)
+ *   IVF_PQ                    : sum(live) / 2 >= train_rows_set; untrained: 0 (a set is always in IVF-PQ mode)
+ *   HNSW                      : sum(deleted) > 0 and sum(deleted) > (sum(live) + sum(deleted)) / 2
+ *   FLAT, BINARY_FLAT         : 0
+ *
+ * shard_rebuild_from: every rank passes its own dst and src.  dst is a fresh shard (shard_create[_binary] under its own unique
+ * id) of the same world and rank, with an empty (IVF types: untrained) index of src's type, metric, dimension, nlist,
+ * nsubvector, nbits, nlinks, efconstruction and device.  *n_rows (nullable) = the live rows this rank's dst holds afterwards.
+ *   IVF_FLAT, BINARY_IVF_FLAT (by list) : let rows_r be src's live rows with b200vs_row_owner(id, world) == r in ascending id
+ *                     order (ties: by src rank, then that rank's list-major export order), taken as stored (cosine rows are
+ *                     not normalised again).  dst ends up equal, byte for byte (trained state, every list's ids and rows, the
+ *                     FP16 mirror), to a fresh shard on which every rank r called shard_train[_binary](rows_r) and then
+ *                     shard_add[_binary](rows_r, ids_r).  Routing the training rows by row_owner keeps the rank-local k-means
+ *                     balanced whatever the old list layout.  At world 1 this equals b200vs_rebuild_from.  No row crosses
+ *                     PCIe: src's live rows are sorted and routed on the device over dst's write stream and communicator.
+ *   HNSW (by row)   : each rank runs b200vs_rebuild_from of its src index into its dst index; nothing moves between ranks.
+ *   FLAT, BINARY_FLAT, IVF_PQ : EVECTOR_NOT_SUPPORT on every rank (an IVF_PQ set stores only codes: rebuild it from host
+ *                     rows with shard_train + shard_add).
+ * EILLEGAL_PARAMETERS, on every rank when any rank meets it (the first in rank order), before any index changes: a different
+ * world or rank, a dst that is not empty or (IVF types) already trained, differing creation parameters, an HNSW dst whose
+ * max_elements is below its rank's live rows, and a rank that would receive fewer than nlist / world training rows
+ * (shard_train's refusal; the rule never asks for a rebuild then).  dst == src is refused on the rank that passes it, before
+ * any collective, so every rank must pass it alike.  An src with no live rows on any rank: OK, dst stays untrained, *n_rows
+ * = 0.  A device failure after the agreement: EINTERNAL on every rank, src unchanged, dst to be discarded.
+ * Locks: src's writes wait for the call, its reads (shard_search, deep, range, on src's own lanes and communicators) go on
+ * and return unchanged results; none of src's communicators is used.  dst's writes wait too.
+ * Peak device memory per rank (by list): src's rows, plus about three copies of this rank's share of the live rows while
+ * they are sorted and routed (the sorted local copy, the partitioned send copy, the received copy; the local copy is freed
+ * once routed), then the training copy rows_r, shard_add's partitioned and received copies of it (cosine: and its
+ * normalised copy) and dst's rows. */
+int b200vs_shard_need_rebuild(b200vs_shard* shard);
+int b200vs_shard_rebuild_from(b200vs_shard* dst, b200vs_shard* src, int64_t* n_rows);
 int b200vs_shard_plan_add_device(b200vs_shard* shard, int64_t n, const float* x_dev);
 int b200vs_shard_plan_commit(b200vs_shard* shard);
 int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
