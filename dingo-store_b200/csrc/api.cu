@@ -510,6 +510,20 @@ int32_t b200vs_dimension(b200vs_index* h) { return h && h->impl ? h->impl->dim :
 int b200vs_save(b200vs_index* h, const char* path) {
   return guarded([&]() -> int { if (!path) fail(B200VS_EILLEGAL_PARAMETERS, "null path"); get(h)->save(path); return B200VS_OK; });
 }
+int b200vs_save_stage(b200vs_index* h) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    h->image.reset();  // a failed stage leaves no image, and the earlier one is not held beside the new one
+    SnapshotImage img;
+    ix->save_image(img);
+    h->image = std::move(img);
+    return B200VS_OK;
+  });
+}
+// b200vs_save_staged is in snapshot_write.cc, a host-only translation unit: it runs in a forked child
+void b200vs_save_unstage(b200vs_index* h) {
+  if (h) h->image.reset();
+}
 int b200vs_load(b200vs_index* h, const char* path) {
   return guarded([&]() -> int {
     if (!path) fail(B200VS_EILLEGAL_PARAMETERS, "null path");

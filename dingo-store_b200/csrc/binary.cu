@@ -111,6 +111,8 @@ struct BinRows {
     B200VS_CUDA(cudaMemcpy(tmp.data(), words.p + (size_t)r0 * w, tmp.size() * 4, cudaMemcpyDeviceToHost));
     for (int64_t i = 0; i < n; ++i) memcpy(out + (size_t)i * nb, tmp.data() + (size_t)i * w, nb);
   }
+  const void* row_data() const { return words.p; }
+  size_t row_pitch() const { return (size_t)w * 4; }  // the packed bytes lead each padded row (little-endian words)
   int64_t bytes() const { return (int64_t)(words.cap * 4 + ids.cap * 8); }
   // the row fields of a tile-scan view; the owner adds the list layout
   TcView view() const {
@@ -213,6 +215,13 @@ struct BinaryFlatIndex : BinaryIndex {
     quiesce();
     rowmap.export_rows(list_off, codes, out_ids);
   }
+  void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) override {
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    rowmap.pack(list_off, out_ids, out_rows);
+  }
 };
 
 IndexBase* make_binary_flat(int d, const b200vs_params& p) { return new BinaryFlatIndex(d, p); }
@@ -278,7 +287,8 @@ struct BinaryIvfIndex : BinaryIndex {
     set_device();
     state_header(blob, nlist);
     std::vector<uint32_t> tmp((size_t)nlist * w);
-    B200VS_CUDA(cudaMemcpy(tmp.data(), cent.p, tmp.size() * 4, cudaMemcpyDeviceToHost));
+    B200VS_CUDA(cudaMemcpyAsync(tmp.data(), cent.p, tmp.size() * 4, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
     for (int c = 0; c < nlist; ++c) memcpy((uint8_t*)blob + 32 + (size_t)c * nb, tmp.data() + (size_t)c * w, nb);
     return (int64_t)need;
   }
@@ -489,6 +499,13 @@ struct BinaryIvfIndex : BinaryIndex {
     set_device();
     quiesce();
     L.export_lists(nlist, list_off, store, codes, out_ids);
+  }
+  void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) override {
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    L.pack(nlist, list_off, store, out_ids, out_rows);
   }
 };
 

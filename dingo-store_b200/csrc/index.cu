@@ -332,6 +332,8 @@ struct RowStore {
   void download(int64_t r0, int64_t n, uint8_t* out) const {
     if (n > 0) B200VS_CUDA(cudaMemcpy(out, vecs.p + (size_t)r0 * d, (size_t)n * d * 4, cudaMemcpyDeviceToHost));
   }
+  const void* row_data() const { return vecs.p; }
+  size_t row_pitch() const { return (size_t)d * 4; }
   int64_t bytes() const { return (int64_t)(vecs.cap * 4 + ids.cap * 8 + norms.cap * 4 + vecs_h.cap * 2 + hscale.cap * 4); }
   // the row fields of a tile-scan view; the owner adds the list layout
   TcView view() const {
@@ -456,6 +458,13 @@ struct FlatIndex : IndexBase {
     quiesce();
     rowmap.export_rows(list_off, reinterpret_cast<uint8_t*>(vectors), out_ids);
   }
+  void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) override {
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    rowmap.pack(list_off, out_ids, out_rows);
+  }
 };
 
 IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p) { return new FlatIndex(m, d, p); }
@@ -548,7 +557,8 @@ struct IvfFlatIndex : IndexBase {
     if (!blob || cap < need) return (int64_t)need;
     set_device();
     state_header(blob, nlist);
-    B200VS_CUDA(cudaMemcpy((char*)blob + 32, centroids.p, (size_t)nlist * dim * 4, cudaMemcpyDeviceToHost));
+    B200VS_CUDA(cudaMemcpyAsync((char*)blob + 32, centroids.p, (size_t)nlist * dim * 4, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
     return (int64_t)need;
   }
 
@@ -656,6 +666,13 @@ struct IvfFlatIndex : IndexBase {
   }
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override;
   int64_t export_list(int list, int64_t cap, float* vectors, int64_t* out_ids) override;
+  void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) override {
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    L.pack(nlist, list_off, store, out_ids, out_rows);
+  }
 };
 
 void IvfFlatIndex::train(int64_t n, const void* x) {

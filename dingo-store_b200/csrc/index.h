@@ -22,10 +22,10 @@
 #include "../../include/b200vs.h"
 #include "common.cuh"
 #include "deep_select.cuh"
+#include "snapshot.h"
 
 namespace b200vs {
 
-extern thread_local std::string g_last_error;
 struct StatusError {
   int code;
   std::string msg;
@@ -399,6 +399,15 @@ struct IndexBase {
   }
   virtual void save(const std::string& path);
   virtual void load(const std::string& path);
+  // b200vs_save_stage: into img, the bytes save(path) would write now.  The rows are packed on the device (pack_lists), and
+  // the rest comes from the host bookkeeping.
+  virtual void save_image(SnapshotImage& img);
+  // export_lists' list offsets, ids and rows (in export_lists' host row format) of the live rows, gathered by one device pack
+  // and brought back with one copy per buffer on the index stream.  out_ids and out_rows need no alignment.
+  virtual void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) {
+    (void)list_off; (void)out_ids; (void)out_rows;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "this index type has no device rows to pack");
+  }
 
   // helpers shared by the index types
   // An AddReq's rows and ids on this device and its ids on the host, with the writer hold taken.  Host rows (row_bytes each)
@@ -460,11 +469,6 @@ struct LaneGuard {
   ~LaneGuard();
 };
 
-}  // namespace b200vs
-struct b200vs_index {  // the opaque handle of include/b200vs.h
-  b200vs::IndexBase* impl;
-};
-namespace b200vs {
 inline IndexBase* index_impl(b200vs_index* h) {
   if (!h || !h->impl) fail(B200VS_EILLEGAL_PARAMETERS, "null index handle");
   return h->impl;

@@ -4,8 +4,9 @@
 // A row store holds an index's device rows: FP32 rows (RowStore, index.cu), padded binary words (BinRows, binary.cu) or PQ
 // code rows (CodeRows, ivf_pq.cu), each with a device id per row (-1 = tombstone / unused slot).  The stores share one
 // shape, used here as a template argument: grow(cap, keep), reset(), move(src, dst, n), write(rows, ids, slots),
-// gather(src, dst, cap), download(r0, n, out) in the export's host format of row_bytes() each, bytes(), and the members
-// ix (the owning index, whose stream and scratch they use) and ids.  The store moves rows; the bookkeeping below decides
+// gather(src, dst, cap), download(r0, n, out) in the export's host format of row_bytes() each, bytes(), the device rows
+// row_data() of row_pitch() bytes each (the export format is each row's first row_bytes()), and the members ix (the owning
+// index, whose stream and scratch they use) and ids.  The store moves rows; the bookkeeping below decides
 // capacities, slots, tombstones, compaction and export order.
 //
 // Inverted lists live in ONE device arena (rows of the payload array), list l owning rows
@@ -26,6 +27,12 @@
 #include "tc_scan.cuh"
 
 namespace b200vs {
+
+// The snapshot pack (b200vs_save_stage, snapshot.cu): row slots[i] of the device rows `rows` (pitch bytes apart) and its id
+// ids[slots[i]] become row i of out_rows (the first row_bytes of it) and out_ids[i], on the host.  One gather kernel packs
+// them on the owner's stream, then one device-to-host copy per buffer and one synchronise.
+void pack_rows(IndexBase* ix, const std::vector<long long>& slots, const void* rows, size_t pitch, const long long* ids, size_t row_bytes,
+               void* out_ids, uint8_t* out_rows);
 
 // ids[r] = -1 for every listed row, on the owner's stream
 inline void tombstone_ids(IndexBase* ix, long long* ids, const std::vector<int64_t>& rows) {
@@ -122,6 +129,15 @@ struct FlatRowMap {
   void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows) const {
     for (int64_t r = 0; r < rows; ++r)
       if (h_ids[r] >= 0) { out_ids.push_back(h_ids[r]); out_rows.push_back(r); }
+  }
+  // export_rows' output through the device pack
+  void pack(int64_t* list_off, void* out_ids, uint8_t* out_rows) const {
+    std::vector<int64_t> ids;
+    std::vector<long long> slots;
+    live_slots(ids, slots);
+    if ((int64_t)slots.size() != count()) fail(B200VS_EINTERNAL, "row bookkeeping out of step with the live count");
+    list_off[0] = 0; list_off[1] = (int64_t)slots.size();
+    pack_rows(store.ix, slots, store.row_data(), store.row_pitch(), store.ids.p, store.row_bytes(), out_ids, out_rows);
   }
   // drop every row, keep the buffers
   void clear() {
@@ -382,6 +398,22 @@ struct IvfLists {
     for (const ListMeta& m : lists)
       for (int p = 0; p < m.len; ++p)
         if (h_ids[m.off + p] >= 0) { out_ids.push_back(h_ids[m.off + p]); out_rows.push_back(m.off + p); }
+  }
+  // export_lists' output through the device pack
+  template <class Store>
+  void pack(int nlist, int64_t* list_off, const Store& store, void* out_ids, uint8_t* out_rows) const {
+    std::vector<long long> slots;
+    slots.reserve((size_t)live);
+    for (int l = 0; l < nlist; ++l) {
+      list_off[l] = (int64_t)slots.size();
+      if (l >= (int)lists.size()) continue;
+      const ListMeta& m = lists[l];
+      for (int p = 0; p < m.len; ++p)
+        if (h_ids[m.off + p] >= 0) slots.push_back(m.off + p);
+    }
+    list_off[nlist] = (int64_t)slots.size();
+    if ((int64_t)slots.size() != live) fail(B200VS_EINTERNAL, "list bookkeeping out of step with the live count");
+    pack_rows(store.ix, slots, store.row_data(), store.row_pitch(), store.ids.p, store.row_bytes(), out_ids, out_rows);
   }
   // every list's live rows, list after list; list_off[nlist + 1] (nullable) gets where each list starts
   template <class Store>

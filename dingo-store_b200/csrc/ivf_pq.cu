@@ -440,6 +440,8 @@ struct CodeRows {
   void download(int64_t r0, int64_t n, uint8_t* out) const {
     if (n > 0) B200VS_CUDA(cudaMemcpy(out, codes.p + (size_t)r0 * cs, (size_t)n * cs, cudaMemcpyDeviceToHost));
   }
+  const void* row_data() const { return codes.p; }
+  size_t row_pitch() const { return (size_t)cs; }
   int64_t bytes() const { return (int64_t)(codes.cap + ids.cap * 8); }
 };
 
@@ -512,8 +514,9 @@ struct IvfPqIndex : IndexBase {
     set_device();
     int64_t hdr[6] = {0x51505649, nlist, dim, (int64_t)metric, M, nbits};
     memcpy(blob, hdr, 48);
-    B200VS_CUDA(cudaMemcpy((char*)blob + 48, centroids.p, nc * 4, cudaMemcpyDeviceToHost));
-    B200VS_CUDA(cudaMemcpy((char*)blob + 48 + nc * 4, codebooks.p, ncb * 4, cudaMemcpyDeviceToHost));
+    B200VS_CUDA(cudaMemcpyAsync((char*)blob + 48, centroids.p, nc * 4, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaMemcpyAsync((char*)blob + 48 + nc * 4, codebooks.p, ncb * 4, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
     return (int64_t)need;
   }
 
@@ -942,6 +945,31 @@ struct IvfPqIndex : IndexBase {
     } catch (...) { fclose(f); throw; }
     fclose(f);
   }
+  // save's bytes: the inner Flat index's rows, or the trained state and the code rows, packed on the device
+  void save_image(SnapshotImage& img) override {
+    RwSharedGuard hold(this);
+    int64_t hdr[8] = {0, (int64_t)mode, (int64_t)metric, dim, nlist, M, 0, 0};
+    memcpy(hdr, "B2VSPQ01", 8);
+    if (mode == kFlat) {
+      const int64_t n = flat->count();
+      hdr[6] = n;
+      img.alloc(sizeof(hdr) + (size_t)n * (8 + (size_t)dim * 4));
+      int64_t off[2];
+      if (n) flat->pack_lists(off, img.bytes.get() + sizeof(hdr), img.bytes.get() + sizeof(hdr) + (size_t)n * 8);
+    } else if (mode == kIvfPq) {
+      const int64_t st_len = get_state(nullptr, 0), n = count();
+      hdr[6] = n; hdr[7] = st_len;
+      const size_t off_at = sizeof(hdr) + (size_t)st_len, ids_at = off_at + ((size_t)nlist + 1) * 8, rows_at = ids_at + (size_t)n * 8;
+      img.alloc(rows_at + (size_t)n * code_size);
+      get_state(img.bytes.get() + sizeof(hdr), (size_t)st_len);
+      std::vector<int64_t> off((size_t)nlist + 1, 0);
+      if (n) pack_lists(off.data(), img.bytes.get() + ids_at, img.bytes.get() + rows_at);
+      memcpy(img.bytes.get() + off_at, off.data(), off.size() * 8);
+    } else {
+      img.alloc(sizeof(hdr));  // untrained: nothing but the header
+    }
+    memcpy(img.bytes.get(), hdr, sizeof(hdr));
+  }
   void load(const std::string& path) override {
     FILE* f = fopen(path.c_str(), "rb");
     if (!f) fail(B200VS_EINTERNAL, "cannot open " + path);
@@ -994,6 +1022,13 @@ struct IvfPqIndex : IndexBase {
     set_device();
     quiesce();
     L.export_lists(nlist, list_off, store, out_codes, out_ids);
+  }
+  void pack_lists(int64_t* list_off, void* out_ids, uint8_t* out_rows) override {
+    RwSharedGuard rl(this);
+    std::lock_guard<std::mutex> gl(gpu_mu);
+    set_device();
+    quiesce();
+    L.pack(nlist, list_off, store, out_ids, out_rows);
   }
 };
 

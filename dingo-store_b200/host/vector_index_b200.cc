@@ -11,6 +11,7 @@ namespace dingodb {
 
 int32_t VectorIndexB200::max_range_search_result_count = 1024;
 int64_t VectorIndexB200::hnsw_device_build_min_rows = 0;
+bool VectorIndexB200::support_fork_save = false;
 
 namespace {
 
@@ -172,7 +173,35 @@ butil::Status VectorIndexB200::Delete(const std::vector<int64_t>& delete_ids) {
   return ToStatus(b200vs_remove_ids(index_, (int64_t)delete_ids.size(), delete_ids.data(), &removed));
 }
 
-butil::Status VectorIndexB200::Save(const std::string& path) { return ToStatus(index_ ? b200vs_save(index_, path.c_str()) : B200VS_EINTERNAL); }
+void VectorIndexB200::LockWrite() {
+  write_gate_.lock();
+  if (!support_fork_save || !index_) return;
+  // LockWrite returns nothing: a failed stage is kept for the Save that follows
+  if (b200vs_save_stage(index_) == B200VS_OK) {
+    stage_state_.store(kStaged);
+  } else {
+    stage_error_ = b200vs_last_error();
+    stage_state_.store(kStageFailed);
+  }
+}
+
+void VectorIndexB200::UnlockWrite() {
+  if (stage_state_.exchange(kNotStaged) == kStaged) b200vs_save_unstage(index_);
+  write_gate_.unlock();
+}
+
+// In the fork flow this runs in the child: with an image staged it reaches only b200vs_save_staged, which takes no lock
+// and calls no CUDA function, and it logs nothing.
+butil::Status VectorIndexB200::Save(const std::string& path) {
+  if (!index_) return ToStatus(B200VS_EINTERNAL);
+  if (!support_fork_save) return ToStatus(b200vs_save(index_, path.c_str()));
+  if (path.empty()) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "path is empty");  // flat.cc:347-349
+  switch (stage_state_.load()) {
+    case kStaged: return ToStatus(b200vs_save_staged(index_, path.c_str()));
+    case kStageFailed: return butil::Status(pb::error::EINTERNAL, stage_error_);
+    default: return ToStatus(b200vs_save(index_, path.c_str()));
+  }
+}
 butil::Status VectorIndexB200::Load(const std::string& path) { return ToStatus(index_ ? b200vs_load(index_, path.c_str()) : B200VS_EINTERNAL); }
 
 // The index-free part of the lowering: RangeFilterFunctor and SortFilterFunctor — the only two ever constructed in src/
@@ -411,7 +440,25 @@ butil::Status VectorIndexB200::RebuildFrom(VectorIndexB200& old) {
   if (!index_ || !old.index_) return butil::Status(pb::error::EINTERNAL, "index not created");
   return ToStatus(b200vs_rebuild_from(index_, old.index_, nullptr));
 }
-bool VectorIndexB200::NeedToSave(int64_t last_save_log_behind) { return SupportSave() && last_save_log_behind > 10000; }  // flat.cc:515-531
+bool VectorIndexB200::NeedToSave(int64_t last_save_log_behind) {
+  if (!SupportSave() || !index_) return false;
+  int64_t count = 0, deleted = 0;
+  if (b200vs_count(index_, &count) != B200VS_OK || b200vs_deleted_count(index_, &deleted) != B200VS_OK) return false;
+  switch (vector_index_type) {
+    case pb::common::VECTOR_INDEX_TYPE_HNSW:  // hnsw.cc:592-609
+      if (count + deleted == 0) return false;
+      break;
+    case pb::common::VECTOR_INDEX_TYPE_IVF_FLAT:  // ivf_flat.cc:786-802, raw_ivf_pq.cc:533-549, ivf_pq.cc:450-462
+    case pb::common::VECTOR_INDEX_TYPE_BINARY_IVF_FLAT:
+    case pb::common::VECTOR_INDEX_TYPE_IVF_PQ:
+      if (b200vs_is_trained(index_) != 1 || count == 0) return false;
+      break;
+    default:  // FLAT, BINARY_FLAT: flat.cc:515-531
+      if (count == 0) return false;
+      break;
+  }
+  return last_save_log_behind > 10000;
+}
 
 namespace {
 butil::Status AbiStatus(int rc) {

@@ -14,7 +14,9 @@
 #include "dingo_shim.h"
 #endif
 
+#include <atomic>
 #include <shared_mutex>
+#include <string>
 
 #include "../../include/b200vs.h"
 
@@ -52,8 +54,9 @@ class VectorIndexB200 : public VectorIndex {
                             const pb::common::VectorSearchParameter& parameter,
                             std::vector<pb::index::VectorWithDistanceResult>& results) override;
 
-  void LockWrite() override { write_gate_.lock(); }
-  void UnlockWrite() override { write_gate_.unlock(); }
+  // With support_fork_save, LockWrite also stages the snapshot (b200vs_save_stage) and UnlockWrite frees it
+  void LockWrite() override;
+  void UnlockWrite() override;
   butil::Status Train(std::vector<float>& train_datas) override;
   butil::Status Train(std::vector<uint8_t>& train_datas) override;  // packed rows, dimension / 8 bytes each
   butil::Status Train(const std::vector<pb::common::VectorWithId>& vectors) override;
@@ -63,10 +66,13 @@ class VectorIndexB200 : public VectorIndex {
   butil::Status RebuildFrom(VectorIndexB200& old);
   bool NeedTrain() override;
   bool IsTrained() override;
+  // the stock plugins' rules (flat.cc:515-531, ivf_flat.cc:786-802, raw_ivf_pq.cc:533-549, ivf_pq.cc:450-462, hnsw.cc:592-609):
+  // no rows (HNSW: no live or deleted node) or untrained: false, else last_save_log_behind > 10000.  False without save support.
   bool NeedToSave(int64_t last_save_log_behind) override;
-  // fork()-based saving (vector_index_snapshot_manager.cc:583-608) cannot carry a CUDA context into the child:
-  // report "no save support" like the DiskANN plugin (vector_index_diskann.cc:267); the server rebuilds from RocksDB.
-  bool SupportSave() override { return false; }
+  // fork()-based saving (vector_index_snapshot_manager.cc:583-608) cannot carry a CUDA context into the child.  Without
+  // support_fork_save the plugin reports "no save support" like the DiskANN plugin (vector_index_diskann.cc:267) and the
+  // server rebuilds from RocksDB; with it, the save is split at the fork (see support_fork_save).
+  bool SupportSave() override { return support_fork_save; }
   pb::common::VectorIndexType VectorIndexSubType() override;  // vector_index.h:238
 
   // largest result count RangeSearch keeps per query (FLAGS_vector_index_max_range_search_result_count, vector_reader.cc:60)
@@ -74,6 +80,12 @@ class VectorIndexB200 : public VectorIndex {
   // HNSW Add / Upsert calls of at least this many rows build the graph on the GPU in batches (b200vs_hnsw_add_batched,
   // library default batch); smaller calls keep the host builder.  0 = off: every call takes the host builder.
   static int64_t hnsw_device_build_min_rows;
+  // Snapshots through the fork-based save (default false: no save support, as before).  When true, SupportSave() is true
+  // for every type; LockWrite takes the write gate and stages in host memory the bytes Save would write (b200vs_save_stage:
+  // the device work runs in the parent, under the gate); Save writes the staged bytes (b200vs_save_staged: no CUDA, no lock,
+  // no logging, so the forked child may call it), or calls b200vs_save when nothing is staged; UnlockWrite frees the staged
+  // bytes and releases the gate.  Costs one host copy of the region's saved rows while the gate is held.
+  static bool support_fork_save;
 
  private:
   butil::Status AddOrUpsert(const std::vector<pb::common::VectorWithId>& vector_with_ids, bool is_upsert);
@@ -86,6 +98,10 @@ class VectorIndexB200 : public VectorIndex {
   int32_t dimension_ = 0;
   pb::common::MetricType metric_type_ = pb::common::METRIC_TYPE_NONE;
   std::shared_mutex write_gate_;  // LockWrite/UnlockWrite of the snapshot path; reads and writes lock inside the library
+  // what LockWrite's stage left for Save: nothing (b200vs_save), an image, or a failed stage and its message
+  enum StageState { kNotStaged, kStaged, kStageFailed };
+  std::atomic<int> stage_state_{kNotStaged};
+  std::string stage_error_;
 };
 
 // VectorIndexUtils::CalcDistanceEntry (src/vector/vector_index_utils.cc:48-76) over the C ABI: same operand meaning

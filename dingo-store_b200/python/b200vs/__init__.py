@@ -42,6 +42,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
     "b200vs_shard_search_deep", "b200vs_shard_search_binary_deep",
     "b200vs_shard_need_rebuild", "b200vs_shard_rebuild_from",
+    "b200vs_save_stage", "b200vs_save_staged", "b200vs_save_unstage",
 ]
 
 
@@ -99,6 +100,10 @@ def lib():
     L.b200vs_dimension.argtypes = [vp]
     L.b200vs_save.argtypes = [vp, ctypes.c_char_p]
     L.b200vs_load.argtypes = [vp, ctypes.c_char_p]
+    L.b200vs_save_stage.argtypes = [vp]
+    L.b200vs_save_staged.argtypes = [vp, ctypes.c_char_p]
+    L.b200vs_save_unstage.argtypes = [vp]
+    L.b200vs_save_unstage.restype = None
     L.b200vs_export_lists.argtypes = [vp, vp, vp, vp, vp]
     L.b200vs_merge_topk_device.argtypes = [i32, i32, i64, i32, vp, vp, vp, vp, vp]
     L.b200vs_last_search_stats.argtypes = [vp, ctypes.POINTER(i64 * 8)]
@@ -464,6 +469,18 @@ class Index:
 
     def load(self, path):
         _check(self.L.b200vs_load(self.h, path.encode()))
+
+    def save_stage(self):
+        """Stage in host memory the bytes save() would write now (b200vs_save_stage)."""
+        _check(self.L.b200vs_save_stage(self.h))
+
+    def save_staged(self, path):
+        """Write the staged bytes to path; calls no CUDA function and takes no lock, so a forked child may call it."""
+        _check(self.L.b200vs_save_staged(self.h, path.encode()))
+
+    def save_unstage(self):
+        """Free the staged bytes; a no-op without any."""
+        self.L.b200vs_save_unstage(self.h)
 
 
 class Shard:

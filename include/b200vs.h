@@ -206,6 +206,25 @@ int32_t b200vs_dimension(b200vs_index* idx);
 int b200vs_save(b200vs_index* idx, const char* path);
 int b200vs_load(b200vs_index* idx, const char* path);
 
+/* Fork-based snapshots (VectorIndexSnapshotManager::SaveVectorIndexSnapshot: LockWrite, fork, Save in the child,
+ * UnlockWrite in the parent).  A forked child cannot use the parent's CUDA context, so the save is split at the fork:
+ *   save_stage   : in the parent, builds in ordinary pageable host memory the exact bytes b200vs_save would write now and
+ *                  keeps them in the handle, replacing an earlier image.  The live rows are packed on the device and brought
+ *                  back with one copy per buffer on the index's stream; HNSW needs no device work.  Runs under the index's
+ *                  reader lock, as b200vs_save does.  A failed host allocation or device step returns EINTERNAL and leaves
+ *                  no image (an earlier one is freed too).
+ *   save_staged  : writes the staged image to path.  Safe in the forked child of a multi-threaded CUDA process: it calls
+ *                  no CUDA function, takes no library lock (another parent thread may have held one at the fork), logs
+ *                  nothing and starts no thread.  The file is byte-identical to what b200vs_save would have written at the
+ *                  moment of save_stage; writes to the index after the stage do not change it, and b200vs_load reads it.
+ *                  No image, or a null or empty path: EILLEGAL_PARAMETERS.  An I/O failure: EINTERNAL, the image is kept.
+ *   save_unstage : frees the image; a no-op without one.  b200vs_destroy frees it too.
+ * The caller serialises stage, staged write and unstage on one handle (the plugin does so under its write gate).  The image
+ * costs one copy of the index's saved bytes in host memory while it is held. */
+int b200vs_save_stage(b200vs_index* idx);
+int b200vs_save_staged(b200vs_index* idx, const char* path);
+void b200vs_save_unstage(b200vs_index* idx);
+
 /* VectorIndex::NeedToRebuild (vector_index.h:198): 1 = rebuild, 0 = not, < 0 = a status negated.  The reference plugins' rules
  * (max_points_per_centroid = 256; count = live rows; train_rows = n of the b200vs_train[_binary] call that trained the index,
  * or the live count after b200vs_load or at b200vs_set_trained_state; it is not saved):
