@@ -19,6 +19,26 @@ namespace {
 
 IndexBase* get(b200vs_index* h) { return index_impl(h); }
 
+// b200vs_rebuild_from[_range]: fill dst from the live rows with lo <= id <= hi of srcs (distinct, dst not among them).  The
+// sources are held under their reader locks and dst under its writer hold, taken in one order, by address, so two calls over
+// overlapping sources (a split's child and parent rebuilding from the parent's index at once) cannot deadlock.  flat_ok:
+// FLAT and BINARY_FLAT are served.
+int64_t rebuild_range(IndexBase* dst, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, bool flat_ok) {
+  std::vector<IndexBase*> order(srcs);
+  order.push_back(dst);
+  std::sort(order.begin(), order.end(), std::less<IndexBase*>());
+  std::vector<std::shared_lock<std::shared_mutex>> reads;
+  std::unique_ptr<WriteHold> hold;
+  for (IndexBase* ix : order) {
+    if (ix == dst) hold.reset(new WriteHold(dst));
+    else reads.emplace_back(ix->rw);
+  }
+  for (IndexBase* src : srcs) check_rebuild_pair(*dst, *src);
+  if (!flat_ok && (dst->type == B200VS_FLAT || dst->type == B200VS_BINARY_FLAT))
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");  // vector_index_flat.h:111
+  return dst->rebuild_from(srcs, lo, hi);
+}
+
 // the float entry points (train / add / search / range search) on a binary index, and the binary ones on a float index
 void check_row_type(IndexBase* ix, bool binary_call) {
   if (ix->binary() != binary_call)
@@ -552,12 +572,31 @@ int b200vs_rebuild_from(b200vs_index* dst_h, b200vs_index* src_h, int64_t* n_row
     IndexBase* dst = get(dst_h);
     IndexBase* src = get(src_h);
     if (dst == src) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src are the same index");
-    std::shared_lock<std::shared_mutex> rl(src->rw);  // searches on src go on; its writers wait
-    WriteHold hold(dst);
-    check_rebuild_pair(*dst, *src);
-    if (dst->type == B200VS_FLAT || dst->type == B200VS_BINARY_FLAT)
-      fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");  // vector_index_flat.h:111
-    const int64_t n = dst->rebuild_from(*src);
+    // every live row: ids are non-negative, and the bounds are inclusive
+    const int64_t n = rebuild_range(dst, {src}, 0, INT64_MAX, false);
+    if (n_rows) *n_rows = n;
+    return B200VS_OK;
+  });
+}
+
+int b200vs_rebuild_from_range(b200vs_index* dst_h, int32_t n_src, b200vs_index* const* srcs_h, int64_t id_min, int64_t id_max,
+                              int64_t* n_rows) {
+  return guarded([&]() -> int {
+    if (n_rows) *n_rows = 0;
+    if (n_src < 1 || n_src > kRebuildMaxSources || !srcs_h)
+      fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from_range: 1 to 16 sources, in a non-null list");
+    IndexBase* dst = get(dst_h);
+    std::vector<IndexBase*> srcs;
+    for (int32_t i = 0; i < n_src; ++i) {
+      IndexBase* src = get(srcs_h[i]);
+      if (src == dst) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from_range: dst is among the sources");
+      if (std::find(srcs.begin(), srcs.end(), src) != srcs.end()) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from_range: a source is listed twice");
+      srcs.push_back(src);
+    }
+    if (id_min > id_max) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from_range: id_min > id_max");
+    // [id_min, id_max) as inclusive bounds; id_max - 1 cannot overflow once the range holds an id
+    const bool none = id_min == id_max;
+    const int64_t n = rebuild_range(dst, srcs, none ? 1 : id_min, none ? 0 : id_max - 1, true);
     if (n_rows) *n_rows = n;
     return B200VS_OK;
   });

@@ -182,6 +182,23 @@ struct BinaryFlatIndex : BinaryIndex {
     WriteHold hold(this);
     return rowmap.remove(n, del);
   }
+  void live_rows(int64_t lo, int64_t hi, RebuildSource& out) override {
+    rowmap.live_slots(out.ids, out.slots, lo, hi);
+    out.rows = rowmap.store.words.p;
+    out.stream = stream;
+  }
+  // the sources' padded rows in ascending id order in one add
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    const int64_t n = sorted_live_rows(this, srcs, lo, hi, w, rows, ids, stream);
+    if (n == 0) return 0;
+    std::vector<int64_t> h_ids(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids.p, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    rowmap.add(n, rows.p, ids.p, h_ids.data());
+    return n;
+  }
   ScanJob job(const SearchCtx& sc) const {
     ScanJob j = hamming_job(rowmap.store.words.p, rowmap.store.ids.p, rowmap.rows);
     j.sc = &sc;
@@ -374,18 +391,16 @@ struct BinaryIvfIndex : BinaryIndex {
     if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
     return false;
   }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
-    std::vector<int64_t> ids;
-    std::vector<long long> slots;
-    L.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, store.words.p, w, rows, out_ids, s);
-    return (int64_t)ids.size();
+  void live_rows(int64_t lo, int64_t hi, RebuildSource& out) override {
+    L.live_slots(out.ids, out.slots, lo, hi);
+    out.rows = store.words.p;
+    out.stream = stream;
   }
-  // train on src's padded rows in ascending id order, then add them in that order
-  int64_t rebuild_from(IndexBase& src) override {
+  // train on the sources' padded rows in ascending id order, then add them in that order
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.sorted_rows(rows, ids, src.stream);
+    const int64_t n = sorted_live_rows(this, srcs, lo, hi, w, rows, ids, stream);
     if (n == 0) return 0;
     train_locked(n, nullptr, rows.p);
     scratch.reset(stream);

@@ -1389,22 +1389,30 @@ struct HnswIndex : IndexBase {
   int64_t deleted_count() const override { return G.ndeleted; }
   // VectorIndexHnsw::NeedToRebuild, hnsw.cc:577-590: tombstones are more than half of every node, live or deleted
   bool need_rebuild() const override { return G.n > 0 && G.ndeleted > 0 && G.ndeleted > G.n / 2; }
-  // the live nodes' stored rows (cosine: already normalised) in ascending label order, through the batched builder with
-  // the default batch; this fresh index's level generator draws the levels, so the graph has no tombstones
-  int64_t rebuild_from(IndexBase& other) override {
-    const HostGraph& S = static_cast<HnswIndex&>(other).G;
-    std::vector<std::pair<int64_t, int64_t>> live;  // (label, node): labels of live nodes are unique
-    live.reserve((size_t)(S.n - S.ndeleted));
-    for (int64_t i = 0; i < S.n; ++i) if (!S.deleted[i]) live.emplace_back(S.labels[i], i);
+  // the sources' live nodes with lo <= label <= hi, their stored rows (cosine: already normalised) in ascending label order,
+  // gathered on the host (the rows live in the host graph), through the batched builder with the default batch; this fresh
+  // index's level generator draws the levels, so the graph has no tombstones
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
+    struct Live { int64_t label; const float* row; };
+    std::vector<Live> live;
+    for (IndexBase* src : srcs) {
+      const HostGraph& S = static_cast<HnswIndex*>(src)->G;
+      for (int64_t i = 0; i < S.n; ++i)
+        if (!S.deleted[i] && S.labels[i] >= lo && S.labels[i] <= hi) live.push_back({S.labels[i], S.data.data() + (size_t)i * dim});
+    }
     const int64_t n = (int64_t)live.size();
-    if (n > max_element_limit) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below src's live rows");
+    if (n > max_element_limit) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below the rows to copy");
     if (n == 0) return 0;
-    std::sort(live.begin(), live.end());
+    std::sort(live.begin(), live.end(), [](const Live& a, const Live& b) { return a.label < b.label; });
+    // the labels of one graph's live nodes are unique: a repeated label is held by two sources
+    for (int64_t i = 1; i < n; ++i)
+      if (live[i].label == live[i - 1].label)
+        fail(B200VS_EVECTOR_ID_DUPLICATED, "rebuild_from_range: id " + std::to_string(live[i].label) + " is held by more than one source");
     std::vector<float> rows((size_t)n * dim);
     std::vector<int64_t> ids(n);
     for (int64_t i = 0; i < n; ++i) {
-      ids[i] = live[i].first;
-      memcpy(&rows[(size_t)i * dim], S.data.data() + (size_t)live[i].second * dim, (size_t)dim * 4);
+      ids[i] = live[i].label;
+      memcpy(&rows[(size_t)i * dim], live[i].row, (size_t)dim * 4);
     }
     add_batched_locked(n, rows.data(), ids.data(), 0, true);
     return n;

@@ -441,14 +441,22 @@ struct FlatIndex : IndexBase {
   int64_t count() const override { return rowmap.count(); }
   int64_t deleted_count() const override { return rowmap.ndeleted; }
   int64_t memory_size() const override { return rowmap.store.bytes(); }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
-    // the inner Flat of an IVF-PQ region takes its writes under its own lock, not under the outer index's
-    RwSharedGuard rl(this);
-    std::vector<int64_t> ids;
-    std::vector<long long> slots;
-    rowmap.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(rowmap.store.vecs.p), dim, rows, out_ids, s);
-    return (int64_t)ids.size();
+  void live_rows(int64_t lo, int64_t hi, RebuildSource& out) override {
+    rowmap.live_slots(out.ids, out.slots, lo, hi);
+    out.rows = reinterpret_cast<const uint32_t*>(rowmap.store.vecs.p);
+    out.stream = stream;
+  }
+  // the sources' stored rows in ascending id order in one add (cosine rows are already normalised)
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    const int64_t n = sorted_live_rows(this, srcs, lo, hi, dim, rows, ids, stream);
+    if (n == 0) return 0;
+    std::vector<int64_t> h_ids(n);
+    B200VS_CUDA(cudaMemcpyAsync(h_ids.data(), ids.p, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+    B200VS_CUDA(cudaStreamSynchronize(stream));
+    rowmap.add(n, reinterpret_cast<const float*>(rows.p), ids.p, h_ids.data());
+    return n;
   }
 
   void export_lists(int64_t* list_off, float* vectors, uint8_t*, int64_t* out_ids) override {
@@ -589,18 +597,17 @@ struct IvfFlatIndex : IndexBase {
     if (nlist == nlist_org && nlist != 1 && L.live >= 256 * nlist_org) return train_rows <= L.live / 2;
     return false;
   }
-  int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& out_ids, cudaStream_t s) override {
-    std::vector<int64_t> ids;
-    std::vector<long long> slots;
-    L.live_slots(ids, slots);
-    sorted_live_rows(this, ids, slots, reinterpret_cast<const uint32_t*>(store.vecs.p), dim, rows, out_ids, s);
-    return (int64_t)ids.size();
+  void live_rows(int64_t lo, int64_t hi, RebuildSource& out) override {
+    L.live_slots(out.ids, out.slots, lo, hi);
+    out.rows = reinterpret_cast<const uint32_t*>(store.vecs.p);
+    out.stream = stream;
   }
-  // train on src's stored rows in ascending id order, then add them in that order; stored cosine rows are already normalised
-  int64_t rebuild_from(IndexBase& src) override {
+  // train on the sources' stored rows in ascending id order, then add them in that order; stored cosine rows are already
+  // normalised
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.sorted_rows(rows, ids, src.stream);
+    const int64_t n = sorted_live_rows(this, srcs, lo, hi, dim, rows, ids, stream);
     if (n == 0) return 0;
     train_locked(n, reinterpret_cast<const float*>(rows.p), true);
     scratch.reset(stream);

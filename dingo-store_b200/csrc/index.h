@@ -243,6 +243,17 @@ struct AddReq {
   }
 };
 
+// One source of a rebuild (b200vs_rebuild_from[_range], IndexBase::live_rows): the live rows of an index inside an id range,
+// as their ids and row slots in the index's storage order from its host bookkeeping, and the device row store they index.
+constexpr int kRebuildMaxSources = 16;
+struct RebuildSource {
+  std::vector<int64_t> ids;
+  std::vector<long long> slots;
+  const uint32_t* rows = nullptr;            // the row store: the same number of 32-bit words per row in every source
+  cudaStream_t stream = nullptr;             // the stream the store's writes run on
+  std::shared_lock<std::shared_mutex> hold;  // the reader lock of an inner index whose writers do not take the outer one
+};
+
 // The header of IndexBase::save's container ("B2VSIDX1" / "B2VSBIN1"), followed by the trained-state blob (state_len
 // bytes), the list offsets (nlist + 1 int64), the ids (count int64) and the rows (count rows, list-major).
 struct IndexFileHdr { char magic[8]; int32_t type, metric, dim, nlist; int64_t state_len, count; };
@@ -319,13 +330,16 @@ struct IndexBase {
   int64_t train_rows = 0;
   // VectorIndex::NeedToRebuild (b200vs_need_rebuild): the reference plugin's rule for this type; callers hold rw shared
   virtual bool need_rebuild() const { return false; }
-  // b200vs_rebuild_from: fill this empty, untrained index (rw and gpu_mu held, scratch reset, check_rebuild_pair passed)
-  // from src's live rows in ascending id order, as a fresh train + add of them would; src is held shared.  Returns the rows.
-  virtual int64_t rebuild_from(IndexBase& src) { (void)src; fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild is not supported for this index type"); }
-  // the live rows in ascending id order on this index's device (rebuild_from's source), built on stream s: rows [n, row
-  // words] and ids [n]; returns n.  Callers hold rw.
-  virtual int64_t sorted_rows(DevBuf<uint32_t>& rows, DevBuf<long long>& ids, cudaStream_t s) {
-    (void)rows; (void)ids; (void)s;
+  // b200vs_rebuild_from[_range]: fill this empty, untrained index (rw and gpu_mu held, scratch reset, check_rebuild_pair
+  // passed for every source) from the live rows with lo <= id <= hi of srcs in ascending id order, as a fresh train + add of
+  // them would; the sources are held shared.  Returns the rows.
+  virtual int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) {
+    (void)srcs; (void)lo; (void)hi;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild is not supported for this index type");
+  }
+  // this index's live rows with lo <= id <= hi as a rebuild source (sorted_live_rows).  Callers hold rw.
+  virtual void live_rows(int64_t lo, int64_t hi, RebuildSource& out) {
+    (void)lo; (void)hi; (void)out;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "this index type has no row store to rebuild from");
   }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }

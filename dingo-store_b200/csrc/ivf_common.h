@@ -125,10 +125,10 @@ struct FlatRowMap {
     publish_len();
     compact_if_needed();
   }
-  // the live (id, row) pairs in row order
-  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows) const {
+  // the live (id, row) pairs with lo <= id <= hi in row order
+  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows, int64_t lo = 0, int64_t hi = INT64_MAX) const {
     for (int64_t r = 0; r < rows; ++r)
-      if (h_ids[r] >= 0) { out_ids.push_back(h_ids[r]); out_rows.push_back(r); }
+      if (h_ids[r] >= 0 && h_ids[r] >= lo && h_ids[r] <= hi) { out_ids.push_back(h_ids[r]); out_rows.push_back(r); }
   }
   // export_rows' output through the device pack
   void pack(int64_t* list_off, void* out_ids, uint8_t* out_rows) const {
@@ -393,11 +393,13 @@ struct IvfLists {
     }
     return o;
   }
-  // the live (id, arena row) pairs, list after list in list order, as export_lists gives them
-  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows) const {
+  // the live (id, arena row) pairs with lo <= id <= hi, list after list in list order, as export_lists gives them
+  void live_slots(std::vector<int64_t>& out_ids, std::vector<long long>& out_rows, int64_t lo = 0, int64_t hi = INT64_MAX) const {
     for (const ListMeta& m : lists)
-      for (int p = 0; p < m.len; ++p)
-        if (h_ids[m.off + p] >= 0) { out_ids.push_back(h_ids[m.off + p]); out_rows.push_back(m.off + p); }
+      for (int p = 0; p < m.len; ++p) {
+        const int64_t id = h_ids[m.off + p];
+        if (id >= 0 && id >= lo && id <= hi) { out_ids.push_back(id); out_rows.push_back(m.off + p); }
+      }
   }
   // export_lists' output through the device pack
   template <class Store>
@@ -570,22 +572,22 @@ void kmeans_gpu_dev(IndexBase* ix, int d, int64_t n, const float* x_dev, int k, 
   kmeans_lloyd(ix, d, m, xs, hx.data(), k, niter, seed, cent, assign, prepare_ids);
 }
 
-// The live rows of an index in ascending id order, on its device (b200vs_rebuild_from, b200vs_shard_rebuild_from): (ids[i],
-// slots[i]), i < n, are the live rows in the index's own storage order, on the host or (on_device) on the device, where a
-// null slots stands for 0, 1, ..., n - 1; they are sorted by id with a stable device radix sort (rows that share an id keep
-// that order), and row slots[i] of src (`words` 32-bit words per row) is gathered into out_rows.  Runs on stream s and
-// returns with it synchronised.
-void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids, const long long* slots, bool on_device, const uint32_t* src,
-                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s);
-inline void sorted_live_rows(IndexBase* ix, const std::vector<int64_t>& ids, const std::vector<long long>& slots, const uint32_t* src,
-                             int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
-  sorted_live_rows(ix, (int64_t)ids.size(), reinterpret_cast<const long long*>(ids.data()), slots.data(), false, src, words, out_rows,
-                   out_ids, s);
-}
+// The rows of a rebuild in ascending id order, on the sources' device (b200vs_rebuild_from[_range],
+// b200vs_shard_rebuild_from): the live rows with lo <= id <= hi of every source (IndexBase::live_rows, filtered on the host
+// before anything is uploaded), concatenated in source order, sorted by id with one stable device radix sort whose values
+// encode (source, slot), so rows that share an id keep source order and then each source's storage order, and gathered by
+// one kernel from each source's row store (`words` 32-bit words per row) into out_rows.  An id held by more than one source
+// is refused with EVECTOR_ID_DUPLICATED (the gather compares adjacent sorted ids).  ix counts the launches.  Runs on stream s
+// and returns the row count with s synchronised.
+int64_t sorted_live_rows(IndexBase* ix, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, int words, DevBuf<uint32_t>& out_rows,
+                         DevBuf<long long>& out_ids, cudaStream_t s);
+// the same sort and gather of the n rows of one device row block src whose ids ids_dev are on the device
+void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids_dev, const uint32_t* src, int words, DevBuf<uint32_t>& out_rows,
+                      DevBuf<long long>& out_ids, cudaStream_t s);
 // out [m, dim] = the +-1 floats (binary_to_real: bit set -> 1, else -1) of padded binary rows words [.., w] (rows ? rows[i] : i)
 void launch_expand_pm1(const uint32_t* words, const long long* rows, int64_t m, int w, int dim, float* out, cudaStream_t s);
-// the refusals b200vs_rebuild_from shares for every type: dst must be empty, untrained, another index of the same type,
-// metric, dimension, result-deciding creation parameters and device
+// the refusals b200vs_rebuild_from[_range] shares for every type and source: dst must be empty, untrained, another index of
+// the same type, metric, dimension, result-deciding creation parameters and device
 void check_rebuild_pair(const IndexBase& dst, const IndexBase& src);
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids);

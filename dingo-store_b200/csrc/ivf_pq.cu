@@ -562,15 +562,19 @@ struct IvfPqIndex : IndexBase {
     if (mode == kIvfPq) return L.live / 2 >= train_rows;
     return false;
   }
-  // from an index in inner-Flat mode: train's rule on its stored rows in ascending id order (IVF-PQ from `need` rows on,
-  // else inner Flat again), then one add of them in that order.  An IVF-PQ mode index keeps only codes: refused.
-  int64_t rebuild_from(IndexBase& other) override {
-    IvfPqIndex& src = static_cast<IvfPqIndex&>(other);
-    if (src.mode == kIvfPq) fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild_from an IVF_PQ index in IVF-PQ mode: only its codes are stored");
-    if (src.mode == kNone) return 0;
+  // a source in inner-Flat mode gives its inner index's rows; an IVF-PQ mode index keeps only codes: refused
+  void live_rows(int64_t lo, int64_t hi, RebuildSource& out) override {
+    if (mode == kIvfPq) fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild_from an IVF_PQ index in IVF-PQ mode: only its codes are stored");
+    if (mode == kNone) return;
+    out.hold = std::shared_lock<std::shared_mutex>(flat->rw);  // the inner index takes its writes under its own lock only
+    flat->live_rows(lo, hi, out);
+  }
+  // from sources in inner-Flat mode: train's rule on their stored rows in ascending id order (IVF-PQ from `need` rows on,
+  // else inner Flat again), then one add of them in that order
+  int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
     DevBuf<uint32_t> rows;
     DevBuf<long long> ids;
-    const int64_t n = src.flat->sorted_rows(rows, ids, src.flat->stream);
+    const int64_t n = sorted_live_rows(this, srcs, lo, hi, dim, rows, ids, stream);
     if (n == 0) return 0;
     const float* x = reinterpret_cast<const float*>(rows.p);
     if (n < train_need()) {

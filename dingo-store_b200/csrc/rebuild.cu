@@ -1,5 +1,6 @@
-// rebuild.cu — the device pieces of b200vs_rebuild_from shared by every index type: the live rows of an index in ascending
-// id order, the training subsample drawn from device rows, and the +-1 expansion of binary rows.
+// rebuild.cu — the device pieces of b200vs_rebuild_from[_range] shared by every index type: the live rows of one or more
+// indexes in an id range in ascending id order, the training subsample drawn from device rows, and the +-1 expansion of
+// binary rows.
 #include <cub/cub.cuh>
 
 #include "index.h"
@@ -17,6 +18,60 @@ __global__ void gather_words_kernel(const uint32_t* __restrict__ src, const long
   const int j = (int)(i % words);
   const long long sr = rows ? rows[r] : r;
   dst[i] = src[(size_t)sr * words + j];
+}
+
+// a rebuild's sort value: the source in the top bits, the row slot in its store below
+constexpr int kSlotBits = 56;
+constexpr long long kSlotMask = (1LL << kSlotBits) - 1;
+static_assert(kRebuildMaxSources <= (1 << (63 - kSlotBits)), "the source must fit above the slot");
+
+struct SourceRows {
+  const uint32_t* p[kRebuildMaxSources];  // each source's row store
+};
+
+// out row r = row (vals[r] & kSlotMask) of source vals[r] >> kSlotBits, one warp per row in T-sized pieces (wt per row).
+// dup (nullable) is set when rows r - 1 and r share an id but come from different sources: the sort keeps equal ids of one
+// source together behind each other, so an id held by two sources always meets such a pair.
+template <class T>
+__global__ void gather_sources_kernel(const __grid_constant__ SourceRows src, const long long* __restrict__ vals,
+                                      const long long* __restrict__ ids, long long n, int wt, T* __restrict__ out, int* __restrict__ dup) {
+  const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const long long v = vals[r];
+  const T* row = reinterpret_cast<const T*>(src.p[v >> kSlotBits]) + (size_t)(v & kSlotMask) * wt;
+  T* o = out + (size_t)r * wt;
+  for (int j = lane; j < wt; j += 32) o[j] = row[j];
+  if (dup && lane == 0 && r > 0 && ids[r] == ids[r - 1] && (vals[r - 1] >> kSlotBits) != (v >> kSlotBits)) *dup = 1;
+}
+
+// the stable sort of n (id, source | slot) pairs by id and the gather of their rows; refuses an id held by two sources
+void sort_gather(IndexBase* ix, int64_t n, const long long* keys, const long long* vals, const SourceRows& src, int nsrc, int words,
+                 DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
+  DevBuf<long long> sorted_vals;
+  sorted_vals.reserve(n, 0, s); out_ids.reserve(n, 0, s);
+  size_t tmp_bytes = 0;
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, out_ids.p, vals, sorted_vals.p, (int)n, 0, 64, s));
+  DevBuf<unsigned char> tmp;
+  tmp.reserve(std::max<size_t>(tmp_bytes, 1), 0, s);
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys, out_ids.p, vals, sorted_vals.p, (int)n, 0, 64, s));
+  out_rows.reserve((size_t)n * words, 0, s);
+  DevBuf<int> dup;
+  if (nsrc > 1) {
+    dup.reserve(1, 0, s);
+    B200VS_CUDA(cudaMemsetAsync(dup.p, 0, 4, s));
+  }
+  const unsigned blocks = (unsigned)cdiv(n, 8);  // 8 warps of 256 threads, a row each
+  if (words % 4 == 0)  // 16-byte rows: every row of a cudaMalloc'ed store starts 16-byte aligned
+    gather_sources_kernel<uint4><<<blocks, 256, 0, s>>>(src, sorted_vals.p, out_ids.p, n, words / 4, reinterpret_cast<uint4*>(out_rows.p), dup.p);
+  else
+    gather_sources_kernel<uint32_t><<<blocks, 256, 0, s>>>(src, sorted_vals.p, out_ids.p, n, words, out_rows.p, dup.p);
+  B200VS_CUDA(cudaGetLastError());
+  int h_dup = 0;
+  if (dup.p) B200VS_CUDA(cudaMemcpyAsync(&h_dup, dup.p, 4, cudaMemcpyDeviceToHost, s));
+  B200VS_CUDA(cudaStreamSynchronize(s));  // the key and value lists and the sort's buffers die here
+  ix->launch_count(3);
+  if (h_dup) fail(B200VS_EVECTOR_ID_DUPLICATED, "rebuild_from_range: an id in the range is held by more than one source");
 }
 
 // bit b of a padded row is bit (b & 31) of word b >> 5 (byte b >> 3 is byte (b >> 3) & 3 of that little-endian word)
@@ -55,33 +110,52 @@ int64_t kmeans_sample_rows(IndexBase* ix, int64_t n, int k, int max_pts, int64_t
   return m;
 }
 
-void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids, const long long* slots, bool on_device, const uint32_t* src,
-                      int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
+int64_t sorted_live_rows(IndexBase* ix, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, int words, DevBuf<uint32_t>& out_rows,
+                         DevBuf<long long>& out_ids, cudaStream_t s) {
+  if (srcs.empty() || srcs.size() > (size_t)kRebuildMaxSources) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild takes 1 to 16 sources");
+  std::vector<RebuildSource> parts(srcs.size());  // holds inner indexes' reader locks until the gather is done
+  // in address order, as the callers take the outer locks: the inner locks some sources take here follow that one order too
+  std::vector<size_t> order(srcs.size());
+  for (size_t k = 0; k < srcs.size(); ++k) order[k] = k;
+  std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return std::less<IndexBase*>()(srcs[a], srcs[b]); });
+  int64_t n = 0;
+  for (size_t k : order) {
+    srcs[k]->live_rows(lo, hi, parts[k]);
+    n += (int64_t)parts[k].ids.size();
+  }
+  if (n == 0) return 0;
+  if (n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild holds at most 2^31 - 1 rows");
+  std::vector<long long> keys, vals;
+  keys.reserve(n); vals.reserve(n);
+  SourceRows table{};
+  for (size_t k = 0; k < parts.size(); ++k) {
+    const RebuildSource& p = parts[k];
+    for (size_t i = 0; i < p.ids.size(); ++i) {
+      if (p.slots[i] > kSlotMask) fail(B200VS_EINTERNAL, "rebuild: row slot out of range");
+      keys.push_back(p.ids[i]);
+      vals.push_back(((long long)k << kSlotBits) | p.slots[i]);
+    }
+    table.p[k] = p.rows;
+    if (!p.ids.empty()) B200VS_CUDA(cudaStreamSynchronize(p.stream));  // every write the source's own stream holds
+  }
+  DevBuf<long long> d_keys, d_vals;
+  d_keys.reserve(n, 0, s); d_vals.reserve(n, 0, s);
+  B200VS_CUDA(cudaMemcpyAsync(d_keys.p, keys.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  B200VS_CUDA(cudaMemcpyAsync(d_vals.p, vals.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  sort_gather(ix, n, d_keys.p, d_vals.p, table, (int)srcs.size(), words, out_rows, out_ids, s);
+  return n;
+}
+
+void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids_dev, const uint32_t* src, int words, DevBuf<uint32_t>& out_rows,
+                      DevBuf<long long>& out_ids, cudaStream_t s) {
   if (n == 0) return;
   if (n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild holds at most 2^31 - 1 rows");
-  DevBuf<long long> keys, vals, sorted_slots;
-  const long long* k_in = ids;
-  const long long* v_in = slots;
-  if (!on_device) {
-    keys.reserve(n, 0, s); vals.reserve(n, 0, s);
-    B200VS_CUDA(cudaMemcpyAsync(keys.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    B200VS_CUDA(cudaMemcpyAsync(vals.p, slots, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    k_in = keys.p; v_in = vals.p;
-  } else if (!slots) {  // the rows' own positions
-    vals.reserve(n, 0, s);
-    launch_iota(vals.p, n, s);
-    v_in = vals.p;
-  }
-  sorted_slots.reserve(n, 0, s); out_ids.reserve(n, 0, s);
-  size_t tmp_bytes = 0;
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in, out_ids.p, v_in, sorted_slots.p, (int)n, 0, 64, s));
-  DevBuf<unsigned char> tmp;
-  tmp.reserve(std::max<size_t>(tmp_bytes, 1), 0, s);
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, k_in, out_ids.p, v_in, sorted_slots.p, (int)n, 0, 64, s));
-  out_rows.reserve((size_t)n * words, 0, s);
-  launch_gather_words(src, sorted_slots.p, n, words, out_rows.p, s);
-  B200VS_CUDA(cudaStreamSynchronize(s));  // the host id and slot lists and the sort's buffers die here
-  ix->launch_count(3);
+  DevBuf<long long> vals;  // source 0, the rows' own positions
+  vals.reserve(n, 0, s);
+  launch_iota(vals.p, n, s);
+  SourceRows table{};
+  table.p[0] = src;
+  sort_gather(ix, n, ids_dev, vals.p, table, 1, words, out_rows, out_ids, s);
 }
 
 void check_rebuild_pair(const IndexBase& dst, const IndexBase& src) {

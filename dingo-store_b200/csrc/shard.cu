@@ -1642,7 +1642,7 @@ int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
   int64_t n = 0;
   check(agree(dst, attempt([&] {
     B200VS_CUDA(cudaStreamSynchronize(s->stream));
-    n = s->sorted_rows(rows, ids, ws);
+    n = sorted_live_rows(s, {s}, 0, INT64_MAX, words, rows, ids, ws);
   }), "shard rebuild_from"));
   // 2) to the training owner (the routing's send and receive copies are reserved in agreed steps)
   Routed rv;
@@ -1654,7 +1654,7 @@ int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
   check(agree(dst, attempt([&] {
     B200VS_CUDA(cudaStreamSynchronize(ws));
     rows.free(); ids.free();
-    sorted_live_rows(d, m, rv.ids.p, nullptr, true, reinterpret_cast<const uint32_t*>(rv.x.p), words, tx, tids, ws);
+    sorted_live_rows(d, m, rv.ids.p, reinterpret_cast<const uint32_t*>(rv.x.p), words, tx, tids, ws);
   }), "shard rebuild_from"));
   rv.x.free(); rv.ids.free();
   int64_t total = 0;
@@ -1763,7 +1763,7 @@ int b200vs_shard_rebuild_from(b200vs_shard* dst_h, b200vs_shard* src_h, int64_t*
     if (dst->rows) {  // HNSW: every row already sits on its owner
       check(agree(dst, attempt([&] {
         WriteHold hold(dst->ix);
-        n = dst->ix->rebuild_from(*src->ix);
+        n = dst->ix->rebuild_from({src->ix}, 0, INT64_MAX);
       }), "shard rebuild_from"));
     } else {
       n = shard_rebuild_lists(dst, src);

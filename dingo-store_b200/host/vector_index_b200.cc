@@ -440,6 +440,16 @@ butil::Status VectorIndexB200::RebuildFrom(VectorIndexB200& old) {
   if (!index_ || !old.index_) return butil::Status(pb::error::EINTERNAL, "index not created");
   return ToStatus(b200vs_rebuild_from(index_, old.index_, nullptr));
 }
+butil::Status VectorIndexB200::RebuildFrom(const std::vector<VectorIndexB200*>& olds, int64_t min_vector_id, int64_t max_vector_id) {
+  if (!index_) return butil::Status(pb::error::EINTERNAL, "index not created");
+  std::vector<b200vs_index*> srcs;
+  for (VectorIndexB200* old : olds) {
+    if (old && !old->index_) return butil::Status(pb::error::EINTERNAL, "index not created");
+    srcs.push_back(old ? old->index_ : nullptr);  // a null entry is refused by the library
+  }
+  const int32_t n_src = srcs.size() > (size_t)INT32_MAX ? -1 : (int32_t)srcs.size();
+  return ToStatus(b200vs_rebuild_from_range(index_, n_src, srcs.data(), min_vector_id, max_vector_id, nullptr));
+}
 bool VectorIndexB200::NeedToSave(int64_t last_save_log_behind) {
   if (!SupportSave() || !index_) return false;
   int64_t count = 0, deleted = 0;

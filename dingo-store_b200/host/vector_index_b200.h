@@ -17,6 +17,7 @@
 #include <atomic>
 #include <shared_mutex>
 #include <string>
+#include <vector>
 
 #include "../../include/b200vs.h"
 
@@ -64,6 +65,10 @@ class VectorIndexB200 : public VectorIndex {
   // Fills this fresh index from old's live rows on the GPU (b200vs_rebuild_from), in place of RebuildVectorIndex's RocksDB
   // scan, Train and Add: the result equals a train + add of old's rows in ascending id order.  old keeps serving reads.
   butil::Status RebuildFrom(VectorIndexB200& old);
+  // Fills this fresh index from the rows with min_vector_id <= id < max_vector_id of olds (b200vs_rebuild_from_range): the
+  // rebuilds of a region split (olds = {share index} for the child, {own index} for the parent) or merge ({own, sibling}).
+  // The caller passes the region's range as VectorCodec::DecodeRangeToVectorId gives it.  The olds keep serving reads.
+  butil::Status RebuildFrom(const std::vector<VectorIndexB200*>& olds, int64_t min_vector_id, int64_t max_vector_id);
   bool NeedTrain() override;
   bool IsTrained() override;
   // the stock plugins' rules (flat.cc:515-531, ivf_flat.cc:786-802, raw_ivf_pq.cc:533-549, ivf_pq.cc:450-462, hnsw.cc:592-609):

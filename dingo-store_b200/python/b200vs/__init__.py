@@ -36,7 +36,7 @@ ABI_SYMBOLS = [
     "b200vs_hnsw_add_batched", "b200vs_debug_hnsw_build_scratch_limit", "b200vs_calc_distance_binary",
     "b200vs_scan_range_begin", "b200vs_scan_range_push", "b200vs_scan_range_finish", "b200vs_scan_range_abort",
     "b200vs_shard_hnsw_add_batched", "b200vs_row_owner", "b200vs_shard_save", "b200vs_shard_load",
-    "b200vs_need_rebuild", "b200vs_rebuild_from",
+    "b200vs_need_rebuild", "b200vs_rebuild_from", "b200vs_rebuild_from_range",
     "b200vs_shard_create_binary", "b200vs_shard_train_binary", "b200vs_shard_add_binary", "b200vs_shard_add_binary_device",
     "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
     "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
@@ -162,6 +162,7 @@ def lib():
     L.b200vs_shard_load.argtypes = [vp, ctypes.c_char_p]
     L.b200vs_need_rebuild.argtypes = [vp]
     L.b200vs_rebuild_from.argtypes = [vp, vp, ctypes.POINTER(i64)]
+    L.b200vs_rebuild_from_range.argtypes = [vp, i32, ctypes.POINTER(vp), i64, i64, ctypes.POINTER(i64)]
     L.b200vs_shard_create_binary.argtypes = [vp, i32, i32, vp, i32, ctypes.POINTER(vp)]
     L.b200vs_shard_train_binary.argtypes = [vp, i64, vp]
     L.b200vs_shard_add_binary.argtypes = [vp, i64, vp, vp]
@@ -462,6 +463,14 @@ class Index:
         """Fill this fresh index from src's live rows in ascending id order, on the device; returns the rows copied."""
         n = ctypes.c_int64(0)
         _check(self.L.b200vs_rebuild_from(self.h, src.h, ctypes.byref(n)))
+        return n.value
+
+    def rebuild_from_range(self, srcs, id_min, id_max):
+        """Fill this fresh index from the live rows with id_min <= id < id_max of the indexes srcs (a region split or merge),
+        in ascending id order, on the device; returns the rows copied.  A None entry passes a null handle."""
+        arr = (ctypes.c_void_p * len(srcs))(*[None if s is None else s.h for s in srcs])
+        n = ctypes.c_int64(0)
+        _check(self.L.b200vs_rebuild_from_range(self.h, len(srcs), arr, id_min, id_max, ctypes.byref(n)))
         return n.value
 
     def save(self, path):

@@ -255,8 +255,40 @@ int b200vs_need_rebuild(b200vs_index* idx);
  * Peak device memory: src's rows, a dense copy of its live rows (n x row bytes) with 32 B per row of sort buffers, and dst's
  * rows, all at once: about three times the live row bytes for IVF_FLAT (plus each IVF-Flat store's FP16 mirror).  A region
  * that does not fit that on its device (e.g. 6.25 M x 1536 FP32 = 38 GB of rows on an 80 GB GPU) keeps the host rebuild;
- * the call then fails with EINTERNAL and leaves src unchanged. */
+ * the call then fails with EINTERNAL and leaves src unchanged.  This is b200vs_rebuild_from_range's code with one source and
+ * every id (a row whose id is INT64_MAX included). */
 int b200vs_rebuild_from(b200vs_index* dst, b200vs_index* src, int64_t* n_rows);
+
+/* Fill dst, a fresh index, from the live rows with id_min <= id < id_max of the indexes srcs[0 .. n_src), on the device: the
+ * rebuilds of a region split or merge (raft_apply_handler.cc:626-660, :1018-1035), whose rows are already held by the old
+ * indexes (a split child: the share index; a split parent: its own index; a merge target: its own index and the sibling).
+ * R = the union over every source of its live rows with id_min <= id < id_max (RangeFilterFunctor's and
+ * DecodeRangeToVectorId's convention: id_max is exclusive).  dst ends up equal, byte for byte (trained state, every list's
+ * ids and rows, the FP16 mirror, PQ codes, the HNSW graph), to a fresh index trained by its type's rule and then filled with
+ * one add of R in ascending id order (rows sharing an id inside one IVF source keep that source's list-major export order),
+ * the rows taken as stored: cosine rows are not normalised again.
+ *   IVF_FLAT, BINARY_IVF_FLAT : b200vs_train[_binary]'s rule on R (nlist degenerates to 1 below nlist rows), then one add
+ *   IVF_PQ in inner-Flat mode : b200vs_train's rule (IVF-PQ from max(256 * nlist, 256 * 2^nbits) rows, else inner Flat), then
+ *                               one add; a source in IVF-PQ mode keeps only codes: EVECTOR_NOT_SUPPORT
+ *   HNSW                      : b200vs_hnsw_add_batched with the default batch; levels from dst's fresh generator, no tombstones
+ *   FLAT, BINARY_FLAT         : one add (b200vs_rebuild_from keeps refusing them)
+ * With one source and [0, INT64_MAX) the result equals b200vs_rebuild_from's on every type that call serves; only a row whose
+ * id is INT64_MAX differs, and dingo never issues that id (IsLegalVectorId).
+ * EILLEGAL_PARAMETERS: n_src outside [1, 16], a null srcs or null entry, id_min > id_max, dst among the sources, a source
+ * listed twice, a source that differs from dst in type, metric, dimension, nlist, nsubvector, nbits, nlinks, efconstruction
+ * or device, a dst that is not empty or (IVF types) already trained, or an HNSW dst whose max_elements is below |R|.
+ * EVECTOR_ID_DUPLICATED: an id in R held by more than one source (the sources of a split or merge hold disjoint ranges).
+ * Every refusal leaves every source and dst unchanged.  An empty R (id_min == id_max included): OK, *n_rows = 0, dst stays
+ * untrained.  A device failure: EINTERNAL; the sources are unchanged, dst may be discarded.  The sources are held under their
+ * reader locks (their searches go on, their writers wait) and dst under its writer lock, all taken in one order (by handle
+ * address), so two calls over overlapping sources, such as a split's child and parent rebuilding from the same index at
+ * once, cannot deadlock.  An IVF_PQ source in inner-Flat mode takes its writes under its inner index's lock only: that lock
+ * is held shared (in the same address order) while the source's rows are listed and gathered, so its writers wait for that
+ * part of the call, not for all of it.  *n_rows (nullable) = |R|.  Peak device memory: the sources' rows, a dense copy of R (|R| x row
+ * bytes) with 32 B per row of sort buffers, and dst's rows, all at once: about three times R's row bytes for IVF_FLAT (plus
+ * each IVF-Flat store's FP16 mirror) when the sources hold little beyond R. */
+int b200vs_rebuild_from_range(b200vs_index* dst, int32_t n_src, b200vs_index* const* srcs, int64_t id_min, int64_t id_max,
+                              int64_t* n_rows);
 
 /* Export the inverted lists in list-major order (list l owns rows [list_off[l], list_off[l+1])) so a CPU
  * implementation can search the identical index.  Any output pointer may be NULL.  Flat: nlist = 1. */

@@ -1,0 +1,20 @@
+"""Runs the C++ test of the plugin's split and merge rebuilds (dingo-store_b200/host/test_plugin_rebuild_range.cc):
+RebuildFrom(olds, min_vector_id, max_vector_id)."""
+import os
+import subprocess
+
+import pytest
+
+import b200vs
+from gpu_util import require_gpu
+
+pytestmark = pytest.mark.gpu
+
+
+def test_cpp_plugin_rebuild_range():
+    require_gpu()
+    exe = os.path.join(b200vs.PKG_ROOT, "host", "test_plugin_rebuild_range")
+    assert os.path.exists(exe), "build it with: make -C dingo-store_b200/host"
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
+    print(r.stdout[-3000:])
+    assert r.returncode == 0 and "PLUGIN REBUILD RANGE TESTS OK" in r.stdout, r.stdout[-3000:] + r.stderr[-1000:]
