@@ -15,15 +15,11 @@
 
 using namespace b200vs;
 
-namespace {
-
-IndexBase* get(b200vs_index* h) { return index_impl(h); }
-
 // b200vs_rebuild_from[_range]: fill dst from the live rows with lo <= id <= hi of srcs (distinct, dst not among them).  The
 // sources are held under their reader locks and dst under its writer hold, taken in one order, by address, so two calls over
 // overlapping sources (a split's child and parent rebuilding from the parent's index at once) cannot deadlock.  flat_ok:
 // FLAT and BINARY_FLAT are served.
-int64_t rebuild_range(IndexBase* dst, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, bool flat_ok) {
+int64_t b200vs::rebuild_range(IndexBase* dst, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, bool flat_ok) {
   std::vector<IndexBase*> order(srcs);
   order.push_back(dst);
   std::sort(order.begin(), order.end(), std::less<IndexBase*>());
@@ -38,6 +34,10 @@ int64_t rebuild_range(IndexBase* dst, const std::vector<IndexBase*>& srcs, int64
     fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");  // vector_index_flat.h:111
   return dst->rebuild_from(srcs, lo, hi);
 }
+
+namespace {
+
+IndexBase* get(b200vs_index* h) { return index_impl(h); }
 
 // the float entry points (train / add / search / range search) on a binary index, and the binary ones on a float index
 void check_row_type(IndexBase* ix, bool binary_call) {

@@ -1392,6 +1392,10 @@ struct HnswIndex : IndexBase {
   // the sources' live nodes with lo <= label <= hi, their stored rows (cosine: already normalised) in ascending label order,
   // gathered on the host (the rows live in the host graph), through the batched builder with the default batch; this fresh
   // index's level generator draws the levels, so the graph has no tombstones
+  void live_ids(int64_t lo, int64_t hi, std::vector<int64_t>& out) override {
+    for (int64_t i = 0; i < G.n; ++i)
+      if (!G.deleted[i] && G.labels[i] >= lo && G.labels[i] <= hi) out.push_back(G.labels[i]);
+  }
   int64_t rebuild_from(const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi) override {
     struct Live { int64_t label; const float* row; };
     std::vector<Live> live;

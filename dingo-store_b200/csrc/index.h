@@ -342,6 +342,13 @@ struct IndexBase {
     (void)lo; (void)hi; (void)out;
     fail(B200VS_EVECTOR_NOT_SUPPORT, "this index type has no row store to rebuild from");
   }
+  // the ids of this index's live rows with lo <= id <= hi, appended to out in storage order (the refusals a sharded rebuild
+  // agrees on before any rank's dst changes).  Callers hold rw.
+  virtual void live_ids(int64_t lo, int64_t hi, std::vector<int64_t>& out) {
+    RebuildSource p;
+    live_rows(lo, hi, p);
+    out.insert(out.end(), p.ids.begin(), p.ids.end());
+  }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }
   virtual int64_t get_state(void* blob, size_t cap) { (void)blob; (void)cap; return 0; }
   // THE write of rows into an index, under the writer hold.  Each type refuses the requests it cannot serve.

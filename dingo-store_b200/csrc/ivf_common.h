@@ -581,9 +581,20 @@ void kmeans_gpu_dev(IndexBase* ix, int d, int64_t n, const float* x_dev, int k, 
 // and returns the row count with s synchronised.
 int64_t sorted_live_rows(IndexBase* ix, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, int words, DevBuf<uint32_t>& out_rows,
                          DevBuf<long long>& out_ids, cudaStream_t s);
-// the same sort and gather of the n rows of one device row block src whose ids ids_dev are on the device
-void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids_dev, const uint32_t* src, int words, DevBuf<uint32_t>& out_rows,
-                      DevBuf<long long>& out_ids, cudaStream_t s);
+// One block of device rows for the sort below: n rows of `words` words at rows, their ids at ids, both on the device.
+struct DeviceRows {
+  int64_t n;
+  const long long* ids;
+  const uint32_t* rows;
+};
+// the same sort and gather of every row of up to kRebuildMaxSources device row blocks, concatenated in block order (one
+// block: no duplicate check); an id held by two blocks is refused with EVECTOR_ID_DUPLICATED
+void sorted_live_rows(IndexBase* ix, const std::vector<DeviceRows>& blocks, int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids,
+                      cudaStream_t s);
+// b200vs_rebuild_from[_range] and the row-sharded shard rebuilds: fill dst from the live rows with lo <= id <= hi of srcs
+// (distinct, dst not among them) under the sources' reader locks and dst's writer hold, taken in address order.  flat_ok:
+// FLAT and BINARY_FLAT are served.
+int64_t rebuild_range(IndexBase* dst, const std::vector<IndexBase*>& srcs, int64_t lo, int64_t hi, bool flat_ok);
 // out [m, dim] = the +-1 floats (binary_to_real: bit set -> 1, else -1) of padded binary rows words [.., w] (rows ? rows[i] : i)
 void launch_expand_pm1(const uint32_t* words, const long long* rows, int64_t m, int w, int dim, float* out, cudaStream_t s);
 // the refusals b200vs_rebuild_from[_range] shares for every type and source: dst must be empty, untrained, another index of

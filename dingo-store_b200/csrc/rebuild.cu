@@ -74,6 +74,12 @@ void sort_gather(IndexBase* ix, int64_t n, const long long* keys, const long lon
   if (h_dup) fail(B200VS_EVECTOR_ID_DUPLICATED, "rebuild_from_range: an id in the range is held by more than one source");
 }
 
+// out[i] = tag | i: the sort values of one block of device rows (the block in the tag's top bits, as in sort_gather)
+__global__ void source_slots_kernel(long long* __restrict__ out, long long n, long long tag) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = tag | i;
+}
+
 // bit b of a padded row is bit (b & 31) of word b >> 5 (byte b >> 3 is byte (b >> 3) & 3 of that little-endian word)
 __global__ void expand_pm1_kernel(const uint32_t* __restrict__ words, const long long* __restrict__ rows, long long m, int w, int dim,
                                   float* __restrict__ out) {
@@ -146,16 +152,29 @@ int64_t sorted_live_rows(IndexBase* ix, const std::vector<IndexBase*>& srcs, int
   return n;
 }
 
-void sorted_live_rows(IndexBase* ix, int64_t n, const long long* ids_dev, const uint32_t* src, int words, DevBuf<uint32_t>& out_rows,
-                      DevBuf<long long>& out_ids, cudaStream_t s) {
+void sorted_live_rows(IndexBase* ix, const std::vector<DeviceRows>& blocks, int words, DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids,
+                      cudaStream_t s) {
+  if (blocks.empty() || blocks.size() > (size_t)kRebuildMaxSources) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild takes 1 to 16 sources");
+  int64_t n = 0;
+  for (const DeviceRows& b : blocks) n += b.n;
   if (n == 0) return;
   if (n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild holds at most 2^31 - 1 rows");
-  DevBuf<long long> vals;  // source 0, the rows' own positions
+  // keys: the blocks' ids back to back (one block: its own ids); values: (block, the row's position in its block)
+  DevBuf<long long> keys, vals;
   vals.reserve(n, 0, s);
-  launch_iota(vals.p, n, s);
+  if (blocks.size() > 1) keys.reserve(n, 0, s);
   SourceRows table{};
-  table.p[0] = src;
-  sort_gather(ix, n, ids_dev, vals.p, table, 1, words, out_rows, out_ids, s);
+  int64_t at = 0;
+  for (size_t k = 0; k < blocks.size(); ++k) {
+    const DeviceRows& b = blocks[k];
+    table.p[k] = b.rows;
+    if (!b.n) continue;
+    if (keys.p) B200VS_CUDA(cudaMemcpyAsync(keys.p + at, b.ids, (size_t)b.n * 8, cudaMemcpyDeviceToDevice, s));
+    source_slots_kernel<<<(unsigned)cdiv(b.n, 256), 256, 0, s>>>(vals.p + at, b.n, (long long)k << kSlotBits);
+    B200VS_CUDA(cudaGetLastError());
+    at += b.n;
+  }
+  sort_gather(ix, n, keys.p ? keys.p : blocks[0].ids, vals.p, table, (int)blocks.size(), words, out_rows, out_ids, s);
 }
 
 void check_rebuild_pair(const IndexBase& dst, const IndexBase& src) {

@@ -398,6 +398,36 @@ owner_check_kernel(const long long* __restrict__ keys, long long n, int W, Owner
   if ((threadIdx.x & 31) == 0 && msk) atomicAdd(bad, (unsigned long long)__popc(msk));
 }
 
+// The write gate of a set (b200vs_shard::add_mu): its writes (add, delete, train, state broadcast, save, load, the rule, a
+// rebuild INTO it) hold it exclusively, one at a time; a rebuild that reads the set holds it shared.  A shared hold is granted
+// whenever no exclusive one is held, even while a writer waits: two rebuilds that read one set (a split's child and parent)
+// never wait for each other's locks, whatever order they start in on each rank.  Their collectives are not ordered by the
+// gate (include/b200vs.h states the caller's rule on NCCL).
+struct Gate {
+  std::mutex mu;
+  std::condition_variable cv;
+  int readers = 0;
+  bool writer = false;
+  void lock() {
+    std::unique_lock<std::mutex> lk(mu);
+    cv.wait(lk, [&] { return !writer && readers == 0; });
+    writer = true;
+  }
+  void unlock() {
+    { std::lock_guard<std::mutex> lk(mu); writer = false; }
+    cv.notify_all();
+  }
+  void lock_shared() {
+    std::unique_lock<std::mutex> lk(mu);
+    cv.wait(lk, [&] { return !writer; });
+    ++readers;
+  }
+  void unlock_shared() {
+    { std::lock_guard<std::mutex> lk(mu); --readers; }
+    cv.notify_all();
+  }
+};
+
 }  // namespace b200vs
 
 using namespace b200vs;
@@ -426,8 +456,8 @@ struct b200vs_shard {
   std::condition_variable seq_cv;
   int64_t next_auto = 0;             // sequence numbers handed out when the caller passes seq < 0
   int64_t next_seq = 0;              // the batch whose turn it is to be enqueued
-  // write path (collective, one at a time)
-  std::mutex add_mu;
+  // write path (collective, one at a time; rebuilds that read this set hold the gate shared)
+  Gate add_mu;
   cudaStream_t ws = nullptr;
   DevBuf<unsigned long long> plan_counts;  // [nlist] rows per list seen by b200vs_shard_plan_add*
   bool planning = false;
@@ -909,7 +939,7 @@ int shard_train(b200vs_shard* h, int64_t n, const void* x, bool binary_call) {
     b200vs_shard* sh = get(h);
     check_row_type(sh, binary_call);
     if (sh->rows) return B200VS_OK;  // FLAT, BINARY_FLAT and HNSW have nothing to train (b200vs_train is a no-op on them too)
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     shard_train_locked(sh, n, x, false);
     return B200VS_OK;
   });
@@ -966,7 +996,7 @@ int b200vs_shard_broadcast_state(b200vs_shard* h, int32_t root) {
     // an HNSW state blob is a whole graph: replicating it would put every row on every rank
     if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no replicated trained state");
     if (root < 0 || root >= sh->world) fail(B200VS_EILLEGAL_PARAMETERS, "bad root");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     broadcast_state_locked(sh, root);
     sh->train_rows_set = live_rows_set(sh);
     return B200VS_OK;
@@ -1567,7 +1597,7 @@ int shard_add(b200vs_shard* h, int64_t n, const void* x, const int64_t* ids, boo
     b200vs_shard* sh = get(h);
     check_row_type(sh, binary_call);
     if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     if (on_device) {
       shard_add_impl(sh, n, x, (const long long*)ids, false, 0);
       return B200VS_OK;
@@ -1612,51 +1642,108 @@ bool shard_need_rebuild_locked(b200vs_shard* sh) {
   }
 }
 
-// The refusals of b200vs_shard_rebuild_from on this rank, decided before any index changes (src is held shared by the caller)
-void check_shard_rebuild(b200vs_shard* dst, b200vs_shard* src) {
-  if (dst->world != src->world || dst->rank != src->rank) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src differ in world or rank");
-  IndexBase *d = dst->ix, *s = src->ix;
-  std::shared_lock<std::shared_mutex> rl(d->rw);
-  check_rebuild_pair(*d, *s);
-  if (d->type == B200VS_FLAT || d->type == B200VS_BINARY_FLAT) fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");
+// The gates of a rebuild, taken in one order (by handle address) and released at scope exit: dst's exclusively, the source
+// sets' shared.  Two rebuilds over overlapping sources (a split's child and parent, a merge beside a split of one of its
+// sources) then never wait for each other on this rank; only the sources' writers wait for them.
+struct RebuildGates {
+  std::vector<std::pair<Gate*, bool>> held;  // (gate, exclusive), in the order taken
+  RebuildGates(b200vs_shard* dst, const std::vector<b200vs_shard*>& srcs) {
+    std::vector<b200vs_shard*> order(srcs);
+    order.push_back(dst);
+    std::sort(order.begin(), order.end(), std::less<b200vs_shard*>());
+    for (b200vs_shard* sh : order) {
+      const bool excl = sh == dst;
+      if (excl) sh->add_mu.lock();
+      else sh->add_mu.lock_shared();
+      held.emplace_back(&sh->add_mu, excl);
+    }
+  }
+  ~RebuildGates() {
+    for (auto it = held.rbegin(); it != held.rend(); ++it) {
+      if (it->second) it->first->unlock();
+      else it->first->unlock_shared();
+    }
+  }
+  RebuildGates(const RebuildGates&) = delete;
+  RebuildGates& operator=(const RebuildGates&) = delete;
+};
+
+// The refusals of a set rebuild on this rank, decided before any index changes.  flat_ok: FLAT and BINARY_FLAT are served
+// (b200vs_shard_rebuild_from_range).  Row-sharded sets: this rank's share of R is listed here, from the host bookkeeping,
+// so that an HNSW dst too small for it and an id held by two sources are refused on every rank before any rank's dst changes
+// (the per-rank rebuild that follows would find them only on the rank that holds them).
+void check_shard_rebuild(b200vs_shard* dst, const std::vector<b200vs_shard*>& srcs, int64_t lo, int64_t hi, bool bad_range, bool flat_ok) {
+  if (bad_range) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from_range: id_min > id_max");
+  for (b200vs_shard* src : srcs)
+    if (dst->world != src->world || dst->rank != src->rank) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src differ in world or rank");
+  IndexBase* d = dst->ix;
+  {
+    std::shared_lock<std::shared_mutex> rl(d->rw);
+    for (b200vs_shard* src : srcs) check_rebuild_pair(*d, *src->ix);
+  }
+  if (!flat_ok && (d->type == B200VS_FLAT || d->type == B200VS_BINARY_FLAT)) fail(B200VS_EVECTOR_NOT_SUPPORT, "a Flat index never needs a rebuild");
   if (d->type == B200VS_IVF_PQ)
     fail(B200VS_EVECTOR_NOT_SUPPORT, "rebuild_from an IVF_PQ set: it stores only codes (rebuild it from host rows with shard_train + shard_add)");
-  if (d->type == B200VS_HNSW && d->params.max_elements > 0 && s->count() > d->params.max_elements)
-    fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below src's live rows");
+  if (!dst->rows) return;
+  std::vector<std::pair<int64_t, size_t>> r;  // (id, source) of this rank's share of R
+  for (size_t k = 0; k < srcs.size(); ++k) {
+    std::vector<int64_t> ids;
+    {
+      std::shared_lock<std::shared_mutex> rl(srcs[k]->ix->rw);
+      srcs[k]->ix->live_ids(lo, hi, ids);
+    }
+    for (const int64_t id : ids) r.emplace_back(id, k);
+  }
+  if (d->type == B200VS_HNSW && d->params.max_elements > 0 && (int64_t)r.size() > d->params.max_elements)
+    fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst max_elements is below this rank's share of the rows");
+  if (srcs.size() < 2) return;
+  std::sort(r.begin(), r.end());
+  for (size_t i = 1; i < r.size(); ++i)
+    if (r[i].first == r[i - 1].first && r[i].second != r[i - 1].second)
+      fail(B200VS_EVECTOR_ID_DUPLICATED, "rebuild_from_range: id " + std::to_string(r[i].first) + " is held by more than one source");
 }
 
-// List-sharded rebuild (IVF_FLAT, BINARY_IVF_FLAT), every step on dst's write stream and communicator: src's live rows in
-// ascending id order (sorted_live_rows), routed to row_owner(id) (route_rows with RowOwner), sorted again by id after the
-// arrival (rank 0's rows first, each rank's in its own order, so ties keep (src rank, list-major position)), then
-// shard_train's flow and shard_add's flow on those device rows.  Every local step before a collective (the sorts, the
-// routing's and the add's copies, the k-means, the state install, the add) is agreed, so a device failure on one rank, an
-// allocation that does not fit included, is returned by every rank.  Returns the live rows this rank's dst holds.
-int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
-  IndexBase *d = dst->ix, *s = src->ix;
+// List-sharded rebuild (IVF_FLAT, BINARY_IVF_FLAT), every step on dst's write stream and communicator.  Each source set in
+// turn: its live rows with lo <= id <= hi in ascending id order (sorted_live_rows), routed to row_owner(id) (route_rows with
+// RowOwner), so every row arrives in a block of its own source set.  Then one stable sort of what arrived, by id, over those
+// blocks (a source set's block holds rank 0's rows first, each rank's in its own order, so ties keep (src rank, list-major
+// position)); the sort's value carries the block, so an id that arrived from two source sets is refused there, after the
+// routing has brought every copy of it to one rank.  Then shard_train's flow and shard_add's flow on those device rows.
+// Every local step before a collective (the sorts, the routing's and the add's copies, the k-means, the state install, the
+// add) is agreed, so a device failure on one rank, an allocation that does not fit included, is returned by every rank.
+// Returns the live rows this rank's dst holds.
+int64_t shard_rebuild_lists(b200vs_shard* dst, const std::vector<b200vs_shard*>& srcs, int64_t lo, int64_t hi, const char* what) {
+  IndexBase* d = dst->ix;
   const int words = d->binary() ? (d->dim / 8 + 3) / 4 : d->dim;
   const cudaStream_t ws = dst->ws;
   d->set_device();
-  // 1) src's live rows sorted by id, behind every write src's own stream holds
-  DevBuf<uint32_t> rows;
-  DevBuf<long long> ids;
-  int64_t n = 0;
-  check(agree(dst, attempt([&] {
-    B200VS_CUDA(cudaStreamSynchronize(s->stream));
-    n = sorted_live_rows(s, {s}, 0, INT64_MAX, words, rows, ids, ws);
-  }), "shard rebuild_from"));
-  // 2) to the training owner (the routing's send and receive copies are reserved in agreed steps)
-  Routed rv;
-  route_rows(dst, n, rows.p, words * 4, ids.p, nullptr, RowOwner{}, rv, true);
-  // 3) stable sort of what arrived by id: rows_r
+  // 1, 2) each source set's rows in the range sorted by id, behind every write its own stream holds, then to the training
+  // owner (the routing's send and receive copies are reserved in agreed steps); the sorted copy dies once routed
+  std::vector<Routed> rv(srcs.size());
+  for (size_t k = 0; k < srcs.size(); ++k) {
+    IndexBase* s = srcs[k]->ix;
+    DevBuf<uint32_t> rows;
+    DevBuf<long long> ids;
+    int64_t n = 0;
+    check(agree(dst, attempt([&] {
+      std::shared_lock<std::shared_mutex> rl(s->rw);
+      B200VS_CUDA(cudaStreamSynchronize(s->stream));
+      n = sorted_live_rows(d, {s}, lo, hi, words, rows, ids, ws);
+    }), what));
+    route_rows(dst, n, rows.p, words * 4, ids.p, nullptr, RowOwner{}, rv[k], true);
+    local_step(dst, true, what, [&] { B200VS_CUDA(cudaStreamSynchronize(ws)); });  // the sent copy is read before rows die
+  }
+  // 3) stable sort of what arrived by id over the source blocks: rows_r; an id from two source sets is refused
   DevBuf<uint32_t> tx;
   DevBuf<long long> tids;
-  const int64_t m = rv.n;
-  check(agree(dst, attempt([&] {
-    B200VS_CUDA(cudaStreamSynchronize(ws));
-    rows.free(); ids.free();
-    sorted_live_rows(d, m, rv.ids.p, reinterpret_cast<const uint32_t*>(rv.x.p), words, tx, tids, ws);
-  }), "shard rebuild_from"));
-  rv.x.free(); rv.ids.free();
+  int64_t m = 0;
+  std::vector<DeviceRows> blocks;
+  for (const Routed& b : rv) {
+    blocks.push_back({b.n, b.ids.p, reinterpret_cast<const uint32_t*>(b.x.p)});
+    m += b.n;
+  }
+  check(agree(dst, attempt([&] { sorted_live_rows(d, blocks, words, tx, tids, ws); }), what));
+  rv.clear();
   int64_t total = 0;
   for (const long long c : all_gather_host(dst, &m)) total += c;
   if (total == 0) return 0;  // nothing live anywhere: dst stays untrained
@@ -1666,7 +1753,7 @@ int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
   const void* xa = tx.p;
   DevBuf<unsigned char> packed;
   const size_t nb = d->query_row_bytes();
-  local_step(dst, true, "shard rebuild_from", [&] {
+  local_step(dst, true, what, [&] {
     if (!d->binary() || nb == (size_t)words * 4 || !m) return;
     packed.reserve((size_t)m * nb, 0, ws);
     B200VS_CUDA(cudaMemcpy2DAsync(packed.p, nb, tx.p, (size_t)words * 4, nb, (size_t)m, cudaMemcpyDeviceToDevice, ws));
@@ -1677,6 +1764,23 @@ int64_t shard_rebuild_lists(b200vs_shard* dst, b200vs_shard* src) {
   shard_add_impl(dst, m, xa, tids.p, false, 0, true);
   std::shared_lock<std::shared_mutex> rl(d->rw);
   return d->count();
+}
+
+// The body of b200vs_shard_rebuild_from[_range] once the arguments are checked: fill dst from the live rows with
+// lo <= id <= hi of the source sets srcs.  The gates come first, then the agreed refusals; row-sharded sets run the
+// single-index rebuild of each rank's sources into its dst index, then one more agreement.  Returns the live rows this
+// rank's dst holds.
+int64_t shard_rebuild(b200vs_shard* dst, const std::vector<b200vs_shard*>& srcs, int64_t lo, int64_t hi, bool bad_range, bool flat_ok,
+                      const char* what) {
+  RebuildGates gates(dst, srcs);
+  dst->ix->set_device();
+  check(agree(dst, attempt([&] { check_shard_rebuild(dst, srcs, lo, hi, bad_range, flat_ok); }), what));
+  if (!dst->rows) return shard_rebuild_lists(dst, srcs, lo, hi, what);
+  std::vector<IndexBase*> ixs;
+  for (b200vs_shard* src : srcs) ixs.push_back(src->ix);
+  int64_t n = 0;
+  check(agree(dst, attempt([&] { n = rebuild_range(dst->ix, ixs, lo, hi, true); }), what));
+  return n;
 }
 
 }  // namespace
@@ -1701,7 +1805,7 @@ int b200vs_shard_hnsw_add_batched(b200vs_shard* h, int64_t n, const float* x, co
     b200vs_shard* sh = get(h);
     if (sh->ix->type != B200VS_HNSW) fail(B200VS_EILLEGAL_PARAMETERS, "batched HNSW construction needs an HNSW index");
     if (n < 0 || (n > 0 && (!x || !ids))) fail(B200VS_EILLEGAL_PARAMETERS, "bad add arguments");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     sh->ix->set_device();
     DevBuf<unsigned char> dx;
     DevBuf<long long> di;
@@ -1716,7 +1820,7 @@ int b200vs_shard_save(b200vs_shard* h, const char* prefix) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
     if (!prefix || !*prefix) fail(B200VS_EILLEGAL_PARAMETERS, "null snapshot prefix");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     shard_save_locked(sh, prefix);
     return B200VS_OK;
   });
@@ -1727,7 +1831,7 @@ int b200vs_shard_load(b200vs_shard* h, const char* prefix) {
   return guarded([&]() -> int {
     b200vs_shard* sh = get(h);
     if (!prefix || !*prefix) fail(B200VS_EILLEGAL_PARAMETERS, "null snapshot prefix");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     shard_load_locked(sh, prefix);
     if (!sh->rows) sh->train_rows_set = live_rows_set(sh);
     return B200VS_OK;
@@ -1739,35 +1843,47 @@ int b200vs_shard_need_rebuild(b200vs_shard* h) {
   int r = 0;
   const int rc = guarded([&]() -> int {
     b200vs_shard* sh = get(h);
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     r = shard_need_rebuild_locked(sh) ? 1 : 0;
     return B200VS_OK;
   });
   return rc == B200VS_OK ? r : -rc;
 }
 
-// Collective rebuild of the fresh set dst from the set src (every rank passes its own dst and src).  src's writers wait on
-// its add_mu and its rank index stays under its reader lock, so src's reads go on; none of src's communicators is used.
-// The refusals are agreed before any index changes.  HNSW: each rank's single-index rebuild_from, then one more agreement.
+// Collective rebuild of the fresh set dst from the set src (every rank passes its own dst and src): the one-source,
+// every-id case of b200vs_shard_rebuild_from_range, with FLAT and BINARY_FLAT refused.
 int b200vs_shard_rebuild_from(b200vs_shard* dst_h, b200vs_shard* src_h, int64_t* n_rows) {
   return guarded([&]() -> int {
     if (n_rows) *n_rows = 0;
     b200vs_shard* dst = get(dst_h);
     b200vs_shard* src = get(src_h);
     if (dst == src) fail(B200VS_EILLEGAL_PARAMETERS, "rebuild_from: dst and src are the same shard");
-    std::scoped_lock g(src->add_mu, dst->add_mu);
-    RwSharedGuard rl(src->ix);
-    dst->ix->set_device();
-    check(agree(dst, attempt([&] { check_shard_rebuild(dst, src); }), "shard rebuild_from"));
-    int64_t n = 0;
-    if (dst->rows) {  // HNSW: every row already sits on its owner
-      check(agree(dst, attempt([&] {
-        WriteHold hold(dst->ix);
-        n = dst->ix->rebuild_from({src->ix}, 0, INT64_MAX);
-      }), "shard rebuild_from"));
-    } else {
-      n = shard_rebuild_lists(dst, src);
+    const int64_t n = shard_rebuild(dst, {src}, 0, INT64_MAX, false, false, "shard rebuild_from");
+    if (n_rows) *n_rows = n;
+    return B200VS_OK;
+  });
+}
+
+// Collective split / merge rebuild of the fresh set dst from the live rows with id_min <= id < id_max of the source sets
+// srcs[0 .. n_src) (every rank passes its own dst and its own rank's source shards).  The argument errors are refused here,
+// on the rank that meets them, before any collective.
+int b200vs_shard_rebuild_from_range(b200vs_shard* dst_h, int32_t n_src, b200vs_shard* const* srcs_h, int64_t id_min, int64_t id_max,
+                                    int64_t* n_rows) {
+  return guarded([&]() -> int {
+    if (n_rows) *n_rows = 0;
+    if (n_src < 1 || n_src > kRebuildMaxSources || !srcs_h)
+      fail(B200VS_EILLEGAL_PARAMETERS, "shard rebuild_from_range: 1 to 16 sources, in a non-null list");
+    b200vs_shard* dst = get(dst_h);
+    std::vector<b200vs_shard*> srcs;
+    for (int32_t i = 0; i < n_src; ++i) {
+      b200vs_shard* src = get(srcs_h[i]);
+      if (src == dst) fail(B200VS_EILLEGAL_PARAMETERS, "shard rebuild_from_range: dst is among the sources");
+      if (std::find(srcs.begin(), srcs.end(), src) != srcs.end()) fail(B200VS_EILLEGAL_PARAMETERS, "shard rebuild_from_range: a source is listed twice");
+      srcs.push_back(src);
     }
+    // [id_min, id_max) as inclusive bounds; id_max - 1 cannot overflow once the range holds an id
+    const bool none = id_min >= id_max;
+    const int64_t n = shard_rebuild(dst, srcs, none ? 1 : id_min, none ? 0 : id_max - 1, id_min > id_max, true, "shard rebuild_from_range");
     if (n_rows) *n_rows = n;
     return B200VS_OK;
   });
@@ -1794,7 +1910,7 @@ int b200vs_shard_remove_ids(b200vs_shard* h, int64_t n, const int64_t* ids, int6
     if (n_removed) *n_removed = 0;
     if (n <= 0) return B200VS_OK;  // "delete_ids.empty() -> OK"
     if (!ids) fail(B200VS_EILLEGAL_PARAMETERS, "null ids");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     IndexBase* ix = sh->ix;
     const int64_t local = ix->remove(n, ids);  // -1: untrained (OK, nothing to do)
     ix->set_device();
@@ -1819,7 +1935,7 @@ int b200vs_shard_plan_add_device(b200vs_shard* h, int64_t n, const float* x_dev)
     if (sh->ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, "a binary index has no list pre-sizing");
     if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
     if (n <= 0 || !x_dev) fail(B200VS_EILLEGAL_PARAMETERS, "bad plan arguments");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     IndexBase* ix = sh->ix;
     ix->set_device();
     const int nlist = ix->nlist_now();
@@ -1843,7 +1959,7 @@ int b200vs_shard_plan_commit(b200vs_shard* h) {
     b200vs_shard* sh = get(h);
     if (sh->ix->binary()) fail(B200VS_EVECTOR_NOT_SUPPORT, "a binary index has no list pre-sizing");
     if (sh->rows) fail(B200VS_EVECTOR_NOT_SUPPORT, "a row-sharded index has no inverted lists to pre-size");
-    std::lock_guard<std::mutex> g(sh->add_mu);
+    std::lock_guard<Gate> g(sh->add_mu);
     IndexBase* ix = sh->ix;
     ix->set_device();
     const int nlist = ix->nlist_now();

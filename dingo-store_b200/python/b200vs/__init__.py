@@ -41,7 +41,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_search_binary", "b200vs_shard_search_binary_device", "b200vs_shard_range_search_binary",
     "b200vs_shard_range_search_binary_device", "b200vs_search_deep", "b200vs_search_binary_deep",
     "b200vs_shard_search_deep", "b200vs_shard_search_binary_deep",
-    "b200vs_shard_need_rebuild", "b200vs_shard_rebuild_from",
+    "b200vs_shard_need_rebuild", "b200vs_shard_rebuild_from", "b200vs_shard_rebuild_from_range",
     "b200vs_save_stage", "b200vs_save_staged", "b200vs_save_unstage",
 ]
 
@@ -175,6 +175,7 @@ def lib():
     L.b200vs_shard_search_binary_deep.argtypes = [vp, i64, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
     L.b200vs_shard_need_rebuild.argtypes = [vp]
     L.b200vs_shard_rebuild_from.argtypes = [vp, vp, ctypes.POINTER(i64)]
+    L.b200vs_shard_rebuild_from_range.argtypes = [vp, i32, ctypes.POINTER(vp), i64, i64, ctypes.POINTER(i64)]
     _lib = L
     return L
 
@@ -578,6 +579,25 @@ class Shard:
         rows this rank's index holds afterwards."""
         n = ctypes.c_int64(0)
         _check(lib().b200vs_shard_rebuild_from(self.h, src.h, ctypes.byref(n)))
+        return n.value
+
+    def rebuild_from_range(self, srcs, id_min, id_max):
+        """b200vs_shard_rebuild_from_range (collective): fill this fresh shard from the live rows with id_min <= id < id_max
+        of the source shards srcs (this rank's shard of each source set: a region split or merge), on the device; returns the
+        live rows this rank's index holds afterwards.  The argument errors the library refuses before any collective (1 to 16
+        sources, none of them None, this shard or listed twice) are refused here without calling it."""
+        srcs = list(srcs)
+        if not 1 <= len(srcs) <= 16:
+            raise B200VSError(EILLEGAL_PARAMETERS, "shard rebuild_from_range: 1 to 16 sources")
+        if any(s is None or not getattr(s, "h", None) for s in srcs):
+            raise B200VSError(EILLEGAL_PARAMETERS, "shard rebuild_from_range: a source is None or closed")
+        if any(s is self for s in srcs):
+            raise B200VSError(EILLEGAL_PARAMETERS, "shard rebuild_from_range: dst is among the sources")
+        if len({id(s) for s in srcs}) != len(srcs):
+            raise B200VSError(EILLEGAL_PARAMETERS, "shard rebuild_from_range: a source is listed twice")
+        arr = (ctypes.c_void_p * len(srcs))(*[s.h for s in srcs])
+        n = ctypes.c_int64(0)
+        _check(lib().b200vs_shard_rebuild_from_range(self.h, len(srcs), arr, int(id_min), int(id_max), ctypes.byref(n)))
         return n.value
 
     def search(self, xq, k, seq=-1, **kw):

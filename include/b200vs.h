@@ -482,9 +482,60 @@ int b200vs_shard_load(b200vs_shard* shard, const char* prefix);
  * Peak device memory per rank (by list): src's rows, plus about three copies of this rank's share of the live rows while
  * they are sorted and routed (the sorted local copy, the partitioned send copy, the received copy; the local copy is freed
  * once routed), then the training copy rows_r, shard_add's partitioned and received copies of it (cosine: and its
- * normalised copy) and dst's rows. */
+ * normalised copy) and dst's rows.
+ *
+ * shard_rebuild_from_range: the split and merge rebuilds of a region served by a sharded set (b200vs_rebuild_from_range's
+ * counterpart).  Every rank passes its own dst and its own rank's shards of the n_src source sets; dst is a fresh shard as
+ * for shard_rebuild_from, of the same world and rank as every source.  R = the union, over every source set and every rank
+ * of it, of the live rows with id_min <= id < id_max (id_max exclusive).  *n_rows (nullable) = the live rows this rank's dst
+ * holds afterwards.
+ *   IVF_FLAT, BINARY_IVF_FLAT (by list) : rows_r = the rows of R with b200vs_row_owner(id, world) == r in ascending id order
+ *                     (ties inside one source set: by source rank, then that rank's list-major export order), taken as stored
+ *                     (cosine rows are not normalised again).  dst ends up equal, byte for byte (trained state, every list's
+ *                     ids and rows, the FP16 mirror), to a fresh set on which every rank r called shard_train[_binary](rows_r)
+ *                     and then shard_add[_binary](rows_r, ids_r).  No row crosses PCIe: each source set's rows in the range are
+ *                     sorted and routed to their owner in turn, then what arrived is sorted by id on the owner, with each
+ *                     row's source set carried in the sort's value, on dst's write stream and communicator.
+ *   FLAT, BINARY_FLAT, HNSW (by row) : every row already sits on row_owner(id, world): each rank runs b200vs_rebuild_from_range
+ *                     of its sources' rank indexes into its dst index, and nothing moves between ranks (HNSW: levels from
+ *                     dst's fresh generator, no tombstones).
+ *   IVF_PQ          : EVECTOR_NOT_SUPPORT on every rank (the set stores only codes).
+ * With one source and [0, INT64_MAX) the result equals shard_rebuild_from's on every type that call serves; at world 1 it
+ * equals b200vs_rebuild_from_range of the rank-0 indexes.  An empty R (id_min == id_max included): OK, dst stays untrained and
+ * *n_rows = 0 on every rank.  dst's training size for shard_need_rebuild becomes the sum of |rows_r|.
+ * EILLEGAL_PARAMETERS, on every rank when any rank meets it (the first in rank order), before any index changes: id_min >
+ * id_max, a source of another world or rank than dst, a source that differs from dst in type, metric, dimension, nlist,
+ * nlinks, efconstruction or device, a dst that is not empty or (IVF types) already trained, an HNSW dst whose max_elements
+ * is below its rank's share of R, and a rank that would receive fewer than nlist / world training rows.
+ * EVECTOR_ID_DUPLICATED, on every rank, before dst changes: an id live in more than one source set (a split's or merge's
+ * sources hold disjoint ranges); copies of one id inside one source set stay legal.  By list, the copies of an id can sit on
+ * different ranks, so the check runs after the routing, where every copy of an id meets on its owner.
+ * Refused on the rank that meets them, before any collective (every rank must pass them alike): n_src outside [1, 16], a
+ * null srcs or null entry, dst among the sources, a source listed twice.  A device failure after the agreement: EINTERNAL on
+ * every rank, the sources unchanged, dst to be discarded.
+ * Concurrency: a set's writes hold its write gate exclusively; a rebuild holds dst's gate exclusively and every source set's
+ * gate shared, all taken in one order (by handle address), and a shared hold is granted whenever no write holds the gate,
+ * even while a write waits for it.  So a source set's writes wait for the call, and its reads (shard_search, deep and range
+ * searches, on its own lanes and communicators) go on and return unchanged results; none of the sources' communicators is
+ * used.  Rebuilds that read the same source sets (a split's child and parent, a merge beside a split of one of its sources)
+ * never wait for each other's locks on a rank, whatever order they start in.  That does not make their collectives safe to
+ * interleave: each rebuild runs its collectives on its own dst communicator and allocates and frees device memory between
+ * them, and cudaFree synchronises the device, so on NCCL over real GPUs one rebuild's free can wait for another's collective
+ * kernel, which waits for a peer rank stuck the same way the other way round.  So on NCCL run a rank's rebuilds one after
+ * another, in the same order on every rank (a split: the child, then the parent); run them at once only over a collective
+ * library whose ranks meet on the host.  A write to a source set and the rebuilds that read it: every rank must order them
+ * the same way, and a write meant to follow a rebuild must be issued only after that rebuild has returned on its rank (a
+ * write that waits for a gate held shared can be overtaken by a rebuild issued after it; a steady stream of overlapping
+ * rebuilds would keep a source's writes waiting).
+ * Peak device memory per rank (by list): the sources' rows, plus, one source set at a time, its sorted local copy of the
+ * range, the partitioned send copy and the received copy (the local copy is freed once routed); then every source set's
+ * received copy at once with 16 B per row of sort keys and values (the value carries the row's source set in its top bits)
+ * and 16 B per row of sorted output, then the training copy rows_r, shard_add's partitioned and received copies of it
+ * (cosine: and its normalised copy) and dst's rows. */
 int b200vs_shard_need_rebuild(b200vs_shard* shard);
 int b200vs_shard_rebuild_from(b200vs_shard* dst, b200vs_shard* src, int64_t* n_rows);
+int b200vs_shard_rebuild_from_range(b200vs_shard* dst, int32_t n_src, b200vs_shard* const* srcs, int64_t id_min, int64_t id_max,
+                                    int64_t* n_rows);
 int b200vs_shard_plan_add_device(b200vs_shard* shard, int64_t n, const float* x_dev);
 int b200vs_shard_plan_commit(b200vs_shard* shard);
 int b200vs_shard_search(b200vs_shard* shard, int64_t seq, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
