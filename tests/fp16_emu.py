@@ -119,6 +119,47 @@ def decoy_l2(rng, d, k=1, nfill=1000):
     return rows, q[None, :], rows.shape[0] - 2, rows.shape[0] - 1
 
 
+# one FP32 mantissa pattern above the FP16 midpoint: 0x1001 in the low 13 bits rounds up by almost half an FP16 ulp
+ABOVE_MID = 0x1001
+
+
+def decoy_ip(rng, d, k=1, nfill=1000):
+    """IP decoy against the FP16 rounding.  The query support is split into S1 and S2.  On S1 the query's coordinates are
+    +-1 with low bits 0x0FFF, so RN takes almost 2^-11 off each, and R is aligned with the same pattern: both operands
+    of <q, R> come out low, so R's approximate score comes out too high.  On S2 the query's coordinates carry 0x1001,
+    which rounds up, and D lies on S2 with the same round-up pattern: <q, D> comes out high, so D's approximate score
+    comes out too low.  D's magnitudes are lowered one FP16 step at a time until <q, D> lies just below <q, R>.  k - 1
+    rows rotated from R towards the query's S2 part are strictly closer.  Returns (rows, query [1, d], row of R, row of
+    D)."""
+    h = d // 2
+    perm = rng.permutation(h)
+    S1, S2 = perm[: h // 2], perm[h // 2:]
+    s1 = rng.choice(np.float32([-1, 1]), S1.size)
+    s2 = rng.choice(np.float32([-1, 1]), S2.size)
+    one_lo, one_hi = E.with_low_bits(np.float32(1.0), BELOW_MID)[0], E.with_low_bits(np.float32(1.0), ABOVE_MID)[0]
+    q = np.zeros(d, np.float32)
+    q[S1], q[S2] = s1 * one_lo, s2 * one_hi
+    R = np.zeros(d, np.float32)
+    R[S1] = s1 * one_lo
+    D = np.zeros(d, np.float32)
+    D[S2] = s2 * one_hi
+    D = E.lower_until_below(q, D, S2, float(q.astype(np.float64) @ R.astype(np.float64)))
+    t = np.zeros(d)
+    t[S2] = s2 / np.sqrt(S2.size)
+    mR = float(np.linalg.norm(R.astype(np.float64)))
+    rows = np.concatenate([E._filler(rng, nfill, d, 0.5 * mR, mR), np.array(E.closer_ip(R, t, k) + [R, D], np.float32).reshape(-1, d)])
+    return rows, q[None, :], rows.shape[0] - 2, rows.shape[0] - 1
+
+
+def decoy_cos(rng, d, k=1, nfill=1000):
+    """Cosine decoy against the FP16 rounding: decoy_ip's rounding patterns (query 0x0FFF on S1, 0x1001 on S2; R 0x0FFF,
+    D 0x1001) at unit norm, laid out by tf32_emu.unit_decoy.  The pair uses 0.51 to 0.55 of the 2 eps window at d = 64
+    to 768, less than decoy_ip's 0.64 to 0.68: at unit norm the query's half-mass coordinates and R's whole-mass
+    coordinates differ by sqrt 2, so the power-of-two scale cannot put both at mantissa 1, where the rounding is largest
+    relative to the value.  Returns (rows, query [1, d], row of R, row of D)."""
+    return E.unit_decoy(rng, d, k, nfill, (BELOW_MID, ABOVE_MID, BELOW_MID, ABOVE_MID))
+
+
 def decoy_margin(rows, q, r, dd, l2=True):
     """(emulated approx score of R - that of D) / (2 eps): the share of the finish kernel's window the decoy uses up."""
     s = approx_scores(rows[[r, dd]], q, l2)[0]

@@ -53,3 +53,22 @@ def test_half_decoys(k, d):
     assert approx[dd] < approx[r], "D's approximate score must lie below R's"
     m = H.decoy_margin(rows, q, r, dd)
     assert 0.6 < m < 1.0, m  # more than half of the 2 eps window
+
+
+@pytest.mark.parametrize("k", [1, 10])
+@pytest.mark.parametrize("d", [64, 128, 768])
+@pytest.mark.parametrize("gen", ["decoy_ip", "decoy_cos"])
+def test_half_ip_and_cos_decoys(gen, k, d):
+    """The IP and cosine pairs on the FP16 mirror: R the exact k-th neighbour, D the next, and more than half of the 2 eps
+    window used up (IP 0.64 to 0.68, cosine 0.51 to 0.55), so a kernel whose window were half as wide returns D.  The
+    cosine pair is at unit norm, within the 1e-5 under which the index's normalisation leaves a vector as it is."""
+    rows, q, r, dd = getattr(H, gen)(np.random.default_rng(k * d + 5), d, k)
+    score = E.true_scores(rows, q, False)[0]
+    order = np.argsort(score, kind="stable")
+    assert order[k - 1] == r and order[k] == dd, "R must be the exact k-th neighbour and D the next"
+    assert score[dd] - score[r] < 1e-4 * abs(score[r]), "D must lie just above R"
+    if gen == "decoy_cos":
+        n2 = np.einsum("ij,ij->i", rows.astype(np.float64), rows.astype(np.float64))
+        assert np.all(np.abs(1 - n2) < 1e-6) and abs(1 - float(np.sum(q.astype(np.float64) ** 2))) < 1e-6
+    m = H.decoy_margin(rows, q, r, dd, l2=False)
+    assert (0.6 if gen == "decoy_ip" else 0.5) < m < 1.0, m

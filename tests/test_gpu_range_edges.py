@@ -67,14 +67,18 @@ def same(a, b):
 # =====================================================================================================================
 # 1. capture-window decoys
 # =====================================================================================================================
-# name -> (index kind, metric, generator): Flat scans TF32 rows, IVF-Flat at d % 8 == 0 its FP16 mirror
-DECOYS = {"tf32-L2": (FLAT, L2, E.decoy_l2), "tf32-IP": (FLAT, IP, E.decoy_ip), "fp16-L2": (IVF_FLAT, L2, H.decoy_l2)}
-DECOY_D, NPAIR = 128, 32
+# name -> (index kind, metric, generator, d): Flat scans TF32 rows, IVF-Flat at d % 8 == 0 its FP16 mirror and at
+# d = 132 (no mirror) its rows in the TF32 list form
+DECOYS = {"tf32-L2": (FLAT, L2, E.decoy_l2, 128), "tf32-IP": (FLAT, IP, E.decoy_ip, 128),
+          "fp16-L2": (IVF_FLAT, L2, H.decoy_l2, 128), "fp16-IP": (IVF_FLAT, IP, H.decoy_ip, 128),
+          "fp16-cos": (IVF_FLAT, COSINE, H.decoy_cos, 128),
+          "tf32list-L2": (IVF_FLAT, L2, E.decoy_l2, 132), "tf32list-IP": (IVF_FLAT, IP, E.decoy_ip, 132)}
+NPAIR = 32
 
 
 def decoy_pairs(name):
-    gen = DECOYS[name][2]
-    return [gen(np.random.default_rng(7000 + p), DECOY_D, 1, nfill=1500) for p in range(NPAIR)]
+    gen, d = DECOYS[name][2:]
+    return [gen(np.random.default_rng(7000 + p), d, 1, nfill=1500) for p in range(NPAIR)]
 
 
 def decoy_centroids(d):
@@ -121,7 +125,7 @@ def window_share(approx_r, rows, q, r, thr, eps, metric):
 def test_decoy_premise(name):
     """On the CPU emulators: R's tile score sits above its true score by more than half of eps beyond the threshold's
     slack, so the decoy test below fails for a kernel whose capture threshold is widened by eps / 2."""
-    kind, metric, _ = DECOYS[name]
+    kind, metric, _, _ = DECOYS[name]
     l2 = metric == L2
     for p, (rows, q, r, _) in enumerate(decoy_pairs(name)):
         _, thr = tight_radius(rows, q[0], r, metric)
@@ -139,13 +143,13 @@ def test_decoy_is_captured(oracle, name):
     """Index p holds pair p among filler rows; the radius admits R by one FP32 step.  The whole 32-query batch stays on
     the tile pass (nothing re-run), R comes back, and every answer equals the exact scan and the restated rule."""
     require_gpu()
-    kind, metric, _ = DECOYS[name]
+    kind, metric, _, d = DECOYS[name]
     pairs = decoy_pairs(name)
     xq = np.concatenate([p[1] for p in pairs])
     for p in range(0, NPAIR, 4):
         rows, q, r, _ = pairs[p]
         ids = np.arange(rows.shape[0], dtype=np.int64) * 7 + 3
-        c = Built(oracle, kind, metric, rows, ids, cent=decoy_centroids(DECOY_D) if kind == IVF_FLAT else None)
+        c = Built(oracle, kind, metric, rows, ids, cent=decoy_centroids(d) if kind == IVF_FLAT else None)
         radius, thr = tight_radius(rows, q[0], r, metric)
         if kind == FLAT:  # the device's own score and eps (TF32 list-scan arithmetic, rows in insertion order)
             S, Eps = c.ix.tc_scores(np.repeat(q, 16, axis=0))

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import b200vs
+import fp16_emu as H
 import tf32_emu as E
 from b200vs import COSINE, FLAT, IP, IVF_FLAT, L2
 from gpu_util import assert_same_results, require_gpu
@@ -44,12 +45,14 @@ def far_centroids(nlist, d, scale=1000.0):
 @pytest.mark.parametrize("metric", [L2, IP])
 @pytest.mark.parametrize("index_type", [FLAT, IVF_FLAT])
 def test_decoys(oracle, index_type, metric, k):
-    """32 queries, each with its own (R, D) pair (tf32_emu.decoy_*): D's exact distance lies just above R's, its approximate
-    score far below.  Index p holds pair p among filler rows; every index is searched with the whole batch and query p
-    must return R as its k-th neighbour.  The L2 decoys use up more than half of the 2 eps window, so a kernel whose eps
-    is half of what it claims returns D."""
+    """32 queries, each with its own (R, D) pair: D's exact distance lies just above R's, its approximate score far below.
+    Index p holds pair p among filler rows; every index is searched with the whole batch and query p must return R as
+    its k-th neighbour.  Each pair is built against the arithmetic that scans it: Flat scans TF32 rows (tf32_emu.decoy_*),
+    IVF-Flat at d = 128 its FP16 mirror (fp16_emu.decoy_*).  The L2 and FP16 IP decoys use up more than half of the 2 eps
+    window, so a kernel whose eps is half of what it claims returns D."""
     d, npair = 128, 32
-    gen = E.decoy_l2 if metric == L2 else E.decoy_ip
+    emu = E if index_type == FLAT else H
+    gen = emu.decoy_l2 if metric == L2 else emu.decoy_ip
     pairs = [gen(np.random.default_rng(1000 * k + p), d, k, nfill=1500) for p in range(npair)]
     xq = np.concatenate([p[1] for p in pairs])
     for p in range(0, npair, 4):  # 8 of the 32 indexes: every query is still searched against 8 different indexes

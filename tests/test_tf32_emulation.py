@@ -57,3 +57,23 @@ def test_decoys(k, d):
         m = E.decoy_margin(rows, q, r, dd, l2)
         # L2: more than half of the 2 eps window, so halving eps drops R from the window
         assert floor < m < 1.0, m
+
+
+@pytest.mark.parametrize("k", [1, 10])
+def test_list_form_decoys(k):
+    """The TF32 list form at d = 132 (16-byte rows, d % 8 != 0: IVF-Flat keeps no FP16 mirror).  L2 uses more than half of
+    the 2 eps window; IP and cosine (unit norm) only about 0.45 and 0.37, because truncation lowers |D| as well, so D's
+    side gains from the query's rounding alone: the GPU tests hold them to these emulated floors."""
+    d = 132
+    assert (4 * d) % 16 == 0 and d % 8 != 0
+    for gen, l2, floor in ((E.decoy_l2, True, 0.6), (E.decoy_ip, False, 0.4), (E.decoy_cos, False, 0.35)):
+        rows, q, r, dd = gen(np.random.default_rng(k * d), d, k)
+        score = E.true_scores(rows, q, l2)[0]
+        order = np.argsort(score, kind="stable")
+        assert order[k - 1] == r and order[k] == dd, "R must be the exact k-th neighbour and D the next"
+        approx = E.approx_scores(rows, q, l2, False)[0]
+        assert approx[dd] < approx[r], "D's approximate score must lie below R's"
+        if gen is E.decoy_cos:
+            n2 = np.einsum("ij,ij->i", rows.astype(np.float64), rows.astype(np.float64))
+            assert np.all(np.abs(1 - n2) < 1e-6)
+        assert floor < E.decoy_margin(rows, q, r, dd, l2) < 1.0

@@ -221,6 +221,83 @@ def decoy_ip(rng, d, k=1, nfill=1000):
     return rows, q[None, :], rows.shape[0] - 2, rows.shape[0] - 1
 
 
+def closer_ip(R, toward, k):
+    """k - 1 rows strictly closer than R by inner product, at R's norm: R rotated towards the unit vector `toward`
+    (orthogonal to R, positive against the query) by 0.05 m rad, so they never raise max ||x|| (eps) above the pair's."""
+    nR = float(np.linalg.norm(R.astype(np.float64)))
+    return [(np.cos(0.05 * m) * R + np.sin(0.05 * m) * nR * toward).astype(np.float32) for m in range(1, k)]
+
+
+def lower_until_below(q, D, S, P):
+    """Lower D's magnitudes on S one step of the 10-bit mantissa grid (TF32 and FP16 alike) at a time, coordinate after coordinate, keeping their low 13 bits, until
+    <q, D> < P.  Returns D."""
+    D = D.copy()
+    i = 0
+    while float(q.astype(np.float64) @ D.astype(np.float64)) >= P:
+        j = S[i % S.size]
+        low = int(_bits(D[j])[0]) & 0x1FFF
+        g = np.float32(np.nextafter(np.float16(abs(tf32_trunc(D[j])[0])), np.float16(0)))
+        D[j] = np.sign(D[j]) * with_low_bits(g, low)[0]
+        i += 1
+    return D
+
+
+def _coord(target, low):
+    """The largest FP32 value <= target whose top 10 mantissa bits lie on the TF32 / FP16 grid and whose low 13 bits are `low`."""
+    g = np.float16(target)
+    while with_low_bits(np.float32(g), low)[0] > target:
+        g = np.nextafter(g, np.float16(0))
+    return with_low_bits(np.float32(g), low)[0]
+
+
+def _unit(x, axis):
+    """x completed to unit norm by one coordinate on `axis` (which x leaves zero): |1 - ||x||^2| stays far below the
+    1e-5 under which the index's cosine normalisation leaves a vector bit for bit as it is."""
+    n2 = float(x.astype(np.float64) @ x.astype(np.float64))
+    assert x[axis] == 0 and n2 < 1
+    x = x.copy()
+    x[axis] = np.float32(np.sqrt(1.0 - n2))
+    return x
+
+
+def unit_decoy(rng, d, k, nfill, pats):
+    """An IP pair at unit norm (the cosine decoys), so the index's cosine normalisation leaves the query, R and D bit for
+    bit as they are.  pats = low 13 bits of (query on S1, query on S2, R, D).  The query puts half of its mass on S1 and
+    half on S2 (n coordinates each), R all of its mass on S1 and D on S2; every coordinate is the largest value within
+    its share of the norm that carries its pattern, and every vector is completed to unit norm by one coordinate on an
+    axis its partner leaves zero.  D's magnitudes are lowered one grid step at a time until <q, D> lies just below
+    <q, R>; k - 1 rows rotated from R towards the query's S2 part are strictly closer; filler rows are unit vectors on
+    [d/2, d).  n = 15 puts R's coordinates near mantissa 1 and the query's near sqrt 2 (their values differ by sqrt 2).
+    Returns (rows, query [1, d], row of R, row of D)."""
+    h = d // 2
+    n = min(15, (h - 3) // 2)
+    perm = rng.permutation(h)
+    S1, S2, (cq, cr, cd) = perm[:n], perm[n:2 * n], perm[2 * n:2 * n + 3]
+    s1 = rng.choice(np.float32([-1, 1]), n)
+    s2 = rng.choice(np.float32([-1, 1]), n)
+    q = np.zeros(d, np.float32)
+    q[S1] = s1 * _coord(np.sqrt(0.5 / n), pats[0])
+    q[S2] = s2 * _coord(np.sqrt(0.5 / n), pats[1])
+    R = np.zeros(d, np.float32)
+    R[S1] = s1 * _coord(np.sqrt(1.0 / n), pats[2])
+    D = np.zeros(d, np.float32)
+    D[S2] = s2 * _coord(np.sqrt(1.0 / n), pats[3])
+    D = lower_until_below(q, D, S2, float(q.astype(np.float64) @ R.astype(np.float64)))
+    q, R, D = _unit(q, cq), _unit(R, cr), _unit(D, cd)
+    t = np.zeros(d)
+    t[S2] = s2 / np.sqrt(n)
+    rows = np.concatenate([_filler(rng, nfill, d, 1.0, 1.0), np.array(closer_ip(R, t, k) + [R, D], np.float32).reshape(-1, d)])
+    return rows, q[None, :], rows.shape[0] - 2, rows.shape[0] - 1
+
+
+def decoy_cos(rng, d, k=1, nfill=1000):
+    """Cosine decoy against the TF32 list scan: decoy_ip's patterns (query 0x0FFF on S1, rounding down, 0x1001 on S2,
+    rounding up; R 0x1FFF, losing almost a TF32 ulp to truncation; D exact in TF32) at unit norm (unit_decoy).  Like
+    decoy_ip it uses less than half of the 2 eps window (about 0.37): truncation only ever lowers |D|, so D's side gains
+    from the query's rounding alone.  Returns (rows, query [1, d], row of R, row of D)."""
+    return unit_decoy(rng, d, k, nfill, (0x0FFF, 0x1001, 0x1FFF, 0x0000))
+
+
 def decoy_margin(rows, q, r, dd, l2):
     """(emulated approx score of R - that of D) / (2 eps): the share of the finish kernel's window the decoy uses up."""
     s = approx_scores(rows[[r, dd]], q, l2, False)[0]
