@@ -77,10 +77,13 @@ void index_read(IndexBase* ix, void* stream, const b200vs_search_params* sp, Bod
 // answers into scratch, and the results come down into out_dist / out_ids [nq, k] (and, for a range search, out_counts
 // [nq]).  A NaN radius admits no row of a float index: empty results, nothing launched (DESIGN.md 4.6); a binary index
 // refuses it.  xq / outputs may be pinned staging (coalesced batches) or caller memory.
+// brute: every stored row (b200vs_brute_force_*) in place of the index's own search.
 void host_read(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_search_params* sp, float* out_dist, int64_t* out_ids,
-               bool range = false, float radius = 0.f, int32_t* out_counts = nullptr, bool deep = false) {
+               bool range = false, float radius = 0.f, int32_t* out_counts = nullptr, bool deep = false, bool brute = false) {
   index_read(ix, nullptr, sp, [&](const SearchCtx& sc, cudaStream_t s) {
     const size_t nk = (size_t)nq * k;
+    if (brute && !ix->brute_force_served())  // before anything is launched, with the stats already cleared
+      fail(B200VS_EVECTOR_NOT_SUPPORT, "brute-force search over an index's rows is served for FLAT, IVF_FLAT and HNSW under L2 / IP");
     if (range && std::isnan(radius) && !ix->binary()) {
       std::fill_n(out_dist, nk, 0.0F);
       std::fill_n(out_ids, nk, (int64_t)-1);
@@ -96,7 +99,8 @@ void host_read(IndexBase* ix, int64_t nq, const void* xq, int k, const b200vs_se
     r.oi = ix->scratch.alloc<long long>(nk);
     if (range) r.oc = ix->scratch.alloc<int>((size_t)nq);
     B200VS_CUDA(cudaMemcpyAsync(dq, xq, qbytes, cudaMemcpyHostToDevice, s));
-    ix->search(r, s);
+    if (brute) brute_force(ix, r, s);
+    else ix->search(r, s);
     ix->phases_finish(s);  // the phases end before the copies back
     B200VS_CUDA(cudaMemcpyAsync(out_dist, r.od, nk * 4, cudaMemcpyDeviceToHost, s));
     B200VS_CUDA(cudaMemcpyAsync(out_ids, r.oi, nk * 8, cudaMemcpyDeviceToHost, s));
@@ -136,9 +140,41 @@ int range_search(b200vs_index* h, int64_t nq, const void* xq, float radius, int 
   });
 }
 
+// b200vs_brute_force_search / b200vs_brute_force_range_search: the arguments' checks and statuses of b200vs_scan_begin /
+// b200vs_scan_range_begin; host_read refuses the types whose rows the scan cannot reproduce
+int host_brute_force(b200vs_index* h, int64_t nq, const float* xq, int k, bool range, float radius, const b200vs_search_params* sp,
+                     float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  return guarded([&]() -> int {
+    IndexBase* ix = get(h);
+    if (nq <= 0 || !xq) fail(B200VS_EILLEGAL_PARAMETERS, "vector_with_ids is empty");
+    if (range) {
+      if (k <= 0) fail(B200VS_EILLEGAL_PARAMETERS, "max_results must be > 0");
+      if (!out_counts) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    } else {
+      if (k <= 0) return B200VS_OK;
+      if (k > kDeepMaxK) fail(B200VS_EILLEGAL_PARAMETERS, "topk above " + std::to_string(kDeepMaxK));
+    }
+    if (!out_ids || !out_dist) fail(B200VS_EILLEGAL_PARAMETERS, "null output");
+    // the top-k of b200vs_scan_*: the deep path past the exact scan's shared-memory select
+    const bool deep = !range && !exact_select_fits(ix->dim, 1, k);
+    host_read(ix, nq, xq, k, sp, out_dist, out_ids, range, radius, out_counts, deep, true);
+    return B200VS_OK;
+  });
+}
+
 }  // namespace
 
 extern "C" {
+
+int b200vs_brute_force_search(b200vs_index* h, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp, float* out_dist,
+                              int64_t* out_ids) {
+  return host_brute_force(h, nq, xq, k, false, 0.f, sp, out_dist, out_ids, nullptr);
+}
+
+int b200vs_brute_force_range_search(b200vs_index* h, int64_t nq, const float* xq, float radius, int32_t max_results,
+                                    const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts) {
+  return host_brute_force(h, nq, xq, max_results, true, radius, sp, out_dist, out_ids, out_counts);
+}
 
 int b200vs_create(b200vs_type type, b200vs_metric metric, int32_t dim, const b200vs_params* params, b200vs_index** out) {
   return guarded([&]() -> int {
@@ -898,7 +934,7 @@ int b200vs_scan_range_push(b200vs_scan_range* st, int64_t n, const float* x, con
     B200VS_CUDA(cudaMemcpyAsync(st->x.p, x, (size_t)n * st->dim * 4, cudaMemcpyHostToDevice, st->s));
     B200VS_CUDA(cudaMemcpyAsync(st->ids.p, ids, (size_t)n * 8, cudaMemcpyHostToDevice, st->s));
     if (st->cosine) launch_normalize_faiss(st->x.p, n, st->dim, st->s);  // vector_index_flat.cc:155
-    launch_range_append(st->l2, st->x.p, st->ids.p, n, st->dim, st->nq, st->q.p, st->sc, st->thr_raw, st->max_results,
+    launch_range_append(st->l2, st->x.p, st->ids.p, nullptr, n, st->dim, st->nq, st->q.p, st->sc, st->thr_raw, st->max_results,
                         st->out_d.p, st->out_i.p, st->counts.p, st->s);
     B200VS_CUDA(cudaStreamSynchronize(st->s));  // the caller may reuse its buffers, and the next push rewrites the tile
     return B200VS_OK;

@@ -32,6 +32,7 @@
 
 #include "index.h"
 #include "scan_kernels.cuh"
+#include "tc_scan.cuh"
 
 namespace b200vs {
 
@@ -1383,6 +1384,34 @@ struct HnswIndex : IndexBase {
     });
     if (!fast) stats[6] += nq;
     timer.stop();
+  }
+
+  // the device mirror's rows, after upload(); a node's id is its label, or -1 once deleted.  The tile scan's row norms are
+  // computed per call when asked for (the mirror keeps none).
+  bool brute_force_rows(TcView& v, bool norms, cudaStream_t s) override {
+    if (metric == B200VS_COSINE) fail(B200VS_EVECTOR_NOT_SUPPORT, "brute-force search of an HNSW cosine index is not supported");
+    upload(s);
+    if (G.n == 0) return false;
+    const int64_t n = G.n;
+    v.vecs = d_data.p;
+    long long* ids = scratch.alloc<long long>(n);
+    launch_node_ids(d_labels.p, d_deleted.p, n, ids, s);
+    launch_count(1);
+    v.ids = ids;
+    if (norms) {
+      float* nr = scratch.alloc<float>(n);
+      launch_row_norms(d_data.p, n, dim, nr, s);
+      launch_count(1);
+      v.norms = nr;
+      v.max_norm = device_max_norm(this, nr, n, s);
+    }
+    long long* off = scratch.alloc<long long>(1);
+    int* len = scratch.alloc<int>(1);
+    const int len1 = (int)std::min<int64_t>(n, 0x7fffffff);
+    B200VS_CUDA(cudaMemsetAsync(off, 0, 8, s));
+    B200VS_CUDA(cudaMemcpyAsync(len, &len1, 4, cudaMemcpyHostToDevice, s));
+    set_flat_layout(v, n, off, len);
+    return true;
   }
 
   int64_t count() const override { return G.n - G.ndeleted; }

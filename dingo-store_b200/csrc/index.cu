@@ -389,27 +389,16 @@ struct FlatIndex : IndexBase {
     return j;
   }
 
-  // VectorIndexFlat::Search / RangeSearch, vector_index_flat.cc:206-323: range radius -> 1 - radius for IP / cosine
-  // (:282-285); faiss range_search keeps L2 dis < radius, IP ip > radius.  Every path selects the same rows.
+  // VectorIndexFlat::Search / RangeSearch, vector_index_flat.cc:206-323
   void search(const SearchReq& r, cudaStream_t s) override {
     refuse_probes(r);
-    const float* q = queries(r, s);
-    const float thr = ip_like() ? 1.0F - r.radius : r.radius;
-    if (r.deep) { run_scan_deep(this, job(*r.sc), r.nq, q, r.k, r.od, r.raw, r.oi, s); return; }
-    const TcView v = rowmap.view();
-    if (rowmap.rows > 0 && tc_eligible(this, v, r.nq, r.k, 1, *r.sc, r.range)) {
-      long long* probes = scratch.alloc<long long>(r.nq);
-      B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)r.nq * 8, s));
-      tc_search(this, v, r, q, probes, 1, thr, s);
-      return;
-    }
-    if (!r.range && flat_small_eligible(device, r.nq, rowmap.rows, dim, r.k, *r.sc)) {  // one query per task is the reference's own shape: single-launch path
-      flat_small_search(this, metric == B200VS_L2, rowmap.store.vecs.p, rowmap.store.ids.p, rowmap.rows, r.nq, q, r.k, *r.sc, r.od, r.oi, r.raw, s);
-      return;
-    }
-    ScanJob j = job(*r.sc);
-    if (r.range) { j.has_thr = true; j.thr_raw = thr; }
-    run_scan(this, j, r.nq, q, r.k, r.raw ? nullptr : r.od, r.raw ? r.od : nullptr, r.oi, r.oc, s);
+    flat_view_search(this, rowmap.view(), r, s);
+  }
+
+  // the store's ids already mark every tombstone
+  bool brute_force_rows(TcView& v, bool, cudaStream_t) override {
+    v = rowmap.view();
+    return rowmap.rows > 0;
   }
 
   void debug_tc_scores(int64_t nq, const float* xq, int arith, float* out_scores, float* out_eps, cudaStream_t s) override {
@@ -476,6 +465,29 @@ struct FlatIndex : IndexBase {
 };
 
 IndexBase* make_flat(b200vs_metric m, int d, const b200vs_params& p) { return new FlatIndex(m, d, p); }
+
+// range radius -> 1 - radius for IP / cosine (vector_index_flat.cc:282-285); faiss range_search keeps L2 dis < radius, IP
+// ip > radius.  Every path selects the same rows.
+void flat_view_search(IndexBase* ix, const TcView& v, const SearchReq& r, cudaStream_t s) {
+  const float* q = ix->queries(r, s);
+  const float thr = ix->ip_like() ? 1.0F - r.radius : r.radius;
+  ScanJob j;
+  j.l2 = ix->metric == B200VS_L2;
+  j.vecs = v.vecs; j.ids = v.ids; j.d = ix->dim; j.mode = 0; j.n = v.arena_rows; j.sc = r.sc;
+  if (r.deep) { run_scan_deep(ix, j, r.nq, q, r.k, r.od, r.raw, r.oi, s); return; }
+  if (v.arena_rows > 0 && tc_eligible(ix, v, r.nq, r.k, 1, *r.sc, r.range)) {
+    long long* probes = ix->scratch.alloc<long long>(r.nq);
+    B200VS_CUDA(cudaMemsetAsync(probes, 0, (size_t)r.nq * 8, s));
+    tc_search(ix, v, r, q, probes, 1, thr, s);
+    return;
+  }
+  if (!r.range && flat_small_eligible(ix->device, r.nq, v.arena_rows, ix->dim, r.k, *r.sc)) {  // one query per task is the reference's own shape: single-launch path
+    flat_small_search(ix, j.l2, v.vecs, v.ids, v.arena_rows, r.nq, q, r.k, *r.sc, r.od, r.oi, r.raw, s);
+    return;
+  }
+  if (r.range) { j.has_thr = true; j.thr_raw = thr; }
+  run_scan(ix, j, r.nq, q, r.k, r.raw ? nullptr : r.od, r.raw ? r.od : nullptr, r.oi, r.oc, s);
+}
 
 // ============================================================================================
 // IVF-Flat
@@ -632,6 +644,24 @@ struct IvfFlatIndex : IndexBase {
   }
 
   void search(const SearchReq& r, cudaStream_t s) override;
+  // the arena with its FP16 mirror; the ids of the slots outside every list's [off, off + len) (capacity slack, the old
+  // places of relocated lists) are -1 in a view built per call
+  bool brute_force_rows(TcView& v, bool, cudaStream_t s) override {
+    if (!trained || L.live == 0) return false;
+    v = store.view();
+    const int64_t rows = L.arena_used;
+    long long* ids = scratch.alloc<long long>(rows);
+    launch_list_ids(store.ids.p, L.d_off.p, L.d_len.p, nlist, rows, ids, s);
+    launch_count(1);
+    v.ids = ids;
+    long long* off = scratch.alloc<long long>(1);
+    int* len = scratch.alloc<int>(1);
+    const int len1 = (int)std::min<int64_t>(rows, 0x7fffffff);
+    B200VS_CUDA(cudaMemsetAsync(off, 0, 8, s));
+    B200VS_CUDA(cudaMemcpyAsync(len, &len1, 4, cudaMemcpyHostToDevice, s));
+    set_flat_layout(v, rows, off, len);
+    return true;
+  }
   void coarse(int64_t nq, const void* xv, bool prepared, int nprobe, int c0, int c1, float* out_score, long long* out_lists,
               cudaStream_t s) override {
     if (!trained) fail(B200VS_EVECTOR_NOT_TRAIN, "not train");

@@ -187,6 +187,7 @@ struct SearchCtx {  // resolved per-search parameters, device filter included
   bool has_filter() const { return has_range || sorted_ids_dev; }
 };
 struct IndexBase;
+struct TcView;
 // resolve search params; uploads the sorted id list into the calling lane's scratch (stream-ordered on s)
 SearchCtx make_ctx(IndexBase* ix, const b200vs_search_params* sp, cudaStream_t s);
 
@@ -211,6 +212,13 @@ struct SearchReq {
 };
 // the results of a search that finds nothing (an untrained or empty index): ids -1, distances 0, range counts 0
 void fill_empty(const SearchReq& r, cudaStream_t s);
+// The search of one Flat view (tc_scan.cuh): a Flat index's rows, or every row slot of another index for a brute-force scan.
+// Top-k through the tile scan, the one-query kernel or the exact scan, deep top-k through the deep path, range through the
+// tile scan or the exact scan; every path selects the same rows (index.cu).
+void flat_view_search(IndexBase* ix, const TcView& v, const SearchReq& r, cudaStream_t s);
+// b200vs_brute_force_search / b200vs_brute_force_range_search (brute_force.cu): r over every row ix->brute_force_rows gives,
+// with the results b200vs_scan_* / b200vs_scan_range_* return for those rows fed in ascending id order.
+void brute_force(IndexBase* ix, const SearchReq& r, cudaStream_t s);
 
 // One write of rows into an index (IndexBase::add).  Host rows come with host ids; device rows (on the index's device) come
 // with device ids, and with the same ids on the host when the caller already holds them.
@@ -348,6 +356,17 @@ struct IndexBase {
     RebuildSource p;
     live_rows(lo, hi, p);
     out.insert(out.end(), p.ids.begin(), p.ids.end());
+  }
+  // b200vs_brute_force_*: the types whose stored rows a brute-force scan reproduces (FLAT, IVF_FLAT, and HNSW under L2 / IP:
+  // IVF_PQ keeps only codes, binary rows have no brute-force path, HNSW cosine rows carry NormalizeVectorForHnsw's bits)
+  bool brute_force_served() const { return type == B200VS_FLAT || type == B200VS_IVF_FLAT || (type == B200VS_HNSW && metric != B200VS_COSINE); }
+  // every row slot of a served index as one Flat view, on stream s with a lane held under the reader lock: the store's rows
+  // and ids, or (where the store's ids do not say so) ids built per call in the lane's scratch, -1 for every tombstone,
+  // unused slot or deleted node.  norms: the row norms the tile scan needs (HNSW computes them per call).  False when there
+  // is nothing to scan (an empty or untrained index).
+  virtual bool brute_force_rows(TcView& v, bool norms, cudaStream_t s) {
+    (void)v; (void)norms; (void)s;
+    fail(B200VS_EVECTOR_NOT_SUPPORT, "brute-force search over an index's rows is served for FLAT, IVF_FLAT and HNSW under L2 / IP");
   }
   virtual void set_state(const void* blob, size_t len) { (void)blob; (void)len; fail(B200VS_EVECTOR_NOT_SUPPORT, "no trained state for this index type"); }
   virtual int64_t get_state(void* blob, size_t cap) { (void)blob; (void)cap; return 0; }
@@ -594,10 +613,11 @@ void run_scan_deep(IndexBase* ix, const ScanJob& job, int64_t nq, const float* q
                    cudaStream_t s);
 
 // b200vs_scan_range_push: append the hits of one tile [n, d] to each query's running list in row order (range_append_kernel).
-// thr_raw is the raw threshold (L2: dist < thr; IP: ip > thr); counts[nq] persists across calls.
-void launch_range_append(bool l2, const float* vecs, const long long* ids, int64_t n, int d, int64_t nq, const float* queries,
-                         const SearchCtx& sc, float thr_raw, int max_results, float* out_dist, long long* out_ids, int* counts,
-                         cudaStream_t s);
+// thr_raw is the raw threshold (L2: dist < thr; IP: ip > thr); counts[nq] persists across calls.  rows (nullable): the walk's
+// i-th row is vecs row rows[i] with id ids[i] (b200vs_brute_force_range_search's gathered list), else row i.
+void launch_range_append(bool l2, const float* vecs, const long long* ids, const long long* rows, int64_t n, int d, int64_t nq,
+                         const float* queries, const SearchCtx& sc, float thr_raw, int max_results, float* out_dist,
+                         long long* out_ids, int* counts, cudaStream_t s);
 void launch_normalize_faiss(float* x, int64_t n, int d, cudaStream_t s);
 void launch_normalize_hnsw(const float* x, float* out, int64_t n, int d, cudaStream_t s);
 void launch_scatter_rows(const float* src, const long long* src_ids, const long long* slots, int64_t n, int d,
@@ -607,6 +627,12 @@ void launch_move_rows(const float* svecs, const long long* sids, const float* sn
                       cudaStream_t s);
 void launch_set_ids(long long* ids, const long long* slots, int64_t n, long long value, cudaStream_t s);
 void launch_iota(long long* p, int64_t n, cudaStream_t s);
+// out[r] = ids[r] for the rows r in [off[l], off[l] + len[l]) of some list l < nlist, -1 for every other r < rows
+// (brute_force.cu)
+void launch_list_ids(const long long* ids, const long long* off, const int* len, int nlist, int64_t rows, long long* out,
+                     cudaStream_t s);
+// out[i] = deleted[i] ? -1 : labels[i] for the n nodes of an HNSW device mirror (brute_force.cu)
+void launch_node_ids(const long long* labels, const unsigned char* deleted, int64_t n, long long* out, cudaStream_t s);
 void launch_negate(float* p, int64_t n, cudaStream_t s);
 // out[i*nr + j] = L2 ? ||a_i - b_j||^2 : 1 - <a_i, b_j>, reference summation order (VectorCalcDistance)
 void launch_pair_distance(bool l2, const float* a, int64_t nl, const float* b, int64_t nr, int d, float* out, cudaStream_t s);

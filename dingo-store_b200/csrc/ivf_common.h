@@ -70,8 +70,7 @@ struct FlatRowMap {
   }
   TcView view() const {
     TcView v = store.view();
-    v.arena_rows = rows; v.list_off = d_off1.p; v.list_len = d_len1.p;
-    v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
+    set_flat_layout(v, rows, d_off1.p, d_len1.p);
     return v;
   }
 
@@ -602,5 +601,11 @@ void launch_expand_pm1(const uint32_t* words, const long long* rows, int64_t m, 
 void check_rebuild_pair(const IndexBase& dst, const IndexBase& src);
 
 void check_batch_ids_unique(int64_t n, const int64_t* ids);
+
+// The stable device radix sort of n (id, value) pairs by id (ids are >= 0), the rebuild's and the brute-force range
+// search's: keys_out / vals_out get the n pairs in ascending id order, pairs with equal ids in their input order.  temp(bytes)
+// hands out the sort's temporary storage.  On stream s.
+void sort_by_id(int64_t n, const long long* keys, long long* keys_out, const long long* vals, long long* vals_out,
+                const std::function<void*(size_t)>& temp, cudaStream_t s);
 
 }  // namespace b200vs

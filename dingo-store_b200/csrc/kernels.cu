@@ -136,9 +136,16 @@ static void run_scan_impl(IndexBase* ix, const ScanJob& job, int64_t nq, const f
   ix->launch_count(2);
 }
 
-void launch_range_append(bool l2, const float* vecs, const long long* ids, int64_t n, int d, int64_t nq, const float* queries,
-                         const SearchCtx& sc, float thr_raw, int max_results, float* out_dist, long long* out_ids, int* counts,
-                         cudaStream_t s) {
+template <class Dist, class Rows>
+static void launch_range_append_rows(const RangeAppendArgs& a, int64_t nq, const Rows& src, cudaStream_t s) {
+  const size_t smem = range_append_smem_bytes(a.d);
+  ensure_smem(range_append_kernel<Dist, Rows>, smem);
+  range_append_kernel<Dist, Rows><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(a, src);
+}
+
+void launch_range_append(bool l2, const float* vecs, const long long* ids, const long long* rows, int64_t n, int d, int64_t nq,
+                         const float* queries, const SearchCtx& sc, float thr_raw, int max_results, float* out_dist,
+                         long long* out_ids, int* counts, cudaStream_t s) {
   if (n <= 0 || nq <= 0) return;
   RangeAppendArgs a;
   a.vecs = vecs; a.ids = ids; a.n = n; a.d = d; a.queries = queries;
@@ -146,13 +153,13 @@ void launch_range_append(bool l2, const float* vecs, const long long* ids, int64
   a.filt.sorted_ids = sc.sorted_ids_dev; a.filt.n_ids = sc.n_ids;
   a.thr_key = f2ord(l2 ? thr_raw : -thr_raw);
   a.max_results = max_results; a.out_dist = out_dist; a.out_ids = out_ids; a.counts = counts;
-  const size_t smem = range_append_smem_bytes(d);
-  if (l2) {
-    ensure_smem(range_append_kernel<Fp32Dist<true>>, smem);
-    range_append_kernel<Fp32Dist<true>><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(a);
+  if (rows) {
+    const ListRows src{rows};
+    if (l2) launch_range_append_rows<Fp32Dist<true>>(a, nq, src, s);
+    else launch_range_append_rows<Fp32Dist<false>>(a, nq, src, s);
   } else {
-    ensure_smem(range_append_kernel<Fp32Dist<false>>, smem);
-    range_append_kernel<Fp32Dist<false>><<<(unsigned)nq, SCAN_THREADS, smem, s>>>(a);
+    if (l2) launch_range_append_rows<Fp32Dist<true>>(a, nq, IdentityRows{}, s);
+    else launch_range_append_rows<Fp32Dist<false>>(a, nq, IdentityRows{}, s);
   }
   B200VS_CUDA(cudaGetLastError());
 }

@@ -50,11 +50,8 @@ void sort_gather(IndexBase* ix, int64_t n, const long long* keys, const long lon
                  DevBuf<uint32_t>& out_rows, DevBuf<long long>& out_ids, cudaStream_t s) {
   DevBuf<long long> sorted_vals;
   sorted_vals.reserve(n, 0, s); out_ids.reserve(n, 0, s);
-  size_t tmp_bytes = 0;
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, out_ids.p, vals, sorted_vals.p, (int)n, 0, 64, s));
   DevBuf<unsigned char> tmp;
-  tmp.reserve(std::max<size_t>(tmp_bytes, 1), 0, s);
-  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys, out_ids.p, vals, sorted_vals.p, (int)n, 0, 64, s));
+  sort_by_id(n, keys, out_ids.p, vals, sorted_vals.p, [&](size_t bytes) -> void* { tmp.reserve(std::max<size_t>(bytes, 1), 0, s); return tmp.p; }, s);
   out_rows.reserve((size_t)n * words, 0, s);
   DevBuf<int> dup;
   if (nsrc > 1) {
@@ -92,6 +89,15 @@ __global__ void expand_pm1_kernel(const uint32_t* __restrict__ words, const long
 }
 
 }  // namespace
+
+void sort_by_id(int64_t n, const long long* keys, long long* keys_out, const long long* vals, long long* vals_out,
+                const std::function<void*(size_t)>& temp, cudaStream_t s) {
+  if (n >= (1LL << 31)) fail(B200VS_EILLEGAL_PARAMETERS, "a sort by id holds at most 2^31 - 1 rows");
+  size_t tmp_bytes = 0;
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys_out, vals, vals_out, (int)n, 0, 64, s));
+  void* tmp = temp(tmp_bytes);
+  B200VS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys_out, vals, vals_out, (int)n, 0, 64, s));
+}
 
 void launch_gather_words(const uint32_t* src, const long long* rows, int64_t n, int words, uint32_t* dst, cudaStream_t s) {
   if (n <= 0) return;

@@ -181,12 +181,13 @@ static __global__ void __launch_bounds__(SCAN_THREADS) scan_key_kernel(const Sca
 }
 
 // Ordered range append (b200vs_scan_range_push, VectorReader::BruteForceRangeSearch): the hits of one tile are appended
-// to each query's running list in row order, until the list holds max_results.  One CTA per query (blockIdx.x, so more
+// to each query's running list in row order, until the list holds max_results.  The walk's i-th row is vecs row src(i) with
+// id ids[i]: the tile's own rows (IdentityRows), or a gathered list of an index's rows (ListRows, b200vs_brute_force_range_search).  One CTA per query (blockIdx.x, so more
 // than 65535 queries fit); the CTA walks the rows SCAN_QUADS at a time, one quad per row, and compacts the step's hits
 // with warp ballots and a prefix over the warps.  No atomics: the result does not depend on scheduling.
 struct RangeAppendArgs {
-  const float* vecs;      // [n, d] tile (normalised for cosine)
-  const long long* ids;   // [n], < 0 = never a hit
+  const float* vecs;      // the rows (normalised for cosine): the [n, d] tile, or the row store a ListRows walk indexes
+  const long long* ids;   // [n] the id of each row of the walk, < 0 = never a hit
   long long n;
   int d;
   const float* queries;   // [nq, d] (normalised for cosine)
@@ -202,8 +203,16 @@ constexpr int RANGE_WARPS = SCAN_THREADS / 32;
 // dynamic shared memory: the query (16-byte padded), then the per-warp hit counts of two steps
 inline size_t range_append_smem_bytes(int d) { return ((size_t)d * 4 + 15) / 16 * 16 + 2 * RANGE_WARPS * sizeof(int); }
 
-template <class Dist>
-static __global__ void __launch_bounds__(SCAN_THREADS) range_append_kernel(const RangeAppendArgs a) {
+struct IdentityRows {
+  __device__ __forceinline__ long long operator()(long long i) const { return i; }
+};
+struct ListRows {
+  const long long* rows;
+  __device__ __forceinline__ long long operator()(long long i) const { return rows[i]; }
+};
+
+template <class Dist, class Rows>
+static __global__ void __launch_bounds__(SCAN_THREADS) range_append_kernel(const RangeAppendArgs a, const Rows src) {
   extern __shared__ __align__(16) unsigned char smem[];
   constexpr int kWarps = RANGE_WARPS;
   const long long qi = blockIdx.x;
@@ -231,7 +240,7 @@ static __global__ void __launch_bounds__(SCAN_THREADS) range_append_kernel(const
     bool hit = false;
     float v = 0.f;
     if (__ballot_sync(0xffffffffu, valid) != 0u) {  // warp-uniform skip
-      v = Dist::eval(a.vecs, row < a.n ? row : base, qs, d, t, vec);
+      v = Dist::eval(a.vecs, src(row < a.n ? row : base), qs, d, t, vec);
       hit = valid && f2ord(Dist::kL2 ? v : -v) < a.thr_key;
     }
     const unsigned m = __ballot_sync(0xffffffffu, hit && t == 0);  // bit 4j = row base + 8 warp + j

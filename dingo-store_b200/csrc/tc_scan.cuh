@@ -88,6 +88,12 @@ struct TcView {
   const float* hscale = nullptr;   //   streams it instead of the FP32 rows; hscale[r] = 2^e (DESIGN.md 3, 4.2)
 };
 
+// The one-list layout of a Flat view over rows [0, rows): off_dev[0] = 0 and len_dev[0] = rows, on the device
+inline void set_flat_layout(TcView& v, int64_t rows, const long long* off_dev, const int* len_dev) {
+  v.arena_rows = rows; v.list_off = off_dev; v.list_len = len_dev;
+  v.nlist = 1; v.flat = true; v.total_chunks = (rows + TC_CHUNK - 1) / TC_CHUNK; v.max_chunks_per_list = (int)v.total_chunks;
+}
+
 // Arithmetic of the tile kernel's scores, and so of the error bound tc_eps()
 enum TcArith : int {
   TC_ARITH_TF32 = 0,   // rows truncated to TF32, queries rounded to nearest (list scan without a mirror)

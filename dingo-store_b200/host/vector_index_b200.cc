@@ -257,6 +257,27 @@ static butil::Status LowerFilters(b200vs_index* index, const std::vector<std::sh
   return butil::Status::OK();
 }
 
+// The results of the brute-force scanners (reader.cc:2022, FillRangeSearchResult utils.cc:657-694): one entry per query,
+// query q's hits from dist / labels [q * stride, ...): the first counts[q] of them (range), or every label >= 0 (top-k)
+static void FillScanResults(size_t nq, size_t stride, const std::vector<float>& dist, const std::vector<int64_t>& labels,
+                            const std::vector<int32_t>* counts, int32_t dimension, pb::common::MetricType metric,
+                            std::vector<pb::index::VectorWithDistanceResult>& results) {
+  results.resize(nq);
+  for (size_t row = 0; row < nq; ++row) {
+    const size_t n = counts ? (size_t)(*counts)[row] : stride;
+    for (size_t i = 0; i < n; ++i) {
+      const size_t pos = row * stride + i;
+      if (labels[pos] < 0) continue;
+      auto* vwd = results[row].add_vector_with_distances();
+      vwd->mutable_vector_with_id()->set_id(labels[pos]);
+      vwd->mutable_vector_with_id()->mutable_vector()->set_dimension(dimension);
+      vwd->mutable_vector_with_id()->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
+      vwd->set_distance(dist[pos]);
+      vwd->set_metric_type(metric);
+    }
+  }
+}
+
 butil::Status VectorIndexB200::Search(const std::vector<pb::common::VectorWithId>& vs, uint32_t topk,
                                       const std::vector<std::shared_ptr<FilterFunctor>>& filters, bool reconstruct,
                                       const pb::common::VectorSearchParameter& parameter,
@@ -379,6 +400,60 @@ butil::Status VectorIndexB200::RangeSearch(const std::vector<pb::common::VectorW
       vwd->set_metric_type(metric_type_);
     }
   }
+  return butil::Status::OK();
+}
+
+// BruteForceSearch / BruteForceRangeSearch's checks and filter lowering, before the library call (index non-null)
+static butil::Status BruteForcePrologue(b200vs_index* index, bool binary, int32_t dimension, const std::vector<pb::common::VectorWithId>& vs,
+                                        int64_t min_vector_id, int64_t max_vector_id,
+                                        const std::vector<std::shared_ptr<VectorIndex::FilterFunctor>>& filters, LoweredFilters& lf) {
+  if (binary) return butil::Status(pb::error::EVECTOR_NOT_SUPPORT, "brute-force search of binary vectors is not implemented");
+  if (vs.empty()) return butil::Status(pb::error::EILLEGAL_PARAMTETERS, "vector_with_ids is empty");
+  auto status = CheckVectorDimension(vs, dimension);
+  if (!status.ok()) return status;
+  status = LowerFilters(index, filters, lf);
+  if (!status.ok()) return status;
+  if (!lf.sp.has_range) { lf.sp.has_range = 1; lf.sp.range_min = min_vector_id; lf.sp.range_max = max_vector_id; }
+  else { lf.sp.range_min = std::max(lf.sp.range_min, min_vector_id); lf.sp.range_max = std::min(lf.sp.range_max, max_vector_id); }
+  return butil::Status::OK();
+}
+
+butil::Status VectorIndexB200::BruteForceSearch(const std::vector<pb::common::VectorWithId>& vs, uint32_t topk, int64_t min_vector_id,
+                                                int64_t max_vector_id, const std::vector<std::shared_ptr<FilterFunctor>>& filters,
+                                                std::vector<pb::index::VectorWithDistanceResult>& results) {
+  if (!index_) return ToStatus(B200VS_EINTERNAL);
+  LoweredFilters lf;
+  auto status = BruteForcePrologue(index_, Binary(), dimension_, vs, min_vector_id, max_vector_id, filters, lf);
+  if (!status.ok()) return status;
+  const size_t nq = vs.size();
+  std::vector<float> distances(nq * topk, 0.0f);
+  std::vector<int64_t> labels(nq * topk, -1);
+  if (topk > 0) {
+    const std::vector<float> x = ExtractVectorValue(vs, dimension_);
+    const int rc = b200vs_brute_force_search(index_, (int64_t)nq, x.data(), (int32_t)topk, &lf.sp, distances.data(), labels.data());
+    if (rc != B200VS_OK) return ToStatus(rc);
+  }
+  FillScanResults(nq, topk, distances, labels, nullptr, dimension_, metric_type_, results);
+  return butil::Status::OK();
+}
+
+butil::Status VectorIndexB200::BruteForceRangeSearch(const std::vector<pb::common::VectorWithId>& vs, float radius, int64_t min_vector_id,
+                                                     int64_t max_vector_id, const std::vector<std::shared_ptr<FilterFunctor>>& filters,
+                                                     std::vector<pb::index::VectorWithDistanceResult>& results) {
+  if (!index_) return ToStatus(B200VS_EINTERNAL);
+  LoweredFilters lf;
+  auto status = BruteForcePrologue(index_, Binary(), dimension_, vs, min_vector_id, max_vector_id, filters, lf);
+  if (!status.ok()) return status;
+  const size_t nq = vs.size();
+  const int32_t cap = max_range_search_result_count;
+  std::vector<float> distances(nq * (size_t)cap);
+  std::vector<int64_t> labels(nq * (size_t)cap);
+  std::vector<int32_t> counts(nq);
+  const std::vector<float> x = ExtractVectorValue(vs, dimension_);
+  const int rc = b200vs_brute_force_range_search(index_, (int64_t)nq, x.data(), radius, cap, &lf.sp, distances.data(), labels.data(),
+                                                 counts.data());
+  if (rc != B200VS_OK) return ToStatus(rc);
+  FillScanResults(nq, (size_t)cap, distances, labels, &counts, dimension_, metric_type_, results);
   return butil::Status::OK();
 }
 
@@ -604,17 +679,7 @@ butil::Status BruteForceScannerB200::Finish(std::vector<pb::index::VectorWithDis
   scan_ = nullptr;  // finish frees the handle
   const int rc = b200vs_scan_finish(s, distances.data(), labels.data());
   if (rc != B200VS_OK) return AbiStatus(rc);
-  for (size_t row = 0; row < nq_; ++row)
-    for (uint32_t i = 0; i < topk_; ++i) {
-      const size_t pos = row * topk_ + i;
-      if (labels[pos] < 0) continue;
-      auto* vwd = results[row].add_vector_with_distances();
-      vwd->mutable_vector_with_id()->set_id(labels[pos]);
-      vwd->mutable_vector_with_id()->mutable_vector()->set_dimension(dimension_);
-      vwd->mutable_vector_with_id()->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
-      vwd->set_distance(distances[pos]);
-      vwd->set_metric_type(metric_type_);
-    }
+  FillScanResults(nq_, topk_, distances, labels, nullptr, dimension_, metric_type_, results);
   return butil::Status::OK();
 }
 
@@ -668,16 +733,7 @@ butil::Status BruteForceRangeScannerB200::Finish(std::vector<pb::index::VectorWi
   scan_ = nullptr;  // finish frees the handle
   const int rc = b200vs_scan_range_finish(s, distances.data(), labels.data(), counts.data());
   if (rc != B200VS_OK) return AbiStatus(rc);
-  for (size_t row = 0; row < nq_; ++row)  // FillRangeSearchResult, utils.cc:657-694; left unsorted (reader.cc:2187-2189)
-    for (int32_t i = 0; i < counts[row]; ++i) {
-      const size_t pos = row * (size_t)cap_ + i;
-      auto* vwd = results[row].add_vector_with_distances();
-      vwd->mutable_vector_with_id()->set_id(labels[pos]);
-      vwd->mutable_vector_with_id()->mutable_vector()->set_dimension(dimension_);
-      vwd->mutable_vector_with_id()->mutable_vector()->set_value_type(pb::common::ValueType::FLOAT);
-      vwd->set_distance(distances[pos]);
-      vwd->set_metric_type(metric_type_);
-    }
+  FillScanResults(nq_, (size_t)cap_, distances, labels, &counts, dimension_, metric_type_, results);  // left unsorted (reader.cc:2187-2189)
   return butil::Status::OK();
 }
 

@@ -69,6 +69,19 @@ class VectorIndexB200 : public VectorIndex {
   // rebuilds of a region split (olds = {share index} for the child, {own index} for the parent) or merge ({own, sibling}).
   // The caller passes the region's range as VectorCodec::DecodeRangeToVectorId gives it.  The olds keep serving reads.
   butil::Status RebuildFrom(const std::vector<VectorIndexB200*>& olds, int64_t min_vector_id, int64_t max_vector_id);
+  // VectorReader::BruteForceSearch / BruteForceRangeSearch answered from this index's own device rows
+  // (b200vs_brute_force_search / b200vs_brute_force_range_search) instead of the region's RocksDB rows: the filters are
+  // lowered as Search lowers them, plus the region's range min_vector_id <= id < max_vector_id (as
+  // VectorCodec::DecodeRangeToVectorId gives it), and results are filled as BruteForceScannerB200 /
+  // BruteForceRangeScannerB200 fill them (one entry per query; range: at most max_range_search_result_count hits in
+  // ascending id order, unsorted).  EVECTOR_NOT_SUPPORT for IVF_PQ, the binary types and HNSW cosine: the caller keeps its
+  // RocksDB loop.  Call them only when this index alone serves the region (no share index, no sibling) and IsReady().
+  butil::Status BruteForceSearch(const std::vector<pb::common::VectorWithId>& vector_with_ids, uint32_t topk, int64_t min_vector_id,
+                                 int64_t max_vector_id, const std::vector<std::shared_ptr<FilterFunctor>>& filters,
+                                 std::vector<pb::index::VectorWithDistanceResult>& results);
+  butil::Status BruteForceRangeSearch(const std::vector<pb::common::VectorWithId>& vector_with_ids, float radius, int64_t min_vector_id,
+                                      int64_t max_vector_id, const std::vector<std::shared_ptr<FilterFunctor>>& filters,
+                                      std::vector<pb::index::VectorWithDistanceResult>& results);
   bool NeedTrain() override;
   bool IsTrained() override;
   // the stock plugins' rules (flat.cc:515-531, ivf_flat.cc:786-802, raw_ivf_pq.cc:533-549, ivf_pq.cc:450-462, hnsw.cc:592-609):

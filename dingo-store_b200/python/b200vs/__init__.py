@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "b200vs_shard_search_deep", "b200vs_shard_search_binary_deep",
     "b200vs_shard_need_rebuild", "b200vs_shard_rebuild_from", "b200vs_shard_rebuild_from_range",
     "b200vs_save_stage", "b200vs_save_staged", "b200vs_save_unstage",
+    "b200vs_brute_force_search", "b200vs_brute_force_range_search",
 ]
 
 
@@ -120,6 +121,8 @@ def lib():
     L.b200vs_scan_range_finish.argtypes = [vp, vp, vp, vp]
     L.b200vs_scan_range_abort.argtypes = [vp]
     L.b200vs_scan_range_abort.restype = None
+    L.b200vs_brute_force_search.argtypes = [vp, i64, vp, i32, ctypes.POINTER(SearchParams), vp, vp]
+    L.b200vs_brute_force_range_search.argtypes = [vp, i64, vp, f32, i32, ctypes.POINTER(SearchParams), vp, vp, vp]
     L.b200vs_set_profiling.argtypes = [vp, ctypes.c_int]
     L.b200vs_last_error.restype = ctypes.c_char_p
     L.b200vs_version.restype = ctypes.c_char_p
@@ -358,6 +361,30 @@ class Index:
         fn = self.L.b200vs_range_search_binary if self.binary else self.L.b200vs_range_search
         _check(fn(self.h, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
                                           ctypes.byref(sp), D.ctypes.data, I.ctypes.data, C.ctypes.data))
+        return D, I, C
+
+    def brute_force_search(self, xq, k, **kw):
+        """Brute-force top-k over the index's own device rows (b200vs_brute_force_search): what BruteForceScan returns for
+        the index's live rows in ascending id order."""
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(k, 0)), dtype=np.float32)
+        I = np.full((nq, max(k, 0)), -1, dtype=np.int64)
+        _check(self.L.b200vs_brute_force_search(self.h, nq, xq.ctypes.data if xq.size else None, k, ctypes.byref(sp), D.ctypes.data,
+                                                I.ctypes.data))
+        return D, I
+
+    def brute_force_range_search(self, xq, radius, max_results=1024, **kw):
+        """Brute-force range search over the index's own device rows (b200vs_brute_force_range_search): per query the
+        first max_results hits in ascending id order, unsorted, as BruteForceRangeScan returns them for the live rows in
+        that order."""
+        xq, nq = self._rows(xq)
+        sp, keep = make_search_params(**kw)
+        D = np.zeros((nq, max(max_results, 0)), dtype=np.float32)
+        I = np.full((nq, max(max_results, 0)), -1, dtype=np.int64)
+        C = np.zeros(nq, dtype=np.int32)
+        _check(self.L.b200vs_brute_force_range_search(self.h, nq, xq.ctypes.data if xq.size else None, float(radius), max_results,
+                                                      ctypes.byref(sp), D.ctypes.data, I.ctypes.data, C.ctypes.data))
         return D, I, C
 
     # ---- introspection ----

@@ -659,6 +659,33 @@ int b200vs_scan_range_push(b200vs_scan_range* scan, int64_t n, const float* x, c
 int b200vs_scan_range_finish(b200vs_scan_range* scan, float* out_dist, int64_t* out_ids, int32_t* out_counts);
 void b200vs_scan_range_abort(b200vs_scan_range* scan);
 
+/* The same brute-force searches answered from an index's own device rows, in place of the RocksDB scan whose rows a reader
+ * pushes through b200vs_scan_* / b200vs_scan_range_* (VectorReader::BruteForceSearch / BruteForceRangeSearch, the road of
+ * every request with use_brute_force and of every range search on HNSW).  Host pointers; readers, under the index's read
+ * lock like b200vs_search.  The result is what b200vs_scan_begin/push/finish (b200vs_scan_range_begin/push/finish) returns
+ * when fed the index's live rows in ascending id order with the same queries, k (radius, max_results), metric and sp, bit
+ * for bit (ids, distance bits, counts):
+ *   - top-k: exact, ordered by (API distance, id), -1 / 0 padded, any k up to B200VS_DEEP_MAX_K (past the exact scan's
+ *     select pool through the deep path, as b200vs_scan_* does).  The rows may be fed in any chunking, with one exception
+ *     that the chunked scan itself carries under IP / COSINE: where 1 - ip rounds two rows' different ip values to one
+ *     distance at the k-th slot, a chunking that splits them may keep the smaller id where one chunk keeps the larger ip;
+ *   - range: per query the FIRST max_results hits in ascending id order (RocksDB key order), unsorted.  Rows sharing an id
+ *     (an IVF_FLAT add without upsert) come in storage order; the scan takes them in that order in separate chunks, as
+ *     b200vs_scan_range_push refuses a repeated id inside one tile.
+ * sp's filters apply (id range, sorted id list, negate); nprobe and efsearch are ignored; exact_only is accepted and changes
+ * nothing.  Stored cosine rows are not normalised again; the queries are normalised as b200vs_scan_begin does.
+ * Types: FLAT, IVF_FLAT (every metric) and HNSW under L2 / IP.  IVF_PQ (codes only), BINARY_FLAT, BINARY_IVF_FLAT and HNSW
+ * under COSINE (its rows carry NormalizeVectorForHnsw's bits, which a scan over raw rows does not reproduce):
+ * EVECTOR_NOT_SUPPORT, nothing launched, the index unchanged; the caller keeps its RocksDB scan.
+ * An empty or untrained index: empty results.  k <= 0: OK, nothing done; k > B200VS_DEEP_MAX_K, max_results <= 0 or a null
+ * output: EILLEGAL_PARAMETERS.  A NaN radius admits no row: every count 0, nothing launched.  No row is copied: top-k scans
+ * the rows in place (tombstones, unused slots and deleted nodes count as id -1 through a per-call id view); range compacts
+ * the live rows that pass the filters into a row list, sorts it by id and walks the rows through it. */
+int b200vs_brute_force_search(b200vs_index* idx, int64_t nq, const float* xq, int32_t k, const b200vs_search_params* sp,
+                              float* out_dist, int64_t* out_ids);
+int b200vs_brute_force_range_search(b200vs_index* idx, int64_t nq, const float* xq, float radius, int32_t max_results,
+                                    const b200vs_search_params* sp, float* out_dist, int64_t* out_ids, int32_t* out_counts);
+
 /* Counters of the last search on this index: [0] kernels launched, [1] queries served by the tensor-core
  * candidate pass; with profiling on (b200vs_set_profiling) also [2] queries of the tensor-core pass that failed
  * certification and were re-run on the exact path (0 with profiling off), [3] device time of the dominant list-scan
